@@ -1,13 +1,13 @@
-# convenience targets; the driver uses __graft_entry__.build(), pytest and bench.py directly
+# convenience targets over __graft_entry__.build(), pytest and bench.py
 PY ?= python
 
-build:            ## nvcc (sm_100a) -> csrc/libmm_engine.so, gcc -> oracle/liborc.so
+build:            ## nvcc (sm_90a) -> csrc/libmm_engine.so, gcc -> oracle/liborc.so
 	$(PY) -c "import __graft_entry__ as g; g.build()"
 
 test:             ## CPU suite: oracle KATs / properties, golden fixtures, ABI export, host mirror, gloo sharding
 	$(PY) -m pytest tests -x -q -m "not gpu"
 
-test-gpu:         ## parity through the C ABI (needs a B200)
+test-gpu:         ## parity through the C ABI (needs an H100)
 	$(PY) -m pytest tests -x -q -m gpu
 
 smoke:            ## one small tick on cuda:0, checked against the oracle

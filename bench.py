@@ -21,6 +21,7 @@ A step = one pass of the hot path (one search tick) over one synthetic player po
 Launch: `python bench.py --gpus 1 --steps K --warmup W`, or under torchrun for N>1
 (one rank per GPU; ranks own disjoint rating groups — no data-path collective).
 `--impl reference` times the CPU restatement of the reference loop (oracle/).
+`--dump-outputs DIR`: the last timed tick's results as .npy files (dump_outputs), to compare two builds.
 """
 import argparse
 import importlib
@@ -38,6 +39,7 @@ if ROOT not in sys.path:
 PKG = "microservice-matchmaking_b200"
 
 B_ALG_TICK = 22      # SURVEY §8(d) strict-parity mode: read id 8 + rating 4 + mode 1 + team_size 1, write id 8
+H100_HBM_GBS = 3350.0  # NVIDIA H100 SXM data sheet, HBM3
 B_CONSUMED_TICK = 20  # what the tick really moves per player: bin 2 (twice: histogram + placement, the second time
 #                       from L2) + id 8 read, id 8 written; rating/mode -> bin is paid at ingest
 
@@ -49,7 +51,69 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return H100_HBM_GBS, "H100 SXM data sheet (not measured)"
+
+
+def gpu_info(gpu_index):
+    try:
+        out = subprocess.run(["nvidia-smi", f"--id={gpu_index}", "--query-gpu=name,power.limit,clocks.max.sm",
+                              "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30).stdout
+        name, plim, smax = [x.strip() for x in out.strip().split(",")]
+        return {"name": name, "power_limit_w": float(plim), "sm_max_mhz": float(smax)}
+    except Exception:
+        return {"name": None, "power_limit_w": None, "sm_max_mhz": None}
+
+
+def _dev_to_host(ptr, n, typestr):
+    import numpy as np
+    import torch
+    if n == 0:
+        return np.zeros(0, np.dtype(typestr))
+
+    class _View:
+        __cuda_array_interface__ = {"shape": (n,), "typestr": typestr, "data": (ptr, False), "strides": None,
+                                    "version": 2}
+    return torch.as_tensor(_View(), device="cuda").cpu().numpy()
+
+
+def dump_outputs(out_dir, eng, st):
+    """The last tick's results (mm_results_device + the pool left queued) -> OUT_DIR/<name>.npy, float64, ids as exact
+    32-bit halves; large arrays as a fixed seeded sample of rows (+ indices), digest.npy checksums all of them."""
+    import numpy as np
+    pkg = importlib.import_module(PKG)
+    p_lob, p_mem = eng.results_device()
+    lob = _dev_to_host(p_lob, st.n_lobbies, "<i8").view(pkg.engine.LOBBY_DTYPE)
+    mem = _dev_to_host(p_mem, st.n_matched, "<i8").view(np.uint64)
+    resid = eng.pool_read()["id"]
+    rng = np.random.default_rng(20240601)
+
+    def sample(n, cap):
+        return np.arange(n) if n <= cap else np.sort(rng.choice(n, cap, replace=False))
+
+    def halves(ids):
+        return np.stack([ids >> np.uint64(32), ids & np.uint64(0xFFFFFFFF)], axis=1).astype(np.float64)
+
+    def digest(words):
+        w = pkg.synth.mix64(np.arange(len(words), dtype=np.uint64))
+        with np.errstate(over="ignore"):
+            h = np.sum(words * w, dtype=np.uint64) if len(words) else np.uint64(0)
+        return [float(h >> np.uint64(32)), float(h & np.uint64(0xFFFFFFFF))]
+
+    li, mi, ri = sample(len(lob), 1 << 18), sample(len(mem), 1 << 20), sample(len(resid), 1 << 18)
+    arrays = {
+        "stats": np.array([st.n_lobbies, st.n_matched, st.n_residual, st.n_dead], np.float64),
+        "lobbies": np.stack([lob[k][li] for k in ("first_member", "n_members", "mode", "group")], axis=1).astype(np.float64),
+        "lobby_index": li.astype(np.float64),
+        "member_ids": halves(mem[mi]),
+        "member_index": mi.astype(np.float64),
+        "residual_ids": halves(resid[ri]),
+        "residual_index": ri.astype(np.float64),
+        "digest": np.array(digest(mem) + digest(lob.view(np.uint64)), np.float64),
+    }
+    assert sum(a.nbytes for a in arrays.values()) <= 64 << 20
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 class ClockSampler:
@@ -207,6 +271,8 @@ def main():
     ap.add_argument("--tick-impl", type=int, default=None, help="1 = one fused cooperative launch (default), 0 = four launches")
     ap.add_argument("--max-spread", type=int, default=None,
                     help="EXTENSION (policy S1, not the BASELINE workload): a lobby spans at most W rating points")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the results of the last timed tick to DIR/<name>.npy (rank 0)")
     args = ap.parse_args()
 
     rank = int(os.environ.get("RANK", "0"))
@@ -251,9 +317,9 @@ def main():
         if args.max_spread is not None:
             eng.set_option("max_spread", args.max_spread)
 
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device="cuda")  # > 50 MB L2 of an H100
 
-    def device_timed(cfg_, ids_, rating_, mode_, ts_, steps, warmup):
+    def device_timed(cfg_, ids_, rating_, mode_, ts_, steps, warmup, dump_dir=None):
         """K ticks of one resident pool (restored from a device snapshot, L2 flushed, both untimed)."""
         eng = pkg.Engine(cfg_)
         options(eng)
@@ -277,14 +343,18 @@ def main():
             phases.append((st.hist_us, st.scan_us, st.place_us, st.epilogue_us))
         barrier()
         wall = time.perf_counter() - t0
+        if dump_dir:
+            dump_outputs(dump_dir, eng, st)
         eng.close()
         return sum(dev_us) * 1e-6, st, phases, wall
 
-    # ---- weak leg (the contract's line): every rank holds a full-size pool of its own seed stream -------------
+    # ---- weak leg (the headline value): every rank holds a full-size pool of its own seed stream -------------
     ids, rating, mode, ts = pkg.synth.gen_pool(1, n, first=rank * n, mode=mode_idx)
+    gpu = gpu_info(local)
     sampler = ClockSampler(local)
     sampler.start()
-    tick_s, st, phases, wall_s = device_timed(cfg, ids, rating, mode, ts, args.steps, args.warmup)
+    tick_s, st, phases, wall_s = device_timed(cfg, ids, rating, mode, ts, args.steps, args.warmup,
+                                              dump_dir=args.dump_outputs if rank == 0 else None)
     launches_per_tick = st.n_launches
     lobbies_per_step = st.n_lobbies
     if world > 1:
@@ -515,13 +585,6 @@ def main():
         tick_avg_s = tick_s / args.steps
         fused = launches_per_tick == 1
         ach = B_ALG_TICK * n / tick_avg_s / 1e9
-        traffic = None
-        tp = os.path.join(ROOT, "profiles", "tick_traffic.json")
-        if os.path.exists(tp) and args.workload == "config3_10m_g32_5v5" and args.order == "rating":
-            try:
-                traffic = json.load(open(tp)).get("dram_bytes_per_launch" if fused else "dram_bytes_split_launches")
-            except Exception:
-                pass
         line = {
             "metric": "matches/sec", "value": value, "unit": "lobbies/s", "n_gpus": world, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": 1e3 * tick_s / args.steps, "higher_is_better": True,
@@ -547,15 +610,15 @@ def main():
             "wall_ms_per_step_incl_restore": 1e3 * wall_s / args.steps,
             "roofline": {"bound": "hbm", "kernel": "k_tick" if fused else "k_hist + k_colscan + k_place + k_epilogue",
                          "achieved": ach, "peak": peak, "unit": "GB/s",
-                         "frac": ach / peak, "traffic": traffic, "peak_source": peak_src,
+                         "frac": ach / peak, "peak_source": peak_src,
                          "bytes_per_player": B_ALG_TICK, "players_per_launch": n, "us_per_launch": 1e6 * tick_avg_s,
-                         "frac_of_8000": ach / 8000.0,
+                         "frac_of_datasheet": ach / H100_HBM_GBS, "datasheet_gbs": H100_HBM_GBS,
                          "consumed": {"bytes_per_player": B_CONSUMED_TICK, "achieved": B_CONSUMED_TICK * n / tick_avg_s / 1e9,
                                       "frac": B_CONSUMED_TICK * n / tick_avg_s / 1e9 / peak,
                                       "note": "the tick reads the 2-byte sort key derived at ingest, not rating + mode + "
                                               "team_size (6 B): on the bytes it really consumes the fraction is lower"}},
             "cpu_baseline": cpu, "e2e": e2e, "strong": strong, "stream": stream,
-            "gpu_launches": launches_per_tick * args.steps, "clocks": clocks,
+            "gpu_launches": launches_per_tick * args.steps, "clocks": clocks, "gpu": gpu,
         }
         print(json.dumps(line), flush=True)
     if world > 1:

@@ -1,5 +1,5 @@
 /*
- * mm_engine.h — C ABI of the B200 opponent-search engine (libmm_engine.so).
+ * mm_engine.h — C ABI of the H100 opponent-search engine (libmm_engine.so).
  *
  * This is the drop-in boundary for the *search stage* of
  * OpenMatchmaking/microservice-matchmaking.  Every entry point names the

@@ -1,4 +1,4 @@
-// mm_common.cuh — shared types and device helpers of the search tick (sm_100a); see mm_kernels.cuh.
+// mm_common.cuh — shared types and device helpers of the search tick (sm_90a); see mm_kernels.cuh.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,4 +1,4 @@
-// mm_engine.cu — C ABI of the B200 opponent-search engine (include/mm_engine.h).
+// mm_engine.cu — C ABI of the H100 opponent-search engine (include/mm_engine.h).
 //
 // Host side of the drop-in for the reference search stage
 // (matchmaking/lib/search/worker.ex + models/{active_user,lobby_state}.ex).  The pool
@@ -789,7 +789,7 @@ int mm_create(const mm_config* cfg, mm_engine** out) {
     // overlap the other's work), else one.  Function attributes are process-global:
     // every kernel gets the device's opt-in maximum.
     const size_t static_smem = sizeof(Geo) + 512;
-    const uint32_t st_max = 2;  // measured: 2 ring stages x 2 CTAs per SM beat 3 x 2 by ~1 us on config3
+    const uint32_t st_max = 2;  // measured on an H100 (config3): a third ring stage is no faster
     for (uint32_t st = st_max; st >= 2 && !e->place_stages; --st)
       if (2 * (place_smem_bytes(e->max_nb, st) + static_smem + 1024) <= e->smem_sm) { e->place_stages = st; e->rows_per_sm = 2; }
     for (uint32_t st = kMaxStages; st >= 1 && !e->place_stages; --st)  // huge key domains: down to a single stage

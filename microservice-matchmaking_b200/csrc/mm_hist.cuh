@@ -133,7 +133,7 @@ __device__ __forceinline__ void rowsum_body(unsigned char* smem_raw, const Geo& 
     desc_fill<BLOCK>(dc, g, meta, tb, s1);
     __syncthreads();
     const uint32_t nt = s1 - tb < kDescCap ? s1 - tb : kDescCap;
-    constexpr uint32_t U = 8;  // loads in flight per thread: the histograms are cold in DRAM, one at a time is 17 x 0.8 us
+    constexpr uint32_t U = 8;  // loads in flight per thread: the histograms are cold in DRAM, one at a time serialises 17 round trips
     for (uint32_t t0 = 0; t0 < nt; t0 += U) {
       uint32_t v[U];
 #pragma unroll

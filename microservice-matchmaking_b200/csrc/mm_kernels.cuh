@@ -1,4 +1,4 @@
-// mm_kernels.cuh — device code of the search tick (sm_100a).
+// mm_kernels.cuh — device code of the search tick (sm_90a).
 //
 // The tick replaces, for every queued player at once, the per-request loop of
 // Search.Worker.consume/5 (reference matchmaking/lib/search/worker.ex:291-324).

@@ -15,8 +15,8 @@ namespace mm {
 // Two ranking paths, chosen per tile (uniform for the CTA):
 //  * FAST — the tile's partition has <= 255 bins (e.g. 5 001 rating values in 32 groups: 157): a one-pass 8-bit
 //    counting sort of the tile in shared memory.  Warp w owns 128 consecutive tile positions; per 32 players the
-//    peers with the same digit are found with <= 8 ballots (MATCH.ANY costs 64 cycles per warp instruction on
-//    B200), the lowest peer bumps the warp's private digit counter; 128 threads then scan the 16 x 256 counter
+//    peers with the same digit are found with <= 8 ballots (MATCH.ANY is a slow multi-pass warp instruction,
+//    see tools/ubench/smem.cu), the lowest peer bumps the warp's private digit counter; 128 threads then scan the 16 x 256 counter
 //    matrix (two 16-bit digits per word, packed adds) into tile-local sorted positions.  Ids are staged AT THEIR
 //    SORTED POSITION in the tile's own ring stage together with their global slot, and the CTA writes the staged
 //    tile back in sorted order: consecutive threads store consecutive slots of a bin's run (about 2048 / bins ids =
@@ -199,7 +199,7 @@ __device__ __forceinline__ void place_body(unsigned char* smem_raw, const Geo& g
         // Peers of the same digit among the warp's 32 players: every lane ORs its bit into the warp's mask table
         // (shared-memory RED), reads the word back — that IS the match mask — and the peers reset the word
         // and bump the warp's running digit counter.  3 shared-memory instructions per 32 players instead of 8
-        // ballots + selects (MATCH.ANY costs 64 cycles per warp instruction on B200).
+        // ballots + selects (MATCH.ANY is a slow multi-pass warp instruction).
         uint32_t* wm = wmask + warp * 256;
         uint16_t* wc = wcnt + warp * 256;
         const uint32_t lbit = 1u << lane;

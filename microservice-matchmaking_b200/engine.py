@@ -34,7 +34,7 @@ def load_library():
         if not os.path.exists(path):
             raise ImportError(
                 f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-                "(nvcc, sm_100a).  There is no CPU fallback for the search tick.")
+                "(nvcc, sm_90a).  There is no CPU fallback for the search tick.")
         _lib = abi.bind(C.CDLL(path))
         if _lib.mm_abi_version() != abi.MM_ABI_VERSION:
             raise ImportError("libmm_engine.so ABI version mismatch")

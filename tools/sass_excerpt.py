@@ -10,7 +10,7 @@ for ln in out.splitlines():
     if m: cur = m.group(1); funcs[cur] = []; continue
     if cur and re.search(r"/\*[0-9a-f]{4,}\*/\s+\S", ln): funcs[cur].append(ln.rstrip())
 KEYS = ("UBLKCP", "SYNCS", "ATOMS", "ATOMG", "REDG", "REDUX", "BAR", "VOTE", "MATCH", "SHFL", "LDS", "STS", "LDG", "STG", "WARPSYNC", "POPC", "MEMBAR", "FENCE", "HMMA", "UTCMMA")
-print("cuobjdump -sass libmm_engine.so (sm_100a), instruction mix of the tick and ingest kernels (static counts) and the TMA / mbarrier / shared-memory-atomic lines of k_tick\n")
+print("cuobjdump -sass libmm_engine.so (sm_90a), instruction mix of the tick and ingest kernels (static counts) and the TMA / mbarrier / shared-memory-atomic lines of k_tick\n")
 for name, lines in funcs.items():
     if not re.search(r"k_tick|k_place|k_hist|k_enq_append|k_enq_claim", name): continue
     c = collections.Counter()

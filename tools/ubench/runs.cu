@@ -1,6 +1,6 @@
 // Microbenchmark: 10 M 8-byte stores to an 80 MB array where every `run` consecutive lanes write `run` consecutive
 // slots at a random base — how much does the store rate improve when a warp instruction touches fewer sectors?
-// (what sorting placement tiles by destination could buy).  nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o runs runs.cu
+// (what sorting placement tiles by destination could buy).  nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o runs runs.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>

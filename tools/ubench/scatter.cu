@@ -1,5 +1,5 @@
-// Microbenchmark: what limits random small stores / loads on B200?
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scatter scatter.cu
+// Microbenchmark: what limits random small stores / loads on an H100?
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scatter scatter.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>

@@ -1,4 +1,4 @@
-// Microbenchmark: shared-memory op throughput with random (bin-like) addresses on B200.
+// Microbenchmark: shared-memory op throughput with random (bin-like) addresses on an H100.
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>
