@@ -68,6 +68,7 @@ struct TickCtr {
   uint32_t n_lobbies, n_matched, n_alive, n_dead, n_resid;
   uint32_t n_tiles;
   uint32_t heavy;  // some bin expects > 8 players per tile: the list ranking uses warp-aggregated nodes
+  uint32_t chist_bad;  // placement tiles whose ranked key counts differ from their chunk histogram (must stay 0)
   unsigned long long t[12]; // fused kernel: %globaltimer (ns) at phase boundaries, CTA 0; [6],[7]: max over CTAs;
                             // [8] last row done with phase 1, [9] min CTA start, [10] last row done placing
 };
@@ -145,6 +146,10 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
       "DONE:\n"
       "}" ::"r"(smem_u32(bar)), "r"(parity) : "memory");
 }
+// plain arrival (release, CTA scope): the thread's earlier shared-memory writes are visible to the phase's waiters
+__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
+}
 __device__ __forceinline__ void mbar_inval(uint64_t* bar) {
   asm volatile("mbarrier.inval.shared::cta.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
@@ -153,6 +158,11 @@ __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.
 // barrier among the first `nthreads` threads of the CTA only (named barrier 1)
 __device__ __forceinline__ void bar_sync_named(uint32_t nthreads) {
   asm volatile("bar.sync 1, %0;" ::"r"(nthreads) : "memory");
+}
+// barrier among the 256 threads of one half of the CTA (threads [256 h, 256 h + 256)): named barrier 2 + h
+__device__ __forceinline__ void bar_sync_half(uint32_t h) {
+  if (h) asm volatile("barrier.sync 3, 256;" ::: "memory");  // literal ids: ptxas reserves only the barriers it sees
+  else asm volatile("barrier.sync 2, 256;" ::: "memory");
 }
 // Grid-wide barrier for the fused tick kernel (cooperative launch: all CTAs are co-resident).
 __device__ __forceinline__ void grid_barrier(unsigned int* bar, unsigned int target) {

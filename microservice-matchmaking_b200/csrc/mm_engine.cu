@@ -637,6 +637,10 @@ int tick_commit(mm_engine* e, uint32_t n, mm_tick_stats* stats) {
   e->pool[e->cur].n = c.n_resid;
   e->last = st;
   if (stats) *stats = st;
+  if (c.chist_bad) {  // placement took slot bases from chunk histograms that disagree with the pool: results are wrong
+    std::snprintf(e->last_err, sizeof(e->last_err), "%u placement tiles disagree with their chunk histograms", c.chist_bad);
+    return MM_E_STATE;
+  }
   return MM_OK;
 }
 
@@ -789,7 +793,7 @@ int mm_create(const mm_config* cfg, mm_engine** out) {
     // overlap the other's work), else one.  Function attributes are process-global:
     // every kernel gets the device's opt-in maximum.
     const size_t static_smem = sizeof(Geo) + 512;
-    const uint32_t st_max = 2;  // measured on an H100 (config3): a third ring stage is no faster
+    const uint32_t st_max = 2;  // measured on an H100 (config3, two tile pipelines): a third ring stage is slower
     for (uint32_t st = st_max; st >= 2 && !e->place_stages; --st)
       if (2 * (place_smem_bytes(e->max_nb, st) + static_smem + 1024) <= e->smem_sm) { e->place_stages = st; e->rows_per_sm = 2; }
     for (uint32_t st = kMaxStages; st >= 1 && !e->place_stages; --st)  // huge key domains: down to a single stage

@@ -137,7 +137,7 @@ __global__ void __launch_bounds__(BLOCK, 2) k_tick(const TickArgs a) {
     __threadfence();
     if (atomicAdd(&ctr->done, 1u) == G - 1) {  // ... and arms the other counter block for the next tick
       TickCtr* nx = a.next_ctr;
-      nx->gbar = 0; nx->done = 0;
+      nx->gbar = 0; nx->done = 0; nx->chist_bad = 0;
       nx->t[6] = 0; nx->t[7] = 0; nx->t[8] = 0; nx->t[10] = 0;
     }
   }

@@ -12,7 +12,10 @@ namespace mm {
 //     slot = outbase[bin] + (players of the bin in earlier rows: M) + rank inside the row.
 // A player at or past binlim[bin] stays queued: one bit in left_bits (one ballot per 32 players, plain word stores).
 //
-// Two ranking paths, chosen per tile (uniform for the CTA):
+// A pool with chunk histograms (every partition <= 255 keys) and rank_impl 3 takes place_halves: two tile pipelines
+// per CTA whose slot bases come from the histograms, so no tile waits for another tile's ranking and no barrier spans
+// the CTA (see there).  Otherwise (a partition with > 255 keys, or rank_impl 2) the whole CTA ranks one tile at a time
+// and takes its slot bases from its own ranking; two ranking paths, chosen per tile (uniform for the CTA):
 //  * FAST — the tile's partition has <= 255 bins (e.g. 5 001 rating values in 32 groups: 157): a one-pass 8-bit
 //    counting sort of the tile in shared memory.  Warp w owns 128 consecutive tile positions; per 32 players the
 //    peers with the same digit are found with <= 8 ballots (MATCH.ANY is a slow multi-pass warp instruction,
@@ -26,8 +29,11 @@ namespace mm {
 //    smaller tile position; ids are scattered straight from registers.  `heavy` ticks (some bin expects > 8
 //    players per tile) aggregate the nodes per warp first (__match_any_sync) so a list never exceeds 64 nodes.
 //
-// Shared memory: ring_ids[stages][kTile] | ring_bins[stages][kTile] | mbarriers + tile descriptors | cnt[keys of one partition] |
-//                union { LIST: head[kHeadSlots] node[kTile] nbin[kTile] ; FAST: wcnt[16][256] u16, sslot[kTile] }.
+// Shared memory (whole CTA): ring_ids[stages][kTile] | ring_bins[stages][kTile] | mbarriers + tile descriptors |
+//                cnt[keys of one partition] | union { LIST: head[kHeadSlots] node[kTile] nbin[kTile] ;
+//                FAST: wmask[16][256], wcnt[16][256] u16, lgd[256], spd[kTile] }.
+// Shared memory (two pipelines): ring_ids | ring_bins | ring_hist[stages][256] | mbarriers + tile descriptors | cnt |
+//                2 x { wmask[8][256], wcnt[8][256] u16, lgd[256], spd[kTile] }.
 // ---------------------------------------------------------------------------------------
 constexpr uint32_t kHeadSlots = 4096;
 constexpr uint32_t NW16 = 16;  // warps per 512-thread CTA
@@ -35,8 +41,23 @@ constexpr uint32_t kPlaceUnionBytes = NW16 * 256 * 4 + NW16 * 256 * 2 + 1024 + k
 
 // max_nb = most sort keys any one partition has: the slot counters are kept per partition, not for the whole key domain
 __host__ __device__ constexpr uint32_t place_cnt_cap(uint32_t max_nb) { return (max_nb > 1024u ? max_nb : 1024u); }
-__host__ __device__ constexpr size_t place_smem_bytes(uint32_t max_nb, uint32_t stages) {
+// Two tile pipelines per CTA (pools with chunk histograms): per pipeline wmask[8][256] u32 | wcnt[8][256] u16 |
+// lgd[256] | spd[kTile]; every ring stage also carries the chunk's 1 KB histogram row.
+constexpr uint32_t kHalfWarps = 8;
+constexpr uint32_t kHalfBytes = kHalfWarps * 256 * 4 + kHalfWarps * 256 * 2 + 256 * 4 + kTile * 4;
+__host__ __device__ constexpr size_t place_smem_whole(uint32_t max_nb, uint32_t stages) {
   return (size_t)stages * kTileBytes + 128 + (size_t)((place_cnt_cap(max_nb) + 3) & ~3u) * 4 + kPlaceUnionBytes + sizeof(DescCache) + 16;
+}
+__host__ __device__ constexpr size_t place_smem_halves(uint32_t max_nb, uint32_t stages) {
+  return (size_t)stages * (kTileBytes + kChunkHist * 4) + 256 + (size_t)((place_cnt_cap(max_nb) + 3) & ~3u) * 4 +
+         2 * kHalfBytes + sizeof(DescCache) + 16;
+}
+// max_nb <= kFastBins: the pool has chunk histograms and places on the two-pipeline path (or, with rank_impl = 2, on
+// the whole-CTA path, whose layout fits in the same allocation)
+__host__ __device__ constexpr size_t place_smem_bytes(uint32_t max_nb, uint32_t stages) {
+  return max_nb <= kFastBins && place_smem_halves(max_nb, stages) > place_smem_whole(max_nb, stages)
+             ? place_smem_halves(max_nb, stages)
+             : place_smem_whole(max_nb, stages);
 }
 
 struct PlaceArgs {
@@ -57,9 +78,292 @@ struct PlaceArgs {
   TickCtr* ctr;
 };
 
+// place_halves<BLOCK>: the FAST ranking for a pool with chunk histograms (every partition <= 255 keys, rank_impl 3).
+// The CTA runs two independent tile pipelines: half h (threads 256 h .. 256 h + 255, 8 warps, 8 players per thread)
+// takes the row's tiles t = h, h + 2, ... and synchronises only on its own named barrier.  The halves share the ring
+// and the row's running slot counters cnt[]; nothing waits for another tile's ranking:
+//  * slot bases: the chunk's histogram row travels with the tile (third bulk copy into the stage).  Tile t takes
+//    cnt[d] as the global slot of its first player of key d and advances cnt[d] by chist[d] — a 256-entry step,
+//    passed from tile t-1 to tile t through the `hand` mbarrier (one phase per tile).  Tile-local first positions l0
+//    are the exclusive scan of the same row.  Bit 31 of a slot base (some player of the (tile, key) cell is past the
+//    key's matched prefix) comes from cnt[d] + chist[d] against binlim.
+//  * ring: stage s has a `full` mbarrier (the three bulk copies) and an `empty` one (the 256 threads of the half that
+//    wrote the tile back); thread 0 of that half waits on `empty` and issues the stage's next tile at once.
+//  * per tile and half: rank (as below: match table / ballots, per-warp counters) | barrier | column scan of the
+//    8 warps' counters + check of their totals against chist | barrier | stage the sorted order | barrier | write back.
+// A tile whose ranked key counts differ from its chunk histogram is not written at all and counted in
+// TickCtr::chist_bad (the tick then fails): the slot bases of the row's later tiles rest on the histograms.
+template <int BLOCK>
+__device__ __forceinline__ void place_halves(unsigned char* smem_raw, const Geo& g, const PlaceArgs a) {
+  static_assert(BLOCK == 512 && kTile == 2048, "tile arrangement is written for 2 x 256 threads x 8 players");
+  constexpr int J = 8;
+  const uint32_t S = a.stages;
+  uint64_t* ring_ids = reinterpret_cast<uint64_t*>(smem_raw);                               // [S][kTile]
+  uint16_t* ring_bins = reinterpret_cast<uint16_t*>(smem_raw + (size_t)S * kTile * 8);      // [S][kTile]
+  uint32_t* ring_hist = reinterpret_cast<uint32_t*>(smem_raw + (size_t)S * kTileBytes);     // [S][kChunkHist]
+  unsigned char* hdr = smem_raw + (size_t)S * (kTileBytes + kChunkHist * 4);
+  uint64_t* full = reinterpret_cast<uint64_t*>(hdr);  // [kMaxStages]
+  uint64_t* empty = full + kMaxStages;                // [kMaxStages]
+  uint64_t* hand = empty + kMaxStages;                // slot-base hand-off, one phase per tile
+  uint32_t* s_nv = reinterpret_cast<uint32_t*>(hand + 1);  // [kMaxStages] valid players
+  uint32_t* s_b0 = s_nv + kMaxStages;                      // [kMaxStages] first bin of the tile's partition
+  uint32_t* s_b1 = s_b0 + kMaxStages;                      // [kMaxStages] its end bin
+  uint32_t* s_sg = s_b1 + kMaxStages;                      // [kMaxStages] partition
+  uint32_t* s_misc = s_sg + kMaxStages;  // [0] players of the row that stay queued, [1, 2] loaded counter window, [3 + h] tile flags of half h
+  uint32_t* s_wt = s_misc + 8;           // [2][8] warp totals of the histogram-row scan
+  uint32_t* cnt = reinterpret_cast<uint32_t*>(hdr + 256);  // [cnt_cap] slot of the next player of each window bin
+  const uint32_t cnt_cap = place_cnt_cap(a.max_nb);
+  unsigned char* halves = reinterpret_cast<unsigned char*>(cnt + ((cnt_cap + 3) & ~3u));
+  DescCache& dc = *reinterpret_cast<DescCache*>(halves + 2 * kHalfBytes);
+
+  const uint32_t tid = threadIdx.x, lane = tid & 31, h = tid >> 8, ht = tid & 255, hw = ht >> 5;
+  const uint32_t lt_mask = (1u << lane) - 1u;
+  uint32_t* wmask = reinterpret_cast<uint32_t*>(halves + h * kHalfBytes);  // [8][256] match masks (zero between items)
+  uint16_t* wcnt = reinterpret_cast<uint16_t*>(wmask + kHalfWarps * 256);  // [8][256] per-warp digit counters
+  uint32_t* lgd = reinterpret_cast<uint32_t*>(wcnt + kHalfWarps * 256);    // [256] (global slot base - l0) | flag
+  uint32_t* spd = lgd + 256;                                                // [kTile] sorted pos -> tile pos | digit << 11
+  const uint32_t row = blockIdx.x;
+  const uint64_t pol_in = policy_evict_first();
+
+  const uint32_t s0 = row * g.tpr < g.NT ? row * g.tpr : g.NT;
+  const uint32_t s1 = s0 + g.tpr < g.NT ? s0 + g.tpr : g.NT;
+  const uint32_t n_tiles = s1 - s0;
+
+  auto issue = [&](uint32_t stage, uint32_t t) {  // descriptor + the tile's three bulk copies
+    uint32_t phys, nvsg;
+    if (t < kDescCap) { phys = dc.phys[t]; nvsg = dc.nvsg[t]; }
+    else { const TileDesc d = geo_tile(g, a.meta, s0 + t); phys = d.phys; nvsg = d.nvalid | (d.seg << 16); }
+    s_nv[stage] = nvsg & 0xFFFFu;
+    s_sg[stage] = nvsg >> 16;
+    s_b0[stage] = a.seg_bin_lo[nvsg >> 16];
+    s_b1[stage] = a.seg_bin_lo[(nvsg >> 16) + 1];
+    mbar_expect_tx(&full[stage], kTileBytes + kChunkHist * 4);
+    tma_load_1d(ring_ids + (size_t)stage * kTile, a.ids + (size_t)phys * kTile, kTile * 8, &full[stage], pol_in);
+    tma_load_1d(ring_bins + (size_t)stage * kTile, a.bins16 + (size_t)phys * kTile, kTile * 2, &full[stage], pol_in);
+    tma_load_1d(ring_hist + (size_t)stage * kChunkHist, a.meta.chist + (size_t)phys * kChunkHist, kChunkHist * 4,
+                &full[stage], pol_in);
+  };
+
+  if (tid == 0) {
+    for (uint32_t s = 0; s < S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 256); }
+    mbar_init(hand, 256);
+    mbar_fence_init();
+    for (uint32_t i = 0; i < 8; ++i) s_misc[i] = 0;
+  }
+  fence_proxy_async();
+  desc_fill<BLOCK>(dc, g, a.meta, s0, s1);
+  for (uint32_t i = tid; i < 2 * (kHalfWarps * 256 * 6 / 4); i += BLOCK) {  // both halves' match + counter tables
+    const uint32_t hh = i / (kHalfWarps * 256 * 6 / 4), k = i % (kHalfWarps * 256 * 6 / 4);
+    reinterpret_cast<uint32_t*>(halves + hh * kHalfBytes)[k] = 0;
+  }
+  __syncthreads();
+  if (tid == 0)
+    for (uint32_t t = 0; t < S && t < n_tiles; ++t) issue(t, t);
+
+  uint32_t nleft = 0;  // lane 0: players of this warp's positions that stay queued
+  const uint32_t row_p_last = n_tiles ? geo_seg_of(g, s1 - 1) : 0u;
+  const bool scanned = geo_use_colscan(g);  // the column-scan phase ran: P holds the row prefixes
+  for (uint32_t t = h; t < n_tiles; t += 2) {
+    const uint32_t st = t % S, parity = (t / S) & 1u;
+    const uint32_t vbase = (s0 + t) * kTile;  // virtual position of the tile's first player
+    const uint16_t* tb = ring_bins + (size_t)st * kTile;
+    const uint64_t* ti = ring_ids + (size_t)st * kTile;
+    // Tile t-1 has taken its slot bases (so its stage, and every earlier one, has landed); then this tile's stage.
+    if (t) mbar_wait(hand, (t - 1) & 1u);
+    mbar_wait(&full[st], parity);
+    const uint32_t valid = s_nv[st];
+    const uint32_t bin0 = s_b0[st], nb = s_b1[st] - bin0;
+    const uint32_t d = ht;  // this thread's key in the histogram-row steps
+    const uint32_t ch = d < nb ? ring_hist[st * kChunkHist + d] : 0u;
+    const uint32_t lim = ch ? __ldcg(&a.binlim[bin0 + d]) : 0u;
+    uint32_t wb = s_misc[1], we = s_misc[2];
+    if (bin0 < wb || bin0 + nb > we) {
+      // (uniform) the row enters a partition whose slot counters are not loaded: load a window of whole partitions
+      // starting with this one (a row's tiles come in partition order; a row usually spans 1-3 partitions, which fit
+      // at once).  cnt[b - wb] = slot of the (row, b) cell's first player.
+      wb = bin0; we = bin0 + nb;
+      for (uint32_t p = s_sg[st] + 1; p <= row_p_last; ++p) {
+        const uint32_t e = a.seg_bin_lo[p + 1];
+        if (e - wb > cnt_cap) break;
+        we = e;
+      }
+      for (uint32_t i = wb + ht; i < we; i += 256) {
+        uint32_t rlo = 0, rhi = 0, v = 0;
+        if (geo_rows_of(g, a.bin_seg[i], rlo, rhi) && row >= rlo && row <= rhi) {
+          // __ldcg: these arrays are produced earlier in the same (fused) launch by other SMs
+          uint32_t pre = 0;
+          if (scanned) pre = __ldcg(&a.P[(size_t)row * a.Kp + i]);
+          else
+            for (uint32_t r = rlo; r < row; r += 8) {  // few rows per partition; 8 independent L2 loads in flight
+              uint32_t v8[8];
+#pragma unroll
+              for (uint32_t u = 0; u < 8; ++u) v8[u] = r + u < row ? __ldcg(&a.M[(size_t)(r + u) * a.Kp + i]) : 0u;
+#pragma unroll
+              for (uint32_t u = 0; u < 8; ++u) pre += v8[u];
+            }
+          v = __ldcg(&a.outbase[i]) + pre;
+        }
+        cnt[i - wb] = v;
+      }
+      bar_sync_half(h);  // the window is loaded, and every thread of the half has read the old bounds
+      if (ht == 0) { s_misc[1] = wb; s_misc[2] = we; }
+    }
+    uint32_t base = 0;  // global slot of the tile's first player of key d
+    if (d < nb) { base = cnt[bin0 - wb + d]; cnt[bin0 - wb + d] = base + ch; }
+    mbar_arrive(hand);  // tile t+1 may take its slot bases
+
+    uint32_t incl = ch;  // inclusive scan of the histogram row inside the warp; the warp totals cross barrier A
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, incl, off);
+      if (lane >= (uint32_t)off) incl += u;
+    }
+    if (lane == 31) s_wt[h * 8 + hw] = incl;
+
+    // ---------------- rank inside the warp: warp hw owns tile positions 256 hw .. 256 hw + 255 ----------------
+    uint32_t pk[J];  // digit | rank among the warp's players of the digit << 8
+    {
+      uint32_t* wm = wmask + hw * 256;
+      uint16_t* wc = wcnt + hw * 256;
+      uint32_t dg[J];
+#pragma unroll
+      for (int j = 0; j < J; ++j) {
+        const uint32_t pos = hw * (32 * J) + j * 32 + lane;
+        const uint32_t dd = (uint32_t)tb[pos] - bin0;  // digits 0 .. nb-1 live, nb = dead / past the tile's end
+        dg[j] = (pos < valid && dd < nb) ? dd : nb;
+      }
+      const uint32_t lbit = 1u << lane;
+      if (nb > 16) {
+#pragma unroll
+        for (int j = 0; j < J; ++j) {
+          atomicOr(&wm[dg[j]], lbit);
+          __syncwarp();
+          const uint32_t peers = wm[dg[j]];
+          const uint32_t cb = wc[dg[j]];
+          __syncwarp();
+          wm[dg[j]] = 0;
+          wc[dg[j]] = (uint16_t)(cb + __popc(peers));
+          __syncwarp();
+          pk[j] = dg[j] | ((cb + __popc(peers & lt_mask)) << 8);
+        }
+      } else {  // a handful of keys (arrival order: one per partition): peers from <= 5 ballots
+        const uint32_t nbits = 32u - __clz(nb);
+#pragma unroll
+        for (int j = 0; j < J; ++j) {
+          uint32_t peers = 0xFFFFFFFFu;
+#pragma unroll
+          for (uint32_t bit = 0; bit < 5; ++bit)
+            if (bit < nbits) {
+              const bool on = (dg[j] >> bit) & 1u;
+              const uint32_t bal = __ballot_sync(0xFFFFFFFFu, on);
+              peers &= on ? bal : ~bal;
+            }
+          const uint32_t cb = wc[dg[j]];
+          __syncwarp();
+          wc[dg[j]] = (uint16_t)(cb + __popc(peers));
+          __syncwarp();
+          pk[j] = dg[j] | ((cb + __popc(peers & lt_mask)) << 8);
+        }
+      }
+    }
+    bar_sync_half(h);  // A: per-warp digit counts and histogram-row warp totals complete
+
+    uint32_t n_live = 0, l0 = 0;
+#pragma unroll
+    for (uint32_t w = 0; w < kHalfWarps; ++w) {
+      const uint32_t v = s_wt[h * 8 + w];
+      if (w < hw) l0 += v;
+      n_live += v;
+    }
+    l0 += incl - ch;  // tile-local sorted position of the first player of key d
+    uint32_t run = l0;
+#pragma unroll
+    for (uint32_t w = 0; w < kHalfWarps; ++w) {  // column scan: warp w's first sorted position of key d
+      const uint32_t c = wcnt[w * 256 + d];
+      wcnt[w * 256 + d] = (uint16_t)run;
+      run += c;
+    }
+    const bool bad = d < nb && run - l0 != ch;  // the ranked count of key d differs from the chunk histogram
+    const bool fl = ch != 0 && base + ch > lim;  // some player of the cell is past the key's matched prefix
+    if (d < nb) lgd[d] = ((base - l0) & 0x7FFFFFFFu) | (fl ? 0x80000000u : 0u);
+    if (fl || bad) atomicOr(&s_misc[3 + h], (fl ? 1u : 0u) | (bad ? 2u : 0u));
+    bar_sync_half(h);  // B: run bases, slot bases and tile flags are complete
+
+    const uint32_t tf = s_misc[3 + h];  // (uniform over the half)
+    uint32_t lmask = 0;  // bit j: my j-th player stays queued
+    if (!(tf & 2u)) {
+#pragma unroll
+      for (int j = 0; j < J; ++j) {
+        const uint32_t dj = pk[j] & 0xFFu;
+        if (dj < nb) {
+          const uint32_t pos = hw * (32 * J) + j * 32 + lane;
+          const uint32_t lpos = wcnt[hw * 256 + dj] + (pk[j] >> 8);
+          bool matched = true;
+          if ((tf & 1u) || a.src_idx) {
+            const uint32_t e = lgd[dj];
+            const uint32_t slot = (e + lpos) & 0x7FFFFFFFu;
+            if (e >> 31) matched = slot < __ldcg(&a.binlim[bin0 + dj]);
+            if (matched && a.src_idx) a.src_idx[slot] = vbase + pos;
+          }
+          // sorted position -> (tile position, digit); 255 = stays queued.  The ids stay where the TMA put them.
+          spd[lpos] = pos | ((matched ? dj : 255u) << 11);
+          if (!matched) lmask |= 1u << j;
+        }
+      }
+    }
+    {  // left_bits: the warp owns 256 consecutive positions = 8 words; lane j stores word j
+      uint32_t mine = 0, all = 0;
+      if (tf & 1u) {
+#pragma unroll
+        for (int j = 0; j < J; ++j) {
+          const uint32_t wv = __ballot_sync(0xFFFFFFFFu, (lmask >> j) & 1u);
+          if (lane == (uint32_t)j) mine = wv;
+          all += __popc(wv);
+        }
+      }
+      if (lane < (uint32_t)J) a.left_bits[(vbase >> 5) + hw * J + lane] = mine;
+      if (lane == 0) nleft += all;
+    }
+    __syncwarp();  // the warp's counter row is read: all-zero again for the half's next tile (only this warp uses it)
+    reinterpret_cast<uint4*>(wcnt + hw * 256)[lane] = make_uint4(0, 0, 0, 0);
+    bar_sync_half(h);  // C: the sorted order of the tile is staged
+    if (ht == 0) {
+      s_misc[3 + h] = 0;
+      if (tf & 2u) atomicAdd(&a.ctr->chist_bad, 1u);
+    }
+    if (!(tf & 2u)) {
+#pragma unroll
+      for (int i = 0; i < J; ++i) {
+        const uint32_t k = i * 256 + ht;
+        if (k < n_live) {
+          const uint32_t v = spd[k], dk = v >> 11;
+          if (dk != 255u) a.members[(lgd[dk] + k) & 0x7FFFFFFFu] = ti[v & 0x7FFu];
+        }
+      }
+    }
+    mbar_arrive(&empty[st]);  // this half is done with stage st
+    if (ht == 0 && t + S < n_tiles) {
+      mbar_wait(&empty[st], parity);
+      issue(st, t + S);
+    }
+  }
+
+  if (lane == 0 && nleft) atomicAdd(&s_misc[0], nleft);
+  __syncthreads();
+  if (tid == 0) {
+    a.rescnt[row] = s_misc[0];  // players of this row that stay queued
+    for (uint32_t s = 0; s < S; ++s) { mbar_inval(&full[s]); mbar_inval(&empty[s]); }
+    mbar_inval(hand);
+  }
+}
+
 template <int BLOCK>
 __device__ __forceinline__ void place_body(unsigned char* smem_raw, const Geo& g, const PlaceArgs a) {
   static_assert(BLOCK == 512 && kTile == 2048, "tile arrangement is written for 512 threads x 4 players");
+  if (a.meta.chist && a.fast_ok) {  // (uniform) every partition has <= 255 keys
+    place_halves<BLOCK>(smem_raw, g, a);
+    return;
+  }
   constexpr int J = kTile / BLOCK;
   constexpr int NW = BLOCK / 32;
   const uint32_t stages = a.stages, K = a.K, Kp = a.Kp;
