@@ -40,6 +40,7 @@ struct mm_engine {
   std::mutex mu;
   int device = 0;
   int n_sms = 0;
+  int clock_khz = 0;  // peak SM clock (MM_TRACE: placement stall cycles -> µs)
   size_t smem_optin = 0, smem_sm = 0;
   cudaStream_t stream = nullptr;
   bool own_stream = true;
@@ -87,7 +88,7 @@ struct mm_engine {
 
   // tick scratch
   uint32_t R = 0;        // row CTAs of a tick
-  uint32_t helpers = 0;  // extra CTAs of the fused launch: the tail, then the lobby headers
+  uint32_t helpers = 0;  // extra CTAs of the fused launch: the tail, then the compacted pool's chunk histograms
   int rows_per_sm = 2;
   int rank_impl = 3;           // 3 = ballot tile sort for partitions of <= 255 bins + lists otherwise; 2 = lists only
   uint32_t place_stages = 0;
@@ -515,8 +516,8 @@ TailArgs tail_args(mm_engine* e) {
 // tiles per row at least; the tile count is bounded from the host-side player count.
 uint32_t tick_rows(const mm_engine* e) {
   const uint64_t tiles = (uint64_t)e->pool[e->cur].n / kTile + e->n_segs;
-  // the lobby headers (one per L players, written by the helper CTAs while the rows place) are ~0.14 / L of the
-  // placement work: small lobbies get more helpers, at the rows' expense
+  // helper CTAs run the tail beside the rows' histograms and clear the compacted pool's chunk histograms; the rows
+  // write the lobby headers after placing (headers_claimed).  Small lobbies keep more helpers, at the rows' expense
   const uint32_t total = e->R + e->helpers;
   const uint32_t want = std::min(32u, std::max(e->helpers, (total * 14 / 100 + e->min_L - 1) / e->min_L));
   return (uint32_t)std::min<uint64_t>(total - want, std::max<uint64_t>(1, (tiles + 1) / 2));
@@ -618,10 +619,16 @@ int tick_commit(mm_engine* e, uint32_t n, mm_tick_stats* stats) {
     st.scan_us = (float)(c.t[2] - c.t[1]) * 1e-3f;
     st.place_us = (float)(c.t[3] - c.t[2]) * 1e-3f;
     st.epilogue_us = (float)(c.t[6] - c.t[3]) * 1e-3f;  // until the last CTA is done
-    if (std::getenv("MM_TRACE"))
-      std::fprintf(stderr, "[mm] t0=0 rows_p1_done=%.1f tail_done=%.1f bar1=%.1f place_start=%.1f rows_place_done=%.1f bar2=%.1f end=%.1f us\n",
+    if (std::getenv("MM_TRACE")) {
+      // placement stalls: per half, averaged over the rows, at the device's peak SM clock
+      const double us = 1e3 / ((double)e->clock_khz * tick_rows(e));
+      std::fprintf(stderr, "[mm] t0=0 rows_p1_done=%.1f tail_done=%.1f bar1=%.1f place_start=%.1f rows_place_done=%.1f bar2=%.1f end=%.1f us"
+                   " | place stall/row hand full empty loop: h0 %.1f %.1f %.1f %.1f h1 %.1f %.1f %.1f %.1f us\n",
                    (c.t[8] - c.t[0]) * 1e-3, (c.t[5] - c.t[0]) * 1e-3, (c.t[1] - c.t[0]) * 1e-3, (c.t[2] - c.t[0]) * 1e-3,
-                   (c.t[10] - c.t[0]) * 1e-3, (c.t[3] - c.t[0]) * 1e-3, (c.t[6] - c.t[0]) * 1e-3);
+                   (c.t[10] - c.t[0]) * 1e-3, (c.t[3] - c.t[0]) * 1e-3, (c.t[6] - c.t[0]) * 1e-3,
+                   c.stall[0][0] * us, c.stall[0][1] * us, c.stall[0][2] * us, c.stall[0][3] * us,
+                   c.stall[1][0] * us, c.stall[1][1] * us, c.stall[1][2] * us, c.stall[1][3] * us);
+    }
   } else {
     CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[1]));
     st.hist_us = ms * 1000.f;
@@ -778,6 +785,7 @@ int mm_create(const mm_config* cfg, mm_engine** out) {
   cudaDeviceProp prop{};
   if (cudaGetDeviceProperties(&prop, e->device) != cudaSuccess) return bail(MM_E_CUDA);
   e->n_sms = prop.multiProcessorCount;
+  if (cudaDeviceGetAttribute(&e->clock_khz, cudaDevAttrClockRate, e->device) != cudaSuccess) return bail(MM_E_CUDA);
   e->smem_optin = prop.sharedMemPerBlockOptin;
   e->smem_sm = prop.sharedMemPerMultiprocessor;
   if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess) return bail(MM_E_CUDA);

@@ -62,17 +62,41 @@ __device__ __forceinline__ void headers_body(const Geo& g, const EpiArgs& a, con
     }
   }
 }
-// segment tables the headers need, into shared memory (helper CTAs of the fused tick)
+// Lobby headers in chunks of kHdrChunk lobbies, claimed from *next by whichever CTA asks (row CTAs of the fused tick
+// once they have placed their tiles): the rows that finish first write them, and no CTA that shares an SM with a
+// placing row streams stores beside it for the whole phase.  (With emission order asked for, the epilogue writes the
+// headers: emit_seq needs every row's src_idx.)
+constexpr uint32_t kHdrChunk = 8192;
 template <int BLOCK>
-__device__ __forceinline__ void headers_only(uint32_t* scratch, const Geo& g, const EpiArgs& a, uint32_t part, uint32_t nparts) {
+__device__ __forceinline__ void headers_claimed(uint32_t* scratch, const EpiArgs& a, uint32_t* next) {
   uint32_t* s_lbase = scratch;                 // [kMaxSegs + 1]
   uint32_t* s_mbase = s_lbase + kMaxSegs + 1;  // [kMaxSegs]
   uint32_t* s_L = s_mbase + kMaxSegs;          // [kMaxSegs]
-  for (uint32_t s = threadIdx.x; s < a.n_segs; s += BLOCK) {
+  uint32_t* s_claim = s_L + kMaxSegs;
+  const uint32_t tid = threadIdx.x, n_segs = a.n_segs, n_groups = a.n_groups;
+  const uint32_t total_lob = __ldcg(&a.ctr->n_lobbies);
+  for (uint32_t s = tid; s < n_segs; s += BLOCK) {
     s_lbase[s] = __ldcg(&a.seg[s].lobby_base); s_mbase[s] = __ldcg(&a.seg[s].member_base); s_L[s] = a.seg_L[s];
   }
-  __syncthreads();
-  headers_body<BLOCK>(g, a, s_lbase, s_mbase, s_L, part, nparts);
+  for (;;) {
+    if (tid == 0) *s_claim = atomicAdd(next, 1u);
+    __syncthreads();  // the claim and (first pass) the segment tables are visible
+    const uint32_t c0 = *s_claim * kHdrChunk;
+    __syncthreads();  // everyone has read the claim before thread 0 overwrites it
+    if (c0 >= total_lob) break;
+    const uint32_t c1 = c0 + kHdrChunk < total_lob ? c0 + kHdrChunk : total_lob;
+    for (uint32_t c = c0 + tid; c < c1; c += BLOCK) {
+      uint32_t lo = 0, hi = n_segs;  // segment of lobby c: the last sg with s_lbase[sg] <= c (empty ones share a base)
+      while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (s_lbase[mid] <= c) lo = mid; else hi = mid; }
+      mm_lobby_hdr h;
+      h.n_members = (uint16_t)s_L[lo];
+      const uint32_t cut = a.part_cut[lo];
+      h.mode = (uint8_t)(cut / n_groups);
+      h.group = (uint8_t)(cut % n_groups);
+      h.first_member = s_mbase[lo] + (c - s_lbase[lo]) * s_L[lo];
+      a.hdr[c] = h;
+    }
+  }
 }
 
 template <int BLOCK>

@@ -51,8 +51,9 @@ __global__ void __launch_bounds__(BLOCK, 2)
 //   rows: histogram of their tiles      || helper 0: the tail (bin totals are resident, kept
 //         (TMA ring of bin tiles)       ||   current by ingest / remove / the previous tick)         | barrier 1
 //   [only when a partition spans many rows: column scan of M by all CTAs                            | barrier 1b]
-//   rows: placement (TMA ring of bin/id tiles, tile sort, sector-complete stores)
-//                                       || helpers: lobby headers                                   | barrier 2
+//   rows: placement (TMA ring of bin/id tiles, tile sort, sector-complete stores), then lobby headers
+//         in chunks claimed by the rows that finish first
+//                                       || helpers: clear the compacted pool's chunk histograms     | barrier 2
 //   all:  pool compaction by leftover rank (+ headers here when emission order was asked for)
 // ---------------------------------------------------------------------------------------
 struct TickArgs {
@@ -125,7 +126,7 @@ __global__ void __launch_bounds__(BLOCK, 2) k_tick(const TickArgs a) {
     const size_t words = (size_t)__ldcg(a.epi.dst_meta.bump) * kChunkHist;
     for (size_t i = (size_t)part * BLOCK + threadIdx.x; i < words; i += (size_t)nparts * BLOCK) a.epi.dst_meta.chist[i] = 0;
   }
-  if (!is_row && !a.epi.write_headers) headers_only<BLOCK>(scratch, geo, a.epi, helper, n_helpers);
+  if (is_row && !a.epi.write_headers) headers_claimed<BLOCK>(scratch, a.epi, &ctr->hdr_next);
   grid_barrier(&ctr->gbar, (bar += G));
   stamp(3);
   epilogue_body<BLOCK>(scratch, geo, a.epi, &ctr->t[7]);
@@ -137,8 +138,9 @@ __global__ void __launch_bounds__(BLOCK, 2) k_tick(const TickArgs a) {
     __threadfence();
     if (atomicAdd(&ctr->done, 1u) == G - 1) {  // ... and arms the other counter block for the next tick
       TickCtr* nx = a.next_ctr;
-      nx->gbar = 0; nx->done = 0; nx->chist_bad = 0;
+      nx->gbar = 0; nx->done = 0; nx->chist_bad = 0; nx->hdr_next = 0;
       nx->t[6] = 0; nx->t[7] = 0; nx->t[8] = 0; nx->t[10] = 0;
+      for (int i = 0; i < 8; ++i) nx->stall[i / 4][i % 4] = 0;
     }
   }
 }

@@ -45,11 +45,12 @@ __host__ __device__ constexpr uint32_t place_cnt_cap(uint32_t max_nb) { return (
 // lgd[256] | spd[kTile]; every ring stage also carries the chunk's 1 KB histogram row.
 constexpr uint32_t kHalfWarps = 8;
 constexpr uint32_t kHalfBytes = kHalfWarps * 256 * 4 + kHalfWarps * 256 * 2 + 256 * 4 + kTile * 4;
+constexpr uint32_t kHalvesHdr = 288;  // mbarriers, tile descriptors, flags, warp totals, stall counters
 __host__ __device__ constexpr size_t place_smem_whole(uint32_t max_nb, uint32_t stages) {
   return (size_t)stages * kTileBytes + 128 + (size_t)((place_cnt_cap(max_nb) + 3) & ~3u) * 4 + kPlaceUnionBytes + sizeof(DescCache) + 16;
 }
 __host__ __device__ constexpr size_t place_smem_halves(uint32_t max_nb, uint32_t stages) {
-  return (size_t)stages * (kTileBytes + kChunkHist * 4) + 256 + (size_t)((place_cnt_cap(max_nb) + 3) & ~3u) * 4 +
+  return (size_t)stages * (kTileBytes + kChunkHist * 4) + kHalvesHdr + (size_t)((place_cnt_cap(max_nb) + 3) & ~3u) * 4 +
          2 * kHalfBytes + sizeof(DescCache) + 16;
 }
 // max_nb <= kFastBins: the pool has chunk histograms and places on the two-pipeline path (or, with rank_impl = 2, on
@@ -111,7 +112,8 @@ __device__ __forceinline__ void place_halves(unsigned char* smem_raw, const Geo&
   uint32_t* s_sg = s_b1 + kMaxStages;                      // [kMaxStages] partition
   uint32_t* s_misc = s_sg + kMaxStages;  // [0] players of the row that stay queued, [1, 2] loaded counter window, [3 + h] tile flags of half h
   uint32_t* s_wt = s_misc + 8;           // [2][8] warp totals of the histogram-row scan
-  uint32_t* cnt = reinterpret_cast<uint32_t*>(hdr + 256);  // [cnt_cap] slot of the next player of each window bin
+  uint32_t* s_ck = s_wt + 16;            // [2][4] stall counters of half h (cycles): hand, full, empty waits; loop
+  uint32_t* cnt = reinterpret_cast<uint32_t*>(hdr + kHalvesHdr);  // [cnt_cap] slot of the next player of each window bin
   const uint32_t cnt_cap = place_cnt_cap(a.max_nb);
   unsigned char* halves = reinterpret_cast<unsigned char*>(cnt + ((cnt_cap + 3) & ~3u));
   DescCache& dc = *reinterpret_cast<DescCache*>(halves + 2 * kHalfBytes);
@@ -148,7 +150,7 @@ __device__ __forceinline__ void place_halves(unsigned char* smem_raw, const Geo&
     for (uint32_t s = 0; s < S; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 256); }
     mbar_init(hand, 256);
     mbar_fence_init();
-    for (uint32_t i = 0; i < 8; ++i) s_misc[i] = 0;
+    for (uint32_t i = 0; i < 8; ++i) { s_misc[i] = 0; s_ck[i] = 0; }
   }
   fence_proxy_async();
   desc_fill<BLOCK>(dc, g, a.meta, s0, s1);
@@ -163,14 +165,19 @@ __device__ __forceinline__ void place_halves(unsigned char* smem_raw, const Geo&
   uint32_t nleft = 0;  // lane 0: players of this warp's positions that stay queued
   const uint32_t row_p_last = n_tiles ? geo_seg_of(g, s1 - 1) : 0u;
   const bool scanned = geo_use_colscan(g);  // the column-scan phase ran: P holds the row prefixes
+  uint32_t* ck = s_ck + 4 * h;  // thread 0 of the half: stall counters, see TickCtr::stall
+  if (ht == 0) ck[3] = (uint32_t)clock();
   for (uint32_t t = h; t < n_tiles; t += 2) {
     const uint32_t st = t % S, parity = (t / S) & 1u;
     const uint32_t vbase = (s0 + t) * kTile;  // virtual position of the tile's first player
     const uint16_t* tb = ring_bins + (size_t)st * kTile;
     const uint64_t* ti = ring_ids + (size_t)st * kTile;
     // Tile t-1 has taken its slot bases (so its stage, and every earlier one, has landed); then this tile's stage.
+    const uint32_t ck0 = (uint32_t)clock();
     if (t) mbar_wait(hand, (t - 1) & 1u);
+    const uint32_t ck1 = (uint32_t)clock();
     mbar_wait(&full[st], parity);
+    if (ht == 0) { ck[0] += ck1 - ck0; ck[1] += (uint32_t)clock() - ck1; }
     const uint32_t valid = s_nv[st];
     const uint32_t bin0 = s_b0[st], nb = s_b1[st] - bin0;
     const uint32_t d = ht;  // this thread's key in the histogram-row steps
@@ -343,9 +350,15 @@ __device__ __forceinline__ void place_halves(unsigned char* smem_raw, const Geo&
     }
     mbar_arrive(&empty[st]);  // this half is done with stage st
     if (ht == 0 && t + S < n_tiles) {
+      const uint32_t ck2 = (uint32_t)clock();
       mbar_wait(&empty[st], parity);
+      ck[2] += (uint32_t)clock() - ck2;
       issue(st, t + S);
     }
+  }
+  if (ht == 0) {
+    ck[3] = (uint32_t)clock() - ck[3];
+    for (uint32_t k = 0; k < 4; ++k) atomicAdd(&a.ctr->stall[h][k], (unsigned long long)ck[k]);
   }
 
   if (lane == 0 && nleft) atomicAdd(&s_misc[0], nleft);
