@@ -204,7 +204,9 @@ int mm_active_size(mm_engine* e, uint32_t* n_ids);
  * number (players offered by earlier calls) + i) of the member whose arrival
  * completed it: sorting lobbies by emit_seq reproduces the serialized reference's
  * emission order in ORDER_ARRIVAL.
- * MM_E_CAP if lobby_cap / member_cap are too small (nothing is consumed).           */
+ * MM_E_CAP if lobby_cap / member_cap are too small (nothing is consumed).
+ * now: the caller's clock, in the unit of the enq_ts stamps; it changes no result and is what mm_queue_stats
+ * measures the matched players' waits against.                                        */
 int mm_tick(mm_engine* e, uint64_t now, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
             uint64_t* member_ids, uint64_t member_cap, uint32_t* emit_seq,
             mm_tick_stats* stats);
@@ -234,6 +236,41 @@ int mm_results_device(mm_engine* e, const mm_lobby_hdr** d_lobbies,
  * queue-depth report (search/worker.ex:326-334).                                    */
 int mm_pool_read(mm_engine* e, uint32_t cap, uint64_t* id, int32_t* rating, uint8_t* mode,
                  uint8_t* team_size, uint32_t* enq_ts, uint32_t* n_out);
+
+/* ---- per-queue status ----------------------------------------------------------
+ * Replaces Search.Worker.status/0's queue depth (search/worker.ex:115-117,326-334: AMQP.Queue.status of the group's
+ * queue) for the players the engine holds, plus what the reference stamps and never reads (created_at,
+ * models/active_user.ex:47): how long they have waited.
+ *
+ * WAIT of a slot: w = (int32_t)((uint32_t)now - enq_ts), negative values clamped to 0.  The caller stamps enq_ts
+ * (mm_enqueue*) and passes now (mm_tick*, mm_queue_stats) in one clock and unit; waits wrap modulo 2^32 and a stamp
+ * "in the future" reads as 0.
+ * BUCKET of a wait: w itself for w < 8; else, with e = 31 - clz(w) (3 <= e <= 30) and s = (w >> (e - 2)) & 3,
+ * bucket 8 + 4 (e - 3) + s, which holds the waits [(4 + s) << (e - 2), (5 + s) << (e - 2)).  Four sub-buckets per
+ * octave, at most 25 % relative width; bucket 119 ends at 2^31.  Buckets 0..7 = {0}..{7}, 8 = [8, 10), 11 = [14, 16),
+ * 12 = [16, 20), 119 = [7 * 2^28, 2^31).                                                                        */
+#define MM_WAIT_BUCKETS 120u
+
+typedef struct mm_queue_stat {
+  uint8_t mode, group;
+  uint16_t reserved;
+  /* the resident pool at `now` */
+  uint32_t n_waiting;  /* live queued players of this (mode, group)                                     */
+  uint32_t n_removed;  /* entries removed (mm_remove / mm_take) while queued; the next tick drops them    */
+  uint32_t max_wait;   /* longest wait among the n_waiting players (0 if none)                          */
+  uint32_t wait_hist[MM_WAIT_BUCKETS];
+  /* the players the LAST tick matched, at that tick's `now` (all zero before the first tick, after a tick that
+     failed, e.g. with MM_E_CAP, and after mm_restore) */
+  uint32_t n_lobbies, n_matched, max_match_wait;
+  uint32_t match_wait_hist[MM_WAIT_BUCKETS];
+} mm_queue_stat; /* 988 bytes */
+
+/* One record per (mode, group) queue, empty ones included, in mode * n_groups + group order: *n_out = n_modes *
+ * n_groups.  MM_E_CAP (and *n_out = the count needed) if cap is smaller.  One pass over the resident mode and
+ * enqueue-stamp columns on the device (and, for the match section, over the pool buffer the last tick read, which no
+ * call writes until the next tick); only the records cross PCIe.  Runs on the engine's stream and leaves pending
+ * async_results copies alone.                                                                                     */
+int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap, uint32_t* n_out);
 
 /* Device-side snapshot / restore of pool + active set (ram_copies analogue,
  * models/active_user.ex:20; used by bench.py to replay one pool K times).          */

@@ -108,17 +108,19 @@ static ERL_NIF_TERM nif_tick(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]
   return enif_make_tuple4(env, atom(env, "ok"), enif_make_binary(env, &lob), enif_make_binary(env, &mem), stats);
 }
 
-/* enqueue_packed(ref, handles :: binary(u32[]), keys :: binary(u16[])) -> {:ok, accepted :: binary}   (6 B per player) */
+/* enqueue_packed(ref, handles :: binary(u32[]), keys :: binary(u16[]) [, enq_ts :: binary(u32[])])
+ *   -> {:ok, accepted :: binary}   (6 B per player, 10 with the enqueue stamps mm_queue_stats measures waits from) */
 static ERL_NIF_TERM nif_enqueue_packed(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
-  engine_res* r; ErlNifBinary hs, ks;
-  (void)argc;
+  engine_res* r; ErlNifBinary hs, ks, ts;
   if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &hs) ||
       !enif_inspect_binary(env, argv[2], &ks) || hs.size != 2 * ks.size)
     return enif_make_badarg(env);
   size_t n = ks.size / 2;
+  if (argc == 4 && (!enif_inspect_binary(env, argv[3], &ts) || ts.size != 4 * n)) return enif_make_badarg(env);
   ERL_NIF_TERM out;
   unsigned char* acc = enif_make_new_binary(env, n, &out);
-  int rc = mm_enqueue_packed(r->e, (uint32_t)n, (const uint32_t*)hs.data, (const uint16_t*)ks.data, NULL, acc);
+  int rc = mm_enqueue_packed(r->e, (uint32_t)n, (const uint32_t*)hs.data, (const uint16_t*)ks.data,
+                             argc == 4 ? (const uint32_t*)ts.data : NULL, acc);
   return rc ? err(env, rc) : enif_make_tuple2(env, atom(env, "ok"), out);
 }
 
@@ -165,6 +167,21 @@ static ERL_NIF_TERM nif_status(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv
   return enif_make_tuple2(env, atom(env, "ok"), m);
 }
 
+/* queue_stats(ref, now_ms) -> {:ok, records :: binary(mm_queue_stat[])}: one 988-byte record per (mode, group) queue,
+ * mode * n_groups + group order — Search.Worker.status/0's per-queue depth plus wait histograms */
+static ERL_NIF_TERM nif_queue_stats(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifUInt64 now; uint32_t n = 0; mm_queue_stat probe;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_uint64(env, argv[1], &now))
+    return enif_make_badarg(env);
+  int rc = mm_queue_stats(r->e, now, &probe, 0, &n);  /* MM_E_CAP: n = records needed */
+  if (rc != MM_E_CAP) return err(env, rc ? rc : MM_E_STATE);
+  ERL_NIF_TERM out;
+  unsigned char* buf = enif_make_new_binary(env, (size_t)n * sizeof(mm_queue_stat), &out);
+  rc = mm_queue_stats(r->e, now, (mm_queue_stat*)buf, n, &n);
+  return rc ? err(env, rc) : enif_make_tuple2(env, atom(env, "ok"), out);
+}
+
 /* set_max_spread(ref, w): extension knob (strategist policy S1); w < 0 restores the reference behaviour */
 static ERL_NIF_TERM nif_set_max_spread(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
   engine_res* r; ErlNifSInt64 w = -1;
@@ -182,9 +199,11 @@ static ErlNifFunc funcs[] = {
   {"in_queue?", 2, nif_in_queue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"tick", 2, nif_tick, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"enqueue_packed", 3, nif_enqueue_packed, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"enqueue_packed", 4, nif_enqueue_packed, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"remove_packed", 2, nif_remove_packed, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"tick_packed", 2, nif_tick_packed, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"status", 1, nif_status, 0},
+  {"queue_stats", 2, nif_queue_stats, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"set_max_spread", 2, nif_set_max_spread, 0},
 };
 ERL_NIF_INIT(Elixir.Matchmaking.Search.Engine, funcs, load, NULL, NULL, NULL)

@@ -46,12 +46,16 @@ defmodule Matchmaking.Search.Engine do
   def remove(_ref, _ids), do: :erlang.nif_error(:nif_not_loaded)
   @doc "Dense-handle engines: handles :: binary(u32[]), keys :: binary(u16[] = mode <<< 13 ||| rating) -> {:ok, codes}"
   def enqueue_packed(_ref, _handles, _keys), do: :erlang.nif_error(:nif_not_loaded)
+  @doc "Same, with enq_ts :: binary(u32[]): the enqueue stamps queue_stats/2 measures waits from (the pool's clock)"
+  def enqueue_packed(_ref, _handles, _keys, _enq_ts), do: :erlang.nif_error(:nif_not_loaded)
   def remove_packed(_ref, _handles), do: :erlang.nif_error(:nif_not_loaded)
   @doc "-> {:ok, lobbies :: binary(mm_lobby_hdr[]), member_handles :: binary(u32[]), stats}"
   def tick_packed(_ref, _now_ms), do: :erlang.nif_error(:nif_not_loaded)
   def in_queue?(_ref, _id), do: :erlang.nif_error(:nif_not_loaded)
   def tick(_ref, _now_ms), do: :erlang.nif_error(:nif_not_loaded)
   def status(_ref), do: :erlang.nif_error(:nif_not_loaded)
+  @doc "-> {:ok, binary(mm_queue_stat[])}: per (mode, group) queue, waiting players and wait histograms (include/mm_engine.h)"
+  def queue_stats(_ref, _now_ms), do: :erlang.nif_error(:nif_not_loaded)
 
   @doc "Extension (not reference behaviour): maximum rating spread of a lobby for the following ticks; < 0 = off."
   def set_max_spread(_ref, _w), do: :erlang.nif_error(:nif_not_loaded)

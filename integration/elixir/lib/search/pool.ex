@@ -10,6 +10,11 @@ defmodule Matchmaking.Search.Pool do
       :tick          Engine.tick_packed -> one AMQP message per lobby with the payload and the publish options of
                      search/worker.ex:250-261,315-319
       in_queue?/1, remove_user/1    replace Matchmaking.Model.ActiveUser (models/active_user.ex:33-66)
+      queue_status/1 one rating group's queues (Engine.queue_stats): waiting players, oldest / p50 / p99 wait, the
+                     last tick's matched players and p99 wait at match, in ms — Search.Worker.status/0's queue depth
+
+  Every batch is stamped with the pool's clock (ms since the pool started, modulo 2^32) and every tick passes the same
+  clock as its `now`, so the engine's waits are in milliseconds.
 
   Player ids are UUID strings (models/active_user.ex:7); the device stores a dense 32-bit handle
   (MM_F_DENSE_IDS).  The id <-> handle table lives here, handles are recycled when a player leaves — no hashing, so
@@ -31,6 +36,7 @@ defmodule Matchmaking.Search.Pool do
   def stage(player, game_mode, rating, ack_ref), do: GenServer.cast(__MODULE__, {:stage, player, game_mode, rating, ack_ref})
   def in_queue?(player_id), do: GenServer.call(__MODULE__, {:in_queue?, player_id})
   def remove_user(player_id), do: GenServer.call(__MODULE__, {:remove_user, player_id})
+  def queue_status(group_index), do: GenServer.call(__MODULE__, {:queue_status, group_index})
 
   @impl true
   def init(opts) do
@@ -38,7 +44,8 @@ defmodule Matchmaking.Search.Pool do
     {:ok, ref} = Engine.new(Engine.pack_config(capacity: capacity, active_capacity: 2 * capacity, dense_ids: true))
     Process.send_after(self(), :flush, @flush_ms)
     Process.send_after(self(), :tick, @tick_ms)
-    {:ok, %{ref: ref, staged: [], n_staged: 0, handle_of: %{}, players: %{}, free: [], next: 0, channel: nil}}
+    {:ok, %{ref: ref, staged: [], n_staged: 0, handle_of: %{}, players: %{}, free: [], next: 0, channel: nil,
+            t0: System.monotonic_time(:millisecond)}}
   end
 
   @impl true
@@ -53,6 +60,21 @@ defmodule Matchmaking.Search.Pool do
     reply = case st.handle_of do
       %{^id => h} -> Engine.in_queue?(st.ref, h)
       _ -> false
+    end
+    {:reply, reply, st}
+  end
+
+  def handle_call({:queue_status, group}, _from, st) do
+    reply = case Engine.queue_stats(st.ref, now_ms(st)) do
+      {:ok, recs} ->
+        for <<mode, g, _::16, waiting::little-32, _removed::little-32, oldest::little-32, hist::binary-size(480),
+              _lobbies::little-32, matched::little-32, _max_match::little-32, mhist::binary-size(480) <- recs>>,
+            g == group, into: %{} do
+          {Engine.mode_name(mode), %{waiting: waiting, oldest_wait_ms: oldest, p50_wait_ms: quantile(hist, 0.5),
+                                     p99_wait_ms: quantile(hist, 0.99), last_tick_matched: matched,
+                                     last_tick_p99_match_wait_ms: quantile(mhist, 0.99)}}
+        end
+      {:error, _} = e -> e
     end
     {:reply, reply, st}
   end
@@ -76,7 +98,7 @@ defmodule Matchmaking.Search.Pool do
   def handle_info(:tick, st) do
     Process.send_after(self(), :tick, @tick_ms)
     st = flush(st)
-    case Engine.tick_packed(st.ref, System.monotonic_time(:millisecond)) do
+    case Engine.tick_packed(st.ref, now_ms(st)) do
       {:ok, lobbies, members, _stats} -> {:noreply, publish(lobbies, members, st)}
       {:error, _reason} -> {:noreply, st}                              # nothing was consumed; the next tick retries
     end
@@ -93,7 +115,9 @@ defmodule Matchmaking.Search.Pool do
     handles = for {h, _, _, _, _, _} <- rows, into: <<>>, do: <<h::little-32>>
     keys = for {_, _, _, m, r, _} <- rows, into: <<>>, do: <<(m * 8192 + r)::little-16>>   # mode << 13 | rating
     st = %{st | staged: [], n_staged: 0}
-    case Engine.enqueue_packed(st.ref, handles, keys) do
+    stamp = now_ms(st)
+    ts = for _ <- rows, into: <<>>, do: <<stamp::little-32>>
+    case Engine.enqueue_packed(st.ref, handles, keys, ts) do
       {:ok, codes} ->
         Enum.zip(:binary.bin_to_list(codes), rows)
         |> Enum.reduce(st, fn
@@ -116,6 +140,20 @@ defmodule Matchmaking.Search.Pool do
     end
   end
   defp release(st, id, h), do: %{st | handle_of: Map.delete(st.handle_of, id), free: [h | st.free]}
+  defp now_ms(st), do: Bitwise.band(System.monotonic_time(:millisecond) - st.t0, 0xFFFFFFFF)
+
+  # upper bound (largest wait) of the bucket holding the q-quantile of a wait histogram (bounds: include/mm_engine.h)
+  defp quantile(hist, q) do
+    counts = for <<c::little-32 <- hist>>, do: c
+    case Enum.sum(counts) do
+      0 -> 0
+      total ->
+        rank = max(1, ceil(q * total))
+        b = counts |> Enum.scan(&+/2) |> Enum.find_index(&(&1 >= rank))
+        if b < 8, do: b, else: Bitwise.bsl(5 + rem(b - 8, 4), div(b - 8, 4) + 1) - 1
+    end
+  end
+
   defp clamp(r) when is_integer(r), do: min(max(r, 0), 8191)
   defp clamp(_), do: 8191                                               # no integer group matches -> default group
 

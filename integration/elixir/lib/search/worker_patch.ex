@@ -19,6 +19,9 @@
     end
   end
 
+  # :115-117, 326-334 — status/0: the broker's queue is nearly always empty (deliveries are acked once resident), so the
+  # group's waiting players come from the engine:  Map.put(status, :waiting, Matchmaking.Search.Pool.queue_status(group))
+
   # application.ex:42-60 — one more child, before the search workers:   {Matchmaking.Search.Pool, []}
   # middleware/worker.ex:65-70 — ActiveUser.in_queue?(id) -> Matchmaking.Search.Pool.in_queue?(id); add_user/1 goes away
   #                             (the enqueue itself answers "already in the queue", code 0)

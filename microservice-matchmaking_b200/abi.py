@@ -72,6 +72,26 @@ class TickStats(C.Structure):
     ]
 
 
+MM_WAIT_BUCKETS = 120
+
+
+class QueueStat(C.Structure):
+    """One (mode, group) queue: the resident pool at `now` and the players the last tick matched (988 bytes)."""
+    _fields_ = [
+        ("mode", C.c_uint8),
+        ("group", C.c_uint8),
+        ("reserved", C.c_uint16),
+        ("n_waiting", C.c_uint32),
+        ("n_removed", C.c_uint32),
+        ("max_wait", C.c_uint32),
+        ("wait_hist", C.c_uint32 * MM_WAIT_BUCKETS),
+        ("n_lobbies", C.c_uint32),
+        ("n_matched", C.c_uint32),
+        ("max_match_wait", C.c_uint32),
+        ("match_wait_hist", C.c_uint32 * MM_WAIT_BUCKETS),
+    ]
+
+
 # every symbol include/mm_engine.h declares: name -> (restype, argtypes)
 _P = C.POINTER
 _vp = C.c_void_p
@@ -98,6 +118,7 @@ PROTOTYPES = {
     "mm_tick_device": (C.c_int, [_vp, C.c_uint64, _P(TickStats)]),
     "mm_results_device": (C.c_int, [_vp, _P(_vp), _P(_vp)]),
     "mm_pool_read": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _P(C.c_uint32)]),
+    "mm_queue_stats": (C.c_int, [_vp, C.c_uint64, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_snapshot": (C.c_int, [_vp]),
     "mm_restore": (C.c_int, [_vp]),
     "mm_set_stream": (C.c_int, [_vp, _vp]),

@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "mm_kernels.cuh"
+#include "mm_stats.cuh"
 
 using namespace mm;
 
@@ -142,6 +143,13 @@ struct mm_engine {
   // last tick
   mm_tick_stats last{};
   bool last_fused = false;
+
+  // mm_queue_stats: the match section reads pool[cur ^ 1] + d_left_bits, which describe the last tick until the next
+  // one starts (its phase A writes the compacted pool's layout into pool[cur ^ 1].m)
+  bool match_valid = false;  // the last tick completed and nothing since has invalidated its section
+  uint32_t tick_now = 0;     // `now` of the tick in progress / the last tick (mod 2^32)
+  uint32_t match_n = 0;      // players resident when that tick started: bounds its tile count
+  uint32_t* d_qstat = nullptr;  // [n_cut] records
 };
 
 namespace {
@@ -642,6 +650,8 @@ int tick_commit(mm_engine* e, uint32_t n, mm_tick_stats* stats) {
   e->gen = next_gen(e);
   e->cur ^= 1;
   e->pool[e->cur].n = c.n_resid;
+  e->match_valid = true;  // pool[cur ^ 1] is now the pool this tick matched
+  e->match_n = n;
   e->last = st;
   if (stats) *stats = st;
   if (c.chist_bad) {  // placement took slot bases from chunk histograms that disagree with the pool: results are wrong
@@ -649,6 +659,13 @@ int tick_commit(mm_engine* e, uint32_t n, mm_tick_stats* stats) {
     return MM_E_STATE;
   }
   return MM_OK;
+}
+
+// Every tick entry point: the tick's `now` is kept for mm_queue_stats, and the last tick's match section is void from
+// here on (a tick that fails after its phase A — MM_E_CAP on the split path — has rewritten pool[cur ^ 1].m).
+void tick_begin(mm_engine* e, uint64_t now) {
+  e->tick_now = (uint32_t)now;
+  e->match_valid = false;
 }
 
 // async_results: the previous tick's host copies must land before its device buffers are overwritten
@@ -881,6 +898,7 @@ int mm_destroy(mm_engine* e) {
   cudaFree(e->d_in_id); cudaFree(e->d_hslot); cudaFree(e->d_in_rating); cudaFree(e->d_in_mode); cudaFree(e->d_code);
   cudaFree(e->d_in_ts); cudaFree(e->d_blocksum); cudaFree(e->d_blockhist); cudaFree(e->d_part); cudaFree(e->d_in_key);
   cudaFree(e->d_in_handle); cudaFree(e->d_rej_idx); cudaFree(e->d_rej_code);
+  cudaFree(e->d_qstat);
   if (e->h_ctr) cudaFreeHost(e->h_ctr);
   if (e->h_small) cudaFreeHost(e->h_small);
   for (auto& ev : e->ev)
@@ -1189,10 +1207,10 @@ int mm_results_wait(mm_engine* e) {
 }
 
 int mm_tick_device(mm_engine* e, uint64_t now, mm_tick_stats* stats) {
-  (void)now;  // strict-parity mode has no time-expanded window (SURVEY F3)
   if (!e) return MM_E_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
   CK(cudaSetDevice(e->device));
+  tick_begin(e, now);
   { int rcw = wait_results(e); if (rcw) return rcw; }
   const uint32_t n = e->pool[e->cur].n;
   e->last_fused = use_fused(e);
@@ -1215,19 +1233,19 @@ int mm_results_device(mm_engine* e, const mm_lobby_hdr** d_lobbies, const uint64
 
 int mm_tick(mm_engine* e, uint64_t now, mm_lobby_hdr* lobbies, uint32_t lobby_cap, uint64_t* member_ids,
             uint64_t member_cap, uint32_t* emit_seq, mm_tick_stats* stats) {
-  (void)now;
   if (!e) return MM_E_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
   CK(cudaSetDevice(e->device));
+  tick_begin(e, now);
   return tick_to_host(e, lobbies, lobby_cap, member_ids, nullptr, member_cap, emit_seq, stats);
 }
 
 int mm_tick_packed(mm_engine* e, uint64_t now, mm_lobby_hdr* lobbies, uint32_t lobby_cap, uint32_t* member_handles,
                    uint64_t member_cap, uint32_t* emit_seq, mm_tick_stats* stats) {
-  (void)now;
   if (!e) return MM_E_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
   CK(cudaSetDevice(e->device));
+  tick_begin(e, now);
   return tick_to_host(e, lobbies, lobby_cap, nullptr, member_handles, member_cap, emit_seq, stats);
 }
 
@@ -1281,6 +1299,41 @@ int mm_pool_read(mm_engine* e, uint32_t cap, uint64_t* id, int32_t* rating, uint
   return MM_OK;
 }
 
+int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap, uint32_t* n_out) {
+  if (!e || !out || !n_out) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const uint32_t n_cut = e->n_cut;
+  *n_out = n_cut;
+  if (cap < n_cut) return MM_E_CAP;
+  CK(cudaSetDevice(e->device));
+  const size_t bytes = (size_t)n_cut * sizeof(mm_queue_stat);
+  if (!e->d_qstat) CK(cudaMalloc(&e->d_qstat, bytes));
+  CK(cudaMemsetAsync(e->d_qstat, 0, bytes, e->stream));
+  StatArgs a{};
+  const Pool& p = e->pool[e->cur];
+  a.sec[0] = StatSection{p.v.mode, p.v.ts, p.m, nullptr, (uint32_t)now};
+  const Pool& q = e->pool[e->cur ^ 1];
+  a.sec[1] = StatSection{q.v.mode, q.v.ts, q.m, e->d_left_bits, e->tick_now};
+  a.n_segs = e->n_segs; a.part_cut = e->d_part_cut; a.out = e->d_qstat;
+  // CTAs: at most the tiles in use (the host-side player counts bound them), at most 8 per SM; each takes a
+  // contiguous run of tiles
+  const uint32_t n_max = std::max(p.n, e->match_valid ? e->match_n : 0u);
+  const uint64_t tiles = (uint64_t)n_max / kTile + e->n_segs;
+  const uint32_t ctas = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(tiles, 8ull * (uint32_t)e->n_sms));
+  k_queue_stats<kStatBlock><<<dim3(ctas, e->match_valid ? 2 : 1), kStatBlock, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out, e->d_qstat, bytes, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  const uint32_t G = e->cfg.n_groups;
+  for (uint32_t c = 0; c < n_cut; ++c) {
+    const mm_mode_desc& md = e->cfg.modes[c / G];
+    out[c].mode = (uint8_t)(c / G);
+    out[c].group = (uint8_t)(c % G);
+    out[c].n_lobbies = out[c].n_matched / ((uint32_t)md.teams * md.team_size);  // whole lobbies of L players
+  }
+  return MM_OK;
+}
+
 int mm_snapshot(mm_engine* e) {
   if (!e) return MM_E_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
@@ -1307,6 +1360,7 @@ int mm_restore(mm_engine* e) {
   if (rc) return rc;
   e->seq_next = e->snap_seq;
   e->gen = next_gen(e);
+  e->match_valid = false;  // the restored pool was not matched by the last tick
   if (e->use_active && p.n) {
     k_restamp<<<dim3(e->n_chunks, e->n_segs), 256, 0, e->stream>>>(p.v, p.m, act_view(e), e->gen);
     CK(cudaGetLastError());

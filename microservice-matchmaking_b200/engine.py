@@ -47,6 +47,53 @@ def _p(a):
 
 LOBBY_DTYPE = np.dtype([("first_member", "<u4"), ("n_members", "<u2"), ("mode", "u1"), ("group", "u1")])
 
+# mm_queue_stat (include/mm_engine.h) as a numpy record
+QUEUE_STAT_DTYPE = np.dtype([
+    ("mode", "u1"), ("group", "u1"), ("reserved", "<u2"),
+    ("n_waiting", "<u4"), ("n_removed", "<u4"), ("max_wait", "<u4"), ("wait_hist", "<u4", (abi.MM_WAIT_BUCKETS,)),
+    ("n_lobbies", "<u4"), ("n_matched", "<u4"), ("max_match_wait", "<u4"),
+    ("match_wait_hist", "<u4", (abi.MM_WAIT_BUCKETS,)),
+])
+
+
+def wait_of(now, enq_ts):
+    """Wait of a player as mm_queue_stats counts it: (now - enq_ts) mod 2^32 read as a signed 32-bit value, negative
+    ("in the future") clamped to 0."""
+    d = (np.asarray(now, np.uint64) - np.asarray(enq_ts, np.uint64)) & np.uint64(0xFFFFFFFF)
+    w = d.astype(np.uint32).view(np.int32) if d.ndim else np.uint32(d).view(np.int32)
+    return np.maximum(w, 0).astype(np.int64)
+
+
+def wait_bucket(w):
+    """Histogram bucket of a wait w in [0, 2^31): w below 8, else 8 + 4 (e - 3) + ((w >> (e - 2)) & 3) with
+    e = floor(log2 w) — four sub-buckets per octave, 120 in all."""
+    w = np.asarray(w, np.int64)
+    e = np.maximum(np.frexp(w.astype(np.float64))[1] - 1, 3)  # floor(log2 w), exact for integers below 2^53
+    b = np.where(w < 8, w, 8 + 4 * (e - 3) + ((w >> (e - 2)) & 3))
+    return b if b.ndim else int(b)
+
+
+def wait_bucket_bounds():
+    """-> (lo, hi) int64[MM_WAIT_BUCKETS]: bucket b holds the waits [lo[b], hi[b]); together [0, 2^31) without gaps."""
+    b = np.arange(abi.MM_WAIT_BUCKETS, dtype=np.int64)
+    e = 3 + (b - 8) // 4
+    s = (b - 8) % 4
+    lo = np.where(b < 8, b, (4 + s) << np.maximum(e - 2, 0))
+    hi = np.where(b < 8, b + 1, (5 + s) << np.maximum(e - 2, 0))
+    return lo, hi
+
+
+def wait_quantile(hist, q):
+    """Upper bound (the largest wait it holds) of the bucket that holds the q-quantile of a wait histogram; 0 for an
+    empty one.  Exact for waits below 8, at most 25 % high above."""
+    hist = np.asarray(hist, np.int64)
+    total = int(hist.sum())
+    if total == 0:
+        return 0
+    rank = min(total, max(1, int(np.ceil(q * total))))
+    b = int(np.searchsorted(np.cumsum(hist), rank))
+    return int(wait_bucket_bounds()[1][b] - 1)
+
 
 class Engine:
     """One GPU-resident player pool + active set + search tick (single writer)."""
@@ -283,6 +330,16 @@ class Engine:
         a, b = C.c_void_p(), C.c_void_p()
         self._check(self.lib.mm_results_device(self.h, C.byref(a), C.byref(b)), "mm_results_device")
         return a.value, b.value
+
+    def queue_stats(self, now=0):
+        """Per-(mode, group) queue status (mm_queue_stats) -> QUEUE_STAT_DTYPE[n_modes * n_groups], record
+        mode * n_groups + group: the pool at `now` and the players the last tick matched at that tick's `now`."""
+        cap = self.cfg.n_modes * self.cfg.n_groups
+        out = np.zeros(cap, QUEUE_STAT_DTYPE)
+        n = C.c_uint32(0)
+        self._check(self.lib.mm_queue_stats(self.h, int(now) & 0xFFFFFFFFFFFFFFFF, _p(out), cap, C.byref(n)),
+                    "mm_queue_stats")
+        return out[:n.value]
 
     def snapshot(self):
         self._check(self.lib.mm_snapshot(self.h), "mm_snapshot")

@@ -144,6 +144,10 @@ class SearchPool:
     delivery is acked only once its player is resident, so the broker must be allowed that many unacked messages);
     flush_every_s: an ingest also happens when the oldest staged delivery has waited this long (and at every tick);
     window: optional WindowSchedule (extension; needs MM_ORDER_RATING); clock: () -> seconds.
+
+    Every ingest batch is stamped with now_ms(), the clock in milliseconds since the pool was created (u32, wraps
+    after 49 days), and every tick passes the same clock as its `now`: the engine's per-queue waits
+    (Engine.queue_stats, SearchWorker.status) are in milliseconds.
     """
 
     def __init__(self, engine, mode_names, group_names, max_batch=65536, window=None, clock=None, flush_every_s=0.005,
@@ -151,6 +155,7 @@ class SearchPool:
         import time
         self.window = window
         self.clock = clock or time.monotonic
+        self._t0 = self.clock()
         self.enqueued_at = {}  # handle -> clock() when the player became resident (insertion = enqueue order)
         self.last_spread = None
         self.engine = engine
@@ -165,6 +170,10 @@ class SearchPool:
         self._staged = []   # (player id, rating, mode, player, worker, tag)
         self._staged_since = None
         self.stats = {"enqueued": 0, "duplicates": 0, "invalid": 0, "lobbies": 0, "failed_batches": 0}
+
+    def now_ms(self):
+        """The pool's clock: milliseconds since the pool was created, modulo 2^32 (the engine's enq_ts / now)."""
+        return int((self.clock() - self._t0) * 1000.0) & 0xFFFFFFFF
 
     # -- models/active_user.ex mirrors ---------------------------------------------------
     def in_queue(self, player_id):  # ActiveUser.in_queue?/1
@@ -207,7 +216,7 @@ class SearchPool:
         rating = np.clip(np.array([s[1] for s in staged], np.int64), -(2 ** 31), 2 ** 31 - 1).astype(np.int32)
         mode = np.array([self.mode_index.get(s[2], 255) if isinstance(s[2], str) else 255 for s in staged], np.uint8)
         try:
-            acc = self.engine.enqueue(ids, rating, mode, None)
+            acc = self.engine.enqueue(ids, rating, mode, np.full(len(staged), self.now_ms(), np.uint32))
         except Exception:                       # nothing was enqueued (mm_enqueue refuses a batch as a whole)
             for pid in fresh:
                 self.handles.release(pid)
@@ -235,9 +244,12 @@ class SearchPool:
         return len(staged)
 
     # -- the tick ---------------------------------------------------------------------------
-    def tick(self, now=0):
-        """One search tick; publishes each lobby like prepare_game_lobby/4. -> lobbies emitted"""
+    def tick(self, now=None):
+        """One search tick; publishes each lobby like prepare_game_lobby/4. -> lobbies emitted.  now: the engine tick's
+        clock (default now_ms(), the clock the ingest stamps)."""
         self.flush()
+        if now is None:
+            now = self.now_ms()
         if self.window:  # the oldest queued player is the first key: dicts keep insertion (= enqueue) order
             oldest = next(iter(self.enqueued_at.values()), None)
             self.last_spread = self.window.spread(self.clock(), oldest)
@@ -261,6 +273,28 @@ class SearchPool:
 
     def _teams_of(self, mode):
         return self.engine.cfg.modes[int(mode)].teams
+
+    def queue_status(self, group_name):
+        """The engine's view of one rating group's queues (Engine.queue_stats at now_ms()), per mode name: players
+        waiting, oldest / p50 / p99 wait, and the last tick's matched players and p99 wait at match, in ms.  Quantiles
+        are the upper bounds of histogram buckets (at most 25 % high).  {} for a group the pool does not know."""
+        from .engine import wait_quantile
+        if group_name not in self.group_names:
+            return {}
+        g = self.group_names.index(group_name)
+        out = {}
+        for r in self.engine.queue_stats(self.now_ms()):
+            if int(r["group"]) != g or int(r["mode"]) >= len(self.mode_names):
+                continue
+            out[self.mode_names[int(r["mode"])]] = {
+                "waiting": int(r["n_waiting"]),
+                "oldest_wait_ms": int(r["max_wait"]),
+                "p50_wait_ms": wait_quantile(r["wait_hist"], 0.50),
+                "p99_wait_ms": wait_quantile(r["wait_hist"], 0.99),
+                "last_tick_matched": int(r["n_matched"]),
+                "last_tick_p99_match_wait_ms": wait_quantile(r["match_wait_hist"], 0.99),
+            }
+        return out
 
 
 class SearchWorker:
@@ -305,6 +339,8 @@ class SearchWorker:
     def status(self):  # worker.ex:115-117, 326-334
         st = dict(self.channel.queue_status(self.config["queue"]["name"]))
         st["pool"] = self.pool.engine.status() if hasattr(self.pool.engine, "status") else {}
+        if hasattr(self.pool.engine, "queue_stats"):  # this worker's own group, per mode (the reference's queue depth)
+            st["waiting"] = self.pool.queue_status(self.group_name)
         return ("ok", st)
 
     def prepare_game_lobby(self, channel_name, exchange_forward, queue_forward, payload):  # worker.ex:250-261
