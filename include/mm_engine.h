@@ -104,10 +104,12 @@ typedef struct mm_tick_stats {
   uint32_t n_dead;        /* removed-while-queued players dropped by this tick         */
   uint32_t n_launches;    /* kernels launched by this tick                             */
   float device_us;        /* CUDA-event time of the whole tick on the engine's stream  */
-  float place_us;         /* CUDA-event time of the dominant (placement) kernel        */
+  float place_us;         /* CUDA-event time of the dominant kernel: placement + pool  */
+                          /* compaction (fused tick: until the last row has compacted) */
   float hist_us;          /* ... of the histogram kernel                               */
   float scan_us;          /* ... of the column-scan kernel                             */
-  float epilogue_us;      /* ... of the epilogue kernel (headers + pool compaction)    */
+  float epilogue_us;      /* ... of the epilogue kernel: lobby headers (fused tick:    */
+                          /* from the end of placement until the last CTA exits)       */
   uint32_t reserved;
 } mm_tick_stats;
 

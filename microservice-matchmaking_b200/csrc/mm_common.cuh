@@ -70,8 +70,11 @@ struct TickCtr {
   uint32_t heavy;  // some bin expects > 8 players per tile: the list ranking uses warp-aggregated nodes
   uint32_t chist_bad;  // placement tiles whose ranked key counts differ from their chunk histogram (must stay 0)
   uint32_t hdr_next;   // fused tick: lobby-header chunks claimed so far (headers_claimed)
-  unsigned long long t[12]; // fused kernel: %globaltimer (ns) at phase boundaries, CTA 0; [6],[7]: max over CTAs;
-                            // [8] last row done with phase 1, [9] min CTA start, [10] last row done placing
+  uint32_t left_bad;   // leftover players whose compacted-pool rank falls outside their partition (must stay 0)
+  uint32_t clr_done;   // fused tick: CTAs done clearing the compacted pool's chunk histograms
+  unsigned long long t[12]; // fused kernel: %globaltimer (ns) at phase boundaries, CTA 0; [3],[6]: max over CTAs;
+                            // [3] last row done placing and compacting, [8] last row done with phase 1,
+                            // [10] last row done placing
   unsigned long long stall[2][4];  // two-pipeline placement, per half, SM clock cycles summed over the rows: waits on
                                    // [0] hand, [1] the tile's loads, [2] a stage's release before a re-issue; [3] tile loop
 };

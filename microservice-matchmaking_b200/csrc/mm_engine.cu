@@ -112,7 +112,6 @@ struct mm_engine {
   mm_lobby_hdr* d_hdr = nullptr;
   uint32_t* d_emit_seq = nullptr;
   uint32_t max_lobbies = 0;
-  uint32_t* d_rescnt = nullptr;
   TickCtr* d_ctr2 = nullptr;  // two counter blocks, used alternately (the fused kernel re-arms the other one)
   TickCtr* d_ctr = nullptr;   // the block of the current / last tick
   int ctr_idx = 0;
@@ -395,10 +394,9 @@ int alloc_tick_scratch(mm_engine* e) {
   if (total > kMaxRows) total = kMaxRows;
   e->helpers = total >= 64 ? 4u : (total > 1 ? 1u : 0u);
   e->R = total - e->helpers;
-  if (e->d_M) { cudaFree(e->d_M); cudaFree(e->d_P); cudaFree(e->d_rescnt); }
+  if (e->d_M) { cudaFree(e->d_M); cudaFree(e->d_P); }
   CK(cudaMalloc(&e->d_M, (size_t)(e->R + 1) * e->Kp * 4));
   CK(cudaMalloc(&e->d_P, (size_t)(e->R + 1) * e->Kp * 4));
-  CK(cudaMalloc(&e->d_rescnt, (size_t)(e->R + 1) * 4));
   return MM_OK;
 }
 
@@ -539,7 +537,7 @@ PlaceArgs place_args(mm_engine* e, bool want_seq) {
   a.seg_bin_lo = e->d_seg_bin_lo; a.bin_seg = e->d_bin_seg; a.M = e->d_M; a.P = e->d_P;
   a.outbase = e->d_outbase; a.binlim = e->d_binlim; a.members = e->d_members;
   a.src_idx = want_seq ? e->d_src_idx : nullptr;
-  a.left_bits = e->d_left_bits; a.rescnt = e->d_rescnt; a.ctr = e->d_ctr;
+  a.left_bits = e->d_left_bits; a.ctr = e->d_ctr;
   return a;
 }
 uint32_t next_gen(const mm_engine* e) { return e->gen >= kGenMask ? 1u : e->gen + 1; }
@@ -547,9 +545,9 @@ EpiArgs epi_args(mm_engine* e, bool want_seq, bool headers) {
   EpiArgs a{};
   a.src = e->pool[e->cur].v; a.dst = e->pool[e->cur ^ 1].v;
   a.src_meta = e->pool[e->cur].m; a.dst_meta = e->pool[e->cur ^ 1].m;
-  a.R = tick_rows(e); a.new_gen = next_gen(e); a.n_segs = e->n_segs; a.n_groups = e->cfg.n_groups; a.Kp = e->Kp;
+  a.new_gen = next_gen(e); a.n_segs = e->n_segs; a.n_groups = e->cfg.n_groups;
   a.write_headers = headers ? 1u : 0u;
-  a.rescnt = e->d_rescnt; a.left_bits = e->d_left_bits; a.act = act_view(e); a.seg = e->d_seg; a.seg_L = e->d_seg_L; a.part_cut = e->d_part_cut;
+  a.act = act_view(e); a.seg = e->d_seg; a.seg_L = e->d_seg_L; a.part_cut = e->d_part_cut;
   a.seg_bin_lo = e->d_seg_bin_lo;
   a.hdr = e->d_hdr; a.src_idx = want_seq ? e->d_src_idx : nullptr; a.emit_seq = want_seq ? e->d_emit_seq : nullptr;
   a.ctr = e->d_ctr;
@@ -570,14 +568,15 @@ int tick_phase_a(mm_engine* e) {
 }
 
 int tick_phase_b(mm_engine* e, bool want_seq) {
-  CK(cudaEventRecord(e->ev[2], e->stream));
   const uint32_t rows = tick_rows(e);
-  k_place<512><<<rows, 512, place_smem_bytes(e->max_nb, e->place_stages), e->stream>>>(place_args(e, want_seq),
-                                                                                  e->pool[e->cur].m.fill, e->n_segs);
-  CK(cudaEventRecord(e->ev[3], e->stream));
   if (e->pool[e->cur ^ 1].m.chist)  // the compacted pool's chunk histograms start empty (the fused tick's helper CTAs do this)
     CK(cudaMemsetAsync(e->pool[e->cur ^ 1].m.chist, 0, (size_t)e->n_chunks * kChunkHist * 4, e->stream));
-  k_epilogue<512><<<std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)e->n_sms, 2 * rows)), 512, 0, e->stream>>>(epi_args(e, want_seq, true));
+  CK(cudaEventRecord(e->ev[2], e->stream));
+  k_place<512><<<rows, 512, place_smem_bytes(e->max_nb, e->place_stages), e->stream>>>(
+      place_args(e, want_seq), epi_args(e, want_seq, true), e->pool[e->cur].m.fill, e->n_segs);
+  CK(cudaEventRecord(e->ev[3], e->stream));
+  k_epilogue<512><<<std::max<uint32_t>(1, std::min<uint32_t>((uint32_t)e->n_sms, 2 * rows)), 512, 0, e->stream>>>(
+      epi_args(e, want_seq, true), rows);
   CK(cudaGetLastError());
   CK(cudaEventRecord(e->ev[4], e->stream));
   CK(cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(TickCtr), cudaMemcpyDeviceToHost, e->stream));
@@ -602,7 +601,7 @@ int tick_fused(mm_engine* e, bool want_seq) {
   e->d_ctr = e->d_ctr2 + e->ctr_idx;  // armed (barrier / stamps zero) by the previous fused tick or by mm_create
   a.tail = tail_args(e);
   a.place = place_args(e, want_seq);
-  a.epi = epi_args(e, want_seq, want_seq || helpers == 0);  // emission order needs the placement's src_idx first
+  a.epi = epi_args(e, want_seq, want_seq);  // emission order needs every row's src_idx first: barrier 2
   a.next_ctr = e->d_ctr2 + (e->ctr_idx ^ 1);
   CK(cudaEventRecord(e->ev[0], e->stream));
   void* params[] = {&a};
@@ -625,12 +624,12 @@ int tick_commit(mm_engine* e, uint32_t n, mm_tick_stats* stats) {
     st.n_launches = 1;
     st.hist_us = (float)(c.t[1] - c.t[0]) * 1e-3f;
     st.scan_us = (float)(c.t[2] - c.t[1]) * 1e-3f;
-    st.place_us = (float)(c.t[3] - c.t[2]) * 1e-3f;
-    st.epilogue_us = (float)(c.t[6] - c.t[3]) * 1e-3f;  // until the last CTA is done
+    st.place_us = (float)(c.t[3] - c.t[2]) * 1e-3f;     // until the last row has placed and compacted
+    st.epilogue_us = (float)(c.t[6] - c.t[3]) * 1e-3f;  // headers and counter re-arm, until the last CTA is done
     if (std::getenv("MM_TRACE")) {
       // placement stalls: per half, averaged over the rows, at the device's peak SM clock
       const double us = 1e3 / ((double)e->clock_khz * tick_rows(e));
-      std::fprintf(stderr, "[mm] t0=0 rows_p1_done=%.1f tail_done=%.1f bar1=%.1f place_start=%.1f rows_place_done=%.1f bar2=%.1f end=%.1f us"
+      std::fprintf(stderr, "[mm] t0=0 rows_p1_done=%.1f tail_done=%.1f bar1=%.1f place_start=%.1f rows_place_done=%.1f rows_compact_done=%.1f end=%.1f us"
                    " | place stall/row hand full empty loop: h0 %.1f %.1f %.1f %.1f h1 %.1f %.1f %.1f %.1f us\n",
                    (c.t[8] - c.t[0]) * 1e-3, (c.t[5] - c.t[0]) * 1e-3, (c.t[1] - c.t[0]) * 1e-3, (c.t[2] - c.t[0]) * 1e-3,
                    (c.t[10] - c.t[0]) * 1e-3, (c.t[3] - c.t[0]) * 1e-3, (c.t[6] - c.t[0]) * 1e-3,
@@ -656,6 +655,10 @@ int tick_commit(mm_engine* e, uint32_t n, mm_tick_stats* stats) {
   if (stats) *stats = st;
   if (c.chist_bad) {  // placement took slot bases from chunk histograms that disagree with the pool: results are wrong
     std::snprintf(e->last_err, sizeof(e->last_err), "%u placement tiles disagree with their chunk histograms", c.chist_bad);
+    return MM_E_STATE;
+  }
+  if (c.left_bad) {  // the compaction found leftovers beyond their partition's share of the compacted pool
+    std::snprintf(e->last_err, sizeof(e->last_err), "%u leftover players fall outside their partition's compacted range", c.left_bad);
     return MM_E_STATE;
   }
   return MM_OK;
@@ -868,7 +871,7 @@ int mm_create(const mm_config* cfg, mm_engine** out) {
   if ((rc = alloc_tick_scratch(e))) return bail(rc);
   {
     size_t sz = std::max(hist_smem_bytes(e->max_nb), place_smem_bytes(e->max_nb, e->place_stages));
-    sz = std::max<size_t>(sz, std::max<size_t>((size_t)kEpiScratchWords * 4, colscan_smem(e)));
+    sz = std::max<size_t>(sz, std::max<size_t>((size_t)std::max(kEpiScratchWords, kRowCompactWords) * 4, colscan_smem(e)));
     int coop = 0, nb = 0;
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, e->device);
     if (coop && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_tick<512>, 512, sz) == cudaSuccess &&
@@ -894,7 +897,7 @@ int mm_destroy(mm_engine* e) {
   cudaFree(e->d_part_cut); cudaFree(e->d_cut_lp_lo);
   cudaFree(e->d_M); cudaFree(e->d_P); cudaFree(e->d_outbase); cudaFree(e->d_binlim); cudaFree(e->d_bin_seg);
   cudaFree(e->d_bin_key); cudaFree(e->d_seg); cudaFree(e->d_members); cudaFree(e->d_members32); cudaFree(e->d_members32_alt); cudaFree(e->d_hdr_alt); cudaFree(e->d_src_idx);
-  cudaFree(e->d_hdr); cudaFree(e->d_emit_seq); cudaFree(e->d_rescnt); cudaFree(e->d_ctr2); cudaFree(e->d_small);
+  cudaFree(e->d_hdr); cudaFree(e->d_emit_seq); cudaFree(e->d_ctr2); cudaFree(e->d_small);
   cudaFree(e->d_in_id); cudaFree(e->d_hslot); cudaFree(e->d_in_rating); cudaFree(e->d_in_mode); cudaFree(e->d_code);
   cudaFree(e->d_in_ts); cudaFree(e->d_blocksum); cudaFree(e->d_blockhist); cudaFree(e->d_part); cudaFree(e->d_in_key);
   cudaFree(e->d_in_handle); cudaFree(e->d_rej_idx); cudaFree(e->d_rej_code);

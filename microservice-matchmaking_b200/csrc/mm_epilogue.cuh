@@ -1,30 +1,27 @@
-// mm_epilogue.cuh — phase 4 of the tick: pool compaction of the leftovers + lobby headers
+// mm_epilogue.cuh — the end of the tick: pool compaction of the leftovers (per row) + lobby headers
 #pragma once
 #include "mm_common.cuh"
 #include "mm_scan.cuh"
+#include "mm_place.cuh"
 
 namespace mm {
 
 // ---------------------------------------------------------------------------------------
-// k_epilogue.  Lobby headers from the segment table — lobby c of segment s = members
-// [member_base + k*L, +L); replaces the payload assembly at search/worker.ex:315-319.
-// Pool compaction, row-parallel and order-preserving: the placement pass left one bit per
-// player that stays queued (left_bits) and the count per row; every CTA scans the R row
-// counts, then walks the bit words of its rows — popcount prefix, slots of the set bits
-// enumerated into shared memory, one thread per leftover player gathers its record from the
-// old pool buffer into the alternate one and re-stamps the player's active-set entry.
-// Replaces save_new_state/3 (search/worker.ex:282-289): the "partial lobby" is the players
-// left resident.
+// Lobby headers from the segment table — lobby c of segment s = members [member_base + k*L, +L); replaces the payload
+// assembly at search/worker.ex:315-319.
+// Pool compaction, row by row and order-preserving (compact_row): right after placing its tiles, a row moves the
+// players it left queued (one bit each in left_bits) into the alternate pool buffer and re-stamps their active-set
+// entries.  Replaces save_new_state/3 (search/worker.ex:282-289): the "partial lobby" is the players left resident.
 // ---------------------------------------------------------------------------------------
 constexpr uint32_t kLeftList = 2048;  // leftover players handled per step of the compaction
-constexpr uint32_t kEpiScratchWords = (kMaxRows + 1) + 64 + (kMaxSegs + 1) + 4 * kMaxSegs + kLeftList;
+constexpr uint32_t kEpiScratchWords = (kMaxSegs + 1) + 2 * kMaxSegs;
+constexpr uint32_t kRowCompactWords = 64 + 4 * kMaxSegs + kLeftList;
+static_assert(kRowCompactWords * 4 <= kPlaceUnionBytes, "the row compaction re-uses the placement's shared memory");
 
 struct EpiArgs {
   PoolView src, dst;
   PoolMeta src_meta, dst_meta;  // dst_meta was filled in by the scan tail
-  uint32_t R, new_gen, n_segs, n_groups, Kp, write_headers;
-  const uint32_t* rescnt;
-  const uint32_t* left_bits;
+  uint32_t new_gen, n_segs, n_groups, write_headers;
   ActiveView act;
   const SegInfo* seg;
   const uint32_t* seg_L;
@@ -99,160 +96,164 @@ __device__ __forceinline__ void headers_claimed(uint32_t* scratch, const EpiArgs
   }
 }
 
+// compact_row<BLOCK>: the row's leftover players -> compacted pool, run by the row right after it has placed its tiles.
+// A bin's slots are handed out in row order — outbase[b] + players of b in earlier rows (pre_b) + rank inside the
+// row — and a player at or past binlim[b] stays queued, so the leftovers of partition p that lie in earlier rows are
+// a closed form of the prefixes the placement's window load uses:
+//     left_before(p) = sum over the bins b of p of  min(pre_b, max(0, outbase[b] + pre_b - binlim[b])).
+// Rows are contiguous in a partition's enqueue order: the leftover of rank k among the row's leftovers of p (in
+// virtual-position order) goes to slot new_chunk[p] * kTile + left_before(p) + k of the compacted pool, which needs
+// nothing from the other rows.  The row walks its own left_bits words (popcount prefix; slots of the set bits listed
+// in shared memory), then one thread per listed player gathers its record from the old pool buffer into the alternate
+// one, adds it to the compacted chunk histogram and re-stamps its active-set entry.  Rows without leftovers return at
+// once (policy S0: only a partition's last row has any).  A rank outside [0, n_left) of its partition is not written;
+// TickCtr::left_bad counts it and the tick fails.
+// nres: the row's leftover players (place_body's result).  clr_done (may be null): the compacted pool's chunk
+// histograms are cleared once it reaches clr_target.
 template <int BLOCK>
-__device__ __forceinline__ void epilogue_body(uint32_t* scratch, const Geo& g, const EpiArgs a,
-                                              unsigned long long* t_mid = nullptr) {
+__device__ __forceinline__ void compact_row(uint32_t* scratch, const Geo& g, const PlaceArgs& pa, const EpiArgs& a,
+                                            uint32_t nres, unsigned int* clr_done, unsigned int clr_target) {
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, row = blockIdx.x;
+  constexpr uint32_t NW = BLOCK / 32;
+  if (nres == 0) return;  // (uniform; place_body ended on a barrier: its shared memory is free)
   const PoolView& src = a.src;
   const PoolView& dst = a.dst;
-  const uint32_t R = a.R, n_segs = a.n_segs;
-  const uint32_t* __restrict__ rescnt = a.rescnt;
-  const uint32_t* __restrict__ left_bits = a.left_bits;
-  const ActiveView act = a.act;
-  const SegInfo* __restrict__ seg = a.seg;
-  const uint32_t* __restrict__ seg_L = a.seg_L;
-  TickCtr* ctr = a.ctr;
-  const uint32_t new_gen = a.new_gen;
-  const uint32_t n = g.NT * kTile;            // virtual positions of this tick
-  const uint32_t chunk = g.tpr * kTile;       // virtual positions per row
-  constexpr uint32_t NW = BLOCK / 32;
   const PoolMeta sm = a.src_meta;
-  auto phys_of = [&](uint32_t v, uint32_t& p) -> uint32_t {  // virtual position of the old pool -> physical slot, partition
-    p = geo_seg_of(g, v / kTile);
-    return __ldcg(&sm.chunk_tab[(size_t)p * sm.max_ch + (v / kTile - g.T0[p])]) * kTile + v % kTile;
+  const uint32_t s0 = row * g.tpr, s1 = s0 + g.tpr < g.NT ? s0 + g.tpr : g.NT;  // the row holds leftovers: s0 < s1
+  const uint32_t p0 = geo_seg_of(g, s0), np = geo_seg_of(g, s1 - 1) - p0 + 1;  // partitions of the row's tiles
+  uint32_t* s_tmp = scratch;           // [64]
+  uint32_t* s_off = s_tmp + 64;        // [np] left_before(p) - row rank of p's first leftover
+  uint32_t* s_cnt = s_off + kMaxSegs;  // [np] leftovers of p in the row -> row rank of p's first leftover
+  uint32_t* s_nl = s_cnt + kMaxSegs;   // [np] players of p that stay queued
+  uint32_t* s_nc = s_nl + kMaxSegs;    // [np] compacted-pool slot of p's first leftover
+  uint32_t* s_list = s_nc + kMaxSegs;  // [kLeftList]
+  const uint32_t nwords = (s1 - s0) * (kTile / 32);
+  const uint32_t* bits = pa.left_bits + (size_t)s0 * (kTile / 32);  // 16-byte aligned: rows start on tile boundaries
+  // 4 bit words (128 players) per thread and step of the walk below; the first step's words are loaded here, beside
+  // the left_before loads (a row of up to 32 tiles is one step of a 512-thread CTA)
+  const uint4 w4_first = 4 * tid < nwords ? __ldcg(reinterpret_cast<const uint4*>(bits + 4 * tid)) : make_uint4(0, 0, 0, 0);
+  for (uint32_t k = tid; k < np; k += BLOCK) {
+    s_off[k] = 0; s_cnt[k] = 0;
+    s_nl[k] = __ldcg(&a.seg[p0 + k].n_left); s_nc[k] = __ldcg(&a.seg[p0 + k].new_chunk) * kTile;
+  }
+  __syncthreads();
+  {  // left_before of the partitions with leftovers: the window load's prefixes (P, or the few rows before this one)
+    const bool scanned = geo_use_colscan(g);
+    for (uint32_t i = a.seg_bin_lo[p0] + tid; i < a.seg_bin_lo[p0 + np]; i += BLOCK) {
+      const uint32_t p = pa.bin_seg[i];
+      uint32_t rlo = 0, rhi = 0;
+      if (!s_nl[p - p0] || !geo_rows_of(g, p, rlo, rhi)) continue;
+      uint32_t pre = 0;
+      if (scanned) pre = __ldcg(&pa.P[(size_t)row * pa.Kp + i]);
+      else
+        for (uint32_t r = rlo; r < row; r += 8) {
+          uint32_t v8[8];
+#pragma unroll
+          for (uint32_t u = 0; u < 8; ++u) v8[u] = r + u < row ? __ldcg(&pa.M[(size_t)(r + u) * pa.Kp + i]) : 0u;
+#pragma unroll
+          for (uint32_t u = 0; u < 8; ++u) pre += v8[u];
+        }
+      const uint32_t end = __ldcg(&pa.outbase[i]) + pre, lim = __ldcg(&pa.binlim[i]);
+      if (end > lim) atomicAdd(&s_off[p - p0], end - lim < pre ? end - lim : pre);
+    }
+  }
+  for (uint32_t w0 = 0; w0 < nwords; w0 += 4 * BLOCK) {  // the row's leftovers per partition (a tile is 64 words)
+    const uint32_t wi = w0 + 4 * tid;
+    const uint4 w4 = w0 == 0 ? w4_first : (wi < nwords ? __ldcg(reinterpret_cast<const uint4*>(bits + wi)) : make_uint4(0, 0, 0, 0));
+    const uint32_t c = __popc(w4.x) + __popc(w4.y) + __popc(w4.z) + __popc(w4.w);
+    if (c) atomicAdd(&s_cnt[geo_seg_of(g, s0 + wi / (kTile / 32)) - p0], c);
+  }
+  if (a.dst_meta.chist && clr_done) grid_wait(clr_done, clr_target);  // before the first chunk-histogram add
+  else __syncthreads();
+  block_excl_scan<BLOCK>(s_cnt, np, s_tmp);
+  for (uint32_t k = tid; k < np; k += BLOCK) s_off[k] -= s_cnt[k];
+
+  uint32_t tbase = 0, fill = 0;  // row rank of s_list[0]; entries in the list (uniform)
+  auto flush = [&](uint32_t count) {
+    __syncthreads();
+    for (uint32_t e = tid; e < count; e += BLOCK) {
+      const uint32_t v = s_list[e];  // virtual position in the old pool
+      const uint32_t p = geo_seg_of(g, v / kTile), k = p - p0;  // a player never leaves its partition
+      const uint32_t loc = tbase + e + s_off[k];
+      if (loc >= s_nl[k]) { atomicAdd(&a.ctr->left_bad, 1u); continue; }
+      const uint32_t i = __ldcg(&sm.chunk_tab[(size_t)p * sm.max_ch + (v / kTile - g.T0[p])]) * kTile + v % kTile;
+      const uint32_t t = s_nc[k] + loc;
+      const uint64_t pid = src.id[i];
+      dst.id[t] = pid; dst.rating[t] = src.rating[i]; dst.mode[t] = src.mode[i];
+      dst.tsize[t] = src.tsize[i]; dst.ts[t] = src.ts[i]; dst.seq[t] = src.seq[i];
+      const uint32_t key = src.bin[i];
+      dst.bin[t] = (uint16_t)key;
+      if (a.dst_meta.chist) atomicAdd(&a.dst_meta.chist[(size_t)(t / kTile) * kChunkHist + (key - a.seg_bin_lo[p])], 1u);
+      if (a.act.on()) {
+        const uint64_t h = act_find(a.act, pid);
+        if (h != ~0ull) *a.act.val(h) = ((unsigned long long)a.new_gen << 32) | t;
+      }
+    }
+    tbase += count;
+    __syncthreads();
   };
-  uint32_t* s_off = scratch;                   // [kMaxRows + 1]
-  uint32_t* s_tmp = s_off + kMaxRows + 1;      // [64]
-  uint32_t* s_lbase = s_tmp + 64;              // [kMaxSegs + 1]
+  uint32_t run = 0;  // row rank of the step's first leftover player
+  for (uint32_t w0 = 0; w0 < nwords && run < nres; w0 += 4 * BLOCK) {
+    const uint32_t wi = w0 + 4 * tid;
+    const uint4 w4 = w0 == 0 ? w4_first : (wi < nwords ? __ldcg(reinterpret_cast<const uint4*>(bits + wi)) : make_uint4(0, 0, 0, 0));
+    const uint32_t wv[4] = {w4.x, w4.y, w4.z, w4.w};
+    const uint32_t c = __popc(w4.x) + __popc(w4.y) + __popc(w4.z) + __popc(w4.w);
+    uint32_t incl = c;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, incl, o);
+      if (lane >= (uint32_t)o) incl += u;
+    }
+    if (lane == 31) s_tmp[warp] = incl;
+    __syncthreads();
+    uint32_t wbase = 0, wtot = 0;
+    for (uint32_t k = 0; k < NW; ++k) { const uint32_t v = s_tmp[k]; if (k < warp) wbase += v; wtot += v; }
+    const uint32_t lpre = run + wbase + incl - c;  // row rank of this thread's first leftover player
+    for (uint32_t q = run; q < run + wtot;) {  // (uniform) ranks [q, q + take) of this step go to the list
+      if (fill == kLeftList) { flush(fill); fill = 0; }
+      const uint32_t room = kLeftList - fill, take = run + wtot - q < room ? run + wtot - q : room;
+      if (c && lpre < q + take && lpre + c > q) {
+        uint32_t r = lpre;
+#pragma unroll
+        for (int k4 = 0; k4 < 4; ++k4) {
+          uint32_t ww = wv[k4];
+          while (ww) {
+            const uint32_t bpos = __ffs(ww) - 1;
+            ww &= ww - 1;
+            if (r >= q && r < q + take) s_list[fill + (r - q)] = s0 * kTile + ((wi + k4) << 5) + bpos;
+            ++r;
+          }
+        }
+      }
+      fill += take;
+      q += take;
+    }
+    run += wtot;
+    __syncthreads();  // s_tmp is rewritten by the next step
+  }
+  if (fill) flush(fill);
+}
+
+// The lobby headers with emission order (emit_seq needs every row's src_idx, so this runs after the placement of the
+// whole pool): written by all CTAs of the launch.
+template <int BLOCK>
+__device__ __forceinline__ void epilogue_body(uint32_t* scratch, const Geo& g, const EpiArgs a) {
+  uint32_t* s_lbase = scratch;                 // [kMaxSegs + 1]
   uint32_t* s_mbase = s_lbase + kMaxSegs + 1;  // [kMaxSegs]
   uint32_t* s_L = s_mbase + kMaxSegs;          // [kMaxSegs]
-  uint32_t* s_leftb = s_L + kMaxSegs;          // [kMaxSegs] rank of the partition's first leftover player
-  uint32_t* s_newch = s_leftb + kMaxSegs;      // [kMaxSegs] the partition's first chunk in the compacted pool
-  uint32_t* s_list = s_newch + kMaxSegs;       // [kLeftList]
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  for (uint32_t s = tid; s < n_segs; s += BLOCK) {
-    s_lbase[s] = __ldcg(&seg[s].lobby_base); s_mbase[s] = __ldcg(&seg[s].member_base); s_L[s] = seg_L[s];
-    s_leftb[s] = __ldcg(&seg[s].left_base); s_newch[s] = __ldcg(&seg[s].new_chunk);
-  }
-  for (uint32_t r = tid; r < R; r += BLOCK) s_off[r] = __ldcg(&rescnt[r]);
-  __syncthreads();
-  const uint32_t total = block_excl_scan<BLOCK>(s_off, R, s_tmp);
-  if (tid == 0) {
-    s_off[R] = total;
-    if (blockIdx.x == 0) ctr->n_resid = total;
+  for (uint32_t s = threadIdx.x; s < a.n_segs; s += BLOCK) {
+    s_lbase[s] = __ldcg(&a.seg[s].lobby_base); s_mbase[s] = __ldcg(&a.seg[s].member_base); s_L[s] = a.seg_L[s];
   }
   __syncthreads();
-  if (a.write_headers)  // fire-and-forget stores first: they drain while the compaction waits on its dependent chains
-    headers_body<BLOCK>(g, a, s_lbase, s_mbase, s_L, blockIdx.x, gridDim.x);
-  // Work is split by leftover RANK, not by row: under policy S0 the leftovers are the latest arrivals of every
-  // partition and sit in the last rows of the pool.  CTA b moves the players with global rank [r0, r1); it walks
-  // the bit words of the rows holding them (popcount prefix from the start of the row), enumerates the pool
-  // slots of its ranks into a shared-memory list (no memory latency) and then, one thread per listed player,
-  // gathers the record into the alternate pool buffer and re-stamps the player's active-set entry — all the
-  // dependent gather / hash-probe chains run in parallel, neighbouring threads touch neighbouring slots.
-  const uint32_t per = (total + gridDim.x - 1) / gridDim.x;
-  const uint32_t r0 = (uint64_t)blockIdx.x * per < total ? blockIdx.x * per : total;
-  const uint32_t r1 = r0 + per < total ? r0 + per : total;
-  if (r1 > r0) {
-    uint32_t tbase = r0, fill = 0;  // global rank of s_list[0]; entries in the list (uniform)
-    uint32_t row_beg = 0;           // pool slot of the current row's first player
-    auto flush = [&](uint32_t count, bool last) {
-      __syncthreads();
-      for (uint32_t e = tid; e < count; e += BLOCK) {
-        const uint32_t v = s_list[e], r = tbase + e;  // virtual position in the old pool, global leftover rank
-        uint32_t p;  // a player never leaves its partition
-        const uint32_t i = phys_of(v, p);
-        const uint32_t loc = r - s_leftb[p];
-        const uint32_t t = (s_newch[p] + loc / kTile) * kTile + loc % kTile;
-        const uint64_t pid = src.id[i];
-        dst.id[t] = pid; dst.rating[t] = src.rating[i]; dst.mode[t] = src.mode[i];
-        dst.tsize[t] = src.tsize[i]; dst.ts[t] = src.ts[i]; dst.seq[t] = src.seq[i];
-        const uint32_t key = src.bin[i];
-        dst.bin[t] = (uint16_t)key;
-        if (a.dst_meta.chist) atomicAdd(&a.dst_meta.chist[(size_t)(t / kTile) * kChunkHist + (key - a.seg_bin_lo[p])], 1u);
-        if (act.on()) {
-          const uint64_t h = act_find(act, pid);
-          if (h != ~0ull) *act.val(h) = ((unsigned long long)new_gen << 32) | t;
-        }
-      }
-      tbase += count;
-      if (!last) __syncthreads();  // the last flush runs on into the lobby headers: the few threads waiting on
-                                   // their gather / probe chains do not hold up the others
-    };
-    uint32_t row = 0;
-    {  // first row holding rank r0: smallest row with s_off[row + 1] > r0
-      uint32_t a = 0, e = R;
-      while (a < e) { const uint32_t mid = (a + e) >> 1; if (s_off[mid + 1] > r0) e = mid; else a = mid + 1; }
-      row = a;
-    }
-    for (; row < R && s_off[row] < r1; ++row) {
-      const uint32_t off = s_off[row], cnt = s_off[row + 1] - off;
-      if (cnt == 0) continue;  // uniform for the CTA
-      const uint64_t beg64 = (uint64_t)row * chunk;
-      const uint32_t beg = beg64 < n ? (uint32_t)beg64 : n;
-      const uint32_t end = (beg64 + chunk < n) ? (uint32_t)(beg64 + chunk) : n;
-      const uint32_t nwords = (end - beg + 31) >> 5;  // beg is a multiple of 32 (chunk is a multiple of kRound)
-      const uint32_t* bits = left_bits + (beg >> 5);
-      row_beg = beg;
-      const uint32_t lo_l = (r0 > off ? r0 : off) - off, hi_l = (r1 < off + cnt ? r1 : off + cnt) - off;  // row-local ranks
-      uint32_t run_l = 0;  // row-local rank of the step's first leftover player
-      // 4 bit words (128 players) per thread and step: a row of 17 tiles is one step of a 512-thread CTA.  nwords is a
-      // multiple of 64 (whole tiles) and `bits` is 16-byte aligned (rows start on tile boundaries).
-      for (uint32_t w0 = 0; w0 < nwords && run_l < hi_l; w0 += 4 * BLOCK) {
-        const uint32_t wi = w0 + 4 * tid;
-        const uint4 w4 = wi < nwords ? __ldcg(reinterpret_cast<const uint4*>(bits + wi)) : make_uint4(0, 0, 0, 0);
-        const uint32_t wv[4] = {w4.x, w4.y, w4.z, w4.w};
-        const uint32_t c = __popc(w4.x) + __popc(w4.y) + __popc(w4.z) + __popc(w4.w);
-        uint32_t incl = c;
-#pragma unroll
-        for (int o = 1; o < 32; o <<= 1) {
-          const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-          if (lane >= (uint32_t)o) incl += u;
-        }
-        if (lane == 31) s_tmp[warp] = incl;
-        __syncthreads();
-        uint32_t wbase = 0, wtot = 0;
-        for (uint32_t k = 0; k < NW; ++k) { const uint32_t v = s_tmp[k]; if (k < warp) wbase += v; wtot += v; }
-        const uint32_t lpre = run_l + wbase + incl - c;  // row-local rank of this thread's first leftover player
-        uint32_t q = lo_l > run_l ? lo_l : run_l;
-        const uint32_t q_end = hi_l < run_l + wtot ? hi_l : run_l + wtot;
-        while (q < q_end) {  // (uniform) ranks [q, q_end) of this step are mine
-          if (fill == kLeftList) { flush(fill, false); fill = 0; }
-          const uint32_t room = kLeftList - fill, take = q_end - q < room ? q_end - q : room;
-          if (c && lpre < q + take && lpre + c > q) {
-            uint32_t r = lpre;
-#pragma unroll
-            for (int k4 = 0; k4 < 4; ++k4) {
-              uint32_t ww = wv[k4];
-              while (ww) {
-                const uint32_t bpos = __ffs(ww) - 1;
-                ww &= ww - 1;
-                if (r >= q && r < q + take) s_list[fill + (r - q)] = row_beg + ((wi + k4) << 5) + bpos;
-                ++r;
-              }
-            }
-          }
-          fill += take;
-          q += take;
-        }
-        run_l += wtot;
-        __syncthreads();  // s_tmp is rewritten by the next step
-      }
-    }
-    if (fill) flush(fill, true);
-  }
-  if (t_mid && tid == 0) {
-    unsigned long long tm;
-    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tm));
-    atomicMax(t_mid, tm);
-  }
+  headers_body<BLOCK>(g, a, s_lbase, s_mbase, s_L, blockIdx.x, gridDim.x);
 }
 
 template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK) k_epilogue(const EpiArgs a) {
+__global__ void __launch_bounds__(BLOCK) k_epilogue(const EpiArgs a, uint32_t R) {
   __shared__ uint32_t scratch[kEpiScratchWords];
   __shared__ Geo geo;
   __shared__ uint32_t s_gtmp[33];
-  geo_build<BLOCK>(geo, a.src_meta.fill, a.n_segs, a.R, s_gtmp);
+  geo_build<BLOCK>(geo, a.src_meta.fill, a.n_segs, R, s_gtmp);
   epilogue_body<BLOCK>(scratch, geo, a);
 }
 

@@ -19,8 +19,9 @@
 //              layout and bin totals of the compacted pool; column prefix of M only when a partition spans many rows
 //   k_place    stable rank inside the row -> final lobby-major slot; tile-local counting sort staged in shared
 //              memory, ids written to member_ids in whole sectors (reads 10 B/player, writes 8 B); players past
-//              their bin's prefix: one bit in left_bits
-//   k_epilogue leftover players -> compacted pool (enqueue order kept inside the partition) + lobby headers
+//              their bin's prefix: one bit in left_bits; then the row moves its own leftover players to the
+//              compacted pool (enqueue order kept inside the partition; compact_row)
+//   k_epilogue lobby headers
 // Integer/HBM-bound work: no tensor cores (BASELINE.json north_star).
 #pragma once
 #include "mm_common.cuh"
@@ -44,17 +45,30 @@ __global__ void __launch_bounds__(BLOCK, 2)
   else hist_body<BLOCK>(smem_raw, geo, bins16, meta, Kp, max_nb, seg_bin_lo, M);
 }
 
+// placement + row compaction (the compacted pool's chunk histograms were cleared before the launch)
+template <int BLOCK>
+__global__ void __launch_bounds__(BLOCK, 2) k_place(const PlaceArgs a, const EpiArgs e, const uint32_t* __restrict__ fill,
+                                                    uint32_t n_segs) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  __shared__ Geo geo;
+  __shared__ uint32_t s_gtmp[33];
+  geo_build<BLOCK>(geo, fill, n_segs, a.R, s_gtmp);
+  const uint32_t nres = place_body<BLOCK>(smem_raw, geo, a, [] {});
+  compact_row<BLOCK>(reinterpret_cast<uint32_t*>(smem_raw), geo, a, e, nres, nullptr, 0u);
+}
+
 // ---------------------------------------------------------------------------------------
 // k_tick<512>: the whole search tick in ONE cooperative launch ("fully matched in one
 // launch", BASELINE.json).  G CTAs = R row CTAs + a few helper CTAs; the CTA's dynamic shared
 // memory is re-used by every phase, the tile geometry is built once:
 //   rows: histogram of their tiles      || helper 0: the tail (bin totals are resident, kept
-//         (TMA ring of bin tiles)       ||   current by ingest / remove / the previous tick)         | barrier 1
-//   [only when a partition spans many rows: column scan of M by all CTAs                            | barrier 1b]
-//   rows: placement (TMA ring of bin/id tiles, tile sort, sector-complete stores), then lobby headers
-//         in chunks claimed by the rows that finish first
-//                                       || helpers: clear the compacted pool's chunk histograms     | barrier 2
-//   all:  pool compaction by leftover rank (+ headers here when emission order was asked for)
+//         (TMA ring of bin tiles)       ||   current by ingest / remove / the previous tick)         | barrier 1:
+//   rows: placement prologue (descriptors, first bulk copies)                  rows arrive before, wait after
+//   [only when a partition spans many rows: whole barrier 1, column scan of M by all CTAs            | barrier 1b]
+//   rows: placement (TMA ring of bin/id tiles, tile sort, sector-complete stores), compaction of the
+//         row's own leftovers, then lobby headers in chunks claimed by the rows that finish first
+//                                       || helpers: clear the compacted pool's chunk histograms (clr_done)
+//   [only when emission order was asked for: barrier 2, headers + emit_seq by all CTAs]
 // ---------------------------------------------------------------------------------------
 struct TickArgs {
   PoolView src;
@@ -110,27 +124,45 @@ __global__ void __launch_bounds__(BLOCK, 2) k_tick(const TickArgs a) {
   if (tail_cta && is_row) run_tail();   // a grid without helpers: after its own row
   if (threadIdx.x == 0) { unsigned long long tm; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tm)); if (is_row) atomicMax(&ctr->t[8], tm); }
   bar += G;
-  if (tail_first) grid_wait(&ctr->gbar, bar); else grid_barrier(&ctr->gbar, bar);
-  stamp(1);
-  if (geo_use_colscan(geo)) {  // (uniform over the grid)
-    for (uint32_t grp = blockIdx.x; grp < (K + 31) / 32; grp += G) colscan_cols_body(scratch, geo, grp, Kp, K, a.tail.bin_seg, a.M, a.P);
-    grid_barrier(&ctr->gbar, (bar += G));
+  // Barrier 1.  A row only arrives here: its placement prologue (descriptors, table zeroing, the first tiles' bulk
+  // copies) needs nothing from the other CTAs and runs before the wait.  The column scan reads every row's M, so
+  // with it the barrier stays whole.  (uniform over the grid)
+  const bool split_bar1 = is_row && !geo_use_colscan(geo);
+  if (split_bar1) grid_arrive(&ctr->gbar);
+  else if (tail_first) grid_wait(&ctr->gbar, bar);
+  else grid_barrier(&ctr->gbar, bar);
+  if (!split_bar1) {
+    stamp(1);
+    if (geo_use_colscan(geo)) {
+      for (uint32_t grp = blockIdx.x; grp < (K + 31) / 32; grp += G) colscan_cols_body(scratch, geo, grp, Kp, K, a.tail.bin_seg, a.M, a.P);
+      grid_barrier(&ctr->gbar, (bar += G));
+    }
+    stamp(2);
   }
-  stamp(2);
-  if (is_row) place_body<BLOCK>(smem_raw, geo, a.place);
-  if (threadIdx.x == 0 && is_row) { unsigned long long tm; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tm)); atomicMax(&ctr->t[10], tm); }
-  if (a.epi.dst_meta.chist && (!is_row || n_helpers == 0)) {
-    // the compacted pool's chunks start with empty histograms (the epilogue fills them): helpers, or the rows when
-    // the grid has no helper
-    const uint32_t part = n_helpers ? helper : blockIdx.x, nparts = n_helpers ? n_helpers : G;
+  // the compacted pool's chunks start with empty histograms (the row compaction fills them): cleared by the helpers,
+  // or by the rows when the grid has no helper; every clearing CTA then counts itself in clr_done
+  const uint32_t n_clear = n_helpers ? n_helpers : G;
+  auto clear_chist = [&]() {
+    const uint32_t part = n_helpers ? helper : blockIdx.x;
     const size_t words = (size_t)__ldcg(a.epi.dst_meta.bump) * kChunkHist;
-    for (size_t i = (size_t)part * BLOCK + threadIdx.x; i < words; i += (size_t)nparts * BLOCK) a.epi.dst_meta.chist[i] = 0;
+    for (size_t i = (size_t)part * BLOCK + threadIdx.x; i < words; i += (size_t)n_clear * BLOCK) a.epi.dst_meta.chist[i] = 0;
+    grid_arrive(&ctr->clr_done);
+  };
+  if (a.epi.dst_meta.chist && !is_row) clear_chist();
+  if (is_row) {
+    const uint32_t nres = place_body<BLOCK>(smem_raw, geo, a.place, [&] {
+      if (split_bar1) { grid_wait(&ctr->gbar, bar); stamp(1); stamp(2); }
+    });
+    if (threadIdx.x == 0) { unsigned long long tm; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tm)); atomicMax(&ctr->t[10], tm); }
+    if (a.epi.dst_meta.chist && n_helpers == 0) clear_chist();
+    compact_row<BLOCK>(scratch, geo, a.place, a.epi, nres, &ctr->clr_done, n_clear);
+    if (threadIdx.x == 0) { unsigned long long tm; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tm)); atomicMax(&ctr->t[3], tm); }
+    if (!a.epi.write_headers) headers_claimed<BLOCK>(scratch, a.epi, &ctr->hdr_next);
   }
-  if (is_row && !a.epi.write_headers) headers_claimed<BLOCK>(scratch, a.epi, &ctr->hdr_next);
-  grid_barrier(&ctr->gbar, (bar += G));
-  stamp(3);
-  epilogue_body<BLOCK>(scratch, geo, a.epi, &ctr->t[7]);
-  stamp(4);  // CTA 0's view
+  if (a.epi.write_headers) {  // emission order: emit_seq reads the src_idx of every row, so barrier 2 stays
+    grid_barrier(&ctr->gbar, (bar += G));
+    epilogue_body<BLOCK>(scratch, geo, a.epi);
+  }
   if (threadIdx.x == 0) {  // the last CTA to finish closes the epilogue phase
     unsigned long long tm;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tm));
@@ -138,8 +170,8 @@ __global__ void __launch_bounds__(BLOCK, 2) k_tick(const TickArgs a) {
     __threadfence();
     if (atomicAdd(&ctr->done, 1u) == G - 1) {  // ... and arms the other counter block for the next tick
       TickCtr* nx = a.next_ctr;
-      nx->gbar = 0; nx->done = 0; nx->chist_bad = 0; nx->hdr_next = 0;
-      nx->t[6] = 0; nx->t[7] = 0; nx->t[8] = 0; nx->t[10] = 0;
+      nx->gbar = 0; nx->done = 0; nx->chist_bad = 0; nx->hdr_next = 0; nx->left_bad = 0; nx->clr_done = 0;
+      nx->t[3] = 0; nx->t[6] = 0; nx->t[8] = 0; nx->t[10] = 0;
       for (int i = 0; i < 8; ++i) nx->stall[i / 4][i % 4] = 0;
     }
   }

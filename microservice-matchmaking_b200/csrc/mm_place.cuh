@@ -75,7 +75,6 @@ struct PlaceArgs {
   uint64_t* members;
   uint32_t* src_idx;    // optional: virtual pool position of every member (emission order in ARRIVAL mode)
   uint32_t* left_bits;  // one bit per virtual pool position: the player stays queued after this tick
-  uint32_t* rescnt;     // [R] players of the row that stay queued
   TickCtr* ctr;
 };
 
@@ -94,8 +93,10 @@ struct PlaceArgs {
 //    8 warps' counters + check of their totals against chist | barrier | stage the sorted order | barrier | write back.
 // A tile whose ranked key counts differ from its chunk histogram is not written at all and counted in
 // TickCtr::chist_bad (the tick then fails): the slot bases of the row's later tiles rest on the histograms.
-template <int BLOCK>
-__device__ __forceinline__ void place_halves(unsigned char* smem_raw, const Geo& g, const PlaceArgs a) {
+// `wait_inputs` returns once the tail's outputs and every row's M are visible (the fused tick's grid barrier 1): the
+// prologue before it (descriptors, table zeroing, the first tiles' bulk copies) reads only the pool being matched.
+template <int BLOCK, class Wait>
+__device__ __forceinline__ uint32_t place_halves(unsigned char* smem_raw, const Geo& g, const PlaceArgs a, Wait&& wait_inputs) {
   static_assert(BLOCK == 512 && kTile == 2048, "tile arrangement is written for 2 x 256 threads x 8 players");
   constexpr int J = 8;
   const uint32_t S = a.stages;
@@ -161,6 +162,7 @@ __device__ __forceinline__ void place_halves(unsigned char* smem_raw, const Geo&
   __syncthreads();
   if (tid == 0)
     for (uint32_t t = 0; t < S && t < n_tiles; ++t) issue(t, t);
+  wait_inputs();
 
   uint32_t nleft = 0;  // lane 0: players of this warp's positions that stay queued
   const uint32_t row_p_last = n_tiles ? geo_seg_of(g, s1 - 1) : 0u;
@@ -363,19 +365,19 @@ __device__ __forceinline__ void place_halves(unsigned char* smem_raw, const Geo&
 
   if (lane == 0 && nleft) atomicAdd(&s_misc[0], nleft);
   __syncthreads();
+  const uint32_t n_res = s_misc[0];  // players of this row that stay queued
   if (tid == 0) {
-    a.rescnt[row] = s_misc[0];  // players of this row that stay queued
     for (uint32_t s = 0; s < S; ++s) { mbar_inval(&full[s]); mbar_inval(&empty[s]); }
     mbar_inval(hand);
   }
+  return n_res;
 }
 
-template <int BLOCK>
-__device__ __forceinline__ void place_body(unsigned char* smem_raw, const Geo& g, const PlaceArgs a) {
+template <int BLOCK, class Wait>
+__device__ __forceinline__ uint32_t place_body(unsigned char* smem_raw, const Geo& g, const PlaceArgs a, Wait&& wait_inputs) {
   static_assert(BLOCK == 512 && kTile == 2048, "tile arrangement is written for 512 threads x 4 players");
   if (a.meta.chist && a.fast_ok) {  // (uniform) every partition has <= 255 keys
-    place_halves<BLOCK>(smem_raw, g, a);
-    return;
+    return place_halves<BLOCK>(smem_raw, g, a, wait_inputs);
   }
   constexpr int J = kTile / BLOCK;
   constexpr int NW = BLOCK / 32;
@@ -438,7 +440,8 @@ __device__ __forceinline__ void place_body(unsigned char* smem_raw, const Geo& g
   if (tid == 0)
     for (uint32_t t = 0; t < stages && t < n_tiles; ++t) issue(t, t);
   for (uint32_t i = tid; i < kHeadSlots + NW * 128; i += BLOCK) head[i] = 0;  // LIST heads = FAST mask table; + FAST counters
-  const bool heavy = __ldcg(&a.ctr->heavy) != 0;
+  wait_inputs();
+  const bool heavy = __ldcg(&a.ctr->heavy) != 0;  // (written by the tail)
   __syncthreads();
 
   uint32_t st = 0, parity = 0;
@@ -758,19 +761,10 @@ __device__ __forceinline__ void place_body(unsigned char* smem_raw, const Geo& g
 
   if (lane == 0 && nleft) atomicAdd(&s_misc[0], nleft);
   __syncthreads();
-  if (tid == 0) {
-    a.rescnt[row] = s_misc[0];  // players of this row that stay queued
+  const uint32_t n_res = s_misc[0];  // players of this row that stay queued
+  if (tid == 0)
     for (uint32_t s = 0; s < stages; ++s) mbar_inval(&full[s]);
-  }
-}
-
-template <int BLOCK>
-__global__ void __launch_bounds__(BLOCK, 2) k_place(const PlaceArgs a, const uint32_t* __restrict__ fill, uint32_t n_segs) {
-  extern __shared__ __align__(128) unsigned char smem_raw[];
-  __shared__ Geo geo;
-  __shared__ uint32_t s_gtmp[33];
-  geo_build<BLOCK>(geo, fill, n_segs, a.R, s_gtmp);
-  place_body<BLOCK>(smem_raw, geo, a);
+  return n_res;
 }
 
 }  // namespace mm

@@ -288,6 +288,7 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
       s_misc[1] = c_mem; s_misc[2] = c_lob;
       *t.dst.bump = c_ch;
       t.ctr->n_lobbies = c_lob; t.ctr->n_matched = c_mem; t.ctr->n_alive = alive; t.ctr->n_dead = dead;
+      t.ctr->n_resid = c_left;
       t.ctr->heavy = s_misc[0];
     }
   }
