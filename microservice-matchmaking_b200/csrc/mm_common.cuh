@@ -74,7 +74,8 @@ struct TickCtr {
   uint32_t clr_done;   // fused tick: CTAs done clearing the compacted pool's chunk histograms
   unsigned long long t[12]; // fused kernel: %globaltimer (ns) at phase boundaries, CTA 0; [3],[6]: max over CTAs;
                             // [3] last row done placing and compacting, [8] last row done with phase 1,
-                            // [10] last row done placing
+                            // [10] last row done placing; two-pipeline placement, max over rows: [4] first tile
+                            // ranked, [7] first slot bases taken
   unsigned long long stall[2][4];  // two-pipeline placement, per half, SM clock cycles summed over the rows: waits on
                                    // [0] hand, [1] the tile's loads, [2] a stage's release before a re-issue; [3] tile loop
 };
@@ -200,6 +201,23 @@ __device__ __forceinline__ void grid_wait(unsigned int* bar, unsigned int target
     __threadfence();
   }
   __syncthreads();
+}
+// grid_wait for the 256 threads of half h of the CTA only (thread 0 of the half polls; then the half's named barrier)
+__device__ __forceinline__ void grid_wait_half(unsigned int* bar, unsigned int target, uint32_t h) {
+  if ((threadIdx.x & 255u) == 0) {
+    unsigned int v;
+    do {
+      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(bar) : "memory");
+      if (v < target) __nanosleep(32);
+    } while (v < target);
+    __threadfence();
+  }
+  bar_sync_half(h);
+}
+__device__ __forceinline__ unsigned long long global_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));
+  return t;
 }
 // global -> shared bulk copy (SASS: UBLKCP), completion counted on `bar`, with an L2 cache-policy hint
 __device__ __forceinline__ void tma_load_1d(void* dst, const void* src, uint32_t bytes, uint64_t* bar, uint64_t pol) {

@@ -601,6 +601,7 @@ int tick_fused(mm_engine* e, bool want_seq) {
   e->d_ctr = e->d_ctr2 + e->ctr_idx;  // armed (barrier / stamps zero) by the previous fused tick or by mm_create
   a.tail = tail_args(e);
   a.place = place_args(e, want_seq);
+  a.place.trace = e->d_ctr->t;  // device address of the launch's time stamps (not dereferenced here)
   a.epi = epi_args(e, want_seq, want_seq);  // emission order needs every row's src_idx first: barrier 2
   a.next_ctr = e->d_ctr2 + (e->ctr_idx ^ 1);
   CK(cudaEventRecord(e->ev[0], e->stream));
@@ -629,10 +630,13 @@ int tick_commit(mm_engine* e, uint32_t n, mm_tick_stats* stats) {
     if (std::getenv("MM_TRACE")) {
       // placement stalls: per half, averaged over the rows, at the device's peak SM clock
       const double us = 1e3 / ((double)e->clock_khz * tick_rows(e));
-      std::fprintf(stderr, "[mm] t0=0 rows_p1_done=%.1f tail_done=%.1f bar1=%.1f place_start=%.1f rows_place_done=%.1f rows_compact_done=%.1f end=%.1f us"
+      // first_ranked / first_bases: the last row to rank its first tile / take that tile's slot bases (two
+      // pipelines only; 0 = not stamped)
+      auto at = [&](int k) { return c.t[k] ? (c.t[k] - c.t[0]) * 1e-3 : 0.0; };
+      std::fprintf(stderr, "[mm] t0=0 rows_p1_done=%.1f tail_done=%.1f first_ranked=%.1f bar1=%.1f place_start=%.1f first_bases=%.1f"
+                   " rows_place_done=%.1f rows_compact_done=%.1f end=%.1f us"
                    " | place stall/row hand full empty loop: h0 %.1f %.1f %.1f %.1f h1 %.1f %.1f %.1f %.1f us\n",
-                   (c.t[8] - c.t[0]) * 1e-3, (c.t[5] - c.t[0]) * 1e-3, (c.t[1] - c.t[0]) * 1e-3, (c.t[2] - c.t[0]) * 1e-3,
-                   (c.t[10] - c.t[0]) * 1e-3, (c.t[3] - c.t[0]) * 1e-3, (c.t[6] - c.t[0]) * 1e-3,
+                   at(8), at(5), at(4), at(1), at(2), at(7), at(10), at(3), at(6),
                    c.stall[0][0] * us, c.stall[0][1] * us, c.stall[0][2] * us, c.stall[0][3] * us,
                    c.stall[1][0] * us, c.stall[1][1] * us, c.stall[1][2] * us, c.stall[1][3] * us);
     }

@@ -108,11 +108,15 @@ __device__ __forceinline__ void headers_claimed(uint32_t* scratch, const EpiArgs
 // one, adds it to the compacted chunk histogram and re-stamps its active-set entry.  Rows without leftovers return at
 // once (policy S0: only a partition's last row has any).  A rank outside [0, n_left) of its partition is not written;
 // TickCtr::left_bad counts it and the tick fails.
-// nres: the row's leftover players (place_body's result).  clr_done (may be null): the compacted pool's chunk
-// histograms are cleared once it reaches clr_target.
+// nres: the row's leftover players (place_body's result).  lb (may be null): left_before of the row's first
+// kLeftBeforeCap partitions, summed by the placement's window loads (place_left_before; outside `scratch`); the
+// others are summed here.  clr_done (may be null): the compacted pool's chunk histograms are cleared once it reaches
+// clr_target.
+static_assert(kRowCompactWords * 4 <= kTileBytes + kChunkHist * 4, "the row compaction leaves the placement header alone");
 template <int BLOCK>
 __device__ __forceinline__ void compact_row(uint32_t* scratch, const Geo& g, const PlaceArgs& pa, const EpiArgs& a,
-                                            uint32_t nres, unsigned int* clr_done, unsigned int clr_target) {
+                                            uint32_t nres, const uint32_t* lb, unsigned int* clr_done,
+                                            unsigned int clr_target) {
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, row = blockIdx.x;
   constexpr uint32_t NW = BLOCK / 32;
   if (nres == 0) return;  // (uniform; place_body ended on a barrier: its shared memory is free)
@@ -132,14 +136,15 @@ __device__ __forceinline__ void compact_row(uint32_t* scratch, const Geo& g, con
   // 4 bit words (128 players) per thread and step of the walk below; the first step's words are loaded here, beside
   // the left_before loads (a row of up to 32 tiles is one step of a 512-thread CTA)
   const uint4 w4_first = 4 * tid < nwords ? __ldcg(reinterpret_cast<const uint4*>(bits + 4 * tid)) : make_uint4(0, 0, 0, 0);
+  const uint32_t n_lb = lb ? kLeftBeforeCap : 0u;  // partitions p0 .. p0 + n_lb - 1 come with their left_before
   for (uint32_t k = tid; k < np; k += BLOCK) {
-    s_off[k] = 0; s_cnt[k] = 0;
+    s_off[k] = k < n_lb ? lb[k] : 0u; s_cnt[k] = 0;
     s_nl[k] = __ldcg(&a.seg[p0 + k].n_left); s_nc[k] = __ldcg(&a.seg[p0 + k].new_chunk) * kTile;
   }
   __syncthreads();
-  {  // left_before of the partitions with leftovers: the window load's prefixes (P, or the few rows before this one)
+  if (np > n_lb) {  // left_before of the other partitions with leftovers: the window load's prefixes (P, or the few rows before this one)
     const bool scanned = geo_use_colscan(g);
-    for (uint32_t i = a.seg_bin_lo[p0] + tid; i < a.seg_bin_lo[p0 + np]; i += BLOCK) {
+    for (uint32_t i = a.seg_bin_lo[p0 + n_lb] + tid; i < a.seg_bin_lo[p0 + np]; i += BLOCK) {
       const uint32_t p = pa.bin_seg[i];
       uint32_t rlo = 0, rhi = 0;
       if (!s_nl[p - p0] || !geo_rows_of(g, p, rlo, rhi)) continue;
@@ -178,10 +183,15 @@ __device__ __forceinline__ void compact_row(uint32_t* scratch, const Geo& g, con
       if (loc >= s_nl[k]) { atomicAdd(&a.ctr->left_bad, 1u); continue; }
       const uint32_t i = __ldcg(&sm.chunk_tab[(size_t)p * sm.max_ch + (v / kTile - g.T0[p])]) * kTile + v % kTile;
       const uint32_t t = s_nc[k] + loc;
+      // every column of the record is loaded before the first store (the two pool buffers may alias as far as the
+      // compiler knows): one round trip instead of seven
       const uint64_t pid = src.id[i];
-      dst.id[t] = pid; dst.rating[t] = src.rating[i]; dst.mode[t] = src.mode[i];
-      dst.tsize[t] = src.tsize[i]; dst.ts[t] = src.ts[i]; dst.seq[t] = src.seq[i];
+      const int32_t rating = src.rating[i];
+      const uint8_t mode = src.mode[i], tsize = src.tsize[i];
+      const uint32_t ts = src.ts[i], seq = src.seq[i];
       const uint32_t key = src.bin[i];
+      dst.id[t] = pid; dst.rating[t] = rating; dst.mode[t] = mode;
+      dst.tsize[t] = tsize; dst.ts[t] = ts; dst.seq[t] = seq;
       dst.bin[t] = (uint16_t)key;
       if (a.dst_meta.chist) atomicAdd(&a.dst_meta.chist[(size_t)(t / kTile) * kChunkHist + (key - a.seg_bin_lo[p])], 1u);
       if (a.act.on()) {

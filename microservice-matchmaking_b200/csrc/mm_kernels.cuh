@@ -53,8 +53,8 @@ __global__ void __launch_bounds__(BLOCK, 2) k_place(const PlaceArgs a, const Epi
   __shared__ Geo geo;
   __shared__ uint32_t s_gtmp[33];
   geo_build<BLOCK>(geo, fill, n_segs, a.R, s_gtmp);
-  const uint32_t nres = place_body<BLOCK>(smem_raw, geo, a, [] {});
-  compact_row<BLOCK>(reinterpret_cast<uint32_t*>(smem_raw), geo, a, e, nres, nullptr, 0u);
+  const uint32_t nres = place_body<BLOCK>(smem_raw, geo, a, [](uint32_t) {});
+  compact_row<BLOCK>(reinterpret_cast<uint32_t*>(smem_raw), geo, a, e, nres, place_left_before(smem_raw, a), nullptr, 0u);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -63,7 +63,8 @@ __global__ void __launch_bounds__(BLOCK, 2) k_place(const PlaceArgs a, const Epi
 // memory is re-used by every phase, the tile geometry is built once:
 //   rows: histogram of their tiles      || helper 0: the tail (bin totals are resident, kept
 //         (TMA ring of bin tiles)       ||   current by ingest / remove / the previous tick)         | barrier 1:
-//   rows: placement prologue (descriptors, first bulk copies)                  rows arrive before, wait after
+//   rows: placement prologue (descriptors, first bulk copies),              rows arrive before, each placement
+//         ranking of each placement pipeline's first tile                   pipeline waits before its first slot bases
 //   [only when a partition spans many rows: whole barrier 1, column scan of M by all CTAs            | barrier 1b]
 //   rows: placement (TMA ring of bin/id tiles, tile sort, sector-complete stores), compaction of the
 //         row's own leftovers, then lobby headers in chunks claimed by the rows that finish first
@@ -122,11 +123,11 @@ __global__ void __launch_bounds__(BLOCK, 2) k_tick(const TickArgs a) {
     else hist_body<BLOCK>(smem_raw, geo, a.src.bin, a.place.meta, Kp, a.place.max_nb, a.tail.seg_bin_lo, a.M);
   }
   if (tail_cta && is_row) run_tail();   // a grid without helpers: after its own row
-  if (threadIdx.x == 0) { unsigned long long tm; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tm)); if (is_row) atomicMax(&ctr->t[8], tm); }
+  if (threadIdx.x == 0 && is_row) atomicMax(&ctr->t[8], global_ns());
   bar += G;
   // Barrier 1.  A row only arrives here: its placement prologue (descriptors, table zeroing, the first tiles' bulk
-  // copies) needs nothing from the other CTAs and runs before the wait.  The column scan reads every row's M, so
-  // with it the barrier stays whole.  (uniform over the grid)
+  // copies) and the ranking of each placement pipeline's first tile need nothing from the other CTAs and run before
+  // the wait.  The column scan reads every row's M, so with it the barrier stays whole.  (uniform over the grid)
   const bool split_bar1 = is_row && !geo_use_colscan(geo);
   if (split_bar1) grid_arrive(&ctr->gbar);
   else if (tail_first) grid_wait(&ctr->gbar, bar);
@@ -150,13 +151,13 @@ __global__ void __launch_bounds__(BLOCK, 2) k_tick(const TickArgs a) {
   };
   if (a.epi.dst_meta.chist && !is_row) clear_chist();
   if (is_row) {
-    const uint32_t nres = place_body<BLOCK>(smem_raw, geo, a.place, [&] {
-      if (split_bar1) { grid_wait(&ctr->gbar, bar); stamp(1); stamp(2); }
+    const uint32_t nres = place_body<BLOCK>(smem_raw, geo, a.place, [&](uint32_t h) {
+      if (split_bar1) { grid_wait_half(&ctr->gbar, bar, h); stamp(1); stamp(2); }
     });
-    if (threadIdx.x == 0) { unsigned long long tm; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tm)); atomicMax(&ctr->t[10], tm); }
+    if (threadIdx.x == 0) atomicMax(&ctr->t[10], global_ns());
     if (a.epi.dst_meta.chist && n_helpers == 0) clear_chist();
-    compact_row<BLOCK>(scratch, geo, a.place, a.epi, nres, &ctr->clr_done, n_clear);
-    if (threadIdx.x == 0) { unsigned long long tm; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(tm)); atomicMax(&ctr->t[3], tm); }
+    compact_row<BLOCK>(scratch, geo, a.place, a.epi, nres, place_left_before(smem_raw, a.place), &ctr->clr_done, n_clear);
+    if (threadIdx.x == 0) atomicMax(&ctr->t[3], global_ns());
     if (!a.epi.write_headers) headers_claimed<BLOCK>(scratch, a.epi, &ctr->hdr_next);
   }
   if (a.epi.write_headers) {  // emission order: emit_seq reads the src_idx of every row, so barrier 2 stays
@@ -171,7 +172,7 @@ __global__ void __launch_bounds__(BLOCK, 2) k_tick(const TickArgs a) {
     if (atomicAdd(&ctr->done, 1u) == G - 1) {  // ... and arms the other counter block for the next tick
       TickCtr* nx = a.next_ctr;
       nx->gbar = 0; nx->done = 0; nx->chist_bad = 0; nx->hdr_next = 0; nx->left_bad = 0; nx->clr_done = 0;
-      nx->t[3] = 0; nx->t[6] = 0; nx->t[8] = 0; nx->t[10] = 0;
+      nx->t[3] = 0; nx->t[4] = 0; nx->t[6] = 0; nx->t[7] = 0; nx->t[8] = 0; nx->t[10] = 0;
       for (int i = 0; i < 8; ++i) nx->stall[i / 4][i % 4] = 0;
     }
   }

@@ -76,7 +76,39 @@ struct PlaceArgs {
   uint32_t* src_idx;    // optional: virtual pool position of every member (emission order in ARRIVAL mode)
   uint32_t* left_bits;  // one bit per virtual pool position: the player stays queued after this tick
   TickCtr* ctr;
+  unsigned long long* trace;  // fused tick: TickCtr::t of the launch (first tile ranked / first slot bases taken); else null
 };
+
+// Shared memory of the two-pipeline placement (see the layout above); the row compaction after it reads the header.
+constexpr uint32_t kLeftBeforeCap = 6;  // partitions of a row whose left_before the window loads keep (header words)
+struct HalvesSmem {
+  uint64_t* ring_ids;   // [S][kTile]
+  uint16_t* ring_bins;  // [S][kTile]
+  uint32_t* ring_hist;  // [S][kChunkHist]
+  unsigned char* hdr;
+  uint32_t* cnt;        // [cnt_cap]
+  unsigned char* halves;
+  DescCache* dc;
+};
+__device__ __forceinline__ HalvesSmem halves_smem(unsigned char* smem_raw, uint32_t S, uint32_t max_nb) {
+  HalvesSmem m;
+  m.ring_ids = reinterpret_cast<uint64_t*>(smem_raw);
+  m.ring_bins = reinterpret_cast<uint16_t*>(smem_raw + (size_t)S * kTile * 8);
+  m.ring_hist = reinterpret_cast<uint32_t*>(smem_raw + (size_t)S * kTileBytes);
+  m.hdr = smem_raw + (size_t)S * (kTileBytes + kChunkHist * 4);
+  m.cnt = reinterpret_cast<uint32_t*>(m.hdr + kHalvesHdr);
+  m.halves = reinterpret_cast<unsigned char*>(m.cnt + ((place_cnt_cap(max_nb) + 3) & ~3u));
+  m.dc = reinterpret_cast<DescCache*>(m.halves + 2 * kHalfBytes);
+  return m;
+}
+// header words 66 .. 71: left_before(p0 + k), k < kLeftBeforeCap, of the row's partitions p0, p0 + 1, ...
+__device__ __forceinline__ uint32_t* halves_left_before(unsigned char* hdr) { return reinterpret_cast<uint32_t*>(hdr + 264); }
+static_assert(264 + 4 * kLeftBeforeCap <= kHalvesHdr, "left_before words fit in the placement header");
+__device__ __forceinline__ bool place_on_halves(const PlaceArgs& a) { return a.meta.chist && a.fast_ok; }
+// after place_body: the left_before words the two-pipeline placement left in shared memory, or null (whole-CTA path)
+__device__ __forceinline__ const uint32_t* place_left_before(unsigned char* smem_raw, const PlaceArgs& a) {
+  return place_on_halves(a) ? halves_left_before(halves_smem(smem_raw, a.stages, a.max_nb).hdr) : nullptr;
+}
 
 // place_halves<BLOCK>: the FAST ranking for a pool with chunk histograms (every partition <= 255 keys, rank_impl 3).
 // The CTA runs two independent tile pipelines: half h (threads 256 h .. 256 h + 255, 8 warps, 8 players per thread)
@@ -89,21 +121,27 @@ struct PlaceArgs {
 //    key's matched prefix) comes from cnt[d] + chist[d] against binlim.
 //  * ring: stage s has a `full` mbarrier (the three bulk copies) and an `empty` one (the 256 threads of the half that
 //    wrote the tile back); thread 0 of that half waits on `empty` and issues the stage's next tile at once.
-//  * per tile and half: rank (as below: match table / ballots, per-warp counters) | barrier | column scan of the
-//    8 warps' counters + check of their totals against chist | barrier | stage the sorted order | barrier | write back.
+//  * per tile and half: rank (as below: match table / ballots, per-warp counters) | barrier | slot bases (hand) +
+//    column scan of the 8 warps' counters + check of their totals against chist | barrier | stage the sorted order |
+//    barrier | write back.
 // A tile whose ranked key counts differ from its chunk histogram is not written at all and counted in
 // TickCtr::chist_bad (the tick then fails): the slot bases of the row's later tiles rest on the histograms.
-// `wait_inputs` returns once the tail's outputs and every row's M are visible (the fused tick's grid barrier 1): the
-// prologue before it (descriptors, table zeroing, the first tiles' bulk copies) reads only the pool being matched.
+// The prologue (descriptors, table zeroing, the first tiles' bulk copies) and the ranking of a tile read only the pool
+// being matched; the slot bases need the other CTAs' outputs.  So a tile ranks first and takes its bases after:
+// `wait_inputs(h)`, called by the 256 threads of half h before its first slot bases, returns once the tail's outputs
+// and every row's M are visible (the fused tick's grid barrier 1); it synchronises only the half.
+// The window loads also sum left_before(p) (see compact_row) for the row's first kLeftBeforeCap partitions into the
+// header (halves_left_before), where the row compaction reads them.
 template <int BLOCK, class Wait>
 __device__ __forceinline__ uint32_t place_halves(unsigned char* smem_raw, const Geo& g, const PlaceArgs a, Wait&& wait_inputs) {
   static_assert(BLOCK == 512 && kTile == 2048, "tile arrangement is written for 2 x 256 threads x 8 players");
   constexpr int J = 8;
   const uint32_t S = a.stages;
-  uint64_t* ring_ids = reinterpret_cast<uint64_t*>(smem_raw);                               // [S][kTile]
-  uint16_t* ring_bins = reinterpret_cast<uint16_t*>(smem_raw + (size_t)S * kTile * 8);      // [S][kTile]
-  uint32_t* ring_hist = reinterpret_cast<uint32_t*>(smem_raw + (size_t)S * kTileBytes);     // [S][kChunkHist]
-  unsigned char* hdr = smem_raw + (size_t)S * (kTileBytes + kChunkHist * 4);
+  const HalvesSmem m = halves_smem(smem_raw, S, a.max_nb);
+  uint64_t* ring_ids = m.ring_ids;    // [S][kTile]
+  uint16_t* ring_bins = m.ring_bins;  // [S][kTile]
+  uint32_t* ring_hist = m.ring_hist;  // [S][kChunkHist]
+  unsigned char* hdr = m.hdr;
   uint64_t* full = reinterpret_cast<uint64_t*>(hdr);  // [kMaxStages]
   uint64_t* empty = full + kMaxStages;                // [kMaxStages]
   uint64_t* hand = empty + kMaxStages;                // slot-base hand-off, one phase per tile
@@ -114,10 +152,11 @@ __device__ __forceinline__ uint32_t place_halves(unsigned char* smem_raw, const 
   uint32_t* s_misc = s_sg + kMaxStages;  // [0] players of the row that stay queued, [1, 2] loaded counter window, [3 + h] tile flags of half h
   uint32_t* s_wt = s_misc + 8;           // [2][8] warp totals of the histogram-row scan
   uint32_t* s_ck = s_wt + 16;            // [2][4] stall counters of half h (cycles): hand, full, empty waits; loop
-  uint32_t* cnt = reinterpret_cast<uint32_t*>(hdr + kHalvesHdr);  // [cnt_cap] slot of the next player of each window bin
+  uint32_t* s_lb = halves_left_before(hdr);  // [kLeftBeforeCap] left_before of the row's partitions p0, p0 + 1, ...
+  uint32_t* cnt = m.cnt;  // [cnt_cap] slot of the next player of each window bin
   const uint32_t cnt_cap = place_cnt_cap(a.max_nb);
-  unsigned char* halves = reinterpret_cast<unsigned char*>(cnt + ((cnt_cap + 3) & ~3u));
-  DescCache& dc = *reinterpret_cast<DescCache*>(halves + 2 * kHalfBytes);
+  unsigned char* halves = m.halves;
+  DescCache& dc = *m.dc;
 
   const uint32_t tid = threadIdx.x, lane = tid & 31, h = tid >> 8, ht = tid & 255, hw = ht >> 5;
   const uint32_t lt_mask = (1u << lane) - 1u;
@@ -152,6 +191,7 @@ __device__ __forceinline__ uint32_t place_halves(unsigned char* smem_raw, const 
     mbar_init(hand, 256);
     mbar_fence_init();
     for (uint32_t i = 0; i < 8; ++i) { s_misc[i] = 0; s_ck[i] = 0; }
+    for (uint32_t i = 0; i < kLeftBeforeCap; ++i) s_lb[i] = 0;
   }
   fence_proxy_async();
   desc_fill<BLOCK>(dc, g, a.meta, s0, s1);
@@ -162,9 +202,9 @@ __device__ __forceinline__ uint32_t place_halves(unsigned char* smem_raw, const 
   __syncthreads();
   if (tid == 0)
     for (uint32_t t = 0; t < S && t < n_tiles; ++t) issue(t, t);
-  wait_inputs();
 
   uint32_t nleft = 0;  // lane 0: players of this warp's positions that stay queued
+  const uint32_t row_p0 = n_tiles ? geo_seg_of(g, s0) : 0u;
   const uint32_t row_p_last = n_tiles ? geo_seg_of(g, s1 - 1) : 0u;
   const bool scanned = geo_use_colscan(g);  // the column-scan phase ran: P holds the row prefixes
   uint32_t* ck = s_ck + 4 * h;  // thread 0 of the half: stall counters, see TickCtr::stall
@@ -174,52 +214,13 @@ __device__ __forceinline__ uint32_t place_halves(unsigned char* smem_raw, const 
     const uint32_t vbase = (s0 + t) * kTile;  // virtual position of the tile's first player
     const uint16_t* tb = ring_bins + (size_t)st * kTile;
     const uint64_t* ti = ring_ids + (size_t)st * kTile;
-    // Tile t-1 has taken its slot bases (so its stage, and every earlier one, has landed); then this tile's stage.
-    const uint32_t ck0 = (uint32_t)clock();
-    if (t) mbar_wait(hand, (t - 1) & 1u);
     const uint32_t ck1 = (uint32_t)clock();
     mbar_wait(&full[st], parity);
-    if (ht == 0) { ck[0] += ck1 - ck0; ck[1] += (uint32_t)clock() - ck1; }
+    if (ht == 0) ck[1] += (uint32_t)clock() - ck1;
     const uint32_t valid = s_nv[st];
     const uint32_t bin0 = s_b0[st], nb = s_b1[st] - bin0;
     const uint32_t d = ht;  // this thread's key in the histogram-row steps
     const uint32_t ch = d < nb ? ring_hist[st * kChunkHist + d] : 0u;
-    const uint32_t lim = ch ? __ldcg(&a.binlim[bin0 + d]) : 0u;
-    uint32_t wb = s_misc[1], we = s_misc[2];
-    if (bin0 < wb || bin0 + nb > we) {
-      // (uniform) the row enters a partition whose slot counters are not loaded: load a window of whole partitions
-      // starting with this one (a row's tiles come in partition order; a row usually spans 1-3 partitions, which fit
-      // at once).  cnt[b - wb] = slot of the (row, b) cell's first player.
-      wb = bin0; we = bin0 + nb;
-      for (uint32_t p = s_sg[st] + 1; p <= row_p_last; ++p) {
-        const uint32_t e = a.seg_bin_lo[p + 1];
-        if (e - wb > cnt_cap) break;
-        we = e;
-      }
-      for (uint32_t i = wb + ht; i < we; i += 256) {
-        uint32_t rlo = 0, rhi = 0, v = 0;
-        if (geo_rows_of(g, a.bin_seg[i], rlo, rhi) && row >= rlo && row <= rhi) {
-          // __ldcg: these arrays are produced earlier in the same (fused) launch by other SMs
-          uint32_t pre = 0;
-          if (scanned) pre = __ldcg(&a.P[(size_t)row * a.Kp + i]);
-          else
-            for (uint32_t r = rlo; r < row; r += 8) {  // few rows per partition; 8 independent L2 loads in flight
-              uint32_t v8[8];
-#pragma unroll
-              for (uint32_t u = 0; u < 8; ++u) v8[u] = r + u < row ? __ldcg(&a.M[(size_t)(r + u) * a.Kp + i]) : 0u;
-#pragma unroll
-              for (uint32_t u = 0; u < 8; ++u) pre += v8[u];
-            }
-          v = __ldcg(&a.outbase[i]) + pre;
-        }
-        cnt[i - wb] = v;
-      }
-      bar_sync_half(h);  // the window is loaded, and every thread of the half has read the old bounds
-      if (ht == 0) { s_misc[1] = wb; s_misc[2] = we; }
-    }
-    uint32_t base = 0;  // global slot of the tile's first player of key d
-    if (d < nb) { base = cnt[bin0 - wb + d]; cnt[bin0 - wb + d] = base + ch; }
-    mbar_arrive(hand);  // tile t+1 may take its slot bases
 
     uint32_t incl = ch;  // inclusive scan of the histogram row inside the warp; the warp totals cross barrier A
 #pragma unroll
@@ -276,6 +277,58 @@ __device__ __forceinline__ uint32_t place_halves(unsigned char* smem_raw, const 
       }
     }
     bar_sync_half(h);  // A: per-warp digit counts and histogram-row warp totals complete
+
+    // ---------------- slot bases: the half's first tile waits for the other CTAs' outputs, every tile for t-1 ----------------
+    if (t == h) {
+      if (a.trace && tid == 0) atomicMax(&a.trace[4], global_ns());  // first tile ranked
+      wait_inputs(h);
+    }
+    const uint32_t ck0 = (uint32_t)clock();
+    if (t) mbar_wait(hand, (t - 1) & 1u);  // tile t-1 has taken its slot bases
+    if (ht == 0) ck[0] += (uint32_t)clock() - ck0;
+    const uint32_t lim = ch ? __ldcg(&a.binlim[bin0 + d]) : 0u;
+    uint32_t wb = s_misc[1], we = s_misc[2];
+    if (bin0 < wb || bin0 + nb > we) {
+      // (uniform) the row enters a partition whose slot counters are not loaded: load a window of whole partitions
+      // starting with this one (a row's tiles come in partition order; a row usually spans 1-3 partitions, which fit
+      // at once).  cnt[b - wb] = slot of the (row, b) cell's first player.  Every partition of the row is loaded by
+      // exactly one window, which also adds its bins' leftovers in earlier rows to left_before.
+      wb = bin0; we = bin0 + nb;
+      for (uint32_t p = s_sg[st] + 1; p <= row_p_last; ++p) {
+        const uint32_t e = a.seg_bin_lo[p + 1];
+        if (e - wb > cnt_cap) break;
+        we = e;
+      }
+      for (uint32_t i = wb + ht; i < we; i += 256) {
+        uint32_t rlo = 0, rhi = 0, v = 0;
+        const uint32_t p = a.bin_seg[i];
+        if (geo_rows_of(g, p, rlo, rhi) && row >= rlo && row <= rhi) {
+          // __ldcg: these arrays are produced earlier in the same (fused) launch by other SMs
+          uint32_t pre = 0;
+          if (scanned) pre = __ldcg(&a.P[(size_t)row * a.Kp + i]);
+          else
+            for (uint32_t r = rlo; r < row; r += 8) {  // few rows per partition; 8 independent L2 loads in flight
+              uint32_t v8[8];
+#pragma unroll
+              for (uint32_t u = 0; u < 8; ++u) v8[u] = r + u < row ? __ldcg(&a.M[(size_t)(r + u) * a.Kp + i]) : 0u;
+#pragma unroll
+              for (uint32_t u = 0; u < 8; ++u) pre += v8[u];
+            }
+          v = __ldcg(&a.outbase[i]) + pre;
+          if (p - row_p0 < kLeftBeforeCap) {
+            const uint32_t bl = __ldcg(&a.binlim[i]);
+            if (v > bl) atomicAdd(&s_lb[p - row_p0], v - bl < pre ? v - bl : pre);
+          }
+        }
+        cnt[i - wb] = v;
+      }
+      bar_sync_half(h);  // the window is loaded, and every thread of the half has read the old bounds
+      if (ht == 0) { s_misc[1] = wb; s_misc[2] = we; }
+    }
+    uint32_t base = 0;  // global slot of the tile's first player of key d
+    if (d < nb) { base = cnt[bin0 - wb + d]; cnt[bin0 - wb + d] = base + ch; }
+    mbar_arrive(hand);  // tile t+1 may take its slot bases
+    if (a.trace && t == 0 && tid == 0) atomicMax(&a.trace[7], global_ns());  // first slot bases taken
 
     uint32_t n_live = 0, l0 = 0;
 #pragma unroll
@@ -362,6 +415,7 @@ __device__ __forceinline__ uint32_t place_halves(unsigned char* smem_raw, const 
     ck[3] = (uint32_t)clock() - ck[3];
     for (uint32_t k = 0; k < 4; ++k) atomicAdd(&a.ctr->stall[h][k], (unsigned long long)ck[k]);
   }
+  if (h == 0 && n_tiles == 0) wait_inputs(0u);  // a row without tiles still leaves with the inputs visible
 
   if (lane == 0 && nleft) atomicAdd(&s_misc[0], nleft);
   __syncthreads();
@@ -373,10 +427,11 @@ __device__ __forceinline__ uint32_t place_halves(unsigned char* smem_raw, const 
   return n_res;
 }
 
+// wait_inputs(h): see place_halves (this path calls it for both halves at once, before its first tile)
 template <int BLOCK, class Wait>
 __device__ __forceinline__ uint32_t place_body(unsigned char* smem_raw, const Geo& g, const PlaceArgs a, Wait&& wait_inputs) {
   static_assert(BLOCK == 512 && kTile == 2048, "tile arrangement is written for 512 threads x 4 players");
-  if (a.meta.chist && a.fast_ok) {  // (uniform) every partition has <= 255 keys
+  if (place_on_halves(a)) {  // (uniform) every partition has <= 255 keys
     return place_halves<BLOCK>(smem_raw, g, a, wait_inputs);
   }
   constexpr int J = kTile / BLOCK;
@@ -440,7 +495,7 @@ __device__ __forceinline__ uint32_t place_body(unsigned char* smem_raw, const Ge
   if (tid == 0)
     for (uint32_t t = 0; t < stages && t < n_tiles; ++t) issue(t, t);
   for (uint32_t i = tid; i < kHeadSlots + NW * 128; i += BLOCK) head[i] = 0;  // LIST heads = FAST mask table; + FAST counters
-  wait_inputs();
+  wait_inputs(tid >> 8);
   const bool heavy = __ldcg(&a.ctr->heavy) != 0;  // (written by the tail)
   __syncthreads();
 
