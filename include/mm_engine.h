@@ -136,13 +136,15 @@ int mm_group_of(const mm_config* cfg, int32_t rating);
  * mm_enqueue replaces, per player: Middleware dedupe + ActiveUser.add_user
  * (middleware/worker.ex:65-70, models/active_user.ex:46-55) and the publish of the
  * request to the group queue (generic/worker.ex:55-69).  Players are appended in
- * call order = enqueue order.  accepted[i]: 1 = queued, 0 = "already in the queue"
- * (also for a repeat inside the same batch: first occurrence wins), 2 = invalid
- * mode / id / rating without a default group, 3 = pool full (the LAST players of the
- * batch that do not fit).  A batch the active set cannot hold at all (more than
- * active_capacity ids resident) is refused as a whole with MM_E_CAP — nothing is
- * enqueued, the caller nacks / retries after mm_remove.  enq_ts may be NULL (stored 0).
- * Every offered player (accepted or not) consumes one enqueue sequence number.     */
+ * call order = enqueue order.  accepted[i]: 1 = queued, 0 = "already in the queue",
+ * 2 = invalid mode / id / rating without a default group, 3 = pool full (the LAST
+ * players of the batch that do not fit).  A repeat inside the batch follows its first
+ * occurrence: 0 if that was queued, 3 if it did not fit.  A removed or taken player
+ * holds its pool slot until the next tick.  A batch the active set cannot hold at all
+ * (more than active_capacity ids resident) is refused as a whole with MM_E_CAP —
+ * nothing is enqueued and no sequence number is consumed; the caller nacks / retries
+ * after mm_remove.  enq_ts may be NULL (stored 0).  Every offered player of an
+ * accepted batch (queued or not) consumes one enqueue sequence number.             */
 int mm_enqueue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating,
                const uint8_t* mode, const uint32_t* enq_ts, uint8_t* accepted);
 /* Same, all five pointers are DEVICE pointers (accepted may be NULL).              */
@@ -170,7 +172,8 @@ int mm_enqueue_packed_end(mm_engine* e, uint8_t* accepted, uint32_t* n_accepted)
 
 /* The ack / nack list of the LAST mm_enqueue* batch without a per-player transfer: the batch indices whose code is
  * not 1 (unordered) and their codes — pass accepted = NULL to mm_enqueue* and ack everything else
- * (search/worker.ex:323 acks per delivery).  MM_E_CAP if there are more than cap (n_rejects says how many).   */
+ * (search/worker.ex:323 acks per delivery).  MM_E_CAP if there are more than cap (n_rejects says how many).
+ * mm_in_queue, mm_remove, mm_take and a refused batch in between do not change the list.                      */
 int mm_enqueue_rejects(mm_engine* e, uint32_t cap, uint32_t* index, uint8_t* code, uint32_t* n_rejects);
 
 /* Replaces ActiveUser.remove_user/1 (models/active_user.ex:57-66; callers

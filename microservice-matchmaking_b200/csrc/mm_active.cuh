@@ -66,8 +66,9 @@ __global__ void k_enq_claim(uint32_t base, uint32_t n, const uint64_t* __restric
 
 // ---- only when n_pool + batch could exceed the capacity: exact "the last ones do not fit" cut --------------------
 // winners = entries whose PENDING index is their own; per-block winner counts.  A chunk's winners are final once
-// every lower batch index has claimed.
-__global__ void k_enq_count(uint32_t base, uint32_t n, ActiveView act, const uint64_t* __restrict__ hslot,
+// every lower batch index has claimed.  A loser keeps PENDING | its winner's index in hslot (unused by the later
+// kernels): k_enq_promote gives it the winner's final code.
+__global__ void k_enq_count(uint32_t base, uint32_t n, ActiveView act, uint64_t* __restrict__ hslot,
                             uint8_t* __restrict__ code, uint32_t* __restrict__ blocksum) {
   __shared__ uint32_t s_cnt;
   if (threadIdx.x == 0) s_cnt = 0;
@@ -76,8 +77,9 @@ __global__ void k_enq_count(uint32_t base, uint32_t n, ActiveView act, const uin
   const uint32_t i = base + t;
   bool win = false;
   if (t < n && code[i] == 1) {
-    win = !act.on() || *act.val(hslot[i]) == (kPending | i);
-    if (!win) code[i] = 0;  // a lower batch index holds the id
+    const unsigned long long v = act.on() ? *act.val(hslot[i]) : (kPending | i);
+    win = v == (kPending | i);
+    if (!win) { code[i] = 0; hslot[i] = v; }  // a lower batch index of this chunk holds the id
   }
   const uint32_t b = __ballot_sync(0xFFFFFFFFu, win);
   if ((threadIdx.x & 31) == 0 && b) atomicAdd(&s_cnt, (uint32_t)__popc(b));
@@ -130,6 +132,16 @@ __global__ void k_enq_cut(uint32_t base, uint32_t n, ActiveView act, const uint6
     }
     atomicAdd(n_rejected_cap, 1u);
   }
+}
+// a repeat whose batch winner was rolled back did not fit either: code 3, as if the repeat had been offered alone
+// (it holds no active-set entry, so it is not counted in n_rejected_cap, which feeds the tombstone count)
+__global__ void k_enq_promote(uint32_t base, uint32_t n, const uint64_t* __restrict__ hslot, uint8_t* __restrict__ code) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= n) return;
+  const uint32_t i = base + t;
+  if (code[i] != 0) return;
+  const uint64_t v = hslot[i];
+  if (v >= kPending && code[(uint32_t)v] == 3) code[i] = 3;
 }
 
 // E2: winners per (ingest block, partition).  blockhist is [n_segs][nblk].

@@ -121,11 +121,15 @@ struct mm_engine {
   uint32_t enq_cap = 0;
   uint64_t *d_in_id = nullptr, *d_hslot = nullptr;
   int32_t* d_in_rating = nullptr;
-  uint8_t *d_in_mode = nullptr, *d_code = nullptr;
+  uint8_t *d_in_mode = nullptr, *d_lookup = nullptr;
   uint16_t *d_part = nullptr, *d_in_key = nullptr;
   uint32_t *d_in_ts = nullptr, *d_in_handle = nullptr, *d_blocksum = nullptr, *d_blockhist = nullptr;
   uint32_t* d_small = nullptr;  // [0] accepted  [1] rejected: pool full  [2] removed  [3] running winner total (cut)
   uint32_t* h_small = nullptr;  // pinned
+  // codes of the last ingest batch: grown only by an ingest batch that passed its capacity check, written only by
+  // ingest, so mm_enqueue_rejects reads them whatever ran since
+  uint8_t* d_code = nullptr;
+  uint32_t code_cap = 0;
   uint32_t last_batch_n = 0;    // entries of the last ingest batch (their codes are still in d_code)
   uint32_t* d_rej_idx = nullptr; uint8_t* d_rej_code = nullptr; uint32_t rej_cap = 0;
 
@@ -403,7 +407,7 @@ int alloc_tick_scratch(mm_engine* e) {
 int ensure_enq_scratch(mm_engine* e, uint32_t n) {
   if (n <= e->enq_cap) return MM_OK;
   cudaFree(e->d_in_id); cudaFree(e->d_hslot); cudaFree(e->d_in_rating); cudaFree(e->d_in_mode);
-  cudaFree(e->d_code); cudaFree(e->d_in_ts); cudaFree(e->d_blocksum); cudaFree(e->d_part); cudaFree(e->d_in_key);
+  cudaFree(e->d_lookup); cudaFree(e->d_in_ts); cudaFree(e->d_blocksum); cudaFree(e->d_part); cudaFree(e->d_in_key);
   cudaFree(e->d_in_handle);
   e->enq_cap = 0;
   const size_t c = (size_t)n + 64;
@@ -411,7 +415,7 @@ int ensure_enq_scratch(mm_engine* e, uint32_t n) {
   CK(cudaMalloc(&e->d_hslot, c * 8));
   CK(cudaMalloc(&e->d_in_rating, c * 4));
   CK(cudaMalloc(&e->d_in_mode, c));
-  CK(cudaMalloc(&e->d_code, c));
+  CK(cudaMalloc(&e->d_lookup, c));
   CK(cudaMalloc(&e->d_part, c * 2));
   CK(cudaMalloc(&e->d_in_key, c * 2));
   CK(cudaMalloc(&e->d_in_handle, c * 4));
@@ -448,6 +452,12 @@ int enq_prepare(mm_engine* e, uint32_t n) {
     }
     if ((rc = rehash(e))) return rc;
   }
+  if (n > e->code_cap) {  // the batch is taken: the previous batch's codes may go
+    cudaFree(e->d_code);
+    e->d_code = nullptr; e->code_cap = 0; e->last_batch_n = 0;
+    CK(cudaMalloc(&e->d_code, (size_t)n + 64));
+    e->code_cap = n;
+  }
   CK(cudaMemsetAsync(e->d_small, 0, 16, e->stream));
   return MM_OK;
 }
@@ -465,6 +475,7 @@ int enq_chunk(mm_engine* e, uint32_t base, uint32_t cnt, const uint64_t* id, con
     k_enq_count<<<nb, 256, 0, e->stream>>>(base, cnt, av, e->d_hslot, e->d_code, e->d_blocksum);
     k_scan_small<<<1, 1024, 0, e->stream>>>(nb, e->d_blocksum, e->d_small + 3);
     k_enq_cut<<<nb, 256, 0, e->stream>>>(base, cnt, av, e->d_hslot, e->d_code, e->d_blocksum, room, e->d_small + 1);
+    if (e->use_active) k_enq_promote<<<nb, 256, 0, e->stream>>>(base, cnt, e->d_hslot, e->d_code);
   }
   k_enq_route<<<nblk, 256, 0, e->stream>>>(base, cnt, av, e->d_hslot, e->d_code, e->d_part, e->n_segs, nblk, e->d_blockhist);
   k_enq_alloc<<<1, 512, 0, e->stream>>>(e->n_segs, nblk, e->d_blockhist, p.m, e->d_small);
@@ -902,7 +913,7 @@ int mm_destroy(mm_engine* e) {
   cudaFree(e->d_M); cudaFree(e->d_P); cudaFree(e->d_outbase); cudaFree(e->d_binlim); cudaFree(e->d_bin_seg);
   cudaFree(e->d_bin_key); cudaFree(e->d_seg); cudaFree(e->d_members); cudaFree(e->d_members32); cudaFree(e->d_members32_alt); cudaFree(e->d_hdr_alt); cudaFree(e->d_src_idx);
   cudaFree(e->d_hdr); cudaFree(e->d_emit_seq); cudaFree(e->d_ctr2); cudaFree(e->d_small);
-  cudaFree(e->d_in_id); cudaFree(e->d_hslot); cudaFree(e->d_in_rating); cudaFree(e->d_in_mode); cudaFree(e->d_code);
+  cudaFree(e->d_in_id); cudaFree(e->d_hslot); cudaFree(e->d_in_rating); cudaFree(e->d_in_mode); cudaFree(e->d_code); cudaFree(e->d_lookup);
   cudaFree(e->d_in_ts); cudaFree(e->d_blocksum); cudaFree(e->d_blockhist); cudaFree(e->d_part); cudaFree(e->d_in_key);
   cudaFree(e->d_in_handle); cudaFree(e->d_rej_idx); cudaFree(e->d_rej_code);
   cudaFree(e->d_qstat);
@@ -1185,9 +1196,9 @@ int mm_in_queue(mm_engine* e, uint32_t n, const uint64_t* id, uint8_t* out) {
   int rc = ensure_enq_scratch(e, n);
   if (rc) return rc;
   CK(cudaMemcpyAsync(e->d_in_id, id, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
-  k_lookup<<<(n + 255) / 256, 256, 0, e->stream>>>(n, e->d_in_id, act_view(e), e->d_code);
+  k_lookup<<<(n + 255) / 256, 256, 0, e->stream>>>(n, e->d_in_id, act_view(e), e->d_lookup);
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(out, e->d_code, n, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(out, e->d_lookup, n, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   return MM_OK;
 }
