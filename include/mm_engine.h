@@ -278,7 +278,13 @@ typedef struct mm_queue_stat {
 int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap, uint32_t* n_out);
 
 /* Device-side snapshot / restore of pool + active set (ram_copies analogue,
- * models/active_user.ex:20; used by bench.py to replay one pool K times).          */
+ * models/active_user.ex:20; used by bench.py to replay one pool K times).
+ * mm_snapshot copies the queued players, the enqueue sequence counter and the whole active set (every id queued or
+ * matched and not yet removed, with the counts behind mm_active_size and the refusal rule of a hashed set).
+ * mm_restore puts all of it back, any number of times: an id enqueued since the snapshot can be offered again, an id
+ * removed since is queued and removable again.  The snapshot of the active set takes 16 B per hashed slot (8 B per
+ * handle with MM_F_DENSE_IDS) of device memory beside the pool's copy; MM_F_NO_DEDUPE engines have no active set.
+ * The last tick's match section of mm_queue_stats is void after mm_restore.                                          */
 int mm_snapshot(mm_engine* e);
 int mm_restore(mm_engine* e);
 

@@ -352,7 +352,8 @@ __global__ void k_remove(uint32_t n, const uint64_t* __restrict__ id, ActiveView
     *act.val(h) = kFreeVal;
   }
   const uint32_t slot = (uint32_t)v, g = (uint32_t)(v >> 32);
-  if (v < kPending && g == gen && slot < n_slots && pool.id[slot] == pid) {
+  // a player taken since the tick (mm_take) is dead already: its bin totals and chunk histogram were updated then
+  if (v < kPending && g == gen && slot < n_slots && pool.id[slot] == pid && pool.mode[slot] != MM_MODE_DEAD) {
     pool.mode[slot] = MM_MODE_DEAD;
     pool_mark_dead(pool, meta, slot, dead_bin, bin_seg, seg_bin_lo);
   }

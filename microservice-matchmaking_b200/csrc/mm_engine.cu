@@ -86,6 +86,8 @@ struct mm_engine {
   Table tab[2];
   int tcur = 0;
   uint64_t n_active = 0, n_tomb = 0;
+  Table snap_tab;  // mm_snapshot: the current table, with its counts
+  uint64_t snap_active = 0, snap_tomb = 0;
 
   // tick scratch
   uint32_t R = 0;        // row CTAs of a tick
@@ -242,6 +244,8 @@ ActiveView act_view(mm_engine* e) {
   }
   return a;
 }
+
+size_t table_bytes(const mm_engine* e) { return e->hcap * (e->dense_ids ? 8 : 16); }
 
 int clear_table(mm_engine* e, Table& t) {
   if (e->dense_ids) {
@@ -908,6 +912,7 @@ int mm_destroy(mm_engine* e) {
   if (e->d2h_stream) cudaStreamSynchronize(e->d2h_stream);
   free_pool(e->pool[0]); free_pool(e->pool[1]); free_pool(e->snap); cudaFree(e->d_left_bits);
   for (auto& t : e->tab) cudaFree(t.kv);
+  cudaFree(e->snap_tab.kv);
   cudaFree(e->d_lut); cudaFree(e->d_grp_lut); cudaFree(e->d_mode_tsize); cudaFree(e->d_seg_bin_lo); cudaFree(e->d_seg_L);
   cudaFree(e->d_part_cut); cudaFree(e->d_cut_lp_lo);
   cudaFree(e->d_M); cudaFree(e->d_P); cudaFree(e->d_outbase); cudaFree(e->d_binlim); cudaFree(e->d_bin_seg);
@@ -1362,6 +1367,12 @@ int mm_snapshot(mm_engine* e) {
   }
   int rc = copy_pool(e, e->snap, e->pool[e->cur]);
   if (rc) return rc;
+  if (e->use_active) {  // the active set as it stands: ids queued, matched and not yet removed, tombstones
+    if (!e->snap_tab.kv) CK(cudaMalloc(&e->snap_tab.kv, table_bytes(e)));
+    CK(cudaMemcpyAsync(e->snap_tab.kv, e->tab[e->tcur].kv, table_bytes(e), cudaMemcpyDeviceToDevice, e->stream));
+    e->snap_active = e->n_active;
+    e->snap_tomb = e->n_tomb;
+  }
   CK(cudaStreamSynchronize(e->stream));
   e->snap_seq = e->seq_next;
   e->has_snap = true;
@@ -1376,6 +1387,11 @@ int mm_restore(mm_engine* e) {
   Pool& p = e->pool[e->cur];
   int rc = copy_pool(e, p, e->snap);
   if (rc) return rc;
+  if (e->use_active) {  // into whichever table is current: a rehash since the snapshot may have switched it
+    CK(cudaMemcpyAsync(e->tab[e->tcur].kv, e->snap_tab.kv, table_bytes(e), cudaMemcpyDeviceToDevice, e->stream));
+    e->n_active = e->snap_active;
+    e->n_tomb = e->snap_tomb;
+  }
   e->seq_next = e->snap_seq;
   e->gen = next_gen(e);
   e->match_valid = false;  // the restored pool was not matched by the last tick
