@@ -261,7 +261,7 @@ typedef struct mm_queue_stat {
   uint16_t reserved;
   /* the resident pool at `now` */
   uint32_t n_waiting;  /* live queued players of this (mode, group)                                     */
-  uint32_t n_removed;  /* entries removed (mm_remove / mm_take) while queued; the next tick drops them    */
+  uint32_t n_removed;  /* entries removed (mm_remove / mm_take / mm_expire) while queued; the next tick drops them */
   uint32_t max_wait;   /* longest wait among the n_waiting players (0 if none)                          */
   uint32_t wait_hist[MM_WAIT_BUCKETS];
   /* the players the LAST tick matched, at that tick's `now` (all zero before the first tick, after a tick that
@@ -276,6 +276,26 @@ typedef struct mm_queue_stat {
  * call writes until the next tick); only the records cross PCIe.  Runs on the engine's stream and leaves pending
  * async_results copies alone.                                                                                     */
 int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap, uint32_t* n_out);
+
+/* ---- search timeout ------------------------------------------------------------
+ * EXTENSION (search timeout): every live queued player whose WAIT at `now` (the definition of mm_queue_stats)
+ * is >= max_wait leaves the pool AND the active set, as if mm_remove had been called with its id: mm_in_queue
+ * reads 0, the id can be enqueued again, and the slot is dropped by the next tick (counted in its n_dead, and in
+ * mm_queue_stats' n_removed until then).  Matched, removed and taken players are not affected.  max_wait = 0
+ * expires every queued player; max_wait >= 2^31 expires none.  MM_F_NO_DEDUPE engines have no active set: only
+ * the pool changes.  The caller tells each expired player so (the reference's answer to a player it cannot
+ * serve: game-lobby/worker.ex:63-71,89-103, an error response and ActiveUser.remove_user).
+ * ids[0..*n_expired): the expired ids (unordered); seq (may be NULL): the enqueue sequence number of each (the
+ * numbering of emit_seq), which also tells apart the entries of a repeated id in an MM_F_NO_DEDUPE engine.
+ * If more than `cap` would expire: MM_E_CAP, *n_expired = the number that would, and NOTHING changes
+ * (so cap = 0 with ids = NULL is a dry run).  One pass over the resident mode and enqueue-stamp columns when cap
+ * is at least mm_pool_size, else a counting pass first.  Runs on the engine's stream; pending async_results
+ * copies are left alone; the last tick's match section of mm_queue_stats is unaffected.                        */
+int mm_expire(mm_engine* e, uint64_t now, uint32_t max_wait, uint64_t* ids, uint32_t* seq, uint32_t cap,
+              uint32_t* n_expired);
+/* Same, ids returned as 32-bit handles (MM_F_DENSE_IDS engines; MM_E_STATE otherwise). */
+int mm_expire_packed(mm_engine* e, uint64_t now, uint32_t max_wait, uint32_t* handles, uint32_t* seq,
+                     uint32_t cap, uint32_t* n_expired);
 
 /* Device-side snapshot / restore of pool + active set (ram_copies analogue,
  * models/active_user.ex:20; used by bench.py to replay one pool K times).

@@ -182,6 +182,24 @@ static ERL_NIF_TERM nif_queue_stats(ErlNifEnv* env, int argc, const ERL_NIF_TERM
   return rc ? err(env, rc) : enif_make_tuple2(env, atom(env, "ok"), out);
 }
 
+/* expire_packed(ref, now_ms, max_wait_ms) -> {:ok, handles :: binary(u32[])}: search timeout (extension) — the
+ * queued players who have waited >= max_wait_ms leave the pool and the active set; the caller answers each one */
+static ERL_NIF_TERM nif_expire_packed(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifUInt64 now; unsigned int max_wait; uint32_t n = 0, got = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_uint64(env, argv[1], &now) ||
+      !enif_get_uint(env, argv[2], &max_wait))
+    return enif_make_badarg(env);
+  if (mm_pool_size(r->e, &n)) return err(env, MM_E_ARG);
+  ErlNifBinary hs;
+  if (!enif_alloc_binary((size_t)n * 4 + 4, &hs)) return err(env, MM_E_CAP);
+  /* cap = every resident player: the engine makes a single pass */
+  int rc = mm_expire_packed(r->e, now, (uint32_t)max_wait, (uint32_t*)hs.data, NULL, n, &got);
+  if (rc) { enif_release_binary(&hs); return err(env, rc); }
+  enif_realloc_binary(&hs, (size_t)got * 4);
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &hs));
+}
+
 /* set_max_spread(ref, w): extension knob (strategist policy S1); w < 0 restores the reference behaviour */
 static ERL_NIF_TERM nif_set_max_spread(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
   engine_res* r; ErlNifSInt64 w = -1;
@@ -204,6 +222,7 @@ static ErlNifFunc funcs[] = {
   {"tick_packed", 2, nif_tick_packed, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"status", 1, nif_status, 0},
   {"queue_stats", 2, nif_queue_stats, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"expire_packed", 3, nif_expire_packed, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"set_max_spread", 2, nif_set_max_spread, 0},
 };
 ERL_NIF_INIT(Elixir.Matchmaking.Search.Engine, funcs, load, NULL, NULL, NULL)

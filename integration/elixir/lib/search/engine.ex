@@ -56,6 +56,11 @@ defmodule Matchmaking.Search.Engine do
   def status(_ref), do: :erlang.nif_error(:nif_not_loaded)
   @doc "-> {:ok, binary(mm_queue_stat[])}: per (mode, group) queue, waiting players and wait histograms (include/mm_engine.h)"
   def queue_stats(_ref, _now_ms), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Extension (search timeout): the queued players who have waited >= max_wait_ms at now_ms leave the pool and the
+  active set, as if removed -> {:ok, handles :: binary(u32[])}; the caller answers each one.
+  """
+  def expire_packed(_ref, _now_ms, _max_wait_ms), do: :erlang.nif_error(:nif_not_loaded)
 
   @doc "Extension (not reference behaviour): maximum rating spread of a lobby for the following ticks; < 0 = off."
   def set_max_spread(_ref, _w), do: :erlang.nif_error(:nif_not_loaded)

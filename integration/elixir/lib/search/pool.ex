@@ -12,6 +12,9 @@ defmodule Matchmaking.Search.Pool do
       in_queue?/1, remove_user/1    replace Matchmaking.Model.ActiveUser (models/active_user.ex:33-66)
       queue_status/1 one rating group's queues (Engine.queue_stats): waiting players, oldest / p50 / p99 wait, the
                      last tick's matched players and p99 wait at match, in ms — Search.Worker.status/0's queue depth
+      search_timeout_ms   option (extension, default nil = off): after each tick's lobbies are published, the players
+                     still queued who have waited at least this long leave the pool (Engine.expire_packed) and get the
+                     error response of game-lobby/worker.ex:63-71,105-116 on their "response-queue"
 
   Every batch is stamped with the pool's clock (ms since the pool started, modulo 2^32) and every tick passes the same
   clock as its `now`, so the engine's waits are in milliseconds.
@@ -28,6 +31,8 @@ defmodule Matchmaking.Search.Pool do
 
   @exchange_forward "open-matchmaking.matchmaking.game-lobby.direct"   # search/worker.ex:31
   @queue_forward "matchmaking.queues.lobbies"                          # search/worker.ex:32
+  @exchange_response "open-matchmaking.responses.direct"               # game-lobby/worker.ex:27
+  @timeout_details "No opponents were found within the search time limit."
   @max_batch 65_536
   @flush_ms 2
   @tick_ms 5
@@ -45,7 +50,7 @@ defmodule Matchmaking.Search.Pool do
     Process.send_after(self(), :flush, @flush_ms)
     Process.send_after(self(), :tick, @tick_ms)
     {:ok, %{ref: ref, staged: [], n_staged: 0, handle_of: %{}, players: %{}, free: [], next: 0, channel: nil,
-            t0: System.monotonic_time(:millisecond)}}
+            t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms)}}
   end
 
   @impl true
@@ -98,9 +103,38 @@ defmodule Matchmaking.Search.Pool do
   def handle_info(:tick, st) do
     Process.send_after(self(), :tick, @tick_ms)
     st = flush(st)
-    case Engine.tick_packed(st.ref, now_ms(st)) do
-      {:ok, lobbies, members, _stats} -> {:noreply, publish(lobbies, members, st)}
+    now = now_ms(st)
+    case Engine.tick_packed(st.ref, now) do
+      {:ok, lobbies, members, _stats} -> {:noreply, expire(publish(lobbies, members, st), now)}
       {:error, _reason} -> {:noreply, st}                              # nothing was consumed; the next tick retries
+    end
+  end
+
+  # -- search timeout (extension): after the lobbies, so a player the tick matched is never timed out ---------------
+  defp expire(%{timeout: nil} = st, _now), do: st
+  defp expire(st, now) do
+    case Engine.expire_packed(st.ref, now, st.timeout) do
+      {:ok, handles} ->
+        for <<h::little-32 <- handles>>, reduce: st do
+          acc ->
+            {player, players} = Map.pop(acc.players, h)
+            send_timeout(acc.channel, player)
+            %{acc | players: players, handle_of: Map.delete(acc.handle_of, player["id"]), free: [h | acc.free]}
+        end
+      {:error, _reason} -> st                                          # nothing changed; the next tick retries
+    end
+  end
+
+  defp send_timeout(channel, player) do
+    case player["response-queue"] do
+      nil -> :ok
+      queue ->
+        payload = Poison.encode!(%{"error" => %{"type" => "MatchmakingError", "details" => @timeout_details},
+                                   "event-name" => player["event-name"]})
+        Matchmaking.Search.Worker.safe_run(channel, fn channel ->
+          AMQP.Basic.publish(channel, @exchange_response, queue, payload,
+            persistent: true, content_type: "application/json")
+        end)
     end
   end
 

@@ -119,6 +119,8 @@ PROTOTYPES = {
     "mm_results_device": (C.c_int, [_vp, _P(_vp), _P(_vp)]),
     "mm_pool_read": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _P(C.c_uint32)]),
     "mm_queue_stats": (C.c_int, [_vp, C.c_uint64, _vp, C.c_uint32, _P(C.c_uint32)]),
+    "mm_expire": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
+    "mm_expire_packed": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_snapshot": (C.c_int, [_vp]),
     "mm_restore": (C.c_int, [_vp]),
     "mm_set_stream": (C.c_int, [_vp, _vp]),

@@ -17,6 +17,7 @@
 #include <new>
 #include <vector>
 
+#include "mm_expire.cuh"
 #include "mm_kernels.cuh"
 #include "mm_stats.cuh"
 
@@ -126,7 +127,9 @@ struct mm_engine {
   uint8_t *d_in_mode = nullptr, *d_lookup = nullptr;
   uint16_t *d_part = nullptr, *d_in_key = nullptr;
   uint32_t *d_in_ts = nullptr, *d_in_handle = nullptr, *d_blocksum = nullptr, *d_blockhist = nullptr;
-  uint32_t* d_small = nullptr;  // [0] accepted  [1] rejected: pool full  [2] removed  [3] running winner total (cut)
+  // [0] accepted  [1] rejected: pool full  [2] removed  [3] running winner total (cut)  [4] rejects
+  // [8] expired  [9] active-set entries erased by mm_expire
+  uint32_t* d_small = nullptr;
   uint32_t* h_small = nullptr;  // pinned
   // codes of the last ingest batch: grown only by an ingest batch that passed its capacity check, written only by
   // ingest, so mm_enqueue_rejects reads them whatever ran since
@@ -155,6 +158,12 @@ struct mm_engine {
   uint32_t tick_now = 0;     // `now` of the tick in progress / the last tick (mod 2^32)
   uint32_t match_n = 0;      // players resident when that tick started: bounds its tile count
   uint32_t* d_qstat = nullptr;  // [n_cut] records
+
+  // mm_expire output (grown on demand to the largest output a call could write; not d_members / d_hdr, which
+  // mm_results_device hands out until the next tick)
+  uint64_t* d_exp_id = nullptr;  // ids, or 32-bit handles in its first half
+  uint32_t* d_exp_seq = nullptr;
+  uint32_t exp_cap = 0;
 };
 
 namespace {
@@ -757,6 +766,66 @@ int tick_to_host(mm_engine* e, mm_lobby_hdr* lobbies, uint32_t lobby_cap, uint64
   return MM_OK;
 }
 
+// mm_expire / mm_expire_packed (one of ids / handles).  A cap that holds every resident player cannot overflow: one
+// pass.  Otherwise a counting pass decides first, so that a refused call leaves everything as it was.
+int expire(mm_engine* e, uint64_t now, uint32_t max_wait, uint64_t* ids, uint32_t* handles, uint32_t* seq, uint32_t cap,
+           uint32_t* n_expired) {
+  const Pool& p = e->pool[e->cur];
+  *n_expired = 0;
+  if (p.n == 0) return MM_OK;
+  ExpireArgs a{};
+  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.now = (uint32_t)now; a.max_wait = max_wait;
+  a.act = act_view(e); a.gen = e->gen; a.dead_bin = e->K; a.bin_seg = e->d_bin_seg; a.seg_bin_lo = e->d_seg_bin_lo;
+  a.ctr = e->d_small + 8;
+  // CTAs: at most the tiles in use, at most 8 per SM; each takes a contiguous run of tiles
+  const uint64_t tiles = (uint64_t)p.n / kTile + e->n_segs;
+  const uint32_t ctas = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(tiles, 8ull * (uint32_t)e->n_sms));
+  uint32_t need = p.n;
+  if (cap < p.n) {
+    CK(cudaMemsetAsync(a.ctr, 0, 8, e->stream));
+    k_expire<kExpBlock><<<ctas, kExpBlock, 0, e->stream>>>(a);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(e->h_small + 8, a.ctr, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    need = e->h_small[8];
+    *n_expired = need;
+    if (need > cap) {
+      std::snprintf(e->last_err, sizeof(e->last_err), "need cap >= %u", need);
+      return MM_E_CAP;
+    }
+    if (need == 0) return MM_OK;
+  }
+  if (need > e->exp_cap || (seq && !e->d_exp_seq)) {
+    const uint32_t c = std::max(need, e->exp_cap);
+    cudaFree(e->d_exp_id); cudaFree(e->d_exp_seq);
+    e->d_exp_id = nullptr; e->d_exp_seq = nullptr; e->exp_cap = 0;
+    CK(cudaMalloc(&e->d_exp_id, (size_t)c * 8));
+    if (seq) CK(cudaMalloc(&e->d_exp_seq, (size_t)c * 4));
+    e->exp_cap = c;
+  }
+  a.commit = 1;
+  a.out_id = ids ? e->d_exp_id : nullptr;
+  a.out_handle = ids ? nullptr : reinterpret_cast<uint32_t*>(e->d_exp_id);
+  a.out_seq = seq ? e->d_exp_seq : nullptr;
+  CK(cudaMemsetAsync(a.ctr, 0, 8, e->stream));
+  k_expire<kExpBlock><<<ctas, kExpBlock, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(e->h_small + 8, a.ctr, 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  const uint32_t n = e->h_small[8], erased = e->h_small[9];
+  if (n) {
+    if (ids) CK(cudaMemcpyAsync(ids, e->d_exp_id, (size_t)n * 8, cudaMemcpyDeviceToHost, e->stream));
+    else CK(cudaMemcpyAsync(handles, e->d_exp_id, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
+    if (seq) CK(cudaMemcpyAsync(seq, e->d_exp_seq, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+  }
+  // active-set bookkeeping as mm_remove's
+  e->n_active -= std::min<uint64_t>(erased, e->n_active);
+  if (e->use_active && !e->dense_ids) e->n_tomb += erased;
+  *n_expired = n;
+  return MM_OK;
+}
+
 }  // namespace
 
 // =======================================================================================
@@ -921,7 +990,7 @@ int mm_destroy(mm_engine* e) {
   cudaFree(e->d_in_id); cudaFree(e->d_hslot); cudaFree(e->d_in_rating); cudaFree(e->d_in_mode); cudaFree(e->d_code); cudaFree(e->d_lookup);
   cudaFree(e->d_in_ts); cudaFree(e->d_blocksum); cudaFree(e->d_blockhist); cudaFree(e->d_part); cudaFree(e->d_in_key);
   cudaFree(e->d_in_handle); cudaFree(e->d_rej_idx); cudaFree(e->d_rej_code);
-  cudaFree(e->d_qstat);
+  cudaFree(e->d_qstat); cudaFree(e->d_exp_id); cudaFree(e->d_exp_seq);
   if (e->h_ctr) cudaFreeHost(e->h_ctr);
   if (e->h_small) cudaFreeHost(e->h_small);
   for (auto& ev : e->ev)
@@ -1355,6 +1424,23 @@ int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap,
     out[c].n_lobbies = out[c].n_matched / ((uint32_t)md.teams * md.team_size);  // whole lobbies of L players
   }
   return MM_OK;
+}
+
+int mm_expire(mm_engine* e, uint64_t now, uint32_t max_wait, uint64_t* ids, uint32_t* seq, uint32_t cap,
+              uint32_t* n_expired) {
+  if (!e || !n_expired || (cap && !ids)) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  return expire(e, now, max_wait, ids, nullptr, seq, cap, n_expired);
+}
+
+int mm_expire_packed(mm_engine* e, uint64_t now, uint32_t max_wait, uint32_t* handles, uint32_t* seq, uint32_t cap,
+                     uint32_t* n_expired) {
+  if (!e || !n_expired || (cap && !handles)) return MM_E_ARG;
+  if (!(e->cfg.flags & MM_F_DENSE_IDS)) return MM_E_STATE;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  return expire(e, now, max_wait, nullptr, handles, seq, cap, n_expired);
 }
 
 int mm_snapshot(mm_engine* e) {

@@ -341,6 +341,24 @@ class Engine:
                     "mm_queue_stats")
         return out[:n.value]
 
+    def expire(self, now, max_wait, want_seq=True):
+        """Search timeout (mm_expire): every queued player whose wait at `now` (as queue_stats counts it) is >=
+        max_wait leaves the pool and the active set, like remove(). -> (ids u64, enqueue seq u32 | None), unordered."""
+        return self._expire(self.lib.mm_expire, np.uint64, now, max_wait, want_seq, "mm_expire")
+
+    def expire_packed(self, now, max_wait, want_seq=True):
+        """expire() on an MM_F_DENSE_IDS engine, ids as u32 handles (mm_expire_packed)."""
+        return self._expire(self.lib.mm_expire_packed, np.uint32, now, max_wait, want_seq, "mm_expire_packed")
+
+    def _expire(self, fn, dtype, now, max_wait, want_seq, what):
+        cap = self.pool_size()  # every resident player fits: the engine makes a single pass
+        ids = np.empty(max(cap, 1), dtype)
+        seq = np.empty(max(cap, 1), np.uint32) if want_seq else None
+        n = C.c_uint32(0)
+        max_wait = max(0, min(int(max_wait), 0xFFFFFFFF))
+        self._check(fn(self.h, int(now) & 0xFFFFFFFFFFFFFFFF, max_wait, _p(ids), _p(seq), cap, C.byref(n)), what)
+        return ids[:n.value], (seq[:n.value] if seq is not None else None)
+
     def snapshot(self):
         self._check(self.lib.mm_snapshot(self.h), "mm_snapshot")
 

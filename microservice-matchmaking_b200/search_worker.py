@@ -42,6 +42,14 @@ EXCHANGE_FORWARD = "open-matchmaking.matchmaking.game-lobby.direct"
 QUEUE_FORWARD = "matchmaking.queues.lobbies"
 EXCHANGE_REQUEUE = "open-matchmaking.matchmaking.requeue.direct"
 QUEUE_REQUEUE = "matchmaking.games.requeue"
+EXCHANGE_RESPONSE = "open-matchmaking.responses.direct"  # game-lobby/worker.ex:27
+TIMEOUT_DETAILS = "No opponents were found within the search time limit."
+
+
+def prepare_timeout_response(player):
+    """The error response of game-lobby/worker.ex:63-71 with the search timeout as its cause."""
+    return json.dumps({"error": {"type": "MatchmakingError", "details": TIMEOUT_DETAILS},
+                       "event-name": player.get("event-name")})
 
 
 def generate_queue_name(suffix):  # worker.ex:46-48
@@ -144,6 +152,9 @@ class SearchPool:
     delivery is acked only once its player is resident, so the broker must be allowed that many unacked messages);
     flush_every_s: an ingest also happens when the oldest staged delivery has waited this long (and at every tick);
     window: optional WindowSchedule (extension; needs MM_ORDER_RATING); clock: () -> seconds.
+    timeout_ms: optional search time limit (extension): after each tick's lobbies are published, every player still
+    queued who has waited at least this long leaves the pool (Engine.expire) and gets the error response of
+    game-lobby/worker.ex:63-71 on its "response-queue".  None (the default) never expires anyone.
 
     Every ingest batch is stamped with now_ms(), the clock in milliseconds since the pool was created (u32, wraps
     after 49 days), and every tick passes the same clock as its `now`: the engine's per-queue waits
@@ -151,9 +162,10 @@ class SearchPool:
     """
 
     def __init__(self, engine, mode_names, group_names, max_batch=65536, window=None, clock=None, flush_every_s=0.005,
-                 handle_capacity=None):
+                 handle_capacity=None, timeout_ms=None):
         import time
         self.window = window
+        self.timeout_ms = timeout_ms
         self.clock = clock or time.monotonic
         self._t0 = self.clock()
         self.enqueued_at = {}  # handle -> clock() when the player became resident (insertion = enqueue order)
@@ -170,6 +182,8 @@ class SearchPool:
         self._staged = []   # (player id, rating, mode, player, worker, tag)
         self._staged_since = None
         self.stats = {"enqueued": 0, "duplicates": 0, "invalid": 0, "lobbies": 0, "failed_batches": 0}
+        if timeout_ms is not None:
+            self.stats["timed_out"] = 0
 
     def now_ms(self):
         """The pool's clock: milliseconds since the pool was created, modulo 2^32 (the engine's enq_ts / now)."""
@@ -269,7 +283,20 @@ class SearchPool:
             worker = self.workers.get(group_name) or next(iter(self.workers.values()))
             worker.prepare_game_lobby(worker.channel_name, EXCHANGE_FORWARD, QUEUE_FORWARD, payload)
         self.stats["lobbies"] += len(lob)
+        if self.timeout_ms is not None:  # after the lobbies: a player this tick matched is never timed out
+            self._expire(now)
         return len(lob)
+
+    def _expire(self, now):
+        expired, _seq = self.engine.expire(now, self.timeout_ms, want_seq=False)
+        for h in expired.tolist():
+            player = self.players.pop(h)
+            self.enqueued_at.pop(h, None)
+            self.handles.release(self.handles.id_of[h])
+            if player.get("response-queue") is not None:
+                worker = next(iter(self.workers.values()))
+                worker.send_response(worker.channel_name, player["response-queue"], prepare_timeout_response(player))
+        self.stats["timed_out"] += len(expired)
 
     def _teams_of(self, mode):
         return self.engine.cfg.modes[int(mode)].teams
@@ -345,6 +372,10 @@ class SearchWorker:
 
     def prepare_game_lobby(self, channel_name, exchange_forward, queue_forward, payload):  # worker.ex:250-261
         return self.channel.basic_publish(exchange_forward, queue_forward, payload, persistent=True,
+                                          content_type="application/json")
+
+    def send_response(self, channel_name, queue_name, payload):  # game-lobby/worker.ex:105-116
+        return self.channel.basic_publish(EXCHANGE_RESPONSE, queue_name, payload, persistent=True,
                                           content_type="application/json")
 
     # worker.ex:291-324 — one delivery
