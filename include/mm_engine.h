@@ -308,6 +308,78 @@ int mm_expire_packed(mm_engine* e, uint64_t now, uint32_t max_wait, uint32_t* ha
 int mm_snapshot(mm_engine* e);
 int mm_restore(mm_engine* e);
 
+/* ---- hand-over: host image of the queue state ------------------------------------------
+ * The copy_store analogue (models/active_user.ex:29-31, models/lobby_state.ex:31-40: mnesiam replicates ActiveUser and
+ * LobbyState to every node, so a restarted node loses no queued player).  Here the engine is the only place a queued
+ * player exists once its delivery is acked: mm_export writes what a new process needs into a host buffer (to disk, to
+ * another host, to another GPU), mm_import loads it into a FRESH engine (nothing ever enqueued, imported or restored),
+ * which then behaves exactly as the source would have.
+ *
+ * IMAGE LAYOUT (little-endian).  mm_image_header, then seven sections, each starting at the next multiple of 8 bytes
+ * after the previous one ends (the first at offset sizeof(mm_image_header) = 624); total_bytes is the end of the last
+ * section rounded up to 8.  Padding bytes are zero.  W = id_bytes, N = n_players, M = n_active:
+ *   1. part_count  u32[n_parts]  queued players of each layout partition, in layout-partition order (the engine's
+ *                                storage of a (mode, group) queue: one partition per queue, or several of <= 255 sort
+ *                                keys each for a wide group without MM_F_WIDE_PARTITIONS)
+ *   2. id          W * N         player ids (u64), or 32-bit handles for MM_F_DENSE_IDS engines
+ *   3. rating      i32[N]
+ *   4. enq_ts      u32[N]
+ *   5. seq         u32[N]        enqueue sequence numbers (the numbering of emit_seq)
+ *   6. mode        u8[N]
+ *   7. active      W * M         ids in the active set that are not queued: players matched by a tick and not yet
+ *                                removed, and players taken by mm_take (unordered)
+ * Sections 2-6 are columns of one player list: partition by partition, in layout-partition order, enqueue order
+ * inside a partition.
+ *
+ * NOT IN THE IMAGE: dead slots (players removed, taken or expired while queued: the next tick would drop them); the
+ * last batch's reject list (mm_enqueue_rejects is empty after import); the last tick's match section of
+ * mm_queue_stats (void after import, as after mm_restore); the mm_snapshot state; the options (max_spread, tick_impl,
+ * rank_impl, async_results: the caller sets them again).
+ *
+ * EQUIVALENCE.  After mm_import, every sequence of calls gives the same results on the imported engine as on the
+ * source: enqueue codes, remove / take / expire outputs, in_queue, active_size, pool_read, the ticks' lobbies,
+ * members, emit_seq, n_lobbies, n_matched, n_residual, and the waiting section of mm_queue_stats.  What differs comes
+ * from the dead slots that were not carried: mm_pool_size, the next tick's pool_before and n_dead, mm_queue_stats'
+ * n_removed, and how soon a pool near capacity answers "full" (code 3): the imported pool has the dead slots' room.
+ *
+ * mm_export: buf = NULL with cap = 0 -> *n_bytes = the size the image needs, MM_OK.  cap smaller than that ->
+ * MM_E_CAP and *n_bytes.  MM_E_STATE while an mm_enqueue_packed_begin batch is staged.  The source engine is never
+ * changed (a checkpoint and a move are the same call); pending async_results copies are left alone.  The device
+ * counts the live slots of every tile, scans the counts and writes the live players compacted, in order; the active
+ * section is compacted from the active-set table.  About 21 B per queued player (17 with handles).  The size query
+ * runs the counting passes too: a caller that wants one call passes a buffer of the layout's size with n_parts =
+ * MM_MAX_GROUPS * MM_MAX_MODES, N = mm_pool_size, M = mm_active_size, W = 8 (an upper bound) and reads *n_bytes.
+ * The image-sized device scratch of both calls is freed before they return.  mm_import moves the image to the device
+ * in one host-to-device copy and runs the load kernels after it; it does not overlap them with a chunked upload as
+ * ingest does (the kernels' share of the call is in DESIGN §5).
+ * mm_import: MM_E_STATE if the engine is not fresh (or has a staged batch).  MM_E_ARG if the image's config differs
+ * from the engine's on n_groups, group_lo / group_hi, default_group, n_modes, modes, order_mode or flags (capacity,
+ * active_capacity and device may differ: a shard can grow or move to another GPU), and for an image that is truncated,
+ * corrupted or hostile: bad magic / version / lengths / section counts, partition counts that do not add up, a mode
+ * >= n_modes, a rating that does not map to the partition it is filed under, an id outside the id range (handles >=
+ * active_capacity), a duplicate id within or across the sections, sequence numbers not strictly increasing in
+ * enqueue order inside a partition (or equal to seq_next).  MM_E_CAP if the players do not fit the capacity (or a
+ * hashed active set).  After any failure the engine is empty and still fresh.                                      */
+#define MM_IMAGE_MAGIC 0x474D494Du /* "MIMG" */
+#define MM_IMAGE_VERSION 1u
+
+typedef struct mm_image_header {
+  uint32_t magic;       /* MM_IMAGE_MAGIC                                                         */
+  uint32_t version;     /* MM_IMAGE_VERSION                                                       */
+  uint32_t abi_version; /* MM_ABI_VERSION of the writer                                           */
+  uint32_t id_bytes;    /* 8: u64 ids; 4: 32-bit handles (MM_F_DENSE_IDS engines)                 */
+  uint64_t total_bytes; /* the whole image, this header included                                  */
+  uint32_t n_parts;     /* layout partitions: entries of section 1                                */
+  uint32_t n_players;   /* queued players: entries of sections 2-6                                */
+  uint32_t n_active;    /* active ids that are not queued: entries of section 7                   */
+  uint32_t seq_next;    /* enqueue sequence number of the next offered player                     */
+  mm_config config;     /* the writer's config (capacity, active_capacity, device: informational) */
+  uint32_t reserved;    /* 0                                                                      */
+} mm_image_header;      /* 624 bytes */
+
+int mm_export(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes);
+int mm_import(mm_engine* e, const void* buf, uint64_t n_bytes);
+
 /* Use an externally owned CUDA stream (cudaStream_t passed as void*).              */
 int mm_set_stream(mm_engine* e, void* cuda_stream);
 

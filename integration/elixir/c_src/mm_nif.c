@@ -200,6 +200,35 @@ static ERL_NIF_TERM nif_expire_packed(ErlNifEnv* env, int argc, const ERL_NIF_TE
   return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &hs));
 }
 
+/* export_image(ref) -> {:ok, image :: binary}: the queued players and the active set (mm_export; layout in
+ * mm_engine.h).  One call: the binary is allocated at the layout's upper bound (mm_engine.h) and shrunk to the image. */
+static ERL_NIF_TERM nif_export_image(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; uint32_t n = 0, a = 0; uint64_t size = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r)) return enif_make_badarg(env);
+  if (mm_pool_size(r->e, &n) || mm_active_size(r->e, &a)) return err(env, MM_E_ARG);
+  uint64_t bound = sizeof(mm_image_header), sec[7];
+  sec[0] = 4ull * MM_MAX_GROUPS * MM_MAX_MODES; sec[1] = 8ull * n; sec[2] = sec[3] = sec[4] = 4ull * n; sec[5] = n;
+  sec[6] = 8ull * a;
+  for (int k = 0; k < 7; ++k) bound = (bound + sec[k] + 7) & ~7ull;
+  ErlNifBinary img;
+  if (!enif_alloc_binary((size_t)bound, &img)) return err(env, MM_E_CAP);
+  int rc = mm_export(r->e, img.data, bound, &size);
+  if (rc) { enif_release_binary(&img); return err(env, rc); }
+  enif_realloc_binary(&img, (size_t)size);
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &img));
+}
+
+/* import_image(ref, image :: binary) -> :ok | {:error, atom}: loads an image into a fresh engine (mm_import) */
+static ERL_NIF_TERM nif_import_image(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary img;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &img))
+    return enif_make_badarg(env);
+  int rc = mm_import(r->e, img.data, img.size);
+  return rc ? err(env, rc) : atom(env, "ok");
+}
+
 /* set_max_spread(ref, w): extension knob (strategist policy S1); w < 0 restores the reference behaviour */
 static ERL_NIF_TERM nif_set_max_spread(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
   engine_res* r; ErlNifSInt64 w = -1;
@@ -223,6 +252,8 @@ static ErlNifFunc funcs[] = {
   {"status", 1, nif_status, 0},
   {"queue_stats", 2, nif_queue_stats, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"expire_packed", 3, nif_expire_packed, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"export_image", 1, nif_export_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"import_image", 2, nif_import_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"set_max_spread", 2, nif_set_max_spread, 0},
 };
 ERL_NIF_INIT(Elixir.Matchmaking.Search.Engine, funcs, load, NULL, NULL, NULL)

@@ -62,6 +62,14 @@ defmodule Matchmaking.Search.Engine do
   """
   def expire_packed(_ref, _now_ms, _max_wait_ms), do: :erlang.nif_error(:nif_not_loaded)
 
+  @doc """
+  Hand-over: the queued players and the active set as one binary (the image of include/mm_engine.h) -> {:ok, image}.
+  The engine is not changed.
+  """
+  def export_image(_ref), do: :erlang.nif_error(:nif_not_loaded)
+  @doc "Loads an export_image/1 image into a fresh engine of the same config -> :ok | {:error, :badarg | :capacity | :state}"
+  def import_image(_ref, _image), do: :erlang.nif_error(:nif_not_loaded)
+
   @doc "Extension (not reference behaviour): maximum rating spread of a lobby for the following ticks; < 0 = off."
   def set_max_spread(_ref, _w), do: :erlang.nif_error(:nif_not_loaded)
 end

@@ -15,6 +15,14 @@ defmodule Matchmaking.Search.Pool do
       search_timeout_ms   option (extension, default nil = off): after each tick's lobbies are published, the players
                      still queued who have waited at least this long leave the pool (Engine.expire_packed) and get the
                      error response of game-lobby/worker.ex:63-71,105-116 on their "response-queue"
+      checkpoint/0   hand-over: flushes the staged deliveries (so every acked player is in it), then returns
+                     :erlang.term_to_binary of the engine image (Engine.export_image), the handle table, the player
+                     documents, the pool clock and the wall time.  resume: <checkpoint> as an option of start_link/1
+                     starts a pool on a fresh engine from it; the clock goes on from the checkpoint plus the time the
+                     pool was down (INTEGRATION.md §3 has the order: stop consuming, checkpoint, start with resume:,
+                     consume again)
+      attach/1       a search worker hands over its open channel (patched init); the pool ticks only once it has a
+                     channel to publish lobbies and timeout responses on — a staged delivery sets it too
 
   Every batch is stamped with the pool's clock (ms since the pool started, modulo 2^32) and every tick passes the same
   clock as its `now`, so the engine's waits are in milliseconds.
@@ -39,18 +47,43 @@ defmodule Matchmaking.Search.Pool do
 
   def start_link(opts \\ []), do: GenServer.start_link(__MODULE__, opts, name: __MODULE__)
   def stage(player, game_mode, rating, ack_ref), do: GenServer.cast(__MODULE__, {:stage, player, game_mode, rating, ack_ref})
+  @doc "A search worker whose channel is open hands its channel name over (patched init, worker_patch.ex)."
+  def attach(channel_name), do: GenServer.cast(__MODULE__, {:attach, channel_name})
   def in_queue?(player_id), do: GenServer.call(__MODULE__, {:in_queue?, player_id})
   def remove_user(player_id), do: GenServer.call(__MODULE__, {:remove_user, player_id})
   def queue_status(group_index), do: GenServer.call(__MODULE__, {:queue_status, group_index})
+  def checkpoint, do: GenServer.call(__MODULE__, :checkpoint, :infinity)
 
   @impl true
   def init(opts) do
     capacity = Keyword.get(opts, :capacity, 16_000_000)
     {:ok, ref} = Engine.new(Engine.pack_config(capacity: capacity, active_capacity: 2 * capacity, dense_ids: true))
-    Process.send_after(self(), :flush, @flush_ms)
-    Process.send_after(self(), :tick, @tick_ms)
-    {:ok, %{ref: ref, staged: [], n_staged: 0, handle_of: %{}, players: %{}, free: [], next: 0, channel: nil,
-            t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms)}}
+    st = %{ref: ref, staged: [], n_staged: 0, handle_of: %{}, players: %{}, free: [], next: 0, channel: nil,
+           t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms)}
+    case resume(st, Keyword.get(opts, :resume)) do
+      {:ok, st} ->
+        Process.send_after(self(), :flush, @flush_ms)
+        Process.send_after(self(), :tick, @tick_ms)
+        {:ok, st}
+      {:error, reason} -> {:stop, {:resume_failed, reason}}
+    end
+  end
+
+  # -- hand-over: the engine image plus the host state ------------------------------------------------------------
+  # The channel name is not carried: a name from the old process does not say that the new process has that channel
+  # open.  Until a search worker attaches its channel (attach/1) or stages a delivery, :tick neither ticks nor
+  # expires, so the players of the image are not matched into lobbies that could not be published.
+  defp resume(st, nil), do: {:ok, st}
+  defp resume(st, blob) do
+    ck = :erlang.binary_to_term(blob, [:safe])
+    case Engine.import_image(st.ref, ck.image) do
+      :ok ->
+        down = max(0, System.os_time(:millisecond) - ck.wall_ms)
+        # now_ms/1 goes on from the checkpoint's value plus the downtime: the engine's enqueue stamps stay valid
+        {:ok, %{st | handle_of: ck.handle_of, players: ck.players, free: ck.free, next: ck.next,
+                     t0: System.monotonic_time(:millisecond) - ck.now_ms - down}}
+      {:error, _} = e -> e
+    end
   end
 
   @impl true
@@ -59,6 +92,8 @@ defmodule Matchmaking.Search.Pool do
                channel: elem(ack_ref, 0)}   # lobbies go out on a search worker's channel, like prepare_game_lobby/4
     {:noreply, if(st.n_staged >= @max_batch, do: flush(st), else: st)}
   end
+
+  def handle_cast({:attach, channel_name}, st), do: {:noreply, %{st | channel: channel_name}}
 
   @impl true
   def handle_call({:in_queue?, id}, _from, st) do
@@ -94,10 +129,27 @@ defmodule Matchmaking.Search.Pool do
     end
   end
 
+  def handle_call(:checkpoint, _from, st) do
+    st = flush(st)
+    case Engine.export_image(st.ref) do
+      {:ok, image} ->
+        ck = %{image: image, handle_of: st.handle_of, players: st.players, free: st.free, next: st.next,
+               now_ms: now_ms(st), wall_ms: System.os_time(:millisecond)}
+        {:reply, {:ok, :erlang.term_to_binary(ck)}, st}
+      {:error, _} = e -> {:reply, e, st}
+    end
+  end
+
   @impl true
   def handle_info(:flush, st) do
     Process.send_after(self(), :flush, @flush_ms)
     {:noreply, flush(st)}
+  end
+
+  # no channel to publish on yet (a resumed pool before any search worker attached): hold the tick and the timeout
+  def handle_info(:tick, %{channel: nil} = st) do
+    Process.send_after(self(), :tick, @tick_ms)
+    {:noreply, st}
   end
 
   def handle_info(:tick, st) do

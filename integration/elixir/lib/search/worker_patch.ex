@@ -19,6 +19,12 @@
     end
   end
 
+  # :229-231 — init/1, once the channel is spawned and configured: the pool publishes lobbies and timeout responses
+  # on a search worker's channel, and a pool resumed from a checkpoint ticks only once one is attached
+  #     @connection.spawn_channel(channel_name)
+  #     @connection.configure_channel(channel_name, opts[:config])
+  #     Matchmaking.Search.Pool.attach(channel_name)
+
   # :115-117, 326-334 — status/0: the broker's queue is nearly always empty (deliveries are acked once resident), so the
   # group's waiting players come from the engine:  Map.put(status, :waiting, Matchmaking.Search.Pool.queue_status(group))
 

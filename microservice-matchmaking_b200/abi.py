@@ -92,6 +92,38 @@ class QueueStat(C.Structure):
     ]
 
 
+MM_IMAGE_MAGIC = 0x474D494D
+MM_IMAGE_VERSION = 1
+
+
+class ImageHeader(C.Structure):
+    """mm_image_header: the first 624 bytes of an mm_export image."""
+    _fields_ = [
+        ("magic", C.c_uint32),
+        ("version", C.c_uint32),
+        ("abi_version", C.c_uint32),
+        ("id_bytes", C.c_uint32),
+        ("total_bytes", C.c_uint64),
+        ("n_parts", C.c_uint32),
+        ("n_players", C.c_uint32),
+        ("n_active", C.c_uint32),
+        ("seq_next", C.c_uint32),
+        ("config", Config),
+        ("reserved", C.c_uint32),
+    ]
+
+
+def image_offsets(n_parts, n_players, n_active, id_bytes):
+    """Section offsets of an image (include/mm_engine.h): part_count, id, rating, enq_ts, seq, mode, active, and the
+    total length.  Every section starts at the next multiple of 8 after the one before it."""
+    sizes = (4 * n_parts, id_bytes * n_players, 4 * n_players, 4 * n_players, 4 * n_players, n_players,
+             id_bytes * n_active)
+    off = [C.sizeof(ImageHeader)]
+    for s in sizes:
+        off.append((off[-1] + s + 7) & ~7)
+    return off
+
+
 # every symbol include/mm_engine.h declares: name -> (restype, argtypes)
 _P = C.POINTER
 _vp = C.c_void_p
@@ -121,6 +153,8 @@ PROTOTYPES = {
     "mm_queue_stats": (C.c_int, [_vp, C.c_uint64, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_expire": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_expire_packed": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
+    "mm_export": (C.c_int, [_vp, _vp, C.c_uint64, _P(C.c_uint64)]),
+    "mm_import": (C.c_int, [_vp, _vp, C.c_uint64]),
     "mm_snapshot": (C.c_int, [_vp]),
     "mm_restore": (C.c_int, [_vp]),
     "mm_set_stream": (C.c_int, [_vp, _vp]),

@@ -18,6 +18,7 @@
 #include <vector>
 
 #include "mm_expire.cuh"
+#include "mm_image.cuh"
 #include "mm_kernels.cuh"
 #include "mm_stats.cuh"
 
@@ -164,6 +165,18 @@ struct mm_engine {
   uint64_t* d_exp_id = nullptr;  // ids, or 32-bit handles in its first half
   uint32_t* d_exp_seq = nullptr;
   uint32_t exp_cap = 0;
+
+  // mm_export / mm_import.  The image-sized buffers (d_img, d_img_act: about the image's size, 210 MB at 10 M queued
+  // players) are freed at the end of every call, so a hand-over leaves no such footprint on either engine; the small
+  // per-tile / per-partition arrays are kept.
+  bool fresh = true;  // nothing ever enqueued, imported or restored: mm_import may load an image
+  uint8_t* d_img = nullptr;  // the image from section 2 (id) on, as it lies in the host buffer
+  size_t img_cap = 0;
+  uint32_t* d_img_tile = nullptr;  // export: live slots per virtual tile -> offsets
+  uint32_t img_tile_cap = 0;
+  uint32_t* d_img_part = nullptr;  // export: [n_segs] live slots per partition; import: part_off[n_segs+1] | slot_base[n_segs]
+  void* d_img_act = nullptr;       // export: the active section
+  uint64_t img_act_cap = 0;        // bytes
 };
 
 namespace {
@@ -455,6 +468,7 @@ int rehash(mm_engine* e) {
 
 // capacity checks + scratch for an ingest batch of n players
 int enq_prepare(mm_engine* e, uint32_t n) {
+  e->fresh = false;
   int rc = ensure_enq_scratch(e, n);
   if (rc) return rc;
   if (e->use_active && !e->dense_ids && (e->n_active + e->n_tomb + n) * 4 > e->hcap * 3) {
@@ -826,6 +840,245 @@ int expire(mm_engine* e, uint64_t now, uint32_t max_wait, uint64_t* ids, uint32_
   return MM_OK;
 }
 
+// ---- mm_export / mm_import -------------------------------------------------------------------------------------------
+// Section offsets of an image (include/mm_engine.h): off[0] part counts, [1] id, [2] rating, [3] enq_ts, [4] seq,
+// [5] mode, [6] active, [7] total bytes.
+struct ImgLayout { uint64_t off[8]; };
+ImgLayout img_layout(uint32_t n_parts, uint32_t n, uint32_t m, uint32_t idb) {
+  auto a8 = [](uint64_t x) { return (x + 7) & ~7ull; };
+  const uint64_t bytes[7] = {4ull * n_parts, (uint64_t)idb * n, 4ull * n, 4ull * n, 4ull * n, (uint64_t)n,
+                             (uint64_t)idb * m};
+  ImgLayout l{};
+  l.off[0] = sizeof(mm_image_header);
+  for (int k = 0; k < 7; ++k) l.off[k + 1] = a8(l.off[k] + bytes[k]);
+  return l;
+}
+ImgCols img_cols(uint8_t* body, const ImgLayout& l, uint32_t idb) {  // body = the image from section 2 (id) on
+  ImgCols c{};
+  c.id = body;
+  c.rating = reinterpret_cast<int32_t*>(body + (l.off[2] - l.off[1]));
+  c.ts = reinterpret_cast<uint32_t*>(body + (l.off[3] - l.off[1]));
+  c.seq = reinterpret_cast<uint32_t*>(body + (l.off[4] - l.off[1]));
+  c.mode = body + (l.off[5] - l.off[1]);
+  c.id_bytes = idb;
+  return c;
+}
+uint32_t id_bytes(const mm_engine* e) { return e->dense_ids ? 4u : 8u; }
+uint64_t id_limit(const mm_engine* e) { return e->dense_ids ? e->hcap : kTombKey; }
+
+template <class T>
+int grow(mm_engine* e, T*& p, uint64_t& cap, uint64_t want) {
+  if (want <= cap) return MM_OK;
+  cudaFree(p);
+  p = nullptr; cap = 0;
+  CK(cudaMalloc(reinterpret_cast<void**>(&p), want));
+  cap = want;
+  return MM_OK;
+}
+
+int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes) {
+  if (e->stage_count) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "a packed batch is staged: call mm_enqueue_packed_end first");
+    return MM_E_STATE;
+  }
+  const Pool& p = e->pool[e->cur];
+  const uint32_t idb = id_bytes(e);
+  int rc;
+  // pass 1: live slots per tile and per partition, the tiles' offsets; the active section
+  const uint32_t tiles = p.n / kTile + e->n_segs;  // bounds the virtual tile count
+  const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(tiles, 8u * (uint32_t)e->n_sms));
+  uint64_t tile_cap = e->img_tile_cap;
+  if ((rc = grow(e, e->d_img_tile, tile_cap, (uint64_t)tiles * 4))) return rc;
+  e->img_tile_cap = (uint32_t)tile_cap;
+  if (!e->d_img_part) CK(cudaMalloc(&e->d_img_part, ((size_t)3 * e->n_segs + 2) * 4));
+  CK(cudaMemsetAsync(e->d_img_tile, 0, (size_t)tiles * 4, e->stream));
+  CK(cudaMemsetAsync(e->d_img_part, 0, (size_t)e->n_segs * 4, e->stream));
+  CK(cudaMemsetAsync(e->d_small + 12, 0, 8, e->stream));
+  ImgExportArgs a{};
+  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.tile_cnt = e->d_img_tile; a.part_cnt = e->d_img_part;
+  if (p.n) k_img_tiles<kImgBlock, false><<<ctas, kImgBlock, 0, e->stream>>>(a);
+  k_scan_small<<<1, 1024, 0, e->stream>>>(tiles, e->d_img_tile, e->d_small + 12);
+  const uint32_t act_cap = (uint32_t)std::min<uint64_t>(e->n_active, 0xFFFFFFFFu);
+  if (e->use_active && act_cap) {
+    if ((rc = grow(e, e->d_img_act, e->img_act_cap, (uint64_t)act_cap * idb))) return rc;
+    const uint64_t n_tab = e->hcap;
+    const uint32_t nb = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n_tab + 255) / 256, 16ull * (uint32_t)e->n_sms));
+    k_img_active<<<nb, 256, 0, e->stream>>>(act_view(e), n_tab, p.v.mode, (uint32_t)pool_slots(e), e->gen, e->d_img_act,
+                                            idb, act_cap, e->d_small + 13);
+  }
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(e->h_small + 12, e->d_small + 12, 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  const uint32_t n = e->h_small[12], m = e->h_small[13];
+  if (m > act_cap) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "%u active ids outside the pool, %u in the active set", m, act_cap);
+    return MM_E_STATE;
+  }
+  const ImgLayout l = img_layout(e->n_segs, n, m, idb);
+  *n_bytes = l.off[7];
+  if (!buf) return MM_OK;
+  if (cap < l.off[7]) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "need cap >= %llu", (unsigned long long)l.off[7]);
+    return MM_E_CAP;
+  }
+  // pass 2: the columns, laid out as in the image (padding zero)
+  uint8_t* out = static_cast<uint8_t*>(buf);
+  const uint64_t col_bytes = l.off[6] - l.off[1];
+  if ((rc = grow(e, e->d_img, e->img_cap, std::max<uint64_t>(col_bytes, 8)))) return rc;
+  if (n) {
+    CK(cudaMemsetAsync(e->d_img, 0, col_bytes, e->stream));
+    a.out = img_cols(e->d_img, l, idb);
+    k_img_tiles<kImgBlock, true><<<ctas, kImgBlock, 0, e->stream>>>(a);
+    CK(cudaGetLastError());
+  }
+  mm_image_header h{};
+  h.magic = MM_IMAGE_MAGIC; h.version = MM_IMAGE_VERSION; h.abi_version = MM_ABI_VERSION; h.id_bytes = idb;
+  h.total_bytes = l.off[7]; h.n_parts = e->n_segs; h.n_players = n; h.n_active = m; h.seq_next = e->seq_next;
+  h.config = e->cfg;
+  std::memcpy(out, &h, sizeof(h));
+  std::memset(out + l.off[0], 0, l.off[1] - l.off[0]);  // the part counts' padding
+  std::memset(out + l.off[6], 0, l.off[7] - l.off[6]);  // the active section and its padding
+  CK(cudaMemcpyAsync(out + l.off[0], e->d_img_part, (size_t)e->n_segs * 4, cudaMemcpyDeviceToHost, e->stream));
+  if (n) CK(cudaMemcpyAsync(out + l.off[1], e->d_img, col_bytes, cudaMemcpyDeviceToHost, e->stream));
+  if (m) CK(cudaMemcpyAsync(out + l.off[6], e->d_img_act, (size_t)m * idb, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
+// the image-sized scratch of mm_export / mm_import (cudaFree waits for the work that uses it)
+void free_img_scratch(mm_engine* e) {
+  cudaFree(e->d_img); cudaFree(e->d_img_act);
+  e->d_img = nullptr; e->img_cap = 0; e->d_img_act = nullptr; e->img_act_cap = 0;
+}
+
+// The current pool buffer and the active set back to an empty engine's state.
+int clear_engine(mm_engine* e) {
+  Pool& p = e->pool[e->cur];
+  CK(cudaMemsetAsync(p.m.fill, 0, (size_t)e->n_segs * 4, e->stream));
+  CK(cudaMemsetAsync(p.m.bump, 0, 4, e->stream));
+  CK(cudaMemsetAsync(p.m.tot, 0, ((size_t)e->Kp + 1) * 4, e->stream));
+  if (p.m.chist) CK(cudaMemsetAsync(p.m.chist, 0, (size_t)e->n_chunks * kChunkHist * 4, e->stream));
+  CK(cudaMemsetAsync(p.v.bin, 0xFF, pool_slots(e) * 2, e->stream));
+  p.n = 0;
+  if (e->use_active) {
+    int rc = clear_table(e, e->tab[e->tcur]);
+    if (rc) return rc;
+  }
+  e->n_active = 0; e->n_tomb = 0;
+  CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
+int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
+  auto bad = [&](const char* what) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "image rejected: %s", what);
+    return (int)MM_E_ARG;
+  };
+  if (!e->fresh || e->stage_count) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "mm_import needs a fresh engine (nothing enqueued, imported or restored)");
+    return MM_E_STATE;
+  }
+  mm_image_header h;
+  if (nb < sizeof(h)) return bad("shorter than its header");
+  std::memcpy(&h, buf, sizeof(h));
+  if (h.magic != MM_IMAGE_MAGIC) return bad("bad magic");
+  if (h.version != MM_IMAGE_VERSION || h.abi_version != MM_ABI_VERSION) return bad("unknown version");
+  if (h.id_bytes != id_bytes(e)) return bad("id width differs from the engine's");
+  if (h.n_parts != e->n_segs) return bad("partition count differs from the engine's layout");
+  const ImgLayout l = img_layout(h.n_parts, h.n_players, h.n_active, h.id_bytes);
+  if (h.total_bytes != l.off[7] || nb != l.off[7]) return bad("length does not match the header's section counts");
+  const mm_config &a = h.config, &c = e->cfg;
+  bool same = a.n_groups == c.n_groups && a.default_group == c.default_group && a.n_modes == c.n_modes &&
+              a.order_mode == c.order_mode && a.flags == c.flags;
+  for (uint32_t g = 0; same && g < c.n_groups; ++g) same = a.group_lo[g] == c.group_lo[g] && a.group_hi[g] == c.group_hi[g];
+  for (uint32_t m = 0; same && m < c.n_modes; ++m)
+    same = a.modes[m].teams == c.modes[m].teams && a.modes[m].team_size == c.modes[m].team_size;
+  if (!same) return bad("config differs from the engine's (groups, default_group, modes, order_mode or flags)");
+  if (!e->use_active && h.n_active) return bad("active section in an image of an engine without an active set");
+  std::vector<uint32_t> cnt(e->n_segs);
+  std::memcpy(cnt.data(), buf + l.off[0], (size_t)e->n_segs * 4);
+  uint64_t sum = 0;
+  for (uint32_t q : cnt) sum += q;
+  if (sum != h.n_players) return bad("partition counts do not add up to the player count");
+  const uint32_t n = h.n_players, m = h.n_active;
+  if (n > e->capacity) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "%u players, capacity %u", n, e->capacity);
+    return MM_E_CAP;
+  }
+  if (e->use_active && !e->dense_ids && ((uint64_t)n + m) * 4 > e->hcap * 3) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "%llu active ids, active set holds %llu",
+                  (unsigned long long)n + m, (unsigned long long)(e->hcap * 3 / 4));
+    return MM_E_CAP;
+  }
+  // every partition on consecutive chunks, in partition order
+  std::vector<uint32_t> tab((size_t)e->n_segs * e->n_chunks, 0), off_base(2 * (size_t)e->n_segs + 1);
+  uint32_t chunk = 0, idx = 0;
+  for (uint32_t s = 0; s < e->n_segs; ++s) {
+    const uint32_t nch = (cnt[s] + kTile - 1) / kTile;
+    for (uint32_t k = 0; k < nch; ++k) tab[(size_t)s * e->n_chunks + k] = chunk + k;
+    off_base[s] = idx;
+    off_base[e->n_segs + 1 + s] = chunk * kTile;
+    idx += cnt[s];
+    chunk += nch;
+  }
+  off_base[e->n_segs] = idx;
+  int rc = clear_engine(e);
+  if (rc) return rc;
+  Pool& p = e->pool[e->cur];
+  const uint64_t body = nb - l.off[1];  // columns and active section
+  if (!e->d_img_part) CK(cudaMalloc(&e->d_img_part, ((size_t)3 * e->n_segs + 2) * 4));
+  if ((rc = grow(e, e->d_img, e->img_cap, std::max<uint64_t>(body, 8)))) return rc;
+  CK(cudaMemcpyAsync(p.m.fill, cnt.data(), (size_t)e->n_segs * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(p.m.chunk_tab, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(p.m.bump, &chunk, 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(e->d_img_part, off_base.data(), off_base.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  if (body) CK(cudaMemcpyAsync(e->d_img, buf + l.off[1], body, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemsetAsync(e->d_small + 14, 0, 4, e->stream));
+  const ImgCols cols = img_cols(e->d_img, l, h.id_bytes);
+  const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((n + 255) / 256, 32u * (uint32_t)e->n_sms));
+  if (n) {
+    ImgLoadArgs la{};
+    la.pool = p.v; la.meta = p.m; la.in = cols; la.n = n; la.n_segs = e->n_segs;
+    la.part_off = e->d_img_part; la.slot_base = e->d_img_part + e->n_segs + 1;
+    la.bm = bin_map(e); la.grp_lut = e->d_grp_lut; la.bin_seg = e->d_bin_seg; la.seg_bin_lo = e->d_seg_bin_lo;
+    la.mode_tsize = e->d_mode_tsize; la.n_modes = e->cfg.n_modes; la.seq_next = h.seq_next; la.id_limit = id_limit(e);
+    la.err = e->d_small + 14;
+    k_img_load<<<grid, 256, 0, e->stream>>>(la);
+  }
+  if (e->use_active) {
+    const ActiveView av = act_view(e);
+    if (n) k_img_insert<<<grid, 256, 0, e->stream>>>(cols.id, h.id_bytes, n, id_limit(e), av, e->d_small + 14);
+    if (m) {
+      const uint32_t g2 = std::max<uint32_t>(1, std::min<uint32_t>((m + 255) / 256, 32u * (uint32_t)e->n_sms));
+      k_img_insert<<<g2, 256, 0, e->stream>>>(e->d_img + (l.off[6] - l.off[1]), h.id_bytes, m, id_limit(e), av,
+                                              e->d_small + 14);
+    }
+  }
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(e->h_small + 14, e->d_small + 14, 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  if (const uint32_t err = e->h_small[14]) {
+    if ((rc = clear_engine(e))) return rc;
+    std::snprintf(e->last_err, sizeof(e->last_err), "image rejected:%s%s%s%s%s%s", err & kImgBadId ? " id out of range" : "",
+                  err & kImgBadMode ? " mode out of range" : "", err & kImgBadRating ? " rating outside its partition" : "",
+                  err & kImgBadSeq ? " sequence numbers out of order" : "", err & kImgDup ? " duplicate id" : "",
+                  err & kImgFull ? " active set full" : "");
+    return MM_E_ARG;
+  }
+  p.n = n;
+  e->seq_next = h.seq_next;
+  if (e->use_active) e->n_active = (uint64_t)n + m;
+  e->fresh = false;
+  e->match_valid = false;
+  e->last_batch_n = 0;
+  if (e->use_active && n) {  // the queued players' entries point at their slots
+    k_restamp<<<dim3(e->n_chunks, e->n_segs), 256, 0, e->stream>>>(p.v, p.m, act_view(e), e->gen);
+    CK(cudaGetLastError());
+  }
+  CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
 }  // namespace
 
 // =======================================================================================
@@ -991,6 +1244,7 @@ int mm_destroy(mm_engine* e) {
   cudaFree(e->d_in_ts); cudaFree(e->d_blocksum); cudaFree(e->d_blockhist); cudaFree(e->d_part); cudaFree(e->d_in_key);
   cudaFree(e->d_in_handle); cudaFree(e->d_rej_idx); cudaFree(e->d_rej_code);
   cudaFree(e->d_qstat); cudaFree(e->d_exp_id); cudaFree(e->d_exp_seq);
+  cudaFree(e->d_img); cudaFree(e->d_img_tile); cudaFree(e->d_img_part); cudaFree(e->d_img_act);
   if (e->h_ctr) cudaFreeHost(e->h_ctr);
   if (e->h_small) cudaFreeHost(e->h_small);
   for (auto& ev : e->ev)
@@ -1443,6 +1697,25 @@ int mm_expire_packed(mm_engine* e, uint64_t now, uint32_t max_wait, uint32_t* ha
   return expire(e, now, max_wait, nullptr, handles, seq, cap, n_expired);
 }
 
+int mm_export(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes) {
+  if (!e || !n_bytes || (cap && !buf)) return MM_E_ARG;
+  *n_bytes = 0;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  const int rc = export_image(e, buf, cap, n_bytes);
+  free_img_scratch(e);
+  return rc;
+}
+
+int mm_import(mm_engine* e, const void* buf, uint64_t n_bytes) {
+  if (!e || (n_bytes && !buf)) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  const int rc = import_image(e, static_cast<const uint8_t*>(buf), n_bytes);
+  free_img_scratch(e);
+  return rc;
+}
+
 int mm_snapshot(mm_engine* e) {
   if (!e) return MM_E_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
@@ -1480,6 +1753,7 @@ int mm_restore(mm_engine* e) {
   }
   e->seq_next = e->snap_seq;
   e->gen = next_gen(e);
+  e->fresh = false;
   e->match_valid = false;  // the restored pool was not matched by the last tick
   if (e->use_active && p.n) {
     k_restamp<<<dim3(e->n_chunks, e->n_segs), 256, 0, e->stream>>>(p.v, p.m, act_view(e), e->gen);

@@ -1,0 +1,235 @@
+// mm_image.cuh — host image of the queue state (mm_export / mm_import; layout in include/mm_engine.h).
+//
+// Export: two passes over the tick's virtual tile sequence (geo_build over the partition fills, as k_expire and
+// k_queue_stats walk it).  Pass 1 counts the live slots of every tile (and of every partition); k_scan_small turns the
+// tile counts into offsets; pass 2 writes the live players of each tile at its offset, compacted and in order, into
+// the image's columns in device memory — so the columns are partition by partition, in enqueue order inside a
+// partition.  k_img_active compacts the active-set entries that are not queued (matched players awaiting mm_remove,
+// players taken by mm_take) out of the hashed or direct-mapped table.
+//
+// Import: the layout is the engine's own (same config), so the host lays out every partition on consecutive chunks
+// from the partition counts; k_img_load writes the columns into their slots, derives the sort key and team size,
+// builds the bin totals and chunk histograms, and checks every player.  k_img_insert puts the ids of both sections
+// into the active set (duplicate check) with the "not queued" value 0 — no generation is 0, so the entry never
+// matches a slot — and k_restamp then points the queued players' entries at their slots.  A failed check sets a bit
+// of one error word; the host then clears the engine.
+#pragma once
+
+#include "mm_active.cuh"
+
+namespace mm {
+
+constexpr uint32_t kImgBlock = 256;  // 8 slots per thread: one tile per CTA step
+static_assert(kImgBlock * 8 == kTile, "a CTA step covers one tile");
+
+// error bits of an import (the host names them in mm_last_error)
+constexpr uint32_t kImgBadId = 1, kImgBadMode = 2, kImgBadRating = 4, kImgBadSeq = 8, kImgDup = 16, kImgFull = 32;
+
+// the player columns of an image, in device memory (id: u64, or u32 handles when id_bytes == 4)
+struct ImgCols {
+  void* id;
+  int32_t* rating;
+  uint32_t* ts;
+  uint32_t* seq;
+  uint8_t* mode;
+  uint32_t id_bytes;
+};
+
+__device__ __forceinline__ uint64_t img_id(const ImgCols& c, uint32_t i) {
+  return c.id_bytes == 8 ? static_cast<const uint64_t*>(c.id)[i] : static_cast<const uint32_t*>(c.id)[i];
+}
+
+struct ImgExportArgs {
+  PoolView pool;
+  PoolMeta meta;
+  uint32_t n_segs;
+  uint32_t* tile_cnt;  // [virtual tiles] pass 1: live slots of the tile; pass 2: the tile's first output index
+  uint32_t* part_cnt;  // [n_segs] pass 1: live slots of the partition (zeroed by the host)
+  ImgCols out;         // pass 2
+};
+
+// Pass 1 (WRITE = false) / pass 2 (WRITE = true).  CTAs take contiguous runs of the virtual tile sequence.
+template <int BLOCK, bool WRITE>
+__global__ void __launch_bounds__(BLOCK) k_img_tiles(const ImgExportArgs a) {
+  __shared__ Geo geo;
+  __shared__ uint32_t s_gtmp[33];
+  __shared__ uint32_t s_warp[BLOCK / 32];
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  geo_build<BLOCK>(geo, a.meta.fill, a.n_segs, gridDim.x, s_gtmp);
+  const uint32_t s0 = blockIdx.x * geo.tpr;
+  if (s0 >= geo.NT) return;  // (uniform)
+  const uint32_t s1 = s0 + geo.tpr < geo.NT ? s0 + geo.tpr : geo.NT;
+  const uint32_t o = tid * 8;
+  for (uint32_t s = s0; s < s1; ++s) {
+    const TileDesc d = geo_tile(geo, a.meta, s);
+    const size_t base = (size_t)d.phys * kTile + o;
+    uint32_t live = 0;  // bit j: slot base + j holds a live player
+    if (o < d.nvalid) {
+      const uint2 m2 = __ldcs(reinterpret_cast<const uint2*>(a.pool.mode + base));
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const uint32_t md = ((j < 4 ? m2.x : m2.y) >> (8 * (j & 3))) & 0xFFu;
+        if (o + j < d.nvalid && md != MM_MODE_DEAD) live |= 1u << j;
+      }
+    }
+    const uint32_t k = __popc(live);
+    uint32_t incl = k;
+#pragma unroll
+    for (int off = 1; off < 32; off <<= 1) {
+      const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, off);
+      if (lane >= (uint32_t)off) incl += v;
+    }
+    if (lane == 31) s_warp[warp] = incl;
+    __syncthreads();
+    uint32_t before = 0, total = 0;
+#pragma unroll
+    for (int w = 0; w < BLOCK / 32; ++w) {
+      const uint32_t v = s_warp[w];
+      before += (uint32_t)w < warp ? v : 0u;
+      total += v;
+    }
+    __syncthreads();  // s_warp is rewritten for the next tile
+    if (!WRITE) {
+      if (tid == 0) {
+        a.tile_cnt[s] = total;
+        if (total) atomicAdd(&a.part_cnt[d.seg], total);
+      }
+      continue;
+    }
+    if (!live) continue;
+    uint32_t q = a.tile_cnt[s] + before + incl - k;
+#pragma unroll 1
+    for (int j = 0; j < 8; ++j) {
+      if (!((live >> j) & 1u)) continue;
+      const size_t slot = base + j;
+      const uint64_t pid = a.pool.id[slot];
+      if (a.out.id_bytes == 8) static_cast<uint64_t*>(a.out.id)[q] = pid;
+      else static_cast<uint32_t*>(a.out.id)[q] = (uint32_t)pid;
+      a.out.rating[q] = a.pool.rating[slot];
+      a.out.ts[q] = a.pool.ts[slot];
+      a.out.seq[q] = a.pool.seq[slot];
+      a.out.mode[q] = a.pool.mode[slot];
+      ++q;
+    }
+  }
+}
+
+// The committed active-set entries that are not a live queued player's: a queued player's entry is exactly
+// gen << 32 | slot with a slot that is not dead (k_expire's check); a taken player keeps such an entry on a dead slot.
+// Output unordered, through a warp-aggregated cursor; at most `cap` are written (the host knows n_active).
+__global__ void k_img_active(ActiveView act, uint64_t n_tab, const uint8_t* __restrict__ pool_mode, uint32_t n_slots,
+                             uint32_t gen, void* out, uint32_t id_bytes, uint32_t cap, uint32_t* __restrict__ ctr) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
+  for (uint64_t s0 = (uint64_t)blockIdx.x * blockDim.x; s0 < n_tab; s0 += stride) {  // uniform per CTA
+    const uint64_t s = s0 + threadIdx.x;
+    bool emit = false;
+    uint64_t pid = 0;
+    if (s < n_tab) {
+      unsigned long long v;
+      if (act.dcap) {
+        pid = s;
+        v = *act.val(s);
+      } else {
+        pid = *act.key(s);
+        v = pid < kTombKey ? *act.val(s) : kFreeVal;
+      }
+      emit = v < kPending;
+      const uint32_t slot = (uint32_t)v;
+      if (emit && (uint32_t)(v >> 32) == gen && slot < n_slots && pool_mode[slot] != MM_MODE_DEAD) emit = false;
+    }
+    const uint32_t b = __ballot_sync(0xFFFFFFFFu, emit);
+    if (!b) continue;
+    uint32_t base = 0;
+    if (lane == 0) base = atomicAdd(ctr, (uint32_t)__popc(b));
+    base = __shfl_sync(0xFFFFFFFFu, base, 0);
+    const uint32_t q = base + __popc(b & ((1u << lane) - 1u));
+    if (emit && q < cap) {
+      if (id_bytes == 8) static_cast<uint64_t*>(out)[q] = pid;
+      else static_cast<uint32_t*>(out)[q] = (uint32_t)pid;
+    }
+  }
+}
+
+struct ImgLoadArgs {
+  PoolView pool;
+  PoolMeta meta;
+  ImgCols in;
+  uint32_t n, n_segs;
+  const uint32_t* part_off;   // [n_segs + 1] first image index of the partition
+  const uint32_t* slot_base;  // [n_segs] pool slot of the partition's first player (its first chunk * kTile)
+  BinMap bm;
+  const uint8_t* grp_lut;
+  const uint16_t* bin_seg;
+  const uint32_t* seg_bin_lo;
+  const uint8_t* mode_tsize;
+  uint32_t n_modes;
+  uint32_t seq_next;
+  uint64_t id_limit;  // ids >= id_limit are invalid (the handle range, or the hashed set's reserved keys)
+  uint32_t* err;
+};
+
+// One image player per thread: check it, then write its slot (nothing is written for a player that fails a check).
+__global__ void __launch_bounds__(256) k_img_load(const ImgLoadArgs a) {
+  __shared__ uint32_t s_off[kMaxSegs + 1], s_base[kMaxSegs];
+  for (uint32_t p = threadIdx.x; p <= a.n_segs; p += blockDim.x) {
+    s_off[p] = a.part_off[p];
+    if (p < a.n_segs) s_base[p] = a.slot_base[p];
+  }
+  __syncthreads();
+  const int32_t hi = a.bm.key_lo + (int32_t)a.bm.KR - 1;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += gridDim.x * blockDim.x) {
+    uint32_t lo = 0, e = a.n_segs;  // the last partition whose first index is <= i (empty ones share it)
+    while (e - lo > 1) { const uint32_t mid = (lo + e) >> 1; if (s_off[mid] <= i) lo = mid; else e = mid; }
+    const uint32_t p = lo;
+    const uint64_t pid = img_id(a.in, i);
+    const uint32_t md = a.in.mode[i];
+    const int32_t rt = a.in.rating[i];
+    const uint32_t u = a.in.seq[i] - a.seq_next;  // enqueue order = this distance ascending; 0 is seq_next itself
+    uint32_t bad = 0, bin = 0;
+    if (pid >= a.id_limit) bad |= kImgBadId;
+    if (md >= a.n_modes) {
+      bad |= kImgBadMode;
+    } else {
+      const int32_t r = rt < a.bm.key_lo ? a.bm.key_lo : (rt > hi ? hi : rt);
+      bin = bin_of(a.bm, a.bm.lut, rt, md);
+      if (a.grp_lut[r - a.bm.key_lo] == 0xFF || a.bin_seg[bin] != p) bad |= kImgBadRating;
+    }
+    if (u == 0 || (i + 1 < s_off[p + 1] && a.in.seq[i + 1] - a.seq_next <= u)) bad |= kImgBadSeq;
+    if (bad) { atomicOr(a.err, bad); continue; }
+    const uint32_t slot = s_base[p] + (i - s_off[p]);
+    a.pool.id[slot] = pid; a.pool.rating[slot] = rt; a.pool.mode[slot] = (uint8_t)md;
+    a.pool.tsize[slot] = a.mode_tsize[md]; a.pool.ts[slot] = a.in.ts[i];
+    a.pool.bin[slot] = (uint16_t)bin; a.pool.seq[slot] = a.in.seq[i];
+    atomicAdd(&a.meta.tot[bin], 1u);
+    if (a.meta.chist) atomicAdd(&a.meta.chist[(size_t)(slot / kTile) * kChunkHist + (bin - a.seg_bin_lo[p])], 1u);
+  }
+}
+
+// Ids of an image section into an empty active set with value 0 ("active, not queued"); a second copy of an id — in
+// the same section or the other — sets kImgDup.
+__global__ void k_img_insert(const void* ids, uint32_t id_bytes, uint32_t n, uint64_t id_limit, ActiveView act,
+                             uint32_t* __restrict__ err) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const uint64_t pid = id_bytes == 8 ? static_cast<const uint64_t*>(ids)[i] : static_cast<const uint32_t*>(ids)[i];
+    if (pid >= id_limit) { atomicOr(err, kImgBadId); continue; }
+    if (act.dcap) {
+      if (atomicCAS(act.val(pid), kFreeVal, 0ull) != kFreeVal) atomicOr(err, kImgDup);
+      continue;
+    }
+    uint64_t h = hash64(pid) & act.mask;
+    bool placed = false;
+    for (uint64_t probe = 0; probe <= act.mask && !placed; ++probe) {
+      unsigned long long k = *act.key(h);
+      if (k == kEmptyKey) {
+        k = atomicCAS(act.key(h), kEmptyKey, (unsigned long long)pid);
+        if (k == kEmptyKey) { *act.val(h) = 0ull; placed = true; break; }
+      }
+      if (k == pid) { atomicOr(err, kImgDup); placed = true; break; }
+      h = (h + 1) & act.mask;
+    }
+    if (!placed) atomicOr(err, kImgFull);
+  }
+}
+
+}  // namespace mm

@@ -95,6 +95,26 @@ def wait_quantile(hist, q):
     return int(wait_bucket_bounds()[1][b] - 1)
 
 
+def read_image(buf):
+    """Parse an mm_export image without a GPU -> (abi.ImageHeader, dict of numpy views: part_count, id, rating,
+    enq_ts, seq, mode, active).  Raises ValueError when the buffer is shorter than its header says."""
+    buf = np.frombuffer(buf, np.uint8) if isinstance(buf, (bytes, bytearray, memoryview)) else np.asarray(buf, np.uint8)
+    if len(buf) < C.sizeof(abi.ImageHeader):
+        raise ValueError("image shorter than its header")
+    h = abi.ImageHeader.from_buffer_copy(buf[:C.sizeof(abi.ImageHeader)].tobytes())
+    off = abi.image_offsets(h.n_parts, h.n_players, h.n_active, h.id_bytes)
+    if len(buf) < off[-1]:
+        raise ValueError("image shorter than its sections")
+    idt = np.uint64 if h.id_bytes == 8 else np.uint32
+    n, m = h.n_players, h.n_active
+    cols = {}
+    for k, (name, dt, cnt) in enumerate((("part_count", np.uint32, h.n_parts), ("id", idt, n), ("rating", np.int32, n),
+                                         ("enq_ts", np.uint32, n), ("seq", np.uint32, n), ("mode", np.uint8, n),
+                                         ("active", idt, m))):
+        cols[name] = buf[off[k]:off[k] + cnt * np.dtype(dt).itemsize].view(dt)
+    return h, cols
+
+
 class Engine:
     """One GPU-resident player pool + active set + search tick (single writer)."""
 
@@ -358,6 +378,23 @@ class Engine:
         max_wait = max(0, min(int(max_wait), 0xFFFFFFFF))
         self._check(fn(self.h, int(now) & 0xFFFFFFFFFFFFFFFF, max_wait, _p(ids), _p(seq), cap, C.byref(n)), what)
         return ids[:n.value], (seq[:n.value] if seq is not None else None)
+
+    def export_state(self):
+        """Host image of the queue state (mm_export) -> uint8 array; the engine is not changed.  Layout:
+        include/mm_engine.h, or read_image()."""
+        # one call: a buffer of the layout's size at its upper bound (every slot in use live, every active id outside
+        # the pool, the most partitions, 8-byte ids) always holds the image
+        bound = abi.image_offsets(abi.MM_MAX_GROUPS * abi.MM_MAX_MODES, self.pool_size(), self.active_size(), 8)[-1]
+        buf = np.empty(bound, np.uint8)
+        n = C.c_uint64(0)
+        self._check(self.lib.mm_export(self.h, _p(buf), bound, C.byref(n)), "mm_export")
+        return buf[:n.value]
+
+    def import_state(self, buf):
+        """Load an image written by export_state() into this engine, which must be fresh (mm_import)."""
+        buf = np.ascontiguousarray(np.frombuffer(buf, np.uint8) if isinstance(buf, (bytes, bytearray, memoryview))
+                                   else buf, np.uint8)
+        self._check(self.lib.mm_import(self.h, _p(buf), len(buf)), "mm_import")
 
     def snapshot(self):
         self._check(self.lib.mm_snapshot(self.h), "mm_snapshot")

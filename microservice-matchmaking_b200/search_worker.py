@@ -162,11 +162,12 @@ class SearchPool:
     """
 
     def __init__(self, engine, mode_names, group_names, max_batch=65536, window=None, clock=None, flush_every_s=0.005,
-                 handle_capacity=None, timeout_ms=None):
+                 handle_capacity=None, timeout_ms=None, wall_clock=None):
         import time
         self.window = window
         self.timeout_ms = timeout_ms
         self.clock = clock or time.monotonic
+        self.wall_clock = wall_clock or time.time  # seconds since the epoch: checkpoint() / resume() bridge the downtime
         self._t0 = self.clock()
         self.enqueued_at = {}  # handle -> clock() when the player became resident (insertion = enqueue order)
         self.last_spread = None
@@ -297,6 +298,57 @@ class SearchPool:
                 worker = next(iter(self.workers.values()))
                 worker.send_response(worker.channel_name, player["response-queue"], prepare_timeout_response(player))
         self.stats["timed_out"] += len(expired)
+
+    # -- hand-over to a new process ------------------------------------------------------------
+    CHECKPOINT_MAGIC = b"MMPOOL01"
+
+    def checkpoint(self):
+        """-> bytes: everything a new process needs to go on serving the queued players (resume()).  The staged
+        deliveries are ingested first, so every acked player is in the image, and pending async results are waited
+        for.  Layout: CHECKPOINT_MAGIC, u64 length of a JSON document (the host state: handle table, player documents,
+        enqueue times, mode / group names, the pool clock and the wall time), the JSON, then the engine image
+        (Engine.export_state, opaque here).  Stop consuming before the call: a delivery staged after it is not in the
+        checkpoint, and it stays unacked, so the broker redelivers it."""
+        self.flush()
+        if hasattr(self.engine, "results_wait"):
+            self.engine.results_wait()
+        image = self.engine.export_state()
+        image = image.tobytes() if isinstance(image, np.ndarray) else bytes(image)
+        t = self.clock()
+        state = {
+            "mode_names": self.mode_names, "group_names": self.group_names,
+            "id_of": self.handles.id_of, "free": self.handles.free,
+            "players": [[h, doc] for h, doc in self.players.items()],
+            "enqueued_at": [[h, t - at] for h, at in self.enqueued_at.items()],  # age at the checkpoint, in order
+            "now_ms": self.now_ms(), "wall": self.wall_clock(),
+        }
+        doc = json.dumps(state).encode()
+        return self.CHECKPOINT_MAGIC + len(doc).to_bytes(8, "little") + doc + image
+
+    @classmethod
+    def resume(cls, engine, blob, mode_names, group_names, **opts):
+        """A pool on a FRESH engine that goes on where checkpoint() stopped: the engine imports the image
+        (Engine.import_state), the handle table, player documents and enqueue times come back, and now_ms() goes on
+        from the checkpoint's value plus the wall time the pool was down — the enqueue stamps in the engine stay
+        valid, and waits (timeout_ms, queue_status) include the downtime.  opts: those of SearchPool()."""
+        head = len(cls.CHECKPOINT_MAGIC)
+        if blob[:head] != cls.CHECKPOINT_MAGIC:
+            raise ValueError("not a SearchPool checkpoint")
+        n = int.from_bytes(blob[head:head + 8], "little")
+        state = json.loads(bytes(blob[head + 8:head + 8 + n]))
+        if state["mode_names"] != list(mode_names) or state["group_names"] != list(group_names):
+            raise ValueError("the checkpoint was taken with other mode or group names")
+        pool = cls(engine, mode_names, group_names, **opts)
+        engine.import_state(bytes(blob[head + 8 + n:]))
+        down = max(0.0, pool.wall_clock() - state["wall"])
+        pool._t0 = pool.clock() - down - state["now_ms"] / 1000.0
+        pool.handles.id_of = list(state["id_of"])
+        pool.handles.free = list(state["free"])
+        pool.handles.handle_of = {pid: h for h, pid in enumerate(pool.handles.id_of) if pid is not None}
+        pool.players = {int(h): doc for h, doc in state["players"]}
+        at = pool.clock() - down
+        pool.enqueued_at = {int(h): at - age for h, age in state["enqueued_at"]}
+        return pool
 
     def _teams_of(self, mode):
         return self.engine.cfg.modes[int(mode)].teams
