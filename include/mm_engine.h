@@ -380,6 +380,51 @@ typedef struct mm_image_header {
 int mm_export(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes);
 int mm_import(mm_engine* e, const void* buf, uint64_t n_bytes);
 
+/* ---- queue move: part of an engine into another running engine ---------------------------
+ * The reference's queues live in RabbitMQ and its state in replicated Mnesia tables, so any node's workers can serve
+ * any rating group (application.ex:26-40).  Here a queued player lives in one engine: mm_export_queues releases
+ * whole (mode, group) queues into an image, mm_merge loads that image into an engine that is already running (scale
+ * out / in, rebalancing rating-group shards).
+ *
+ * mm_export_queues: `queues` holds n_modes * n_groups bytes in the record order of mm_queue_stats (mode * n_groups +
+ * group); a non-zero byte selects the queue.  The image has the mm_image_header layout with magic
+ * MM_QUEUE_IMAGE_MAGIC: part_count is zero for the partitions of unselected queues, sections 2-6 hold the selected
+ * queues' live players (partition by partition, enqueue order inside a partition), and section 7 is EMPTY — an id that
+ * is matched (or taken) and not yet removed cannot be attributed to a queue, so it stays in the source's active set
+ * and its mm_remove goes to the source.  buf = NULL with cap = 0 -> *n_bytes = the size, nothing changes; cap too
+ * small -> MM_E_CAP and *n_bytes, nothing changes.  A call that writes the image RELEASES its players in the same
+ * call, exactly as mm_remove of their ids would (dead slots until the next tick, counted in n_removed): a tick between
+ * an export and a release would match players who are already on their way.  MM_E_STATE while an
+ * mm_enqueue_packed_begin batch is staged; pending async_results copies are left alone.
+ *
+ * mm_merge: refusals, all decided before anything changes:
+ *   MM_E_ARG   bad magic (an mm_export image is refused here, and mm_import refuses a queue image), version, lengths,
+ *              id width, a config that differs on the fields mm_import compares, a player whose mode is >= n_modes,
+ *              whose rating has no group or does not map to its partition, whose id or handle is out of range, or
+ *              sequence numbers out of order inside a partition (a device pre-pass over the image columns);
+ *   MM_E_STATE a queue the image's players fall into holds a LIVE player here (dead slots are fine), or a staged
+ *              packed batch;
+ *   MM_E_CAP   the players that would be queued do not fit the capacity (pool slots in use + players queued), or the
+ *              3/4 load of a hashed active set, or more players would be rejected than `cap` holds (*n_rejected then
+ *              holds the count).  These are exact: the ids that would be rejected are counted first when needed.
+ * The load is one ingest batch: each queue's players in the source's enqueue order, appended per partition, with the
+ * image's enq_ts; they take this engine's next n_players sequence numbers in that order.  An id already in this
+ * engine's active set, or a later copy of an id inside the image, is not queued: its image index goes to `rejected`
+ * (ascending).  MM_F_NO_DEDUPE engines reject nothing.  mm_enqueue_rejects still describes the last mm_enqueue*
+ * batch afterwards.
+ *
+ * EQUIVALENCE.  After a move, the source behaves like a twin that called mm_remove on the moved ids.  On the target,
+ * every later call sequence gives, for the moved queues, what the source would have given: lobbies, members,
+ * n_matched, in_queue, pool_read and the waiting section of mm_queue_stats; emit_seq as an order (sorting a moved
+ * queue's lobbies by emit_seq gives the source's order; the numbers are the target's).  Queues never depend on each
+ * other (S0 and S1 alike), so the unselected queues of both engines are unaffected.  Merging the image back into the
+ * source restores the source's results; until the source's next tick the released players' dead slots still count
+ * against its capacity, so a source that was nearly full may refuse it (MM_E_CAP) until then.                                                                               */
+#define MM_QUEUE_IMAGE_MAGIC 0x5155514Du /* "MQUQ": same header and sections as an mm_export image */
+
+int mm_export_queues(mm_engine* e, const uint8_t* queues, void* buf, uint64_t cap, uint64_t* n_bytes);
+int mm_merge(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t cap, uint32_t* rejected, uint32_t* n_rejected);
+
 /* Use an externally owned CUDA stream (cudaStream_t passed as void*).              */
 int mm_set_stream(mm_engine* e, void* cuda_stream);
 

@@ -229,6 +229,50 @@ static ERL_NIF_TERM nif_import_image(ErlNifEnv* env, int argc, const ERL_NIF_TER
   return rc ? err(env, rc) : atom(env, "ok");
 }
 
+/* export_queues(ref, queues :: binary(u8[n_modes * n_groups])) -> {:ok, image :: binary}: the selected (mode, group)
+ * queues leave the engine in a queue image (mm_export_queues; the players are released in the same call).  One call:
+ * the binary is allocated at the layout's upper bound without an active section and shrunk to the image. */
+static ERL_NIF_TERM nif_export_queues(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary sel; uint32_t n = 0; uint64_t size = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &sel) ||
+      sel.size == 0 || sel.size > MM_MAX_GROUPS * MM_MAX_MODES)
+    return enif_make_badarg(env);
+  if (mm_pool_size(r->e, &n)) return err(env, MM_E_ARG);
+  /* the engine reads n_modes * n_groups bytes: pad a short binary with "not selected" */
+  uint8_t queues[MM_MAX_GROUPS * MM_MAX_MODES] = {0};
+  memcpy(queues, sel.data, sel.size);
+  uint64_t bound = sizeof(mm_image_header), sec[7];
+  sec[0] = 4ull * MM_MAX_GROUPS * MM_MAX_MODES; sec[1] = 8ull * n; sec[2] = sec[3] = sec[4] = 4ull * n; sec[5] = n;
+  sec[6] = 0;
+  for (int k = 0; k < 7; ++k) bound = (bound + sec[k] + 7) & ~7ull;
+  ErlNifBinary img;
+  if (!enif_alloc_binary((size_t)bound, &img)) return err(env, MM_E_CAP);
+  int rc = mm_export_queues(r->e, queues, img.data, bound, &size);
+  if (rc) { enif_release_binary(&img); return err(env, rc); }
+  enif_realloc_binary(&img, (size_t)size);
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &img));
+}
+
+/* merge_image(ref, image :: binary) -> {:ok, rejected :: binary(u32[])} | {:error, atom}: loads a queue image into
+ * this running engine (mm_merge); `rejected` holds the image indices of players not queued (already active here). */
+static ERL_NIF_TERM nif_merge_image(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary img, rej; uint32_t cap = 0, got = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &img))
+    return enif_make_badarg(env);
+  if (img.size >= sizeof(mm_image_header)) {
+    mm_image_header h;
+    memcpy(&h, img.data, sizeof(h));
+    cap = h.n_players < img.size ? h.n_players : (uint32_t)img.size;  /* a corrupt count must not size the list */
+  }
+  if (!enif_alloc_binary((size_t)cap * 4, &rej)) return err(env, MM_E_CAP);
+  int rc = mm_merge(r->e, img.data, img.size, cap, (uint32_t*)rej.data, &got);
+  if (rc) { enif_release_binary(&rej); return err(env, rc); }
+  enif_realloc_binary(&rej, (size_t)got * 4);
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &rej));
+}
+
 /* set_max_spread(ref, w): extension knob (strategist policy S1); w < 0 restores the reference behaviour */
 static ERL_NIF_TERM nif_set_max_spread(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
   engine_res* r; ErlNifSInt64 w = -1;
@@ -254,6 +298,8 @@ static ErlNifFunc funcs[] = {
   {"expire_packed", 3, nif_expire_packed, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"export_image", 1, nif_export_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"import_image", 2, nif_import_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"export_queues", 2, nif_export_queues, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"merge_image", 2, nif_merge_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"set_max_spread", 2, nif_set_max_spread, 0},
 };
 ERL_NIF_INIT(Elixir.Matchmaking.Search.Engine, funcs, load, NULL, NULL, NULL)

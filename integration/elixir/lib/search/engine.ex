@@ -70,6 +70,20 @@ defmodule Matchmaking.Search.Engine do
   @doc "Loads an export_image/1 image into a fresh engine of the same config -> :ok | {:error, :badarg | :capacity | :state}"
   def import_image(_ref, _image), do: :erlang.nif_error(:nif_not_loaded)
 
+  @doc """
+  Queue move: the selected (mode, group) queues (queues :: binary, one byte per queue in queue_stats/2 record order,
+  mode * n_groups + group, non-zero = selected) leave the engine in a queue image -> {:ok, image}.  The players are
+  released as if removed, in the same call; matched players not yet removed stay here.
+  """
+  def export_queues(_ref, _queues), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Loads an export_queues/2 image into this running engine -> {:ok, rejected :: binary(u32[] image indices)} |
+  {:error, :badarg | :capacity | :state}; a refusal changes nothing.
+  """
+  def merge_image(_ref, _image), do: :erlang.nif_error(:nif_not_loaded)
+  def n_modes, do: length(@modes)
+  def n_groups, do: length(@rating_groups)
+
   @doc "Extension (not reference behaviour): maximum rating spread of a lobby for the following ticks; < 0 = off."
   def set_max_spread(_ref, _w), do: :erlang.nif_error(:nif_not_loaded)
 end

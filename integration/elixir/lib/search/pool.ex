@@ -21,6 +21,8 @@ defmodule Matchmaking.Search.Pool do
                      starts a pool on a fresh engine from it; the clock goes on from the checkpoint plus the time the
                      pool was down (INTEGRATION.md §3 has the order: stop consuming, checkpoint, start with resume:,
                      consume again)
+      move_out/1, move_in/1   queue move between running pools: the queues of some rating groups leave this pool
+                     with the players' documents and are merged into another pool (INTEGRATION.md §5)
       attach/1       a search worker hands over its open channel (patched init); the pool ticks only once it has a
                      channel to publish lobbies and timeout responses on — a staged delivery sets it too
 
@@ -53,6 +55,19 @@ defmodule Matchmaking.Search.Pool do
   def remove_user(player_id), do: GenServer.call(__MODULE__, {:remove_user, player_id})
   def queue_status(group_index), do: GenServer.call(__MODULE__, {:queue_status, group_index})
   def checkpoint, do: GenServer.call(__MODULE__, :checkpoint, :infinity)
+  @doc """
+  Queue move, old owner: the staged deliveries are ingested, then the queues of these rating groups (indices, all
+  modes) leave the engine (Engine.export_queues) with the players' documents -> {:ok, blob} for move_in/1 on the new
+  owner.  Reroute the groups' deliveries to the new owner first (INTEGRATION.md §5).
+  """
+  def move_out(groups), do: GenServer.call(__MODULE__, {:move_out, groups}, :infinity)
+  @doc """
+  Queue move, new owner: the moved players get handles of this pool, their enqueue stamps are shifted into its clock
+  (bridged by the wall time), the engine merges the image (Engine.merge_image) and the documents of players already
+  queued here are dropped -> {:ok, merged} | {:error, reason}; a refusal changes nothing (merge the blob back into the
+  old owner, or keep it and retry).
+  """
+  def move_in(blob), do: GenServer.call(__MODULE__, {:move_in, blob}, :infinity)
 
   @impl true
   def init(opts) do
@@ -139,6 +154,77 @@ defmodule Matchmaking.Search.Pool do
       {:error, _} = e -> {:reply, e, st}
     end
   end
+
+  # -- queue move: part of this pool into another running pool (INTEGRATION.md §5) ---------------------------------
+  def handle_call({:move_out, groups}, _from, st) do
+    st = flush(st)
+    n_groups = Engine.n_groups()
+    queues = for _m <- 0..(Engine.n_modes() - 1), g <- 0..(n_groups - 1), into: <<>>,
+               do: <<(if g in groups, do: 1, else: 0)>>
+    case Engine.export_queues(st.ref, queues) do
+      {:ok, image} ->
+        {n, id_off, _} = image_sections(image)
+        handles = for <<h::little-32 <- binary_part(image, id_off, 4 * n)>>, do: h
+        {moved, st} = Enum.map_reduce(handles, st, fn h, acc ->
+          {player, players} = Map.pop(acc.players, h)
+          {{player["id"], player}, release(%{acc | players: players}, player["id"], h)}
+        end)
+        blob = %{image: image, players: moved, n_modes: Engine.n_modes(), n_groups: n_groups,
+                 now_ms: now_ms(st), wall_ms: System.os_time(:millisecond)}
+        {:reply, {:ok, :erlang.term_to_binary(blob)}, st}
+      {:error, _} = e -> {:reply, e, st}
+    end
+  end
+
+  def handle_call({:move_in, blob}, _from, st) do
+    st = flush(st)
+    mv = :erlang.binary_to_term(blob, [:safe])
+    if mv.n_modes != Engine.n_modes() or mv.n_groups != Engine.n_groups() do
+      {:reply, {:error, :other_queues}, st}
+    else
+      # handles of this pool for the moved ids; the image's id column is rewritten with them
+      {rows, st} = Enum.map_reduce(mv.players, st, fn {id, player}, acc ->
+        {h, fresh, acc} = acquire(acc, id)
+        {{h, fresh, id, player}, acc}
+      end)
+      {n, id_off, ts_off} = image_sections(mv.image)
+      # enqueue stamps into this pool's clock: the wait at move_out plus the wall time in between, as resume/2 does
+      down = max(0, System.os_time(:millisecond) - mv.wall_ms)
+      shift = Bitwise.band(now_ms(st) - down - mv.now_ms, 0xFFFFFFFF)
+      ids = for {h, _, _, _} <- rows, into: <<>>, do: <<h::little-32>>
+      ts = for <<t::little-32 <- binary_part(mv.image, ts_off, 4 * n)>>, into: <<>>,
+             do: <<Bitwise.band(t + shift, 0xFFFFFFFF)::little-32>>
+      image = binary_part(mv.image, 0, id_off) <> ids <>
+              binary_part(mv.image, id_off + 4 * n, ts_off - id_off - 4 * n) <> ts <>
+              binary_part(mv.image, ts_off + 4 * n, byte_size(mv.image) - ts_off - 4 * n)
+      case Engine.merge_image(st.ref, image) do
+        {:ok, rejected} ->
+          rej = MapSet.new(for <<i::little-32 <- rejected>>, do: i)
+          st = rows |> Enum.with_index() |> Enum.reduce(st, fn {{h, fresh, id, _}, i}, acc ->
+            # a rejected player is already queued here: keep this pool's player and document
+            if MapSet.member?(rej, i) and fresh, do: release(acc, id, h), else: acc
+          end)
+          players = for {{h, _, _, player}, i} <- Enum.with_index(rows), not MapSet.member?(rej, i), into: st.players,
+                      do: {h, player}
+          {:reply, {:ok, n - MapSet.size(rej)}, %{st | players: players}}
+        {:error, _} = e ->
+          st = Enum.reduce(rows, st, fn {h, fresh, id, _}, acc -> if fresh, do: release(acc, id, h), else: acc end)
+          {:reply, e, st}
+      end
+    end
+  end
+
+  # The image's player columns (include/mm_engine.h): the 624-byte header, part_count u32[n_parts], then id (u32
+  # handles on this MM_F_DENSE_IDS engine), rating, enq_ts, seq, mode, each section starting at a multiple of 8.
+  defp image_sections(image) do
+    <<_::binary-size(24), n_parts::little-32, n::little-32, _::binary>> = image
+    a8 = fn x -> Bitwise.band(x + 7, Bitwise.bnot(7)) end
+    id_off = a8.(624 + 4 * n_parts)
+    rating_off = a8.(id_off + 4 * n)
+    ts_off = a8.(rating_off + 4 * n)
+    {n, id_off, ts_off}
+  end
+
 
   @impl true
   def handle_info(:flush, st) do

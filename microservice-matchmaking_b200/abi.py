@@ -93,6 +93,7 @@ class QueueStat(C.Structure):
 
 
 MM_IMAGE_MAGIC = 0x474D494D
+MM_QUEUE_IMAGE_MAGIC = 0x5155514D  # mm_export_queues: same header and sections, no active section
 MM_IMAGE_VERSION = 1
 
 
@@ -155,6 +156,8 @@ PROTOTYPES = {
     "mm_expire_packed": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_export": (C.c_int, [_vp, _vp, C.c_uint64, _P(C.c_uint64)]),
     "mm_import": (C.c_int, [_vp, _vp, C.c_uint64]),
+    "mm_export_queues": (C.c_int, [_vp, _vp, _vp, C.c_uint64, _P(C.c_uint64)]),
+    "mm_merge": (C.c_int, [_vp, _vp, C.c_uint64, C.c_uint32, _vp, _P(C.c_uint32)]),
     "mm_snapshot": (C.c_int, [_vp]),
     "mm_restore": (C.c_int, [_vp]),
     "mm_set_stream": (C.c_int, [_vp, _vp]),

@@ -177,6 +177,15 @@ struct mm_engine {
   uint32_t* d_img_part = nullptr;  // export: [n_segs] live slots per partition; import: part_off[n_segs+1] | slot_base[n_segs]
   void* d_img_act = nullptr;       // export: the active section
   uint64_t img_act_cap = 0;        // bytes
+
+  // mm_export_queues / mm_merge.  Like the image buffers, the batch-sized merge scratch is freed by every call.
+  std::vector<uint16_t> h_part_cut;   // host copies of d_part_cut / d_cut_lp_lo
+  std::vector<uint32_t> h_cut_lp_lo;
+  uint8_t* d_sel = nullptr;           // [n_segs] selected partitions
+  uint32_t* d_mrg_src = nullptr;      // merge batch index -> image index
+  uint8_t* d_mrg_code = nullptr;      // the merge batch's ingest codes (d_code keeps the last mm_enqueue* batch's)
+  uint32_t mrg_code_cap = 0;
+  unsigned long long* d_mrg_seen = nullptr;  // duplicate count: scratch id set
 };
 
 namespace {
@@ -383,6 +392,8 @@ int build_tables(mm_engine* e) {
   e->n_segs = (uint32_t)seg_lo.size();
   if (e->n_segs > kMaxSegs) return MM_E_ARG;
   cut_lp_lo[e->n_cut] = e->n_segs;
+  e->h_part_cut = part_cut;
+  e->h_cut_lp_lo = cut_lp_lo;
   seg_lo.push_back(e->K);
   e->max_nb = 1;
   for (uint32_t sgi = 0; sgi < e->n_segs; ++sgi) e->max_nb = std::max(e->max_nb, seg_lo[sgi + 1] - seg_lo[sgi]);
@@ -466,13 +477,14 @@ int rehash(mm_engine* e) {
   return MM_OK;
 }
 
-// capacity checks + scratch for an ingest batch of n players
-int enq_prepare(mm_engine* e, uint32_t n) {
+// capacity checks + scratch for an ingest batch of n players, of which at most n_new can add an active-set entry
+// (mm_merge counts them exactly; every other batch passes n)
+int enq_prepare(mm_engine* e, uint32_t n, uint32_t n_new) {
   e->fresh = false;
   int rc = ensure_enq_scratch(e, n);
   if (rc) return rc;
-  if (e->use_active && !e->dense_ids && (e->n_active + e->n_tomb + n) * 4 > e->hcap * 3) {
-    if ((e->n_active + n) * 4 > e->hcap * 3) {
+  if (e->use_active && !e->dense_ids && (e->n_active + e->n_tomb + n_new) * 4 > e->hcap * 3) {
+    if ((e->n_active + n_new) * 4 > e->hcap * 3) {
       std::snprintf(e->last_err, sizeof(e->last_err), "active set full: %llu ids resident, batch of %u, capacity %llu",
                     (unsigned long long)e->n_active, n, (unsigned long long)(e->hcap * 3 / 4));
       return MM_E_CAP;
@@ -535,7 +547,7 @@ int enq_finish(mm_engine* e, uint32_t n, uint8_t* accepted_dev, uint32_t* n_acce
 template <class Upload>
 int enqueue_batch(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating, const uint8_t* mode,
                   const uint32_t* ts, uint32_t chunk, Upload upload) {
-  int rc = enq_prepare(e, n);
+  int rc = enq_prepare(e, n, n);
   if (rc) return rc;
   const bool may_overflow = (uint64_t)e->pool[e->cur].n + n > e->capacity;
   for (uint32_t base = 0; base < n; base += chunk) {
@@ -876,7 +888,19 @@ int grow(mm_engine* e, T*& p, uint64_t& cap, uint64_t want) {
   return MM_OK;
 }
 
-int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes) {
+// d_sel <- the partitions of the (mode, group) queues whose byte in `queues` (n_cut bytes) is non-zero
+int upload_sel(mm_engine* e, const uint8_t* queues) {
+  std::vector<uint8_t> sel(e->n_segs);
+  for (uint32_t s = 0; s < e->n_segs; ++s) sel[s] = queues[e->h_part_cut[s]] != 0;
+  if (!e->d_sel) CK(cudaMalloc(&e->d_sel, kMaxSegs));
+  CK(cudaMemcpyAsync(e->d_sel, sel.data(), e->n_segs, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaStreamSynchronize(e->stream));  // `sel` is pageable and goes out of scope
+  return MM_OK;
+}
+
+// mm_export (queues = null) and mm_export_queues (queues: n_cut selection bytes; the image has no active section, and
+// a call that writes it releases the exported players through k_expire with the same selection and max_wait = 0)
+int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes, const uint8_t* queues) {
   if (e->stage_count) {
     std::snprintf(e->last_err, sizeof(e->last_err), "a packed batch is staged: call mm_enqueue_packed_end first");
     return MM_E_STATE;
@@ -884,6 +908,7 @@ int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes) {
   const Pool& p = e->pool[e->cur];
   const uint32_t idb = id_bytes(e);
   int rc;
+  if (queues && (rc = upload_sel(e, queues))) return rc;
   // pass 1: live slots per tile and per partition, the tiles' offsets; the active section
   const uint32_t tiles = p.n / kTile + e->n_segs;  // bounds the virtual tile count
   const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(tiles, 8u * (uint32_t)e->n_sms));
@@ -896,9 +921,10 @@ int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes) {
   CK(cudaMemsetAsync(e->d_small + 12, 0, 8, e->stream));
   ImgExportArgs a{};
   a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.tile_cnt = e->d_img_tile; a.part_cnt = e->d_img_part;
+  a.sel = queues ? e->d_sel : nullptr;
   if (p.n) k_img_tiles<kImgBlock, false><<<ctas, kImgBlock, 0, e->stream>>>(a);
   k_scan_small<<<1, 1024, 0, e->stream>>>(tiles, e->d_img_tile, e->d_small + 12);
-  const uint32_t act_cap = (uint32_t)std::min<uint64_t>(e->n_active, 0xFFFFFFFFu);
+  const uint32_t act_cap = queues ? 0u : (uint32_t)std::min<uint64_t>(e->n_active, 0xFFFFFFFFu);
   if (e->use_active && act_cap) {
     if ((rc = grow(e, e->d_img_act, e->img_act_cap, (uint64_t)act_cap * idb))) return rc;
     const uint64_t n_tab = e->hcap;
@@ -932,7 +958,7 @@ int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes) {
     CK(cudaGetLastError());
   }
   mm_image_header h{};
-  h.magic = MM_IMAGE_MAGIC; h.version = MM_IMAGE_VERSION; h.abi_version = MM_ABI_VERSION; h.id_bytes = idb;
+  h.magic = queues ? MM_QUEUE_IMAGE_MAGIC : MM_IMAGE_MAGIC; h.version = MM_IMAGE_VERSION; h.abi_version = MM_ABI_VERSION; h.id_bytes = idb;
   h.total_bytes = l.off[7]; h.n_parts = e->n_segs; h.n_players = n; h.n_active = m; h.seq_next = e->seq_next;
   h.config = e->cfg;
   std::memcpy(out, &h, sizeof(h));
@@ -941,7 +967,22 @@ int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes) {
   CK(cudaMemcpyAsync(out + l.off[0], e->d_img_part, (size_t)e->n_segs * 4, cudaMemcpyDeviceToHost, e->stream));
   if (n) CK(cudaMemcpyAsync(out + l.off[1], e->d_img, col_bytes, cudaMemcpyDeviceToHost, e->stream));
   if (m) CK(cudaMemcpyAsync(out + l.off[6], e->d_img_act, (size_t)m * idb, cudaMemcpyDeviceToHost, e->stream));
+  if (queues && n) {  // release the exported players, as mm_remove would: dead slots until the next tick
+    ExpireArgs x{};
+    x.pool = p.v; x.meta = p.m; x.n_segs = e->n_segs; x.now = 0; x.max_wait = 0; x.commit = 1;
+    x.act = act_view(e); x.gen = e->gen; x.dead_bin = e->K; x.bin_seg = e->d_bin_seg; x.seg_bin_lo = e->d_seg_bin_lo;
+    x.sel = e->d_sel; x.ctr = e->d_small + 8;
+    CK(cudaMemsetAsync(x.ctr, 0, 8, e->stream));
+    k_expire<kExpBlock><<<ctas, kExpBlock, 0, e->stream>>>(x);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(e->h_small + 8, x.ctr, 8, cudaMemcpyDeviceToHost, e->stream));
+  }
   CK(cudaStreamSynchronize(e->stream));
+  if (queues && n) {
+    const uint32_t erased = e->h_small[9];
+    e->n_active -= std::min<uint64_t>(erased, e->n_active);
+    if (e->use_active && !e->dense_ids) e->n_tomb += erased;
+  }
   return MM_OK;
 }
 
@@ -949,6 +990,8 @@ int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes) {
 void free_img_scratch(mm_engine* e) {
   cudaFree(e->d_img); cudaFree(e->d_img_act);
   e->d_img = nullptr; e->img_cap = 0; e->d_img_act = nullptr; e->img_act_cap = 0;
+  cudaFree(e->d_mrg_src); cudaFree(e->d_mrg_code); cudaFree(e->d_mrg_seen);
+  e->d_mrg_src = nullptr; e->d_mrg_code = nullptr; e->mrg_code_cap = 0; e->d_mrg_seen = nullptr;
 }
 
 // The current pool buffer and the active set back to an empty engine's state.
@@ -969,6 +1012,16 @@ int clear_engine(mm_engine* e) {
   return MM_OK;
 }
 
+// the config fields an image must share with the engine that loads it (capacity, active_capacity, device may differ)
+bool same_layout(const mm_config& a, const mm_config& c) {
+  bool same = a.n_groups == c.n_groups && a.default_group == c.default_group && a.n_modes == c.n_modes &&
+              a.order_mode == c.order_mode && a.flags == c.flags;
+  for (uint32_t g = 0; same && g < c.n_groups; ++g) same = a.group_lo[g] == c.group_lo[g] && a.group_hi[g] == c.group_hi[g];
+  for (uint32_t m = 0; same && m < c.n_modes; ++m)
+    same = a.modes[m].teams == c.modes[m].teams && a.modes[m].team_size == c.modes[m].team_size;
+  return same;
+}
+
 int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
   auto bad = [&](const char* what) {
     std::snprintf(e->last_err, sizeof(e->last_err), "image rejected: %s", what);
@@ -987,13 +1040,8 @@ int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
   if (h.n_parts != e->n_segs) return bad("partition count differs from the engine's layout");
   const ImgLayout l = img_layout(h.n_parts, h.n_players, h.n_active, h.id_bytes);
   if (h.total_bytes != l.off[7] || nb != l.off[7]) return bad("length does not match the header's section counts");
-  const mm_config &a = h.config, &c = e->cfg;
-  bool same = a.n_groups == c.n_groups && a.default_group == c.default_group && a.n_modes == c.n_modes &&
-              a.order_mode == c.order_mode && a.flags == c.flags;
-  for (uint32_t g = 0; same && g < c.n_groups; ++g) same = a.group_lo[g] == c.group_lo[g] && a.group_hi[g] == c.group_hi[g];
-  for (uint32_t m = 0; same && m < c.n_modes; ++m)
-    same = a.modes[m].teams == c.modes[m].teams && a.modes[m].team_size == c.modes[m].team_size;
-  if (!same) return bad("config differs from the engine's (groups, default_group, modes, order_mode or flags)");
+  if (!same_layout(h.config, e->cfg))
+    return bad("config differs from the engine's (groups, default_group, modes, order_mode or flags)");
   if (!e->use_active && h.n_active) return bad("active section in an image of an engine without an active set");
   std::vector<uint32_t> cnt(e->n_segs);
   std::memcpy(cnt.data(), buf + l.off[0], (size_t)e->n_segs * 4);
@@ -1077,6 +1125,161 @@ int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
   }
   CK(cudaStreamSynchronize(e->stream));
   return MM_OK;
+}
+
+// live players per partition of the current pool, restricted to the partitions in d_sel (the export count pass)
+int count_live(mm_engine* e, std::vector<uint32_t>& per_part) {
+  const Pool& p = e->pool[e->cur];
+  per_part.assign(e->n_segs, 0);
+  if (!p.n) return MM_OK;
+  const uint32_t tiles = p.n / kTile + e->n_segs;
+  const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(tiles, 8u * (uint32_t)e->n_sms));
+  uint64_t tile_cap = e->img_tile_cap;
+  int rc;
+  if ((rc = grow(e, e->d_img_tile, tile_cap, (uint64_t)tiles * 4))) return rc;
+  e->img_tile_cap = (uint32_t)tile_cap;
+  if (!e->d_img_part) CK(cudaMalloc(&e->d_img_part, ((size_t)3 * e->n_segs + 2) * 4));
+  CK(cudaMemsetAsync(e->d_img_part, 0, (size_t)e->n_segs * 4, e->stream));
+  ImgExportArgs a{};
+  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.tile_cnt = e->d_img_tile; a.part_cnt = e->d_img_part;
+  a.sel = e->d_sel;
+  k_img_tiles<kImgBlock, false><<<ctas, kImgBlock, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(per_part.data(), e->d_img_part, (size_t)e->n_segs * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
+// mm_merge: every check first (header, config, the queues' live players here, the device pre-pass over the players,
+// the capacities and the reject list's size), then one ingest batch through enq_prepare / enq_chunk / enq_finish with
+// its codes in d_mrg_code, so that mm_enqueue_rejects still reads the last mm_enqueue* batch.
+int merge_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uint32_t* rejected, uint32_t* n_rejected) {
+  auto bad = [&](const char* what) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "queue image rejected: %s", what);
+    return (int)MM_E_ARG;
+  };
+  if (e->stage_count) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "a packed batch is staged: call mm_enqueue_packed_end first");
+    return MM_E_STATE;
+  }
+  mm_image_header h;
+  if (nb < sizeof(h)) return bad("shorter than its header");
+  std::memcpy(&h, buf, sizeof(h));
+  if (h.magic != MM_QUEUE_IMAGE_MAGIC) return bad("bad magic (not an mm_export_queues image)");
+  if (h.version != MM_IMAGE_VERSION || h.abi_version != MM_ABI_VERSION) return bad("unknown version");
+  if (h.id_bytes != id_bytes(e)) return bad("id width differs from the engine's");
+  if (h.n_parts != e->n_segs) return bad("partition count differs from the engine's layout");
+  if (h.n_active) return bad("a queue image has no active section");
+  const ImgLayout l = img_layout(h.n_parts, h.n_players, 0, h.id_bytes);
+  if (h.total_bytes != l.off[7] || nb != l.off[7]) return bad("length does not match the header's section counts");
+  if (!same_layout(h.config, e->cfg))
+    return bad("config differs from the engine's (groups, default_group, modes, order_mode or flags)");
+  std::vector<uint32_t> cnt(e->n_segs), off(e->n_segs + 1, 0);
+  std::memcpy(cnt.data(), buf + l.off[0], (size_t)e->n_segs * 4);
+  uint64_t sum = 0;
+  for (uint32_t s = 0; s < e->n_segs; ++s) { off[s] = (uint32_t)std::min<uint64_t>(sum, 0xFFFFFFFFu); sum += cnt[s]; }
+  if (sum != h.n_players) return bad("partition counts do not add up to the player count");
+  const uint32_t n = h.n_players;
+  off[e->n_segs] = n;
+  if (n == 0) return MM_OK;
+  // the queues the image fills must hold no live player here
+  std::vector<uint8_t> touched(e->n_cut, 0);
+  for (uint32_t s = 0; s < e->n_segs; ++s)
+    if (cnt[s]) touched[e->h_part_cut[s]] = 1;
+  int rc;
+  if ((rc = upload_sel(e, touched.data()))) return rc;
+  std::vector<uint32_t> live;
+  if ((rc = count_live(e, live))) return rc;
+  for (uint32_t s = 0; s < e->n_segs; ++s)
+    if (live[s]) {
+      const uint32_t c = e->h_part_cut[s];
+      std::snprintf(e->last_err, sizeof(e->last_err), "queue (mode %u, group %u) holds %u live players here",
+                    c / e->cfg.n_groups, c % e->cfg.n_groups, live[s]);
+      return MM_E_STATE;
+    }
+  // upload once; the pre-pass checks every player and writes the ingest batch in the queues' enqueue order
+  if ((rc = ensure_enq_scratch(e, n))) return rc;
+  const uint64_t body = l.off[6] - l.off[1];
+  if ((rc = grow(e, e->d_img, e->img_cap, std::max<uint64_t>(body, 8)))) return rc;
+  CK(cudaMalloc(&e->d_mrg_src, ((size_t)n + 64) * 4));
+  if (!e->d_img_part) CK(cudaMalloc(&e->d_img_part, ((size_t)3 * e->n_segs + 2) * 4));
+  CK(cudaMemcpyAsync(e->d_img, buf + l.off[1], body, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(e->d_img_part, off.data(), off.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemsetAsync(e->d_small + 14, 0, 8, e->stream));
+  const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((n + 255) / 256, 32u * (uint32_t)e->n_sms));
+  MrgOrderArgs oa{};
+  oa.in = img_cols(e->d_img, l, h.id_bytes); oa.n = n; oa.n_segs = e->n_segs; oa.part_off = e->d_img_part;
+  oa.part_cut = e->d_part_cut; oa.cut_lp_lo = e->d_cut_lp_lo; oa.bm = bin_map(e); oa.grp_lut = e->d_grp_lut;
+  oa.bin_seg = e->d_bin_seg; oa.n_modes = e->cfg.n_modes; oa.seq_next = h.seq_next; oa.id_limit = id_limit(e);
+  oa.out_id = e->d_in_id; oa.out_rating = e->d_in_rating; oa.out_mode = e->d_in_mode; oa.out_ts = e->d_in_ts;
+  oa.src = e->d_mrg_src; oa.err = e->d_small + 14;
+  k_mrg_order<<<grid, 256, 0, e->stream>>>(oa);
+  CK(cudaGetLastError());
+  // the exact reject count, when the reject list or a capacity could be too small for every player being queued
+  const Pool& p = e->pool[e->cur];
+  const bool hashed = e->use_active && !e->dense_ids;
+  const bool tight = (uint64_t)p.n + n > e->capacity || (hashed && (e->n_active + n) * 4 > e->hcap * 3);
+  if (e->use_active && (cap < n || tight)) {
+    uint64_t sc = 1024;
+    while (sc < 2ull * n) sc <<= 1;
+    CK(cudaMalloc(&e->d_mrg_seen, sc * 8));
+    CK(cudaMemsetAsync(e->d_mrg_seen, 0xFF, sc * 8, e->stream));
+    k_mrg_dups<<<grid, 256, 0, e->stream>>>(e->d_in_id, n, act_view(e), e->d_mrg_seen, sc - 1, e->d_small + 15);
+    CK(cudaGetLastError());
+  }
+  CK(cudaMemcpyAsync(e->h_small + 14, e->d_small + 14, 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  if (const uint32_t err = e->h_small[14]) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "queue image rejected:%s%s%s%s", err & kImgBadId ? " id out of range" : "",
+                  err & kImgBadMode ? " mode out of range" : "", err & kImgBadRating ? " rating outside its partition" : "",
+                  err & kImgBadSeq ? " sequence numbers out of order" : "");
+    return MM_E_ARG;
+  }
+  const uint32_t n_rej = e->h_small[15], accepted = n - n_rej;
+  if (n_rej > cap) {
+    *n_rejected = n_rej;
+    std::snprintf(e->last_err, sizeof(e->last_err), "%u rejected players, cap %u", n_rej, cap);
+    return MM_E_CAP;
+  }
+  if ((uint64_t)p.n + accepted > e->capacity) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "%u players merged into %u slots in use, capacity %u", accepted, p.n,
+                  e->capacity);
+    return MM_E_CAP;
+  }
+  if (hashed && (e->n_active + accepted) * 4 > e->hcap * 3) {
+    std::snprintf(e->last_err, sizeof(e->last_err), "active set full: %llu ids resident, %u merged, capacity %llu",
+                  (unsigned long long)e->n_active, accepted, (unsigned long long)(e->hcap * 3 / 4));
+    return MM_E_CAP;
+  }
+  // the ingest, with the merge's own code buffer
+  auto ingest = [&]() -> int {
+    int r = enq_prepare(e, n, accepted);
+    for (uint32_t base = 0; !r && base < n; base += kEnqChunkDev)
+      r = enq_chunk(e, base, std::min(kEnqChunkDev, n - base), e->d_in_id, e->d_in_rating, e->d_in_mode, e->d_in_ts, false);
+    uint32_t n_acc = 0;
+    if (!r) r = enq_finish(e, n, nullptr, &n_acc);
+    if (r || n_acc == n) return r;
+    uint32_t* d_out = e->d_in_handle;  // free once the batch is in
+    CK(cudaMemsetAsync(e->d_small + 4, 0, 4, e->stream));
+    k_mrg_rejects<<<(n + 255) / 256, 256, 0, e->stream>>>(n, e->d_code, e->d_mrg_src, d_out, e->d_small + 4);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(e->h_small + 4, e->d_small + 4, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    const uint32_t k = std::min(e->h_small[4], cap);
+    CK(cudaMemcpyAsync(rejected, d_out, (size_t)k * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    std::sort(rejected, rejected + k);
+    *n_rejected = k;
+    return MM_OK;
+  };
+  const uint32_t last_n = e->last_batch_n;
+  std::swap(e->d_code, e->d_mrg_code);
+  std::swap(e->code_cap, e->mrg_code_cap);
+  rc = ingest();
+  std::swap(e->d_code, e->d_mrg_code);
+  std::swap(e->code_cap, e->mrg_code_cap);
+  e->last_batch_n = last_n;
+  return rc;
 }
 
 }  // namespace
@@ -1245,6 +1448,7 @@ int mm_destroy(mm_engine* e) {
   cudaFree(e->d_in_handle); cudaFree(e->d_rej_idx); cudaFree(e->d_rej_code);
   cudaFree(e->d_qstat); cudaFree(e->d_exp_id); cudaFree(e->d_exp_seq);
   cudaFree(e->d_img); cudaFree(e->d_img_tile); cudaFree(e->d_img_part); cudaFree(e->d_img_act);
+  cudaFree(e->d_sel); cudaFree(e->d_mrg_src); cudaFree(e->d_mrg_code); cudaFree(e->d_mrg_seen);
   if (e->h_ctr) cudaFreeHost(e->h_ctr);
   if (e->h_small) cudaFreeHost(e->h_small);
   for (auto& ev : e->ev)
@@ -1702,7 +1906,27 @@ int mm_export(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes) {
   *n_bytes = 0;
   std::lock_guard<std::mutex> lk(e->mu);
   CK(cudaSetDevice(e->device));
-  const int rc = export_image(e, buf, cap, n_bytes);
+  const int rc = export_image(e, buf, cap, n_bytes, nullptr);
+  free_img_scratch(e);
+  return rc;
+}
+
+int mm_export_queues(mm_engine* e, const uint8_t* queues, void* buf, uint64_t cap, uint64_t* n_bytes) {
+  if (!e || !queues || !n_bytes || (cap && !buf)) return MM_E_ARG;
+  *n_bytes = 0;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  const int rc = export_image(e, buf, cap, n_bytes, queues);
+  free_img_scratch(e);
+  return rc;
+}
+
+int mm_merge(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t cap, uint32_t* rejected, uint32_t* n_rejected) {
+  if (!e || !n_rejected || (n_bytes && !buf) || (cap && !rejected)) return MM_E_ARG;
+  *n_rejected = 0;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  const int rc = merge_image(e, static_cast<const uint8_t*>(buf), n_bytes, cap, rejected, n_rejected);
   free_img_scratch(e);
   return rc;
 }

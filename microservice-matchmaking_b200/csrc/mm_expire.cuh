@@ -6,6 +6,8 @@
 // take contiguous runs of the virtual tile sequence the tick uses (geo_build over the partition fills), as
 // k_queue_stats does, so the grid never covers chunks that are not in use.  The same kernel without `commit` only
 // counts: the host runs it first when the caller's output might be too small, so that a refused call changes nothing.
+// mm_export_queues releases the players it exports with this kernel too: a partition selection, max_wait = 0 and no
+// id output.
 #pragma once
 
 #include "mm_active.cuh"
@@ -29,6 +31,7 @@ struct ExpireArgs {
   uint64_t* out_id;                // one of out_id / out_handle receives the expired ids (unordered)
   uint32_t* out_handle;
   uint32_t* out_seq;               // may be null
+  const uint8_t* sel;              // [n_segs] or null: only the partitions with a non-zero byte (mm_export_queues)
   uint32_t* ctr;                   // [0] expired (the output cursor)  [1] active-set entries erased; zeroed by the host
 };
 
@@ -48,7 +51,7 @@ __global__ void __launch_bounds__(BLOCK) k_expire(const ExpireArgs a) {
     const size_t base = (size_t)d.phys * kTile + o;
     uint2 m2 = make_uint2(0, 0);
     uint32_t hit = 0;  // bit j: slot base + j expires
-    if (o < d.nvalid) {
+    if (o < d.nvalid && (!a.sel || a.sel[d.seg])) {
       m2 = __ldcs(reinterpret_cast<const uint2*>(a.pool.mode + base));
       const uint4 t0 = __ldcs(reinterpret_cast<const uint4*>(a.pool.ts + base));
       const uint4 t1 = __ldcs(reinterpret_cast<const uint4*>(a.pool.ts + base) + 1);
@@ -85,7 +88,7 @@ __global__ void __launch_bounds__(BLOCK) k_expire(const ExpireArgs a) {
       const uint32_t slot = (uint32_t)(base + j);
       const uint64_t pid = a.pool.id[slot];
       if (a.out_id) a.out_id[q] = pid;
-      else a.out_handle[q] = (uint32_t)pid;
+      else if (a.out_handle) a.out_handle[q] = (uint32_t)pid;
       if (a.out_seq) a.out_seq[q] = a.pool.seq[slot];
       ++q;
       pool_mark_dead(a.pool, a.meta, slot, a.dead_bin, a.bin_seg, a.seg_bin_lo);

@@ -13,6 +13,9 @@
 // into the active set (duplicate check) with the "not queued" value 0 — no generation is 0, so the entry never
 // matches a slot — and k_restamp then points the queued players' entries at their slots.  A failed check sets a bit
 // of one error word; the host then clears the engine.
+//
+// Queue move (mm_export_queues / mm_merge): the export passes with a partition selection; the merge kernels at the
+// end of this file check a queue image and turn it into one ingest batch for a running engine.
 #pragma once
 
 #include "mm_active.cuh"
@@ -45,6 +48,7 @@ struct ImgExportArgs {
   uint32_t n_segs;
   uint32_t* tile_cnt;  // [virtual tiles] pass 1: live slots of the tile; pass 2: the tile's first output index
   uint32_t* part_cnt;  // [n_segs] pass 1: live slots of the partition (zeroed by the host)
+  const uint8_t* sel;  // [n_segs] or null: only the partitions with a non-zero byte (mm_export_queues)
   ImgCols out;         // pass 2
 };
 
@@ -63,8 +67,8 @@ __global__ void __launch_bounds__(BLOCK) k_img_tiles(const ImgExportArgs a) {
   for (uint32_t s = s0; s < s1; ++s) {
     const TileDesc d = geo_tile(geo, a.meta, s);
     const size_t base = (size_t)d.phys * kTile + o;
-    uint32_t live = 0;  // bit j: slot base + j holds a live player
-    if (o < d.nvalid) {
+    uint32_t live = 0;  // bit j: slot base + j holds a live player of a selected partition
+    if (o < d.nvalid && (!a.sel || a.sel[d.seg])) {
       const uint2 m2 = __ldcs(reinterpret_cast<const uint2*>(a.pool.mode + base));
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
@@ -230,6 +234,105 @@ __global__ void k_img_insert(const void* ids, uint32_t id_bytes, uint32_t n, uin
     }
     if (!placed) atomicOr(err, kImgFull);
   }
+}
+
+// ---- mm_merge: a queue image (mm_export_queues) into a running engine, through the ingest ----------------------------
+// k_mrg_order checks every image player (as k_img_load) and writes the ingest batch: the players of each (mode, group)
+// queue in the source's enqueue order.  A queue's partitions are consecutive in the image and each is sorted by
+// sequence number, so a player's position in its queue is its index in its partition plus, for every other partition
+// of the queue, the number of that partition's players enqueued before it (a binary search; equal numbers from a
+// crafted image are ordered by partition, so the positions stay a permutation).  src[pos] = the image index.
+struct MrgOrderArgs {
+  ImgCols in;
+  uint32_t n, n_segs;
+  const uint32_t* part_off;   // [n_segs + 1] first image index of the partition
+  const uint16_t* part_cut;   // [n_segs] partition -> (mode, group) queue
+  const uint32_t* cut_lp_lo;  // [n_cut + 1] first partition of the queue
+  BinMap bm;
+  const uint8_t* grp_lut;
+  const uint16_t* bin_seg;
+  uint32_t n_modes, seq_next;
+  uint64_t id_limit;
+  uint64_t* out_id;  // the ingest batch columns
+  int32_t* out_rating;
+  uint8_t* out_mode;
+  uint32_t* out_ts;
+  uint32_t* src;
+  uint32_t* err;
+};
+
+__global__ void __launch_bounds__(256) k_mrg_order(const MrgOrderArgs a) {
+  __shared__ uint32_t s_off[kMaxSegs + 1];
+  for (uint32_t p = threadIdx.x; p <= a.n_segs; p += blockDim.x) s_off[p] = a.part_off[p];
+  __syncthreads();
+  const int32_t hi = a.bm.key_lo + (int32_t)a.bm.KR - 1;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += gridDim.x * blockDim.x) {
+    uint32_t lo = 0, e = a.n_segs;  // the last partition whose first index is <= i (empty ones share it)
+    while (e - lo > 1) { const uint32_t mid = (lo + e) >> 1; if (s_off[mid] <= i) lo = mid; else e = mid; }
+    const uint32_t p = lo;
+    const uint64_t pid = img_id(a.in, i);
+    const uint32_t md = a.in.mode[i];
+    const int32_t rt = a.in.rating[i];
+    const uint32_t u = a.in.seq[i] - a.seq_next;
+    uint32_t bad = 0;
+    if (pid >= a.id_limit) bad |= kImgBadId;
+    if (md >= a.n_modes) {
+      bad |= kImgBadMode;
+    } else {
+      const int32_t r = rt < a.bm.key_lo ? a.bm.key_lo : (rt > hi ? hi : rt);
+      if (a.grp_lut[r - a.bm.key_lo] == 0xFF || a.bin_seg[bin_of(a.bm, a.bm.lut, rt, md)] != p) bad |= kImgBadRating;
+    }
+    if (u == 0 || (i + 1 < s_off[p + 1] && a.in.seq[i + 1] - a.seq_next <= u)) bad |= kImgBadSeq;
+    if (bad) { atomicOr(a.err, bad); continue; }
+    const uint32_t c = a.part_cut[p], q0 = a.cut_lp_lo[c], q1 = a.cut_lp_lo[c + 1];
+    uint32_t pos = s_off[q0] + (i - s_off[p]);
+    for (uint32_t q = q0; q < q1; ++q) {
+      if (q == p) continue;
+      uint32_t l = s_off[q], r = s_off[q + 1];  // players of q enqueued before i: u' < u (u' <= u for q < p)
+      while (l < r) {
+        const uint32_t mid = (l + r) >> 1;
+        const uint32_t v = a.in.seq[mid] - a.seq_next;
+        if (v < u || (q < p && v == u)) l = mid + 1; else r = mid;
+      }
+      pos += l - s_off[q];
+    }
+    a.out_id[pos] = pid; a.out_rating[pos] = rt; a.out_mode[pos] = (uint8_t)md; a.out_ts[pos] = a.in.ts[i];
+    a.src[pos] = i;
+  }
+}
+
+// Only when the caller's reject list or a capacity might be too small: the exact number of batch entries the ingest
+// will not queue — ids already in the active set, and every copy of an id after the first (one copy wins the insert
+// into `seen`, an empty scratch set of 2^k keys, at most half full).
+__global__ void k_mrg_dups(const uint64_t* __restrict__ id, uint32_t n, ActiveView act, unsigned long long* seen,
+                           uint64_t seen_mask, uint32_t* __restrict__ count) {
+  uint32_t dup = 0;
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    const uint64_t pid = id[i];
+    const uint64_t h = act_find(act, pid);
+    if (h != ~0ull && (!act.dcap || *act.val(h) != kFreeVal)) { ++dup; continue; }
+    for (uint64_t s = hash64(pid) & seen_mask;; s = (s + 1) & seen_mask) {
+      const unsigned long long k = atomicCAS(&seen[s], kEmptyKey, (unsigned long long)pid);
+      if (k == kEmptyKey) break;
+      if (k == pid) { ++dup; break; }
+    }
+  }
+  dup = __reduce_add_sync(0xFFFFFFFFu, dup);
+  if ((threadIdx.x & 31) == 0 && dup) atomicAdd(count, dup);
+}
+
+// the batch entries the ingest did not queue -> their image indices (unordered)
+__global__ void k_mrg_rejects(uint32_t n, const uint8_t* __restrict__ code, const uint32_t* __restrict__ src,
+                              uint32_t* __restrict__ out, uint32_t* __restrict__ count) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  const bool rej = i < n && code[i] != 1;
+  const uint32_t b = __ballot_sync(0xFFFFFFFFu, rej);
+  if (!b) return;
+  const uint32_t lane = threadIdx.x & 31;
+  uint32_t base = 0;
+  if (lane == 0) base = atomicAdd(count, (uint32_t)__popc(b));
+  base = __shfl_sync(0xFFFFFFFFu, base, 0);
+  if (rej) out[base + __popc(b & ((1u << lane) - 1u))] = src[i];
 }
 
 }  // namespace mm

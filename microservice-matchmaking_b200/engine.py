@@ -396,6 +396,31 @@ class Engine:
                                    else buf, np.uint8)
         self._check(self.lib.mm_import(self.h, _p(buf), len(buf)), "mm_import")
 
+    def export_queues(self, mask):
+        """Release whole (mode, group) queues into a queue image (mm_export_queues) -> uint8 array.  mask: bool per
+        queue in queue_stats() record order (mode * n_groups + group), or [n_modes][n_groups].  The exported players
+        leave this engine as if remove() had been called with their ids; matched-not-removed ids stay here."""
+        mask = np.ascontiguousarray(np.asarray(mask, bool).reshape(-1), np.uint8)
+        assert len(mask) == self.cfg.n_modes * self.cfg.n_groups
+        bound = abi.image_offsets(abi.MM_MAX_GROUPS * abi.MM_MAX_MODES, self.pool_size(), 0, 8)[-1]
+        buf = np.empty(bound, np.uint8)
+        n = C.c_uint64(0)
+        self._check(self.lib.mm_export_queues(self.h, _p(mask), _p(buf), bound, C.byref(n)), "mm_export_queues")
+        return buf[:n.value]
+
+    def merge_queues(self, buf):
+        """Load a queue image (export_queues) into this running engine (mm_merge) -> image indices (u32, ascending)
+        of the players that were not queued: ids already active here, and later copies of an id."""
+        buf = np.ascontiguousarray(np.frombuffer(buf, np.uint8) if isinstance(buf, (bytes, bytearray, memoryview))
+                                   else buf, np.uint8)
+        hs = C.sizeof(abi.ImageHeader)
+        n = abi.ImageHeader.from_buffer_copy(buf[:hs].tobytes()).n_players if len(buf) >= hs else 0
+        n = min(n, len(buf))  # a player takes more than a byte: a corrupt count must not size the reject list
+        rej = np.empty(max(n, 1), np.uint32)
+        k = C.c_uint32(0)
+        self._check(self.lib.mm_merge(self.h, _p(buf), len(buf), n, _p(rej), C.byref(k)), "mm_merge")
+        return rej[:k.value]
+
     def snapshot(self):
         self._check(self.lib.mm_snapshot(self.h), "mm_snapshot")
 

@@ -350,6 +350,94 @@ class SearchPool:
         pool.enqueued_at = {int(h): at - age for h, age in state["enqueued_at"]}
         return pool
 
+    # -- moving queues to another running pool -----------------------------------------------------
+    MOVE_MAGIC = b"MMMOVE01"
+
+    def move_out(self, group_names, mode_names=None):
+        """Release the queues of these groups (all modes, or only `mode_names`) to another running pool: -> bytes for
+        move_in().  The staged deliveries are ingested first.  The engine releases the players in the same call that
+        writes their image (Engine.export_queues), and this pool forgets their handles and documents.  Layout:
+        MOVE_MAGIC, u64 length of a JSON document (mode / group names, the pool clock and the wall time, and per moved
+        player in image order its id, document and age), the JSON, then the queue image.  Reroute the groups'
+        deliveries to the new owner before the call: a delivery staged after it stays here."""
+        self.flush()
+        if hasattr(self.engine, "results_wait"):
+            self.engine.results_wait()
+        G, M = len(self.group_names), len(self.mode_names)
+        mask = np.zeros((M, G), bool)
+        modes = range(M) if mode_names is None else [self.mode_names.index(m) for m in mode_names]
+        for g in group_names:
+            for m in modes:
+                mask[m, self.group_names.index(g)] = True
+        from .engine import read_image
+        image = np.ascontiguousarray(self.engine.export_queues(mask), np.uint8)
+        _h, cols = read_image(image)
+        t = self.clock()
+        moved = []
+        for h in cols["id"].tolist():
+            pid = self.handles.id_of[h]
+            at = self.enqueued_at.pop(h, None)
+            moved.append([pid, self.players.pop(h), None if at is None else t - at])
+            self.handles.release(pid)
+        state = {"mode_names": self.mode_names, "group_names": self.group_names, "players": moved,
+                 "now_ms": self.now_ms(), "wall": self.wall_clock()}
+        doc = json.dumps(state).encode()
+        return self.MOVE_MAGIC + len(doc).to_bytes(8, "little") + doc + image.tobytes()
+
+    def move_in(self, blob):
+        """Load what move_out() released into this pool: every moved player gets a handle of this pool (the image's id
+        column is rewritten), its enqueue stamp is shifted into this pool's clock (bridged by the wall time, as in
+        resume(), so waits and the timeout count the time in the old pool), the engine merges the image
+        (Engine.merge_queues), and the documents of players it rejects (already queued here) are dropped.  Staged
+        deliveries are ingested first.  -> players merged.  ValueError if the mode or group names differ, or if this
+        pool's handle range cannot hold the players."""
+        head = len(self.MOVE_MAGIC)
+        if bytes(blob[:head]) != self.MOVE_MAGIC:
+            raise ValueError("not a SearchPool queue move")
+        n = int.from_bytes(blob[head:head + 8], "little")
+        state = json.loads(bytes(blob[head + 8:head + 8 + n]))
+        if state["mode_names"] != self.mode_names or state["group_names"] != self.group_names:
+            raise ValueError("the queues were moved out of a pool with other mode or group names")
+        self.flush()
+        from .engine import read_image
+        image = np.frombuffer(bytes(blob[head + 8 + n:]), np.uint8).copy()
+        _h, cols = read_image(image)
+        players = state["players"]
+        handles, fresh = [], []
+        for pid, _doc, _age in players:
+            h, is_new = self.handles.acquire(pid)
+            if h is None:
+                for p in fresh:
+                    self.handles.release(p)
+                raise ValueError("this pool's handle range cannot hold the moved players")
+            handles.append(h)
+            fresh.append(pid if is_new else None)
+        fresh_ids = [p for p in fresh if p is not None]
+        cols["id"][:] = np.asarray(handles, cols["id"].dtype)
+        down = max(0.0, self.wall_clock() - state["wall"])
+        shift = (self.now_ms() - int(round(down * 1000.0)) - int(state["now_ms"])) & 0xFFFFFFFF
+        cols["enq_ts"][:] = (cols["enq_ts"].astype(np.uint64) + np.uint64(shift)).astype(np.uint32)
+        try:
+            rejected = set(self.engine.merge_queues(image).tolist())
+        except Exception:
+            for p in fresh_ids:
+                self.handles.release(p)
+            raise
+        t = self.clock() - down
+        merged = 0
+        for i, ((pid, doc, age), h, new) in enumerate(zip(players, handles, fresh)):
+            if i in rejected:  # already queued here: keep this pool's player, drop the moved document
+                if new is not None:
+                    self.handles.release(pid)
+                continue
+            self.players[h] = doc
+            if self.window and age is not None:
+                self.enqueued_at[h] = t - age
+            merged += 1
+        if self.window:  # oldest first: the window reads the first entry
+            self.enqueued_at = dict(sorted(self.enqueued_at.items(), key=lambda kv: kv[1]))
+        return merged
+
     def _teams_of(self, mode):
         return self.engine.cfg.modes[int(mode)].teams
 

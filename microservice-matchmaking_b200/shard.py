@@ -16,9 +16,48 @@ def owner_of_group(g, n_groups, world):
     return (np.asarray(g, np.int64) * world) // n_groups
 
 
-def groups_of_rank(rank, n_groups, world):
+def groups_of_rank(rank, n_groups, world, owners=None):
+    """owners: optional owner rank per group (balanced_owners); default floor(g * P / G)."""
     g = np.arange(n_groups)
-    return g[owner_of_group(g, n_groups, world) == rank]
+    own = owner_of_group(g, n_groups, world) if owners is None else np.asarray(owners, np.int64)
+    return g[own == rank]
+
+
+def balanced_owners(load, world):
+    """Contiguous owner ranks (non-decreasing in the group) that minimise the largest per-rank load; load[g] >= 0, e.g.
+    the queue depths of mm_queue_stats summed over the modes.  Among the optimal splits, every rank takes as many
+    groups as it can, lowest rank first (the lexicographically smallest owner array), so every rank computes the same
+    answer.  -> int64[G]"""
+    load = np.asarray(load, np.float64)
+    G = len(load)
+    if G == 0:
+        return np.zeros(0, np.int64)
+    if world < 1 or (load < 0).any():
+        raise ValueError("balanced_owners needs world >= 1 and loads >= 0")
+    pre = np.concatenate([[0.0], np.cumsum(load)])
+
+    def greedy(cap):  # every rank takes the longest run of groups that stays within cap; None if P ranks do not do
+        own = np.empty(G, np.int64)
+        r, start = 0, 0
+        for g in range(G):
+            if pre[g + 1] - pre[g] > cap:
+                return None
+            if pre[g + 1] - pre[start] > cap:
+                r, start = r + 1, g
+                if r >= world:
+                    return None
+            own[g] = r
+        return own
+
+    cands = np.unique((pre[None, :] - pre[:, None])[np.triu_indices(G + 1, 1)])  # every run's load: one is optimal
+    lo, hi = 0, len(cands) - 1
+    while lo < hi:
+        mid = (lo + hi) // 2
+        if greedy(cands[mid]) is None:
+            lo = mid + 1
+        else:
+            hi = mid
+    return greedy(cands[lo])
 
 
 def group_of_rating(cfg, rating):
@@ -33,10 +72,12 @@ def group_of_rating(cfg, rating):
     return grp
 
 
-def route(cfg, rating, world):
-    """-> owner rank of every player (-1: unroutable, no default group)."""
+def route(cfg, rating, world, owners=None):
+    """-> owner rank of every player (-1: unroutable, no default group).  owners: optional owner rank per group
+    (balanced_owners, or the `new` array of a move_queues); default floor(g * P / G)."""
     grp = group_of_rating(cfg, rating)
-    own = owner_of_group(np.maximum(grp, 0), cfg.n_groups, world)
+    g0 = np.maximum(grp, 0)
+    own = owner_of_group(g0, cfg.n_groups, world) if owners is None else np.asarray(owners, np.int64)[g0]
     return np.where(grp < 0, -1, own)
 
 
@@ -233,3 +274,102 @@ def boundary_pass(pkg, cfg, W, world, rank, engine, comm, make_engine=None, cach
     hdr = np.concatenate(lob_parts) if lob_parts else None
     members = np.concatenate(mem_parts) if mem_parts else np.zeros(0, np.uint64)
     return dict(hdr=hdr, member_ids=members, **stats)
+
+
+# ======================================================================================================================
+# Moving rating groups between ranks (mm_export_queues / mm_merge).  A group's queues, all modes, go from the rank that
+# owns it to another one while both keep running: scale out / in, or a rebalance by balanced_owners() when the
+# rating distribution leaves one rank with most of the pool.
+# ======================================================================================================================
+def _status(x):
+    return int(np.asarray(x).view(np.int64).reshape(-1)[0])
+
+
+def can_take(cfg, engine, g, n):
+    """Would a merge of n players of group g into `engine` pass mm_merge's checks?  No live player in any of the
+    group's queues, n more pool slots within the capacity (the slots in use count dead ones until the next tick), and
+    for a hashed active set n more entries within its 3/4 load.  Conservative: rejected ids would need no room."""
+    if int(engine.queue_stats(0)["n_waiting"].reshape(cfg.n_modes, cfg.n_groups)[:, g].sum()):
+        return False
+    if engine.pool_size() + n > engine.cfg.capacity:
+        return False
+    flags = int(engine.cfg.flags)
+    if not flags & 1 and not flags & 2:  # hashed active set (neither MM_F_NO_DEDUPE nor MM_F_DENSE_IDS): mm_create's size
+        want = engine.cfg.active_capacity or 2 * engine.cfg.capacity
+        h = 1024
+        while h * 3 < want * 4 + 64:
+            h <<= 1
+        if (engine.active_size() + n) * 4 > h * 3:
+            return False
+    return True
+
+
+def move_queues(pkg, cfg, old, new, rank, engine, comm):
+    """Move every group g with old[g] != new[g] from rank old[g] to rank new[g]; every rank of the job calls this with
+    the same arrays.  Moves run in ascending group order on every rank; each involves exactly two ranks, and every
+    message below is answered whatever fails, so blocking point-to-point calls can neither deadlock nor wait forever.
+    One move, all messages int64 arrays:
+
+      1. source -> target: [n], the group's live players here (mm_queue_stats), or [-1] if they cannot be counted;
+      2. target -> source: [0] if it can take them (can_take: no live player of the group, room in the pool and the
+         active set), else [1] — the source has released nothing yet, so a refusal here changes nothing;
+      3. source -> target: the queue image (Engine.export_queues: the players are released in the same call) as one
+         int64 array (an image is a multiple of 8 bytes and at least its 624-byte header), or [-1] if the export failed;
+      4. target -> source: [0] if Engine.merge_queues took it, else [1].
+
+    If step 4 fails anyway (a CUDA error, an active set that filled in between), the source merges the image back.
+    Should that fail too (the released players' dead slots still count in the source's pool until its next tick), the
+    image is kept in `stranded` instead of being lost: merge it into the source (Engine.merge_queues) after its next
+    tick.  -> dict(moved=[groups], failed=[groups], stranded={group: image}) as seen by this rank.
+
+    Routing is the caller's job: new deliveries of a moved group must go to its new owner (route(..., owners=new))
+    on every rank from the move on, and those of a failed move to the old one."""
+    old, new = np.asarray(old, np.int64), np.asarray(new, np.int64)
+    out = {"moved": [], "failed": [], "stranded": {}}
+    for g in range(cfg.n_groups):
+        src, dst = int(old[g]), int(new[g])
+        if src == dst or rank not in (src, dst):
+            continue
+        if rank == src:
+            try:
+                n = int(engine.queue_stats(0)["n_waiting"].reshape(cfg.n_modes, cfg.n_groups)[:, g].sum())
+            except Exception:
+                n = -1
+            comm.send(src, dst, (np.array([n], np.int64),))
+            (reply,) = comm.recv(dst, src)
+            ok = n >= 0 and _status(reply) == 0
+            if ok:
+                mask = np.zeros((cfg.n_modes, cfg.n_groups), bool)
+                mask[:, g] = True
+                try:  # a refused export (e.g. a staged packed batch) changes nothing; the target still gets a message
+                    img = np.ascontiguousarray(engine.export_queues(mask), np.uint8)
+                except Exception:
+                    img = None
+                comm.send(src, dst, (img.view(np.int64) if img is not None else np.array([-1], np.int64),))
+                (status,) = comm.recv(dst, src)
+                ok = img is not None and _status(status) == 0
+                if img is not None and not ok:  # the group's queues hold only dead slots here now: the image goes back
+                    try:
+                        engine.merge_queues(img)
+                    except pkg.EngineError:
+                        out["stranded"][g] = img
+        else:
+            (prop,) = comm.recv(src, dst)
+            n = _status(prop)
+            try:
+                ok = n >= 0 and can_take(cfg, engine, g, n)
+            except Exception:
+                ok = False
+            comm.send(dst, src, (np.array([0 if ok else 1], np.int64),))
+            if ok:
+                (arr,) = comm.recv(src, dst)
+                arr = np.ascontiguousarray(arr)
+                ok = len(arr) > 1
+                if ok:
+                    try:
+                        engine.merge_queues(arr.view(np.uint8))
+                    except Exception:
+                        ok = False
+                comm.send(dst, src, (np.array([0 if ok else 1], np.int64),))
+        out["moved" if ok else "failed"].append(g)
+    return out
