@@ -10,11 +10,13 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <mutex>
 #include <new>
+#include <utility>
 #include <vector>
 
 #include "mm_expire.cuh"
@@ -26,14 +28,65 @@ using namespace mm;
 
 namespace {
 
+// A device array the engine owns: n elements at p (one cudaMalloc), freed by reset() and the destructor.  reserve()
+// grows it by free-then-allocate, so the old contents are lost; after a failed allocation the array is empty.  Kernels
+// take the raw pointer (the conversion below).
+template <class T>
+struct DevArray {
+  T* p = nullptr;
+  size_t n = 0;
+
+  DevArray() = default;
+  DevArray(const DevArray&) = delete;
+  DevArray& operator=(const DevArray&) = delete;
+  DevArray(DevArray&& o) noexcept : p(std::exchange(o.p, nullptr)), n(std::exchange(o.n, 0)) {}
+  DevArray& operator=(DevArray&& o) noexcept {
+    if (this != &o) { reset(); p = std::exchange(o.p, nullptr); n = std::exchange(o.n, 0); }
+    return *this;
+  }
+  ~DevArray() { reset(); }
+
+  cudaError_t reserve(size_t want) {
+    if (want <= n) return cudaSuccess;
+    reset();
+    const cudaError_t err = cudaMalloc(reinterpret_cast<void**>(&p), want * sizeof(T));
+    if (err != cudaSuccess) { p = nullptr; return err; }
+    n = want;
+    return cudaSuccess;
+  }
+  void reset() {
+    if (p) cudaFree(p);
+    p = nullptr; n = 0;
+  }
+  operator T*() const { return p; }
+  T* operator->() const { return p; }
+};
+
 struct Pool {
-  PoolView v{};
+  PoolView v{};  // the arrays below, as the kernels take them
   PoolMeta m{};
   uint32_t n = 0;  // host mirror of the sum of the partition fills (dead players included)
+  DevArray<uint64_t> id;
+  DevArray<int32_t> rating;
+  DevArray<uint8_t> mode, tsize;
+  DevArray<uint32_t> ts, seq;
+  DevArray<uint16_t> bin;
+  DevArray<uint32_t> fill, chunk_tab, bump, tot, chist;
 };
 
 struct Table {
-  unsigned long long* kv = nullptr;  // hashed: hcap x {key, value}; direct: dcap values
+  DevArray<unsigned long long> kv;  // hashed: hcap x {key, value}; direct: dcap values
+};
+
+// The counters the kernels of one call write, in device memory with a pinned host mirror.  The fields of one line are
+// zeroed together before their kernels run.
+struct Counters {
+  uint32_t accepted, pool_full, winners;  // ingest: queued; rolled back because the pool is full; running winner total
+  uint32_t removed;                       // mm_remove / mm_take
+  uint32_t rejects;                       // mm_enqueue_rejects / mm_merge: batch entries not queued, compacted
+  uint32_t expired, erased;               // k_expire: players expired or released; active-set entries erased
+  uint32_t img_players, img_active;       // export: live players; active ids outside the pool
+  uint32_t img_err, mrg_dups;             // mm_import / mm_merge: kImg* error bits; batch entries that will not queue
 };
 
 }  // namespace
@@ -60,14 +113,14 @@ struct mm_engine {
   uint32_t KR = 0, stride = 0, K = 0, Kp = 0;
   uint32_t n_segs = 0;  // layout partitions (see build_tables)
   uint32_t n_cut = 0;   // (mode, group) cut segments
-  uint16_t* d_part_cut = nullptr;   // [n_segs] partition -> cut segment
-  uint32_t* d_cut_lp_lo = nullptr;  // [n_cut + 1] first partition of the cut segment
-  uint16_t* d_lut = nullptr;
-  uint8_t* d_grp_lut = nullptr;
-  uint8_t* d_mode_tsize = nullptr;
-  uint32_t* d_seg_bin_lo = nullptr;
-  uint32_t* d_seg_L = nullptr;
-  uint16_t* d_bin_seg = nullptr;  // [Kp] bin -> (mode, group) segment
+  DevArray<uint16_t> d_part_cut;   // [n_segs] partition -> cut segment
+  DevArray<uint32_t> d_cut_lp_lo;  // [n_cut + 1] first partition of the cut segment
+  DevArray<uint16_t> d_lut;
+  DevArray<uint8_t> d_grp_lut;
+  DevArray<uint8_t> d_mode_tsize;
+  DevArray<uint32_t> d_seg_bin_lo;
+  DevArray<uint32_t> d_seg_L;
+  DevArray<uint16_t> d_bin_seg;  // [Kp] bin -> (mode, group) segment
   uint32_t min_L = 1;
   uint32_t max_nb = 1;  // most sort keys any one (mode, group) partition has
 
@@ -100,50 +153,47 @@ struct mm_engine {
   int fused_ok = 0;  // k_tick<512> can be launched cooperatively with R CTAs
   int tick_impl = 1; // 1 = one fused cooperative launch when possible, 0 = four launches
   size_t tick_smem = 0;
-  uint32_t *d_M = nullptr, *d_P = nullptr;  // row histograms, their column prefixes (only for many-row partitions)
-  uint32_t *d_outbase = nullptr, *d_binlim = nullptr;
-  uint16_t* d_bin_key = nullptr;
+  DevArray<uint32_t> d_M, d_P;  // row histograms, their column prefixes (only for many-row partitions)
+  DevArray<uint32_t> d_outbase, d_binlim;
+  DevArray<uint16_t> d_bin_key;
   int32_t max_spread = -1;  // < 0: policy S0 (reference behaviour); >= 0: policy S1 (extension)
-  SegInfo* d_seg = nullptr;
-  uint32_t* d_left_bits = nullptr;  // one bit per virtual pool position: stays queued after the tick
-  uint64_t* d_members = nullptr;
-  uint32_t* d_members32 = nullptr;  // mm_tick_packed: member handles narrowed for the host copy
+  DevArray<SegInfo> d_seg;
+  DevArray<uint32_t> d_left_bits;  // one bit per virtual pool position: stays queued after the tick
+  DevArray<uint64_t> d_members;
+  DevArray<uint32_t> d_members32;  // mm_tick_packed: member handles narrowed for the host copy
   // async_results + mm_tick_packed: headers and narrowed handles alternate between two buffer sets, so the next
   // tick's kernels need not wait for this tick's host copies
-  uint32_t* d_members32_alt = nullptr;
-  mm_lobby_hdr* d_hdr_alt = nullptr;
-  uint32_t* d_src_idx = nullptr;
-  mm_lobby_hdr* d_hdr = nullptr;
-  uint32_t* d_emit_seq = nullptr;
+  DevArray<uint32_t> d_members32_alt;
+  DevArray<mm_lobby_hdr> d_hdr_alt;
+  DevArray<uint32_t> d_src_idx;
+  DevArray<mm_lobby_hdr> d_hdr;
+  DevArray<uint32_t> d_emit_seq;
   uint32_t max_lobbies = 0;
-  TickCtr* d_ctr2 = nullptr;  // two counter blocks, used alternately (the fused kernel re-arms the other one)
-  TickCtr* d_ctr = nullptr;   // the block of the current / last tick
+  DevArray<TickCtr> d_ctr2;  // two counter blocks, used alternately (the fused kernel re-arms the other one)
+  TickCtr* d_ctr = nullptr;  // the block of the current / last tick
   int ctr_idx = 0;
   TickCtr* h_ctr = nullptr;  // pinned
 
   // enqueue scratch (grown on demand)
-  uint32_t enq_cap = 0;
-  uint64_t *d_in_id = nullptr, *d_hslot = nullptr;
-  int32_t* d_in_rating = nullptr;
-  uint8_t *d_in_mode = nullptr, *d_lookup = nullptr;
-  uint16_t *d_part = nullptr, *d_in_key = nullptr;
-  uint32_t *d_in_ts = nullptr, *d_in_handle = nullptr, *d_blocksum = nullptr, *d_blockhist = nullptr;
-  // [0] accepted  [1] rejected: pool full  [2] removed  [3] running winner total (cut)  [4] rejects
-  // [8] expired  [9] active-set entries erased by mm_expire
-  uint32_t* d_small = nullptr;
-  uint32_t* h_small = nullptr;  // pinned
+  DevArray<uint64_t> d_in_id, d_hslot;
+  DevArray<int32_t> d_in_rating;
+  DevArray<uint8_t> d_in_mode, d_lookup;
+  DevArray<uint16_t> d_part, d_in_key;
+  DevArray<uint32_t> d_in_ts, d_in_handle, d_blocksum, d_blockhist;
+  DevArray<Counters> d_cnt;
+  Counters* h_cnt = nullptr;  // pinned
   // codes of the last ingest batch: grown only by an ingest batch that passed its capacity check, written only by
   // ingest, so mm_enqueue_rejects reads them whatever ran since
-  uint8_t* d_code = nullptr;
-  uint32_t code_cap = 0;
+  DevArray<uint8_t> d_code;
   uint32_t last_batch_n = 0;    // entries of the last ingest batch (their codes are still in d_code)
-  uint32_t* d_rej_idx = nullptr; uint8_t* d_rej_code = nullptr; uint32_t rej_cap = 0;
+  DevArray<uint32_t> d_rej_idx;
+  DevArray<uint8_t> d_rej_code;
 
   // mm_enqueue_packed_begin / _end: two staging slots for packed batches whose upload is in flight (FIFO)
   struct Stage {
-    uint32_t *handle = nullptr, *ts = nullptr;
-    uint16_t* key = nullptr;
-    uint32_t cap = 0, n = 0;
+    DevArray<uint32_t> handle, ts;
+    DevArray<uint16_t> key;
+    uint32_t n = 0;
     bool has_ts = false;
     cudaEvent_t ready = nullptr;  // recorded on the copy stream behind the slot's last copy
   } stage[2];
@@ -158,34 +208,29 @@ struct mm_engine {
   bool match_valid = false;  // the last tick completed and nothing since has invalidated its section
   uint32_t tick_now = 0;     // `now` of the tick in progress / the last tick (mod 2^32)
   uint32_t match_n = 0;      // players resident when that tick started: bounds its tile count
-  uint32_t* d_qstat = nullptr;  // [n_cut] records
+  DevArray<uint32_t> d_qstat;  // [n_cut] records
 
   // mm_expire output (grown on demand to the largest output a call could write; not d_members / d_hdr, which
   // mm_results_device hands out until the next tick)
-  uint64_t* d_exp_id = nullptr;  // ids, or 32-bit handles in its first half
-  uint32_t* d_exp_seq = nullptr;
-  uint32_t exp_cap = 0;
+  DevArray<uint64_t> d_exp_id;  // ids, or 32-bit handles in its first half
+  DevArray<uint32_t> d_exp_seq;
 
   // mm_export / mm_import.  The image-sized buffers (d_img, d_img_act: about the image's size, 210 MB at 10 M queued
   // players) are freed at the end of every call, so a hand-over leaves no such footprint on either engine; the small
   // per-tile / per-partition arrays are kept.
   bool fresh = true;  // nothing ever enqueued, imported or restored: mm_import may load an image
-  uint8_t* d_img = nullptr;  // the image from section 2 (id) on, as it lies in the host buffer
-  size_t img_cap = 0;
-  uint32_t* d_img_tile = nullptr;  // export: live slots per virtual tile -> offsets
-  uint32_t img_tile_cap = 0;
-  uint32_t* d_img_part = nullptr;  // export: [n_segs] live slots per partition; import: part_off[n_segs+1] | slot_base[n_segs]
-  void* d_img_act = nullptr;       // export: the active section
-  uint64_t img_act_cap = 0;        // bytes
+  DevArray<uint8_t> d_img;  // the image from section 2 (id) on, as it lies in the host buffer
+  DevArray<uint32_t> d_img_tile;  // export: live slots per virtual tile -> offsets
+  DevArray<uint32_t> d_img_part;  // export: [n_segs] live slots per partition; import: part_off[n_segs+1] | slot_base[n_segs]
+  DevArray<uint8_t> d_img_act;    // export: the active section
 
   // mm_export_queues / mm_merge.  Like the image buffers, the batch-sized merge scratch is freed by every call.
   std::vector<uint16_t> h_part_cut;   // host copies of d_part_cut / d_cut_lp_lo
   std::vector<uint32_t> h_cut_lp_lo;
-  uint8_t* d_sel = nullptr;           // [n_segs] selected partitions
-  uint32_t* d_mrg_src = nullptr;      // merge batch index -> image index
-  uint8_t* d_mrg_code = nullptr;      // the merge batch's ingest codes (d_code keeps the last mm_enqueue* batch's)
-  uint32_t mrg_code_cap = 0;
-  unsigned long long* d_mrg_seen = nullptr;  // duplicate count: scratch id set
+  DevArray<uint8_t> d_sel;            // [n_segs] selected partitions
+  DevArray<uint32_t> d_mrg_src;       // merge batch index -> image index
+  DevArray<uint8_t> d_mrg_code;       // the merge batch's ingest codes (d_code keeps the last mm_enqueue* batch's)
+  DevArray<unsigned long long> d_mrg_seen;  // duplicate count: scratch id set
 };
 
 namespace {
@@ -202,6 +247,22 @@ int fail(mm_engine* e, cudaError_t err, const char* what) {
     if (_err != cudaSuccess) return fail(e, _err, #call); \
   } while (0)
 
+// mm_last_error <- the formatted message; returns `code`
+__attribute__((format(printf, 3, 4))) int set_err(mm_engine* e, int code, const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  std::vsnprintf(e->last_err, sizeof(e->last_err), fmt, ap);
+  va_end(ap);
+  return code;
+}
+
+// the counters to their host mirror, once the engine stream's work is done
+int read_counters(mm_engine* e) {
+  CK(cudaMemcpyAsync(e->h_cnt, e->d_cnt, sizeof(Counters), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
 // Allow a kernel the device's whole opt-in shared memory (minus its static part).  Function attributes are
 // process-global: an engine with a small key domain must never lower the limit another engine relies on.
 template <class F>
@@ -217,35 +278,30 @@ size_t pool_slots(const mm_engine* e) { return (size_t)e->n_chunks * kTile; }
 
 int alloc_pool(mm_engine* e, Pool& p) {
   const size_t c = pool_slots(e);
-  CK(cudaMalloc(&p.v.id, c * 8));
-  CK(cudaMalloc(&p.v.rating, c * 4));
-  CK(cudaMalloc(&p.v.mode, c));
-  CK(cudaMalloc(&p.v.tsize, c));
-  CK(cudaMalloc(&p.v.ts, c * 4));
-  CK(cudaMalloc(&p.v.bin, c * 2));
-  CK(cudaMalloc(&p.v.seq, c * 4));
-  p.m.max_ch = e->n_chunks;
-  CK(cudaMalloc(&p.m.fill, (size_t)e->n_segs * 4));
-  CK(cudaMalloc(&p.m.chunk_tab, (size_t)e->n_segs * e->n_chunks * 4));
-  CK(cudaMalloc(&p.m.bump, 4));
-  CK(cudaMalloc(&p.m.tot, ((size_t)e->Kp + 1) * 4));
-  p.m.chist = nullptr;
+  CK(p.id.reserve(c));
+  CK(p.rating.reserve(c));
+  CK(p.mode.reserve(c));
+  CK(p.tsize.reserve(c));
+  CK(p.ts.reserve(c));
+  CK(p.bin.reserve(c));
+  CK(p.seq.reserve(c));
+  CK(p.fill.reserve(e->n_segs));
+  CK(p.chunk_tab.reserve((size_t)e->n_segs * e->n_chunks));
+  CK(p.bump.reserve(1));
+  CK(p.tot.reserve((size_t)e->Kp + 1));
   if (e->max_nb <= kFastBins) {  // per-chunk key histograms: the tick skips its counting pass over the pool
-    CK(cudaMalloc(&p.m.chist, (size_t)e->n_chunks * kChunkHist * 4));
-    CK(cudaMemset(p.m.chist, 0, (size_t)e->n_chunks * kChunkHist * 4));
+    CK(p.chist.reserve((size_t)e->n_chunks * kChunkHist));
+    CK(cudaMemset(p.chist, 0, (size_t)e->n_chunks * kChunkHist * 4));
   }
-  CK(cudaMemset(p.m.tot, 0, ((size_t)e->Kp + 1) * 4));
-  CK(cudaMemset(p.m.fill, 0, (size_t)e->n_segs * 4));
-  CK(cudaMemset(p.m.bump, 0, 4));
+  CK(cudaMemset(p.tot, 0, ((size_t)e->Kp + 1) * 4));
+  CK(cudaMemset(p.fill, 0, (size_t)e->n_segs * 4));
+  CK(cudaMemset(p.bump, 0, 4));
   // chunks are read whole by the TMA tiles: keep the bin column defined (and "dead") past the fills
-  CK(cudaMemset(p.v.bin, 0xFF, c * 2));
+  CK(cudaMemset(p.bin, 0xFF, c * 2));
+  p.v = PoolView{p.id, p.rating, p.mode, p.tsize, p.ts, p.bin, p.seq};
+  p.m = PoolMeta{p.fill, p.chunk_tab, p.bump, p.tot, p.chist, e->n_chunks};
   p.n = 0;
   return MM_OK;
-}
-void free_pool(Pool& p) {
-  cudaFree(p.v.id); cudaFree(p.v.rating); cudaFree(p.v.mode); cudaFree(p.v.tsize); cudaFree(p.v.ts); cudaFree(p.v.bin);
-  cudaFree(p.v.seq); cudaFree(p.m.fill); cudaFree(p.m.chunk_tab); cudaFree(p.m.bump); cudaFree(p.m.tot); cudaFree(p.m.chist);
-  p = Pool{};
 }
 int copy_pool(mm_engine* e, Pool& dst, const Pool& src) {
   const size_t c = pool_slots(e);
@@ -283,7 +339,7 @@ int clear_table(mm_engine* e, Table& t) {
     CK(cudaMemsetAsync(t.kv, 0xFF, e->hcap * 8, e->stream));  // FREE = all ones
     return MM_OK;
   }
-  k_fill_kv<<<1024, 256, 0, e->stream>>>(reinterpret_cast<ulonglong2*>(t.kv), e->hcap, kEmptyKey, kFreeVal);
+  k_fill_kv<<<1024, 256, 0, e->stream>>>(reinterpret_cast<ulonglong2*>(t.kv.p), e->hcap, kEmptyKey, kFreeVal);
   CK(cudaGetLastError());
   return MM_OK;
 }
@@ -322,6 +378,14 @@ uint32_t tail_layout(const mm_engine* e) {
 }
 size_t colscan_smem(const mm_engine* e) {
   return (size_t)std::max<uint32_t>(kColScratchWords, tail_words(e->Kp, tail_layout(e))) * 4;
+}
+
+// a host table to a device array of its size
+template <class T>
+int upload_table(mm_engine* e, DevArray<T>& d, const std::vector<T>& h) {
+  CK(d.reserve(h.size()));
+  CK(cudaMemcpy(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
+  return MM_OK;
 }
 
 // Build the key -> bin LUT and the (mode, group) segment table (see mm_kernels.cuh).
@@ -400,27 +464,16 @@ int build_tables(mm_engine* e) {
   std::vector<uint16_t> bin_seg(e->Kp, 0);
   for (uint32_t sgi = 0; sgi < e->n_segs; ++sgi)
     for (uint32_t b = seg_lo[sgi]; b < seg_lo[sgi + 1]; ++b) bin_seg[b] = (uint16_t)sgi;
-  CK(cudaMalloc(&e->d_part_cut, e->n_segs * 2));
-  CK(cudaMemcpy(e->d_part_cut, part_cut.data(), e->n_segs * 2, cudaMemcpyHostToDevice));
-  CK(cudaMalloc(&e->d_cut_lp_lo, (e->n_cut + 1) * 4));
-  CK(cudaMemcpy(e->d_cut_lp_lo, cut_lp_lo.data(), (e->n_cut + 1) * 4, cudaMemcpyHostToDevice));
   std::vector<uint16_t> bin_key(e->Kp, 0);
   if (!key_of.empty())
     for (uint32_t b = 0; b < e->K; ++b) bin_key[b] = key_of[b % e->stride];
-  CK(cudaMalloc(&e->d_bin_seg, e->Kp * 2));
-  CK(cudaMemcpy(e->d_bin_seg, bin_seg.data(), e->Kp * 2, cudaMemcpyHostToDevice));
-  CK(cudaMalloc(&e->d_bin_key, e->Kp * 2));
-  CK(cudaMemcpy(e->d_bin_key, bin_key.data(), e->Kp * 2, cudaMemcpyHostToDevice));
-  CK(cudaMalloc(&e->d_lut, e->KR * 2));
-  CK(cudaMalloc(&e->d_grp_lut, e->KR));
-  CK(cudaMalloc(&e->d_mode_tsize, MM_MAX_MODES));
-  CK(cudaMalloc(&e->d_seg_bin_lo, (e->n_segs + 1) * 4));
-  CK(cudaMalloc(&e->d_seg_L, e->n_segs * 4));
-  CK(cudaMemcpy(e->d_lut, lut.data(), e->KR * 2, cudaMemcpyHostToDevice));
-  CK(cudaMemcpy(e->d_grp_lut, grp.data(), e->KR, cudaMemcpyHostToDevice));
-  CK(cudaMemcpy(e->d_mode_tsize, tsz.data(), MM_MAX_MODES, cudaMemcpyHostToDevice));
-  CK(cudaMemcpy(e->d_seg_bin_lo, seg_lo.data(), (e->n_segs + 1) * 4, cudaMemcpyHostToDevice));
-  CK(cudaMemcpy(e->d_seg_L, seg_L.data(), e->n_segs * 4, cudaMemcpyHostToDevice));
+  int rc;
+  if ((rc = upload_table(e, e->d_part_cut, part_cut)) || (rc = upload_table(e, e->d_cut_lp_lo, cut_lp_lo)) ||
+      (rc = upload_table(e, e->d_bin_seg, bin_seg)) || (rc = upload_table(e, e->d_bin_key, bin_key)) ||
+      (rc = upload_table(e, e->d_lut, lut)) || (rc = upload_table(e, e->d_grp_lut, grp)) ||
+      (rc = upload_table(e, e->d_mode_tsize, tsz)) || (rc = upload_table(e, e->d_seg_bin_lo, seg_lo)) ||
+      (rc = upload_table(e, e->d_seg_L, seg_L)))
+    return rc;
   return MM_OK;
 }
 
@@ -435,30 +488,60 @@ int alloc_tick_scratch(mm_engine* e) {
   if (total > kMaxRows) total = kMaxRows;
   e->helpers = total >= 64 ? 4u : (total > 1 ? 1u : 0u);
   e->R = total - e->helpers;
-  if (e->d_M) { cudaFree(e->d_M); cudaFree(e->d_P); }
-  CK(cudaMalloc(&e->d_M, (size_t)(e->R + 1) * e->Kp * 4));
-  CK(cudaMalloc(&e->d_P, (size_t)(e->R + 1) * e->Kp * 4));
+  CK(e->d_M.reserve((size_t)(e->R + 1) * e->Kp));
+  CK(e->d_P.reserve((size_t)(e->R + 1) * e->Kp));
   return MM_OK;
 }
 
+// mm_create: both pool buffers, the active set, the tick's outputs and scratch, the counters
+int alloc_buffers(mm_engine* e) {
+  int rc;
+  if ((rc = alloc_pool(e, e->pool[0])) || (rc = alloc_pool(e, e->pool[1]))) return rc;
+  CK(e->d_left_bits.reserve(pool_slots(e) / 32 + 64));
+  if (e->use_active) {
+    const uint64_t want = e->cfg.active_capacity ? e->cfg.active_capacity : 2ull * e->cfg.capacity;
+    if (e->dense_ids) {
+      e->hcap = want;  // handles 0 .. active_capacity - 1
+      CK(e->tab[0].kv.reserve(e->hcap));
+    } else {
+      uint64_t h = 1024;
+      while (h * 3 < want * 4 + 64) h <<= 1;  // load factor <= 0.75 at active_capacity
+      e->hcap = h;
+      for (auto& t : e->tab) CK(t.kv.reserve(2 * h));  // {key, value} per slot
+    }
+    if ((rc = clear_table(e, e->tab[0]))) return rc;
+  }
+  const size_t cap = (size_t)e->capacity + 64;
+  e->max_lobbies = e->capacity / e->min_L + 1;
+  CK(e->d_outbase.reserve(e->Kp + 1));
+  CK(e->d_binlim.reserve(e->Kp + 1));
+  CK(e->d_seg.reserve(e->n_segs));
+  CK(e->d_members.reserve(cap));
+  CK(e->d_src_idx.reserve(cap));
+  CK(e->d_hdr.reserve(e->max_lobbies));
+  CK(e->d_emit_seq.reserve(e->max_lobbies));
+  CK(e->d_ctr2.reserve(2));
+  CK(e->d_cnt.reserve(1));
+  CK(e->d_blockhist.reserve((size_t)e->n_segs * (kEnqChunkDev / kIngestItems + 1)));
+  CK(cudaMemset(e->d_ctr2, 0, 2 * sizeof(TickCtr)));
+  e->d_ctr = e->d_ctr2;
+  CK(cudaMallocHost(&e->h_ctr, sizeof(TickCtr)));
+  CK(cudaMallocHost(&e->h_cnt, sizeof(Counters)));
+  return alloc_tick_scratch(e);
+}
+
 int ensure_enq_scratch(mm_engine* e, uint32_t n) {
-  if (n <= e->enq_cap) return MM_OK;
-  cudaFree(e->d_in_id); cudaFree(e->d_hslot); cudaFree(e->d_in_rating); cudaFree(e->d_in_mode);
-  cudaFree(e->d_lookup); cudaFree(e->d_in_ts); cudaFree(e->d_blocksum); cudaFree(e->d_part); cudaFree(e->d_in_key);
-  cudaFree(e->d_in_handle);
-  e->enq_cap = 0;
   const size_t c = (size_t)n + 64;
-  CK(cudaMalloc(&e->d_in_id, c * 8));
-  CK(cudaMalloc(&e->d_hslot, c * 8));
-  CK(cudaMalloc(&e->d_in_rating, c * 4));
-  CK(cudaMalloc(&e->d_in_mode, c));
-  CK(cudaMalloc(&e->d_lookup, c));
-  CK(cudaMalloc(&e->d_part, c * 2));
-  CK(cudaMalloc(&e->d_in_key, c * 2));
-  CK(cudaMalloc(&e->d_in_handle, c * 4));
-  CK(cudaMalloc(&e->d_in_ts, c * 4));
-  CK(cudaMalloc(&e->d_blocksum, (std::min<size_t>(c, kEnqChunkDev) / 256 + 2) * 4));
-  e->enq_cap = n;
+  CK(e->d_in_id.reserve(c));
+  CK(e->d_hslot.reserve(c));
+  CK(e->d_in_rating.reserve(c));
+  CK(e->d_in_mode.reserve(c));
+  CK(e->d_lookup.reserve(c));
+  CK(e->d_part.reserve(c));
+  CK(e->d_in_key.reserve(c));
+  CK(e->d_in_handle.reserve(c));
+  CK(e->d_in_ts.reserve(c));
+  CK(e->d_blocksum.reserve(std::min<size_t>(c, kEnqChunkDev) / 256 + 2));
   return MM_OK;
 }
 
@@ -484,20 +567,16 @@ int enq_prepare(mm_engine* e, uint32_t n, uint32_t n_new) {
   int rc = ensure_enq_scratch(e, n);
   if (rc) return rc;
   if (e->use_active && !e->dense_ids && (e->n_active + e->n_tomb + n_new) * 4 > e->hcap * 3) {
-    if ((e->n_active + n_new) * 4 > e->hcap * 3) {
-      std::snprintf(e->last_err, sizeof(e->last_err), "active set full: %llu ids resident, batch of %u, capacity %llu",
-                    (unsigned long long)e->n_active, n, (unsigned long long)(e->hcap * 3 / 4));
-      return MM_E_CAP;
-    }
+    if ((e->n_active + n_new) * 4 > e->hcap * 3)
+      return set_err(e, MM_E_CAP, "active set full: %llu ids resident, batch of %u, capacity %llu",
+                     (unsigned long long)e->n_active, n, (unsigned long long)(e->hcap * 3 / 4));
     if ((rc = rehash(e))) return rc;
   }
-  if (n > e->code_cap) {  // the batch is taken: the previous batch's codes may go
-    cudaFree(e->d_code);
-    e->d_code = nullptr; e->code_cap = 0; e->last_batch_n = 0;
-    CK(cudaMalloc(&e->d_code, (size_t)n + 64));
-    e->code_cap = n;
+  if ((size_t)n + 64 > e->d_code.n) {  // the batch is taken: the previous batch's codes may go
+    e->last_batch_n = 0;
+    CK(e->d_code.reserve((size_t)n + 64));
   }
-  CK(cudaMemsetAsync(e->d_small, 0, 16, e->stream));
+  CK(cudaMemsetAsync(&e->d_cnt->accepted, 0, 3 * 4, e->stream));  // accepted, pool_full, winners
   return MM_OK;
 }
 
@@ -512,12 +591,12 @@ int enq_chunk(mm_engine* e, uint32_t base, uint32_t cnt, const uint64_t* id, con
   if (may_overflow) {  // the batch might not fit: the winners past the pool capacity are rolled back (code 3)
     const uint32_t room = e->capacity > p.n ? e->capacity - p.n : 0u;
     k_enq_count<<<nb, 256, 0, e->stream>>>(base, cnt, av, e->d_hslot, e->d_code, e->d_blocksum);
-    k_scan_small<<<1, 1024, 0, e->stream>>>(nb, e->d_blocksum, e->d_small + 3);
-    k_enq_cut<<<nb, 256, 0, e->stream>>>(base, cnt, av, e->d_hslot, e->d_code, e->d_blocksum, room, e->d_small + 1);
+    k_scan_small<<<1, 1024, 0, e->stream>>>(nb, e->d_blocksum, &e->d_cnt->winners);
+    k_enq_cut<<<nb, 256, 0, e->stream>>>(base, cnt, av, e->d_hslot, e->d_code, e->d_blocksum, room, &e->d_cnt->pool_full);
     if (e->use_active) k_enq_promote<<<nb, 256, 0, e->stream>>>(base, cnt, e->d_hslot, e->d_code);
   }
   k_enq_route<<<nblk, 256, 0, e->stream>>>(base, cnt, av, e->d_hslot, e->d_code, e->d_part, e->n_segs, nblk, e->d_blockhist);
-  k_enq_alloc<<<1, 512, 0, e->stream>>>(e->n_segs, nblk, e->d_blockhist, p.m, e->d_small);
+  k_enq_alloc<<<1, 512, 0, e->stream>>>(e->n_segs, nblk, e->d_blockhist, p.m, &e->d_cnt->accepted);
   const size_t smem = (size_t)(2 * e->n_segs + 64) * 4 + (size_t)(((8 * (e->n_segs + 1) + 1) & ~1u) + 2 * kIngestItems) * 2;
   k_enq_append<<<nblk, 256, smem, e->stream>>>(base, cnt, id, rating, mode, ts, e->d_mode_tsize, av, e->d_hslot, e->d_code,
                                                e->d_part, e->n_segs, nblk, e->d_blockhist, p.v, p.m, e->gen, e->seq_next,
@@ -529,15 +608,32 @@ int enq_chunk(mm_engine* e, uint32_t base, uint32_t cnt, const uint64_t* id, con
 // counters of the finished batch -> host state
 int enq_finish(mm_engine* e, uint32_t n, uint8_t* accepted_dev, uint32_t* n_accepted) {
   Pool& p = e->pool[e->cur];
-  CK(cudaMemcpyAsync(e->h_small, e->d_small, 16, cudaMemcpyDeviceToHost, e->stream));
   if (accepted_dev) CK(cudaMemcpyAsync(accepted_dev, e->d_code, n, cudaMemcpyDeviceToDevice, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  const uint32_t acc = e->h_small[0], rej = e->h_small[1];
+  int rc = read_counters(e);
+  if (rc) return rc;
+  const uint32_t acc = e->h_cnt->accepted, rej = e->h_cnt->pool_full;
   p.n += acc;
   e->seq_next += n;
   e->last_batch_n = n;
   if (e->use_active) { e->n_active += acc; if (!e->dense_ids) e->n_tomb += rej; }
   if (n_accepted) *n_accepted = acc;
+  return MM_OK;
+}
+
+// The end of a batch uploaded from the host: the counters, then the codes to the caller's host array.  After a failed
+// upload or ingest, the stream the batch's copies ran on is drained first.
+int enq_finish_host(mm_engine* e, int rc, cudaStream_t drain, uint32_t n, uint8_t* accepted, uint32_t* n_accepted) {
+  if (rc) { cudaStreamSynchronize(drain); return rc; }
+  if ((rc = enq_finish(e, n, nullptr, n_accepted)) || !accepted) return rc;
+  CK(cudaMemcpyAsync(accepted, e->d_code, n, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
+// the engine stream waits for the copies queued on the copy stream so far
+int copy_fence(mm_engine* e) {
+  CK(cudaEventRecord(e->ev_copy, e->copy_stream));
+  CK(cudaStreamWaitEvent(e->stream, e->ev_copy, 0));
   return MM_OK;
 }
 
@@ -586,7 +682,7 @@ PlaceArgs place_args(mm_engine* e, bool want_seq) {
   a.K = e->K; a.Kp = e->Kp; a.R = tick_rows(e); a.stages = e->place_stages; a.fast_ok = e->rank_impl == 3; a.max_nb = e->max_nb;
   a.seg_bin_lo = e->d_seg_bin_lo; a.bin_seg = e->d_bin_seg; a.M = e->d_M; a.P = e->d_P;
   a.outbase = e->d_outbase; a.binlim = e->d_binlim; a.members = e->d_members;
-  a.src_idx = want_seq ? e->d_src_idx : nullptr;
+  a.src_idx = want_seq ? e->d_src_idx.p : nullptr;
   a.left_bits = e->d_left_bits; a.ctr = e->d_ctr;
   return a;
 }
@@ -599,7 +695,7 @@ EpiArgs epi_args(mm_engine* e, bool want_seq, bool headers) {
   a.write_headers = headers ? 1u : 0u;
   a.act = act_view(e); a.seg = e->d_seg; a.seg_L = e->d_seg_L; a.part_cut = e->d_part_cut;
   a.seg_bin_lo = e->d_seg_bin_lo;
-  a.hdr = e->d_hdr; a.src_idx = want_seq ? e->d_src_idx : nullptr; a.emit_seq = want_seq ? e->d_emit_seq : nullptr;
+  a.hdr = e->d_hdr; a.src_idx = want_seq ? e->d_src_idx.p : nullptr; a.emit_seq = want_seq ? e->d_emit_seq.p : nullptr;
   a.ctr = e->d_ctr;
   return a;
 }
@@ -707,14 +803,10 @@ int tick_commit(mm_engine* e, uint32_t n, mm_tick_stats* stats) {
   e->match_n = n;
   e->last = st;
   if (stats) *stats = st;
-  if (c.chist_bad) {  // placement took slot bases from chunk histograms that disagree with the pool: results are wrong
-    std::snprintf(e->last_err, sizeof(e->last_err), "%u placement tiles disagree with their chunk histograms", c.chist_bad);
-    return MM_E_STATE;
-  }
-  if (c.left_bad) {  // the compaction found leftovers beyond their partition's share of the compacted pool
-    std::snprintf(e->last_err, sizeof(e->last_err), "%u leftover players fall outside their partition's compacted range", c.left_bad);
-    return MM_E_STATE;
-  }
+  if (c.chist_bad)  // placement took slot bases from chunk histograms that disagree with the pool: results are wrong
+    return set_err(e, MM_E_STATE, "%u placement tiles disagree with their chunk histograms", c.chist_bad);
+  if (c.left_bad)  // the compaction found leftovers beyond their partition's share of the compacted pool
+    return set_err(e, MM_E_STATE, "%u leftover players fall outside their partition's compacted range", c.left_bad);
   return MM_OK;
 }
 
@@ -759,17 +851,14 @@ int tick_to_host(mm_engine* e, mm_lobby_hdr* lobbies, uint32_t lobby_cap, uint64
     // the counts are final after phase A: check the caller's capacities before consuming
     CK(cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(TickCtr), cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
-    if ((lobbies && e->h_ctr->n_lobbies > lobby_cap) || (want_members && e->h_ctr->n_matched > member_cap)) {
-      std::snprintf(e->last_err, sizeof(e->last_err), "need lobby_cap >= %u, member_cap >= %u", e->h_ctr->n_lobbies,
-                    e->h_ctr->n_matched);
-      return MM_E_CAP;
-    }
+    if ((lobbies && e->h_ctr->n_lobbies > lobby_cap) || (want_members && e->h_ctr->n_matched > member_cap))
+      return set_err(e, MM_E_CAP, "need lobby_cap >= %u, member_cap >= %u", e->h_ctr->n_lobbies, e->h_ctr->n_matched);
     if ((rc = tick_phase_b(e, emit_seq != nullptr))) return rc;
   }
   if ((rc = tick_commit(e, n, stats))) return rc;
   const TickCtr& c = *e->h_ctr;
   if (member_handles && c.n_matched) {
-    if (!e->d_members32) CK(cudaMalloc(&e->d_members32, ((size_t)e->capacity + 64) * 4));
+    CK(e->d_members32.reserve((size_t)e->capacity + 64));
     k_narrow<<<std::max(1, 4 * e->n_sms), 256, 0, e->stream>>>(c.n_matched, e->d_members, e->d_members32);
     CK(cudaGetLastError());
     if (e->async_results) CK(cudaStreamSynchronize(e->stream));  // the copy stream must see the narrowed handles
@@ -792,6 +881,32 @@ int tick_to_host(mm_engine* e, mm_lobby_hdr* lobbies, uint32_t lobby_cap, uint64
   return MM_OK;
 }
 
+// The virtual tiles of a pool of n players (an upper bound: the host-side player count bounds them), and the CTAs of a
+// tile walk over them: at most the tiles, at most 8 per SM; each CTA takes a contiguous run of tiles.
+uint32_t tile_count(const mm_engine* e, uint32_t n) { return n / kTile + e->n_segs; }
+uint32_t tile_ctas(const mm_engine* e, uint32_t n) {
+  return std::max<uint32_t>(1, std::min<uint32_t>(tile_count(e, n), 8u * (uint32_t)e->n_sms));
+}
+
+// active-set entries erased by mm_remove, mm_expire or an export release: a hashed set keeps a tombstone for each
+void erase_active(mm_engine* e, uint32_t erased) {
+  e->n_active -= std::min<uint64_t>(erased, e->n_active);
+  if (e->use_active && !e->dense_ids) e->n_tomb += erased;
+}
+
+// k_expire over the current pool, with the counters expired / erased zeroed first.  The caller sets now, max_wait,
+// commit, the outputs and the selection in `a`.
+int launch_expire(mm_engine* e, ExpireArgs a) {
+  const Pool& p = e->pool[e->cur];
+  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs;
+  a.act = act_view(e); a.gen = e->gen; a.dead_bin = e->K; a.bin_seg = e->d_bin_seg; a.seg_bin_lo = e->d_seg_bin_lo;
+  a.ctr = &e->d_cnt->expired;
+  CK(cudaMemsetAsync(a.ctr, 0, 2 * 4, e->stream));  // expired, erased
+  k_expire<kExpBlock><<<tile_ctas(e, p.n), kExpBlock, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  return MM_OK;
+}
+
 // mm_expire / mm_expire_packed (one of ids / handles).  A cap that holds every resident player cannot overflow: one
 // pass.  Otherwise a counting pass decides first, so that a refused call leaves everything as it was.
 int expire(mm_engine* e, uint64_t now, uint32_t max_wait, uint64_t* ids, uint32_t* handles, uint32_t* seq, uint32_t cap,
@@ -800,54 +915,31 @@ int expire(mm_engine* e, uint64_t now, uint32_t max_wait, uint64_t* ids, uint32_
   *n_expired = 0;
   if (p.n == 0) return MM_OK;
   ExpireArgs a{};
-  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.now = (uint32_t)now; a.max_wait = max_wait;
-  a.act = act_view(e); a.gen = e->gen; a.dead_bin = e->K; a.bin_seg = e->d_bin_seg; a.seg_bin_lo = e->d_seg_bin_lo;
-  a.ctr = e->d_small + 8;
-  // CTAs: at most the tiles in use, at most 8 per SM; each takes a contiguous run of tiles
-  const uint64_t tiles = (uint64_t)p.n / kTile + e->n_segs;
-  const uint32_t ctas = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(tiles, 8ull * (uint32_t)e->n_sms));
+  a.now = (uint32_t)now; a.max_wait = max_wait;
   uint32_t need = p.n;
+  int rc;
   if (cap < p.n) {
-    CK(cudaMemsetAsync(a.ctr, 0, 8, e->stream));
-    k_expire<kExpBlock><<<ctas, kExpBlock, 0, e->stream>>>(a);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(e->h_small + 8, a.ctr, 4, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
-    need = e->h_small[8];
+    if ((rc = launch_expire(e, a)) || (rc = read_counters(e))) return rc;
+    need = e->h_cnt->expired;
     *n_expired = need;
-    if (need > cap) {
-      std::snprintf(e->last_err, sizeof(e->last_err), "need cap >= %u", need);
-      return MM_E_CAP;
-    }
+    if (need > cap) return set_err(e, MM_E_CAP, "need cap >= %u", need);
     if (need == 0) return MM_OK;
   }
-  if (need > e->exp_cap || (seq && !e->d_exp_seq)) {
-    const uint32_t c = std::max(need, e->exp_cap);
-    cudaFree(e->d_exp_id); cudaFree(e->d_exp_seq);
-    e->d_exp_id = nullptr; e->d_exp_seq = nullptr; e->exp_cap = 0;
-    CK(cudaMalloc(&e->d_exp_id, (size_t)c * 8));
-    if (seq) CK(cudaMalloc(&e->d_exp_seq, (size_t)c * 4));
-    e->exp_cap = c;
-  }
+  CK(e->d_exp_id.reserve(need));
+  if (seq) CK(e->d_exp_seq.reserve(e->d_exp_id.n));
   a.commit = 1;
-  a.out_id = ids ? e->d_exp_id : nullptr;
-  a.out_handle = ids ? nullptr : reinterpret_cast<uint32_t*>(e->d_exp_id);
-  a.out_seq = seq ? e->d_exp_seq : nullptr;
-  CK(cudaMemsetAsync(a.ctr, 0, 8, e->stream));
-  k_expire<kExpBlock><<<ctas, kExpBlock, 0, e->stream>>>(a);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(e->h_small + 8, a.ctr, 8, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  const uint32_t n = e->h_small[8], erased = e->h_small[9];
+  a.out_id = ids ? e->d_exp_id.p : nullptr;
+  a.out_handle = ids ? nullptr : reinterpret_cast<uint32_t*>(e->d_exp_id.p);
+  a.out_seq = seq ? e->d_exp_seq.p : nullptr;
+  if ((rc = launch_expire(e, a)) || (rc = read_counters(e))) return rc;
+  const uint32_t n = e->h_cnt->expired;
   if (n) {
     if (ids) CK(cudaMemcpyAsync(ids, e->d_exp_id, (size_t)n * 8, cudaMemcpyDeviceToHost, e->stream));
     else CK(cudaMemcpyAsync(handles, e->d_exp_id, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
     if (seq) CK(cudaMemcpyAsync(seq, e->d_exp_seq, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
   }
-  // active-set bookkeeping as mm_remove's
-  e->n_active -= std::min<uint64_t>(erased, e->n_active);
-  if (e->use_active && !e->dense_ids) e->n_tomb += erased;
+  erase_active(e, e->h_cnt->erased);
   *n_expired = n;
   return MM_OK;
 }
@@ -878,83 +970,70 @@ ImgCols img_cols(uint8_t* body, const ImgLayout& l, uint32_t idb) {  // body = t
 uint32_t id_bytes(const mm_engine* e) { return e->dense_ids ? 4u : 8u; }
 uint64_t id_limit(const mm_engine* e) { return e->dense_ids ? e->hcap : kTombKey; }
 
-template <class T>
-int grow(mm_engine* e, T*& p, uint64_t& cap, uint64_t want) {
-  if (want <= cap) return MM_OK;
-  cudaFree(p);
-  p = nullptr; cap = 0;
-  CK(cudaMalloc(reinterpret_cast<void**>(&p), want));
-  cap = want;
-  return MM_OK;
-}
-
 // d_sel <- the partitions of the (mode, group) queues whose byte in `queues` (n_cut bytes) is non-zero
 int upload_sel(mm_engine* e, const uint8_t* queues) {
   std::vector<uint8_t> sel(e->n_segs);
   for (uint32_t s = 0; s < e->n_segs; ++s) sel[s] = queues[e->h_part_cut[s]] != 0;
-  if (!e->d_sel) CK(cudaMalloc(&e->d_sel, kMaxSegs));
+  CK(e->d_sel.reserve(kMaxSegs));
   CK(cudaMemcpyAsync(e->d_sel, sel.data(), e->n_segs, cudaMemcpyHostToDevice, e->stream));
   CK(cudaStreamSynchronize(e->stream));  // `sel` is pageable and goes out of scope
+  return MM_OK;
+}
+
+// Export pass 1 over the current pool: the live slots of every virtual tile into d_img_tile and of every partition
+// into d_img_part[0, n_segs), counting only the partitions in d_sel when `sel` is set.  `a` is left set for pass 2.
+int count_tiles(mm_engine* e, bool sel, ImgExportArgs& a) {
+  const Pool& p = e->pool[e->cur];
+  const uint32_t tiles = tile_count(e, p.n);
+  CK(e->d_img_tile.reserve(tiles));
+  CK(e->d_img_part.reserve((size_t)3 * e->n_segs + 2));
+  CK(cudaMemsetAsync(e->d_img_tile, 0, (size_t)tiles * 4, e->stream));
+  CK(cudaMemsetAsync(e->d_img_part, 0, (size_t)e->n_segs * 4, e->stream));
+  a = ImgExportArgs{};
+  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.tile_cnt = e->d_img_tile; a.part_cnt = e->d_img_part;
+  a.sel = sel ? e->d_sel.p : nullptr;
+  if (p.n) k_img_tiles<kImgBlock, false><<<tile_ctas(e, p.n), kImgBlock, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
   return MM_OK;
 }
 
 // mm_export (queues = null) and mm_export_queues (queues: n_cut selection bytes; the image has no active section, and
 // a call that writes it releases the exported players through k_expire with the same selection and max_wait = 0)
 int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes, const uint8_t* queues) {
-  if (e->stage_count) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "a packed batch is staged: call mm_enqueue_packed_end first");
-    return MM_E_STATE;
-  }
+  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
   const Pool& p = e->pool[e->cur];
   const uint32_t idb = id_bytes(e);
   int rc;
   if (queues && (rc = upload_sel(e, queues))) return rc;
   // pass 1: live slots per tile and per partition, the tiles' offsets; the active section
-  const uint32_t tiles = p.n / kTile + e->n_segs;  // bounds the virtual tile count
-  const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(tiles, 8u * (uint32_t)e->n_sms));
-  uint64_t tile_cap = e->img_tile_cap;
-  if ((rc = grow(e, e->d_img_tile, tile_cap, (uint64_t)tiles * 4))) return rc;
-  e->img_tile_cap = (uint32_t)tile_cap;
-  if (!e->d_img_part) CK(cudaMalloc(&e->d_img_part, ((size_t)3 * e->n_segs + 2) * 4));
-  CK(cudaMemsetAsync(e->d_img_tile, 0, (size_t)tiles * 4, e->stream));
-  CK(cudaMemsetAsync(e->d_img_part, 0, (size_t)e->n_segs * 4, e->stream));
-  CK(cudaMemsetAsync(e->d_small + 12, 0, 8, e->stream));
-  ImgExportArgs a{};
-  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.tile_cnt = e->d_img_tile; a.part_cnt = e->d_img_part;
-  a.sel = queues ? e->d_sel : nullptr;
-  if (p.n) k_img_tiles<kImgBlock, false><<<ctas, kImgBlock, 0, e->stream>>>(a);
-  k_scan_small<<<1, 1024, 0, e->stream>>>(tiles, e->d_img_tile, e->d_small + 12);
+  ImgExportArgs a;
+  if ((rc = count_tiles(e, queues != nullptr, a))) return rc;
+  CK(cudaMemsetAsync(&e->d_cnt->img_players, 0, 2 * 4, e->stream));  // img_players, img_active
+  k_scan_small<<<1, 1024, 0, e->stream>>>(tile_count(e, p.n), e->d_img_tile, &e->d_cnt->img_players);
   const uint32_t act_cap = queues ? 0u : (uint32_t)std::min<uint64_t>(e->n_active, 0xFFFFFFFFu);
   if (e->use_active && act_cap) {
-    if ((rc = grow(e, e->d_img_act, e->img_act_cap, (uint64_t)act_cap * idb))) return rc;
+    CK(e->d_img_act.reserve((size_t)act_cap * idb));
     const uint64_t n_tab = e->hcap;
     const uint32_t nb = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n_tab + 255) / 256, 16ull * (uint32_t)e->n_sms));
     k_img_active<<<nb, 256, 0, e->stream>>>(act_view(e), n_tab, p.v.mode, (uint32_t)pool_slots(e), e->gen, e->d_img_act,
-                                            idb, act_cap, e->d_small + 13);
+                                            idb, act_cap, &e->d_cnt->img_active);
   }
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(e->h_small + 12, e->d_small + 12, 8, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  const uint32_t n = e->h_small[12], m = e->h_small[13];
-  if (m > act_cap) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "%u active ids outside the pool, %u in the active set", m, act_cap);
-    return MM_E_STATE;
-  }
+  if ((rc = read_counters(e))) return rc;
+  const uint32_t n = e->h_cnt->img_players, m = e->h_cnt->img_active;
+  if (m > act_cap) return set_err(e, MM_E_STATE, "%u active ids outside the pool, %u in the active set", m, act_cap);
   const ImgLayout l = img_layout(e->n_segs, n, m, idb);
   *n_bytes = l.off[7];
   if (!buf) return MM_OK;
-  if (cap < l.off[7]) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "need cap >= %llu", (unsigned long long)l.off[7]);
-    return MM_E_CAP;
-  }
+  if (cap < l.off[7]) return set_err(e, MM_E_CAP, "need cap >= %llu", (unsigned long long)l.off[7]);
   // pass 2: the columns, laid out as in the image (padding zero)
   uint8_t* out = static_cast<uint8_t*>(buf);
   const uint64_t col_bytes = l.off[6] - l.off[1];
-  if ((rc = grow(e, e->d_img, e->img_cap, std::max<uint64_t>(col_bytes, 8)))) return rc;
+  CK(e->d_img.reserve(std::max<uint64_t>(col_bytes, 8)));
   if (n) {
     CK(cudaMemsetAsync(e->d_img, 0, col_bytes, e->stream));
     a.out = img_cols(e->d_img, l, idb);
-    k_img_tiles<kImgBlock, true><<<ctas, kImgBlock, 0, e->stream>>>(a);
+    k_img_tiles<kImgBlock, true><<<tile_ctas(e, p.n), kImgBlock, 0, e->stream>>>(a);
     CK(cudaGetLastError());
   }
   mm_image_header h{};
@@ -967,31 +1046,21 @@ int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes, const
   CK(cudaMemcpyAsync(out + l.off[0], e->d_img_part, (size_t)e->n_segs * 4, cudaMemcpyDeviceToHost, e->stream));
   if (n) CK(cudaMemcpyAsync(out + l.off[1], e->d_img, col_bytes, cudaMemcpyDeviceToHost, e->stream));
   if (m) CK(cudaMemcpyAsync(out + l.off[6], e->d_img_act, (size_t)m * idb, cudaMemcpyDeviceToHost, e->stream));
-  if (queues && n) {  // release the exported players, as mm_remove would: dead slots until the next tick
-    ExpireArgs x{};
-    x.pool = p.v; x.meta = p.m; x.n_segs = e->n_segs; x.now = 0; x.max_wait = 0; x.commit = 1;
-    x.act = act_view(e); x.gen = e->gen; x.dead_bin = e->K; x.bin_seg = e->d_bin_seg; x.seg_bin_lo = e->d_seg_bin_lo;
-    x.sel = e->d_sel; x.ctr = e->d_small + 8;
-    CK(cudaMemsetAsync(x.ctr, 0, 8, e->stream));
-    k_expire<kExpBlock><<<ctas, kExpBlock, 0, e->stream>>>(x);
-    CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(e->h_small + 8, x.ctr, 8, cudaMemcpyDeviceToHost, e->stream));
+  if (!(queues && n)) {
+    CK(cudaStreamSynchronize(e->stream));
+    return MM_OK;
   }
-  CK(cudaStreamSynchronize(e->stream));
-  if (queues && n) {
-    const uint32_t erased = e->h_small[9];
-    e->n_active -= std::min<uint64_t>(erased, e->n_active);
-    if (e->use_active && !e->dense_ids) e->n_tomb += erased;
-  }
+  // release the exported players, as mm_remove would: dead slots until the next tick (max_wait 0: every selected one)
+  ExpireArgs x{};
+  x.commit = 1; x.sel = e->d_sel;
+  if ((rc = launch_expire(e, x)) || (rc = read_counters(e))) return rc;
+  erase_active(e, e->h_cnt->erased);
   return MM_OK;
 }
 
-// the image-sized scratch of mm_export / mm_import (cudaFree waits for the work that uses it)
+// the image-sized scratch of mm_export / mm_import / mm_merge (cudaFree waits for the work that uses it)
 void free_img_scratch(mm_engine* e) {
-  cudaFree(e->d_img); cudaFree(e->d_img_act);
-  e->d_img = nullptr; e->img_cap = 0; e->d_img_act = nullptr; e->img_act_cap = 0;
-  cudaFree(e->d_mrg_src); cudaFree(e->d_mrg_code); cudaFree(e->d_mrg_seen);
-  e->d_mrg_src = nullptr; e->d_mrg_code = nullptr; e->mrg_code_cap = 0; e->d_mrg_seen = nullptr;
+  e->d_img.reset(); e->d_img_act.reset(); e->d_mrg_src.reset(); e->d_mrg_code.reset(); e->d_mrg_seen.reset();
 }
 
 // The current pool buffer and the active set back to an empty engine's state.
@@ -1022,42 +1091,54 @@ bool same_layout(const mm_config& a, const mm_config& c) {
   return same;
 }
 
-int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
-  auto bad = [&](const char* what) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "image rejected: %s", what);
-    return (int)MM_E_ARG;
-  };
-  if (!e->fresh || e->stage_count) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "mm_import needs a fresh engine (nothing enqueued, imported or restored)");
-    return MM_E_STATE;
-  }
-  mm_image_header h;
+// The header checks of mm_import and mm_merge.  `magic` is the image kind's, `prefix` starts every message, and
+// `no_active` refuses an active section (null: one is allowed).  -> the header, its layout and the partition counts
+int check_header(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t magic, const char* prefix,
+                 const char* bad_magic, const char* no_active, mm_image_header& h, ImgLayout& l,
+                 std::vector<uint32_t>& cnt) {
+  auto bad = [&](const char* what) { return set_err(e, MM_E_ARG, "%s: %s", prefix, what); };
   if (nb < sizeof(h)) return bad("shorter than its header");
   std::memcpy(&h, buf, sizeof(h));
-  if (h.magic != MM_IMAGE_MAGIC) return bad("bad magic");
+  if (h.magic != magic) return bad(bad_magic);
   if (h.version != MM_IMAGE_VERSION || h.abi_version != MM_ABI_VERSION) return bad("unknown version");
   if (h.id_bytes != id_bytes(e)) return bad("id width differs from the engine's");
   if (h.n_parts != e->n_segs) return bad("partition count differs from the engine's layout");
-  const ImgLayout l = img_layout(h.n_parts, h.n_players, h.n_active, h.id_bytes);
+  l = img_layout(h.n_parts, h.n_players, h.n_active, h.id_bytes);
   if (h.total_bytes != l.off[7] || nb != l.off[7]) return bad("length does not match the header's section counts");
   if (!same_layout(h.config, e->cfg))
     return bad("config differs from the engine's (groups, default_group, modes, order_mode or flags)");
-  if (!e->use_active && h.n_active) return bad("active section in an image of an engine without an active set");
-  std::vector<uint32_t> cnt(e->n_segs);
+  if (no_active && h.n_active) return bad(no_active);
+  cnt.resize(e->n_segs);
   std::memcpy(cnt.data(), buf + l.off[0], (size_t)e->n_segs * 4);
   uint64_t sum = 0;
   for (uint32_t q : cnt) sum += q;
   if (sum != h.n_players) return bad("partition counts do not add up to the player count");
+  return MM_OK;
+}
+
+// the kImg* bits the device checks of an image's players set, named
+int img_err(mm_engine* e, const char* prefix, uint32_t err) {
+  return set_err(e, MM_E_ARG, "%s:%s%s%s%s%s%s", prefix, err & kImgBadId ? " id out of range" : "",
+                 err & kImgBadMode ? " mode out of range" : "", err & kImgBadRating ? " rating outside its partition" : "",
+                 err & kImgBadSeq ? " sequence numbers out of order" : "", err & kImgDup ? " duplicate id" : "",
+                 err & kImgFull ? " active set full" : "");
+}
+
+int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
+  if (!e->fresh || e->stage_count)
+    return set_err(e, MM_E_STATE, "mm_import needs a fresh engine (nothing enqueued, imported or restored)");
+  mm_image_header h;
+  ImgLayout l;
+  std::vector<uint32_t> cnt;
+  int rc = check_header(e, buf, nb, MM_IMAGE_MAGIC, "image rejected", "bad magic",
+                        e->use_active ? nullptr : "active section in an image of an engine without an active set", h, l,
+                        cnt);
+  if (rc) return rc;
   const uint32_t n = h.n_players, m = h.n_active;
-  if (n > e->capacity) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "%u players, capacity %u", n, e->capacity);
-    return MM_E_CAP;
-  }
-  if (e->use_active && !e->dense_ids && ((uint64_t)n + m) * 4 > e->hcap * 3) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "%llu active ids, active set holds %llu",
-                  (unsigned long long)n + m, (unsigned long long)(e->hcap * 3 / 4));
-    return MM_E_CAP;
-  }
+  if (n > e->capacity) return set_err(e, MM_E_CAP, "%u players, capacity %u", n, e->capacity);
+  if (e->use_active && !e->dense_ids && ((uint64_t)n + m) * 4 > e->hcap * 3)
+    return set_err(e, MM_E_CAP, "%llu active ids, active set holds %llu", (unsigned long long)n + m,
+                   (unsigned long long)(e->hcap * 3 / 4));
   // every partition on consecutive chunks, in partition order
   std::vector<uint32_t> tab((size_t)e->n_segs * e->n_chunks, 0), off_base(2 * (size_t)e->n_segs + 1);
   uint32_t chunk = 0, idx = 0;
@@ -1070,18 +1151,17 @@ int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
     chunk += nch;
   }
   off_base[e->n_segs] = idx;
-  int rc = clear_engine(e);
-  if (rc) return rc;
+  if ((rc = clear_engine(e))) return rc;
   Pool& p = e->pool[e->cur];
   const uint64_t body = nb - l.off[1];  // columns and active section
-  if (!e->d_img_part) CK(cudaMalloc(&e->d_img_part, ((size_t)3 * e->n_segs + 2) * 4));
-  if ((rc = grow(e, e->d_img, e->img_cap, std::max<uint64_t>(body, 8)))) return rc;
+  CK(e->d_img_part.reserve((size_t)3 * e->n_segs + 2));
+  CK(e->d_img.reserve(std::max<uint64_t>(body, 8)));
   CK(cudaMemcpyAsync(p.m.fill, cnt.data(), (size_t)e->n_segs * 4, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(p.m.chunk_tab, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(p.m.bump, &chunk, 4, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(e->d_img_part, off_base.data(), off_base.size() * 4, cudaMemcpyHostToDevice, e->stream));
   if (body) CK(cudaMemcpyAsync(e->d_img, buf + l.off[1], body, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemsetAsync(e->d_small + 14, 0, 4, e->stream));
+  CK(cudaMemsetAsync(&e->d_cnt->img_err, 0, 4, e->stream));
   const ImgCols cols = img_cols(e->d_img, l, h.id_bytes);
   const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((n + 255) / 256, 32u * (uint32_t)e->n_sms));
   if (n) {
@@ -1090,28 +1170,23 @@ int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
     la.part_off = e->d_img_part; la.slot_base = e->d_img_part + e->n_segs + 1;
     la.bm = bin_map(e); la.grp_lut = e->d_grp_lut; la.bin_seg = e->d_bin_seg; la.seg_bin_lo = e->d_seg_bin_lo;
     la.mode_tsize = e->d_mode_tsize; la.n_modes = e->cfg.n_modes; la.seq_next = h.seq_next; la.id_limit = id_limit(e);
-    la.err = e->d_small + 14;
+    la.err = &e->d_cnt->img_err;
     k_img_load<<<grid, 256, 0, e->stream>>>(la);
   }
   if (e->use_active) {
     const ActiveView av = act_view(e);
-    if (n) k_img_insert<<<grid, 256, 0, e->stream>>>(cols.id, h.id_bytes, n, id_limit(e), av, e->d_small + 14);
+    if (n) k_img_insert<<<grid, 256, 0, e->stream>>>(cols.id, h.id_bytes, n, id_limit(e), av, &e->d_cnt->img_err);
     if (m) {
       const uint32_t g2 = std::max<uint32_t>(1, std::min<uint32_t>((m + 255) / 256, 32u * (uint32_t)e->n_sms));
       k_img_insert<<<g2, 256, 0, e->stream>>>(e->d_img + (l.off[6] - l.off[1]), h.id_bytes, m, id_limit(e), av,
-                                              e->d_small + 14);
+                                              &e->d_cnt->img_err);
     }
   }
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(e->h_small + 14, e->d_small + 14, 4, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  if (const uint32_t err = e->h_small[14]) {
+  if ((rc = read_counters(e))) return rc;
+  if (const uint32_t err = e->h_cnt->img_err) {
     if ((rc = clear_engine(e))) return rc;
-    std::snprintf(e->last_err, sizeof(e->last_err), "image rejected:%s%s%s%s%s%s", err & kImgBadId ? " id out of range" : "",
-                  err & kImgBadMode ? " mode out of range" : "", err & kImgBadRating ? " rating outside its partition" : "",
-                  err & kImgBadSeq ? " sequence numbers out of order" : "", err & kImgDup ? " duplicate id" : "",
-                  err & kImgFull ? " active set full" : "");
-    return MM_E_ARG;
+    return img_err(e, "image rejected", err);
   }
   p.n = n;
   e->seq_next = h.seq_next;
@@ -1129,22 +1204,11 @@ int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
 
 // live players per partition of the current pool, restricted to the partitions in d_sel (the export count pass)
 int count_live(mm_engine* e, std::vector<uint32_t>& per_part) {
-  const Pool& p = e->pool[e->cur];
   per_part.assign(e->n_segs, 0);
-  if (!p.n) return MM_OK;
-  const uint32_t tiles = p.n / kTile + e->n_segs;
-  const uint32_t ctas = std::max<uint32_t>(1, std::min<uint32_t>(tiles, 8u * (uint32_t)e->n_sms));
-  uint64_t tile_cap = e->img_tile_cap;
-  int rc;
-  if ((rc = grow(e, e->d_img_tile, tile_cap, (uint64_t)tiles * 4))) return rc;
-  e->img_tile_cap = (uint32_t)tile_cap;
-  if (!e->d_img_part) CK(cudaMalloc(&e->d_img_part, ((size_t)3 * e->n_segs + 2) * 4));
-  CK(cudaMemsetAsync(e->d_img_part, 0, (size_t)e->n_segs * 4, e->stream));
-  ImgExportArgs a{};
-  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.tile_cnt = e->d_img_tile; a.part_cnt = e->d_img_part;
-  a.sel = e->d_sel;
-  k_img_tiles<kImgBlock, false><<<ctas, kImgBlock, 0, e->stream>>>(a);
-  CK(cudaGetLastError());
+  if (!e->pool[e->cur].n) return MM_OK;
+  ImgExportArgs a;
+  int rc = count_tiles(e, true, a);
+  if (rc) return rc;
   CK(cudaMemcpyAsync(per_part.data(), e->d_img_part, (size_t)e->n_segs * 4, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   return MM_OK;
@@ -1154,65 +1218,46 @@ int count_live(mm_engine* e, std::vector<uint32_t>& per_part) {
 // the capacities and the reject list's size), then one ingest batch through enq_prepare / enq_chunk / enq_finish with
 // its codes in d_mrg_code, so that mm_enqueue_rejects still reads the last mm_enqueue* batch.
 int merge_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uint32_t* rejected, uint32_t* n_rejected) {
-  auto bad = [&](const char* what) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "queue image rejected: %s", what);
-    return (int)MM_E_ARG;
-  };
-  if (e->stage_count) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "a packed batch is staged: call mm_enqueue_packed_end first");
-    return MM_E_STATE;
-  }
+  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
   mm_image_header h;
-  if (nb < sizeof(h)) return bad("shorter than its header");
-  std::memcpy(&h, buf, sizeof(h));
-  if (h.magic != MM_QUEUE_IMAGE_MAGIC) return bad("bad magic (not an mm_export_queues image)");
-  if (h.version != MM_IMAGE_VERSION || h.abi_version != MM_ABI_VERSION) return bad("unknown version");
-  if (h.id_bytes != id_bytes(e)) return bad("id width differs from the engine's");
-  if (h.n_parts != e->n_segs) return bad("partition count differs from the engine's layout");
-  if (h.n_active) return bad("a queue image has no active section");
-  const ImgLayout l = img_layout(h.n_parts, h.n_players, 0, h.id_bytes);
-  if (h.total_bytes != l.off[7] || nb != l.off[7]) return bad("length does not match the header's section counts");
-  if (!same_layout(h.config, e->cfg))
-    return bad("config differs from the engine's (groups, default_group, modes, order_mode or flags)");
-  std::vector<uint32_t> cnt(e->n_segs), off(e->n_segs + 1, 0);
-  std::memcpy(cnt.data(), buf + l.off[0], (size_t)e->n_segs * 4);
-  uint64_t sum = 0;
-  for (uint32_t s = 0; s < e->n_segs; ++s) { off[s] = (uint32_t)std::min<uint64_t>(sum, 0xFFFFFFFFu); sum += cnt[s]; }
-  if (sum != h.n_players) return bad("partition counts do not add up to the player count");
+  ImgLayout l;
+  std::vector<uint32_t> cnt;
+  int rc = check_header(e, buf, nb, MM_QUEUE_IMAGE_MAGIC, "queue image rejected",
+                        "bad magic (not an mm_export_queues image)", "a queue image has no active section", h, l, cnt);
+  if (rc) return rc;
   const uint32_t n = h.n_players;
-  off[e->n_segs] = n;
   if (n == 0) return MM_OK;
+  std::vector<uint32_t> off(e->n_segs + 1, n);  // first image index of each partition
+  for (uint32_t s = 0, sum = 0; s < e->n_segs; ++s) { off[s] = sum; sum += cnt[s]; }
   // the queues the image fills must hold no live player here
   std::vector<uint8_t> touched(e->n_cut, 0);
   for (uint32_t s = 0; s < e->n_segs; ++s)
     if (cnt[s]) touched[e->h_part_cut[s]] = 1;
-  int rc;
   if ((rc = upload_sel(e, touched.data()))) return rc;
   std::vector<uint32_t> live;
   if ((rc = count_live(e, live))) return rc;
   for (uint32_t s = 0; s < e->n_segs; ++s)
     if (live[s]) {
       const uint32_t c = e->h_part_cut[s];
-      std::snprintf(e->last_err, sizeof(e->last_err), "queue (mode %u, group %u) holds %u live players here",
-                    c / e->cfg.n_groups, c % e->cfg.n_groups, live[s]);
-      return MM_E_STATE;
+      return set_err(e, MM_E_STATE, "queue (mode %u, group %u) holds %u live players here", c / e->cfg.n_groups,
+                     c % e->cfg.n_groups, live[s]);
     }
   // upload once; the pre-pass checks every player and writes the ingest batch in the queues' enqueue order
   if ((rc = ensure_enq_scratch(e, n))) return rc;
   const uint64_t body = l.off[6] - l.off[1];
-  if ((rc = grow(e, e->d_img, e->img_cap, std::max<uint64_t>(body, 8)))) return rc;
-  CK(cudaMalloc(&e->d_mrg_src, ((size_t)n + 64) * 4));
-  if (!e->d_img_part) CK(cudaMalloc(&e->d_img_part, ((size_t)3 * e->n_segs + 2) * 4));
+  CK(e->d_img.reserve(std::max<uint64_t>(body, 8)));
+  CK(e->d_mrg_src.reserve((size_t)n + 64));
+  CK(e->d_img_part.reserve((size_t)3 * e->n_segs + 2));
   CK(cudaMemcpyAsync(e->d_img, buf + l.off[1], body, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(e->d_img_part, off.data(), off.size() * 4, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemsetAsync(e->d_small + 14, 0, 8, e->stream));
+  CK(cudaMemsetAsync(&e->d_cnt->img_err, 0, 2 * 4, e->stream));  // img_err, mrg_dups
   const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((n + 255) / 256, 32u * (uint32_t)e->n_sms));
   MrgOrderArgs oa{};
   oa.in = img_cols(e->d_img, l, h.id_bytes); oa.n = n; oa.n_segs = e->n_segs; oa.part_off = e->d_img_part;
   oa.part_cut = e->d_part_cut; oa.cut_lp_lo = e->d_cut_lp_lo; oa.bm = bin_map(e); oa.grp_lut = e->d_grp_lut;
   oa.bin_seg = e->d_bin_seg; oa.n_modes = e->cfg.n_modes; oa.seq_next = h.seq_next; oa.id_limit = id_limit(e);
   oa.out_id = e->d_in_id; oa.out_rating = e->d_in_rating; oa.out_mode = e->d_in_mode; oa.out_ts = e->d_in_ts;
-  oa.src = e->d_mrg_src; oa.err = e->d_small + 14;
+  oa.src = e->d_mrg_src; oa.err = &e->d_cnt->img_err;
   k_mrg_order<<<grid, 256, 0, e->stream>>>(oa);
   CK(cudaGetLastError());
   // the exact reject count, when the reject list or a capacity could be too small for every player being queued
@@ -1222,35 +1267,23 @@ int merge_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uin
   if (e->use_active && (cap < n || tight)) {
     uint64_t sc = 1024;
     while (sc < 2ull * n) sc <<= 1;
-    CK(cudaMalloc(&e->d_mrg_seen, sc * 8));
+    CK(e->d_mrg_seen.reserve(sc));
     CK(cudaMemsetAsync(e->d_mrg_seen, 0xFF, sc * 8, e->stream));
-    k_mrg_dups<<<grid, 256, 0, e->stream>>>(e->d_in_id, n, act_view(e), e->d_mrg_seen, sc - 1, e->d_small + 15);
+    k_mrg_dups<<<grid, 256, 0, e->stream>>>(e->d_in_id, n, act_view(e), e->d_mrg_seen, sc - 1, &e->d_cnt->mrg_dups);
     CK(cudaGetLastError());
   }
-  CK(cudaMemcpyAsync(e->h_small + 14, e->d_small + 14, 8, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  if (const uint32_t err = e->h_small[14]) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "queue image rejected:%s%s%s%s", err & kImgBadId ? " id out of range" : "",
-                  err & kImgBadMode ? " mode out of range" : "", err & kImgBadRating ? " rating outside its partition" : "",
-                  err & kImgBadSeq ? " sequence numbers out of order" : "");
-    return MM_E_ARG;
-  }
-  const uint32_t n_rej = e->h_small[15], accepted = n - n_rej;
+  if ((rc = read_counters(e))) return rc;
+  if (const uint32_t err = e->h_cnt->img_err) return img_err(e, "queue image rejected", err);
+  const uint32_t n_rej = e->h_cnt->mrg_dups, accepted = n - n_rej;
   if (n_rej > cap) {
     *n_rejected = n_rej;
-    std::snprintf(e->last_err, sizeof(e->last_err), "%u rejected players, cap %u", n_rej, cap);
-    return MM_E_CAP;
+    return set_err(e, MM_E_CAP, "%u rejected players, cap %u", n_rej, cap);
   }
-  if ((uint64_t)p.n + accepted > e->capacity) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "%u players merged into %u slots in use, capacity %u", accepted, p.n,
-                  e->capacity);
-    return MM_E_CAP;
-  }
-  if (hashed && (e->n_active + accepted) * 4 > e->hcap * 3) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "active set full: %llu ids resident, %u merged, capacity %llu",
-                  (unsigned long long)e->n_active, accepted, (unsigned long long)(e->hcap * 3 / 4));
-    return MM_E_CAP;
-  }
+  if ((uint64_t)p.n + accepted > e->capacity)
+    return set_err(e, MM_E_CAP, "%u players merged into %u slots in use, capacity %u", accepted, p.n, e->capacity);
+  if (hashed && (e->n_active + accepted) * 4 > e->hcap * 3)
+    return set_err(e, MM_E_CAP, "active set full: %llu ids resident, %u merged, capacity %llu",
+                   (unsigned long long)e->n_active, accepted, (unsigned long long)(e->hcap * 3 / 4));
   // the ingest, with the merge's own code buffer
   auto ingest = [&]() -> int {
     int r = enq_prepare(e, n, accepted);
@@ -1260,12 +1293,11 @@ int merge_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uin
     if (!r) r = enq_finish(e, n, nullptr, &n_acc);
     if (r || n_acc == n) return r;
     uint32_t* d_out = e->d_in_handle;  // free once the batch is in
-    CK(cudaMemsetAsync(e->d_small + 4, 0, 4, e->stream));
-    k_mrg_rejects<<<(n + 255) / 256, 256, 0, e->stream>>>(n, e->d_code, e->d_mrg_src, d_out, e->d_small + 4);
+    CK(cudaMemsetAsync(&e->d_cnt->rejects, 0, 4, e->stream));
+    k_mrg_rejects<<<(n + 255) / 256, 256, 0, e->stream>>>(n, e->d_code, e->d_mrg_src, d_out, &e->d_cnt->rejects);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(e->h_small + 4, e->d_small + 4, 4, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
-    const uint32_t k = std::min(e->h_small[4], cap);
+    if ((r = read_counters(e))) return r;
+    const uint32_t k = std::min(e->h_cnt->rejects, cap);
     CK(cudaMemcpyAsync(rejected, d_out, (size_t)k * 4, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
     std::sort(rejected, rejected + k);
@@ -1274,12 +1306,33 @@ int merge_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uin
   };
   const uint32_t last_n = e->last_batch_n;
   std::swap(e->d_code, e->d_mrg_code);
-  std::swap(e->code_cap, e->mrg_code_cap);
   rc = ingest();
   std::swap(e->d_code, e->d_mrg_code);
-  std::swap(e->code_cap, e->mrg_code_cap);
   e->last_batch_n = last_n;
   return rc;
+}
+
+// mm_remove (take = false: the ids leave the active set too) and mm_take (they stay in it)
+int remove_or_take(mm_engine* e, uint32_t n, const uint64_t* id, uint32_t* n_out, bool take) {
+  if (n_out) *n_out = 0;
+  if (!e || (n && !id)) return MM_E_ARG;
+  if (!e->use_active) return MM_E_STATE;
+  if (n == 0) return MM_OK;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  int rc = ensure_enq_scratch(e, n);
+  if (rc) return rc;
+  const Pool& p = e->pool[e->cur];
+  CK(cudaMemcpyAsync(e->d_in_id, id, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemsetAsync(&e->d_cnt->removed, 0, 4, e->stream));
+  (take ? k_take : k_remove)<<<(n + 255) / 256, 256, 0, e->stream>>>(
+      n, e->d_in_id, act_view(e), p.v, p.m, (uint32_t)pool_slots(e), e->gen, e->K, e->d_bin_seg, e->d_seg_bin_lo,
+      &e->d_cnt->removed);
+  CK(cudaGetLastError());
+  if ((rc = read_counters(e))) return rc;
+  if (!take) erase_active(e, e->h_cnt->removed);
+  if (n_out) *n_out = e->h_cnt->removed;
+  return MM_OK;
 }
 
 }  // namespace
@@ -1370,49 +1423,15 @@ int mm_create(const mm_config* cfg, mm_engine** out) {
       if (2 * (place_smem_bytes(e->max_nb, st) + static_smem + 1024) <= e->smem_sm) { e->place_stages = st; e->rows_per_sm = 2; }
     for (uint32_t st = kMaxStages; st >= 1 && !e->place_stages; --st)  // huge key domains: down to a single stage
       if (place_smem_bytes(e->max_nb, st) + static_smem + 1024 <= e->smem_optin) { e->place_stages = st; e->rows_per_sm = 1; }
-    if (!e->place_stages || colscan_smem(e) + static_smem + 1024 > e->smem_optin) {
-      std::snprintf(e->last_err, sizeof(e->last_err), "key domain too large for shared memory: %u bins", e->Kp);
-      return bail(MM_E_ARG);
-    }
+    if (!e->place_stages || colscan_smem(e) + static_smem + 1024 > e->smem_optin)
+      return bail(set_err(e, MM_E_ARG, "key domain too large for shared memory: %u bins", e->Kp));
     bool ok = allow_max_smem(e, k_colscan) == cudaSuccess && allow_max_smem(e, k_hist<512>) == cudaSuccess &&
               allow_max_smem(e, k_place<512>) == cudaSuccess && allow_max_smem(e, k_tick<512>) == cudaSuccess;
     if (!ok) return bail(fail(e, cudaGetLastError(), "cudaFuncSetAttribute"));
   }
   e->n_chunks = (e->capacity + kTile - 1) / kTile + e->n_segs + 2;
   if ((uint64_t)e->n_chunks * e->n_segs * 4 > (8ull << 30)) return bail(MM_E_CAP);
-  if ((rc = alloc_pool(e, e->pool[0])) || (rc = alloc_pool(e, e->pool[1]))) return bail(rc);
-  if (cudaMalloc(&e->d_left_bits, (pool_slots(e) / 32 + 64) * 4) != cudaSuccess) return bail(MM_E_CUDA);
-  if (e->use_active) {
-    const uint64_t want = cfg->active_capacity ? cfg->active_capacity : 2ull * cfg->capacity;
-    if (e->dense_ids) {
-      e->hcap = want;  // handles 0 .. active_capacity - 1
-      for (auto& t : e->tab) t.kv = nullptr;
-      if (cudaMalloc(&e->tab[0].kv, e->hcap * 8) != cudaSuccess) return bail(MM_E_CUDA);
-    } else {
-      uint64_t h = 1024;
-      while (h * 3 < want * 4 + 64) h <<= 1;  // load factor <= 0.75 at active_capacity
-      e->hcap = h;
-      for (auto& t : e->tab)
-        if (cudaMalloc(&t.kv, h * 16) != cudaSuccess) return bail(MM_E_CUDA);
-    }
-    if ((rc = clear_table(e, e->tab[0]))) return bail(rc);
-  }
-  const size_t cap = (size_t)e->capacity + 64;
-  e->max_lobbies = e->capacity / e->min_L + 1;
-  auto A = [&](void** p, size_t bytes) { return cudaMalloc(p, bytes) == cudaSuccess; };
-  if (!A((void**)&e->d_outbase, (e->Kp + 1) * 4) ||
-      !A((void**)&e->d_binlim, (e->Kp + 1) * 4) || !A((void**)&e->d_seg, e->n_segs * sizeof(SegInfo)) ||
-      !A((void**)&e->d_members, cap * 8) || !A((void**)&e->d_src_idx, cap * 4) ||
-      !A((void**)&e->d_hdr, (size_t)e->max_lobbies * sizeof(mm_lobby_hdr)) ||
-      !A((void**)&e->d_emit_seq, (size_t)e->max_lobbies * 4) || !A((void**)&e->d_ctr2, 2 * sizeof(TickCtr)) ||
-      !A((void**)&e->d_small, 64) ||
-      !A((void**)&e->d_blockhist, (size_t)e->n_segs * (kEnqChunkDev / kIngestItems + 1) * 4))
-    return bail(fail(e, cudaGetLastError(), "cudaMalloc"));
-  if (cudaMemset(e->d_ctr2, 0, 2 * sizeof(TickCtr)) != cudaSuccess) return bail(MM_E_CUDA);
-  e->d_ctr = e->d_ctr2;
-  if (cudaMallocHost(&e->h_ctr, sizeof(TickCtr)) != cudaSuccess || cudaMallocHost(&e->h_small, 64) != cudaSuccess)
-    return bail(MM_E_CUDA);
-  if ((rc = alloc_tick_scratch(e))) return bail(rc);
+  if ((rc = alloc_buffers(e))) return bail(rc);
   {
     size_t sz = std::max(hist_smem_bytes(e->max_nb), place_smem_bytes(e->max_nb, e->place_stages));
     sz = std::max<size_t>(sz, std::max<size_t>((size_t)std::max(kEpiScratchWords, kRowCompactWords) * 4, colscan_smem(e)));
@@ -1435,31 +1454,18 @@ int mm_destroy(mm_engine* e) {
   cudaSetDevice(e->device);
   if (e->stream) cudaStreamSynchronize(e->stream);
   if (e->d2h_stream) cudaStreamSynchronize(e->d2h_stream);
-  free_pool(e->pool[0]); free_pool(e->pool[1]); free_pool(e->snap); cudaFree(e->d_left_bits);
-  for (auto& t : e->tab) cudaFree(t.kv);
-  cudaFree(e->snap_tab.kv);
-  cudaFree(e->d_lut); cudaFree(e->d_grp_lut); cudaFree(e->d_mode_tsize); cudaFree(e->d_seg_bin_lo); cudaFree(e->d_seg_L);
-  cudaFree(e->d_part_cut); cudaFree(e->d_cut_lp_lo);
-  cudaFree(e->d_M); cudaFree(e->d_P); cudaFree(e->d_outbase); cudaFree(e->d_binlim); cudaFree(e->d_bin_seg);
-  cudaFree(e->d_bin_key); cudaFree(e->d_seg); cudaFree(e->d_members); cudaFree(e->d_members32); cudaFree(e->d_members32_alt); cudaFree(e->d_hdr_alt); cudaFree(e->d_src_idx);
-  cudaFree(e->d_hdr); cudaFree(e->d_emit_seq); cudaFree(e->d_ctr2); cudaFree(e->d_small);
-  cudaFree(e->d_in_id); cudaFree(e->d_hslot); cudaFree(e->d_in_rating); cudaFree(e->d_in_mode); cudaFree(e->d_code); cudaFree(e->d_lookup);
-  cudaFree(e->d_in_ts); cudaFree(e->d_blocksum); cudaFree(e->d_blockhist); cudaFree(e->d_part); cudaFree(e->d_in_key);
-  cudaFree(e->d_in_handle); cudaFree(e->d_rej_idx); cudaFree(e->d_rej_code);
-  cudaFree(e->d_qstat); cudaFree(e->d_exp_id); cudaFree(e->d_exp_seq);
-  cudaFree(e->d_img); cudaFree(e->d_img_tile); cudaFree(e->d_img_part); cudaFree(e->d_img_act);
-  cudaFree(e->d_sel); cudaFree(e->d_mrg_src); cudaFree(e->d_mrg_code); cudaFree(e->d_mrg_seen);
   if (e->h_ctr) cudaFreeHost(e->h_ctr);
-  if (e->h_small) cudaFreeHost(e->h_small);
+  if (e->h_cnt) cudaFreeHost(e->h_cnt);
   for (auto& ev : e->ev)
     if (ev) cudaEventDestroy(ev);
   if (e->stream && e->own_stream) cudaStreamDestroy(e->stream);
-  for (auto& st : e->stage) { cudaFree(st.handle); cudaFree(st.key); cudaFree(st.ts); if (st.ready) cudaEventDestroy(st.ready); }
+  for (auto& st : e->stage)
+    if (st.ready) cudaEventDestroy(st.ready);
   if (e->d2h_stream) cudaStreamDestroy(e->d2h_stream);
   if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
   if (e->ev_copy) cudaEventDestroy(e->ev_copy);
+  delete e;  // frees the device arrays (on e->device, current here)
   cudaGetLastError();
-  delete e;
   return MM_OK;
 }
 
@@ -1489,9 +1495,9 @@ int mm_set_option(mm_engine* e, const char* name, int64_t value) {
     e->async_results = value != 0;
     if (e->async_results) {  // second set of the packed result buffers, allocated here rather than inside a tick
       CK(cudaSetDevice(e->device));
-      if (!e->d_hdr_alt) CK(cudaMalloc(&e->d_hdr_alt, (size_t)e->max_lobbies * sizeof(mm_lobby_hdr)));
-      if (!e->d_members32) CK(cudaMalloc(&e->d_members32, ((size_t)e->capacity + 64) * 4));
-      if (!e->d_members32_alt) CK(cudaMalloc(&e->d_members32_alt, ((size_t)e->capacity + 64) * 4));
+      CK(e->d_hdr_alt.reserve(e->max_lobbies));
+      CK(e->d_members32.reserve((size_t)e->capacity + 64));
+      CK(e->d_members32_alt.reserve((size_t)e->capacity + 64));
     }
     return MM_OK;
   }
@@ -1533,19 +1539,10 @@ int mm_enqueue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rati
     CK(cudaMemcpyAsync(e->d_in_mode + base, mode + base, (size_t)cnt, cudaMemcpyHostToDevice, e->copy_stream));
     if (enq_ts)
       CK(cudaMemcpyAsync(e->d_in_ts + base, enq_ts + base, (size_t)cnt * 4, cudaMemcpyHostToDevice, e->copy_stream));
-    CK(cudaEventRecord(e->ev_copy, e->copy_stream));
-    CK(cudaStreamWaitEvent(e->stream, e->ev_copy, 0));
-    return MM_OK;
+    return copy_fence(e);
   };
-  rc = enqueue_batch(e, n, e->d_in_id, e->d_in_rating, e->d_in_mode, enq_ts ? e->d_in_ts : nullptr, kEnqChunk, upload);
-  if (rc) { cudaStreamSynchronize(e->copy_stream); return rc; }
-  rc = enq_finish(e, n, nullptr, nullptr);
-  if (rc) return rc;
-  if (accepted) {
-    CK(cudaMemcpyAsync(accepted, e->d_code, n, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
-  }
-  return MM_OK;
+  rc = enqueue_batch(e, n, e->d_in_id, e->d_in_rating, e->d_in_mode, enq_ts ? e->d_in_ts.p : nullptr, kEnqChunk, upload);
+  return enq_finish_host(e, rc, e->copy_stream, n, accepted, nullptr);
 }
 
 int mm_enqueue_packed(mm_engine* e, uint32_t n, const uint32_t* handle, const uint16_t* key, const uint32_t* enq_ts,
@@ -1561,41 +1558,28 @@ int mm_enqueue_packed(mm_engine* e, uint32_t n, const uint32_t* handle, const ui
     CK(cudaMemcpyAsync(e->d_in_key + base, key + base, (size_t)cnt * 2, cudaMemcpyHostToDevice, e->copy_stream));
     if (enq_ts)
       CK(cudaMemcpyAsync(e->d_in_ts + base, enq_ts + base, (size_t)cnt * 4, cudaMemcpyHostToDevice, e->copy_stream));
-    CK(cudaEventRecord(e->ev_copy, e->copy_stream));
-    CK(cudaStreamWaitEvent(e->stream, e->ev_copy, 0));
+    int r = copy_fence(e);
+    if (r) return r;
     k_unpack<<<(cnt + 255) / 256, 256, 0, e->stream>>>(cnt, e->d_in_handle + base, e->d_in_key + base, e->d_in_id + base,
                                                        e->d_in_rating + base, e->d_in_mode + base);
     CK(cudaGetLastError());
     return MM_OK;
   };
-  rc = enqueue_batch(e, n, e->d_in_id, e->d_in_rating, e->d_in_mode, enq_ts ? e->d_in_ts : nullptr, kEnqChunk, upload);
-  if (rc) { cudaStreamSynchronize(e->copy_stream); return rc; }
-  rc = enq_finish(e, n, nullptr, nullptr);
-  if (rc) return rc;
-  if (accepted) {
-    CK(cudaMemcpyAsync(accepted, e->d_code, n, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
-  }
-  return MM_OK;
+  rc = enqueue_batch(e, n, e->d_in_id, e->d_in_rating, e->d_in_mode, enq_ts ? e->d_in_ts.p : nullptr, kEnqChunk, upload);
+  return enq_finish_host(e, rc, e->copy_stream, n, accepted, nullptr);
 }
 
 int mm_enqueue_packed_begin(mm_engine* e, uint32_t n, const uint32_t* handle, const uint16_t* key, const uint32_t* enq_ts) {
   if (!e || !n || !handle || !key) return MM_E_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
   CK(cudaSetDevice(e->device));
-  if (e->stage_count == 2) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "both staging slots hold a batch: call mm_enqueue_packed_end first");
-    return MM_E_STATE;
-  }
+  if (e->stage_count == 2)
+    return set_err(e, MM_E_STATE, "both staging slots hold a batch: call mm_enqueue_packed_end first");
   mm_engine::Stage& st = e->stage[(e->stage_head + e->stage_count) & 1];
-  if (n > st.cap) {  // the slot's previous batch was consumed by an _end that synchronised the engine stream
-    cudaFree(st.handle); cudaFree(st.key); cudaFree(st.ts);
-    st.handle = nullptr; st.key = nullptr; st.ts = nullptr; st.cap = 0;
-    CK(cudaMalloc(&st.handle, ((size_t)n + 64) * 4));
-    CK(cudaMalloc(&st.key, ((size_t)n + 64) * 2));
-    CK(cudaMalloc(&st.ts, ((size_t)n + 64) * 4));
-    st.cap = n;
-  }
+  // (a slot's previous batch was consumed by an _end that synchronised the engine stream: it may be reallocated)
+  CK(st.handle.reserve((size_t)n + 64));
+  CK(st.key.reserve((size_t)n + 64));
+  CK(st.ts.reserve((size_t)n + 64));
   if (!st.ready) CK(cudaEventCreateWithFlags(&st.ready, cudaEventDisableTiming));
   CK(cudaMemcpyAsync(st.handle, handle, (size_t)n * 4, cudaMemcpyHostToDevice, e->copy_stream));
   CK(cudaMemcpyAsync(st.key, key, (size_t)n * 2, cudaMemcpyHostToDevice, e->copy_stream));
@@ -1610,10 +1594,7 @@ int mm_enqueue_packed_end(mm_engine* e, uint8_t* accepted, uint32_t* n_accepted)
   if (!e) return MM_E_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
   CK(cudaSetDevice(e->device));
-  if (e->stage_count == 0) {
-    std::snprintf(e->last_err, sizeof(e->last_err), "no staged batch: call mm_enqueue_packed_begin first");
-    return MM_E_STATE;
-  }
+  if (e->stage_count == 0) return set_err(e, MM_E_STATE, "no staged batch: call mm_enqueue_packed_begin first");
   mm_engine::Stage& st = e->stage[e->stage_head];
   e->stage_head ^= 1; --e->stage_count;  // the slot is released whatever happens below
   const uint32_t n = st.n;
@@ -1626,15 +1607,8 @@ int mm_enqueue_packed_end(mm_engine* e, uint8_t* accepted, uint32_t* n_accepted)
     CK(cudaGetLastError());
     return MM_OK;
   };
-  rc = enqueue_batch(e, n, e->d_in_id, e->d_in_rating, e->d_in_mode, st.has_ts ? st.ts : nullptr, kEnqChunkDev, unpack);
-  if (rc) { cudaStreamSynchronize(e->stream); return rc; }
-  rc = enq_finish(e, n, nullptr, n_accepted);
-  if (rc) return rc;
-  if (accepted) {
-    CK(cudaMemcpyAsync(accepted, e->d_code, n, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaStreamSynchronize(e->stream));
-  }
-  return MM_OK;
+  rc = enqueue_batch(e, n, e->d_in_id, e->d_in_rating, e->d_in_mode, st.has_ts ? st.ts.p : nullptr, kEnqChunkDev, unpack);
+  return enq_finish_host(e, rc, e->stream, n, accepted, n_accepted);
 }
 
 int mm_enqueue_rejects(mm_engine* e, uint32_t cap, uint32_t* index, uint8_t* code, uint32_t* n_rejects) {
@@ -1644,19 +1618,15 @@ int mm_enqueue_rejects(mm_engine* e, uint32_t cap, uint32_t* index, uint8_t* cod
   *n_rejects = 0;
   const uint32_t n = e->last_batch_n;
   if (n == 0) return MM_OK;
-  if (cap > e->rej_cap) {
-    cudaFree(e->d_rej_idx); cudaFree(e->d_rej_code);
-    e->rej_cap = 0;
-    CK(cudaMalloc(&e->d_rej_idx, (size_t)cap * 4));
-    CK(cudaMalloc(&e->d_rej_code, (size_t)cap));
-    e->rej_cap = cap;
-  }
-  CK(cudaMemsetAsync(e->d_small + 4, 0, 4, e->stream));
-  k_compact_rejects<<<(n + 255) / 256, 256, 0, e->stream>>>(n, e->d_code, cap, e->d_rej_idx, e->d_rej_code, e->d_small + 4);
+  CK(e->d_rej_idx.reserve(cap));
+  CK(e->d_rej_code.reserve(cap));
+  CK(cudaMemsetAsync(&e->d_cnt->rejects, 0, 4, e->stream));
+  k_compact_rejects<<<(n + 255) / 256, 256, 0, e->stream>>>(n, e->d_code, cap, e->d_rej_idx, e->d_rej_code,
+                                                             &e->d_cnt->rejects);
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(e->h_small + 4, e->d_small + 4, 4, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  const uint32_t cnt = e->h_small[4];
+  int rc = read_counters(e);
+  if (rc) return rc;
+  const uint32_t cnt = e->h_cnt->rejects;
   *n_rejects = cnt;
   const uint32_t m = std::min(cnt, cap);
   if (m) {
@@ -1668,48 +1638,11 @@ int mm_enqueue_rejects(mm_engine* e, uint32_t cap, uint32_t* index, uint8_t* cod
 }
 
 int mm_remove(mm_engine* e, uint32_t n, const uint64_t* id, uint32_t* n_removed) {
-  if (n_removed) *n_removed = 0;
-  if (!e || (n && !id)) return MM_E_ARG;
-  if (!e->use_active) return MM_E_STATE;
-  if (n == 0) return MM_OK;
-  std::lock_guard<std::mutex> lk(e->mu);
-  CK(cudaSetDevice(e->device));
-  int rc = ensure_enq_scratch(e, n);
-  if (rc) return rc;
-  const Pool& p = e->pool[e->cur];
-  CK(cudaMemcpyAsync(e->d_in_id, id, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemsetAsync(e->d_small, 0, 16, e->stream));
-  k_remove<<<(n + 255) / 256, 256, 0, e->stream>>>(n, e->d_in_id, act_view(e), p.v, p.m, (uint32_t)pool_slots(e), e->gen, e->K,
-                                                   e->d_bin_seg, e->d_seg_bin_lo, e->d_small + 2);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(e->h_small, e->d_small, 16, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  const uint32_t rem = e->h_small[2];
-  e->n_active -= std::min<uint64_t>(rem, e->n_active);
-  if (!e->dense_ids) e->n_tomb += rem;
-  if (n_removed) *n_removed = rem;
-  return MM_OK;
+  return remove_or_take(e, n, id, n_removed, false);
 }
 
 int mm_take(mm_engine* e, uint32_t n, const uint64_t* id, uint32_t* n_taken) {
-  if (n_taken) *n_taken = 0;
-  if (!e || (n && !id)) return MM_E_ARG;
-  if (!e->use_active) return MM_E_STATE;
-  if (n == 0) return MM_OK;
-  std::lock_guard<std::mutex> lk(e->mu);
-  CK(cudaSetDevice(e->device));
-  int rc = ensure_enq_scratch(e, n);
-  if (rc) return rc;
-  const Pool& p = e->pool[e->cur];
-  CK(cudaMemcpyAsync(e->d_in_id, id, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemsetAsync(e->d_small, 0, 16, e->stream));
-  k_take<<<(n + 255) / 256, 256, 0, e->stream>>>(n, e->d_in_id, act_view(e), p.v, p.m, (uint32_t)pool_slots(e), e->gen, e->K,
-                                                 e->d_bin_seg, e->d_seg_bin_lo, e->d_small + 2);
-  CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(e->h_small, e->d_small, 16, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  if (n_taken) *n_taken = e->h_small[2];
-  return MM_OK;
+  return remove_or_take(e, n, id, n_taken, true);
 }
 
 int mm_remove_packed(mm_engine* e, uint32_t n, const uint32_t* handle, uint32_t* n_removed) {
@@ -1857,7 +1790,7 @@ int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap,
   if (cap < n_cut) return MM_E_CAP;
   CK(cudaSetDevice(e->device));
   const size_t bytes = (size_t)n_cut * sizeof(mm_queue_stat);
-  if (!e->d_qstat) CK(cudaMalloc(&e->d_qstat, bytes));
+  CK(e->d_qstat.reserve(bytes / 4));
   CK(cudaMemsetAsync(e->d_qstat, 0, bytes, e->stream));
   StatArgs a{};
   const Pool& p = e->pool[e->cur];
@@ -1865,12 +1798,8 @@ int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap,
   const Pool& q = e->pool[e->cur ^ 1];
   a.sec[1] = StatSection{q.v.mode, q.v.ts, q.m, e->d_left_bits, e->tick_now};
   a.n_segs = e->n_segs; a.part_cut = e->d_part_cut; a.out = e->d_qstat;
-  // CTAs: at most the tiles in use (the host-side player counts bound them), at most 8 per SM; each takes a
-  // contiguous run of tiles
   const uint32_t n_max = std::max(p.n, e->match_valid ? e->match_n : 0u);
-  const uint64_t tiles = (uint64_t)n_max / kTile + e->n_segs;
-  const uint32_t ctas = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>(tiles, 8ull * (uint32_t)e->n_sms));
-  k_queue_stats<kStatBlock><<<dim3(ctas, e->match_valid ? 2 : 1), kStatBlock, 0, e->stream>>>(a);
+  k_queue_stats<kStatBlock><<<dim3(tile_ctas(e, n_max), e->match_valid ? 2 : 1), kStatBlock, 0, e->stream>>>(a);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, e->d_qstat, bytes, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
@@ -1951,7 +1880,7 @@ int mm_snapshot(mm_engine* e) {
   int rc = copy_pool(e, e->snap, e->pool[e->cur]);
   if (rc) return rc;
   if (e->use_active) {  // the active set as it stands: ids queued, matched and not yet removed, tombstones
-    if (!e->snap_tab.kv) CK(cudaMalloc(&e->snap_tab.kv, table_bytes(e)));
+    CK(e->snap_tab.kv.reserve(table_bytes(e) / 8));
     CK(cudaMemcpyAsync(e->snap_tab.kv, e->tab[e->tcur].kv, table_bytes(e), cudaMemcpyDeviceToDevice, e->stream));
     e->snap_active = e->n_active;
     e->snap_tomb = e->n_tomb;

@@ -173,6 +173,40 @@ struct ImgLoadArgs {
   uint32_t* err;
 };
 
+// Image player i as k_img_load and k_mrg_order check it.  p: its partition, the last whose first index in s_off is
+// <= i (empty ones share it); u: its enqueue order, the distance of its sequence number above seq_next (0 is seq_next
+// itself); bin: its sort key (valid when bad has no kImgBadMode); bad: the kImg* bits of the checks it fails.
+struct ImgPlayer {
+  uint64_t pid;
+  int32_t rt;
+  uint32_t p, md, u, bin, bad;
+};
+__device__ __forceinline__ ImgPlayer img_player(const ImgCols& in, uint32_t i, const uint32_t* s_off, uint32_t n_segs,
+                                                const BinMap& bm, const uint8_t* grp_lut, const uint16_t* bin_seg,
+                                                uint32_t n_modes, uint32_t seq_next, uint64_t id_limit) {
+  ImgPlayer q;
+  uint32_t lo = 0, e = n_segs;
+  while (e - lo > 1) { const uint32_t mid = (lo + e) >> 1; if (s_off[mid] <= i) lo = mid; else e = mid; }
+  q.p = lo;
+  q.pid = img_id(in, i);
+  q.md = in.mode[i];
+  q.rt = in.rating[i];
+  q.u = in.seq[i] - seq_next;
+  q.bin = 0;
+  q.bad = 0;
+  if (q.pid >= id_limit) q.bad |= kImgBadId;
+  if (q.md >= n_modes) {
+    q.bad |= kImgBadMode;
+  } else {
+    const int32_t hi = bm.key_lo + (int32_t)bm.KR - 1;
+    const int32_t r = q.rt < bm.key_lo ? bm.key_lo : (q.rt > hi ? hi : q.rt);
+    q.bin = bin_of(bm, bm.lut, q.rt, q.md);
+    if (grp_lut[r - bm.key_lo] == 0xFF || bin_seg[q.bin] != q.p) q.bad |= kImgBadRating;
+  }
+  if (q.u == 0 || (i + 1 < s_off[q.p + 1] && in.seq[i + 1] - seq_next <= q.u)) q.bad |= kImgBadSeq;
+  return q;
+}
+
 // One image player per thread: check it, then write its slot (nothing is written for a player that fails a check).
 __global__ void __launch_bounds__(256) k_img_load(const ImgLoadArgs a) {
   __shared__ uint32_t s_off[kMaxSegs + 1], s_base[kMaxSegs];
@@ -181,32 +215,16 @@ __global__ void __launch_bounds__(256) k_img_load(const ImgLoadArgs a) {
     if (p < a.n_segs) s_base[p] = a.slot_base[p];
   }
   __syncthreads();
-  const int32_t hi = a.bm.key_lo + (int32_t)a.bm.KR - 1;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += gridDim.x * blockDim.x) {
-    uint32_t lo = 0, e = a.n_segs;  // the last partition whose first index is <= i (empty ones share it)
-    while (e - lo > 1) { const uint32_t mid = (lo + e) >> 1; if (s_off[mid] <= i) lo = mid; else e = mid; }
-    const uint32_t p = lo;
-    const uint64_t pid = img_id(a.in, i);
-    const uint32_t md = a.in.mode[i];
-    const int32_t rt = a.in.rating[i];
-    const uint32_t u = a.in.seq[i] - a.seq_next;  // enqueue order = this distance ascending; 0 is seq_next itself
-    uint32_t bad = 0, bin = 0;
-    if (pid >= a.id_limit) bad |= kImgBadId;
-    if (md >= a.n_modes) {
-      bad |= kImgBadMode;
-    } else {
-      const int32_t r = rt < a.bm.key_lo ? a.bm.key_lo : (rt > hi ? hi : rt);
-      bin = bin_of(a.bm, a.bm.lut, rt, md);
-      if (a.grp_lut[r - a.bm.key_lo] == 0xFF || a.bin_seg[bin] != p) bad |= kImgBadRating;
-    }
-    if (u == 0 || (i + 1 < s_off[p + 1] && a.in.seq[i + 1] - a.seq_next <= u)) bad |= kImgBadSeq;
-    if (bad) { atomicOr(a.err, bad); continue; }
-    const uint32_t slot = s_base[p] + (i - s_off[p]);
-    a.pool.id[slot] = pid; a.pool.rating[slot] = rt; a.pool.mode[slot] = (uint8_t)md;
-    a.pool.tsize[slot] = a.mode_tsize[md]; a.pool.ts[slot] = a.in.ts[i];
-    a.pool.bin[slot] = (uint16_t)bin; a.pool.seq[slot] = a.in.seq[i];
-    atomicAdd(&a.meta.tot[bin], 1u);
-    if (a.meta.chist) atomicAdd(&a.meta.chist[(size_t)(slot / kTile) * kChunkHist + (bin - a.seg_bin_lo[p])], 1u);
+    const ImgPlayer q =
+        img_player(a.in, i, s_off, a.n_segs, a.bm, a.grp_lut, a.bin_seg, a.n_modes, a.seq_next, a.id_limit);
+    if (q.bad) { atomicOr(a.err, q.bad); continue; }
+    const uint32_t slot = s_base[q.p] + (i - s_off[q.p]);
+    a.pool.id[slot] = q.pid; a.pool.rating[slot] = q.rt; a.pool.mode[slot] = (uint8_t)q.md;
+    a.pool.tsize[slot] = a.mode_tsize[q.md]; a.pool.ts[slot] = a.in.ts[i];
+    a.pool.bin[slot] = (uint16_t)q.bin; a.pool.seq[slot] = a.in.seq[i];
+    atomicAdd(&a.meta.tot[q.bin], 1u);
+    if (a.meta.chist) atomicAdd(&a.meta.chist[(size_t)(slot / kTile) * kChunkHist + (q.bin - a.seg_bin_lo[q.p])], 1u);
   }
 }
 
@@ -265,26 +283,11 @@ __global__ void __launch_bounds__(256) k_mrg_order(const MrgOrderArgs a) {
   __shared__ uint32_t s_off[kMaxSegs + 1];
   for (uint32_t p = threadIdx.x; p <= a.n_segs; p += blockDim.x) s_off[p] = a.part_off[p];
   __syncthreads();
-  const int32_t hi = a.bm.key_lo + (int32_t)a.bm.KR - 1;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += gridDim.x * blockDim.x) {
-    uint32_t lo = 0, e = a.n_segs;  // the last partition whose first index is <= i (empty ones share it)
-    while (e - lo > 1) { const uint32_t mid = (lo + e) >> 1; if (s_off[mid] <= i) lo = mid; else e = mid; }
-    const uint32_t p = lo;
-    const uint64_t pid = img_id(a.in, i);
-    const uint32_t md = a.in.mode[i];
-    const int32_t rt = a.in.rating[i];
-    const uint32_t u = a.in.seq[i] - a.seq_next;
-    uint32_t bad = 0;
-    if (pid >= a.id_limit) bad |= kImgBadId;
-    if (md >= a.n_modes) {
-      bad |= kImgBadMode;
-    } else {
-      const int32_t r = rt < a.bm.key_lo ? a.bm.key_lo : (rt > hi ? hi : rt);
-      if (a.grp_lut[r - a.bm.key_lo] == 0xFF || a.bin_seg[bin_of(a.bm, a.bm.lut, rt, md)] != p) bad |= kImgBadRating;
-    }
-    if (u == 0 || (i + 1 < s_off[p + 1] && a.in.seq[i + 1] - a.seq_next <= u)) bad |= kImgBadSeq;
-    if (bad) { atomicOr(a.err, bad); continue; }
-    const uint32_t c = a.part_cut[p], q0 = a.cut_lp_lo[c], q1 = a.cut_lp_lo[c + 1];
+    const ImgPlayer x =
+        img_player(a.in, i, s_off, a.n_segs, a.bm, a.grp_lut, a.bin_seg, a.n_modes, a.seq_next, a.id_limit);
+    if (x.bad) { atomicOr(a.err, x.bad); continue; }
+    const uint32_t p = x.p, c = a.part_cut[p], q0 = a.cut_lp_lo[c], q1 = a.cut_lp_lo[c + 1];
     uint32_t pos = s_off[q0] + (i - s_off[p]);
     for (uint32_t q = q0; q < q1; ++q) {
       if (q == p) continue;
@@ -292,11 +295,11 @@ __global__ void __launch_bounds__(256) k_mrg_order(const MrgOrderArgs a) {
       while (l < r) {
         const uint32_t mid = (l + r) >> 1;
         const uint32_t v = a.in.seq[mid] - a.seq_next;
-        if (v < u || (q < p && v == u)) l = mid + 1; else r = mid;
+        if (v < x.u || (q < p && v == x.u)) l = mid + 1; else r = mid;
       }
       pos += l - s_off[q];
     }
-    a.out_id[pos] = pid; a.out_rating[pos] = rt; a.out_mode[pos] = (uint8_t)md; a.out_ts[pos] = a.in.ts[i];
+    a.out_id[pos] = x.pid; a.out_rating[pos] = x.rt; a.out_mode[pos] = (uint8_t)x.md; a.out_ts[pos] = a.in.ts[i];
     a.src[pos] = i;
   }
 }
