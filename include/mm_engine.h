@@ -188,6 +188,46 @@ int mm_remove_packed(mm_engine* e, uint32_t n, const uint32_t* handle, uint32_t*
  * the lobby stage removes them (game-lobby/worker.ex:80).  Ids that are not queued are ignored.               */
 int mm_take(mm_engine* e, uint32_t n, const uint64_t* id, uint32_t* n_taken);
 
+/* EXTENSION (cross-group boundary pass on the device, DESIGN.md §6): the band gather and the band walk of
+ * shard.boundary_pass without reading the pool to the host.  Both calls need what shard.check_bands needs: W >= 0,
+ * MM_ORDER_RATING, contiguous ascending groups, each at least 2W wide (else MM_E_ARG); MM_E_STATE with a staged
+ * packed batch or on an MM_F_NO_DEDUPE engine.  Every refusal is decided before anything changes and sets
+ * mm_last_error.  A player whose rating lies outside every group (a default-group fallback) is never a candidate.
+ *
+ * mm_band_candidates: the upper side of the boundary group-1 | group (1 <= group < n_groups, else MM_E_ARG): the live
+ * queued players of group g with rating in (hi_{g-1}, hi_{g-1} + W], sorted by (mode, rating, enqueue order) — what a
+ * rank sends to the owner of group g-1.  MM_E_CAP (and *n_out = the count) if cap is smaller; cap = 0 is a dry run.
+ * Reads only the key column of the partitions that hold band keys; nothing changes.                              */
+int mm_band_candidates(mm_engine* e, int32_t W, uint32_t group, uint64_t* ids, int32_t* rating, uint8_t* mode,
+                       uint32_t cap, uint32_t* n_out);
+
+typedef struct mm_band_stats {
+  uint32_t n_lobbies, n_matched; /* boundary lobbies and their members                         */
+  uint32_t n_taken;              /* local players taken out of this pool                       */
+  uint32_t n_upper_taken;        /* upper-side candidates given by the caller and consumed     */
+  float device_us;               /* CUDA-event time of the call's device work                  */
+  uint32_t reserved[3];
+} mm_band_stats; /* 32 bytes */
+
+/* mm_band_match: the bands of the boundaries g|g+1 for g_first <= g <= g_last < n_groups - 1, every mode.  Band
+ * (g, m): the live queued players of group g with rating in (hi_g - W, hi_g] and those of group g+1 with rating in
+ * (hi_g, hi_g + W], matched by the S1 windowed walk (orc_run_windowed) in (rating, enqueue order) — the tick's walk
+ * (mm_scan.cuh), run on the band's per-rating counts.  The upper side of boundary g_last|g_last+1 comes from the
+ * caller's columns when upper_remote != 0 (another rank's mm_band_candidates; n_upper may be 0), otherwise from this
+ * engine.  lobbies: ordered by (g, mode, emission), group = the LOWER group g, first_member into member_ids, members
+ * in join order.  Local matched players leave the pool in the same call exactly as mm_take takes them (they stay in
+ * the active set; the last tick's match section of mm_queue_stats is unaffected); upper_taken[i] = 1 for every
+ * caller-given candidate a lobby consumed (the caller hands those ids back to the owner's mm_take).
+ * MM_E_ARG also for: a boundary range out of bounds; upper columns without upper_remote, on an MM_F_DENSE_IDS engine
+ * (another engine's handles are not ids here), not sorted by (mode, rating), with a rating outside
+ * (hi_{g_last}, hi_{g_last} + W] or a mode >= n_modes (checked on the device).  MM_E_CAP if lobby_cap or member_cap
+ * is too small: stats then holds the counts and nothing is taken (zero capacities: a dry run).  Only candidates,
+ * headers, members and upper_taken cross PCIe.                                                                  */
+int mm_band_match(mm_engine* e, int32_t W, uint32_t g_first, uint32_t g_last, uint32_t upper_remote,
+                  const uint64_t* up_ids, const int32_t* up_rating, const uint8_t* up_mode, uint32_t n_upper,
+                  mm_lobby_hdr* lobbies, uint32_t lobby_cap, uint64_t* member_ids, uint64_t member_cap,
+                  uint8_t* upper_taken, mm_band_stats* stats);
+
 /* Replaces ActiveUser.in_queue?/1 (models/active_user.ex:33-44), batched.          */
 int mm_in_queue(mm_engine* e, uint32_t n, const uint64_t* id, uint8_t* out);
 

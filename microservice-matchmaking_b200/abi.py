@@ -72,6 +72,18 @@ class TickStats(C.Structure):
     ]
 
 
+class BandStats(C.Structure):
+    """mm_band_stats: counts of one mm_band_match call (32 bytes)."""
+    _fields_ = [
+        ("n_lobbies", C.c_uint32),
+        ("n_matched", C.c_uint32),
+        ("n_taken", C.c_uint32),
+        ("n_upper_taken", C.c_uint32),
+        ("device_us", C.c_float),
+        ("reserved", C.c_uint32 * 3),
+    ]
+
+
 MM_WAIT_BUCKETS = 120
 
 
@@ -142,6 +154,9 @@ PROTOTYPES = {
     "mm_remove": (C.c_int, [_vp, C.c_uint32, _vp, _P(C.c_uint32)]),
     "mm_remove_packed": (C.c_int, [_vp, C.c_uint32, _vp, _P(C.c_uint32)]),
     "mm_take": (C.c_int, [_vp, C.c_uint32, _vp, _P(C.c_uint32)]),
+    "mm_band_candidates": (C.c_int, [_vp, C.c_int32, C.c_uint32, _vp, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
+    "mm_band_match": (C.c_int, [_vp, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, _vp, _vp, _vp, C.c_uint32,
+                                _vp, C.c_uint32, _vp, C.c_uint64, _vp, _P(BandStats)]),
     "mm_in_queue": (C.c_int, [_vp, C.c_uint32, _vp, _vp]),
     "mm_pool_size": (C.c_int, [_vp, _P(C.c_uint32)]),
     "mm_active_size": (C.c_int, [_vp, _P(C.c_uint32)]),

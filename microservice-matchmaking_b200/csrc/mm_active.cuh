@@ -360,6 +360,19 @@ __global__ void k_remove(uint32_t n, const uint64_t* __restrict__ id, ActiveView
   atomicAdd(n_removed, 1u);
 }
 
+// A queued slot leaves the pool the way mm_take takes it (its active-set entry is left as it is); false if it was dead
+// already.  A twin in the same batch must not count twice: the mode byte is the claim.
+__device__ __forceinline__ bool pool_take_slot(PoolView pool, const PoolMeta& meta, uint32_t slot, uint32_t dead_bin,
+                                               const uint16_t* __restrict__ bin_seg,
+                                               const uint32_t* __restrict__ seg_bin_lo) {
+  const uint32_t word = slot & ~3u, sh = (slot & 3u) * 8;
+  uint32_t* mw = reinterpret_cast<uint32_t*>(pool.mode + word);
+  const uint32_t old = atomicOr(mw, 0xFFu << sh);
+  if (((old >> sh) & 0xFFu) == MM_MODE_DEAD) return false;
+  pool_mark_dead(pool, meta, slot, dead_bin, bin_seg, seg_bin_lo);
+  return true;
+}
+
 // mm_take: queued players matched OUTSIDE this engine's tick (the cross-group boundary pass, shard.py) leave the pool
 // but stay in the active set — exactly like members of an emitted lobby, who are "in the queue" until the lobby stage
 // removes them (game-lobby/worker.ex:80).
@@ -373,15 +386,9 @@ __global__ void k_take(uint32_t n, const uint64_t* __restrict__ id, ActiveView a
   if (h == ~0ull) return;
   const unsigned long long v = *act.val(h);
   const uint32_t slot = (uint32_t)v, g = (uint32_t)(v >> 32);
-  if (v < kPending && g == gen && slot < n_slots && pool.id[slot] == pid) {
-    // a twin in the same batch must not count twice: the mode byte is the claim
-    const uint32_t word = slot & ~3u, sh = (slot & 3u) * 8;
-    uint32_t* mw = reinterpret_cast<uint32_t*>(pool.mode + word);
-    const uint32_t old = atomicOr(mw, 0xFFu << sh);
-    if (((old >> sh) & 0xFFu) == MM_MODE_DEAD) return;
-    pool_mark_dead(pool, meta, slot, dead_bin, bin_seg, seg_bin_lo);
+  if (v < kPending && g == gen && slot < n_slots && pool.id[slot] == pid &&
+      pool_take_slot(pool, meta, slot, dead_bin, bin_seg, seg_bin_lo))
     atomicAdd(n_taken, 1u);
-  }
 }
 
 // ActiveUser.in_queue?/1 (models/active_user.ex:33-44), batched.

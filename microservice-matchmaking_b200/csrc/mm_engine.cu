@@ -19,6 +19,7 @@
 #include <utility>
 #include <vector>
 
+#include "mm_band.cuh"
 #include "mm_expire.cuh"
 #include "mm_image.cuh"
 #include "mm_kernels.cuh"
@@ -231,6 +232,18 @@ struct mm_engine {
   DevArray<uint32_t> d_mrg_src;       // merge batch index -> image index
   DevArray<uint8_t> d_mrg_code;       // the merge batch's ingest codes (d_code keeps the last mm_enqueue* batch's)
   DevArray<unsigned long long> d_mrg_seen;  // duplicate count: scratch id set
+
+  // mm_band_candidates / mm_band_match (mm_band.cuh): sized by the band keys and the candidates, grown on demand
+  struct Band {
+    DevArray<uint32_t> map, fill, qoff, qtiles, M, tot, pos, kbase, klim, band_mb, band_lb, rstart, ctr;
+    DevArray<uint64_t> id;        // candidate ids / members
+    DevArray<int32_t> rating;     // candidate ratings
+    DevArray<uint8_t> mode;       // candidate modes
+    DevArray<uint64_t> up_id;     // the caller's upper-side columns
+    DevArray<int32_t> up_rating;
+    DevArray<uint8_t> up_mode, up_taken;
+    DevArray<mm_lobby_hdr> hdr;
+  } band;
 };
 
 namespace {
@@ -1335,6 +1348,160 @@ int remove_or_take(mm_engine* e, uint32_t n, const uint64_t* id, uint32_t* n_out
   return MM_OK;
 }
 
+// ---- boundary pass: mm_band_candidates / mm_band_match (mm_band.cuh) ----------------------------------------------
+// The refusals both calls share (shard.check_bands' rules, then the engine's state).
+int band_check(mm_engine* e, int32_t W) {
+  const mm_config& c = e->cfg;
+  if (W < 0) return set_err(e, MM_E_ARG, "W must be >= 0");
+  if (c.order_mode != MM_ORDER_RATING) return set_err(e, MM_E_ARG, "the boundary pass needs MM_ORDER_RATING");
+  for (uint32_t g = 0; g < c.n_groups; ++g) {
+    if ((int64_t)c.group_hi[g] - c.group_lo[g] + 1 < 2 * (int64_t)W)
+      return set_err(e, MM_E_ARG, "rating group %u is narrower than 2 x W: boundary bands would overlap", g);
+    if (g && (int64_t)c.group_lo[g] != (int64_t)c.group_hi[g - 1] + 1)
+      return set_err(e, MM_E_ARG, "the boundary pass needs contiguous ascending rating groups");
+  }
+  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (!e->use_active) return set_err(e, MM_E_STATE, "an MM_F_NO_DEDUPE engine cannot take matched players");
+  return MM_OK;
+}
+
+uint32_t band_ctas(const mm_engine* e, uint32_t n) {
+  return std::max<uint32_t>(1, std::min<uint32_t>((tile_count(e, n) + kBandWarps - 1) / kBandWarps, 4u * (uint32_t)e->n_sms));
+}
+
+// Arguments and scratch of one call: n_bounds boundaries from g_first | g_first+1, every mode.  Every scratch array is
+// sized by the band keys, the candidates or the per-key tile counts; none by the pool's capacity.
+int band_setup(mm_engine* e, int32_t W, uint32_t g_first, uint32_t n_bounds, bool skip_lower, bool remote_last,
+               BandArgs& a) {
+  const mm_config& c = e->cfg;
+  const Pool& p = e->pool[e->cur];
+  auto& s = e->band;
+  a = BandArgs{};
+  a.pool = p.v; a.meta = p.m; a.fill = p.m.fill;
+  a.n_segs = e->n_segs; a.K = e->K; a.bm = bin_map(e); a.bin_seg = e->d_bin_seg; a.seg_bin_lo = e->d_seg_bin_lo;
+  a.W = W; a.n_modes = c.n_modes; a.g_first = g_first; a.n_bands = n_bounds * c.n_modes;
+  a.n_keys = a.n_bands * 2u * (uint32_t)W;
+  a.skip_lower = skip_lower; a.remote_last = remote_last;
+  for (uint32_t g = 0; g < c.n_groups; ++g) a.hi[g] = c.group_hi[g];
+  for (uint32_t m = 0; m < c.n_modes; ++m) a.L[m] = (uint32_t)c.modes[m].teams * c.modes[m].team_size;
+  const size_t nk = std::max<size_t>(a.n_keys, 1);
+  const size_t cols = (size_t)tile_count(e, p.n) * std::min<uint32_t>(e->max_nb, 2u * (uint32_t)W);
+  CK(s.map.reserve(e->Kp)); CK(s.fill.reserve(e->n_segs)); CK(s.qoff.reserve(nk + 1)); CK(s.qtiles.reserve(nk));
+  CK(s.M.reserve(std::max<size_t>(cols, 1))); CK(s.tot.reserve(nk)); CK(s.kbase.reserve(nk)); CK(s.klim.reserve(nk));
+  CK(s.rstart.reserve(nk)); CK(s.pos.reserve((size_t)a.n_bands * (2u * (uint32_t)W + 1)));
+  CK(s.band_mb.reserve(a.n_bands + 1)); CK(s.band_lb.reserve(a.n_bands + 1)); CK(s.ctr.reserve(kBcWords));
+  a.meta.fill = s.fill; a.map = s.map; a.bfill = s.fill; a.qoff = s.qoff; a.qtiles = s.qtiles; a.M = s.M; a.tot = s.tot;
+  a.pos = s.pos; a.kbase = s.kbase; a.klim = s.klim; a.band_mb = s.band_mb; a.band_lb = s.band_lb; a.ctr = s.ctr;
+  CK(cudaMemsetAsync(s.ctr, 0, kBcWords * 4, e->stream));
+  CK(cudaMemsetAsync(s.tot, 0, nk * 4, e->stream));
+  if (!a.n_keys) return MM_OK;
+  // gather: bin -> key map and count columns, per-(key, tile) counts, per-key prefixes and totals
+  CK(cudaMemsetAsync(s.map, 0xFF, (size_t)e->Kp * 4, e->stream));
+  CK(cudaMemsetAsync(s.M, 0, std::max<size_t>(cols, 1) * 4, e->stream));
+  k_band_prep<<<1, kBandPrepBlock, 0, e->stream>>>(a);
+  k_band_count<kBandBlock><<<band_ctas(e, p.n), kBandBlock, 0, e->stream>>>(a);
+  k_band_scan<<<(a.n_keys + 7) / 8, 256, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  return MM_OK;
+}
+
+int band_read_ctr(mm_engine* e, uint32_t (&h)[kBcWords]) {
+  CK(cudaMemcpyAsync(h, e->band.ctr, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
+int band_candidates(mm_engine* e, int32_t W, uint32_t group, uint64_t* ids, int32_t* rating, uint8_t* mode,
+                    uint32_t cap, uint32_t* n_out) {
+  int rc = band_check(e, W);
+  if (rc) return rc;
+  if (group == 0 || group >= e->cfg.n_groups)
+    return set_err(e, MM_E_ARG, "group %u has no low boundary: need 1 <= group < n_groups = %u", group, e->cfg.n_groups);
+  if (W == 0) return MM_OK;
+  BandArgs a;
+  if ((rc = band_setup(e, W, group - 1, 1, true, false, a))) return rc;
+  k_band_bases<<<1, kBandWalkBlock, 0, e->stream>>>(a, 0);
+  CK(cudaGetLastError());
+  uint32_t h[kBcWords];
+  if ((rc = band_read_ctr(e, h))) return rc;
+  const uint32_t n = h[kBcKeys];
+  *n_out = n;
+  if (n > cap) return set_err(e, MM_E_CAP, "need cap >= %u", n);
+  if (n == 0) return MM_OK;
+  auto& s = e->band;
+  CK(s.id.reserve(n)); CK(s.rating.reserve(n)); CK(s.mode.reserve(n));
+  k_band_place<kBandBlock><<<band_ctas(e, e->pool[e->cur].n), kBandBlock, 0, e->stream>>>(
+      a, BandOut{s.id, s.rating, s.mode, 0u});
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(ids, s.id, (size_t)n * 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(rating, s.rating, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(mode, s.mode, n, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
+int band_match(mm_engine* e, int32_t W, uint32_t g_first, uint32_t g_last, uint32_t upper_remote, const uint64_t* up_ids,
+               const int32_t* up_rating, const uint8_t* up_mode, uint32_t n_upper, mm_lobby_hdr* lobbies,
+               uint32_t lobby_cap, uint64_t* member_ids, uint64_t member_cap, uint8_t* upper_taken, mm_band_stats* st) {
+  int rc = band_check(e, W);
+  if (rc) return rc;
+  const uint32_t G = e->cfg.n_groups;
+  if (g_first > g_last || g_last + 1 >= G)
+    return set_err(e, MM_E_ARG, "boundaries %u..%u: need g_first <= g_last < n_groups - 1 = %u", g_first, g_last, G - 1);
+  if (!upper_remote && n_upper) return set_err(e, MM_E_ARG, "upper candidates given without upper_remote");
+  if (upper_remote && e->dense_ids)
+    return set_err(e, MM_E_ARG, "upper candidates on an MM_F_DENSE_IDS engine: another engine's handles are not ids here");
+  auto& s = e->band;
+  CK(cudaEventRecord(e->ev[0], e->stream));
+  BandArgs a;
+  if ((rc = band_setup(e, W, g_first, g_last - g_first + 1, false, upper_remote != 0, a))) return rc;
+  if (n_upper) {  // the caller's columns: checked, counted into their keys
+    CK(s.up_id.reserve(n_upper)); CK(s.up_rating.reserve(n_upper)); CK(s.up_mode.reserve(n_upper));
+    CK(s.up_taken.reserve(n_upper));
+    CK(cudaMemcpyAsync(s.up_id, up_ids, (size_t)n_upper * 8, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(s.up_rating, up_rating, (size_t)n_upper * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(s.up_mode, up_mode, n_upper, cudaMemcpyHostToDevice, e->stream));
+    k_band_upper<<<(n_upper + 255) / 256, 256, 0, e->stream>>>(a, n_upper, s.up_rating, s.up_mode, s.rstart);
+  }
+  if (a.n_keys) k_band_bases<<<1, kBandWalkBlock, 0, e->stream>>>(a, 1);
+  CK(cudaGetLastError());
+  uint32_t h[kBcWords];
+  if ((rc = band_read_ctr(e, h))) return rc;
+  if (h[kBcErr] & kBandErrMode) return set_err(e, MM_E_ARG, "an upper candidate's mode is >= n_modes");
+  if (h[kBcErr] & kBandErrRating)
+    return set_err(e, MM_E_ARG, "an upper candidate's rating is outside (%d, %lld]", e->cfg.group_hi[g_last],
+                   (long long)e->cfg.group_hi[g_last] + W);
+  if (h[kBcErr] & kBandErrOrder) return set_err(e, MM_E_ARG, "the upper candidates are not sorted by (mode, rating)");
+  const uint32_t nl = h[kBcLobbies], nm = h[kBcMatched], nu = h[kBcUpper];
+  st->n_lobbies = nl; st->n_matched = nm; st->n_upper_taken = nu; st->n_taken = nm - nu;
+  if (lobby_cap < nl || member_cap < nm)
+    return set_err(e, MM_E_CAP, "need lobby_cap >= %u and member_cap >= %u", nl, nm);
+  // from here on the call changes the pool: the local members are taken as they are placed
+  const uint32_t ctas = band_ctas(e, e->pool[e->cur].n);
+  if (nm) {
+    CK(s.id.reserve(nm));
+    if (nm > nu) k_band_place<kBandBlock><<<ctas, kBandBlock, 0, e->stream>>>(a, BandOut{s.id, nullptr, nullptr, 1u});
+  }
+  if (n_upper)
+    k_band_upper_place<<<(n_upper + 255) / 256, 256, 0, e->stream>>>(a, n_upper, s.up_id, s.up_rating, s.up_mode,
+                                                                     s.rstart, s.id, s.up_taken);
+  if (nl) {
+    CK(s.hdr.reserve(nl));
+    k_band_hdr<<<(nl + 255) / 256, 256, 0, e->stream>>>(a, nl, s.hdr);
+  }
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e->ev[4], e->stream));
+  if (nl) CK(cudaMemcpyAsync(lobbies, s.hdr, (size_t)nl * sizeof(mm_lobby_hdr), cudaMemcpyDeviceToHost, e->stream));
+  if (nm) CK(cudaMemcpyAsync(member_ids, s.id, (size_t)nm * 8, cudaMemcpyDeviceToHost, e->stream));
+  if (n_upper) CK(cudaMemcpyAsync(upper_taken, s.up_taken, n_upper, cudaMemcpyDeviceToHost, e->stream));
+  if ((rc = band_read_ctr(e, h))) return rc;
+  st->n_taken = h[kBcTaken];
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]));
+  st->device_us = ms * 1000.f;
+  return MM_OK;
+}
+
 }  // namespace
 
 // =======================================================================================
@@ -1643,6 +1810,29 @@ int mm_remove(mm_engine* e, uint32_t n, const uint64_t* id, uint32_t* n_removed)
 
 int mm_take(mm_engine* e, uint32_t n, const uint64_t* id, uint32_t* n_taken) {
   return remove_or_take(e, n, id, n_taken, true);
+}
+
+int mm_band_candidates(mm_engine* e, int32_t W, uint32_t group, uint64_t* ids, int32_t* rating, uint8_t* mode,
+                       uint32_t cap, uint32_t* n_out) {
+  if (!e || !n_out || (cap && (!ids || !rating || !mode))) return MM_E_ARG;
+  *n_out = 0;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  return band_candidates(e, W, group, ids, rating, mode, cap, n_out);
+}
+
+int mm_band_match(mm_engine* e, int32_t W, uint32_t g_first, uint32_t g_last, uint32_t upper_remote,
+                  const uint64_t* up_ids, const int32_t* up_rating, const uint8_t* up_mode, uint32_t n_upper,
+                  mm_lobby_hdr* lobbies, uint32_t lobby_cap, uint64_t* member_ids, uint64_t member_cap,
+                  uint8_t* upper_taken, mm_band_stats* stats) {
+  if (!e || !stats || (lobby_cap && !lobbies) || (member_cap && !member_ids) ||
+      (n_upper && (!up_ids || !up_rating || !up_mode || !upper_taken)))
+    return MM_E_ARG;
+  std::memset(stats, 0, sizeof(*stats));
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  return band_match(e, W, g_first, g_last, upper_remote, up_ids, up_rating, up_mode, n_upper, lobbies, lobby_cap,
+                    member_ids, member_cap, upper_taken, stats);
 }
 
 int mm_remove_packed(mm_engine* e, uint32_t n, const uint32_t* handle, uint32_t* n_removed) {

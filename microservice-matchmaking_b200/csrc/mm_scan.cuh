@@ -87,6 +87,37 @@ __host__ __device__ constexpr uint32_t tail_words(uint32_t Kp, uint32_t layout) 
   return kTailScratchWords + (Kp + 2) + ((layout & 1u) ? (Kp + 2) : 0u) + ((layout & 2u) ? (Kp + 3) / 2 : 0u);
 }
 
+// The S1 walk on a histogram (oracle: orc_run_windowed), one bin v of a segment [.., hi) at a time.  bb holds the
+// sorted position of every bin's first player (bb[v + 1] = b1 ends bin v); `keys` indexes like an array of the bins'
+// ascending keys.  Off the carry chain:
+//   reach = sorted position where keys exceed key_v + W (binary search over the segment's keys)
+//   rsel  = min(reach, b1 - 1 + L): the seeds of bin v are cur, cur + L, ... < min(b1, reach - L + 1)
+template <class Keys>
+__device__ __forceinline__ uint32_t s1_rsel(const uint32_t* bb, const Keys& keys, uint32_t v, uint32_t hi, int32_t W,
+                                            uint32_t L, uint32_t b1) {
+  const int32_t lim = (int32_t)keys[v] + W;
+  uint32_t a = v, e = hi;  // last bin in [v, hi) with key <= lim
+  while (e - a > 1) { const uint32_t mid = (a + e) >> 1; if ((int32_t)keys[mid] <= lim) a = mid; else e = mid; }
+  const uint32_t reach = bb[a + 1], cap = b1 - 1 + L;
+  return reach < cap ? reach : cap;
+}
+// On the chain: pos = next unconsumed position; bin [B0, B1) with rsel RS.  With a = RS - cur the bin seeds a / L
+// lobbies and p2 = RS - a mod L is the next unconsumed position (a mod L by a reciprocal multiply, Mrec =
+// 0xFFFFFFFF / L).  -> matched players of the bin (always a prefix of it); pos advances.  An empty or padding bin
+// (B0 = B1 <= pos) leaves pos alone and matches nothing.
+__device__ __forceinline__ uint32_t s1_step(uint32_t& pos, uint32_t B0, uint32_t B1, uint32_t RS, uint32_t L,
+                                            uint32_t Mrec) {
+  const uint32_t cur = pos > B0 ? pos : B0;
+  const uint32_t a = RS - cur;                      // meaningful when cur < B1 (then RS > cur)
+  uint32_t rem = a - __umulhi(a, Mrec) * L;         // a mod L, or a mod L + L
+  rem = rem < rem - L ? rem : rem - L;              // unsigned: picks the one below L
+  const uint32_t p2 = RS - rem;                     // next unconsumed position after this bin's lobbies
+  const bool inside = cur < B1, full = p2 >= B1;
+  const uint32_t m = (!inside || full) ? B1 - B0 : p2 - B0;
+  pos = !inside ? pos : (full ? p2 : B1);           // the rest of a partly matched bin stays queued
+  return m;
+}
+
 // The tail.  One pipeline for both policies:
 //   bin totals -> bases s_bb -> matched prefix of every bin -> member slot of the bin's first player.
 // S0 (reference behaviour): a (mode, group) partition of n players emits floor(n/L) lobbies, the n mod L
@@ -154,11 +185,8 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
     __syncthreads();
     const int32_t W = t.max_spread;
     // One warp walks TWO partitions at a time (two independent carry chains in flight).  Per bin, off the chain:
-    //   reach  = sorted position where keys exceed key_v + W (binary search over the partition's keys)
-    //   rsel   = min(reach, b1 - 1 + L): the seeds of bin v are cur, cur + L, ... < min(b1, reach - L + 1), so with
-    //            a = rsel - cur the bin seeds a / L lobbies and p2 = rsel - a mod L is the next unconsumed position
-    // and on the chain only: cur = max(pos, b0); a; a mod L by a reciprocal multiply; p2; select.  Empty bins
-    // fall out of the same arithmetic (cur >= b1), so the 32 bins of a batch are visited by an unrolled loop.
+    // s1_rsel; on the chain only: s1_step.  Empty bins fall out of the same arithmetic (cur >= b1), so the 32 bins
+    // of a batch are visited by an unrolled loop.
     for (uint32_t sg = tid; sg < n_segs; sg += kScanBlock) s_ns[sg] = s_bb[s_lo[sg + 1]] - s_bb[s_lo[sg]];
     // the walk runs over whole CUT segments (a window may span the partitions of a wide rating group)
     for (uint32_t sg0 = warp; sg0 < t.n_cut; sg0 += 2 * NW) {
@@ -182,11 +210,7 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
           b0[q] = b1[q] = rs[q] = 0u; mine[q] = 0u;
           if (valid[q]) {
             b0[q] = s_bb[v]; b1[q] = s_bb[v + 1];
-            const int32_t lim = (int32_t)keys[v] + W;
-            uint32_t a = v, e = hi[q];  // last bin in [v, hi) with key <= lim
-            while (e - a > 1) { const uint32_t mid = (a + e) >> 1; if ((int32_t)keys[mid] <= lim) a = mid; else e = mid; }
-            const uint32_t reach = s_bb[a + 1], cap = b1[q] - 1 + L[q];
-            rs[q] = reach < cap ? reach : cap;
+            rs[q] = s1_rsel(s_bb, keys, v, hi[q], W, L[q], b1[q]);
           }
         }
 #pragma unroll 8
@@ -195,14 +219,7 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
           for (int q = 0; q < 2; ++q) {
             const uint32_t B0 = __shfl_sync(0xFFFFFFFFu, b0[q], l), B1 = __shfl_sync(0xFFFFFFFFu, b1[q], l);
             const uint32_t RS = __shfl_sync(0xFFFFFFFFu, rs[q], l);
-            const uint32_t cur = pos[q] > B0 ? pos[q] : B0;
-            const uint32_t a = RS - cur;                      // meaningful when cur < B1 (then RS > cur)
-            uint32_t rem = a - __umulhi(a, Mrec[q]) * L[q];   // a mod L, or a mod L + L
-            rem = rem < rem - L[q] ? rem : rem - L[q];        // unsigned: picks the one below L
-            const uint32_t p2 = RS - rem;                     // next unconsumed position after this bin's lobbies
-            const bool inside = cur < B1, full = p2 >= B1;
-            const uint32_t m = (!inside || full) ? B1 - B0 : p2 - B0;  // matched players of the bin (a prefix)
-            pos[q] = !inside ? pos[q] : (full ? p2 : B1);     // the rest of a partly matched bin stays queued
+            const uint32_t m = s1_step(pos[q], B0, B1, RS, L[q], Mrec[q]);
             if ((int)lane == l) mine[q] = m;
           }
         }

@@ -285,6 +285,48 @@ class Engine:
         self._check(self.lib.mm_take(self.h, len(ids), _p(ids), C.byref(nt)), "mm_take")
         return nt.value
 
+    # -- boundary pass on the device (mm_band_candidates / mm_band_match) ----------------------------------------
+    def band_candidates(self, W, group):
+        """The upper side of the boundary group-1 | group: live queued players of `group` with rating in
+        (hi_{group-1}, hi_{group-1} + W], sorted by (mode, rating, enqueue order) -> (ids u64, rating i32, mode u8)."""
+        cap = 1 << 14
+        while True:
+            ids, rating, mode = np.empty(cap, np.uint64), np.empty(cap, np.int32), np.empty(cap, np.uint8)
+            n = C.c_uint32(0)
+            rc = self.lib.mm_band_candidates(self.h, int(W), int(group), _p(ids), _p(rating), _p(mode), cap, C.byref(n))
+            if rc == abi.MM_E_CAP and n.value > cap:
+                cap = n.value
+                continue
+            self._check(rc, "mm_band_candidates")
+            k = n.value
+            return ids[:k], rating[:k], mode[:k]
+
+    def band_match(self, W, g_first, g_last, upper=None):
+        """Match the bands of the boundaries g|g+1, g_first <= g <= g_last, and take the local matched players.
+        upper: (ids, rating, mode) of the upper side of boundary g_last|g_last+1 from another engine
+        (band_candidates), or None to read it from this engine.
+        -> (lobbies[LOBBY_DTYPE], member_ids u64, upper_taken bool[len(upper ids)], BandStats)"""
+        remote = upper is not None
+        if remote:
+            up = (np.ascontiguousarray(upper[0], np.uint64), np.ascontiguousarray(upper[1], np.int32),
+                  np.ascontiguousarray(upper[2], np.uint8))
+        else:
+            up = (np.zeros(0, np.uint64), np.zeros(0, np.int32), np.zeros(0, np.uint8))
+        n_up = len(up[0])
+        taken = np.zeros(max(n_up, 1), np.uint8)
+        lobby_cap, member_cap = 1 << 10, 1 << 12  # resized from the counts of an MM_E_CAP refusal
+        while True:
+            lob = np.empty(lobby_cap, LOBBY_DTYPE)
+            mem = np.empty(member_cap, np.uint64)
+            st = abi.BandStats()
+            rc = self.lib.mm_band_match(self.h, int(W), int(g_first), int(g_last), int(remote), _p(up[0]), _p(up[1]),
+                                        _p(up[2]), n_up, _p(lob), lobby_cap, _p(mem), member_cap, _p(taken), C.byref(st))
+            if rc == abi.MM_E_CAP and (st.n_lobbies > lobby_cap or st.n_matched > member_cap):
+                lobby_cap, member_cap = max(lobby_cap, st.n_lobbies), max(member_cap, st.n_matched)
+                continue
+            self._check(rc, "mm_band_match")
+            return lob[:st.n_lobbies], mem[:st.n_matched], taken[:n_up].astype(bool), st
+
     def in_queue(self, ids):
         ids = np.ascontiguousarray(ids, np.uint64)
         out = np.empty(len(ids), np.uint8)

@@ -276,6 +276,44 @@ def boundary_pass(pkg, cfg, W, world, rank, engine, comm, make_engine=None, cach
     return dict(hdr=hdr, member_ids=members, **stats)
 
 
+def boundary_pass_device(pkg, cfg, W, world, rank, engine, comm):
+    """boundary_pass on the device: the same bands, lobbies, takes, messages and result dict, but the candidates are
+    gathered and the bands matched inside `engine` (mm_band_candidates / mm_band_match, DESIGN §6) — the pool is never
+    read to the host and no band engine exists.  Only the candidate columns sent down, the lobby headers, the members
+    and the consumed ids cross PCIe.  `engine` is a pkg.Engine that has just ticked; boundary_pass stays the reference
+    (and the only path for engines without the device calls)."""
+    check_bands(cfg, W)
+    G = cfg.n_groups
+    mine = groups_of_rank(rank, G, world)
+    stats = {"sent": 0, "received": 0, "matched": 0, "lobbies": 0}
+    if len(mine) == 0:
+        return dict(hdr=None, member_ids=np.zeros(0, np.uint64), **stats)
+    a, b = int(mine[0]), int(mine[-1])
+    if rank > 0:  # my lowest group's low-side band goes down to the owner of group a-1
+        cand = engine.band_candidates(W, a)
+        comm.send(rank, rank - 1, cand)
+        stats["sent"] += len(cand[0])
+    hdr, members = None, np.zeros(0, np.uint64)
+    g_last = min(b, G - 2)
+    if a <= g_last:
+        remote = g_last + 1 > b
+        upper = None
+        if remote:
+            upper = comm.recv(rank + 1, rank)
+            stats["received"] += len(upper[0])
+        lob, mem, taken, _st = engine.band_match(W, a, g_last, upper)
+        if remote:
+            comm.send(rank, rank + 1, (np.asarray(upper[0], np.uint64)[taken],))
+        if len(lob):
+            hdr, members = lob, mem
+            stats["matched"] += len(mem); stats["lobbies"] += len(lob)
+    if rank > 0:  # what the lower rank consumed of my candidates leaves my pool
+        (gone,) = comm.recv(rank - 1, rank)
+        if len(gone):
+            assert engine.take(gone) == len(gone)
+    return dict(hdr=hdr, member_ids=members, **stats)
+
+
 # ======================================================================================================================
 # Moving rating groups between ranks (mm_export_queues / mm_merge).  A group's queues, all modes, go from the rank that
 # owns it to another one while both keep running: scale out / in, or a rebalance by balanced_owners() when the
