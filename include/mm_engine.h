@@ -188,6 +188,45 @@ int mm_remove_packed(mm_engine* e, uint32_t n, const uint32_t* handle, uint32_t*
  * the lobby stage removes them (game-lobby/worker.ex:80).  Ids that are not queued are ignored.               */
 int mm_take(mm_engine* e, uint32_t n, const uint64_t* id, uint32_t* n_taken);
 
+/* EXTENSION (requeue): players of a lobby that did not start (a member declined the ready check, no game server
+ * could be allocated: game-lobby/worker.ex:89-103) go back into their queue at their enqueue position, as the
+ * reference keeps the remaining members of a partial lobby in place when one leaves (search/worker.ex:312-321).
+ * Entry i carries what the player had when it was queued: id (a handle on MM_F_DENSE_IDS engines, as mm_enqueue
+ * takes it), rating, mode, enq_ts (may be NULL: 0) and seq, its enqueue sequence number (the numbering of emit_seq;
+ * an image's section 5).  The engine no longer has these once a tick has compacted the pool, so the caller keeps
+ * them.  Entries are in AGE ORDER: (seq[i] - seq_next) mod 2^32 strictly ascending (the order of mm_pool_read).
+ * codes[i] (may be NULL):
+ *   1  requeued: the id was in the active set and is not a live queued player (matched by any earlier tick, taken by
+ *      mm_take or mm_band_match).  It goes back into the partition its rating and mode map to, at the position its
+ *      seq gives among that partition's live players, with its rating, enq_ts and seq: its wait and the search
+ *      timeout count from its first enqueue.  mm_in_queue reads 1; mm_active_size does not change.
+ *   0  already a live queued player: nothing changes.
+ *   4  not in the active set (removed, expired, moved out, never queued): not requeued, the player left.
+ * *n_requeued = the entries with code 1.  n = 0 does nothing.  Pending async_results copies, the last tick's match
+ * section of mm_queue_stats, the snapshot and the mm_enqueue_rejects list are left alone.
+ * Refusals, all decided before anything changes (mm_last_error names the cause):
+ *   MM_E_ARG   a mode >= n_modes, a rating without a group, an id out of range, entries not in strict age order, a seq
+ *              equal to seq_next, a seq equal to that of a live player of the partition a code-1 entry goes to, an id
+ *              given twice;
+ *   MM_E_STATE an MM_F_NO_DEDUPE engine (no active set tells matched from gone), a staged packed batch;
+ *   MM_E_CAP   the pool does not hold the result.  The call writes every partition that receives a player (a TOUCHED
+ *              partition) anew on fresh chunks and leaves its old chunks to the next tick, so with U = the slots in use
+ *              (mm_pool_size) minus the touched partitions' dead slots plus the requeued players, and H = the slots of
+ *              the chunks (2048 slots each) left behind by this and earlier requeues since the last tick (the touched
+ *              partitions' old chunks: ceil(slots / 2048) each), the call needs U + H <= capacity.  Until the next
+ *              tick, enqueue and mm_merge count H as slots in use.
+ * Afterwards mm_pool_size = U.  Cost: the touched partitions' live players, read and written once.
+ *
+ * EQUIVALENCE.  Take mm_export of the engine just before the call, insert the code-1 entries into sections 2-6 in their
+ * partition at their sequence position, remove their ids from section 7 and keep seq_next: every later call sequence
+ * gives the same results on the engine as on a fresh engine that mm_import'ed that image.  What may differ is what
+ * differs after mm_import (dead slots are not carried): mm_pool_size, the next tick's pool_before and n_dead,
+ * mm_queue_stats' n_removed, and when a pool near capacity answers "full" (here H counts too).                 */
+int mm_requeue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating, const uint8_t* mode,
+               const uint32_t* enq_ts, const uint32_t* seq, uint8_t* codes, uint32_t* n_requeued);
+/* The enqueue sequence number the next offered player will get.                                                   */
+int mm_seq_next(mm_engine* e, uint32_t* seq_next);
+
 /* EXTENSION (cross-group boundary pass on the device, DESIGN.md §6): the band gather and the band walk of
  * shard.boundary_pass without reading the pool to the host.  Both calls need what shard.check_bands needs: W >= 0,
  * MM_ORDER_RATING, contiguous ascending groups, each at least 2W wide (else MM_E_ARG); MM_E_STATE with a staged

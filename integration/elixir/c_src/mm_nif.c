@@ -13,6 +13,7 @@
  *            -L../../../microservice-matchmaking_b200/csrc -lmm_engine -o priv/mm_nif.so
  */
 #include <erl_nif.h>
+#include <stdlib.h>
 #include <string.h>
 
 #include "mm_engine.h"
@@ -273,6 +274,67 @@ static ERL_NIF_TERM nif_merge_image(ErlNifEnv* env, int argc, const ERL_NIF_TERM
   return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &rej));
 }
 
+/* seq_next(ref) -> {:ok, seq}: the enqueue sequence number the next offered player will get (mm_seq_next) */
+static ERL_NIF_TERM nif_seq_next(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; uint32_t s = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r)) return enif_make_badarg(env);
+  int rc = mm_seq_next(r->e, &s);
+  return rc ? err(env, rc) : enif_make_tuple2(env, atom(env, "ok"), enif_make_uint(env, s));
+}
+
+/* qsort of (age, index) pairs by age: the age (seq - seq_next mod 2^32) is computed into the key first */
+static int rq_cmp(const void* a, const void* b) {
+  const uint32_t ux = *(const uint32_t*)a, uy = *(const uint32_t*)b;
+  return ux < uy ? -1 : ux > uy;
+}
+/* requeue(ref, handles :: binary(u32[]), ratings :: binary(i32[]), modes :: binary(u8[]), enq_ts :: binary(u32[]),
+ * seq :: binary(u32[])) -> {:ok, codes :: binary(u8[])} (1 requeued, 0 still queued, 4 gone; in the caller's order):
+ * the members of a lobby that did not start go back into their queue at their enqueue position (mm_requeue).  The
+ * entries are sorted by age here. */
+static ERL_NIF_TERM nif_requeue(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary hs, rt, md, ts, sq, codes; uint32_t got = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &hs) ||
+      !enif_inspect_binary(env, argv[2], &rt) || !enif_inspect_binary(env, argv[3], &md) ||
+      !enif_inspect_binary(env, argv[4], &ts) || !enif_inspect_binary(env, argv[5], &sq))
+    return enif_make_badarg(env);
+  const size_t n = hs.size / 4;
+  if (hs.size % 4 || rt.size != 4 * n || md.size != n || ts.size != 4 * n || sq.size != 4 * n) return enif_make_badarg(env);
+  if (!enif_alloc_binary(n, &codes)) return err(env, MM_E_CAP);
+  if (n == 0) return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &codes));
+  uint32_t* key = enif_alloc(n * 8);  /* (age, index) pairs */
+  uint64_t* id = enif_alloc(n * 8);
+  int32_t* rating = enif_alloc(n * 4);
+  uint8_t* mode = enif_alloc(n);
+  uint32_t *stamp = enif_alloc(n * 4), *seq = enif_alloc(n * 4);
+  uint8_t* out = enif_alloc(n);
+  int rc = MM_E_CAP;
+  uint32_t seq_next = 0;
+  if (key && id && rating && mode && stamp && seq && out && !(rc = mm_seq_next(r->e, &seq_next))) {
+    for (size_t i = 0; i < n; ++i) {
+      uint32_t s;
+      memcpy(&s, sq.data + 4 * i, 4);
+      key[2 * i] = s - seq_next;
+      key[2 * i + 1] = (uint32_t)i;
+    }
+    qsort(key, n, 8, rq_cmp);
+    for (size_t k = 0; k < n; ++k) {
+      const uint32_t i = key[2 * k + 1];
+      uint32_t h;
+      memcpy(&h, hs.data + 4 * i, 4); id[k] = h;
+      memcpy(&rating[k], rt.data + 4 * i, 4); mode[k] = md.data[i];
+      memcpy(&stamp[k], ts.data + 4 * i, 4); memcpy(&seq[k], sq.data + 4 * i, 4);
+    }
+    rc = mm_requeue(r->e, (uint32_t)n, id, rating, mode, stamp, seq, out, &got);
+    if (!rc)
+      for (size_t k = 0; k < n; ++k) codes.data[key[2 * k + 1]] = out[k];
+  }
+  enif_free(key); enif_free(id); enif_free(rating); enif_free(mode); enif_free(stamp); enif_free(seq); enif_free(out);
+  if (rc) { enif_release_binary(&codes); return err(env, rc); }
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &codes));
+}
+
 /* set_max_spread(ref, w): extension knob (strategist policy S1); w < 0 restores the reference behaviour */
 static ERL_NIF_TERM nif_set_max_spread(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
   engine_res* r; ErlNifSInt64 w = -1;
@@ -300,6 +362,8 @@ static ErlNifFunc funcs[] = {
   {"import_image", 2, nif_import_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"export_queues", 2, nif_export_queues, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"merge_image", 2, nif_merge_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"seq_next", 1, nif_seq_next, 0},
   {"set_max_spread", 2, nif_set_max_spread, 0},
 };
 ERL_NIF_INIT(Elixir.Matchmaking.Search.Engine, funcs, load, NULL, NULL, NULL)

@@ -34,6 +34,14 @@ defmodule Matchmaking.Search.Engine do
         (if Keyword.get(opts, :dense_ids, false), do: 2, else: 0)::little-32>>   # MM_F_DENSE_IDS
   end
 
+  @doc "(mode, group) queue index (mode * n_groups + group) of a rating: first group that holds it, else the default."
+  def queue_of(rating, mode) do
+    n = length(@rating_groups)
+    g = Enum.find_index(@rating_groups, fn {lo, hi} -> rating >= lo and rating <= hi end) ||
+          (if div(n, 2) + 1 < n, do: div(n, 2) + 1, else: -1)
+    if g < 0, do: -1, else: mode * n + g
+  end
+
   def mode_index(name), do: Enum.find_index(@modes, fn {n, _, _} -> n == name end)
   def mode_name(index), do: elem(Enum.at(@modes, index), 0)
   def teams_of(index), do: elem(Enum.at(@modes, index), 1)
@@ -81,6 +89,14 @@ defmodule Matchmaking.Search.Engine do
   {:error, :badarg | :capacity | :state}; a refusal changes nothing.
   """
   def merge_image(_ref, _image), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Requeue (extension): the members of a lobby that did not start go back into their queue at their enqueue position
+  (mm_requeue).  handles: binary(u32[]); ratings: binary(i32[]); modes: binary(u8[]); enq_ts, seq: binary(u32[]) — the
+  columns each player had when it was queued -> {:ok, codes :: binary(u8[])}: 1 requeued, 0 still queued, 4 gone.
+  """
+  def requeue(_ref, _handles, _ratings, _modes, _enq_ts, _seq), do: :erlang.nif_error(:nif_not_loaded)
+  @doc "The enqueue sequence number the next offered player will get (mm_seq_next) -> {:ok, seq}."
+  def seq_next(_ref), do: :erlang.nif_error(:nif_not_loaded)
   def n_modes, do: length(@modes)
   def n_groups, do: length(@rating_groups)
 

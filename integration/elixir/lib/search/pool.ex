@@ -68,12 +68,21 @@ defmodule Matchmaking.Search.Pool do
   old owner, or keep it and retry).
   """
   def move_in(blob), do: GenServer.call(__MODULE__, {:move_in, blob}, :infinity)
+  @doc """
+  Requeue (extension): the members of a lobby that did not start (a declined ready check, no game server) go back into
+  their queue at their enqueue position (Engine.requeue); players = the lobby's player documents.  -> one outcome per
+  player: :requeued (queued again: its wait and the search timeout go on from its first enqueue), :queued (still
+  queued) or :gone (removed, timed out, never queued, or its queue has moved to another pool: answer it as today).
+  """
+  def requeue(players), do: GenServer.call(__MODULE__, {:requeue, players}, :infinity)
 
   @impl true
   def init(opts) do
     capacity = Keyword.get(opts, :capacity, 16_000_000)
     {:ok, ref} = Engine.new(Engine.pack_config(capacity: capacity, active_capacity: 2 * capacity, dense_ids: true))
+    # queued: handle -> {rating, mode, enq_ts, seq} at its enqueue, what requeue/1 hands back (kept until remove_user)
     st = %{ref: ref, staged: [], n_staged: 0, handle_of: %{}, players: %{}, free: [], next: 0, channel: nil,
+           queued: %{}, moved_out: MapSet.new(),
            t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms)}
     case resume(st, Keyword.get(opts, :resume)) do
       {:ok, st} ->
@@ -96,6 +105,7 @@ defmodule Matchmaking.Search.Pool do
         down = max(0, System.os_time(:millisecond) - ck.wall_ms)
         # now_ms/1 goes on from the checkpoint's value plus the downtime: the engine's enqueue stamps stay valid
         {:ok, %{st | handle_of: ck.handle_of, players: ck.players, free: ck.free, next: ck.next,
+                     queued: Map.get(ck, :queued, %{}), moved_out: Map.get(ck, :moved_out, MapSet.new()),
                      t0: System.monotonic_time(:millisecond) - ck.now_ms - down}}
       {:error, _} = e -> e
     end
@@ -140,7 +150,8 @@ defmodule Matchmaking.Search.Pool do
       {nil, _} -> {:reply, {:ok, :removed}, st}                       # Mnesia.delete of a missing key is fine too
       {h, rest} ->
         Engine.remove_packed(st.ref, <<h::little-32>>)
-        {:reply, {:ok, :removed}, %{st | handle_of: rest, players: Map.delete(st.players, h), free: [h | st.free]}}
+        {:reply, {:ok, :removed}, %{st | handle_of: rest, players: Map.delete(st.players, h), free: [h | st.free],
+                                         queued: Map.delete(st.queued, h)}}
     end
   end
 
@@ -149,7 +160,7 @@ defmodule Matchmaking.Search.Pool do
     case Engine.export_image(st.ref) do
       {:ok, image} ->
         ck = %{image: image, handle_of: st.handle_of, players: st.players, free: st.free, next: st.next,
-               now_ms: now_ms(st), wall_ms: System.os_time(:millisecond)}
+               queued: st.queued, moved_out: st.moved_out, now_ms: now_ms(st), wall_ms: System.os_time(:millisecond)}
         {:reply, {:ok, :erlang.term_to_binary(ck)}, st}
       {:error, _} = e -> {:reply, e, st}
     end
@@ -167,8 +178,10 @@ defmodule Matchmaking.Search.Pool do
         handles = for <<h::little-32 <- binary_part(image, id_off, 4 * n)>>, do: h
         {moved, st} = Enum.map_reduce(handles, st, fn h, acc ->
           {player, players} = Map.pop(acc.players, h)
-          {{player["id"], player}, release(%{acc | players: players}, player["id"], h)}
+          {{player["id"], player}, release(%{acc | players: players, queued: Map.delete(acc.queued, h)}, player["id"], h)}
         end)
+        moved_q = for m <- 0..(Engine.n_modes() - 1), g <- groups, do: m * n_groups + g
+        st = %{st | moved_out: MapSet.union(st.moved_out, MapSet.new(moved_q))}
         blob = %{image: image, players: moved, n_modes: Engine.n_modes(), n_groups: n_groups,
                  now_ms: now_ms(st), wall_ms: System.os_time(:millisecond)}
         {:reply, {:ok, :erlang.term_to_binary(blob)}, st}
@@ -197,9 +210,25 @@ defmodule Matchmaking.Search.Pool do
       image = binary_part(mv.image, 0, id_off) <> ids <>
               binary_part(mv.image, id_off + 4 * n, ts_off - id_off - 4 * n) <> ts <>
               binary_part(mv.image, ts_off + 4 * n, byte_size(mv.image) - ts_off - 4 * n)
+      {:ok, seq0} = Engine.seq_next(st.ref)
       case Engine.merge_image(st.ref, image) do
         {:ok, rejected} ->
           rej = MapSet.new(for <<i::little-32 <- rejected>>, do: i)
+          # mm_merge numbers its batch queue by queue, in the source's enqueue order inside a queue: sort the image
+          # indices by (queue, age), number them, and put the numbers back in image order (n log n, lists walked once)
+          {cols, src_next} = image_cols(mv.image)
+          seqs = cols |> Enum.with_index()
+                 |> Enum.sort_by(fn {{r, m, _t, s}, _i} -> {Engine.queue_of(r, m), Bitwise.band(s - src_next, 0xFFFFFFFF)} end)
+                 |> Enum.with_index(fn {_, i}, k -> {i, Bitwise.band(seq0 + k, 0xFFFFFFFF)} end)
+                 |> Enum.sort() |> Enum.map(&elem(&1, 1))
+          st = Enum.zip([rows, cols, seqs]) |> Enum.with_index() |> Enum.reduce(st, fn {{{h, _, _, _}, {r, m, t, _}, q}, i}, acc ->
+            if MapSet.member?(rej, i) do
+              acc
+            else
+              %{acc | queued: Map.put(acc.queued, h, {r, m, Bitwise.band(t + shift, 0xFFFFFFFF), q}),
+                      moved_out: MapSet.delete(acc.moved_out, Engine.queue_of(r, m))}
+            end
+          end)
           st = rows |> Enum.with_index() |> Enum.reduce(st, fn {{h, fresh, id, _}, i}, acc ->
             # a rejected player is already queued here: keep this pool's player and document
             if MapSet.member?(rej, i) and fresh, do: release(acc, id, h), else: acc
@@ -214,6 +243,40 @@ defmodule Matchmaking.Search.Pool do
     end
   end
 
+  # -- requeue (extension): a lobby that did not start ----------------------------------------------------------------
+  def handle_call({:requeue, players}, _from, st) do
+    st = flush(st)
+    rows = for {p, i} <- Enum.with_index(players), h = Map.get(st.handle_of, p["id"]), h != nil,
+               rec = Map.get(st.queued, h), rec != nil, not MapSet.member?(st.moved_out, Engine.queue_of(elem(rec, 0), elem(rec, 1))),
+               do: {i, h, rec}
+    rows = Enum.uniq_by(rows, fn {_, h, _} -> h end)
+    bin = fn f -> for {_, _, rec} <- rows, into: <<>>, do: f.(rec) end
+    result =
+      if rows == [] do
+        {:ok, <<>>}
+      else
+        Engine.requeue(st.ref, (for {_, h, _} <- rows, into: <<>>, do: <<h::little-32>>),
+                       bin.(fn {r, _, _, _} -> <<r::little-signed-32>> end), bin.(fn {_, m, _, _} -> <<m>> end),
+                       bin.(fn {_, _, t, _} -> <<t::little-32>> end), bin.(fn {_, _, _, s} -> <<s::little-32>> end))
+      end
+    case result do
+      {:ok, codes} ->
+        by_h = Map.new(Enum.zip(rows, :binary.bin_to_list(codes)), fn {{_, h, _}, c} -> {h, c} end)
+        outcome = Enum.map(players, fn p ->
+          case by_h[Map.get(st.handle_of, p["id"])] do
+            1 -> :requeued
+            0 -> :queued
+            _ -> :gone
+          end
+        end)
+        docs = List.to_tuple(players)
+        back = for {{i, h, _}, 1} <- Enum.zip(rows, :binary.bin_to_list(codes)), into: st.players,
+                 do: {h, elem(docs, i)}
+        {:reply, outcome, %{st | players: back}}
+      {:error, _} = e -> {:reply, e, st}
+    end
+  end
+
   # The image's player columns (include/mm_engine.h): the 624-byte header, part_count u32[n_parts], then id (u32
   # handles on this MM_F_DENSE_IDS engine), rating, enq_ts, seq, mode, each section starting at a multiple of 8.
   defp image_sections(image) do
@@ -225,6 +288,20 @@ defmodule Matchmaking.Search.Pool do
     {n, id_off, ts_off}
   end
 
+
+  # {rating, mode, enq_ts, seq} of every player of an image, and the header's seq_next
+  defp image_cols(image) do
+    <<_::binary-size(24), n_parts::little-32, n::little-32, _::binary-size(4), src_next::little-32, _::binary>> = image
+    a8 = fn x -> Bitwise.band(x + 7, Bitwise.bnot(7)) end
+    id_off = a8.(624 + 4 * n_parts)
+    rt_off = a8.(id_off + 4 * n)
+    ts_off = a8.(rt_off + 4 * n)
+    sq_off = a8.(ts_off + 4 * n)
+    md_off = a8.(sq_off + 4 * n)
+    col = fn off, w -> for <<v::little-size(w) <- binary_part(image, off, div(w, 8) * n)>>, do: v end
+    rts = for <<v::little-signed-32 <- binary_part(image, rt_off, 4 * n)>>, do: v
+    {Enum.zip([rts, col.(md_off, 8), col.(ts_off, 32), col.(sq_off, 32)]), src_next}
+  end
 
   @impl true
   def handle_info(:flush, st) do
@@ -257,7 +334,8 @@ defmodule Matchmaking.Search.Pool do
           acc ->
             {player, players} = Map.pop(acc.players, h)
             send_timeout(acc.channel, player)
-            %{acc | players: players, handle_of: Map.delete(acc.handle_of, player["id"]), free: [h | acc.free]}
+            %{acc | players: players, handle_of: Map.delete(acc.handle_of, player["id"]), free: [h | acc.free],
+                    queued: Map.delete(acc.queued, h)}
         end
       {:error, _reason} -> st                                          # nothing changed; the next tick retries
     end
@@ -288,14 +366,18 @@ defmodule Matchmaking.Search.Pool do
     keys = for {_, _, _, m, r, _} <- rows, into: <<>>, do: <<(m * 8192 + r)::little-16>>   # mode << 13 | rating
     st = %{st | staged: [], n_staged: 0}
     stamp = now_ms(st)
+    {:ok, seq0} = Engine.seq_next(st.ref)   # every offered entry of an accepted batch takes one sequence number
     ts = for _ <- rows, into: <<>>, do: <<stamp::little-32>>
     case Engine.enqueue_packed(st.ref, handles, keys, ts) do
       {:ok, codes} ->
-        Enum.zip(:binary.bin_to_list(codes), rows)
+        Enum.zip([:binary.bin_to_list(codes), rows, 0..(length(rows) - 1)])
         |> Enum.reduce(st, fn
-          {1, {h, _, player, _, _, ack_ref}}, acc -> ack(ack_ref); %{acc | players: Map.put(acc.players, h, player)}
-          {0, {_, _, _, _, _, ack_ref}}, acc -> ack(ack_ref); acc       # "You are already in the queue."
-          {_, {h, fresh, player, _, _, ack_ref}}, acc -> nack(ack_ref); if(fresh, do: release(acc, player["id"], h), else: acc)
+          {1, {h, _, player, m, r, ack_ref}, i}, acc ->
+            ack(ack_ref)
+            %{acc | players: Map.put(acc.players, h, player),
+                    queued: Map.put(acc.queued, h, {r, m, stamp, Bitwise.band(seq0 + i, 0xFFFFFFFF)})}
+          {0, {_, _, _, _, _, ack_ref}, _}, acc -> ack(ack_ref); acc    # "You are already in the queue."
+          {_, {h, fresh, player, _, _, ack_ref}, _}, acc -> nack(ack_ref); if(fresh, do: release(acc, player["id"], h), else: acc)
         end)
       {:error, _reason} ->                                              # the engine refused the whole batch
         Enum.reduce(rows, st, fn {h, fresh, player, _, _, ack_ref}, acc ->

@@ -154,6 +154,8 @@ PROTOTYPES = {
     "mm_remove": (C.c_int, [_vp, C.c_uint32, _vp, _P(C.c_uint32)]),
     "mm_remove_packed": (C.c_int, [_vp, C.c_uint32, _vp, _P(C.c_uint32)]),
     "mm_take": (C.c_int, [_vp, C.c_uint32, _vp, _P(C.c_uint32)]),
+    "mm_requeue": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp, _P(C.c_uint32)]),
+    "mm_seq_next": (C.c_int, [_vp, _P(C.c_uint32)]),
     "mm_band_candidates": (C.c_int, [_vp, C.c_int32, C.c_uint32, _vp, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_band_match": (C.c_int, [_vp, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, _vp, _vp, _vp, C.c_uint32,
                                 _vp, C.c_uint32, _vp, C.c_uint64, _vp, _P(BandStats)]),

@@ -417,9 +417,11 @@ __global__ void k_rehash(ActiveView oldt, ActiveView newt) {
 }
 
 // After mm_restore / a generation wrap: point every queued player's entry at its slot again.
-// grid = (chunks in use, partitions): block (k, p) handles the partition's k-th chunk.
-__global__ void k_restamp(PoolView pool, PoolMeta meta, ActiveView act, uint32_t gen) {
+// grid = (chunks in use, partitions): block (k, p) handles the partition's k-th chunk.  sel (may be null): only the
+// partitions with a non-zero byte (mm_requeue).
+__global__ void k_restamp(PoolView pool, PoolMeta meta, ActiveView act, uint32_t gen, const uint8_t* __restrict__ sel) {
   const uint32_t p = blockIdx.y, k = blockIdx.x;
+  if (sel && !sel[p]) return;
   const uint32_t fill = meta.fill[p];
   if ((uint64_t)k * kTile >= fill || !act.on()) return;
   const uint32_t cnt = fill - k * kTile < kTile ? fill - k * kTile : kTile;

@@ -23,6 +23,7 @@
 #include "mm_expire.cuh"
 #include "mm_image.cuh"
 #include "mm_kernels.cuh"
+#include "mm_requeue.cuh"
 #include "mm_stats.cuh"
 
 using namespace mm;
@@ -67,6 +68,7 @@ struct Pool {
   PoolView v{};  // the arrays below, as the kernels take them
   PoolMeta m{};
   uint32_t n = 0;  // host mirror of the sum of the partition fills (dead players included)
+  uint32_t held = 0;  // slots of the chunks mm_requeue left behind: in no partition's list, reclaimed by the next tick
   DevArray<uint64_t> id;
   DevArray<int32_t> rating;
   DevArray<uint8_t> mode, tsize;
@@ -233,6 +235,13 @@ struct mm_engine {
   DevArray<uint8_t> d_mrg_code;       // the merge batch's ingest codes (d_code keeps the last mm_enqueue* batch's)
   DevArray<unsigned long long> d_mrg_seen;  // duplicate count: scratch id set
 
+  // mm_requeue: the entries go through the ingest scratch (d_in_*; seq in d_in_handle), their codes through d_mrg_code,
+  // the id check through d_mrg_seen, the grouped entries through d_mrg_src and d_rq_u, the gathered and merged columns
+  // through d_img (all freed by every call); the block counts and partition tables below are kept
+  DevArray<uint32_t> d_rq_u;     // grouped entries: age (seq - seq_next)
+  DevArray<uint32_t> d_rq_hist;  // [n_segs][blocks] code-1 entries -> the block's first grouped index
+  DevArray<uint32_t> d_rq_seg;   // rq_off[n_segs + 1] | m_off[n_segs + 1] | slot_base[n_segs]
+
   // mm_band_candidates / mm_band_match (mm_band.cuh): sized by the band keys and the candidates, grown on demand
   struct Band {
     DevArray<uint32_t> map, fill, qoff, qtiles, M, tot, pos, kbase, klim, band_mb, band_lb, rstart, ctr;
@@ -314,6 +323,7 @@ int alloc_pool(mm_engine* e, Pool& p) {
   p.v = PoolView{p.id, p.rating, p.mode, p.tsize, p.ts, p.bin, p.seq};
   p.m = PoolMeta{p.fill, p.chunk_tab, p.bump, p.tot, p.chist, e->n_chunks};
   p.n = 0;
+  p.held = 0;
   return MM_OK;
 }
 int copy_pool(mm_engine* e, Pool& dst, const Pool& src) {
@@ -332,6 +342,7 @@ int copy_pool(mm_engine* e, Pool& dst, const Pool& src) {
   if (src.m.chist)
     CK(cudaMemcpyAsync(dst.m.chist, src.m.chist, (size_t)e->n_chunks * kChunkHist * 4, cudaMemcpyDeviceToDevice, e->stream));
   dst.n = src.n;
+  dst.held = src.held;
   return MM_OK;
 }
 
@@ -602,7 +613,8 @@ int enq_chunk(mm_engine* e, uint32_t base, uint32_t cnt, const uint64_t* id, con
   k_enq_claim<<<nb, 256, 0, e->stream>>>(base, cnt, id, rating, mode, e->d_grp_lut, e->key_lo, e->KR, e->cfg.n_modes,
                                          bin_map(e), e->d_bin_seg, av, e->d_hslot, e->d_code, e->d_part);
   if (may_overflow) {  // the batch might not fit: the winners past the pool capacity are rolled back (code 3)
-    const uint32_t room = e->capacity > p.n ? e->capacity - p.n : 0u;
+    const uint64_t used = (uint64_t)p.n + p.held;
+    const uint32_t room = e->capacity > used ? (uint32_t)(e->capacity - used) : 0u;
     k_enq_count<<<nb, 256, 0, e->stream>>>(base, cnt, av, e->d_hslot, e->d_code, e->d_blocksum);
     k_scan_small<<<1, 1024, 0, e->stream>>>(nb, e->d_blocksum, &e->d_cnt->winners);
     k_enq_cut<<<nb, 256, 0, e->stream>>>(base, cnt, av, e->d_hslot, e->d_code, e->d_blocksum, room, &e->d_cnt->pool_full);
@@ -658,7 +670,7 @@ int enqueue_batch(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* r
                   const uint32_t* ts, uint32_t chunk, Upload upload) {
   int rc = enq_prepare(e, n, n);
   if (rc) return rc;
-  const bool may_overflow = (uint64_t)e->pool[e->cur].n + n > e->capacity;
+  const bool may_overflow = (uint64_t)e->pool[e->cur].n + e->pool[e->cur].held + n > e->capacity;
   for (uint32_t base = 0; base < n; base += chunk) {
     const uint32_t cnt = std::min(chunk, n - base);
     if ((rc = upload(base, cnt))) return rc;
@@ -812,6 +824,7 @@ int tick_commit(mm_engine* e, uint32_t n, mm_tick_stats* stats) {
   e->gen = next_gen(e);
   e->cur ^= 1;
   e->pool[e->cur].n = c.n_resid;
+  e->pool[e->cur].held = 0;
   e->match_valid = true;  // pool[cur ^ 1] is now the pool this tick matched
   e->match_n = n;
   e->last = st;
@@ -1074,6 +1087,7 @@ int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes, const
 // the image-sized scratch of mm_export / mm_import / mm_merge (cudaFree waits for the work that uses it)
 void free_img_scratch(mm_engine* e) {
   e->d_img.reset(); e->d_img_act.reset(); e->d_mrg_src.reset(); e->d_mrg_code.reset(); e->d_mrg_seen.reset();
+  e->d_rq_u.reset();
 }
 
 // The current pool buffer and the active set back to an empty engine's state.
@@ -1085,6 +1099,7 @@ int clear_engine(mm_engine* e) {
   if (p.m.chist) CK(cudaMemsetAsync(p.m.chist, 0, (size_t)e->n_chunks * kChunkHist * 4, e->stream));
   CK(cudaMemsetAsync(p.v.bin, 0xFF, pool_slots(e) * 2, e->stream));
   p.n = 0;
+  p.held = 0;
   if (e->use_active) {
     int rc = clear_table(e, e->tab[e->tcur]);
     if (rc) return rc;
@@ -1208,7 +1223,7 @@ int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
   e->match_valid = false;
   e->last_batch_n = 0;
   if (e->use_active && n) {  // the queued players' entries point at their slots
-    k_restamp<<<dim3(e->n_chunks, e->n_segs), 256, 0, e->stream>>>(p.v, p.m, act_view(e), e->gen);
+    k_restamp<<<dim3(e->n_chunks, e->n_segs), 256, 0, e->stream>>>(p.v, p.m, act_view(e), e->gen, nullptr);
     CK(cudaGetLastError());
   }
   CK(cudaStreamSynchronize(e->stream));
@@ -1276,7 +1291,7 @@ int merge_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uin
   // the exact reject count, when the reject list or a capacity could be too small for every player being queued
   const Pool& p = e->pool[e->cur];
   const bool hashed = e->use_active && !e->dense_ids;
-  const bool tight = (uint64_t)p.n + n > e->capacity || (hashed && (e->n_active + n) * 4 > e->hcap * 3);
+  const bool tight = (uint64_t)p.n + p.held + n > e->capacity || (hashed && (e->n_active + n) * 4 > e->hcap * 3);
   if (e->use_active && (cap < n || tight)) {
     uint64_t sc = 1024;
     while (sc < 2ull * n) sc <<= 1;
@@ -1292,8 +1307,9 @@ int merge_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uin
     *n_rejected = n_rej;
     return set_err(e, MM_E_CAP, "%u rejected players, cap %u", n_rej, cap);
   }
-  if ((uint64_t)p.n + accepted > e->capacity)
-    return set_err(e, MM_E_CAP, "%u players merged into %u slots in use, capacity %u", accepted, p.n, e->capacity);
+  if ((uint64_t)p.n + p.held + accepted > e->capacity)
+    return set_err(e, MM_E_CAP, "%u players merged into %u slots in use, capacity %u", accepted, p.n + p.held,
+                   e->capacity);
   if (hashed && (e->n_active + accepted) * 4 > e->hcap * 3)
     return set_err(e, MM_E_CAP, "active set full: %llu ids resident, %u merged, capacity %llu",
                    (unsigned long long)e->n_active, accepted, (unsigned long long)(e->hcap * 3 / 4));
@@ -1345,6 +1361,157 @@ int remove_or_take(mm_engine* e, uint32_t n, const uint64_t* id, uint32_t* n_out
   if ((rc = read_counters(e))) return rc;
   if (!take) erase_active(e, e->h_cnt->removed);
   if (n_out) *n_out = e->h_cnt->removed;
+  return MM_OK;
+}
+
+// ---- mm_requeue (mm_requeue.cuh) ------------------------------------------------------------------------------------
+// The columns of up to n players (8-byte ids) carved from `at`, which moves past them.
+ImgCols carve_cols(uint8_t*& at, size_t n) {
+  auto a8 = [](size_t x) { return (x + 7) & ~(size_t)7; };
+  ImgCols c{};
+  c.id = at; at += a8(8 * n);
+  c.rating = reinterpret_cast<int32_t*>(at); at += a8(4 * n);
+  c.ts = reinterpret_cast<uint32_t*>(at); at += a8(4 * n);
+  c.seq = reinterpret_cast<uint32_t*>(at); at += a8(4 * n);
+  c.mode = at; at += a8(n);
+  c.id_bytes = 8;
+  return c;
+}
+size_t cols_bytes(size_t n) { return 21 * n + 40; }
+
+int rq_err(mm_engine* e, uint32_t err) {
+  return set_err(e, MM_E_ARG, "requeue refused:%s%s%s%s%s%s%s", err & kRqBadId ? " id out of range" : "",
+                 err & kRqBadMode ? " mode out of range" : "", err & kRqBadRating ? " rating without a group" : "",
+                 err & kRqOrder ? " entries not in age order" : "",
+                 err & kRqSeqNext ? " sequence number equal to seq_next" : "", err & kRqDup ? " duplicate id" : "",
+                 err & kRqSeqLive ? " sequence number of a live player of the partition" : "");
+}
+
+// Three device phases, each ended by one read of the counters; the pool changes only in the third.
+//   1. check and classify the entries, group them, count the touched partitions' live players: every refusal but the
+//      sequence collision, and the exact sizes of the gather and the merge
+//   2. gather the touched partitions' live players and merge: the collision refusal, then the capacity one
+//   3. layout, load, restamp
+// The gathered and merged columns are sized by the touched partitions' live players and the entries, never by the pool.
+int requeue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating, const uint8_t* mode, const uint32_t* ts,
+            const uint32_t* seq, uint8_t* codes, uint32_t* n_requeued) {
+  if (!e->use_active)
+    return set_err(e, MM_E_STATE, "requeue needs the active set: an MM_F_NO_DEDUPE engine cannot tell matched from gone");
+  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (n == 0) return MM_OK;
+  Pool& p = e->pool[e->cur];
+  const uint32_t S = e->n_segs, nblk = (n + kRqItems - 1) / kRqItems;
+  int rc;
+  if ((rc = ensure_enq_scratch(e, n))) return rc;
+  uint64_t sc = 1024;
+  while (sc < 2ull * n) sc <<= 1;
+  CK(e->d_mrg_code.reserve((size_t)n + 64));
+  CK(e->d_mrg_src.reserve((size_t)n + 64));
+  CK(e->d_rq_u.reserve((size_t)n + 64));
+  CK(e->d_mrg_seen.reserve(sc));
+  CK(e->d_rq_hist.reserve((size_t)S * nblk));
+  CK(e->d_rq_seg.reserve(3 * (size_t)S + 2));
+  CK(e->d_sel.reserve(kMaxSegs));
+  uint32_t* rq_off = e->d_rq_seg;
+  uint32_t* m_off = rq_off + S + 1;
+  uint32_t* slot_base = m_off + S + 1;
+  uint32_t* d_seq = e->d_in_handle;
+  CK(cudaMemcpyAsync(e->d_in_id, id, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(e->d_in_rating, rating, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(e->d_in_mode, mode, n, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(d_seq, seq, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  if (ts) CK(cudaMemcpyAsync(e->d_in_ts, ts, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemsetAsync(e->d_mrg_seen, 0xFF, sc * 8, e->stream));
+  CK(cudaMemsetAsync(&e->d_cnt->img_players, 0, 3 * 4, e->stream));  // img_players, img_active, img_err
+  RqCheckArgs ca{};
+  ca.id = e->d_in_id; ca.rating = e->d_in_rating; ca.mode = e->d_in_mode; ca.seq = d_seq;
+  ca.n = n; ca.n_segs = S; ca.nblk = nblk; ca.bm = bin_map(e); ca.grp_lut = e->d_grp_lut; ca.bin_seg = e->d_bin_seg;
+  ca.n_modes = e->cfg.n_modes; ca.seq_next = e->seq_next; ca.id_limit = id_limit(e);
+  ca.act = act_view(e); ca.pool_mode = p.v.mode; ca.n_slots = (uint32_t)pool_slots(e); ca.gen = e->gen;
+  ca.seen = e->d_mrg_seen; ca.seen_mask = sc - 1;
+  ca.code = e->d_mrg_code; ca.part = e->d_part; ca.blockhist = e->d_rq_hist; ca.err = &e->d_cnt->img_err;
+  k_rq_check<<<nblk, 256, 0, e->stream>>>(ca);
+  k_rq_scan<<<1, 512, 0, e->stream>>>(S, nblk, e->d_rq_hist, rq_off, e->d_sel);
+  // export pass 1 over the touched partitions (unselected tiles are skipped without a pool load)
+  ImgExportArgs xa;
+  if ((rc = count_tiles(e, true, xa))) return rc;
+  k_scan_small<<<1, 1024, 0, e->stream>>>(tile_count(e, p.n), e->d_img_tile, &e->d_cnt->img_players);
+  k_rq_group<<<nblk, 256, 0, e->stream>>>(n, S, nblk, e->d_part, d_seq, e->seq_next, e->d_rq_hist, e->d_mrg_src,
+                                          e->d_rq_u);
+  CK(cudaGetLastError());
+  // read 1: counters, partition tables, fills, bump
+  std::vector<uint32_t> h_rq(S + 1), live(S), fill(S);
+  uint32_t bump = 0;
+  CK(cudaMemcpyAsync(h_rq.data(), rq_off, (size_t)(S + 1) * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(live.data(), e->d_img_part, (size_t)S * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(fill.data(), p.m.fill, (size_t)S * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(&bump, p.m.bump, 4, cudaMemcpyDeviceToHost, e->stream));
+  if ((rc = read_counters(e))) return rc;
+  if (const uint32_t err = e->h_cnt->img_err) return rq_err(e, err);
+  const uint32_t n_rq = h_rq[S], n_live = e->h_cnt->img_players;
+  ImgCols merged{};
+  if (n_rq) {
+    // export pass 2: the touched partitions' live players, partition by partition, in enqueue order; then the merge
+    CK(e->d_img.reserve(cols_bytes(n_live) + cols_bytes((size_t)n_live + n_rq)));
+    uint8_t* at = e->d_img;
+    const ImgCols gath = carve_cols(at, n_live);
+    merged = carve_cols(at, (size_t)n_live + n_rq);
+    if (n_live) {
+      xa.out = gath;
+      k_img_tiles<kImgBlock, true><<<tile_ctas(e, p.n), kImgBlock, 0, e->stream>>>(xa);
+    }
+    RqMergeArgs ma{};
+    ma.live = gath; ma.live_cnt = e->d_img_part; ma.n_segs = S; ma.seq_next = e->seq_next; ma.rq_off = rq_off;
+    ma.grp_src = e->d_mrg_src; ma.grp_u = e->d_rq_u;
+    ma.id = e->d_in_id; ma.rating = e->d_in_rating; ma.mode = e->d_in_mode; ma.ts = ts ? e->d_in_ts.p : nullptr;
+    ma.seq = d_seq; ma.out = merged; ma.m_off = m_off; ma.err = &e->d_cnt->img_err;
+    const uint64_t total = (uint64_t)n_live + n_rq;
+    const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((total + 255) / 256, 32ull * (uint32_t)e->n_sms));
+    k_rq_merge<<<grid, 256, 0, e->stream>>>(ma);
+    CK(cudaGetLastError());
+    // read 2: the sequence collision
+    if ((rc = read_counters(e))) return rc;
+    if (const uint32_t err = e->h_cnt->img_err) return rq_err(e, err);
+  }
+  // the touched partitions on fresh chunks from the bump on, in partition order (import_image's layout)
+  std::vector<uint32_t> base(S, 0);
+  uint32_t chunk = bump;
+  uint64_t dead = 0, left = 0;  // the touched partitions' dead slots; their chunks, left to the next tick
+  for (uint32_t s = 0; s < S; ++s) {
+    const uint32_t r = h_rq[s + 1] - h_rq[s];
+    if (!r) continue;
+    dead += fill[s] - live[s];
+    left += (fill[s] + kTile - 1) / kTile;
+    base[s] = chunk * kTile;
+    chunk += (live[s] + r + kTile - 1) / kTile;
+  }
+  const uint64_t used = (uint64_t)p.n - dead + n_rq, held = p.held + left * kTile;
+  if (used + held > e->capacity)
+    return set_err(e, MM_E_CAP, "requeue needs %llu pool slots in use and %llu left to the next tick, capacity %u",
+                   (unsigned long long)used, (unsigned long long)held, e->capacity);
+  if (n_rq) {
+    CK(cudaMemcpyAsync(slot_base, base.data(), (size_t)S * 4, cudaMemcpyHostToDevice, e->stream));
+    k_rq_layout<<<S, 256, 0, e->stream>>>(p.m, S, e->d_sel, m_off, slot_base, e->d_seg_bin_lo, e->K, (uint32_t)dead, chunk);
+    ImgLoadArgs la{};
+    la.pool = p.v; la.meta = p.m; la.in = merged; la.n = n_live + n_rq; la.n_segs = S;
+    la.part_off = m_off; la.slot_base = slot_base;
+    la.bm = bin_map(e); la.grp_lut = e->d_grp_lut; la.bin_seg = e->d_bin_seg; la.seg_bin_lo = e->d_seg_bin_lo;
+    la.mode_tsize = e->d_mode_tsize; la.n_modes = e->cfg.n_modes; la.seq_next = e->seq_next; la.id_limit = id_limit(e);
+    la.err = &e->d_cnt->img_err;
+    const uint32_t g2 = std::max<uint32_t>(1, std::min<uint32_t>((la.n + 255) / 256, 32u * (uint32_t)e->n_sms));
+    k_img_load<<<g2, 256, 0, e->stream>>>(la);
+    k_restamp<<<dim3(e->n_chunks, S), 256, 0, e->stream>>>(p.v, p.m, act_view(e), e->gen, e->d_sel);
+    CK(cudaGetLastError());
+  }
+  if (codes) CK(cudaMemcpyAsync(codes, e->d_mrg_code, n, cudaMemcpyDeviceToHost, e->stream));
+  if ((rc = read_counters(e))) return rc;
+  if (n_rq) {
+    p.n = (uint32_t)used;
+    p.held = (uint32_t)held;
+  }
+  if (n_requeued) *n_requeued = n_rq;
+  if (e->h_cnt->img_err)  // the merged list failed the load's own checks: nothing above lets that happen
+    return set_err(e, MM_E_STATE, "requeue: the merged players failed the load checks (0x%x)", e->h_cnt->img_err);
   return MM_OK;
 }
 
@@ -1812,6 +1979,24 @@ int mm_take(mm_engine* e, uint32_t n, const uint64_t* id, uint32_t* n_taken) {
   return remove_or_take(e, n, id, n_taken, true);
 }
 
+int mm_requeue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating, const uint8_t* mode,
+               const uint32_t* enq_ts, const uint32_t* seq, uint8_t* codes, uint32_t* n_requeued) {
+  if (n_requeued) *n_requeued = 0;
+  if (!e || (n && (!id || !rating || !mode || !seq))) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  const int rc = requeue(e, n, id, rating, mode, enq_ts, seq, codes, n_requeued);
+  free_img_scratch(e);
+  return rc;
+}
+
+int mm_seq_next(mm_engine* e, uint32_t* seq_next) {
+  if (!e || !seq_next) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  *seq_next = e->seq_next;
+  return MM_OK;
+}
+
 int mm_band_candidates(mm_engine* e, int32_t W, uint32_t group, uint64_t* ids, int32_t* rating, uint8_t* mode,
                        uint32_t cap, uint32_t* n_out) {
   if (!e || !n_out || (cap && (!ids || !rating || !mode))) return MM_E_ARG;
@@ -2099,7 +2284,7 @@ int mm_restore(mm_engine* e) {
   e->fresh = false;
   e->match_valid = false;  // the restored pool was not matched by the last tick
   if (e->use_active && p.n) {
-    k_restamp<<<dim3(e->n_chunks, e->n_segs), 256, 0, e->stream>>>(p.v, p.m, act_view(e), e->gen);
+    k_restamp<<<dim3(e->n_chunks, e->n_segs), 256, 0, e->stream>>>(p.v, p.m, act_view(e), e->gen, nullptr);
     CK(cudaGetLastError());
   }
   CK(cudaStreamSynchronize(e->stream));

@@ -285,6 +285,33 @@ class Engine:
         self._check(self.lib.mm_take(self.h, len(ids), _p(ids), C.byref(nt)), "mm_take")
         return nt.value
 
+    def seq_next(self):
+        """The enqueue sequence number the next offered player will get (mm_seq_next)."""
+        v = C.c_uint32(0)
+        self._check(self.lib.mm_seq_next(self.h, C.byref(v)), "mm_seq_next")
+        return v.value
+
+    def requeue(self, ids, rating, mode, enq_ts, seq):
+        """Put players of a lobby that did not start back into their queue at their enqueue position (mm_requeue).
+        The columns are what each player had when it was queued (enq_ts may be None).  The entries may come in any
+        order: they are sorted by age here.  -> codes u8[n] in the caller's order: 1 requeued, 0 still queued,
+        4 not in the active set (the player left)."""
+        ids = np.ascontiguousarray(ids, np.uint64)
+        n = len(ids)
+        seq = np.ascontiguousarray(seq, np.uint32)
+        assert len(rating) == n and len(mode) == n and len(seq) == n
+        order = np.argsort((seq - np.uint32(self.seq_next())).astype(np.uint32))  # numbers are unique: no tie to keep
+        cols = [np.ascontiguousarray(np.asarray(a)[order], dt) for a, dt in
+                ((ids, np.uint64), (rating, np.int32), (mode, np.uint8), (seq, np.uint32))]
+        ts = None if enq_ts is None else np.ascontiguousarray(np.asarray(enq_ts)[order], np.uint32)
+        codes = np.empty(n, np.uint8)
+        k = C.c_uint32(0)
+        self._check(self.lib.mm_requeue(self.h, n, _p(cols[0]), _p(cols[1]), _p(cols[2]), _p(ts), _p(cols[3]),
+                                        _p(codes), C.byref(k)), "mm_requeue")
+        out = np.empty(n, np.uint8)
+        out[order] = codes
+        return out
+
     # -- boundary pass on the device (mm_band_candidates / mm_band_match) ----------------------------------------
     def band_candidates(self, W, group):
         """The upper side of the boundary group-1 | group: live queued players of `group` with rating in

@@ -26,6 +26,7 @@ The AMQP connection is duck-typed (declare_exchange / declare_queue / bind / qos
 basic_consume / basic_publish / basic_ack / basic_nack / queue_status) so the same code
 drives a real client or the in-memory broker used by the tests.
 """
+import heapq
 import json
 import math
 
@@ -170,6 +171,7 @@ class SearchPool:
         self.wall_clock = wall_clock or time.time  # seconds since the epoch: checkpoint() / resume() bridge the downtime
         self._t0 = self.clock()
         self.enqueued_at = {}  # handle -> clock() when the player became resident (insertion = enqueue order)
+        self.matched_at = {}   # window: the enqueued_at of players matched and not yet removed (requeue() puts it back)
         self.last_spread = None
         self.engine = engine
         self.mode_names = list(mode_names)
@@ -179,6 +181,10 @@ class SearchPool:
         self.flush_every_s = flush_every_s
         self.handles = HandleTable(handle_capacity)
         self.players = {}   # handle -> decoded player document (without "game-mode")
+        # handle -> [rating, mode, enq_ts, seq] at its enqueue: what requeue() hands the engine back (kept from flush()
+        # until remove_user, for engines with seq_next())
+        self.queued = {}
+        self.moved_out = set()  # queues (mode * n_groups + group) released by move_out() and not moved back in
         self.workers = {}   # group name -> worker that publishes the group's lobbies
         self._staged = []   # (player id, rating, mode, player, worker, tag)
         self._staged_since = None
@@ -203,7 +209,59 @@ class SearchPool:
             self.handles.release(player_id)
             self.players.pop(h, None)
             self.enqueued_at.pop(h, None)
+            self.matched_at.pop(h, None)
+            self.queued.pop(h, None)
         return ("ok", "removed")
+
+    def requeue(self, players):
+        """Put the members of a lobby that did not start (a declined ready check, no game server) back into their
+        queue at their enqueue position (Engine.requeue): their wait and the search timeout go on from their first
+        enqueue.  players: the lobby's player documents, as the lobby stage has them.  -> one outcome per player:
+        "requeued" (queued again; its document is back in the pool), "queued" (still queued: nothing changed) or
+        "gone" (not in this pool's active set — removed, timed out, never queued — or its queue has moved to another
+        pool: answer it as today, remove_user and an error response)."""
+        self.flush()
+        out = ["gone"] * len(players)
+        pos, hs = {}, []
+        for i, doc in enumerate(players):
+            h = self.handles.lookup(doc.get("id"))
+            rec = self.queued.get(h) if h is not None else None
+            if rec is None or h in pos or self._queue_of(rec[0], rec[1]) in self.moved_out:
+                continue
+            pos[h] = i
+            hs.append(h)
+        back = []  # window: (clock value, handle) of the requeued players
+        if hs:
+            rec = np.array([self.queued[h] for h in hs], np.int64)
+            codes = self.engine.requeue(np.array(hs, np.uint64), rec[:, 0].astype(np.int32), rec[:, 1].astype(np.uint8),
+                                        rec[:, 2].astype(np.uint32), rec[:, 3].astype(np.uint32))
+            for h, c in zip(hs, codes.tolist()):
+                if c == 1:
+                    out[pos[h]] = "requeued"
+                    self.players[h] = players[pos[h]]
+                    at = self.matched_at.pop(h, None)
+                    if self.window and at is not None:
+                        back.append((at, h))
+                elif c == 0:
+                    out[pos[h]] = "queued"
+        if back:  # into the oldest-first order the window reads: one merge of two sorted runs
+            back.sort()
+            self.enqueued_at = dict(heapq.merge(self.enqueued_at.items(), ((h, at) for at, h in back),
+                                                key=lambda kv: kv[1]))
+        for i, doc in enumerate(players):  # a repeated document shares its first copy's outcome
+            h = self.handles.lookup(doc.get("id"))
+            if h in pos and pos[h] != i:
+                out[i] = out[pos[h]]
+        self.stats["requeued"] = self.stats.get("requeued", 0) + out.count("requeued")
+        return out
+
+    def _queue_of(self, rating, mode):
+        """(mode, group) queue index of a rating: the first group that holds it, else the default group (-1: none)."""
+        cfg = self.engine.cfg
+        for g in range(cfg.n_groups):
+            if cfg.group_lo[g] <= rating <= cfg.group_hi[g]:
+                return int(mode) * cfg.n_groups + g
+        return int(mode) * cfg.n_groups + cfg.default_group if cfg.default_group >= 0 else -1
 
     # -- ingest -----------------------------------------------------------------------------
     def stage(self, worker, tag, player, game_mode, rating):
@@ -230,8 +288,11 @@ class SearchPool:
             ids[i] = h
         rating = np.clip(np.array([s[1] for s in staged], np.int64), -(2 ** 31), 2 ** 31 - 1).astype(np.int32)
         mode = np.array([self.mode_index.get(s[2], 255) if isinstance(s[2], str) else 255 for s in staged], np.uint8)
+        stamp = self.now_ms()
+        # every offered entry of an accepted batch takes one sequence number: entry i gets seq0 + i
+        seq0 = self.engine.seq_next() if hasattr(self.engine, "seq_next") else None
         try:
-            acc = self.engine.enqueue(ids, rating, mode, np.full(len(staged), self.now_ms(), np.uint32))
+            acc = self.engine.enqueue(ids, rating, mode, np.full(len(staged), stamp, np.uint32))
         except Exception:                       # nothing was enqueued (mm_enqueue refuses a batch as a whole)
             for pid in fresh:
                 self.handles.release(pid)
@@ -241,9 +302,11 @@ class SearchPool:
             return 0
         t_resident = self.clock() if self.window else None
         fresh = set(fresh)
-        for code, h, (pid, _r, _m, player, worker, tag) in zip(acc, ids.tolist(), staged):
+        for i, (code, h, (pid, _r, _m, player, worker, tag)) in enumerate(zip(acc, ids.tolist(), staged)):
             if code == 1:
                 self.players[h] = player
+                if seq0 is not None:
+                    self.queued[h] = [int(rating[i]), int(mode[i]), stamp, (seq0 + i) & 0xFFFFFFFF]
                 if self.window:
                     self.enqueued_at[h] = t_resident
                 self.stats["enqueued"] += 1
@@ -275,9 +338,11 @@ class SearchPool:
             group_name = self.group_names[h["group"]]
             first, n = int(h["first_member"]), int(h["n_members"])
             members = [self.players.pop(int(x)) for x in mem[first:first + n]]
-            if self.window:
+            if self.window:  # kept aside until remove_user: requeue() puts it back
                 for x in mem[first:first + n]:
-                    self.enqueued_at.pop(int(x), None)
+                    at = self.enqueued_at.pop(int(x), None)
+                    if at is not None:
+                        self.matched_at[int(x)] = at
             size = n // self._teams_of(h["mode"])
             teams = {f"team {t + 1}": members[t * size:(t + 1) * size] for t in range(n // size)}
             payload = json.dumps({"teams": teams, "game-mode": mode_name})      # worker.ex:315-318
@@ -293,6 +358,7 @@ class SearchPool:
         for h in expired.tolist():
             player = self.players.pop(h)
             self.enqueued_at.pop(h, None)
+            self.queued.pop(h, None)
             self.handles.release(self.handles.id_of[h])
             if player.get("response-queue") is not None:
                 worker = next(iter(self.workers.values()))
@@ -320,6 +386,9 @@ class SearchPool:
             "id_of": self.handles.id_of, "free": self.handles.free,
             "players": [[h, doc] for h, doc in self.players.items()],
             "enqueued_at": [[h, t - at] for h, at in self.enqueued_at.items()],  # age at the checkpoint, in order
+            "matched_at": [[h, t - at] for h, at in self.matched_at.items()],
+            "queued": [[h, rec] for h, rec in self.queued.items()],  # queued, or matched and not yet removed
+            "moved_out": sorted(self.moved_out),
             "now_ms": self.now_ms(), "wall": self.wall_clock(),
         }
         doc = json.dumps(state).encode()
@@ -348,6 +417,9 @@ class SearchPool:
         pool.players = {int(h): doc for h, doc in state["players"]}
         at = pool.clock() - down
         pool.enqueued_at = {int(h): at - age for h, age in state["enqueued_at"]}
+        pool.matched_at = {int(h): at - age for h, age in state.get("matched_at", [])}
+        pool.queued = {int(h): rec for h, rec in state.get("queued", [])}  # the image keeps every sequence number
+        pool.moved_out = set(state.get("moved_out", []))
         return pool
 
     # -- moving queues to another running pool -----------------------------------------------------
@@ -374,8 +446,10 @@ class SearchPool:
         _h, cols = read_image(image)
         t = self.clock()
         moved = []
+        self.moved_out |= set(np.flatnonzero(mask.reshape(-1)).tolist())
         for h in cols["id"].tolist():
             pid = self.handles.id_of[h]
+            self.queued.pop(h, None)
             at = self.enqueued_at.pop(h, None)
             moved.append([pid, self.players.pop(h), None if at is None else t - at])
             self.handles.release(pid)
@@ -417,6 +491,7 @@ class SearchPool:
         down = max(0.0, self.wall_clock() - state["wall"])
         shift = (self.now_ms() - int(round(down * 1000.0)) - int(state["now_ms"])) & 0xFFFFFFFF
         cols["enq_ts"][:] = (cols["enq_ts"].astype(np.uint64) + np.uint64(shift)).astype(np.uint32)
+        seq0 = self.engine.seq_next() if hasattr(self.engine, "seq_next") else None
         try:
             rejected = set(self.engine.merge_queues(image).tolist())
         except Exception:
@@ -424,6 +499,16 @@ class SearchPool:
                 self.handles.release(p)
             raise
         t = self.clock() - down
+        hdr = _h.config
+        grp = np.full(len(handles), hdr.default_group, np.int64)
+        for g in reversed(range(hdr.n_groups)):  # the first group that holds the rating
+            grp[(cols["rating"] >= hdr.group_lo[g]) & (cols["rating"] <= hdr.group_hi[g])] = g
+        queue = cols["mode"].astype(np.int64) * hdr.n_groups + grp
+        self.moved_out -= set(queue.tolist())
+        if seq0 is not None:  # mm_merge numbers its batch queue by queue, in the source's enqueue order in a queue
+            order = np.lexsort(((cols["seq"] - np.uint32(_h.seq_next)).astype(np.uint32), queue))
+            new_seq = np.empty(len(handles), np.int64)
+            new_seq[order] = (seq0 + np.arange(len(handles))) & 0xFFFFFFFF
         merged = 0
         for i, ((pid, doc, age), h, new) in enumerate(zip(players, handles, fresh)):
             if i in rejected:  # already queued here: keep this pool's player, drop the moved document
@@ -431,6 +516,8 @@ class SearchPool:
                     self.handles.release(pid)
                 continue
             self.players[h] = doc
+            if seq0 is not None:
+                self.queued[h] = [int(cols["rating"][i]), int(cols["mode"][i]), int(cols["enq_ts"][i]), int(new_seq[i])]
             if self.window and age is not None:
                 self.enqueued_at[h] = t - age
             merged += 1
