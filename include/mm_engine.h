@@ -356,6 +356,47 @@ typedef struct mm_queue_stat {
  * async_results copies alone.                                                                                     */
 int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap, uint32_t* n_out);
 
+/* ---- lobby budget: how many lobbies a tick may emit ------------------------------
+ * EXTENSION (flow control).  The reference emits one lobby at a time behind prefetch_count: 10 (search/worker.ex:29),
+ * and its lobby stage answers the players of a lobby it finds no game server for with an error
+ * (game-lobby/worker.ex:89-103,118-141); a request the strategist does not add stays a queued player
+ * (search/worker.ex:239-248,308-310).  Here the caller tells the tick how many lobbies it may emit — per (mode, group)
+ * queue, to pause or drain a rating group, and per game mode, because game servers host modes — and the rest stays
+ * queued, in order, with its waits and the search timeout running on.  Which players form a lobby, in which order and
+ * on which team is untouched (S0 and S1 alike): the budget only decides how many of a queue's lobbies, in their
+ * emission order, come out this tick.
+ *
+ * mm_set_lobby_budget: per_queue holds n_modes * n_groups entries in the record order of mm_queue_stats (mode *
+ * n_groups + group), per_mode holds n_modes; either may be NULL (= all unlimited).  Values are lobbies per tick;
+ * MM_BUDGET_UNLIMITED = no limit, 0 = the queue (mode) emits nothing.  Takes effect from the next tick and stays until
+ * set again.  It is an option in the sense of NOT IN THE IMAGE below: mm_export does not carry it, mm_snapshot /
+ * mm_restore leave it alone, an imported engine starts unlimited.  Default: unlimited, and then every result of every
+ * call is bit for bit what it is without this section.
+ *
+ * DEFINITION.  For queue q = (m, g) let c_q be the lobbies the tick would emit from it with no budget (under the
+ * current max_spread), c'_q = min(c_q, per_queue[q]) and C_m the sum of c'_q over the groups of mode m.  If C_m <=
+ * per_mode[m], a_q = c'_q.  Otherwise the mode's budget B = per_mode[m] is apportioned by largest remainder, in 64-bit
+ * integers: a_q = floor(B c'_q / C_m), and the B - sum(a_q) groups with the largest (B c'_q) mod C_m get one more, ties
+ * to the lower group index (then a_q <= c'_q and the a_q of the mode add up to B).  The tick emits the FIRST a_q
+ * LOBBIES of the queue in its emission order — the lobbies the unbudgeted tick would have put at the queue's first a_q
+ * header positions, same members, same member order, same emit_seq — and every other player of the queue stays queued
+ * in enqueue order, exactly as a residual player does.  Lobbies stay ordered by (mode, group, emission);
+ * mm_tick_stats.n_lobbies / n_matched / n_residual and the match section of mm_queue_stats count what was emitted and
+ * what stays.  The lobbies of mm_band_match are outside the tick and outside the budget.
+ *
+ * mm_lobby_budget_report: per queue, c_q (candidates) and a_q (emitted) of the last completed tick, zeros before the
+ * first tick and after one that failed; c_q - a_q is what the budget held back.  mm_lobby_candidates: c_q for the pool
+ * as it is now, budgets ignored — a dry run of the lobby cut on the resident per-key player counts that changes
+ * nothing: not the pool, not the last tick's results or the match section of mm_queue_stats, not pending
+ * async_results copies.  Removed-while-queued players are not counted, as the tick drops them.  It is what lets
+ * several engines share one mode budget: gather every engine's c_q, apportion once, set each engine's per-queue
+ * budgets.  Both: cap / n_out as in mm_queue_stats (MM_E_CAP and *n_out = n_modes * n_groups if cap is smaller);
+ * MM_E_STATE while an mm_enqueue_packed_begin batch is staged.  Refusals are decided before anything changes.      */
+#define MM_BUDGET_UNLIMITED 0xFFFFFFFFu
+int mm_set_lobby_budget(mm_engine* e, const uint32_t* per_queue, const uint32_t* per_mode);
+int mm_lobby_budget_report(mm_engine* e, uint32_t* candidates, uint32_t* emitted, uint32_t cap, uint32_t* n_out);
+int mm_lobby_candidates(mm_engine* e, uint32_t* candidates, uint32_t cap, uint32_t* n_out);
+
 /* ---- search timeout ------------------------------------------------------------
  * EXTENSION (search timeout): every live queued player whose WAIT at `now` (the definition of mm_queue_stats)
  * is >= max_wait leaves the pool AND the active set, as if mm_remove had been called with its id: mm_in_queue
@@ -413,7 +454,7 @@ int mm_restore(mm_engine* e);
  * NOT IN THE IMAGE: dead slots (players removed, taken or expired while queued: the next tick would drop them); the
  * last batch's reject list (mm_enqueue_rejects is empty after import); the last tick's match section of
  * mm_queue_stats (void after import, as after mm_restore); the mm_snapshot state; the options (max_spread, tick_impl,
- * rank_impl, async_results: the caller sets them again).
+ * rank_impl, async_results, the lobby budget: the caller sets them again).
  *
  * EQUIVALENCE.  After mm_import, every sequence of calls gives the same results on the imported engine as on the
  * source: enqueue codes, remove / take / expire outputs, in_queue, active_size, pool_read, the ticks' lobbies,

@@ -335,6 +335,54 @@ static ERL_NIF_TERM nif_requeue(ErlNifEnv* env, int argc, const ERL_NIF_TERM arg
   return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &codes));
 }
 
+/* set_lobby_budget(ref, per_queue :: binary(u32[n_modes * n_groups]) | <<>>, per_mode :: binary(u32[n_modes]) | <<>>)
+ * -> :ok: lobbies every queue / every mode may emit per tick from the next tick on (mm_set_lobby_budget); an empty
+ * binary = no limit, 0xFFFFFFFF in an entry = no limit for it.  The engine reads n_modes * n_groups / n_modes entries:
+ * any other non-empty length is a badarg (status/1 gives neither count, so the lengths come from queue_stats). */
+static ERL_NIF_TERM nif_set_lobby_budget(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary pq, pm; uint32_t nq = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &pq) ||
+      !enif_inspect_binary(env, argv[2], &pm))
+    return enif_make_badarg(env);
+  mm_lobby_candidates(r->e, NULL, 0, &nq);  /* cap 0: only the number of queues */
+  if ((pq.size && pq.size != (size_t)nq * 4) || pm.size % 4 || pm.size > 4 * MM_MAX_MODES || (pm.size && nq % (pm.size / 4)))
+    return enif_make_badarg(env);
+  uint32_t q[MM_MAX_GROUPS * MM_MAX_MODES], m[MM_MAX_MODES];
+  memcpy(q, pq.data, pq.size);
+  memcpy(m, pm.data, pm.size);
+  int rc = mm_set_lobby_budget(r->e, pq.size ? q : NULL, pm.size ? m : NULL);
+  return rc ? err(env, rc) : atom(env, "ok");
+}
+
+/* lobby_budget_report(ref) -> {:ok, candidates :: binary(u32[]), emitted :: binary(u32[])} per queue, of the last
+ * completed tick (mm_lobby_budget_report); lobby_candidates(ref) -> {:ok, binary(u32[])} for the pool as it is now,
+ * budgets ignored, nothing changes (mm_lobby_candidates). */
+static ERL_NIF_TERM nif_lobby_budget_report(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary c, a; uint32_t n = 0;
+  const uint32_t cap = MM_MAX_GROUPS * MM_MAX_MODES;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r)) return enif_make_badarg(env);
+  if (!enif_alloc_binary((size_t)cap * 4, &c)) return err(env, MM_E_CAP);
+  if (!enif_alloc_binary((size_t)cap * 4, &a)) { enif_release_binary(&c); return err(env, MM_E_CAP); }
+  int rc = mm_lobby_budget_report(r->e, (uint32_t*)c.data, (uint32_t*)a.data, cap, &n);
+  if (rc) { enif_release_binary(&c); enif_release_binary(&a); return err(env, rc); }
+  enif_realloc_binary(&c, (size_t)n * 4);
+  enif_realloc_binary(&a, (size_t)n * 4);
+  return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &c), enif_make_binary(env, &a));
+}
+static ERL_NIF_TERM nif_lobby_candidates(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary c; uint32_t n = 0;
+  const uint32_t cap = MM_MAX_GROUPS * MM_MAX_MODES;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r)) return enif_make_badarg(env);
+  if (!enif_alloc_binary((size_t)cap * 4, &c)) return err(env, MM_E_CAP);
+  int rc = mm_lobby_candidates(r->e, (uint32_t*)c.data, cap, &n);
+  if (rc) { enif_release_binary(&c); return err(env, rc); }
+  enif_realloc_binary(&c, (size_t)n * 4);
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &c));
+}
+
 /* set_max_spread(ref, w): extension knob (strategist policy S1); w < 0 restores the reference behaviour */
 static ERL_NIF_TERM nif_set_max_spread(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
   engine_res* r; ErlNifSInt64 w = -1;
@@ -365,5 +413,8 @@ static ErlNifFunc funcs[] = {
   {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"seq_next", 1, nif_seq_next, 0},
   {"set_max_spread", 2, nif_set_max_spread, 0},
+  {"set_lobby_budget", 3, nif_set_lobby_budget, 0},
+  {"lobby_budget_report", 1, nif_lobby_budget_report, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"lobby_candidates", 1, nif_lobby_candidates, ERL_NIF_DIRTY_JOB_CPU_BOUND},
 };
 ERL_NIF_INIT(Elixir.Matchmaking.Search.Engine, funcs, load, NULL, NULL, NULL)

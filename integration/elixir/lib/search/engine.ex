@@ -100,6 +100,18 @@ defmodule Matchmaking.Search.Engine do
   def n_modes, do: length(@modes)
   def n_groups, do: length(@rating_groups)
 
+  @doc """
+  Extension (flow control, mm_set_lobby_budget): lobbies every (mode, group) queue / every mode may emit per tick, from
+  the next tick until set again.  per_queue: binary(u32[n_modes * n_groups]), queue mode * n_groups + group; per_mode:
+  binary(u32[n_modes]); <<>> = no limit, 0xFFFFFFFF in an entry = no limit for it, 0 = emits nothing.  A mode's budget
+  is shared over its groups by largest remainder; a queue emits its first lobbies, everyone else stays queued.
+  """
+  def set_lobby_budget(_ref, _per_queue, _per_mode), do: :erlang.nif_error(:nif_not_loaded)
+  @doc "-> {:ok, candidates, emitted} (binary(u32[]) per queue) of the last tick: what it could have emitted and did."
+  def lobby_budget_report(_ref), do: :erlang.nif_error(:nif_not_loaded)
+  @doc "-> {:ok, binary(u32[])}: the lobbies a tick without a budget would emit from every queue now; changes nothing."
+  def lobby_candidates(_ref), do: :erlang.nif_error(:nif_not_loaded)
+
   @doc "Extension (not reference behaviour): maximum rating spread of a lobby for the following ticks; < 0 = off."
   def set_max_spread(_ref, _w), do: :erlang.nif_error(:nif_not_loaded)
 end

@@ -15,6 +15,11 @@ defmodule Matchmaking.Search.Pool do
       search_timeout_ms   option (extension, default nil = off): after each tick's lobbies are published, the players
                      still queued who have waited at least this long leave the pool (Engine.expire_packed) and get the
                      error response of game-lobby/worker.ex:63-71,105-116 on their "response-queue"
+      lobby_budget   option (extension, default nil = no limit): a zero-arity function -> %{mode name => lobbies}, asked
+                     before every tick — the free game-server slots (game-lobby/worker.ex:118-141).  The tick emits at
+                     most that many lobbies of the mode, shared over the rating groups in proportion to what each could
+                     emit (Engine.set_lobby_budget); the rest stay queued in order.  pause/1, resume_queues/1 stop and
+                     restart the queues of rating groups; a checkpoint carries neither
       checkpoint/0   hand-over: flushes the staged deliveries (so every acked player is in it), then returns
                      :erlang.term_to_binary of the engine image (Engine.export_image), the handle table, the player
                      documents, the pool clock and the wall time.  resume: <checkpoint> as an option of start_link/1
@@ -75,6 +80,9 @@ defmodule Matchmaking.Search.Pool do
   queued) or :gone (removed, timed out, never queued, or its queue has moved to another pool: answer it as today).
   """
   def requeue(players), do: GenServer.call(__MODULE__, {:requeue, players}, :infinity)
+  @doc "The queues of these rating groups (indices, all modes) emit no lobby until resume_queues/1; players stay queued."
+  def pause(groups), do: GenServer.call(__MODULE__, {:pause, groups, true})
+  def resume_queues(groups), do: GenServer.call(__MODULE__, {:pause, groups, false})
 
   @impl true
   def init(opts) do
@@ -83,7 +91,8 @@ defmodule Matchmaking.Search.Pool do
     # queued: handle -> {rating, mode, enq_ts, seq} at its enqueue, what requeue/1 hands back (kept until remove_user)
     st = %{ref: ref, staged: [], n_staged: 0, handle_of: %{}, players: %{}, free: [], next: 0, channel: nil,
            queued: %{}, moved_out: MapSet.new(),
-           t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms)}
+           t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms),
+           lobby_budget: Keyword.get(opts, :lobby_budget), paused: MapSet.new()}
     case resume(st, Keyword.get(opts, :resume)) do
       {:ok, st} ->
         Process.send_after(self(), :flush, @flush_ms)
@@ -319,10 +328,30 @@ defmodule Matchmaking.Search.Pool do
     Process.send_after(self(), :tick, @tick_ms)
     st = flush(st)
     now = now_ms(st)
+    if st.lobby_budget, do: set_budget(st, st.lobby_budget.())
     case Engine.tick_packed(st.ref, now) do
       {:ok, lobbies, members, _stats} -> {:noreply, expire(publish(lobbies, members, st), now)}
       {:error, _reason} -> {:noreply, st}                              # nothing was consumed; the next tick retries
     end
+  end
+
+  # -- lobby budget (extension): per-mode budgets from the callback, paused groups as per-queue budget 0 --------------
+  @unlimited 0xFFFFFFFF
+  defp set_budget(st, per_mode) do
+    n_groups = Engine.n_groups()
+    per_queue = for _m <- 0..(Engine.n_modes() - 1), g <- 0..(n_groups - 1), into: <<>>,
+                    do: <<(if MapSet.member?(st.paused, g), do: 0, else: @unlimited)::little-32>>
+    modes = if per_mode == nil, do: <<>>, else:
+      (for m <- 0..(Engine.n_modes() - 1), into: <<>>,
+           do: <<min(max(Map.get(per_mode, Engine.mode_name(m), @unlimited), 0), @unlimited)::little-32>>)
+    :ok = Engine.set_lobby_budget(st.ref, per_queue, modes)
+  end
+
+  def handle_call({:pause, groups, on}, _from, st) do
+    paused = if on, do: MapSet.union(st.paused, MapSet.new(groups)), else: MapSet.difference(st.paused, MapSet.new(groups))
+    st = %{st | paused: paused}
+    if st.lobby_budget == nil, do: set_budget(st, nil)   # with a callback the next tick sets both together
+    {:reply, :ok, st}
   end
 
   # -- search timeout (extension): after the lobbies, so a player the tick matched is never timed out ---------------

@@ -24,6 +24,8 @@ MM_F_NO_DEDUPE = 1
 MM_F_DENSE_IDS = 2
 MM_F_WIDE_PARTITIONS = 4
 
+MM_BUDGET_UNLIMITED = 0xFFFFFFFF
+
 
 class ModeDesc(C.Structure):
     _fields_ = [("teams", C.c_uint16), ("team_size", C.c_uint16)]
@@ -169,6 +171,9 @@ PROTOTYPES = {
     "mm_results_device": (C.c_int, [_vp, _P(_vp), _P(_vp)]),
     "mm_pool_read": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _P(C.c_uint32)]),
     "mm_queue_stats": (C.c_int, [_vp, C.c_uint64, _vp, C.c_uint32, _P(C.c_uint32)]),
+    "mm_set_lobby_budget": (C.c_int, [_vp, _vp, _vp]),
+    "mm_lobby_budget_report": (C.c_int, [_vp, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
+    "mm_lobby_candidates": (C.c_int, [_vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_expire": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_expire_packed": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_export": (C.c_int, [_vp, _vp, C.c_uint64, _P(C.c_uint64)]),

@@ -213,6 +213,16 @@ struct mm_engine {
   uint32_t match_n = 0;      // players resident when that tick started: bounds its tile count
   DevArray<uint32_t> d_qstat;  // [n_cut] records
 
+  // lobby budget (mm_set_lobby_budget): lobbies a queue / a mode may emit per tick.  An empty host vector = no limit
+  // anywhere; the device copy is brought up to date by the next tick.  Not part of images or snapshots.
+  std::vector<uint32_t> bud_queue, bud_mode;  // [n_cut], [n_modes]
+  bool bud_stale = false;
+  DevArray<uint32_t> d_bud;       // [n_cut] per queue | [n_modes] per mode
+  DevArray<uint32_t> d_cand;      // [n_cut] budgeted ticks: lobbies every queue had, budgets ignored
+  DevArray<uint32_t> d_cand_dry;  // mm_lobby_candidates: [n_cut] counts | [Kp + 1] parked matched counts (tail layout 0)
+  bool report_valid = false;      // the last tick completed: d_seg (and d_cand, if report_budgeted) describe it
+  bool report_budgeted = false;
+
   // mm_expire output (grown on demand to the largest output a call could write; not d_members / d_hdr, which
   // mm_results_device hands out until the next tick)
   DevArray<uint64_t> d_exp_id;  // ids, or 32-bit handles in its first half
@@ -687,7 +697,26 @@ TailArgs tail_args(mm_engine* e) {
   t.bin_key = e->d_bin_key; t.outbase = e->d_outbase; t.binlim = e->d_binlim; t.seg = e->d_seg; t.ctr = e->d_ctr;
   t.fill = e->pool[e->cur].m.fill;
   t.dst = e->pool[e->cur ^ 1].m;
+  t.n_groups = e->cfg.n_groups;
+  t.bud_queue = e->bud_queue.empty() ? nullptr : e->d_bud.p;
+  t.bud_mode = e->bud_mode.empty() ? nullptr : e->d_bud.p + e->n_cut;
+  t.cand = e->d_cand;
   return t;
+}
+// the budgets set since the last tick -> their device copy (before a tick's launches)
+int budget_upload(mm_engine* e) {
+  e->report_budgeted = !e->bud_queue.empty() || !e->bud_mode.empty();
+  if (!e->bud_stale) return MM_OK;
+  e->bud_stale = false;
+  if (!e->report_budgeted) return MM_OK;
+  CK(e->d_bud.reserve(e->n_cut + e->cfg.n_modes));
+  CK(e->d_cand.reserve(e->n_cut));
+  if (!e->bud_queue.empty())
+    CK(cudaMemcpyAsync(e->d_bud, e->bud_queue.data(), (size_t)e->n_cut * 4, cudaMemcpyHostToDevice, e->stream));
+  if (!e->bud_mode.empty())
+    CK(cudaMemcpyAsync(e->d_bud + e->n_cut, e->bud_mode.data(), (size_t)e->cfg.n_modes * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaStreamSynchronize(e->stream));  // the host vectors may change as soon as the tick returns
+  return MM_OK;
 }
 // Rows (CTAs) a tick uses: small pools do not pay the grid barriers and per-row set-up of the full grid.  About two
 // tiles per row at least; the tile count is bounded from the host-side player count.
@@ -728,12 +757,15 @@ EpiArgs epi_args(mm_engine* e, bool want_seq, bool headers) {
 // launches k_hist + k_colscan (phase A of a tick): the counters are final afterwards
 int tick_phase_a(mm_engine* e) {
   const Pool& p = e->pool[e->cur];
+  { const int rc = budget_upload(e); if (rc) return rc; }
   CK(cudaMemsetAsync(e->d_ctr, 0, sizeof(TickCtr), e->stream));
   CK(cudaEventRecord(e->ev[0], e->stream));
   const uint32_t rows = tick_rows(e);
   k_hist<512><<<rows, 512, hist_smem_bytes(e->max_nb), e->stream>>>(p.v.bin, p.m, e->n_segs, rows, e->Kp, e->max_nb, e->d_seg_bin_lo, e->d_M);
   CK(cudaEventRecord(e->ev[1], e->stream));
-  k_colscan<<<(e->K + 31) / 32 + 1, kScanBlock, colscan_smem(e), e->stream>>>(rows, e->d_M, e->d_P, tail_args(e));
+  const uint32_t scan_ctas = (e->K + 31) / 32 + 1;
+  if (e->report_budgeted) k_colscan<true><<<scan_ctas, kScanBlock, colscan_smem(e), e->stream>>>(rows, e->d_M, e->d_P, tail_args(e));
+  else k_colscan<false><<<scan_ctas, kScanBlock, colscan_smem(e), e->stream>>>(rows, e->d_M, e->d_P, tail_args(e));
   CK(cudaGetLastError());
   return MM_OK;
 }
@@ -760,6 +792,7 @@ bool use_fused(const mm_engine* e) { return e->tick_impl == 1 && e->fused_ok; }
 // the whole tick in one cooperative launch (k_tick)
 int tick_fused(mm_engine* e, bool want_seq) {
   TickArgs a{};
+  { const int rc = budget_upload(e); if (rc) return rc; }
   const uint32_t rows = tick_rows(e);
   // a grid that does not fill the GPU spends the spare CTA slots on helpers: at a few tiles per row the lobby headers
   // (one per L players) are as much work as the placement
@@ -777,7 +810,8 @@ int tick_fused(mm_engine* e, bool want_seq) {
   a.next_ctr = e->d_ctr2 + (e->ctr_idx ^ 1);
   CK(cudaEventRecord(e->ev[0], e->stream));
   void* params[] = {&a};
-  CK(cudaLaunchCooperativeKernel((const void*)k_tick<512>, dim3(rows + helpers), dim3(512), params, e->tick_smem, e->stream));
+  const void* kernel = e->report_budgeted ? (const void*)k_tick<512, true> : (const void*)k_tick<512>;
+  CK(cudaLaunchCooperativeKernel(kernel, dim3(rows + helpers), dim3(512), params, e->tick_smem, e->stream));
   CK(cudaEventRecord(e->ev[4], e->stream));
   CK(cudaMemcpyAsync(e->h_ctr, e->d_ctr, sizeof(TickCtr), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
@@ -826,6 +860,7 @@ int tick_commit(mm_engine* e, uint32_t n, mm_tick_stats* stats) {
   e->pool[e->cur].n = c.n_resid;
   e->pool[e->cur].held = 0;
   e->match_valid = true;  // pool[cur ^ 1] is now the pool this tick matched
+  e->report_valid = true;
   e->match_n = n;
   e->last = st;
   if (stats) *stats = st;
@@ -841,6 +876,7 @@ int tick_commit(mm_engine* e, uint32_t n, mm_tick_stats* stats) {
 void tick_begin(mm_engine* e, uint64_t now) {
   e->tick_now = (uint32_t)now;
   e->match_valid = false;
+  e->report_valid = false;
 }
 
 // async_results: the previous tick's host copies must land before its device buffers are overwritten
@@ -1759,8 +1795,10 @@ int mm_create(const mm_config* cfg, mm_engine** out) {
       if (place_smem_bytes(e->max_nb, st) + static_smem + 1024 <= e->smem_optin) { e->place_stages = st; e->rows_per_sm = 1; }
     if (!e->place_stages || colscan_smem(e) + static_smem + 1024 > e->smem_optin)
       return bail(set_err(e, MM_E_ARG, "key domain too large for shared memory: %u bins", e->Kp));
-    bool ok = allow_max_smem(e, k_colscan) == cudaSuccess && allow_max_smem(e, k_hist<512>) == cudaSuccess &&
-              allow_max_smem(e, k_place<512>) == cudaSuccess && allow_max_smem(e, k_tick<512>) == cudaSuccess;
+    bool ok = allow_max_smem(e, k_colscan<false>) == cudaSuccess && allow_max_smem(e, k_colscan<true>) == cudaSuccess &&
+              allow_max_smem(e, k_lobby_candidates) == cudaSuccess && allow_max_smem(e, k_hist<512>) == cudaSuccess &&
+              allow_max_smem(e, k_place<512>) == cudaSuccess && allow_max_smem(e, k_tick<512>) == cudaSuccess &&
+              allow_max_smem(e, k_tick<512, true>) == cudaSuccess;
     if (!ok) return bail(fail(e, cudaGetLastError(), "cudaFuncSetAttribute"));
   }
   e->n_chunks = (e->capacity + kTile - 1) / kTile + e->n_segs + 2;
@@ -1771,8 +1809,10 @@ int mm_create(const mm_config* cfg, mm_engine** out) {
     sz = std::max<size_t>(sz, std::max<size_t>((size_t)std::max(kEpiScratchWords, kRowCompactWords) * 4, colscan_smem(e)));
     int coop = 0, nb = 0;
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, e->device);
+    int nb_bud = 0;  // both forms of the fused kernel must fit: a budget must not change which tick form runs
     if (coop && cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, k_tick<512>, 512, sz) == cudaSuccess &&
-        (uint32_t)nb * (uint32_t)e->n_sms >= e->R + e->helpers) {
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb_bud, k_tick<512, true>, 512, sz) == cudaSuccess &&
+        (uint32_t)std::min(nb, nb_bud) * (uint32_t)e->n_sms >= e->R + e->helpers) {
       e->fused_ok = 1;
       e->tick_smem = sz;
     }
@@ -2185,6 +2225,64 @@ int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap,
     out[c].group = (uint8_t)(c % G);
     out[c].n_lobbies = out[c].n_matched / ((uint32_t)md.teams * md.team_size);  // whole lobbies of L players
   }
+  return MM_OK;
+}
+
+int mm_set_lobby_budget(mm_engine* e, const uint32_t* per_queue, const uint32_t* per_mode) {
+  if (!e) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  // an array without a limit in it is kept as "no array": the tick then takes its unbudgeted path
+  auto keep = [](std::vector<uint32_t>& v, const uint32_t* src, uint32_t n) {
+    v.clear();
+    if (src && std::any_of(src, src + n, [](uint32_t b) { return b != MM_BUDGET_UNLIMITED; })) v.assign(src, src + n);
+  };
+  keep(e->bud_queue, per_queue, e->n_cut);
+  keep(e->bud_mode, per_mode, e->cfg.n_modes);
+  e->bud_stale = true;
+  return MM_OK;
+}
+
+int mm_lobby_budget_report(mm_engine* e, uint32_t* candidates, uint32_t* emitted, uint32_t cap, uint32_t* n_out) {
+  if (!e || !n_out || (cap && (!candidates || !emitted))) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const uint32_t n_cut = e->n_cut;
+  *n_out = n_cut;
+  if (cap < n_cut) return set_err(e, MM_E_CAP, "need cap >= %u", n_cut);
+  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  std::fill(candidates, candidates + n_cut, 0u);
+  std::fill(emitted, emitted + n_cut, 0u);
+  if (!e->report_valid) return MM_OK;
+  CK(cudaSetDevice(e->device));
+  // emitted: the partition table the tick wrote (a queue's lobbies are credited to the partitions they start in)
+  std::vector<SegInfo> seg(e->n_segs);
+  CK(cudaMemcpyAsync(seg.data(), e->d_seg, (size_t)e->n_segs * sizeof(SegInfo), cudaMemcpyDeviceToHost, e->stream));
+  if (e->report_budgeted) CK(cudaMemcpyAsync(candidates, e->d_cand, (size_t)n_cut * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  for (uint32_t s = 0; s < e->n_segs; ++s) emitted[e->h_part_cut[s]] += seg[s].n_lobbies;
+  if (!e->report_budgeted) std::copy(emitted, emitted + n_cut, candidates);
+  return MM_OK;
+}
+
+int mm_lobby_candidates(mm_engine* e, uint32_t* candidates, uint32_t cap, uint32_t* n_out) {
+  if (!e || !n_out || (cap && !candidates)) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const uint32_t n_cut = e->n_cut;
+  *n_out = n_cut;
+  if (cap < n_cut) return set_err(e, MM_E_CAP, "need cap >= %u", n_cut);
+  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  CK(cudaSetDevice(e->device));
+  const uint32_t layout = tail_layout(e);
+  CK(e->d_cand_dry.reserve(n_cut + (layout & 1u ? 0u : e->Kp + 1)));
+  TailArgs t = tail_args(e);
+  // count only: the tail writes the counts (and, for a key domain too large for shared memory, its parked matched
+  // counts) into this call's own scratch; the tick's outputs and the compacted pool's layout are not touched
+  t.cand = e->d_cand_dry; t.binlim = e->d_cand_dry + n_cut;
+  t.bud_queue = t.bud_mode = nullptr;
+  t.outbase = nullptr; t.seg = nullptr; t.ctr = nullptr; t.dst = PoolMeta{};
+  k_lobby_candidates<<<1, kScanBlock, (size_t)tail_words(e->Kp, layout) * 4, e->stream>>>(t);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(candidates, e->d_cand_dry, (size_t)n_cut * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
   return MM_OK;
 }
 

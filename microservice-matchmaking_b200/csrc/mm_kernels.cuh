@@ -82,7 +82,8 @@ struct TickArgs {
   TickCtr* next_ctr;  // the OTHER counter block (ticks alternate): re-armed by the last CTA so no memset precedes a launch
 };
 
-template <int BLOCK>
+// kBudget: the tail with the lobby-budget code (mm_scan.cuh); launched only when a budget is set
+template <int BLOCK, bool kBudget = false>
 __global__ void __launch_bounds__(BLOCK, 2) k_tick(const TickArgs a) {
   static_assert(BLOCK == kScanBlock, "the column-scan phase is written for 512-thread CTAs");
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -105,7 +106,7 @@ __global__ void __launch_bounds__(BLOCK, 2) k_tick(const TickArgs a) {
   stamp(0);
   const bool tail_cta = blockIdx.x == G - 1;
   auto run_tail = [&]() {
-    colscan_tail_body(scratch, a.tail);
+    colscan_tail_body<false, kBudget>(scratch, a.tail);
     if (threadIdx.x == 0) {
       unsigned long long t;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));

@@ -81,6 +81,11 @@ struct TailArgs {
   TickCtr* ctr;
   const uint32_t* fill;               // [n_segs] partition fills of the pool being matched
   PoolMeta dst;                       // out: layout of the compacted pool (fill, chunk table, chunks used)
+  // lobby budget (flow control), read only by the tail instantiations with kBudget / kCountOnly
+  const uint32_t* bud_queue;          // [n_cut] lobbies a (mode, group) queue may emit this tick (0xFFFFFFFF: no limit), or null
+  const uint32_t* bud_mode;           // [n_cut / n_groups] lobbies a mode may emit this tick, or null
+  uint32_t n_groups;                  // cut segment c = mode * n_groups + group
+  uint32_t* cand;                     // [n_cut] out (budgeted tick, count-only tail): lobbies the queue has, budgets ignored
 };
 // shared-memory words of the tail for a layout: bases | matched counts (bit 0) | keys (bit 1)
 __host__ __device__ constexpr uint32_t tail_words(uint32_t Kp, uint32_t layout) {
@@ -118,6 +123,125 @@ __device__ __forceinline__ uint32_t s1_step(uint32_t& pos, uint32_t B0, uint32_t
   return m;
 }
 
+// Tables of the tail in its scratch (word offsets; the per-bin arrays follow at kTailScratchWords)
+constexpr uint32_t kTailLo = 68 + 3 * kMaxSegs;           // s_lo  [kMaxSegs + 1] first bin of the partition
+constexpr uint32_t kTailNch = kTailLo + kMaxSegs + 1;     // s_nch [kMaxSegs + 1]
+constexpr uint32_t kTailL = kTailNch + kMaxSegs + 1;      // s_L   [kMaxSegs] lobby size of the partition
+constexpr uint32_t kTailClp = kTailL + 2 * kMaxSegs;      // s_clp [kMaxSegs + 1] first partition of the cut segment
+constexpr uint32_t kTailMs = kTailClp + kMaxSegs + 1;     // s_ms  [kMaxSegs + 1]
+// The lobby budget keeps two per-queue arrays where the partition table later puts s_ms / s_nch (they are spent by then):
+constexpr uint32_t kTailCand = kTailMs;    // s_c  [n_cut] lobbies of the queue, budgets ignored
+constexpr uint32_t kTailAllot = kTailNch;  // s_al [n_cut] lobbies it may emit
+
+// Lobbies of every (mode, group) queue from the tail's tables -> out[c] (shared or global).  S0: the queue's players /
+// L, from the bases s_bb; S1 (s_m: the bins' matched counts after the walk): its matched players / L, one warp per queue.
+__device__ __forceinline__ void tail_count_lobbies(const uint32_t* scratch, const uint32_t* s_m, uint32_t n_cut,
+                                                   bool windowed, uint32_t* out) {
+  const uint32_t *s_lo = scratch + kTailLo, *s_L = scratch + kTailL, *s_clp = scratch + kTailClp;
+  const uint32_t* s_bb = scratch + kTailScratchWords;
+  const uint32_t lane = threadIdx.x & 31;
+  if (!windowed) {
+    for (uint32_t c = threadIdx.x; c < n_cut; c += kScanBlock)
+      out[c] = (s_bb[s_lo[s_clp[c + 1]]] - s_bb[s_lo[s_clp[c]]]) / s_L[s_clp[c]];
+    return;
+  }
+  for (uint32_t c = threadIdx.x >> 5; c < n_cut; c += kScanBlock / 32) {
+    uint32_t sum = 0;
+    for (uint32_t v = s_lo[s_clp[c]] + lane; v < s_lo[s_clp[c + 1]]; v += 32) sum += s_m[v];
+    sum = __reduce_add_sync(0xFFFFFFFFu, sum);
+    if (lane == 0) out[c] = sum / s_L[s_clp[c]];
+  }
+}
+
+// Lobby budget, the whole block, called with the tail's tables and (S1) matched counts in place:
+//   s_c[q]  = lobbies queue q = m * G + g would emit (also written to cand[q])
+//   s_al[q] = lobbies it may emit.  c' = min(c, bud_queue[q]); if the mode's sum C of c' exceeds its budget B, B is
+//             apportioned by largest remainder: floor(B c' / C) each, and the B - sum groups with the largest
+//             (B c') mod C get one more, ties to the lower group.  One warp per mode (<= 64 groups: two per lane,
+//             remainder ranks by comparison).  Restated on the host by shard.apportion.
+//   S0 clip: the queue's matched end moves to its (a_q L)-th sorted position: the partitions' matched counts s_mt,
+//             which the caller has filled for the unbudgeted cut, are written again.
+//   S1 clip: one warp per queue, bin v keeps the matched players that come before the queue's (a_q L)-th matched
+//             player: m'_v = clamp(a_q L - matched players of the queue's earlier bins, 0, m_v).
+// Not inlined, and no argument is passed by address: the budget instantiation of the fused kernel keeps the register
+// allocation of its placement loops.
+__device__ __noinline__ void tail_budget(uint32_t* scratch, uint32_t* s_m, uint32_t n_cut, uint32_t n_segs, uint32_t G,
+                                         bool windowed,
+                                         const uint32_t* bud_queue, const uint32_t* bud_mode, uint32_t* cand) {
+  const uint32_t *s_lo = scratch + kTailLo, *s_L = scratch + kTailL, *s_clp = scratch + kTailClp;
+  uint32_t *s_c = scratch + kTailCand, *s_al = scratch + kTailAllot;
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  tail_count_lobbies(scratch, s_m, n_cut, windowed, s_c);
+  __syncthreads();
+  if (warp < n_cut / G) {
+    const uint32_t m = warp;
+    uint32_t c[2], al[2], C = 0;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint32_t g = lane + 32 * j;
+      c[j] = g < G ? s_c[m * G + g] : 0u;
+      if (g < G && bud_queue) { const uint32_t b = bud_queue[m * G + g]; c[j] = c[j] < b ? c[j] : b; }
+      al[j] = c[j];
+      C += c[j];
+    }
+    C = __reduce_add_sync(0xFFFFFFFFu, C);  // < 2^31: every lobby has a player of its own
+    const uint32_t B = bud_mode ? bud_mode[m] : 0xFFFFFFFFu;
+    if (C > B) {  // (uniform over the warp)
+      uint32_t rem[2], fl = 0;
+#pragma unroll
+      for (int j = 0; j < 2; ++j) {
+        const uint64_t p = (uint64_t)B * c[j];
+        al[j] = (uint32_t)(p / C); rem[j] = (uint32_t)(p % C);
+        fl += al[j];
+      }
+      const uint32_t extra = B - __reduce_add_sync(0xFFFFFFFFu, fl);  // fewer than the groups with a remainder
+      uint32_t rank[2] = {0u, 0u};  // groups that come before this one by (remainder descending, group ascending)
+      for (int l = 0; l < 32; ++l)
+#pragma unroll
+        for (int k = 0; k < 2; ++k) {
+          const uint32_t r = __shfl_sync(0xFFFFFFFFu, rem[k], l), g2 = l + 32 * k;
+#pragma unroll
+          for (int j = 0; j < 2; ++j) rank[j] += (r > rem[j] || (r == rem[j] && g2 < lane + 32 * j)) ? 1u : 0u;
+        }
+#pragma unroll
+      for (int j = 0; j < 2; ++j) al[j] += rank[j] < extra ? 1u : 0u;
+    }
+#pragma unroll
+    for (int j = 0; j < 2; ++j)
+      if (lane + 32 * j < G) s_al[m * G + lane + 32 * j] = al[j];
+  }
+  for (uint32_t q = threadIdx.x; q < n_cut; q += kScanBlock) cand[q] = s_c[q];
+  __syncthreads();
+  if (!windowed) {  // the partitions' matched counts again, with the queue's matched end at a_q L
+    const uint32_t *s_bb = scratch + kTailScratchWords, *s_pc = scratch + kTailL + kMaxSegs;
+    uint32_t* s_mt = scratch + 68 + 2 * kMaxSegs;
+    for (uint32_t sg = threadIdx.x; sg < n_segs; sg += kScanBlock) {
+      const uint32_t q = s_pc[sg], mend = s_bb[s_lo[s_clp[q]]] + s_al[q] * s_L[sg];
+      const uint32_t a = s_bb[s_lo[sg]], b = s_bb[s_lo[sg + 1]];
+      s_mt[sg] = (mend < a ? a : (mend > b ? b : mend)) - a;
+    }
+    return;
+  }
+  for (uint32_t q = warp; q < n_cut; q += kScanBlock / 32) {
+    if (s_al[q] == s_c[q]) continue;
+    const uint32_t lo = s_lo[s_clp[q]], hi = s_lo[s_clp[q + 1]], limit = s_al[q] * s_L[s_clp[q]];
+    uint32_t before = 0;
+    for (uint32_t off = lo; off < hi; off += 32) {
+      const uint32_t v = off + lane, m = v < hi ? s_m[v] : 0u;
+      uint32_t incl = m;
+#pragma unroll
+      for (int d = 1; d < 32; d <<= 1) {
+        const uint32_t up = __shfl_up_sync(0xFFFFFFFFu, incl, d);
+        if (lane >= (uint32_t)d) incl += up;
+      }
+      const uint32_t b = before + incl - m, room = b < limit ? limit - b : 0u;
+      if (v < hi) s_m[v] = m < room ? m : room;
+      before += __shfl_sync(0xFFFFFFFFu, incl, 31);
+    }
+  }
+  __syncthreads();
+}
+
 // The tail.  One pipeline for both policies:
 //   bin totals -> bases s_bb -> matched prefix of every bin -> member slot of the bin's first player.
 // S0 (reference behaviour): a (mode, group) partition of n players emits floor(n/L) lobbies, the n mod L
@@ -128,6 +252,13 @@ __device__ __forceinline__ uint32_t s1_step(uint32_t& pos, uint32_t B0, uint32_t
 //   cur, cur+L, ... while the seed is still in bin v and its L-th player has key <= key_v + W; whatever is
 //   left of bin v afterwards cannot seed and stays queued.  Two-pointer over the bins of the segment.
 // Very large key domains (layout bit 0 clear) park m_v in global memory and scan it in place of the bases.
+// Lobby budget (t.bud_queue / t.bud_mode): under both policies the first a lobbies of a cut segment are its first a L
+// matched players in sorted order, so an allowance a_q clips the matched counts — S0: the segment's matched end; S1:
+// the bins' matched counts past a_q L, before they are scanned into member slots — and everything downstream sees a
+// smaller matched prefix per bin.  kBudget selects the tail with the budget code: a tick without a budget runs the
+// instantiation without it, instruction for instruction the tail it has always run.  kCountOnly (k_lobby_candidates): stop at the per-queue lobby counts, write t.cand
+// (and, for layout bit 0 clear, the parked counts in t.binlim) and nothing else.
+template <bool kCountOnly = false, bool kBudget = false>
 __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailArgs t) {
   constexpr uint32_t NW = kScanBlock / 32;
   uint32_t* s_tmp = scratch;            // [64]
@@ -135,13 +266,14 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
   uint32_t* s_a = scratch + 68;         // [kMaxSegs] leftovers of earlier segments
   uint32_t* s_ns = s_a + kMaxSegs;      // [kMaxSegs] alive players of the segment
   uint32_t* s_mt = s_ns + kMaxSegs;     // [kMaxSegs] matched players of the segment
-  uint32_t* s_lo = s_mt + kMaxSegs;     // [kMaxSegs + 1] first bin of the segment
-  uint32_t* s_nch = s_lo + kMaxSegs + 1;   // [kMaxSegs + 1] first chunk of the segment in the compacted pool
-  uint32_t* s_L = s_nch + kMaxSegs + 1;    // [kMaxSegs] lobby size of the segment
+  uint32_t* s_lo = scratch + kTailLo;      // [kMaxSegs + 1] first bin of the segment
+  uint32_t* s_nch = scratch + kTailNch;    // [kMaxSegs + 1] first chunk of the segment in the compacted pool
+  uint32_t* s_L = scratch + kTailL;        // [kMaxSegs] lobby size of the segment
   uint32_t* s_pc = s_L + kMaxSegs;         // [kMaxSegs] cut segment of the partition
-  uint32_t* s_clp = s_pc + kMaxSegs;       // [kMaxSegs + 1] first partition of the cut segment
-  uint32_t* s_ms = s_clp + kMaxSegs + 1;   // [kMaxSegs + 1] member slot of the partition's first matched player
+  uint32_t* s_clp = scratch + kTailClp;    // [kMaxSegs + 1] first partition of the cut segment
+  uint32_t* s_ms = scratch + kTailMs;      // [kMaxSegs + 1] member slot of the partition's first matched player
   uint32_t* s_bb = scratch + kTailScratchWords;  // [Kp + 1] sorted position of the bin's first player
+  static_assert(kTailMs + kMaxSegs + 1 <= kTailScratchWords, "the tail's tables end before its per-bin arrays");
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, Kp = t.Kp, K = t.K, n_segs = t.n_segs;
   if (tid == 0) s_misc[0] = 0;
   for (uint32_t sg = tid; sg <= n_segs; sg += kScanBlock) s_lo[sg] = t.seg_bin_lo[sg];  // all the cold loads at once
@@ -150,7 +282,7 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
   for (uint32_t i = tid; i < Kp; i += kScanBlock) s_bb[i] = __ldcg(&t.tot[i]);  // coalesced, independent loads
   __syncthreads();
   // list-ranked partitions only: does some bin expect > 8 players per tile of its partition?
-  for (uint32_t sg = warp; sg < n_segs; sg += NW) {
+  for (uint32_t sg = warp; !kCountOnly && sg < n_segs; sg += NW) {
     if (s_lo[sg + 1] - s_lo[sg] <= kFastBins) continue;
     uint32_t mx = 0;
     for (uint32_t v = s_lo[sg] + lane; v < s_lo[sg + 1]; v += 32) mx = s_bb[v] > mx ? s_bb[v] : mx;
@@ -167,8 +299,8 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
   uint32_t* s_m = m_smem ? s_bb + Kp + 2 : t.binlim;  // S1: [Kp + 1] matched players of the bin
 
   if (!windowed) {
-    // S0: a cut segment of n players gives n / L lobbies: its first (n / L) * L sorted positions are matched; a
-    // partition holds the part of that prefix that falls into its own position range.
+    if (kCountOnly) { tail_count_lobbies(scratch, nullptr, t.n_cut, false, t.cand); return; }
+    // S0: a cut segment of n players gives n / L lobbies: its first (n / L) * L sorted positions are matched; a partition holds the part of that prefix that falls into its own position range.
     for (uint32_t sg = tid; sg < n_segs; sg += kScanBlock) {
       const uint32_t c = s_pc[sg], cs = s_bb[s_lo[s_clp[c]]], ce = s_bb[s_lo[s_clp[c + 1]]], L = s_L[sg];
       const uint32_t mend = cs + (ce - cs) / L * L;
@@ -176,6 +308,7 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
       s_ns[sg] = b - a;
       s_mt[sg] = (mend < a ? a : (mend > b ? b : mend)) - a;
     }
+    if constexpr (kBudget) tail_budget(scratch, nullptr, t.n_cut, t.n_segs, t.n_groups, false, t.bud_queue, t.bud_mode, t.cand);
   } else {
     uint16_t* s_key = reinterpret_cast<uint16_t*>(s_bb + (m_smem ? 2 : 1) * (Kp + 2));
     const uint16_t* keys = key_smem ? s_key : t.bin_key;
@@ -234,6 +367,8 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
       s_m = s_bb;
       __syncthreads();
     }
+    if (kCountOnly) { tail_count_lobbies(scratch, s_m, t.n_cut, true, t.cand); return; }
+    if constexpr (kBudget) tail_budget(scratch, s_m, t.n_cut, t.n_segs, t.n_groups, true, t.bud_queue, t.bud_mode, t.cand);
     // member slots = exclusive scan of the matched counts (members of successive partitions are contiguous)
     const uint32_t nm = block_excl_scan<kScanBlock>(s_m, Kp, s_tmp);
     if (tid == 0) s_m[Kp] = nm;
@@ -333,6 +468,7 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
   __syncthreads();
 }
 
+template <bool kBudget>
 __global__ void __launch_bounds__(kScanBlock) k_colscan(uint32_t R, const uint32_t* __restrict__ M, uint32_t* __restrict__ P,
                                                         const TailArgs t) {
   extern __shared__ __align__(16) uint32_t scratch[];  // max(kColScratchWords, tail_words(Kp, layout)) words
@@ -342,8 +478,14 @@ __global__ void __launch_bounds__(kScanBlock) k_colscan(uint32_t R, const uint32
     geo_build<kScanBlock>(geo, t.fill, t.n_segs, R, s_gtmp);
     if (geo_use_colscan(geo)) colscan_cols_body(scratch, geo, blockIdx.x, t.Kp, t.K, t.bin_seg, M, P);
   } else {
-    colscan_tail_body(scratch, t);
+    colscan_tail_body<false, kBudget>(scratch, t);
   }
+}
+
+// mm_lobby_candidates: the tail up to the per-queue lobby counts, on the resident bin totals (tail_words words)
+__global__ void __launch_bounds__(kScanBlock) k_lobby_candidates(const TailArgs t) {
+  extern __shared__ __align__(16) uint32_t scratch[];
+  colscan_tail_body<true>(scratch, t);
 }
 
 }  // namespace mm

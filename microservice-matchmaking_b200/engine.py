@@ -430,6 +430,40 @@ class Engine:
                     "mm_queue_stats")
         return out[:n.value]
 
+    # -- lobby budget ----------------------------------------------------------------
+    def set_lobby_budget(self, per_queue=None, per_mode=None):
+        """Lobbies every (mode, group) queue / every mode may emit per tick, from the next tick until set again
+        (mm_set_lobby_budget).  per_queue: n_modes * n_groups values in queue_stats() record order (or
+        [n_modes][n_groups]); per_mode: n_modes values; None, or abi.MM_BUDGET_UNLIMITED in an entry = no limit."""
+        def arr(a, n):
+            if a is None:
+                return None
+            a = np.ascontiguousarray(np.asarray(a, np.int64).reshape(-1).clip(0, abi.MM_BUDGET_UNLIMITED), np.uint32)
+            assert len(a) == n
+            return a
+        q = arr(per_queue, self.cfg.n_modes * self.cfg.n_groups)
+        m = arr(per_mode, self.cfg.n_modes)
+        self._check(self.lib.mm_set_lobby_budget(self.h, _p(q), _p(m)), "mm_set_lobby_budget")
+
+    def lobby_budget_report(self):
+        """-> (candidates u32[n_modes * n_groups], emitted u32[...]) of the last completed tick: the lobbies every queue
+        had, budgets ignored, and the lobbies it emitted (mm_lobby_budget_report)."""
+        cap = self.cfg.n_modes * self.cfg.n_groups
+        cand, emitted = np.zeros(cap, np.uint32), np.zeros(cap, np.uint32)
+        n = C.c_uint32(0)
+        self._check(self.lib.mm_lobby_budget_report(self.h, _p(cand), _p(emitted), cap, C.byref(n)),
+                    "mm_lobby_budget_report")
+        return cand[:n.value], emitted[:n.value]
+
+    def lobby_candidates(self):
+        """-> u32[n_modes * n_groups]: the lobbies a tick without a budget would emit from every queue of the pool as it
+        is now; nothing changes (mm_lobby_candidates)."""
+        cap = self.cfg.n_modes * self.cfg.n_groups
+        cand = np.zeros(cap, np.uint32)
+        n = C.c_uint32(0)
+        self._check(self.lib.mm_lobby_candidates(self.h, _p(cand), cap, C.byref(n)), "mm_lobby_candidates")
+        return cand[:n.value]
+
     def expire(self, now, max_wait, want_seq=True):
         """Search timeout (mm_expire): every queued player whose wait at `now` (as queue_stats counts it) is >=
         max_wait leaves the pool and the active set, like remove(). -> (ids u64, enqueue seq u32 | None), unordered."""

@@ -156,6 +156,12 @@ class SearchPool:
     timeout_ms: optional search time limit (extension): after each tick's lobbies are published, every player still
     queued who has waited at least this long leaves the pool (Engine.expire) and gets the error response of
     game-lobby/worker.ex:63-71 on its "response-queue".  None (the default) never expires anyone.
+    lobby_budget: optional flow control (extension): a callable () -> {mode name: lobbies} asked before every tick —
+    the free game-server slots, what the lobby stage would otherwise find out per lobby (calculate_required_slots,
+    game-lobby/worker.ex:118-141); a mode it does not name is unlimited.  The tick emits at most that many lobbies of
+    the mode (Engine.set_lobby_budget), shared over the rating groups in proportion to what each could emit; the rest
+    stay ordinary queued players (timeout_ms, requeue, move_out, checkpoint treat them as such).  pause() / resume_queues()
+    set single queues to 0 / unlimited.  A checkpoint does not carry budgets or pauses: resume() starts unlimited.
 
     Every ingest batch is stamped with now_ms(), the clock in milliseconds since the pool was created (u32, wraps
     after 49 days), and every tick passes the same clock as its `now`: the engine's per-queue waits
@@ -163,10 +169,12 @@ class SearchPool:
     """
 
     def __init__(self, engine, mode_names, group_names, max_batch=65536, window=None, clock=None, flush_every_s=0.005,
-                 handle_capacity=None, timeout_ms=None, wall_clock=None):
+                 handle_capacity=None, timeout_ms=None, wall_clock=None, lobby_budget=None):
         import time
         self.window = window
         self.timeout_ms = timeout_ms
+        self.lobby_budget = lobby_budget
+        self.paused = set()  # queues (mode * n_groups + group) that emit nothing until resume_queues()
         self.clock = clock or time.monotonic
         self.wall_clock = wall_clock or time.time  # seconds since the epoch: checkpoint() / resume() bridge the downtime
         self._t0 = self.clock()
@@ -332,6 +340,8 @@ class SearchPool:
             oldest = next(iter(self.enqueued_at.values()), None)
             self.last_spread = self.window.spread(self.clock(), oldest)
             self.engine.set_option("max_spread", self.last_spread)
+        if self.lobby_budget is not None:
+            self._set_budget(self.lobby_budget())
         lob, mem, _seq, _st = self.engine.tick(now)
         for h in lob:
             mode_name = self.mode_names[h["mode"]]
@@ -352,6 +362,42 @@ class SearchPool:
         if self.timeout_ms is not None:  # after the lobbies: a player this tick matched is never timed out
             self._expire(now)
         return len(lob)
+
+    # -- lobby budget ------------------------------------------------------------------------
+    def _queues(self, group_names, mode_names):
+        modes = range(len(self.mode_names)) if mode_names is None else [self.mode_names.index(m) for m in mode_names]
+        return {m * len(self.group_names) + self.group_names.index(g) for g in group_names for m in modes}
+
+    def _set_budget(self, per_mode=None):
+        from .abi import MM_BUDGET_UNLIMITED
+        queue = np.full(len(self.mode_names) * len(self.group_names), MM_BUDGET_UNLIMITED, np.uint32)
+        queue[sorted(self.paused)] = 0
+        mode = None
+        if per_mode is not None:
+            mode = np.array([min(max(int(per_mode.get(m, MM_BUDGET_UNLIMITED)), 0), MM_BUDGET_UNLIMITED)
+                             for m in self.mode_names], np.uint32)
+        self.engine.set_lobby_budget(per_queue=queue, per_mode=mode)
+
+    def pause(self, group_names, mode_names=None):
+        """The queues of these groups (all modes, or only `mode_names`) emit no lobby from the next tick on; their
+        players stay queued in order, waits and the search timeout running.  Undone by resume_queues()."""
+        self.paused |= self._queues(group_names, mode_names)
+        if self.lobby_budget is None:  # (with a budget callable the next tick sets both together)
+            self._set_budget()
+
+    def resume_queues(self, group_names, mode_names=None):
+        self.paused -= self._queues(group_names, mode_names)
+        if self.lobby_budget is None:
+            self._set_budget()
+
+    def held_back(self, group_name):
+        """{mode name: lobbies the last tick could have emitted from the group's queue and did not} (candidates minus
+        emitted, Engine.lobby_budget_report); {} for an unknown group."""
+        if group_name not in self.group_names:
+            return {}
+        cand, emitted = self.engine.lobby_budget_report()
+        g, G = self.group_names.index(group_name), len(self.group_names)
+        return {name: int(cand[m * G + g]) - int(emitted[m * G + g]) for m, name in enumerate(self.mode_names)}
 
     def _expire(self, now):
         expired, _seq = self.engine.expire(now, self.timeout_ms, want_seq=False)
@@ -595,6 +641,8 @@ class SearchWorker:
         st["pool"] = self.pool.engine.status() if hasattr(self.pool.engine, "status") else {}
         if hasattr(self.pool.engine, "queue_stats"):  # this worker's own group, per mode (the reference's queue depth)
             st["waiting"] = self.pool.queue_status(self.group_name)
+        if hasattr(self.pool.engine, "lobby_budget_report"):  # lobbies the last tick's budget held back, per mode
+            st["held_back"] = self.pool.held_back(self.group_name)
         return ("ok", st)
 
     def prepare_game_lobby(self, channel_name, exchange_forward, queue_forward, payload):  # worker.ex:250-261

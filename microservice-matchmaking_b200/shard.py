@@ -411,3 +411,68 @@ def move_queues(pkg, cfg, old, new, rank, engine, comm):
                 comm.send(dst, src, (np.array([0 if ok else 1], np.int64),))
         out["moved" if ok else "failed"].append(g)
     return out
+
+
+# ======================================================================================================================
+# One lobby budget per game mode over several engines (mm_set_lobby_budget, include/mm_engine.h).  A mode's budget is
+# apportioned over ALL its rating groups by their candidate lobbies; sharded by group, no engine sees all of them.  Every
+# engine reports its own (Engine.lobby_candidates, a dry run that changes nothing), the counts are gathered, every rank
+# computes the same apportionment and sets the per-queue budgets of its own engine: K engines under one mode budget then
+# emit exactly what a single engine with per_mode would.
+# ======================================================================================================================
+UNLIMITED = 0xFFFFFFFF
+
+
+def apportion(budget, cand):
+    """Largest-remainder apportionment of `budget` lobbies over queues with cand[g] candidate lobbies each, the rule
+    of mm_set_lobby_budget in 64-bit integers: everything if sum(cand) <= budget, else floor(budget * cand[g] / sum)
+    each and one more for the budget - sum(floors) queues with the largest (budget * cand[g]) mod sum, ties to the
+    lower index.  -> int64[len(cand)], never above cand."""
+    c = np.asarray(cand, np.uint64)
+    total, budget = int(c.sum(dtype=np.uint64)), int(budget)
+    if total <= budget:
+        return c.astype(np.int64)
+    prod = c * np.uint64(budget)  # budget < total <= 2^32 and cand < 2^32: the product fits 64 bits
+    a, rem = (prod // np.uint64(total)).astype(np.int64), prod % np.uint64(total)
+    extra = budget - int(a.sum())
+    first = np.lexsort((np.arange(len(c)), np.uint64(total) - rem))  # remainder descending, then index ascending
+    a[first[:extra]] += 1
+    return a
+
+
+def queue_budgets(cfg, per_mode, cand):
+    """Per-queue budgets (u32[n_modes * n_groups], queue_stats() record order) that make engines holding parts of a
+    pool emit what one engine with `per_mode` would: cand = the candidate lobbies of every queue over the whole pool."""
+    cand = np.asarray(cand, np.int64).reshape(cfg.n_modes, cfg.n_groups)
+    out = np.empty((cfg.n_modes, cfg.n_groups), np.int64)
+    for m in range(cfg.n_modes):
+        b = int(per_mode[m])
+        out[m] = cand[m] if b >= UNLIMITED else apportion(b, cand[m])
+    return out.reshape(-1).astype(np.uint32)
+
+
+def set_mode_budget(engines, per_mode, comm=None, rank=0, world=1):
+    """Put the engines of a job under one lobby budget per game mode for the next tick.  engines: all of the job's
+    engines when they share this process, or this rank's engine (with comm, rank, world: every rank calls this with the
+    same per_mode; the counts travel as int64 arrays over comm.send / comm.recv, ranks pairing up in a fixed order so
+    that blocking calls cannot deadlock).  Call it before every tick: the candidates change with the pool.
+    -> the per-queue budgets that were set."""
+    engines = list(engines) if isinstance(engines, (list, tuple)) else [engines]
+    cfg = engines[0].cfg
+    cand = sum(np.asarray(e.lobby_candidates(), np.int64) for e in engines)
+    if comm is not None:
+        mine = cand.copy()
+        for peer in range(world):
+            if peer == rank:
+                continue
+            if rank < peer:
+                comm.send(rank, peer, (mine,))
+                (theirs,) = comm.recv(peer, rank)
+            else:
+                (theirs,) = comm.recv(peer, rank)
+                comm.send(rank, peer, (mine,))
+            cand = cand + np.asarray(theirs).view(np.int64)
+    budgets = queue_budgets(cfg, per_mode, cand)
+    for e in engines:
+        e.set_lobby_budget(per_queue=budgets)
+    return budgets
