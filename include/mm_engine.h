@@ -500,6 +500,42 @@ typedef struct mm_image_header {
 int mm_export(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes);
 int mm_import(mm_engine* e, const void* buf, uint64_t n_bytes);
 
+/* EXTENSION (regroup on import): load an mm_export image written under ANOTHER config into a fresh engine, so that a
+ * new RatingGroups table (config/config.exs:27-36), a new default group, an added or dropped game mode, another
+ * order_mode or MM_F_WIDE_PARTITIONS can be deployed without dropping the queue.  The image's config may differ from
+ * the engine's on n_groups, group_lo / group_hi, default_group, n_modes, modes, order_mode and MM_F_WIDE_PARTITIONS;
+ * it must match on the id width (MM_F_DENSE_IDS) and MM_F_NO_DEDUPE.
+ * Each queued player goes to the layout partition its (rating, mode) maps to under the ENGINE's config, in age order
+ * inside it ((seq - seq_next) mod 2^32 ascending: the order of mm_requeue and mm_pool_read), with its id, rating,
+ * mode, enq_ts and seq; seq_next is kept, and the active section goes into the active set unchanged.  A player whose
+ * rating has no group here (default_group = -1) or whose mode is >= n_modes is REJECTED: not queued, not in the
+ * active set; its image index goes to rejected[] (ascending) and *n_rejected counts them — the caller answers those
+ * players (they left).
+ * Refusals, all decided by one read of the device's counters before the pool is written; after any of them the engine
+ * is empty and still fresh:
+ *   MM_E_STATE the engine is not fresh, or a packed batch is staged;
+ *   MM_E_ARG   a queue image; another id width or MM_F_NO_DEDUPE; an image's config that is not a valid config
+ *              (capacity aside); and everything mm_import refuses in an image on an engine created with the IMAGE's
+ *              config, with mm_import's mm_last_error wording: bad lengths or counts, a mode >= the image's n_modes, a
+ *              rating outside the partition it is filed under, an id out of the engine's id range or repeated
+ *              anywhere in the image, sequence numbers out of order inside an image partition or equal to seq_next.
+ *              Also two players the re-filing puts into one partition with the same seq ("sequence numbers out of
+ *              order");
+ *   MM_E_CAP   more than `cap` players would be rejected (*n_rejected = the count: cap = 0 with rejected = NULL is a
+ *              dry run), or the kept players do not fit under mm_import's capacity rules.
+ * Cost: one pass to classify, a stable counting scatter by new partition, and ceil(log2 k) merge rounds when up to
+ * k image partitions feed one new partition (none when groups only split or their bounds move); then mm_import's load.
+ *
+ * EQUIVALENCE.  Let R be the image re-filed: header config = the engine's config, section 1 = the kept players per
+ * layout partition of the engine, sections 2-6 = the kept players partition by partition in age order inside a
+ * partition, section 7 unchanged, the same seq_next.  After mm_import_regroup(img), every later call sequence gives
+ * the same results as on a fresh engine that called mm_import(R): as if each kept player had been enqueued into this
+ * engine in its original order, with its original stamp and number.  When the configs are equal, R is the image itself.
+ * Not covered: queue images (mm_merge still needs equal configs) and sharded deployments (a re-cut moves players
+ * between ranks).                                                                                                   */
+int mm_import_regroup(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t cap, uint32_t* rejected,
+                      uint32_t* n_rejected);
+
 /* ---- queue move: part of an engine into another running engine ---------------------------
  * The reference's queues live in RabbitMQ and its state in replicated Mnesia tables, so any node's workers can serve
  * any rating group (application.ex:26-40).  Here a queued player lives in one engine: mm_export_queues releases

@@ -274,6 +274,26 @@ static ERL_NIF_TERM nif_merge_image(ErlNifEnv* env, int argc, const ERL_NIF_TERM
   return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &rej));
 }
 
+/* import_regroup(ref, image :: binary) -> {:ok, rejected :: binary(u32[])} | {:error, atom}: loads an image written
+ * under another config (groups, modes, order) into a fresh engine (mm_import_regroup); `rejected` holds the image
+ * indices, ascending, of the players the engine's config has no queue for (not queued: the caller answers them). */
+static ERL_NIF_TERM nif_import_regroup(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary img, rej; uint32_t cap = 0, got = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &img))
+    return enif_make_badarg(env);
+  if (img.size >= sizeof(mm_image_header)) {
+    mm_image_header h;
+    memcpy(&h, img.data, sizeof(h));
+    cap = h.n_players < img.size ? h.n_players : (uint32_t)img.size;  /* a corrupt count must not size the list */
+  }
+  if (!enif_alloc_binary((size_t)cap * 4, &rej)) return err(env, MM_E_CAP);
+  int rc = mm_import_regroup(r->e, img.data, img.size, cap, (uint32_t*)rej.data, &got);
+  if (rc) { enif_release_binary(&rej); return err(env, rc); }
+  enif_realloc_binary(&rej, (size_t)got * 4);
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &rej));
+}
+
 /* seq_next(ref) -> {:ok, seq}: the enqueue sequence number the next offered player will get (mm_seq_next) */
 static ERL_NIF_TERM nif_seq_next(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
   engine_res* r; uint32_t s = 0;
@@ -410,6 +430,7 @@ static ErlNifFunc funcs[] = {
   {"import_image", 2, nif_import_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"export_queues", 2, nif_export_queues, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"merge_image", 2, nif_merge_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"import_regroup", 2, nif_import_regroup, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"seq_next", 1, nif_seq_next, 0},
   {"set_max_spread", 2, nif_set_max_spread, 0},

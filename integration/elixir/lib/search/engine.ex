@@ -77,6 +77,13 @@ defmodule Matchmaking.Search.Engine do
   def export_image(_ref), do: :erlang.nif_error(:nif_not_loaded)
   @doc "Loads an export_image/1 image into a fresh engine of the same config -> :ok | {:error, :badarg | :capacity | :state}"
   def import_image(_ref, _image), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Regroup on import (extension): loads an export_image/1 image written under ANOTHER config (rating groups, default
+  group, modes, order) into this fresh engine (mm_import_regroup); every player keeps its place -> {:ok, rejected ::
+  binary(u32[])}, the image indices (ascending) of the players this config has no queue for, or {:error, :badarg |
+  :capacity | :state}; after a refusal the engine is still fresh.
+  """
+  def import_regroup(_ref, _image), do: :erlang.nif_error(:nif_not_loaded)
 
   @doc """
   Queue move: the selected (mode, group) queues (queues :: binary, one byte per queue in queue_stats/2 record order,

@@ -25,7 +25,9 @@ defmodule Matchmaking.Search.Pool do
                      documents, the pool clock and the wall time.  resume: <checkpoint> as an option of start_link/1
                      starts a pool on a fresh engine from it; the clock goes on from the checkpoint plus the time the
                      pool was down (INTEGRATION.md §3 has the order: stop consuming, checkpoint, start with resume:,
-                     consume again)
+                     consume again).  regroup: true with resume: deploys another config (RatingGroups, modes)
+                     without dropping the queue (Engine.import_regroup): players the new config has no queue for
+                     leave the pool and get the search-timeout error response once a search worker has attached
       move_out/1, move_in/1   queue move between running pools: the queues of some rating groups leave this pool
                      with the players' documents and are merged into another pool (INTEGRATION.md §5)
       attach/1       a search worker hands over its open channel (patched init); the pool ticks only once it has a
@@ -92,8 +94,8 @@ defmodule Matchmaking.Search.Pool do
     st = %{ref: ref, staged: [], n_staged: 0, handle_of: %{}, players: %{}, free: [], next: 0, channel: nil,
            queued: %{}, moved_out: MapSet.new(),
            t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms),
-           lobby_budget: Keyword.get(opts, :lobby_budget), paused: MapSet.new()}
-    case resume(st, Keyword.get(opts, :resume)) do
+           lobby_budget: Keyword.get(opts, :lobby_budget), paused: MapSet.new(), regroup_dropped: []}
+    case resume(st, Keyword.get(opts, :resume), Keyword.get(opts, :regroup, false)) do
       {:ok, st} ->
         Process.send_after(self(), :flush, @flush_ms)
         Process.send_after(self(), :tick, @tick_ms)
@@ -106,17 +108,40 @@ defmodule Matchmaking.Search.Pool do
   # The channel name is not carried: a name from the old process does not say that the new process has that channel
   # open.  Until a search worker attaches its channel (attach/1) or stages a delivery, :tick neither ticks nor
   # expires, so the players of the image are not matched into lobbies that could not be published.
-  defp resume(st, nil), do: {:ok, st}
-  defp resume(st, blob) do
+  # regroup: the engine was created with another config than the checkpoint's (a new RatingGroups table or mode list;
+  # a mode keeps its index).  A checkpoint with queues moved out is refused: those queues live in another pool under
+  # the old groups.  The players the new config has no queue for are dropped here and answered by the first tick.
+  defp resume(st, nil, _regroup), do: {:ok, st}
+  defp resume(st, blob, regroup) do
     ck = :erlang.binary_to_term(blob, [:safe])
-    case Engine.import_image(st.ref, ck.image) do
-      :ok ->
+    loaded = cond do
+      not regroup -> with :ok <- Engine.import_image(st.ref, ck.image), do: {:ok, <<>>}
+      MapSet.size(Map.get(ck, :moved_out, MapSet.new())) > 0 -> {:error, :moved_out}
+      true -> Engine.import_regroup(st.ref, ck.image)
+    end
+    case loaded do
+      {:ok, rejected} ->
         down = max(0, System.os_time(:millisecond) - ck.wall_ms)
         # now_ms/1 goes on from the checkpoint's value plus the downtime: the engine's enqueue stamps stay valid
-        {:ok, %{st | handle_of: ck.handle_of, players: ck.players, free: ck.free, next: ck.next,
-                     queued: Map.get(ck, :queued, %{}), moved_out: Map.get(ck, :moved_out, MapSet.new()),
-                     t0: System.monotonic_time(:millisecond) - ck.now_ms - down}}
+        st = %{st | handle_of: ck.handle_of, players: ck.players, free: ck.free, next: ck.next,
+                    queued: Map.get(ck, :queued, %{}), moved_out: Map.get(ck, :moved_out, MapSet.new()),
+                    t0: System.monotonic_time(:millisecond) - ck.now_ms - down}
+        {:ok, drop_rejected(st, ck.image, rejected)}
       {:error, _} = e -> e
+    end
+  end
+
+  # the image's handle (section 2: u32, after the header and the partition counts) of each rejected index
+  defp drop_rejected(st, _image, <<>>), do: st
+  defp drop_rejected(st, image, rejected) do
+    <<_::binary-size(24), n_parts::little-32, _::binary>> = image
+    ids_at = div(624 + 4 * n_parts + 7, 8) * 8
+    for <<i::little-32 <- rejected>>, reduce: st do
+      acc ->
+        <<_::binary-size(ids_at + 4 * i), h::little-32, _::binary>> = image
+        {player, players} = Map.pop(acc.players, h)
+        %{acc | players: players, handle_of: Map.delete(acc.handle_of, player["id"]), free: [h | acc.free],
+                queued: Map.delete(acc.queued, h), regroup_dropped: [player | acc.regroup_dropped]}
     end
   end
 
@@ -326,7 +351,8 @@ defmodule Matchmaking.Search.Pool do
 
   def handle_info(:tick, st) do
     Process.send_after(self(), :tick, @tick_ms)
-    st = flush(st)
+    for player <- st.regroup_dropped, do: send_timeout(st.channel, player)   # resume with regroup: true
+    st = flush(%{st | regroup_dropped: []})
     now = now_ms(st)
     if st.lobby_budget, do: set_budget(st, st.lobby_budget.())
     case Engine.tick_packed(st.ref, now) do

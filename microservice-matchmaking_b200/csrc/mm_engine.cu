@@ -23,6 +23,7 @@
 #include "mm_expire.cuh"
 #include "mm_image.cuh"
 #include "mm_kernels.cuh"
+#include "mm_regroup.cuh"
 #include "mm_requeue.cuh"
 #include "mm_stats.cuh"
 
@@ -90,6 +91,8 @@ struct Counters {
   uint32_t expired, erased;               // k_expire: players expired or released; active-set entries erased
   uint32_t img_players, img_active;       // export: live players; active ids outside the pool
   uint32_t img_err, mrg_dups;             // mm_import / mm_merge: kImg* error bits; batch entries that will not queue
+                                          // (mm_import_regroup: repeated ids)
+  uint32_t rg_kmax;                       // mm_import_regroup: most image partitions feeding one new partition
 };
 
 }  // namespace
@@ -251,6 +254,10 @@ struct mm_engine {
   DevArray<uint32_t> d_rq_u;     // grouped entries: age (seq - seq_next)
   DevArray<uint32_t> d_rq_hist;  // [n_segs][blocks] code-1 entries -> the block's first grouped index
   DevArray<uint32_t> d_rq_seg;   // rq_off[n_segs + 1] | m_off[n_segs + 1] | slot_base[n_segs]
+
+  // mm_import_regroup (mm_regroup.cuh): the image's layout tables and the re-filing scratch, carved from one
+  // allocation that every call frees
+  DevArray<uint8_t> d_rg;
 
   // mm_band_candidates / mm_band_match (mm_band.cuh): sized by the band keys and the candidates, grown on demand
   struct Band {
@@ -422,22 +429,32 @@ int upload_table(mm_engine* e, DevArray<T>& d, const std::vector<T>& h) {
   return MM_OK;
 }
 
-// Build the key -> bin LUT and the (mode, group) segment table (see mm_kernels.cuh).
-int build_tables(mm_engine* e) {
-  const mm_config& c = e->cfg;
+// The layout of a config (see mm_kernels.cuh): the key -> bin LUT, the rating -> group table and the (mode, group)
+// cut segments with their layout partitions.  A pure host function: mm_create uploads its tables (build_tables), and
+// mm_import_regroup builds the layout of an image's config as well, to check the image against it.
+struct Layout {
+  int32_t key_lo = 0;
+  uint32_t KR = 0, stride = 0, K = 0, Kp = 0;
+  uint32_t n_segs = 0, n_cut = 0, min_L = 0xFFFFFFFFu, max_nb = 1;
+  std::vector<uint8_t> grp, tsz;                        // [KR] clamp key -> group (0xFF: none); [MM_MAX_MODES]
+  std::vector<uint16_t> lut, bin_seg, bin_key, part_cut;  // [KR], [Kp], [Kp], [n_segs]
+  std::vector<uint32_t> seg_lo, seg_L, cut_lp_lo;       // [n_segs + 1], [n_segs], [n_cut + 1]
+};
+
+int build_layout(const mm_config& c, Layout& y) {
   int32_t rmin = c.group_lo[0], rmax = c.group_hi[0];
   for (uint32_t g = 1; g < c.n_groups; ++g) { rmin = std::min(rmin, c.group_lo[g]); rmax = std::max(rmax, c.group_hi[g]); }
-  e->key_lo = rmin - 1;
+  y.key_lo = rmin - 1;
   const uint64_t KR64 = (uint64_t)((int64_t)rmax - rmin + 3);
   if (KR64 > 65535u) return MM_E_ARG;  // rating span must fit the 16-bit LUT
-  e->KR = (uint32_t)KR64;
+  y.KR = (uint32_t)KR64;
   const uint32_t G = c.n_groups;
-  std::vector<uint8_t> grp(e->KR);
-  for (uint32_t k = 0; k < e->KR; ++k) {
-    const int g = group_of(&c, (int64_t)e->key_lo + k);
-    grp[k] = g < 0 ? 0xFF : (uint8_t)g;
+  y.grp.assign(y.KR, 0);
+  for (uint32_t k = 0; k < y.KR; ++k) {
+    const int g = group_of(&c, (int64_t)y.key_lo + k);
+    y.grp[k] = g < 0 ? 0xFF : (uint8_t)g;
   }
-  std::vector<uint16_t> lut(e->KR, 0);
+  y.lut.assign(y.KR, 0);
   std::vector<uint32_t> first(G + 1, 0);
   std::vector<uint16_t> key_of;  // rating order: bin (inside a mode) -> clamp key
   if (c.order_mode == MM_ORDER_RATING) {
@@ -445,68 +462,76 @@ int build_tables(mm_engine* e) {
     uint32_t next = 0;
     for (uint32_t g = 0; g < G; ++g) {
       first[g] = next;
-      for (uint32_t k = 0; k < e->KR; ++k)
-        if (grp[k] == g) { lut[k] = (uint16_t)next++; key_of.push_back((uint16_t)k); }
+      for (uint32_t k = 0; k < y.KR; ++k)
+        if (y.grp[k] == g) { y.lut[k] = (uint16_t)next++; key_of.push_back((uint16_t)k); }
     }
     first[G] = next;
-    e->stride = std::max(next, 1u);
+    y.stride = std::max(next, 1u);
   } else {
-    for (uint32_t k = 0; k < e->KR; ++k) lut[k] = grp[k] == 0xFF ? 0 : grp[k];
+    for (uint32_t k = 0; k < y.KR; ++k) y.lut[k] = y.grp[k] == 0xFF ? 0 : y.grp[k];
     for (uint32_t g = 0; g <= G; ++g) first[g] = g;
-    e->stride = G;
+    y.stride = G;
   }
-  e->K = c.n_modes * e->stride;
-  e->Kp = e->K + 1;
-  if (e->Kp > 65535u) return MM_E_ARG;  // the resident sort key is 16 bits
+  y.K = c.n_modes * y.stride;
+  y.Kp = y.K + 1;
+  if (y.Kp > 65535u) return MM_E_ARG;  // the resident sort key is 16 bits
   // Layout partitions: a (mode, group) CUT SEGMENT — the unit of the lobby cut — is stored as one or more PARTITIONS
   // of at most kFastBins consecutive sort keys each, so that every tile ranks on the 8-bit path and carries a chunk
   // histogram whatever the width of the rating group (the reference's default groups span 500 - 1 500 ratings,
   // config/config.exs:27-36).  Narrow groups: one partition per segment.
-  e->n_cut = c.n_modes * G;
-  std::vector<uint32_t> seg_lo, seg_L, cut_lp_lo(e->n_cut + 1);
-  std::vector<uint16_t> part_cut;
-  e->min_L = 0xFFFFFFFFu;
-  std::vector<uint8_t> tsz(MM_MAX_MODES, 0);
+  y.n_cut = c.n_modes * G;
+  y.cut_lp_lo.assign(y.n_cut + 1, 0);
+  y.min_L = 0xFFFFFFFFu;
+  y.tsz.assign(MM_MAX_MODES, 0);
   bool split = !(c.flags & MM_F_WIDE_PARTITIONS);
   for (int attempt = 0; attempt < 2; ++attempt) {
-    seg_lo.clear(); seg_L.clear(); part_cut.clear();
+    y.seg_lo.clear(); y.seg_L.clear(); y.part_cut.clear();
     for (uint32_t m = 0; m < c.n_modes; ++m) {
       const uint32_t L = (uint32_t)c.modes[m].teams * c.modes[m].team_size;
-      e->min_L = std::min(e->min_L, L);
-      tsz[m] = (uint8_t)c.modes[m].team_size;
+      y.min_L = std::min(y.min_L, L);
+      y.tsz[m] = (uint8_t)c.modes[m].team_size;
       for (uint32_t g = 0; g < G; ++g) {
-        const uint32_t lo = m * e->stride + first[g], nk = first[g + 1] - first[g];
+        const uint32_t lo = m * y.stride + first[g], nk = first[g + 1] - first[g];
         const uint32_t nsub = split ? std::max(1u, (nk + kFastBins - 1) / kFastBins) : 1u;
         const uint32_t per = (nk + nsub - 1) / nsub;
-        cut_lp_lo[m * G + g] = (uint32_t)seg_lo.size();
+        y.cut_lp_lo[m * G + g] = (uint32_t)y.seg_lo.size();
         for (uint32_t j = 0; j < nsub; ++j) {
-          seg_lo.push_back(lo + std::min(nk, j * per)); seg_L.push_back(L); part_cut.push_back((uint16_t)(m * G + g));
+          y.seg_lo.push_back(lo + std::min(nk, j * per)); y.seg_L.push_back(L); y.part_cut.push_back((uint16_t)(m * G + g));
         }
       }
     }
-    if (seg_lo.size() <= kMaxSegs) break;
+    if (y.seg_lo.size() <= kMaxSegs) break;
     split = false;  // too many partitions for the on-chip tables: whole segments, list ranking for the wide ones
   }
-  e->n_segs = (uint32_t)seg_lo.size();
-  if (e->n_segs > kMaxSegs) return MM_E_ARG;
-  cut_lp_lo[e->n_cut] = e->n_segs;
-  e->h_part_cut = part_cut;
-  e->h_cut_lp_lo = cut_lp_lo;
-  seg_lo.push_back(e->K);
-  e->max_nb = 1;
-  for (uint32_t sgi = 0; sgi < e->n_segs; ++sgi) e->max_nb = std::max(e->max_nb, seg_lo[sgi + 1] - seg_lo[sgi]);
-  std::vector<uint16_t> bin_seg(e->Kp, 0);
-  for (uint32_t sgi = 0; sgi < e->n_segs; ++sgi)
-    for (uint32_t b = seg_lo[sgi]; b < seg_lo[sgi + 1]; ++b) bin_seg[b] = (uint16_t)sgi;
-  std::vector<uint16_t> bin_key(e->Kp, 0);
+  y.n_segs = (uint32_t)y.seg_lo.size();
+  if (y.n_segs > kMaxSegs) return MM_E_ARG;
+  y.cut_lp_lo[y.n_cut] = y.n_segs;
+  y.seg_lo.push_back(y.K);
+  y.max_nb = 1;
+  for (uint32_t sgi = 0; sgi < y.n_segs; ++sgi) y.max_nb = std::max(y.max_nb, y.seg_lo[sgi + 1] - y.seg_lo[sgi]);
+  y.bin_seg.assign(y.Kp, 0);
+  for (uint32_t sgi = 0; sgi < y.n_segs; ++sgi)
+    for (uint32_t b = y.seg_lo[sgi]; b < y.seg_lo[sgi + 1]; ++b) y.bin_seg[b] = (uint16_t)sgi;
+  y.bin_key.assign(y.Kp, 0);
   if (!key_of.empty())
-    for (uint32_t b = 0; b < e->K; ++b) bin_key[b] = key_of[b % e->stride];
-  int rc;
-  if ((rc = upload_table(e, e->d_part_cut, part_cut)) || (rc = upload_table(e, e->d_cut_lp_lo, cut_lp_lo)) ||
-      (rc = upload_table(e, e->d_bin_seg, bin_seg)) || (rc = upload_table(e, e->d_bin_key, bin_key)) ||
-      (rc = upload_table(e, e->d_lut, lut)) || (rc = upload_table(e, e->d_grp_lut, grp)) ||
-      (rc = upload_table(e, e->d_mode_tsize, tsz)) || (rc = upload_table(e, e->d_seg_bin_lo, seg_lo)) ||
-      (rc = upload_table(e, e->d_seg_L, seg_L)))
+    for (uint32_t b = 0; b < y.K; ++b) y.bin_key[b] = key_of[b % y.stride];
+  return MM_OK;
+}
+
+// The engine's layout (build_layout of its config) into its fields and device tables.
+int build_tables(mm_engine* e) {
+  Layout y;
+  int rc = build_layout(e->cfg, y);
+  if (rc) return rc;
+  e->key_lo = y.key_lo; e->KR = y.KR; e->stride = y.stride; e->K = y.K; e->Kp = y.Kp;
+  e->n_segs = y.n_segs; e->n_cut = y.n_cut; e->min_L = y.min_L; e->max_nb = y.max_nb;
+  e->h_part_cut = y.part_cut;
+  e->h_cut_lp_lo = y.cut_lp_lo;
+  if ((rc = upload_table(e, e->d_part_cut, y.part_cut)) || (rc = upload_table(e, e->d_cut_lp_lo, y.cut_lp_lo)) ||
+      (rc = upload_table(e, e->d_bin_seg, y.bin_seg)) || (rc = upload_table(e, e->d_bin_key, y.bin_key)) ||
+      (rc = upload_table(e, e->d_lut, y.lut)) || (rc = upload_table(e, e->d_grp_lut, y.grp)) ||
+      (rc = upload_table(e, e->d_mode_tsize, y.tsz)) || (rc = upload_table(e, e->d_seg_bin_lo, y.seg_lo)) ||
+      (rc = upload_table(e, e->d_seg_L, y.seg_L)))
     return rc;
   return MM_OK;
 }
@@ -1123,7 +1148,7 @@ int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes, const
 // the image-sized scratch of mm_export / mm_import / mm_merge (cudaFree waits for the work that uses it)
 void free_img_scratch(mm_engine* e) {
   e->d_img.reset(); e->d_img_act.reset(); e->d_mrg_src.reset(); e->d_mrg_code.reset(); e->d_mrg_seen.reset();
-  e->d_rq_u.reset();
+  e->d_rq_u.reset(); e->d_rg.reset();
 }
 
 // The current pool buffer and the active set back to an empty engine's state.
@@ -1155,25 +1180,39 @@ bool same_layout(const mm_config& a, const mm_config& c) {
   return same;
 }
 
-// The header checks of mm_import and mm_merge.  `magic` is the image kind's, `prefix` starts every message, and
-// `no_active` refuses an active section (null: one is allowed).  -> the header, its layout and the partition counts
+// The header checks of mm_import, mm_merge and mm_import_regroup.  `magic` is the image kind's, `prefix` starts every
+// message, and `no_active` refuses an active section (null: one is allowed).  regroup = null: the image's config must
+// be the engine's (same_layout); otherwise it may differ except on the id width and MM_F_NO_DEDUPE, must be a valid
+// config (capacity aside), and *regroup receives its layout, whose partition count the image must have.
+// -> the header, its layout and the partition counts
 int check_header(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t magic, const char* prefix,
                  const char* bad_magic, const char* no_active, mm_image_header& h, ImgLayout& l,
-                 std::vector<uint32_t>& cnt) {
+                 std::vector<uint32_t>& cnt, Layout* regroup = nullptr) {
   auto bad = [&](const char* what) { return set_err(e, MM_E_ARG, "%s: %s", prefix, what); };
   if (nb < sizeof(h)) return bad("shorter than its header");
   std::memcpy(&h, buf, sizeof(h));
   if (h.magic != magic) return bad(bad_magic);
   if (h.version != MM_IMAGE_VERSION || h.abi_version != MM_ABI_VERSION) return bad("unknown version");
   if (h.id_bytes != id_bytes(e)) return bad("id width differs from the engine's");
-  if (h.n_parts != e->n_segs) return bad("partition count differs from the engine's layout");
+  uint32_t n_parts = e->n_segs;
+  if (regroup) {
+    if ((h.config.flags ^ e->cfg.flags) & (MM_F_NO_DEDUPE | MM_F_DENSE_IDS))
+      return bad("MM_F_NO_DEDUPE or MM_F_DENSE_IDS differs from the engine's");
+    mm_config c = h.config;
+    c.capacity = 1;  // the writer's capacity does not matter here
+    if (check_config(&c) || build_layout(c, *regroup)) return bad("the image's config is not a valid config");
+    n_parts = regroup->n_segs;
+  }
+  if (h.n_parts != n_parts)
+    return bad(regroup ? "partition count differs from the image config's layout"
+                       : "partition count differs from the engine's layout");
   l = img_layout(h.n_parts, h.n_players, h.n_active, h.id_bytes);
   if (h.total_bytes != l.off[7] || nb != l.off[7]) return bad("length does not match the header's section counts");
-  if (!same_layout(h.config, e->cfg))
+  if (!regroup && !same_layout(h.config, e->cfg))
     return bad("config differs from the engine's (groups, default_group, modes, order_mode or flags)");
   if (no_active && h.n_active) return bad(no_active);
-  cnt.resize(e->n_segs);
-  std::memcpy(cnt.data(), buf + l.off[0], (size_t)e->n_segs * 4);
+  cnt.resize(n_parts);
+  std::memcpy(cnt.data(), buf + l.off[0], (size_t)n_parts * 4);
   uint64_t sum = 0;
   for (uint32_t q : cnt) sum += q;
   if (sum != h.n_players) return bad("partition counts do not add up to the player count");
@@ -1188,22 +1227,22 @@ int img_err(mm_engine* e, const char* prefix, uint32_t err) {
                  err & kImgFull ? " active set full" : "");
 }
 
-int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
-  if (!e->fresh || e->stage_count)
-    return set_err(e, MM_E_STATE, "mm_import needs a fresh engine (nothing enqueued, imported or restored)");
-  mm_image_header h;
-  ImgLayout l;
-  std::vector<uint32_t> cnt;
-  int rc = check_header(e, buf, nb, MM_IMAGE_MAGIC, "image rejected", "bad magic",
-                        e->use_active ? nullptr : "active section in an image of an engine without an active set", h, l,
-                        cnt);
-  if (rc) return rc;
-  const uint32_t n = h.n_players, m = h.n_active;
-  if (n > e->capacity) return set_err(e, MM_E_CAP, "%u players, capacity %u", n, e->capacity);
-  if (e->use_active && !e->dense_ids && ((uint64_t)n + m) * 4 > e->hcap * 3)
-    return set_err(e, MM_E_CAP, "%llu active ids, active set holds %llu", (unsigned long long)n + m,
+// The capacity refusals of a load: n queued players and m active ids outside the pool.
+int load_fits(mm_engine* e, uint64_t n, uint64_t m) {
+  if (n > e->capacity) return set_err(e, MM_E_CAP, "%llu players, capacity %u", (unsigned long long)n, e->capacity);
+  if (e->use_active && !e->dense_ids && (n + m) * 4 > e->hcap * 3)
+    return set_err(e, MM_E_CAP, "%llu active ids, active set holds %llu", (unsigned long long)(n + m),
                    (unsigned long long)(e->hcap * 3 / 4));
-  // every partition on consecutive chunks, in partition order
+  return MM_OK;
+}
+
+// The load tail of mm_import and mm_import_regroup: a fresh engine's pool and active set from image columns already in
+// device memory — cnt[s] players of layout partition s, in `cols` partition by partition in enqueue order, and the m
+// ids of the active section at `act`.  Every partition goes on consecutive chunks, in partition order; k_img_load
+// checks every player under the engine's layout while it writes it, k_img_insert refuses a repeated id, and a failed
+// check leaves the engine empty and fresh.
+int load_columns(mm_engine* e, const std::vector<uint32_t>& cnt, const ImgCols& cols, uint32_t n, const void* act,
+                 uint32_t m, uint32_t seq_next, const char* prefix) {
   std::vector<uint32_t> tab((size_t)e->n_segs * e->n_chunks, 0), off_base(2 * (size_t)e->n_segs + 1);
   uint32_t chunk = 0, idx = 0;
   for (uint32_t s = 0; s < e->n_segs; ++s) {
@@ -1215,45 +1254,41 @@ int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
     chunk += nch;
   }
   off_base[e->n_segs] = idx;
+  int rc;
   if ((rc = clear_engine(e))) return rc;
   Pool& p = e->pool[e->cur];
-  const uint64_t body = nb - l.off[1];  // columns and active section
   CK(e->d_img_part.reserve((size_t)3 * e->n_segs + 2));
-  CK(e->d_img.reserve(std::max<uint64_t>(body, 8)));
   CK(cudaMemcpyAsync(p.m.fill, cnt.data(), (size_t)e->n_segs * 4, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(p.m.chunk_tab, tab.data(), tab.size() * 4, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(p.m.bump, &chunk, 4, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(e->d_img_part, off_base.data(), off_base.size() * 4, cudaMemcpyHostToDevice, e->stream));
-  if (body) CK(cudaMemcpyAsync(e->d_img, buf + l.off[1], body, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemsetAsync(&e->d_cnt->img_err, 0, 4, e->stream));
-  const ImgCols cols = img_cols(e->d_img, l, h.id_bytes);
   const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((n + 255) / 256, 32u * (uint32_t)e->n_sms));
   if (n) {
     ImgLoadArgs la{};
     la.pool = p.v; la.meta = p.m; la.in = cols; la.n = n; la.n_segs = e->n_segs;
     la.part_off = e->d_img_part; la.slot_base = e->d_img_part + e->n_segs + 1;
     la.bm = bin_map(e); la.grp_lut = e->d_grp_lut; la.bin_seg = e->d_bin_seg; la.seg_bin_lo = e->d_seg_bin_lo;
-    la.mode_tsize = e->d_mode_tsize; la.n_modes = e->cfg.n_modes; la.seq_next = h.seq_next; la.id_limit = id_limit(e);
+    la.mode_tsize = e->d_mode_tsize; la.n_modes = e->cfg.n_modes; la.seq_next = seq_next; la.id_limit = id_limit(e);
     la.err = &e->d_cnt->img_err;
     k_img_load<<<grid, 256, 0, e->stream>>>(la);
   }
   if (e->use_active) {
     const ActiveView av = act_view(e);
-    if (n) k_img_insert<<<grid, 256, 0, e->stream>>>(cols.id, h.id_bytes, n, id_limit(e), av, &e->d_cnt->img_err);
+    if (n) k_img_insert<<<grid, 256, 0, e->stream>>>(cols.id, cols.id_bytes, n, id_limit(e), av, &e->d_cnt->img_err);
     if (m) {
       const uint32_t g2 = std::max<uint32_t>(1, std::min<uint32_t>((m + 255) / 256, 32u * (uint32_t)e->n_sms));
-      k_img_insert<<<g2, 256, 0, e->stream>>>(e->d_img + (l.off[6] - l.off[1]), h.id_bytes, m, id_limit(e), av,
-                                              &e->d_cnt->img_err);
+      k_img_insert<<<g2, 256, 0, e->stream>>>(act, cols.id_bytes, m, id_limit(e), av, &e->d_cnt->img_err);
     }
   }
   CK(cudaGetLastError());
   if ((rc = read_counters(e))) return rc;
   if (const uint32_t err = e->h_cnt->img_err) {
     if ((rc = clear_engine(e))) return rc;
-    return img_err(e, "image rejected", err);
+    return img_err(e, prefix, err);
   }
   p.n = n;
-  e->seq_next = h.seq_next;
+  e->seq_next = seq_next;
   if (e->use_active) e->n_active = (uint64_t)n + m;
   e->fresh = false;
   e->match_valid = false;
@@ -1264,6 +1299,23 @@ int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
   }
   CK(cudaStreamSynchronize(e->stream));
   return MM_OK;
+}
+
+int import_image(mm_engine* e, const uint8_t* buf, uint64_t nb) {
+  if (!e->fresh || e->stage_count)
+    return set_err(e, MM_E_STATE, "mm_import needs a fresh engine (nothing enqueued, imported or restored)");
+  mm_image_header h;
+  ImgLayout l;
+  std::vector<uint32_t> cnt;
+  int rc = check_header(e, buf, nb, MM_IMAGE_MAGIC, "image rejected", "bad magic",
+                        e->use_active ? nullptr : "active section in an image of an engine without an active set", h, l,
+                        cnt);
+  if (rc || (rc = load_fits(e, h.n_players, h.n_active))) return rc;
+  const uint64_t body = nb - l.off[1];  // columns and active section
+  CK(e->d_img.reserve(std::max<uint64_t>(body, 8)));
+  if (body) CK(cudaMemcpyAsync(e->d_img, buf + l.off[1], body, cudaMemcpyHostToDevice, e->stream));
+  return load_columns(e, cnt, img_cols(e->d_img, l, h.id_bytes), h.n_players, e->d_img + (l.off[6] - l.off[1]),
+                      h.n_active, h.seq_next, "image rejected");
 }
 
 // live players per partition of the current pool, restricted to the partitions in d_sel (the export count pass)
@@ -1548,6 +1600,133 @@ int requeue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating,
   if (n_requeued) *n_requeued = n_rq;
   if (e->h_cnt->img_err)  // the merged list failed the load's own checks: nothing above lets that happen
     return set_err(e, MM_E_STATE, "requeue: the merged players failed the load checks (0x%x)", e->h_cnt->img_err);
+  return MM_OK;
+}
+
+// ---- mm_import_regroup (mm_regroup.cuh) -------------------------------------------------------------------------
+// Every refusal is decided by one read of the counters, before the load tail
+// writes the pool.
+int regroup_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uint32_t* rejected,
+                  uint32_t* n_rejected) {
+  if (!e->fresh || e->stage_count)
+    return set_err(e, MM_E_STATE, "mm_import_regroup needs a fresh engine (nothing enqueued, imported or restored)");
+  mm_image_header h;
+  ImgLayout l;
+  std::vector<uint32_t> cnt;
+  Layout y;  // the image's layout
+  int rc = check_header(e, buf, nb, MM_IMAGE_MAGIC, "image rejected", "bad magic",
+                        e->use_active ? nullptr : "active section in an image of an engine without an active set", h, l,
+                        cnt, &y);
+  if (rc) return rc;
+  const uint32_t n = h.n_players, m = h.n_active, S = e->n_segs, SI = y.n_segs, idb = h.id_bytes;
+  const uint64_t body = nb - l.off[1];
+  CK(e->d_img.reserve(std::max<uint64_t>(body, 8)));
+  if (body) CK(cudaMemcpyAsync(e->d_img, buf + l.off[1], body, cudaMemcpyHostToDevice, e->stream));
+  const ImgCols in = img_cols(e->d_img, l, idb);
+  const void* act = e->d_img + (l.off[6] - l.off[1]);
+  if (n == 0) return load_columns(e, std::vector<uint32_t>(S, 0), in, 0, act, m, h.seq_next, "image rejected");
+  // scratch: the image's tables, the classification, the scatter and merge buffers, the gathered columns
+  const uint32_t nblk = (n + kRqItems - 1) / kRqItems;
+  uint64_t sc = 0;  // the repeated-id set: at most half full
+  if (e->use_active) for (sc = 1024; sc < 2ull * ((uint64_t)n + m); sc <<= 1) {}
+  std::vector<uint32_t> off(SI + 1, 0);
+  for (uint32_t s = 0; s < SI; ++s) off[s + 1] = off[s] + cnt[s];
+  const size_t pair_n = (size_t)SI * S;
+  size_t o = 0;  // the scratch arrays' offsets in d_rg, 8-byte aligned
+  auto take = [&o](size_t bytes) { const size_t x = o; o += (bytes + 7) & ~(size_t)7; return x; };
+  const size_t o_seen = take(8 * sc), o_lut = take(2 * (size_t)y.KR), o_grp = take(y.KR), o_bseg = take(2 * (size_t)y.Kp),
+               o_off = take(4 * ((size_t)SI + 1)), o_rq = take(4 * ((size_t)S + 2)), o_sel = take((size_t)S + 1),
+               o_hist = take(4 * ((size_t)S + 1) * nblk), o_pair = take(4 * pair_n), o_ord = take(2 * pair_n),
+               o_run = take(4 * (size_t)S * (SI + 1)), o_kq = take(4 * (size_t)S), o_part = take(2 * (size_t)n),
+               o_pimg = take(2 * (size_t)n), o_src0 = take(4 * (size_t)n), o_src1 = take(4 * (size_t)n),
+               o_age0 = take(4 * (size_t)n), o_age1 = take(4 * (size_t)n), o_rej = take(4 * (size_t)n),
+               o_out = take(cols_bytes(n));
+  CK(e->d_rg.reserve(o));
+  uint8_t* const base = e->d_rg;
+  auto* seen = reinterpret_cast<unsigned long long*>(base + o_seen);
+  auto* lut_i = reinterpret_cast<uint16_t*>(base + o_lut);
+  uint8_t* grp_i = base + o_grp;
+  auto* bseg_i = reinterpret_cast<uint16_t*>(base + o_bseg);
+  auto* off_i = reinterpret_cast<uint32_t*>(base + o_off);
+  auto* rq_off = reinterpret_cast<uint32_t*>(base + o_rq);
+  uint8_t* sel = base + o_sel;
+  auto* bhist = reinterpret_cast<uint32_t*>(base + o_hist);
+  auto* pair = reinterpret_cast<uint32_t*>(base + o_pair);
+  auto* ord = reinterpret_cast<uint16_t*>(base + o_ord);
+  auto* run_start = reinterpret_cast<uint32_t*>(base + o_run);
+  auto* kq = reinterpret_cast<uint32_t*>(base + o_kq);
+  auto* part = reinterpret_cast<uint16_t*>(base + o_part);
+  auto* pimg = reinterpret_cast<uint16_t*>(base + o_pimg);
+  uint32_t* src[2] = {reinterpret_cast<uint32_t*>(base + o_src0), reinterpret_cast<uint32_t*>(base + o_src1)};
+  uint32_t* age[2] = {reinterpret_cast<uint32_t*>(base + o_age0), reinterpret_cast<uint32_t*>(base + o_age1)};
+  auto* rej = reinterpret_cast<uint32_t*>(base + o_rej);
+  uint8_t* at = base + o_out;
+  ImgCols out = carve_cols(at, n);
+  out.id_bytes = idb;
+  CK(cudaMemcpyAsync(lut_i, y.lut.data(), (size_t)y.KR * 2, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(grp_i, y.grp.data(), y.KR, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(bseg_i, y.bin_seg.data(), (size_t)y.Kp * 2, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(off_i, off.data(), off.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemsetAsync(pair, 0, pair_n * 4, e->stream));
+  CK(cudaMemsetAsync(ord, 0, pair_n * 2, e->stream));
+  CK(cudaMemsetAsync(src[1], 0, (size_t)n * 4, e->stream));  // a merge that writes holes (a refused image) stays in range
+  CK(cudaMemsetAsync(&e->d_cnt->img_err, 0, 3 * 4, e->stream));  // img_err, mrg_dups, rg_kmax
+  // 1. classify
+  RgClassifyArgs ca{};
+  ca.in = in; ca.n = n; ca.nblk = nblk; ca.part_off = off_i; ca.n_img_segs = SI;
+  ca.bm_img = BinMap{lut_i, y.key_lo, y.KR, y.stride, y.K};
+  ca.grp_img = grp_i; ca.bin_seg_img = bseg_i; ca.n_modes_img = h.config.n_modes; ca.seq_next = h.seq_next;
+  ca.id_limit = id_limit(e);
+  ca.bm = bin_map(e); ca.grp_lut = e->d_grp_lut; ca.bin_seg = e->d_bin_seg; ca.n_modes = e->cfg.n_modes; ca.n_segs = S;
+  ca.part = part; ca.pimg = pimg; ca.blockhist = bhist; ca.pair = pair; ca.err = &e->d_cnt->img_err;
+  k_rg_classify<<<nblk, 256, 0, e->stream>>>(ca);
+  const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((n + 255) / 256, 32u * (uint32_t)e->n_sms));
+  if (e->use_active) {
+    CK(cudaMemsetAsync(seen, 0xFF, sc * 8, e->stream));
+    k_rg_dups<<<grid, 256, 0, e->stream>>>(in.id, act, idb, n, m, seen, sc - 1, &e->d_cnt->mrg_dups);
+  }
+  // 2. order: the stable scatter by new partition (reject bucket S last), the plan of the runs, the merge rounds
+  k_rq_scan<<<1, 512, 0, e->stream>>>(S + 1, nblk, bhist, rq_off, sel);
+  k_rq_group<<<nblk, 256, 0, e->stream>>>(n, S + 1, nblk, part, in.seq, h.seq_next, bhist, src[0], age[0]);
+  k_rg_plan<<<1, 1024, 0, e->stream>>>(SI, S, pair, rq_off, ord, run_start, kq, &e->d_cnt->rg_kmax);
+  uint32_t rounds = 0;  // enough for any k_max <= SI; the rounds past the need return at once
+  while ((1u << rounds) < SI) ++rounds;
+  for (uint32_t t = 0; t < rounds; ++t) {
+    RgMergeArgs ma{};
+    ma.rq_off = rq_off; ma.n_segs = S; ma.n_img_segs = SI; ma.round = t; ma.pimg = pimg; ma.ord = ord;
+    ma.run_start = run_start; ma.kq = kq; ma.kmax = &e->d_cnt->rg_kmax;
+    ma.src_in = src[t & 1]; ma.u_in = age[t & 1]; ma.src_out = src[(t + 1) & 1]; ma.u_out = age[(t + 1) & 1];
+    k_rg_merge<<<grid, 256, 0, e->stream>>>(ma);
+  }
+  // 3. duplicate ages, the gathered columns, the reject list
+  RgFinishArgs fa{};
+  fa.rq_off = rq_off; fa.n_segs = S; fa.n = n; fa.kmax = &e->d_cnt->rg_kmax;
+  fa.src[0] = src[0]; fa.src[1] = src[1]; fa.u[0] = age[0]; fa.u[1] = age[1];
+  fa.in = in; fa.out = out; fa.rejected = rej; fa.err = &e->d_cnt->img_err;
+  k_rg_finish<<<grid, 256, 0, e->stream>>>(fa);
+  CK(cudaGetLastError());
+  // 4. one read decides every refusal
+  std::vector<uint32_t> h_off(S + 2);
+  CK(cudaMemcpyAsync(h_off.data(), rq_off, h_off.size() * 4, cudaMemcpyDeviceToHost, e->stream));
+  if ((rc = read_counters(e))) return rc;
+  if (const uint32_t err = e->h_cnt->img_err) return img_err(e, "image rejected", err);
+  if (e->h_cnt->mrg_dups) return img_err(e, "image rejected", kImgDup);
+  const uint32_t kept = h_off[S], n_rej = h_off[S + 1] - kept;
+  if (kept + n_rej != n)  // every player that passed the checks is kept or rejected
+    return set_err(e, MM_E_STATE, "regroup: %u kept and %u rejected of %u players", kept, n_rej, n);
+  if (n_rej > cap) {
+    *n_rejected = n_rej;
+    return set_err(e, MM_E_CAP, "%u rejected players, cap %u", n_rej, cap);
+  }
+  if ((rc = load_fits(e, kept, m))) return rc;
+  if (n_rej) {
+    CK(cudaMemcpyAsync(rejected, rej, (size_t)n_rej * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+  }
+  std::vector<uint32_t> per(S);
+  for (uint32_t s = 0; s < S; ++s) per[s] = h_off[s + 1] - h_off[s];
+  if ((rc = load_columns(e, per, out, kept, act, m, h.seq_next, "image rejected"))) return rc;
+  *n_rejected = n_rej;
   return MM_OK;
 }
 
@@ -2338,6 +2517,17 @@ int mm_import(mm_engine* e, const void* buf, uint64_t n_bytes) {
   std::lock_guard<std::mutex> lk(e->mu);
   CK(cudaSetDevice(e->device));
   const int rc = import_image(e, static_cast<const uint8_t*>(buf), n_bytes);
+  free_img_scratch(e);
+  return rc;
+}
+
+int mm_import_regroup(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t cap, uint32_t* rejected,
+                      uint32_t* n_rejected) {
+  if (!e || !n_rejected || (n_bytes && !buf) || (cap && !rejected)) return MM_E_ARG;
+  *n_rejected = 0;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  const int rc = regroup_image(e, static_cast<const uint8_t*>(buf), n_bytes, cap, rejected, n_rejected);
   free_img_scratch(e);
   return rc;
 }

@@ -102,10 +102,10 @@ __global__ void __launch_bounds__(256) k_rq_check(const RqCheckArgs a) {
 
 // One CTA: per partition (one warp each) the exclusive scan of its block counts; the partitions' offsets rq_off[0 ..
 // n_segs] among all code-1 entries; every block count then becomes the block's first index in the grouped list.
-// sel[p] = the partition receives players.
+// sel[p] = the partition receives players.  n_segs may be kMaxSegs + 1 (mm_import_regroup adds a reject bucket).
 __global__ void __launch_bounds__(512) k_rq_scan(uint32_t n_segs, uint32_t nblk, uint32_t* __restrict__ blockhist,
                                                  uint32_t* __restrict__ rq_off, uint8_t* __restrict__ sel) {
-  __shared__ uint32_t s_off[kMaxSegs], s_tmp[64];
+  __shared__ uint32_t s_off[kMaxSegs + 1], s_tmp[64];
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (uint32_t p = warp; p < n_segs; p += 16) {
     uint32_t carry = 0;
@@ -137,16 +137,17 @@ __global__ void __launch_bounds__(512) k_rq_scan(uint32_t n_segs, uint32_t nblk,
 
 // The code-1 entries partition by partition, in age order: grp_src[k] = the entry, grp_u[k] = its age (seq - seq_next).
 // The rank inside the block is stable: peers of a partition in a warp by __match_any_sync, per-warp counters in shared
-// memory, a prefix over the block's 8 warps (each warp holds 128 consecutive entries).
+// memory, a prefix over the block's 8 warps (each warp holds 128 consecutive entries).  n_segs <= kMaxSegs + 1, as in
+// k_rq_scan.
 __global__ void __launch_bounds__(256) k_rq_group(uint32_t n, uint32_t n_segs, uint32_t nblk,
                                                   const uint16_t* __restrict__ part, const uint32_t* __restrict__ seq,
                                                   uint32_t seq_next, const uint32_t* __restrict__ blockbase,
                                                   uint32_t* __restrict__ grp_src, uint32_t* __restrict__ grp_u) {
-  __shared__ uint16_t s_wc[8][kMaxSegs + 1];
-  __shared__ uint32_t s_base[kMaxSegs];
+  __shared__ uint16_t s_wc[8][kMaxSegs + 2];
+  __shared__ uint32_t s_base[kMaxSegs + 1];
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t S1 = n_segs + 1;  // digit n_segs = not a code-1 entry
-  for (uint32_t k = tid; k < 8 * (kMaxSegs + 1); k += 256) (&s_wc[0][0])[k] = 0;
+  for (uint32_t k = tid; k < 8 * (kMaxSegs + 2); k += 256) (&s_wc[0][0])[k] = 0;
   for (uint32_t p = tid; p < n_segs; p += 256) s_base[p] = blockbase[(size_t)p * nblk + blockIdx.x];
   __syncthreads();
   uint32_t dg[4], rk[4];

@@ -499,6 +499,21 @@ class Engine:
                                    else buf, np.uint8)
         self._check(self.lib.mm_import(self.h, _p(buf), len(buf)), "mm_import")
 
+    def import_regroup(self, buf):
+        """Load an image written by export_state() under ANOTHER config (rating groups, default group, modes, order,
+        MM_F_WIDE_PARTITIONS) into this fresh engine (mm_import_regroup): every player keeps its id, rating, mode,
+        stamp and sequence number and goes to the queue its rating and mode map to here.  -> image indices (u32,
+        ascending) of the players this config has no queue for: they are not queued, and the caller answers them."""
+        buf = np.ascontiguousarray(np.frombuffer(buf, np.uint8) if isinstance(buf, (bytes, bytearray, memoryview))
+                                   else buf, np.uint8)
+        hs = C.sizeof(abi.ImageHeader)
+        n = abi.ImageHeader.from_buffer_copy(buf[:hs].tobytes()).n_players if len(buf) >= hs else 0
+        n = min(n, len(buf))  # a player takes more than a byte: a corrupt count must not size the reject list
+        rej = np.empty(max(n, 1), np.uint32)
+        k = C.c_uint32(0)
+        self._check(self.lib.mm_import_regroup(self.h, _p(buf), len(buf), n, _p(rej), C.byref(k)), "mm_import_regroup")
+        return rej[:k.value]
+
     def export_queues(self, mask):
         """Release whole (mode, group) queues into a queue image (mm_export_queues) -> uint8 array.  mask: bool per
         queue in queue_stats() record order (mode * n_groups + group), or [n_modes][n_groups].  The exported players

@@ -226,15 +226,19 @@ class SearchPool:
         queue at their enqueue position (Engine.requeue): their wait and the search timeout go on from their first
         enqueue.  players: the lobby's player documents, as the lobby stage has them.  -> one outcome per player:
         "requeued" (queued again; its document is back in the pool), "queued" (still queued: nothing changed) or
-        "gone" (not in this pool's active set — removed, timed out, never queued — or its queue has moved to another
-        pool: answer it as today, remove_user and an error response)."""
+        "gone" (not in this pool's active set — removed, timed out, never queued — its queue has moved to another pool,
+        or its rating or mode has no queue under this pool's config after a resume(regroup=True): answer it as today,
+        remove_user and an error response)."""
         self.flush()
         out = ["gone"] * len(players)
         pos, hs = {}, []
         for i, doc in enumerate(players):
             h = self.handles.lookup(doc.get("id"))
             rec = self.queued.get(h) if h is not None else None
-            if rec is None or h in pos or self._queue_of(rec[0], rec[1]) in self.moved_out:
+            if rec is None or h in pos or rec[1] >= self.engine.cfg.n_modes:
+                continue
+            q = self._queue_of(rec[0], rec[1])
+            if q < 0 or q in self.moved_out:
                 continue
             pos[h] = i
             hs.append(h)
@@ -441,20 +445,41 @@ class SearchPool:
         return self.CHECKPOINT_MAGIC + len(doc).to_bytes(8, "little") + doc + image
 
     @classmethod
-    def resume(cls, engine, blob, mode_names, group_names, **opts):
+    def resume(cls, engine, blob, mode_names, group_names, regroup=False, **opts):
         """A pool on a FRESH engine that goes on where checkpoint() stopped: the engine imports the image
         (Engine.import_state), the handle table, player documents and enqueue times come back, and now_ms() goes on
         from the checkpoint's value plus the wall time the pool was down — the enqueue stamps in the engine stay
-        valid, and waits (timeout_ms, queue_status) include the downtime.  opts: those of SearchPool()."""
+        valid, and waits (timeout_ms, queue_status) include the downtime.  opts: those of SearchPool().
+
+        regroup=True deploys a new config (rating groups, default group, modes, order) without dropping the queue:
+        the engine, created with the new config, re-files the checkpoint's players (Engine.import_regroup), each
+        keeping its place.  Group names may differ freely; a mode keeps its index, so one mode list must be a prefix
+        of the other.  Players whose rating or mode has no queue under the new config are not queued: their handles
+        and records are dropped and their documents are in the returned pool's `regroup_dropped` — answer them with
+        the error response timeout_ms uses (prepare_timeout_response) once the workers are up.  A checkpoint of a pool
+        with queues moved out (move_out) is refused: those queues live in another pool under the old groups."""
         head = len(cls.CHECKPOINT_MAGIC)
         if blob[:head] != cls.CHECKPOINT_MAGIC:
             raise ValueError("not a SearchPool checkpoint")
         n = int.from_bytes(blob[head:head + 8], "little")
         state = json.loads(bytes(blob[head + 8:head + 8 + n]))
-        if state["mode_names"] != list(mode_names) or state["group_names"] != list(group_names):
+        if regroup:
+            old, new = state["mode_names"], list(mode_names)
+            if old[:len(new)] != new[:len(old)]:
+                raise ValueError("regroup keeps each mode's index: one mode list must be a prefix of the other")
+            if state.get("moved_out"):
+                raise ValueError("the checkpoint's pool has queues moved out to another pool under the old groups")
+        elif state["mode_names"] != list(mode_names) or state["group_names"] != list(group_names):
             raise ValueError("the checkpoint was taken with other mode or group names")
         pool = cls(engine, mode_names, group_names, **opts)
-        engine.import_state(bytes(blob[head + 8 + n:]))
+        image = bytes(blob[head + 8 + n:])
+        rejected = []
+        if regroup:
+            from .engine import read_image
+            idx = engine.import_regroup(image)
+            rejected = read_image(image)[1]["id"][idx].tolist()
+        else:
+            engine.import_state(image)
         down = max(0.0, pool.wall_clock() - state["wall"])
         pool._t0 = pool.clock() - down - state["now_ms"] / 1000.0
         pool.handles.id_of = list(state["id_of"])
@@ -466,6 +491,12 @@ class SearchPool:
         pool.matched_at = {int(h): at - age for h, age in state.get("matched_at", [])}
         pool.queued = {int(h): rec for h, rec in state.get("queued", [])}  # the image keeps every sequence number
         pool.moved_out = set(state.get("moved_out", []))
+        pool.regroup_dropped = []
+        for h in rejected:  # not queued under the new config: they left
+            pool.regroup_dropped.append(pool.players.pop(h))
+            for d in (pool.queued, pool.enqueued_at, pool.matched_at):
+                d.pop(h, None)
+            pool.handles.release(pool.handles.id_of[h])
         return pool
 
     # -- moving queues to another running pool -----------------------------------------------------
