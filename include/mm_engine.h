@@ -531,10 +531,56 @@ int mm_import(mm_engine* e, const void* buf, uint64_t n_bytes);
  * partition, section 7 unchanged, the same seq_next.  After mm_import_regroup(img), every later call sequence gives
  * the same results as on a fresh engine that called mm_import(R): as if each kept player had been enqueued into this
  * engine in its original order, with its original stamp and number.  When the configs are equal, R is the image itself.
- * Not covered: queue images (mm_merge still needs equal configs) and sharded deployments (a re-cut moves players
- * between ranks).                                                                                                   */
+ * Not covered: queue images (mm_merge still needs equal configs); a sharded deployment is re-cut with
+ * mm_import_regroup_many below.                                                                                     */
 int mm_import_regroup(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t cap, uint32_t* rejected,
                       uint32_t* n_rejected);
+
+/* EXTENSION (re-cut of a sharded deployment): load up to 64 mm_export images (not queue images) into a FRESH engine.
+ * All of them were written under ONE config, which may differ from the engine's exactly as mm_import_regroup allows
+ * (typically: the old ranks of a deployment sharded by rating group, each exporting its engine, and the new ranks
+ * taking the queues they own under a new group table and owner array).
+ *   keep: n_modes * n_groups bytes of THIS engine's config in the record order of mm_queue_stats (mode * n_groups +
+ *   group); NULL = every queue.  Each image player goes to the queue its (rating, mode) maps to under the engine's
+ *   config: loaded if keep selects the queue; SKIPPED (counted in *n_elsewhere: another rank owns it) if the queue
+ *   exists but is not selected; REJECTED if the engine has no queue for it — rej_image[i], rej_index[i] name the
+ *   image and the player's index in it, ascending by (image, index).
+ *   active_image: the image whose active section (section 7) goes into the active set; UINT32_MAX = none.  In a re-cut
+ *   every rank takes its own: its matched-not-removed ids stay where the lobby stage's mm_remove goes.
+ * ORDER inside a new queue (layout partition).  Take each image's players of that partition in the order
+ * mm_import_regroup would give them (age order, (seq - seq_next) mod 2^32 ascending, with that image's seq_next).
+ * Key each such sequence by the RUNNING MAXIMUM of enq_ts along it, and interleave the images as a stable merge by
+ * that key, ties to the lower image index — the same as a classic head-comparison merge.  With stamps that never
+ * decrease with age (what SearchPool writes) this is plain stamp order, ties by image and then age; with one image it
+ * is mm_import_regroup's order whatever the stamps.
+ * SEQUENCE NUMBERS.  n_images == 1: every number and seq_next are kept — the call is mm_import_regroup plus keep and
+ * active_image.  n_images > 1: the numbers of different engines cannot be compared, so the kept players are numbered
+ * 0 .. n_kept-1 by one global total order, (running-max stamp, image, age, then the lower partition), and seq_next =
+ * n_kept: every partition stays strictly increasing and emit_seq stays an arrival order across queues.  Stamps are
+ * kept, so waits, mm_expire and mm_queue_stats carry over unchanged.
+ * Refusals, all decided by one read of the device's counters before the pool is written; after any of them the engine
+ * is empty and still fresh:
+ *   MM_E_STATE the engine is not fresh, or a packed batch is staged;
+ *   MM_E_ARG   everything mm_import_regroup refuses in any image, with its wording; images whose configs differ from
+ *              each other (groups, default_group, modes, order_mode, flags); n_images of 0 or more than 64;
+ *              active_image out of range; an id repeated within or across the loaded images or the taken active
+ *              section (engines with an active set);
+ *   MM_E_CAP   more than `cap` rejects (*n_rejected = the count: cap = 0 with NULL outputs is a dry run), or the kept
+ *              players do not fit under mm_import's capacity rules.
+ * Cost: every image runs mm_import_regroup's passes; with n_images > 1, ceil(log2 n_images) merge rounds over the
+ * kept players by (running-max stamp, image, age), a segmented max scan for the running maxima, and
+ * ceil(log2 n_parts) rounds that merge the partitions' lists into the global order.  The images are uploaded once
+ * each; the scratch is one allocation sized by the images, freed before the call returns.
+ * EQUIVALENCE.  Let R be the restated image: header config = the engine's config, section 1 = the kept players per
+ * layout partition, sections 2-6 = the kept players partition by partition in the merged order above with the numbers
+ * above, section 7 = active_image's section (empty for none), seq_next as above.  After mm_import_regroup_many, every
+ * later call sequence gives what a fresh engine gives after mm_import(R).
+ * Not covered: a re-cut that changes the number of ranks; host records above the engine (SearchPool's player
+ * documents and requeue records); requeue (mm_requeue) of players matched before a re-cut with n_images > 1, whose old
+ * seq has no place in the new numbering.                                                                            */
+int mm_import_regroup_many(mm_engine* e, uint32_t n_images, const void* const* bufs, const uint64_t* n_bytes,
+                           const uint8_t* keep, uint32_t active_image, uint32_t cap, uint32_t* rej_image,
+                           uint32_t* rej_index, uint32_t* n_rejected, uint32_t* n_elsewhere);
 
 /* ---- queue move: part of an engine into another running engine ---------------------------
  * The reference's queues live in RabbitMQ and its state in replicated Mnesia tables, so any node's workers can serve

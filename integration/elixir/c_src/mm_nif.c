@@ -294,6 +294,55 @@ static ERL_NIF_TERM nif_import_regroup(ErlNifEnv* env, int argc, const ERL_NIF_T
   return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &rej));
 }
 
+/* import_regroup_many(ref, images :: [binary], keep :: binary | nil, active_image :: integer | nil) ->
+ * {:ok, rejected :: binary((u32 image, u32 index)[]), n_elsewhere} | {:error, atom}: a re-cut of a sharded deployment
+ * (mm_import_regroup_many): the old ranks' images, of one config, re-filed into this fresh engine; `keep` selects this
+ * rank's queues (one byte per queue in queue_stats/2 record order; nil = all), `active_image` the image whose active
+ * section it takes (nil = none).  `rejected` pairs name the players this config has no queue for, ascending. */
+static ERL_NIF_TERM nif_import_regroup_many(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary keep, out; unsigned len = 0; uint32_t cap = 0, got = 0, elsewhere = 0, act = UINT32_MAX;
+  const void* bufs[64]; uint64_t sizes[64];
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_list_length(env, argv[1], &len) || len > 64)
+    return enif_make_badarg(env);
+  const int has_keep = !enif_is_identical(argv[2], atom(env, "nil"));
+  if (has_keep && !enif_inspect_binary(env, argv[2], &keep)) return enif_make_badarg(env);
+  if (!enif_is_identical(argv[3], atom(env, "nil")) && !enif_get_uint(env, argv[3], &act)) return enif_make_badarg(env);
+  ERL_NIF_TERM head, tail = argv[1];
+  for (unsigned k = 0; k < len; ++k) {
+    ErlNifBinary img;
+    if (!enif_get_list_cell(env, tail, &head, &tail) || !enif_inspect_binary(env, head, &img)) return enif_make_badarg(env);
+    bufs[k] = img.data;
+    sizes[k] = img.size;
+    if (img.size >= sizeof(mm_image_header)) {
+      mm_image_header h;
+      memcpy(&h, img.data, sizeof(h));
+      const uint32_t n = h.n_players < img.size ? h.n_players : (uint32_t)img.size;  /* a corrupt count must not size it */
+      cap = cap + n < cap ? UINT32_MAX : cap + n;
+    }
+  }
+  if (has_keep) {  /* one byte per queue: mm_queue_stats with cap 0 gives the queue count */
+    uint32_t n_cut = 0;
+    mm_queue_stats(r->e, 0, NULL, 0, &n_cut);
+    if (keep.size != n_cut) return enif_make_badarg(env);
+  }
+  if (!enif_alloc_binary((size_t)cap * 8, &out)) return err(env, MM_E_CAP);
+  uint32_t* img_of = (uint32_t*)enif_alloc((size_t)(cap ? cap : 1) * 4);
+  if (!img_of) { enif_release_binary(&out); return err(env, MM_E_CAP); }
+  uint32_t* idx = (uint32_t*)out.data;
+  int rc = mm_import_regroup_many(r->e, len, bufs, sizes, has_keep ? keep.data : NULL, act, cap, img_of, idx, &got,
+                                  &elsewhere);
+  if (rc) { enif_free(img_of); enif_release_binary(&out); return err(env, rc); }
+  for (uint32_t i = got; i-- > 0;) {  /* interleave in place, from the back: (image, index) pairs */
+    const uint32_t v = idx[i];
+    idx[2 * i + 1] = v;
+    idx[2 * i] = img_of[i];
+  }
+  enif_free(img_of);
+  enif_realloc_binary(&out, (size_t)got * 8);
+  return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &out), enif_make_uint(env, elsewhere));
+}
+
 /* seq_next(ref) -> {:ok, seq}: the enqueue sequence number the next offered player will get (mm_seq_next) */
 static ERL_NIF_TERM nif_seq_next(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
   engine_res* r; uint32_t s = 0;
@@ -431,6 +480,7 @@ static ErlNifFunc funcs[] = {
   {"export_queues", 2, nif_export_queues, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"merge_image", 2, nif_merge_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"import_regroup", 2, nif_import_regroup, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"import_regroup_many", 4, nif_import_regroup_many, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"seq_next", 1, nif_seq_next, 0},
   {"set_max_spread", 2, nif_set_max_spread, 0},

@@ -86,6 +86,15 @@ defmodule Matchmaking.Search.Engine do
   def import_regroup(_ref, _image), do: :erlang.nif_error(:nif_not_loaded)
 
   @doc """
+  Re-cut of a sharded deployment (extension): loads the export_image/1 images of the old ranks (one config, possibly
+  another than this engine's) into this fresh engine (mm_import_regroup_many).  keep :: binary | nil selects this
+  rank's queues (one byte per queue in queue_stats/2 record order); active_image :: integer | nil is the image whose
+  active section this engine takes -> {:ok, rejected :: binary((u32 image, u32 index)[]), n_elsewhere} or
+  {:error, :badarg | :capacity | :state}; after a refusal the engine is still fresh.
+  """
+  def import_regroup_many(_ref, _images, _keep, _active_image), do: :erlang.nif_error(:nif_not_loaded)
+
+  @doc """
   Queue move: the selected (mode, group) queues (queues :: binary, one byte per queue in queue_stats/2 record order,
   mode * n_groups + group, non-zero = selected) leave the engine in a queue image -> {:ok, image}.  The players are
   released as if removed, in the same call; matched players not yet removed stay here.

@@ -181,6 +181,8 @@ PROTOTYPES = {
     "mm_export_queues": (C.c_int, [_vp, _vp, _vp, C.c_uint64, _P(C.c_uint64)]),
     "mm_merge": (C.c_int, [_vp, _vp, C.c_uint64, C.c_uint32, _vp, _P(C.c_uint32)]),
     "mm_import_regroup": (C.c_int, [_vp, _vp, C.c_uint64, C.c_uint32, _vp, _P(C.c_uint32)]),
+    "mm_import_regroup_many": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp,
+                                         _P(C.c_uint32), _P(C.c_uint32)]),
     "mm_snapshot": (C.c_int, [_vp]),
     "mm_restore": (C.c_int, [_vp]),
     "mm_set_stream": (C.c_int, [_vp, _vp]),

@@ -23,6 +23,7 @@
 #include "mm_expire.cuh"
 #include "mm_image.cuh"
 #include "mm_kernels.cuh"
+#include "mm_recut.cuh"
 #include "mm_regroup.cuh"
 #include "mm_requeue.cuh"
 #include "mm_stats.cuh"
@@ -1603,130 +1604,296 @@ int requeue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating,
   return MM_OK;
 }
 
-// ---- mm_import_regroup (mm_regroup.cuh) -------------------------------------------------------------------------
-// Every refusal is decided by one read of the counters, before the load tail
-// writes the pool.
-int regroup_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uint32_t* rejected,
-                  uint32_t* n_rejected) {
+// ---- mm_import_regroup / mm_import_regroup_many (mm_regroup.cuh, mm_recut.cuh) -----------------------------------
+// K images of one config: each runs the regroup pipeline on its own; for K > 1 the images' runs are merged and the
+// kept players renumbered on the device.  Every refusal is decided by one read of the counters, before the load tail
+// writes the pool.  `who` names the call in the state refusal; keep_cut: n_cut selection bytes (null: all); act_img:
+// the image whose active section is taken (>= K: none).
+int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const* bufs, const uint64_t* nbs,
+                 const uint8_t* keep_cut, uint32_t act_img, uint32_t cap, uint32_t* rej_image, uint32_t* rej_index,
+                 uint32_t* n_rejected, uint32_t* n_elsewhere) {
   if (!e->fresh || e->stage_count)
-    return set_err(e, MM_E_STATE, "mm_import_regroup needs a fresh engine (nothing enqueued, imported or restored)");
-  mm_image_header h;
-  ImgLayout l;
-  std::vector<uint32_t> cnt;
-  Layout y;  // the image's layout
-  int rc = check_header(e, buf, nb, MM_IMAGE_MAGIC, "image rejected", "bad magic",
-                        e->use_active ? nullptr : "active section in an image of an engine without an active set", h, l,
-                        cnt, &y);
-  if (rc) return rc;
-  const uint32_t n = h.n_players, m = h.n_active, S = e->n_segs, SI = y.n_segs, idb = h.id_bytes;
-  const uint64_t body = nb - l.off[1];
-  CK(e->d_img.reserve(std::max<uint64_t>(body, 8)));
-  if (body) CK(cudaMemcpyAsync(e->d_img, buf + l.off[1], body, cudaMemcpyHostToDevice, e->stream));
-  const ImgCols in = img_cols(e->d_img, l, idb);
-  const void* act = e->d_img + (l.off[6] - l.off[1]);
-  if (n == 0) return load_columns(e, std::vector<uint32_t>(S, 0), in, 0, act, m, h.seq_next, "image rejected");
-  // scratch: the image's tables, the classification, the scatter and merge buffers, the gathered columns
-  const uint32_t nblk = (n + kRqItems - 1) / kRqItems;
+    return set_err(e, MM_E_STATE, "%s needs a fresh engine (nothing enqueued, imported or restored)", who);
+  if (K == 0 || K > kRcMaxImages) return set_err(e, MM_E_ARG, "n_images must be 1 .. %u", kRcMaxImages);
+  if (act_img != 0xFFFFFFFFu && act_img >= K) return set_err(e, MM_E_ARG, "active_image out of range");
+  std::vector<mm_image_header> h(K);
+  std::vector<ImgLayout> l(K);
+  std::vector<std::vector<uint32_t>> cnt(K);
+  Layout y;  // the images' layout
+  int rc;
+  for (uint32_t k = 0; k < K; ++k) {
+    const char* no_active =
+        k == act_img && !e->use_active ? "active section in an image of an engine without an active set" : nullptr;
+    if ((rc = check_header(e, bufs[k], nbs[k], MM_IMAGE_MAGIC, "image rejected", "bad magic", no_active, h[k], l[k],
+                           cnt[k], &y)))
+      return rc;
+    if (k && !same_layout(h[k].config, h[0].config))
+      return set_err(e, MM_E_ARG, "image rejected: its config differs from image 0's");
+  }
+  const uint32_t S = e->n_segs, SI = y.n_segs, idb = h[0].id_bytes;
+  const uint32_t m = act_img < K ? h[act_img].n_active : 0;
+  std::vector<uint32_t> base(K + 1, 0), nblk(K);
+  uint64_t total = 0;
+  for (uint32_t k = 0; k < K; ++k) {
+    total += h[k].n_players;
+    if (total > 0x7FFFFFFFu) return set_err(e, MM_E_CAP, "more than 2^31 - 1 players in the images");
+    base[k + 1] = (uint32_t)total;
+    nblk[k] = (h[k].n_players + kRqItems - 1) / kRqItems;
+  }
+  const uint32_t N = base[K];
+  std::vector<uint64_t> boff(K + 1, 0);  // each image's body (section 2 on) in d_img, 16-byte aligned
+  for (uint32_t k = 0; k < K; ++k) boff[k + 1] = boff[k] + ((nbs[k] - l[k].off[1] + 15) & ~(uint64_t)15);
+  CK(e->d_img.reserve(std::max<uint64_t>(boff[K], 8)));
+  for (uint32_t k = 0; k < K; ++k)
+    if (nbs[k] > l[k].off[1])
+      CK(cudaMemcpyAsync(e->d_img + boff[k], bufs[k] + l[k].off[1], nbs[k] - l[k].off[1], cudaMemcpyHostToDevice,
+                         e->stream));
+  std::vector<ImgCols> in(K);
+  for (uint32_t k = 0; k < K; ++k) in[k] = img_cols(e->d_img + boff[k], l[k], idb);
+  const void* act = act_img < K ? (const void*)(e->d_img + boff[act_img] + (l[act_img].off[6] - l[act_img].off[1]))
+                                : (const void*)e->d_img.p;
+  const uint32_t seq_next = K == 1 ? h[0].seq_next : 0;  // K > 1: renumbered, seq_next = the kept count
+  if (n_elsewhere) *n_elsewhere = 0;
+  if (N == 0) return load_columns(e, std::vector<uint32_t>(S, 0), in[0], 0, act, m, seq_next, "image rejected");
+  // scratch: the images' tables, the classification, the scatter and merge buffers, the gathered columns
   uint64_t sc = 0;  // the repeated-id set: at most half full
-  if (e->use_active) for (sc = 1024; sc < 2ull * ((uint64_t)n + m); sc <<= 1) {}
-  std::vector<uint32_t> off(SI + 1, 0);
-  for (uint32_t s = 0; s < SI; ++s) off[s + 1] = off[s] + cnt[s];
-  const size_t pair_n = (size_t)SI * S;
-  size_t o = 0;  // the scratch arrays' offsets in d_rg, 8-byte aligned
-  auto take = [&o](size_t bytes) { const size_t x = o; o += (bytes + 7) & ~(size_t)7; return x; };
+  if (e->use_active) for (sc = 1024; sc < 2ull * ((uint64_t)N + m); sc <<= 1) {}
+  std::vector<uint32_t> off((size_t)K * (SI + 1), 0);
+  for (uint32_t k = 0; k < K; ++k)
+    for (uint32_t s = 0; s < SI; ++s) off[(size_t)k * (SI + 1) + s + 1] = off[(size_t)k * (SI + 1) + s] + cnt[k][s];
+  std::vector<uint8_t> keep;  // per new partition
+  if (keep_cut) {
+    keep.resize(S);
+    for (uint32_t q = 0; q < S; ++q) keep[q] = keep_cut[e->h_part_cut[q]] != 0;
+  }
+  uint64_t hist_n = 0;
+  for (uint32_t k = 0; k < K; ++k) hist_n += (uint64_t)(S + 1) * nblk[k];
+  const size_t pair_n = (size_t)SI * S, R1 = S + 2;  // per image: (image partition, new partition) pairs; rq_off
+  const uint32_t nrb = (N + kRcBlock - 1) / kRcBlock;
+  size_t o = 0;  // the scratch arrays' offsets in d_rg, 16-byte aligned
+  auto take = [&o](size_t bytes) { const size_t x = o; o += (bytes + 15) & ~(size_t)15; return x; };
   const size_t o_seen = take(8 * sc), o_lut = take(2 * (size_t)y.KR), o_grp = take(y.KR), o_bseg = take(2 * (size_t)y.Kp),
-               o_off = take(4 * ((size_t)SI + 1)), o_rq = take(4 * ((size_t)S + 2)), o_sel = take((size_t)S + 1),
-               o_hist = take(4 * ((size_t)S + 1) * nblk), o_pair = take(4 * pair_n), o_ord = take(2 * pair_n),
-               o_run = take(4 * (size_t)S * (SI + 1)), o_kq = take(4 * (size_t)S), o_part = take(2 * (size_t)n),
-               o_pimg = take(2 * (size_t)n), o_src0 = take(4 * (size_t)n), o_src1 = take(4 * (size_t)n),
-               o_age0 = take(4 * (size_t)n), o_age1 = take(4 * (size_t)n), o_rej = take(4 * (size_t)n),
-               o_out = take(cols_bytes(n));
+               o_off = take(4 * off.size()), o_rq = take(4 * R1 * K), o_sel = take((size_t)S + 1),
+               o_keep = take(keep.size()), o_skip = take(4 * (size_t)K), o_hist = take(4 * hist_n),
+               o_pair = take(4 * pair_n * K), o_ord = take(2 * pair_n * K), o_run = take(4 * (size_t)S * (SI + 1) * K),
+               o_kq = take(4 * (size_t)S * K), o_part = take(2 * (size_t)N), o_pimg = take(2 * (size_t)N),
+               o_src0 = take(4 * (size_t)N), o_src1 = take(4 * (size_t)N), o_age0 = take(4 * (size_t)N),
+               o_age1 = take(4 * (size_t)N), o_rej = take(K == 1 ? 4 * (size_t)N : 0), o_out = take(cols_bytes(N));
+  // K > 1: the image runs' merge and the numbering
+  const bool many = K > 1;
+  auto take2 = [&](size_t bytes) { return many ? take(bytes) : 0; };
+  const size_t o_rqg = take2(4 * ((size_t)S + 1)), o_one = take2(4 * 4), o_pair2 = take2(4 * (size_t)K * S),
+               o_ord2 = take2(2 * (size_t)K * S), o_run2 = take2(4 * (size_t)S * (K + 1)), o_kq2 = take2(4 * (size_t)S),
+               o_ident = take2(2 * (size_t)S), o_s2a = take2(4 * (size_t)N), o_s2b = take2(4 * (size_t)N),
+               o_keya = take2(sizeof(RcKey) * N), o_keyb = take2(sizeof(RcKey) * N), o_head = take2(N),
+               o_img = take2(2 * (size_t)N), o_qv = take2(2 * (size_t)N), o_agg = take2(sizeof(RcSeg) * nrb),
+               o_carry = take2(sizeof(RcSeg) * nrb), o_first = take2(4 * (size_t)nrb), o_pos = take2(4 * (size_t)N),
+               o_imgs = take2(sizeof(ImgCols) * K), o_base = take2(4 * (size_t)K);
   CK(e->d_rg.reserve(o));
-  uint8_t* const base = e->d_rg;
-  auto* seen = reinterpret_cast<unsigned long long*>(base + o_seen);
-  auto* lut_i = reinterpret_cast<uint16_t*>(base + o_lut);
-  uint8_t* grp_i = base + o_grp;
-  auto* bseg_i = reinterpret_cast<uint16_t*>(base + o_bseg);
-  auto* off_i = reinterpret_cast<uint32_t*>(base + o_off);
-  auto* rq_off = reinterpret_cast<uint32_t*>(base + o_rq);
-  uint8_t* sel = base + o_sel;
-  auto* bhist = reinterpret_cast<uint32_t*>(base + o_hist);
-  auto* pair = reinterpret_cast<uint32_t*>(base + o_pair);
-  auto* ord = reinterpret_cast<uint16_t*>(base + o_ord);
-  auto* run_start = reinterpret_cast<uint32_t*>(base + o_run);
-  auto* kq = reinterpret_cast<uint32_t*>(base + o_kq);
-  auto* part = reinterpret_cast<uint16_t*>(base + o_part);
-  auto* pimg = reinterpret_cast<uint16_t*>(base + o_pimg);
-  uint32_t* src[2] = {reinterpret_cast<uint32_t*>(base + o_src0), reinterpret_cast<uint32_t*>(base + o_src1)};
-  uint32_t* age[2] = {reinterpret_cast<uint32_t*>(base + o_age0), reinterpret_cast<uint32_t*>(base + o_age1)};
-  auto* rej = reinterpret_cast<uint32_t*>(base + o_rej);
-  uint8_t* at = base + o_out;
-  ImgCols out = carve_cols(at, n);
+  uint8_t* const sb = e->d_rg;
+  auto at = [sb](size_t x) { return sb + x; };
+  auto* seen = reinterpret_cast<unsigned long long*>(at(o_seen));
+  auto* lut_i = reinterpret_cast<uint16_t*>(at(o_lut));
+  uint8_t* grp_i = at(o_grp);
+  auto* bseg_i = reinterpret_cast<uint16_t*>(at(o_bseg));
+  auto* off_i = reinterpret_cast<uint32_t*>(at(o_off));
+  auto* rq_off = reinterpret_cast<uint32_t*>(at(o_rq));
+  uint8_t* sel = at(o_sel);
+  auto* skip = reinterpret_cast<uint32_t*>(at(o_skip));
+  auto* part = reinterpret_cast<uint16_t*>(at(o_part));
+  auto* pimg = reinterpret_cast<uint16_t*>(at(o_pimg));
+  uint32_t* src[2] = {reinterpret_cast<uint32_t*>(at(o_src0)), reinterpret_cast<uint32_t*>(at(o_src1))};
+  uint32_t* age[2] = {reinterpret_cast<uint32_t*>(at(o_age0)), reinterpret_cast<uint32_t*>(at(o_age1))};
+  uint8_t* ocur = at(o_out);
+  ImgCols out = carve_cols(ocur, N);
   out.id_bytes = idb;
   CK(cudaMemcpyAsync(lut_i, y.lut.data(), (size_t)y.KR * 2, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(grp_i, y.grp.data(), y.KR, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(bseg_i, y.bin_seg.data(), (size_t)y.Kp * 2, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(off_i, off.data(), off.size() * 4, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemsetAsync(pair, 0, pair_n * 4, e->stream));
-  CK(cudaMemsetAsync(ord, 0, pair_n * 2, e->stream));
-  CK(cudaMemsetAsync(src[1], 0, (size_t)n * 4, e->stream));  // a merge that writes holes (a refused image) stays in range
+  if (keep_cut) CK(cudaMemcpyAsync(at(o_keep), keep.data(), S, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemsetAsync(skip, 0, 4 * (size_t)K, e->stream));
+  CK(cudaMemsetAsync(at(o_pair), 0, pair_n * 4 * K, e->stream));
+  CK(cudaMemsetAsync(at(o_ord), 0, pair_n * 2 * K, e->stream));
+  CK(cudaMemsetAsync(src[1], 0, (size_t)N * 4, e->stream));  // a merge that writes holes (a refused image) stays in range
   CK(cudaMemsetAsync(&e->d_cnt->img_err, 0, 3 * 4, e->stream));  // img_err, mrg_dups, rg_kmax
-  // 1. classify
-  RgClassifyArgs ca{};
-  ca.in = in; ca.n = n; ca.nblk = nblk; ca.part_off = off_i; ca.n_img_segs = SI;
-  ca.bm_img = BinMap{lut_i, y.key_lo, y.KR, y.stride, y.K};
-  ca.grp_img = grp_i; ca.bin_seg_img = bseg_i; ca.n_modes_img = h.config.n_modes; ca.seq_next = h.seq_next;
-  ca.id_limit = id_limit(e);
-  ca.bm = bin_map(e); ca.grp_lut = e->d_grp_lut; ca.bin_seg = e->d_bin_seg; ca.n_modes = e->cfg.n_modes; ca.n_segs = S;
-  ca.part = part; ca.pimg = pimg; ca.blockhist = bhist; ca.pair = pair; ca.err = &e->d_cnt->img_err;
-  k_rg_classify<<<nblk, 256, 0, e->stream>>>(ca);
-  const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((n + 255) / 256, 32u * (uint32_t)e->n_sms));
-  if (e->use_active) {
-    CK(cudaMemsetAsync(seen, 0xFF, sc * 8, e->stream));
-    k_rg_dups<<<grid, 256, 0, e->stream>>>(in.id, act, idb, n, m, seen, sc - 1, &e->d_cnt->mrg_dups);
+  if (e->use_active) CK(cudaMemsetAsync(seen, 0xFF, sc * 8, e->stream));
+  // 1. per image: classify, repeated ids, the stable scatter by new partition (reject bucket S last), the run plan
+  const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((N + 255) / 256, 32u * (uint32_t)e->n_sms));
+  uint64_t hoff = 0;
+  for (uint32_t k = 0; k < K; ++k) {
+    const uint32_t n = h[k].n_players, b = base[k];
+    auto* bhist = reinterpret_cast<uint32_t*>(at(o_hist)) + hoff;
+    hoff += (uint64_t)(S + 1) * nblk[k];
+    auto* pair = reinterpret_cast<uint32_t*>(at(o_pair)) + pair_n * k;
+    auto* ord = reinterpret_cast<uint16_t*>(at(o_ord)) + pair_n * k;
+    auto* run_start = reinterpret_cast<uint32_t*>(at(o_run)) + (size_t)S * (SI + 1) * k;
+    auto* kq = reinterpret_cast<uint32_t*>(at(o_kq)) + (size_t)S * k;
+    const bool take_act = k == act_img && m;
+    if (n) {
+      RgClassifyArgs ca{};
+      ca.in = in[k]; ca.n = n; ca.nblk = nblk[k]; ca.part_off = off_i + (size_t)k * (SI + 1); ca.n_img_segs = SI;
+      ca.bm_img = BinMap{lut_i, y.key_lo, y.KR, y.stride, y.K};
+      ca.grp_img = grp_i; ca.bin_seg_img = bseg_i; ca.n_modes_img = h[k].config.n_modes; ca.seq_next = h[k].seq_next;
+      ca.id_limit = id_limit(e);
+      ca.bm = bin_map(e); ca.grp_lut = e->d_grp_lut; ca.bin_seg = e->d_bin_seg; ca.n_modes = e->cfg.n_modes; ca.n_segs = S;
+      ca.keep = keep_cut ? at(o_keep) : nullptr; ca.n_skip = skip + k;
+      ca.part = part + b; ca.pimg = pimg + b; ca.blockhist = bhist; ca.pair = pair; ca.err = &e->d_cnt->img_err;
+      k_rg_classify<<<nblk[k], 256, 0, e->stream>>>(ca);
+    }
+    if (e->use_active && (n || take_act))
+      k_rg_dups<<<grid, 256, 0, e->stream>>>(in[k].id, act, idb, n, take_act ? m : 0, seen, sc - 1,
+                                              &e->d_cnt->mrg_dups);
+    if (n) {
+      k_rq_scan<<<1, 512, 0, e->stream>>>(S + 1, nblk[k], bhist, rq_off + R1 * k, sel);
+      k_rq_group<<<nblk[k], 256, 0, e->stream>>>(n, S + 1, nblk[k], part + b, in[k].seq, h[k].seq_next, bhist,
+                                                  src[0] + b, age[0] + b);
+      k_rg_plan<<<1, 1024, 0, e->stream>>>(SI, S, pair, rq_off + R1 * k, ord, run_start, kq, &e->d_cnt->rg_kmax);
+    } else {
+      CK(cudaMemsetAsync(rq_off + R1 * k, 0, 4 * R1, e->stream));
+    }
   }
-  // 2. order: the stable scatter by new partition (reject bucket S last), the plan of the runs, the merge rounds
-  k_rq_scan<<<1, 512, 0, e->stream>>>(S + 1, nblk, bhist, rq_off, sel);
-  k_rq_group<<<nblk, 256, 0, e->stream>>>(n, S + 1, nblk, part, in.seq, h.seq_next, bhist, src[0], age[0]);
-  k_rg_plan<<<1, 1024, 0, e->stream>>>(SI, S, pair, rq_off, ord, run_start, kq, &e->d_cnt->rg_kmax);
-  uint32_t rounds = 0;  // enough for any k_max <= SI; the rounds past the need return at once
+  // 2. per image: the merge rounds by age (enough for any k_max <= SI; the rounds past the need return at once)
+  uint32_t rounds = 0;
   while ((1u << rounds) < SI) ++rounds;
-  for (uint32_t t = 0; t < rounds; ++t) {
-    RgMergeArgs ma{};
-    ma.rq_off = rq_off; ma.n_segs = S; ma.n_img_segs = SI; ma.round = t; ma.pimg = pimg; ma.ord = ord;
-    ma.run_start = run_start; ma.kq = kq; ma.kmax = &e->d_cnt->rg_kmax;
-    ma.src_in = src[t & 1]; ma.u_in = age[t & 1]; ma.src_out = src[(t + 1) & 1]; ma.u_out = age[(t + 1) & 1];
-    k_rg_merge<<<grid, 256, 0, e->stream>>>(ma);
+  for (uint32_t k = 0; k < K; ++k) {
+    const uint32_t b = base[k];
+    if (!h[k].n_players) continue;
+    for (uint32_t t = 0; t < rounds; ++t) {
+      RgMergeArgs ma{};
+      ma.rq_off = rq_off + R1 * k; ma.n_segs = S; ma.n_img_segs = SI; ma.round = t; ma.pimg = pimg + b;
+      ma.ord = reinterpret_cast<uint16_t*>(at(o_ord)) + pair_n * k;
+      ma.run_start = reinterpret_cast<uint32_t*>(at(o_run)) + (size_t)S * (SI + 1) * k;
+      ma.kq = reinterpret_cast<uint32_t*>(at(o_kq)) + (size_t)S * k; ma.kmax = &e->d_cnt->rg_kmax;
+      ma.src_in = src[t & 1] + b; ma.u_in = age[t & 1] + b; ma.src_out = src[(t + 1) & 1] + b;
+      ma.u_out = age[(t + 1) & 1] + b;
+      k_rg_merge<<<grid, 256, 0, e->stream>>>(ma);
+    }
   }
-  // 3. duplicate ages, the gathered columns, the reject list
-  RgFinishArgs fa{};
-  fa.rq_off = rq_off; fa.n_segs = S; fa.n = n; fa.kmax = &e->d_cnt->rg_kmax;
-  fa.src[0] = src[0]; fa.src[1] = src[1]; fa.u[0] = age[0]; fa.u[1] = age[1];
-  fa.in = in; fa.out = out; fa.rejected = rej; fa.err = &e->d_cnt->img_err;
-  k_rg_finish<<<grid, 256, 0, e->stream>>>(fa);
+  // 3. one image: duplicate ages, the gathered columns, the reject list (mm_import_regroup's tail)
+  if (!many) {
+    RgFinishArgs fa{};
+    fa.rq_off = rq_off; fa.n_segs = S; fa.n = N; fa.kmax = &e->d_cnt->rg_kmax;
+    fa.src[0] = src[0]; fa.src[1] = src[1]; fa.u[0] = age[0]; fa.u[1] = age[1];
+    fa.in = in[0]; fa.out = out; fa.rejected = reinterpret_cast<uint32_t*>(at(o_rej)); fa.err = &e->d_cnt->img_err;
+    k_rg_finish<<<grid, 256, 0, e->stream>>>(fa);
+  } else {
+    // 3'. several images: their runs of every new partition merged by (running-max stamp, image, age), then numbered
+    auto* rq_glob = reinterpret_cast<uint32_t*>(at(o_rqg));
+    auto* rq_one = reinterpret_cast<uint32_t*>(at(o_one));  // {0, kept, S, unused}
+    auto* pair2 = reinterpret_cast<uint32_t*>(at(o_pair2));
+    auto* ord2 = reinterpret_cast<uint16_t*>(at(o_ord2));
+    auto* run2 = reinterpret_cast<uint32_t*>(at(o_run2));
+    auto* kq2 = reinterpret_cast<uint32_t*>(at(o_kq2));
+    auto* ident = reinterpret_cast<uint16_t*>(at(o_ident));
+    uint32_t* s2[2] = {reinterpret_cast<uint32_t*>(at(o_s2a)), reinterpret_cast<uint32_t*>(at(o_s2b))};
+    RcKey* key[2] = {reinterpret_cast<RcKey*>(at(o_keya)), reinterpret_cast<RcKey*>(at(o_keyb))};
+    auto* head = at(o_head);
+    auto* img = reinterpret_cast<uint16_t*>(at(o_img));
+    auto* qv = reinterpret_cast<uint16_t*>(at(o_qv));
+    auto* agg = reinterpret_cast<RcSeg*>(at(o_agg));
+    auto* carry = reinterpret_cast<RcSeg*>(at(o_carry));
+    auto* first = reinterpret_cast<uint32_t*>(at(o_first));
+    auto* pos = reinterpret_cast<uint32_t*>(at(o_pos));
+    auto* d_imgs = reinterpret_cast<ImgCols*>(at(o_imgs));
+    auto* d_base = reinterpret_cast<uint32_t*>(at(o_base));
+    uint32_t* const kmax2 = rq_one + 3;
+    std::vector<uint16_t> id16(S);
+    for (uint32_t q = 0; q < S; ++q) id16[q] = (uint16_t)q;
+    const uint32_t SS[2] = {S, 0};
+    CK(cudaMemcpyAsync(ident, id16.data(), (size_t)S * 2, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(rq_one + 2, SS, 8, cudaMemcpyHostToDevice, e->stream));  // S for the numbering rounds; kmax2 = 0
+    CK(cudaMemcpyAsync(d_imgs, in.data(), sizeof(ImgCols) * K, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(d_base, base.data(), 4 * (size_t)K, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemsetAsync(ord2, 0, 2 * (size_t)K * S, e->stream));
+    CK(cudaMemsetAsync(s2[0], 0, 4 * (size_t)N, e->stream));  // holes (a refused image) stay in range
+    CK(cudaMemsetAsync(s2[1], 0, 4 * (size_t)N, e->stream));
+    CK(cudaMemsetAsync(img, 0, 2 * (size_t)N, e->stream));
+    CK(cudaMemsetAsync(qv, 0, 2 * (size_t)N, e->stream));
+    k_rc_sum<<<1, 1024, 0, e->stream>>>(K, S, rq_off, rq_glob, rq_one, pair2);
+    k_rg_plan<<<1, 1024, 0, e->stream>>>(K, S, pair2, rq_glob, ord2, run2, kq2, kmax2);
+    for (uint32_t k = 0; k < K; ++k) {
+      if (!h[k].n_players) continue;
+      RcGatherArgs ga{};
+      ga.k = k; ga.base = base[k]; ga.n = h[k].n_players; ga.n_segs = S; ga.n_img = K; ga.rq_off = rq_off + R1 * k;
+      ga.kmax = &e->d_cnt->rg_kmax; ga.src[0] = src[0] + base[k]; ga.src[1] = src[1] + base[k];
+      ga.age[0] = age[0] + base[k]; ga.age[1] = age[1] + base[k]; ga.ord = ord2; ga.run_start = run2;
+      ga.ts = in[k].ts; ga.src_out = s2[0]; ga.key_out = key[0]; ga.head = head; ga.img = img; ga.qv = qv;
+      ga.err = &e->d_cnt->img_err;
+      const uint32_t g = std::max<uint32_t>(1, std::min<uint32_t>((h[k].n_players + 255) / 256, 32u * (uint32_t)e->n_sms));
+      k_rc_gather<<<g, 256, 0, e->stream>>>(ga);
+    }
+    k_rc_runmax<<<nrb, 256, 0, e->stream>>>(rq_one + 1, key[0], head, agg, first);
+    k_rc_carry<<<1, 1024, 0, e->stream>>>(rq_one + 1, agg, carry);
+    k_rc_apply<<<nrb, 256, 0, e->stream>>>(rq_one + 1, key[0], carry, first);
+    uint32_t r2 = 0;
+    while ((1u << r2) < K) ++r2;
+    for (uint32_t t = 0; t < r2; ++t) {
+      RgMergeArgsT<RcKey> ma{};
+      ma.rq_off = rq_glob; ma.n_segs = S; ma.n_img_segs = K; ma.round = t; ma.pimg = img; ma.ord = ord2;
+      ma.run_start = run2; ma.kq = kq2; ma.kmax = kmax2;
+      ma.src_in = s2[t & 1]; ma.u_in = key[t & 1]; ma.src_out = s2[(t + 1) & 1]; ma.u_out = key[(t + 1) & 1];
+      k_rg_merge<<<grid, 256, 0, e->stream>>>(ma);
+    }
+    RcFinishArgs fa{};
+    fa.rq_glob = rq_glob; fa.n_segs = S; fa.kmax = kmax2; fa.src[0] = s2[0]; fa.src[1] = s2[1];
+    fa.key[0] = key[0]; fa.key[1] = key[1]; fa.imgs = d_imgs; fa.img = img; fa.base = d_base; fa.out = out; fa.pos = pos;
+    k_rc_finish<<<grid, 256, 0, e->stream>>>(fa);
+    uint32_t r3 = 0;
+    while ((1u << r3) < S) ++r3;
+    for (uint32_t t = 0; t < r3; ++t) {  // the partitions' lists are the runs of one list: run q = partition q
+      RgMergeArgsT<RcKey> ma{};
+      ma.rq_off = rq_one; ma.n_segs = 1; ma.n_img_segs = S; ma.round = t; ma.pimg = qv; ma.ord = ident;
+      ma.run_start = rq_glob; ma.kq = rq_one + 2; ma.kmax = rq_one + 2;
+      ma.src_in = s2[t & 1]; ma.u_in = key[t & 1]; ma.src_out = s2[(t + 1) & 1]; ma.u_out = key[(t + 1) & 1];
+      k_rg_merge<<<grid, 256, 0, e->stream>>>(ma);
+    }
+    k_rc_number<<<grid, 256, 0, e->stream>>>(rq_one + 1, s2[r3 & 1], pos, out.seq);
+  }
   CK(cudaGetLastError());
   // 4. one read decides every refusal
-  std::vector<uint32_t> h_off(S + 2);
+  std::vector<uint32_t> h_off(R1 * K), h_skip(K);
   CK(cudaMemcpyAsync(h_off.data(), rq_off, h_off.size() * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(h_skip.data(), skip, 4 * (size_t)K, cudaMemcpyDeviceToHost, e->stream));
   if ((rc = read_counters(e))) return rc;
   if (const uint32_t err = e->h_cnt->img_err) return img_err(e, "image rejected", err);
   if (e->h_cnt->mrg_dups) return img_err(e, "image rejected", kImgDup);
-  const uint32_t kept = h_off[S], n_rej = h_off[S + 1] - kept;
-  if (kept + n_rej != n)  // every player that passed the checks is kept or rejected
-    return set_err(e, MM_E_STATE, "regroup: %u kept and %u rejected of %u players", kept, n_rej, n);
+  uint32_t kept = 0, n_rej = 0, n_skip = 0;
+  for (uint32_t k = 0; k < K; ++k) {
+    const uint32_t* r = h_off.data() + R1 * k;
+    if (r[S + 1] + h_skip[k] != h[k].n_players)  // every player that passed the checks is kept, skipped or rejected
+      return set_err(e, MM_E_STATE, "regroup: %u kept or rejected and %u skipped of %u players", r[S + 1], h_skip[k],
+                     h[k].n_players);
+    kept += r[S]; n_rej += r[S + 1] - r[S]; n_skip += h_skip[k];
+  }
   if (n_rej > cap) {
     *n_rejected = n_rej;
     return set_err(e, MM_E_CAP, "%u rejected players, cap %u", n_rej, cap);
   }
   if ((rc = load_fits(e, kept, m))) return rc;
   if (n_rej) {
-    CK(cudaMemcpyAsync(rejected, rej, (size_t)n_rej * 4, cudaMemcpyDeviceToHost, e->stream));
+    if (!many) {
+      CK(cudaMemcpyAsync(rej_index, at(o_rej), (size_t)n_rej * 4, cudaMemcpyDeviceToHost, e->stream));
+    } else {  // each image's reject bucket, in image order: (image, index) ascending
+      for (uint32_t k = 0, w = 0; k < K; ++k) {
+        const uint32_t* r = h_off.data() + R1 * k;
+        if (r[S + 1] > r[S])
+          CK(cudaMemcpyAsync(rej_index + w, src[0] + base[k] + r[S], (size_t)(r[S + 1] - r[S]) * 4,
+                             cudaMemcpyDeviceToHost, e->stream));
+        w += r[S + 1] - r[S];
+      }
+    }
     CK(cudaStreamSynchronize(e->stream));
+    if (rej_image)
+      for (uint32_t k = 0, w = 0; k < K; ++k)
+        for (uint32_t j = h_off[R1 * k + S]; j < h_off[R1 * k + S + 1]; ++j) rej_image[w++] = k;
   }
-  std::vector<uint32_t> per(S);
-  for (uint32_t s = 0; s < S; ++s) per[s] = h_off[s + 1] - h_off[s];
-  if ((rc = load_columns(e, per, out, kept, act, m, h.seq_next, "image rejected"))) return rc;
+  std::vector<uint32_t> per(S, 0);
+  for (uint32_t k = 0; k < K; ++k)
+    for (uint32_t s = 0; s < S; ++s) per[s] += h_off[R1 * k + s + 1] - h_off[R1 * k + s];
+  if ((rc = load_columns(e, per, out, kept, act, m, many ? kept : seq_next, "image rejected"))) return rc;
   *n_rejected = n_rej;
+  if (n_elsewhere) *n_elsewhere = n_skip;
   return MM_OK;
 }
 
@@ -2527,7 +2694,28 @@ int mm_import_regroup(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t 
   *n_rejected = 0;
   std::lock_guard<std::mutex> lk(e->mu);
   CK(cudaSetDevice(e->device));
-  const int rc = regroup_image(e, static_cast<const uint8_t*>(buf), n_bytes, cap, rejected, n_rejected);
+  const uint8_t* b = static_cast<const uint8_t*>(buf);
+  const int rc = regroup_many(e, "mm_import_regroup", 1, &b, &n_bytes, nullptr, 0, cap, nullptr, rejected, n_rejected,
+                              nullptr);
+  free_img_scratch(e);
+  return rc;
+}
+
+int mm_import_regroup_many(mm_engine* e, uint32_t n_images, const void* const* bufs, const uint64_t* n_bytes,
+                           const uint8_t* keep, uint32_t active_image, uint32_t cap, uint32_t* rej_image,
+                           uint32_t* rej_index, uint32_t* n_rejected, uint32_t* n_elsewhere) {
+  if (!e || !n_rejected || !n_elsewhere || (n_images && (!bufs || !n_bytes)) || (cap && (!rej_image || !rej_index)))
+    return MM_E_ARG;
+  *n_rejected = 0;
+  *n_elsewhere = 0;
+  for (uint32_t k = 0; k < n_images && k < kRcMaxImages; ++k)
+    if (n_bytes[k] && !bufs[k]) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  std::vector<const uint8_t*> b(n_images <= kRcMaxImages ? n_images : 0);
+  for (size_t k = 0; k < b.size(); ++k) b[k] = static_cast<const uint8_t*>(bufs[k]);
+  const int rc = regroup_many(e, "mm_import_regroup_many", n_images, b.data(), n_bytes, keep, active_image, cap,
+                              rej_image, rej_index, n_rejected, n_elsewhere);
   free_img_scratch(e);
   return rc;
 }

@@ -4,7 +4,9 @@
 //
 //   k_rg_classify  one pass over the image columns: every player checked under the IMAGE's layout (img_player, the
 //                  checks of k_img_load), then given its partition under the ENGINE's layout, or the reject bucket
-//                  n_segs (no group, or a mode the engine does not have).  Counts per (1024-player block, bucket) for
+//                  n_segs (no group, or a mode the engine does not have); a player of a partition `keep` does not
+//                  select (mm_import_regroup_many) is skipped: counted, and left out like a player that failed a check.
+//                  Counts per (1024-player block, bucket) for
 //                  the stable counting scatter of mm_requeue.cuh (k_rq_scan, k_rq_group), and per (image partition,
 //                  new partition) pair: the sorted runs each new partition will hold.
 //   k_rg_dups      one copy per id over the players and the active section (what k_img_insert refuses), before
@@ -40,7 +42,9 @@ struct RgClassifyArgs {
   const uint8_t* grp_lut;
   const uint16_t* bin_seg;
   uint32_t n_modes, n_segs;
-  uint16_t* part;             // [n] new partition; n_segs = rejected; kNoPart = failed a check
+  const uint8_t* keep;        // [n_segs] selected new partitions; null: all
+  uint32_t* n_skip;           // players of unselected partitions (keep != null)
+  uint16_t* part;             // [n] new partition; n_segs = rejected; kNoPart = failed a check or skipped
   uint16_t* pimg;             // [n] image partition
   uint32_t* blockhist;        // [n_segs + 1][nblk]
   uint32_t* pair;             // [n_img_segs][n_segs] kept players per (image partition, new partition)
@@ -54,7 +58,7 @@ __global__ void __launch_bounds__(256) k_rg_classify(const RgClassifyArgs a) {
   for (uint32_t p = tid; p <= a.n_img_segs; p += 256) s_off[p] = a.part_off[p];
   for (uint32_t p = tid; p <= a.n_segs; p += 256) s_hist[p] = 0;
   __syncthreads();
-  uint32_t bad = 0;
+  uint32_t bad = 0, skip = 0;
 #pragma unroll 1
   for (int j = 0; j < 4; ++j) {
     const uint32_t i = blockIdx.x * kRqItems + warp * 128 + j * 32 + lane;
@@ -71,6 +75,7 @@ __global__ void __launch_bounds__(256) k_rg_classify(const RgClassifyArgs a) {
         const int32_t hi = a.bm.key_lo + (int32_t)a.bm.KR - 1;
         const int32_t r = x.rt < a.bm.key_lo ? a.bm.key_lo : (x.rt > hi ? hi : x.rt);
         q = a.grp_lut[r - a.bm.key_lo] == 0xFF ? a.n_segs : a.bin_seg[bin_of(a.bm, a.bm.lut, x.rt, x.md)];
+        if (a.keep && q < a.n_segs && !a.keep[q]) { q = kNoPart; ++skip; }
       }
       if (q != kNoPart) atomicAdd(&s_hist[q], 1u);
       if (q < a.n_segs) key = x.p * a.n_segs + q;
@@ -82,6 +87,8 @@ __global__ void __launch_bounds__(256) k_rg_classify(const RgClassifyArgs a) {
   }
   bad = __reduce_or_sync(0xFFFFFFFFu, bad);
   if (lane == 0 && bad) atomicOr(a.err, bad);
+  skip = __reduce_add_sync(0xFFFFFFFFu, skip);
+  if (lane == 0 && skip) atomicAdd(a.n_skip, skip);
   __syncthreads();
   for (uint32_t p = tid; p <= a.n_segs; p += 256) a.blockhist[(size_t)p * a.nblk + blockIdx.x] = s_hist[p];
 }
@@ -152,7 +159,8 @@ __device__ __forceinline__ uint32_t rg_part_of(const uint32_t* s_off, uint32_t n
   return lo;
 }
 
-struct RgMergeArgs {
+template <class Key>
+struct RgMergeArgsT {
   const uint32_t* rq_off;     // [n_segs + 2] (k_rq_scan over n_segs + 1 buckets)
   uint32_t n_segs, n_img_segs, round;
   const uint16_t* pimg;
@@ -161,12 +169,15 @@ struct RgMergeArgs {
   const uint32_t* kq;
   const uint32_t* kmax;
   const uint32_t* src_in;     // image index of the player at a position
-  const uint32_t* u_in;       // its age
+  const Key* u_in;            // its key: the age (mm_import_regroup), an RcKey (mm_recut.cuh)
   uint32_t* src_out;
-  uint32_t* u_out;
+  Key* u_out;
 };
+using RgMergeArgs = RgMergeArgsT<uint32_t>;
 
-__global__ void __launch_bounds__(256) k_rg_merge(const RgMergeArgs a) {
+// Key: ordered by < and ==; every run must be sorted by it.
+template <class Key>
+__global__ void __launch_bounds__(256) k_rg_merge(const RgMergeArgsT<Key> a) {
   __shared__ uint32_t s_off[kMaxSegs + 1];
   if ((1u << a.round) >= *a.kmax) return;  // (uniform) every partition is one sorted run already
   for (uint32_t p = threadIdx.x; p <= a.n_segs; p += blockDim.x) s_off[p] = a.rq_off[p];
@@ -174,7 +185,8 @@ __global__ void __launch_bounds__(256) k_rg_merge(const RgMergeArgs a) {
   const uint32_t kept = s_off[a.n_segs], t = a.round;
   for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < kept; k += gridDim.x * blockDim.x) {
     const uint32_t q = rg_part_of(s_off, a.n_segs, k);
-    const uint32_t src = a.src_in[k], u = a.u_in[k];
+    const uint32_t src = a.src_in[k];
+    const Key u = a.u_in[k];
     const uint32_t s = a.ord[(size_t)a.pimg[src] * a.n_segs + q] >> t, ps = s ^ 1u, K = a.kq[q];
     const uint32_t* rs = a.run_start + (size_t)q * (a.n_img_segs + 1);
     uint32_t dst = k;
@@ -183,7 +195,8 @@ __global__ void __launch_bounds__(256) k_rg_merge(const RgMergeArgs a) {
       uint32_t l = C, r = D;
       const bool left = !(s & 1u);  // left: the partner's players older than u; right: older or of the same age
       while (l < r) {
-        const uint32_t mid = (l + r) >> 1, v = a.u_in[mid];
+        const uint32_t mid = (l + r) >> 1;
+        const Key v = a.u_in[mid];
         if (v < u || (!left && v == u)) l = mid + 1; else r = mid;
       }
       dst = left ? k + (l - C) : k - A + l;

@@ -514,6 +514,36 @@ class Engine:
         self._check(self.lib.mm_import_regroup(self.h, _p(buf), len(buf), n, _p(rej), C.byref(k)), "mm_import_regroup")
         return rej[:k.value]
 
+    def import_regroup_many(self, images, keep=None, active_image=None):
+        """Load several export_state() images written under ONE config (the old ranks of a sharded deployment) into
+        this fresh engine, re-filed under its config (mm_import_regroup_many).  keep: bool per (mode, group) queue of
+        this config ([n_modes, n_groups] or flat in mm_queue_stats order; None = all): players of an unselected queue
+        are skipped.  active_image: the image whose active section this engine takes (None = none).  Inside a queue the
+        images interleave by running-max stamp (ties to the lower image); with more than one image the kept players
+        are renumbered 0 .. n_kept-1 (include/mm_engine.h).  -> (rejected, n_elsewhere): rejected = int64 [n, 2]
+        (image, index) pairs, ascending, of the players this config has no queue for; n_elsewhere = players skipped."""
+        bufs = [np.ascontiguousarray(np.frombuffer(b, np.uint8) if isinstance(b, (bytes, bytearray, memoryview))
+                                     else b, np.uint8) for b in images]
+        K = len(bufs)
+        ptrs = (C.c_void_p * max(K, 1))(*[b.ctypes.data for b in bufs])
+        lens = (C.c_uint64 * max(K, 1))(*[len(b) for b in bufs])
+        hs = C.sizeof(abi.ImageHeader)
+        n = sum(min(abi.ImageHeader.from_buffer_copy(b[:hs].tobytes()).n_players, len(b)) if len(b) >= hs else 0
+                for b in bufs)  # a player takes more than a byte: a corrupt count must not size the reject list
+        n = min(n, 0xFFFFFFFF)
+        sel = None
+        if keep is not None:
+            sel = np.ascontiguousarray(np.asarray(keep, bool).reshape(-1), np.uint8)
+            if len(sel) != self.cfg.n_modes * self.cfg.n_groups:
+                raise ValueError("keep needs n_modes * n_groups entries")
+        rimg, ridx = np.empty(max(n, 1), np.uint32), np.empty(max(n, 1), np.uint32)
+        k, e = C.c_uint32(0), C.c_uint32(0)
+        self._check(self.lib.mm_import_regroup_many(self.h, K, ptrs, lens, _p(sel),
+                                                    0xFFFFFFFF if active_image is None else int(active_image), n,
+                                                    _p(rimg), _p(ridx), C.byref(k), C.byref(e)),
+                    "mm_import_regroup_many")
+        return np.stack([rimg[:k.value], ridx[:k.value]], 1).astype(np.int64), int(e.value)
+
     def export_queues(self, mask):
         """Release whole (mode, group) queues into a queue image (mm_export_queues) -> uint8 array.  mask: bool per
         queue in queue_stats() record order (mode * n_groups + group), or [n_modes][n_groups].  The exported players

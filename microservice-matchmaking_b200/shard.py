@@ -414,6 +414,109 @@ def move_queues(pkg, cfg, old, new, rank, engine, comm):
 
 
 # ======================================================================================================================
+# Re-cut: a new rating-group table and owner array for every rank at once (mm_import_regroup_many).  Every old rank
+# exports its engine; each new rank loads the images of the old ranks whose players can map to a queue it owns under
+# the new table, keeps those queues, and takes its own active section.  The world size does not change.
+# ======================================================================================================================
+def recut_sends(old_cfg, new_cfg, old_owners, new_owners, world):
+    """-> bool [world, world]: send[s, d] = an image of old rank s can hold a player that new rank d keeps (s != d).
+    Every rating behaves like one of the clamped domain [min(rmin) - 1, max(rmax) + 1] of the two configs."""
+    lo = min(min(c.group_lo[g] for g in range(c.n_groups)) for c in (old_cfg, new_cfg)) - 1
+    hi = max(max(c.group_hi[g] for g in range(c.n_groups)) for c in (old_cfg, new_cfg)) + 1
+    r = np.arange(lo, hi + 1, dtype=np.int64)
+    go, gn = group_of_rating(old_cfg, r), group_of_rating(new_cfg, r)
+    ok = (go >= 0) & (gn >= 0)
+    send = np.zeros((world, world), bool)  # a mode both configs have maps a rating to the same groups in every mode
+    send[np.asarray(old_owners, np.int64)[go[ok]], np.asarray(new_owners, np.int64)[gn[ok]]] = True
+    np.fill_diagonal(send, False)
+    return send
+
+
+def _exchange(rank, world, comm, out, want):
+    """Point-to-point with every other rank in ascending pair order (every rank's pairs come in one global order, so
+    blocking calls cannot deadlock): out(d) -> the arrays for d or None; want(s) -> whether s sends to me.
+    -> {s: arrays received}"""
+    got = {}
+    for other in range(world):
+        if other == rank:
+            continue
+        for step in ((0, 1) if rank < other else (1, 0)):
+            if step == 0:
+                arrays = out(other)
+                if arrays is not None:
+                    comm.send(rank, other, arrays)
+            elif want(other):
+                got[other] = comm.recv(other, rank)
+    return got
+
+
+def recut(pkg, old_cfg, new_cfg, old_owners, new_owners, rank, engine, comm, make_engine=None):
+    """Re-cut a deployment sharded by rating group to a new group table and owner array; every rank of the job calls
+    this with the same arguments.  world = 1 + the largest rank in either owner array, and every rank below it calls.
+      1. every rank exports its engine (export_state: the old engine is never changed);
+      2. every rank computes the same send matrix (recut_sends) and old rank s sends its image, as one int64 array,
+         to every rank d with send[s, d] (or [-1] if its export failed); a rank always keeps its own image;
+      3. every rank creates an engine under new_cfg (make_engine, default pkg.Engine) and calls import_regroup_many
+         with the images in old-rank order, keep = the queues of the groups new_owners gives it, active_image = its
+         own image;
+      4. every rank sends its status ([0] ok, [1] failed) to every other rank.  Only if all succeeded does each rank
+         keep its new engine and close the old one; otherwise every rank closes its new engine and keeps the old one,
+         untouched: a failure anywhere loses no player.
+    Preconditions: no ingest or tick on any rank during the call, and routing switches to route(new_cfg, ...,
+    owners=new_owners) after it.  While it runs, each rank holds its old engine, its new one and the images it loads.
+    With more than one old image a rank's players are renumbered (include/mm_engine.h): requeue records of players
+    matched before the re-cut do not carry over.
+    -> dict(ok, engine: the engine this rank uses from now on, dropped: ids of this rank's own players that have no
+    queue under new_cfg (they left: answer them), elsewhere: players skipped here because another rank owns them,
+    bytes_sent: bytes this rank sent)."""
+    make_engine = make_engine or pkg.Engine
+    old_owners, new_owners = np.asarray(old_owners, np.int64), np.asarray(new_owners, np.int64)
+    world = int(max(old_owners.max(initial=0), new_owners.max(initial=0))) + 1
+    send = recut_sends(old_cfg, new_cfg, old_owners, new_owners, world)
+    sent = [0]
+
+    def counted(arrays):
+        sent[0] += sum(np.asarray(a).nbytes for a in arrays)
+        return arrays
+
+    try:
+        img = np.ascontiguousarray(engine.export_state(), np.uint8)
+    except Exception:
+        img = None
+    mine = img.view(np.int64) if img is not None else np.array([-1], np.int64)
+    got = _exchange(rank, world, comm, lambda d: counted((mine,)) if send[rank, d] else None,
+                    lambda s: bool(send[s, rank]))
+    images, own = [], None
+    for s in range(world):
+        if s == rank:
+            own = len(images)
+            images.append(img)
+        elif send[s, rank]:
+            arr = np.ascontiguousarray(got[s][0])
+            images.append(arr.view(np.uint8) if len(arr) > 1 else None)
+    new, dropped, elsewhere = None, np.zeros(0, np.uint64), 0
+    ok = all(x is not None for x in images)
+    if ok:
+        try:
+            new = make_engine(new_cfg)
+            keep = np.broadcast_to(new_owners == rank, (new_cfg.n_modes, new_cfg.n_groups))
+            rejected, elsewhere = new.import_regroup_many(images, keep=keep, active_image=own)
+            ids = pkg.engine.read_image(images[own])[1]["id"]
+            dropped = np.asarray(ids[rejected[rejected[:, 0] == own, 1]], np.uint64)
+        except Exception:
+            ok = False
+    status = np.array([0 if ok else 1], np.int64)
+    got = _exchange(rank, world, comm, lambda d: counted((status,)), lambda s: True)
+    ok = ok and all(_status(got[s][0]) == 0 for s in got)
+    if ok:
+        engine.close()
+        return dict(ok=True, engine=new, dropped=dropped, elsewhere=int(elsewhere), bytes_sent=sent[0])
+    if new is not None:
+        new.close()
+    return dict(ok=False, engine=engine, dropped=np.zeros(0, np.uint64), elsewhere=0, bytes_sent=sent[0])
+
+
+# ======================================================================================================================
 # One lobby budget per game mode over several engines (mm_set_lobby_budget, include/mm_engine.h).  A mode's budget is
 # apportioned over ALL its rating groups by their candidate lobbies; sharded by group, no engine sees all of them.  Every
 # engine reports its own (Engine.lobby_candidates, a dry run that changes nothing), the counts are gathered, every rank
