@@ -267,6 +267,47 @@ int mm_band_match(mm_engine* e, int32_t W, uint32_t g_first, uint32_t g_last, ui
                   mm_lobby_hdr* lobbies, uint32_t lobby_cap, uint64_t* member_ids, uint64_t member_cap,
                   uint8_t* upper_taken, mm_band_stats* stats);
 
+/* EXTENSION (backfill, DESIGN.md §4): a running lobby that lost members (a player left during the loading screen, a
+ * member declined and the rest should stay together) asks for k players from its queue instead of being disbanded —
+ * the reference saves a partial lobby in its shrunken state and fills it with the next players of its queue
+ * (search/worker.ex:312-321, models/lobby_state.ex).                                                              */
+typedef struct mm_backfill_req {
+  uint8_t mode, group; /* the (mode, group) queue to take from                                                  */
+  uint16_t reserved;   /* 0                                                                                     */
+  uint32_t count;      /* open slots: players wanted                                                            */
+  int32_t target;      /* rating the slots should be filled around (MM_ORDER_RATING)                            */
+  int32_t window;      /* max |rating - target| in clamped ratings; < 0 = no limit                              */
+} mm_backfill_req;     /* 16 bytes */
+
+/* mm_backfill: requests are served one at a time, in index order; request j is served against the live queued players
+ * of its queue that no earlier request of the same call took.
+ *   MM_ORDER_RATING  with c(x) = x clamped to [rmin - 1, rmax + 1] (the tick's key clamp), request j ranks the
+ *                    candidates by (|c(rating) - c(target)|, c(rating), enqueue order) — at equal distance the lower
+ *                    rating first, inside one rating the older player first — and takes the first
+ *                    min(count, #{candidates with |c(rating) - c(target)| <= window}) of them (no limit when window < 0).
+ *                    A request on the default group sees everything the tick files there, out-of-range players at their
+ *                    clamped ratings; with overlapping groups a group's ratings need not be contiguous: distances are in
+ *                    ratings, not in key indices.
+ *   MM_ORDER_ARRIVAL request j takes the count oldest players of its queue; target is ignored, window must be < 0.
+ * A request may be filled only in part: n_taken[j] says how many players it got (a caller that wants all or nothing
+ * hands a short fill back to mm_requeue).  member_ids holds request 0's players, then request 1's, ..., each in the
+ * rank order above (handles on MM_F_DENSE_IDS engines); *n_total = the sum of n_taken.  Taken players leave the pool
+ * exactly as mm_take takes them and stay in the active set as matched players until mm_remove, so mm_requeue puts them
+ * back (code 1).  The last tick's match section of mm_queue_stats, the lobby budget, pending async_results copies, the
+ * snapshot and the mm_enqueue_rejects list are left alone.  n = 0 does nothing.
+ * Refusals, all decided before anything changes (mm_last_error names the cause and the request index):
+ *   MM_E_ARG   a mode >= n_modes, a group >= n_groups, reserved != 0, window >= 0 on an MM_ORDER_ARRIVAL engine;
+ *   MM_E_STATE a staged packed batch, an MM_F_NO_DEDUPE engine (no active set holds matched players);
+ *   MM_E_CAP   member_cap < *n_total.  n_taken and *n_total are still written: member_cap = 0 is a dry run.
+ * Cost: the plan runs on the per-bin totals; the gather reads the key column of the partitions holding a taken player,
+ * and places up to the tile of each partition's last taken player.  Only the requests, n_taken and member_ids cross
+ * PCIe.
+ *
+ * EQUIVALENCE.  The call leaves the engine in the state mm_take of the returned ids would leave it in: every later
+ * call sequence gives the same results on both engines.                                                           */
+int mm_backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_taken, uint64_t* member_ids,
+                uint64_t member_cap, uint32_t* n_total);
+
 /* Replaces ActiveUser.in_queue?/1 (models/active_user.ex:33-44), batched.          */
 int mm_in_queue(mm_engine* e, uint32_t n, const uint64_t* id, uint8_t* out);
 

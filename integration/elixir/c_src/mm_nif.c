@@ -404,6 +404,36 @@ static ERL_NIF_TERM nif_requeue(ErlNifEnv* env, int argc, const ERL_NIF_TERM arg
   return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &codes));
 }
 
+/* backfill(ref, requests :: binary(mm_backfill_req[]: mode u8, group u8, 0 :: u16, count u32, target i32, window i32))
+ * -> {:ok, n_taken :: binary(u32[]), handles :: binary(u32[])}: the open slots of running lobbies filled from their
+ * queues, nearest rating first (mm_backfill); handles holds request 0's players, then request 1's, ...  The member
+ * buffer is sized from the dry run's total (member_cap = 0). */
+static ERL_NIF_TERM nif_backfill(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary rq, taken, hs; uint32_t total = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &rq))
+    return enif_make_badarg(env);
+  if (rq.size % sizeof(mm_backfill_req)) return enif_make_badarg(env);
+  const uint32_t n = (uint32_t)(rq.size / sizeof(mm_backfill_req));
+  mm_backfill_req* req = enif_alloc(rq.size + 1);
+  if (!req || !enif_alloc_binary(4 * (size_t)n, &taken)) { enif_free(req); return err(env, MM_E_CAP); }
+  memcpy(req, rq.data, rq.size);
+  int rc = mm_backfill(r->e, n, req, (uint32_t*)taken.data, NULL, 0, &total);  /* the dry run: counts only */
+  if (rc == MM_E_CAP || rc == MM_OK) {
+    uint64_t* id = enif_alloc(8 * (size_t)total + 8);
+    if (!id || !enif_alloc_binary(4 * (size_t)total, &hs)) rc = MM_E_CAP;
+    else {
+      rc = mm_backfill(r->e, n, req, (uint32_t*)taken.data, id, total, &total);
+      if (rc) enif_release_binary(&hs);
+      else for (uint32_t k = 0; k < total; ++k) { const uint32_t h = (uint32_t)id[k]; memcpy(hs.data + 4 * (size_t)k, &h, 4); }
+    }
+    enif_free(id);
+  }
+  enif_free(req);
+  if (rc) { enif_release_binary(&taken); return err(env, rc); }
+  return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &taken), enif_make_binary(env, &hs));
+}
+
 /* set_lobby_budget(ref, per_queue :: binary(u32[n_modes * n_groups]) | <<>>, per_mode :: binary(u32[n_modes]) | <<>>)
  * -> :ok: lobbies every queue / every mode may emit per tick from the next tick on (mm_set_lobby_budget); an empty
  * binary = no limit, 0xFFFFFFFF in an entry = no limit for it.  The engine reads n_modes * n_groups / n_modes entries:
@@ -482,6 +512,7 @@ static ErlNifFunc funcs[] = {
   {"import_regroup", 2, nif_import_regroup, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"import_regroup_many", 4, nif_import_regroup_many, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"backfill", 2, nif_backfill, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"seq_next", 1, nif_seq_next, 0},
   {"set_max_spread", 2, nif_set_max_spread, 0},
   {"set_lobby_budget", 3, nif_set_lobby_budget, 0},

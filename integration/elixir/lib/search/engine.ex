@@ -111,6 +111,13 @@ defmodule Matchmaking.Search.Engine do
   columns each player had when it was queued -> {:ok, codes :: binary(u8[])}: 1 requeued, 0 still queued, 4 gone.
   """
   def requeue(_ref, _handles, _ratings, _modes, _enq_ts, _seq), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Backfill (extension): the open slots of running lobbies filled from their queues, nearest rating first (mm_backfill).
+  requests: binary of 16-byte records <<mode, group, 0::16, count::little-32, target::little-signed-32,
+  window::little-signed-32>> (window < 0: no limit) -> {:ok, n_taken :: binary(u32[]), handles :: binary(u32[])}:
+  request 0's players, then request 1's, ...; they leave the pool and stay in the active set until remove_user.
+  """
+  def backfill(_ref, _requests), do: :erlang.nif_error(:nif_not_loaded)
   @doc "The enqueue sequence number the next offered player will get (mm_seq_next) -> {:ok, seq}."
   def seq_next(_ref), do: :erlang.nif_error(:nif_not_loaded)
   def n_modes, do: length(@modes)

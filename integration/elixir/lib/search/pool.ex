@@ -82,6 +82,13 @@ defmodule Matchmaking.Search.Pool do
   queued) or :gone (removed, timed out, never queued, or its queue has moved to another pool: answer it as today).
   """
   def requeue(players), do: GenServer.call(__MODULE__, {:requeue, players}, :infinity)
+  @doc """
+  Backfill (extension): a running lobby that lost members asks for players instead of being disbanded.  requests:
+  [{mode_name, group_index, target_rating, count}] or [{..., count, window}], served in order (Engine.backfill) -> one
+  list of player documents per request (shorter than count when the queue runs short).  Backfilled players leave the
+  pool as matched players do: requeue/1 puts them back, remove_user forgets them.
+  """
+  def backfill(requests), do: GenServer.call(__MODULE__, {:backfill, requests}, :infinity)
   @doc "The queues of these rating groups (indices, all modes) emit no lobby until resume_queues/1; players stay queued."
   def pause(groups), do: GenServer.call(__MODULE__, {:pause, groups, true})
   def resume_queues(groups), do: GenServer.call(__MODULE__, {:pause, groups, false})
@@ -307,6 +314,27 @@ defmodule Matchmaking.Search.Pool do
         back = for {{i, h, _}, 1} <- Enum.zip(rows, :binary.bin_to_list(codes)), into: st.players,
                  do: {h, elem(docs, i)}
         {:reply, outcome, %{st | players: back}}
+      {:error, _} = e -> {:reply, e, st}
+    end
+  end
+
+  def handle_call({:backfill, requests}, _from, st) do
+    st = flush(st)
+    req = for r <- requests, into: <<>> do
+      {mode, group, target, count, window} =
+        case r do
+          {m, g, t, c} -> {m, g, t, c, -1}
+          {m, g, t, c, w} -> {m, g, t, c, w}
+        end
+      <<(Engine.mode_index(mode) || 255), group, 0::16, count::little-32, target::little-signed-32,
+        window::little-signed-32>>
+    end
+    case Engine.backfill(st.ref, req) do
+      {:ok, n_taken, handles} ->
+        hs = for <<h::little-32 <- handles>>, do: h
+        {out, _} = Enum.map_reduce(for(<<k::little-32 <- n_taken>>, do: k), hs, &Enum.split(&2, &1))
+        docs = Enum.map(out, fn part -> Enum.map(part, &Map.fetch!(st.players, &1)) end)
+        {:reply, {:ok, docs}, %{st | players: Map.drop(st.players, hs)}}
       {:error, _} = e -> {:reply, e, st}
     end
   end

@@ -89,6 +89,18 @@ class BandStats(C.Structure):
 MM_WAIT_BUCKETS = 120
 
 
+class BackfillReq(C.Structure):
+    """mm_backfill_req: one backfill request (16 bytes)."""
+    _fields_ = [
+        ("mode", C.c_uint8),
+        ("group", C.c_uint8),
+        ("reserved", C.c_uint16),
+        ("count", C.c_uint32),
+        ("target", C.c_int32),
+        ("window", C.c_int32),
+    ]
+
+
 class QueueStat(C.Structure):
     """One (mode, group) queue: the resident pool at `now` and the players the last tick matched (988 bytes)."""
     _fields_ = [
@@ -161,6 +173,7 @@ PROTOTYPES = {
     "mm_band_candidates": (C.c_int, [_vp, C.c_int32, C.c_uint32, _vp, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_band_match": (C.c_int, [_vp, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, _vp, _vp, _vp, C.c_uint32,
                                 _vp, C.c_uint32, _vp, C.c_uint64, _vp, _P(BandStats)]),
+    "mm_backfill": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, C.c_uint64, _P(C.c_uint32)]),
     "mm_in_queue": (C.c_int, [_vp, C.c_uint32, _vp, _vp]),
     "mm_pool_size": (C.c_int, [_vp, _P(C.c_uint32)]),
     "mm_active_size": (C.c_int, [_vp, _P(C.c_uint32)]),

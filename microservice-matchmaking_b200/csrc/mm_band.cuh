@@ -8,7 +8,8 @@
 //
 // Gather (k_band_prep, k_band_count, k_band_scan): every band key that lies in this pool has one sort-key bin (bin =
 // mode * stride + lut[rating]); k_band_prep maps bin -> q, selects the partitions that hold such bins and gives every
-// key a column of per-tile counts over its partition's tiles.  The other partitions get a fill of 0 in the geometry
+// key a column of per-tile counts over its partition's tiles.  The key numbering is the caller's (BandKeyBins here,
+// the backfill's own in mm_backfill.cuh); the rest of the gather and the place pass are shared.  The other partitions get a fill of 0 in the geometry
 // the gather kernels build, so their tiles are never read.  k_band_count counts every tile's band players per key
 // from the 2-byte bin column (dead slots sit in the removed bin, which maps to no key); k_band_scan turns each column
 // into exclusive prefixes and the key's total.
@@ -19,7 +20,8 @@
 //
 // Place (k_band_place): each band player lands at its key's base + its stable rank among the key's players (earlier
 // tiles from the prefixes, earlier slots of its own tile by a warp-ordered pass), if that rank is below the key's
-// limit; a match call takes the local players it places (pool_take_slot, as mm_take).  The caller's upper-side
+// limit; a match call takes the local players it places (pool_take_slot, as mm_take).  k_band_limit first cuts every
+// selected partition after the tile of the last player any of its keys outputs, so the place pass reads no tile past it.  The caller's upper-side
 // candidates (another rank's band) are checked, counted and placed by k_band_upper / k_band_upper_place.
 #pragma once
 
@@ -58,6 +60,7 @@ struct BandArgs {
   uint32_t* bfill;                // [n_segs] fills of the selected partitions, 0 for the others
   uint32_t* qoff;                 // [n_keys + 1] first count of the key's column
   uint32_t* qtiles;               // [n_keys] tiles of the key's partition
+  uint32_t* qseg;                 // [n_keys] the key's partition (written for local keys)
   uint32_t* M;                    // per-(key, tile) counts -> exclusive prefixes -> running ranks (k_band_place)
   uint32_t* tot;                  // [n_keys] band players per key (local + caller's)
   uint32_t* pos;                  // [n_bands * (2W + 1)] walk: sorted position of every key's first player in its band
@@ -76,8 +79,17 @@ __device__ __forceinline__ uint32_t band_bin(const BandArgs& a, uint32_t q, bool
   return m * a.bm.stride + a.bm.lut[r - a.bm.key_lo];
 }
 
-// One CTA: bin -> key map (a.map preset to kBandNone), partition selection, the keys' count columns.
-__global__ void __launch_bounds__(kBandPrepBlock) k_band_prep(const BandArgs a) {
+// The band numbering: key q -> its bin, local = the key's players are gathered from this pool.
+struct BandKeyBins {
+  __device__ __forceinline__ uint32_t operator()(const BandArgs& a, uint32_t q, bool& local) const {
+    return band_bin(a, q, local);
+  }
+};
+
+// One CTA: bin -> key map (a.map preset to kBandNone), partition selection, the keys' count columns.  KeyBins numbers
+// the keys: kb(a, q, local) -> the bin of key q.
+template <class KeyBins>
+__global__ void __launch_bounds__(kBandPrepBlock) k_band_prep(const BandArgs a, const KeyBins kb) {
   __shared__ uint32_t s_sel[kMaxSegs];
   __shared__ uint32_t s_tmp[33];
   __shared__ uint32_t s_carry;
@@ -90,10 +102,11 @@ __global__ void __launch_bounds__(kBandPrepBlock) k_band_prep(const BandArgs a) 
     uint32_t tiles = 0;
     if (q < a.n_keys) {
       bool local;
-      const uint32_t bin = band_bin(a, q, local);
+      const uint32_t bin = kb(a, q, local);
       if (local) {
         const uint32_t p = a.bin_seg[bin];
         a.map[bin] = q;
+        a.qseg[q] = p;
         s_sel[p] = 1;
         tiles = (__ldcg(&a.fill[p]) + kTile - 1) / kTile;
       }
@@ -184,6 +197,27 @@ __global__ void __launch_bounds__(256) k_band_scan(const BandArgs a) {
     carry += __shfl_sync(0xFFFFFFFFu, incl, 31);
   }
   if (lane == 0) a.tot[q] = carry;
+}
+
+// One CTA, once klim is known: the last tile of its partition that holds one of key q's first min(klim, tot) players
+// (the last tile whose exclusive prefix is below that count), and every selected partition's fill cut after the last
+// such tile of its keys (0: none of its players is output).  The place pass then skips the tiles past it without
+// loading their key columns; the running ranks of the tiles it does place are unchanged.
+__global__ void __launch_bounds__(kBandPrepBlock) k_band_limit(const BandArgs a) {
+  __shared__ uint32_t s_lim[kMaxSegs];
+  const uint32_t tid = threadIdx.x;
+  for (uint32_t p = tid; p < a.n_segs; p += kBandPrepBlock) s_lim[p] = 0;
+  __syncthreads();
+  for (uint32_t q = tid; q < a.n_keys; q += kBandPrepBlock) {
+    const uint32_t n = a.qtiles[q], lim = min(a.klim[q], a.tot[q]);
+    if (n == 0 || lim == 0) continue;
+    const uint32_t* col = a.M + a.qoff[q];
+    uint32_t lo = 0, hi = n;  // col[lo] < lim <= col[hi] (col[n] read as the total)
+    while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (col[mid] < lim) lo = mid; else hi = mid; }
+    atomicMax(&s_lim[a.qseg[q]], lo + 1);
+  }
+  __syncthreads();
+  for (uint32_t p = tid; p < a.n_segs; p += kBandPrepBlock) a.bfill[p] = min(a.bfill[p], s_lim[p] * kTile);
 }
 
 // The caller's upper-side candidates of the last boundary: checked (mode, rating range, (mode, rating) order), then

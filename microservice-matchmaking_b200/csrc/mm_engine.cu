@@ -19,6 +19,7 @@
 #include <utility>
 #include <vector>
 
+#include "mm_backfill.cuh"
 #include "mm_band.cuh"
 #include "mm_expire.cuh"
 #include "mm_image.cuh"
@@ -262,7 +263,7 @@ struct mm_engine {
 
   // mm_band_candidates / mm_band_match (mm_band.cuh): sized by the band keys and the candidates, grown on demand
   struct Band {
-    DevArray<uint32_t> map, fill, qoff, qtiles, M, tot, pos, kbase, klim, band_mb, band_lb, rstart, ctr;
+    DevArray<uint32_t> map, fill, qoff, qtiles, qseg, M, tot, pos, kbase, klim, band_mb, band_lb, rstart, ctr;
     DevArray<uint64_t> id;        // candidate ids / members
     DevArray<int32_t> rating;     // candidate ratings
     DevArray<uint8_t> mode;       // candidate modes
@@ -271,6 +272,15 @@ struct mm_engine {
     DevArray<uint8_t> up_mode, up_taken;
     DevArray<mm_lobby_hdr> hdr;
   } band;
+
+  // mm_backfill (mm_backfill.cuh): sized by the requests, the pieces, the bins and the players taken, grown on demand;
+  // the gather runs on the band arrays above
+  struct Backfill {
+    DevArray<uint32_t> in;  // requests in queue order (BfReq) | first request of every queue | the queues with requests
+    DevArray<uint32_t> rem, key_bin, kbase, klim, n_taken, req_base, ctr;
+    DevArray<BfPiece> piece;
+    DevArray<uint64_t> staging, members;
+  } bf;
 };
 
 namespace {
@@ -1918,40 +1928,58 @@ uint32_t band_ctas(const mm_engine* e, uint32_t n) {
   return std::max<uint32_t>(1, std::min<uint32_t>((tile_count(e, n) + kBandWarps - 1) / kBandWarps, 4u * (uint32_t)e->n_sms));
 }
 
+// The pool and table fields of the gather's arguments (every caller's)
+BandArgs band_args(mm_engine* e) {
+  const Pool& p = e->pool[e->cur];
+  BandArgs a{};
+  a.pool = p.v; a.meta = p.m; a.fill = p.m.fill;
+  a.n_segs = e->n_segs; a.K = e->K; a.bm = bin_map(e); a.bin_seg = e->d_bin_seg; a.seg_bin_lo = e->d_seg_bin_lo;
+  return a;
+}
+
+// The gather every caller shares, once a.n_keys is set: scratch of the per-key arrays and of `cols` per-(key, tile)
+// counts, then the bin -> key map and count columns (k_band_prep with the caller's numbering kb), the per-(key, tile)
+// counts, per-key prefixes and totals.
+template <class KeyBins>
+int band_gather(mm_engine* e, BandArgs& a, size_t cols, const KeyBins& kb) {
+  auto& s = e->band;
+  const size_t nk = std::max<size_t>(a.n_keys, 1);
+  cols = std::max<size_t>(cols, 1);
+  CK(s.map.reserve(e->Kp)); CK(s.fill.reserve(e->n_segs)); CK(s.qoff.reserve(nk + 1)); CK(s.qtiles.reserve(nk));
+  CK(s.qseg.reserve(nk)); CK(s.M.reserve(cols)); CK(s.tot.reserve(nk)); CK(s.ctr.reserve(kBcWords));
+  a.meta.fill = s.fill; a.map = s.map; a.bfill = s.fill; a.qoff = s.qoff; a.qtiles = s.qtiles; a.qseg = s.qseg;
+  a.M = s.M; a.tot = s.tot; a.ctr = s.ctr;
+  CK(cudaMemsetAsync(s.ctr, 0, kBcWords * 4, e->stream));
+  CK(cudaMemsetAsync(s.tot, 0, nk * 4, e->stream));
+  if (!a.n_keys) return MM_OK;
+  CK(cudaMemsetAsync(s.map, 0xFF, (size_t)e->Kp * 4, e->stream));
+  CK(cudaMemsetAsync(s.M, 0, cols * 4, e->stream));
+  k_band_prep<<<1, kBandPrepBlock, 0, e->stream>>>(a, kb);
+  k_band_count<kBandBlock><<<band_ctas(e, e->pool[e->cur].n), kBandBlock, 0, e->stream>>>(a);
+  k_band_scan<<<(a.n_keys + 7) / 8, 256, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  return MM_OK;
+}
+
 // Arguments and scratch of one call: n_bounds boundaries from g_first | g_first+1, every mode.  Every scratch array is
 // sized by the band keys, the candidates or the per-key tile counts; none by the pool's capacity.
 int band_setup(mm_engine* e, int32_t W, uint32_t g_first, uint32_t n_bounds, bool skip_lower, bool remote_last,
                BandArgs& a) {
   const mm_config& c = e->cfg;
-  const Pool& p = e->pool[e->cur];
   auto& s = e->band;
-  a = BandArgs{};
-  a.pool = p.v; a.meta = p.m; a.fill = p.m.fill;
-  a.n_segs = e->n_segs; a.K = e->K; a.bm = bin_map(e); a.bin_seg = e->d_bin_seg; a.seg_bin_lo = e->d_seg_bin_lo;
+  a = band_args(e);
   a.W = W; a.n_modes = c.n_modes; a.g_first = g_first; a.n_bands = n_bounds * c.n_modes;
   a.n_keys = a.n_bands * 2u * (uint32_t)W;
   a.skip_lower = skip_lower; a.remote_last = remote_last;
   for (uint32_t g = 0; g < c.n_groups; ++g) a.hi[g] = c.group_hi[g];
   for (uint32_t m = 0; m < c.n_modes; ++m) a.L[m] = (uint32_t)c.modes[m].teams * c.modes[m].team_size;
   const size_t nk = std::max<size_t>(a.n_keys, 1);
-  const size_t cols = (size_t)tile_count(e, p.n) * std::min<uint32_t>(e->max_nb, 2u * (uint32_t)W);
-  CK(s.map.reserve(e->Kp)); CK(s.fill.reserve(e->n_segs)); CK(s.qoff.reserve(nk + 1)); CK(s.qtiles.reserve(nk));
-  CK(s.M.reserve(std::max<size_t>(cols, 1))); CK(s.tot.reserve(nk)); CK(s.kbase.reserve(nk)); CK(s.klim.reserve(nk));
+  CK(s.kbase.reserve(nk)); CK(s.klim.reserve(nk));
   CK(s.rstart.reserve(nk)); CK(s.pos.reserve((size_t)a.n_bands * (2u * (uint32_t)W + 1)));
-  CK(s.band_mb.reserve(a.n_bands + 1)); CK(s.band_lb.reserve(a.n_bands + 1)); CK(s.ctr.reserve(kBcWords));
-  a.meta.fill = s.fill; a.map = s.map; a.bfill = s.fill; a.qoff = s.qoff; a.qtiles = s.qtiles; a.M = s.M; a.tot = s.tot;
-  a.pos = s.pos; a.kbase = s.kbase; a.klim = s.klim; a.band_mb = s.band_mb; a.band_lb = s.band_lb; a.ctr = s.ctr;
-  CK(cudaMemsetAsync(s.ctr, 0, kBcWords * 4, e->stream));
-  CK(cudaMemsetAsync(s.tot, 0, nk * 4, e->stream));
-  if (!a.n_keys) return MM_OK;
-  // gather: bin -> key map and count columns, per-(key, tile) counts, per-key prefixes and totals
-  CK(cudaMemsetAsync(s.map, 0xFF, (size_t)e->Kp * 4, e->stream));
-  CK(cudaMemsetAsync(s.M, 0, std::max<size_t>(cols, 1) * 4, e->stream));
-  k_band_prep<<<1, kBandPrepBlock, 0, e->stream>>>(a);
-  k_band_count<kBandBlock><<<band_ctas(e, p.n), kBandBlock, 0, e->stream>>>(a);
-  k_band_scan<<<(a.n_keys + 7) / 8, 256, 0, e->stream>>>(a);
-  CK(cudaGetLastError());
-  return MM_OK;
+  CK(s.band_mb.reserve(a.n_bands + 1)); CK(s.band_lb.reserve(a.n_bands + 1));
+  a.pos = s.pos; a.kbase = s.kbase; a.klim = s.klim; a.band_mb = s.band_mb; a.band_lb = s.band_lb;
+  const size_t cols = (size_t)tile_count(e, e->pool[e->cur].n) * std::min<uint32_t>(e->max_nb, 2u * (uint32_t)W);
+  return band_gather(e, a, cols, BandKeyBins{});
 }
 
 int band_read_ctr(mm_engine* e, uint32_t (&h)[kBcWords]) {
@@ -1979,6 +2007,7 @@ int band_candidates(mm_engine* e, int32_t W, uint32_t group, uint64_t* ids, int3
   if (n == 0) return MM_OK;
   auto& s = e->band;
   CK(s.id.reserve(n)); CK(s.rating.reserve(n)); CK(s.mode.reserve(n));
+  k_band_limit<<<1, kBandPrepBlock, 0, e->stream>>>(a);
   k_band_place<kBandBlock><<<band_ctas(e, e->pool[e->cur].n), kBandBlock, 0, e->stream>>>(
       a, BandOut{s.id, s.rating, s.mode, 0u});
   CK(cudaGetLastError());
@@ -2029,7 +2058,10 @@ int band_match(mm_engine* e, int32_t W, uint32_t g_first, uint32_t g_last, uint3
   const uint32_t ctas = band_ctas(e, e->pool[e->cur].n);
   if (nm) {
     CK(s.id.reserve(nm));
-    if (nm > nu) k_band_place<kBandBlock><<<ctas, kBandBlock, 0, e->stream>>>(a, BandOut{s.id, nullptr, nullptr, 1u});
+    if (nm > nu) {
+      k_band_limit<<<1, kBandPrepBlock, 0, e->stream>>>(a);
+      k_band_place<kBandBlock><<<ctas, kBandBlock, 0, e->stream>>>(a, BandOut{s.id, nullptr, nullptr, 1u});
+    }
   }
   if (n_upper)
     k_band_upper_place<<<(n_upper + 255) / 256, 256, 0, e->stream>>>(a, n_upper, s.up_id, s.up_rating, s.up_mode,
@@ -2048,6 +2080,88 @@ int band_match(mm_engine* e, int32_t W, uint32_t g_first, uint32_t g_last, uint3
   float ms = 0.f;
   CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]));
   st->device_us = ms * 1000.f;
+  return MM_OK;
+}
+
+// ---- mm_backfill (mm_backfill.cuh) ---------------------------------------------------------------------------------
+int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_taken, uint64_t* member_ids,
+             uint64_t member_cap, uint32_t* n_total) {
+  const mm_config& c = e->cfg;
+  const bool rating = c.order_mode == MM_ORDER_RATING;
+  for (uint32_t j = 0; j < n; ++j) {
+    const mm_backfill_req& r = req[j];
+    if (r.mode >= c.n_modes) return set_err(e, MM_E_ARG, "request %u: mode %u >= n_modes = %u", j, r.mode, c.n_modes);
+    if (r.group >= c.n_groups)
+      return set_err(e, MM_E_ARG, "request %u: group %u >= n_groups = %u", j, r.group, c.n_groups);
+    if (r.reserved) return set_err(e, MM_E_ARG, "request %u: reserved must be 0", j);
+    if (!rating && r.window >= 0)
+      return set_err(e, MM_E_ARG, "request %u: a window on an MM_ORDER_ARRIVAL engine (pass window < 0)", j);
+  }
+  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (!e->use_active) return set_err(e, MM_E_STATE, "an MM_F_NO_DEDUPE engine cannot hold taken players");
+  if (n == 0) return MM_OK;
+  // the requests grouped by queue, stably (a counting sort), with the targets as clamp keys
+  const uint32_t G = c.n_groups, nc = e->n_cut;
+  std::vector<uint32_t> qr(nc + 1, 0);
+  for (uint32_t j = 0; j < n; ++j) ++qr[req[j].mode * G + req[j].group + 1];
+  for (uint32_t q = 0; q < nc; ++q) qr[q + 1] += qr[q];
+  const size_t rw = sizeof(BfReq) / 4;
+  std::vector<uint32_t> in(rw * n + nc + 1);
+  std::copy(qr.begin(), qr.end(), in.begin() + rw * n);
+  std::vector<uint32_t> at(qr.begin(), qr.end() - 1);
+  for (uint32_t j = 0; j < n; ++j) {
+    const mm_backfill_req& r = req[j];
+    const int64_t t = std::min<int64_t>(std::max<int64_t>((int64_t)r.target - e->key_lo, 0), (int64_t)e->KR - 1);
+    const BfReq b{j, r.count, (int32_t)t, r.window};
+    std::memcpy(&in[rw * at[r.mode * G + r.group]++], &b, sizeof(b));
+  }
+  for (uint32_t q = 0; q < nc; ++q)
+    if (qr[q + 1] > qr[q]) in.push_back(q);
+  const uint32_t nq = (uint32_t)(in.size() - (rw * n + nc + 1));
+  auto& s = e->bf;
+  const Pool& p = e->pool[e->cur];
+  const size_t K = e->K;
+  CK(s.in.reserve(in.size())); CK(s.rem.reserve(K)); CK(s.key_bin.reserve(K)); CK(s.kbase.reserve(K));
+  CK(s.klim.reserve(K)); CK(s.n_taken.reserve(n)); CK(s.req_base.reserve(n)); CK(s.ctr.reserve(kBfWords));
+  CK(s.piece.reserve(n + K));  // every bin a request reaches but the last is emptied: at most n + K pieces
+  CK(cudaMemcpyAsync(s.in, in.data(), in.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(s.rem, p.m.tot, K * 4, cudaMemcpyDeviceToDevice, e->stream));
+  CK(cudaMemsetAsync(s.ctr, 0, kBfWords * 4, e->stream));
+  BfArgs f{};
+  f.tot = p.m.tot; f.rem = s.rem; f.bin_key = e->d_bin_key; f.seg_bin_lo = e->d_seg_bin_lo; f.cut_lp_lo = e->d_cut_lp_lo;
+  f.bin_seg = e->d_bin_seg; f.fill = p.m.fill; f.rating_order = rating; f.K = e->K;
+  f.req = reinterpret_cast<const BfReq*>(s.in.p); f.qr = s.in + rw * n; f.queues = s.in + rw * n + nc + 1; f.nq = nq;
+  f.n_taken = s.n_taken; f.piece = s.piece; f.key_bin = s.key_bin; f.kbase = s.kbase; f.klim = s.klim; f.ctr = s.ctr;
+  // plan: what every request takes, on the per-bin totals; then the bins with a take as keys
+  k_bf_plan<<<(nq + kBfPlanWarps - 1) / kBfPlanWarps, kBfPlanWarps * 32, 0, e->stream>>>(f);
+  k_bf_keys<<<1, kBfKeysBlock, 0, e->stream>>>(f);
+  CK(cudaGetLastError());
+  uint32_t h[kBfWords];
+  CK(cudaMemcpyAsync(n_taken, s.n_taken, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(h, s.ctr, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  const uint32_t total = h[kBfPlayers];
+  *n_total = total;
+  if (member_cap < total) return set_err(e, MM_E_CAP, "need member_cap >= %u", total);
+  if (total == 0) return MM_OK;
+  // from here on the call changes the pool: the band gather over the keys' partitions, placed and taken into staging
+  BandArgs a = band_args(e);
+  a.n_keys = h[kBfKeys];
+  a.kbase = s.kbase; a.klim = s.klim;
+  int rc = band_gather(e, a, h[kBfCols], BfKeyBins{s.key_bin});
+  if (rc) return rc;
+  CK(s.staging.reserve(total)); CK(s.members.reserve(total));
+  k_band_limit<<<1, kBandPrepBlock, 0, e->stream>>>(a);
+  k_band_place<kBandBlock><<<band_ctas(e, p.n), kBandBlock, 0, e->stream>>>(a, BandOut{s.staging, nullptr, nullptr, 1u});
+  std::vector<uint32_t> base(n);
+  for (uint32_t j = 0, acc = 0; j < n; ++j) { base[j] = acc; acc += n_taken[j]; }
+  CK(cudaMemcpyAsync(s.req_base, base.data(), (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  const uint32_t np = h[kBfPieces];
+  k_bf_out<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, s.piece, e->band.map, s.kbase,
+                                                                               s.req_base, s.staging, s.members);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(member_ids, s.members, (size_t)total * 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
   return MM_OK;
 }
 
@@ -2404,6 +2518,15 @@ int mm_band_match(mm_engine* e, int32_t W, uint32_t g_first, uint32_t g_last, ui
   CK(cudaSetDevice(e->device));
   return band_match(e, W, g_first, g_last, upper_remote, up_ids, up_rating, up_mode, n_upper, lobbies, lobby_cap,
                     member_ids, member_cap, upper_taken, stats);
+}
+
+int mm_backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_taken, uint64_t* member_ids,
+                uint64_t member_cap, uint32_t* n_total) {
+  if (!e || !n_total || (n && (!req || !n_taken)) || (member_cap && !member_ids)) return MM_E_ARG;
+  *n_total = 0;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  return backfill(e, n, req, n_taken, member_ids, member_cap, n_total);
 }
 
 int mm_remove_packed(mm_engine* e, uint32_t n, const uint32_t* handle, uint32_t* n_removed) {

@@ -354,6 +354,34 @@ class Engine:
             self._check(rc, "mm_band_match")
             return lob[:st.n_lobbies], mem[:st.n_matched], taken[:n_up].astype(bool), st
 
+    # -- backfill (mm_backfill) ------------------------------------------------------------------------------------
+    def backfill(self, mode, group, target, count, window=None):
+        """Fill the open slots of running lobbies from their queues: request j takes up to count[j] live queued players
+        of queue (mode[j], group[j]), nearest to target[j] first within `window` (None or < 0: no limit) on a
+        rating-order engine, the oldest first on an arrival-order one (target ignored, window must be None or < 0).
+        Arguments are scalars or arrays of one length.  -> (n_taken u32[n], [member ids u64 of request j, ...])"""
+        cols = np.broadcast_arrays(*(np.asarray(x, np.int64) for x in
+                                     (mode, group, target, count, -1 if window is None else window)))
+        n = cols[0].size
+        req = np.zeros(n, np.dtype([("mode", "u1"), ("group", "u1"), ("reserved", "<u2"), ("count", "<u4"),
+                                    ("target", "<i4"), ("window", "<i4")]))
+        for name, col in zip(("mode", "group", "target", "count", "window"), cols):
+            req[name] = col.ravel()
+        n_taken = np.zeros(max(n, 1), np.uint32)
+        cap = 1 << 12  # resized from the total of an MM_E_CAP refusal
+        while True:
+            mem = np.empty(cap, np.uint64)
+            total = C.c_uint32(0)
+            rc = self.lib.mm_backfill(self.h, n, _p(req), _p(n_taken), _p(mem), cap, C.byref(total))
+            if rc == abi.MM_E_CAP and total.value > cap:
+                cap = total.value
+                continue
+            self._check(rc, "mm_backfill")
+            n_taken = n_taken[:n].copy()
+            if n == 0:
+                return n_taken, []
+            return n_taken, np.split(mem[:total.value], np.cumsum(n_taken.astype(np.int64))[:-1])
+
     def in_queue(self, ids):
         ids = np.ascontiguousarray(ids, np.uint64)
         out = np.empty(len(ids), np.uint8)

@@ -267,6 +267,31 @@ class SearchPool:
         self.stats["requeued"] = self.stats.get("requeued", 0) + out.count("requeued")
         return out
 
+    def backfill(self, requests):
+        """Fill the open slots of running lobbies from their queues (Engine.backfill): a lobby that lost members asks
+        for players instead of being disbanded.  requests: (game-mode name, group name, target rating, count) or
+        (..., count, window) tuples, served in order; each takes up to `count` queued players of its queue, nearest to
+        the target rating first within `window` (the oldest first on an arrival-order engine).  -> per request, the
+        player documents taken (fewer than count when the queue runs short).  Taken players leave the pool as matched
+        players do: requeue() puts them back, remove_user() forgets them."""
+        self.flush()
+        if not requests:
+            return []
+        cols = [(self.mode_index[r[0]], self.group_names.index(r[1]), int(r[2]), int(r[3]),
+                 -1 if len(r) < 5 or r[4] is None else int(r[4])) for r in requests]
+        mode, group, target, count, window = (np.array(c, np.int64) for c in zip(*cols))
+        _n_taken, members = self.engine.backfill(mode, group, target, count, window)
+        out = []
+        for ids in members:
+            out.append([self.players.pop(int(x)) for x in ids])
+            if self.window:  # kept aside until remove_user: requeue() puts it back
+                for x in ids:
+                    at = self.enqueued_at.pop(int(x), None)
+                    if at is not None:
+                        self.matched_at[int(x)] = at
+        self.stats["backfilled"] = self.stats.get("backfilled", 0) + sum(len(d) for d in out)
+        return out
+
     def _queue_of(self, rating, mode):
         """(mode, group) queue index of a rating: the first group that holds it, else the default group (-1: none)."""
         cfg = self.engine.cfg
