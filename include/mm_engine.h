@@ -311,6 +311,55 @@ int mm_backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* 
 /* Replaces ActiveUser.in_queue?/1 (models/active_user.ex:33-44), batched.          */
 int mm_in_queue(mm_engine* e, uint32_t n, const uint64_t* id, uint8_t* out);
 
+/* EXTENSION (search status): where one player's search stands — the per-player counterpart of mm_queue_stats, for a
+ * client that polls its search and an operator who asks why a player is not matched.  The reference answers only
+ * ActiveUser.in_queue?/1 (models/active_user.ex:33-44), which mm_in_queue covers.                                 */
+#define MM_LOCATE_STAYS 0xFFFFFFFFu
+typedef struct mm_player_status {
+  uint8_t state;        /* 0 not in the active set, 1 queued (live), 2 in the active set but not queued               */
+  uint8_t mode, group;  /* its (mode, group) queue; a default-group fallback reports the default group                */
+  uint8_t reserved;     /* 0                                                                                          */
+  int32_t rating;       /* as enqueued                                                                                */
+  uint32_t enq_ts, seq; /* its stamp and enqueue sequence number (the numbering of emit_seq)                          */
+  uint32_t wait;        /* WAIT at `now`, the definition of mm_queue_stats                                            */
+  uint32_t ahead;       /* live players of its queue that the tick feeds before it                                    */
+  uint32_t depth;       /* live players of its queue (= that queue's n_waiting in mm_queue_stats)                     */
+  uint32_t lobby;       /* next tick: ordinal of its lobby among that queue's emitted lobbies; MM_LOCATE_STAYS        */
+  uint16_t member;      /* next tick: index in the lobby (team = member / team_size); 0xFFFF if it stays              */
+  uint16_t reserved2;   /* 0                                                                                          */
+} mm_player_status;     /* 36 bytes */
+
+/* mm_locate: out[i] describes id[i] (a handle on MM_F_DENSE_IDS engines, as mm_in_queue takes it).
+ *   state 1  the active-set entry points at a live slot of the current pool generation that holds this id (the test
+ *            of mm_remove): a queued player.
+ *   state 2  the id is in the active set but is not a live queued player: matched by a tick, or taken by mm_take,
+ *            mm_band_match or mm_backfill, and not yet removed (mm_requeue's code 1).
+ *   state 0  every id mm_in_queue answers 0 for (removed, expired, moved out, never queued, a handle out of range).
+ *   States 0 and 2 leave every other field 0, except lobby = MM_LOCATE_STAYS and member = 0xFFFF.  A repeated id gets
+ *   the same record each time.
+ * FEED ORDER of a queue: MM_ORDER_ARRIVAL enqueue order; MM_ORDER_RATING (c(rating), enqueue order) with c the tick's
+ * key clamp to [rmin - 1, rmax + 1].  Enqueue order is age order, (seq - seq_next) mod 2^32 ascending; requeued,
+ * merged and regrouped players sit where those calls put them.  ahead = the live players of the queue before the
+ * player in this order (0 <= ahead < depth); a wide group stored as several partitions is one queue.
+ * NEXT-TICK PREDICTION.  If the next call that changes the engine is an mm_tick* of any form (any `now`) and neither
+ * the options nor the lobby budget change in between, that tick puts the player at member index `member` of the
+ * `lobby`-th lobby it emits from the player's queue, counting from 0 in header order; MM_LOCATE_STAYS: the tick leaves
+ * the player queued.  This holds under S0, S1 (max_spread) and the per-queue and per-mode lobby budget.  Under S0
+ * without a budget it reduces to lobby = ahead / L when ahead < floor(depth / L) * L.
+ * No side effects: the pool, the active set, the snapshot, the mm_enqueue_rejects list, the last tick's results and
+ * the match section of mm_queue_stats, mm_lobby_budget_report and pending async_results copies are left alone.  n = 0
+ * does nothing.
+ * Refusals, all decided before anything runs (mm_last_error names the cause):
+ *   MM_E_ARG   null pointers with n > 0;
+ *   MM_E_STATE an MM_F_NO_DEDUPE engine (no active set maps an id to its slot), a staged packed batch.
+ * Cost: one warp per id.  A probe of the active set, then the player's rank in its bin: with resident chunk histograms
+ * (every partition of <= 255 sort keys) one 4-byte read per earlier chunk of its partition plus at most 4 KB of its own
+ * chunk's bin column; without them (MM_F_WIDE_PARTITIONS, or more than 512 partitions) the bin column of the partition
+ * up to the player (2 B per slot).  Per call, a one-CTA dry run of the tick's lobby cut on the resident bin totals and
+ * a reverse chunk map; scratch of 3 (Kp + 2) + 2 n_cut + n_modes + (chunks) words and 44 B per id.  Only the ids and the
+ * records cross PCIe.                                                                                              */
+int mm_locate(mm_engine* e, uint64_t now, uint32_t n, const uint64_t* id, mm_player_status* out);
+
 int mm_pool_size(mm_engine* e, uint32_t* n_players);
 int mm_active_size(mm_engine* e, uint32_t* n_ids);
 

@@ -434,6 +434,25 @@ static ERL_NIF_TERM nif_backfill(ErlNifEnv* env, int argc, const ERL_NIF_TERM ar
   return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &taken), enif_make_binary(env, &hs));
 }
 
+/* locate(ref, now :: u64, handles :: binary(u32[])) -> {:ok, records :: binary(mm_player_status[])}: where each
+ * player's search stands (mm_locate): state, queue, wait at `now`, players ahead and queue depth, and the lobby ordinal
+ * / member index the next tick gives it (0xFFFFFFFF: it stays queued). */
+static ERL_NIF_TERM nif_locate(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifUInt64 now; ErlNifBinary hb, out;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_uint64(env, argv[1], &now) ||
+      !enif_inspect_binary(env, argv[2], &hb) || hb.size % 4)
+    return enif_make_badarg(env);
+  const uint32_t n = (uint32_t)(hb.size / 4);
+  uint64_t* id = enif_alloc(8 * (size_t)n + 8);
+  if (!id || !enif_alloc_binary(sizeof(mm_player_status) * (size_t)n, &out)) { enif_free(id); return err(env, MM_E_CAP); }
+  for (uint32_t k = 0; k < n; ++k) { uint32_t h; memcpy(&h, hb.data + 4 * (size_t)k, 4); id[k] = h; }
+  const int rc = mm_locate(r->e, now, n, id, (mm_player_status*)out.data);
+  enif_free(id);
+  if (rc) { enif_release_binary(&out); return err(env, rc); }
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &out));
+}
+
 /* set_lobby_budget(ref, per_queue :: binary(u32[n_modes * n_groups]) | <<>>, per_mode :: binary(u32[n_modes]) | <<>>)
  * -> :ok: lobbies every queue / every mode may emit per tick from the next tick on (mm_set_lobby_budget); an empty
  * binary = no limit, 0xFFFFFFFF in an entry = no limit for it.  The engine reads n_modes * n_groups / n_modes entries:
@@ -513,6 +532,7 @@ static ErlNifFunc funcs[] = {
   {"import_regroup_many", 4, nif_import_regroup_many, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"backfill", 2, nif_backfill, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"locate", 3, nif_locate, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"seq_next", 1, nif_seq_next, 0},
   {"set_max_spread", 2, nif_set_max_spread, 0},
   {"set_lobby_budget", 3, nif_set_lobby_budget, 0},

@@ -45,6 +45,7 @@ defmodule Matchmaking.Search.Engine do
   def mode_index(name), do: Enum.find_index(@modes, fn {n, _, _} -> n == name end)
   def mode_name(index), do: elem(Enum.at(@modes, index), 0)
   def teams_of(index), do: elem(Enum.at(@modes, index), 1)
+  def team_size(index), do: elem(Enum.at(@modes, index), 2)
 
   # Player ids (UUID strings) are mapped to dense device handles by a table in Matchmaking.Search.Pool — not by a
   # hash: no collisions, no hash function the Elixir and Python hosts would have to agree on.
@@ -118,6 +119,13 @@ defmodule Matchmaking.Search.Engine do
   request 0's players, then request 1's, ...; they leave the pool and stay in the active set until remove_user.
   """
   def backfill(_ref, _requests), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Search status (extension): where each player's search stands (mm_locate).  handles: binary(u32[]) -> {:ok, records}:
+  36-byte records <<state, mode, group, 0, rating::little-signed-32, enq_ts::little-32, seq::little-32,
+  wait::little-32, ahead::little-32, depth::little-32, lobby::little-32, member::little-16, 0::16>>; state 0 gone,
+  1 queued, 2 matched or taken and not yet removed; lobby 0xFFFFFFFF: the next tick leaves the player queued.
+  """
+  def locate(_ref, _now, _handles), do: :erlang.nif_error(:nif_not_loaded)
   @doc "The enqueue sequence number the next offered player will get (mm_seq_next) -> {:ok, seq}."
   def seq_next(_ref), do: :erlang.nif_error(:nif_not_loaded)
   def n_modes, do: length(@modes)

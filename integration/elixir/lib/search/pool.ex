@@ -89,6 +89,13 @@ defmodule Matchmaking.Search.Pool do
   pool as matched players do: requeue/1 puts them back, remove_user forgets them.
   """
   def backfill(requests), do: GenServer.call(__MODULE__, {:backfill, requests}, :infinity)
+  @doc """
+  Search status (extension): one map per player id, without ingesting the staged deliveries (Engine.locate):
+  %{state: :searching | :matched | :staged | :unknown, game_mode, group, wait_ms, position, queue_size,
+  next_tick: %{lobby: ordinal among the queue's lobbies, team: index} | nil}.  The prediction is for the engine as it
+  is set now: a pool whose spread or budgets change before each tick predicts under the current ones.
+  """
+  def search_status(player_ids), do: GenServer.call(__MODULE__, {:search_status, player_ids})
   @doc "The queues of these rating groups (indices, all modes) emit no lobby until resume_queues/1; players stay queued."
   def pause(groups), do: GenServer.call(__MODULE__, {:pause, groups, true})
   def resume_queues(groups), do: GenServer.call(__MODULE__, {:pause, groups, false})
@@ -316,6 +323,38 @@ defmodule Matchmaking.Search.Pool do
         {:reply, outcome, %{st | players: back}}
       {:error, _} = e -> {:reply, e, st}
     end
+  end
+
+  def handle_call({:search_status, ids}, _from, st) do
+    known = for id <- ids, h = Map.get(st.handle_of, id), do: {id, h}
+    recs =
+      case known do
+        [] -> %{}
+        _ ->
+          {:ok, bin} = Engine.locate(st.ref, now_ms(st), for({_, h} <- known, into: <<>>, do: <<h::little-32>>))
+          parts = for <<rec::binary-size(36) <- bin>>, do: rec
+          Map.new(Enum.zip(Enum.map(known, &elem(&1, 0)), parts))
+      end
+    # st.staged is newest first: Map.new keeps the last entry of a key, the player's first delivery
+    staged = Map.new(st.staged, fn {player, mode, _rating, _ack} -> {player["id"], mode} end)
+    reply =
+      Enum.map(ids, fn id ->
+        base = %{state: :unknown, game_mode: nil, group: nil, wait_ms: nil, position: nil, queue_size: nil, next_tick: nil}
+        case Map.get(recs, id) do
+          <<1, m, g, 0, _r::little-signed-32, _ts::little-32, _seq::little-32, w::little-32, ahead::little-32,
+            depth::little-32, lob::little-32, mem::little-16, _::16>> ->
+            nt = if lob == 0xFFFFFFFF, do: nil, else: %{lobby: lob, team: div(mem, Engine.team_size(m))}
+            %{base | state: :searching, game_mode: Engine.mode_name(m), group: g, wait_ms: w, position: ahead,
+              queue_size: depth, next_tick: nt}
+          <<2, _::binary>> -> %{base | state: :matched}
+          _ ->
+            case Map.get(staged, id) do
+              nil -> base
+              mode -> %{base | state: :staged, game_mode: mode}
+            end
+        end
+      end)
+    {:reply, reply, st}
   end
 
   def handle_call({:backfill, requests}, _from, st) do

@@ -101,6 +101,28 @@ class BackfillReq(C.Structure):
     ]
 
 
+MM_LOCATE_STAYS = 0xFFFFFFFF
+
+
+class PlayerStatus(C.Structure):
+    """mm_player_status: one player's search status (36 bytes)."""
+    _fields_ = [
+        ("state", C.c_uint8),
+        ("mode", C.c_uint8),
+        ("group", C.c_uint8),
+        ("reserved", C.c_uint8),
+        ("rating", C.c_int32),
+        ("enq_ts", C.c_uint32),
+        ("seq", C.c_uint32),
+        ("wait", C.c_uint32),
+        ("ahead", C.c_uint32),
+        ("depth", C.c_uint32),
+        ("lobby", C.c_uint32),
+        ("member", C.c_uint16),
+        ("reserved2", C.c_uint16),
+    ]
+
+
 class QueueStat(C.Structure):
     """One (mode, group) queue: the resident pool at `now` and the players the last tick matched (988 bytes)."""
     _fields_ = [
@@ -175,6 +197,7 @@ PROTOTYPES = {
                                 _vp, C.c_uint32, _vp, C.c_uint64, _vp, _P(BandStats)]),
     "mm_backfill": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, C.c_uint64, _P(C.c_uint32)]),
     "mm_in_queue": (C.c_int, [_vp, C.c_uint32, _vp, _vp]),
+    "mm_locate": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp]),
     "mm_pool_size": (C.c_int, [_vp, _P(C.c_uint32)]),
     "mm_active_size": (C.c_int, [_vp, _P(C.c_uint32)]),
     "mm_tick": (C.c_int, [_vp, C.c_uint64, _vp, C.c_uint32, _vp, C.c_uint64, _vp, _P(TickStats)]),

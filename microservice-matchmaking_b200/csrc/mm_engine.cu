@@ -24,6 +24,7 @@
 #include "mm_expire.cuh"
 #include "mm_image.cuh"
 #include "mm_kernels.cuh"
+#include "mm_locate.cuh"
 #include "mm_recut.cuh"
 #include "mm_regroup.cuh"
 #include "mm_requeue.cuh"
@@ -281,6 +282,14 @@ struct mm_engine {
     DevArray<BfPiece> piece;
     DevArray<uint64_t> staging, members;
   } bf;
+
+  // mm_locate (mm_locate.cuh): the queried ids, the records and the call's tables (preview bases, member slots,
+  // budgets, reverse chunk map), grown on demand; no other call reads or writes them
+  struct Locate {
+    DevArray<uint64_t> id;
+    DevArray<mm_player_status> out;
+    DevArray<uint32_t> tab;  // pos [Kp + 2] | outbase [Kp + 2] | binlim [Kp + 2] | cand [n_cut] | budgets [n_cut + n_modes] | rmap [n_chunks]
+  } loc;
 };
 
 namespace {
@@ -2165,6 +2174,37 @@ int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_t
   return MM_OK;
 }
 
+// ---- mm_locate (mm_locate.cuh) -------------------------------------------------------------------------------------
+int locate(mm_engine* e, uint64_t now, uint32_t n, const uint64_t* id, mm_player_status* out) {
+  auto& s = e->loc;
+  const Pool& p = e->pool[e->cur];
+  const size_t wb = (size_t)e->Kp + 2, nc = e->n_cut, nm = e->cfg.n_modes;
+  CK(s.id.reserve(n)); CK(s.out.reserve(n)); CK(s.tab.reserve(3 * wb + 2 * nc + nm + e->n_chunks));
+  uint32_t *pos = s.tab, *ob = pos + wb, *bl = ob + wb, *cand = bl + wb, *bud = cand + nc, *rmap = bud + nc + nm;
+  CK(cudaMemcpyAsync(s.id, id, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
+  // the budgets as set now (the tick's device copy is brought up to date only by the next tick)
+  if (!e->bud_queue.empty()) CK(cudaMemcpyAsync(bud, e->bud_queue.data(), nc * 4, cudaMemcpyHostToDevice, e->stream));
+  if (!e->bud_mode.empty()) CK(cudaMemcpyAsync(bud + nc, e->bud_mode.data(), nm * 4, cudaMemcpyHostToDevice, e->stream));
+  TailArgs t = tail_args(e);
+  t.outbase = ob; t.binlim = bl; t.cand = cand; t.seg = nullptr; t.ctr = nullptr;
+  t.dst = PoolMeta{}; t.dst.tot = pos;
+  t.bud_queue = e->bud_queue.empty() ? nullptr : bud;
+  t.bud_mode = e->bud_mode.empty() ? nullptr : bud + nc;
+  const size_t smem = (size_t)tail_words(e->Kp, t.layout) * 4;
+  k_locate_preview<<<1, kScanBlock, smem, e->stream>>>(t);
+  k_loc_rmap<<<e->n_segs, 256, 0, e->stream>>>(p.m, rmap);
+  LocateArgs a{};
+  a.n = n; a.id = s.id; a.act = act_view(e); a.pool = p.v; a.meta = p.m;
+  a.n_slots = (uint32_t)pool_slots(e); a.gen = e->gen; a.n_groups = e->cfg.n_groups; a.now = (uint32_t)now;
+  a.bin_seg = e->d_bin_seg; a.seg_bin_lo = e->d_seg_bin_lo; a.seg_L = e->d_seg_L; a.part_cut = e->d_part_cut;
+  a.cut_lp_lo = e->d_cut_lp_lo; a.rmap = rmap; a.pos = pos; a.outbase = ob; a.binlim = bl; a.out = s.out;
+  k_locate<<<(uint32_t)(((size_t)n * 32 + 255) / 256), 256, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out, s.out, (size_t)n * sizeof(mm_player_status), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
 }  // namespace
 
 // =======================================================================================
@@ -2258,7 +2298,8 @@ int mm_create(const mm_config* cfg, mm_engine** out) {
     bool ok = allow_max_smem(e, k_colscan<false>) == cudaSuccess && allow_max_smem(e, k_colscan<true>) == cudaSuccess &&
               allow_max_smem(e, k_lobby_candidates) == cudaSuccess && allow_max_smem(e, k_hist<512>) == cudaSuccess &&
               allow_max_smem(e, k_place<512>) == cudaSuccess && allow_max_smem(e, k_tick<512>) == cudaSuccess &&
-              allow_max_smem(e, k_tick<512, true>) == cudaSuccess;
+              allow_max_smem(e, k_tick<512, true>) == cudaSuccess &&
+              allow_max_smem(e, k_locate_preview) == cudaSuccess;
     if (!ok) return bail(fail(e, cudaGetLastError(), "cudaFuncSetAttribute"));
   }
   e->n_chunks = (e->capacity + kTile - 1) / kTile + e->n_segs + 2;
@@ -2550,6 +2591,17 @@ int mm_in_queue(mm_engine* e, uint32_t n, const uint64_t* id, uint8_t* out) {
   CK(cudaMemcpyAsync(out, e->d_lookup, n, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   return MM_OK;
+}
+
+int mm_locate(mm_engine* e, uint64_t now, uint32_t n, const uint64_t* id, mm_player_status* out) {
+  if (!e) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (n && (!id || !out)) return set_err(e, MM_E_ARG, "null id or out array with n = %u", n);
+  if (!e->use_active) return set_err(e, MM_E_STATE, "an MM_F_NO_DEDUPE engine has no active set to find ids in");
+  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (n == 0) return MM_OK;
+  CK(cudaSetDevice(e->device));
+  return locate(e, now, n, id, out);
 }
 
 int mm_pool_size(mm_engine* e, uint32_t* n) {

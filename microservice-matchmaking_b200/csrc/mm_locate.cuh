@@ -1,0 +1,116 @@
+// mm_locate.cuh — mm_locate: the search status of single players, answered on the device from the resident pool
+//
+// Three launches, none of which writes anything but the call's own scratch:
+//   k_locate_preview  the tick's tail (mm_scan.cuh, kPreview) on the resident bin totals with the engine's max_spread
+//                     and lobby budget: the sorted position of every bin's first player (pos), and the member slots
+//                     of every bin's matched prefix (outbase / binlim) the next tick would use
+//   k_loc_rmap        physical chunk -> its index in its partition's chunk list (one entry per chunk in use)
+//   k_locate          one warp per query: the active-set probe (mm_remove's test), then the player's rank among the
+//                     live players of its bin that the tick places before it, and the answer
+// The tick places the players of a bin in partition storage order, so a player's rank is the live players of its bin
+// in the partition's earlier chunks plus those before it in its own chunk.  With resident chunk histograms the earlier
+// chunks cost one 4-byte read each; without them (MM_F_WIDE_PARTITIONS, or more than kMaxSegs partitions) the warp
+// counts the bin column of the earlier chunks.  The own chunk is counted from the bin column (at most 4 KB).
+#pragma once
+#include "mm_kernels.cuh"
+
+namespace mm {
+
+static_assert(sizeof(mm_player_status) == 36, "mm_player_status is 36 bytes (include/mm_engine.h)");
+
+// Always the budget form of the tail: with no budget set (null t.bud_queue / t.bud_mode) every queue is allotted all
+// of its lobbies and the cut is the unbudgeted one.  (The form without the budget code spills at this launch bound.)
+__global__ void __launch_bounds__(kScanBlock) k_locate_preview(const TailArgs t) {
+  extern __shared__ __align__(16) uint32_t scratch[];
+  colscan_tail_body<false, true, true>(scratch, t);
+}
+
+// rmap[chunk_tab[sg][k]] = k for the chunks of every partition in use (one CTA per partition)
+__global__ void k_loc_rmap(const PoolMeta m, uint32_t* __restrict__ rmap) {
+  const uint32_t sg = blockIdx.x, nch = (__ldg(&m.fill[sg]) + kTile - 1) / kTile;
+  for (uint32_t k = threadIdx.x; k < nch; k += blockDim.x) rmap[__ldg(&m.chunk_tab[(size_t)sg * m.max_ch + k])] = k;
+}
+
+struct LocateArgs {
+  uint32_t n;
+  const uint64_t* id;        // [n] queried ids (handles on MM_F_DENSE_IDS engines)
+  ActiveView act;
+  PoolView pool;
+  PoolMeta meta;             // the resident pool's partitions
+  uint32_t n_slots, gen, n_groups, now;
+  const uint16_t* bin_seg;   // [Kp] bin -> partition
+  const uint32_t* seg_bin_lo;  // [n_segs + 1]
+  const uint32_t* seg_L;     // [n_segs]
+  const uint16_t* part_cut;  // [n_segs] partition -> (mode, group) queue
+  const uint32_t* cut_lp_lo; // [n_cut + 1] first partition of the queue
+  const uint32_t* rmap;      // k_loc_rmap
+  const uint32_t* pos;       // [Kp + 1] k_locate_preview: sorted position of the bin's first player
+  const uint32_t* outbase;   // [Kp] k_locate_preview: member slot of the bin's first player
+  const uint32_t* binlim;    // [Kp] k_locate_preview: end of the bin's matched member slots
+  mm_player_status* out;     // [n]
+};
+
+__global__ void __launch_bounds__(256) k_locate(const LocateArgs a) {
+  const uint32_t lane = threadIdx.x & 31, q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (q >= a.n) return;  // (uniform over the warp)
+  const uint64_t pid = a.id[q];
+  uint32_t state = 0, slot = 0;
+  if (lane == 0 && a.act.on()) {
+    const uint64_t h = act_find(a.act, pid);
+    if (h != ~0ull) {
+      const unsigned long long v = *a.act.val(h);
+      state = (a.act.dcap && v == kFreeVal) ? 0u : 2u;  // a hashed key is found only while it is active
+      slot = (uint32_t)v;
+      if (v < kPending && (uint32_t)(v >> 32) == a.gen && slot < a.n_slots && a.pool.id[slot] == pid &&
+          a.pool.mode[slot] != MM_MODE_DEAD)
+        state = 1;
+    }
+  }
+  state = __shfl_sync(0xFFFFFFFFu, state, 0);
+  slot = __shfl_sync(0xFFFFFFFFu, slot, 0);
+  mm_player_status r{};
+  r.lobby = MM_LOCATE_STAYS;
+  r.member = 0xFFFFu;
+  if (state != 1) {
+    r.state = (uint8_t)state;
+    if (lane == 0) a.out[q] = r;
+    return;
+  }
+  const uint32_t v = a.pool.bin[slot], sg = a.bin_seg[v], chunk = slot / kTile, off = slot % kTile;
+  const uint32_t k = a.rmap[chunk];
+  const uint32_t* tab = a.meta.chunk_tab + (size_t)sg * a.meta.max_ch;
+  uint32_t rank = 0;
+  if (a.meta.chist) {
+    const uint32_t key = v - a.seg_bin_lo[sg];
+    for (uint32_t j = lane; j < k; j += 32) rank += a.meta.chist[(size_t)tab[j] * kChunkHist + key];
+  } else {
+    for (uint32_t j = 0; j < k; ++j) {
+      const uint16_t* b = a.pool.bin + (size_t)tab[j] * kTile;
+      for (uint32_t o = lane; o < kTile; o += 32) rank += b[o] == v ? 1u : 0u;
+    }
+  }
+  const uint16_t* own = a.pool.bin + (size_t)chunk * kTile;
+  for (uint32_t o = lane; o < off; o += 32) rank += own[o] == v ? 1u : 0u;
+  rank = __reduce_add_sync(0xFFFFFFFFu, rank);
+  if (lane != 0) return;
+  const uint32_t c = a.part_cut[sg], b0 = a.seg_bin_lo[a.cut_lp_lo[c]], b1 = a.seg_bin_lo[a.cut_lp_lo[c + 1]];
+  r.state = 1;
+  r.mode = a.pool.mode[slot];
+  r.group = (uint8_t)(c % a.n_groups);
+  r.rating = a.pool.rating[slot];
+  r.enq_ts = a.pool.ts[slot];
+  r.seq = a.pool.seq[slot];
+  const int32_t w = (int32_t)(a.now - r.enq_ts);
+  r.wait = w < 0 ? 0u : (uint32_t)w;
+  r.ahead = a.pos[v] - a.pos[b0] + rank;
+  r.depth = a.pos[b1] - a.pos[b0];
+  const uint32_t m = a.outbase[v] + rank;  // the member slot the tick gives the player
+  if (m < a.binlim[v]) {
+    const uint32_t rel = m - a.outbase[b0], L = a.seg_L[sg];  // the queue's lobby k = its member slots [k L, k L + L)
+    r.lobby = rel / L;
+    r.member = (uint16_t)(rel % L);
+  }
+  a.out[q] = r;
+}
+
+}  // namespace mm

@@ -258,7 +258,10 @@ __device__ __noinline__ void tail_budget(uint32_t* scratch, uint32_t* s_m, uint3
 // smaller matched prefix per bin.  kBudget selects the tail with the budget code: a tick without a budget runs the
 // instantiation without it, instruction for instruction the tail it has always run.  kCountOnly (k_lobby_candidates): stop at the per-queue lobby counts, write t.cand
 // (and, for layout bit 0 clear, the parked counts in t.binlim) and nothing else.
-template <bool kCountOnly = false, bool kBudget = false>
+// kPreview (mm_locate): the whole cut, budget included when kBudget, into the caller's own scratch: t.outbase, t.binlim,
+// t.cand (kBudget) and, in t.dst.tot, the sorted position of every bin's first player ([Kp + 1]: the bases s_bb).
+// Nothing else is written: not t.seg, t.ctr or the rest of t.dst.
+template <bool kCountOnly = false, bool kBudget = false, bool kPreview = false>
 __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailArgs t) {
   constexpr uint32_t NW = kScanBlock / 32;
   uint32_t* s_tmp = scratch;            // [64]
@@ -293,6 +296,8 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
   const uint32_t total = block_excl_scan<kScanBlock>(s_bb, Kp, s_tmp);
   if (tid == 0) s_bb[Kp] = total;
   __syncthreads();
+  if constexpr (kPreview)
+    for (uint32_t v = tid; v <= Kp; v += kScanBlock) t.dst.tot[v] = s_bb[v];
   const uint32_t alive = s_bb[K], dead = total - alive;
   const bool windowed = t.max_spread >= 0;
   const bool m_smem = (t.layout & 1u) != 0, key_smem = (t.layout & 2u) != 0;
@@ -377,7 +382,7 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
       t.outbase[v] = s_m[v];
       t.binlim[v] = s_m[v + 1];  // = outbase + matched players of the bin
       // bin totals of the compacted pool: what was there minus the matched prefix; removed players are gone
-      t.dst.tot[v] = v < K ? __ldcg(&t.tot[v]) - (s_m[v + 1] - s_m[v]) : 0u;
+      if constexpr (!kPreview) t.dst.tot[v] = v < K ? __ldcg(&t.tot[v]) - (s_m[v + 1] - s_m[v]) : 0u;
     }
     for (uint32_t sg = tid; sg < n_segs; sg += kScanBlock) s_mt[sg] = s_m[s_lo[sg + 1]] - s_m[s_lo[sg]];
   }
@@ -403,7 +408,7 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
         s_ms[sg] = c_mem + i_mem - mt;
         s_a[sg] = c_left + i_left - nleft;
         s_nch[sg] = c_ch + i_ch - nch;
-        t.dst.fill[sg] = nleft;
+        if constexpr (!kPreview) t.dst.fill[sg] = nleft;
       }
       c_mem += __shfl_sync(0xFFFFFFFFu, i_mem, 31);
       c_left += __shfl_sync(0xFFFFFFFFu, i_left, 31); c_ch += __shfl_sync(0xFFFFFFFFu, i_ch, 31);
@@ -431,17 +436,19 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
         SegInfo si;
         si.n = s_ns[sg]; si.n_lobbies = nl; si.member_base = hb; si.lobby_base = c_lob + i_lob - nl;
         si.left_base = s_a[sg]; si.new_chunk = s_nch[sg]; si.n_left = s_ns[sg] - s_mt[sg]; si.reserved = 0;
-        t.seg[sg] = si;
+        if constexpr (!kPreview) t.seg[sg] = si;
       }
       c_lob += __shfl_sync(0xFFFFFFFFu, i_lob, 31);
     }
     if (lane == 0) {
       s_nch[n_segs] = c_ch;
       s_misc[1] = c_mem; s_misc[2] = c_lob;
-      *t.dst.bump = c_ch;
-      t.ctr->n_lobbies = c_lob; t.ctr->n_matched = c_mem; t.ctr->n_alive = alive; t.ctr->n_dead = dead;
-      t.ctr->n_resid = c_left;
-      t.ctr->heavy = s_misc[0];
+      if constexpr (!kPreview) {
+        *t.dst.bump = c_ch;
+        t.ctr->n_lobbies = c_lob; t.ctr->n_matched = c_mem; t.ctr->n_alive = alive; t.ctr->n_dead = dead;
+        t.ctr->n_resid = c_left;
+        t.ctr->heavy = s_misc[0];
+      }
     }
   }
   __syncthreads();
@@ -456,15 +463,19 @@ __device__ __forceinline__ void colscan_tail_body(uint32_t* scratch, const TailA
         const uint32_t o = (b0 < mend ? b0 : mend), l = (b1 < mend ? b1 : mend);
         t.outbase[v] = o - shift;
         t.binlim[v] = l - shift;
-        t.dst.tot[v] = (b1 - b0) - (l - o);  // bin totals of the compacted pool: the unmatched tail of the bin
+        if constexpr (!kPreview) t.dst.tot[v] = (b1 - b0) - (l - o);  // bin totals of the compacted pool: the unmatched tail of the bin
       }
     }
-    for (uint32_t v = K + tid; v < Kp; v += kScanBlock) { t.outbase[v] = n_matched; t.binlim[v] = n_matched; t.dst.tot[v] = 0; }
+    for (uint32_t v = K + tid; v < Kp; v += kScanBlock) {
+      t.outbase[v] = n_matched; t.binlim[v] = n_matched;
+      if constexpr (!kPreview) t.dst.tot[v] = 0;
+    }
   }
-  for (uint32_t sg = warp; sg < n_segs; sg += NW) {  // chunk lists of the compacted pool
-    const uint32_t c0 = s_nch[sg], c1 = s_nch[sg + 1];
-    for (uint32_t k = lane; k < c1 - c0; k += 32) t.dst.chunk_tab[(size_t)sg * t.dst.max_ch + k] = c0 + k;
-  }
+  if constexpr (!kPreview)
+    for (uint32_t sg = warp; sg < n_segs; sg += NW) {  // chunk lists of the compacted pool
+      const uint32_t c0 = s_nch[sg], c1 = s_nch[sg + 1];
+      for (uint32_t k = lane; k < c1 - c0; k += 32) t.dst.chunk_tab[(size_t)sg * t.dst.max_ch + k] = c0 + k;
+    }
   __syncthreads();
 }
 

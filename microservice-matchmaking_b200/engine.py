@@ -47,6 +47,13 @@ def _p(a):
 
 LOBBY_DTYPE = np.dtype([("first_member", "<u4"), ("n_members", "<u2"), ("mode", "u1"), ("group", "u1")])
 
+# mm_player_status (include/mm_engine.h) as a numpy record
+PLAYER_STATUS_DTYPE = np.dtype([
+    ("state", "u1"), ("mode", "u1"), ("group", "u1"), ("reserved", "u1"), ("rating", "<i4"), ("enq_ts", "<u4"),
+    ("seq", "<u4"), ("wait", "<u4"), ("ahead", "<u4"), ("depth", "<u4"), ("lobby", "<u4"), ("member", "<u2"),
+    ("reserved2", "<u2")])
+assert PLAYER_STATUS_DTYPE.itemsize == C.sizeof(abi.PlayerStatus)
+
 # mm_queue_stat (include/mm_engine.h) as a numpy record
 QUEUE_STAT_DTYPE = np.dtype([
     ("mode", "u1"), ("group", "u1"), ("reserved", "<u2"),
@@ -387,6 +394,16 @@ class Engine:
         out = np.empty(len(ids), np.uint8)
         self._check(self.lib.mm_in_queue(self.h, len(ids), _p(ids), _p(out)), "mm_in_queue")
         return out.astype(bool)
+
+    def locate(self, ids, now=0):
+        """Search status of each id (mm_locate) -> PLAYER_STATUS_DTYPE[len(ids)]: state (0 gone, 1 queued, 2 matched or
+        taken and not yet removed), its queue, rating, stamp, seq, wait at `now`, players ahead of it in its queue's feed
+        order and the queue's depth, and the lobby ordinal / member index the next tick gives it (lobby =
+        abi.MM_LOCATE_STAYS: it stays queued)."""
+        ids = np.ascontiguousarray(ids, np.uint64)
+        out = np.zeros(len(ids), PLAYER_STATUS_DTYPE)
+        self._check(self.lib.mm_locate(self.h, int(now) & 0xFFFFFFFFFFFFFFFF, len(ids), _p(ids), _p(out)), "mm_locate")
+        return out
 
     def pool_size(self):
         v = C.c_uint32(0)

@@ -292,6 +292,46 @@ class SearchPool:
         self.stats["backfilled"] = self.stats.get("backfilled", 0) + sum(len(d) for d in out)
         return out
 
+    def search_status(self, player_ids):
+        """Where each player's search stands (Engine.locate at now_ms()), without ingesting the staged deliveries.
+        -> one dict per player id: "state" is "searching" (queued), "matched" (placed in a lobby, or taken by backfill,
+        and not yet removed), "staged" (received, not yet ingested: only its "game_mode" and "group" are known) or
+        "unknown"; "game_mode" and "group" name its queue; "wait_ms" is its wait; "position" counts the players of its
+        queue that the tick feeds before it and "queue_size" the players of the queue; "next_tick" is {"lobby": ordinal
+        among the queue's lobbies of the next tick, "team": team index} or None if the next tick leaves it queued.
+        The prediction holds for the engine as it is set now.  A pool with a WindowSchedule or a lobby_budget callable
+        sets max_spread and the budgets again before each tick, so its prediction is "under the current spread and
+        budget" — the next tick may use others.  Fields that do not apply to a state are None."""
+        empty = dict(state="unknown", game_mode=None, group=None, wait_ms=None, position=None, queue_size=None,
+                     next_tick=None)
+        out = [dict(empty) for _ in player_ids]
+        known = [(i, h) for i, pid in enumerate(player_ids) for h in [self.handles.lookup(pid)] if h is not None]
+        if known:
+            rec = self.engine.locate(np.array([h for _i, h in known], np.uint64), self.now_ms())
+            for (i, _h), r in zip(known, rec):
+                if r["state"] == 2:
+                    out[i]["state"] = "matched"
+                elif r["state"] == 1:
+                    m = int(r["mode"])
+                    nxt = None
+                    if int(r["lobby"]) != 0xFFFFFFFF:
+                        nxt = {"lobby": int(r["lobby"]), "team": int(r["member"]) // self.engine.cfg.modes[m].team_size}
+                    out[i].update(state="searching", game_mode=self.mode_names[m], group=self.group_names[int(r["group"])],
+                                  wait_ms=int(r["wait"]), position=int(r["ahead"]), queue_size=int(r["depth"]),
+                                  next_tick=nxt)
+        staged = {}
+        for s in self._staged:  # the first delivery of a player names its queue
+            staged.setdefault(s[0], s)
+        for i, pid in enumerate(player_ids):
+            s = staged.get(pid)
+            if out[i]["state"] != "unknown" or s is None:
+                continue
+            mode = self.mode_index.get(s[2]) if isinstance(s[2], str) else None
+            q = self._queue_of(s[1], mode) if mode is not None else -1
+            out[i].update(state="staged", game_mode=s[2] if mode is not None else None,
+                          group=self.group_names[q % len(self.group_names)] if q >= 0 else None)
+        return out
+
     def _queue_of(self, rating, mode):
         """(mode, group) queue index of a rating: the first group that holds it, else the default group (-1: none)."""
         cfg = self.engine.cfg
