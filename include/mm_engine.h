@@ -446,6 +446,58 @@ typedef struct mm_queue_stat {
  * async_results copies alone.                                                                                     */
 int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap, uint32_t* n_out);
 
+/* ---- match quality -------------------------------------------------------------
+ * EXTENSION (measurement): how even the last tick's lobbies are, the other half of the wait / quality trade-off that
+ * mm_queue_stats reports the wait half of.  max_spread, a widening window schedule, the lobby budget and a new
+ * rating-group table all move it; the tick itself returns only ids, and the ratings stay on the device.
+ *
+ * DEFINITION.  c(r) = min(max(r, rmin - 1), rmax + 1), rmin / rmax over all groups: the tick's key clamp (the c of
+ * mm_backfill and mm_locate).  The rating of a player is the one the pool holds for it (what mm_pool_read returns).
+ * Per lobby: take lobby h of the last completed tick, in the tick's header order; its mode has T teams of S players
+ * (L = T S), its members are x_0 .. x_{L-1} in member order and r_i = c(rating(x_i)).  min_rating = min r_i,
+ * max_rating = max r_i, SPREAD = max_rating - min_rating, rating_sum = sum r_i (64-bit), team sums
+ * s_t = sum of r_i over i in [t S, (t + 1) S), IMBALANCE = max_t s_t - min_t s_t (0 when T = 1), saturated at
+ * 2^32 - 1.  Per (mode, group) queue, over that queue's lobbies of the last tick: n_lobbies, the largest spread and
+ * imbalance, their sums (64-bit, for means) and their histograms in the BUCKETS of mm_queue_stats applied to rating
+ * points (a value of 2^31 or more counts in bucket 119).
+ *
+ * WHICH TICK: the last completed tick of any form — mm_tick, mm_tick_packed or mm_tick_device, fused or split
+ * (tick_impl), with or without async_results and emit_seq, under S0 or S1 and any lobby budget.  per_lobby[h]
+ * describes lobbies[h] of that tick; per_queue holds one record per queue, empty ones included, in the order of
+ * mm_queue_stats (mode * n_groups + group).  The lobbies of mm_band_match and the players of mm_backfill are outside
+ * the tick and not covered.
+ * VOID exactly when the match section of mm_queue_stats is (before the first tick, after a tick that failed, after
+ * mm_restore and after the import loads): *n_out = 0 and *n_lobbies = 0, nothing is written.
+ * READ-ONLY: no other call changes the report until the next tick, and the call changes nothing — not the pool, the
+ * active set, the last tick's results, the snapshot, the reject list or pending async_results copies.
+ * REFUSALS, decided before anything runs: MM_E_ARG for a null e, per_queue, n_out or n_lobbies; MM_E_CAP when
+ * cap < n_modes * n_groups (*n_out = the records needed) or when per_lobby is not NULL and lobby_cap is below the
+ * tick's lobby count (*n_lobbies = the count needed); nothing is written then.  per_lobby = NULL skips the per-lobby
+ * output.
+ * COST: one pass over the 2-byte sort-key column and the last tick's left bits of the pool it read (MM_ORDER_RATING;
+ * the lobby values then come from per-key prefix sums), or over the mode and rating columns (MM_ORDER_ARRIVAL), plus
+ * per-lobby work; only the records cross PCIe.  Device memory, allocated by the first call and kept: 24 bytes per
+ * lobby the pool could hold (capacity / smallest L + 1), 12 bytes per sort key, 992 bytes per queue, 4 bytes per
+ * chunk, and on MM_ORDER_ARRIVAL engines 8 more bytes per such lobby and 4 bytes per player of capacity.        */
+typedef struct mm_lobby_quality {
+  int32_t min_rating, max_rating; /* c(rating) of the lowest and highest member                    */
+  int64_t rating_sum;             /* sum of the members' c(rating)                                  */
+  uint32_t imbalance;             /* max - min team rating sum (0 for one team), saturated          */
+  uint32_t reserved;              /* 0                                                              */
+} mm_lobby_quality;               /* 24 bytes */
+
+typedef struct mm_queue_quality {
+  uint8_t mode, group;
+  uint16_t reserved;
+  uint32_t n_lobbies, max_spread, max_imbalance;
+  uint64_t sum_spread, sum_imbalance;
+  uint32_t spread_hist[MM_WAIT_BUCKETS];
+  uint32_t imbalance_hist[MM_WAIT_BUCKETS];
+} mm_queue_quality;               /* 992 bytes */
+
+int mm_match_quality(mm_engine* e, mm_queue_quality* per_queue, uint32_t cap, uint32_t* n_out,
+                     mm_lobby_quality* per_lobby, uint32_t lobby_cap, uint32_t* n_lobbies);
+
 /* ---- lobby budget: how many lobbies a tick may emit ------------------------------
  * EXTENSION (flow control).  The reference emits one lobby at a time behind prefetch_count: 10 (search/worker.ex:29),
  * and its lobby stage answers the players of a lobby it finds no game server for with an error

@@ -183,6 +183,26 @@ static ERL_NIF_TERM nif_queue_stats(ErlNifEnv* env, int argc, const ERL_NIF_TERM
   return rc ? err(env, rc) : enif_make_tuple2(env, atom(env, "ok"), out);
 }
 
+/* match_quality(ref) -> {:ok, records :: binary(mm_queue_quality[])}: one 992-byte record per (mode, group) queue,
+ * mode * n_groups + group order — the rating spread and team imbalance of the last tick's lobbies (extension); an
+ * empty binary while the report is void (no tick yet, a failed tick, a restore or an import since) */
+static ERL_NIF_TERM nif_match_quality(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; uint32_t n = 0, n_lob = 0; mm_queue_quality probe;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r)) return enif_make_badarg(env);
+  int rc = mm_match_quality(r->e, &probe, 0, &n, NULL, 0, &n_lob);  /* MM_E_CAP: n = records needed */
+  if (rc != MM_E_CAP) return err(env, rc ? rc : MM_E_STATE);
+  mm_queue_quality* tmp = (mm_queue_quality*)enif_alloc((size_t)n * sizeof(mm_queue_quality));
+  if (!tmp) return err(env, MM_E_CAP);
+  rc = mm_match_quality(r->e, tmp, n, &n, NULL, 0, &n_lob);  /* n = 0 when void */
+  if (rc) { enif_free(tmp); return err(env, rc); }
+  ERL_NIF_TERM out;
+  unsigned char* buf = enif_make_new_binary(env, (size_t)n * sizeof(mm_queue_quality), &out);
+  memcpy(buf, tmp, (size_t)n * sizeof(mm_queue_quality));
+  enif_free(tmp);
+  return enif_make_tuple2(env, atom(env, "ok"), out);
+}
+
 /* expire_packed(ref, now_ms, max_wait_ms) -> {:ok, handles :: binary(u32[])}: search timeout (extension) — the
  * queued players who have waited >= max_wait_ms leave the pool and the active set; the caller answers each one */
 static ERL_NIF_TERM nif_expire_packed(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
@@ -321,9 +341,10 @@ static ERL_NIF_TERM nif_import_regroup_many(ErlNifEnv* env, int argc, const ERL_
       cap = cap + n < cap ? UINT32_MAX : cap + n;
     }
   }
-  if (has_keep) {  /* one byte per queue: mm_queue_stats with cap 0 gives the queue count */
+  if (has_keep) {  /* one byte per queue: mm_queue_stats with cap 0 gives the queue count (it needs a record) */
     uint32_t n_cut = 0;
-    mm_queue_stats(r->e, 0, NULL, 0, &n_cut);
+    mm_queue_stat probe;
+    mm_queue_stats(r->e, 0, &probe, 0, &n_cut);
     if (keep.size != n_cut) return enif_make_badarg(env);
   }
   if (!enif_alloc_binary((size_t)cap * 8, &out)) return err(env, MM_E_CAP);
@@ -523,6 +544,7 @@ static ErlNifFunc funcs[] = {
   {"tick_packed", 2, nif_tick_packed, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"status", 1, nif_status, 0},
   {"queue_stats", 2, nif_queue_stats, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"match_quality", 1, nif_match_quality, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"expire_packed", 3, nif_expire_packed, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"export_image", 1, nif_export_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"import_image", 2, nif_import_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},

@@ -66,6 +66,12 @@ defmodule Matchmaking.Search.Engine do
   @doc "-> {:ok, binary(mm_queue_stat[])}: per (mode, group) queue, waiting players and wait histograms (include/mm_engine.h)"
   def queue_stats(_ref, _now_ms), do: :erlang.nif_error(:nif_not_loaded)
   @doc """
+  Extension (match quality): the rating spread and team imbalance of the last tick's lobbies per (mode, group) queue
+  (mm_match_quality) -> {:ok, binary(mm_queue_quality[])}, in queue_stats/2 record order; an empty binary while the
+  report is void (no tick yet, a failed tick, a restore or an import since).
+  """
+  def match_quality(_ref), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
   Extension (search timeout): the queued players who have waited >= max_wait_ms at now_ms leave the pool and the
   active set, as if removed -> {:ok, handles :: binary(u32[])}; the caller answers each one.
   """

@@ -11,7 +11,9 @@ defmodule Matchmaking.Search.Pool do
                      search/worker.ex:250-261,315-319
       in_queue?/1, remove_user/1    replace Matchmaking.Model.ActiveUser (models/active_user.ex:33-66)
       queue_status/1 one rating group's queues (Engine.queue_stats): waiting players, oldest / p50 / p99 wait, the
-                     last tick's matched players and p99 wait at match, in ms — Search.Worker.status/0's queue depth
+                     last tick's matched players and p99 wait at match, in ms — Search.Worker.status/0's queue depth;
+                     with Engine.match_quality also the last tick's lobbies, mean / p50 / p99 / max rating spread and
+                     mean / p99 / max team imbalance, in rating points (zero lobbies while the report is void)
       search_timeout_ms   option (extension, default nil = off): after each tick's lobbies are published, the players
                      still queued who have waited at least this long leave the pool (Engine.expire_packed) and get the
                      error response of game-lobby/worker.ex:63-71,105-116 on their "response-queue"
@@ -178,18 +180,32 @@ defmodule Matchmaking.Search.Pool do
   end
 
   def handle_call({:queue_status, group}, _from, st) do
-    reply = case Engine.queue_stats(st.ref, now_ms(st)) do
-      {:ok, recs} ->
-        for <<mode, g, _::16, waiting::little-32, _removed::little-32, oldest::little-32, hist::binary-size(480),
-              _lobbies::little-32, matched::little-32, _max_match::little-32, mhist::binary-size(480) <- recs>>,
-            g == group, into: %{} do
-          {Engine.mode_name(mode), %{waiting: waiting, oldest_wait_ms: oldest, p50_wait_ms: quantile(hist, 0.5),
-                                     p99_wait_ms: quantile(hist, 0.99), last_tick_matched: matched,
-                                     last_tick_p99_match_wait_ms: quantile(mhist, 0.99)}}
-        end
-      {:error, _} = e -> e
+    reply = with {:ok, recs} <- Engine.queue_stats(st.ref, now_ms(st)),
+                 {:ok, qrecs} <- Engine.match_quality(st.ref) do
+      quality = quality_of(qrecs, group)
+      for <<mode, g, _::16, waiting::little-32, _removed::little-32, oldest::little-32, hist::binary-size(480),
+            _lobbies::little-32, matched::little-32, _max_match::little-32, mhist::binary-size(480) <- recs>>,
+          g == group, into: %{} do
+        {Engine.mode_name(mode),
+         Map.merge(%{waiting: waiting, oldest_wait_ms: oldest, p50_wait_ms: quantile(hist, 0.5),
+                     p99_wait_ms: quantile(hist, 0.99), last_tick_matched: matched,
+                     last_tick_p99_match_wait_ms: quantile(mhist, 0.99)},
+                   Map.get(quality, mode, %{last_tick_lobbies: 0}))}
+      end
     end
     {:reply, reply, st}
+  end
+
+  # mm_queue_quality records of one group -> %{mode => quality fields}; quantiles are bucket upper bounds as for waits
+  defp quality_of(qrecs, group) do
+    for <<mode, g, _::16, n::little-32, max_spread::little-32, max_imb::little-32, sum_spread::little-64,
+          sum_imb::little-64, shist::binary-size(480), ihist::binary-size(480) <- qrecs>>,
+        g == group, into: %{} do
+      mean = fn s -> if n > 0, do: s / n, else: 0.0 end
+      {mode, %{last_tick_lobbies: n, mean_spread: mean.(sum_spread), p50_spread: quantile(shist, 0.5),
+               p99_spread: quantile(shist, 0.99), max_spread: max_spread, mean_imbalance: mean.(sum_imb),
+               p99_imbalance: quantile(ihist, 0.99), max_imbalance: max_imb}}
+    end
   end
 
   def handle_call({:remove_user, id}, _from, st) do

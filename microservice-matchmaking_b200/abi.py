@@ -140,6 +140,33 @@ class QueueStat(C.Structure):
     ]
 
 
+class LobbyQuality(C.Structure):
+    """mm_lobby_quality: rating spread, sum and team imbalance of one lobby of the last tick (24 bytes)."""
+    _fields_ = [
+        ("min_rating", C.c_int32),
+        ("max_rating", C.c_int32),
+        ("rating_sum", C.c_int64),
+        ("imbalance", C.c_uint32),
+        ("reserved", C.c_uint32),
+    ]
+
+
+class QueueQuality(C.Structure):
+    """mm_queue_quality: spread and imbalance of one (mode, group) queue's lobbies of the last tick (992 bytes)."""
+    _fields_ = [
+        ("mode", C.c_uint8),
+        ("group", C.c_uint8),
+        ("reserved", C.c_uint16),
+        ("n_lobbies", C.c_uint32),
+        ("max_spread", C.c_uint32),
+        ("max_imbalance", C.c_uint32),
+        ("sum_spread", C.c_uint64),
+        ("sum_imbalance", C.c_uint64),
+        ("spread_hist", C.c_uint32 * MM_WAIT_BUCKETS),
+        ("imbalance_hist", C.c_uint32 * MM_WAIT_BUCKETS),
+    ]
+
+
 MM_IMAGE_MAGIC = 0x474D494D
 MM_QUEUE_IMAGE_MAGIC = 0x5155514D  # mm_export_queues: same header and sections, no active section
 MM_IMAGE_VERSION = 1
@@ -207,6 +234,7 @@ PROTOTYPES = {
     "mm_results_device": (C.c_int, [_vp, _P(_vp), _P(_vp)]),
     "mm_pool_read": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _P(C.c_uint32)]),
     "mm_queue_stats": (C.c_int, [_vp, C.c_uint64, _vp, C.c_uint32, _P(C.c_uint32)]),
+    "mm_match_quality": (C.c_int, [_vp, _vp, C.c_uint32, _P(C.c_uint32), _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_set_lobby_budget": (C.c_int, [_vp, _vp, _vp]),
     "mm_lobby_budget_report": (C.c_int, [_vp, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_lobby_candidates": (C.c_int, [_vp, _vp, C.c_uint32, _P(C.c_uint32)]),

@@ -25,6 +25,7 @@
 #include "mm_image.cuh"
 #include "mm_kernels.cuh"
 #include "mm_locate.cuh"
+#include "mm_quality.cuh"
 #include "mm_recut.cuh"
 #include "mm_regroup.cuh"
 #include "mm_requeue.cuh"
@@ -290,6 +291,15 @@ struct mm_engine {
     DevArray<mm_player_status> out;
     DevArray<uint32_t> tab;  // pos [Kp + 2] | outbase [Kp + 2] | binlim [Kp + 2] | cand [n_cut] | budgets [n_cut + n_modes] | rmap [n_chunks]
   } loc;
+
+  // mm_match_quality (mm_quality.cuh): allocated by the first call at the capacity's bounds and kept, so a polled call
+  // never allocates; no other call reads or writes them
+  struct Quality {
+    DevArray<uint32_t> w;             // per-bin, per-queue, per-tile and (arrival order) per-lobby / per-team words
+    DevArray<long long> csum;         // [Kp] rating order: per-bin prefix of count x c
+    DevArray<mm_lobby_quality> lob;   // [max_lobbies]
+    DevArray<mm_queue_quality> rec;   // [n_cut]
+  } mq;
 };
 
 namespace {
@@ -2205,6 +2215,72 @@ int locate(mm_engine* e, uint64_t now, uint32_t n, const uint64_t* id, mm_player
   return MM_OK;
 }
 
+// ---- mm_match_quality (mm_quality.cuh) -----------------------------------------------------------------------------
+// The report of a valid last tick with n_lob lobbies (the caller has checked the capacities).
+int match_quality(mm_engine* e, mm_queue_quality* per_queue, mm_lobby_quality* per_lobby, uint32_t n_lob) {
+  auto& s = e->mq;
+  const bool arrival = e->cfg.order_mode == MM_ORDER_ARRIVAL;
+  const uint32_t n_cut = e->n_cut, G = e->cfg.n_groups;
+  const size_t n_tiles = (size_t)e->n_chunks + e->n_segs;
+  // word scratch: cnt [Kp] | qlob [n_cut + 1] | qteam [n_cut + 1] | arrival order: tile offsets [n_tiles] | partition
+  // live counts [n_segs] | scan total [1] | lmin [max_lobbies] | lmax [max_lobbies] | team sums [capacity]
+  const size_t o_qlob = e->Kp, o_qteam = o_qlob + n_cut + 1, o_tile = o_qteam + n_cut + 1, o_part = o_tile + n_tiles,
+               o_tot = o_part + e->n_segs, o_lmin = o_tot + 1, o_lmax = o_lmin + e->max_lobbies,
+               o_tsum = o_lmax + e->max_lobbies;
+  CK(s.w.reserve(arrival ? o_tsum + e->capacity + 64 : o_tile));
+  if (!arrival) CK(s.csum.reserve(e->Kp));
+  CK(s.lob.reserve(e->max_lobbies));
+  CK(s.rec.reserve(n_cut));
+  CK(cudaMemsetAsync(s.rec, 0, (size_t)n_cut * sizeof(mm_queue_quality), e->stream));
+  if (n_lob) {
+    const Pool& p = e->pool[e->cur ^ 1];  // the pool the last tick read
+    MqArgs a{};
+    a.pool = p.v; a.meta = p.m; a.left_bits = e->d_left_bits;
+    a.n_segs = e->n_segs; a.n_cut = n_cut; a.n_groups = G; a.K = e->K; a.key_lo = e->key_lo; a.KR = e->KR;
+    a.bin_key = e->d_bin_key; a.seg_bin_lo = e->d_seg_bin_lo; a.seg_L = e->d_seg_L; a.part_cut = e->d_part_cut;
+    a.cut_lp_lo = e->d_cut_lp_lo; a.mode_tsize = e->d_mode_tsize;
+    a.cnt = s.w; a.csum = arrival ? nullptr : s.csum.p; a.qlob = s.w + o_qlob; a.qteam = s.w + o_qteam;
+    a.lob = s.lob; a.n_lob = n_lob; a.qrec = s.rec;
+    CK(cudaMemsetAsync(a.cnt, 0, (size_t)e->Kp * 4, e->stream));
+    const uint32_t ctas = tile_ctas(e, e->match_n);
+    k_mq_count<kMqBlock><<<ctas, kMqBlock, 0, e->stream>>>(a);
+    k_mq_scan<kMqBlock><<<n_cut, kMqBlock, 0, e->stream>>>(a, !arrival);
+    k_mq_base<kMqBlock><<<1, kMqBlock, 0, e->stream>>>(a);
+    if (arrival) {
+      a.tile_off = s.w + o_tile; a.lmin = s.w + o_lmin; a.lmax = s.w + o_lmax; a.tsum = s.w + o_tsum;
+      // every team holds at least one matched player: the tick's matched count bounds the team-sum words
+      CK(cudaMemsetAsync(a.lmin, 0xFF, (size_t)n_lob * 4, e->stream));
+      CK(cudaMemsetAsync(a.lmax, 0, (size_t)n_lob * 4, e->stream));
+      CK(cudaMemsetAsync(a.tsum, 0, (size_t)e->last.n_matched * 4, e->stream));
+      CK(cudaMemsetAsync(s.w + o_part, 0, ((size_t)e->n_segs + 1) * 4, e->stream));  // partition counts, scan total
+      // live slots per virtual tile -> the live slots before each tile (mm_export's count and scan)
+      ImgExportArgs x{};
+      x.pool = p.v; x.meta = p.m; x.n_segs = e->n_segs; x.tile_cnt = s.w + o_tile; x.part_cnt = s.w + o_part;
+      k_img_tiles<kImgBlock, false><<<ctas, kImgBlock, 0, e->stream>>>(x);
+      k_scan_small<<<1, 1024, 0, e->stream>>>(tile_count(e, e->match_n), s.w + o_tile, s.w + o_tot);
+      k_mq_arrival<kMqBlock><<<ctas, kMqBlock, 0, e->stream>>>(a);
+      k_mq_lobby<true><<<(n_lob + 255) / 256, 256, 0, e->stream>>>(a);
+    } else {
+      k_mq_lobby<false><<<(n_lob + 255) / 256, 256, 0, e->stream>>>(a);
+    }
+    const uint32_t qctas = std::max<uint32_t>(1, std::min<uint32_t>(n_lob / 1024 + 1, 8u * (uint32_t)e->n_sms));
+    k_mq_queue<kMqBlock><<<qctas, kMqBlock, 0, e->stream>>>(a);
+    CK(cudaGetLastError());
+    if (per_lobby) CK(cudaMemcpyAsync(per_lobby, s.lob, (size_t)n_lob * sizeof(mm_lobby_quality), cudaMemcpyDeviceToHost, e->stream));
+  }
+  uint32_t n_dev = 0;  // the lobbies the pool's matched players make up: the tick's own count
+  if (n_lob) CK(cudaMemcpyAsync(&n_dev, s.w + o_qlob + n_cut, 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(per_queue, s.rec, (size_t)n_cut * sizeof(mm_queue_quality), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  for (uint32_t c = 0; c < n_cut; ++c) {
+    per_queue[c].mode = (uint8_t)(c / G);
+    per_queue[c].group = (uint8_t)(c % G);
+  }
+  if (n_dev != n_lob)
+    return set_err(e, MM_E_STATE, "the last tick's pool holds %u matched lobbies, the tick emitted %u", n_dev, n_lob);
+  return MM_OK;
+}
+
 }  // namespace
 
 // =======================================================================================
@@ -2747,6 +2823,23 @@ int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap,
     out[c].n_lobbies = out[c].n_matched / ((uint32_t)md.teams * md.team_size);  // whole lobbies of L players
   }
   return MM_OK;
+}
+
+int mm_match_quality(mm_engine* e, mm_queue_quality* per_queue, uint32_t cap, uint32_t* n_out,
+                     mm_lobby_quality* per_lobby, uint32_t lobby_cap, uint32_t* n_lobbies) {
+  if (!e || !per_queue || !n_out || !n_lobbies) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  const uint32_t n_lob = e->match_valid ? e->last.n_lobbies : 0u;
+  *n_out = e->n_cut;
+  *n_lobbies = n_lob;
+  if (cap < e->n_cut) return set_err(e, MM_E_CAP, "need cap >= %u", e->n_cut);
+  if (per_lobby && lobby_cap < n_lob) return set_err(e, MM_E_CAP, "need lobby_cap >= %u", n_lob);
+  if (!e->match_valid) {  // void: no tick, a failed one, or a pool loaded since (mm_queue_stats' match section)
+    *n_out = 0;
+    return MM_OK;
+  }
+  CK(cudaSetDevice(e->device));
+  return match_quality(e, per_queue, per_lobby, n_lob);
 }
 
 int mm_set_lobby_budget(mm_engine* e, const uint32_t* per_queue, const uint32_t* per_mode) {

@@ -62,6 +62,18 @@ QUEUE_STAT_DTYPE = np.dtype([
     ("match_wait_hist", "<u4", (abi.MM_WAIT_BUCKETS,)),
 ])
 
+# mm_lobby_quality / mm_queue_quality (include/mm_engine.h) as numpy records
+LOBBY_QUALITY_DTYPE = np.dtype([("min_rating", "<i4"), ("max_rating", "<i4"), ("rating_sum", "<i8"),
+                                ("imbalance", "<u4"), ("reserved", "<u4")])
+assert LOBBY_QUALITY_DTYPE.itemsize == C.sizeof(abi.LobbyQuality)
+QUALITY_DTYPE = np.dtype([
+    ("mode", "u1"), ("group", "u1"), ("reserved", "<u2"),
+    ("n_lobbies", "<u4"), ("max_spread", "<u4"), ("max_imbalance", "<u4"), ("sum_spread", "<u8"),
+    ("sum_imbalance", "<u8"), ("spread_hist", "<u4", (abi.MM_WAIT_BUCKETS,)),
+    ("imbalance_hist", "<u4", (abi.MM_WAIT_BUCKETS,)),
+])
+assert QUALITY_DTYPE.itemsize == C.sizeof(abi.QueueQuality)
+
 
 def wait_of(now, enq_ts):
     """Wait of a player as mm_queue_stats counts it: (now - enq_ts) mod 2^32 read as a signed 32-bit value, negative
@@ -77,6 +89,14 @@ def wait_bucket(w):
     w = np.asarray(w, np.int64)
     e = np.maximum(np.frexp(w.astype(np.float64))[1] - 1, 3)  # floor(log2 w), exact for integers below 2^53
     b = np.where(w < 8, w, 8 + 4 * (e - 3) + ((w >> (e - 2)) & 3))
+    return b if b.ndim else int(b)
+
+
+def quality_bucket(v):
+    """Histogram bucket of a spread or imbalance in rating points (mm_match_quality): wait_bucket's, with every value
+    of 2^31 or more in the last bucket."""
+    v = np.asarray(v, np.int64)
+    b = np.where(v >= 1 << 31, abi.MM_WAIT_BUCKETS - 1, wait_bucket(np.minimum(v, (1 << 31) - 1)))
     return b if b.ndim else int(b)
 
 
@@ -474,6 +494,24 @@ class Engine:
         self._check(self.lib.mm_queue_stats(self.h, int(now) & 0xFFFFFFFFFFFFFFFF, _p(out), cap, C.byref(n)),
                     "mm_queue_stats")
         return out[:n.value]
+
+    def match_quality(self, want_lobbies=False):
+        """Rating spread and team imbalance of the last tick's lobbies (mm_match_quality) -> (QUALITY_DTYPE[n_modes *
+        n_groups] in queue_stats() record order, LOBBY_QUALITY_DTYPE[n_lobbies] in the tick's lobby order, or None
+        without want_lobbies).  Both are empty when the report is void (no tick yet, a failed tick, a pool loaded
+        since)."""
+        cap = self.cfg.n_modes * self.cfg.n_groups
+        lobby_cap = 1 << 12 if want_lobbies else 0  # resized from the count of an MM_E_CAP refusal
+        n, nl = C.c_uint32(0), C.c_uint32(0)
+        while True:
+            out = np.zeros(cap, QUALITY_DTYPE)
+            lob = np.zeros(lobby_cap, LOBBY_QUALITY_DTYPE) if want_lobbies else None
+            rc = self.lib.mm_match_quality(self.h, _p(out), cap, C.byref(n), _p(lob), lobby_cap, C.byref(nl))
+            if rc == abi.MM_E_CAP and (n.value > cap or (want_lobbies and nl.value > lobby_cap)):
+                cap, lobby_cap = max(cap, n.value), max(lobby_cap, nl.value)
+                continue
+            self._check(rc, "mm_match_quality")
+            return out[:n.value], (lob[:nl.value] if want_lobbies else None)
 
     # -- lobby budget ----------------------------------------------------------------
     def set_lobby_budget(self, per_queue=None, per_mode=None):

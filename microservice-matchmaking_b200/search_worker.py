@@ -692,6 +692,32 @@ class SearchPool:
             }
         return out
 
+    def match_quality(self, group_name):
+        """How even the last tick's lobbies of one rating group are (Engine.match_quality), per mode name: lobbies, the
+        mean / p50 / p99 / max rating spread and the mean / p99 / max team imbalance, in rating points.  Quantiles are
+        the upper bounds of histogram buckets (at most 25 % high).  {} for a group the pool does not know, and while
+        the report is void (before the first tick, after a failed one, after a restore or an import)."""
+        from .engine import wait_quantile
+        if group_name not in self.group_names:
+            return {}
+        g = self.group_names.index(group_name)
+        out = {}
+        for r in self.engine.match_quality()[0]:
+            if int(r["group"]) != g or int(r["mode"]) >= len(self.mode_names):
+                continue
+            n = int(r["n_lobbies"])
+            out[self.mode_names[int(r["mode"])]] = {
+                "lobbies": n,
+                "mean_spread": int(r["sum_spread"]) / n if n else 0.0,
+                "p50_spread": wait_quantile(r["spread_hist"], 0.50),
+                "p99_spread": wait_quantile(r["spread_hist"], 0.99),
+                "max_spread": int(r["max_spread"]),
+                "mean_imbalance": int(r["sum_imbalance"]) / n if n else 0.0,
+                "p99_imbalance": wait_quantile(r["imbalance_hist"], 0.99),
+                "max_imbalance": int(r["max_imbalance"]),
+            }
+        return out
+
 
 class SearchWorker:
     """Matchmaking.Search.Worker — one consumer of `matchmaking.queues.<group>`."""
@@ -737,6 +763,8 @@ class SearchWorker:
         st["pool"] = self.pool.engine.status() if hasattr(self.pool.engine, "status") else {}
         if hasattr(self.pool.engine, "queue_stats"):  # this worker's own group, per mode (the reference's queue depth)
             st["waiting"] = self.pool.queue_status(self.group_name)
+        if hasattr(self.pool.engine, "match_quality"):  # how even this group's lobbies of the last tick are, per mode
+            st["quality"] = self.pool.match_quality(self.group_name)
         if hasattr(self.pool.engine, "lobby_budget_report"):  # lobbies the last tick's budget held back, per mode
             st["held_back"] = self.pool.held_back(self.group_name)
         return ("ok", st)
