@@ -114,20 +114,12 @@ __global__ void __launch_bounds__(kBfPlanWarps * 32) k_bf_plan(const BfArgs a) {
       __syncwarp();
       uint32_t bin = 0, v = 0;
       if (lane < nv) { bin = s_bin[warp][lane]; v = a.rem[bin]; }
-      uint32_t incl = v;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-        if (lane >= (uint32_t)o) incl += u;
-      }
+      const uint32_t incl = warp_incl_scan(v);
       const uint32_t excl = incl - v, before = min(excl, need), take = min(v, need - before);
-      const uint32_t mine = take ? 1u << lane : 0u, pb = __ballot_sync(0xFFFFFFFFu, take != 0);
-      uint32_t base = 0;
-      if (pb && lane == 0) base = atomicAdd(&a.ctr[kBfPieces], (uint32_t)__popc(pb));
-      base = __shfl_sync(0xFFFFFFFFu, base, 0);
+      const uint32_t at = warp_append(&a.ctr[kBfPieces], take != 0);
       if (take) {
         const uint32_t t = a.tot[bin];
-        a.piece[base + __popc(pb & (mine - 1))] = BfPiece{r.idx, bin, t - v, take, got + before};
+        a.piece[at] = BfPiece{r.idx, bin, t - v, take, got + before};
         a.rem[bin] = v - take;
       }
       const uint32_t sum = __shfl_sync(0xFFFFFFFFu, incl, 31);

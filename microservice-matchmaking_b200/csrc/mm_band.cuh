@@ -92,11 +92,10 @@ template <class KeyBins>
 __global__ void __launch_bounds__(kBandPrepBlock) k_band_prep(const BandArgs a, const KeyBins kb) {
   __shared__ uint32_t s_sel[kMaxSegs];
   __shared__ uint32_t s_tmp[33];
-  __shared__ uint32_t s_carry;
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t tid = threadIdx.x;
   for (uint32_t p = tid; p < a.n_segs; p += kBandPrepBlock) s_sel[p] = 0;
-  if (tid == 0) s_carry = 0;
   __syncthreads();
+  uint32_t carry = 0;
   for (uint32_t q0 = 0; q0 < a.n_keys; q0 += kBandPrepBlock) {  // a running exclusive scan of the column lengths
     const uint32_t q = q0 + tid;
     uint32_t tiles = 0;
@@ -112,32 +111,10 @@ __global__ void __launch_bounds__(kBandPrepBlock) k_band_prep(const BandArgs a, 
       }
       a.qtiles[q] = tiles;
     }
-    uint32_t incl = tiles;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-      if (lane >= (uint32_t)off) incl += v;
-    }
-    if (lane == 31) s_tmp[warp] = incl;
-    __syncthreads();
-    if (warp == 0) {
-      const uint32_t w = lane < kBandPrepBlock / 32 ? s_tmp[lane] : 0u;
-      uint32_t wi = w;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, wi, off);
-        if (lane >= (uint32_t)off) wi += v;
-      }
-      s_tmp[lane] = wi - w;
-      if (lane == 31) s_tmp[32] = wi;
-    }
-    __syncthreads();
-    if (q < a.n_keys) a.qoff[q] = s_carry + s_tmp[warp] + incl - tiles;
-    __syncthreads();
-    if (tid == 0) s_carry += s_tmp[32];
-    __syncthreads();
+    const uint32_t off = block_scan_step<kBandPrepBlock>(tiles, carry, s_tmp);
+    if (q < a.n_keys) a.qoff[q] = off;
   }
-  if (tid == 0) a.qoff[a.n_keys] = s_carry;
+  if (tid == 0) a.qoff[a.n_keys] = carry;
   for (uint32_t p = tid; p < a.n_segs; p += kBandPrepBlock) a.bfill[p] = s_sel[p] ? __ldcg(&a.fill[p]) : 0u;
 }
 
@@ -181,22 +158,9 @@ __global__ void __launch_bounds__(BLOCK) k_band_count(const BandArgs a) {
 __global__ void __launch_bounds__(256) k_band_scan(const BandArgs a) {
   const uint32_t lane = threadIdx.x & 31, q = blockIdx.x * 8 + (threadIdx.x >> 5);
   if (q >= a.n_keys) return;
-  const uint32_t n = a.qtiles[q];
   uint32_t* col = a.M + a.qoff[q];
-  uint32_t carry = 0;
-  for (uint32_t i0 = 0; i0 < n; i0 += 32) {
-    const uint32_t i = i0 + lane;
-    const uint32_t v = i < n ? col[i] : 0u;
-    uint32_t incl = v;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-      if (lane >= (uint32_t)off) incl += u;
-    }
-    if (i < n) col[i] = carry + incl - v;
-    carry += __shfl_sync(0xFFFFFFFFu, incl, 31);
-  }
-  if (lane == 0) a.tot[q] = carry;
+  const uint32_t total = warp_col_scan(col, col, a.qtiles[q]);
+  if (lane == 0) a.tot[q] = total;
 }
 
 // One CTA, once klim is known: the last tile of its partition that holds one of key q's first min(klim, tot) players
@@ -211,10 +175,8 @@ __global__ void __launch_bounds__(kBandPrepBlock) k_band_limit(const BandArgs a)
   for (uint32_t q = tid; q < a.n_keys; q += kBandPrepBlock) {
     const uint32_t n = a.qtiles[q], lim = min(a.klim[q], a.tot[q]);
     if (n == 0 || lim == 0) continue;
-    const uint32_t* col = a.M + a.qoff[q];
-    uint32_t lo = 0, hi = n;  // col[lo] < lim <= col[hi] (col[n] read as the total)
-    while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (col[mid] < lim) lo = mid; else hi = mid; }
-    atomicMax(&s_lim[a.qseg[q]], lo + 1);
+    // the last tile with col[t] < lim (col[0] = 0 < lim)
+    atomicMax(&s_lim[a.qseg[q]], last_le(a.M + a.qoff[q], 0, n, lim - 1) + 1);
   }
   __syncthreads();
   for (uint32_t p = tid; p < a.n_segs; p += kBandPrepBlock) a.bfill[p] = min(a.bfill[p], s_lim[p] * kTile);
@@ -256,41 +218,16 @@ struct BandKeys {
 __global__ void __launch_bounds__(kBandWalkBlock) k_band_bases(const BandArgs a, uint32_t match) {
   __shared__ uint32_t s_tmp[33];
   __shared__ uint32_t s_bm[kMaxSegs + 1], s_bl[kMaxSegs + 1];
-  __shared__ uint32_t s_carry;
   constexpr uint32_t NW = kBandWalkBlock / 32;
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   if (!match) {
-    if (tid == 0) s_carry = 0;
-    __syncthreads();
+    uint32_t carry = 0;
     for (uint32_t q0 = 0; q0 < a.n_keys; q0 += kBandWalkBlock) {
       const uint32_t q = q0 + tid;
-      const uint32_t v = q < a.n_keys ? a.tot[q] : 0u;
-      uint32_t incl = v;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-        if (lane >= (uint32_t)off) incl += u;
-      }
-      if (lane == 31) s_tmp[warp] = incl;
-      __syncthreads();
-      if (warp == 0) {
-        const uint32_t w = lane < NW ? s_tmp[lane] : 0u;
-        uint32_t wi = w;
-#pragma unroll
-        for (int off = 1; off < 32; off <<= 1) {
-          const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, wi, off);
-          if (lane >= (uint32_t)off) wi += u;
-        }
-        s_tmp[lane] = wi - w;
-        if (lane == 31) s_tmp[32] = wi;
-      }
-      __syncthreads();
-      if (q < a.n_keys) { a.kbase[q] = s_carry + s_tmp[warp] + incl - v; a.klim[q] = kBandNone; }
-      __syncthreads();
-      if (tid == 0) s_carry += s_tmp[32];
-      __syncthreads();
+      const uint32_t base = block_scan_step<kBandWalkBlock>(q < a.n_keys ? a.tot[q] : 0u, carry, s_tmp);
+      if (q < a.n_keys) { a.kbase[q] = base; a.klim[q] = kBandNone; }
     }
-    if (tid == 0) a.ctr[kBcKeys] = s_carry;
+    if (tid == 0) a.ctr[kBcKeys] = carry;
     return;
   }
   const uint32_t twoW = 2u * (uint32_t)a.W, nb = a.n_bands;
@@ -298,20 +235,8 @@ __global__ void __launch_bounds__(kBandWalkBlock) k_band_bases(const BandArgs a,
   for (uint32_t b = warp; b < nb; b += NW) {
     const uint32_t q0 = b * twoW, L = a.L[b % a.n_modes], Mrec = 0xFFFFFFFFu / L;
     uint32_t* bb = a.pos + b * (twoW + 1);
-    uint32_t carry = 0;
-    for (uint32_t off = 0; off < twoW; off += 32) {  // sorted positions inside the band
-      const uint32_t v = off + lane;
-      const uint32_t c = v < twoW ? a.tot[q0 + v] : 0u;
-      uint32_t incl = c;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-        if (lane >= (uint32_t)o) incl += u;
-      }
-      if (v < twoW) bb[v] = carry + incl - c;
-      carry += __shfl_sync(0xFFFFFFFFu, incl, 31);
-    }
-    if (lane == 0) bb[twoW] = carry;
+    const uint32_t n_band = warp_col_scan(a.tot + q0, bb, twoW);  // sorted positions inside the band
+    if (lane == 0) bb[twoW] = n_band;
     __syncwarp();
     const bool remote_band = a.remote_last && b / a.n_modes + 1 == nb / a.n_modes;
     uint32_t wpos = 0, mcarry = 0;
@@ -326,12 +251,7 @@ __global__ void __launch_bounds__(kBandWalkBlock) k_band_bases(const BandArgs a,
         const uint32_t m = s1_step(wpos, B0, B1, RS, L, Mrec);
         if ((int)lane == l) mine = m;
       }
-      uint32_t incl = mine;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, incl, o);
-        if (lane >= (uint32_t)o) incl += u;
-      }
+      const uint32_t incl = warp_incl_scan(mine);
       if (valid) { a.klim[q0 + v] = mine; a.kbase[q0 + v] = mcarry + incl - mine; }  // relative to the band for now
       if (valid && remote_band && v >= (uint32_t)a.W) upper += mine;
       mcarry += __shfl_sync(0xFFFFFFFFu, incl, 31);
@@ -346,12 +266,7 @@ __global__ void __launch_bounds__(kBandWalkBlock) k_band_bases(const BandArgs a,
     for (uint32_t b0 = 0; b0 < nb; b0 += 32) {
       const uint32_t b = b0 + lane;
       const uint32_t m = b < nb ? s_bm[b] : 0u, l = b < nb ? m / a.L[b % a.n_modes] : 0u;
-      uint32_t im = m, il = l;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, im, o), w = __shfl_up_sync(0xFFFFFFFFu, il, o);
-        if (lane >= (uint32_t)o) { im += u; il += w; }
-      }
+      const uint32_t im = warp_incl_scan(m), il = warp_incl_scan(l);
       if (b < nb) { s_bm[b] = cm + im - m; s_bl[b] = cl + il - l; }
       cm += __shfl_sync(0xFFFFFFFFu, im, 31);
       cl += __shfl_sync(0xFFFFFFFFu, il, 31);
@@ -397,12 +312,7 @@ __global__ void __launch_bounds__(BLOCK) k_band_place(const BandArgs a, const Ba
       uint32_t cnt = 0;
 #pragma unroll
       for (int k = 0; k < 8; ++k) cnt += q[k] != kBandNone;
-      uint32_t incl = cnt;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const uint32_t u = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-        if (lane >= (uint32_t)off) incl += u;
-      }
+      const uint32_t incl = warp_incl_scan(cnt);
       const uint32_t n = __shfl_sync(0xFFFFFFFFu, incl, 31);
       if (n == 0) continue;
       uint32_t w = incl - cnt;
@@ -457,8 +367,7 @@ __global__ void k_band_upper_place(const BandArgs a, uint32_t n, const uint64_t*
 __global__ void k_band_hdr(const BandArgs a, uint32_t n_lobbies, mm_lobby_hdr* __restrict__ hdr) {
   const uint32_t k = blockIdx.x * blockDim.x + threadIdx.x;
   if (k >= n_lobbies) return;
-  uint32_t lo = 0, hi = a.n_bands;  // last band with band_lb <= k
-  while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (a.band_lb[mid] <= k) lo = mid; else hi = mid; }
+  const uint32_t lo = last_le(a.band_lb, 0, a.n_bands, k);
   const uint32_t m = lo % a.n_modes, L = a.L[m];
   mm_lobby_hdr h;
   h.first_member = a.band_mb[lo] + (k - a.band_lb[lo]) * L;

@@ -263,6 +263,160 @@ __device__ __forceinline__ uint32_t block_excl_scan(uint32_t* a, uint32_t n, uin
   return total;
 }
 
+// ---- scans, searches and cursors of the off-tick kernels (DESIGN §4) ------------------------------------------------
+__device__ __forceinline__ uint32_t shfl_up(uint32_t v, int off) { return __shfl_up_sync(0xFFFFFFFFu, v, off); }
+__device__ __forceinline__ long long shfl_up(long long v, int off) { return __shfl_up_sync(0xFFFFFFFFu, v, off); }
+struct Plus {
+  template <class T>
+  __device__ __forceinline__ T operator()(const T& a, const T& b) const { return a + b; }
+};
+
+// Inclusive scan over the lanes of a warp, op(earlier, later).  A value type needs an shfl_up overload.
+template <class T, class Op = Plus>
+__device__ __forceinline__ T warp_incl_scan(T x, Op op = Op()) {
+  const uint32_t lane = threadIdx.x & 31;
+#pragma unroll
+  for (int off = 1; off < 32; off <<= 1) {
+    const T y = shfl_up(x, off);
+    if (lane >= (uint32_t)off) x = op(y, x);
+  }
+  return x;
+}
+
+// One warp: exclusive scan of in[0..n) into out[0..n) (in == out is fine); returns the total.
+__device__ __forceinline__ uint32_t warp_col_scan(const uint32_t* in, uint32_t* out, uint32_t n) {
+  const uint32_t lane = threadIdx.x & 31;
+  uint32_t carry = 0;
+  for (uint32_t i0 = 0; i0 < n; i0 += 32) {
+    const uint32_t i = i0 + lane;
+    const uint32_t v = i < n ? in[i] : 0u;
+    const uint32_t incl = warp_incl_scan(v);
+    if (i < n) out[i] = carry + incl - v;
+    carry += __shfl_sync(0xFFFFFFFFu, incl, 31);
+  }
+  return carry;
+}
+
+// One step of a running exclusive scan of an array longer than the CTA: thread t gives element t of the step.  Returns
+// carry + the elements before it and adds the step's total to carry (every thread's copy).  s_tmp: BLOCK / 32 + 1.
+template <int BLOCK, class T>
+__device__ __forceinline__ T block_scan_step(const T v, T& carry, T* s_tmp) {
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const T incl = warp_incl_scan(v);
+  if (lane == 31) s_tmp[warp] = incl;
+  __syncthreads();
+  if (warp == 0) {
+    const T w = lane < BLOCK / 32 ? s_tmp[lane] : T{};
+    const T wi = warp_incl_scan(w);
+    if (lane < BLOCK / 32) s_tmp[lane] = wi - w;
+    if (lane == 31) s_tmp[BLOCK / 32] = wi;
+  }
+  __syncthreads();
+  const T r = carry + s_tmp[warp] + incl - v;
+  carry = carry + s_tmp[BLOCK / 32];
+  __syncthreads();  // s_tmp is rewritten by the next step
+  return r;
+}
+
+// CTA offsets of per-thread counts: lane 31's warp_total is its warp's count.  Returns the counts of the warps before
+// this thread's; total = the CTA's.  s_warp: BLOCK / 32 words, free again when it returns.
+template <int BLOCK>
+__device__ __forceinline__ uint32_t block_warp_offsets(uint32_t warp_total, uint32_t& total, uint32_t* s_warp) {
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 31) s_warp[warp] = warp_total;
+  __syncthreads();
+  uint32_t before = 0;
+  total = 0;
+#pragma unroll
+  for (int w = 0; w < BLOCK / 32; ++w) {
+    const uint32_t v = s_warp[w];
+    before += (uint32_t)w < warp ? v : 0u;
+    total += v;
+  }
+  __syncthreads();
+  return before;
+}
+
+// Exclusive scan of one value per thread over a CTA of BLOCK threads, op(earlier, later), id the identity.
+// s_warp: BLOCK / 32 values, free again when it returns.
+template <int BLOCK, class T, class Op>
+__device__ __forceinline__ T block_excl_scan_op(T x, T id, Op op, T* s_warp) {
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  const T in = warp_incl_scan(x, op);
+  if (lane == 31) s_warp[warp] = in;
+  __syncthreads();
+  if (warp == 0) {
+    const T w = warp_incl_scan(lane < BLOCK / 32 ? s_warp[lane] : id, op);
+    if (lane < BLOCK / 32) s_warp[lane] = w;  // inclusive over the warps
+  }
+  __syncthreads();
+  T ex = shfl_up(in, 1);
+  if (lane == 0) ex = id;
+  const T r = warp ? op(s_warp[warp - 1], ex) : ex;
+  __syncthreads();
+  return r;
+}
+
+// The last i in [lo, hi) with off[i] <= x (off ascending, off[lo] <= x; equal entries resolve to the last).
+__device__ __forceinline__ uint32_t last_le(const uint32_t* off, uint32_t lo, uint32_t hi, uint32_t x) {
+  while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (off[mid] <= x) lo = mid; else hi = mid; }
+  return lo;
+}
+// The first i in [l, r) where pred(i) stops holding (pred true on a prefix of the range), r when it always holds.
+template <class Pred>
+__device__ __forceinline__ uint32_t first_not(uint32_t l, uint32_t r, Pred pred) {
+  while (l < r) { const uint32_t mid = (l + r) >> 1; if (pred(mid)) l = mid + 1; else r = mid; }
+  return l;
+}
+
+// Warp-aggregated output cursor: every lane asks for k slots and gets the first of them; one atomicAdd on *ctr per
+// warp, none when the warp asks for nothing.  All 32 lanes call it.
+__device__ __forceinline__ uint32_t warp_append(uint32_t* ctr, uint32_t k) {
+  const uint32_t incl = warp_incl_scan(k), total = __shfl_sync(0xFFFFFFFFu, incl, 31);
+  uint32_t base = 0;
+  if ((threadIdx.x & 31) == 31 && total) base = atomicAdd(ctr, total);
+  return __shfl_sync(0xFFFFFFFFu, base, 31) + incl - k;
+}
+// The same cursor for at most one slot per lane: a ballot in place of the scan.
+__device__ __forceinline__ uint32_t warp_append(uint32_t* ctr, bool want) {
+  const uint32_t lane = threadIdx.x & 31, b = __ballot_sync(0xFFFFFFFFu, want);
+  uint32_t base = 0;
+  if (lane == 0 && b) base = atomicAdd(ctr, (uint32_t)__popc(b));
+  return __shfl_sync(0xFFFFFFFFu, base, 0) + __popc(b & ((1u << lane) - 1u));
+}
+// Warp-aggregated histogram add of every lane's 8 keys: one atomic per distinct key of each slot, one in all when the
+// warp's 256 keys are equal.  Key `none` counts nowhere.
+__device__ __forceinline__ void warp_hist8_add(uint32_t* hist, const uint32_t (&b)[8], uint32_t none) {
+  const uint32_t lane = threadIdx.x & 31, b0 = __shfl_sync(0xFFFFFFFFu, b[0], 0);
+  bool same = true;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) same &= b[j] == b0;
+  if (__all_sync(0xFFFFFFFFu, same)) {
+    if (lane == 0 && b0 != none) atomicAdd(&hist[b0], 8u * 32u);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const uint32_t m = __match_any_sync(0xFFFFFFFFu, b[j]);
+      if (b[j] != none && lane == (uint32_t)(__ffs(m) - 1)) atomicAdd(&hist[b[j]], (uint32_t)__popc(m));
+    }
+  }
+}
+
+// Scratch id set of mask + 1 keys (kEmptyKey-filled, at most half full): true for the first copy of pid to arrive.
+__device__ __forceinline__ bool seen_insert(unsigned long long* seen, uint64_t mask, uint64_t pid) {
+  for (uint64_t s = hash64(pid) & mask;; s = (s + 1) & mask) {
+    const unsigned long long k = atomicCAS(&seen[s], kEmptyKey, (unsigned long long)pid);
+    if (k == kEmptyKey) return true;
+    if (k == pid) return false;
+  }
+}
+
+// A rating's clamp key: the rating clamped into [key_lo, key_lo + KR), minus key_lo.
+__device__ __forceinline__ uint32_t clamp_key(int32_t key_lo, uint32_t KR, int32_t r) {
+  const int32_t hi = key_lo + (int32_t)KR - 1;
+  return (uint32_t)((r < key_lo ? key_lo : (r > hi ? hi : r)) - key_lo);
+}
+
 // Every CTA derives the tick's tile geometry from the partition fills (n_segs <= 512 values: one block scan).
 template <int BLOCK>
 __device__ __forceinline__ void geo_build(Geo& g, const uint32_t* __restrict__ fill, uint32_t n_segs, uint32_t R,
@@ -319,6 +473,31 @@ __device__ __forceinline__ void desc_fill(DescCache& c, const Geo& g, const Pool
       c.nvsg[k] = d.nvalid | (d.seg << 16);
     }
 }
+// Off-tick pool walks: the grid's CTAs are the rows, and a CTA takes the run [s0, s1) of the virtual tile sequence;
+// false (uniform) when its run is empty.
+template <int BLOCK>
+__device__ __forceinline__ bool geo_cta_run(Geo& g, const uint32_t* fill, uint32_t n_segs, uint32_t* s_tmp,
+                                            uint32_t& s0, uint32_t& s1) {
+  geo_build<BLOCK>(g, fill, n_segs, gridDim.x, s_tmp);
+  s0 = blockIdx.x * g.tpr;
+  if (s0 >= g.NT) return false;
+  s1 = s0 + g.tpr < g.NT ? s0 + g.tpr : g.NT;
+  return true;
+}
+// A thread's 8 slots [o, o + 8) of a walk (o = 8 tid): byte j of their packed mode bytes, and their streamed stamps or
+// bins (8-aligned, one or two 16-byte loads).
+__device__ __forceinline__ uint32_t mode8_at(uint2 m2, int j) { return ((j < 4 ? m2.x : m2.y) >> (8 * (j & 3))) & 0xFFu; }
+__device__ __forceinline__ void ld_stamps8(const uint32_t* p, uint32_t v[8]) {
+  const uint4 t0 = __ldcs(reinterpret_cast<const uint4*>(p)), t1 = __ldcs(reinterpret_cast<const uint4*>(p) + 1);
+  v[0] = t0.x; v[1] = t0.y; v[2] = t0.z; v[3] = t0.w; v[4] = t1.x; v[5] = t1.y; v[6] = t1.z; v[7] = t1.w;
+}
+__device__ __forceinline__ void ld_bins8(const uint16_t* p, uint32_t v[8]) {
+  const uint4 b = __ldcs(reinterpret_cast<const uint4*>(p));
+  const uint32_t w[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+  for (int j = 0; j < 8; ++j) v[j] = (w[j >> 1] >> (16 * (j & 1))) & 0xFFFFu;
+}
+
 // Row prefixes of the histogram matrix: with few rows per partition (R rows over tens of partitions) every row sums
 // the rows before it on the fly; only when a partition spans many rows (one rating group over the whole pool) is the
 // column-scan phase (and its grid barrier) worth it.  Uniform: every CTA derives the same answer from the geometry.

@@ -1001,6 +1001,20 @@ int tick_to_host(mm_engine* e, mm_lobby_hdr* lobbies, uint32_t lobby_cap, uint64
 // The virtual tiles of a pool of n players (an upper bound: the host-side player count bounds them), and the CTAs of a
 // tile walk over them: at most the tiles, at most 8 per SM; each CTA takes a contiguous run of tiles.
 uint32_t tile_count(const mm_engine* e, uint32_t n) { return n / kTile + e->n_segs; }
+// 1-D grid of 256-thread CTAs over n items: at most per_sm CTAs per SM, one at least.
+uint32_t grid256(const mm_engine* e, uint64_t n, uint32_t per_sm) {
+  return (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n + 255) / 256, (uint64_t)per_sm * (uint32_t)e->n_sms));
+}
+// Keys of the scratch id set (seen_insert) for n ids: a power of two, at least 1024, at most half full.
+uint64_t seen_keys(uint64_t n) {
+  uint64_t sc = 1024;
+  while (sc < 2 * n) sc <<= 1;
+  return sc;
+}
+// The refusal of every call that reads or rewrites the pool while a packed batch is staged.
+int staged_err(mm_engine* e) {
+  return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+}
 uint32_t tile_ctas(const mm_engine* e, uint32_t n) {
   return std::max<uint32_t>(1, std::min<uint32_t>(tile_count(e, n), 8u * (uint32_t)e->n_sms));
 }
@@ -1117,7 +1131,7 @@ int count_tiles(mm_engine* e, bool sel, ImgExportArgs& a) {
 // mm_export (queues = null) and mm_export_queues (queues: n_cut selection bytes; the image has no active section, and
 // a call that writes it releases the exported players through k_expire with the same selection and max_wait = 0)
 int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes, const uint8_t* queues) {
-  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (e->stage_count) return staged_err(e);
   const Pool& p = e->pool[e->cur];
   const uint32_t idb = id_bytes(e);
   int rc;
@@ -1131,7 +1145,7 @@ int export_image(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes, const
   if (e->use_active && act_cap) {
     CK(e->d_img_act.reserve((size_t)act_cap * idb));
     const uint64_t n_tab = e->hcap;
-    const uint32_t nb = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((n_tab + 255) / 256, 16ull * (uint32_t)e->n_sms));
+    const uint32_t nb = grid256(e, n_tab, 16);
     k_img_active<<<nb, 256, 0, e->stream>>>(act_view(e), n_tab, p.v.mode, (uint32_t)pool_slots(e), e->gen, e->d_img_act,
                                             idb, act_cap, &e->d_cnt->img_active);
   }
@@ -1271,6 +1285,18 @@ int load_fits(mm_engine* e, uint64_t n, uint64_t m) {
 // ids of the active section at `act`.  Every partition goes on consecutive chunks, in partition order; k_img_load
 // checks every player under the engine's layout while it writes it, k_img_insert refuses a repeated id, and a failed
 // check leaves the engine empty and fresh.
+// k_img_load's arguments: n players of `in` into pool p, partition s's first at part_off[s], laid out from slot_base[s].
+ImgLoadArgs load_args(mm_engine* e, const Pool& p, const ImgCols& in, uint32_t n, const uint32_t* part_off,
+                      const uint32_t* slot_base, uint32_t seq_next) {
+  ImgLoadArgs la{};
+  la.pool = p.v; la.meta = p.m; la.in = in; la.n = n; la.n_segs = e->n_segs;
+  la.part_off = part_off; la.slot_base = slot_base;
+  la.bm = bin_map(e); la.grp_lut = e->d_grp_lut; la.bin_seg = e->d_bin_seg; la.seg_bin_lo = e->d_seg_bin_lo;
+  la.mode_tsize = e->d_mode_tsize; la.n_modes = e->cfg.n_modes; la.seq_next = seq_next; la.id_limit = id_limit(e);
+  la.err = &e->d_cnt->img_err;
+  return la;
+}
+
 int load_columns(mm_engine* e, const std::vector<uint32_t>& cnt, const ImgCols& cols, uint32_t n, const void* act,
                  uint32_t m, uint32_t seq_next, const char* prefix) {
   std::vector<uint32_t> tab((size_t)e->n_segs * e->n_chunks, 0), off_base(2 * (size_t)e->n_segs + 1);
@@ -1293,21 +1319,15 @@ int load_columns(mm_engine* e, const std::vector<uint32_t>& cnt, const ImgCols& 
   CK(cudaMemcpyAsync(p.m.bump, &chunk, 4, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(e->d_img_part, off_base.data(), off_base.size() * 4, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemsetAsync(&e->d_cnt->img_err, 0, 4, e->stream));
-  const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((n + 255) / 256, 32u * (uint32_t)e->n_sms));
-  if (n) {
-    ImgLoadArgs la{};
-    la.pool = p.v; la.meta = p.m; la.in = cols; la.n = n; la.n_segs = e->n_segs;
-    la.part_off = e->d_img_part; la.slot_base = e->d_img_part + e->n_segs + 1;
-    la.bm = bin_map(e); la.grp_lut = e->d_grp_lut; la.bin_seg = e->d_bin_seg; la.seg_bin_lo = e->d_seg_bin_lo;
-    la.mode_tsize = e->d_mode_tsize; la.n_modes = e->cfg.n_modes; la.seq_next = seq_next; la.id_limit = id_limit(e);
-    la.err = &e->d_cnt->img_err;
-    k_img_load<<<grid, 256, 0, e->stream>>>(la);
-  }
+  const uint32_t grid = grid256(e, n, 32);
+  if (n)
+    k_img_load<<<grid, 256, 0, e->stream>>>(
+        load_args(e, p, cols, n, e->d_img_part, e->d_img_part + e->n_segs + 1, seq_next));
   if (e->use_active) {
     const ActiveView av = act_view(e);
     if (n) k_img_insert<<<grid, 256, 0, e->stream>>>(cols.id, cols.id_bytes, n, id_limit(e), av, &e->d_cnt->img_err);
     if (m) {
-      const uint32_t g2 = std::max<uint32_t>(1, std::min<uint32_t>((m + 255) / 256, 32u * (uint32_t)e->n_sms));
+      const uint32_t g2 = grid256(e, m, 32);
       k_img_insert<<<g2, 256, 0, e->stream>>>(act, cols.id_bytes, m, id_limit(e), av, &e->d_cnt->img_err);
     }
   }
@@ -1364,7 +1384,7 @@ int count_live(mm_engine* e, std::vector<uint32_t>& per_part) {
 // the capacities and the reject list's size), then one ingest batch through enq_prepare / enq_chunk / enq_finish with
 // its codes in d_mrg_code, so that mm_enqueue_rejects still reads the last mm_enqueue* batch.
 int merge_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uint32_t* rejected, uint32_t* n_rejected) {
-  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (e->stage_count) return staged_err(e);
   mm_image_header h;
   ImgLayout l;
   std::vector<uint32_t> cnt;
@@ -1397,7 +1417,7 @@ int merge_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uin
   CK(cudaMemcpyAsync(e->d_img, buf + l.off[1], body, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(e->d_img_part, off.data(), off.size() * 4, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemsetAsync(&e->d_cnt->img_err, 0, 2 * 4, e->stream));  // img_err, mrg_dups
-  const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((n + 255) / 256, 32u * (uint32_t)e->n_sms));
+  const uint32_t grid = grid256(e, n, 32);
   MrgOrderArgs oa{};
   oa.in = img_cols(e->d_img, l, h.id_bytes); oa.n = n; oa.n_segs = e->n_segs; oa.part_off = e->d_img_part;
   oa.part_cut = e->d_part_cut; oa.cut_lp_lo = e->d_cut_lp_lo; oa.bm = bin_map(e); oa.grp_lut = e->d_grp_lut;
@@ -1411,8 +1431,7 @@ int merge_image(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t cap, uin
   const bool hashed = e->use_active && !e->dense_ids;
   const bool tight = (uint64_t)p.n + p.held + n > e->capacity || (hashed && (e->n_active + n) * 4 > e->hcap * 3);
   if (e->use_active && (cap < n || tight)) {
-    uint64_t sc = 1024;
-    while (sc < 2ull * n) sc <<= 1;
+    const uint64_t sc = seen_keys(n);
     CK(e->d_mrg_seen.reserve(sc));
     CK(cudaMemsetAsync(e->d_mrg_seen, 0xFF, sc * 8, e->stream));
     k_mrg_dups<<<grid, 256, 0, e->stream>>>(e->d_in_id, n, act_view(e), e->d_mrg_seen, sc - 1, &e->d_cnt->mrg_dups);
@@ -1515,14 +1534,13 @@ int requeue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating,
             const uint32_t* seq, uint8_t* codes, uint32_t* n_requeued) {
   if (!e->use_active)
     return set_err(e, MM_E_STATE, "requeue needs the active set: an MM_F_NO_DEDUPE engine cannot tell matched from gone");
-  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (e->stage_count) return staged_err(e);
   if (n == 0) return MM_OK;
   Pool& p = e->pool[e->cur];
   const uint32_t S = e->n_segs, nblk = (n + kRqItems - 1) / kRqItems;
   int rc;
   if ((rc = ensure_enq_scratch(e, n))) return rc;
-  uint64_t sc = 1024;
-  while (sc < 2ull * n) sc <<= 1;
+  const uint64_t sc = seen_keys(n);
   CK(e->d_mrg_code.reserve((size_t)n + 64));
   CK(e->d_mrg_src.reserve((size_t)n + 64));
   CK(e->d_rq_u.reserve((size_t)n + 64));
@@ -1584,7 +1602,7 @@ int requeue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating,
     ma.id = e->d_in_id; ma.rating = e->d_in_rating; ma.mode = e->d_in_mode; ma.ts = ts ? e->d_in_ts.p : nullptr;
     ma.seq = d_seq; ma.out = merged; ma.m_off = m_off; ma.err = &e->d_cnt->img_err;
     const uint64_t total = (uint64_t)n_live + n_rq;
-    const uint32_t grid = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((total + 255) / 256, 32ull * (uint32_t)e->n_sms));
+    const uint32_t grid = grid256(e, total, 32);
     k_rq_merge<<<grid, 256, 0, e->stream>>>(ma);
     CK(cudaGetLastError());
     // read 2: the sequence collision
@@ -1610,14 +1628,8 @@ int requeue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating,
   if (n_rq) {
     CK(cudaMemcpyAsync(slot_base, base.data(), (size_t)S * 4, cudaMemcpyHostToDevice, e->stream));
     k_rq_layout<<<S, 256, 0, e->stream>>>(p.m, S, e->d_sel, m_off, slot_base, e->d_seg_bin_lo, e->K, (uint32_t)dead, chunk);
-    ImgLoadArgs la{};
-    la.pool = p.v; la.meta = p.m; la.in = merged; la.n = n_live + n_rq; la.n_segs = S;
-    la.part_off = m_off; la.slot_base = slot_base;
-    la.bm = bin_map(e); la.grp_lut = e->d_grp_lut; la.bin_seg = e->d_bin_seg; la.seg_bin_lo = e->d_seg_bin_lo;
-    la.mode_tsize = e->d_mode_tsize; la.n_modes = e->cfg.n_modes; la.seq_next = e->seq_next; la.id_limit = id_limit(e);
-    la.err = &e->d_cnt->img_err;
-    const uint32_t g2 = std::max<uint32_t>(1, std::min<uint32_t>((la.n + 255) / 256, 32u * (uint32_t)e->n_sms));
-    k_img_load<<<g2, 256, 0, e->stream>>>(la);
+    k_img_load<<<grid256(e, n_live + n_rq, 32), 256, 0, e->stream>>>(
+        load_args(e, p, merged, n_live + n_rq, m_off, slot_base, e->seq_next));
     k_restamp<<<dim3(e->n_chunks, S), 256, 0, e->stream>>>(p.v, p.m, act_view(e), e->gen, e->d_sel);
     CK(cudaGetLastError());
   }
@@ -1685,8 +1697,7 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
   if (n_elsewhere) *n_elsewhere = 0;
   if (N == 0) return load_columns(e, std::vector<uint32_t>(S, 0), in[0], 0, act, m, seq_next, "image rejected");
   // scratch: the images' tables, the classification, the scatter and merge buffers, the gathered columns
-  uint64_t sc = 0;  // the repeated-id set: at most half full
-  if (e->use_active) for (sc = 1024; sc < 2ull * ((uint64_t)N + m); sc <<= 1) {}
+  const uint64_t sc = e->use_active ? seen_keys((uint64_t)N + m) : 0;  // the repeated-id set
   std::vector<uint32_t> off((size_t)K * (SI + 1), 0);
   for (uint32_t k = 0; k < K; ++k)
     for (uint32_t s = 0; s < SI; ++s) off[(size_t)k * (SI + 1) + s + 1] = off[(size_t)k * (SI + 1) + s] + cnt[k][s];
@@ -1748,7 +1759,7 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
   CK(cudaMemsetAsync(&e->d_cnt->img_err, 0, 3 * 4, e->stream));  // img_err, mrg_dups, rg_kmax
   if (e->use_active) CK(cudaMemsetAsync(seen, 0xFF, sc * 8, e->stream));
   // 1. per image: classify, repeated ids, the stable scatter by new partition (reject bucket S last), the run plan
-  const uint32_t grid = std::max<uint32_t>(1, std::min<uint32_t>((N + 255) / 256, 32u * (uint32_t)e->n_sms));
+  const uint32_t grid = grid256(e, N, 32);
   uint64_t hoff = 0;
   for (uint32_t k = 0; k < K; ++k) {
     const uint32_t n = h[k].n_players, b = base[k];
@@ -1849,7 +1860,7 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
       ga.age[0] = age[0] + base[k]; ga.age[1] = age[1] + base[k]; ga.ord = ord2; ga.run_start = run2;
       ga.ts = in[k].ts; ga.src_out = s2[0]; ga.key_out = key[0]; ga.head = head; ga.img = img; ga.qv = qv;
       ga.err = &e->d_cnt->img_err;
-      const uint32_t g = std::max<uint32_t>(1, std::min<uint32_t>((h[k].n_players + 255) / 256, 32u * (uint32_t)e->n_sms));
+      const uint32_t g = grid256(e, h[k].n_players, 32);
       k_rc_gather<<<g, 256, 0, e->stream>>>(ga);
     }
     k_rc_runmax<<<nrb, 256, 0, e->stream>>>(rq_one + 1, key[0], head, agg, first);
@@ -1938,7 +1949,7 @@ int band_check(mm_engine* e, int32_t W) {
     if (g && (int64_t)c.group_lo[g] != (int64_t)c.group_hi[g - 1] + 1)
       return set_err(e, MM_E_ARG, "the boundary pass needs contiguous ascending rating groups");
   }
-  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (e->stage_count) return staged_err(e);
   if (!e->use_active) return set_err(e, MM_E_STATE, "an MM_F_NO_DEDUPE engine cannot take matched players");
   return MM_OK;
 }
@@ -2116,7 +2127,7 @@ int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_t
     if (!rating && r.window >= 0)
       return set_err(e, MM_E_ARG, "request %u: a window on an MM_ORDER_ARRIVAL engine (pass window < 0)", j);
   }
-  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (e->stage_count) return staged_err(e);
   if (!e->use_active) return set_err(e, MM_E_STATE, "an MM_F_NO_DEDUPE engine cannot hold taken players");
   if (n == 0) return MM_OK;
   // the requests grouped by queue, stably (a counting sort), with the targets as clamp keys
@@ -2674,7 +2685,7 @@ int mm_locate(mm_engine* e, uint64_t now, uint32_t n, const uint64_t* id, mm_pla
   std::lock_guard<std::mutex> lk(e->mu);
   if (n && (!id || !out)) return set_err(e, MM_E_ARG, "null id or out array with n = %u", n);
   if (!e->use_active) return set_err(e, MM_E_STATE, "an MM_F_NO_DEDUPE engine has no active set to find ids in");
-  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (e->stage_count) return staged_err(e);
   if (n == 0) return MM_OK;
   CK(cudaSetDevice(e->device));
   return locate(e, now, n, id, out);
@@ -2862,7 +2873,7 @@ int mm_lobby_budget_report(mm_engine* e, uint32_t* candidates, uint32_t* emitted
   const uint32_t n_cut = e->n_cut;
   *n_out = n_cut;
   if (cap < n_cut) return set_err(e, MM_E_CAP, "need cap >= %u", n_cut);
-  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (e->stage_count) return staged_err(e);
   std::fill(candidates, candidates + n_cut, 0u);
   std::fill(emitted, emitted + n_cut, 0u);
   if (!e->report_valid) return MM_OK;
@@ -2883,7 +2894,7 @@ int mm_lobby_candidates(mm_engine* e, uint32_t* candidates, uint32_t cap, uint32
   const uint32_t n_cut = e->n_cut;
   *n_out = n_cut;
   if (cap < n_cut) return set_err(e, MM_E_CAP, "need cap >= %u", n_cut);
-  if (e->stage_count) return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
+  if (e->stage_count) return staged_err(e);
   CK(cudaSetDevice(e->device));
   const uint32_t layout = tail_layout(e);
   CK(e->d_cand_dry.reserve(n_cut + (layout & 1u ? 0u : e->Kp + 1)));

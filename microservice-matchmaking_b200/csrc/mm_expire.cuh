@@ -40,10 +40,8 @@ __global__ void __launch_bounds__(BLOCK) k_expire(const ExpireArgs a) {
   __shared__ Geo geo;
   __shared__ uint32_t s_gtmp[33];
   const uint32_t tid = threadIdx.x, lane = tid & 31;
-  geo_build<BLOCK>(geo, a.meta.fill, a.n_segs, gridDim.x, s_gtmp);
-  const uint32_t s0 = blockIdx.x * geo.tpr;
-  if (s0 >= geo.NT) return;  // (uniform)
-  const uint32_t s1 = s0 + geo.tpr < geo.NT ? s0 + geo.tpr : geo.NT;
+  uint32_t s0, s1;
+  if (!geo_cta_run<BLOCK>(geo, a.meta.fill, a.n_segs, s_gtmp, s0, s1)) return;  // (uniform)
   const uint32_t o = tid * 8;
   uint32_t counted = 0, erased = 0;
   for (uint32_t s = s0; s < s1; ++s) {
@@ -53,30 +51,16 @@ __global__ void __launch_bounds__(BLOCK) k_expire(const ExpireArgs a) {
     uint32_t hit = 0;  // bit j: slot base + j expires
     if (o < d.nvalid && (!a.sel || a.sel[d.seg])) {
       m2 = __ldcs(reinterpret_cast<const uint2*>(a.pool.mode + base));
-      const uint4 t0 = __ldcs(reinterpret_cast<const uint4*>(a.pool.ts + base));
-      const uint4 t1 = __ldcs(reinterpret_cast<const uint4*>(a.pool.ts + base) + 1);
-      const uint32_t ts[8] = {t0.x, t0.y, t0.z, t0.w, t1.x, t1.y, t1.z, t1.w};
+      uint32_t ts[8];
+      ld_stamps8(a.pool.ts + base, ts);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint32_t md = ((j < 4 ? m2.x : m2.y) >> (8 * (j & 3))) & 0xFFu;
-        if (o + j < d.nvalid && md != MM_MODE_DEAD && stat_wait(a.now, ts[j]) >= a.max_wait) hit |= 1u << j;
-      }
+      for (int j = 0; j < 8; ++j)
+        if (o + j < d.nvalid && mode8_at(m2, j) != MM_MODE_DEAD && stat_wait(a.now, ts[j]) >= a.max_wait) hit |= 1u << j;
     }
     const uint32_t k = __popc(hit);
     if (!a.commit) { counted += k; continue; }  // (uniform)
-    // warp-aggregated output cursor: one global atomic per warp and tile
-    uint32_t incl = k;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-      if (lane >= (uint32_t)off) incl += v;
-    }
-    const uint32_t total = __shfl_sync(0xFFFFFFFFu, incl, 31);
-    uint32_t wbase = 0;
-    if (lane == 31 && total) wbase = atomicAdd(&a.ctr[0], total);
-    wbase = __shfl_sync(0xFFFFFFFFu, wbase, 31);
+    uint32_t q = warp_append(&a.ctr[0], k);  // one global atomic per warp and tile
     if (!hit) continue;
-    uint32_t q = wbase + incl - k;
     uint2 dead = m2;  // the thread's 8 mode bytes with the expired ones set to DEAD: one store
 #pragma unroll
     for (int j = 0; j < 8; ++j)

@@ -41,6 +41,15 @@ struct ImgCols {
 __device__ __forceinline__ uint64_t img_id(const ImgCols& c, uint32_t i) {
   return c.id_bytes == 8 ? static_cast<const uint64_t*>(c.id)[i] : static_cast<const uint32_t*>(c.id)[i];
 }
+__device__ __forceinline__ void img_set_id(const ImgCols& c, uint32_t i, uint64_t pid) {
+  if (c.id_bytes == 8) static_cast<uint64_t*>(c.id)[i] = pid;
+  else static_cast<uint32_t*>(c.id)[i] = (uint32_t)pid;
+}
+// player s of `in` -> player d of `out`, every column
+__device__ __forceinline__ void img_copy(const ImgCols& out, uint32_t d, const ImgCols& in, uint32_t s) {
+  img_set_id(out, d, img_id(in, s));
+  out.rating[d] = in.rating[s]; out.ts[d] = in.ts[s]; out.seq[d] = in.seq[s]; out.mode[d] = in.mode[s];
+}
 
 struct ImgExportArgs {
   PoolView pool;
@@ -58,11 +67,9 @@ __global__ void __launch_bounds__(BLOCK) k_img_tiles(const ImgExportArgs a) {
   __shared__ Geo geo;
   __shared__ uint32_t s_gtmp[33];
   __shared__ uint32_t s_warp[BLOCK / 32];
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  geo_build<BLOCK>(geo, a.meta.fill, a.n_segs, gridDim.x, s_gtmp);
-  const uint32_t s0 = blockIdx.x * geo.tpr;
-  if (s0 >= geo.NT) return;  // (uniform)
-  const uint32_t s1 = s0 + geo.tpr < geo.NT ? s0 + geo.tpr : geo.NT;
+  const uint32_t tid = threadIdx.x;
+  uint32_t s0, s1;
+  if (!geo_cta_run<BLOCK>(geo, a.meta.fill, a.n_segs, s_gtmp, s0, s1)) return;  // (uniform)
   const uint32_t o = tid * 8;
   for (uint32_t s = s0; s < s1; ++s) {
     const TileDesc d = geo_tile(geo, a.meta, s);
@@ -72,27 +79,12 @@ __global__ void __launch_bounds__(BLOCK) k_img_tiles(const ImgExportArgs a) {
       const uint2 m2 = __ldcs(reinterpret_cast<const uint2*>(a.pool.mode + base));
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const uint32_t md = ((j < 4 ? m2.x : m2.y) >> (8 * (j & 3))) & 0xFFu;
-        if (o + j < d.nvalid && md != MM_MODE_DEAD) live |= 1u << j;
+        if (o + j < d.nvalid && mode8_at(m2, j) != MM_MODE_DEAD) live |= 1u << j;
       }
     }
-    const uint32_t k = __popc(live);
-    uint32_t incl = k;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-      if (lane >= (uint32_t)off) incl += v;
-    }
-    if (lane == 31) s_warp[warp] = incl;
-    __syncthreads();
-    uint32_t before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < BLOCK / 32; ++w) {
-      const uint32_t v = s_warp[w];
-      before += (uint32_t)w < warp ? v : 0u;
-      total += v;
-    }
-    __syncthreads();  // s_warp is rewritten for the next tile
+    const uint32_t k = __popc(live), incl = warp_incl_scan(k);
+    uint32_t total;
+    const uint32_t before = block_warp_offsets<BLOCK>(incl, total, s_warp);
     if (!WRITE) {
       if (tid == 0) {
         a.tile_cnt[s] = total;
@@ -106,9 +98,7 @@ __global__ void __launch_bounds__(BLOCK) k_img_tiles(const ImgExportArgs a) {
     for (int j = 0; j < 8; ++j) {
       if (!((live >> j) & 1u)) continue;
       const size_t slot = base + j;
-      const uint64_t pid = a.pool.id[slot];
-      if (a.out.id_bytes == 8) static_cast<uint64_t*>(a.out.id)[q] = pid;
-      else static_cast<uint32_t*>(a.out.id)[q] = (uint32_t)pid;
+      img_set_id(a.out, q, a.pool.id[slot]);
       a.out.rating[q] = a.pool.rating[slot];
       a.out.ts[q] = a.pool.ts[slot];
       a.out.seq[q] = a.pool.seq[slot];
@@ -123,7 +113,6 @@ __global__ void __launch_bounds__(BLOCK) k_img_tiles(const ImgExportArgs a) {
 // Output unordered, through a warp-aggregated cursor; at most `cap` are written (the host knows n_active).
 __global__ void k_img_active(ActiveView act, uint64_t n_tab, const uint8_t* __restrict__ pool_mode, uint32_t n_slots,
                              uint32_t gen, void* out, uint32_t id_bytes, uint32_t cap, uint32_t* __restrict__ ctr) {
-  const uint32_t lane = threadIdx.x & 31;
   const uint64_t stride = (uint64_t)gridDim.x * blockDim.x;
   for (uint64_t s0 = (uint64_t)blockIdx.x * blockDim.x; s0 < n_tab; s0 += stride) {  // uniform per CTA
     const uint64_t s = s0 + threadIdx.x;
@@ -142,12 +131,7 @@ __global__ void k_img_active(ActiveView act, uint64_t n_tab, const uint8_t* __re
       const uint32_t slot = (uint32_t)v;
       if (emit && (uint32_t)(v >> 32) == gen && slot < n_slots && pool_mode[slot] != MM_MODE_DEAD) emit = false;
     }
-    const uint32_t b = __ballot_sync(0xFFFFFFFFu, emit);
-    if (!b) continue;
-    uint32_t base = 0;
-    if (lane == 0) base = atomicAdd(ctr, (uint32_t)__popc(b));
-    base = __shfl_sync(0xFFFFFFFFu, base, 0);
-    const uint32_t q = base + __popc(b & ((1u << lane) - 1u));
+    const uint32_t q = warp_append(ctr, emit);
     if (emit && q < cap) {
       if (id_bytes == 8) static_cast<uint64_t*>(out)[q] = pid;
       else static_cast<uint32_t*>(out)[q] = (uint32_t)pid;
@@ -185,9 +169,7 @@ __device__ __forceinline__ ImgPlayer img_player(const ImgCols& in, uint32_t i, c
                                                 const BinMap& bm, const uint8_t* grp_lut, const uint16_t* bin_seg,
                                                 uint32_t n_modes, uint32_t seq_next, uint64_t id_limit) {
   ImgPlayer q;
-  uint32_t lo = 0, e = n_segs;
-  while (e - lo > 1) { const uint32_t mid = (lo + e) >> 1; if (s_off[mid] <= i) lo = mid; else e = mid; }
-  q.p = lo;
+  q.p = last_le(s_off, 0, n_segs, i);
   q.pid = img_id(in, i);
   q.md = in.mode[i];
   q.rt = in.rating[i];
@@ -198,10 +180,8 @@ __device__ __forceinline__ ImgPlayer img_player(const ImgCols& in, uint32_t i, c
   if (q.md >= n_modes) {
     q.bad |= kImgBadMode;
   } else {
-    const int32_t hi = bm.key_lo + (int32_t)bm.KR - 1;
-    const int32_t r = q.rt < bm.key_lo ? bm.key_lo : (q.rt > hi ? hi : q.rt);
     q.bin = bin_of(bm, bm.lut, q.rt, q.md);
-    if (grp_lut[r - bm.key_lo] == 0xFF || bin_seg[q.bin] != q.p) q.bad |= kImgBadRating;
+    if (grp_lut[clamp_key(bm.key_lo, bm.KR, q.rt)] == 0xFF || bin_seg[q.bin] != q.p) q.bad |= kImgBadRating;
   }
   if (q.u == 0 || (i + 1 < s_off[q.p + 1] && in.seq[i + 1] - seq_next <= q.u)) q.bad |= kImgBadSeq;
   return q;
@@ -291,13 +271,11 @@ __global__ void __launch_bounds__(256) k_mrg_order(const MrgOrderArgs a) {
     uint32_t pos = s_off[q0] + (i - s_off[p]);
     for (uint32_t q = q0; q < q1; ++q) {
       if (q == p) continue;
-      uint32_t l = s_off[q], r = s_off[q + 1];  // players of q enqueued before i: u' < u (u' <= u for q < p)
-      while (l < r) {
-        const uint32_t mid = (l + r) >> 1;
-        const uint32_t v = a.in.seq[mid] - a.seq_next;
-        if (v < x.u || (q < p && v == x.u)) l = mid + 1; else r = mid;
-      }
-      pos += l - s_off[q];
+      // players of q enqueued before i: u' < u (u' <= u for q < p)
+      pos += first_not(s_off[q], s_off[q + 1], [&](uint32_t k) {
+               const uint32_t v = a.in.seq[k] - a.seq_next;
+               return v < x.u || (q < p && v == x.u);
+             }) - s_off[q];
     }
     a.out_id[pos] = x.pid; a.out_rating[pos] = x.rt; a.out_mode[pos] = (uint8_t)x.md; a.out_ts[pos] = a.in.ts[i];
     a.src[pos] = i;
@@ -314,11 +292,7 @@ __global__ void k_mrg_dups(const uint64_t* __restrict__ id, uint32_t n, ActiveVi
     const uint64_t pid = id[i];
     const uint64_t h = act_find(act, pid);
     if (h != ~0ull && (!act.dcap || *act.val(h) != kFreeVal)) { ++dup; continue; }
-    for (uint64_t s = hash64(pid) & seen_mask;; s = (s + 1) & seen_mask) {
-      const unsigned long long k = atomicCAS(&seen[s], kEmptyKey, (unsigned long long)pid);
-      if (k == kEmptyKey) break;
-      if (k == pid) { ++dup; break; }
-    }
+    if (!seen_insert(seen, seen_mask, pid)) ++dup;
   }
   dup = __reduce_add_sync(0xFFFFFFFFu, dup);
   if ((threadIdx.x & 31) == 0 && dup) atomicAdd(count, dup);
@@ -329,13 +303,8 @@ __global__ void k_mrg_rejects(uint32_t n, const uint8_t* __restrict__ code, cons
                               uint32_t* __restrict__ out, uint32_t* __restrict__ count) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   const bool rej = i < n && code[i] != 1;
-  const uint32_t b = __ballot_sync(0xFFFFFFFFu, rej);
-  if (!b) return;
-  const uint32_t lane = threadIdx.x & 31;
-  uint32_t base = 0;
-  if (lane == 0) base = atomicAdd(count, (uint32_t)__popc(b));
-  base = __shfl_sync(0xFFFFFFFFu, base, 0);
-  if (rej) out[base + __popc(b & ((1u << lane) - 1u))] = src[i];
+  const uint32_t at = warp_append(count, rej);
+  if (rej) out[at] = src[i];
 }
 
 }  // namespace mm

@@ -75,98 +75,64 @@ __device__ __forceinline__ void mq_shape(const MqArgs& a, uint32_t q, uint32_t& 
   S = a.mode_tsize[q / a.n_groups];
 }
 // queue of header position h: the last q with qlob[q] <= h (queues without lobbies share their successor's base)
-__device__ __forceinline__ uint32_t mq_queue_of(const MqArgs& a, uint32_t h) {
-  uint32_t lo = 0, hi = a.n_cut;
-  while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (a.qlob[mid] <= h) lo = mid; else hi = mid; }
-  return lo;
-}
+__device__ __forceinline__ uint32_t mq_queue_of(const MqArgs& a, uint32_t h) { return last_le(a.qlob, 0, a.n_cut, h); }
 
 // matched players per bin (cnt zeroed by the host).  CTAs take contiguous runs of the virtual tile sequence.
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK) k_mq_count(const MqArgs a) {
   __shared__ Geo geo;
   __shared__ uint32_t s_gtmp[33];
-  const uint32_t tid = threadIdx.x, lane = tid & 31;
-  geo_build<BLOCK>(geo, a.meta.fill, a.n_segs, gridDim.x, s_gtmp);
-  const uint32_t s0 = blockIdx.x * geo.tpr;
-  if (s0 >= geo.NT) return;  // (uniform)
-  const uint32_t s1 = s0 + geo.tpr < geo.NT ? s0 + geo.tpr : geo.NT;
-  const uint32_t o = tid * 8;
+  uint32_t s0, s1;
+  if (!geo_cta_run<BLOCK>(geo, a.meta.fill, a.n_segs, s_gtmp, s0, s1)) return;  // (uniform)
+  const uint32_t o = threadIdx.x * 8;
   for (uint32_t s = s0; s < s1; ++s) {
     const TileDesc d = geo_tile(geo, a.meta, s);
     uint32_t b[8];
 #pragma unroll
     for (int j = 0; j < 8; ++j) b[j] = kMqNone;
     if (o < d.nvalid) {
-      const uint4 k4 = __ldcs(reinterpret_cast<const uint4*>(a.pool.bin + (size_t)d.phys * kTile + o));
+      uint32_t v[8];
+      ld_bins8(a.pool.bin + (size_t)d.phys * kTile + o, v);
       const uint32_t left = (__ldcs(&a.left_bits[((size_t)s * kTile + o) >> 5]) >> (o & 31)) & 0xFFu;
-      const uint32_t w[4] = {k4.x, k4.y, k4.z, k4.w};
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint32_t v = (w[j >> 1] >> (16 * (j & 1))) & 0xFFFFu;
-        if (o + j < d.nvalid && v < a.K && !((left >> j) & 1u)) b[j] = v;
-      }
+      for (int j = 0; j < 8; ++j)
+        if (o + j < d.nvalid && v[j] < a.K && !((left >> j) & 1u)) b[j] = v[j];
     }
-    // warp-aggregated: one atomic per distinct bin of the warp (one in all when the warp's 256 slots share it)
-    const uint32_t b0 = __shfl_sync(0xFFFFFFFFu, b[0], 0);
-    bool same = true;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) same &= b[j] == b0;
-    if (__all_sync(0xFFFFFFFFu, same)) {
-      if (lane == 0 && b0 != kMqNone) atomicAdd(&a.cnt[b0], 8u * 32u);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint32_t m = __match_any_sync(0xFFFFFFFFu, b[j]);
-        if (b[j] != kMqNone && lane == (uint32_t)(__ffs(m) - 1)) atomicAdd(&a.cnt[b[j]], (uint32_t)__popc(m));
-      }
-    }
+    warp_hist8_add(a.cnt, b, kMqNone);
   }
 }
+
+// (members, sum of c) of a run of bins, scanned together by k_mq_scan
+struct MqSum {
+  uint32_t c;
+  long long w;
+};
+__device__ __forceinline__ MqSum operator+(const MqSum& x, const MqSum& y) { return MqSum{x.c + y.c, x.w + y.w}; }
+__device__ __forceinline__ MqSum operator-(const MqSum& x, const MqSum& y) { return MqSum{x.c - y.c, x.w - y.w}; }
+__device__ __forceinline__ MqSum shfl_up(const MqSum& v, int off) { return MqSum{shfl_up(v.c, off), shfl_up(v.w, off)}; }
 
 // One CTA per queue: cnt -> each bin's first member inside the queue, csum -> the sum of c before it (rating order),
 // qlob[q] = the queue's lobbies.
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK) k_mq_scan(const MqArgs a, bool rating) {
-  __shared__ uint32_t s_c[BLOCK / 32];
-  __shared__ long long s_w[BLOCK / 32];
-  const uint32_t q = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  __shared__ MqSum s_tmp[BLOCK / 32 + 1];
+  const uint32_t q = blockIdx.x, tid = threadIdx.x;
   const uint32_t b0 = a.seg_bin_lo[a.cut_lp_lo[q]], b1 = a.seg_bin_lo[a.cut_lp_lo[q + 1]];
-  uint32_t run_c = 0;
-  long long run_w = 0;
+  MqSum run{0u, 0ll};
   for (uint32_t base = b0; base < b1; base += BLOCK) {
     const uint32_t b = base + tid;
     const uint32_t c = b < b1 ? a.cnt[b] : 0u;
-    const long long w = rating && c ? (long long)c * (a.key_lo + (int32_t)a.bin_key[b]) : 0ll;
-    uint32_t ic = c;
-    long long iw = w;
-#pragma unroll
-    for (int off = 1; off < 32; off <<= 1) {
-      const uint32_t vc = __shfl_up_sync(0xFFFFFFFFu, ic, off);
-      const long long vw = __shfl_up_sync(0xFFFFFFFFu, iw, off);
-      if (lane >= (uint32_t)off) { ic += vc; iw += vw; }
-    }
-    if (lane == 31) { s_c[warp] = ic; s_w[warp] = iw; }
-    __syncthreads();
-    uint32_t bc = 0, tc = 0;
-    long long bw = 0, tw = 0;
-#pragma unroll
-    for (int k = 0; k < BLOCK / 32; ++k) {
-      if ((uint32_t)k < warp) { bc += s_c[k]; bw += s_w[k]; }
-      tc += s_c[k]; tw += s_w[k];
-    }
-    __syncthreads();  // s_c / s_w are rewritten by the next round
+    const MqSum v{c, rating && c ? (long long)c * (a.key_lo + (int32_t)a.bin_key[b]) : 0ll};
+    const MqSum x = block_scan_step<BLOCK>(v, run, s_tmp);
     if (b < b1) {
-      a.cnt[b] = run_c + bc + ic - c;
-      if (rating) a.csum[b] = run_w + bw + iw - w;
+      a.cnt[b] = x.c;
+      if (rating) a.csum[b] = x.w;
     }
-    run_c += tc;
-    run_w += tw;
   }
   if (tid == 0) {
     uint32_t L, S;
     mq_shape(a, q, L, S);
-    a.qlob[q] = run_c / L;
+    a.qlob[q] = run.c / L;
   }
 }
 
@@ -198,11 +164,8 @@ __global__ void __launch_bounds__(BLOCK) k_mq_arrival(const MqArgs a) {
   __shared__ uint32_t s_gtmp[33];
   __shared__ uint32_t s_warp[BLOCK / 32];
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  geo_build<BLOCK>(geo, a.meta.fill, a.n_segs, gridDim.x, s_gtmp);
-  const uint32_t s0 = blockIdx.x * geo.tpr;
-  if (s0 >= geo.NT) return;  // (uniform)
-  const uint32_t s1 = s0 + geo.tpr < geo.NT ? s0 + geo.tpr : geo.NT;
-  const int32_t hi = a.key_lo + (int32_t)a.KR - 1;
+  uint32_t s0, s1;
+  if (!geo_cta_run<BLOCK>(geo, a.meta.fill, a.n_segs, s_gtmp, s0, s1)) return;  // (uniform)
   for (uint32_t s = s0; s < s1; ++s) {
     const TileDesc d = geo_tile(geo, a.meta, s);
     const uint32_t q = a.part_cut[d.seg];
@@ -218,23 +181,11 @@ __global__ void __launch_bounds__(BLOCK) k_mq_arrival(const MqArgs a) {
       const uint32_t left = __ldcs(&a.left_bits[((size_t)s * kTile + o0 + warp * 32) >> 5]);
       const bool matched = live && !((left >> lane) & 1u);
       const uint32_t bal = __ballot_sync(0xFFFFFFFFu, live);
-      if (lane == 0) s_warp[warp] = __popc(bal);
-      __syncthreads();
-      uint32_t before = 0, total = 0;
-#pragma unroll
-      for (int w = 0; w < BLOCK / 32; ++w) {
-        const uint32_t v = s_warp[w];
-        before += (uint32_t)w < warp ? v : 0u;
-        total += v;
-      }
-      __syncthreads();  // s_warp is rewritten by the next step
+      uint32_t total;
+      const uint32_t before = block_warp_offsets<BLOCK>(__popc(bal), total, s_warp);
       const uint32_t rho = rho0 + before + __popc(bal & ((1u << lane) - 1u));
       rho0 += total;
-      uint32_t v = 0;
-      if (matched) {
-        const int32_t r = a.pool.rating[slot];
-        v = (uint32_t)((r < a.key_lo ? a.key_lo : (r > hi ? hi : r)) - a.key_lo);
-      }
+      const uint32_t v = matched ? clamp_key(a.key_lo, a.KR, a.pool.rating[slot]) : 0u;
       const uint32_t lk = rho / L, tk = rho / S;
       uint32_t mn = matched ? v : 0xFFFFFFFFu, mx = v, sm = v;
 #pragma unroll
@@ -284,10 +235,8 @@ __global__ void __launch_bounds__(256) k_mq_lobby(const MqArgs a) {
     // bin of the queue's member x: the last bin whose first member is <= x (empty bins share their successor's)
     uint32_t from = b0;
     auto bin_at = [&](uint32_t x) {
-      uint32_t lo = from, hi = b1;
-      while (hi - lo > 1) { const uint32_t mid = (lo + hi) >> 1; if (a.cnt[mid] <= x) lo = mid; else hi = mid; }
-      from = lo;  // members are asked for in ascending order
-      return lo;
+      from = last_le(a.cnt, from, b1, x);  // members are asked for in ascending order
+      return from;
     };
     auto c_of = [&](uint32_t b) { return (long long)a.key_lo + a.bin_key[b]; };
     // F(x): sum of c over the queue's members [0, x), x > 0

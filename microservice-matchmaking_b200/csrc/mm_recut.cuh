@@ -75,7 +75,7 @@ __global__ void __launch_bounds__(256) k_rc_gather(const RcGatherArgs a) {
   const uint32_t* age = a.age[b];
   bool bad = false;
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < kept; i += gridDim.x * blockDim.x) {
-    const uint32_t q = rg_part_of(s_off, a.n_segs, i), local = src[i];
+    const uint32_t q = last_le(s_off, 0, a.n_segs, i), local = src[i];
     if (i + 1 < s_off[q + 1] && age[i + 1] == age[i]) bad = true;
     if (local >= a.n) { bad = true; continue; }  // only after a failed check: the merge had holes
     const uint32_t v = a.base + local;
@@ -99,35 +99,11 @@ struct RcSeg {
   uint32_t f, v;
 };
 __device__ __forceinline__ RcSeg rc_seg(RcSeg a, RcSeg b) { return RcSeg{a.f | b.f, b.f ? b.v : max(a.v, b.v)}; }
-
-// exclusive segmented scan of one value per thread over a CTA of T threads; s_warp: T / 32 entries
-template <int T>
-__device__ __forceinline__ RcSeg rc_block_excl(RcSeg x, RcSeg* s_warp) {
-  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  RcSeg in = x;
-#pragma unroll
-  for (int off = 1; off < 32; off <<= 1) {
-    const RcSeg y{__shfl_up_sync(0xFFFFFFFFu, in.f, off), __shfl_up_sync(0xFFFFFFFFu, in.v, off)};
-    if (lane >= (uint32_t)off) in = rc_seg(y, in);
-  }
-  if (lane == 31) s_warp[warp] = in;
-  __syncthreads();
-  if (warp == 0) {
-    RcSeg w = lane < T / 32 ? s_warp[lane] : RcSeg{0, 0};
-#pragma unroll
-    for (int off = 1; off < T / 32; off <<= 1) {
-      const RcSeg y{__shfl_up_sync(0xFFFFFFFFu, w.f, off), __shfl_up_sync(0xFFFFFFFFu, w.v, off)};
-      if (lane >= (uint32_t)off) w = rc_seg(y, w);
-    }
-    if (lane < T / 32) s_warp[lane] = w;  // inclusive over the warps
-  }
-  __syncthreads();
-  RcSeg ex{__shfl_up_sync(0xFFFFFFFFu, in.f, 1), __shfl_up_sync(0xFFFFFFFFu, in.v, 1)};
-  if (lane == 0) ex = RcSeg{0, 0};
-  const RcSeg r = warp ? rc_seg(s_warp[warp - 1], ex) : ex;
-  __syncthreads();  // s_warp may be reused
-  return r;
-}
+__device__ __forceinline__ RcSeg shfl_up(const RcSeg& s, int off) { return RcSeg{shfl_up(s.f, off), shfl_up(s.v, off)}; }
+// the CTA scans' combine operator (block_excl_scan_op)
+struct RcSegOp {
+  __device__ __forceinline__ RcSeg operator()(RcSeg a, RcSeg b) const { return rc_seg(a, b); }
+};
 
 // Block b scans positions [b * kRcBlock, (b + 1) * kRcBlock) of the n = *kept: the stamp field of key.hi becomes the
 // max since the last run start inside the block; agg[b] = the block's (f, v), first[b] = its first run start (or its
@@ -152,7 +128,7 @@ __global__ void __launch_bounds__(256) k_rc_runmax(const uint32_t* __restrict__ 
     t = rc_seg(t, RcSeg{f[j], v[j]});
     if (f[j]) atomicMin(&s_first, p - b0);
   }
-  RcSeg run = rc_block_excl<256>(t, s_warp);
+  RcSeg run = block_excl_scan_op<256>(t, RcSeg{0, 0}, RcSegOp{}, s_warp);
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
     const uint32_t p = p0 + j;
@@ -172,7 +148,7 @@ __global__ void __launch_bounds__(1024) k_rc_carry(const uint32_t* __restrict__ 
   const uint32_t b0 = threadIdx.x * per, b1 = min(nb, b0 + per);
   RcSeg t{0, 0};
   for (uint32_t b = b0; b < b1; ++b) t = rc_seg(t, agg[b]);
-  RcSeg run = rc_block_excl<1024>(t, s_warp);
+  RcSeg run = block_excl_scan_op<1024>(t, RcSeg{0, 0}, RcSegOp{}, s_warp);
   for (uint32_t b = b0; b < b1; ++b) {
     carry[b] = run;
     run = rc_seg(run, agg[b]);

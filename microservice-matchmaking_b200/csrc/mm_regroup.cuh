@@ -72,9 +72,7 @@ __global__ void __launch_bounds__(256) k_rg_classify(const RgClassifyArgs a) {
       } else if (x.md >= a.n_modes) {
         q = a.n_segs;
       } else {
-        const int32_t hi = a.bm.key_lo + (int32_t)a.bm.KR - 1;
-        const int32_t r = x.rt < a.bm.key_lo ? a.bm.key_lo : (x.rt > hi ? hi : x.rt);
-        q = a.grp_lut[r - a.bm.key_lo] == 0xFF ? a.n_segs : a.bin_seg[bin_of(a.bm, a.bm.lut, x.rt, x.md)];
+        q = a.grp_lut[clamp_key(a.bm.key_lo, a.bm.KR, x.rt)] == 0xFF ? a.n_segs : a.bin_seg[bin_of(a.bm, a.bm.lut, x.rt, x.md)];
         if (a.keep && q < a.n_segs && !a.keep[q]) { q = kNoPart; ++skip; }
       }
       if (q != kNoPart) atomicAdd(&s_hist[q], 1u);
@@ -102,11 +100,7 @@ __global__ void k_rg_dups(const void* ids, const void* act_ids, uint32_t id_byte
     const void* col = i < n ? ids : act_ids;
     const uint32_t k = i < n ? i : i - n;
     const uint64_t pid = id_bytes == 8 ? static_cast<const uint64_t*>(col)[k] : static_cast<const uint32_t*>(col)[k];
-    for (uint64_t s = hash64(pid) & seen_mask;; s = (s + 1) & seen_mask) {
-      const unsigned long long v = atomicCAS(&seen[s], kEmptyKey, (unsigned long long)pid);
-      if (v == kEmptyKey) break;
-      if (v == pid) { ++dup; break; }
-    }
+    if (!seen_insert(seen, seen_mask, pid)) ++dup;
   }
   dup = __reduce_add_sync(0xFFFFFFFFu, dup);
   if ((threadIdx.x & 31) == 0 && dup) atomicAdd(count, dup);
@@ -126,12 +120,7 @@ __global__ void __launch_bounds__(1024) k_rg_plan(uint32_t n_img_segs, uint32_t 
     for (uint32_t p0 = 0; p0 < n_img_segs; p0 += 32) {
       const uint32_t p = p0 + lane;
       const uint32_t c = p < n_img_segs ? pair[(size_t)p * n_segs + q] : 0u;
-      uint32_t incl = c;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const uint32_t v = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-        if (lane >= (uint32_t)off) incl += v;
-      }
+      const uint32_t incl = warp_incl_scan(c);
       const uint32_t nz = __ballot_sync(0xFFFFFFFFu, c != 0);
       if (c) {
         const uint32_t j = k + __popc(nz & ((1u << lane) - 1u));
@@ -151,13 +140,6 @@ __global__ void __launch_bounds__(1024) k_rg_plan(uint32_t n_img_segs, uint32_t 
 
 // rounds of k_rg_merge that do work for k_max runs
 __device__ __forceinline__ uint32_t rg_rounds(uint32_t kmax) { return kmax <= 1 ? 0u : 32u - __clz(kmax - 1); }
-
-// the last q with s_off[q] <= k (s_off: n + 1 ascending offsets)
-__device__ __forceinline__ uint32_t rg_part_of(const uint32_t* s_off, uint32_t n, uint32_t k) {
-  uint32_t lo = 0, e = n;
-  while (e - lo > 1) { const uint32_t mid = (lo + e) >> 1; if (s_off[mid] <= k) lo = mid; else e = mid; }
-  return lo;
-}
 
 template <class Key>
 struct RgMergeArgsT {
@@ -184,7 +166,7 @@ __global__ void __launch_bounds__(256) k_rg_merge(const RgMergeArgsT<Key> a) {
   __syncthreads();
   const uint32_t kept = s_off[a.n_segs], t = a.round;
   for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < kept; k += gridDim.x * blockDim.x) {
-    const uint32_t q = rg_part_of(s_off, a.n_segs, k);
+    const uint32_t q = last_le(s_off, 0, a.n_segs, k);
     const uint32_t src = a.src_in[k];
     const Key u = a.u_in[k];
     const uint32_t s = a.ord[(size_t)a.pimg[src] * a.n_segs + q] >> t, ps = s ^ 1u, K = a.kq[q];
@@ -192,13 +174,11 @@ __global__ void __launch_bounds__(256) k_rg_merge(const RgMergeArgsT<Key> a) {
     uint32_t dst = k;
     if ((ps << t) < K) {
       const uint32_t A = rs[s << t], C = rs[ps << t], D = rs[min((ps + 1) << t, K)];
-      uint32_t l = C, r = D;
       const bool left = !(s & 1u);  // left: the partner's players older than u; right: older or of the same age
-      while (l < r) {
-        const uint32_t mid = (l + r) >> 1;
-        const Key v = a.u_in[mid];
-        if (v < u || (!left && v == u)) l = mid + 1; else r = mid;
-      }
+      const uint32_t l = first_not(C, D, [&](uint32_t m) {
+        const Key v = a.u_in[m];
+        return v < u || (!left && v == u);
+      });
       dst = left ? k + (l - C) : k - A + l;
     }
     a.src_out[dst] = src;
@@ -227,12 +207,10 @@ __global__ void __launch_bounds__(256) k_rg_finish(const RgFinishArgs a) {
   bool bad = false;
   for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < total; k += gridDim.x * blockDim.x) {
     if (k >= kept) { a.rejected[k - kept] = a.src[0][k]; continue; }
-    const uint32_t q = rg_part_of(s_off, a.n_segs, k), i = src[k];
+    const uint32_t q = last_le(s_off, 0, a.n_segs, k), i = src[k];
     if (k + 1 < s_off[q + 1] && age[k + 1] == age[k]) bad = true;
     if (i >= a.n) { bad = true; continue; }  // only after a failed check: the merge had holes
-    if (a.in.id_bytes == 8) static_cast<uint64_t*>(a.out.id)[k] = static_cast<const uint64_t*>(a.in.id)[i];
-    else static_cast<uint32_t*>(a.out.id)[k] = static_cast<const uint32_t*>(a.in.id)[i];
-    a.out.rating[k] = a.in.rating[i]; a.out.ts[k] = a.in.ts[i]; a.out.seq[k] = a.in.seq[i]; a.out.mode[k] = a.in.mode[i];
+    img_copy(a.out, k, a.in, i);
   }
   if (__any_sync(0xFFFFFFFFu, bad) && (threadIdx.x & 31) == 0) atomicOr(a.err, kImgBadSeq);
 }

@@ -2,8 +2,8 @@
 // position their enqueue sequence number gives them.
 //
 // The call is an in-engine export, merge and import of the partitions it touches:
-//   k_rq_check  checks every entry (the checks of k_enq_claim / img_player, strict age order, one copy per id through a
-//               scratch set as k_mrg_dups) and classifies its active-set entry: 0 = a live queued player (gen << 32 |
+//   k_rq_check  checks every entry (the checks of img_player, clamp_key for the group, strict age order, one copy per id
+//               through seen_insert) and classifies its active-set entry: 0 = a live queued player (gen << 32 |
 //               slot on a live slot, the test of k_img_active), 1 = active and not queued (matched, taken), 4 = not
 //               active.  Code-1 entries are counted per (ingest-sized block, partition).
 //   k_rq_scan   turns the block counts into each block's first index among its partition's code-1 entries, the
@@ -12,7 +12,7 @@
 //   k_rq_group  writes the code-1 entries partition by partition, in age order (a stable counting sort).
 //   k_rq_merge  gives every player of a touched partition its index in the merged list: a live player's index plus the
 //               requeued entries of its partition that are older, a requeued entry's rank plus the live players that
-//               are older (binary searches, as k_mrg_order).  An equal sequence number is a collision.
+//               are older (binary searches: last_le, first_not).  An equal sequence number is a collision.
 //   k_rq_layout puts the touched partitions on fresh chunks (the host's layout, as import_image) and rebuilds their bin
 //               totals; k_img_load then writes the merged columns, and k_restamp points the entries at the new slots.
 #pragma once
@@ -66,20 +66,14 @@ __global__ void __launch_bounds__(256) k_rq_check(const RqCheckArgs a) {
     if (md >= a.n_modes) {
       b |= kRqBadMode;
     } else {
-      const int32_t hi = a.bm.key_lo + (int32_t)a.bm.KR - 1;
-      const int32_t r = a.rating[i] < a.bm.key_lo ? a.bm.key_lo : (a.rating[i] > hi ? hi : a.rating[i]);
-      if (a.grp_lut[r - a.bm.key_lo] == 0xFF) b |= kRqBadRating;
+      if (a.grp_lut[clamp_key(a.bm.key_lo, a.bm.KR, a.rating[i])] == 0xFF) b |= kRqBadRating;
       else p = a.bin_seg[bin_of(a.bm, a.bm.lut, a.rating[i], md)];
     }
     if (u == 0) b |= kRqSeqNext;
     if (i + 1 < a.n && a.seq[i + 1] - a.seq_next <= u) b |= kRqOrder;
     uint8_t c = 4;
     if (!(b & kRqBadId)) {
-      for (uint64_t s = hash64(pid) & a.seen_mask;; s = (s + 1) & a.seen_mask) {
-        const unsigned long long k = atomicCAS(&a.seen[s], kEmptyKey, (unsigned long long)pid);
-        if (k == kEmptyKey) break;
-        if (k == pid) { b |= kRqDup; break; }
-      }
+      if (!seen_insert(a.seen, a.seen_mask, pid)) b |= kRqDup;
       const uint64_t h = act_find(a.act, pid);
       const unsigned long long v = h == ~0ull ? kFreeVal : *a.act.val(h);
       if (v < kPending) {
@@ -108,20 +102,8 @@ __global__ void __launch_bounds__(512) k_rq_scan(uint32_t n_segs, uint32_t nblk,
   __shared__ uint32_t s_off[kMaxSegs + 1], s_tmp[64];
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   for (uint32_t p = warp; p < n_segs; p += 16) {
-    uint32_t carry = 0;
     uint32_t* hrow = blockhist + (size_t)p * nblk;
-    for (uint32_t b0 = 0; b0 < nblk; b0 += 32) {
-      const uint32_t b = b0 + lane;
-      const uint32_t v = b < nblk ? hrow[b] : 0u;
-      uint32_t incl = v;
-#pragma unroll
-      for (int off = 1; off < 32; off <<= 1) {
-        const uint32_t x = __shfl_up_sync(0xFFFFFFFFu, incl, off);
-        if (lane >= (uint32_t)off) incl += x;
-      }
-      if (b < nblk) hrow[b] = carry + incl - v;
-      carry += __shfl_sync(0xFFFFFFFFu, incl, 31);
-    }
+    const uint32_t carry = warp_col_scan(hrow, hrow, nblk);
     if (lane == 0) { s_off[p] = carry; sel[p] = carry != 0; }
   }
   __syncthreads();
@@ -216,26 +198,18 @@ __global__ void __launch_bounds__(256) k_rq_merge(const RqMergeArgs a) {
   for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n; t += gridDim.x * blockDim.x) {
     const bool is_live = t < n_live;
     const uint32_t x = is_live ? t : t - n_live;
-    const uint32_t* s_off = is_live ? s_live : s_rq;
-    uint32_t p = 0, e = a.n_segs;  // the last partition whose first index is <= x
-    while (e - p > 1) { const uint32_t mid = (p + e) >> 1; if (s_off[mid] <= x) p = mid; else e = mid; }
-    uint32_t dst;
+    const uint32_t p = last_le(is_live ? s_live : s_rq, 0, a.n_segs, x);
     if (is_live) {  // + the requeued entries of p that are older
       const uint32_t u = a.live.seq[x] - a.seq_next;
-      uint32_t l = s_rq[p], r = s_rq[p + 1];
-      while (l < r) { const uint32_t mid = (l + r) >> 1; if (a.grp_u[mid] < u) l = mid + 1; else r = mid; }
-      dst = s_live[p] + s_rq[p] + (x - s_live[p]) + (l - s_rq[p]);
-      static_cast<uint64_t*>(a.out.id)[dst] = static_cast<const uint64_t*>(a.live.id)[x];
-      a.out.rating[dst] = a.live.rating[x]; a.out.ts[dst] = a.live.ts[x]; a.out.seq[dst] = a.live.seq[x];
-      a.out.mode[dst] = a.live.mode[x];
+      const uint32_t l = first_not(s_rq[p], s_rq[p + 1], [&](uint32_t k) { return a.grp_u[k] < u; });
+      img_copy(a.out, s_live[p] + s_rq[p] + (x - s_live[p]) + (l - s_rq[p]), a.live, x);
     } else {  // + the live players of p that are older; one of the same age is a collision
       const uint32_t u = a.grp_u[x];
-      uint32_t l = s_live[p], r = s_live[p + 1];
-      while (l < r) { const uint32_t mid = (l + r) >> 1; if (a.live.seq[mid] - a.seq_next < u) l = mid + 1; else r = mid; }
+      const uint32_t l = first_not(s_live[p], s_live[p + 1], [&](uint32_t k) { return a.live.seq[k] - a.seq_next < u; });
       if (l < s_live[p + 1] && a.live.seq[l] - a.seq_next == u) { atomicOr(a.err, kRqSeqLive); continue; }
-      dst = s_live[p] + s_rq[p] + (x - s_rq[p]) + (l - s_live[p]);
+      const uint32_t dst = s_live[p] + s_rq[p] + (x - s_rq[p]) + (l - s_live[p]);
       const uint32_t i = a.grp_src[x];
-      static_cast<uint64_t*>(a.out.id)[dst] = a.id[i];
+      img_set_id(a.out, dst, a.id[i]);
       a.out.rating[dst] = a.rating[i]; a.out.ts[dst] = a.ts ? a.ts[i] : 0u; a.out.seq[dst] = a.seq[i];
       a.out.mode[dst] = a.mode[i];
     }

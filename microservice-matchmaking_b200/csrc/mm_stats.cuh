@@ -62,10 +62,8 @@ __global__ void __launch_bounds__(BLOCK) k_queue_stats(const StatArgs a) {
   // word offsets inside the record (see mm_queue_stat)
   const uint32_t o_cnt = match ? 125u : 1u, o_max = match ? 126u : 3u, o_hist = match ? 127u : 4u, o_dead = 2u;
   const uint32_t tid = threadIdx.x, lane = tid & 31;
-  geo_build<BLOCK>(geo, sec.meta.fill, a.n_segs, gridDim.x, s_gtmp);
-  const uint32_t s0 = blockIdx.x * geo.tpr;
-  if (s0 >= geo.NT) return;  // (uniform)
-  const uint32_t s1 = s0 + geo.tpr < geo.NT ? s0 + geo.tpr : geo.NT;
+  uint32_t s0, s1;
+  if (!geo_cta_run<BLOCK>(geo, sec.meta.fill, a.n_segs, s_gtmp, s0, s1)) return;  // (uniform)
   for (uint32_t i = tid; i < kWaitBuckets; i += BLOCK) s_hist[i] = 0;
   if (tid == 0) { s_cnt = 0; s_dead = 0; s_max = 0; }
   __syncthreads();
@@ -99,16 +97,14 @@ __global__ void __launch_bounds__(BLOCK) k_queue_stats(const StatArgs a) {
     if (o < d.nvalid) {
       const size_t slot = (size_t)d.phys * kTile + o;
       const uint2 m2 = __ldcs(reinterpret_cast<const uint2*>(sec.mode + slot));
-      const uint4 t0 = __ldcs(reinterpret_cast<const uint4*>(sec.ts + slot));
-      const uint4 t1 = __ldcs(reinterpret_cast<const uint4*>(sec.ts + slot) + 1);
+      uint32_t ts[8];
+      ld_stamps8(sec.ts + slot, ts);
       // match section: a set bit = stayed queued (virtual position s * kTile + o; 8 bits of one word)
       const uint32_t left = match ? (__ldcs(&sec.left_bits[((size_t)s * kTile + o) >> 5]) >> (o & 31)) & 0xFFu : 0u;
-      const uint32_t ts[8] = {t0.x, t0.y, t0.z, t0.w, t1.x, t1.y, t1.z, t1.w};
 #pragma unroll
       for (int j = 0; j < 8; ++j) {
         if (o + j >= d.nvalid) continue;
-        const uint32_t md = ((j < 4 ? m2.x : m2.y) >> (8 * (j & 3))) & 0xFFu;
-        if (md == MM_MODE_DEAD) { ++dead; continue; }
+        if (mode8_at(m2, j) == MM_MODE_DEAD) { ++dead; continue; }
         if ((left >> j) & 1u) continue;
         const uint32_t w = stat_wait(sec.now, ts[j]);
         b[j] = stat_bucket(w);
@@ -116,20 +112,7 @@ __global__ void __launch_bounds__(BLOCK) k_queue_stats(const StatArgs a) {
         mx = w > mx ? w : mx;
       }
     }
-    // warp-aggregated: one shared atomic per distinct bucket of the warp (one in all when the warp's 256 share it)
-    const uint32_t b0 = __shfl_sync(0xFFFFFFFFu, b[0], 0);
-    bool same = true;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) same &= b[j] == b0;
-    if (__all_sync(0xFFFFFFFFu, same)) {
-      if (lane == 0 && b0 != kNoBucket) atomicAdd(&s_hist[b0], 8u * 32u);
-    } else {
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint32_t m = __match_any_sync(0xFFFFFFFFu, b[j]);
-        if (b[j] != kNoBucket && lane == (uint32_t)(__ffs(m) - 1)) atomicAdd(&s_hist[b[j]], (uint32_t)__popc(m));
-      }
-    }
+    warp_hist8_add(s_hist, b, kNoBucket);
     cnt = __reduce_add_sync(0xFFFFFFFFu, cnt);
     dead = __reduce_add_sync(0xFFFFFFFFu, dead);
     mx = __reduce_max_sync(0xFFFFFFFFu, mx);
