@@ -308,6 +308,70 @@ typedef struct mm_backfill_req {
 int mm_backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_taken, uint64_t* member_ids,
                 uint64_t member_cap, uint32_t* n_total);
 
+/* EXTENSION (widening search, DESIGN.md §6): the longer a player has waited, the wider the range of ratings it
+ * accepts.  The tick's max_spread (policy S1) is one window for the whole pool; mm_widen forms lobbies around the
+ * players who have waited longest, each in a window of its own that grows with its wait.  A separate call: the tick is
+ * unchanged. */
+#define MM_WIDEN_OFF 0xFFFFFFFFu
+/* one rule per (mode, group) queue, in mm_queue_stats record order (mode * n_groups + group) */
+typedef struct mm_widen_rule {
+  uint32_t min_wait;  /* anchors: live queued players whose WAIT >= min_wait; MM_WIDEN_OFF = queue not touched     */
+  uint32_t step;      /* > 0                                                                                       */
+  int32_t w0;         /* >= 0: window (rating points, either side) of a player at exactly min_wait                 */
+  int32_t inc;        /* >= 0: added per whole `step` of wait past min_wait                                        */
+  int32_t w_max;      /* >= w0                                                                                     */
+  uint32_t reserved;  /* 0                                                                                         */
+} mm_widen_rule;      /* 24 bytes */
+
+typedef struct mm_widen_stats {
+  uint32_t n_anchors;   /* anchors considered                                              */
+  uint32_t n_lobbies, n_matched;
+  uint32_t n_absorbed;  /* anchors an earlier lobby of the call had already taken          */
+  float device_us;      /* CUDA-event time of the call's device work                       */
+  uint32_t reserved[3];
+} mm_widen_stats;       /* 32 bytes */
+
+/* mm_widen: WAIT is the definition of mm_queue_stats, c(x) the tick's key clamp (x clamped to [rmin - 1, rmax + 1], as
+ * in mm_backfill) and AGE ORDER (seq - seq_next) mod 2^32 ascending.  Every queue q whose rule is not MM_WIDEN_OFF is
+ * served on its own, with L = teams x team_size of its mode:
+ *   U = the live queued players of q (across all partitions of a wide group)
+ *   A = the players of U with WAIT >= min_wait, in age order
+ *   for a in A:
+ *     if a is not in U: a is ABSORBED (an earlier lobby took it); next
+ *     w = min(w_max, w0 + floor((WAIT(a) - min_wait) / step) * inc)                (64-bit)
+ *     C = the players x of U with |c(r_x) - c(r_a)| <= w, ranked by (|c(r_x) - c(r_a)|, c(r_x), age)
+ *     if |C| < L: a stays queued; next                                             (all or nothing)
+ *     the first L of C form a lobby and leave U
+ * Only the anchor's window counts: widening favours the player who waited, and a lobby spans at most 2w.  Members of
+ * a lobby are in (c(rating), age) order, so team t is members [tS, (t+1)S) (the tick's S0 member order in rating
+ * order).  lobbies are ordered by (mode, group, emission order within the queue), group = the queue's group,
+ * first_member into member_ids (handles on MM_F_DENSE_IDS engines).  A default group holds its out-of-range players
+ * at their clamped ratings; with overlapping groups distances are in ratings, not in key indices.  Widening never
+ * crosses a group boundary.
+ * THE ANCHOR IS IN ITS OWN LOBBY whenever stamps never decrease with age (an older anchor of the same rating that
+ * failed would make this one fail too), which SearchPool's ingest and requeue keep.  Otherwise (e.g. after mm_merge) an
+ * anchor with at least L older untaken players of its rating forms their lobby and stays queued itself.
+ * Taken players leave the pool exactly as mm_take takes them: their slots are dead until the next tick and count in
+ * n_removed; they stay in the active set as matched players (mm_locate state 2, mm_requeue code 1, mm_remove forgets
+ * them).  The last tick's results, the match section of mm_queue_stats, mm_match_quality, the lobby budget and its
+ * report, the snapshot, the mm_enqueue_rejects list, pending async_results copies and the options are left alone;
+ * widen lobbies are outside the tick's lobby budget, as mm_band_match's are.
+ * Refusals, all decided before anything changes (mm_last_error names the cause):
+ *   MM_E_ARG   a null e, rules or stats; on a queue that is not MM_WIDEN_OFF: step 0, w0 < 0, inc < 0, w_max < w0 or
+ *              reserved != 0; an MM_ORDER_ARRIVAL engine (windows need rating order);
+ *   MM_E_STATE an MM_F_NO_DEDUPE engine (no active set holds matched players), a staged packed batch;
+ *   MM_E_CAP   lobby_cap or member_cap too small: stats holds the counts and nothing is taken (zero capacities: a dry
+ *              run).
+ * Cost: one pass over the mode and stamp columns of the served queues' partitions, a rank per anchor, one warp per
+ * queue walking the per-bin totals sequentially over its anchors (a queue with very many anchors dominates the call),
+ * and the backfill gather over the partitions holding a taken player.  Only the rules, headers, members and stats
+ * cross PCIe.
+ *
+ * EQUIVALENCE.  The call leaves the engine in the state mm_take of the returned ids would leave it in: every later
+ * call sequence gives the same results on both engines.                                                           */
+int mm_widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
+             uint64_t* member_ids, uint64_t member_cap, mm_widen_stats* stats);
+
 /* Replaces ActiveUser.in_queue?/1 (models/active_user.ex:33-44), batched.          */
 int mm_in_queue(mm_engine* e, uint32_t n, const uint64_t* id, uint8_t* out);
 

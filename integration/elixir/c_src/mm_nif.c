@@ -455,6 +455,40 @@ static ERL_NIF_TERM nif_backfill(ErlNifEnv* env, int argc, const ERL_NIF_TERM ar
   return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &taken), enif_make_binary(env, &hs));
 }
 
+/* widen(ref, now :: u64, rules :: binary(mm_widen_rule[n_modes * n_groups]))
+ *   -> {:ok, lobbies :: binary(mm_lobby_hdr[]), handles :: binary(u32[])}: lobbies formed around the players who waited longest, each in a rating window that grows
+ * with its wait (mm_widen).  badarg unless the binary holds exactly one rule per (mode, group) queue.  The buffers are
+ * sized from the dry run's counts (zero capacities). */
+static ERL_NIF_TERM nif_widen(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifUInt64 now; ErlNifBinary rb, lb, hs; mm_widen_stats st; uint32_t nq = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_uint64(env, argv[1], &now) ||
+      !enif_inspect_binary(env, argv[2], &rb))
+    return enif_make_badarg(env);
+  mm_lobby_candidates(r->e, NULL, 0, &nq);  /* cap 0: only the number of queues; mm_widen reads one rule for each */
+  if (rb.size != (size_t)nq * sizeof(mm_widen_rule)) return enif_make_badarg(env);
+  mm_widen_rule* rules = enif_alloc(rb.size + 1);
+  if (!rules) return err(env, MM_E_CAP);
+  memcpy(rules, rb.data, rb.size);
+  int rc = mm_widen(r->e, now, rules, NULL, 0, NULL, 0, &st);  /* the dry run: counts only */
+  if (rc == MM_E_CAP || rc == MM_OK) {
+    const uint32_t nl = st.n_lobbies, nm = st.n_matched;
+    uint64_t* id = enif_alloc(8 * (size_t)nm + 8);
+    if (!id || !enif_alloc_binary(sizeof(mm_lobby_hdr) * (size_t)nl, &lb)) rc = MM_E_CAP;
+    else if (!enif_alloc_binary(4 * (size_t)nm, &hs)) { enif_release_binary(&lb); rc = MM_E_CAP; }
+    else {
+      rc = mm_widen(r->e, now, rules, (mm_lobby_hdr*)lb.data, nl, id, nm, &st);
+      if (rc) { enif_release_binary(&lb); enif_release_binary(&hs); }
+      else
+        for (uint32_t k = 0; k < nm; ++k) { const uint32_t h = (uint32_t)id[k]; memcpy(hs.data + 4 * (size_t)k, &h, 4); }
+    }
+    enif_free(id);
+  }
+  enif_free(rules);
+  if (rc) return err(env, rc);
+  return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &lb), enif_make_binary(env, &hs));
+}
+
 /* locate(ref, now :: u64, handles :: binary(u32[])) -> {:ok, records :: binary(mm_player_status[])}: where each
  * player's search stands (mm_locate): state, queue, wait at `now`, players ahead and queue depth, and the lobby ordinal
  * / member index the next tick gives it (0xFFFFFFFF: it stays queued). */
@@ -554,6 +588,7 @@ static ErlNifFunc funcs[] = {
   {"import_regroup_many", 4, nif_import_regroup_many, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"backfill", 2, nif_backfill, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"widen", 3, nif_widen, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"locate", 3, nif_locate, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"seq_next", 1, nif_seq_next, 0},
   {"set_max_spread", 2, nif_set_max_spread, 0},

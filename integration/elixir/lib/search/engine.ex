@@ -126,6 +126,14 @@ defmodule Matchmaking.Search.Engine do
   """
   def backfill(_ref, _requests), do: :erlang.nif_error(:nif_not_loaded)
   @doc """
+  Widening search (extension): lobbies formed around the players who waited longest, each in a rating window that
+  grows with its wait (mm_widen).  rules: binary of n_modes * n_groups 24-byte records <<min_wait::little-32,
+  step::little-32, w0::little-signed-32, inc::little-signed-32, w_max::little-signed-32, 0::32>>, queue
+  mode * n_groups + group, min_wait 0xFFFFFFFF = off -> {:ok, lobbies :: binary(mm_lobby_hdr[]), handles ::
+  binary(u32[])}; the members leave the pool and stay in the active set until remove_user.
+  """
+  def widen(_ref, _now, _rules), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
   Search status (extension): where each player's search stands (mm_locate).  handles: binary(u32[]) -> {:ok, records}:
   36-byte records <<state, mode, group, 0, rating::little-signed-32, enq_ts::little-32, seq::little-32,
   wait::little-32, ahead::little-32, depth::little-32, lobby::little-32, member::little-16, 0::16>>; state 0 gone,

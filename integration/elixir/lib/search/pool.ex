@@ -17,6 +17,11 @@ defmodule Matchmaking.Search.Pool do
       search_timeout_ms   option (extension, default nil = off): after each tick's lobbies are published, the players
                      still queued who have waited at least this long leave the pool (Engine.expire_packed) and get the
                      error response of game-lobby/worker.ex:63-71,105-116 on their "response-queue"
+      widen          option (extension, default nil = off, needs a rating-order engine): %{mode name => {min_wait_ms,
+                     w0, step_ms, inc, w_max}}.  After each tick's lobbies are published, and before the search timeout,
+                     every player of the mode who has waited at least min_wait_ms anchors a lobby in a rating window of
+                     w0 points either side, plus inc per whole step_ms past min_wait_ms, at most w_max (Engine.widen);
+                     its lobbies are published like the tick's
       lobby_budget   option (extension, default nil = no limit): a zero-arity function -> %{mode name => lobbies}, asked
                      before every tick — the free game-server slots (game-lobby/worker.ex:118-141).  The tick emits at
                      most that many lobbies of the mode, shared over the rating groups in proportion to what each could
@@ -110,7 +115,8 @@ defmodule Matchmaking.Search.Pool do
     st = %{ref: ref, staged: [], n_staged: 0, handle_of: %{}, players: %{}, free: [], next: 0, channel: nil,
            queued: %{}, moved_out: MapSet.new(),
            t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms),
-           lobby_budget: Keyword.get(opts, :lobby_budget), paused: MapSet.new(), regroup_dropped: []}
+           lobby_budget: Keyword.get(opts, :lobby_budget), paused: MapSet.new(), regroup_dropped: [],
+           widen: Keyword.get(opts, :widen)}
     case resume(st, Keyword.get(opts, :resume), Keyword.get(opts, :regroup, false)) do
       {:ok, st} ->
         Process.send_after(self(), :flush, @flush_ms)
@@ -439,7 +445,7 @@ defmodule Matchmaking.Search.Pool do
     now = now_ms(st)
     if st.lobby_budget, do: set_budget(st, st.lobby_budget.())
     case Engine.tick_packed(st.ref, now) do
-      {:ok, lobbies, members, _stats} -> {:noreply, expire(publish(lobbies, members, st), now)}
+      {:ok, lobbies, members, _stats} -> {:noreply, expire(widen(publish(lobbies, members, st), now), now)}
       {:error, _reason} -> {:noreply, st}                              # nothing was consumed; the next tick retries
     end
   end
@@ -461,6 +467,23 @@ defmodule Matchmaking.Search.Pool do
     st = %{st | paused: paused}
     if st.lobby_budget == nil, do: set_budget(st, nil)   # with a callback the next tick sets both together
     {:reply, :ok, st}
+  end
+
+  # -- widening search (extension): before the timeout, so a player who waited long gets its widest window first ----
+  defp widen(%{widen: nil} = st, _now), do: st
+  defp widen(st, now) do
+    rules = for m <- 0..(Engine.n_modes() - 1), _g <- 0..(Engine.n_groups() - 1), into: <<>> do
+      case Map.get(st.widen, Engine.mode_name(m)) do
+        {min_wait, w0, step, inc, w_max} ->
+          <<min_wait::little-32, step::little-32, w0::little-signed-32, inc::little-signed-32, w_max::little-signed-32,
+            0::32>>
+        nil -> <<0xFFFFFFFF::little-32, 1::little-32, 0::32, 0::32, 0::32, 0::32>>
+      end
+    end
+    case Engine.widen(st.ref, now, rules) do
+      {:ok, lobbies, members} -> publish(lobbies, members, st)
+      {:error, _reason} -> st                                          # nothing was taken
+    end
   end
 
   # -- search timeout (extension): after the lobbies, so a player the tick matched is never timed out ---------------

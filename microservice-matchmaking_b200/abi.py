@@ -101,6 +101,33 @@ class BackfillReq(C.Structure):
     ]
 
 
+MM_WIDEN_OFF = 0xFFFFFFFF
+
+
+class WidenRule(C.Structure):
+    """mm_widen_rule: the widening window of one (mode, group) queue (24 bytes)."""
+    _fields_ = [
+        ("min_wait", C.c_uint32),
+        ("step", C.c_uint32),
+        ("w0", C.c_int32),
+        ("inc", C.c_int32),
+        ("w_max", C.c_int32),
+        ("reserved", C.c_uint32),
+    ]
+
+
+class WidenStats(C.Structure):
+    """mm_widen_stats: counts of one mm_widen call (32 bytes)."""
+    _fields_ = [
+        ("n_anchors", C.c_uint32),
+        ("n_lobbies", C.c_uint32),
+        ("n_matched", C.c_uint32),
+        ("n_absorbed", C.c_uint32),
+        ("device_us", C.c_float),
+        ("reserved", C.c_uint32 * 3),
+    ]
+
+
 MM_LOCATE_STAYS = 0xFFFFFFFF
 
 
@@ -223,6 +250,7 @@ PROTOTYPES = {
     "mm_band_match": (C.c_int, [_vp, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, _vp, _vp, _vp, C.c_uint32,
                                 _vp, C.c_uint32, _vp, C.c_uint64, _vp, _P(BandStats)]),
     "mm_backfill": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, C.c_uint64, _P(C.c_uint32)]),
+    "mm_widen": (C.c_int, [_vp, C.c_uint64, _vp, _vp, C.c_uint32, _vp, C.c_uint64, _P(WidenStats)]),
     "mm_in_queue": (C.c_int, [_vp, C.c_uint32, _vp, _vp]),
     "mm_locate": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp]),
     "mm_pool_size": (C.c_int, [_vp, _P(C.c_uint32)]),

@@ -30,6 +30,7 @@
 #include "mm_regroup.cuh"
 #include "mm_requeue.cuh"
 #include "mm_stats.cuh"
+#include "mm_widen.cuh"
 
 using namespace mm;
 
@@ -283,6 +284,15 @@ struct mm_engine {
     DevArray<BfPiece> piece;
     DevArray<uint64_t> staging, members;
   } bf;
+
+  // mm_widen (mm_widen.cuh): the call's tables and the anchors, grown on demand; the plan's rem, the keys, the pieces,
+  // the staging and the members are the backfill arrays above
+  struct Widen {
+    DevArray<uint32_t> tab;  // rules [n_cut] | qlob | qlbase | qmbase [n_cut] | part [n_segs + 1] | cur [n_segs] | cta
+                             // [grid] | rmap [n_chunks] | ctr [kWdWords]
+    DevArray<uint32_t> anc;  // rec (2 words) | slot | age | rank | mbase, each [anchors]
+    DevArray<mm_lobby_hdr> hdr;
+  } wd;
 
   // mm_locate (mm_locate.cuh): the queried ids, the records and the call's tables (preview bases, member slots,
   // budgets, reverse chunk map), grown on demand; no other call reads or writes them
@@ -2114,6 +2124,24 @@ int band_match(mm_engine* e, int32_t W, uint32_t g_first, uint32_t g_last, uint3
 }
 
 // ---- mm_backfill (mm_backfill.cuh) ---------------------------------------------------------------------------------
+// The prefixes k_bf_keys made keys (counters h) leave the pool: the band gather over the keys' partitions places them
+// into bf.staging at kbase[key] + rank and takes them.  bf.members is sized for them too.
+int bf_take(mm_engine* e, const uint32_t* h) {
+  auto& s = e->bf;
+  const uint32_t total = h[kBfPlayers];
+  BandArgs a = band_args(e);
+  a.n_keys = h[kBfKeys];
+  a.kbase = s.kbase; a.klim = s.klim;
+  int rc = band_gather(e, a, h[kBfCols], BfKeyBins{s.key_bin});
+  if (rc) return rc;
+  CK(s.staging.reserve(total)); CK(s.members.reserve(total));
+  k_band_limit<<<1, kBandPrepBlock, 0, e->stream>>>(a);
+  k_band_place<kBandBlock><<<band_ctas(e, e->pool[e->cur].n), kBandBlock, 0, e->stream>>>(
+      a, BandOut{s.staging, nullptr, nullptr, 1u});
+  CK(cudaGetLastError());
+  return MM_OK;
+}
+
 int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_taken, uint64_t* member_ids,
              uint64_t member_cap, uint32_t* n_total) {
   const mm_config& c = e->cfg;
@@ -2174,15 +2202,9 @@ int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_t
   *n_total = total;
   if (member_cap < total) return set_err(e, MM_E_CAP, "need member_cap >= %u", total);
   if (total == 0) return MM_OK;
-  // from here on the call changes the pool: the band gather over the keys' partitions, placed and taken into staging
-  BandArgs a = band_args(e);
-  a.n_keys = h[kBfKeys];
-  a.kbase = s.kbase; a.klim = s.klim;
-  int rc = band_gather(e, a, h[kBfCols], BfKeyBins{s.key_bin});
+  // from here on the call changes the pool
+  int rc = bf_take(e, h);
   if (rc) return rc;
-  CK(s.staging.reserve(total)); CK(s.members.reserve(total));
-  k_band_limit<<<1, kBandPrepBlock, 0, e->stream>>>(a);
-  k_band_place<kBandBlock><<<band_ctas(e, p.n), kBandBlock, 0, e->stream>>>(a, BandOut{s.staging, nullptr, nullptr, 1u});
   std::vector<uint32_t> base(n);
   for (uint32_t j = 0, acc = 0; j < n; ++j) { base[j] = acc; acc += n_taken[j]; }
   CK(cudaMemcpyAsync(s.req_base, base.data(), (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
@@ -2192,6 +2214,104 @@ int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_t
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(member_ids, s.members, (size_t)total * 8, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
+// ---- mm_widen (mm_widen.cuh) ---------------------------------------------------------------------------------------
+int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
+          uint64_t* member_ids, uint64_t member_cap, mm_widen_stats* st) {
+  const mm_config& c = e->cfg;
+  const uint32_t G = c.n_groups, nc = e->n_cut;
+  std::vector<WdRule> rule(nc);
+  bool any = false;
+  for (uint32_t q = 0; q < nc; ++q) {
+    const mm_widen_rule& r = rules[q];
+    const mm_mode_desc& md = c.modes[q / G];
+    rule[q] = WdRule{r.min_wait, r.step, r.w0, r.inc, r.w_max, (uint32_t)md.teams * md.team_size};
+    if (r.min_wait == MM_WIDEN_OFF) continue;
+    if (r.step == 0 || r.w0 < 0 || r.inc < 0 || r.w_max < r.w0 || r.reserved)
+      return set_err(e, MM_E_ARG, "rule %u (mode %u, group %u): need step > 0, w0 >= 0, inc >= 0, w_max >= w0 and "
+                     "reserved = 0", q, q / G, q % G);
+    any = true;
+  }
+  if (c.order_mode != MM_ORDER_RATING) return set_err(e, MM_E_ARG, "widening windows need MM_ORDER_RATING");
+  if (!e->use_active) return set_err(e, MM_E_STATE, "an MM_F_NO_DEDUPE engine cannot hold taken players");
+  if (e->stage_count) return staged_err(e);
+  const Pool& p = e->pool[e->cur];
+  if (!any || p.n == 0) return MM_OK;
+  auto& s = e->wd;
+  auto& b = e->bf;
+  CK(cudaEventRecord(e->ev[0], e->stream));
+  const uint32_t ctas = tile_ctas(e, p.n), rw = sizeof(WdRule) / 4;
+  const size_t o_qlob = rw * nc, o_qlb = o_qlob + nc, o_qmb = o_qlb + nc, o_part = o_qmb + nc,
+               o_cur = o_part + e->n_segs + 1, o_cta = o_cur + e->n_segs, o_rmap = o_cta + ctas,
+               o_ctr = o_rmap + e->n_chunks;
+  CK(s.tab.reserve(o_ctr + kWdWords));
+  uint32_t* t = s.tab;
+  CK(cudaMemcpyAsync(t, rule.data(), nc * sizeof(WdRule), cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemsetAsync(t + o_part, 0, (size_t)(e->n_segs + 1) * 4, e->stream));
+  CK(cudaMemsetAsync(t + o_cta, 0, (size_t)ctas * 4, e->stream));
+  CK(cudaMemsetAsync(t + o_ctr, 0, kWdWords * 4, e->stream));
+  WdArgs a{};
+  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.n_cut = nc; a.n_groups = G; a.now = (uint32_t)now;
+  a.seq_next = e->seq_next; a.rule = reinterpret_cast<const WdRule*>(t); a.part_cut = e->d_part_cut;
+  a.cut_lp_lo = e->d_cut_lp_lo; a.seg_bin_lo = e->d_seg_bin_lo; a.bin_seg = e->d_bin_seg; a.bin_key = e->d_bin_key;
+  a.tot = p.m.tot; a.rmap = t + o_rmap; a.cta = t + o_cta; a.part = t + o_part; a.cur = t + o_cur;
+  a.qlob = t + o_qlob; a.qlbase = t + o_qlb; a.qmbase = t + o_qmb; a.ctr = t + o_ctr;
+  // anchors: counted, then written in (partition, age) order
+  k_wd_anchors<kWdBlock><<<ctas, kWdBlock, 0, e->stream>>>(a, 0);
+  k_wd_part_scan<<<1, 1024, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  uint32_t na = 0;
+  CK(cudaMemcpyAsync(&na, t + o_part + e->n_segs, 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  st->n_anchors = na;
+  if (na == 0) return MM_OK;
+  CK(s.anc.reserve((size_t)na * 6));
+  a.n_anchors = na; a.rec = reinterpret_cast<uint2*>(s.anc.p);  // first: 8-byte aligned
+  a.a_slot = s.anc + 2 * (size_t)na; a.a_age = s.anc + 3 * (size_t)na; a.a_rank = s.anc + 4 * (size_t)na;
+  a.mbase = s.anc + 5 * (size_t)na;
+  const size_t K = e->K;
+  CK(b.rem.reserve(K)); CK(b.key_bin.reserve(K)); CK(b.kbase.reserve(K)); CK(b.klim.reserve(K));
+  CK(b.piece.reserve(na + K));  // every bin a lobby reaches but its last is emptied: at most lobbies + K pieces
+  CK(cudaMemcpyAsync(b.rem, p.m.tot, K * 4, cudaMemcpyDeviceToDevice, e->stream));
+  a.rem = b.rem; a.piece = b.piece;
+  k_wd_anchors<kWdBlock><<<ctas, kWdBlock, 0, e->stream>>>(a, 1);
+  k_loc_rmap<<<e->n_segs, 256, 0, e->stream>>>(p.m, t + o_rmap);
+  k_wd_rank<<<(uint32_t)(((size_t)na * 32 + 255) / 256), 256, 0, e->stream>>>(a);
+  // plan on the per-bin totals, then the bins with a take as keys
+  k_wd_plan<<<(nc + kWdPlanWarps - 1) / kWdPlanWarps, kWdPlanWarps * 32, 0, e->stream>>>(a);
+  BfArgs f{};
+  f.tot = p.m.tot; f.rem = b.rem; f.bin_seg = e->d_bin_seg; f.fill = p.m.fill; f.K = e->K;
+  f.key_bin = b.key_bin; f.kbase = b.kbase; f.klim = b.klim; f.ctr = a.ctr;
+  k_bf_keys<<<1, kBfKeysBlock, 0, e->stream>>>(f);
+  k_wd_bases<<<1, 32, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  uint32_t h[kWdWords];
+  CK(cudaMemcpyAsync(h, a.ctr, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  const uint32_t nl = h[kWdLobbies], nm = h[kBfPlayers];
+  st->n_lobbies = nl; st->n_matched = nm; st->n_absorbed = h[kWdAbsorbed];
+  if (lobby_cap < nl || member_cap < nm)
+    return set_err(e, MM_E_CAP, "need lobby_cap >= %u and member_cap >= %u", nl, nm);
+  if (nl == 0) return MM_OK;
+  // from here on the call changes the pool
+  int rc = bf_take(e, h);
+  if (rc) return rc;
+  CK(s.hdr.reserve(nl));
+  a.hdr = s.hdr;
+  k_wd_hdr<<<(nl + 255) / 256, 256, 0, e->stream>>>(a, nl);
+  const uint32_t np = h[kBfPieces];
+  k_bf_out<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, a.mbase,
+                                                                               b.staging, b.members);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e->ev[4], e->stream));
+  CK(cudaMemcpyAsync(lobbies, s.hdr, (size_t)nl * sizeof(mm_lobby_hdr), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(member_ids, b.members, (size_t)nm * 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]));
+  st->device_us = ms * 1000.f;
   return MM_OK;
 }
 
@@ -2655,6 +2775,18 @@ int mm_backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* 
   std::lock_guard<std::mutex> lk(e->mu);
   CK(cudaSetDevice(e->device));
   return backfill(e, n, req, n_taken, member_ids, member_cap, n_total);
+}
+
+int mm_widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
+             uint64_t* member_ids, uint64_t member_cap, mm_widen_stats* stats) {
+  if (!e) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!rules || !stats) return set_err(e, MM_E_ARG, "null rules or stats");
+  std::memset(stats, 0, sizeof(*stats));
+  if ((lobby_cap && !lobbies) || (member_cap && !member_ids))
+    return set_err(e, MM_E_ARG, "null lobbies or member_ids with a non-zero capacity");
+  CK(cudaSetDevice(e->device));
+  return widen(e, now, rules, lobbies, lobby_cap, member_ids, member_cap, stats);
 }
 
 int mm_remove_packed(mm_engine* e, uint32_t n, const uint32_t* handle, uint32_t* n_removed) {

@@ -31,6 +31,28 @@ __global__ void k_loc_rmap(const PoolMeta m, uint32_t* __restrict__ rmap) {
   for (uint32_t k = threadIdx.x; k < nch; k += blockDim.x) rmap[__ldg(&m.chunk_tab[(size_t)sg * m.max_ch + k])] = k;
 }
 
+// One warp: the live players of bin v (partition sg) stored before `slot` in the partition — the player's rank in its
+// bin in enqueue order.  Every lane gets the answer.
+__device__ __forceinline__ uint32_t bin_rank(const PoolView& pool, const PoolMeta& meta, const uint32_t* seg_bin_lo,
+                                             const uint32_t* rmap, uint32_t slot, uint32_t v, uint32_t sg) {
+  const uint32_t lane = threadIdx.x & 31, chunk = slot / kTile, off = slot % kTile;
+  const uint32_t k = rmap[chunk];
+  const uint32_t* tab = meta.chunk_tab + (size_t)sg * meta.max_ch;
+  uint32_t rank = 0;
+  if (meta.chist) {
+    const uint32_t key = v - seg_bin_lo[sg];
+    for (uint32_t j = lane; j < k; j += 32) rank += meta.chist[(size_t)tab[j] * kChunkHist + key];
+  } else {
+    for (uint32_t j = 0; j < k; ++j) {
+      const uint16_t* b = pool.bin + (size_t)tab[j] * kTile;
+      for (uint32_t o = lane; o < kTile; o += 32) rank += b[o] == v ? 1u : 0u;
+    }
+  }
+  const uint16_t* own = pool.bin + (size_t)chunk * kTile;
+  for (uint32_t o = lane; o < off; o += 32) rank += own[o] == v ? 1u : 0u;
+  return __reduce_add_sync(0xFFFFFFFFu, rank);
+}
+
 struct LocateArgs {
   uint32_t n;
   const uint64_t* id;        // [n] queried ids (handles on MM_F_DENSE_IDS engines)
@@ -76,22 +98,8 @@ __global__ void __launch_bounds__(256) k_locate(const LocateArgs a) {
     if (lane == 0) a.out[q] = r;
     return;
   }
-  const uint32_t v = a.pool.bin[slot], sg = a.bin_seg[v], chunk = slot / kTile, off = slot % kTile;
-  const uint32_t k = a.rmap[chunk];
-  const uint32_t* tab = a.meta.chunk_tab + (size_t)sg * a.meta.max_ch;
-  uint32_t rank = 0;
-  if (a.meta.chist) {
-    const uint32_t key = v - a.seg_bin_lo[sg];
-    for (uint32_t j = lane; j < k; j += 32) rank += a.meta.chist[(size_t)tab[j] * kChunkHist + key];
-  } else {
-    for (uint32_t j = 0; j < k; ++j) {
-      const uint16_t* b = a.pool.bin + (size_t)tab[j] * kTile;
-      for (uint32_t o = lane; o < kTile; o += 32) rank += b[o] == v ? 1u : 0u;
-    }
-  }
-  const uint16_t* own = a.pool.bin + (size_t)chunk * kTile;
-  for (uint32_t o = lane; o < off; o += 32) rank += own[o] == v ? 1u : 0u;
-  rank = __reduce_add_sync(0xFFFFFFFFu, rank);
+  const uint32_t v = a.pool.bin[slot], sg = a.bin_seg[v];
+  const uint32_t rank = bin_rank(a.pool, a.meta, a.seg_bin_lo, a.rmap, slot, v, sg);
   if (lane != 0) return;
   const uint32_t c = a.part_cut[sg], b0 = a.seg_bin_lo[a.cut_lp_lo[c]], b1 = a.seg_bin_lo[a.cut_lp_lo[c + 1]];
   r.state = 1;

@@ -409,6 +409,38 @@ class Engine:
                 return n_taken, []
             return n_taken, np.split(mem[:total.value], np.cumsum(n_taken.astype(np.int64))[:-1])
 
+    # -- widening search (mm_widen) --------------------------------------------------------------------------------
+    WIDEN_RULE_DTYPE = np.dtype([("min_wait", "<u4"), ("step", "<u4"), ("w0", "<i4"), ("inc", "<i4"),
+                                 ("w_max", "<i4"), ("reserved", "<u4")])
+
+    def widen_rules(self, rules=None):
+        """A rule array for widen(): every queue off, then rules[(mode, group)] = (min_wait, w0, step, inc, w_max)."""
+        out = np.zeros(self.cfg.n_modes * self.cfg.n_groups, self.WIDEN_RULE_DTYPE)
+        out["min_wait"] = abi.MM_WIDEN_OFF
+        out["step"] = 1
+        for (m, g), (min_wait, w0, step, inc, w_max) in (rules or {}).items():
+            out[m * self.cfg.n_groups + g] = (min_wait, step, w0, inc, w_max, 0)
+        return out
+
+    def widen(self, now, rules, lobby_cap=1 << 10, member_cap=1 << 12):
+        """Form lobbies around the live queued players who have waited at least their queue's min_wait, each in a
+        rating window that grows with its wait (mm_widen).  rules: WIDEN_RULE_DTYPE[n_modes * n_groups], or the dict
+        widen_rules() takes.  -> (lobbies[LOBBY_DTYPE], member_ids u64, WidenStats).  An MM_E_CAP refusal is retried
+        once with its counts."""
+        if isinstance(rules, dict):
+            rules = self.widen_rules(rules)
+        rules = np.ascontiguousarray(rules, self.WIDEN_RULE_DTYPE)
+        for attempt in range(2):
+            lob = np.empty(max(lobby_cap, 1), LOBBY_DTYPE)
+            mem = np.empty(max(member_cap, 1), np.uint64)
+            st = abi.WidenStats()
+            rc = self.lib.mm_widen(self.h, int(now), _p(rules), _p(lob), lobby_cap, _p(mem), member_cap, C.byref(st))
+            if rc == abi.MM_E_CAP and attempt == 0:
+                lobby_cap, member_cap = max(lobby_cap, st.n_lobbies), max(member_cap, st.n_matched)
+                continue
+            self._check(rc, "mm_widen")
+            return lob[:st.n_lobbies], mem[:st.n_matched], st
+
     def in_queue(self, ids):
         ids = np.ascontiguousarray(ids, np.uint64)
         out = np.empty(len(ids), np.uint8)

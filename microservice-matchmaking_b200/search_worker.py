@@ -32,6 +32,8 @@ import math
 
 import numpy as np
 
+from . import abi
+
 # module attributes of the reference (worker.ex:23-40)
 DEFAULT_EXCHANGE_PATH = "open-matchmaking.matchmaking"
 DEFAULT_EXCHANGE_TYPE = "direct"
@@ -133,8 +135,8 @@ class WindowSchedule:
         W(now) = min(w_max, w0 + growth_per_s * (now - enqueue_time(oldest queued player)))
 
     so a sparse pool relaxes until its oldest player can be matched and tightens again once
-    it has left.  One window per tick for the whole pool: the per-player form needs the
-    sorted order on the device first and is future work."""
+    it has left.  One window per tick for the whole pool; per-player windows run after the
+    tick (SearchPool(widen=...), Engine.widen)."""
 
     def __init__(self, w0, growth_per_s, w_max):
         self.w0, self.growth_per_s, self.w_max = int(w0), float(growth_per_s), int(w_max)
@@ -162,6 +164,11 @@ class SearchPool:
     the mode (Engine.set_lobby_budget), shared over the rating groups in proportion to what each could emit; the rest
     stay ordinary queued players (timeout_ms, requeue, move_out, checkpoint treat them as such).  pause() / resume_queues()
     set single queues to 0 / unlimited.  A checkpoint does not carry budgets or pauses: resume() starts unlimited.
+    widen: optional per-player search windows (extension; needs MM_ORDER_RATING): {mode name: (min_wait_ms, w0,
+    step_ms, inc, w_max)}.  After each tick's lobbies are published, and before timeout_ms expires anyone, every player
+    of the mode who has waited at least min_wait_ms anchors a lobby in a rating window of w0 points either side, plus
+    inc per whole step_ms waited past min_wait_ms, at most w_max (Engine.widen, every rating group of the mode).  Its
+    lobbies are published like the tick's; stats["widened"] counts them.
 
     Every ingest batch is stamped with now_ms(), the clock in milliseconds since the pool was created (u32, wraps
     after 49 days), and every tick passes the same clock as its `now`: the engine's per-queue waits
@@ -169,9 +176,13 @@ class SearchPool:
     """
 
     def __init__(self, engine, mode_names, group_names, max_batch=65536, window=None, clock=None, flush_every_s=0.005,
-                 handle_capacity=None, timeout_ms=None, wall_clock=None, lobby_budget=None):
+                 handle_capacity=None, timeout_ms=None, wall_clock=None, lobby_budget=None, widen=None):
         import time
+        if widen and engine.cfg.order_mode != abi.MM_ORDER_RATING:
+            raise ValueError("widen needs an MM_ORDER_RATING engine: windows are rating distances")
         self.window = window
+        self.widen = {(i, g): tuple(int(x) for x in widen[m]) for i, m in enumerate(mode_names) if m in (widen or {})
+                      for g in range(len(group_names))}
         self.timeout_ms = timeout_ms
         self.lobby_budget = lobby_budget
         self.paused = set()  # queues (mode * n_groups + group) that emit nothing until resume_queues()
@@ -199,6 +210,8 @@ class SearchPool:
         self.stats = {"enqueued": 0, "duplicates": 0, "invalid": 0, "lobbies": 0, "failed_batches": 0}
         if timeout_ms is not None:
             self.stats["timed_out"] = 0
+        if self.widen:
+            self.stats["widened"] = 0
 
     def now_ms(self):
         """The pool's clock: milliseconds since the pool was created, modulo 2^32 (the engine's enq_ts / now)."""
@@ -412,6 +425,20 @@ class SearchPool:
         if self.lobby_budget is not None:
             self._set_budget(self.lobby_budget())
         lob, mem, _seq, _st = self.engine.tick(now)
+        self._publish(lob, mem)
+        self.stats["lobbies"] += len(lob)
+        n_lob = len(lob)
+        if self.widen:  # before the timeout: a player who waited long gets its widest window before it is dropped
+            wlob, wmem, _st = self.engine.widen(now, self.widen)
+            self._publish(wlob, wmem)
+            self.stats["widened"] += len(wlob)
+            n_lob += len(wlob)
+        if self.timeout_ms is not None:  # after the lobbies: a player this tick matched is never timed out
+            self._expire(now)
+        return n_lob
+
+    def _publish(self, lob, mem):
+        """Publish each lobby like prepare_game_lobby/4, through the worker of its group."""
         for h in lob:
             mode_name = self.mode_names[h["mode"]]
             group_name = self.group_names[h["group"]]
@@ -427,10 +454,6 @@ class SearchPool:
             payload = json.dumps({"teams": teams, "game-mode": mode_name})      # worker.ex:315-318
             worker = self.workers.get(group_name) or next(iter(self.workers.values()))
             worker.prepare_game_lobby(worker.channel_name, EXCHANGE_FORWARD, QUEUE_FORWARD, payload)
-        self.stats["lobbies"] += len(lob)
-        if self.timeout_ms is not None:  # after the lobbies: a player this tick matched is never timed out
-            self._expire(now)
-        return len(lob)
 
     # -- lobby budget ------------------------------------------------------------------------
     def _queues(self, group_names, mode_names):
