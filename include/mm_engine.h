@@ -87,7 +87,9 @@ typedef struct mm_config {
 } mm_config;
 
 /* One emitted lobby.  Members are member_ids[first_member .. first_member+n_members)
- * in join order; team t = members [t*S, (t+1)*S)  (policy S0: first team with room).
+ * in join order; team t = members [t*S, (t+1)*S)  (policy S0: first team with room; with
+ * mm_set_option("team_balance") the members of a balanced mode are reordered into the
+ * two teams with the least rating difference, and team t is still [t*S, (t+1)*S)).
  * Replaces the payload built at search/worker.ex:315-319.                           */
 typedef struct mm_lobby_hdr {
   uint32_t first_member;
@@ -104,6 +106,7 @@ typedef struct mm_tick_stats {
   uint32_t n_dead;        /* removed-while-queued players dropped by this tick         */
   uint32_t n_launches;    /* kernels launched by this tick                             */
   float device_us;        /* CUDA-event time of the whole tick on the engine's stream  */
+                          /* (with "team_balance": plus its balance pass)              */
   float place_us;         /* CUDA-event time of the dominant kernel: placement + pool  */
                           /* compaction (fused tick: until the last row has compacted) */
   float hist_us;          /* ... of the histogram kernel                               */
@@ -344,7 +347,8 @@ typedef struct mm_widen_stats {
  *     the first L of C form a lobby and leave U
  * Only the anchor's window counts: widening favours the player who waited, and a lobby spans at most 2w.  Members of
  * a lobby are in (c(rating), age) order, so team t is members [tS, (t+1)S) (the tick's S0 member order in rating
- * order).  lobbies are ordered by (mode, group, emission order within the queue), group = the queue's group,
+ * order; "team_balance" then re-splits the lobbies of a balanced mode).  lobbies are ordered by (mode, group, emission
+ * order within the queue), group = the queue's group,
  * first_member into member_ids (handles on MM_F_DENSE_IDS engines).  A default group holds its out-of-range players
  * at their clamped ratings; with overlapping groups distances are in ratings, not in key indices.  Widening never
  * crosses a group boundary.
@@ -408,7 +412,8 @@ typedef struct mm_player_status {
  * NEXT-TICK PREDICTION.  If the next call that changes the engine is an mm_tick* of any form (any `now`) and neither
  * the options nor the lobby budget change in between, that tick puts the player at member index `member` of the
  * `lobby`-th lobby it emits from the player's queue, counting from 0 in header order; MM_LOCATE_STAYS: the tick leaves
- * the player queued.  This holds under S0, S1 (max_spread) and the per-queue and per-mode lobby budget.  Under S0
+ * the player queued.  This holds under S0, S1 (max_spread), the per-queue and per-mode lobby budget and "team_balance"
+ * (member is then the player's index in the balanced lobby).  Under S0
  * without a budget it reduces to lobby = ahead / L when ahead < floor(depth / L) * L.
  * No side effects: the pool, the active set, the snapshot, the mm_enqueue_rejects list, the last tick's results and
  * the match section of mm_queue_stats, mm_lobby_budget_report and pending async_results copies are left alone.  n = 0
@@ -529,7 +534,8 @@ int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap,
  * (tick_impl), with or without async_results and emit_seq, under S0 or S1 and any lobby budget.  per_lobby[h]
  * describes lobbies[h] of that tick; per_queue holds one record per queue, empty ones included, in the order of
  * mm_queue_stats (mode * n_groups + group).  The lobbies of mm_band_match and the players of mm_backfill are outside
- * the tick and not covered.
+ * the tick and not covered.  After a tick with "team_balance" (mm_set_option) the imbalance of a balanced lobby is
+ * that of the teams it was emitted with.
  * VOID exactly when the match section of mm_queue_stats is (before the first tick, after a tick that failed, after
  * mm_restore and after the import loads): *n_out = 0 and *n_lobbies = 0, nothing is written.
  * READ-ONLY: no other call changes the report until the next tick, and the call changes nothing — not the pool, the
@@ -844,6 +850,30 @@ int mm_set_stream(mm_engine* e, void* cuda_stream);
  *                   `value` rating points — greedy walk over the rating-sorted partition, a player whose window cannot
  *                   be filled stays queued (oracle: orc_run_windowed).  < 0 (default) = reference behaviour (S0).
  *                   MM_ORDER_RATING only (MM_E_ARG otherwise).  Takes effect from the next tick.
+ *   "team_balance"  EXTENSION (balanced teams): a mask, bit m = balance the lobbies of game mode m; 0 (default) = off.
+ *                   MM_E_ARG if a set bit names a mode >= n_modes, a mode whose teams != 2 or whose team_size > 8
+ *                   (L <= 16: at most C(15, 7) = 6435 splits per lobby).  A 1v1 mode is accepted and changes nothing.
+ *                   Both feed orders.  For every lobby of a masked mode, with m_0 .. m_{L-1} its members in the order
+ *                   the tick (or mm_widen) forms them and c_i = c(rating(m_i)) the tick's key clamp to [rmin - 1,
+ *                   rmax + 1] (as in mm_match_quality): over the sets A of S members with m_0 in A, minimise
+ *                   |sum_A c - sum_rest c| (64-bit); ties go to the smallest M(A) = sum of 2^i over i in A, i > 0.  The
+ *                   lobby's members become A's members in their old relative order, then the others in theirs, so
+ *                   team 1 is still members [0, S) and team 2 [S, 2S) (the team-major contract of mm_lobby_hdr).
+ *                   Lobby membership, lobby order, headers and emit_seq do not change; with the option off every
+ *                   output is what it was.  Applies to every lobby a tick of any form emits (mm_tick, mm_tick_packed,
+ *                   async_results, mm_tick_device / mm_results_device, fused or split) and to every mm_widen lobby;
+ *                   the mask in force when the call runs decides.  mm_backfill (the caller owns the running lobby's
+ *                   teams) and mm_band_match are not balanced.  Not part of an image: mm_export / mm_import do not
+ *                   carry it.  mm_match_quality: after a balanced tick, imbalance (per lobby, max_imbalance,
+ *                   sum_imbalance, imbalance_hist) describes the teams emitted; spread and rating sums are unchanged.
+ *                   mm_locate: under its condition (neither the options nor the lobby budget change before the tick),
+ *                   member is the player's index in the balanced lobby.  Cost: after the tick, one warp per lobby of a
+ *                   masked mode (the L ids read and, unless the split is the identity, written back); in arrival order
+ *                   also one pass over the mode, rating and left bits of the pool the tick read.  The pass is part of
+ *                   the tick: its CUDA-event time is added to mm_tick_stats.device_us (the phase times leave it out),
+ *                   and mm_tick_device returns once it is done, so mm_results_device's members are final.  Device memory,
+ *                   allocated by the first balanced call and kept: 4 bytes per lobby the pool could hold, 4 bytes per
+ *                   player of capacity and, in arrival order, 4 bytes per chunk.
  *   "async_results" 1 = mm_tick does not wait for its device-to-host copies (see mm_results_wait); default 0   */
 int mm_set_option(mm_engine* e, const char* name, int64_t value);
 

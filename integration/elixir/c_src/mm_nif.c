@@ -566,6 +566,17 @@ static ERL_NIF_TERM nif_set_max_spread(ErlNifEnv* env, int argc, const ERL_NIF_T
   return rc ? err(env, rc) : atom(env, "ok");
 }
 
+/* set_team_balance(ref, mask): extension knob (balanced teams); bit m splits every lobby of mode m into the two teams
+ * with the least rating difference, 0 = off; a mask naming a mode that cannot be balanced returns the engine error */
+static ERL_NIF_TERM nif_set_team_balance(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifSInt64 mask = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_int64(env, argv[1], &mask))
+    return enif_make_badarg(env);
+  int rc = mm_set_option(r->e, "team_balance", (int64_t)mask);
+  return rc ? err(env, rc) : atom(env, "ok");
+}
+
 static ErlNifFunc funcs[] = {
   {"new", 1, nif_new, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"enqueue", 4, nif_enqueue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
@@ -592,6 +603,7 @@ static ErlNifFunc funcs[] = {
   {"locate", 3, nif_locate, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"seq_next", 1, nif_seq_next, 0},
   {"set_max_spread", 2, nif_set_max_spread, 0},
+  {"set_team_balance", 2, nif_set_team_balance, 0},
   {"set_lobby_budget", 3, nif_set_lobby_budget, 0},
   {"lobby_budget_report", 1, nif_lobby_budget_report, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"lobby_candidates", 1, nif_lobby_candidates, ERL_NIF_DIRTY_JOB_CPU_BOUND},

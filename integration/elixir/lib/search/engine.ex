@@ -159,4 +159,10 @@ defmodule Matchmaking.Search.Engine do
 
   @doc "Extension (not reference behaviour): maximum rating spread of a lobby for the following ticks; < 0 = off."
   def set_max_spread(_ref, _w), do: :erlang.nif_error(:nif_not_loaded)
+
+  @doc """
+  Extension (not reference behaviour): bit m of mask splits every lobby of mode m into the two teams with the least
+  rating difference (two-team modes of at most 8 players a team); 0 = off.  Team t is still members [t S, (t + 1) S).
+  """
+  def set_team_balance(_ref, _mask), do: :erlang.nif_error(:nif_not_loaded)
 end

@@ -22,6 +22,9 @@ defmodule Matchmaking.Search.Pool do
                      every player of the mode who has waited at least min_wait_ms anchors a lobby in a rating window of
                      w0 points either side, plus inc per whole step_ms past min_wait_ms, at most w_max (Engine.widen);
                      its lobbies are published like the tick's
+      balance_teams  option (extension, default nil = off): a list of mode names.  Every lobby of those modes, from the
+                     tick and from widen, is split into the two teams with the least rating difference
+                     (Engine.set_team_balance); the lobby's players are the same, only who plays with whom changes
       lobby_budget   option (extension, default nil = no limit): a zero-arity function -> %{mode name => lobbies}, asked
                      before every tick — the free game-server slots (game-lobby/worker.ex:118-141).  The tick emits at
                      most that many lobbies of the mode, shared over the rating groups in proportion to what each could
@@ -111,6 +114,10 @@ defmodule Matchmaking.Search.Pool do
   def init(opts) do
     capacity = Keyword.get(opts, :capacity, 16_000_000)
     {:ok, ref} = Engine.new(Engine.pack_config(capacity: capacity, active_capacity: 2 * capacity, dense_ids: true))
+    case Keyword.get(opts, :balance_teams) do
+      nil -> :ok
+      modes -> :ok = Engine.set_team_balance(ref, Enum.reduce(modes, 0, &Bitwise.bor(&2, Bitwise.bsl(1, Engine.mode_index(&1)))))
+    end
     # queued: handle -> {rating, mode, enq_ts, seq} at its enqueue, what requeue/1 hands back (kept until remove_user)
     st = %{ref: ref, staged: [], n_staged: 0, handle_of: %{}, players: %{}, free: [], next: 0, channel: nil,
            queued: %{}, moved_out: MapSet.new(),

@@ -498,6 +498,35 @@ __device__ __forceinline__ void ld_bins8(const uint16_t* p, uint32_t v[8]) {
   for (int j = 0; j < 8; ++j) v[j] = (w[j >> 1] >> (16 * (j & 1))) & 0xFFFFu;
 }
 
+// Arrival-order walk over the pool a tick read: every slot of the CTA's tile run [s0, s1), BLOCK at a time, with its
+// live rank rho among the live slots of its partition in storage order and whether the tick matched it (live, left bit
+// clear).  tile_off holds the live slots of the virtual tiles before each tile (k_img_tiles + k_scan_small).  Tiles
+// for which want(d) is false are skipped; f(d, slot, matched, rho) runs on every thread of every step (uniform).
+template <int BLOCK, class Want, class F>
+__device__ __forceinline__ void live_rank_walk(const Geo& geo, const PoolMeta& meta, const uint8_t* mode,
+                                               const uint32_t* left_bits, const uint32_t* tile_off, uint32_t s0,
+                                               uint32_t s1, uint32_t* s_warp, Want want, F f) {
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  for (uint32_t s = s0; s < s1; ++s) {
+    const TileDesc d = geo_tile(geo, meta, s);
+    if (!want(d)) continue;  // (uniform)
+    uint32_t rho0 = tile_off[s] - tile_off[geo.T0[d.seg]];  // live players of the partition before the tile
+    for (uint32_t o0 = 0; o0 < kTile; o0 += BLOCK) {  // (uniform)
+      if (o0 >= d.nvalid) break;
+      const uint32_t o = o0 + tid;
+      const size_t slot = (size_t)d.phys * kTile + o;
+      const bool live = o < d.nvalid && mode[slot] != MM_MODE_DEAD;
+      const uint32_t left = __ldcs(&left_bits[((size_t)s * kTile + o0 + warp * 32) >> 5]);
+      const uint32_t bal = __ballot_sync(0xFFFFFFFFu, live);
+      uint32_t total;
+      const uint32_t before = block_warp_offsets<BLOCK>(__popc(bal), total, s_warp);
+      const uint32_t rho = rho0 + before + __popc(bal & ((1u << lane) - 1u));
+      rho0 += total;
+      f(d, slot, live && !((left >> lane) & 1u), rho);
+    }
+  }
+}
+
 // Row prefixes of the histogram matrix: with few rows per partition (R rows over tens of partitions) every row sums
 // the rows before it on the fly; only when a partition spans many rows (one rating group over the whole pool) is the
 // column-scan phase (and its grid barrier) worth it.  Uniform: every CTA derives the same answer from the geometry.

@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "mm_backfill.cuh"
+#include "mm_balance.cuh"
 #include "mm_band.cuh"
 #include "mm_expire.cuh"
 #include "mm_image.cuh"
@@ -116,7 +117,7 @@ struct mm_engine {
   cudaStream_t d2h_stream = nullptr;   // async_results: a tick's host copies, overlapped with the next ingest
   bool async_results = false, results_pending = false;
   bool last_packed = false;  // the pending host copies read only d_hdr / d_members32
-  cudaEvent_t ev[5]{};  // tick start | after hist | after colscan | after place | after epilogue
+  cudaEvent_t ev[7]{};  // tick start | after hist | after colscan | after place | after epilogue | balance pass: start | end
   char last_err[512] = {0};
 
   // key domain
@@ -168,6 +169,8 @@ struct mm_engine {
   DevArray<uint32_t> d_outbase, d_binlim;
   DevArray<uint16_t> d_bin_key;
   int32_t max_spread = -1;  // < 0: policy S0 (reference behaviour); >= 0: policy S1 (extension)
+  uint32_t tb_mask = 0;     // team_balance: bit m = lobbies of mode m are split into balanced teams (extension)
+  uint32_t tb_last = 0;     // the mask the last tick's balance pass ran with (0: it did not run)
   DevArray<SegInfo> d_seg;
   DevArray<uint32_t> d_left_bits;  // one bit per virtual pool position: stays queued after the tick
   DevArray<uint64_t> d_members;
@@ -310,6 +313,14 @@ struct mm_engine {
     DevArray<mm_lobby_quality> lob;   // [max_lobbies]
     DevArray<mm_queue_quality> rec;   // [n_cut]
   } mq;
+
+  // team_balance (mm_balance.cuh): allocated by the first balanced tick or mm_widen and kept.  imb is read only by
+  // mm_match_quality and written only by a tick, so it describes the last tick's lobbies until the next one.
+  struct Balance {
+    DevArray<uint32_t> imb;   // [max_lobbies] the last tick's balanced imbalance per header position
+    DevArray<uint32_t> cval;  // [capacity + 64] c - key_lo per member slot (arrival-order ticks, mm_widen)
+    DevArray<uint32_t> w;     // arrival order: live slots per tile -> offsets [n_tiles] | per partition [n_segs] | total
+  } tb;
 };
 
 namespace {
@@ -953,6 +964,8 @@ int wait_results(mm_engine* e) {
   return MM_OK;
 }
 
+int balance_tick(mm_engine* e, mm_tick_stats* stats);  // (below)
+
 // mm_tick / mm_tick_packed: run the tick and copy lobbies + members (u64 ids or u32 handles) to host buffers
 int tick_to_host(mm_engine* e, mm_lobby_hdr* lobbies, uint32_t lobby_cap, uint64_t* member_ids, uint32_t* member_handles,
                  uint64_t member_cap, uint32_t* emit_seq, mm_tick_stats* stats) {
@@ -983,6 +996,7 @@ int tick_to_host(mm_engine* e, mm_lobby_hdr* lobbies, uint32_t lobby_cap, uint64
     if ((rc = tick_phase_b(e, emit_seq != nullptr))) return rc;
   }
   if ((rc = tick_commit(e, n, stats))) return rc;
+  if ((rc = balance_tick(e, stats))) return rc;
   const TickCtr& c = *e->h_ctr;
   if (member_handles && c.n_matched) {
     CK(e->d_members32.reserve((size_t)e->capacity + 64));
@@ -1027,6 +1041,55 @@ int staged_err(mm_engine* e) {
 }
 uint32_t tile_ctas(const mm_engine* e, uint32_t n) {
   return std::max<uint32_t>(1, std::min<uint32_t>(tile_count(e, n), 8u * (uint32_t)e->n_sms));
+}
+
+// team_balance: the balance pass over the results of the tick that has just committed (d_outbase and pool[cur ^ 1]
+// still describe it).  Records the mask it ran with for mm_match_quality.  It returns with the engine stream idle, as
+// the tick itself does: mm_results_device and the async_results copy stream read the members on streams of their own.
+// Its CUDA-event time is added to the tick's device_us.
+int balance_tick(mm_engine* e, mm_tick_stats* stats) {
+  e->tb_last = 0;
+  const uint32_t n_lob = e->last.n_lobbies;
+  if (!e->tb_mask || !n_lob) return MM_OK;
+  auto& s = e->tb;
+  CK(s.imb.reserve(e->max_lobbies));
+  TbArgs t{};
+  t.hdr = e->d_hdr; t.n_lob = n_lob; t.members = e->d_members; t.mask = e->tb_mask; t.mode_tsize = e->d_mode_tsize;
+  t.outbase = e->d_outbase; t.bin_key = e->d_bin_key; t.K = e->K; t.imb = s.imb;
+  const uint32_t grid = grid256(e, (uint64_t)n_lob * 32, 8);
+  CK(cudaEventRecord(e->ev[5], e->stream));
+  if (e->cfg.order_mode == MM_ORDER_ARRIVAL) {
+    const Pool& p = e->pool[e->cur ^ 1];  // the pool the tick read
+    const size_t n_tiles = (size_t)e->n_chunks + e->n_segs;
+    CK(s.cval.reserve((size_t)e->capacity + 64));
+    CK(s.w.reserve(n_tiles + e->n_segs + 1));
+    CK(cudaMemsetAsync(s.w + n_tiles, 0, ((size_t)e->n_segs + 1) * 4, e->stream));
+    // live slots per virtual tile -> the live slots before each tile (mm_export's count and scan)
+    ImgExportArgs x{};
+    x.pool = p.v; x.meta = p.m; x.n_segs = e->n_segs; x.tile_cnt = s.w; x.part_cnt = s.w + n_tiles;
+    const uint32_t ctas = tile_ctas(e, e->match_n);
+    k_img_tiles<kImgBlock, false><<<ctas, kImgBlock, 0, e->stream>>>(x);
+    k_scan_small<<<1, 1024, 0, e->stream>>>(tile_count(e, e->match_n), s.w, s.w + n_tiles + e->n_segs);
+    TbArrivalArgs a{};
+    a.pool = p.v; a.meta = p.m; a.left_bits = e->d_left_bits; a.tile_off = s.w;
+    a.n_segs = e->n_segs; a.n_groups = e->cfg.n_groups; a.mask = e->tb_mask; a.key_lo = e->key_lo; a.KR = e->KR;
+    a.part_cut = e->d_part_cut; a.mode_tsize = e->d_mode_tsize; a.seg_bin_lo = e->d_seg_bin_lo;
+    a.outbase = e->d_outbase; a.cval = s.cval;
+    k_tb_arrival<kMqBlock><<<ctas, kMqBlock, 0, e->stream>>>(a);
+    t.cval = s.cval;
+    k_tb_lobby<true><<<grid, 256, 0, e->stream>>>(t);
+  } else {
+    k_tb_lobby<false><<<grid, 256, 0, e->stream>>>(t);
+  }
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e->ev[6], e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, e->ev[5], e->ev[6]));
+  e->last.device_us += ms * 1000.f;
+  if (stats) stats->device_us = e->last.device_us;
+  e->tb_last = e->tb_mask;
+  return MM_OK;
 }
 
 // active-set entries erased by mm_remove, mm_expire or an export release: a hashed set keeps a tombstone for each
@@ -2304,6 +2367,15 @@ int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* 
   const uint32_t np = h[kBfPieces];
   k_bf_out<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, a.mbase,
                                                                                b.staging, b.members);
+  if (e->tb_mask) {  // team_balance: each member's c from its piece's bin, then the tick's balance kernel
+    CK(e->tb.cval.reserve((size_t)e->capacity + 64));
+    k_tb_pieces<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, a.mbase, e->d_bin_key,
+                                                                                  e->tb.cval);
+    TbArgs t{};
+    t.hdr = s.hdr; t.n_lob = nl; t.members = b.members; t.mask = e->tb_mask; t.mode_tsize = e->d_mode_tsize;
+    t.cval = e->tb.cval;
+    k_tb_lobby<true><<<grid256(e, (uint64_t)nl * 32, 8), 256, 0, e->stream>>>(t);
+  }
   CK(cudaGetLastError());
   CK(cudaEventRecord(e->ev[4], e->stream));
   CK(cudaMemcpyAsync(lobbies, s.hdr, (size_t)nl * sizeof(mm_lobby_hdr), cudaMemcpyDeviceToHost, e->stream));
@@ -2339,6 +2411,8 @@ int locate(mm_engine* e, uint64_t now, uint32_t n, const uint64_t* id, mm_player
   a.n_slots = (uint32_t)pool_slots(e); a.gen = e->gen; a.n_groups = e->cfg.n_groups; a.now = (uint32_t)now;
   a.bin_seg = e->d_bin_seg; a.seg_bin_lo = e->d_seg_bin_lo; a.seg_L = e->d_seg_L; a.part_cut = e->d_part_cut;
   a.cut_lp_lo = e->d_cut_lp_lo; a.rmap = rmap; a.pos = pos; a.outbase = ob; a.binlim = bl; a.out = s.out;
+  a.tb_mask = e->tb_mask; a.arrival = e->cfg.order_mode == MM_ORDER_ARRIVAL; a.mode_tsize = e->d_mode_tsize;
+  a.bin_key = e->d_bin_key; a.key_lo = e->key_lo; a.KR = e->KR;
   k_locate<<<(uint32_t)(((size_t)n * 32 + 255) / 256), 256, 0, e->stream>>>(a);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, s.out, (size_t)n * sizeof(mm_player_status), cudaMemcpyDeviceToHost, e->stream));
@@ -2372,6 +2446,7 @@ int match_quality(mm_engine* e, mm_queue_quality* per_queue, mm_lobby_quality* p
     a.cut_lp_lo = e->d_cut_lp_lo; a.mode_tsize = e->d_mode_tsize;
     a.cnt = s.w; a.csum = arrival ? nullptr : s.csum.p; a.qlob = s.w + o_qlob; a.qteam = s.w + o_qteam;
     a.lob = s.lob; a.n_lob = n_lob; a.qrec = s.rec;
+    a.tb_mask = e->tb_last; a.tb_imb = e->tb.imb;
     CK(cudaMemsetAsync(a.cnt, 0, (size_t)e->Kp * 4, e->stream));
     const uint32_t ctas = tile_ctas(e, e->match_n);
     k_mq_count<kMqBlock><<<ctas, kMqBlock, 0, e->stream>>>(a);
@@ -2589,6 +2664,19 @@ int mm_set_option(mm_engine* e, const char* name, int64_t value) {
     if (value >= 0 && e->cfg.order_mode != MM_ORDER_RATING) return MM_E_ARG;
     if (value > 0x7FFFFFFF) return MM_E_ARG;
     e->max_spread = value < 0 ? -1 : (int32_t)value;
+    return MM_OK;
+  }
+  if (!std::strcmp(name, "team_balance")) {
+    // EXTENSION (balanced teams, mm_balance.cuh): bit m splits every lobby of mode m into the two teams with the least
+    // rating difference.  Exact two-way partitioning only: two teams of at most kTbMaxS players.
+    if (value < 0 || value >= (int64_t)1 << e->cfg.n_modes)
+      return set_err(e, MM_E_ARG, "team_balance 0x%llx names a mode >= n_modes = %u", (unsigned long long)value,
+                     e->cfg.n_modes);
+    for (uint32_t m = 0; m < e->cfg.n_modes; ++m)
+      if (((value >> m) & 1) && (e->cfg.modes[m].teams != 2 || e->cfg.modes[m].team_size > kTbMaxS))
+        return set_err(e, MM_E_ARG, "team_balance: mode %u has %u teams of %u (two teams of at most %u only)", m,
+                       e->cfg.modes[m].teams, e->cfg.modes[m].team_size, kTbMaxS);
+    e->tb_mask = (uint32_t)value;
     return MM_OK;
   }
   if (!std::strcmp(name, "tick_impl")) { e->tick_impl = value != 0; return MM_OK; }
@@ -2859,7 +2947,8 @@ int mm_tick_device(mm_engine* e, uint64_t now, mm_tick_stats* stats) {
     if ((rc = tick_phase_a(e))) return rc;
     if ((rc = tick_phase_b(e, false))) return rc;
   }
-  return tick_commit(e, n, stats);
+  if ((rc = tick_commit(e, n, stats))) return rc;
+  return balance_tick(e, stats);
 }
 
 int mm_results_device(mm_engine* e, const mm_lobby_hdr** d_lobbies, const uint64_t** d_member_ids) {

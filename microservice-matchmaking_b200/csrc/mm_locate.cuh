@@ -11,7 +11,11 @@
 // in the partition's earlier chunks plus those before it in its own chunk.  With resident chunk histograms the earlier
 // chunks cost one 4-byte read each; without them (MM_F_WIDE_PARTITIONS, or more than kMaxSegs partitions) the warp
 // counts the bin column of the earlier chunks.  The own chunk is counted from the bin column (at most 4 KB).
+// With team_balance set for the player's mode, the predicted lobby is split as the tick's balance pass will split it
+// (tb_split): its members' c from the preview's per-bin member ranges (rating order), or from the L consecutive live
+// players of the partition around the player (arrival order), found by walking the mode and rating columns.
 #pragma once
+#include "mm_balance.cuh"
 #include "mm_kernels.cuh"
 
 namespace mm {
@@ -70,9 +74,44 @@ struct LocateArgs {
   const uint32_t* outbase;   // [Kp] k_locate_preview: member slot of the bin's first player
   const uint32_t* binlim;    // [Kp] k_locate_preview: end of the bin's matched member slots
   mm_player_status* out;     // [n]
+  uint32_t tb_mask;          // team_balance: modes whose lobbies the next tick balances
+  bool arrival;              // MM_ORDER_ARRIVAL
+  const uint8_t* mode_tsize; // [MM_MAX_MODES]
+  const uint16_t* bin_key;   // [Kp] c - key_lo of the bin
+  int32_t key_lo;
+  uint32_t KR;
 };
 
+// Arrival order, one warp: the lobby of the player at `slot` (partition sg) is L consecutive live players of the
+// partition in storage order, the player being member j.  c - key_lo of member i goes to cw[i].
+__device__ __forceinline__ void loc_arrival_lobby(const LocateArgs& a, uint32_t slot, uint32_t sg, uint32_t j,
+                                                  uint32_t L, uint32_t* cw) {
+  const uint32_t lane = threadIdx.x & 31, fill = a.meta.fill[sg];
+  const uint32_t* tab = a.meta.chunk_tab + (size_t)sg * a.meta.max_ch;
+  auto at = [&](uint32_t p) { return (size_t)tab[p / kTile] * kTile + p % kTile; };
+  auto c_of = [&](size_t s) { return clamp_key(a.key_lo, a.KR, a.pool.rating[s]); };
+  const uint32_t p0 = a.rmap[slot / kTile] * kTile + slot % kTile;  // the player's index in its partition
+  if (lane == 0) cw[j] = c_of(slot);
+  // members j - 1 .. 0: the nearest live players before it (lane l looks at index p - 1 - l)
+  for (uint32_t need = j, p = p0; need && p;) {  // (uniform)
+    const bool live = p > lane && a.pool.mode[at(p - 1 - lane)] != MM_MODE_DEAD;
+    const uint32_t bal = __ballot_sync(0xFFFFFFFFu, live), k = __popc(bal & ((1u << lane) - 1u));
+    if (live && k < need) cw[need - 1 - k] = c_of(at(p - 1 - lane));
+    need -= __popc(bal) < need ? __popc(bal) : need;
+    p = p > 32 ? p - 32 : 0;
+  }
+  // members j + 1 .. L - 1: the nearest live players after it
+  for (uint32_t need = L - 1 - j, p = p0 + 1; need && p < fill;) {  // (uniform)
+    const bool live = p + lane < fill && a.pool.mode[at(p + lane)] != MM_MODE_DEAD;
+    const uint32_t bal = __ballot_sync(0xFFFFFFFFu, live), k = __popc(bal & ((1u << lane) - 1u));
+    if (live && k < need) cw[L - need + k] = c_of(at(p + lane));
+    need -= __popc(bal) < need ? __popc(bal) : need;
+    p += 32;
+  }
+}
+
 __global__ void __launch_bounds__(256) k_locate(const LocateArgs a) {
+  __shared__ uint32_t s_c[8][16];  // team_balance: c - key_lo of the predicted lobby's members, per warp
   const uint32_t lane = threadIdx.x & 31, q = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (q >= a.n) return;  // (uniform over the warp)
   const uint64_t pid = a.id[q];
@@ -100,7 +139,6 @@ __global__ void __launch_bounds__(256) k_locate(const LocateArgs a) {
   }
   const uint32_t v = a.pool.bin[slot], sg = a.bin_seg[v];
   const uint32_t rank = bin_rank(a.pool, a.meta, a.seg_bin_lo, a.rmap, slot, v, sg);
-  if (lane != 0) return;
   const uint32_t c = a.part_cut[sg], b0 = a.seg_bin_lo[a.cut_lp_lo[c]], b1 = a.seg_bin_lo[a.cut_lp_lo[c + 1]];
   r.state = 1;
   r.mode = a.pool.mode[slot];
@@ -117,8 +155,22 @@ __global__ void __launch_bounds__(256) k_locate(const LocateArgs a) {
     const uint32_t rel = m - a.outbase[b0], L = a.seg_L[sg];  // the queue's lobby k = its member slots [k L, k L + L)
     r.lobby = rel / L;
     r.member = (uint16_t)(rel % L);
+    const uint32_t S = a.mode_tsize[r.mode];
+    if (((a.tb_mask >> r.mode) & 1u) && S > 1) {  // (uniform) the balance pass reorders the lobby
+      uint32_t* cw = s_c[(threadIdx.x >> 5) & 7];
+      if (a.arrival) {
+        loc_arrival_lobby(a, slot, sg, r.member, L, cw);
+      } else if (lane < L) {
+        const uint32_t x = a.outbase[b0] + r.lobby * L + lane;  // member slot of the lobby's member `lane`
+        cw[lane] = a.bin_key[last_le(a.outbase, b0, b1, x)];
+      }
+      __syncwarp();
+      unsigned long long imb;
+      const uint32_t mf = tb_split(lane < L ? cw[lane] : 0u, L, S, &imb);
+      r.member = (uint16_t)tb_new_index(mf, r.member, S);
+    }
   }
-  a.out[q] = r;
+  if (lane == 0) a.out[q] = r;
 }
 
 }  // namespace mm

@@ -21,6 +21,8 @@
 //                      c - key_lo (never negative) and exact integer atomics into per-lobby scratch
 //   k_mq_lobby<true>   one thread per lobby: the record from its scratch
 // Both: k_mq_queue     the per-queue records: shared-memory histograms, flushed with atomics per queue run
+// A lobby of a mode the last tick balanced (team_balance, mm_balance.cuh) has other teams than the pool's order gives:
+// its imbalance is the one k_tb_lobby stored for its header position, and every other value is order-free.
 #pragma once
 #include <cstddef>
 
@@ -67,6 +69,8 @@ struct MqArgs {
   mm_lobby_quality* lob;        // [lobbies]
   uint32_t n_lob;               // the tick's lobbies
   mm_queue_quality* qrec;       // [n_cut], zeroed before k_mq_queue
+  uint32_t tb_mask;             // the modes the last tick balanced (mm_balance.cuh): their S > 1 lobbies' imbalance
+  const uint32_t* tb_imb;       // [lobbies] ... is the balanced one, per header position
 };
 
 // lobby size L and team size S of queue q
@@ -163,28 +167,16 @@ __global__ void __launch_bounds__(BLOCK) k_mq_arrival(const MqArgs a) {
   __shared__ Geo geo;
   __shared__ uint32_t s_gtmp[33];
   __shared__ uint32_t s_warp[BLOCK / 32];
-  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t lane = threadIdx.x & 31;
   uint32_t s0, s1;
   if (!geo_cta_run<BLOCK>(geo, a.meta.fill, a.n_segs, s_gtmp, s0, s1)) return;  // (uniform)
-  for (uint32_t s = s0; s < s1; ++s) {
-    const TileDesc d = geo_tile(geo, a.meta, s);
-    const uint32_t q = a.part_cut[d.seg];
-    uint32_t L, S;
-    mq_shape(a, q, L, S);
-    const uint32_t n_q = a.qlob[q + 1] - a.qlob[q], T = L / S;
-    uint32_t rho0 = a.tile_off[s] - a.tile_off[geo.T0[d.seg]];  // live players of the partition before the tile
-    for (uint32_t o0 = 0; o0 < kTile; o0 += BLOCK) {  // (uniform)
-      if (o0 >= d.nvalid) break;
-      const uint32_t o = o0 + tid;
-      const size_t slot = (size_t)d.phys * kTile + o;
-      const bool live = o < d.nvalid && a.pool.mode[slot] != MM_MODE_DEAD;
-      const uint32_t left = __ldcs(&a.left_bits[((size_t)s * kTile + o0 + warp * 32) >> 5]);
-      const bool matched = live && !((left >> lane) & 1u);
-      const uint32_t bal = __ballot_sync(0xFFFFFFFFu, live);
-      uint32_t total;
-      const uint32_t before = block_warp_offsets<BLOCK>(__popc(bal), total, s_warp);
-      const uint32_t rho = rho0 + before + __popc(bal & ((1u << lane) - 1u));
-      rho0 += total;
+  auto all = [](const TileDesc&) { return true; };
+  live_rank_walk<BLOCK>(geo, a.meta, a.pool.mode, a.left_bits, a.tile_off, s0, s1, s_warp, all,
+                        [&](const TileDesc& d, size_t slot, bool matched, uint32_t rho) {
+      const uint32_t q = a.part_cut[d.seg];
+      uint32_t L, S;
+      mq_shape(a, q, L, S);
+      const uint32_t n_q = a.qlob[q + 1] - a.qlob[q], T = L / S;
       const uint32_t v = matched ? clamp_key(a.key_lo, a.KR, a.pool.rating[slot]) : 0u;
       const uint32_t lk = rho / L, tk = rho / S;
       uint32_t mn = matched ? v : 0xFFFFFFFFu, mx = v, sm = v;
@@ -203,8 +195,7 @@ __global__ void __launch_bounds__(BLOCK) k_mq_arrival(const MqArgs a) {
         atomicMax(&a.lmax[h], mx);
       }
       if (tk < n_q * T && sm && (lane == 0 || p_tk != tk)) atomicAdd(&a.tsum[a.qteam[q] + tk], sm);
-    }
-  }
+    });
 }
 
 // One thread per lobby: its record.  Rating order: from the per-bin prefixes; arrival order: from k_mq_arrival.
@@ -259,6 +250,7 @@ __global__ void __launch_bounds__(256) k_mq_lobby(const MqArgs a) {
   }
   const unsigned long long imb = (unsigned long long)(smax - smin);
   r.imbalance = imb > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)imb;
+  if (((a.tb_mask >> (q / a.n_groups)) & 1u) && S > 1) r.imbalance = a.tb_imb[h];  // the teams actually emitted
   a.lob[h] = r;
 }
 

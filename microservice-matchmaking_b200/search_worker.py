@@ -169,6 +169,10 @@ class SearchPool:
     of the mode who has waited at least min_wait_ms anchors a lobby in a rating window of w0 points either side, plus
     inc per whole step_ms waited past min_wait_ms, at most w_max (Engine.widen, every rating group of the mode).  Its
     lobbies are published like the tick's; stats["widened"] counts them.
+    balance_teams: optional list of mode names (extension; two-team modes of at most 8 players a team): every lobby of
+    those modes, from the tick and from widen, is split into the two teams with the least rating difference
+    (mm_set_option("team_balance")).  Membership and lobby order are unchanged; team t is still members
+    [t * team_size, (t + 1) * team_size).  resume() sets it again on the new engine.
 
     Every ingest batch is stamped with now_ms(), the clock in milliseconds since the pool was created (u32, wraps
     after 49 days), and every tick passes the same clock as its `now`: the engine's per-queue waits
@@ -176,7 +180,8 @@ class SearchPool:
     """
 
     def __init__(self, engine, mode_names, group_names, max_batch=65536, window=None, clock=None, flush_every_s=0.005,
-                 handle_capacity=None, timeout_ms=None, wall_clock=None, lobby_budget=None, widen=None):
+                 handle_capacity=None, timeout_ms=None, wall_clock=None, lobby_budget=None, widen=None,
+                 balance_teams=None):
         import time
         if widen and engine.cfg.order_mode != abi.MM_ORDER_RATING:
             raise ValueError("widen needs an MM_ORDER_RATING engine: windows are rating distances")
@@ -196,6 +201,11 @@ class SearchPool:
         self.mode_names = list(mode_names)
         self.mode_index = {m: i for i, m in enumerate(self.mode_names)}
         self.group_names = list(group_names)
+        if balance_teams:
+            unknown = [m for m in balance_teams if m not in self.mode_index]
+            if unknown:
+                raise ValueError(f"balance_teams names unknown modes {unknown}")
+            engine.set_option("team_balance", sum(1 << self.mode_index[m] for m in set(balance_teams)))
         self.max_batch = max_batch
         self.flush_every_s = flush_every_s
         self.handles = HandleTable(handle_capacity)
