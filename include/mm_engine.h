@@ -376,6 +376,77 @@ typedef struct mm_widen_stats {
 int mm_widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
              uint64_t* member_ids, uint64_t member_cap, mm_widen_stats* stats);
 
+/* EXTENSION (parties, DESIGN.md §4): players who queue together are matched into one lobby and one team.  Parties live
+ * in a table beside the pool that the tick never reads; mm_party_match, called before the tick, forms their lobbies, so
+ * parties get the first pick of the solos.  mm_set_option("party_capacity", P) sets how many party members the table
+ * holds (default 0: every party call is refused with MM_E_STATE; MM_E_ARG below the members queued now).
+ *
+ * mm_enqueue_party: party j's members are the next size[j] entries of ids / rating (handles on MM_F_DENSE_IDS
+ * engines).  Its rating R = floor(sum(rating) / size) (64-bit sum, floor toward minus infinity), its group
+ * mm_group_of(R) (with the default-group fallback).  Every offered party of an accepted batch consumes one enqueue
+ * sequence number (the numbering of emit_seq: parties and solos share age order).  accepted[j] (may be null):
+ *   2  invalid: mode >= n_modes, size < 2 or > the mode's team_size, an invalid id, an id twice in the party, R
+ *      without a group;
+ *   0  otherwise, if a member was in the active set before the call or is a member of an earlier party of the batch
+ *      (accepted or not);
+ *   3  otherwise, if the party does not fit the table: the last parties that do not fit;
+ *   1  queued.
+ * A queued member is in the active set (mm_in_queue 1, mm_active_size counts it) but not in the pool (mm_pool_size,
+ * mm_queue_stats, the tick, mm_take, mm_widen, mm_backfill and the boundary pass do not see it).  mm_remove of any
+ * member dissolves the whole party (every member leaves the active set and counts in n_removed); mm_expire expires
+ * whole parties whose WAIT >= max_wait, listing every member with the party's seq (cap and the dry run count members;
+ * the party members follow the solos); mm_locate reports state 3; mm_requeue gives a queued member code 0.
+ * mm_export, mm_export_queues, mm_merge and mm_snapshot are refused with MM_E_STATE while a party is queued (images
+ * do not carry parties); mm_restore empties the table.
+ * Refusals, decided before anything changes: MM_E_ARG null pointers with n > 0, an MM_ORDER_ARRIVAL engine;
+ * MM_E_STATE no party capacity, an MM_F_NO_DEDUPE engine, a staged packed batch; MM_E_CAP a batch the active set
+ * cannot hold at all.                                                                                                */
+int mm_enqueue_party(mm_engine* e, uint32_t n_parties, const uint8_t* size, const uint64_t* ids, const int32_t* rating,
+                     const uint8_t* mode, const uint32_t* enq_ts, uint8_t* accepted);
+
+typedef struct mm_party_stats {
+  uint32_t n_anchors;   /* anchors considered                                  */
+  uint32_t n_lobbies, n_matched;
+  uint32_t n_parties;   /* parties placed into lobbies                         */
+  uint32_t n_absorbed;  /* anchors an earlier lobby of the call had placed     */
+  float device_us;      /* CUDA-event time of the call's device work           */
+  uint32_t reserved[2];
+} mm_party_stats;       /* 32 bytes */
+
+/* mm_party_match: one mm_widen_rule per (mode, group) queue in mm_queue_stats order (MM_WIDEN_OFF: the queue is not
+ * served); WAIT, c() and age order as in mm_widen; L = T x S of the queue's mode.  Every served queue q on its own:
+ *   U = the live queued solos of q;  P = the queued parties of q
+ *   A = the parties of P with WAIT >= min_wait, in age order
+ *   for a in A:
+ *     if an earlier lobby of the call placed a: a is ABSORBED; next
+ *     w = min(w_max, w0 + floor((WAIT(a) - min_wait) / step) * inc)                                   (64-bit)
+ *     room[t] = S for every team; a goes to team 0
+ *     Q = the unplaced parties b != a of P with |c(R_b) - c(R_a)| <= w, by (|c(R_b) - c(R_a)|, c(R_b), age)
+ *     for b in Q: b goes to the lowest team t with room[t] >= size(b); if there is none, b is skipped
+ *     open = sum(room)
+ *     C = the players x of U with |c(r_x) - c(R_a)| <= w, by (|c(r_x) - c(R_a)|, c(r_x), age)
+ *     if |C| < open: a stays queued and nothing is placed; next                                  (all or nothing)
+ *     a lobby is formed: its parties leave P, the first `open` of C leave U
+ * Members are team-major (team t = members [tS, (t+1)S)): a team's parties in placement order, each with its members
+ * in enqueue order, then the solos, which fill the open slots of team 0, then team 1, ... in C's order.  Lobbies are
+ * ordered by (mode, group, emission within the queue), group = the queue's group.  Solos taken leave the pool exactly
+ * as mm_take takes them; matched party members stay in the active set as matched players (mm_locate state 2,
+ * mm_requeue code 1: back as a solo).  team_balance does not split party lobbies; the last tick's results,
+ * mm_match_quality, the lobby budget and pending async_results copies are left alone.
+ * Refusals, all decided before anything changes (mm_last_error names the cause): MM_E_ARG the rule checks of mm_widen,
+ * a served mode of more than 256 teams, an MM_ORDER_ARRIVAL engine; MM_E_STATE no party capacity, an MM_F_NO_DEDUPE
+ * engine, a staged packed batch; MM_E_CAP lobby_cap or member_cap too small (stats holds the counts and nothing is
+ * taken: zero capacities make a dry run).                                                                          */
+int mm_party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
+                   uint64_t* member_ids, uint64_t member_cap, mm_party_stats* stats);
+
+/* mm_party_read: the queued parties in age order (a test and diagnostic aid, like mm_pool_read): size, seq, enq_ts,
+ * mode, group and R per party, member ids and ratings in party order.  MM_E_CAP (with the counts) if party_cap or
+ * member_cap is too small.                                                                                          */
+int mm_party_read(mm_engine* e, uint32_t party_cap, uint32_t member_cap, uint8_t* size, uint32_t* seq, uint32_t* enq_ts,
+                  uint8_t* mode, uint8_t* group, int32_t* rating, uint64_t* member_ids, int32_t* member_rating,
+                  uint32_t* n_parties, uint32_t* n_members);
+
 /* Replaces ActiveUser.in_queue?/1 (models/active_user.ex:33-44), batched.          */
 int mm_in_queue(mm_engine* e, uint32_t n, const uint64_t* id, uint8_t* out);
 
@@ -384,7 +455,9 @@ int mm_in_queue(mm_engine* e, uint32_t n, const uint64_t* id, uint8_t* out);
  * ActiveUser.in_queue?/1 (models/active_user.ex:33-44), which mm_in_queue covers.                                 */
 #define MM_LOCATE_STAYS 0xFFFFFFFFu
 typedef struct mm_player_status {
-  uint8_t state;        /* 0 not in the active set, 1 queued (live), 2 in the active set but not queued               */
+  uint8_t state;        /* 0 not in the active set, 1 queued (live), 2 in the active set but not queued, 3 queued in a
+                           party (its own rating; the party's mode, group, enq_ts, seq and wait; ahead = depth = 0,
+                           lobby = MM_LOCATE_STAYS)                                                                   */
   uint8_t mode, group;  /* its (mode, group) queue; a default-group fallback reports the default group                */
   uint8_t reserved;     /* 0                                                                                          */
   int32_t rating;       /* as enqueued                                                                                */

@@ -489,6 +489,65 @@ static ERL_NIF_TERM nif_widen(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[
   return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &lb), enif_make_binary(env, &hs));
 }
 
+/* enqueue_party(ref, sizes :: binary(u8[]), handles :: binary(u32[]), ratings :: binary(i32[]), modes :: binary(u8[]),
+ * enq_ts :: binary(u32[])) -> {:ok, codes :: binary(u8[])}: party j's members are the next sizes[j] handles and ratings
+ * (mm_enqueue_party); codes 1 queued, 0 a member already queued, 2 invalid, 3 the party table is full.  badarg unless
+ * the sizes add up to the handles and ratings and every per-party binary has one entry per party. */
+static ERL_NIF_TERM nif_enqueue_party(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary sb, hb, rtb, mb, tb, out;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &sb) ||
+      !enif_inspect_binary(env, argv[2], &hb) || !enif_inspect_binary(env, argv[3], &rtb) ||
+      !enif_inspect_binary(env, argv[4], &mb) || !enif_inspect_binary(env, argv[5], &tb))
+    return enif_make_badarg(env);
+  const uint32_t n = (uint32_t)sb.size;
+  size_t m = 0;
+  for (uint32_t j = 0; j < n; ++j) m += sb.data[j];
+  if (hb.size != 4 * m || rtb.size != 4 * m || mb.size != n || tb.size != 4 * (size_t)n) return enif_make_badarg(env);
+  uint64_t* id = enif_alloc(8 * m + 8);
+  if (!id || !enif_alloc_binary(n, &out)) { enif_free(id); return err(env, MM_E_CAP); }
+  for (size_t k = 0; k < m; ++k) { uint32_t h; memcpy(&h, hb.data + 4 * k, 4); id[k] = h; }
+  const int rc = mm_enqueue_party(r->e, n, sb.data, id, (const int32_t*)rtb.data, mb.data, (const uint32_t*)tb.data,
+                                  out.data);
+  enif_free(id);
+  if (rc) { enif_release_binary(&out); return err(env, rc); }
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &out));
+}
+
+/* party_match(ref, now :: u64, rules :: binary(mm_widen_rule[n_modes * n_groups]))
+ *   -> {:ok, lobbies :: binary(mm_lobby_hdr[]), handles :: binary(u32[])}: lobbies around the parties that waited
+ * longest, each party whole on one team (mm_party_match).  badarg unless the binary holds exactly one rule per (mode,
+ * group) queue.  The buffers are sized from the dry run's counts (zero capacities). */
+static ERL_NIF_TERM nif_party_match(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifUInt64 now; ErlNifBinary rb, lb, hs; mm_party_stats st; uint32_t nq = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_uint64(env, argv[1], &now) ||
+      !enif_inspect_binary(env, argv[2], &rb))
+    return enif_make_badarg(env);
+  mm_lobby_candidates(r->e, NULL, 0, &nq);
+  if (rb.size != (size_t)nq * sizeof(mm_widen_rule)) return enif_make_badarg(env);
+  mm_widen_rule* rules = enif_alloc(rb.size + 1);
+  if (!rules) return err(env, MM_E_CAP);
+  memcpy(rules, rb.data, rb.size);
+  int rc = mm_party_match(r->e, now, rules, NULL, 0, NULL, 0, &st);  /* the dry run: counts only */
+  if (rc == MM_E_CAP || rc == MM_OK) {
+    const uint32_t nl = st.n_lobbies, nm = st.n_matched;
+    uint64_t* id = enif_alloc(8 * (size_t)nm + 8);
+    if (!id || !enif_alloc_binary(sizeof(mm_lobby_hdr) * (size_t)nl, &lb)) rc = MM_E_CAP;
+    else if (!enif_alloc_binary(4 * (size_t)nm, &hs)) { enif_release_binary(&lb); rc = MM_E_CAP; }
+    else {
+      rc = mm_party_match(r->e, now, rules, (mm_lobby_hdr*)lb.data, nl, id, nm, &st);
+      if (rc) { enif_release_binary(&lb); enif_release_binary(&hs); }
+      else
+        for (uint32_t k = 0; k < nm; ++k) { const uint32_t h = (uint32_t)id[k]; memcpy(hs.data + 4 * (size_t)k, &h, 4); }
+    }
+    enif_free(id);
+  }
+  enif_free(rules);
+  if (rc) return err(env, rc);
+  return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &lb), enif_make_binary(env, &hs));
+}
+
 /* locate(ref, now :: u64, handles :: binary(u32[])) -> {:ok, records :: binary(mm_player_status[])}: where each
  * player's search stands (mm_locate): state, queue, wait at `now`, players ahead and queue depth, and the lobby ordinal
  * / member index the next tick gives it (0xFFFFFFFF: it stays queued). */
@@ -577,6 +636,16 @@ static ERL_NIF_TERM nif_set_team_balance(ErlNifEnv* env, int argc, const ERL_NIF
   return rc ? err(env, rc) : atom(env, "ok");
 }
 
+/* set_party_capacity(ref, members): extension knob (parties); how many party members the engine holds */
+static ERL_NIF_TERM nif_set_party_capacity(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifSInt64 cap = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_int64(env, argv[1], &cap))
+    return enif_make_badarg(env);
+  int rc = mm_set_option(r->e, "party_capacity", (int64_t)cap);
+  return rc ? err(env, rc) : atom(env, "ok");
+}
+
 static ErlNifFunc funcs[] = {
   {"new", 1, nif_new, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"enqueue", 4, nif_enqueue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
@@ -600,6 +669,9 @@ static ErlNifFunc funcs[] = {
   {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"backfill", 2, nif_backfill, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"widen", 3, nif_widen, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"enqueue_party", 6, nif_enqueue_party, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"party_match", 3, nif_party_match, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"set_party_capacity", 2, nif_set_party_capacity, 0},
   {"locate", 3, nif_locate, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"seq_next", 1, nif_seq_next, 0},
   {"set_max_spread", 2, nif_set_max_spread, 0},

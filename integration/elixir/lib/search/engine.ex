@@ -134,6 +134,21 @@ defmodule Matchmaking.Search.Engine do
   """
   def widen(_ref, _now, _rules), do: :erlang.nif_error(:nif_not_loaded)
   @doc """
+  Parties (extension): queue players together (mm_enqueue_party).  sizes: binary(u8[]) per party; handles
+  binary(u32[]) and ratings binary(little-signed-32[]) of the members, party after party; modes binary(u8[]) and enq_ts
+  binary(little-32[]) per party -> {:ok, codes :: binary(u8[])}: 1 queued, 0 a member already queued, 2 invalid, 3 the
+  party table is full.
+  """
+  def enqueue_party(_ref, _sizes, _handles, _ratings, _modes, _enq_ts), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Parties (extension): lobbies around the parties that waited longest, each party whole on one team (mm_party_match);
+  rules as widen/3 takes them -> {:ok, lobbies, handles}.  Run it before the tick: parties get the first pick of the
+  solos.  The solos leave the pool and every member stays in the active set until remove_user.
+  """
+  def party_match(_ref, _now, _rules), do: :erlang.nif_error(:nif_not_loaded)
+  @doc "Parties (extension): how many party members the engine holds (mm_set_option(\"party_capacity\"))."
+  def set_party_capacity(_ref, _members), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
   Search status (extension): where each player's search stands (mm_locate).  handles: binary(u32[]) -> {:ok, records}:
   36-byte records <<state, mode, group, 0, rating::little-signed-32, enq_ts::little-32, seq::little-32,
   wait::little-32, ahead::little-32, depth::little-32, lobby::little-32, member::little-16, 0::16>>; state 0 gone,

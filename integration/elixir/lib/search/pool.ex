@@ -22,6 +22,12 @@ defmodule Matchmaking.Search.Pool do
                      every player of the mode who has waited at least min_wait_ms anchors a lobby in a rating window of
                      w0 points either side, plus inc per whole step_ms past min_wait_ms, at most w_max (Engine.widen);
                      its lobbies are published like the tick's
+      parties        option (extension, default nil = off, needs a rating-order engine): %{mode name => {min_wait_ms,
+                     w0, step_ms, inc, w_max}}, the party window of the mode.  Before each tick, every party of the
+                     mode that has waited at least min_wait_ms anchors a lobby (Engine.party_match): the other parties
+                     of its window go to the first team with room, the nearest solos fill the rest; a party plays on
+                     one team.  Parties arrive through stage_party/3, one delivery per party, acked or nacked as one
+      party_capacity option (extension, default 0): how many party members the engine holds (Engine.set_party_capacity)
       balance_teams  option (extension, default nil = off): a list of mode names.  Every lobby of those modes, from the
                      tick and from widen, is split into the two teams with the least rating difference
                      (Engine.set_team_balance); the lobby's players are the same, only who plays with whom changes
@@ -66,6 +72,8 @@ defmodule Matchmaking.Search.Pool do
 
   def start_link(opts \\ []), do: GenServer.start_link(__MODULE__, opts, name: __MODULE__)
   def stage(player, game_mode, rating, ack_ref), do: GenServer.cast(__MODULE__, {:stage, player, game_mode, rating, ack_ref})
+  @doc "Parties (extension): players = [{player, rating}] queued together; the delivery is acked or nacked as one."
+  def stage_party(players, game_mode, ack_ref), do: GenServer.cast(__MODULE__, {:stage_party, players, game_mode, ack_ref})
   @doc "A search worker whose channel is open hands its channel name over (patched init, worker_patch.ex)."
   def attach(channel_name), do: GenServer.cast(__MODULE__, {:attach, channel_name})
   def in_queue?(player_id), do: GenServer.call(__MODULE__, {:in_queue?, player_id})
@@ -118,12 +126,16 @@ defmodule Matchmaking.Search.Pool do
       nil -> :ok
       modes -> :ok = Engine.set_team_balance(ref, Enum.reduce(modes, 0, &Bitwise.bor(&2, Bitwise.bsl(1, Engine.mode_index(&1)))))
     end
+    case Keyword.get(opts, :party_capacity) do
+      nil -> :ok
+      members -> :ok = Engine.set_party_capacity(ref, members)
+    end
     # queued: handle -> {rating, mode, enq_ts, seq} at its enqueue, what requeue/1 hands back (kept until remove_user)
     st = %{ref: ref, staged: [], n_staged: 0, handle_of: %{}, players: %{}, free: [], next: 0, channel: nil,
            queued: %{}, moved_out: MapSet.new(),
            t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms),
            lobby_budget: Keyword.get(opts, :lobby_budget), paused: MapSet.new(), regroup_dropped: [],
-           widen: Keyword.get(opts, :widen)}
+           widen: Keyword.get(opts, :widen), parties: Keyword.get(opts, :parties), staged_parties: [], party_of: %{}}
     case resume(st, Keyword.get(opts, :resume), Keyword.get(opts, :regroup, false)) do
       {:ok, st} ->
         Process.send_after(self(), :flush, @flush_ms)
@@ -181,6 +193,10 @@ defmodule Matchmaking.Search.Pool do
     {:noreply, if(st.n_staged >= @max_batch, do: flush(st), else: st)}
   end
 
+  def handle_cast({:stage_party, players, game_mode, ack_ref}, st) do
+    {:noreply, %{st | staged_parties: [{players, game_mode, ack_ref} | st.staged_parties], channel: elem(ack_ref, 0)}}
+  end
+
   def handle_cast({:attach, channel_name}, st), do: {:noreply, %{st | channel: channel_name}}
 
   @impl true
@@ -225,10 +241,16 @@ defmodule Matchmaking.Search.Pool do
     st = flush(st)
     case Map.pop(st.handle_of, id) do
       {nil, _} -> {:reply, {:ok, :removed}, st}                       # Mnesia.delete of a missing key is fine too
-      {h, rest} ->
-        Engine.remove_packed(st.ref, <<h::little-32>>)
-        {:reply, {:ok, :removed}, %{st | handle_of: rest, players: Map.delete(st.players, h), free: [h | st.free],
-                                         queued: Map.delete(st.queued, h)}}
+      {h, _rest} ->
+        Engine.remove_packed(st.ref, <<h::little-32>>)   # a queued party member: the engine removes the whole party
+        hs = Map.get(st.party_of, h, [h])
+        st = Enum.reduce(hs, st, fn x, acc ->
+          {player, players} = Map.pop(acc.players, x)
+          pid = if x == h, do: id, else: player && player["id"]
+          %{acc | handle_of: Map.delete(acc.handle_of, pid), players: players, free: [x | acc.free],
+                  queued: Map.delete(acc.queued, x), party_of: Map.delete(acc.party_of, x)}
+        end)
+        {:reply, {:ok, :removed}, st}
     end
   end
 
@@ -451,6 +473,7 @@ defmodule Matchmaking.Search.Pool do
     st = flush(%{st | regroup_dropped: []})
     now = now_ms(st)
     if st.lobby_budget, do: set_budget(st, st.lobby_budget.())
+    st = party_match(st, now)   # before the tick: parties get the first pick of the solos
     case Engine.tick_packed(st.ref, now) do
       {:ok, lobbies, members, _stats} -> {:noreply, expire(widen(publish(lobbies, members, st), now), now)}
       {:error, _reason} -> {:noreply, st}                              # nothing was consumed; the next tick retries
@@ -493,6 +516,61 @@ defmodule Matchmaking.Search.Pool do
     end
   end
 
+  # -- parties (extension): one rule per queue, as widen; a party's members stay in the active set until remove_user --
+  defp party_match(%{parties: nil} = st, _now), do: st
+  defp party_match(st, now) do
+    rules = for m <- 0..(Engine.n_modes() - 1), _g <- 0..(Engine.n_groups() - 1), into: <<>> do
+      case Map.get(st.parties, Engine.mode_name(m)) do
+        {min_wait, w0, step, inc, w_max} ->
+          <<min_wait::little-32, step::little-32, w0::little-signed-32, inc::little-signed-32, w_max::little-signed-32,
+            0::32>>
+        nil -> <<0xFFFFFFFF::little-32, 1::little-32, 0::32, 0::32, 0::32, 0::32>>
+      end
+    end
+    case Engine.party_match(st.ref, now, rules) do
+      {:ok, lobbies, members} ->
+        st = publish(lobbies, members, st)
+        %{st | party_of: Map.drop(st.party_of, for(<<h::little-32 <- members>>, do: h))}
+      {:error, _reason} -> st                                          # nothing was taken
+    end
+  end
+
+  # one mm_enqueue_party per flush; each party's delivery is acked (1 queued, 0 a member already queued) or nacked
+  defp flush_parties(%{staged_parties: []} = st), do: st
+  defp flush_parties(st) do
+    batch = Enum.reverse(st.staged_parties)
+    {rows, st} = Enum.map_reduce(batch, %{st | staged_parties: []}, fn {players, mode, ack_ref}, acc ->
+      {members, acc} = Enum.map_reduce(players, acc, fn {player, rating}, a ->
+        {h, fresh, a} = acquire(a, player["id"])
+        {{h, fresh, player, clamp(rating)}, a}
+      end)
+      {{members, Engine.mode_index(mode) || 255, ack_ref}, acc}
+    end)
+    sizes = for {ms, _, _} <- rows, into: <<>>, do: <<min(length(ms), 255)>>
+    handles = for {ms, _, _} <- rows, {h, _, _, _} <- ms, into: <<>>, do: <<h::little-32>>
+    ratings = for {ms, _, _} <- rows, {_, _, _, r} <- ms, into: <<>>, do: <<r::little-signed-32>>
+    modes = for {_, m, _} <- rows, into: <<>>, do: <<m>>
+    stamp = now_ms(st)
+    ts = for _ <- rows, into: <<>>, do: <<stamp::little-32>>
+    drop = fn acc, ms -> Enum.reduce(ms, acc, fn {h, fresh, p, _}, a -> if(fresh, do: release(a, p["id"], h), else: a) end) end
+    case (if Enum.all?(rows, fn {ms, _, _} -> length(ms) <= 255 end),
+            do: Engine.enqueue_party(st.ref, sizes, handles, ratings, modes, ts), else: {:error, :party_too_large}) do
+      {:ok, codes} ->
+        Enum.zip(:binary.bin_to_list(codes), rows)
+        |> Enum.reduce(st, fn
+          {1, {ms, _, ack_ref}}, acc ->
+            ack(ack_ref)
+            hs = for {h, _, _, _} <- ms, do: h
+            Enum.reduce(ms, acc, fn {h, _, p, _}, a ->
+              %{a | players: Map.put(a.players, h, p), party_of: Map.put(a.party_of, h, hs)}
+            end)
+          {0, {_, _, ack_ref}}, acc -> ack(ack_ref); acc                 # a member is already in the queue
+          {_, {ms, _, ack_ref}}, acc -> nack(ack_ref); drop.(acc, ms)     # invalid, or the party table is full
+        end)
+      {:error, _reason} -> Enum.reduce(rows, st, fn {ms, _, ack_ref}, acc -> nack(ack_ref); drop.(acc, ms) end)
+    end
+  end
+
   # -- search timeout (extension): after the lobbies, so a player the tick matched is never timed out ---------------
   defp expire(%{timeout: nil} = st, _now), do: st
   defp expire(st, now) do
@@ -503,7 +581,7 @@ defmodule Matchmaking.Search.Pool do
             {player, players} = Map.pop(acc.players, h)
             send_timeout(acc.channel, player)
             %{acc | players: players, handle_of: Map.delete(acc.handle_of, player["id"]), free: [h | acc.free],
-                    queued: Map.delete(acc.queued, h)}
+                    queued: Map.delete(acc.queued, h), party_of: Map.delete(acc.party_of, h)}
         end
       {:error, _reason} -> st                                          # nothing changed; the next tick retries
     end
@@ -523,8 +601,9 @@ defmodule Matchmaking.Search.Pool do
   end
 
   # -- ingest: one mm_enqueue_packed per batch -----------------------------------------------------------------------
-  defp flush(%{staged: []} = st), do: st
-  defp flush(st) do
+  defp flush(st), do: st |> flush_solos() |> flush_parties()
+  defp flush_solos(%{staged: []} = st), do: st
+  defp flush_solos(st) do
     batch = Enum.reverse(st.staged)
     {rows, st} = Enum.map_reduce(batch, st, fn {player, mode, rating, ack_ref}, acc ->
       {h, fresh, acc} = acquire(acc, player["id"])

@@ -8,6 +8,22 @@
 
   # :291-324 — consume/5: no LobbyState pop, no strategist RPC, no per-player Mnesia lookups; the ack moves to the pool
   defp consume(channel_name, _group_name, tag, _headers, payload) do
+    case Poison.decode(payload) do
+      {:ok, %{"party" => party, "game-mode" => game_mode}} when is_list(party) and party != [] and is_binary(game_mode) ->
+        consume_party(channel_name, tag, party, game_mode)   # extension: players who queue together, one delivery
+      _ -> consume_player(channel_name, tag, payload)
+    end
+  end
+
+  defp consume_party(channel_name, tag, party, game_mode) do
+    players = for %{"id" => id, "rating" => r} = p <- party, (is_binary(id) or is_integer(id)) and is_number(r),
+                do: {p, trunc(r)}
+    if length(players) == length(party),
+      do: Matchmaking.Search.Pool.stage_party(players, game_mode, {channel_name, tag}),
+      else: nack(channel_name, tag)
+  end
+
+  defp consume_player(channel_name, tag, payload) do
     with {:ok, %{"id" => _} = player_data} <- Poison.decode(payload),
          {game_mode, player} when is_binary(game_mode) <- Map.pop(player_data, "game-mode"),
          rating when is_number(rating) <- player_data["rating"] || get_in(player_data, ["detail", "rating"]) do

@@ -128,6 +128,21 @@ class WidenStats(C.Structure):
     ]
 
 
+class PartyStats(C.Structure):
+    """mm_party_stats: counts of one mm_party_match call (32 bytes)."""
+    _fields_ = [
+        ("n_anchors", C.c_uint32),
+        ("n_lobbies", C.c_uint32),
+        ("n_matched", C.c_uint32),
+        ("n_parties", C.c_uint32),
+        ("n_absorbed", C.c_uint32),
+        ("device_us", C.c_float),
+        ("reserved", C.c_uint32 * 2),
+    ]
+
+
+assert C.sizeof(WidenRule) == 24 and C.sizeof(WidenStats) == 32 and C.sizeof(PartyStats) == 32
+
 MM_LOCATE_STAYS = 0xFFFFFFFF
 
 
@@ -251,6 +266,10 @@ PROTOTYPES = {
                                 _vp, C.c_uint32, _vp, C.c_uint64, _vp, _P(BandStats)]),
     "mm_backfill": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, C.c_uint64, _P(C.c_uint32)]),
     "mm_widen": (C.c_int, [_vp, C.c_uint64, _vp, _vp, C.c_uint32, _vp, C.c_uint64, _P(WidenStats)]),
+    "mm_enqueue_party": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "mm_party_match": (C.c_int, [_vp, C.c_uint64, _vp, _vp, C.c_uint32, _vp, C.c_uint64, _P(PartyStats)]),
+    "mm_party_read": (C.c_int, [_vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _P(C.c_uint32),
+                                _P(C.c_uint32)]),
     "mm_in_queue": (C.c_int, [_vp, C.c_uint32, _vp, _vp]),
     "mm_locate": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp]),
     "mm_pool_size": (C.c_int, [_vp, _P(C.c_uint32)]),

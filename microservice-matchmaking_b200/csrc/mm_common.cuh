@@ -99,6 +99,21 @@ struct ActiveView {
   __device__ __forceinline__ unsigned long long* val(uint64_t h) const { return dcap ? kv + h : kv + 2 * h + 1; }
 };
 
+// Party members (mm_party.cuh): a queued member's value is kPtVal(row of its party), pool generation 0, which no pool
+// ever has; a matched member's is kPtMatched, a slot past every pool.
+constexpr uint64_t kPtMatched = ((uint64_t)kGenMask << 32) | 0xFFFFFFFFull;
+__device__ __forceinline__ uint64_t kPtVal(uint32_t row) { return row; }
+__device__ __forceinline__ bool pt_queued(uint64_t v) { return (v >> 32) == 0; }  // of a committed value (< kPending)
+
+struct PartyView {  // the party table as the kernels take it (mm_party.cuh); all null without party_capacity
+  uint32_t *seq, *ts, *off;
+  int32_t* R;
+  uint16_t* bin;
+  uint8_t *mode, *grp, *size, *dead;  // dead: 0 queued, 1 gone, 2 dissolving (mm_remove)
+  uint64_t* mid;                      // members: ids and ratings, a party's at its row's offset in enqueue order
+  int32_t* mrat;
+};
+
 __device__ __forceinline__ uint64_t hash64(uint64_t x) {
   x ^= x >> 33; x *= 0xFF51AFD7ED558CCDull; x ^= x >> 33; x *= 0xC4CEB9FE1A85EC53ull; x ^= x >> 33;
   return x;

@@ -26,6 +26,7 @@
 #include "mm_image.cuh"
 #include "mm_kernels.cuh"
 #include "mm_locate.cuh"
+#include "mm_party.cuh"
 #include "mm_quality.cuh"
 #include "mm_recut.cuh"
 #include "mm_regroup.cuh"
@@ -321,6 +322,28 @@ struct mm_engine {
     DevArray<uint32_t> cval;  // [capacity + 64] c - key_lo per member slot (arrival-order ticks, mm_widen)
     DevArray<uint32_t> w;     // arrival order: live slots per tile -> offsets [n_tiles] | per partition [n_segs] | total
   } tb;
+
+  // parties (mm_party.cuh): the table in two buffers (compaction moves it from one to the other), sized by
+  // party_capacity; the batch and match scratch grown on demand.  Not part of images or snapshots.
+  struct Party {
+    uint32_t cap = 0;                  // party_capacity: members the table holds (0: no table)
+    uint32_t n_rows = 0, n_mem = 0;    // rows and member entries in use, gone parties included
+    uint32_t live = 0;                 // members of queued parties
+    struct Buf {
+      DevArray<uint32_t> seq, ts, off;
+      DevArray<int32_t> R, mrat;
+      DevArray<uint16_t> bin;
+      DevArray<uint8_t> mode, grp, size, dead;
+      DevArray<uint64_t> mid;
+    } buf[2];
+    int cur = 0;
+    DevArray<uint8_t> in_size, in_mode, in_pre, in_code;
+    DevArray<uint32_t> in_ts, in_moff, in_mparty, in_msz, in_one;
+    DevArray<uint64_t> in_id, in_hslot;
+    DevArray<int32_t> in_rating;
+    DevArray<uint32_t> pb, pcur, tmp, sorted, lob, pos;  // match: [K + 1], [K], then [rows] each (tmp: compaction)
+    DevArray<uint32_t> ctr;                              // [kPtWords + 2]
+  } pt;
 };
 
 namespace {
@@ -422,6 +445,13 @@ ActiveView act_view(mm_engine* e) {
     else a.mask = e->hcap - 1;
   }
   return a;
+}
+
+// the party table in buffer b as the kernels take it (all null without party_capacity)
+PartyView pt_view(mm_engine* e, int b) {
+  auto& t = e->pt.buf[b];
+  if (!e->pt.cap) return PartyView{};
+  return PartyView{t.seq, t.ts, t.off, t.R, t.bin, t.mode, t.grp, t.size, t.dead, t.mid, t.mrat};
 }
 
 size_t table_bytes(const mm_engine* e) { return e->hcap * (e->dense_ids ? 8 : 16); }
@@ -672,16 +702,21 @@ int rehash(mm_engine* e) {
 
 // capacity checks + scratch for an ingest batch of n players, of which at most n_new can add an active-set entry
 // (mm_merge counts them exactly; every other batch passes n)
-int enq_prepare(mm_engine* e, uint32_t n, uint32_t n_new) {
-  e->fresh = false;
-  int rc = ensure_enq_scratch(e, n);
-  if (rc) return rc;
+// a hashed active set that could not take n_new more ids: rehashed, or MM_E_CAP (a batch of n entries)
+int act_room(mm_engine* e, uint32_t n, uint32_t n_new) {
   if (e->use_active && !e->dense_ids && (e->n_active + e->n_tomb + n_new) * 4 > e->hcap * 3) {
     if ((e->n_active + n_new) * 4 > e->hcap * 3)
       return set_err(e, MM_E_CAP, "active set full: %llu ids resident, batch of %u, capacity %llu",
                      (unsigned long long)e->n_active, n, (unsigned long long)(e->hcap * 3 / 4));
-    if ((rc = rehash(e))) return rc;
+    return rehash(e);
   }
+  return MM_OK;
+}
+
+int enq_prepare(mm_engine* e, uint32_t n, uint32_t n_new) {
+  e->fresh = false;
+  int rc = ensure_enq_scratch(e, n);
+  if (rc || (rc = act_room(e, n, n_new))) return rc;
   if ((size_t)n + 64 > e->d_code.n) {  // the batch is taken: the previous batch's codes may go
     e->last_batch_n = 0;
     CK(e->d_code.reserve((size_t)n + 64));
@@ -1039,6 +1074,10 @@ uint64_t seen_keys(uint64_t n) {
 int staged_err(mm_engine* e) {
   return set_err(e, MM_E_STATE, "a packed batch is staged: call mm_enqueue_packed_end first");
 }
+// The refusal of the image calls and mm_snapshot while a party is queued.
+int parties_err(mm_engine* e) {
+  return set_err(e, MM_E_STATE, "%u party members are queued: images and snapshots do not carry parties", e->pt.live);
+}
 uint32_t tile_ctas(const mm_engine* e, uint32_t n) {
   return std::max<uint32_t>(1, std::min<uint32_t>(tile_count(e, n), 8u * (uint32_t)e->n_sms));
 }
@@ -1107,6 +1146,12 @@ int launch_expire(mm_engine* e, ExpireArgs a) {
   a.ctr = &e->d_cnt->expired;
   CK(cudaMemsetAsync(a.ctr, 0, 2 * 4, e->stream));  // expired, erased
   k_expire<kExpBlock><<<tile_ctas(e, p.n), kExpBlock, 0, e->stream>>>(a);
+  if (e->pt.live && !a.sel) {  // whole parties, behind the solos
+    CK(cudaMemsetAsync(e->pt.ctr, 0, kPtWords * 4, e->stream));
+    k_pt_expire<<<(e->pt.n_rows + 255) / 256, 256, 0, e->stream>>>(e->pt.n_rows, pt_view(e, e->pt.cur), a.now,
+                                                                    a.max_wait, a.commit, a.act, a.out_id, a.out_handle,
+                                                                    a.out_seq, a.ctr, e->pt.ctr);
+  }
   CK(cudaGetLastError());
   return MM_OK;
 }
@@ -1117,12 +1162,13 @@ int expire(mm_engine* e, uint64_t now, uint32_t max_wait, uint64_t* ids, uint32_
            uint32_t* n_expired) {
   const Pool& p = e->pool[e->cur];
   *n_expired = 0;
-  if (p.n == 0) return MM_OK;
+  const uint32_t most = p.n + e->pt.live;
+  if (most == 0) return MM_OK;
   ExpireArgs a{};
   a.now = (uint32_t)now; a.max_wait = max_wait;
-  uint32_t need = p.n;
+  uint32_t need = most;
   int rc;
-  if (cap < p.n) {
+  if (cap < most) {
     if ((rc = launch_expire(e, a)) || (rc = read_counters(e))) return rc;
     need = e->h_cnt->expired;
     *n_expired = need;
@@ -1135,8 +1181,12 @@ int expire(mm_engine* e, uint64_t now, uint32_t max_wait, uint64_t* ids, uint32_
   a.out_id = ids ? e->d_exp_id.p : nullptr;
   a.out_handle = ids ? nullptr : reinterpret_cast<uint32_t*>(e->d_exp_id.p);
   a.out_seq = seq ? e->d_exp_seq.p : nullptr;
-  if ((rc = launch_expire(e, a)) || (rc = read_counters(e))) return rc;
+  uint32_t gone = 0;
+  if ((rc = launch_expire(e, a))) return rc;
+  if (e->pt.live) CK(cudaMemcpyAsync(&gone, e->pt.ctr + kPtGone, 4, cudaMemcpyDeviceToHost, e->stream));
+  if ((rc = read_counters(e))) return rc;  // (synchronises the stream: `gone` has arrived)
   const uint32_t n = e->h_cnt->expired;
+  e->pt.live -= gone;
   if (n) {
     if (ids) CK(cudaMemcpyAsync(ids, e->d_exp_id, (size_t)n * 8, cudaMemcpyDeviceToHost, e->stream));
     else CK(cudaMemcpyAsync(handles, e->d_exp_id, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
@@ -1564,11 +1614,24 @@ int remove_or_take(mm_engine* e, uint32_t n, const uint64_t* id, uint32_t* n_out
   const Pool& p = e->pool[e->cur];
   CK(cudaMemcpyAsync(e->d_in_id, id, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemsetAsync(&e->d_cnt->removed, 0, 4, e->stream));
+  const bool parties = !take && e->pt.live;  // a removed party member dissolves its whole party
+  const PartyView t = pt_view(e, e->pt.cur);
+  if (parties) {
+    CK(cudaMemsetAsync(e->pt.ctr, 0, kPtWords * 4, e->stream));
+    k_pt_mark<<<(n + 255) / 256, 256, 0, e->stream>>>(n, e->d_in_id, act_view(e), t);
+  }
   (take ? k_take : k_remove)<<<(n + 255) / 256, 256, 0, e->stream>>>(
       n, e->d_in_id, act_view(e), p.v, p.m, (uint32_t)pool_slots(e), e->gen, e->K, e->d_bin_seg, e->d_seg_bin_lo,
       &e->d_cnt->removed);
+  uint32_t gone = 0;
+  if (parties) {
+    k_pt_dissolve<<<(e->pt.n_rows + 255) / 256, 256, 0, e->stream>>>(e->pt.n_rows, t, act_view(e), &e->d_cnt->removed,
+                                                                      e->pt.ctr);
+    CK(cudaMemcpyAsync(&gone, e->pt.ctr + kPtGone, 4, cudaMemcpyDeviceToHost, e->stream));
+  }
   CK(cudaGetLastError());
-  if ((rc = read_counters(e))) return rc;
+  if ((rc = read_counters(e))) return rc;  // (synchronises the stream: `gone` has arrived)
+  e->pt.live -= gone;
   if (!take) erase_active(e, e->h_cnt->removed);
   if (n_out) *n_out = e->h_cnt->removed;
   return MM_OK;
@@ -2281,12 +2344,12 @@ int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_t
 }
 
 // ---- mm_widen (mm_widen.cuh) ---------------------------------------------------------------------------------------
-int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
-          uint64_t* member_ids, uint64_t member_cap, mm_widen_stats* st) {
+// The rules of mm_widen / mm_party_match as the device reads them, and the refusals both share.  any: a queue is served.
+int wd_rules(mm_engine* e, const mm_widen_rule* rules, std::vector<WdRule>& rule, bool& any) {
   const mm_config& c = e->cfg;
   const uint32_t G = c.n_groups, nc = e->n_cut;
-  std::vector<WdRule> rule(nc);
-  bool any = false;
+  rule.resize(nc);
+  any = false;
   for (uint32_t q = 0; q < nc; ++q) {
     const mm_widen_rule& r = rules[q];
     const mm_mode_desc& md = c.modes[q / G];
@@ -2300,6 +2363,15 @@ int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* 
   if (c.order_mode != MM_ORDER_RATING) return set_err(e, MM_E_ARG, "widening windows need MM_ORDER_RATING");
   if (!e->use_active) return set_err(e, MM_E_STATE, "an MM_F_NO_DEDUPE engine cannot hold taken players");
   if (e->stage_count) return staged_err(e);
+  return MM_OK;
+}
+
+int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
+          uint64_t* member_ids, uint64_t member_cap, mm_widen_stats* st) {
+  const uint32_t G = e->cfg.n_groups, nc = e->n_cut;
+  std::vector<WdRule> rule;
+  bool any = false;
+  if (int rc = wd_rules(e, rules, rule, any)) return rc;
   const Pool& p = e->pool[e->cur];
   if (!any || p.n == 0) return MM_OK;
   auto& s = e->wd;
@@ -2412,7 +2484,7 @@ int locate(mm_engine* e, uint64_t now, uint32_t n, const uint64_t* id, mm_player
   a.bin_seg = e->d_bin_seg; a.seg_bin_lo = e->d_seg_bin_lo; a.seg_L = e->d_seg_L; a.part_cut = e->d_part_cut;
   a.cut_lp_lo = e->d_cut_lp_lo; a.rmap = rmap; a.pos = pos; a.outbase = ob; a.binlim = bl; a.out = s.out;
   a.tb_mask = e->tb_mask; a.arrival = e->cfg.order_mode == MM_ORDER_ARRIVAL; a.mode_tsize = e->d_mode_tsize;
-  a.bin_key = e->d_bin_key; a.key_lo = e->key_lo; a.KR = e->KR;
+  a.bin_key = e->d_bin_key; a.key_lo = e->key_lo; a.KR = e->KR; a.pt = pt_view(e, e->pt.cur);
   k_locate<<<(uint32_t)(((size_t)n * 32 + 255) / 256), 256, 0, e->stream>>>(a);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(out, s.out, (size_t)n * sizeof(mm_player_status), cudaMemcpyDeviceToHost, e->stream));
@@ -2484,6 +2556,295 @@ int match_quality(mm_engine* e, mm_queue_quality* per_queue, mm_lobby_quality* p
   }
   if (n_dev != n_lob)
     return set_err(e, MM_E_STATE, "the last tick's pool holds %u matched lobbies, the tick emitted %u", n_dev, n_lob);
+  return MM_OK;
+}
+
+// ---- parties (mm_party.cuh) ----------------------------------------------------------------------------------------
+uint32_t pt_rows_cap(const mm_engine* e) { return e->pt.cap / 2 + 1; }  // a party has at least two members
+
+// The table's buffer b and the match scratch at the capacity's sizes (b's contents are lost).
+int pt_alloc(mm_engine* e, int b) {
+  auto& t = e->pt.buf[b];
+  const size_t r = pt_rows_cap(e), m = (size_t)e->pt.cap + 1;
+  t = mm_engine::Party::Buf{};
+  CK(t.seq.reserve(r)); CK(t.ts.reserve(r)); CK(t.off.reserve(r)); CK(t.R.reserve(r)); CK(t.bin.reserve(r));
+  CK(t.mode.reserve(r)); CK(t.grp.reserve(r)); CK(t.size.reserve(r)); CK(t.dead.reserve(r));
+  CK(t.mid.reserve(m)); CK(t.mrat.reserve(m));
+  auto& s = e->pt;
+  for (auto* a : {&s.tmp, &s.sorted, &s.lob, &s.pos}) { a->reset(); CK(a->reserve(r)); }
+  CK(s.pb.reserve((size_t)e->K + 1)); CK(s.pcur.reserve(e->K)); CK(s.ctr.reserve(kPtWords + 2));
+  return MM_OK;
+}
+
+// Compaction: the queued parties' rows, stable, into the other buffer (their members' active-set values follow).
+int pt_compact(mm_engine* e) {
+  auto& s = e->pt;
+  if (!s.n_rows) { s.n_mem = 0; return MM_OK; }
+  const uint32_t n = s.n_rows, g = (n + 255) / 256;
+  uint32_t* tot = s.ctr + kPtWords;
+  CK(cudaMemsetAsync(tot, 0, 8, e->stream));
+  k_pt_keep<<<g, 256, 0, e->stream>>>(n, pt_view(e, s.cur), s.tmp, s.sorted);
+  k_scan_small<<<1, 1024, 0, e->stream>>>(n, s.tmp, tot);
+  k_scan_small<<<1, 1024, 0, e->stream>>>(n, s.sorted, tot + 1);
+  k_pt_move<<<g, 256, 0, e->stream>>>(n, pt_view(e, s.cur), pt_view(e, s.cur ^ 1), s.tmp, s.sorted, act_view(e));
+  CK(cudaGetLastError());
+  uint32_t h[2];
+  CK(cudaMemcpyAsync(h, tot, 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  s.n_rows = h[0]; s.n_mem = h[1]; s.cur ^= 1;
+  return MM_OK;
+}
+
+// mm_set_option("party_capacity", P): both buffers at the new size, the queued parties kept.
+int pt_set_capacity(mm_engine* e, int64_t value) {
+  auto& s = e->pt;
+  if (value < 0 || value > 0x7FFF0000)
+    return set_err(e, MM_E_ARG, "party_capacity %lld is out of range", (long long)value);
+  if ((uint64_t)value < s.live)
+    return set_err(e, MM_E_ARG, "party_capacity %lld is below the %u party members queued", (long long)value, s.live);
+  if ((uint32_t)value == s.cap) return MM_OK;
+  int rc;
+  if (value == 0) {
+    s = mm_engine::Party{};  // nothing is queued
+    return MM_OK;
+  }
+  if (s.n_rows && (rc = pt_compact(e))) return rc;  // the queued parties now fill buffer cur from row 0
+  const uint32_t old = s.cap;
+  s.cap = (uint32_t)value;
+  if ((rc = pt_alloc(e, s.cur ^ 1))) { s.cap = old; return rc; }
+  if (s.n_rows) {
+    const PartyView d = pt_view(e, s.cur ^ 1);
+    s.cap = old;
+    const PartyView o = pt_view(e, s.cur);
+    s.cap = (uint32_t)value;
+    const size_t r = s.n_rows, m = s.n_mem;
+    CK(cudaMemcpyAsync(d.seq, o.seq, r * 4, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpyAsync(d.ts, o.ts, r * 4, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpyAsync(d.off, o.off, r * 4, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpyAsync(d.R, o.R, r * 4, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpyAsync(d.bin, o.bin, r * 2, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpyAsync(d.mode, o.mode, r, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpyAsync(d.grp, o.grp, r, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpyAsync(d.size, o.size, r, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpyAsync(d.dead, o.dead, r, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpyAsync(d.mid, o.mid, m * 8, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaMemcpyAsync(d.mrat, o.mrat, m * 4, cudaMemcpyDeviceToDevice, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+  }
+  s.cur ^= 1;
+  return pt_alloc(e, s.cur ^ 1);
+}
+
+// the refusals every party call shares
+int pt_check(mm_engine* e) {
+  if (e->cfg.order_mode != MM_ORDER_RATING) return set_err(e, MM_E_ARG, "parties need MM_ORDER_RATING");
+  if (!e->pt.cap) return set_err(e, MM_E_STATE, "no party capacity: set the option party_capacity first");
+  if (!e->use_active) return set_err(e, MM_E_STATE, "an MM_F_NO_DEDUPE engine cannot hold parties");
+  if (e->stage_count) return staged_err(e);
+  return MM_OK;
+}
+
+int enqueue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t* ids, const int32_t* rating,
+                  const uint8_t* mode, const uint32_t* enq_ts, uint8_t* accepted) {
+  int rc = pt_check(e);
+  if (rc || n == 0) return rc;
+  auto& s = e->pt;
+  std::vector<uint32_t> moff(n), mparty;
+  uint32_t m = 0;
+  for (uint32_t j = 0; j < n; ++j) {
+    moff[j] = m;
+    m += size[j];
+    mparty.insert(mparty.end(), size[j], j);
+  }
+  if ((rc = act_room(e, m, m))) return rc;
+  e->fresh = false;
+  if (s.n_mem + (uint64_t)m > s.cap && (rc = pt_compact(e))) return rc;
+  CK(s.in_size.reserve(n)); CK(s.in_mode.reserve(n)); CK(s.in_code.reserve(n)); CK(s.in_ts.reserve(n));
+  CK(s.in_moff.reserve(n)); CK(s.in_msz.reserve(n)); CK(s.in_one.reserve(n));
+  const size_t mm = std::max<uint32_t>(m, 1);
+  CK(s.in_pre.reserve(mm)); CK(s.in_mparty.reserve(mm)); CK(s.in_id.reserve(mm)); CK(s.in_hslot.reserve(mm));
+  CK(s.in_rating.reserve(mm));
+  CK(cudaMemcpyAsync(s.in_size, size, n, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(s.in_mode, mode, n, cudaMemcpyHostToDevice, e->stream));
+  if (enq_ts) CK(cudaMemcpyAsync(s.in_ts, enq_ts, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(s.in_moff, moff.data(), (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  if (m) {
+    CK(cudaMemcpyAsync(s.in_mparty, mparty.data(), (size_t)m * 4, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(s.in_id, ids, (size_t)m * 8, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(s.in_rating, rating, (size_t)m * 4, cudaMemcpyHostToDevice, e->stream));
+  }
+  CK(cudaMemsetAsync(s.ctr, 0, (kPtWords + 2) * 4, e->stream));
+  PtEnqArgs a{};
+  a.n = n; a.m = m; a.size = s.in_size; a.moff = s.in_moff; a.mparty = s.in_mparty; a.id = s.in_id;
+  a.rating = s.in_rating; a.mode = s.in_mode; a.ts = enq_ts ? s.in_ts.p : nullptr; a.act = act_view(e);
+  a.bm = bin_map(e); a.grp_lut = e->d_grp_lut; a.mode_tsize = e->d_mode_tsize; a.n_modes = e->cfg.n_modes;
+  a.hslot = s.in_hslot; a.pre = s.in_pre; a.code = s.in_code; a.msz = s.in_msz; a.one = s.in_one;
+  a.tot = s.ctr + kPtWords; a.room = s.cap - s.n_mem; a.rows0 = s.n_rows; a.mem0 = s.n_mem; a.seq0 = e->seq_next;
+  a.pt = pt_view(e, s.cur); a.ctr = s.ctr;
+  const uint32_t gm = (m + 255) / 256, gn = (n + 255) / 256;
+  if (m) k_pt_claim<<<gm, 256, 0, e->stream>>>(a);
+  k_pt_resolve<<<gn, 256, 0, e->stream>>>(a);
+  k_scan_small<<<1, 1024, 0, e->stream>>>(n, s.in_msz, a.tot);
+  k_scan_small<<<1, 1024, 0, e->stream>>>(n, s.in_one, a.tot + 1);
+  k_pt_commit<<<gn, 256, 0, e->stream>>>(a);
+  if (m) k_pt_members<<<gm, 256, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  std::vector<uint8_t> code(n);
+  uint32_t h[kPtWords];
+  CK(cudaMemcpyAsync(code.data(), s.in_code, n, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(h, s.ctr, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  uint32_t rows = 0;
+  for (uint32_t j = 0; j < n; ++j) rows += code[j] == 1;
+  const uint32_t acc = h[kPtAccepted];
+  s.n_rows += rows; s.n_mem += acc; s.live += acc;
+  e->n_active += acc;
+  if (!e->dense_ids) e->n_tomb += h[kPtReleased];
+  e->seq_next += n;
+  if (accepted) std::memcpy(accepted, code.data(), n);
+  return MM_OK;
+}
+
+int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
+                uint64_t* member_ids, uint64_t member_cap, mm_party_stats* st) {
+  const mm_config& c = e->cfg;
+  const uint32_t G = c.n_groups, nc = e->n_cut;
+  std::vector<WdRule> rule;
+  bool any = false;
+  int rc = wd_rules(e, rules, rule, any);
+  if (rc) return rc;
+  for (uint32_t q = 0; q < nc; ++q)
+    if (rule[q].min_wait != MM_WIDEN_OFF && c.modes[q / G].teams > kPtMaxTeams)
+      return set_err(e, MM_E_ARG, "rule %u: mode %u has %u teams (parties: at most %u)", q, q / G, c.modes[q / G].teams,
+                     kPtMaxTeams);
+  if ((rc = pt_check(e))) return rc;
+  auto& s = e->pt;
+  if (!any || !s.live) return MM_OK;
+  CK(cudaEventRecord(e->ev[0], e->stream));
+  if ((rc = pt_compact(e))) return rc;
+  const Pool& p = e->pool[e->cur];
+  const uint32_t nr = s.n_rows, K = e->K, gr = (nr + 255) / 256;
+  // the rows by (bin, age)
+  PtArgs x{};
+  x.t = pt_view(e, s.cur); x.n_rows = nr; x.pb = s.pb; x.pcur = s.pcur; x.sorted = s.sorted;
+  x.lob = s.lob; x.pos = s.pos; x.mode_tsize = e->d_mode_tsize; x.ctr = s.ctr;
+  CK(cudaMemsetAsync(s.pb, 0, ((size_t)K + 1) * 4, e->stream));
+  CK(cudaMemsetAsync(s.ctr, 0, (kPtWords + 2) * 4, e->stream));
+  k_pt_count<<<gr, 256, 0, e->stream>>>(x, s.pb);
+  k_scan_small<<<1, 1024, 0, e->stream>>>(K + 1, s.pb, s.ctr + kPtWords);
+  CK(cudaMemcpyAsync(s.pcur, s.pb, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
+  k_pt_scatter<<<1, kPtScatterBlock, 0, e->stream>>>(x);
+  CK(cudaMemcpyAsync(s.pcur, s.pb, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));  // the plan's cursors
+  // the plan, on the solo pool's per-bin totals (the mm_widen scratch)
+  auto& w = e->wd;
+  auto& b = e->bf;
+  const uint32_t rw = sizeof(WdRule) / 4;
+  const size_t o_qlob = rw * nc, o_qlb = o_qlob + nc, o_qmb = o_qlb + nc, o_ctr = o_qmb + nc;
+  CK(w.tab.reserve(o_ctr + kWdWords));
+  CK(w.anc.reserve((size_t)nr * 3));
+  uint32_t maxT = 1;
+  for (uint32_t m = 0; m < c.n_modes; ++m) maxT = std::max<uint32_t>(maxT, c.modes[m].teams);
+  const size_t n_pieces = std::min<uint64_t>((uint64_t)nr * maxT, p.n) + K;  // each team's walk empties all bins but its last
+  CK(b.rem.reserve(K)); CK(b.key_bin.reserve(K)); CK(b.kbase.reserve(K)); CK(b.klim.reserve(K));
+  CK(b.piece.reserve(n_pieces));
+  uint32_t* t = w.tab;
+  CK(cudaMemcpyAsync(t, rule.data(), nc * sizeof(WdRule), cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemsetAsync(t + o_qlob, 0, nc * 4, e->stream));
+  CK(cudaMemsetAsync(t + o_ctr, 0, kWdWords * 4, e->stream));
+  CK(cudaMemcpyAsync(b.rem, p.m.tot, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
+  WdArgs a{};
+  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.n_cut = nc; a.n_groups = G; a.now = (uint32_t)now;
+  a.seq_next = e->seq_next; a.rule = reinterpret_cast<const WdRule*>(t); a.part_cut = e->d_part_cut;
+  a.cut_lp_lo = e->d_cut_lp_lo; a.seg_bin_lo = e->d_seg_bin_lo; a.bin_seg = e->d_bin_seg; a.bin_key = e->d_bin_key;
+  a.tot = p.m.tot; a.rem = b.rem; a.piece = b.piece;
+  a.qlob = t + o_qlob; a.qlbase = t + o_qlb; a.qmbase = t + o_qmb; a.ctr = t + o_ctr;
+  a.rec = reinterpret_cast<uint2*>(w.anc.p); a.mbase = w.anc + 2 * (size_t)nr;
+  k_pt_plan<<<(nc + kPtPlanWarps - 1) / kPtPlanWarps, kPtPlanWarps * 32, 0, e->stream>>>(x, a);
+  BfArgs f{};
+  f.tot = p.m.tot; f.rem = b.rem; f.bin_seg = e->d_bin_seg; f.fill = p.m.fill; f.K = K;
+  f.key_bin = b.key_bin; f.kbase = b.kbase; f.klim = b.klim; f.ctr = a.ctr;
+  k_bf_keys<<<1, kBfKeysBlock, 0, e->stream>>>(f);
+  k_wd_bases<<<1, 32, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e->ev[4], e->stream));
+  uint32_t h[kWdWords], hp[kPtWords];
+  std::vector<uint32_t> qlob(nc);
+  CK(cudaMemcpyAsync(h, a.ctr, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(hp, s.ctr, sizeof(hp), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(qlob.data(), a.qlob, nc * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  uint64_t nm = 0;
+  for (uint32_t q = 0; q < nc; ++q)
+    if (rule[q].min_wait != MM_WIDEN_OFF) nm += (uint64_t)qlob[q] * rule[q].L;
+  const uint32_t nl = h[kWdLobbies], ns = h[kBfPlayers];
+  st->n_anchors = hp[kPtAnchors]; st->n_lobbies = nl; st->n_matched = (uint32_t)nm; st->n_parties = hp[kPtPlaced];
+  st->n_absorbed = h[kWdAbsorbed];
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]));
+  st->device_us = ms * 1000.f;  // a refused or empty call reports the table, sort and plan it ran
+  if (lobby_cap < nl || member_cap < nm)
+    return set_err(e, MM_E_CAP, "need lobby_cap >= %u and member_cap >= %llu", nl, (unsigned long long)nm);
+  if (nl == 0) return MM_OK;
+  // from here on the call changes the pool and the table
+  if (ns && (rc = bf_take(e, h))) return rc;
+  CK(b.members.reserve(nm));
+  CK(w.hdr.reserve(nl));
+  a.hdr = w.hdr;
+  k_wd_hdr<<<(nl + 255) / 256, 256, 0, e->stream>>>(a, nl);
+  const uint32_t np = h[kBfPieces];
+  if (np)
+    k_bf_out<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase,
+                                                                                 a.mbase, b.staging, b.members);
+  x.members = b.members;
+  k_pt_out<<<gr, 256, 0, e->stream>>>(x, a.mbase, act_view(e));
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e->ev[4], e->stream));
+  CK(cudaMemcpyAsync(lobbies, w.hdr, (size_t)nl * sizeof(mm_lobby_hdr), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(member_ids, b.members, (size_t)nm * 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  s.live -= (uint32_t)(nm - ns);
+  CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]));
+  st->device_us = ms * 1000.f;
+  return MM_OK;
+}
+
+int party_read(mm_engine* e, uint32_t party_cap, uint32_t member_cap, uint8_t* size, uint32_t* seq, uint32_t* enq_ts,
+               uint8_t* mode, uint8_t* group, int32_t* rating, uint64_t* member_ids, int32_t* member_rating,
+               uint32_t* n_parties, uint32_t* n_members) {
+  auto& s = e->pt;
+  const uint32_t r = s.n_rows, m = s.n_mem;
+  std::vector<uint32_t> hseq(r), hts(r), hoff(r);
+  std::vector<int32_t> hR(r), hmr(m);
+  std::vector<uint8_t> hmode(r), hgrp(r), hsize(r), hdead(r);
+  std::vector<uint64_t> hmid(m);
+  const PartyView t = pt_view(e, s.cur);
+  if (r) {
+    CK(cudaMemcpyAsync(hseq.data(), t.seq, r * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(hts.data(), t.ts, r * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(hoff.data(), t.off, r * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(hR.data(), t.R, r * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(hmode.data(), t.mode, r, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(hgrp.data(), t.grp, r, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(hsize.data(), t.size, r, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(hdead.data(), t.dead, r, cudaMemcpyDeviceToHost, e->stream));
+  }
+  if (m) {
+    CK(cudaMemcpyAsync(hmid.data(), t.mid, (size_t)m * 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(hmr.data(), t.mrat, (size_t)m * 4, cudaMemcpyDeviceToHost, e->stream));
+  }
+  CK(cudaStreamSynchronize(e->stream));
+  uint32_t np = 0, nm = 0;
+  for (uint32_t i = 0; i < r; ++i)
+    if (!hdead[i]) { ++np; nm += hsize[i]; }
+  *n_parties = np; *n_members = nm;
+  if (np > party_cap || nm > member_cap)
+    return set_err(e, MM_E_CAP, "need party_cap >= %u and member_cap >= %u", np, nm);
+  for (uint32_t i = 0, k = 0, o = 0; i < r; ++i) {
+    if (hdead[i]) continue;
+    size[k] = hsize[i]; seq[k] = hseq[i]; enq_ts[k] = hts[i]; mode[k] = hmode[i]; group[k] = hgrp[i]; rating[k] = hR[i];
+    for (uint32_t j = 0; j < hsize[i]; ++j, ++o) { member_ids[o] = hmid[hoff[i] + j]; member_rating[o] = hmr[hoff[i] + j]; }
+    ++k;
+  }
   return MM_OK;
 }
 
@@ -2680,6 +3041,7 @@ int mm_set_option(mm_engine* e, const char* name, int64_t value) {
     return MM_OK;
   }
   if (!std::strcmp(name, "tick_impl")) { e->tick_impl = value != 0; return MM_OK; }
+  if (!std::strcmp(name, "party_capacity")) return pt_set_capacity(e, value);  // EXTENSION (parties, mm_party.cuh)
   return MM_E_ARG;
 }
 
@@ -2875,6 +3237,39 @@ int mm_widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hd
     return set_err(e, MM_E_ARG, "null lobbies or member_ids with a non-zero capacity");
   CK(cudaSetDevice(e->device));
   return widen(e, now, rules, lobbies, lobby_cap, member_ids, member_cap, stats);
+}
+
+int mm_enqueue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t* ids, const int32_t* rating,
+                     const uint8_t* mode, const uint32_t* enq_ts, uint8_t* accepted) {
+  if (!e) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (n && (!size || !ids || !rating || !mode)) return set_err(e, MM_E_ARG, "null size, ids, rating or mode with n = %u", n);
+  CK(cudaSetDevice(e->device));
+  return enqueue_party(e, n, size, ids, rating, mode, enq_ts, accepted);
+}
+
+int mm_party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
+                   uint64_t* member_ids, uint64_t member_cap, mm_party_stats* stats) {
+  if (!e) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!rules || !stats) return set_err(e, MM_E_ARG, "null rules or stats");
+  std::memset(stats, 0, sizeof(*stats));
+  if ((lobby_cap && !lobbies) || (member_cap && !member_ids))
+    return set_err(e, MM_E_ARG, "null lobbies or member_ids with a non-zero capacity");
+  CK(cudaSetDevice(e->device));
+  return party_match(e, now, rules, lobbies, lobby_cap, member_ids, member_cap, stats);
+}
+
+int mm_party_read(mm_engine* e, uint32_t party_cap, uint32_t member_cap, uint8_t* size, uint32_t* seq, uint32_t* enq_ts,
+                  uint8_t* mode, uint8_t* group, int32_t* rating, uint64_t* member_ids, int32_t* member_rating,
+                  uint32_t* n_parties, uint32_t* n_members) {
+  if (!e || !n_parties || !n_members || (party_cap && (!size || !seq || !enq_ts || !mode || !group || !rating)) ||
+      (member_cap && (!member_ids || !member_rating)))
+    return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  return party_read(e, party_cap, member_cap, size, seq, enq_ts, mode, group, rating, member_ids, member_rating,
+                    n_parties, n_members);
 }
 
 int mm_remove_packed(mm_engine* e, uint32_t n, const uint32_t* handle, uint32_t* n_removed) {
@@ -3153,6 +3548,7 @@ int mm_export(mm_engine* e, void* buf, uint64_t cap, uint64_t* n_bytes) {
   if (!e || !n_bytes || (cap && !buf)) return MM_E_ARG;
   *n_bytes = 0;
   std::lock_guard<std::mutex> lk(e->mu);
+  if (e->pt.live) return parties_err(e);
   CK(cudaSetDevice(e->device));
   const int rc = export_image(e, buf, cap, n_bytes, nullptr);
   free_img_scratch(e);
@@ -3163,6 +3559,7 @@ int mm_export_queues(mm_engine* e, const uint8_t* queues, void* buf, uint64_t ca
   if (!e || !queues || !n_bytes || (cap && !buf)) return MM_E_ARG;
   *n_bytes = 0;
   std::lock_guard<std::mutex> lk(e->mu);
+  if (e->pt.live) return parties_err(e);
   CK(cudaSetDevice(e->device));
   const int rc = export_image(e, buf, cap, n_bytes, queues);
   free_img_scratch(e);
@@ -3173,6 +3570,7 @@ int mm_merge(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t cap, uint
   if (!e || !n_rejected || (n_bytes && !buf) || (cap && !rejected)) return MM_E_ARG;
   *n_rejected = 0;
   std::lock_guard<std::mutex> lk(e->mu);
+  if (e->pt.live) return parties_err(e);
   CK(cudaSetDevice(e->device));
   const int rc = merge_image(e, static_cast<const uint8_t*>(buf), n_bytes, cap, rejected, n_rejected);
   free_img_scratch(e);
@@ -3223,6 +3621,7 @@ int mm_import_regroup_many(mm_engine* e, uint32_t n_images, const void* const* b
 int mm_snapshot(mm_engine* e) {
   if (!e) return MM_E_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
+  if (e->pt.live) return parties_err(e);
   CK(cudaSetDevice(e->device));
   if (!e->snap.v.id) {
     int rc = alloc_pool(e, e->snap);
@@ -3258,6 +3657,7 @@ int mm_restore(mm_engine* e) {
   e->seq_next = e->snap_seq;
   e->gen = next_gen(e);
   e->fresh = false;
+  e->pt.n_rows = e->pt.n_mem = e->pt.live = 0;  // a snapshot never holds parties
   e->match_valid = false;  // the restored pool was not matched by the last tick
   if (e->use_active && p.n) {
     k_restamp<<<dim3(e->n_chunks, e->n_segs), 256, 0, e->stream>>>(p.v, p.m, act_view(e), e->gen, nullptr);

@@ -78,6 +78,7 @@ struct LocateArgs {
   bool arrival;              // MM_ORDER_ARRIVAL
   const uint8_t* mode_tsize; // [MM_MAX_MODES]
   const uint16_t* bin_key;   // [Kp] c - key_lo of the bin
+  PartyView pt;              // the party table (state 3)
   int32_t key_lo;
   uint32_t KR;
 };
@@ -125,6 +126,8 @@ __global__ void __launch_bounds__(256) k_locate(const LocateArgs a) {
       if (v < kPending && (uint32_t)(v >> 32) == a.gen && slot < a.n_slots && a.pool.id[slot] == pid &&
           a.pool.mode[slot] != MM_MODE_DEAD)
         state = 1;
+      else if (v < kPending && pt_queued(v))
+        state = 3;  // slot = the party's row
     }
   }
   state = __shfl_sync(0xFFFFFFFFu, state, 0);
@@ -132,6 +135,21 @@ __global__ void __launch_bounds__(256) k_locate(const LocateArgs a) {
   mm_player_status r{};
   r.lobby = MM_LOCATE_STAYS;
   r.member = 0xFFFFu;
+  if (state == 3) {  // queued in a party: the member's own rating, the party's queue, stamp, seq and wait
+    const uint32_t o = a.pt.off[slot], n = a.pt.size[slot];
+    for (uint32_t k = lane; k < n; k += 32)
+      if (a.pt.mid[o + k] == pid) r.rating = a.pt.mrat[o + k];
+    r.rating = __reduce_or_sync(0xFFFFFFFFu, (uint32_t)r.rating);  // one lane holds the id
+    r.state = 3;
+    r.mode = a.pt.mode[slot];
+    r.group = a.pt.grp[slot];
+    r.enq_ts = a.pt.ts[slot];
+    r.seq = a.pt.seq[slot];
+    const int32_t w = (int32_t)(a.now - r.enq_ts);
+    r.wait = w < 0 ? 0u : (uint32_t)w;
+    if (lane == 0) a.out[q] = r;
+    return;
+  }
   if (state != 1) {
     r.state = (uint8_t)state;
     if (lane == 0) a.out[q] = r;

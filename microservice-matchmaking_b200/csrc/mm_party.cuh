@@ -1,0 +1,412 @@
+// mm_party.cuh — parties on the device (mm_enqueue_party / mm_party_match, DESIGN §4): players who queue together are
+// matched into one lobby and one team.  Parties live in a table of their own beside the pool, which the tick never
+// reads.
+//
+// Table: one row per party in age order (= insertion order: every party of an accepted batch consumes one enqueue
+// sequence number, so rows and solos share the numbering of emit_seq), its members in a member array at the row's
+// offset.  A queued member's active-set value is kPtVal(row) (pool generation 0, which no pool ever has); a matched
+// member's is kPtMatched (a slot past every pool), which every call reads as a matched player.  Rows of matched,
+// dissolved and expired parties stay in place, `dead`, until the next compaction (k_pt_keep / k_pt_move: stable, by age).
+//
+// Enqueue: k_pt_claim claims every member id in the active set as k_enq_claim does (the lowest batch index wins);
+// k_pt_resolve gives every party its code 2 (invalid) or 0 (a member was queued before the call, or belongs to an
+// earlier party of the batch, accepted or not) from its own members alone; the candidates' member counts are scanned
+// (k_scan_small) and k_pt_commit cuts the last parties that do not fit (code 3) and writes the rows; k_pt_members
+// writes the member rows and active-set values, and frees every id whose first occurrence lost.
+//
+// Match: after compaction the rows are counting-sorted by (bin, age) — bins are the solo pool's, so a queue's parties
+// are the runs of its bins — and k_pt_plan serves one queue per warp.  The warp takes the queue's anchors in age
+// order, walks the bins outward from the anchor's bin in (distance, rating) order for co-parties (sequential: every
+// placement changes the rooms), then counts the solos of the open slots with wd_walk<false>.  Only a full lobby commits:
+// the same co-party walk again, then one wd_walk<true, walk order> per team with open slots, so the solos fill team 0,
+// then team 1, ... in their rank order.  The solo pieces go through k_bf_keys, the band pipeline and k_bf_out like
+// mm_widen's; k_wd_bases / k_wd_hdr write the headers and bases and k_pt_out copies the party members.
+#pragma once
+
+#include "mm_widen.cuh"
+
+namespace mm {
+
+static_assert(sizeof(mm_party_stats) == 32, "mm_party_stats is 32 bytes (include/mm_engine.h)");
+
+constexpr uint32_t kPtPlanWarps = 4;
+constexpr uint32_t kPtMaxTeams = 256;
+constexpr uint32_t kPtNone = 0xFFFFFFFFu;
+
+// the counters of one party call (zeroed by the host)
+enum PtCtr : uint32_t { kPtAccepted = 0, kPtReleased, kPtRows, kPtMembers, kPtGone, kPtAnchors, kPtPlaced, kPtWords };
+
+// ---- enqueue ----------------------------------------------------------------------------------------------------------
+struct PtEnqArgs {
+  uint32_t n, m;                 // parties, members
+  const uint8_t* size;           // [n]
+  const uint32_t* moff;          // [n] first member of the party in the batch
+  const uint32_t* mparty;        // [m] member -> party
+  const uint64_t* id;            // [m]
+  const int32_t* rating;         // [m]
+  const uint8_t* mode;           // [n]
+  const uint32_t* ts;            // [n] or null
+  ActiveView act;
+  BinMap bm;
+  const uint8_t* grp_lut;
+  const uint8_t* mode_tsize;
+  uint32_t n_modes;
+  uint64_t* hslot;               // [m] active-set slot of the member's id (~0: invalid id)
+  uint8_t* pre;                  // [m] 1: the id was committed before the call
+  uint8_t* code;                 // [n]
+  uint32_t* msz;                 // [n] candidates' member counts -> exclusive scan
+  uint32_t* one;                 // [n] candidates: 1 -> exclusive scan
+  uint32_t* tot;                 // [2] scan totals (zeroed)
+  uint32_t room;                 // members the table still holds
+  uint32_t rows0, mem0, seq0;    // first free row and member entry, seq of party 0
+  PartyView pt;
+  uint32_t* ctr;
+};
+
+__global__ void k_pt_claim(const PtEnqArgs a) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= a.m) return;
+  const uint64_t pid = a.id[j];
+  const uint32_t p = a.mparty[j];
+  a.pre[j] = 0;
+  a.hslot[j] = ~0ull;
+  if (a.act.dcap ? pid >= a.act.dcap : pid >= kTombKey) return;
+  if (a.act.dcap) {
+    a.pre[j] = atomicMin(a.act.val(pid), kPending | p) < kPending;
+    a.hslot[j] = pid;
+    return;
+  }
+  uint64_t h = hash64(pid) & a.act.mask;
+  for (uint64_t probe = 0; probe <= a.act.mask; ++probe) {
+    unsigned long long k = *a.act.key(h);
+    if (k == kEmptyKey) {
+      k = atomicCAS(a.act.key(h), kEmptyKey, pid);
+      if (k == kEmptyKey) k = pid;
+    }
+    if (k == pid) {
+      a.pre[j] = atomicMin(a.act.val(h), kPending | p) < kPending;
+      a.hslot[j] = h;
+      return;
+    }
+    h = (h + 1) & a.act.mask;
+  }
+}
+
+// One thread per party: 2 (invalid) before 0 (a member taken before the call or by an earlier party) before 1.
+__global__ void k_pt_resolve(const PtEnqArgs a) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= a.n) return;
+  const uint32_t s = a.size[p], o = a.moff[p], md = a.mode[p];
+  bool bad = md >= a.n_modes || s < 2 || s > a.mode_tsize[md < a.n_modes ? md : 0], taken = false;
+  long long sum = 0;
+  for (uint32_t k = 0; k < s; ++k) {
+    const uint64_t h = a.hslot[o + k];
+    sum += a.rating[o + k];
+    if (h == ~0ull) { bad = true; continue; }
+    for (uint32_t k2 = 0; k2 < k; ++k2) bad |= a.id[o + k2] == a.id[o + k];
+    taken |= a.pre[o + k] || *a.act.val(h) != (kPending | p);
+  }
+  long long R = 0;
+  if (s) {
+    R = sum / (long long)s;
+    if (R * (long long)s > sum) --R;  // floor toward minus infinity
+  }
+  const int32_t Rc = R < INT32_MIN ? INT32_MIN : (R > INT32_MAX ? INT32_MAX : (int32_t)R);
+  if (!bad && a.grp_lut[clamp_key(a.bm.key_lo, a.bm.KR, Rc)] == 0xFF) bad = true;
+  const uint8_t c = bad ? 2 : (taken ? 0 : 1);
+  a.code[p] = c;
+  a.msz[p] = c == 1 ? s : 0u;
+  a.one[p] = c == 1;
+}
+
+// One thread per party after the scans: the cut, then the accepted rows.
+__global__ void k_pt_commit(const PtEnqArgs a) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= a.n || a.code[p] != 1) return;
+  const uint32_t s = a.size[p], o = a.moff[p];
+  if (a.msz[p] + s > a.room) { a.code[p] = 3; return; }
+  const uint32_t row = a.rows0 + a.one[p], md = a.mode[p];
+  long long sum = 0;
+  for (uint32_t k = 0; k < s; ++k) sum += a.rating[o + k];
+  long long R = sum / (long long)s;
+  if (R * (long long)s > sum) --R;
+  const int32_t Rc = (int32_t)R;  // the mean of 32-bit ratings
+  a.pt.seq[row] = a.seq0 + p;
+  a.pt.ts[row] = a.ts ? a.ts[p] : 0u;
+  a.pt.off[row] = a.mem0 + a.msz[p];
+  a.pt.R[row] = Rc;
+  a.pt.bin[row] = (uint16_t)bin_of(a.bm, a.bm.lut, Rc, md);
+  a.pt.mode[row] = (uint8_t)md;
+  a.pt.grp[row] = a.grp_lut[clamp_key(a.bm.key_lo, a.bm.KR, Rc)];
+  a.pt.size[row] = (uint8_t)s;
+  a.pt.dead[row] = 0;
+  atomicAdd(&a.ctr[kPtAccepted], s);
+}
+
+// One thread per member: accepted parties' member rows and active-set values; ids whose first occurrence lost are freed.
+__global__ void k_pt_members(const PtEnqArgs a) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= a.m) return;
+  const uint64_t h = a.hslot[j];
+  if (h == ~0ull || a.pre[j]) return;
+  const uint32_t p = a.mparty[j];
+  if (*a.act.val(h) != (kPending | p)) return;  // an earlier party holds the id
+  if (a.code[p] == 1) {
+    const uint32_t m = a.mem0 + a.msz[p] + (j - a.moff[p]);
+    a.pt.mid[m] = a.id[j];
+    a.pt.mrat[m] = a.rating[j];
+    *a.act.val(h) = kPtVal(a.rows0 + a.one[p]);
+    return;
+  }
+  if (atomicExch(a.act.val(h), kFreeVal) != kFreeVal) {  // a repeat inside the party frees it once
+    if (!a.act.dcap) *a.act.key(h) = kTombKey;
+    atomicAdd(&a.ctr[kPtReleased], 1u);
+  }
+}
+
+// ---- compaction -------------------------------------------------------------------------------------------------------
+__global__ void k_pt_keep(uint32_t n_rows, PartyView t, uint32_t* __restrict__ keep, uint32_t* __restrict__ msz) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rows) return;
+  const bool k = t.dead[r] == 0;
+  keep[r] = k;
+  msz[r] = k ? t.size[r] : 0u;
+}
+
+// rows kept -> their place in `d` (keep / msz hold the exclusive scans); the members' active-set values follow the row
+__global__ void k_pt_move(uint32_t n_rows, PartyView s, PartyView d, const uint32_t* __restrict__ keep,
+                          const uint32_t* __restrict__ msz, ActiveView act) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rows || s.dead[r]) return;
+  const uint32_t q = keep[r], o = msz[r], so = s.off[r], n = s.size[r];
+  d.seq[q] = s.seq[r]; d.ts[q] = s.ts[r]; d.off[q] = o; d.R[q] = s.R[r]; d.bin[q] = s.bin[r];
+  d.mode[q] = s.mode[r]; d.grp[q] = s.grp[r]; d.size[q] = (uint8_t)n; d.dead[q] = 0;
+  for (uint32_t k = 0; k < n; ++k) {
+    const uint64_t pid = s.mid[so + k];
+    d.mid[o + k] = pid;
+    d.mrat[o + k] = s.mrat[so + k];
+    const uint64_t h = act_find(act, pid);
+    if (h != ~0ull) *act.val(h) = kPtVal(q);
+  }
+}
+
+// ---- remove and expire ------------------------------------------------------------------------------------------------
+// mm_remove, before k_remove: every party with a removed member is marked for dissolution.
+__global__ void k_pt_mark(uint32_t n, const uint64_t* __restrict__ id, ActiveView act, PartyView t) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || !act.on()) return;
+  const uint64_t h = act_find(act, id[i]);
+  if (h == ~0ull) return;
+  const uint64_t v = *act.val(h);
+  if (v != kFreeVal && pt_queued(v)) t.dead[(uint32_t)v] = 2;
+}
+
+// A party member's entry leaves the set if it still is the row's.  -> 1 if it did.
+__device__ __forceinline__ uint32_t pt_free(ActiveView act, uint64_t pid, uint32_t row) {
+  const uint64_t h = act_find(act, pid);
+  if (h == ~0ull) return 0;
+  if (act.dcap) return atomicCAS(act.val(h), kPtVal(row), kFreeVal) == kPtVal(row);
+  if (*act.val(h) != kPtVal(row) || atomicCAS(act.key(h), (unsigned long long)pid, kTombKey) != pid) return 0;
+  *act.val(h) = kFreeVal;
+  return 1;
+}
+
+// after k_remove: the other members of every marked party leave (counted with the removed ones), the row is gone
+__global__ void k_pt_dissolve(uint32_t n_rows, PartyView t, ActiveView act, uint32_t* __restrict__ n_removed,
+                              uint32_t* __restrict__ ctr) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rows || t.dead[r] != 2) return;
+  uint32_t freed = 0;
+  for (uint32_t k = 0; k < t.size[r]; ++k) freed += pt_free(act, t.mid[t.off[r] + k], r);
+  t.dead[r] = 1;
+  if (freed) atomicAdd(n_removed, freed);
+  atomicAdd(&ctr[kPtGone], t.size[r]);
+}
+
+// mm_expire: whole parties whose WAIT >= max_wait, after k_expire on the same counters (ctr[0] the output cursor,
+// ctr[1] the entries erased).  Without `commit` only ctr[0] counts.
+__global__ void k_pt_expire(uint32_t n_rows, PartyView t, uint32_t now, uint32_t max_wait, uint32_t commit,
+                            ActiveView act, uint64_t* __restrict__ out_id, uint32_t* __restrict__ out_handle,
+                            uint32_t* __restrict__ out_seq, uint32_t* __restrict__ ctr, uint32_t* __restrict__ pctr) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rows || t.dead[r] || stat_wait(now, t.ts[r]) < max_wait) return;
+  const uint32_t n = t.size[r];
+  const uint32_t q = atomicAdd(&ctr[0], n);
+  if (!commit) return;
+  uint32_t erased = 0;
+  for (uint32_t k = 0; k < n; ++k) {
+    const uint64_t pid = t.mid[t.off[r] + k];
+    if (out_id) out_id[q + k] = pid;
+    else if (out_handle) out_handle[q + k] = (uint32_t)pid;
+    if (out_seq) out_seq[q + k] = t.seq[r];
+    erased += pt_free(act, pid, r);
+  }
+  t.dead[r] = 1;
+  if (erased) atomicAdd(&ctr[1], erased);
+  atomicAdd(&pctr[kPtGone], n);
+}
+
+// ---- match ------------------------------------------------------------------------------------------------------------
+struct PtArgs {
+  PartyView t;
+  uint32_t n_rows;
+  const uint32_t* pb;      // [K + 1] first sorted party of the bin (exclusive scan of the bin counts)
+  uint32_t* pcur;          // [K] scatter cursors, then the plan's first party of the bin not known to be placed
+  uint32_t* sorted;        // [n_rows] rows by (bin, age)
+  uint32_t* lob;           // [n_rows] lobby record of a placed party, kPtNone
+  uint32_t* pos;           // [n_rows] member offset of a placed party inside its lobby
+  const uint8_t* mode_tsize;  // [MM_MAX_MODES]
+  uint64_t* members;       // lobby members (k_pt_out)
+  uint32_t* ctr;           // [kPtWords]
+};
+
+__global__ void k_pt_count(const PtArgs p, uint32_t* __restrict__ cnt) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= p.n_rows) return;
+  p.lob[r] = kPtNone;
+  atomicAdd(&cnt[p.t.bin[r]], 1u);
+}
+// Stable scatter by bin (row order is age order), one CTA over tiles of 1024 rows in order.  Inside a tile, a row's
+// place is the bin's cursor + its bin's rows in the warps before it (the warps' run tables in shared memory) + its
+// rank among its warp's peers (__match_any_sync); the first warp holding a bin then advances the bin's cursor.
+constexpr uint32_t kPtScatterBlock = 1024;
+__global__ void __launch_bounds__(kPtScatterBlock) k_pt_scatter(const PtArgs p) {
+  constexpr uint32_t W = kPtScatterBlock / 32;
+  __shared__ uint32_t s_bin[W][32], s_cnt[W][32];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (uint32_t r0 = 0; r0 < p.n_rows; r0 += kPtScatterBlock) {
+    const uint32_t r = r0 + threadIdx.x;
+    const uint32_t b = r < p.n_rows ? p.t.bin[r] : 0xFFFFFFFFu;
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, b);
+    const bool lead = (__ffs(peers) - 1) == lane;
+    s_bin[warp][lane] = lead ? b : 0xFFFFFFFFu;
+    s_cnt[warp][lane] = __popc(peers);
+    __syncthreads();
+    uint32_t before = 0, after = 0, base = 0;
+    if (lead && b != 0xFFFFFFFFu) {
+      for (uint32_t w = 0; w < W; ++w) {
+        if (w == warp) continue;
+        for (uint32_t l = 0; l < 32; ++l)
+          if (s_bin[w][l] == b) { (w < warp ? before : after) += s_cnt[w][l]; break; }
+      }
+      base = p.pcur[b];
+    }
+    __syncthreads();  // every cursor is read before the first warp of a bin advances it
+    if (lead && b != 0xFFFFFFFFu && before == 0) p.pcur[b] = base + __popc(peers) + after;
+    const uint32_t at = __shfl_sync(0xFFFFFFFFu, base + before, __ffs(peers) - 1);
+    if (b != 0xFFFFFFFFu) p.sorted[at + __popc(peers & ((1u << lane) - 1u))] = r;
+    __syncthreads();
+  }
+}
+
+// The co-party walk of anchor row `ar` (bin pos of the queue's bins [lo, hi), window win): every unplaced party of the
+// window in (distance, rating, age) order goes to the lowest team with room for it.  room[] holds the teams' free
+// slots on entry (the anchor's taken).  commit: the placed parties get lobby record r and their member offsets.
+// Uniform over the warp; lane 0 writes.  -> the free slots left.
+__device__ uint32_t pt_walk(const PtArgs& p, const WdArgs& a, uint32_t ar, uint32_t pos, uint32_t lo, uint32_t hi,
+                            uint32_t win, uint16_t* room, uint32_t T, uint32_t S, uint32_t open, bool commit, uint32_t r,
+                            uint32_t& n_placed) {
+  const uint32_t lane = threadIdx.x & 31;
+  const int32_t target = (int32_t)a.bin_key[pos];
+  uint32_t l = pos, h = pos;  // next bins: l - 1 below, h at or above
+  while (open >= 2) {
+    uint32_t d_l = kBfFar, d_h = kBfFar;
+    if (l > lo) { const uint32_t d = (uint32_t)(target - (int32_t)a.bin_key[l - 1]); if (d <= win) d_l = d; }
+    if (h < hi) { const uint32_t d = (uint32_t)((int32_t)a.bin_key[h] - target); if (d <= win) d_h = d; }
+    if (d_l == kBfFar && d_h == kBfFar) break;
+    const uint32_t b = d_l <= d_h ? --l : h++;  // a lower bin first at equal distance
+    uint32_t i = p.pcur[b];
+    while (i < p.pb[b + 1] && p.lob[p.sorted[i]] != kPtNone) ++i;  // the bin's placed prefix is skipped for good
+    __syncwarp();
+    if (lane == 0) p.pcur[b] = i;
+    __syncwarp();
+    for (; i < p.pb[b + 1] && open >= 2; ++i) {
+      const uint32_t x = p.sorted[i];
+      if (x == ar || p.lob[x] != kPtNone) continue;
+      const uint32_t s = p.t.size[x];
+      uint32_t t = 0;
+      while (t < T && room[t] < s) ++t;
+      if (t == T) continue;
+      if (commit && lane == 0) { p.lob[x] = r; p.pos[x] = t * S + (S - room[t]); }
+      __syncwarp();
+      if (lane == 0) room[t] = (uint16_t)(room[t] - s);
+      __syncwarp();
+      open -= s;
+      ++n_placed;
+    }
+  }
+  return open;
+}
+
+__global__ void __launch_bounds__(kPtPlanWarps * 32) k_pt_plan(const PtArgs p, const WdArgs a) {
+  __shared__ uint32_t s_bin[kPtPlanWarps][32];
+  __shared__ uint16_t s_room[kPtPlanWarps][kPtMaxTeams];
+  const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, c = blockIdx.x * kPtPlanWarps + warp;
+  if (c >= a.n_cut) return;
+  const WdRule u = a.rule[c];
+  if (u.min_wait == MM_WIDEN_OFF) return;
+  const uint32_t lo = a.seg_bin_lo[a.cut_lp_lo[c]], hi = a.seg_bin_lo[a.cut_lp_lo[c + 1]];
+  const uint32_t S = p.mode_tsize[c / a.n_groups], T = u.L / S;  // the host refuses T > kPtMaxTeams
+  uint16_t* room = s_room[warp];
+  uint32_t n_lob = 0, n_anc = 0, n_abs = 0, n_placed = 0;
+  if (p.pb[hi] == p.pb[lo]) { if (lane == 0) a.qlob[c] = 0; return; }
+  for (uint32_t r0 = 0; r0 < p.n_rows; r0 += 32) {  // the anchors: the queue's parties that waited long enough, by age
+    const uint32_t x = r0 + lane;
+    const bool is_a = x < p.n_rows && p.t.bin[x] >= lo && p.t.bin[x] < hi && stat_wait(a.now, p.t.ts[x]) >= u.min_wait;
+    uint32_t bal = __ballot_sync(0xFFFFFFFFu, is_a);
+    while (bal) {
+      const uint32_t ar = r0 + __ffs(bal) - 1;
+      bal &= bal - 1;
+      ++n_anc;
+      if (p.lob[ar] != kPtNone) { ++n_abs; continue; }  // an earlier lobby of the call placed it
+      const uint32_t wait = stat_wait(a.now, p.t.ts[ar]);
+      const long long w = min((long long)u.w_max, (long long)u.w0 + (long long)((wait - u.min_wait) / u.step) * u.inc);
+      const uint32_t win = (uint32_t)min(w, (long long)kBfFar - 1), pos = p.t.bin[ar], sa = p.t.size[ar];
+      for (uint32_t t = lane; t < T; t += 32) room[t] = (uint16_t)(t == 0 ? S - sa : S);
+      __syncwarp();
+      uint32_t np = 0;
+      const uint32_t open = pt_walk(p, a, ar, pos, lo, hi, win, room, T, S, u.L - sa, false, 0, np);
+      uint32_t left = 0;
+      if (open && wd_walk<false>(a, s_bin[warp], pos, lo, hi, win, open, left, 0) < open) continue;  // all or nothing
+      uint32_t r = 0;
+      if (lane == 0) r = atomicAdd(&a.ctr[kWdLobbies], 1u);
+      r = __shfl_sync(0xFFFFFFFFu, r, 0);
+      if (lane == 0) { a.rec[r] = make_uint2(c, n_lob); p.lob[ar] = r; p.pos[ar] = 0; }
+      ++n_lob;
+      for (uint32_t t = lane; t < T; t += 32) room[t] = (uint16_t)(t == 0 ? S - sa : S);
+      __syncwarp();
+      pt_walk(p, a, ar, pos, lo, hi, win, room, T, S, u.L - sa, true, r, n_placed);
+      ++n_placed;
+      for (uint32_t t = 0; t < T; ++t) {  // the solos fill the open slots team by team, in their rank order
+        const uint32_t need = room[t];
+        if (!need) continue;
+        left = t * S + (S - need);
+        wd_walk<true, true>(a, s_bin[warp], pos, lo, hi, win, need, left, r);
+      }
+      __syncwarp();
+    }
+  }
+  if (lane == 0) {
+    a.qlob[c] = n_lob;
+    atomicAdd(&p.ctr[kPtAnchors], n_anc);
+    atomicAdd(&p.ctr[kPtPlaced], n_placed);
+    if (n_abs) atomicAdd(&a.ctr[kWdAbsorbed], n_abs);
+  }
+}
+
+// One thread per row: a placed party's members into its lobby; they become matched players and the row is gone.
+__global__ void k_pt_out(const PtArgs p, const uint32_t* __restrict__ mbase, ActiveView act) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= p.n_rows || p.lob[r] == kPtNone) return;
+  uint64_t* dst = p.members + mbase[p.lob[r]] + p.pos[r];
+  const uint32_t o = p.t.off[r];
+  for (uint32_t k = 0; k < p.t.size[r]; ++k) {
+    const uint64_t pid = p.t.mid[o + k];
+    dst[k] = pid;
+    const uint64_t h = act_find(act, pid);
+    if (h != ~0ull) *act.val(h) = kPtMatched;
+  }
+  p.t.dead[r] = 1;
+}
+
+}  // namespace mm

@@ -78,7 +78,8 @@ __global__ void __launch_bounds__(256) k_rq_check(const RqCheckArgs a) {
       const unsigned long long v = h == ~0ull ? kFreeVal : *a.act.val(h);
       if (v < kPending) {
         const uint32_t slot = (uint32_t)v;
-        const bool live = (uint32_t)(v >> 32) == a.gen && slot < a.n_slots && a.pool_mode[slot] != MM_MODE_DEAD;
+        const bool live = ((uint32_t)(v >> 32) == a.gen && slot < a.n_slots && a.pool_mode[slot] != MM_MODE_DEAD) ||
+                          pt_queued(v);  // queued in a party
         c = live ? 0 : 1;
       }
     }

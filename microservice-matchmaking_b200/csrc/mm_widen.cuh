@@ -151,8 +151,9 @@ __global__ void __launch_bounds__(256) k_wd_rank(const WdArgs a) {
 
 // The outward walk of k_bf_plan from bin pos of the queue [lo, hi) within distance win: the first `need` players in
 // (distance, rating, enqueue order).  Returns how many it found (at most need) and, in left, how many of them lie below
-// pos.  kTake: the players are taken (rem) and written as pieces of lobby record r, whose left players come first.
-template <bool kTake>
+// pos.  kTake: the players are taken (rem) and written as pieces of lobby record r, whose left players come first;
+// kWalkOrder (mm_party_match): the pieces are written in walk order instead, from offset `left` of the lobby.
+template <bool kTake, bool kWalkOrder = false>
 __device__ __forceinline__ uint32_t wd_walk(const WdArgs& a, uint32_t* s_bin, uint32_t pos, uint32_t lo, uint32_t hi,
                                             uint32_t win, uint32_t need, uint32_t& left, uint32_t r) {
   const uint32_t lane = threadIdx.x & 31;
@@ -186,7 +187,8 @@ __device__ __forceinline__ uint32_t wd_walk(const WdArgs& a, uint32_t* s_bin, ui
       const uint32_t at = warp_append(&a.ctr[kBfPieces], take != 0);
       if (take) {
         // member order: the left bins in ascending rating (reverse walk order), then the right bins in walk order
-        const uint32_t poff = is_l ? left_all - (got_l + il_incl) : left_all + got_r + ir_incl - tr;
+        const uint32_t poff = kWalkOrder ? left_all + got + before
+                                         : (is_l ? left_all - (got_l + il_incl) : left_all + got_r + ir_incl - tr);
         a.piece[at] = BfPiece{r, bin, a.tot[bin] - v, take, poff};
         a.rem[bin] = v - take;
       }

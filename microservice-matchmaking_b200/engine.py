@@ -441,6 +441,64 @@ class Engine:
             self._check(rc, "mm_widen")
             return lob[:st.n_lobbies], mem[:st.n_matched], st
 
+    # -- parties (mm_enqueue_party / mm_party_match / mm_party_read) ---------------------------------------------
+    def enqueue_party(self, sizes, ids, rating, mode, enq_ts=None):
+        """Queue parties: party j's members are the next sizes[j] entries of ids / rating.  -> codes u8[n_parties]:
+        1 queued, 0 a member already queued (or in an earlier party of the batch), 2 invalid, 3 the table is full."""
+        sizes = np.ascontiguousarray(sizes, np.uint8)
+        ids = np.ascontiguousarray(ids, np.uint64)
+        rating = np.ascontiguousarray(rating, np.int32)
+        mode = np.ascontiguousarray(mode, np.uint8)
+        n = len(sizes)
+        assert len(mode) == n and len(ids) == len(rating) == int(sizes.sum(dtype=np.int64))
+        if enq_ts is not None:
+            enq_ts = np.ascontiguousarray(enq_ts, np.uint32)
+            assert len(enq_ts) == n
+        acc = np.empty(max(n, 1), np.uint8)
+        self._check(self.lib.mm_enqueue_party(self.h, n, _p(sizes), _p(ids), _p(rating), _p(mode), _p(enq_ts), _p(acc)),
+                    "mm_enqueue_party")
+        return acc[:n]
+
+    def party_match(self, now, rules, lobby_cap=1 << 10, member_cap=1 << 12):
+        """Form lobbies around the queued parties that waited at least their queue's min_wait (mm_party_match).
+        rules as widen() takes them.  -> (lobbies[LOBBY_DTYPE], member_ids u64, PartyStats).  An MM_E_CAP refusal is
+        retried once with its counts."""
+        if isinstance(rules, dict):
+            rules = self.widen_rules(rules)
+        rules = np.ascontiguousarray(rules, self.WIDEN_RULE_DTYPE)
+        for attempt in range(2):
+            lob = np.empty(max(lobby_cap, 1), LOBBY_DTYPE)
+            mem = np.empty(max(member_cap, 1), np.uint64)
+            st = abi.PartyStats()
+            rc = self.lib.mm_party_match(self.h, int(now), _p(rules), _p(lob), lobby_cap, _p(mem), member_cap,
+                                         C.byref(st))
+            if rc == abi.MM_E_CAP and attempt == 0:
+                lobby_cap, member_cap = max(lobby_cap, st.n_lobbies), max(member_cap, st.n_matched)
+                continue
+            self._check(rc, "mm_party_match")
+            return lob[:st.n_lobbies], mem[:st.n_matched], st
+
+    def party_read(self):
+        """The queued parties in age order (mm_party_read) -> dict of per-party columns size, seq, enq_ts, mode, group,
+        rating (R) and `members`, a list of (ids u64, ratings i32) per party."""
+        pc, mc = 1 << 10, 1 << 12
+        while True:
+            cols = dict(size=np.empty(pc, np.uint8), seq=np.empty(pc, np.uint32), enq_ts=np.empty(pc, np.uint32),
+                        mode=np.empty(pc, np.uint8), group=np.empty(pc, np.uint8), rating=np.empty(pc, np.int32))
+            mid, mrt = np.empty(mc, np.uint64), np.empty(mc, np.int32)
+            np_, nm = C.c_uint32(0), C.c_uint32(0)
+            rc = self.lib.mm_party_read(self.h, pc, mc, *(_p(cols[k]) for k in ("size", "seq", "enq_ts", "mode", "group",
+                                                                                 "rating")),
+                                        _p(mid), _p(mrt), C.byref(np_), C.byref(nm))
+            if rc == abi.MM_E_CAP and (np_.value > pc or nm.value > mc):
+                pc, mc = max(pc, np_.value), max(mc, nm.value)
+                continue
+            self._check(rc, "mm_party_read")
+            out = {k: v[:np_.value] for k, v in cols.items()}
+            cut = np.cumsum(out["size"].astype(np.int64))[:-1]
+            out["members"] = list(zip(np.split(mid[:nm.value], cut), np.split(mrt[:nm.value], cut))) if np_.value else []
+            return out
+
     def in_queue(self, ids):
         ids = np.ascontiguousarray(ids, np.uint64)
         out = np.empty(len(ids), np.uint8)
@@ -590,12 +648,17 @@ class Engine:
 
     def _expire(self, fn, dtype, now, max_wait, want_seq, what):
         cap = self.pool_size()  # every resident player fits: the engine makes a single pass
-        ids = np.empty(max(cap, 1), dtype)
-        seq = np.empty(max(cap, 1), np.uint32) if want_seq else None
-        n = C.c_uint32(0)
         max_wait = max(0, min(int(max_wait), 0xFFFFFFFF))
-        self._check(fn(self.h, int(now) & 0xFFFFFFFFFFFFFFFF, max_wait, _p(ids), _p(seq), cap, C.byref(n)), what)
-        return ids[:n.value], (seq[:n.value] if seq is not None else None)
+        for attempt in range(2):  # queued party members may not fit: a refusal counts them and changes nothing
+            ids = np.empty(max(cap, 1), dtype)
+            seq = np.empty(max(cap, 1), np.uint32) if want_seq else None
+            n = C.c_uint32(0)
+            rc = fn(self.h, int(now) & 0xFFFFFFFFFFFFFFFF, max_wait, _p(ids), _p(seq), cap, C.byref(n))
+            if rc == abi.MM_E_CAP and attempt == 0:
+                cap = n.value
+                continue
+            self._check(rc, what)
+            return ids[:n.value], (seq[:n.value] if seq is not None else None)
 
     def export_state(self):
         """Host image of the queue state (mm_export) -> uint8 array; the engine is not changed.  Layout:

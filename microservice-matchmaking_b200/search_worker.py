@@ -173,6 +173,13 @@ class SearchPool:
     those modes, from the tick and from widen, is split into the two teams with the least rating difference
     (mm_set_option("team_balance")).  Membership and lobby order are unchanged; team t is still members
     [t * team_size, (t + 1) * team_size).  resume() sets it again on the new engine.
+    parties / party_capacity: optional parties (extension; needs MM_ORDER_RATING): players who queue together, staged
+    with stage_party() and acked or nacked as one delivery, are matched into one lobby and one team.  party_capacity
+    sets how many party members the engine holds (mm_set_option("party_capacity")); parties = {mode name: (min_wait_ms,
+    w0, step_ms, inc, w_max)} is the party window of the mode, as widen takes it.  Every tick runs Engine.party_match
+    before the tick itself, so parties get the first pick of the solos; its lobbies are published like the tick's and
+    stats["party_lobbies"] counts them.  A party member removed with remove_user() takes its whole party out; a matched
+    member's requeue() answers "gone" (the caller enqueues the party again).
 
     Every ingest batch is stamped with now_ms(), the clock in milliseconds since the pool was created (u32, wraps
     after 49 days), and every tick passes the same clock as its `now`: the engine's per-queue waits
@@ -181,13 +188,21 @@ class SearchPool:
 
     def __init__(self, engine, mode_names, group_names, max_batch=65536, window=None, clock=None, flush_every_s=0.005,
                  handle_capacity=None, timeout_ms=None, wall_clock=None, lobby_budget=None, widen=None,
-                 balance_teams=None):
+                 balance_teams=None, parties=None, party_capacity=None):
         import time
         if widen and engine.cfg.order_mode != abi.MM_ORDER_RATING:
             raise ValueError("widen needs an MM_ORDER_RATING engine: windows are rating distances")
+        if (parties or party_capacity) and engine.cfg.order_mode != abi.MM_ORDER_RATING:
+            raise ValueError("parties need an MM_ORDER_RATING engine: party windows are rating distances")
         self.window = window
         self.widen = {(i, g): tuple(int(x) for x in widen[m]) for i, m in enumerate(mode_names) if m in (widen or {})
                       for g in range(len(group_names))}
+        self.party_rules = {(i, g): tuple(int(x) for x in parties[m]) for i, m in enumerate(mode_names)
+                            if m in (parties or {}) for g in range(len(group_names))}
+        if party_capacity:
+            engine.set_option("party_capacity", int(party_capacity))
+        self.party_of = {}  # handle -> the handles of its queued party (remove_user takes the whole party out)
+        self._staged_parties = []  # (worker, tag, [player documents], game mode)
         self.timeout_ms = timeout_ms
         self.lobby_budget = lobby_budget
         self.paused = set()  # queues (mode * n_groups + group) that emit nothing until resume_queues()
@@ -222,6 +237,8 @@ class SearchPool:
             self.stats["timed_out"] = 0
         if self.widen:
             self.stats["widened"] = 0
+        if self.party_rules or party_capacity:
+            self.stats["party_lobbies"] = 0
 
     def now_ms(self):
         """The pool's clock: milliseconds since the pool was created, modulo 2^32 (the engine's enq_ts / now)."""
@@ -236,12 +253,14 @@ class SearchPool:
         self.flush()
         h = self.handles.lookup(player_id)
         if h is not None:
-            self.engine.remove([h])
-            self.handles.release(player_id)
-            self.players.pop(h, None)
-            self.enqueued_at.pop(h, None)
-            self.matched_at.pop(h, None)
-            self.queued.pop(h, None)
+            self.engine.remove([h])  # a queued party member: the engine removes its whole party
+            for x in self.party_of.pop(h, (h,)):
+                self.party_of.pop(x, None)
+                self.handles.release(self.handles.id_of[x])
+                self.players.pop(x, None)
+                self.enqueued_at.pop(x, None)
+                self.matched_at.pop(x, None)
+                self.queued.pop(x, None)
         return ("ok", "removed")
 
     def requeue(self, players):
@@ -371,12 +390,99 @@ class SearchPool:
         if len(self._staged) >= self.max_batch or self.clock() - self._staged_since >= self.flush_every_s:
             self.flush()
 
-    def flush(self):
-        """mm_enqueue the staged deliveries; ack each one once its player is resident.  Never raises: a batch the
-        engine refuses (active set full, CUDA error) is nacked as a whole — the broker redelivers it."""
-        staged, self._staged = self._staged, []
+    def stage_party(self, worker, tag, players, game_mode):
+        """One delivery that queues several players together: players = their documents (each with "id" and
+        "rating").  Ingested at the next flush, after the staged solos; acked once the party is queued (or a member was
+        already queued), nacked if it is invalid or the party table is full."""
+        if not self._staged and not self._staged_parties:
+            self._staged_since = self.clock()
+        self._staged_parties.append((worker, tag, list(players), game_mode))
+        if len(self._staged) + len(self._staged_parties) >= self.max_batch or \
+                self.clock() - self._staged_since >= self.flush_every_s:
+            self.flush()
+
+    def _flush_parties(self):
+        """mm_enqueue_party the staged parties; ack or nack each party's delivery by its code."""
+        staged, self._staged_parties = self._staged_parties, []
         if not staged:
             return 0
+        fresh, ids, rating, sizes, mode = [], [], [], [], []
+        for (_w, _t, players, game_mode) in staged:
+            sizes.append(len(players))
+            mode.append(self.mode_index.get(game_mode, 255) if isinstance(game_mode, str) else 255)
+            for doc in players:
+                h, is_new = self.handles.acquire(doc["id"])
+                if h is None:
+                    h = 2 ** 64 - 1
+                elif is_new:
+                    fresh.append(doc["id"])
+                ids.append(h)
+                rating.append(int(doc["rating"]))
+        sizes = np.minimum(np.array(sizes, np.int64), 255).astype(np.uint8)  # a longer list is invalid (code 2)
+        ids = np.array(ids, np.uint64)
+        rating = np.clip(np.array(rating, np.int64), -(2 ** 31), 2 ** 31 - 1).astype(np.int32)
+        try:
+            if np.any(sizes.astype(np.int64) != [len(s[2]) for s in staged]):
+                raise ValueError("a party of more than 255 players")
+            codes = self.engine.enqueue_party(sizes, ids, rating, np.array(mode, np.uint8),
+                                              np.full(len(staged), self.now_ms(), np.uint32))
+        except Exception:  # nothing was enqueued
+            for pid in fresh:
+                self.handles.release(pid)
+            for (worker, tag, _p, _m) in staged:
+                worker.nack(worker.channel_name, tag)
+            self.stats["failed_batches"] += 1
+            return 0
+        fresh, off = set(fresh), 0
+        for code, (worker, tag, players, _m) in zip(codes.tolist(), staged):
+            hs = ids[off:off + len(players)].tolist()
+            off += len(players)
+            if code == 1:
+                for h, doc in zip(hs, players):
+                    self.players[h] = doc
+                    self.party_of[h] = tuple(hs)
+                self.stats["enqueued"] += len(players)
+                worker.ack(worker.channel_name, tag)
+            elif code == 0:  # a member is already queued
+                self.stats["duplicates"] += 1
+                worker.ack(worker.channel_name, tag)
+            else:  # invalid, or the party table is full
+                for h, doc in zip(hs, players):
+                    if doc["id"] in fresh and self.handles.lookup(doc["id"]) == h and h not in self.players:
+                        self.handles.release(doc["id"])
+                self.stats["invalid"] += 1
+                worker.nack(worker.channel_name, tag)
+        return len(staged)
+
+    def party_status(self, group_name):
+        """Queued parties of one rating group, per mode name (Engine.party_read): {"parties", "players"}."""
+        if group_name not in self.group_names or not hasattr(self.engine, "party_read"):
+            return {}
+        g = self.group_names.index(group_name)
+        pr = self.engine.party_read()
+        out = {}
+        for m, grp, size in zip(pr["mode"].tolist(), pr["group"].tolist(), pr["size"].tolist()):
+            if grp == g and m < len(self.mode_names):
+                d = out.setdefault(self.mode_names[m], {"parties": 0, "players": 0})
+                d["parties"] += 1
+                d["players"] += size
+        return out
+
+    def flush(self):
+        """mm_enqueue the staged deliveries; ack each one once its player is resident.  Never raises: a batch the
+        engine refuses (active set full, CUDA error) is nacked as a whole — the broker redelivers it.  Staged parties
+        follow (_flush_parties)."""
+        staged, self._staged = self._staged, []
+        if self._staged_parties and not staged:
+            return self._flush_parties()
+        if not staged:
+            return 0
+        try:
+            return self._flush_solos(staged)
+        finally:
+            self._flush_parties()
+
+    def _flush_solos(self, staged):
         fresh = []
         ids = np.empty(len(staged), np.uint64)
         for i, s in enumerate(staged):
@@ -434,10 +540,18 @@ class SearchPool:
             self.engine.set_option("max_spread", self.last_spread)
         if self.lobby_budget is not None:
             self._set_budget(self.lobby_budget())
+        n_lob = 0
+        if self.party_rules:  # before the tick: parties get the first pick of the solos
+            plob, pmem, _st = self.engine.party_match(now, self.party_rules)
+            for x in pmem.tolist():
+                self.party_of.pop(x, None)
+            self._publish(plob, pmem)
+            self.stats["party_lobbies"] += len(plob)
+            n_lob += len(plob)
         lob, mem, _seq, _st = self.engine.tick(now)
         self._publish(lob, mem)
         self.stats["lobbies"] += len(lob)
-        n_lob = len(lob)
+        n_lob += len(lob)
         if self.widen:  # before the timeout: a player who waited long gets its widest window before it is dropped
             wlob, wmem, _st = self.engine.widen(now, self.widen)
             self._publish(wlob, wmem)
@@ -504,6 +618,7 @@ class SearchPool:
     def _expire(self, now):
         expired, _seq = self.engine.expire(now, self.timeout_ms, want_seq=False)
         for h in expired.tolist():
+            self.party_of.pop(h, None)
             player = self.players.pop(h)
             self.enqueued_at.pop(h, None)
             self.queued.pop(h, None)
@@ -800,6 +915,8 @@ class SearchWorker:
             st["quality"] = self.pool.match_quality(self.group_name)
         if hasattr(self.pool.engine, "lobby_budget_report"):  # lobbies the last tick's budget held back, per mode
             st["held_back"] = self.pool.held_back(self.group_name)
+        if self.pool.party_rules and hasattr(self.pool.engine, "party_read"):  # this group's queued parties, per mode
+            st["parties"] = self.pool.party_status(self.group_name)
         return ("ok", st)
 
     def prepare_game_lobby(self, channel_name, exchange_forward, queue_forward, payload):  # worker.ex:250-261
@@ -819,6 +936,8 @@ class SearchWorker:
         if not isinstance(player_data, dict):                     # "[1, 2]" decodes, but is not a request
             return self.nack(channel_name, tag)
         game_mode = player_data.pop("game-mode", None)           # :294
+        if "party" in player_data:  # extension: several players queued together, one delivery
+            return self._consume_party(channel_name, tag, player_data["party"], game_mode)
         rating = player_data.get("rating")                        # generic/worker.ex:57 reads it top-level
         if rating is None and isinstance(player_data.get("detail"), dict):
             rating = player_data["detail"].get("rating")
@@ -830,6 +949,20 @@ class SearchWorker:
             rating = 2 ** 31 - 1  # falls between the integer ranges -> default group (generic/worker.ex:46-53)
         rating = max(-(2 ** 31), min(2 ** 31 - 1, int(rating)))
         self.pool.stage(self, tag, player_data, game_mode, rating)
+
+    def _consume_party(self, channel_name, tag, party, game_mode):
+        """{"party": [player documents], "game-mode": ...}: each document needs an "id" and a numeric "rating"."""
+        docs = []
+        for doc in party if isinstance(party, list) else [None]:
+            rating = doc.get("rating") if isinstance(doc, dict) else None
+            if (not isinstance(doc, dict) or "id" not in doc or not isinstance(doc["id"], (str, int))
+                    or isinstance(rating, bool) or not isinstance(rating, (int, float))
+                    or (isinstance(rating, float) and not math.isfinite(rating))):
+                return self.nack(channel_name, tag)
+            docs.append(dict(doc, rating=max(-(2 ** 31), min(2 ** 31 - 1, int(rating)))))
+        if not isinstance(game_mode, str) or not docs:
+            return self.nack(channel_name, tag)
+        self.pool.stage_party(self, tag, docs, game_mode)
 
     # worker.ex:337-368
     def handle_info(self, msg):
