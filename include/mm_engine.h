@@ -397,7 +397,8 @@ int mm_widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hd
  * whole parties whose WAIT >= max_wait, listing every member with the party's seq (cap and the dry run count members;
  * the party members follow the solos); mm_locate reports state 3; mm_requeue gives a queued member code 0.
  * mm_export, mm_export_queues, mm_merge and mm_snapshot are refused with MM_E_STATE while a party is queued (images
- * do not carry parties); mm_restore empties the table.
+ * do not carry parties); mm_restore empties the table.  Parties travel in a party image of their own
+ * (mm_export_parties / mm_merge_parties below): release them, take the image, merge them back.
  * Refusals, decided before anything changes: MM_E_ARG null pointers with n > 0, an MM_ORDER_ARRIVAL engine;
  * MM_E_STATE no party capacity, an MM_F_NO_DEDUPE engine, a staged packed batch; MM_E_CAP a batch the active set
  * cannot hold at all.                                                                                                */
@@ -446,6 +447,52 @@ int mm_party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lo
 int mm_party_read(mm_engine* e, uint32_t party_cap, uint32_t member_cap, uint8_t* size, uint32_t* seq, uint32_t* enq_ts,
                   uint8_t* mode, uint8_t* group, int32_t* rating, uint64_t* member_ids, int32_t* member_rating,
                   uint32_t* n_parties, uint32_t* n_members);
+
+/* Party hand-over: the queued parties in a PARTY IMAGE, so that checkpoint / resume, regroup and queue moves carry them.
+ * The image calls above keep refusing while a party is queued; a host layer releases the parties (mm_export_parties),
+ * uses the image call, and merges the parties where they belong (mm_merge_parties).
+ *
+ * PARTY IMAGE LAYOUT (little-endian).  mm_image_header with magic MM_PARTY_IMAGE_MAGIC, n_parts = P parties, n_players
+ * = M members, n_active = 0, the writer's seq_next and config; then six sections, each starting at the next multiple
+ * of 8 bytes after the previous one ends, padding zero, total_bytes the end of the last rounded up to 8:
+ *   1. size    u8[P]     2. seq   u32[P]     3. enq_ts  u32[P]     4. mode  u8[P]
+ *   5. id      W * M     member ids (u64), or 32-bit handles on MM_F_DENSE_IDS engines
+ *   6. rating  i32[M]
+ * Parties in age order, members in party order.  R, group and bin are not stored: the loading engine derives them
+ * under its own config (so a party image follows mm_import_regroup).
+ *
+ * mm_export_parties: `queues` = n_modes * n_groups bytes in mm_queue_stats order (non-zero: selected), NULL = every
+ * queue.  buf = NULL with cap = 0 -> *n_bytes = the size, nothing changes; cap too small -> MM_E_CAP and *n_bytes,
+ * nothing changes.  A call that writes the image RELEASES the selected parties in the same call, as mm_export_queues
+ * does for solos: their members leave the active set (mm_in_queue 0) and their rows are gone.  Matched party members
+ * are not in the image; they stay in this engine's active set, like matched solos.  Refusals, before anything
+ * changes: MM_E_ARG an MM_ORDER_ARRIVAL engine; MM_E_STATE no party capacity, an MM_F_NO_DEDUPE engine, a staged
+ * packed batch.  The image-sized device scratch is freed before the call returns.
+ *
+ * mm_merge_parties: without flags, exactly one mm_enqueue_party batch of the image's columns (the same codes, sequence
+ * numbers seq_next + index, R / group / bin under THIS engine's config), except that it is all or nothing on room: if
+ * any party would get code 3 the call returns MM_E_CAP and changes nothing (exact: decided after the codes 0 and 2).
+ * code[j] (may be null) per image party: 1 merged; 0 a member is in the active set, or in an earlier party of the
+ * image; 2 no place here (mode >= n_modes, a size above the mode's team_size, an id twice in the party, an R without a
+ * group).  *n_merged counts the 1s.
+ * flags = MM_PARTY_KEEP_SEQ (resume): every party keeps its image seq and seq_next does not move; allowed only when no
+ * party is queued here and seq_next equals the image's (right after mm_import / mm_import_regroup of the image taken
+ * at the same stop, or after the release on the source), else MM_E_STATE.
+ * Refusals, before anything changes: MM_E_ARG bad magic, version or lengths, another id width, an image of an
+ * MM_F_NO_DEDUPE engine, a size below 2, sizes that do not add up to M, an id or handle out of range, seq not strictly
+ * increasing in age order ((seq - seq_next) mod 2^32) or equal to seq_next, unknown flags; MM_E_STATE as
+ * mm_export_parties, and the MM_PARTY_KEEP_SEQ condition; MM_E_CAP the table or a hashed active set cannot take the
+ * merged parties.
+ *
+ * EQUIVALENCE.  mm_export_parties leaves the engine as mm_remove of one member of each exported party would.  After
+ * mm_import (or mm_import_regroup) of an mm_export image and mm_merge_parties(MM_PARTY_KEEP_SEQ) of the party image
+ * taken at the same stop, every later call sequence gives what the source gives, on every output mm_import's
+ * EQUIVALENCE names and on the party calls.                                                                          */
+#define MM_PARTY_IMAGE_MAGIC 0x5954504Du /* "MPTY" */
+#define MM_PARTY_KEEP_SEQ 1u
+int mm_export_parties(mm_engine* e, const uint8_t* queues, void* buf, uint64_t cap, uint64_t* n_bytes);
+int mm_merge_parties(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t flags, uint8_t* code,
+                     uint32_t* n_merged);
 
 /* Replaces ActiveUser.in_queue?/1 (models/active_user.ex:33-44), batched.          */
 int mm_in_queue(mm_engine* e, uint32_t n, const uint64_t* id, uint8_t* out);

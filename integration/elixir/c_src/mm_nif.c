@@ -275,6 +275,49 @@ static ERL_NIF_TERM nif_export_queues(ErlNifEnv* env, int argc, const ERL_NIF_TE
   return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &img));
 }
 
+/* export_parties(ref, queues :: binary(u8[n_modes * n_groups]) | nil) -> {:ok, image :: binary}: the queued parties
+ * of the selected queues (nil: every queue) leave the engine in a party image (mm_export_parties; released in the same
+ * call).  Sized by the dry run, then written. */
+static ERL_NIF_TERM nif_export_parties(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary sel; uint64_t size = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r)) return enif_make_badarg(env);
+  uint8_t queues[MM_MAX_GROUPS * MM_MAX_MODES] = {0};
+  const uint8_t* q = NULL;
+  if (enif_inspect_binary(env, argv[1], &sel)) {
+    if (sel.size == 0 || sel.size > MM_MAX_GROUPS * MM_MAX_MODES) return enif_make_badarg(env);
+    memcpy(queues, sel.data, sel.size);  /* padded with "not selected" */
+    q = queues;
+  }
+  int rc = mm_export_parties(r->e, q, NULL, 0, &size);
+  if (rc) return err(env, rc);
+  ErlNifBinary img;
+  if (!enif_alloc_binary((size_t)size, &img)) return err(env, MM_E_CAP);
+  rc = mm_export_parties(r->e, q, img.data, size, &size);
+  if (rc) { enif_release_binary(&img); return err(env, rc); }
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &img));
+}
+
+/* merge_parties(ref, image :: binary, keep_seq :: boolean) -> {:ok, codes :: binary(u8[])} | {:error, atom}: merges a
+ * party image (mm_merge_parties): codes per party 1 merged, 0 a member already active, 2 no queue here; keep_seq (after
+ * import_image / import_regroup of the image taken at the same stop): every party keeps its sequence number. */
+static ERL_NIF_TERM nif_merge_parties(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary img, codes; uint32_t n = 0, got = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &img))
+    return enif_make_badarg(env);
+  const uint32_t flags = enif_is_identical(argv[2], atom(env, "true")) ? MM_PARTY_KEEP_SEQ : 0u;
+  if (img.size >= sizeof(mm_image_header)) {
+    mm_image_header h;
+    memcpy(&h, img.data, sizeof(h));
+    n = h.n_parts < img.size ? h.n_parts : (uint32_t)img.size;  /* a corrupt count must not size the codes */
+  }
+  if (!enif_alloc_binary((size_t)n, &codes)) return err(env, MM_E_CAP);
+  int rc = mm_merge_parties(r->e, img.data, img.size, flags, codes.data, &got);
+  if (rc) { enif_release_binary(&codes); return err(env, rc); }
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &codes));
+}
+
 /* merge_image(ref, image :: binary) -> {:ok, rejected :: binary(u32[])} | {:error, atom}: loads a queue image into
  * this running engine (mm_merge); `rejected` holds the image indices of players not queued (already active here). */
 static ERL_NIF_TERM nif_merge_image(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
@@ -664,6 +707,8 @@ static ErlNifFunc funcs[] = {
   {"import_image", 2, nif_import_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"export_queues", 2, nif_export_queues, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"merge_image", 2, nif_merge_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"export_parties", 2, nif_export_parties, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"merge_parties", 3, nif_merge_parties, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"import_regroup", 2, nif_import_regroup, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"import_regroup_many", 4, nif_import_regroup_many, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},

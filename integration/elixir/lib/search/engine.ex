@@ -113,6 +113,17 @@ defmodule Matchmaking.Search.Engine do
   """
   def merge_image(_ref, _image), do: :erlang.nif_error(:nif_not_loaded)
   @doc """
+  Party hand-over: the queued parties of the selected queues (queues as export_queues/2 takes them, or nil for every
+  queue) leave the engine in a party image -> {:ok, image}, released as if one member of each were removed.
+  """
+  def export_parties(_ref, _queues), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Merges a party image -> {:ok, codes :: binary(u8[] per party)}: 1 merged, 0 a member already active, 2 no queue here.
+  keep_seq = true after import_image / import_regroup of the image taken at the same stop: every party keeps its number.
+  All or nothing on room: {:error, :capacity} changes nothing.
+  """
+  def merge_parties(_ref, _image, _keep_seq), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
   Requeue (extension): the members of a lobby that did not start go back into their queue at their enqueue position
   (mm_requeue).  handles: binary(u32[]); ratings: binary(i32[]); modes: binary(u8[]); enq_ts, seq: binary(u32[]) — the
   columns each player had when it was queued -> {:ok, codes :: binary(u8[])}: 1 requeued, 0 still queued, 4 gone.

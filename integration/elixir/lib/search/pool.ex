@@ -135,7 +135,8 @@ defmodule Matchmaking.Search.Pool do
            queued: %{}, moved_out: MapSet.new(),
            t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms),
            lobby_budget: Keyword.get(opts, :lobby_budget), paused: MapSet.new(), regroup_dropped: [],
-           widen: Keyword.get(opts, :widen), parties: Keyword.get(opts, :parties), staged_parties: [], party_of: %{}}
+           widen: Keyword.get(opts, :widen), parties: Keyword.get(opts, :parties), staged_parties: [], party_of: %{},
+           party_capacity: Keyword.get(opts, :party_capacity), stranded_parties: []}
     case resume(st, Keyword.get(opts, :resume), Keyword.get(opts, :regroup, false)) do
       {:ok, st} ->
         Process.send_after(self(), :flush, @flush_ms)
@@ -166,9 +167,52 @@ defmodule Matchmaking.Search.Pool do
         # now_ms/1 goes on from the checkpoint's value plus the downtime: the engine's enqueue stamps stay valid
         st = %{st | handle_of: ck.handle_of, players: ck.players, free: ck.free, next: ck.next,
                     queued: Map.get(ck, :queued, %{}), moved_out: Map.get(ck, :moved_out, MapSet.new()),
-                    t0: System.monotonic_time(:millisecond) - ck.now_ms - down}
-        {:ok, drop_rejected(st, ck.image, rejected)}
+                    party_of: Map.get(ck, :party_of, %{}), t0: System.monotonic_time(:millisecond) - ck.now_ms - down}
+        st = drop_rejected(st, ck.image, rejected)
+        case Map.get(ck, :party_image) do
+          nil -> {:ok, st}
+          parties ->  # with their numbers; a party with no queue under this config leaves like a rejected solo
+            with {:ok, codes} <- Engine.merge_parties(st.ref, parties, true) do
+              gone = for {hs, c} <- party_list(parties, codes), c != 1, h <- hs, do: h
+              {:ok, Enum.reduce(gone, st, fn h, acc ->
+                 {player, players} = Map.pop(acc.players, h)
+                 %{acc | players: players, handle_of: Map.delete(acc.handle_of, player["id"]), free: [h | acc.free],
+                         party_of: Map.delete(acc.party_of, h), regroup_dropped: [player | acc.regroup_dropped]}
+               end)}
+            end
+        end
       {:error, _} = e -> e
+    end
+  end
+
+  # every party of a party image as {[member handles], its code or nil}, in image order (include/mm_engine.h: sizes at
+  # 624, then seq, enq_ts, mode, the u32 handles)
+  defp party_list(image, codes) do
+    <<_::binary-size(24), p::little-32, _::binary>> = image
+    a8 = fn x -> Bitwise.band(x + 7, Bitwise.bnot(7)) end
+    id_off = a8.(a8.(a8.(a8.(624 + p) + 4 * p) + 4 * p) + p)
+    sizes = for <<s <- binary_part(image, 624, p)>>, do: s
+    handles = for <<h::little-32 <- binary_part(image, id_off, 4 * Enum.sum(sizes))>>, do: h
+    {parties, _} = Enum.map_reduce(sizes, handles, &Enum.split(&2, &1))
+    Enum.zip(parties, Stream.concat(for(<<c <- codes>>, do: c), Stream.repeatedly(fn -> nil end)))
+  end
+
+  # mm_export, mm_export_queues and mm_merge refuse while a party is queued: with party capacity, every queued party
+  # steps aside (Engine.export_parties) around `fun` and comes back, with its number when the sequence did not move.
+  # -> {result of fun, the party image or nil, st}.  A refused export is fun's error and changes nothing; a party
+  # image that cannot come back is kept in st.stranded_parties (merge it with Engine.merge_parties/3).
+  defp around_parties(%{party_capacity: nil} = st, fun), do: {fun.(), nil, st}
+  defp around_parties(st, fun) do
+    with {:ok, own} <- Engine.export_parties(st.ref, nil),
+         {:ok, s0} <- Engine.seq_next(st.ref) do
+      res = fun.()
+      keep = match?({:ok, ^s0}, Engine.seq_next(st.ref))
+      case Engine.merge_parties(st.ref, own, keep) do
+        {:ok, _} -> {res, own, st}
+        {:error, _} -> {res, own, %{st | stranded_parties: [own | st.stranded_parties]}}
+      end
+    else
+      {:error, _} = e -> {e, nil, st}
     end
   end
 
@@ -256,12 +300,13 @@ defmodule Matchmaking.Search.Pool do
 
   def handle_call(:checkpoint, _from, st) do
     st = flush(st)
-    case Engine.export_image(st.ref) do
-      {:ok, image} ->
+    case around_parties(st, fn -> Engine.export_image(st.ref) end) do
+      {{:ok, image}, parties, st} ->
         ck = %{image: image, handle_of: st.handle_of, players: st.players, free: st.free, next: st.next,
                queued: st.queued, moved_out: st.moved_out, now_ms: now_ms(st), wall_ms: System.os_time(:millisecond)}
+        ck = if parties, do: Map.merge(ck, %{party_image: parties, party_of: st.party_of}), else: ck
         {:reply, {:ok, :erlang.term_to_binary(ck)}, st}
-      {:error, _} = e -> {:reply, e, st}
+      {{:error, _} = e, _, st} -> {:reply, e, st}
     end
   end
 
@@ -271,8 +316,21 @@ defmodule Matchmaking.Search.Pool do
     n_groups = Engine.n_groups()
     queues = for _m <- 0..(Engine.n_modes() - 1), g <- 0..(n_groups - 1), into: <<>>,
                do: <<(if g in groups, do: 1, else: 0)>>
-    case Engine.export_queues(st.ref, queues) do
-      {:ok, image} ->
+    # with parties: the moved queues' parties in a party image of their own, the others step aside around the export
+    exported = if st.party_capacity, do: Engine.export_parties(st.ref, queues), else: {:ok, nil}
+    case exported do
+      {:error, _} = e -> {:reply, e, st}   # refused before anything changed
+      {:ok, moved_parties} -> move_out_queues(st, groups, queues, n_groups, moved_parties)
+    end
+  end
+
+  defp move_out_queues(st, groups, queues, n_groups, moved_parties) do
+    case around_parties(st, fn -> Engine.export_queues(st.ref, queues) end) do
+      {{:error, _} = e, _, st} ->  # the moved parties come back (new numbers)
+        st = if moved_parties && match?({:error, _}, Engine.merge_parties(st.ref, moved_parties, false)),
+               do: %{st | stranded_parties: [moved_parties | st.stranded_parties]}, else: st
+        {:reply, e, st}
+      {{:ok, image}, _, st} ->
         {n, id_off, _} = image_sections(image)
         handles = for <<h::little-32 <- binary_part(image, id_off, 4 * n)>>, do: h
         {moved, st} = Enum.map_reduce(handles, st, fn h, acc ->
@@ -283,8 +341,19 @@ defmodule Matchmaking.Search.Pool do
         st = %{st | moved_out: MapSet.union(st.moved_out, MapSet.new(moved_q))}
         blob = %{image: image, players: moved, n_modes: Engine.n_modes(), n_groups: n_groups,
                  now_ms: now_ms(st), wall_ms: System.os_time(:millisecond)}
+        {blob, st} =
+          if moved_parties do  # the members' ids and documents leave with the party image
+            hs = for {party, _} <- party_list(moved_parties, <<>>), h <- party, do: h
+            {members, st} = Enum.map_reduce(hs, st, fn h, acc ->
+              {player, players} = Map.pop(acc.players, h)
+              {{player["id"], player},
+               release(%{acc | players: players, party_of: Map.delete(acc.party_of, h)}, player["id"], h)}
+            end)
+            {Map.merge(blob, %{party_image: moved_parties, party_players: members}), st}
+          else
+            {blob, st}
+          end
         {:reply, {:ok, :erlang.term_to_binary(blob)}, st}
-      {:error, _} = e -> {:reply, e, st}
     end
   end
 
@@ -300,47 +369,100 @@ defmodule Matchmaking.Search.Pool do
         {{h, fresh, id, player}, acc}
       end)
       {n, id_off, ts_off} = image_sections(mv.image)
-      # enqueue stamps into this pool's clock: the wait at move_out plus the wall time in between, as resume/2 does
-      down = max(0, System.os_time(:millisecond) - mv.wall_ms)
-      shift = Bitwise.band(now_ms(st) - down - mv.now_ms, 0xFFFFFFFF)
-      ids = for {h, _, _, _} <- rows, into: <<>>, do: <<h::little-32>>
-      ts = for <<t::little-32 <- binary_part(mv.image, ts_off, 4 * n)>>, into: <<>>,
-             do: <<Bitwise.band(t + shift, 0xFFFFFFFF)::little-32>>
-      image = binary_part(mv.image, 0, id_off) <> ids <>
-              binary_part(mv.image, id_off + 4 * n, ts_off - id_off - 4 * n) <> ts <>
-              binary_part(mv.image, ts_off + 4 * n, byte_size(mv.image) - ts_off - 4 * n)
-      {:ok, seq0} = Engine.seq_next(st.ref)
-      case Engine.merge_image(st.ref, image) do
-        {:ok, rejected} ->
-          rej = MapSet.new(for <<i::little-32 <- rejected>>, do: i)
-          # mm_merge numbers its batch queue by queue, in the source's enqueue order inside a queue: sort the image
-          # indices by (queue, age), number them, and put the numbers back in image order (n log n, lists walked once)
-          {cols, src_next} = image_cols(mv.image)
-          seqs = cols |> Enum.with_index()
-                 |> Enum.sort_by(fn {{r, m, _t, s}, _i} -> {Engine.queue_of(r, m), Bitwise.band(s - src_next, 0xFFFFFFFF)} end)
-                 |> Enum.with_index(fn {_, i}, k -> {i, Bitwise.band(seq0 + k, 0xFFFFFFFF)} end)
-                 |> Enum.sort() |> Enum.map(&elem(&1, 1))
-          st = Enum.zip([rows, cols, seqs]) |> Enum.with_index() |> Enum.reduce(st, fn {{{h, _, _, _}, {r, m, t, _}, q}, i}, acc ->
-            if MapSet.member?(rej, i) do
-              acc
-            else
-              %{acc | queued: Map.put(acc.queued, h, {r, m, Bitwise.band(t + shift, 0xFFFFFFFF), q}),
-                      moved_out: MapSet.delete(acc.moved_out, Engine.queue_of(r, m))}
-            end
-          end)
-          st = rows |> Enum.with_index() |> Enum.reduce(st, fn {{h, fresh, id, _}, i}, acc ->
-            # a rejected player is already queued here: keep this pool's player and document
-            if MapSet.member?(rej, i) and fresh, do: release(acc, id, h), else: acc
-          end)
-          players = for {{h, _, _, player}, i} <- Enum.with_index(rows), not MapSet.member?(rej, i), into: st.players,
-                      do: {h, player}
-          {:reply, {:ok, n - MapSet.size(rej)}, %{st | players: players}}
-        {:error, _} = e ->
+      moved_members = length(Map.get(mv, :party_players, []))
+      cond do
+        moved_members > 0 and map_size(st.party_of) + moved_members > (st.party_capacity || 0) ->
+          # the party table cannot take the moved parties: refused before anything changes
           st = Enum.reduce(rows, st, fn {h, fresh, id, _}, acc -> if fresh, do: release(acc, id, h), else: acc end)
-          {:reply, e, st}
+          {:reply, {:error, :capacity}, st}
+        true -> move_in_image(st, mv, rows, n, id_off, ts_off)
       end
     end
   end
+
+  defp move_in_image(st, mv, rows, n, id_off, ts_off) do
+    # enqueue stamps into this pool's clock: the wait at move_out plus the wall time in between, as resume/2 does
+    down = max(0, System.os_time(:millisecond) - mv.wall_ms)
+    shift = Bitwise.band(now_ms(st) - down - mv.now_ms, 0xFFFFFFFF)
+    ids = for {h, _, _, _} <- rows, into: <<>>, do: <<h::little-32>>
+    ts = for <<t::little-32 <- binary_part(mv.image, ts_off, 4 * n)>>, into: <<>>,
+           do: <<Bitwise.band(t + shift, 0xFFFFFFFF)::little-32>>
+    image = binary_part(mv.image, 0, id_off) <> ids <>
+            binary_part(mv.image, id_off + 4 * n, ts_off - id_off - 4 * n) <> ts <>
+            binary_part(mv.image, ts_off + 4 * n, byte_size(mv.image) - ts_off - 4 * n)
+    {:ok, seq0} = Engine.seq_next(st.ref)
+    {merged, _, st} = around_parties(st, fn -> Engine.merge_image(st.ref, image) end)
+    case merged do
+      {:ok, rejected} ->
+        rej = MapSet.new(for <<i::little-32 <- rejected>>, do: i)
+        # mm_merge numbers its batch queue by queue, in the source's enqueue order inside a queue: sort the image
+        # indices by (queue, age), number them, and put the numbers back in image order (n log n, lists walked once)
+        {cols, src_next} = image_cols(mv.image)
+        seqs = cols |> Enum.with_index()
+               |> Enum.sort_by(fn {{r, m, _t, s}, _i} -> {Engine.queue_of(r, m), Bitwise.band(s - src_next, 0xFFFFFFFF)} end)
+               |> Enum.with_index(fn {_, i}, k -> {i, Bitwise.band(seq0 + k, 0xFFFFFFFF)} end)
+               |> Enum.sort() |> Enum.map(&elem(&1, 1))
+        st = Enum.zip([rows, cols, seqs]) |> Enum.with_index() |> Enum.reduce(st, fn {{{h, _, _, _}, {r, m, t, _}, q}, i}, acc ->
+          if MapSet.member?(rej, i) do
+            acc
+          else
+            %{acc | queued: Map.put(acc.queued, h, {r, m, Bitwise.band(t + shift, 0xFFFFFFFF), q}),
+                    moved_out: MapSet.delete(acc.moved_out, Engine.queue_of(r, m))}
+          end
+        end)
+        st = rows |> Enum.with_index() |> Enum.reduce(st, fn {{h, fresh, id, _}, i}, acc ->
+          # a rejected player is already queued here: keep this pool's player and document
+          if MapSet.member?(rej, i) and fresh, do: release(acc, id, h), else: acc
+        end)
+        players = for {{h, _, _, player}, i} <- Enum.with_index(rows), not MapSet.member?(rej, i), into: st.players,
+                    do: {h, player}
+        case move_in_parties(%{st | players: players}, mv, shift) do
+          {:ok, st} -> {:reply, {:ok, n - MapSet.size(rej)}, st}
+          # the solos are in; the party image is kept in stranded_parties (with this pool's handles and clock)
+          {{:error, reason}, st} -> {:reply, {:error, {:parties_not_merged, reason, n - MapSet.size(rej)}}, st}
+        end
+      {:error, _} = e ->
+        st = Enum.reduce(rows, st, fn {h, fresh, id, _}, acc -> if fresh, do: release(acc, id, h), else: acc end)
+        {:reply, e, st}
+    end
+  end
+
+  # The party image of a move, after its solos: this pool's handles for the members, the stamps in this pool's clock,
+  # one merge (new numbers here); the members of parties that did not merge give their fresh handles back.
+  defp move_in_parties(st, %{party_image: pimg, party_players: members}, shift) do
+    {rows, st} = Enum.map_reduce(members, st, fn {id, player}, acc ->
+      {h, fresh, acc} = acquire(acc, id)
+      {{h, fresh, id, player}, acc}
+    end)
+    <<_::binary-size(24), p::little-32, _::binary>> = pimg
+    a8 = fn x -> Bitwise.band(x + 7, Bitwise.bnot(7)) end
+    ts_off = a8.(a8.(624 + p) + 4 * p)
+    id_off = a8.(a8.(ts_off + 4 * p) + p)
+    ts = for <<t::little-32 <- binary_part(pimg, ts_off, 4 * p)>>, into: <<>>,
+           do: <<Bitwise.band(t + shift, 0xFFFFFFFF)::little-32>>
+    ids = for {h, _, _, _} <- rows, into: <<>>, do: <<h::little-32>>
+    image = binary_part(pimg, 0, ts_off) <> ts <> binary_part(pimg, ts_off + 4 * p, id_off - ts_off - 4 * p) <> ids <>
+            binary_part(pimg, id_off + byte_size(ids), byte_size(pimg) - id_off - byte_size(ids))
+    case Engine.merge_parties(st.ref, image, false) do
+      {:ok, codes} ->
+        {st, _} = Enum.reduce(party_list(image, codes), {st, rows}, fn {hs, c}, {acc, left} ->
+          {mine, left} = Enum.split(left, length(hs))
+          acc = Enum.reduce(mine, acc, fn {h, fresh, id, player}, a ->
+            cond do
+              c == 1 -> %{a | players: Map.put(a.players, h, player), party_of: Map.put(a.party_of, h, hs)}
+              fresh -> release(a, id, h)
+              true -> a
+            end
+          end)
+          {acc, left}
+        end)
+        {:ok, st}
+      {:error, reason} ->  # the members keep their handles and documents until the kept image is merged
+        players = for {h, _, _, player} <- rows, into: st.players, do: {h, player}
+        {{:error, reason}, %{st | players: players, stranded_parties: [image | st.stranded_parties]}}
+    end
+  end
+  defp move_in_parties(st, _mv, _shift), do: {:ok, st}
 
   # -- requeue (extension): a lobby that did not start ----------------------------------------------------------------
   def handle_call({:requeue, players}, _from, st) do

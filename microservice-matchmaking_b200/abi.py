@@ -212,6 +212,8 @@ class QueueQuality(C.Structure):
 MM_IMAGE_MAGIC = 0x474D494D
 MM_QUEUE_IMAGE_MAGIC = 0x5155514D  # mm_export_queues: same header and sections, no active section
 MM_IMAGE_VERSION = 1
+MM_PARTY_IMAGE_MAGIC = 0x5954504D  # mm_export_parties: the mm_image_header, then the party sections
+MM_PARTY_KEEP_SEQ = 1  # mm_merge_parties: every party keeps its image seq (resume)
 
 
 class ImageHeader(C.Structure):
@@ -236,6 +238,16 @@ def image_offsets(n_parts, n_players, n_active, id_bytes):
     total length.  Every section starts at the next multiple of 8 after the one before it."""
     sizes = (4 * n_parts, id_bytes * n_players, 4 * n_players, 4 * n_players, 4 * n_players, n_players,
              id_bytes * n_active)
+    off = [C.sizeof(ImageHeader)]
+    for s in sizes:
+        off.append((off[-1] + s + 7) & ~7)
+    return off
+
+
+def party_image_offsets(n_parties, n_members, id_bytes):
+    """Section offsets of a party image (include/mm_engine.h): size, seq, enq_ts, mode, id, rating, and the total
+    length.  Every section starts at the next multiple of 8 after the one before it."""
+    sizes = (n_parties, 4 * n_parties, 4 * n_parties, n_parties, id_bytes * n_members, 4 * n_members)
     off = [C.sizeof(ImageHeader)]
     for s in sizes:
         off.append((off[-1] + s + 7) & ~7)
@@ -270,6 +282,8 @@ PROTOTYPES = {
     "mm_party_match": (C.c_int, [_vp, C.c_uint64, _vp, _vp, C.c_uint32, _vp, C.c_uint64, _P(PartyStats)]),
     "mm_party_read": (C.c_int, [_vp, C.c_uint32, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _P(C.c_uint32),
                                 _P(C.c_uint32)]),
+    "mm_export_parties": (C.c_int, [_vp, _vp, _vp, C.c_uint64, _P(C.c_uint64)]),
+    "mm_merge_parties": (C.c_int, [_vp, _vp, C.c_uint64, C.c_uint32, _vp, _P(C.c_uint32)]),
     "mm_in_queue": (C.c_int, [_vp, C.c_uint32, _vp, _vp]),
     "mm_locate": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp]),
     "mm_pool_size": (C.c_int, [_vp, _P(C.c_uint32)]),

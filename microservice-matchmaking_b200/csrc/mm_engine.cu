@@ -338,7 +338,7 @@ struct mm_engine {
     } buf[2];
     int cur = 0;
     DevArray<uint8_t> in_size, in_mode, in_pre, in_code;
-    DevArray<uint32_t> in_ts, in_moff, in_mparty, in_msz, in_one;
+    DevArray<uint32_t> in_ts, in_moff, in_mparty, in_msz, in_one, in_seq;
     DevArray<uint64_t> in_id, in_hslot;
     DevArray<int32_t> in_rating;
     DevArray<uint32_t> pb, pcur, tmp, sorted, lob, pos;  // match: [K + 1], [K], then [rows] each (tmp: compaction)
@@ -2644,10 +2644,13 @@ int pt_check(mm_engine* e) {
   return MM_OK;
 }
 
-int enqueue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t* ids, const int32_t* rating,
-                  const uint8_t* mode, const uint32_t* enq_ts, uint8_t* accepted) {
-  int rc = pt_check(e);
-  if (rc || n == 0) return rc;
+// The enqueue pipeline of mm_enqueue_party and mm_merge_parties (after pt_check, n > 0).  seq: every party's own
+// number (MM_PARTY_KEEP_SEQ: seq_next does not move), else seq_next + index.  exact: MM_E_CAP with every claim undone
+// if a party would get code 3, decided from the scanned member count of the code-1 parties (one counter read) before
+// any row or active-set value is written.
+int pt_enqueue(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t* ids, const int32_t* rating,
+               const uint8_t* mode, const uint32_t* enq_ts, const uint32_t* seq, bool exact, uint8_t* accepted) {
+  int rc;
   auto& s = e->pt;
   std::vector<uint32_t> moff(n), mparty;
   uint32_t m = 0;
@@ -2657,10 +2660,14 @@ int enqueue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t*
     mparty.insert(mparty.end(), size[j], j);
   }
   if ((rc = act_room(e, m, m))) return rc;
-  e->fresh = false;
+  if (!exact) e->fresh = false;
   if (s.n_mem + (uint64_t)m > s.cap && (rc = pt_compact(e))) return rc;
   CK(s.in_size.reserve(n)); CK(s.in_mode.reserve(n)); CK(s.in_code.reserve(n)); CK(s.in_ts.reserve(n));
   CK(s.in_moff.reserve(n)); CK(s.in_msz.reserve(n)); CK(s.in_one.reserve(n));
+  if (seq) {
+    CK(s.in_seq.reserve(n));
+    CK(cudaMemcpyAsync(s.in_seq, seq, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  }
   const size_t mm = std::max<uint32_t>(m, 1);
   CK(s.in_pre.reserve(mm)); CK(s.in_mparty.reserve(mm)); CK(s.in_id.reserve(mm)); CK(s.in_hslot.reserve(mm));
   CK(s.in_rating.reserve(mm));
@@ -2680,12 +2687,25 @@ int enqueue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t*
   a.bm = bin_map(e); a.grp_lut = e->d_grp_lut; a.mode_tsize = e->d_mode_tsize; a.n_modes = e->cfg.n_modes;
   a.hslot = s.in_hslot; a.pre = s.in_pre; a.code = s.in_code; a.msz = s.in_msz; a.one = s.in_one;
   a.tot = s.ctr + kPtWords; a.room = s.cap - s.n_mem; a.rows0 = s.n_rows; a.mem0 = s.n_mem; a.seq0 = e->seq_next;
-  a.pt = pt_view(e, s.cur); a.ctr = s.ctr;
+  a.seq = seq ? s.in_seq.p : nullptr; a.pt = pt_view(e, s.cur); a.ctr = s.ctr;
   const uint32_t gm = (m + 255) / 256, gn = (n + 255) / 256;
   if (m) k_pt_claim<<<gm, 256, 0, e->stream>>>(a);
   k_pt_resolve<<<gn, 256, 0, e->stream>>>(a);
   k_scan_small<<<1, 1024, 0, e->stream>>>(n, s.in_msz, a.tot);
   k_scan_small<<<1, 1024, 0, e->stream>>>(n, s.in_one, a.tot + 1);
+  if (exact) {
+    uint32_t want = 0;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(&want, a.tot, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+    if (want > a.room) {
+      if (m) k_pt_unclaim<<<gm, 256, 0, e->stream>>>(a);
+      CK(cudaGetLastError());
+      CK(cudaStreamSynchronize(e->stream));
+      return set_err(e, MM_E_CAP, "%u party members to merge, the party table has room for %u", want, a.room);
+    }
+    e->fresh = false;
+  }
   k_pt_commit<<<gn, 256, 0, e->stream>>>(a);
   if (m) k_pt_members<<<gm, 256, 0, e->stream>>>(a);
   CK(cudaGetLastError());
@@ -2700,8 +2720,142 @@ int enqueue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t*
   s.n_rows += rows; s.n_mem += acc; s.live += acc;
   e->n_active += acc;
   if (!e->dense_ids) e->n_tomb += h[kPtReleased];
-  e->seq_next += n;
+  if (!seq) e->seq_next += n;
   if (accepted) std::memcpy(accepted, code.data(), n);
+  return MM_OK;
+}
+
+int enqueue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t* ids, const int32_t* rating,
+                  const uint8_t* mode, const uint32_t* enq_ts, uint8_t* accepted) {
+  int rc = pt_check(e);
+  if (rc || n == 0) return rc;
+  return pt_enqueue(e, n, size, ids, rating, mode, enq_ts, nullptr, false, accepted);
+}
+
+// Section offsets of a party image (include/mm_engine.h): [0] size, [1] seq, [2] enq_ts, [3] mode, [4] id, [5] rating,
+// [6] total bytes.
+struct PtImgLayout { uint64_t off[7]; };
+PtImgLayout pt_img_layout(uint32_t P, uint32_t M, uint32_t W) {
+  auto a8 = [](uint64_t x) { return (x + 7) & ~7ull; };
+  const uint64_t bytes[6] = {(uint64_t)P, 4ull * P, 4ull * P, (uint64_t)P, (uint64_t)W * M, 4ull * M};
+  PtImgLayout l{};
+  l.off[0] = sizeof(mm_image_header);
+  for (int k = 0; k < 6; ++k) l.off[k + 1] = a8(l.off[k] + bytes[k]);
+  return l;
+}
+
+// mm_export_parties: select and count (k_pt_sel, the scans, one counter read), then the columns gathered in age order
+// into device scratch and released in the same pass (k_pt_export), one device-to-host copy.
+int export_parties(mm_engine* e, const uint8_t* queues, void* buf, uint64_t cap, uint64_t* n_bytes) {
+  int rc = pt_check(e);
+  if (rc) return rc;
+  auto& s = e->pt;
+  const uint32_t nr = s.n_rows, W = id_bytes(e), g = (nr + 255) / 256;
+  const PartyView t = pt_view(e, s.cur);
+  const uint8_t* sel = nullptr;
+  uint32_t h[2] = {0, 0};  // parties, members
+  uint32_t* tot = s.ctr + kPtWords;
+  if (nr) {
+    if (queues) {
+      CK(e->d_sel.reserve(kMaxSegs));
+      CK(cudaMemcpyAsync(e->d_sel, queues, e->n_cut, cudaMemcpyHostToDevice, e->stream));
+      sel = e->d_sel;
+    }
+    CK(cudaMemsetAsync(s.ctr, 0, (kPtWords + 2) * 4, e->stream));
+    k_pt_sel<<<g, 256, 0, e->stream>>>(nr, t, sel, e->cfg.n_groups, s.tmp, s.sorted);
+    k_scan_small<<<1, 1024, 0, e->stream>>>(nr, s.tmp, tot);
+    k_scan_small<<<1, 1024, 0, e->stream>>>(nr, s.sorted, tot + 1);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(h, tot, 8, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+  }
+  const uint32_t P = h[0], M = h[1];
+  const PtImgLayout l = pt_img_layout(P, M, W);
+  *n_bytes = l.off[6];
+  if (!buf) return MM_OK;
+  if (cap < l.off[6]) return set_err(e, MM_E_CAP, "need cap >= %llu", (unsigned long long)l.off[6]);
+  uint8_t* out = static_cast<uint8_t*>(buf);
+  mm_image_header hd{};
+  hd.magic = MM_PARTY_IMAGE_MAGIC; hd.version = MM_IMAGE_VERSION; hd.abi_version = MM_ABI_VERSION; hd.id_bytes = W;
+  hd.total_bytes = l.off[6]; hd.n_parts = P; hd.n_players = M; hd.n_active = 0; hd.seq_next = e->seq_next;
+  hd.config = e->cfg;
+  std::memcpy(out, &hd, sizeof(hd));
+  if (!P) return MM_OK;
+  const uint64_t body = l.off[6] - l.off[0];
+  CK(e->d_img.reserve(body));
+  uint8_t* d = e->d_img;
+  CK(cudaMemsetAsync(d, 0, body, e->stream));
+  PtImgCols c{};
+  c.size = d; c.seq = reinterpret_cast<uint32_t*>(d + (l.off[1] - l.off[0]));
+  c.ts = reinterpret_cast<uint32_t*>(d + (l.off[2] - l.off[0])); c.mode = d + (l.off[3] - l.off[0]);
+  c.id = d + (l.off[4] - l.off[0]); c.rating = reinterpret_cast<int32_t*>(d + (l.off[5] - l.off[0])); c.id_bytes = W;
+  k_pt_export<<<g, 256, 0, e->stream>>>(nr, t, sel, e->cfg.n_groups, s.tmp, s.sorted, c, act_view(e),
+                                        s.ctr + kPtReleased);
+  CK(cudaGetLastError());
+  uint32_t freed = 0;
+  CK(cudaMemcpyAsync(out + l.off[0], d, body, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(&freed, s.ctr + kPtReleased, 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  s.live -= M;
+  erase_active(e, freed);
+  return MM_OK;
+}
+
+// mm_merge_parties: every image check on the host, then pt_enqueue with its exact room decision.
+int merge_parties(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t flags, uint8_t* code, uint32_t* n_merged) {
+  int rc = pt_check(e);
+  if (rc) return rc;
+  auto bad = [&](const char* what) { return set_err(e, MM_E_ARG, "party image rejected: %s", what); };
+  if (flags & ~MM_PARTY_KEEP_SEQ) return bad("unknown flags");
+  mm_image_header h;
+  if (nb < sizeof(h)) return bad("shorter than its header");
+  std::memcpy(&h, buf, sizeof(h));
+  if (h.magic != MM_PARTY_IMAGE_MAGIC) return bad("bad magic (not an mm_export_parties image)");
+  if (h.version != MM_IMAGE_VERSION || h.abi_version != MM_ABI_VERSION) return bad("unknown version");
+  if (h.id_bytes != id_bytes(e)) return bad("id width differs from the engine's");
+  if (h.config.flags & MM_F_NO_DEDUPE) return bad("written by an MM_F_NO_DEDUPE engine");
+  const uint32_t P = h.n_parts, M = h.n_players, W = h.id_bytes;
+  const PtImgLayout l = pt_img_layout(P, M, W);
+  if (h.n_active || h.total_bytes != l.off[6] || nb != l.off[6])
+    return bad("length does not match the header's section counts");
+  const uint8_t* size = buf + l.off[0];
+  const uint8_t* mode = buf + l.off[3];
+  std::vector<uint32_t> seq(P), ts(P);
+  std::vector<int32_t> rating(M);
+  std::vector<uint64_t> ids(M);
+  std::memcpy(seq.data(), buf + l.off[1], (size_t)P * 4);
+  std::memcpy(ts.data(), buf + l.off[2], (size_t)P * 4);
+  std::memcpy(rating.data(), buf + l.off[5], (size_t)M * 4);
+  uint64_t sum = 0;
+  for (uint32_t j = 0; j < P; ++j) {
+    if (size[j] < 2) return bad("a party of fewer than 2 members");
+    sum += size[j];
+  }
+  if (sum != M) return bad("party sizes do not add up to the member count");
+  const uint64_t lim = id_limit(e);
+  for (uint32_t k = 0; k < M; ++k) {
+    if (W == 8) std::memcpy(&ids[k], buf + l.off[4] + 8ull * k, 8);
+    else { uint32_t x; std::memcpy(&x, buf + l.off[4] + 4ull * k, 4); ids[k] = x; }
+    if (ids[k] >= lim) return bad("id out of range");
+  }
+  for (uint32_t j = 0; j < P; ++j) {
+    const uint32_t age = seq[j] - h.seq_next;  // (seq - seq_next) mod 2^32: the oldest first
+    if (age == 0 || (j && age <= seq[j - 1] - h.seq_next)) return bad("sequence numbers out of order");
+  }
+  const bool keep = flags & MM_PARTY_KEEP_SEQ;
+  if (keep && (e->pt.live || e->seq_next != h.seq_next))
+    return set_err(e, MM_E_STATE,
+                   "MM_PARTY_KEEP_SEQ needs no queued party and seq_next %u (the image's): %u party members queued, "
+                   "seq_next %u", h.seq_next, e->pt.live, e->seq_next);
+  if (P == 0) return MM_OK;
+  std::vector<uint8_t> c(P);
+  if ((rc = pt_enqueue(e, P, size, ids.data(), rating.data(), mode, ts.data(), keep ? seq.data() : nullptr, true,
+                       c.data())))
+    return rc;
+  uint32_t k = 0;
+  for (uint8_t x : c) k += x == 1;
+  *n_merged = k;
+  if (code) std::memcpy(code, c.data(), P);
   return MM_OK;
 }
 
@@ -3270,6 +3424,25 @@ int mm_party_read(mm_engine* e, uint32_t party_cap, uint32_t member_cap, uint8_t
   CK(cudaSetDevice(e->device));
   return party_read(e, party_cap, member_cap, size, seq, enq_ts, mode, group, rating, member_ids, member_rating,
                     n_parties, n_members);
+}
+
+int mm_export_parties(mm_engine* e, const uint8_t* queues, void* buf, uint64_t cap, uint64_t* n_bytes) {
+  if (!e || !n_bytes || (cap && !buf)) return MM_E_ARG;
+  *n_bytes = 0;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  const int rc = export_parties(e, queues, buf, cap, n_bytes);
+  free_img_scratch(e);
+  return rc;
+}
+
+int mm_merge_parties(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t flags, uint8_t* code,
+                     uint32_t* n_merged) {
+  if (!e || !n_merged || (n_bytes && !buf)) return MM_E_ARG;
+  *n_merged = 0;
+  std::lock_guard<std::mutex> lk(e->mu);
+  CK(cudaSetDevice(e->device));
+  return merge_parties(e, static_cast<const uint8_t*>(buf), n_bytes, flags, code, n_merged);
 }
 
 int mm_remove_packed(mm_engine* e, uint32_t n, const uint32_t* handle, uint32_t* n_removed) {

@@ -21,6 +21,11 @@
 // the same co-party walk again, then one wd_walk<true, walk order> per team with open slots, so the solos fill team 0,
 // then team 1, ... in their rank order.  The solo pieces go through k_bf_keys, the band pipeline and k_bf_out like
 // mm_widen's; k_wd_bases / k_wd_hdr write the headers and bases and k_pt_out copies the party members.
+//
+// Hand-over (mm_export_parties / mm_merge_parties): k_pt_sel and two k_scan_small give every selected live row its
+// image index and member offset, k_pt_export gathers the columns in age order and releases the row (pt_release, as
+// k_pt_dissolve does).  The merge is the enqueue pipeline with the image's numbers (PtEnqArgs::seq) or new ones; its
+// refusal for room comes before k_pt_commit, and k_pt_unclaim gives the claims back.
 #pragma once
 
 #include "mm_widen.cuh"
@@ -59,6 +64,7 @@ struct PtEnqArgs {
   uint32_t* tot;                 // [2] scan totals (zeroed)
   uint32_t room;                 // members the table still holds
   uint32_t rows0, mem0, seq0;    // first free row and member entry, seq of party 0
+  const uint32_t* seq;           // [n] the parties' own numbers (mm_merge_parties, MM_PARTY_KEEP_SEQ), or null
   PartyView pt;
   uint32_t* ctr;
 };
@@ -131,7 +137,7 @@ __global__ void k_pt_commit(const PtEnqArgs a) {
   long long R = sum / (long long)s;
   if (R * (long long)s > sum) --R;
   const int32_t Rc = (int32_t)R;  // the mean of 32-bit ratings
-  a.pt.seq[row] = a.seq0 + p;
+  a.pt.seq[row] = a.seq ? a.seq[p] : a.seq0 + p;
   a.pt.ts[row] = a.ts ? a.ts[p] : 0u;
   a.pt.off[row] = a.mem0 + a.msz[p];
   a.pt.R[row] = Rc;
@@ -211,16 +217,79 @@ __device__ __forceinline__ uint32_t pt_free(ActiveView act, uint64_t pid, uint32
   return 1;
 }
 
+// Row r's members leave the active set (the entries that still are the row's) and the row is gone.  -> entries freed
+__device__ __forceinline__ uint32_t pt_release(PartyView t, ActiveView act, uint32_t r) {
+  uint32_t freed = 0;
+  for (uint32_t k = 0; k < t.size[r]; ++k) freed += pt_free(act, t.mid[t.off[r] + k], r);
+  t.dead[r] = 1;
+  return freed;
+}
+
 // after k_remove: the other members of every marked party leave (counted with the removed ones), the row is gone
 __global__ void k_pt_dissolve(uint32_t n_rows, PartyView t, ActiveView act, uint32_t* __restrict__ n_removed,
                               uint32_t* __restrict__ ctr) {
   const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= n_rows || t.dead[r] != 2) return;
-  uint32_t freed = 0;
-  for (uint32_t k = 0; k < t.size[r]; ++k) freed += pt_free(act, t.mid[t.off[r] + k], r);
-  t.dead[r] = 1;
+  const uint32_t freed = pt_release(t, act, r);
   if (freed) atomicAdd(n_removed, freed);
   atomicAdd(&ctr[kPtGone], t.size[r]);
+}
+
+// ---- hand-over (mm_export_parties / mm_merge_parties) -----------------------------------------------------------------
+// The party image's columns (include/mm_engine.h), from section 1 (size) on.
+struct PtImgCols {
+  uint8_t* size;
+  uint32_t* seq;
+  uint32_t* ts;
+  uint8_t* mode;
+  uint8_t* id;  // id_bytes per member
+  int32_t* rating;
+  uint32_t id_bytes;
+};
+
+// a live row of a selected queue (sel: one byte per (mode, group) queue, null: every queue)
+__device__ __forceinline__ bool pt_selected(const PartyView& t, const uint8_t* sel, uint32_t n_groups, uint32_t r) {
+  return t.dead[r] == 0 && (!sel || sel[t.mode[r] * n_groups + t.grp[r]]);
+}
+
+// the export's rows: 1 and the member count per selected row (k_pt_keep's shape), for the two scans
+__global__ void k_pt_sel(uint32_t n_rows, PartyView t, const uint8_t* __restrict__ sel, uint32_t n_groups,
+                         uint32_t* __restrict__ keep, uint32_t* __restrict__ msz) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rows) return;
+  const bool k = pt_selected(t, sel, n_groups, r);
+  keep[r] = k;
+  msz[r] = k ? t.size[r] : 0u;
+}
+
+// One thread per selected row, after the scans: its columns at its image index (age order), then its release.
+__global__ void k_pt_export(uint32_t n_rows, PartyView t, const uint8_t* __restrict__ sel, uint32_t n_groups,
+                            const uint32_t* __restrict__ keep, const uint32_t* __restrict__ msz, PtImgCols out,
+                            ActiveView act, uint32_t* __restrict__ n_freed) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rows || !pt_selected(t, sel, n_groups, r)) return;
+  const uint32_t q = keep[r], o = msz[r], so = t.off[r], n = t.size[r];
+  out.size[q] = (uint8_t)n; out.seq[q] = t.seq[r]; out.ts[q] = t.ts[r]; out.mode[q] = t.mode[r];
+  for (uint32_t k = 0; k < n; ++k) {
+    const uint64_t pid = t.mid[so + k];
+    if (out.id_bytes == 8) reinterpret_cast<uint64_t*>(out.id)[o + k] = pid;
+    else reinterpret_cast<uint32_t*>(out.id)[o + k] = (uint32_t)pid;
+    out.rating[o + k] = t.mrat[so + k];
+  }
+  const uint32_t freed = pt_release(t, act, r);
+  if (freed) atomicAdd(n_freed, freed);
+}
+
+// mm_merge_parties refused for room, after k_pt_claim and before any commit: every claim of the batch is undone.  An
+// id claimed without `pre` was free before the call; hashed, k_pt_claim inserted its key into an empty slot (it never
+// takes a tombstone), so the slot goes back to empty and every probe chain is what it was.
+__global__ void k_pt_unclaim(const PtEnqArgs a) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= a.m) return;
+  const uint64_t h = a.hslot[j];
+  if (h == ~0ull || a.pre[j]) return;
+  *a.act.val(h) = kFreeVal;
+  if (!a.act.dcap) *a.act.key(h) = kEmptyKey;
 }
 
 // mm_expire: whole parties whose WAIT >= max_wait, after k_expire on the same counters (ctr[0] the output cursor,

@@ -142,6 +142,37 @@ def read_image(buf):
     return h, cols
 
 
+def active_set_limit(cfg):
+    """Ids a hashed active set holds at its 3/4 load (the table size mm_create picks for cfg); None for an engine
+    without one (MM_F_NO_DEDUPE) or with a direct-mapped handle table (MM_F_DENSE_IDS)."""
+    if int(cfg.flags) & 3:
+        return None
+    want = cfg.active_capacity or 2 * cfg.capacity
+    h = 1024
+    while h * 3 < want * 4 + 64:
+        h <<= 1
+    return h * 3 // 4
+
+
+def read_party_image(buf):
+    """Parse an mm_export_parties image without a GPU -> (abi.ImageHeader, dict of numpy views: size, seq, enq_ts, mode
+    per party, id and rating per member).  Raises ValueError when the buffer is shorter than its header says."""
+    buf = np.frombuffer(buf, np.uint8) if isinstance(buf, (bytes, bytearray, memoryview)) else np.asarray(buf, np.uint8)
+    if len(buf) < C.sizeof(abi.ImageHeader):
+        raise ValueError("party image shorter than its header")
+    h = abi.ImageHeader.from_buffer_copy(buf[:C.sizeof(abi.ImageHeader)].tobytes())
+    off = abi.party_image_offsets(h.n_parts, h.n_players, h.id_bytes)
+    if len(buf) < off[-1]:
+        raise ValueError("party image shorter than its sections")
+    idt = np.uint64 if h.id_bytes == 8 else np.uint32
+    p, m = h.n_parts, h.n_players
+    cols = {}
+    for k, (name, dt, cnt) in enumerate((("size", np.uint8, p), ("seq", np.uint32, p), ("enq_ts", np.uint32, p),
+                                         ("mode", np.uint8, p), ("id", idt, m), ("rating", np.int32, m))):
+        cols[name] = buf[off[k]:off[k] + cnt * np.dtype(dt).itemsize].view(dt)
+    return h, cols
+
+
 class Engine:
     """One GPU-resident player pool + active set + search tick (single writer)."""
 
@@ -499,6 +530,38 @@ class Engine:
             out["members"] = list(zip(np.split(mid[:nm.value], cut), np.split(mrt[:nm.value], cut))) if np_.value else []
             return out
 
+    def export_parties(self, mask=None):
+        """Release the queued parties of the selected (mode, group) queues into a party image (mm_export_parties) ->
+        uint8 array (read_party_image).  mask: bool per queue as export_queues takes it, or None for every queue.  The
+        exported parties leave this engine as if remove() had been called with one member of each."""
+        sel = None
+        if mask is not None:
+            sel = np.ascontiguousarray(np.asarray(mask, bool).reshape(-1), np.uint8)
+            assert len(sel) == self.cfg.n_modes * self.cfg.n_groups
+        n = C.c_uint64(0)
+        self._check(self.lib.mm_export_parties(self.h, _p(sel), None, 0, C.byref(n)), "mm_export_parties")
+        for attempt in range(2):  # the size query and the export are two calls: a party enqueued between them is retried
+            buf = np.empty(n.value, np.uint8)
+            rc = self.lib.mm_export_parties(self.h, _p(sel), _p(buf), n.value, C.byref(n))
+            if rc == abi.MM_E_CAP and attempt == 0:
+                continue
+            self._check(rc, "mm_export_parties")
+            return buf[:n.value]
+
+    def merge_parties(self, buf, keep_seq=False):
+        """Merge a party image (export_parties) into this engine (mm_merge_parties): one enqueue_party batch of its
+        columns, all or nothing on room.  keep_seq: every party keeps its number (after import_state / import_regroup
+        of the image taken at the same stop).  -> codes u8[n_parties] as enqueue_party gives them (never 3)."""
+        buf = np.ascontiguousarray(np.frombuffer(buf, np.uint8) if isinstance(buf, (bytes, bytearray, memoryview))
+                                   else buf, np.uint8)
+        hs = C.sizeof(abi.ImageHeader)
+        n = abi.ImageHeader.from_buffer_copy(buf[:hs].tobytes()).n_parts if len(buf) >= hs else 0
+        code = np.zeros(max(min(n, len(buf)), 1), np.uint8)  # a party takes more than a byte: a corrupt count is capped
+        k = C.c_uint32(0)
+        self._check(self.lib.mm_merge_parties(self.h, _p(buf), len(buf), abi.MM_PARTY_KEEP_SEQ if keep_seq else 0,
+                                              _p(code), C.byref(k)), "mm_merge_parties")
+        return code[:n]
+
     def in_queue(self, ids):
         ids = np.ascontiguousarray(ids, np.uint64)
         out = np.empty(len(ids), np.uint8)
@@ -756,8 +819,12 @@ class Engine:
     def set_stream(self, cuda_stream):
         self._check(self.lib.mm_set_stream(self.h, C.c_void_p(cuda_stream)), "mm_set_stream")
 
+    party_capacity = 0  # the option "party_capacity" as last set
+
     def set_option(self, name, value):
         self._check(self.lib.mm_set_option(self.h, name.encode(), int(value)), "mm_set_option")
+        if name == "party_capacity":
+            self.party_capacity = int(value)
 
     def status(self):
         """Search.Worker.status/0 analogue (search/worker.ex:115-117,326-334): queue depth."""

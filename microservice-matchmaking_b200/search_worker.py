@@ -199,6 +199,7 @@ class SearchPool:
                       for g in range(len(group_names))}
         self.party_rules = {(i, g): tuple(int(x) for x in parties[m]) for i, m in enumerate(mode_names)
                             if m in (parties or {}) for g in range(len(group_names))}
+        self.party_capacity = int(party_capacity or 0)
         if party_capacity:
             engine.set_option("party_capacity", int(party_capacity))
         self.party_of = {}  # handle -> the handles of its queued party (remove_user takes the whole party out)
@@ -636,12 +637,24 @@ class SearchPool:
         deliveries are ingested first, so every acked player is in the image, and pending async results are waited
         for.  Layout: CHECKPOINT_MAGIC, u64 length of a JSON document (the host state: handle table, player documents,
         enqueue times, mode / group names, the pool clock and the wall time), the JSON, then the engine image
-        (Engine.export_state, opaque here).  Stop consuming before the call: a delivery staged after it is not in the
-        checkpoint, and it stays unacked, so the broker redelivers it."""
+        (Engine.export_state, opaque here).  A pool with party_capacity releases its queued parties around the export
+        (Engine.export_parties) and merges them back with their numbers, so it goes on unchanged; its JSON gains
+        "party_of" (the queued parties' handles) and "party_image" (the party image's length in bytes), and the party
+        image goes between the JSON and the engine image.  A pool without party capacity writes neither.  Stop
+        consuming before the call: a delivery staged after it is not in the checkpoint, and it stays unacked, so the
+        broker redelivers it."""
         self.flush()
         if hasattr(self.engine, "results_wait"):
             self.engine.results_wait()
-        image = self.engine.export_state()
+        parties = None
+        if self.party_capacity:  # released around the image and merged back with their numbers: the engine goes on
+            parties = np.ascontiguousarray(self.engine.export_parties(), np.uint8)
+            try:
+                image = self.engine.export_state()
+            finally:
+                self.engine.merge_parties(parties, keep_seq=True)
+        else:
+            image = self.engine.export_state()
         image = image.tobytes() if isinstance(image, np.ndarray) else bytes(image)
         t = self.clock()
         state = {
@@ -654,6 +667,10 @@ class SearchPool:
             "moved_out": sorted(self.moved_out),
             "now_ms": self.now_ms(), "wall": self.wall_clock(),
         }
+        if parties is not None:  # the party image goes between the JSON and the engine image
+            state["party_of"] = sorted({tuple(p) for p in self.party_of.values()})
+            state["party_image"] = len(parties)
+            image = parties.tobytes() + image
         doc = json.dumps(state).encode()
         return self.CHECKPOINT_MAGIC + len(doc).to_bytes(8, "little") + doc + image
 
@@ -686,6 +703,10 @@ class SearchPool:
             raise ValueError("the checkpoint was taken with other mode or group names")
         pool = cls(engine, mode_names, group_names, **opts)
         image = bytes(blob[head + 8 + n:])
+        k = int(state.get("party_image", 0))
+        parties, image = image[:k], image[k:]
+        if k and not pool.party_capacity:
+            raise ValueError("the checkpoint holds parties: resume it with a party_capacity")
         rejected = []
         if regroup:
             from .engine import read_image
@@ -693,6 +714,13 @@ class SearchPool:
             rejected = read_image(image)[1]["id"][idx].tolist()
         else:
             engine.import_state(image)
+        if k:  # the parties keep their numbers; a party with no queue under this config leaves like a rejected solo
+            from .engine import read_party_image
+            codes = engine.merge_parties(parties, keep_seq=True)
+            _h, pc = read_party_image(parties)
+            for c, hs in zip(codes.tolist(), np.split(pc["id"], np.cumsum(pc["size"].astype(np.int64))[:-1])):
+                if c != 1:
+                    rejected += hs.tolist()
         down = max(0.0, pool.wall_clock() - state["wall"])
         pool._t0 = pool.clock() - down - state["now_ms"] / 1000.0
         pool.handles.id_of = list(state["id_of"])
@@ -704,8 +732,10 @@ class SearchPool:
         pool.matched_at = {int(h): at - age for h, age in state.get("matched_at", [])}
         pool.queued = {int(h): rec for h, rec in state.get("queued", [])}  # the image keeps every sequence number
         pool.moved_out = set(state.get("moved_out", []))
+        pool.party_of = {int(h): tuple(int(x) for x in hs) for hs in state.get("party_of", []) for h in hs}
         pool.regroup_dropped = []
         for h in rejected:  # not queued under the new config: they left
+            pool.party_of.pop(h, None)
             pool.regroup_dropped.append(pool.players.pop(h))
             for d in (pool.queued, pool.enqueued_at, pool.matched_at):
                 d.pop(h, None)
@@ -720,8 +750,12 @@ class SearchPool:
         move_in().  The staged deliveries are ingested first.  The engine releases the players in the same call that
         writes their image (Engine.export_queues), and this pool forgets their handles and documents.  Layout:
         MOVE_MAGIC, u64 length of a JSON document (mode / group names, the pool clock and the wall time, and per moved
-        player in image order its id, document and age), the JSON, then the queue image.  Reroute the groups'
-        deliveries to the new owner before the call: a delivery staged after it stays here."""
+        player in image order its id, document and age), the JSON, then the queue image.  A pool with party_capacity
+        also releases the moved queues' parties into a party image (Engine.export_parties; its other parties step aside
+        around the export and come back with their numbers): the JSON gains "party_players" (per member in image order
+        its id and document) and "party_image" (the party image's length in bytes), and the party image goes between the
+        JSON and the queue image.  Reroute the groups' deliveries to the new owner before the call: a delivery staged
+        after it stays here."""
         self.flush()
         if hasattr(self.engine, "results_wait"):
             self.engine.results_wait()
@@ -731,8 +765,20 @@ class SearchPool:
         for g in group_names:
             for m in modes:
                 mask[m, self.group_names.index(g)] = True
-        from .engine import read_image
-        image = np.ascontiguousarray(self.engine.export_queues(mask), np.uint8)
+        from .engine import read_image, read_party_image
+        pimage = None
+        if self.party_capacity:  # mm_export_queues refuses while a party is queued: the others go back with their numbers
+            pimage = np.ascontiguousarray(self.engine.export_parties(mask), np.uint8)
+            rest = np.ascontiguousarray(self.engine.export_parties(~mask), np.uint8)
+            try:
+                image = np.ascontiguousarray(self.engine.export_queues(mask), np.uint8)
+            except Exception:
+                self.engine.merge_parties(rest, keep_seq=True)
+                self.engine.merge_parties(pimage)
+                raise
+            self.engine.merge_parties(rest, keep_seq=True)
+        else:
+            image = np.ascontiguousarray(self.engine.export_queues(mask), np.uint8)
         _h, cols = read_image(image)
         t = self.clock()
         moved = []
@@ -745,6 +791,16 @@ class SearchPool:
             self.handles.release(pid)
         state = {"mode_names": self.mode_names, "group_names": self.group_names, "players": moved,
                  "now_ms": self.now_ms(), "wall": self.wall_clock()}
+        if pimage is not None:  # per party member in image order its id and document; the party image before the queue's
+            members = []
+            for h in read_party_image(pimage)[1]["id"].tolist():
+                pid = self.handles.id_of[h]
+                self.party_of.pop(h, None)
+                members.append([pid, self.players.pop(h)])
+                self.handles.release(pid)
+            state["party_players"] = members
+            state["party_image"] = len(pimage)
+            image = np.concatenate([pimage, image])
         doc = json.dumps(state).encode()
         return self.MOVE_MAGIC + len(doc).to_bytes(8, "little") + doc + image.tobytes()
 
@@ -753,8 +809,11 @@ class SearchPool:
         column is rewritten), its enqueue stamp is shifted into this pool's clock (bridged by the wall time, as in
         resume(), so waits and the timeout count the time in the old pool), the engine merges the image
         (Engine.merge_queues), and the documents of players it rejects (already queued here) are dropped.  Staged
-        deliveries are ingested first.  -> players merged.  ValueError if the mode or group names differ, or if this
-        pool's handle range cannot hold the players."""
+        deliveries are ingested first.  Moved parties merge after the solos (Engine.merge_parties, new numbers here);
+        this pool's own parties step aside around the queue merge and come back, renumbered in their order when the
+        queue image took numbers.  -> players merged (solos).  ValueError, before anything changes, if the mode or
+        group names differ, if this pool's handle range cannot hold the players, or if the move carries parties and
+        this pool's party table or hashed active set cannot hold them."""
         head = len(self.MOVE_MAGIC)
         if bytes(blob[:head]) != self.MOVE_MAGIC:
             raise ValueError("not a SearchPool queue move")
@@ -762,31 +821,57 @@ class SearchPool:
         state = json.loads(bytes(blob[head + 8:head + 8 + n]))
         if state["mode_names"] != self.mode_names or state["group_names"] != self.group_names:
             raise ValueError("the queues were moved out of a pool with other mode or group names")
+        k = int(state.get("party_image", 0))
+        if k and not self.party_capacity:
+            raise ValueError("the move carries parties: this pool has no party_capacity")
         self.flush()
-        from .engine import read_image
+        from .engine import read_image, read_party_image
         image = np.frombuffer(bytes(blob[head + 8 + n:]), np.uint8).copy()
+        pimage, image = image[:k], image[k:]
         _h, cols = read_image(image)
         players = state["players"]
+        party_players = state.get("party_players", [])
+        if k:  # the parties merge after the solos: their room is checked before anything changes
+            from .engine import active_set_limit
+            queued = int(self.engine.party_read()["size"].sum(dtype=np.int64))
+            if queued + len(party_players) > self.party_capacity:
+                raise ValueError(f"this pool's party table holds {self.party_capacity} members: {queued} queued, "
+                                 f"{len(party_players)} moved")
+            limit = active_set_limit(self.engine.cfg)
+            if limit is not None and self.engine.active_size() + len(players) + len(party_players) > limit:
+                raise ValueError("this pool's active set cannot hold the moved players and parties")
         handles, fresh = [], []
-        for pid, _doc, _age in players:
+        for pid, *_rest in players + party_players:
             h, is_new = self.handles.acquire(pid)
             if h is None:
                 for p in fresh:
-                    self.handles.release(p)
+                    if p is not None:
+                        self.handles.release(p)
                 raise ValueError("this pool's handle range cannot hold the moved players")
             handles.append(h)
             fresh.append(pid if is_new else None)
         fresh_ids = [p for p in fresh if p is not None]
+        handles, phandles = handles[:len(players)], handles[len(players):]
+        fresh, pfresh = fresh[:len(players)], fresh[len(players):]
         cols["id"][:] = np.asarray(handles, cols["id"].dtype)
         down = max(0.0, self.wall_clock() - state["wall"])
         shift = (self.now_ms() - int(round(down * 1000.0)) - int(state["now_ms"])) & 0xFFFFFFFF
         cols["enq_ts"][:] = (cols["enq_ts"].astype(np.uint64) + np.uint64(shift)).astype(np.uint32)
+        if k:  # the party columns get the same handles and clock
+            _ph, pcols = read_party_image(pimage)
+            pcols["id"][:] = np.asarray(phandles, pcols["id"].dtype)
+            pcols["enq_ts"][:] = (pcols["enq_ts"].astype(np.uint64) + np.uint64(shift)).astype(np.uint32)
+        own = None
+        if self.party_capacity:  # mm_merge refuses while a party is queued here: ours step aside and come back
+            own = np.ascontiguousarray(self.engine.export_parties(), np.uint8)
         seq0 = self.engine.seq_next() if hasattr(self.engine, "seq_next") else None
         try:
             rejected = set(self.engine.merge_queues(image).tolist())
         except Exception:
             for p in fresh_ids:
                 self.handles.release(p)
+            if own is not None:
+                self.engine.merge_parties(own, keep_seq=True)
             raise
         t = self.clock() - down
         hdr = _h.config
@@ -813,6 +898,27 @@ class SearchPool:
             merged += 1
         if self.window:  # oldest first: the window reads the first entry
             self.enqueued_at = dict(sorted(self.enqueued_at.items(), key=lambda kv: kv[1]))
+        # the solos are recorded: ours come back (with their numbers when the queue image took none, else renumbered in
+        # their order), then the moved parties, whose room was checked above
+        if own is not None:
+            self.engine.merge_parties(own, keep_seq=self.engine.seq_next() == seq0)
+        if k:
+            try:
+                codes = self.engine.merge_parties(pimage)
+            except Exception:
+                codes = np.zeros(len(pcols["size"]), np.uint8)
+                raise
+            finally:
+                at = 0
+                for c, size in zip(codes.tolist(), pcols["size"].tolist()):
+                    hs = phandles[at:at + size]
+                    for i in range(at, at + size):
+                        if c == 1:
+                            self.players[phandles[i]] = party_players[i][1]
+                            self.party_of[phandles[i]] = tuple(hs)
+                        elif pfresh[i] is not None and phandles[i] not in self.players:
+                            self.handles.release(pfresh[i])
+                    at += size
         return merged
 
     def _teams_of(self, mode):

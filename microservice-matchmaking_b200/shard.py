@@ -323,23 +323,60 @@ def _status(x):
     return int(np.asarray(x).view(np.int64).reshape(-1)[0])
 
 
-def can_take(cfg, engine, g, n):
-    """Would a merge of n players of group g into `engine` pass mm_merge's checks?  No live player in any of the
-    group's queues, n more pool slots within the capacity (the slots in use count dead ones until the next tick), and
-    for a hashed active set n more entries within its 3/4 load.  Conservative: rejected ids would need no room."""
+def _party_members(engine, g=None):
+    """Members of the parties queued in `engine` (of group g only, unless None); 0 for an engine without parties."""
+    if not getattr(engine, "party_capacity", 0):
+        return 0
+    pr = engine.party_read()
+    return int(pr["size"][pr["group"] == g].sum() if g is not None else pr["size"].sum())
+
+
+def can_take(cfg, engine, g, n, n_party=0):
+    """Would a merge of n players and n_party party members of group g into `engine` pass mm_merge's and
+    mm_merge_parties' checks?  No live player in any of the group's queues, n more pool slots within the capacity (the
+    slots in use count dead ones until the next tick), n_party more members within the party capacity, and for a
+    hashed active set n + n_party more entries within its 3/4 load.  Conservative: rejected ids would need no room."""
     if int(engine.queue_stats(0)["n_waiting"].reshape(cfg.n_modes, cfg.n_groups)[:, g].sum()):
         return False
     if engine.pool_size() + n > engine.cfg.capacity:
         return False
-    flags = int(engine.cfg.flags)
-    if not flags & 1 and not flags & 2:  # hashed active set (neither MM_F_NO_DEDUPE nor MM_F_DENSE_IDS): mm_create's size
-        want = engine.cfg.active_capacity or 2 * engine.cfg.capacity
-        h = 1024
-        while h * 3 < want * 4 + 64:
-            h <<= 1
-        if (engine.active_size() + n) * 4 > h * 3:
-            return False
+    if n_party and _party_members(engine) + n_party > getattr(engine, "party_capacity", 0):
+        return False
+    from .engine import active_set_limit
+    limit = active_set_limit(engine.cfg)  # a hashed active set: its 3/4 load
+    if limit is not None and engine.active_size() + n + n_party > limit:
+        return False
     return True
+
+
+def _merge_with_parties(engine, img, pimg=None):
+    """merge_queues(img) into an engine that may hold parties: mm_merge refuses while a party is queued, so the
+    engine's own parties step aside (export_parties) and come back, with their numbers when the queue image took
+    none (else renumbered in their order); then the party image pimg merges if the queue image went in.  Every step
+    is caught.  -> (True if img merged, [party images that did not go back in])"""
+    own, left = None, []
+    if getattr(engine, "party_capacity", 0):
+        try:
+            own = np.ascontiguousarray(engine.export_parties(), np.uint8)
+            seq0 = engine.seq_next()
+        except Exception:  # a refused export changes nothing
+            return False, []
+    try:
+        engine.merge_queues(img)
+        ok = True
+    except Exception:
+        ok = False
+    if own is not None:
+        try:
+            engine.merge_parties(own, keep_seq=engine.seq_next() == seq0)
+        except Exception:
+            left.append(own)
+    if ok and pimg is not None:
+        try:
+            engine.merge_parties(pimg)
+        except Exception:
+            left.append(pimg)
+    return ok, left
 
 
 def move_queues(pkg, cfg, old, new, rank, engine, comm):
@@ -349,16 +386,26 @@ def move_queues(pkg, cfg, old, new, rank, engine, comm):
     One move, all messages int64 arrays:
 
       1. source -> target: [n], the group's live players here (mm_queue_stats), or [-1] if they cannot be counted;
-      2. target -> source: [0] if it can take them (can_take: no live player of the group, room in the pool and the
-         active set), else [1] — the source has released nothing yet, so a refusal here changes nothing;
+         [n, m] when m members of the group's queued parties go along;
+      2. target -> source: [0] if it can take them (can_take: no live player of the group, room in the pool, the party
+         table and the active set), else [1] — the source has released nothing yet, so a refusal here changes nothing;
       3. source -> target: the queue image (Engine.export_queues: the players are released in the same call) as one
-         int64 array (an image is a multiple of 8 bytes and at least its 624-byte header), or [-1] if the export failed;
+         int64 array (an image is a multiple of 8 bytes and at least its 624-byte header), or [-1] if the export failed.
+         With parties, the group's party image (Engine.export_parties) follows the queue image in the same array;
       4. target -> source: [0] if Engine.merge_queues took it, else [1].
 
-    If step 4 fails anyway (a CUDA error, an active set that filled in between), the source merges the image back.
-    Should that fail too (the released players' dead slots still count in the source's pool until its next tick), the
-    image is kept in `stranded` instead of being lost: merge it into the source (Engine.merge_queues) after its next
-    tick.  -> dict(moved=[groups], failed=[groups], stranded={group: image}) as seen by this rank.
+    mm_export_queues and mm_merge refuse while a party is queued, so an engine with parties releases the others around
+    them (export_parties) and merges them back (merge_parties: with their numbers where the sequence did not move).
+    The target merges the moved parties after the solos.
+
+    Every engine call of a move is caught, so the peer always gets its next message.  If step 4 fails anyway (a CUDA
+    error, an active set that filled in between), the source merges the image back, and the party image (new numbers
+    there).  Should that fail too (the released players' dead slots still count in the source's pool until its next
+    tick), the image is kept in `stranded` instead of being lost: merge it into the source (Engine.merge_queues) after
+    its next tick.  With parties, stranded[g] is a tuple of the images this rank could not put back: queue images
+    (magic MM_QUEUE_IMAGE_MAGIC) go to Engine.merge_queues, party images (MM_PARTY_IMAGE_MAGIC) to Engine.merge_parties
+    — on the target, a moved party image that did not merge after its solos did, or the target's own parties.
+    -> dict(moved=[groups], failed=[groups], stranded={group: image or tuple of images}) as seen by this rank.
 
     Routing is the caller's job: new deliveries of a moved group must go to its new owner (route(..., owners=new))
     on every rank from the move on, and those of a failed move to the old one."""
@@ -371,43 +418,62 @@ def move_queues(pkg, cfg, old, new, rank, engine, comm):
         if rank == src:
             try:
                 n = int(engine.queue_stats(0)["n_waiting"].reshape(cfg.n_modes, cfg.n_groups)[:, g].sum())
+                m = _party_members(engine, g)
             except Exception:
-                n = -1
-            comm.send(src, dst, (np.array([n], np.int64),))
+                n, m = -1, 0
+            comm.send(src, dst, (np.array([n, m] if m else [n], np.int64),))
             (reply,) = comm.recv(dst, src)
             ok = n >= 0 and _status(reply) == 0
+            left = []  # images that could not go back into this engine
             if ok:
                 mask = np.zeros((cfg.n_modes, cfg.n_groups), bool)
                 mask[:, g] = True
+                pimg = rest = img = None
                 try:  # a refused export (e.g. a staged packed batch) changes nothing; the target still gets a message
+                    if getattr(engine, "party_capacity", 0):
+                        pimg = np.ascontiguousarray(engine.export_parties(mask), np.uint8)
+                        rest = np.ascontiguousarray(engine.export_parties(~mask), np.uint8)
                     img = np.ascontiguousarray(engine.export_queues(mask), np.uint8)
                 except Exception:
                     img = None
-                comm.send(src, dst, (img.view(np.int64) if img is not None else np.array([-1], np.int64),))
+                for b, keep in ((rest, True), (pimg if img is None else None, False)):
+                    if b is not None:
+                        try:
+                            engine.merge_parties(b, keep_seq=keep)
+                        except Exception:
+                            left.append(b)
+                if img is None:
+                    pimg = None
+                msg = np.array([-1], np.int64)
+                if img is not None:
+                    msg = img.view(np.int64) if pimg is None else np.concatenate([img, pimg]).view(np.int64)
+                comm.send(src, dst, (msg,))
                 (status,) = comm.recv(dst, src)
                 ok = img is not None and _status(status) == 0
-                if img is not None and not ok:  # the group's queues hold only dead slots here now: the image goes back
-                    try:
-                        engine.merge_queues(img)
-                    except pkg.EngineError:
-                        out["stranded"][g] = img
+                if img is not None and not ok:  # the group's queues hold only dead slots here now: the images go back
+                    back, rest_left = _merge_with_parties(engine, img, pimg)
+                    left += rest_left if back else [img] + ([pimg] if pimg is not None else []) + rest_left
+            if left:
+                out["stranded"][g] = left[0] if len(left) == 1 and left[0] is img else tuple(left)
         else:
             (prop,) = comm.recv(src, dst)
             n = _status(prop)
+            n_party = int(np.asarray(prop).reshape(-1)[1]) if np.asarray(prop).size > 1 else 0
             try:
-                ok = n >= 0 and can_take(cfg, engine, g, n)
+                ok = n >= 0 and can_take(cfg, engine, g, n, n_party)
             except Exception:
                 ok = False
             comm.send(dst, src, (np.array([0 if ok else 1], np.int64),))
             if ok:
                 (arr,) = comm.recv(src, dst)
-                arr = np.ascontiguousarray(arr)
-                ok = len(arr) > 1
+                arr = np.ascontiguousarray(arr).view(np.uint8)
+                ok = len(arr) > 8
                 if ok:
-                    try:
-                        engine.merge_queues(arr.view(np.uint8))
-                    except Exception:
-                        ok = False
+                    q = int(arr[16:24].view(np.uint64)[0])  # the queue image's total_bytes; its party image follows
+                    img, pimg = arr[:q], (arr[q:] if len(arr) > q else None)
+                    ok, left = _merge_with_parties(engine, img, pimg)
+                    if left:  # taken: what did not merge here is kept (the source has released it)
+                        out["stranded"][g] = tuple(left)
                 comm.send(dst, src, (np.array([0 if ok else 1], np.int64),))
         out["moved" if ok else "failed"].append(g)
     return out
