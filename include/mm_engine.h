@@ -432,8 +432,13 @@ typedef struct mm_party_stats {
  * in enqueue order, then the solos, which fill the open slots of team 0, then team 1, ... in C's order.  Lobbies are
  * ordered by (mode, group, emission within the queue), group = the queue's group.  Solos taken leave the pool exactly
  * as mm_take takes them; matched party members stay in the active set as matched players (mm_locate state 2,
- * mm_requeue code 1: back as a solo).  team_balance does not split party lobbies; the last tick's results,
- * mm_match_quality, the lobby budget and pending async_results copies are left alone.
+ * mm_requeue code 1: back as a solo, with its own rating and the party's seq).  The members of a party share that one
+ * seq, so mm_requeue takes at most one of them per call (two are not in strict age order: MM_E_ARG) and refuses a
+ * member whose partition holds a co-member requeued earlier (the seq of a live player there: MM_E_ARG); a member whose
+ * rating maps to another partition is requeued.  Only R needs a group, so a member whose own rating has none cannot be
+ * requeued (MM_E_ARG).  To put a whole party back, enqueue it again with mm_enqueue_party.  team_balance does not
+ * split party lobbies; the last tick's results, mm_match_quality, the lobby budget and pending async_results copies
+ * are left alone.
  * Refusals, all decided before anything changes (mm_last_error names the cause): MM_E_ARG the rule checks of mm_widen,
  * a served mode of more than 256 teams, an MM_ORDER_ARRIVAL engine; MM_E_STATE no party capacity, an MM_F_NO_DEDUPE
  * engine, a staged packed batch; MM_E_CAP lobby_cap or member_cap too small (stats holds the counts and nothing is

@@ -11,7 +11,8 @@ namespace mm {
 // while an enqueue batch is being resolved, (pool_generation << 32 | pool_slot) once the player is queued.
 // Generations are 31-bit (kGenMask), so a committed value is always below PENDING.  Generation 0 is never a pool's:
 // (0 << 32 | row) = kPtVal(row) is a member of the queued party in that row of the party table (mm_party.cuh), and
-// kPtMatched (generation kGenMask, slot 0xFFFFFFFF, past every pool) a matched party member.  Every pool-side test
+// kPtMatched (generation kGenMask, slot 0xFFFFFFFF, past every pool) a matched party member, and any matched or taken
+// player an image load put in the set.  Every pool-side test
 // (generation == gen, slot < slots, id at the slot) reads both as "not a live pool slot".
 //
 // Ingest of one chunk of a batch = claim -> [count, scan, cut: only when the batch could overflow the pool]

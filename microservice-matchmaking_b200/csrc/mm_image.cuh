@@ -10,8 +10,9 @@
 // Import: the layout is the engine's own (same config), so the host lays out every partition on consecutive chunks
 // from the partition counts; k_img_load writes the columns into their slots, derives the sort key and team size,
 // builds the bin totals and chunk histograms, and checks every player.  k_img_insert puts the ids of both sections
-// into the active set (duplicate check) with the "not queued" value 0 — no generation is 0, so the entry never
-// matches a slot — and k_restamp then points the queued players' entries at their slots.  A failed check sets a bit
+// into the active set (duplicate check) with the "not queued" value kPtMatched — a slot past every pool, so the entry
+// never matches a slot, and not generation 0, which names a queued party's row — and k_restamp then points the queued
+// players' entries at their slots.  A failed check sets a bit
 // of one error word; the host then clears the engine.
 //
 // Queue move (mm_export_queues / mm_merge): the export passes with a partition selection; the merge kernels at the
@@ -208,15 +209,15 @@ __global__ void __launch_bounds__(256) k_img_load(const ImgLoadArgs a) {
   }
 }
 
-// Ids of an image section into an empty active set with value 0 ("active, not queued"); a second copy of an id — in
-// the same section or the other — sets kImgDup.
+// Ids of an image section into an empty active set with value kPtMatched ("active, not queued"); a second copy of an
+// id — in the same section or the other — sets kImgDup.
 __global__ void k_img_insert(const void* ids, uint32_t id_bytes, uint32_t n, uint64_t id_limit, ActiveView act,
                              uint32_t* __restrict__ err) {
   for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
     const uint64_t pid = id_bytes == 8 ? static_cast<const uint64_t*>(ids)[i] : static_cast<const uint32_t*>(ids)[i];
     if (pid >= id_limit) { atomicOr(err, kImgBadId); continue; }
     if (act.dcap) {
-      if (atomicCAS(act.val(pid), kFreeVal, 0ull) != kFreeVal) atomicOr(err, kImgDup);
+      if (atomicCAS(act.val(pid), kFreeVal, (unsigned long long)kPtMatched) != kFreeVal) atomicOr(err, kImgDup);
       continue;
     }
     uint64_t h = hash64(pid) & act.mask;
@@ -225,7 +226,7 @@ __global__ void k_img_insert(const void* ids, uint32_t id_bytes, uint32_t n, uin
       unsigned long long k = *act.key(h);
       if (k == kEmptyKey) {
         k = atomicCAS(act.key(h), kEmptyKey, (unsigned long long)pid);
-        if (k == kEmptyKey) { *act.val(h) = 0ull; placed = true; break; }
+        if (k == kEmptyKey) { *act.val(h) = kPtMatched; placed = true; break; }
       }
       if (k == pid) { atomicOr(err, kImgDup); placed = true; break; }
       h = (h + 1) & act.mask;

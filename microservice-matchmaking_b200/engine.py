@@ -353,12 +353,14 @@ class Engine:
         """Put players of a lobby that did not start back into their queue at their enqueue position (mm_requeue).
         The columns are what each player had when it was queued (enq_ts may be None).  The entries may come in any
         order: they are sorted by age here.  -> codes u8[n] in the caller's order: 1 requeued, 0 still queued,
-        4 not in the active set (the player left)."""
+        4 not in the active set (the player left).  The members of a matched party share the party's seq: at most one
+        of them per call, not one whose partition already holds a co-member requeued earlier, and not one whose own
+        rating has no group (each MM_E_ARG)."""
         ids = np.ascontiguousarray(ids, np.uint64)
         n = len(ids)
         seq = np.ascontiguousarray(seq, np.uint32)
         assert len(rating) == n and len(mode) == n and len(seq) == n
-        order = np.argsort((seq - np.uint32(self.seq_next())).astype(np.uint32))  # numbers are unique: no tie to keep
+        order = np.argsort((seq - np.uint32(self.seq_next())).astype(np.uint32))  # a tie is refused: no order to keep
         cols = [np.ascontiguousarray(np.asarray(a)[order], dt) for a, dt in
                 ((ids, np.uint64), (rating, np.int32), (mode, np.uint8), (seq, np.uint32))]
         ts = None if enq_ts is None else np.ascontiguousarray(np.asarray(enq_ts)[order], np.uint32)
