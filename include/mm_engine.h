@@ -436,7 +436,7 @@ typedef struct mm_party_stats {
  * seq, so mm_requeue takes at most one of them per call (two are not in strict age order: MM_E_ARG) and refuses a
  * member whose partition holds a co-member requeued earlier (the seq of a live player there: MM_E_ARG); a member whose
  * rating maps to another partition is requeued.  Only R needs a group, so a member whose own rating has none cannot be
- * requeued (MM_E_ARG).  To put a whole party back, enqueue it again with mm_enqueue_party.  team_balance does not
+ * requeued (MM_E_ARG).  To put a whole party back at its age position, use mm_requeue_party.  team_balance does not
  * split party lobbies; the last tick's results, mm_match_quality, the lobby budget and pending async_results copies
  * are left alone.
  * Refusals, all decided before anything changes (mm_last_error names the cause): MM_E_ARG the rule checks of mm_widen,
@@ -498,6 +498,41 @@ int mm_party_read(mm_engine* e, uint32_t party_cap, uint32_t member_cap, uint8_t
 int mm_export_parties(mm_engine* e, const uint8_t* queues, void* buf, uint64_t cap, uint64_t* n_bytes);
 int mm_merge_parties(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t flags, uint8_t* code,
                      uint32_t* n_merged);
+
+/* mm_requeue_party: the parties of a party lobby that did not start (a declined ready check, no free game server) go
+ * back into the party table as parties, at the position their enqueue sequence numbers give them, as mm_requeue does for
+ * solos.  Arguments as mm_enqueue_party: party j's members are the next size[j] entries of ids / rating (handles on
+ * MM_F_DENSE_IDS engines), plus what the party had when it was queued: enq_ts (may be NULL: 0) and seq.  R =
+ * floor(sum / size) and its group mm_group_of(R), as at enqueue; a caller may pass only the members still willing,
+ * which makes a smaller party with R from those members.  Parties are in AGE ORDER: (seq[j] - seq_next) mod 2^32
+ * strictly ascending.  codes[j] (may be NULL), in this order:
+ *   0  a member is queued (a live solo, or a member of a queued party): nothing changes for this party;
+ *   4  otherwise, a member is not in the active set (removed, expired, moved out, never queued): not requeued;
+ *   1  otherwise (every member active and matched: by a tick, mm_party_match, mm_widen, mm_backfill, mm_band_match,
+ *      mm_take or the matched section of an image load): the party gets a row among the queued parties at its age
+ *      position, with its seq, enq_ts, mode, R, group and its members in the order given.  mm_in_queue reads 1,
+ *      mm_locate reports state 3 with the wait counted from enq_ts; mm_active_size and seq_next do not change; the next
+ *      mm_party_match treats the row like any other queued party.
+ * *n_requeued (may be NULL) = the code-1 parties.  n = 0 does nothing.  The engine trusts the columns, as mm_requeue
+ * does.  The solo pool, the last tick's results, mm_match_quality, the match section of mm_queue_stats, the lobby
+ * budget, the snapshot, the mm_enqueue_rejects list and pending async_results copies are left alone.  The call inserts
+ * no key into a hashed active set.  Cost: one pass over the party table plus the call's members.
+ * Refusals, all decided before anything changes (mm_last_error names the cause):
+ *   MM_E_ARG   an MM_ORDER_ARRIVAL engine; null pointers with n > 0; a mode >= n_modes; a size < 2 or above the mode's
+ *              team_size; an id out of range; an id given twice anywhere in the call; an R without a group; parties not
+ *              in strict age order; a seq equal to seq_next; a code-1 party whose seq is that of a queued party;
+ *   MM_E_STATE no party capacity, an MM_F_NO_DEDUPE engine, a staged packed batch;
+ *   MM_E_CAP   the code-1 parties' members exceed party_capacity minus the party members queued now (exact: a table
+ *              with exactly enough room takes them).
+ *
+ * EQUIVALENCE.  Take mm_export_parties(NULL) and then mm_export of the engine just before the call; insert the code-1
+ * parties into the party image at their sequence position and remove their member ids from section 7 of the engine
+ * image.  A fresh engine that mm_import's the engine image and then mm_merge_parties(MM_PARTY_KEEP_SEQ) the party image
+ * gives the same results as this engine for every later call sequence, except what mm_import itself changes (dead
+ * slots, the next tick's pool_before and n_dead, mm_queue_stats' n_removed).                                        */
+int mm_requeue_party(mm_engine* e, uint32_t n_parties, const uint8_t* size, const uint64_t* ids, const int32_t* rating,
+                     const uint8_t* mode, const uint32_t* enq_ts, const uint32_t* seq, uint8_t* codes,
+                     uint32_t* n_requeued);
 
 /* Replaces ActiveUser.in_queue?/1 (models/active_user.ex:33-44), batched.          */
 int mm_in_queue(mm_engine* e, uint32_t n, const uint64_t* id, uint8_t* out);

@@ -557,6 +557,63 @@ static ERL_NIF_TERM nif_enqueue_party(ErlNifEnv* env, int argc, const ERL_NIF_TE
   return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &out));
 }
 
+/* requeue_party(ref, sizes :: binary(u8[]), handles :: binary(u32[]), ratings :: binary(i32[]), modes :: binary(u8[]),
+ * enq_ts :: binary(u32[]), seq :: binary(u32[])) -> {:ok, codes :: binary(u8[])} (1 requeued, 0 a member still
+ * queued, 4 a member gone; in the caller's order): the parties of a lobby that did not start go back into the party
+ * table at their age position (mm_requeue_party).  Party j's members are the next sizes[j] handles and ratings; the
+ * parties are sorted by age here.  badarg unless the sizes add up to the handles and ratings and every per-party
+ * binary has one entry per party. */
+static ERL_NIF_TERM nif_requeue_party(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary sb, hb, rtb, mb, tb, qb, codes; uint32_t got = 0, seq_next = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &sb) ||
+      !enif_inspect_binary(env, argv[2], &hb) || !enif_inspect_binary(env, argv[3], &rtb) ||
+      !enif_inspect_binary(env, argv[4], &mb) || !enif_inspect_binary(env, argv[5], &tb) ||
+      !enif_inspect_binary(env, argv[6], &qb))
+    return enif_make_badarg(env);
+  const size_t n = sb.size;
+  size_t m = 0;
+  for (size_t j = 0; j < n; ++j) m += sb.data[j];
+  if (hb.size != 4 * m || rtb.size != 4 * m || mb.size != n || tb.size != 4 * n || qb.size != 4 * n)
+    return enif_make_badarg(env);
+  if (!enif_alloc_binary(n, &codes)) return err(env, MM_E_CAP);
+  if (n == 0) return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &codes));
+  uint32_t* key = enif_alloc(n * 8);  /* (age, index) pairs */
+  uint32_t* off = enif_alloc(n * 4);  /* first member of party i in the caller's order */
+  uint8_t *size = enif_alloc(n), *mode = enif_alloc(n), *out = enif_alloc(n);
+  uint32_t *stamp = enif_alloc(n * 4), *seq = enif_alloc(n * 4);
+  uint64_t* id = enif_alloc(m * 8 + 8);
+  int32_t* rating = enif_alloc(m * 4 + 4);
+  int rc = MM_E_CAP;
+  if (key && off && size && mode && out && stamp && seq && id && rating && !(rc = mm_seq_next(r->e, &seq_next))) {
+    for (size_t i = 0, o = 0; i < n; o += sb.data[i], ++i) {
+      uint32_t q;
+      memcpy(&q, qb.data + 4 * i, 4);
+      key[2 * i] = q - seq_next;
+      key[2 * i + 1] = (uint32_t)i;
+      off[i] = (uint32_t)o;
+    }
+    qsort(key, n, 8, rq_cmp);
+    for (size_t k = 0, o = 0; k < n; ++k) {
+      const uint32_t i = key[2 * k + 1];
+      size[k] = sb.data[i]; mode[k] = mb.data[i];
+      memcpy(&stamp[k], tb.data + 4 * i, 4); memcpy(&seq[k], qb.data + 4 * i, 4);
+      for (uint32_t x = 0; x < size[k]; ++x, ++o) {
+        uint32_t h;
+        memcpy(&h, hb.data + 4 * ((size_t)off[i] + x), 4); id[o] = h;
+        memcpy(&rating[o], rtb.data + 4 * ((size_t)off[i] + x), 4);
+      }
+    }
+    rc = mm_requeue_party(r->e, (uint32_t)n, size, id, rating, mode, stamp, seq, out, &got);
+    if (!rc)
+      for (size_t k = 0; k < n; ++k) codes.data[key[2 * k + 1]] = out[k];
+  }
+  enif_free(key); enif_free(off); enif_free(size); enif_free(mode); enif_free(out); enif_free(stamp); enif_free(seq);
+  enif_free(id); enif_free(rating);
+  if (rc) { enif_release_binary(&codes); return err(env, rc); }
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &codes));
+}
+
 /* party_match(ref, now :: u64, rules :: binary(mm_widen_rule[n_modes * n_groups]))
  *   -> {:ok, lobbies :: binary(mm_lobby_hdr[]), handles :: binary(u32[])}: lobbies around the parties that waited
  * longest, each party whole on one team (mm_party_match).  badarg unless the binary holds exactly one rule per (mode,
@@ -712,6 +769,7 @@ static ErlNifFunc funcs[] = {
   {"import_regroup", 2, nif_import_regroup, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"import_regroup_many", 4, nif_import_regroup_many, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"requeue_party", 7, nif_requeue_party, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"backfill", 2, nif_backfill, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"widen", 3, nif_widen, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"enqueue_party", 6, nif_enqueue_party, ERL_NIF_DIRTY_JOB_CPU_BOUND},

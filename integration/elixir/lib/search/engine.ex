@@ -157,6 +157,13 @@ defmodule Matchmaking.Search.Engine do
   solos.  The solos leave the pool and every member stays in the active set until remove_user.
   """
   def party_match(_ref, _now, _rules), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Parties (extension): the parties of a lobby that did not start go back into the party table as parties, at their age
+  position (mm_requeue_party).  Party j's members are the next sizes[j] handles and ratings; modes, enq_ts and seq per
+  party, what it had when it was queued -> {:ok, codes :: binary(u8[])}: 1 requeued, 0 a member still queued, 4 a
+  member gone.
+  """
+  def requeue_party(_ref, _sizes, _handles, _ratings, _modes, _enq_ts, _seq), do: :erlang.nif_error(:nif_not_loaded)
   @doc "Parties (extension): how many party members the engine holds (mm_set_option(\"party_capacity\"))."
   def set_party_capacity(_ref, _members), do: :erlang.nif_error(:nif_not_loaded)
   @doc """

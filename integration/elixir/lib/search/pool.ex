@@ -28,6 +28,14 @@ defmodule Matchmaking.Search.Pool do
                      of its window go to the first team with room, the nearest solos fill the rest; a party plays on
                      one team.  Parties arrive through stage_party/3, one delivery per party, acked or nacked as one
       party_capacity option (extension, default 0): how many party members the engine holds (Engine.set_party_capacity)
+      requeue_parties option (extension, default false): requeue/1 puts matched parties back as parties at their age
+                     position (Engine.requeue_party).  The pool keeps a book of every queued party (members, ratings,
+                     mode, stamp, seq) and moves it aside when party_match places the party; two or more members of one
+                     matched party go back as one party, a lone member as a solo with the party's seq.  The parties
+                     go first; if the engine refuses them (the party table is full) they answer :gone and the solos go
+                     on.  A lone member whose co-member went back the same way and is still queued in the same queue
+                     answers :gone (one player of a party number per partition).  Off, requeue/1 answers a matched
+                     party member :gone
       balance_teams  option (extension, default nil = off): a list of mode names.  Every lobby of those modes, from the
                      tick and from widen, is split into the two teams with the least rating difference
                      (Engine.set_team_balance); the lobby's players are the same, only who plays with whom changes
@@ -136,7 +144,9 @@ defmodule Matchmaking.Search.Pool do
            t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms),
            lobby_budget: Keyword.get(opts, :lobby_budget), paused: MapSet.new(), regroup_dropped: [],
            widen: Keyword.get(opts, :widen), parties: Keyword.get(opts, :parties), staged_parties: [], party_of: %{},
-           party_capacity: Keyword.get(opts, :party_capacity), stranded_parties: []}
+           party_capacity: Keyword.get(opts, :party_capacity), stranded_parties: [],
+           # requeue_parties: handle -> {members, ratings, mode, enq_ts, seq} of its queued (party_book) or matched party
+           requeue_parties: Keyword.get(opts, :requeue_parties, false), party_book: %{}, matched_parties: %{}}
     case resume(st, Keyword.get(opts, :resume), Keyword.get(opts, :regroup, false)) do
       {:ok, st} ->
         Process.send_after(self(), :flush, @flush_ms)
@@ -167,7 +177,9 @@ defmodule Matchmaking.Search.Pool do
         # now_ms/1 goes on from the checkpoint's value plus the downtime: the engine's enqueue stamps stay valid
         st = %{st | handle_of: ck.handle_of, players: ck.players, free: ck.free, next: ck.next,
                     queued: Map.get(ck, :queued, %{}), moved_out: Map.get(ck, :moved_out, MapSet.new()),
-                    party_of: Map.get(ck, :party_of, %{}), t0: System.monotonic_time(:millisecond) - ck.now_ms - down}
+                    party_of: Map.get(ck, :party_of, %{}), party_book: Map.get(ck, :party_book, %{}),
+                    matched_parties: Map.get(ck, :matched_parties, %{}),
+                    t0: System.monotonic_time(:millisecond) - ck.now_ms - down}
         st = drop_rejected(st, ck.image, rejected)
         case Map.get(ck, :party_image) do
           nil -> {:ok, st}
@@ -177,7 +189,8 @@ defmodule Matchmaking.Search.Pool do
               {:ok, Enum.reduce(gone, st, fn h, acc ->
                  {player, players} = Map.pop(acc.players, h)
                  %{acc | players: players, handle_of: Map.delete(acc.handle_of, player["id"]), free: [h | acc.free],
-                         party_of: Map.delete(acc.party_of, h), regroup_dropped: [player | acc.regroup_dropped]}
+                         party_of: Map.delete(acc.party_of, h), party_book: Map.delete(acc.party_book, h),
+                         regroup_dropped: [player | acc.regroup_dropped]}
                end)}
             end
         end
@@ -201,14 +214,39 @@ defmodule Matchmaking.Search.Pool do
   # steps aside (Engine.export_parties) around `fun` and comes back, with its number when the sequence did not move.
   # -> {result of fun, the party image or nil, st}.  A refused export is fun's error and changes nothing; a party
   # image that cannot come back is kept in st.stranded_parties (merge it with Engine.merge_parties/3).
+  # requeue_parties: the parties of a party image merged without their numbers got s1 + their index (mm_merge_parties);
+  # the merged ones (code 1) get their book entry with that number, from the image's columns
+  defp book_parties(%{requeue_parties: false} = st, _image, _codes, _s1), do: st
+  defp book_parties(st, image, codes, s1) do
+    <<_::binary-size(24), p::little-32, m::little-32, _::binary>> = image
+    a8 = fn x -> Bitwise.band(x + 7, Bitwise.bnot(7)) end
+    ts_off = a8.(a8.(624 + p) + 4 * p)
+    mode_off = a8.(ts_off + 4 * p)
+    rating_off = a8.(a8.(mode_off + p) + 4 * m)
+    ts = for <<t::little-32 <- binary_part(image, ts_off, 4 * p)>>, do: t
+    modes = :binary.bin_to_list(binary_part(image, mode_off, p))
+    ratings = for <<r::little-signed-32 <- binary_part(image, rating_off, 4 * m)>>, do: r
+    {st, _} =
+      party_list(image, codes)
+      |> Enum.zip(Enum.zip([ts, modes, 0..max(p - 1, 0)]))
+      |> Enum.reduce({st, ratings}, fn {{hs, c}, {t, mode, j}}, {acc, left} ->
+        {rat, left} = Enum.split(left, length(hs))
+        rec = {hs, rat, mode, t, Bitwise.band(s1 + j, 0xFFFFFFFF)}
+        acc = if c == 1, do: %{acc | party_book: Enum.reduce(hs, acc.party_book, &Map.put(&2, &1, rec))}, else: acc
+        {acc, left}
+      end)
+    st
+  end
+
   defp around_parties(%{party_capacity: nil} = st, fun), do: {fun.(), nil, st}
   defp around_parties(st, fun) do
     with {:ok, own} <- Engine.export_parties(st.ref, nil),
          {:ok, s0} <- Engine.seq_next(st.ref) do
       res = fun.()
-      keep = match?({:ok, ^s0}, Engine.seq_next(st.ref))
+      {:ok, s1} = Engine.seq_next(st.ref)
+      keep = s1 == s0
       case Engine.merge_parties(st.ref, own, keep) do
-        {:ok, _} -> {res, own, st}
+        {:ok, codes} -> {res, own, if(keep, do: st, else: book_parties(st, own, codes, s1))}
         {:error, _} -> {res, own, %{st | stranded_parties: [own | st.stranded_parties]}}
       end
     else
@@ -292,7 +330,8 @@ defmodule Matchmaking.Search.Pool do
           {player, players} = Map.pop(acc.players, x)
           pid = if x == h, do: id, else: player && player["id"]
           %{acc | handle_of: Map.delete(acc.handle_of, pid), players: players, free: [x | acc.free],
-                  queued: Map.delete(acc.queued, x), party_of: Map.delete(acc.party_of, x)}
+                  queued: Map.delete(acc.queued, x), party_of: Map.delete(acc.party_of, x),
+                  party_book: Map.delete(acc.party_book, x), matched_parties: Map.delete(acc.matched_parties, x)}
         end)
         {:reply, {:ok, :removed}, st}
     end
@@ -305,6 +344,9 @@ defmodule Matchmaking.Search.Pool do
         ck = %{image: image, handle_of: st.handle_of, players: st.players, free: st.free, next: st.next,
                queued: st.queued, moved_out: st.moved_out, now_ms: now_ms(st), wall_ms: System.os_time(:millisecond)}
         ck = if parties, do: Map.merge(ck, %{party_image: parties, party_of: st.party_of}), else: ck
+        # the matched players stay in the engine image: their parties' book goes with them
+        ck = if st.requeue_parties,
+               do: Map.merge(ck, %{party_book: st.party_book, matched_parties: st.matched_parties}), else: ck
         {:reply, {:ok, :erlang.term_to_binary(ck)}, st}
       {{:error, _} = e, _, st} -> {:reply, e, st}
     end
@@ -443,8 +485,10 @@ defmodule Matchmaking.Search.Pool do
     ids = for {h, _, _, _} <- rows, into: <<>>, do: <<h::little-32>>
     image = binary_part(pimg, 0, ts_off) <> ts <> binary_part(pimg, ts_off + 4 * p, id_off - ts_off - 4 * p) <> ids <>
             binary_part(pimg, id_off + byte_size(ids), byte_size(pimg) - id_off - byte_size(ids))
+    {:ok, s1} = Engine.seq_next(st.ref)
     case Engine.merge_parties(st.ref, image, false) do
       {:ok, codes} ->
+        st = book_parties(st, image, codes, s1)
         {st, _} = Enum.reduce(party_list(image, codes), {st, rows}, fn {hs, c}, {acc, left} ->
           {mine, left} = Enum.split(left, length(hs))
           acc = Enum.reduce(mine, acc, fn {h, fresh, id, player}, a ->
@@ -467,10 +511,32 @@ defmodule Matchmaking.Search.Pool do
   # -- requeue (extension): a lobby that did not start ----------------------------------------------------------------
   def handle_call({:requeue, players}, _from, st) do
     st = flush(st)
+    {party_rows, solo_rows} = if st.requeue_parties, do: party_requeue_rows(st, players), else: {[], []}
+    # the parties first: a refused call (the party table is full) changes nothing, and its parties answer :gone
+    pcodes =
+      case (if party_rows == [], do: {:ok, <<>>}, else: requeue_parties(st, party_rows)) do
+        {:ok, pcodes} -> pcodes
+        {:error, _reason} -> :binary.copy(<<4>>, length(party_rows))
+      end
+    whole = for {{_, hs, _, _} = row, c} <- Enum.zip(party_rows, :binary.bin_to_list(pcodes)), {i, h} <- hs,
+              do: {{i, h, row}, c}
+    docs = List.to_tuple(players)
+    # a party requeued whole is a queued party again
+    st = Enum.reduce(Enum.zip(party_rows, :binary.bin_to_list(pcodes)), st, fn
+      {{_, hs, rat, {_, _, mode, ts, seq}}, 1}, acc ->
+        members = for {_, h} <- hs, do: h
+        rec = {members, rat, mode, ts, seq}
+        acc = %{acc | players: Enum.reduce(hs, acc.players, fn {i, h}, a -> Map.put(a, h, elem(docs, i)) end)}
+        Enum.reduce(members, acc, fn h, a ->
+          %{a | matched_parties: Map.delete(a.matched_parties, h), party_of: Map.put(a.party_of, h, members),
+                party_book: Map.put(a.party_book, h, rec)}
+        end)
+      _, acc -> acc
+    end)
     rows = for {p, i} <- Enum.with_index(players), h = Map.get(st.handle_of, p["id"]), h != nil,
                rec = Map.get(st.queued, h), rec != nil, not MapSet.member?(st.moved_out, Engine.queue_of(elem(rec, 0), elem(rec, 1))),
                do: {i, h, rec}
-    rows = Enum.uniq_by(rows, fn {_, h, _} -> h end)
+    rows = Enum.uniq_by(rows ++ solo_rows, fn {_, h, _} -> h end)
     bin = fn f -> for {_, _, rec} <- rows, into: <<>>, do: f.(rec) end
     result =
       if rows == [] do
@@ -482,7 +548,11 @@ defmodule Matchmaking.Search.Pool do
       end
     case result do
       {:ok, codes} ->
-        by_h = Map.new(Enum.zip(rows, :binary.bin_to_list(codes)), fn {{_, h, _}, c} -> {h, c} end)
+        solo = Enum.zip(rows, :binary.bin_to_list(codes))
+        queued_members = for {p, i} <- Enum.with_index(players), h = Map.get(st.handle_of, p["id"]), h != nil,
+                           Map.has_key?(st.party_book, h), not Enum.any?(whole, &match?({{_, ^h, _}, _}, &1)),
+                           do: {{i, h, nil}, 0}
+        by_h = Map.new(solo ++ whole ++ queued_members, fn {{_, h, _}, c} -> {h, c} end)
         outcome = Enum.map(players, fn p ->
           case by_h[Map.get(st.handle_of, p["id"])] do
             1 -> :requeued
@@ -490,12 +560,54 @@ defmodule Matchmaking.Search.Pool do
             _ -> :gone
           end
         end)
-        docs = List.to_tuple(players)
-        back = for {{i, h, _}, 1} <- Enum.zip(rows, :binary.bin_to_list(codes)), into: st.players,
-                 do: {h, elem(docs, i)}
-        {:reply, outcome, %{st | players: back}}
+        back = for {{i, h, _}, 1} <- solo, into: st.players, do: {h, elem(docs, i)}
+        st = %{st | players: back}
+        # a lone member requeued as a solo is a solo from now on
+        st = Enum.reduce(solo, st, fn
+          {{_, h, rec}, 1}, acc when is_map_key(acc.matched_parties, h) ->
+            %{acc | queued: Map.put(acc.queued, h, rec), matched_parties: Map.delete(acc.matched_parties, h)}
+          _, acc -> acc
+        end)
+        {:reply, outcome, st}
       {:error, _} = e -> {:reply, e, st}
     end
+  end
+
+  # requeue_parties: the matched party members among `players`, by party -> {parties (two or more members: {index of
+  # the first, [{index, handle}], ratings, record}), lone members as solo rows {index, handle, {rating, mode, ts, seq}}}
+  defp party_requeue_rows(st, players) do
+    asked = for {p, i} <- Enum.with_index(players), h = Map.get(st.handle_of, p["id"]), h != nil,
+                Map.has_key?(st.matched_parties, h), do: {i, h}
+    asked = Enum.uniq_by(asked, fn {_, h} -> h end)
+    asked
+    |> Enum.group_by(fn {_, h} -> elem(st.matched_parties[h], 4) end)
+    |> Enum.reduce({[], []}, fn {_seq, hs}, {parties, solos} ->
+      {members, ratings, mode, ts, seq} = rec = st.matched_parties[elem(hd(hs), 1)]
+      at = Map.new(hs, fn {i, h} -> {h, i} end)
+      mine = for {h, r} <- Enum.zip(members, ratings), Map.has_key?(at, h), do: {at[h], h, r}
+      rat = for {_, _, r} <- mine, do: r
+      q = Engine.queue_of(if(length(rat) == 1, do: hd(rat), else: Integer.floor_div(Enum.sum(rat), length(rat))), mode)
+      cond do
+        MapSet.member?(st.moved_out, q) -> {parties, solos}
+        # a lone member goes back as a solo with the party's number, unless a co-member sent back the same way holds
+        # it, still queued, in the same queue (mm_requeue would refuse the whole call): then it answers :gone
+        length(mine) == 1 and Enum.any?(members, fn x ->
+          x != elem(hd(mine), 1) and Map.has_key?(st.queued, x) and Map.has_key?(st.players, x) and
+            Engine.queue_of(elem(st.queued[x], 0), elem(st.queued[x], 1)) == q
+        end) -> {parties, solos}
+        length(mine) == 1 -> {parties, [{elem(hd(mine), 0), elem(hd(mine), 1), {hd(rat), mode, ts, seq}} | solos]}
+        true -> {[{elem(hd(mine), 0), for({i, h, _} <- mine, do: {i, h}), rat, rec} | parties], solos}
+      end
+    end)
+  end
+
+  defp requeue_parties(st, rows) do
+    Engine.requeue_party(st.ref, (for {_, hs, _, _} <- rows, into: <<>>, do: <<length(hs)>>),
+                         (for {_, hs, _, _} <- rows, {_, h} <- hs, into: <<>>, do: <<h::little-32>>),
+                         (for {_, _, rat, _} <- rows, r <- rat, into: <<>>, do: <<r::little-signed-32>>),
+                         (for {_, _, _, {_, _, m, _, _}} <- rows, into: <<>>, do: <<m>>),
+                         (for {_, _, _, {_, _, _, t, _}} <- rows, into: <<>>, do: <<t::little-32>>),
+                         (for {_, _, _, {_, _, _, _, s}} <- rows, into: <<>>, do: <<s::little-32>>))
   end
 
   def handle_call({:search_status, ids}, _from, st) do
@@ -652,7 +764,11 @@ defmodule Matchmaking.Search.Pool do
     case Engine.party_match(st.ref, now, rules) do
       {:ok, lobbies, members} ->
         st = publish(lobbies, members, st)
-        %{st | party_of: Map.drop(st.party_of, for(<<h::little-32 <- members>>, do: h))}
+        placed = for <<h::little-32 <- members>>, do: h
+        # requeue_parties: a placed party's book entry moves aside, so requeue/1 can put the party back whole
+        matched = for h <- placed, rec = Map.get(st.party_book, h), rec != nil, into: st.matched_parties, do: {h, rec}
+        %{st | party_of: Map.drop(st.party_of, placed), party_book: Map.drop(st.party_book, placed),
+               matched_parties: matched}
       {:error, _reason} -> st                                          # nothing was taken
     end
   end
@@ -674,20 +790,23 @@ defmodule Matchmaking.Search.Pool do
     modes = for {_, m, _} <- rows, into: <<>>, do: <<m>>
     stamp = now_ms(st)
     ts = for _ <- rows, into: <<>>, do: <<stamp::little-32>>
+    {:ok, seq0} = Engine.seq_next(st.ref)   # party j of the batch gets seq0 + j
     drop = fn acc, ms -> Enum.reduce(ms, acc, fn {h, fresh, p, _}, a -> if(fresh, do: release(a, p["id"], h), else: a) end) end
     case (if Enum.all?(rows, fn {ms, _, _} -> length(ms) <= 255 end),
             do: Engine.enqueue_party(st.ref, sizes, handles, ratings, modes, ts), else: {:error, :party_too_large}) do
       {:ok, codes} ->
-        Enum.zip(:binary.bin_to_list(codes), rows)
+        Enum.zip([:binary.bin_to_list(codes), rows, 0..(length(rows) - 1)])
         |> Enum.reduce(st, fn
-          {1, {ms, _, ack_ref}}, acc ->
+          {1, {ms, mode, ack_ref}, j}, acc ->
             ack(ack_ref)
             hs = for {h, _, _, _} <- ms, do: h
+            rec = {hs, (for {_, _, _, r} <- ms, do: r), mode, stamp, Bitwise.band(seq0 + j, 0xFFFFFFFF)}
             Enum.reduce(ms, acc, fn {h, _, p, _}, a ->
-              %{a | players: Map.put(a.players, h, p), party_of: Map.put(a.party_of, h, hs)}
+              a = %{a | players: Map.put(a.players, h, p), party_of: Map.put(a.party_of, h, hs)}
+              if a.requeue_parties, do: %{a | party_book: Map.put(a.party_book, h, rec)}, else: a
             end)
-          {0, {_, _, ack_ref}}, acc -> ack(ack_ref); acc                 # a member is already in the queue
-          {_, {ms, _, ack_ref}}, acc -> nack(ack_ref); drop.(acc, ms)     # invalid, or the party table is full
+          {0, {_, _, ack_ref}, _}, acc -> ack(ack_ref); acc                 # a member is already in the queue
+          {_, {ms, _, ack_ref}, _}, acc -> nack(ack_ref); drop.(acc, ms)     # invalid, or the party table is full
         end)
       {:error, _reason} -> Enum.reduce(rows, st, fn {ms, _, ack_ref}, acc -> nack(ack_ref); drop.(acc, ms) end)
     end
@@ -703,7 +822,8 @@ defmodule Matchmaking.Search.Pool do
             {player, players} = Map.pop(acc.players, h)
             send_timeout(acc.channel, player)
             %{acc | players: players, handle_of: Map.delete(acc.handle_of, player["id"]), free: [h | acc.free],
-                    queued: Map.delete(acc.queued, h), party_of: Map.delete(acc.party_of, h)}
+                    queued: Map.delete(acc.queued, h), party_of: Map.delete(acc.party_of, h),
+                    party_book: Map.delete(acc.party_book, h)}
         end
       {:error, _reason} -> st                                          # nothing changed; the next tick retries
     end

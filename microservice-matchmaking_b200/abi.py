@@ -284,6 +284,7 @@ PROTOTYPES = {
                                 _P(C.c_uint32)]),
     "mm_export_parties": (C.c_int, [_vp, _vp, _vp, C.c_uint64, _P(C.c_uint64)]),
     "mm_merge_parties": (C.c_int, [_vp, _vp, C.c_uint64, C.c_uint32, _vp, _P(C.c_uint32)]),
+    "mm_requeue_party": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _P(C.c_uint32)]),
     "mm_in_queue": (C.c_int, [_vp, C.c_uint32, _vp, _vp]),
     "mm_locate": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp]),
     "mm_pool_size": (C.c_int, [_vp, _P(C.c_uint32)]),

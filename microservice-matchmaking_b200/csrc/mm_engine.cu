@@ -339,6 +339,7 @@ struct mm_engine {
     int cur = 0;
     DevArray<uint8_t> in_size, in_mode, in_pre, in_code;
     DevArray<uint32_t> in_ts, in_moff, in_mparty, in_msz, in_one, in_seq;
+    DevArray<uint32_t> in_at, rq_ctr;  // mm_requeue_party: the requeued rows' places, the call's counters
     DevArray<uint64_t> in_id, in_hslot;
     DevArray<int32_t> in_rating;
     DevArray<uint32_t> pb, pcur, tmp, sorted, lob, pos;  // match: [K + 1], [K], then [rows] each (tmp: compaction)
@@ -2859,6 +2860,97 @@ int merge_parties(mm_engine* e, const uint8_t* buf, uint64_t nb, uint32_t flags,
   return MM_OK;
 }
 
+int pq_err(mm_engine* e, uint32_t err) {
+  return set_err(e, MM_E_ARG, "party requeue refused:%s%s%s%s%s%s%s%s", err & kPqBadId ? " id out of range" : "",
+                 err & kPqBadMode ? " mode out of range" : "",
+                 err & kPqBadSize ? " size below 2 or above the mode's team_size" : "",
+                 err & kPqBadRating ? " party rating without a group" : "",
+                 err & kPqOrder ? " parties not in age order" : "",
+                 err & kPqSeqNext ? " sequence number equal to seq_next" : "", err & kPqDup ? " duplicate id" : "",
+                 err & kPqSeqLive ? " sequence number of a queued party" : "");
+}
+
+// mm_requeue_party: check, code and seat on the device, one counter read that decides every refusal, then the merge of
+// the live rows and the requeued parties into the other buffer (mm_party.cuh, "requeue").  The solo pool is not read
+// beyond the mode byte of a member's own slot.
+int requeue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t* ids, const int32_t* rating,
+                  const uint8_t* mode, const uint32_t* enq_ts, const uint32_t* seq, uint8_t* codes,
+                  uint32_t* n_requeued) {
+  int rc = pt_check(e);
+  if (rc || n == 0) return rc;
+  auto& s = e->pt;
+  std::vector<uint32_t> moff(n);
+  uint32_t m = 0;
+  for (uint32_t j = 0; j < n; ++j) {
+    moff[j] = m;
+    m += size[j];
+  }
+  const size_t mm = std::max<uint32_t>(m, 1);
+  const uint64_t sc = seen_keys(m);
+  CK(s.in_size.reserve(n)); CK(s.in_mode.reserve(n)); CK(s.in_code.reserve(n)); CK(s.in_ts.reserve(n));
+  CK(s.in_moff.reserve(n)); CK(s.in_msz.reserve(n)); CK(s.in_one.reserve(n)); CK(s.in_seq.reserve(n));
+  CK(s.in_at.reserve(2 * (size_t)n));
+  CK(s.in_pre.reserve(mm)); CK(s.in_id.reserve(mm)); CK(s.in_hslot.reserve(mm)); CK(s.in_rating.reserve(mm));
+  CK(s.rq_ctr.reserve(kPqWords));
+  CK(e->d_mrg_seen.reserve(sc));
+  CK(cudaMemcpyAsync(s.in_size, size, n, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(s.in_mode, mode, n, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(s.in_seq, seq, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  if (enq_ts) CK(cudaMemcpyAsync(s.in_ts, enq_ts, (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(s.in_moff, moff.data(), (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  if (m) {
+    CK(cudaMemcpyAsync(s.in_id, ids, (size_t)m * 8, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(s.in_rating, rating, (size_t)m * 4, cudaMemcpyHostToDevice, e->stream));
+  }
+  CK(cudaMemsetAsync(e->d_mrg_seen, 0xFF, sc * 8, e->stream));
+  CK(cudaMemsetAsync(s.rq_ctr, 0, kPqWords * 4, e->stream));
+  const Pool& p = e->pool[e->cur];
+  const uint32_t nr = s.n_rows;
+  PqArgs a{};
+  a.n = n; a.m = m; a.size = s.in_size; a.moff = s.in_moff; a.id = s.in_id; a.rating = s.in_rating;
+  a.mode = s.in_mode; a.ts = enq_ts ? s.in_ts.p : nullptr; a.seq = s.in_seq; a.seq_next = e->seq_next;
+  a.id_limit = id_limit(e); a.act = act_view(e); a.pool_mode = p.v.mode; a.n_slots = (uint32_t)pool_slots(e);
+  a.gen = e->gen; a.seen = e->d_mrg_seen; a.seen_mask = sc - 1; a.bm = bin_map(e); a.grp_lut = e->d_grp_lut;
+  a.mode_tsize = e->d_mode_tsize; a.n_modes = e->cfg.n_modes;
+  a.hslot = s.in_hslot; a.cls = s.in_pre; a.code = s.in_code; a.msz = s.in_msz; a.one = s.in_one; a.at = s.in_at;
+  a.t = pt_view(e, s.cur); a.n_rows = nr; a.keep = s.tmp; a.lmsz = s.sorted; a.lseq = s.lob; a.lmo = s.pos;
+  a.d = pt_view(e, s.cur ^ 1);
+  a.ctr = s.rq_ctr;
+  const uint32_t gm = (m + 255) / 256, gn = (n + 255) / 256, gr = (nr + 255) / 256;
+  if (m) k_pq_check<<<gm, 256, 0, e->stream>>>(a);
+  k_pq_party<<<gn, 256, 0, e->stream>>>(a);
+  k_scan_small<<<1, 1024, 0, e->stream>>>(n, s.in_msz, s.rq_ctr + kPqMem);
+  k_scan_small<<<1, 1024, 0, e->stream>>>(n, s.in_one, s.rq_ctr + kPqRows);
+  if (nr) {
+    k_pt_keep<<<gr, 256, 0, e->stream>>>(nr, a.t, s.tmp, s.sorted);
+    k_scan_small<<<1, 1024, 0, e->stream>>>(nr, s.tmp, s.rq_ctr + kPqLiveRows);
+    k_scan_small<<<1, 1024, 0, e->stream>>>(nr, s.sorted, s.rq_ctr + kPqLiveMem);
+    k_pq_live<<<gr, 256, 0, e->stream>>>(a);
+  }
+  k_pq_seat<<<gn, 256, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  uint32_t h[kPqWords];
+  CK(cudaMemcpyAsync(h, s.rq_ctr, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  if (h[kPqErr]) return pq_err(e, h[kPqErr]);
+  if (h[kPqMem] > s.cap - s.live)
+    return set_err(e, MM_E_CAP, "%u party members to requeue, the party table has room for %u", h[kPqMem],
+                   s.cap - s.live);
+  if (h[kPqRows]) {
+    if (nr) k_pq_move<<<gr, 256, 0, e->stream>>>(a);
+    k_pq_write<<<gn, 256, 0, e->stream>>>(a);
+    CK(cudaGetLastError());
+  }
+  if (codes) CK(cudaMemcpyAsync(codes, s.in_code, n, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  if (h[kPqRows]) {
+    s.n_rows = h[kPqLiveRows] + h[kPqRows]; s.n_mem = h[kPqLiveMem] + h[kPqMem]; s.live += h[kPqMem];
+    s.cur ^= 1;
+  }
+  if (n_requeued) *n_requeued = h[kPqRows];
+  return MM_OK;
+}
+
 int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
                 uint64_t* member_ids, uint64_t member_cap, mm_party_stats* st) {
   const mm_config& c = e->cfg;
@@ -3400,6 +3492,20 @@ int mm_enqueue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64
   if (n && (!size || !ids || !rating || !mode)) return set_err(e, MM_E_ARG, "null size, ids, rating or mode with n = %u", n);
   CK(cudaSetDevice(e->device));
   return enqueue_party(e, n, size, ids, rating, mode, enq_ts, accepted);
+}
+
+int mm_requeue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t* ids, const int32_t* rating,
+                     const uint8_t* mode, const uint32_t* enq_ts, const uint32_t* seq, uint8_t* codes,
+                     uint32_t* n_requeued) {
+  if (n_requeued) *n_requeued = 0;
+  if (!e) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (n && (!size || !ids || !rating || !mode || !seq))
+    return set_err(e, MM_E_ARG, "null size, ids, rating, mode or seq with n = %u", n);
+  CK(cudaSetDevice(e->device));
+  const int rc = requeue_party(e, n, size, ids, rating, mode, enq_ts, seq, codes, n_requeued);
+  free_img_scratch(e);
+  return rc;
 }
 
 int mm_party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,

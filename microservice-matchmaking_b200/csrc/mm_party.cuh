@@ -2,9 +2,10 @@
 // matched into one lobby and one team.  Parties live in a table of their own beside the pool, which the tick never
 // reads.
 //
-// Table: one row per party in age order (= insertion order: every party of an accepted batch consumes one enqueue
-// sequence number, so rows and solos share the numbering of emit_seq), its members in a member array at the row's
-// offset.  A queued member's active-set value is kPtVal(row) (pool generation 0, which no pool ever has); a matched
+// Table: one row per party, the LIVE rows in age order (every party of an accepted batch consumes one enqueue sequence
+// number, so rows and solos share the numbering of emit_seq), its members in a member array at the row's offset.  Dead
+// rows need not be in order with the live ones: mm_merge_parties(MM_PARTY_KEEP_SEQ) on a table whose parties were all
+// released appends the image's (older) numbers after the released rows.  A queued member's active-set value is kPtVal(row) (pool generation 0, which no pool ever has); a matched
 // member's is kPtMatched (a slot past every pool), which every call reads as a matched player.  Rows of matched,
 // dissolved and expired parties stay in place, `dead`, until the next compaction (k_pt_keep / k_pt_move: stable, by age).
 //
@@ -26,6 +27,9 @@
 // image index and member offset, k_pt_export gathers the columns in age order and releases the row (pt_release, as
 // k_pt_dissolve does).  The merge is the enqueue pipeline with the image's numbers (PtEnqArgs::seq) or new ones; its
 // refusal for room comes before k_pt_commit, and k_pt_unclaim gives the claims back.
+//
+// Requeue (mm_requeue_party): matched parties back into the table at their age position, a merge of the live rows and
+// the requeued parties into the other buffer (k_pq_*, "requeue" below).
 #pragma once
 
 #include "mm_widen.cuh"
@@ -179,12 +183,10 @@ __global__ void k_pt_keep(uint32_t n_rows, PartyView t, uint32_t* __restrict__ k
   msz[r] = k ? t.size[r] : 0u;
 }
 
-// rows kept -> their place in `d` (keep / msz hold the exclusive scans); the members' active-set values follow the row
-__global__ void k_pt_move(uint32_t n_rows, PartyView s, PartyView d, const uint32_t* __restrict__ keep,
-                          const uint32_t* __restrict__ msz, ActiveView act) {
-  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= n_rows || s.dead[r]) return;
-  const uint32_t q = keep[r], o = msz[r], so = s.off[r], n = s.size[r];
+// live row r of `s` -> row q of `d`, its members from entry o on; the members' active-set values follow the row
+__device__ __forceinline__ void pt_move_row(const PartyView& s, uint32_t r, const PartyView& d, uint32_t q, uint32_t o,
+                                            const ActiveView& act) {
+  const uint32_t so = s.off[r], n = s.size[r];
   d.seq[q] = s.seq[r]; d.ts[q] = s.ts[r]; d.off[q] = o; d.R[q] = s.R[r]; d.bin[q] = s.bin[r];
   d.mode[q] = s.mode[r]; d.grp[q] = s.grp[r]; d.size[q] = (uint8_t)n; d.dead[q] = 0;
   for (uint32_t k = 0; k < n; ++k) {
@@ -194,6 +196,14 @@ __global__ void k_pt_move(uint32_t n_rows, PartyView s, PartyView d, const uint3
     const uint64_t h = act_find(act, pid);
     if (h != ~0ull) *act.val(h) = kPtVal(q);
   }
+}
+
+// rows kept -> their place in `d` (keep / msz hold the exclusive scans)
+__global__ void k_pt_move(uint32_t n_rows, PartyView s, PartyView d, const uint32_t* __restrict__ keep,
+                          const uint32_t* __restrict__ msz, ActiveView act) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= n_rows || s.dead[r]) return;
+  pt_move_row(s, r, d, keep[r], msz[r], act);
 }
 
 // ---- remove and expire ------------------------------------------------------------------------------------------------
@@ -290,6 +300,172 @@ __global__ void k_pt_unclaim(const PtEnqArgs a) {
   if (h == ~0ull || a.pre[j]) return;
   *a.act.val(h) = kFreeVal;
   if (!a.act.dcap) *a.act.key(h) = kEmptyKey;
+}
+
+// ---- requeue (mm_requeue_party) ---------------------------------------------------------------------------------------
+// A merge of two age-sorted lists, the table's live rows and the requeued parties, into the other buffer (as a
+// compaction).  k_pq_check classifies every member's entry, k_pq_party gives every party its checks and code, the scans
+// (k_scan_small) number the code-1 parties and their members and, over k_pt_keep, the live rows and theirs; k_pq_live
+// lists the live rows' seqs and member offsets in live-row order (= age order; the dead rows are left out, since they
+// need not be in order with the live ones).  k_pq_seat finds each code-1 party's age in that list (one binary search:
+// its rank among the live rows, and the collision with a live row of the same seq).  After the one counter read that decides every refusal, k_pq_move moves each live row to
+// its own rank plus the code-1 parties older than it (one binary search over the call's ages) and k_pq_write writes the
+// requeued rows, their members and active-set values.
+
+// error bits (the host names them in mm_last_error)
+constexpr uint32_t kPqBadId = 1, kPqBadMode = 2, kPqBadSize = 4, kPqBadRating = 8, kPqOrder = 16, kPqSeqNext = 32,
+                   kPqDup = 64, kPqSeqLive = 128;
+// the counters of one requeue (zeroed by the host): error bits, the code-1 parties' members and rows (scan totals), the
+// live rows and their members (scan totals)
+enum PqCtr : uint32_t { kPqErr = 0, kPqMem, kPqRows, kPqLiveRows, kPqLiveMem, kPqWords };
+
+struct PqArgs {
+  uint32_t n, m;                 // parties, members
+  const uint8_t* size;           // [n]
+  const uint32_t* moff;          // [n] first member of the party in the call
+  const uint64_t* id;            // [m]
+  const int32_t* rating;         // [m]
+  const uint8_t* mode;           // [n]
+  const uint32_t* ts;            // [n] or null
+  const uint32_t* seq;           // [n]
+  uint32_t seq_next;
+  uint64_t id_limit;
+  ActiveView act;
+  const uint8_t* pool_mode;      // the live-slot test of k_rq_check
+  uint32_t n_slots, gen;
+  unsigned long long* seen;      // empty scratch id set of seen_mask + 1 keys, at most half full
+  uint64_t seen_mask;
+  BinMap bm;
+  const uint8_t* grp_lut;
+  const uint8_t* mode_tsize;
+  uint32_t n_modes;
+  uint64_t* hslot;               // [m] active-set slot of the member's id (~0: none)
+  uint8_t* cls;                  // [m] 0 queued (a live solo or a queued party's member), 1 matched, 4 not active
+  uint8_t* code;                 // [n]
+  uint32_t* msz;                 // [n] code-1 member counts -> exclusive scan
+  uint32_t* one;                 // [n] code-1: 1 -> exclusive scan
+  uint32_t* at;                  // [2n] code-1 party p: its row (at[p]) and first member entry (at[n + p]) in d
+  PartyView t;                   // the table (buffer cur)
+  uint32_t n_rows;
+  const uint32_t* keep;          // [n_rows] k_pt_keep -> exclusive scans
+  const uint32_t* lmsz;
+  uint32_t* lseq;                // [live rows] the live rows' seqs, in live-row order (k_pq_live)
+  uint32_t* lmo;                 // [live rows] their first member entries among the live rows' members
+  PartyView d;                   // buffer cur ^ 1
+  uint32_t* ctr;                 // [kPqWords]
+};
+
+// floor(sum / s) of s >= 1 ratings (64-bit sum, toward minus infinity), clamped into int32 for a hostile s
+__device__ __forceinline__ int32_t pq_mean(const int32_t* r, uint32_t s) {
+  long long sum = 0;
+  for (uint32_t k = 0; k < s; ++k) sum += r[k];
+  long long R = sum / (long long)s;
+  if (R * (long long)s > sum) --R;
+  return R < INT32_MIN ? INT32_MIN : (R > INT32_MAX ? INT32_MAX : (int32_t)R);
+}
+
+// One thread per member: a repeated id (seen_insert), then its active-set entry: live solo or queued party member (0),
+// matched (1), not active (4).
+__global__ void k_pq_check(const PqArgs a) {
+  const uint32_t j = blockIdx.x * blockDim.x + threadIdx.x;
+  if (j >= a.m) return;
+  const uint64_t pid = a.id[j];
+  uint64_t h = ~0ull;
+  uint8_t c = 4;
+  if (pid >= a.id_limit) {
+    atomicOr(&a.ctr[kPqErr], kPqBadId);
+  } else {
+    if (!seen_insert(a.seen, a.seen_mask, pid)) atomicOr(&a.ctr[kPqErr], kPqDup);
+    h = act_find(a.act, pid);
+    const unsigned long long v = h == ~0ull ? kFreeVal : *a.act.val(h);
+    if (v < kPending) {
+      const uint32_t slot = (uint32_t)v;
+      const bool queued = ((uint32_t)(v >> 32) == a.gen && slot < a.n_slots && a.pool_mode[slot] != MM_MODE_DEAD) ||
+                          pt_queued(v);
+      c = queued ? 0 : 1;
+    }
+  }
+  a.hslot[j] = h;
+  a.cls[j] = c;
+}
+
+// One thread per party: its argument checks and its code, 0 (a member queued) before 4 (a member not active) before 1.
+__global__ void k_pq_party(const PqArgs a) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= a.n) return;
+  const uint32_t s = a.size[p], o = a.moff[p], md = a.mode[p], u = a.seq[p] - a.seq_next;
+  uint32_t bad = 0;
+  if (md >= a.n_modes) bad |= kPqBadMode;
+  if (s < 2 || (md < a.n_modes && s > a.mode_tsize[md])) bad |= kPqBadSize;
+  if (u == 0) bad |= kPqSeqNext;
+  if (p + 1 < a.n && a.seq[p + 1] - a.seq_next <= u) bad |= kPqOrder;
+  if (s && a.grp_lut[clamp_key(a.bm.key_lo, a.bm.KR, pq_mean(a.rating + o, s))] == 0xFF) bad |= kPqBadRating;
+  bool queued = false, gone = false;
+  for (uint32_t k = 0; k < s; ++k) {
+    queued |= a.cls[o + k] == 0;
+    gone |= a.cls[o + k] == 4;
+  }
+  const uint8_t c = queued ? 0 : (gone ? 4 : 1);
+  a.code[p] = c;
+  a.msz[p] = c == 1 ? s : 0u;
+  a.one[p] = c == 1;
+  if (bad) atomicOr(&a.ctr[kPqErr], bad);
+}
+
+// age of a sequence number: (seq - seq_next) mod 2^32, the oldest first
+__device__ __forceinline__ uint32_t pq_age(uint32_t seq, uint32_t seq_next) { return seq - seq_next; }
+
+// One thread per live row, after the scans: its seq and member offset at its rank among the live rows.
+__global__ void k_pq_live(const PqArgs a) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= a.n_rows || a.t.dead[r]) return;
+  a.lseq[a.keep[r]] = a.t.seq[r];
+  a.lmo[a.keep[r]] = a.lmsz[r];
+}
+
+// One thread per code-1 party, after k_pq_live: its row and first member entry in d = its rank among the code-1
+// parties plus the live rows older than it; a live row of the same age is a collision.
+__global__ void k_pq_seat(const PqArgs a) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= a.n || a.code[p] != 1) return;
+  const uint32_t u = pq_age(a.seq[p], a.seq_next), L = a.ctr[kPqLiveRows];
+  const uint32_t l = first_not(0, L, [&](uint32_t k) { return pq_age(a.lseq[k], a.seq_next) < u; });
+  if (l < L && pq_age(a.lseq[l], a.seq_next) == u) atomicOr(&a.ctr[kPqErr], kPqSeqLive);
+  a.at[p] = a.one[p] + l;
+  a.at[a.n + p] = a.msz[p] + (l < L ? a.lmo[l] : a.ctr[kPqLiveMem]);
+}
+
+// One thread per live row: to its rank among the live rows (= its age rank) plus the code-1 parties older than it.
+__global__ void k_pq_move(const PqArgs a) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= a.n_rows || a.t.dead[r]) return;
+  const uint32_t u = pq_age(a.t.seq[r], a.seq_next);
+  const uint32_t l = first_not(0, a.n, [&](uint32_t p) { return pq_age(a.seq[p], a.seq_next) < u; });
+  const uint32_t q = a.keep[r] + (l < a.n ? a.one[l] : a.ctr[kPqRows]);
+  const uint32_t o = a.lmsz[r] + (l < a.n ? a.msz[l] : a.ctr[kPqMem]);
+  pt_move_row(a.t, r, a.d, q, o, a.act);
+}
+
+// One thread per code-1 party: its row and members in d, in the order given; its members' values become kPtVal(row).
+__global__ void k_pq_write(const PqArgs a) {
+  const uint32_t p = blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= a.n || a.code[p] != 1) return;
+  const uint32_t s = a.size[p], o = a.moff[p], md = a.mode[p], q = a.at[p], mo = a.at[a.n + p];
+  const int32_t R = pq_mean(a.rating + o, s);
+  a.d.seq[q] = a.seq[p];
+  a.d.ts[q] = a.ts ? a.ts[p] : 0u;
+  a.d.off[q] = mo;
+  a.d.R[q] = R;
+  a.d.bin[q] = (uint16_t)bin_of(a.bm, a.bm.lut, R, md);
+  a.d.mode[q] = (uint8_t)md;
+  a.d.grp[q] = a.grp_lut[clamp_key(a.bm.key_lo, a.bm.KR, R)];
+  a.d.size[q] = (uint8_t)s;
+  a.d.dead[q] = 0;
+  for (uint32_t k = 0; k < s; ++k) {
+    a.d.mid[mo + k] = a.id[o + k];
+    a.d.mrat[mo + k] = a.rating[o + k];
+    *a.act.val(a.hslot[o + k]) = kPtVal(q);
+  }
 }
 
 // mm_expire: whole parties whose WAIT >= max_wait, after k_expire on the same counters (ctr[0] the output cursor,

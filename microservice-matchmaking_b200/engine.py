@@ -564,6 +564,34 @@ class Engine:
                                               _p(code), C.byref(k)), "mm_merge_parties")
         return code[:n]
 
+    def requeue_party(self, sizes, ids, rating, mode, enq_ts, seq):
+        """Put the parties of a lobby that did not start back into the party table as parties, at their age position
+        (mm_requeue_party).  Party j's members are the next sizes[j] entries of ids / rating; mode, enq_ts (may be
+        None) and seq are per party, what it had when it was queued.  The parties may come in any order: they are
+        sorted by age here.  -> codes u8[n] in the caller's order: 1 requeued, 0 a member still queued, 4 a member not
+        in the active set (the party was not requeued)."""
+        sizes = np.ascontiguousarray(sizes, np.uint8)
+        ids = np.ascontiguousarray(ids, np.uint64)
+        rating = np.ascontiguousarray(rating, np.int32)
+        seq = np.ascontiguousarray(seq, np.uint32)
+        n = len(sizes)
+        assert len(mode) == n and len(seq) == n and len(ids) == len(rating) == int(sizes.sum(dtype=np.int64))
+        order = np.argsort((seq - np.uint32(self.seq_next())).astype(np.uint32), kind="stable")  # a tie is refused
+        start = np.concatenate([[0], np.cumsum(sizes.astype(np.int64))])
+        so = sizes[order].astype(np.int64)  # the members of party order[k] follow those of order[k - 1]
+        take = np.repeat(start[order], so) + np.arange(len(ids)) - np.repeat(np.cumsum(so) - so, so)
+        cols = [np.ascontiguousarray(a, dt) for a, dt in ((sizes[order], np.uint8), (ids[take], np.uint64),
+                                                          (rating[take], np.int32), (np.asarray(mode)[order], np.uint8),
+                                                          (seq[order], np.uint32))]
+        ts = None if enq_ts is None else np.ascontiguousarray(np.asarray(enq_ts)[order], np.uint32)
+        codes = np.empty(max(n, 1), np.uint8)
+        k = C.c_uint32(0)
+        self._check(self.lib.mm_requeue_party(self.h, n, _p(cols[0]), _p(cols[1]), _p(cols[2]), _p(cols[3]), _p(ts),
+                                              _p(cols[4]), _p(codes), C.byref(k)), "mm_requeue_party")
+        out = np.empty(n, np.uint8)
+        out[order] = codes[:n]
+        return out
+
     def in_queue(self, ids):
         ids = np.ascontiguousarray(ids, np.uint64)
         out = np.empty(len(ids), np.uint8)

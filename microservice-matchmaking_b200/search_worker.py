@@ -180,6 +180,10 @@ class SearchPool:
     before the tick itself, so parties get the first pick of the solos; its lobbies are published like the tick's and
     stats["party_lobbies"] counts them.  A party member removed with remove_user() takes its whole party out; a matched
     member's requeue() answers "gone" (the caller enqueues the party again).
+    requeue_parties: with parties, requeue() puts matched parties back as parties (extension, Engine.requeue_party):
+    the pool keeps a book of every queued party (members, ratings, mode, stamp and enqueue sequence number) and moves a
+    party's entry aside when party_match places it, until remove_user or a requeue.  Off (the default), requeue() of a
+    matched party member answers "gone" as described above.
 
     Every ingest batch is stamped with now_ms(), the clock in milliseconds since the pool was created (u32, wraps
     after 49 days), and every tick passes the same clock as its `now`: the engine's per-queue waits
@@ -188,7 +192,7 @@ class SearchPool:
 
     def __init__(self, engine, mode_names, group_names, max_batch=65536, window=None, clock=None, flush_every_s=0.005,
                  handle_capacity=None, timeout_ms=None, wall_clock=None, lobby_budget=None, widen=None,
-                 balance_teams=None, parties=None, party_capacity=None):
+                 balance_teams=None, parties=None, party_capacity=None, requeue_parties=False):
         import time
         if widen and engine.cfg.order_mode != abi.MM_ORDER_RATING:
             raise ValueError("widen needs an MM_ORDER_RATING engine: windows are rating distances")
@@ -203,6 +207,11 @@ class SearchPool:
         if party_capacity:
             engine.set_option("party_capacity", int(party_capacity))
         self.party_of = {}  # handle -> the handles of its queued party (remove_user takes the whole party out)
+        # requeue_parties: handle -> the record of its party ({"members", "rating", "mode", "ts", "seq"}, one dict shared
+        # by the members), while the party is queued (party_book) and once party_match has placed it (matched_parties)
+        self.requeue_parties = bool(requeue_parties)
+        self.party_book = {}
+        self.matched_parties = {}
         self._staged_parties = []  # (worker, tag, [player documents], game mode)
         self.timeout_ms = timeout_ms
         self.lobby_budget = lobby_budget
@@ -257,6 +266,8 @@ class SearchPool:
             self.engine.remove([h])  # a queued party member: the engine removes its whole party
             for x in self.party_of.pop(h, (h,)):
                 self.party_of.pop(x, None)
+                self.party_book.pop(x, None)
+                self.matched_parties.pop(x, None)
                 self.handles.release(self.handles.id_of[x])
                 self.players.pop(x, None)
                 self.enqueued_at.pop(x, None)
@@ -271,29 +282,92 @@ class SearchPool:
         "requeued" (queued again; its document is back in the pool), "queued" (still queued: nothing changed) or
         "gone" (not in this pool's active set — removed, timed out, never queued — its queue has moved to another pool,
         or its rating or mode has no queue under this pool's config after a resume(regroup=True): answer it as today,
-        remove_user and an error response)."""
+        remove_user and an error response).  With requeue_parties, the matched party members among `players` go back by
+        party: two or more members of one party as one party with the party's stamp and number (Engine.requeue_party;
+        the members not among `players` stay out of it), a lone member as a solo with its own rating and the party's
+        stamp and number.  The parties go first; if the engine refuses them (the party table is full), they answer
+        "gone" and the solos go on.  A lone member whose co-member went back the same way and is still queued in the
+        same (mode, group) queue answers "gone": the engine holds one player of a party number per partition."""
         self.flush()
         out = ["gone"] * len(players)
-        pos, hs = {}, []
+        n_modes = self.engine.cfg.n_modes
+        pos, hs, solo_rec, by_party = {}, [], {}, {}
         for i, doc in enumerate(players):
             h = self.handles.lookup(doc.get("id"))
-            rec = self.queued.get(h) if h is not None else None
-            if rec is None or h in pos or rec[1] >= self.engine.cfg.n_modes:
+            if h is None or h in pos:
+                continue
+            if h in self.party_book:  # a member of a queued party: nothing to put back
+                pos[h] = i
+                out[i] = "queued"
+                continue
+            party = self.matched_parties.get(h) if self.requeue_parties else None
+            if party is not None:
+                pos[h] = i
+                by_party.setdefault(id(party), (party, set()))[1].add(h)
+                continue
+            rec = self.queued.get(h)
+            if rec is None or rec[1] >= n_modes:
                 continue
             q = self._queue_of(rec[0], rec[1])
             if q < 0 or q in self.moved_out:
                 continue
             pos[h] = i
             hs.append(h)
+        parties = []  # (member handles, ratings, record) of the parties that go back whole
+        for party, asked in by_party.values():
+            mem = [x for x in party["members"] if x in asked]
+            rat = [party["rating"][party["members"].index(x)] for x in mem]
+            if party["mode"] >= n_modes:
+                continue
+            q = self._queue_of(rat[0] if len(mem) == 1 else sum(rat) // len(rat), party["mode"])
+            if q < 0 or q in self.moved_out:
+                continue
+            if len(mem) == 1:  # a lone member goes back as a solo with the party's number
+                # ... which a co-member sent back the same way and still queued in this queue holds already: mm_requeue
+                # would refuse the whole call, so this one is answered "gone"
+                if any(x != mem[0] and x in self.queued and x in self.players and
+                       self._queue_of(self.queued[x][0], self.queued[x][1]) == q for x in party["members"]):
+                    continue
+                solo_rec[mem[0]] = [rat[0], party["mode"], party["ts"], party["seq"]]
+                hs.append(mem[0])
+            else:
+                parties.append((mem, rat, party))
+        if parties:  # first: a refused call (the table is full) changes nothing, and its parties answer "gone"
+            sizes = np.array([len(m) for m, _r, _p in parties], np.uint8)
+            try:
+                codes = self.engine.requeue_party(
+                    sizes, np.array([x for m, _r, _p in parties for x in m], np.uint64),
+                    np.array([x for _m, r, _p in parties for x in r], np.int32),
+                    np.array([p["mode"] for _m, _r, p in parties], np.uint8),
+                    np.array([p["ts"] for _m, _r, p in parties], np.uint32),
+                    np.array([p["seq"] for _m, _r, p in parties], np.uint32))
+            except Exception:
+                codes = np.full(len(parties), 4, np.uint8)
+                self.stats["failed_requeues"] = self.stats.get("failed_requeues", 0) + 1
+            for (mem, rat, party), c in zip(parties, codes.tolist()):
+                if c == 1:
+                    rec = dict(party, members=tuple(mem), rating=tuple(rat))
+                    for h in mem:
+                        out[pos[h]] = "requeued"
+                        self.players[h] = players[pos[h]]
+                        self.matched_parties.pop(h, None)
+                        self.party_of[h] = tuple(mem)
+                        self.party_book[h] = rec
+                elif c == 0:
+                    for h in mem:
+                        out[pos[h]] = "queued"
         back = []  # window: (clock value, handle) of the requeued players
         if hs:
-            rec = np.array([self.queued[h] for h in hs], np.int64)
+            rec = np.array([self.queued[h] if h in self.queued else solo_rec[h] for h in hs], np.int64)
             codes = self.engine.requeue(np.array(hs, np.uint64), rec[:, 0].astype(np.int32), rec[:, 1].astype(np.uint8),
                                         rec[:, 2].astype(np.uint32), rec[:, 3].astype(np.uint32))
             for h, c in zip(hs, codes.tolist()):
                 if c == 1:
                     out[pos[h]] = "requeued"
                     self.players[h] = players[pos[h]]
+                    if h in solo_rec:  # a solo from now on
+                        self.queued[h] = solo_rec[h]
+                        self.matched_parties.pop(h, None)
                     at = self.matched_at.pop(h, None)
                     if self.window and at is not None:
                         back.append((at, h))
@@ -425,8 +499,10 @@ class SearchPool:
         try:
             if np.any(sizes.astype(np.int64) != [len(s[2]) for s in staged]):
                 raise ValueError("a party of more than 255 players")
+            seq0 = self.engine.seq_next() if self.requeue_parties else 0  # party j of the batch gets seq0 + j
+            stamp = self.now_ms()
             codes = self.engine.enqueue_party(sizes, ids, rating, np.array(mode, np.uint8),
-                                              np.full(len(staged), self.now_ms(), np.uint32))
+                                              np.full(len(staged), stamp, np.uint32))
         except Exception:  # nothing was enqueued
             for pid in fresh:
                 self.handles.release(pid)
@@ -435,13 +511,17 @@ class SearchPool:
             self.stats["failed_batches"] += 1
             return 0
         fresh, off = set(fresh), 0
-        for code, (worker, tag, players, _m) in zip(codes.tolist(), staged):
+        for j, (code, (worker, tag, players, _m)) in enumerate(zip(codes.tolist(), staged)):
             hs = ids[off:off + len(players)].tolist()
+            rec = dict(members=tuple(hs), rating=tuple(rating[off:off + len(players)].tolist()), mode=int(mode[j]),
+                       ts=stamp, seq=(seq0 + j) & 0xFFFFFFFF)
             off += len(players)
             if code == 1:
                 for h, doc in zip(hs, players):
                     self.players[h] = doc
                     self.party_of[h] = tuple(hs)
+                    if self.requeue_parties:
+                        self.party_book[h] = rec
                 self.stats["enqueued"] += len(players)
                 worker.ack(worker.channel_name, tag)
             elif code == 0:  # a member is already queued
@@ -546,6 +626,9 @@ class SearchPool:
             plob, pmem, _st = self.engine.party_match(now, self.party_rules)
             for x in pmem.tolist():
                 self.party_of.pop(x, None)
+                rec = self.party_book.pop(x, None)
+                if rec is not None:  # requeue() can put the party back whole
+                    self.matched_parties[x] = rec
             self._publish(plob, pmem)
             self.stats["party_lobbies"] += len(plob)
             n_lob += len(plob)
@@ -620,6 +703,7 @@ class SearchPool:
         expired, _seq = self.engine.expire(now, self.timeout_ms, want_seq=False)
         for h in expired.tolist():
             self.party_of.pop(h, None)
+            self.party_book.pop(h, None)
             player = self.players.pop(h)
             self.enqueued_at.pop(h, None)
             self.queued.pop(h, None)
@@ -669,6 +753,9 @@ class SearchPool:
         }
         if parties is not None:  # the party image goes between the JSON and the engine image
             state["party_of"] = sorted({tuple(p) for p in self.party_of.values()})
+            if self.requeue_parties:  # the matched players stay in the engine image: their parties' book goes too
+                state["party_book"] = self._book_records(self.party_book)
+                state["matched_parties"] = self._book_records(self.matched_parties)
             state["party_image"] = len(parties)
             image = parties.tobytes() + image
         doc = json.dumps(state).encode()
@@ -733,14 +820,50 @@ class SearchPool:
         pool.queued = {int(h): rec for h, rec in state.get("queued", [])}  # the image keeps every sequence number
         pool.moved_out = set(state.get("moved_out", []))
         pool.party_of = {int(h): tuple(int(x) for x in hs) for hs in state.get("party_of", []) for h in hs}
+        if pool.requeue_parties:
+            pool.party_book = cls._book_of(state.get("party_book", []))
+            pool.matched_parties = cls._book_of(state.get("matched_parties", []))
         pool.regroup_dropped = []
         for h in rejected:  # not queued under the new config: they left
             pool.party_of.pop(h, None)
+            pool.party_book.pop(h, None)
             pool.regroup_dropped.append(pool.players.pop(h))
             for d in (pool.queued, pool.enqueued_at, pool.matched_at):
                 d.pop(h, None)
             pool.handles.release(pool.handles.id_of[h])
         return pool
+
+    @staticmethod
+    def _book_records(book):
+        """The distinct party records of a book, as JSON."""
+        recs = {id(r): r for r in book.values()}
+        return [dict(r, members=list(r["members"]), rating=list(r["rating"])) for r in recs.values()]
+
+    @staticmethod
+    def _book_of(records):
+        """_book_records -> handle -> record (one dict shared by the members)."""
+        book = {}
+        for r in records:
+            rec = dict(r, members=tuple(int(x) for x in r["members"]), rating=tuple(int(x) for x in r["rating"]))
+            book.update((h, rec) for h in rec["members"])
+        return book
+
+    def _book_parties(self, image, seq0, codes=None, handles=None):
+        """requeue_parties: the parties of a party image merged without their numbers get seq0 + their index.  With
+        handles (a moved-in image, in image member order), the merged ones (code 1) get a record."""
+        from .engine import read_party_image
+        _h, pc = read_party_image(image)
+        cut = np.cumsum(pc["size"].astype(np.int64))
+        for j, (lo, hi) in enumerate(zip(np.concatenate([[0], cut[:-1]]).tolist(), cut.tolist())):
+            seq = (seq0 + j) & 0xFFFFFFFF
+            if handles is None:
+                rec = self.party_book.get(int(pc["id"][lo]))
+                if rec is not None:
+                    rec["seq"] = seq
+            elif codes[j] == 1:
+                rec = dict(members=tuple(handles[lo:hi]), rating=tuple(pc["rating"][lo:hi].tolist()),
+                           mode=int(pc["mode"][j]), ts=int(pc["enq_ts"][j]), seq=seq)
+                self.party_book.update((h, rec) for h in rec["members"])
 
     # -- moving queues to another running pool -----------------------------------------------------
     MOVE_MAGIC = b"MMMOVE01"
@@ -796,6 +919,7 @@ class SearchPool:
             for h in read_party_image(pimage)[1]["id"].tolist():
                 pid = self.handles.id_of[h]
                 self.party_of.pop(h, None)
+                self.party_book.pop(h, None)
                 members.append([pid, self.players.pop(h)])
                 self.handles.release(pid)
             state["party_players"] = members
@@ -901,10 +1025,16 @@ class SearchPool:
         # the solos are recorded: ours come back (with their numbers when the queue image took none, else renumbered in
         # their order), then the moved parties, whose room was checked above
         if own is not None:
-            self.engine.merge_parties(own, keep_seq=self.engine.seq_next() == seq0)
+            s_own = self.engine.seq_next()
+            self.engine.merge_parties(own, keep_seq=s_own == seq0)
+            if s_own != seq0 and self.requeue_parties:  # renumbered in their order
+                self._book_parties(own, s_own)
         if k:
+            s_moved = self.engine.seq_next()
             try:
                 codes = self.engine.merge_parties(pimage)
+                if self.requeue_parties:
+                    self._book_parties(pimage, s_moved, codes.tolist(), phandles)
             except Exception:
                 codes = np.zeros(len(pcols["size"]), np.uint8)
                 raise
