@@ -411,7 +411,7 @@ typedef struct mm_party_stats {
   uint32_t n_parties;   /* parties placed into lobbies                         */
   uint32_t n_absorbed;  /* anchors an earlier lobby of the call had placed     */
   float device_us;      /* CUDA-event time of the call's device work           */
-  uint32_t reserved[2];
+  uint64_t sum_imbalance;  /* "party_balance": summed imbalance of the emitted lobbies of masked modes (0: off) */
 } mm_party_stats;       /* 32 bytes */
 
 /* mm_party_match: one mm_widen_rule per (mode, group) queue in mm_queue_stats order (MM_WIDEN_OFF: the queue is not
@@ -438,7 +438,10 @@ typedef struct mm_party_stats {
  * rating maps to another partition is requeued.  Only R needs a group, so a member whose own rating has none cannot be
  * requeued (MM_E_ARG).  To put a whole party back at its age position, use mm_requeue_party.  team_balance does not
  * split party lobbies; the last tick's results, mm_match_quality, the lobby budget and pending async_results copies
- * are left alone.
+ * are left alone.  With mm_set_option("party_balance") a lobby of a masked mode is split into its most even teams with
+ * every party kept whole, so its teams no longer read "a team's parties, then its solos": EQUIVALENCE, the call leaves
+ * the engine exactly as the same call without the option would, and its member order is the party_balance rule
+ * applied to that call's lobbies (each party's members stay contiguous and in enqueue order).
  * Refusals, all decided before anything changes (mm_last_error names the cause): MM_E_ARG the rule checks of mm_widen,
  * a served mode of more than 256 teams, an MM_ORDER_ARRIVAL engine; MM_E_STATE no party capacity, an MM_F_NO_DEDUPE
  * engine, a staged packed batch; MM_E_CAP lobby_cap or member_cap too small (stats holds the counts and nothing is
@@ -1034,6 +1037,27 @@ int mm_set_stream(mm_engine* e, void* cuda_stream);
  *                   and mm_tick_device returns once it is done, so mm_results_device's members are final.  Device memory,
  *                   allocated by the first balanced call and kept: 4 bytes per lobby the pool could hold, 4 bytes per
  *                   player of capacity and, in arrival order, 4 bytes per chunk.
+ *   "party_balance" EXTENSION (balanced party lobbies): a mask, bit m = balance the mm_party_match lobbies of game
+ *                   mode m; 0 (default) = off.  team_balance's refusals (MM_E_ARG: a mode >= n_modes, teams != 2,
+ *                   team_size > 8); a 1v1 mode is accepted and changes nothing; party_capacity need not be set.
+ *                   Independent of team_balance: team_balance never splits party lobbies and party_balance splits
+ *                   nothing else (tick, mm_widen, mm_backfill).  For every lobby of a masked mode that mm_party_match
+ *                   forms, with m_0 .. m_{L-1} its members in the order the call forms them without the option and
+ *                   c_i = c(rating of m_i) clamped to [rmin - 1, rmax + 1] (a party member's own rating, not the
+ *                   party's R; a solo's pool rating): a set A of S members is admissible when it holds m_0 and, of
+ *                   every party of the lobby, all members or none.  Over the admissible sets, minimise |sum_A c -
+ *                   sum_rest c| (64-bit); ties go to the smallest M(A) = sum of 2^i over i in A, i > 0.  The lobby's
+ *                   members become A's members in their old relative order, then the others in theirs (team 1 =
+ *                   members [0, S)).  The lobby as formed is admissible, so its imbalance never grows.  Which lobbies
+ *                   form, their headers and order, the solos taken, the parties placed, the party table, the active
+ *                   set and seq_next do not change; with the option off every output is what it was.  A dry run or
+ *                   an MM_E_CAP refusal runs no balance pass.  mm_party_stats.sum_imbalance sums the emitted
+ *                   lobbies' imbalances.  Not part of an image: mm_export / mm_import do not carry it.  Cost: after
+ *                   the call's member copy, one thread per placed party (its members' c and its lobby's continuation
+ *                   bits), one warp per solo piece (as mm_widen) and one warp per lobby of a masked mode (the L ids
+ *                   read and, unless the split is the identity, written back); the pass is inside device_us.
+ *                   Device memory, allocated by the first balanced call and kept: 4 bytes per member slot of the
+ *                   largest call (at least capacity + 64), 4 bytes per lobby of the largest call and 8 bytes.
  *   "async_results" 1 = mm_tick does not wait for its device-to-host copies (see mm_results_wait); default 0   */
 int mm_set_option(mm_engine* e, const char* name, int64_t value);
 

@@ -736,6 +736,18 @@ static ERL_NIF_TERM nif_set_team_balance(ErlNifEnv* env, int argc, const ERL_NIF
   return rc ? err(env, rc) : atom(env, "ok");
 }
 
+/* set_party_balance(ref, mask): extension knob (balanced party lobbies); bit m splits every party_match lobby of mode
+ * m into its most even teams that keep every party whole, 0 = off; a mask naming a mode that cannot be balanced
+ * returns the engine error */
+static ERL_NIF_TERM nif_set_party_balance(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifSInt64 mask = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_int64(env, argv[1], &mask))
+    return enif_make_badarg(env);
+  int rc = mm_set_option(r->e, "party_balance", (int64_t)mask);
+  return rc ? err(env, rc) : atom(env, "ok");
+}
+
 /* set_party_capacity(ref, members): extension knob (parties); how many party members the engine holds */
 static ERL_NIF_TERM nif_set_party_capacity(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
   engine_res* r; ErlNifSInt64 cap = 0;
@@ -779,6 +791,7 @@ static ErlNifFunc funcs[] = {
   {"seq_next", 1, nif_seq_next, 0},
   {"set_max_spread", 2, nif_set_max_spread, 0},
   {"set_team_balance", 2, nif_set_team_balance, 0},
+  {"set_party_balance", 2, nif_set_party_balance, 0},
   {"set_lobby_budget", 3, nif_set_lobby_budget, 0},
   {"lobby_budget_report", 1, nif_lobby_budget_report, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"lobby_candidates", 1, nif_lobby_candidates, ERL_NIF_DIRTY_JOB_CPU_BOUND},

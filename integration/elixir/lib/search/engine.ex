@@ -198,4 +198,11 @@ defmodule Matchmaking.Search.Engine do
   rating difference (two-team modes of at most 8 players a team); 0 = off.  Team t is still members [t S, (t + 1) S).
   """
   def set_team_balance(_ref, _mask), do: :erlang.nif_error(:nif_not_loaded)
+
+  @doc """
+  Extension (not reference behaviour): bit m of mask splits every party_match lobby of mode m into its most even teams
+  that keep every party whole (two-team modes of at most 8 players a team); 0 = off.  Independent of
+  set_team_balance/2, which never splits party lobbies.
+  """
+  def set_party_balance(_ref, _mask), do: :erlang.nif_error(:nif_not_loaded)
 end

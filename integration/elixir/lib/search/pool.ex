@@ -39,6 +39,9 @@ defmodule Matchmaking.Search.Pool do
       balance_teams  option (extension, default nil = off): a list of mode names.  Every lobby of those modes, from the
                      tick and from widen, is split into the two teams with the least rating difference
                      (Engine.set_team_balance); the lobby's players are the same, only who plays with whom changes
+      balance_parties option (extension, default nil = off): a list of mode names.  Every party lobby of those modes
+                     is split into its most even teams that keep every party whole (Engine.set_party_balance); the
+                     published teams follow that order.  Independent of balance_teams
       lobby_budget   option (extension, default nil = no limit): a zero-arity function -> %{mode name => lobbies}, asked
                      before every tick — the free game-server slots (game-lobby/worker.ex:118-141).  The tick emits at
                      most that many lobbies of the mode, shared over the rating groups in proportion to what each could
@@ -133,6 +136,10 @@ defmodule Matchmaking.Search.Pool do
     case Keyword.get(opts, :balance_teams) do
       nil -> :ok
       modes -> :ok = Engine.set_team_balance(ref, Enum.reduce(modes, 0, &Bitwise.bor(&2, Bitwise.bsl(1, Engine.mode_index(&1)))))
+    end
+    case Keyword.get(opts, :balance_parties) do
+      nil -> :ok
+      modes -> :ok = Engine.set_party_balance(ref, Enum.reduce(modes, 0, &Bitwise.bor(&2, Bitwise.bsl(1, Engine.mode_index(&1)))))
     end
     case Keyword.get(opts, :party_capacity) do
       nil -> :ok

@@ -137,7 +137,7 @@ class PartyStats(C.Structure):
         ("n_parties", C.c_uint32),
         ("n_absorbed", C.c_uint32),
         ("device_us", C.c_float),
-        ("reserved", C.c_uint32 * 2),
+        ("sum_imbalance", C.c_uint64),  # party_balance: summed imbalance of the emitted lobbies of masked modes
     ]
 
 

@@ -12,8 +12,11 @@
 //                     arrival order: k_tb_arrival walks the pool the tick read (live_rank_walk, as k_mq_arrival does)
 //                     and writes every matched player's c - key_lo at its member slot;
 //                     mm_widen: k_tb_pieces writes c - key_lo of every piece's bin at the piece's member slots.
+//                     mm_party_match: k_tb_pieces for the solos, k_tb_parties (mm_party.cuh) for the party members.
 //   k_tb_lobby        one warp per lobby of a masked mode with S > 1: reads the L ids, writes them back permuted (not
-//                     when the permutation is the identity) and stores the lobby's imbalance.
+//                     when the permutation is the identity) and stores the lobby's imbalance.  mm_party_match's form
+//                     (party_balance) reads each lobby's continuation word, so no split cuts a party, and sums the
+//                     imbalances.
 #pragma once
 #include "mm_backfill.cuh"
 
@@ -59,8 +62,13 @@ __device__ const TbStarts kTbStarts = tb_starts();
 
 // One warp, every lane: lane i < L = 2S holds c_i (c - key_lo of member i in the lobby's current order).  Over the sets A of
 // S members with member 0 in A, minimise |sum_A c - sum_rest c| (64-bit); ties go to the smallest M(A) = sum of 2^i
-// over i in A, i > 0.  Returns the mask of A (bit 0 set) on every lane and the imbalance in *imb.
-__device__ __forceinline__ uint32_t tb_split(uint32_t ci, uint32_t L, uint32_t S, unsigned long long* imb) {
+// over i in A, i > 0.  cont: bit i set when member i belongs to the same party as member i - 1; a set A is admissible
+// when it holds all of every party or none of it, ((A ^ (A << 1)) & cont) == 0.  The identity (members [0, S)) is
+// admissible whenever the lobby's parties do not straddle the teams, so some lane finds a winner; a lane that finds no
+// admissible set keeps ~0.  cont == 0 (a compile-time constant for the tick, mm_widen and mm_locate) admits every set.
+// Returns the mask of A (bit 0 set) on every lane and the imbalance in *imb.
+__device__ __forceinline__ uint32_t tb_split(uint32_t ci, uint32_t L, uint32_t S, uint32_t cont,
+                                             unsigned long long* imb) {
   const uint32_t lane = threadIdx.x & 31;
   uint32_t c[16];
   long long total = 0;
@@ -82,8 +90,8 @@ __device__ __forceinline__ uint32_t tb_split(uint32_t ci, uint32_t L, uint32_t S
       for (int j = 0; j < 15; ++j) sa += ((x >> j) & 1u) ? (long long)c[j + 1] : 0ll;
       const long long d = 2 * sa - total;
       const unsigned long long ad = (unsigned long long)(d < 0 ? -d : d);
-      const uint32_t m = x << 1;
-      if (ad < best_d || (ad == best_d && m < best_m)) { best_d = ad; best_m = m; }
+      const uint32_t m = x << 1, mf = m | 1u;
+      if (((mf ^ (mf << 1)) & cont) == 0 && (ad < best_d || (ad == best_d && m < best_m))) { best_d = ad; best_m = m; }
       if (++r == r1) break;
       const uint32_t t = x | (x - 1);  // Gosper: the next larger mask with k bits
       x = (t + 1) | (((~t & (t + 1)) - 1) >> __ffs(x));
@@ -116,12 +124,16 @@ struct TbArgs {
   const uint16_t* bin_key;   // [Kp] c - key_lo of the bin
   uint32_t K;                // live bins
   uint32_t* imb;             // [n_lob] imbalance per header position (saturated), or null
+  const uint32_t* cont;      // kCont: [n_lob] continuation bits per header position (tb_split)
+  unsigned long long* imb_sum;  // kCont: += the imbalances of the balanced lobbies
 };
 
-// The balanced teams of every lobby of a masked mode with S > 1 (one warp per lobby, grid-stride).
-template <bool kCval>
+// The balanced teams of every lobby of a masked mode with S > 1 (one warp per lobby, grid-stride).  kCont: party
+// lobbies (mm_party_match), whose splits keep every party whole.
+template <bool kCval, bool kCont = false>
 __global__ void __launch_bounds__(256) k_tb_lobby(const TbArgs a) {
   const uint32_t lane = threadIdx.x & 31, nw = gridDim.x * (blockDim.x >> 5);
+  unsigned long long sum = 0;
   for (uint32_t h = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; h < a.n_lob; h += nw) {
     const mm_lobby_hdr hd = a.hdr[h];
     const uint32_t S = a.mode_tsize[hd.mode], L = hd.n_members;
@@ -134,11 +146,13 @@ __global__ void __launch_bounds__(256) k_tb_lobby(const TbArgs a) {
       c = kCval ? a.cval[m] : a.bin_key[last_le(a.outbase, 0, a.K, m)];
     }
     unsigned long long imb;
-    const uint32_t mf = tb_split(c, L, S, &imb);
+    const uint32_t mf = tb_split(c, L, S, kCont ? a.cont[h] : 0u, &imb);
     __syncwarp();  // every lane's load of its slot is ordered before another lane's store to it
     if (mf != (1u << S) - 1u && lane < L) a.members[hd.first_member + tb_new_index(mf, lane, S)] = id;
     if (a.imb && lane == 0) a.imb[h] = imb > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)imb;
+    if (kCont) sum += imb;
   }
+  if (kCont && lane == 0 && sum) atomicAdd(a.imb_sum, sum);
 }
 
 struct TbArrivalArgs {

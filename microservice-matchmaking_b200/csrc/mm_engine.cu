@@ -172,6 +172,7 @@ struct mm_engine {
   int32_t max_spread = -1;  // < 0: policy S0 (reference behaviour); >= 0: policy S1 (extension)
   uint32_t tb_mask = 0;     // team_balance: bit m = lobbies of mode m are split into balanced teams (extension)
   uint32_t tb_last = 0;     // the mask the last tick's balance pass ran with (0: it did not run)
+  uint32_t pb_mask = 0;     // party_balance: bit m = party lobbies of mode m are split, every party whole (extension)
   DevArray<SegInfo> d_seg;
   DevArray<uint32_t> d_left_bits;  // one bit per virtual pool position: stays queued after the tick
   DevArray<uint64_t> d_members;
@@ -319,8 +320,11 @@ struct mm_engine {
   // mm_match_quality and written only by a tick, so it describes the last tick's lobbies until the next one.
   struct Balance {
     DevArray<uint32_t> imb;   // [max_lobbies] the last tick's balanced imbalance per header position
-    DevArray<uint32_t> cval;  // [capacity + 64] c - key_lo per member slot (arrival-order ticks, mm_widen)
+    DevArray<uint32_t> cval;  // [capacity + 64, or a party call's members] c - key_lo per member slot (arrival-order
+                              // ticks, mm_widen, mm_party_match)
     DevArray<uint32_t> w;     // arrival order: live slots per tile -> offsets [n_tiles] | per partition [n_segs] | total
+    DevArray<uint32_t> cont;  // party_balance: [a party call's lobbies] continuation bits per header position
+    DevArray<unsigned long long> sum;  // party_balance: [1] the call's summed imbalance
   } tb;
 
   // parties (mm_party.cuh): the table in two buffers (compaction moves it from one to the other), sized by
@@ -3043,10 +3047,28 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
                                                                                  a.mbase, b.staging, b.members);
   x.members = b.members;
   k_pt_out<<<gr, 256, 0, e->stream>>>(x, a.mbase, act_view(e));
+  auto& tb = e->tb;
+  if (e->pb_mask) {  // party_balance: each member's c (solos from their piece's bin, party members their own), then
+                     // the split that keeps every party whole
+    CK(tb.cval.reserve(std::max<size_t>((size_t)e->capacity + 64, nm)));
+    CK(tb.cont.reserve(nl));
+    CK(tb.sum.reserve(1));
+    CK(cudaMemsetAsync(tb.cont, 0, (size_t)nl * 4, e->stream));
+    CK(cudaMemsetAsync(tb.sum, 0, 8, e->stream));
+    if (np)
+      k_tb_pieces<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, a.mbase, e->d_bin_key,
+                                                                                    tb.cval);
+    k_tb_parties<<<gr, 256, 0, e->stream>>>(x, a, e->pb_mask, e->key_lo, e->KR, tb.cval, tb.cont);
+    TbArgs v{};
+    v.hdr = w.hdr; v.n_lob = nl; v.members = b.members; v.mask = e->pb_mask; v.mode_tsize = e->d_mode_tsize;
+    v.cval = tb.cval; v.cont = tb.cont; v.imb_sum = tb.sum;
+    k_tb_lobby<true, true><<<grid256(e, (uint64_t)nl * 32, 8), 256, 0, e->stream>>>(v);
+  }
   CK(cudaGetLastError());
   CK(cudaEventRecord(e->ev[4], e->stream));
   CK(cudaMemcpyAsync(lobbies, w.hdr, (size_t)nl * sizeof(mm_lobby_hdr), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaMemcpyAsync(member_ids, b.members, (size_t)nm * 8, cudaMemcpyDeviceToHost, e->stream));
+  if (e->pb_mask) CK(cudaMemcpyAsync(&st->sum_imbalance, tb.sum, 8, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   s.live -= (uint32_t)(nm - ns);
   CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]));
@@ -3091,6 +3113,18 @@ int party_read(mm_engine* e, uint32_t party_cap, uint32_t member_cap, uint8_t* s
     for (uint32_t j = 0; j < hsize[i]; ++j, ++o) { member_ids[o] = hmid[hoff[i] + j]; member_rating[o] = hmr[hoff[i] + j]; }
     ++k;
   }
+  return MM_OK;
+}
+
+// The mask of team_balance / party_balance: set bits name modes < n_modes of two teams of at most kTbMaxS players.
+int tb_check_mask(mm_engine* e, const char* name, int64_t value) {
+  if (value < 0 || value >= (int64_t)1 << e->cfg.n_modes)
+    return set_err(e, MM_E_ARG, "%s 0x%llx names a mode >= n_modes = %u", name, (unsigned long long)value,
+                   e->cfg.n_modes);
+  for (uint32_t m = 0; m < e->cfg.n_modes; ++m)
+    if (((value >> m) & 1) && (e->cfg.modes[m].teams != 2 || e->cfg.modes[m].team_size > kTbMaxS))
+      return set_err(e, MM_E_ARG, "%s: mode %u has %u teams of %u (two teams of at most %u only)", name, m,
+                     e->cfg.modes[m].teams, e->cfg.modes[m].team_size, kTbMaxS);
   return MM_OK;
 }
 
@@ -3276,14 +3310,15 @@ int mm_set_option(mm_engine* e, const char* name, int64_t value) {
   if (!std::strcmp(name, "team_balance")) {
     // EXTENSION (balanced teams, mm_balance.cuh): bit m splits every lobby of mode m into the two teams with the least
     // rating difference.  Exact two-way partitioning only: two teams of at most kTbMaxS players.
-    if (value < 0 || value >= (int64_t)1 << e->cfg.n_modes)
-      return set_err(e, MM_E_ARG, "team_balance 0x%llx names a mode >= n_modes = %u", (unsigned long long)value,
-                     e->cfg.n_modes);
-    for (uint32_t m = 0; m < e->cfg.n_modes; ++m)
-      if (((value >> m) & 1) && (e->cfg.modes[m].teams != 2 || e->cfg.modes[m].team_size > kTbMaxS))
-        return set_err(e, MM_E_ARG, "team_balance: mode %u has %u teams of %u (two teams of at most %u only)", m,
-                       e->cfg.modes[m].teams, e->cfg.modes[m].team_size, kTbMaxS);
+    if (int rc = tb_check_mask(e, name, value)) return rc;
     e->tb_mask = (uint32_t)value;
+    return MM_OK;
+  }
+  if (!std::strcmp(name, "party_balance")) {
+    // EXTENSION (balanced party lobbies, mm_balance.cuh): bit m splits every mm_party_match lobby of mode m into the
+    // two teams with the least rating difference that keep every party whole.
+    if (int rc = tb_check_mask(e, name, value)) return rc;
+    e->pb_mask = (uint32_t)value;
     return MM_OK;
   }
   if (!std::strcmp(name, "tick_impl")) { e->tick_impl = value != 0; return MM_OK; }

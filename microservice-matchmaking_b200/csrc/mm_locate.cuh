@@ -184,7 +184,7 @@ __global__ void __launch_bounds__(256) k_locate(const LocateArgs a) {
       }
       __syncwarp();
       unsigned long long imb;
-      const uint32_t mf = tb_split(lane < L ? cw[lane] : 0u, L, S, &imb);
+      const uint32_t mf = tb_split(lane < L ? cw[lane] : 0u, L, S, 0u, &imb);
       r.member = (uint16_t)tb_new_index(mf, r.member, S);
     }
   }

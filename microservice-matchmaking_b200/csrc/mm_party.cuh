@@ -23,6 +23,10 @@
 // then team 1, ... in their rank order.  The solo pieces go through k_bf_keys, the band pipeline and k_bf_out like
 // mm_widen's; k_wd_bases / k_wd_hdr write the headers and bases and k_pt_out copies the party members.
 //
+// Balance (mm_set_option "party_balance", mm_balance.cuh): after k_pt_out, k_tb_pieces gives every solo its c and
+// k_tb_parties every placed member of a masked mode its own c and its lobby the party's continuation bits; then
+// k_tb_lobby<true, true> splits each lobby of a masked mode, every party kept whole.
+//
 // Hand-over (mm_export_parties / mm_merge_parties): k_pt_sel and two k_scan_small give every selected live row its
 // image index and member offset, k_pt_export gathers the columns in age order and releases the row (pt_release, as
 // k_pt_dissolve does).  The merge is the enqueue pipeline with the image's numbers (PtEnqArgs::seq) or new ones; its
@@ -652,6 +656,20 @@ __global__ void k_pt_out(const PtArgs p, const uint32_t* __restrict__ mbase, Act
     if (h != ~0ull) *act.val(h) = kPtMatched;
   }
   p.t.dead[r] = 1;
+}
+
+// party_balance: one thread per row placed in this call into a lobby of a masked mode — its members' c - key_lo at
+// their member slots, and bits pos + 1 .. pos + size - 1 (member i continues member i - 1's party) in the continuation
+// word of the lobby's header position (cont zeroed by the host).
+__global__ void k_tb_parties(const PtArgs p, const WdArgs a, uint32_t mask, int32_t key_lo, uint32_t KR,
+                             uint32_t* __restrict__ cval, uint32_t* __restrict__ cont) {
+  const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+  if (r >= p.n_rows || p.lob[r] == kPtNone || !((mask >> p.t.mode[r]) & 1u)) return;
+  const uint32_t l = p.lob[r], at = p.pos[r], n = p.t.size[r], o = p.t.off[r];
+  const uint2 x = a.rec[l];
+  uint32_t* dst = cval + a.mbase[l] + at;
+  for (uint32_t k = 0; k < n; ++k) dst[k] = clamp_key(key_lo, KR, p.t.mrat[o + k]);
+  atomicOr(&cont[a.qlbase[x.x] + x.y], ((1u << (n - 1)) - 1u) << (at + 1));
 }
 
 }  // namespace mm

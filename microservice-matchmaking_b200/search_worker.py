@@ -173,6 +173,10 @@ class SearchPool:
     those modes, from the tick and from widen, is split into the two teams with the least rating difference
     (mm_set_option("team_balance")).  Membership and lobby order are unchanged; team t is still members
     [t * team_size, (t + 1) * team_size).  resume() sets it again on the new engine.
+    balance_parties: optional list of mode names (extension; two-team modes of at most 8 players a team): every
+    party_match lobby of those modes is split into its most even teams that keep every party whole
+    (mm_set_option("party_balance")); the published "teams" follow that order.  Independent of balance_teams, which
+    never splits party lobbies.  resume() sets it again on the new engine.
     parties / party_capacity: optional parties (extension; needs MM_ORDER_RATING): players who queue together, staged
     with stage_party() and acked or nacked as one delivery, are matched into one lobby and one team.  party_capacity
     sets how many party members the engine holds (mm_set_option("party_capacity")); parties = {mode name: (min_wait_ms,
@@ -192,7 +196,7 @@ class SearchPool:
 
     def __init__(self, engine, mode_names, group_names, max_batch=65536, window=None, clock=None, flush_every_s=0.005,
                  handle_capacity=None, timeout_ms=None, wall_clock=None, lobby_budget=None, widen=None,
-                 balance_teams=None, parties=None, party_capacity=None, requeue_parties=False):
+                 balance_teams=None, parties=None, party_capacity=None, requeue_parties=False, balance_parties=None):
         import time
         if widen and engine.cfg.order_mode != abi.MM_ORDER_RATING:
             raise ValueError("widen needs an MM_ORDER_RATING engine: windows are rating distances")
@@ -226,11 +230,13 @@ class SearchPool:
         self.mode_names = list(mode_names)
         self.mode_index = {m: i for i, m in enumerate(self.mode_names)}
         self.group_names = list(group_names)
-        if balance_teams:
-            unknown = [m for m in balance_teams if m not in self.mode_index]
-            if unknown:
-                raise ValueError(f"balance_teams names unknown modes {unknown}")
-            engine.set_option("team_balance", sum(1 << self.mode_index[m] for m in set(balance_teams)))
+        for arg, option, names in (("balance_teams", "team_balance", balance_teams),
+                                   ("balance_parties", "party_balance", balance_parties)):
+            if names:
+                unknown = [m for m in names if m not in self.mode_index]
+                if unknown:
+                    raise ValueError(f"{arg} names unknown modes {unknown}")
+                engine.set_option(option, sum(1 << self.mode_index[m] for m in set(names)))
         self.max_batch = max_batch
         self.flush_every_s = flush_every_s
         self.handles = HandleTable(handle_capacity)
