@@ -957,6 +957,63 @@ int mm_import_regroup_many(mm_engine* e, uint32_t n_images, const void* const* b
                            const uint8_t* keep, uint32_t active_image, uint32_t cap, uint32_t* rej_image,
                            uint32_t* rej_index, uint32_t* n_rejected, uint32_t* n_elsewhere);
 
+/* EXTENSION (re-cut with parties queued): mm_import_regroup_many that also takes, beside engine image k, the party
+ * image (mm_export_parties) its rank wrote at the same stop: released first, then exported.  The solo arguments mean
+ * what they mean for mm_import_regroup_many; `parties` may be NULL, and then (as with every party image NULL or empty)
+ * the call IS mm_import_regroup_many, byte for byte.                                                                 */
+typedef struct mm_recut_parties {
+  const void* const* bufs;  /* [n_images] party image k, written at the same stop as engine image k; NULL = none   */
+  const uint64_t* n_bytes;  /* [n_images] its length (0 with NULL)                                                 */
+  uint32_t cap;             /* room in rej_image / rej_index, in parties                                           */
+  uint32_t* rej_image;      /* out: rejected parties as (image, party index in its party image), ascending         */
+  uint32_t* rej_index;
+  uint32_t n_rejected;      /* out: parties this config has no queue for                                           */
+  uint32_t n_elsewhere;     /* out: parties of an existing queue that `keep` does not select                       */
+  uint32_t n_loaded;        /* out                                                                                 */
+  uint32_t reserved;        /* 0                                                                                   */
+} mm_recut_parties;
+
+/* Party j of image k gets its R = floor(sum of member ratings / size) recomputed, as mm_merge_parties does, and is
+ *   REJECTED if its mode is >= n_modes, its size is above its mode's team_size, or R has no group: its members do not
+ *   enter the active set; the caller answers them (parties->rej_image / rej_index);
+ *   SKIPPED (parties->n_elsewhere) if its queue (mode, group(R)) exists but `keep` does not select it;
+ *   KEPT otherwise.
+ * ORDER AND NUMBERS.  n_images == 1: every number and seq_next are kept; the call equals mm_import_regroup_many of the
+ * one image followed by mm_merge_parties(MM_PARTY_KEEP_SEQ) of the kept parties.  n_images > 1: image k's kept parties
+ * of one new queue, in age order, form a run keyed by the running maximum of enq_ts along it; kept solos keep their
+ * keys (the running maximum along their (image, new partition) runs).  Every kept solo and kept party is numbered by
+ * its position in ONE total order, (running-max stamp, image, age) — within one image solos and parties share the age
+ * numbering — and seq_next = kept solos + kept parties.  With monotone stamps (what SearchPool writes) this is plain
+ * stamp order, ties by image and then age.
+ * LOAD.  The solos as mm_import_regroup_many loads them; the kept parties into the party table in the new age order,
+ * with their new numbers, mode, stamp and members, and R / group / bin under this config; each member's active-set
+ * value is its row's.  active_image's section 7 goes in as before (matched party members are already in it).
+ * Refusals, all decided by one read of the device's counters before anything is written; after any of them the engine
+ * is empty and still fresh, and its party table is empty:
+ *   MM_E_ARG   everything mm_import_regroup_many refuses; a non-null party image mm_merge_parties would refuse as
+ *              malformed (magic, version, lengths, a size below 2, sizes that do not add up to the member count,
+ *              numbers not strictly increasing in age order, an id out of range); party image k whose config or
+ *              seq_next differs from engine image k's (not written at the same stop); a party number equal to that of
+ *              a solo of its image; an id repeated in a party, across parties, or against any loaded solo or the taken
+ *              active section; a non-empty party image on an MM_ORDER_ARRIVAL or MM_F_NO_DEDUPE engine;
+ *   MM_E_STATE what mm_import_regroup_many gives; a non-empty party image while party_capacity is 0;
+ *   MM_E_CAP   the solo capacity rules; more rejected parties than parties->cap (parties->n_rejected = the count: cap
+ *              0 with NULL outputs is a dry run); kept members above party_capacity (exactly enough room loads); solos
+ *              plus party members past the 3/4 load of a hashed active set.
+ * EQUIVALENCE.  Let R be the restated engine image, built as for mm_import_regroup_many but with the numbers and
+ * seq_next above, and RP the restated party image: this engine's config, the kept parties in the new age order with
+ * their new numbers, members in party order, R's seq_next.  After the call, every later call sequence gives what a
+ * fresh engine with the same party_capacity gives after mm_import(R) and mm_merge_parties(RP, MM_PARTY_KEEP_SEQ).
+ * Cost: mm_import_regroup_many's passes, plus per party image one classify pass and the stable scatter by queue; with
+ * n_images > 1 the parties' queue runs go through the same running-max scan and merges, ceil(log2 n_queues) rounds
+ * order the parties, and one more merge round interleaves them with the solos' global order.
+ * Not covered: a re-cut that changes the number of ranks; mm_requeue / mm_requeue_party of players and parties matched
+ * before a re-cut with n_images > 1 (their old numbers have no place in the new numbering); SearchPool host records. */
+int mm_import_regroup_many_parties(mm_engine* e, uint32_t n_images, const void* const* bufs, const uint64_t* n_bytes,
+                                   const uint8_t* keep, uint32_t active_image, uint32_t cap, uint32_t* rej_image,
+                                   uint32_t* rej_index, uint32_t* n_rejected, uint32_t* n_elsewhere,
+                                   mm_recut_parties* parties);
+
 /* ---- queue move: part of an engine into another running engine ---------------------------
  * The reference's queues live in RabbitMQ and its state in replicated Mnesia tables, so any node's workers can serve
  * any rating group (application.ex:26-40).  Here a queued player lives in one engine: mm_export_queues releases

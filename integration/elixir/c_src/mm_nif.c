@@ -407,6 +407,91 @@ static ERL_NIF_TERM nif_import_regroup_many(ErlNifEnv* env, int argc, const ERL_
   return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &out), enif_make_uint(env, elsewhere));
 }
 
+/* import_regroup_many_parties(ref, images :: [binary], party_images :: [binary | nil], keep :: binary | nil,
+ * active_image :: integer | nil) -> {:ok, rejected, n_elsewhere, party_rejected, party_elsewhere} | {:error, atom}: the
+ * re-cut with the old ranks' queued parties (mm_import_regroup_many_parties); party_images[k] is the export_parties/2
+ * image rank k took just before images[k] (nil or <<>> = none).  rejected / party_rejected: binaries of (u32 image,
+ * u32 index) pairs, ascending — the players and the parties this config has no queue for. */
+static int interleave(ErlNifBinary* out, uint32_t* img_of, uint32_t got) {
+  uint32_t* idx = (uint32_t*)out->data;
+  for (uint32_t i = got; i-- > 0;) {  /* (image, index) pairs, from the back */
+    const uint32_t v = idx[i];
+    idx[2 * i + 1] = v;
+    idx[2 * i] = img_of[i];
+  }
+  return enif_realloc_binary(out, (size_t)got * 8);
+}
+
+static ERL_NIF_TERM nif_import_regroup_many_parties(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary keep, out, pout; unsigned len = 0, plen = 0;
+  uint32_t cap = 0, pcap = 0, got = 0, elsewhere = 0, act = UINT32_MAX;
+  const void* bufs[64]; uint64_t sizes[64]; const void* pbufs[64]; uint64_t psizes[64];
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_list_length(env, argv[1], &len) || len > 64 ||
+      !enif_get_list_length(env, argv[2], &plen) || plen != len)
+    return enif_make_badarg(env);
+  const int has_keep = !enif_is_identical(argv[3], atom(env, "nil"));
+  if (has_keep && !enif_inspect_binary(env, argv[3], &keep)) return enif_make_badarg(env);
+  if (!enif_is_identical(argv[4], atom(env, "nil")) && !enif_get_uint(env, argv[4], &act)) return enif_make_badarg(env);
+  ERL_NIF_TERM head, tail = argv[1], ptail = argv[2];
+  for (unsigned k = 0; k < len; ++k) {
+    ErlNifBinary img;
+    if (!enif_get_list_cell(env, tail, &head, &tail) || !enif_inspect_binary(env, head, &img)) return enif_make_badarg(env);
+    bufs[k] = img.data;
+    sizes[k] = img.size;
+    if (img.size >= sizeof(mm_image_header)) {
+      mm_image_header h;
+      memcpy(&h, img.data, sizeof(h));
+      const uint32_t n = h.n_players < img.size ? h.n_players : (uint32_t)img.size;  /* a corrupt count must not size it */
+      cap = cap + n < cap ? UINT32_MAX : cap + n;
+    }
+    pbufs[k] = NULL;
+    psizes[k] = 0;
+    if (!enif_get_list_cell(env, ptail, &head, &ptail)) return enif_make_badarg(env);
+    if (enif_is_identical(head, atom(env, "nil"))) continue;
+    if (!enif_inspect_binary(env, head, &img)) return enif_make_badarg(env);
+    if (img.size) { pbufs[k] = img.data; psizes[k] = img.size; }
+    if (img.size >= sizeof(mm_image_header)) {
+      mm_image_header h;
+      memcpy(&h, img.data, sizeof(h));
+      const uint32_t n = h.n_parts < img.size ? h.n_parts : (uint32_t)img.size;
+      pcap = pcap + n < pcap ? UINT32_MAX : pcap + n;
+    }
+  }
+  if (has_keep) {
+    uint32_t n_cut = 0;
+    mm_queue_stat probe;
+    mm_queue_stats(r->e, 0, &probe, 0, &n_cut);
+    if (keep.size != n_cut) return enif_make_badarg(env);
+  }
+  if (!enif_alloc_binary((size_t)cap * 8, &out)) return err(env, MM_E_CAP);
+  if (!enif_alloc_binary((size_t)pcap * 8, &pout)) { enif_release_binary(&out); return err(env, MM_E_CAP); }
+  uint32_t* img_of = (uint32_t*)enif_alloc((size_t)(cap ? cap : 1) * 4);
+  uint32_t* pimg_of = (uint32_t*)enif_alloc((size_t)(pcap ? pcap : 1) * 4);
+  if (!img_of || !pimg_of) {
+    if (img_of) enif_free(img_of);
+    if (pimg_of) enif_free(pimg_of);
+    enif_release_binary(&out); enif_release_binary(&pout);
+    return err(env, MM_E_CAP);
+  }
+  mm_recut_parties p;
+  memset(&p, 0, sizeof(p));
+  p.bufs = pbufs; p.n_bytes = psizes; p.cap = pcap; p.rej_image = pimg_of; p.rej_index = (uint32_t*)pout.data;
+  int rc = mm_import_regroup_many_parties(r->e, len, bufs, sizes, has_keep ? keep.data : NULL, act, cap, img_of,
+                                          (uint32_t*)out.data, &got, &elsewhere, &p);
+  if (rc) {
+    enif_free(img_of); enif_free(pimg_of); enif_release_binary(&out); enif_release_binary(&pout);
+    return err(env, rc);
+  }
+  interleave(&out, img_of, got);
+  interleave(&pout, pimg_of, p.n_rejected);
+  enif_free(img_of);
+  enif_free(pimg_of);
+  ERL_NIF_TERM t[5] = {atom(env, "ok"), enif_make_binary(env, &out), enif_make_uint(env, elsewhere),
+                       enif_make_binary(env, &pout), enif_make_uint(env, p.n_elsewhere)};
+  return enif_make_tuple_from_array(env, t, 5);
+}
+
 /* seq_next(ref) -> {:ok, seq}: the enqueue sequence number the next offered player will get (mm_seq_next) */
 static ERL_NIF_TERM nif_seq_next(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
   engine_res* r; uint32_t s = 0;
@@ -780,6 +865,7 @@ static ErlNifFunc funcs[] = {
   {"merge_parties", 3, nif_merge_parties, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"import_regroup", 2, nif_import_regroup, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"import_regroup_many", 4, nif_import_regroup_many, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"import_regroup_many_parties", 5, nif_import_regroup_many_parties, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"requeue_party", 7, nif_requeue_party, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"backfill", 2, nif_backfill, ERL_NIF_DIRTY_JOB_CPU_BOUND},

@@ -102,6 +102,15 @@ defmodule Matchmaking.Search.Engine do
   def import_regroup_many(_ref, _images, _keep, _active_image), do: :erlang.nif_error(:nif_not_loaded)
 
   @doc """
+  Re-cut with parties queued (extension): import_regroup_many/4 with, beside images[k], the export_parties/2 image
+  party_images[k] that rank k took just before it (nil or <<>> = none); solos and parties are numbered in one order
+  (mm_import_regroup_many_parties) -> {:ok, rejected, n_elsewhere, party_rejected :: binary((u32 image, u32 index)[]),
+  party_elsewhere} or {:error, :badarg | :capacity | :state}; after a refusal the engine is still fresh.
+  """
+  def import_regroup_many_parties(_ref, _images, _party_images, _keep, _active_image),
+    do: :erlang.nif_error(:nif_not_loaded)
+
+  @doc """
   Queue move: the selected (mode, group) queues (queues :: binary, one byte per queue in queue_stats/2 record order,
   mode * n_groups + group, non-zero = selected) leave the engine in a queue image -> {:ok, image}.  The players are
   released as if removed, in the same call; matched players not yet removed stay here.

@@ -233,6 +233,21 @@ class ImageHeader(C.Structure):
     ]
 
 
+class RecutParties(C.Structure):
+    """mm_recut_parties: the party images of mm_import_regroup_many_parties and what the call reports about them."""
+    _fields_ = [
+        ("bufs", C.c_void_p),
+        ("n_bytes", C.c_void_p),
+        ("cap", C.c_uint32),
+        ("rej_image", C.c_void_p),
+        ("rej_index", C.c_void_p),
+        ("n_rejected", C.c_uint32),
+        ("n_elsewhere", C.c_uint32),
+        ("n_loaded", C.c_uint32),
+        ("reserved", C.c_uint32),
+    ]
+
+
 def image_offsets(n_parts, n_players, n_active, id_bytes):
     """Section offsets of an image (include/mm_engine.h): part_count, id, rating, enq_ts, seq, mode, active, and the
     total length.  Every section starts at the next multiple of 8 after the one before it."""
@@ -309,6 +324,8 @@ PROTOTYPES = {
     "mm_import_regroup": (C.c_int, [_vp, _vp, C.c_uint64, C.c_uint32, _vp, _P(C.c_uint32)]),
     "mm_import_regroup_many": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp,
                                          _P(C.c_uint32), _P(C.c_uint32)]),
+    "mm_import_regroup_many_parties": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, C.c_uint32, C.c_uint32, _vp, _vp,
+                                                 _P(C.c_uint32), _P(C.c_uint32), _P(RecutParties)]),
     "mm_snapshot": (C.c_int, [_vp]),
     "mm_restore": (C.c_int, [_vp]),
     "mm_set_stream": (C.c_int, [_vp, _vp]),

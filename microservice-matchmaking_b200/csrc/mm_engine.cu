@@ -1226,6 +1226,18 @@ ImgCols img_cols(uint8_t* body, const ImgLayout& l, uint32_t idb) {  // body = t
   c.id_bytes = idb;
   return c;
 }
+// Section offsets of a party image (include/mm_engine.h): [0] size, [1] seq, [2] enq_ts, [3] mode, [4] id, [5] rating,
+// [6] total bytes.
+struct PtImgLayout { uint64_t off[7]; };
+PtImgLayout pt_img_layout(uint32_t P, uint32_t M, uint32_t W) {
+  auto a8 = [](uint64_t x) { return (x + 7) & ~7ull; };
+  const uint64_t bytes[6] = {(uint64_t)P, 4ull * P, 4ull * P, (uint64_t)P, (uint64_t)W * M, 4ull * M};
+  PtImgLayout l{};
+  l.off[0] = sizeof(mm_image_header);
+  for (int k = 0; k < 6; ++k) l.off[k + 1] = a8(l.off[k] + bytes[k]);
+  return l;
+}
+
 uint32_t id_bytes(const mm_engine* e) { return e->dense_ids ? 4u : 8u; }
 uint64_t id_limit(const mm_engine* e) { return e->dense_ids ? e->hcap : kTombKey; }
 
@@ -1790,10 +1802,11 @@ int requeue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating,
 // K images of one config: each runs the regroup pipeline on its own; for K > 1 the images' runs are merged and the
 // kept players renumbered on the device.  Every refusal is decided by one read of the counters, before the load tail
 // writes the pool.  `who` names the call in the state refusal; keep_cut: n_cut selection bytes (null: all); act_img:
-// the image whose active section is taken (>= K: none).
+// the image whose active section is taken (>= K: none); pp: the party images (mm_import_regroup_many_parties) or
+// null.  Without a non-empty party image every step is mm_import_regroup_many's.
 int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const* bufs, const uint64_t* nbs,
                  const uint8_t* keep_cut, uint32_t act_img, uint32_t cap, uint32_t* rej_image, uint32_t* rej_index,
-                 uint32_t* n_rejected, uint32_t* n_elsewhere) {
+                 uint32_t* n_rejected, uint32_t* n_elsewhere, mm_recut_parties* pp) {
   if (!e->fresh || e->stage_count)
     return set_err(e, MM_E_STATE, "%s needs a fresh engine (nothing enqueued, imported or restored)", who);
   if (K == 0 || K > kRcMaxImages) return set_err(e, MM_E_ARG, "n_images must be 1 .. %u", kRcMaxImages);
@@ -1814,6 +1827,45 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
   }
   const uint32_t S = e->n_segs, SI = y.n_segs, idb = h[0].id_bytes;
   const uint32_t m = act_img < K ? h[act_img].n_active : 0;
+  // the party images: header checks on the host; P parties and M members in all
+  std::vector<uint32_t> pbase(K + 1, 0), mcount(K, 0), pnblk(K, 0);
+  std::vector<PtImgLayout> pl(K);
+  uint64_t P = 0, M = 0;
+  if (pp) {
+    pp->n_rejected = pp->n_elsewhere = pp->n_loaded = 0;
+    for (uint32_t k = 0; k < K; ++k) {
+      pbase[k] = (uint32_t)P;
+      const uint64_t nb = pp->n_bytes ? pp->n_bytes[k] : 0;
+      const uint8_t* b = pp->bufs ? static_cast<const uint8_t*>(pp->bufs[k]) : nullptr;
+      if (!b || !nb) continue;
+      auto bad = [&](const char* what) { return set_err(e, MM_E_ARG, "party image %u rejected: %s", k, what); };
+      mm_image_header ph;
+      if (nb < sizeof(ph)) return bad("shorter than its header");
+      std::memcpy(&ph, b, sizeof(ph));
+      if (ph.magic != MM_PARTY_IMAGE_MAGIC) return bad("bad magic (not an mm_export_parties image)");
+      if (ph.version != MM_IMAGE_VERSION || ph.abi_version != MM_ABI_VERSION) return bad("unknown version");
+      if (ph.id_bytes != idb) return bad("id width differs from the engine's");
+      if (ph.config.flags & MM_F_NO_DEDUPE) return bad("written by an MM_F_NO_DEDUPE engine");
+      pl[k] = pt_img_layout(ph.n_parts, ph.n_players, ph.id_bytes);
+      if (ph.n_active || ph.total_bytes != pl[k].off[6] || nb != pl[k].off[6])
+        return bad("length does not match the header's section counts");
+      if (!same_layout(ph.config, h[k].config) || ph.seq_next != h[k].seq_next)
+        return bad("config or seq_next differs from its engine image's (not written at the same stop)");
+      P += ph.n_parts;
+      M += ph.n_players;
+      mcount[k] = ph.n_players;
+      pnblk[k] = (ph.n_parts + kRqItems - 1) / kRqItems;
+      if (P > 0x7FFFFFFFu || M > 0x7FFFFFFFu) return set_err(e, MM_E_CAP, "more than 2^31 - 1 parties or members");
+    }
+    pbase[K] = (uint32_t)P;
+    if (P) {
+      if (e->cfg.order_mode != MM_ORDER_RATING) return set_err(e, MM_E_ARG, "party images need MM_ORDER_RATING");
+      if (!e->use_active) return set_err(e, MM_E_ARG, "an MM_F_NO_DEDUPE engine cannot hold parties");
+      if (!e->pt.cap) return set_err(e, MM_E_STATE, "no party capacity: set the option party_capacity first");
+    }
+  }
+  const bool parties = P != 0;
+  const uint32_t C = e->n_cut;
   std::vector<uint32_t> base(K + 1, 0), nblk(K);
   uint64_t total = 0;
   for (uint32_t k = 0; k < K; ++k) {
@@ -1836,9 +1888,10 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
                                 : (const void*)e->d_img.p;
   const uint32_t seq_next = K == 1 ? h[0].seq_next : 0;  // K > 1: renumbered, seq_next = the kept count
   if (n_elsewhere) *n_elsewhere = 0;
-  if (N == 0) return load_columns(e, std::vector<uint32_t>(S, 0), in[0], 0, act, m, seq_next, "image rejected");
+  if (N == 0 && !parties)
+    return load_columns(e, std::vector<uint32_t>(S, 0), in[0], 0, act, m, seq_next, "image rejected");
   // scratch: the images' tables, the classification, the scatter and merge buffers, the gathered columns
-  const uint64_t sc = e->use_active ? seen_keys((uint64_t)N + m) : 0;  // the repeated-id set
+  const uint64_t sc = e->use_active ? seen_keys((uint64_t)N + m + M) : 0;  // the repeated-id set
   std::vector<uint32_t> off((size_t)K * (SI + 1), 0);
   for (uint32_t k = 0; k < K; ++k)
     for (uint32_t s = 0; s < SI; ++s) off[(size_t)k * (SI + 1) + s + 1] = off[(size_t)k * (SI + 1) + s] + cnt[k][s];
@@ -1859,17 +1912,35 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
                o_pair = take(4 * pair_n * K), o_ord = take(2 * pair_n * K), o_run = take(4 * (size_t)S * (SI + 1) * K),
                o_kq = take(4 * (size_t)S * K), o_part = take(2 * (size_t)N), o_pimg = take(2 * (size_t)N),
                o_src0 = take(4 * (size_t)N), o_src1 = take(4 * (size_t)N), o_age0 = take(4 * (size_t)N),
-               o_age1 = take(4 * (size_t)N), o_rej = take(K == 1 ? 4 * (size_t)N : 0), o_out = take(cols_bytes(N));
+               o_age1 = take(4 * (size_t)N), o_rej = take(K == 1 ? 4 * (size_t)N : 0), o_out = take(cols_bytes(N + P));
   // K > 1: the image runs' merge and the numbering
   const bool many = K > 1;
   auto take2 = [&](size_t bytes) { return many ? take(bytes) : 0; };
   const size_t o_rqg = take2(4 * ((size_t)S + 1)), o_one = take2(4 * 4), o_pair2 = take2(4 * (size_t)K * S),
                o_ord2 = take2(2 * (size_t)K * S), o_run2 = take2(4 * (size_t)S * (K + 1)), o_kq2 = take2(4 * (size_t)S),
-               o_ident = take2(2 * (size_t)S), o_s2a = take2(4 * (size_t)N), o_s2b = take2(4 * (size_t)N),
-               o_keya = take2(sizeof(RcKey) * N), o_keyb = take2(sizeof(RcKey) * N), o_head = take2(N),
-               o_img = take2(2 * (size_t)N), o_qv = take2(2 * (size_t)N), o_agg = take2(sizeof(RcSeg) * nrb),
-               o_carry = take2(sizeof(RcSeg) * nrb), o_first = take2(4 * (size_t)nrb), o_pos = take2(4 * (size_t)N),
+               o_ident = take2(4 * ((size_t)S + C)), o_s2a = take2(4 * (N + P)), o_s2b = take2(4 * (N + P)),
+               o_keya = take2(sizeof(RcKey) * (N + P)), o_keyb = take2(sizeof(RcKey) * (N + P)), o_head = take2(N),
+               o_img = take2(2 * (N + P)), o_qv = take2(2 * (N + P)), o_agg = take2(sizeof(RcSeg) * nrb),
+               o_carry = take2(sizeof(RcSeg) * nrb), o_first = take2(4 * (size_t)nrb), o_pos = take2(4 * (N + P)),
                o_imgs = take2(sizeof(ImgCols) * K), o_base = take2(4 * (size_t)K);
+  // the parties: their images, classification, scatter by queue, and (K > 1) the queue merge and their order
+  auto take3 = [&](size_t bytes) { return parties ? take(bytes) : 0; };
+  auto take4 = [&](size_t bytes) { return parties && many ? take(bytes) : 0; };
+  std::vector<uint64_t> pboff(K + 1, 0);
+  for (uint32_t k = 0; k < K; ++k) pboff[k + 1] = pboff[k] + (parties && pbase[k + 1] > pbase[k] ? (pl[k].off[6] - pl[k].off[0] + 15) & ~(uint64_t)15 : 0);
+  uint64_t phist_n = 0;
+  for (uint32_t k = 0; k < K; ++k) phist_n += (uint64_t)(C + 1) * pnblk[k];
+  const size_t R2 = C + 2, nrbp = (P + kRcBlock - 1) / kRcBlock;
+  const size_t o_pbody = take3(pboff[K]), o_pcols = take3(sizeof(PtImgCols) * K), o_pbase = take3(4 * ((size_t)K + 1)),
+               o_seqset = take3(8 * seen_keys(P)), o_pctr = take3(4 * (kRpWords + 3 * (size_t)K)),
+               o_pmoff = take3(4 * P), o_ppart = take3(2 * P), o_pk = take3(2 * P), o_pR = take3(4 * P),
+               o_pflag = take3(4 * P), o_phist = take3(4 * phist_n), o_rqp = take3(4 * R2 * K), o_psel = take3(C + 1), o_pkeep = take3(keep_cut ? C : 0), o_psz = take3(P),
+               o_psrc = take3(4 * P), o_page = take3(4 * P), o_rsrc = take3(4 * P), o_rsz = take3(4 * P + 8),
+               o_pqone = take4(4 * 4), o_pglob = take4(4 * ((size_t)C + 1)), o_ppair = take4(4 * (size_t)K * C),
+               o_pord = take4(2 * (size_t)K * C), o_prun = take4(4 * (size_t)C * (K + 1)), o_pkq = take4(4 * (size_t)C),
+               o_ps2a = take4(4 * P), o_ps2b = take4(4 * P), o_pkeya = take4(sizeof(RcKey) * P),
+               o_pkeyb = take4(sizeof(RcKey) * P), o_phead = take4(P), o_pagg = take4(sizeof(RcSeg) * nrbp),
+               o_pcarry = take4(sizeof(RcSeg) * nrbp), o_pfirst = take4(4 * nrbp), o_fin = take4(4 * 8);
   CK(e->d_rg.reserve(o));
   uint8_t* const sb = e->d_rg;
   auto at = [sb](size_t x) { return sb + x; };
@@ -1886,7 +1957,7 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
   uint32_t* src[2] = {reinterpret_cast<uint32_t*>(at(o_src0)), reinterpret_cast<uint32_t*>(at(o_src1))};
   uint32_t* age[2] = {reinterpret_cast<uint32_t*>(at(o_age0)), reinterpret_cast<uint32_t*>(at(o_age1))};
   uint8_t* ocur = at(o_out);
-  ImgCols out = carve_cols(ocur, N);
+  ImgCols out = carve_cols(ocur, N + P);  // seq: the kept parties' numbers at N + row
   out.id_bytes = idb;
   CK(cudaMemcpyAsync(lut_i, y.lut.data(), (size_t)y.KR * 2, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(grp_i, y.grp.data(), y.KR, cudaMemcpyHostToDevice, e->stream));
@@ -1934,6 +2005,72 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
       CK(cudaMemsetAsync(rq_off + R1 * k, 0, 4 * R1, e->stream));
     }
   }
+  // 1'. per party image: sizes -> member offsets, classify (and the seq set), the repeated ids, the stable scatter by
+  // queue (reject bucket C last); then every solo of the image probes the seq set
+  const uint64_t psc = parties ? seen_keys(P) : 0;
+  auto* pctr = reinterpret_cast<uint32_t*>(at(o_pctr));  // RpCtr | skip[K] | kept members[K] | member sums[K]
+  auto* pmoff = reinterpret_cast<uint32_t*>(at(o_pmoff));
+  auto* ppart = reinterpret_cast<uint16_t*>(at(o_ppart));
+  auto* ppk = reinterpret_cast<uint16_t*>(at(o_pk));
+  auto* pR = reinterpret_cast<int32_t*>(at(o_pR));
+  auto* pflag = reinterpret_cast<uint32_t*>(at(o_pflag));
+  auto* rqp = reinterpret_cast<uint32_t*>(at(o_rqp));
+  auto* psrc = reinterpret_cast<uint32_t*>(at(o_psrc));
+  auto* page = reinterpret_cast<uint32_t*>(at(o_page));
+  auto* rsrc = reinterpret_cast<uint32_t*>(at(o_rsrc));
+  auto* rsz = reinterpret_cast<uint32_t*>(at(o_rsz));
+  auto* seqset = reinterpret_cast<unsigned long long*>(at(o_seqset));
+  uint8_t* psz = at(o_psz);
+  std::vector<PtImgCols> pc(K);
+  if (parties) {
+    for (uint32_t k = 0; k < K; ++k) {
+      if (pbase[k + 1] == pbase[k]) continue;
+      const uint8_t* b = static_cast<const uint8_t*>(pp->bufs[k]);
+      uint8_t* d = at(o_pbody) + pboff[k];
+      CK(cudaMemcpyAsync(d, b + pl[k].off[0], pl[k].off[6] - pl[k].off[0], cudaMemcpyHostToDevice, e->stream));
+      PtImgCols& c = pc[k];
+      c.size = d; c.seq = reinterpret_cast<uint32_t*>(d + (pl[k].off[1] - pl[k].off[0]));
+      c.ts = reinterpret_cast<uint32_t*>(d + (pl[k].off[2] - pl[k].off[0])); c.mode = d + (pl[k].off[3] - pl[k].off[0]);
+      c.id = d + (pl[k].off[4] - pl[k].off[0]);
+      c.rating = reinterpret_cast<int32_t*>(d + (pl[k].off[5] - pl[k].off[0])); c.id_bytes = idb;
+    }
+    CK(cudaMemcpyAsync(at(o_pcols), pc.data(), sizeof(PtImgCols) * K, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(at(o_pbase), pbase.data(), 4 * ((size_t)K + 1), cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemsetAsync(pctr, 0, 4 * (kRpWords + 3 * (size_t)K), e->stream));
+    CK(cudaMemsetAsync(seqset, 0xFF, psc * 8, e->stream));
+    CK(cudaMemsetAsync(rsz, 0, 4 * P + 8, e->stream));
+    if (keep_cut) CK(cudaMemcpyAsync(at(o_pkeep), keep_cut, C, cudaMemcpyHostToDevice, e->stream));
+    uint64_t phoff = 0;
+    for (uint32_t k = 0; k < K; ++k) {
+      const uint32_t np = pbase[k + 1] - pbase[k], pb = pbase[k];
+      auto* bhist = reinterpret_cast<uint32_t*>(at(o_phist)) + phoff;
+      phoff += (uint64_t)(C + 1) * pnblk[k];
+      if (np) {
+        k_rp_sizes<<<(np + 255) / 256, 256, 0, e->stream>>>(np, pc[k].size, pmoff + pb);
+        k_scan_small<<<1, 1024, 0, e->stream>>>(np, pmoff + pb, pctr + kRpWords + 2 * K + k);
+        RpClassifyArgs ca{};
+        ca.in = pc[k]; ca.k = k; ca.n = np; ca.m = mcount[k]; ca.nblk = pnblk[k]; ca.seq_next = h[k].seq_next;
+        ca.moff = pmoff + pb; ca.id_limit = id_limit(e); ca.bm = bin_map(e); ca.grp_lut = e->d_grp_lut;
+        ca.mode_tsize = e->d_mode_tsize; ca.n_modes = e->cfg.n_modes; ca.n_groups = e->cfg.n_groups; ca.n_cut = C;
+        ca.keep = keep_cut ? at(o_pkeep) : nullptr;
+        ca.seqset = seqset; ca.seq_mask = psc - 1; ca.part = ppart + pb; ca.pk = ppk + pb; ca.R = pR + pb;
+        ca.flag = pflag + pb; ca.size = psz + pb; ca.blockhist = bhist; ca.ctr = pctr; ca.skip = pctr + kRpWords + k;
+        ca.kmem = pctr + kRpWords + K + k;
+        k_rp_classify<<<pnblk[k], 256, 0, e->stream>>>(ca);
+        if (mcount[k])
+          k_rg_dups<<<grid256(e, mcount[k], 32), 256, 0, e->stream>>>(pc[k].id, nullptr, idb, mcount[k], 0, seen, sc - 1,
+                                                                     &e->d_cnt->mrg_dups);
+        k_rq_scan<<<1, 512, 0, e->stream>>>(C + 1, pnblk[k], bhist, rqp + R2 * k, at(o_psel));
+        k_rq_group<<<pnblk[k], 256, 0, e->stream>>>(np, C + 1, pnblk[k], ppart + pb, pc[k].seq, h[k].seq_next, bhist,
+                                                     psrc + pb, page + pb);
+      } else {
+        CK(cudaMemsetAsync(rqp + R2 * k, 0, 4 * R2, e->stream));
+      }
+      if (np && h[k].n_players)
+        k_rp_probe<<<grid256(e, h[k].n_players, 32), 256, 0, e->stream>>>(k, h[k].n_players, in[k].seq, h[k].seq_next,
+                                                                           seqset, psc - 1, pctr + kRpSeqDup);
+    }
+  }
   // 2. per image: the merge rounds by age (enough for any k_max <= SI; the rounds past the need return at once)
   uint32_t rounds = 0;
   while ((1u << rounds) < SI) ++rounds;
@@ -1979,18 +2116,22 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
     auto* d_imgs = reinterpret_cast<ImgCols*>(at(o_imgs));
     auto* d_base = reinterpret_cast<uint32_t*>(at(o_base));
     uint32_t* const kmax2 = rq_one + 3;
-    std::vector<uint16_t> id16(S);
+    // ident: run q of the numbering rounds is partition q, run S + c party queue c; with parties, then the side of
+    // the final merge round (0: the solos' list, 1: the parties')
+    std::vector<uint16_t> id16(parties ? 2 * ((size_t)S + C) : S);
     for (uint32_t q = 0; q < S; ++q) id16[q] = (uint16_t)q;
+    if (parties)
+      for (uint32_t c = 0; c < C; ++c) { id16[S + c] = (uint16_t)c; id16[2 * S + C + c] = 1; }
     const uint32_t SS[2] = {S, 0};
-    CK(cudaMemcpyAsync(ident, id16.data(), (size_t)S * 2, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(ident, id16.data(), id16.size() * 2, cudaMemcpyHostToDevice, e->stream));
     CK(cudaMemcpyAsync(rq_one + 2, SS, 8, cudaMemcpyHostToDevice, e->stream));  // S for the numbering rounds; kmax2 = 0
     CK(cudaMemcpyAsync(d_imgs, in.data(), sizeof(ImgCols) * K, cudaMemcpyHostToDevice, e->stream));
     CK(cudaMemcpyAsync(d_base, base.data(), 4 * (size_t)K, cudaMemcpyHostToDevice, e->stream));
     CK(cudaMemsetAsync(ord2, 0, 2 * (size_t)K * S, e->stream));
-    CK(cudaMemsetAsync(s2[0], 0, 4 * (size_t)N, e->stream));  // holes (a refused image) stay in range
-    CK(cudaMemsetAsync(s2[1], 0, 4 * (size_t)N, e->stream));
-    CK(cudaMemsetAsync(img, 0, 2 * (size_t)N, e->stream));
-    CK(cudaMemsetAsync(qv, 0, 2 * (size_t)N, e->stream));
+    CK(cudaMemsetAsync(s2[0], 0, 4 * (N + P), e->stream));  // holes (a refused image) stay in range
+    CK(cudaMemsetAsync(s2[1], 0, 4 * (N + P), e->stream));
+    CK(cudaMemsetAsync(img, 0, 2 * (N + P), e->stream));
+    CK(cudaMemsetAsync(qv, 0, 2 * (N + P), e->stream));
     k_rc_sum<<<1, 1024, 0, e->stream>>>(K, S, rq_off, rq_glob, rq_one, pair2);
     k_rg_plan<<<1, 1024, 0, e->stream>>>(K, S, pair2, rq_glob, ord2, run2, kq2, kmax2);
     for (uint32_t k = 0; k < K; ++k) {
@@ -1999,14 +2140,16 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
       ga.k = k; ga.base = base[k]; ga.n = h[k].n_players; ga.n_segs = S; ga.n_img = K; ga.rq_off = rq_off + R1 * k;
       ga.kmax = &e->d_cnt->rg_kmax; ga.src[0] = src[0] + base[k]; ga.src[1] = src[1] + base[k];
       ga.age[0] = age[0] + base[k]; ga.age[1] = age[1] + base[k]; ga.ord = ord2; ga.run_start = run2;
-      ga.ts = in[k].ts; ga.src_out = s2[0]; ga.key_out = key[0]; ga.head = head; ga.img = img; ga.qv = qv;
+      ga.ts = in[k].ts; ga.src_out = s2[0]; ga.key_out = key[0]; ga.head = head; ga.img = img; ga.qv = qv; ga.qoff = 0;
       ga.err = &e->d_cnt->img_err;
       const uint32_t g = grid256(e, h[k].n_players, 32);
       k_rc_gather<<<g, 256, 0, e->stream>>>(ga);
     }
-    k_rc_runmax<<<nrb, 256, 0, e->stream>>>(rq_one + 1, key[0], head, agg, first);
-    k_rc_carry<<<1, 1024, 0, e->stream>>>(rq_one + 1, agg, carry);
-    k_rc_apply<<<nrb, 256, 0, e->stream>>>(rq_one + 1, key[0], carry, first);
+    if (nrb) {  // (no solo: parties only)
+      k_rc_runmax<<<nrb, 256, 0, e->stream>>>(rq_one + 1, key[0], head, agg, first);
+      k_rc_carry<<<1, 1024, 0, e->stream>>>(rq_one + 1, agg, carry);
+      k_rc_apply<<<nrb, 256, 0, e->stream>>>(rq_one + 1, key[0], carry, first);
+    }
     uint32_t r2 = 0;
     while ((1u << r2) < K) ++r2;
     for (uint32_t t = 0; t < r2; ++t) {
@@ -2029,16 +2172,110 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
       ma.src_in = s2[t & 1]; ma.u_in = key[t & 1]; ma.src_out = s2[(t + 1) & 1]; ma.u_out = key[(t + 1) & 1];
       k_rg_merge<<<grid, 256, 0, e->stream>>>(ma);
     }
-    k_rc_number<<<grid, 256, 0, e->stream>>>(rq_one + 1, s2[r3 & 1], pos, out.seq);
+    if (!parties) {
+      k_rc_number<<<grid, 256, 0, e->stream>>>(rq_one + 1, s2[r3 & 1], pos, out.seq);
+    } else {
+      // the parties' queue runs: merged by (running max, image, age) as the solos' partition runs are
+      auto* pqone = reinterpret_cast<uint32_t*>(at(o_pqone));  // {0, kept parties, C, kmax}
+      auto* pglob = reinterpret_cast<uint32_t*>(at(o_pglob));
+      auto* ppair = reinterpret_cast<uint32_t*>(at(o_ppair));
+      auto* pord = reinterpret_cast<uint16_t*>(at(o_pord));
+      auto* prun = reinterpret_cast<uint32_t*>(at(o_prun));
+      auto* pkq = reinterpret_cast<uint32_t*>(at(o_pkq));
+      uint32_t* ps2[2] = {reinterpret_cast<uint32_t*>(at(o_ps2a)), reinterpret_cast<uint32_t*>(at(o_ps2b))};
+      RcKey* pkey[2] = {reinterpret_cast<RcKey*>(at(o_pkeya)), reinterpret_cast<RcKey*>(at(o_pkeyb))};
+      auto* fin = reinterpret_cast<uint32_t*>(at(o_fin));
+      const uint32_t CC[2] = {C, 0}, gp = grid256(e, P, 32);
+      CK(cudaMemcpyAsync(pqone + 2, CC, 8, cudaMemcpyHostToDevice, e->stream));
+      CK(cudaMemsetAsync(pord, 0, 2 * (size_t)K * C, e->stream));
+      CK(cudaMemsetAsync(ps2[0], 0, 4 * P, e->stream));
+      CK(cudaMemsetAsync(ps2[1], 0, 4 * P, e->stream));
+      k_rc_sum<<<1, 1024, 0, e->stream>>>(K, C, rqp, pglob, pqone, ppair);
+      k_rg_plan<<<1, 1024, 0, e->stream>>>(K, C, ppair, pglob, pord, prun, pkq, pqone + 3);
+      for (uint32_t k = 0; k < K; ++k) {
+        const uint32_t np = pbase[k + 1] - pbase[k], pb = pbase[k];
+        if (!np) continue;
+        RcGatherArgs ga{};
+        ga.k = k; ga.base = N + pb; ga.n = np; ga.n_segs = C; ga.n_img = K; ga.rq_off = rqp + R2 * k;
+        ga.kmax = &e->d_cnt->rg_kmax; ga.src[0] = ga.src[1] = psrc + pb; ga.age[0] = ga.age[1] = page + pb;
+        ga.ord = pord; ga.run_start = prun; ga.ts = pc[k].ts; ga.src_out = ps2[0]; ga.key_out = pkey[0];
+        ga.head = at(o_phead); ga.img = img; ga.qv = qv; ga.qoff = S; ga.err = &e->d_cnt->img_err;
+        k_rc_gather<<<grid256(e, np, 32), 256, 0, e->stream>>>(ga);
+      }
+      auto* pagg = reinterpret_cast<RcSeg*>(at(o_pagg));
+      auto* pfirst = reinterpret_cast<uint32_t*>(at(o_pfirst));
+      k_rc_runmax<<<(uint32_t)nrbp, 256, 0, e->stream>>>(pqone + 1, pkey[0], at(o_phead), pagg, pfirst);
+      k_rc_carry<<<1, 1024, 0, e->stream>>>(pqone + 1, pagg, reinterpret_cast<RcSeg*>(at(o_pcarry)));
+      k_rc_apply<<<(uint32_t)nrbp, 256, 0, e->stream>>>(pqone + 1, pkey[0], reinterpret_cast<RcSeg*>(at(o_pcarry)),
+                                                        pfirst);
+      for (uint32_t t = 0; t < r2; ++t) {
+        RgMergeArgsT<RcKey> ma{};
+        ma.rq_off = pglob; ma.n_segs = C; ma.n_img_segs = K; ma.round = t; ma.pimg = img; ma.ord = pord;
+        ma.run_start = prun; ma.kq = pkq; ma.kmax = pqone + 3;
+        ma.src_in = ps2[t & 1]; ma.u_in = pkey[t & 1]; ma.src_out = ps2[(t + 1) & 1]; ma.u_out = pkey[(t + 1) & 1];
+        k_rg_merge<<<gp, 256, 0, e->stream>>>(ma);
+      }
+      k_rp_norm<<<gp, 256, 0, e->stream>>>(pqone + 1, pqone + 3, ps2[0], ps2[1], pkey[0], pkey[1]);
+      // the queues' lists into the parties' one order: their rows
+      uint32_t r3p = 0;
+      while ((1u << r3p) < C) ++r3p;
+      for (uint32_t t = 0; t < r3p; ++t) {
+        RgMergeArgsT<RcKey> ma{};
+        ma.rq_off = pqone; ma.n_segs = 1; ma.n_img_segs = C; ma.round = t; ma.pimg = qv; ma.ord = ident;
+        ma.run_start = pglob; ma.kq = pqone + 2; ma.kmax = pqone + 2;
+        ma.src_in = ps2[t & 1]; ma.u_in = pkey[t & 1]; ma.src_out = ps2[(t + 1) & 1]; ma.u_out = pkey[(t + 1) & 1];
+        k_rg_merge<<<gp, 256, 0, e->stream>>>(ma);
+      }
+      // after the solos' global list, then one round merges the two lists; k_rc_number numbers both
+      const uint32_t bs = r3 & 1;
+      RpPlaceArgs pa{};
+      pa.kept_p = pqone + 1; pa.kept_s = rq_one + 1; pa.psrc = ps2[r3p & 1]; pa.pkey = pkey[r3p & 1]; pa.n_solo = N;
+      pa.size = psz; pa.gsrc = s2[bs]; pa.gkey = key[bs]; pa.pos = pos; pa.rsrc = rsrc; pa.rsz = rsz; pa.fin = fin;
+      k_rp_place<<<gp, 256, 0, e->stream>>>(pa);
+      RgMergeArgsT<RcKey> ma{};
+      ma.rq_off = fin; ma.n_segs = 1; ma.n_img_segs = 2; ma.round = 0; ma.pimg = qv; ma.ord = ident + S + C;
+      ma.run_start = fin + 2; ma.kq = fin + 5; ma.kmax = fin + 5;
+      ma.src_in = s2[bs]; ma.u_in = key[bs]; ma.src_out = s2[bs ^ 1]; ma.u_out = key[bs ^ 1];
+      k_rg_merge<<<grid256(e, N + P, 32), 256, 0, e->stream>>>(ma);
+      k_rc_number<<<grid256(e, N + P, 32), 256, 0, e->stream>>>(fin + 1, s2[bs ^ 1], pos, out.seq);
+    }
+  }
+  if (parties && !many && P) {  // one image: the kept parties keep their order and numbers
+    k_scan_small<<<1, 1024, 0, e->stream>>>((uint32_t)P, pflag, rsz + P);
+    k_rp_rows1<<<(uint32_t)((P + 255) / 256), 256, 0, e->stream>>>((uint32_t)P, ppart, C, pflag, psz, pc[0].seq, rsrc,
+                                                                   rsz, out.seq + N);
   }
   CK(cudaGetLastError());
   // 4. one read decides every refusal
-  std::vector<uint32_t> h_off(R1 * K), h_skip(K);
+  std::vector<uint32_t> h_off(R1 * K), h_skip(K), h_poff(parties ? R2 * K : 0), h_pctr(parties ? kRpWords + 3 * K : 0);
   CK(cudaMemcpyAsync(h_off.data(), rq_off, h_off.size() * 4, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaMemcpyAsync(h_skip.data(), skip, 4 * (size_t)K, cudaMemcpyDeviceToHost, e->stream));
+  if (parties) {
+    CK(cudaMemcpyAsync(h_poff.data(), rqp, h_poff.size() * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(h_pctr.data(), pctr, h_pctr.size() * 4, cudaMemcpyDeviceToHost, e->stream));
+  }
   if ((rc = read_counters(e))) return rc;
   if (const uint32_t err = e->h_cnt->img_err) return img_err(e, "image rejected", err);
+  uint32_t p_kept = 0, p_rej = 0, p_skip = 0, p_mem = 0;
+  if (parties) {
+    const uint32_t err = h_pctr[kRpErrBits];
+    for (uint32_t k = 0; k < K; ++k)
+      if (h_pctr[kRpWords + 2 * K + k] != mcount[k]) return set_err(e, MM_E_ARG, "party image %u rejected: party sizes do not add up to the member count", k);
+    if (err)
+      return set_err(e, MM_E_ARG, "party image rejected:%s%s%s", err & kRpBadSize ? " a party of fewer than 2 members" : "",
+                     err & kRpBadSeq ? " sequence numbers out of order" : "", err & kRpBadId ? " id out of range" : "");
+    if (h_pctr[kRpSeqDup]) return set_err(e, MM_E_ARG, "party image rejected: a party's sequence number is a solo's");
+  }
   if (e->h_cnt->mrg_dups) return img_err(e, "image rejected", kImgDup);
+  if (parties)
+    for (uint32_t k = 0; k < K; ++k) {
+      const uint32_t* r = h_poff.data() + R2 * k;
+      const uint32_t np = pbase[k + 1] - pbase[k];
+      if (r[C + 1] + h_pctr[kRpWords + k] != np)
+        return set_err(e, MM_E_STATE, "regroup: %u parties kept or rejected and %u skipped of %u", r[C + 1],
+                       h_pctr[kRpWords + k], np);
+      p_kept += r[C]; p_rej += r[C + 1] - r[C]; p_skip += h_pctr[kRpWords + k]; p_mem += h_pctr[kRpWords + K + k];
+    }
   uint32_t kept = 0, n_rej = 0, n_skip = 0;
   for (uint32_t k = 0; k < K; ++k) {
     const uint32_t* r = h_off.data() + R1 * k;
@@ -2051,7 +2288,13 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
     *n_rejected = n_rej;
     return set_err(e, MM_E_CAP, "%u rejected players, cap %u", n_rej, cap);
   }
-  if ((rc = load_fits(e, kept, m))) return rc;
+  if (parties && p_rej > pp->cap) {
+    pp->n_rejected = p_rej;
+    return set_err(e, MM_E_CAP, "%u rejected parties, cap %u", p_rej, pp->cap);
+  }
+  if (p_mem > e->pt.cap)
+    return set_err(e, MM_E_CAP, "%u party members to load, party_capacity %u", p_mem, e->pt.cap);
+  if ((rc = load_fits(e, kept, (uint64_t)m + p_mem))) return rc;
   if (n_rej) {
     if (!many) {
       CK(cudaMemcpyAsync(rej_index, at(o_rej), (size_t)n_rej * 4, cudaMemcpyDeviceToHost, e->stream));
@@ -2069,12 +2312,42 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
       for (uint32_t k = 0, w = 0; k < K; ++k)
         for (uint32_t j = h_off[R1 * k + S]; j < h_off[R1 * k + S + 1]; ++j) rej_image[w++] = k;
   }
+  if (p_rej) {  // each party image's reject bucket, in image order: (image, index) ascending
+    for (uint32_t k = 0, w = 0; k < K; ++k) {
+      const uint32_t* r = h_poff.data() + R2 * k;
+      if (r[C + 1] > r[C])
+        CK(cudaMemcpyAsync(pp->rej_index + w, psrc + pbase[k] + r[C], (size_t)(r[C + 1] - r[C]) * 4,
+                           cudaMemcpyDeviceToHost, e->stream));
+      w += r[C + 1] - r[C];
+    }
+    CK(cudaStreamSynchronize(e->stream));
+    if (pp->rej_image)
+      for (uint32_t k = 0, w = 0; k < K; ++k)
+        for (uint32_t j = h_poff[R2 * k + C]; j < h_poff[R2 * k + C + 1]; ++j) pp->rej_image[w++] = k;
+  }
   std::vector<uint32_t> per(S, 0);
   for (uint32_t k = 0; k < K; ++k)
     for (uint32_t s = 0; s < S; ++s) per[s] += h_off[R1 * k + s + 1] - h_off[R1 * k + s];
-  if ((rc = load_columns(e, per, out, kept, act, m, many ? kept : seq_next, "image rejected"))) return rc;
+  if ((rc = load_columns(e, per, out, kept, act, m, many ? kept + p_kept : seq_next, "image rejected"))) return rc;
   *n_rejected = n_rej;
   if (n_elsewhere) *n_elsewhere = n_skip;
+  if (!parties) return MM_OK;
+  pp->n_rejected = p_rej;
+  pp->n_elsewhere = p_skip;
+  if (p_kept) {  // the table rows in the new age order, members and active-set values
+    auto& t = e->pt;
+    k_scan_small<<<1, 1024, 0, e->stream>>>(p_kept, rsz, rsz + P + 1);
+    RpWriteArgs wa{};
+    wa.imgs = reinterpret_cast<const PtImgCols*>(at(o_pcols)); wa.pbase = reinterpret_cast<const uint32_t*>(at(o_pbase));
+    wa.pk = ppk; wa.moff = pmoff; wa.R = pR; wa.rsrc = rsrc; wa.rseq = out.seq + N; wa.roff = rsz; wa.rows = p_kept;
+    wa.bm = bin_map(e); wa.grp_lut = e->d_grp_lut; wa.pt = pt_view(e, t.cur); wa.act = act_view(e);
+    k_rp_write<<<(p_kept + 255) / 256, 256, 0, e->stream>>>(wa);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(e->stream));
+    t.n_rows = p_kept; t.n_mem = p_mem; t.live = p_mem;
+    e->n_active += p_mem;
+  }
+  pp->n_loaded = p_kept;
   return MM_OK;
 }
 
@@ -2735,18 +3008,6 @@ int enqueue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t*
   int rc = pt_check(e);
   if (rc || n == 0) return rc;
   return pt_enqueue(e, n, size, ids, rating, mode, enq_ts, nullptr, false, accepted);
-}
-
-// Section offsets of a party image (include/mm_engine.h): [0] size, [1] seq, [2] enq_ts, [3] mode, [4] id, [5] rating,
-// [6] total bytes.
-struct PtImgLayout { uint64_t off[7]; };
-PtImgLayout pt_img_layout(uint32_t P, uint32_t M, uint32_t W) {
-  auto a8 = [](uint64_t x) { return (x + 7) & ~7ull; };
-  const uint64_t bytes[6] = {(uint64_t)P, 4ull * P, 4ull * P, (uint64_t)P, (uint64_t)W * M, 4ull * M};
-  PtImgLayout l{};
-  l.off[0] = sizeof(mm_image_header);
-  for (int k = 0; k < 6; ++k) l.off[k + 1] = a8(l.off[k] + bytes[k]);
-  return l;
 }
 
 // mm_export_parties: select and count (k_pt_sel, the scans, one counter read), then the columns gathered in age order
@@ -3908,7 +4169,7 @@ int mm_import_regroup(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t 
   CK(cudaSetDevice(e->device));
   const uint8_t* b = static_cast<const uint8_t*>(buf);
   const int rc = regroup_many(e, "mm_import_regroup", 1, &b, &n_bytes, nullptr, 0, cap, nullptr, rejected, n_rejected,
-                              nullptr);
+                              nullptr, nullptr);
   free_img_scratch(e);
   return rc;
 }
@@ -3916,18 +4177,30 @@ int mm_import_regroup(mm_engine* e, const void* buf, uint64_t n_bytes, uint32_t 
 int mm_import_regroup_many(mm_engine* e, uint32_t n_images, const void* const* bufs, const uint64_t* n_bytes,
                            const uint8_t* keep, uint32_t active_image, uint32_t cap, uint32_t* rej_image,
                            uint32_t* rej_index, uint32_t* n_rejected, uint32_t* n_elsewhere) {
+  return mm_import_regroup_many_parties(e, n_images, bufs, n_bytes, keep, active_image, cap, rej_image, rej_index,
+                                        n_rejected, n_elsewhere, nullptr);
+}
+
+int mm_import_regroup_many_parties(mm_engine* e, uint32_t n_images, const void* const* bufs, const uint64_t* n_bytes,
+                                   const uint8_t* keep, uint32_t active_image, uint32_t cap, uint32_t* rej_image,
+                                   uint32_t* rej_index, uint32_t* n_rejected, uint32_t* n_elsewhere,
+                                   mm_recut_parties* parties) {
   if (!e || !n_rejected || !n_elsewhere || (n_images && (!bufs || !n_bytes)) || (cap && (!rej_image || !rej_index)))
     return MM_E_ARG;
+  if (parties && (parties->reserved || (parties->cap && (!parties->rej_image || !parties->rej_index)))) return MM_E_ARG;
   *n_rejected = 0;
   *n_elsewhere = 0;
   for (uint32_t k = 0; k < n_images && k < kRcMaxImages; ++k)
     if (n_bytes[k] && !bufs[k]) return MM_E_ARG;
+  if (parties && n_images && parties->n_bytes && !parties->bufs) return MM_E_ARG;
+  for (uint32_t k = 0; parties && parties->n_bytes && k < n_images && k < kRcMaxImages; ++k)
+    if (parties->n_bytes[k] && !parties->bufs[k]) return MM_E_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
   CK(cudaSetDevice(e->device));
   std::vector<const uint8_t*> b(n_images <= kRcMaxImages ? n_images : 0);
   for (size_t k = 0; k < b.size(); ++k) b[k] = static_cast<const uint8_t*>(bufs[k]);
   const int rc = regroup_many(e, "mm_import_regroup_many", n_images, b.data(), n_bytes, keep, active_image, cap,
-                              rej_image, rej_index, n_rejected, n_elsewhere);
+                              rej_image, rej_index, n_rejected, n_elsewhere, parties);
   free_img_scratch(e);
   return rc;
 }

@@ -815,6 +815,52 @@ class Engine:
                     "mm_import_regroup_many")
         return np.stack([rimg[:k.value], ridx[:k.value]], 1).astype(np.int64), int(e.value)
 
+    def import_regroup_many_parties(self, images, party_images, keep=None, active_image=None):
+        """import_regroup_many() with the queued parties: party_images[k] is what export_parties() gave on the rank
+        that wrote images[k], taken just before it (None or empty = no parties).  Parties are classified under this
+        config as solos are, and numbered with the solos in one order (mm_import_regroup_many_parties).  -> (rejected,
+        n_elsewhere, party_rejected, party_elsewhere): party_rejected = int64 [n, 2] (image, party index) pairs,
+        ascending, of the parties this config has no queue for; party_elsewhere = parties skipped."""
+        def arr(b):
+            return np.ascontiguousarray(np.frombuffer(b, np.uint8) if isinstance(b, (bytes, bytearray, memoryview))
+                                        else b, np.uint8)
+        bufs = [arr(b) for b in images]
+        pbufs = [None if b is None else arr(b) for b in party_images]
+        K = len(bufs)
+        if len(pbufs) != K:
+            raise ValueError("one party image (or None) per image")
+        ptrs = (C.c_void_p * max(K, 1))(*[b.ctypes.data for b in bufs])
+        lens = (C.c_uint64 * max(K, 1))(*[len(b) for b in bufs])
+        pptrs = (C.c_void_p * max(K, 1))(*[b.ctypes.data if b is not None and len(b) else None for b in pbufs])
+        plens = (C.c_uint64 * max(K, 1))(*[len(b) if b is not None else 0 for b in pbufs])
+        hs = C.sizeof(abi.ImageHeader)
+        n = sum(min(abi.ImageHeader.from_buffer_copy(b[:hs].tobytes()).n_players, len(b)) if len(b) >= hs else 0
+                for b in bufs)  # a player takes more than a byte: a corrupt count must not size the reject list
+        n = min(n, 0xFFFFFFFF)
+        np_ = sum(min(abi.ImageHeader.from_buffer_copy(b[:hs].tobytes()).n_parts, len(b))
+                  for b in pbufs if b is not None and len(b) >= hs)
+        np_ = min(np_, 0xFFFFFFFF)
+        sel = None
+        if keep is not None:
+            sel = np.ascontiguousarray(np.asarray(keep, bool).reshape(-1), np.uint8)
+            if len(sel) != self.cfg.n_modes * self.cfg.n_groups:
+                raise ValueError("keep needs n_modes * n_groups entries")
+        rimg, ridx = np.empty(max(n, 1), np.uint32), np.empty(max(n, 1), np.uint32)
+        pimg, pidx = np.empty(max(np_, 1), np.uint32), np.empty(max(np_, 1), np.uint32)
+        rp = abi.RecutParties()
+        rp.bufs = C.cast(pptrs, C.c_void_p)
+        rp.n_bytes = C.cast(plens, C.c_void_p)
+        rp.cap = np_
+        rp.rej_image, rp.rej_index = pimg.ctypes.data, pidx.ctypes.data
+        k, e = C.c_uint32(0), C.c_uint32(0)
+        self._check(self.lib.mm_import_regroup_many_parties(self.h, K, ptrs, lens, _p(sel),
+                                                            0xFFFFFFFF if active_image is None else int(active_image),
+                                                            n, _p(rimg), _p(ridx), C.byref(k), C.byref(e),
+                                                            C.byref(rp)),
+                    "mm_import_regroup_many_parties")
+        return (np.stack([rimg[:k.value], ridx[:k.value]], 1).astype(np.int64), int(e.value),
+                np.stack([pimg[:rp.n_rejected], pidx[:rp.n_rejected]], 1).astype(np.int64), int(rp.n_elsewhere))
+
     def export_queues(self, mask):
         """Release whole (mode, group) queues into a queue image (mm_export_queues) -> uint8 array.  mask: bool per
         queue in queue_stats() record order (mode * n_groups + group), or [n_modes][n_groups].  The exported players

@@ -516,7 +516,7 @@ def _exchange(rank, world, comm, out, want):
     return got
 
 
-def recut(pkg, old_cfg, new_cfg, old_owners, new_owners, rank, engine, comm, make_engine=None):
+def recut(pkg, old_cfg, new_cfg, old_owners, new_owners, rank, engine, comm, make_engine=None, party_capacity=None):
     """Re-cut a deployment sharded by rating group to a new group table and owner array; every rank of the job calls
     this with the same arguments.  world = 1 + the largest rank in either owner array, and every rank below it calls.
       1. every rank exports its engine (export_state: the old engine is never changed);
@@ -528,45 +528,85 @@ def recut(pkg, old_cfg, new_cfg, old_owners, new_owners, rank, engine, comm, mak
       4. every rank sends its status ([0] ok, [1] failed) to every other rank.  Only if all succeeded does each rank
          keep its new engine and close the old one; otherwise every rank closes its new engine and keeps the old one,
          untouched: a failure anywhere loses no player.
+    Parties (an engine with party_capacity): mm_export refuses while a party is queued, so in step 1 the rank first
+    releases its parties (export_parties) and then exports its engine: both images come from the same stop.  The party
+    image follows the engine image in the array of step 2 (the send matrix is unchanged: a party's R is a rating of the
+    clamped domain), the new engine gets party_capacity (default: the old engine's) and loads both kinds with
+    import_regroup_many_parties.  On failure anywhere every rank merges its own party image back into its old engine
+    with keep_seq (valid right after the release: nothing else is queued as a party and seq_next has not moved), which
+    leaves it as it was; a party image that cannot go back is returned as `stranded` (merge it with
+    Engine.merge_parties).  Engines without party capacity take the path above unchanged.
     Preconditions: no ingest or tick on any rank during the call, and routing switches to route(new_cfg, ...,
     owners=new_owners) after it.  While it runs, each rank holds its old engine, its new one and the images it loads.
-    With more than one old image a rank's players are renumbered (include/mm_engine.h): requeue records of players
-    matched before the re-cut do not carry over.
+    With more than one old image a rank's players and parties are renumbered (include/mm_engine.h): requeue records
+    of players and parties matched before the re-cut do not carry over.
     -> dict(ok, engine: the engine this rank uses from now on, dropped: ids of this rank's own players that have no
     queue under new_cfg (they left: answer them), elsewhere: players skipped here because another rank owns them,
-    bytes_sent: bytes this rank sent)."""
+    bytes_sent: bytes this rank sent; with parties also dropped_parties: the member ids of this rank's own parties that
+    have no queue under new_cfg, parties_elsewhere, stranded: this rank's party image if it could not go back, else
+    None)."""
     make_engine = make_engine or pkg.Engine
     old_owners, new_owners = np.asarray(old_owners, np.int64), np.asarray(new_owners, np.int64)
     world = int(max(old_owners.max(initial=0), new_owners.max(initial=0))) + 1
     send = recut_sends(old_cfg, new_cfg, old_owners, new_owners, world)
     sent = [0]
+    parties = bool(getattr(engine, "party_capacity", 0))
+    if party_capacity is None:
+        party_capacity = getattr(engine, "party_capacity", 0)
 
     def counted(arrays):
         sent[0] += sum(np.asarray(a).nbytes for a in arrays)
         return arrays
 
+    pimg = img = None
     try:
+        if parties:
+            pimg = np.ascontiguousarray(engine.export_parties(), np.uint8)
         img = np.ascontiguousarray(engine.export_state(), np.uint8)
     except Exception:
         img = None
-    mine = img.view(np.int64) if img is not None else np.array([-1], np.int64)
+    if img is None:
+        mine = np.array([-1], np.int64)
+    else:
+        mine = img.view(np.int64) if not parties else np.concatenate([img, pimg]).view(np.int64)
     got = _exchange(rank, world, comm, lambda d: counted((mine,)) if send[rank, d] else None,
                     lambda s: bool(send[s, rank]))
-    images, own = [], None
+    images, pimages, own = [], [], None
     for s in range(world):
         if s == rank:
             own = len(images)
             images.append(img)
+            pimages.append(pimg)
         elif send[s, rank]:
-            arr = np.ascontiguousarray(got[s][0])
-            images.append(arr.view(np.uint8) if len(arr) > 1 else None)
+            arr = np.ascontiguousarray(got[s][0]).view(np.uint8)
+            if len(arr) <= 8:
+                images.append(None)
+                pimages.append(None)
+                continue
+            q = int(arr[16:24].view(np.uint64)[0])  # the engine image's total_bytes; its party image follows
+            images.append(arr[:q])
+            pimages.append(arr[q:] if len(arr) > q else None)
     new, dropped, elsewhere = None, np.zeros(0, np.uint64), 0
+    dropped_parties, p_else = np.zeros(0, np.uint64), 0
     ok = all(x is not None for x in images)
+    use_parties = parties or any(p is not None for p in pimages)
     if ok:
         try:
             new = make_engine(new_cfg)
             keep = np.broadcast_to(new_owners == rank, (new_cfg.n_modes, new_cfg.n_groups))
-            rejected, elsewhere = new.import_regroup_many(images, keep=keep, active_image=own)
+            if use_parties:
+                if party_capacity:
+                    new.set_option("party_capacity", party_capacity)
+                rejected, elsewhere, prej, p_else = new.import_regroup_many_parties(images, pimages, keep=keep,
+                                                                                    active_image=own)
+                if pimg is not None and len(prej):
+                    _h, c = pkg.engine.read_party_image(pimg.tobytes())
+                    off = np.concatenate([[0], np.cumsum(c["size"].astype(np.int64))])
+                    mine_rej = prej[prej[:, 0] == own, 1]
+                    dropped_parties = np.concatenate(
+                        [np.zeros(0, np.uint64)] + [np.asarray(c["id"][off[j]:off[j + 1]], np.uint64) for j in mine_rej])
+            else:
+                rejected, elsewhere = new.import_regroup_many(images, keep=keep, active_image=own)
             ids = pkg.engine.read_image(images[own])[1]["id"]
             dropped = np.asarray(ids[rejected[rejected[:, 0] == own, 1]], np.uint64)
         except Exception:
@@ -576,10 +616,22 @@ def recut(pkg, old_cfg, new_cfg, old_owners, new_owners, rank, engine, comm, mak
     ok = ok and all(_status(got[s][0]) == 0 for s in got)
     if ok:
         engine.close()
-        return dict(ok=True, engine=new, dropped=dropped, elsewhere=int(elsewhere), bytes_sent=sent[0])
+        out = dict(ok=True, engine=new, dropped=dropped, elsewhere=int(elsewhere), bytes_sent=sent[0])
+        if parties:
+            out.update(dropped_parties=dropped_parties, parties_elsewhere=int(p_else), stranded=None)
+        return out
     if new is not None:
         new.close()
-    return dict(ok=False, engine=engine, dropped=np.zeros(0, np.uint64), elsewhere=0, bytes_sent=sent[0])
+    out = dict(ok=False, engine=engine, dropped=np.zeros(0, np.uint64), elsewhere=0, bytes_sent=sent[0])
+    if parties:
+        stranded = None
+        if pimg is not None:
+            try:
+                engine.merge_parties(pimg, keep_seq=True)
+            except Exception:
+                stranded = pimg
+        out.update(dropped_parties=np.zeros(0, np.uint64), parties_elsewhere=0, stranded=stranded)
+    return out
 
 
 # ======================================================================================================================
