@@ -731,6 +731,54 @@ typedef struct mm_queue_quality {
 int mm_match_quality(mm_engine* e, mm_queue_quality* per_queue, uint32_t cap, uint32_t* n_out,
                      mm_lobby_quality* per_lobby, uint32_t lobby_cap, uint32_t* n_lobbies);
 
+/* ---- off-tick match report -------------------------------------------------------
+ * EXTENSION (measurement): the match section of mm_queue_stats and the mm_match_quality report for the lobbies formed
+ * OUTSIDE the tick, by mm_party_match and mm_widen.  Widening matches exactly the players who waited longest, so the
+ * tail of the queue -> match wait and the spread that widening trades for it show here and not in the tick's reports.
+ *
+ * WHICH CALL: the last call of `source` on this engine (MM_OFFTICK_PARTY_MATCH: mm_party_match, MM_OFFTICK_WIDEN:
+ * mm_widen).  VOID before the first such call and after one that returned anything but MM_OK (a refusal, an MM_E_CAP
+ * dry run): *n_out = 0 and *n_lobbies = 0, nothing is written.  A call that returned MM_OK without lobbies (no queue
+ * served, no live party, no anchor filled a lobby) gives a valid, empty report: n_modes * n_groups zero records.
+ * Nothing else changes a source's report: not ticks of any form, the other source, enqueue, remove, expire, requeue
+ * (solo and party), backfill, the band pass, options, the lobby budget, snapshot / restore or export / merge.  Engines
+ * loaded by mm_import* are fresh, so their reports start void.  MM_ORDER_ARRIVAL and MM_F_NO_DEDUPE engines refuse
+ * both calls, so their reports are always void.
+ * PER LOBBY: per_lobby[h] describes lobbies[h] of that call, in its header order, by the DEFINITION of
+ * mm_match_quality: c(r) clamped to [rmin - 1, rmax + 1], min_rating, max_rating, rating_sum and the team imbalance.  A
+ * solo's rating is its pool rating; a party member's is its own rating as enqueued (not the party's R).  Members are
+ * taken in the order the call returned them, so with "team_balance" (mm_widen lobbies of masked modes) or
+ * "party_balance" (mm_party_match lobbies of masked modes) the imbalance is that of the emitted teams.
+ * WAIT of a member: the WAIT of mm_queue_stats at the call's `now`, from a solo's own enq_ts and from a party member's
+ * party's enq_ts.
+ * PER QUEUE, one record per (mode, group) queue, empty ones included, in mm_queue_stats order: waits[q] holds
+ * n_lobbies, n_matched (members), max_match_wait and match_wait_hist over every member of the queue's lobbies of that
+ * call, in the BUCKETS of mm_queue_stats; quality[q] every mm_queue_quality field as mm_match_quality defines it, over
+ * those lobbies.  waits, quality and per_lobby may each be NULL, which skips that output.
+ * READ-ONLY: the call changes nothing — not the pool, the party table, the active set, the results of any call, the
+ * snapshot, the reject list or pending async_results copies.
+ * REFUSALS, decided before anything is written: MM_E_ARG a null e, n_out or n_lobbies, or an unknown source; MM_E_CAP
+ * cap < n_modes * n_groups while waits or quality is not NULL (*n_out = the records needed), or per_lobby not NULL
+ * with lobby_cap below the call's lobby count (*n_lobbies = the count needed).
+ * COST AND MEMORY: the capture runs inside mm_party_match / mm_widen, after the balance pass, and its device time is
+ * part of their device_us: the enqueue stamp of every taken solo is written beside its id by the take, then one warp
+ * per lobby over its member slots, one pass over the members for the waits and the per-queue quality records.  Kept
+ * per source, allocated by the first call and grown to the largest call: 24 bytes per lobby and 1488 bytes per queue;
+ * shared by the two calls: 8 bytes per member and 4 bytes per lobby of the largest call, 8 bytes per queue, and the c
+ * column "team_balance" also uses (4 bytes per player of capacity).  mm_offtick_report itself is device-to-host copies of those records only.                                          */
+#define MM_OFFTICK_PARTY_MATCH 0u
+#define MM_OFFTICK_WIDEN 1u
+
+typedef struct mm_match_waits {    /* the match section of mm_queue_stat, for one off-tick call */
+  uint8_t mode, group;
+  uint16_t reserved;               /* 0 */
+  uint32_t n_lobbies, n_matched, max_match_wait;
+  uint32_t match_wait_hist[MM_WAIT_BUCKETS];
+} mm_match_waits;                  /* 496 bytes */
+
+int mm_offtick_report(mm_engine* e, uint32_t source, mm_match_waits* waits, mm_queue_quality* quality, uint32_t cap,
+                      uint32_t* n_out, mm_lobby_quality* per_lobby, uint32_t lobby_cap, uint32_t* n_lobbies);
+
 /* ---- lobby budget: how many lobbies a tick may emit ------------------------------
  * EXTENSION (flow control).  The reference emits one lobby at a time behind prefetch_count: 10 (search/worker.ex:29),
  * and its lobby stage answers the players of a lobby it finds no game server for with an error

@@ -203,6 +203,26 @@ static ERL_NIF_TERM nif_match_quality(ErlNifEnv* env, int argc, const ERL_NIF_TE
   return enif_make_tuple2(env, atom(env, "ok"), out);
 }
 
+/* offtick_report(ref, source) -> {:ok, waits :: binary(mm_match_waits[]), quality :: binary(mm_queue_quality[])}:
+ * one record of each per (mode, group) queue, mode * n_groups + group order — the waits and the rating quality of the
+ * lobbies the last mm_party_match (source 0) or mm_widen (source 1) formed (extension); empty binaries while the report
+ * is void (no such call yet, or its last one failed) */
+static ERL_NIF_TERM nif_offtick_report(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; unsigned int source; uint32_t n = 0, n_lob = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_uint(env, argv[1], &source))
+    return enif_make_badarg(env);
+  int rc = mm_offtick_report(r->e, source, NULL, NULL, 0, &n, NULL, 0, &n_lob);  /* n = records, 0 when void */
+  if (rc) return err(env, rc);
+  ERL_NIF_TERM wout, qout;
+  unsigned char* wb = enif_make_new_binary(env, (size_t)n * sizeof(mm_match_waits), &wout);
+  unsigned char* qb = enif_make_new_binary(env, (size_t)n * sizeof(mm_queue_quality), &qout);
+  /* nothing runs between the two calls: the engine's lock is taken per call, and only this engine's own calls change
+     the report, which this process serialises */
+  if (n) rc = mm_offtick_report(r->e, source, (mm_match_waits*)wb, (mm_queue_quality*)qb, n, &n, NULL, 0, &n_lob);
+  return rc ? err(env, rc) : enif_make_tuple3(env, atom(env, "ok"), wout, qout);
+}
+
 /* expire_packed(ref, now_ms, max_wait_ms) -> {:ok, handles :: binary(u32[])}: search timeout (extension) — the
  * queued players who have waited >= max_wait_ms leave the pool and the active set; the caller answers each one */
 static ERL_NIF_TERM nif_expire_packed(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
@@ -856,6 +876,7 @@ static ErlNifFunc funcs[] = {
   {"status", 1, nif_status, 0},
   {"queue_stats", 2, nif_queue_stats, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"match_quality", 1, nif_match_quality, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"offtick_report", 2, nif_offtick_report, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"expire_packed", 3, nif_expire_packed, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"export_image", 1, nif_export_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"import_image", 2, nif_import_image, ERL_NIF_DIRTY_JOB_CPU_BOUND},

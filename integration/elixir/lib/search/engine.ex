@@ -72,6 +72,13 @@ defmodule Matchmaking.Search.Engine do
   """
   def match_quality(_ref), do: :erlang.nif_error(:nif_not_loaded)
   @doc """
+  Extension (off-tick report): the waits and the rating quality of the lobbies the last party_match (source 0) or
+  widen (source 1) formed, per (mode, group) queue (mm_offtick_report) -> {:ok, binary(mm_match_waits[]),
+  binary(mm_queue_quality[])}, in queue_stats/2 record order; empty binaries while the report is void (no such call
+  yet, or its last one failed).
+  """
+  def offtick_report(_ref, _source), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
   Extension (search timeout): the queued players who have waited >= max_wait_ms at now_ms leave the pool and the
   active set, as if removed -> {:ok, handles :: binary(u32[])}; the caller answers each one.
   """

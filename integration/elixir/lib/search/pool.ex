@@ -14,6 +14,9 @@ defmodule Matchmaking.Search.Pool do
                      last tick's matched players and p99 wait at match, in ms — Search.Worker.status/0's queue depth;
                      with Engine.match_quality also the last tick's lobbies, mean / p50 / p99 / max rating spread and
                      mean / p99 / max team imbalance, in rating points (zero lobbies while the report is void)
+                     and, with the parties / widen options, Engine.offtick_report's party_match / widen maps: the
+                     last step's party or widened lobbies, matched players, p50 / p99 / max wait at match in ms and
+                     mean / p99 / max rating spread and team imbalance (absent while that report is void)
       search_timeout_ms   option (extension, default nil = off): after each tick's lobbies are published, the players
                      still queued who have waited at least this long leave the pool (Engine.expire_packed) and get the
                      error response of game-lobby/worker.ex:63-71,105-116 on their "response-queue"
@@ -308,10 +311,34 @@ defmodule Matchmaking.Search.Pool do
          Map.merge(%{waiting: waiting, oldest_wait_ms: oldest, p50_wait_ms: quantile(hist, 0.5),
                      p99_wait_ms: quantile(hist, 0.99), last_tick_matched: matched,
                      last_tick_p99_match_wait_ms: quantile(mhist, 0.99)},
-                   Map.get(quality, mode, %{last_tick_lobbies: 0}))}
+                   Map.get(quality, mode, %{last_tick_lobbies: 0}))
+         |> Map.merge(Map.get(offtick_of(st, group), mode, %{}))}
       end
     end
     {:reply, reply, st}
+  end
+
+  # the party_match (source 0) and widen (source 1) reports of one group -> %{mode => %{party_match: .., widen: ..}},
+  # for the sources the pool runs; a void report adds nothing
+  defp offtick_of(st, group) do
+    for {key, src, on} <- [{:party_match, 0, st.parties}, {:widen, 1, st.widen}], on != nil,
+        {:ok, wrecs, qrecs} <- [Engine.offtick_report(st.ref, src)],
+        {mode, fields} <- offtick_fields(wrecs, qrecs, group),
+        reduce: %{} do
+      acc -> Map.update(acc, mode, %{key => fields}, &Map.put(&1, key, fields))
+    end
+  end
+
+  defp offtick_fields(wrecs, qrecs, group) do
+    quality = quality_of(qrecs, group)
+    for <<mode, g, _::16, lobbies::little-32, matched::little-32, max_wait::little-32, whist::binary-size(480) <- wrecs>>,
+        g == group do
+      q = Map.fetch!(quality, mode)
+      {mode, %{lobbies: lobbies, matched: matched, p50_match_wait_ms: quantile(whist, 0.5),
+               p99_match_wait_ms: quantile(whist, 0.99), max_match_wait_ms: max_wait, mean_spread: q.mean_spread,
+               p99_spread: q.p99_spread, max_spread: q.max_spread, mean_imbalance: q.mean_imbalance,
+               p99_imbalance: q.p99_imbalance, max_imbalance: q.max_imbalance}}
+    end
   end
 
   # mm_queue_quality records of one group -> %{mode => quality fields}; quantiles are bucket upper bounds as for waits

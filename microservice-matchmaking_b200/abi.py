@@ -209,6 +209,23 @@ class QueueQuality(C.Structure):
     ]
 
 
+MM_OFFTICK_PARTY_MATCH = 0  # mm_offtick_report sources
+MM_OFFTICK_WIDEN = 1
+
+
+class MatchWaits(C.Structure):
+    """mm_match_waits: the match section of mm_queue_stat for one off-tick call's lobbies of a queue (496 bytes)."""
+    _fields_ = [
+        ("mode", C.c_uint8),
+        ("group", C.c_uint8),
+        ("reserved", C.c_uint16),
+        ("n_lobbies", C.c_uint32),
+        ("n_matched", C.c_uint32),
+        ("max_match_wait", C.c_uint32),
+        ("match_wait_hist", C.c_uint32 * MM_WAIT_BUCKETS),
+    ]
+
+
 MM_IMAGE_MAGIC = 0x474D494D
 MM_QUEUE_IMAGE_MAGIC = 0x5155514D  # mm_export_queues: same header and sections, no active section
 MM_IMAGE_VERSION = 1
@@ -312,6 +329,8 @@ PROTOTYPES = {
     "mm_pool_read": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _P(C.c_uint32)]),
     "mm_queue_stats": (C.c_int, [_vp, C.c_uint64, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_match_quality": (C.c_int, [_vp, _vp, C.c_uint32, _P(C.c_uint32), _vp, C.c_uint32, _P(C.c_uint32)]),
+    "mm_offtick_report": (C.c_int, [_vp, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32), _vp, C.c_uint32,
+                                    _P(C.c_uint32)]),
     "mm_set_lobby_budget": (C.c_int, [_vp, _vp, _vp]),
     "mm_lobby_budget_report": (C.c_int, [_vp, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_lobby_candidates": (C.c_int, [_vp, _vp, C.c_uint32, _P(C.c_uint32)]),

@@ -173,15 +173,16 @@ struct BfKeyBins {
 };
 
 // Pieces to request order: piece p's cnt players sit in staging at kbase[key of its bin] + roff; they go to the request's
-// output at req_base[req] + poff.  One warp per piece.
+// output at req_base[req] + poff.  One warp per piece.  T: the ids, or (the off-tick report) the stamps beside them.
+template <class T>
 __global__ void k_bf_out(uint32_t n_pieces, const BfPiece* __restrict__ piece, const uint32_t* __restrict__ map,
                          const uint32_t* __restrict__ kbase, const uint32_t* __restrict__ req_base,
-                         const uint64_t* __restrict__ staging, uint64_t* __restrict__ members) {
+                         const T* __restrict__ staging, T* __restrict__ members) {
   const uint32_t lane = threadIdx.x & 31, p = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (p >= n_pieces) return;
   const BfPiece c = piece[p];
-  const uint64_t* src = staging + kbase[map[c.bin]] + c.roff;
-  uint64_t* dst = members + req_base[c.req] + c.poff;
+  const T* src = staging + kbase[map[c.bin]] + c.roff;
+  T* dst = members + req_base[c.req] + c.poff;
   for (uint32_t i = lane; i < c.cnt; i += 32) dst[i] = src[i];
 }
 

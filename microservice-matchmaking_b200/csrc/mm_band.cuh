@@ -285,12 +285,14 @@ __global__ void __launch_bounds__(kBandWalkBlock) k_band_bases(const BandArgs a,
 // step a warp lists its band players in order in shared memory, then ranks them 32 at a time: peers of one key by
 // __match_any_sync, the key's running rank in M (the tile's exclusive prefix after k_band_scan; only this warp touches
 // the tile's entries).  A player whose rank is below klim[q] goes to kbase[q] + rank: its id, rating and mode to the
-// candidate columns, or its id to the members, and then it is taken (take = 1).
+// candidate columns, or its id to the members, and then it is taken (take = 1); its enqueue stamp beside the id when ts
+// is not null (mm_widen / mm_party_match: the off-tick report, mm_offtick.cuh).
 struct BandOut {
   uint64_t* id;
   int32_t* rating;  // candidates only
   uint8_t* mode;    // candidates only
   uint32_t take;
+  uint32_t* ts = nullptr;
 };
 template <int BLOCK>
 __global__ void __launch_bounds__(BLOCK) k_band_place(const BandArgs a, const BandOut out) {
@@ -339,6 +341,7 @@ __global__ void __launch_bounds__(BLOCK) k_band_place(const BandArgs a, const Ba
             const uint32_t at = a.kbase[qq] + rank;
             out.id[at] = a.pool.id[slot];
             if (out.rating) { out.rating[at] = a.pool.rating[slot]; out.mode[at] = a.pool.mode[slot]; }
+            if (out.ts) out.ts[at] = a.pool.ts[slot];
             if (out.take && pool_take_slot(a.pool, a.meta, slot, a.K, a.bin_seg, a.seg_bin_lo)) ++taken;
           }
         }

@@ -26,6 +26,7 @@
 #include "mm_image.cuh"
 #include "mm_kernels.cuh"
 #include "mm_locate.cuh"
+#include "mm_offtick.cuh"
 #include "mm_party.cuh"
 #include "mm_quality.cuh"
 #include "mm_recut.cuh"
@@ -288,6 +289,7 @@ struct mm_engine {
     DevArray<uint32_t> rem, key_bin, kbase, klim, n_taken, req_base, ctr;
     DevArray<BfPiece> piece;
     DevArray<uint64_t> staging, members;
+    DevArray<uint32_t> staging_ts;  // mm_widen / mm_party_match: the taken solos' stamps beside staging
   } bf;
 
   // mm_widen (mm_widen.cuh): the call's tables and the anchors, grown on demand; the plan's rem, the keys, the pieces,
@@ -326,6 +328,22 @@ struct mm_engine {
     DevArray<uint32_t> cont;  // party_balance: [a party call's lobbies] continuation bits per header position
     DevArray<unsigned long long> sum;  // party_balance: [1] the call's summed imbalance
   } tb;
+
+  // the off-tick report (mm_offtick.cuh): one kept report per source (MM_OFFTICK_PARTY_MATCH, MM_OFFTICK_WIDEN), written
+  // only by that source's calls and read only by mm_offtick_report; the capture scratch is shared by the two calls.
+  // Grown on demand, never shrunk.
+  struct OffTick {
+    DevArray<uint32_t> ts;   // [a call's members] enq_ts per member slot
+    DevArray<uint32_t> imb;  // [a call's lobbies] the balance pass's imbalance per header position
+    DevArray<uint32_t> qb;   // lobby bases [n_cut + 1] | member bases [n_cut + 1]
+    struct Report {
+      bool valid = false;    // the source's last call returned MM_OK
+      uint32_t n_lob = 0;    // its lobbies
+      DevArray<mm_lobby_quality> lob;
+      DevArray<mm_queue_quality> quality;
+      DevArray<mm_match_waits> waits;
+    } rep[2];
+  } ot;
 
   // parties (mm_party.cuh): the table in two buffers (compaction moves it from one to the other), sized by
   // party_capacity; the batch and match scratch grown on demand.  Not part of images or snapshots.
@@ -2530,7 +2548,7 @@ int band_match(mm_engine* e, int32_t W, uint32_t g_first, uint32_t g_last, uint3
 // ---- mm_backfill (mm_backfill.cuh) ---------------------------------------------------------------------------------
 // The prefixes k_bf_keys made keys (counters h) leave the pool: the band gather over the keys' partitions places them
 // into bf.staging at kbase[key] + rank and takes them.  bf.members is sized for them too.
-int bf_take(mm_engine* e, const uint32_t* h) {
+int bf_take(mm_engine* e, const uint32_t* h, bool stamps = false) {
   auto& s = e->bf;
   const uint32_t total = h[kBfPlayers];
   BandArgs a = band_args(e);
@@ -2539,9 +2557,10 @@ int bf_take(mm_engine* e, const uint32_t* h) {
   int rc = band_gather(e, a, h[kBfCols], BfKeyBins{s.key_bin});
   if (rc) return rc;
   CK(s.staging.reserve(total)); CK(s.members.reserve(total));
+  if (stamps) CK(s.staging_ts.reserve(total));
   k_band_limit<<<1, kBandPrepBlock, 0, e->stream>>>(a);
   k_band_place<kBandBlock><<<band_ctas(e, e->pool[e->cur].n), kBandBlock, 0, e->stream>>>(
-      a, BandOut{s.staging, nullptr, nullptr, 1u});
+      a, BandOut{s.staging, nullptr, nullptr, 1u, stamps ? s.staging_ts.p : nullptr});
   CK(cudaGetLastError());
   return MM_OK;
 }
@@ -2614,10 +2633,38 @@ int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_t
   CK(cudaMemcpyAsync(s.req_base, base.data(), (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
   const uint32_t np = h[kBfPieces];
   k_bf_out<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, s.piece, e->band.map, s.kbase,
-                                                                               s.req_base, s.staging, s.members);
+                                                                               s.req_base, s.staging.p, s.members.p);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(member_ids, s.members, (size_t)total * 8, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
+// ---- the off-tick report (mm_offtick.cuh) --------------------------------------------------------------------------
+// Report `src` of a party / widen call with nl > 0 lobbies and nm members, from its headers and bases (w), the member
+// slots' c - key_lo (tb.cval) and stamps (ot.ts), and the imbalances its balance pass (bal_mask) stored in ot.imb.
+int ot_capture(mm_engine* e, uint32_t src, const WdArgs& w, uint32_t nl, uint32_t nm, uint32_t bal_mask) {
+  auto& o = e->ot;
+  auto& r = o.rep[src];
+  const uint32_t nc = e->n_cut;
+  CK(r.lob.reserve(nl)); CK(r.quality.reserve(nc)); CK(r.waits.reserve(nc)); CK(o.qb.reserve(2 * ((size_t)nc + 1)));
+  CK(cudaMemsetAsync(r.quality, 0, nc * sizeof(mm_queue_quality), e->stream));
+  CK(cudaMemsetAsync(r.waits, 0, nc * sizeof(mm_match_waits), e->stream));
+  OtArgs a{};
+  a.hdr = w.hdr; a.n_lob = nl; a.n_mem = nm; a.n_cut = nc; a.n_groups = e->cfg.n_groups; a.now = w.now;
+  a.key_lo = e->key_lo; a.mode_tsize = e->d_mode_tsize; a.cval = e->tb.cval; a.ts = o.ts; a.bal_mask = bal_mask;
+  a.bal_imb = o.imb; a.qlbase = w.qlbase; a.qmbase = w.qmbase; a.qb = o.qb; a.qm = o.qb + nc + 1; a.lob = r.lob;
+  a.waits = r.waits;
+  k_ot_bases<<<1, kOtBlock, 0, e->stream>>>(a);
+  k_ot_lobby<<<grid256(e, (uint64_t)nl * 32, 8), kOtBlock, 0, e->stream>>>(a);
+  MqArgs q{};  // k_mq_queue reads only the lobby records, their queue bases and the records it adds into
+  q.n_cut = nc; q.qlob = a.qb; q.lob = r.lob; q.n_lob = nl; q.qrec = r.quality;
+  const uint32_t qctas = std::max<uint32_t>(1, std::min<uint32_t>(nl / 1024 + 1, 8u * (uint32_t)e->n_sms));
+  k_mq_queue<kMqBlock><<<qctas, kMqBlock, 0, e->stream>>>(q);
+  const uint32_t wctas = std::max<uint32_t>(1, std::min<uint32_t>(nm / 4096 + 1, 8u * (uint32_t)e->n_sms));
+  k_ot_waits<kOtBlock><<<wctas, kOtBlock, 0, e->stream>>>(a);
+  CK(cudaGetLastError());
+  r.n_lob = nl;
   return MM_OK;
 }
 
@@ -2709,24 +2756,26 @@ int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* 
     return set_err(e, MM_E_CAP, "need lobby_cap >= %u and member_cap >= %u", nl, nm);
   if (nl == 0) return MM_OK;
   // from here on the call changes the pool
-  int rc = bf_take(e, h);
+  int rc = bf_take(e, h, true);
   if (rc) return rc;
   CK(s.hdr.reserve(nl));
   a.hdr = s.hdr;
   k_wd_hdr<<<(nl + 255) / 256, 256, 0, e->stream>>>(a, nl);
-  const uint32_t np = h[kBfPieces];
-  k_bf_out<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, a.mbase,
-                                                                               b.staging, b.members);
-  if (e->tb_mask) {  // team_balance: each member's c from its piece's bin, then the tick's balance kernel
-    CK(e->tb.cval.reserve((size_t)e->capacity + 64));
-    k_tb_pieces<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, a.mbase, e->d_bin_key,
-                                                                                  e->tb.cval);
+  const uint32_t np = h[kBfPieces], pgrid = (uint32_t)(((size_t)np * 32 + 255) / 256);
+  k_bf_out<<<pgrid, 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, a.mbase, b.staging.p, b.members.p);
+  // each member's stamp and c from its piece (the off-tick report; c also feeds team_balance)
+  auto& o = e->ot;
+  CK(e->tb.cval.reserve((size_t)e->capacity + 64));
+  CK(o.ts.reserve(nm)); CK(o.imb.reserve(nl));
+  k_bf_out<<<pgrid, 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, a.mbase, b.staging_ts.p, o.ts.p);
+  k_tb_pieces<<<pgrid, 256, 0, e->stream>>>(np, b.piece, a.mbase, e->d_bin_key, e->tb.cval);
+  if (e->tb_mask) {  // team_balance: the tick's balance kernel
     TbArgs t{};
     t.hdr = s.hdr; t.n_lob = nl; t.members = b.members; t.mask = e->tb_mask; t.mode_tsize = e->d_mode_tsize;
-    t.cval = e->tb.cval;
+    t.cval = e->tb.cval; t.imb = o.imb;
     k_tb_lobby<true><<<grid256(e, (uint64_t)nl * 32, 8), 256, 0, e->stream>>>(t);
   }
-  CK(cudaGetLastError());
+  if ((rc = ot_capture(e, MM_OFFTICK_WIDEN, a, nl, nm, e->tb_mask))) return rc;
   CK(cudaEventRecord(e->ev[4], e->stream));
   CK(cudaMemcpyAsync(lobbies, s.hdr, (size_t)nl * sizeof(mm_lobby_hdr), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaMemcpyAsync(member_ids, b.members, (size_t)nm * 8, cudaMemcpyDeviceToHost, e->stream));
@@ -3297,35 +3346,40 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
     return set_err(e, MM_E_CAP, "need lobby_cap >= %u and member_cap >= %llu", nl, (unsigned long long)nm);
   if (nl == 0) return MM_OK;
   // from here on the call changes the pool and the table
-  if (ns && (rc = bf_take(e, h))) return rc;
+  if (ns && (rc = bf_take(e, h, true))) return rc;
   CK(b.members.reserve(nm));
   CK(w.hdr.reserve(nl));
   a.hdr = w.hdr;
   k_wd_hdr<<<(nl + 255) / 256, 256, 0, e->stream>>>(a, nl);
-  const uint32_t np = h[kBfPieces];
+  const uint32_t np = h[kBfPieces], pgrid = (uint32_t)(((size_t)np * 32 + 255) / 256);
   if (np)
-    k_bf_out<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase,
-                                                                                 a.mbase, b.staging, b.members);
+    k_bf_out<<<pgrid, 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, a.mbase, b.staging.p, b.members.p);
   x.members = b.members;
   k_pt_out<<<gr, 256, 0, e->stream>>>(x, a.mbase, act_view(e));
+  // each member's stamp and c (solos from their piece, party members their own rating and their party's stamp) for
+  // the off-tick report; c and the continuation bits also feed party_balance's split, which keeps every party whole
   auto& tb = e->tb;
-  if (e->pb_mask) {  // party_balance: each member's c (solos from their piece's bin, party members their own), then
-                     // the split that keeps every party whole
-    CK(tb.cval.reserve(std::max<size_t>((size_t)e->capacity + 64, nm)));
+  auto& o = e->ot;
+  CK(tb.cval.reserve(std::max<size_t>((size_t)e->capacity + 64, nm)));
+  CK(o.ts.reserve(nm)); CK(o.imb.reserve(nl));
+  if (e->pb_mask) {
     CK(tb.cont.reserve(nl));
     CK(tb.sum.reserve(1));
     CK(cudaMemsetAsync(tb.cont, 0, (size_t)nl * 4, e->stream));
     CK(cudaMemsetAsync(tb.sum, 0, 8, e->stream));
-    if (np)
-      k_tb_pieces<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, a.mbase, e->d_bin_key,
-                                                                                    tb.cval);
-    k_tb_parties<<<gr, 256, 0, e->stream>>>(x, a, e->pb_mask, e->key_lo, e->KR, tb.cval, tb.cont);
+  }
+  if (np) {
+    k_bf_out<<<pgrid, 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, a.mbase, b.staging_ts.p, o.ts.p);
+    k_tb_pieces<<<pgrid, 256, 0, e->stream>>>(np, b.piece, a.mbase, e->d_bin_key, tb.cval);
+  }
+  k_tb_parties<<<gr, 256, 0, e->stream>>>(x, a, e->pb_mask, e->key_lo, e->KR, tb.cval, tb.cont, o.ts);
+  if (e->pb_mask) {
     TbArgs v{};
     v.hdr = w.hdr; v.n_lob = nl; v.members = b.members; v.mask = e->pb_mask; v.mode_tsize = e->d_mode_tsize;
-    v.cval = tb.cval; v.cont = tb.cont; v.imb_sum = tb.sum;
+    v.cval = tb.cval; v.cont = tb.cont; v.imb_sum = tb.sum; v.imb = o.imb;
     k_tb_lobby<true, true><<<grid256(e, (uint64_t)nl * 32, 8), 256, 0, e->stream>>>(v);
   }
-  CK(cudaGetLastError());
+  if ((rc = ot_capture(e, MM_OFFTICK_PARTY_MATCH, a, nl, (uint32_t)nm, e->pb_mask))) return rc;
   CK(cudaEventRecord(e->ev[4], e->stream));
   CK(cudaMemcpyAsync(lobbies, w.hdr, (size_t)nl * sizeof(mm_lobby_hdr), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaMemcpyAsync(member_ids, b.members, (size_t)nm * 8, cudaMemcpyDeviceToHost, e->stream));
@@ -3773,12 +3827,17 @@ int mm_widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hd
              uint64_t* member_ids, uint64_t member_cap, mm_widen_stats* stats) {
   if (!e) return MM_E_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
+  auto& rep = e->ot.rep[MM_OFFTICK_WIDEN];  // void until this call returns MM_OK; its capture sets the lobby count
+  rep.valid = false;
+  rep.n_lob = 0;
   if (!rules || !stats) return set_err(e, MM_E_ARG, "null rules or stats");
   std::memset(stats, 0, sizeof(*stats));
   if ((lobby_cap && !lobbies) || (member_cap && !member_ids))
     return set_err(e, MM_E_ARG, "null lobbies or member_ids with a non-zero capacity");
   CK(cudaSetDevice(e->device));
-  return widen(e, now, rules, lobbies, lobby_cap, member_ids, member_cap, stats);
+  const int rc = widen(e, now, rules, lobbies, lobby_cap, member_ids, member_cap, stats);
+  rep.valid = rc == MM_OK;
+  return rc;
 }
 
 int mm_enqueue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t* ids, const int32_t* rating,
@@ -3808,12 +3867,17 @@ int mm_party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lo
                    uint64_t* member_ids, uint64_t member_cap, mm_party_stats* stats) {
   if (!e) return MM_E_ARG;
   std::lock_guard<std::mutex> lk(e->mu);
+  auto& rep = e->ot.rep[MM_OFFTICK_PARTY_MATCH];  // void until this call returns MM_OK; its capture sets the lobby count
+  rep.valid = false;
+  rep.n_lob = 0;
   if (!rules || !stats) return set_err(e, MM_E_ARG, "null rules or stats");
   std::memset(stats, 0, sizeof(*stats));
   if ((lobby_cap && !lobbies) || (member_cap && !member_ids))
     return set_err(e, MM_E_ARG, "null lobbies or member_ids with a non-zero capacity");
   CK(cudaSetDevice(e->device));
-  return party_match(e, now, rules, lobbies, lobby_cap, member_ids, member_cap, stats);
+  const int rc = party_match(e, now, rules, lobbies, lobby_cap, member_ids, member_cap, stats);
+  rep.valid = rc == MM_OK;
+  return rc;
 }
 
 int mm_party_read(mm_engine* e, uint32_t party_cap, uint32_t member_cap, uint8_t* size, uint32_t* seq, uint32_t* enq_ts,
@@ -4042,6 +4106,48 @@ int mm_match_quality(mm_engine* e, mm_queue_quality* per_queue, uint32_t cap, ui
   }
   CK(cudaSetDevice(e->device));
   return match_quality(e, per_queue, per_lobby, n_lob);
+}
+
+int mm_offtick_report(mm_engine* e, uint32_t source, mm_match_waits* waits, mm_queue_quality* quality, uint32_t cap,
+                      uint32_t* n_out, mm_lobby_quality* per_lobby, uint32_t lobby_cap, uint32_t* n_lobbies) {
+  if (!e || !n_out || !n_lobbies) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (source > MM_OFFTICK_WIDEN) return set_err(e, MM_E_ARG, "unknown source %u", source);
+  const auto& r = e->ot.rep[source];
+  const uint32_t n_cut = e->n_cut, G = e->cfg.n_groups, n_lob = r.valid ? r.n_lob : 0u;
+  *n_out = n_cut;
+  *n_lobbies = n_lob;
+  if ((waits || quality) && cap < n_cut) return set_err(e, MM_E_CAP, "need cap >= %u", n_cut);
+  if (per_lobby && lobby_cap < n_lob) return set_err(e, MM_E_CAP, "need lobby_cap >= %u", n_lob);
+  if (!r.valid) {  // no call of the source yet, or its last one did not return MM_OK
+    *n_out = 0;
+    return MM_OK;
+  }
+  if (n_lob) {
+    CK(cudaSetDevice(e->device));
+    if (waits) CK(cudaMemcpyAsync(waits, r.waits, (size_t)n_cut * sizeof(mm_match_waits), cudaMemcpyDeviceToHost, e->stream));
+    if (quality)
+      CK(cudaMemcpyAsync(quality, r.quality, (size_t)n_cut * sizeof(mm_queue_quality), cudaMemcpyDeviceToHost, e->stream));
+    if (per_lobby)
+      CK(cudaMemcpyAsync(per_lobby, r.lob, (size_t)n_lob * sizeof(mm_lobby_quality), cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaStreamSynchronize(e->stream));
+  } else {  // a valid call without lobbies: zero records
+    if (waits) std::memset(waits, 0, (size_t)n_cut * sizeof(mm_match_waits));
+    if (quality) std::memset(quality, 0, (size_t)n_cut * sizeof(mm_queue_quality));
+  }
+  for (uint32_t c = 0; c < n_cut; ++c) {
+    const mm_mode_desc& md = e->cfg.modes[c / G];
+    if (waits) {
+      waits[c].mode = (uint8_t)(c / G);
+      waits[c].group = (uint8_t)(c % G);
+      waits[c].n_lobbies = waits[c].n_matched / ((uint32_t)md.teams * md.team_size);  // whole lobbies of L members
+    }
+    if (quality) {
+      quality[c].mode = (uint8_t)(c / G);
+      quality[c].group = (uint8_t)(c % G);
+    }
+  }
+  return MM_OK;
 }
 
 int mm_set_lobby_budget(mm_engine* e, const uint32_t* per_queue, const uint32_t* per_mode) {

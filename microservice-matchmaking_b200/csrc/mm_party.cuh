@@ -24,8 +24,9 @@
 // mm_widen's; k_wd_bases / k_wd_hdr write the headers and bases and k_pt_out copies the party members.
 //
 // Balance (mm_set_option "party_balance", mm_balance.cuh): after k_pt_out, k_tb_pieces gives every solo its c and
-// k_tb_parties every placed member of a masked mode its own c and its lobby the party's continuation bits; then
-// k_tb_lobby<true, true> splits each lobby of a masked mode, every party kept whole.
+// k_tb_parties every placed member its own c and its party's stamp (the off-tick report, mm_offtick.cuh) and, in a
+// masked mode, its lobby the party's continuation bits; then k_tb_lobby<true, true> splits each lobby of a masked
+// mode, every party kept whole.
 //
 // Hand-over (mm_export_parties / mm_merge_parties): k_pt_sel and two k_scan_small give every selected live row its
 // image index and member offset, k_pt_export gathers the columns in age order and releases the row (pt_release, as
@@ -658,18 +659,23 @@ __global__ void k_pt_out(const PtArgs p, const uint32_t* __restrict__ mbase, Act
   p.t.dead[r] = 1;
 }
 
-// party_balance: one thread per row placed in this call into a lobby of a masked mode — its members' c - key_lo at
-// their member slots, and bits pos + 1 .. pos + size - 1 (member i continues member i - 1's party) in the continuation
-// word of the lobby's header position (cont zeroed by the host).
+// One thread per row placed in this call, every mode: its members' c - key_lo and the party's enq_ts at their member
+// slots (the off-tick report, mm_offtick.cuh); for a lobby of a party_balance mode (mask), bits pos + 1 .. pos + size
+// - 1 (member i continues member i - 1's party) in the continuation word of the lobby's header position (cont zeroed by
+// the host).
 __global__ void k_tb_parties(const PtArgs p, const WdArgs a, uint32_t mask, int32_t key_lo, uint32_t KR,
-                             uint32_t* __restrict__ cval, uint32_t* __restrict__ cont) {
+                             uint32_t* __restrict__ cval, uint32_t* __restrict__ cont, uint32_t* __restrict__ ts) {
   const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= p.n_rows || p.lob[r] == kPtNone || !((mask >> p.t.mode[r]) & 1u)) return;
-  const uint32_t l = p.lob[r], at = p.pos[r], n = p.t.size[r], o = p.t.off[r];
+  if (r >= p.n_rows || p.lob[r] == kPtNone) return;
+  const uint32_t l = p.lob[r], at = p.pos[r], n = p.t.size[r], o = p.t.off[r], stamp = p.t.ts[r];
   const uint2 x = a.rec[l];
   uint32_t* dst = cval + a.mbase[l] + at;
-  for (uint32_t k = 0; k < n; ++k) dst[k] = clamp_key(key_lo, KR, p.t.mrat[o + k]);
-  atomicOr(&cont[a.qlbase[x.x] + x.y], ((1u << (n - 1)) - 1u) << (at + 1));
+  uint32_t* dts = ts + a.mbase[l] + at;
+  for (uint32_t k = 0; k < n; ++k) {
+    dst[k] = clamp_key(key_lo, KR, p.t.mrat[o + k]);
+    dts[k] = stamp;
+  }
+  if ((mask >> p.t.mode[r]) & 1u) atomicOr(&cont[a.qlbase[x.x] + x.y], ((1u << (n - 1)) - 1u) << (at + 1));
 }
 
 }  // namespace mm

@@ -74,6 +74,13 @@ QUALITY_DTYPE = np.dtype([
 ])
 assert QUALITY_DTYPE.itemsize == C.sizeof(abi.QueueQuality)
 
+# mm_match_waits (include/mm_engine.h) as a numpy record: the match section of QUEUE_STAT_DTYPE
+WAITS_DTYPE = np.dtype([
+    ("mode", "u1"), ("group", "u1"), ("reserved", "<u2"), ("n_lobbies", "<u4"), ("n_matched", "<u4"),
+    ("max_match_wait", "<u4"), ("match_wait_hist", "<u4", (abi.MM_WAIT_BUCKETS,)),
+])
+assert WAITS_DTYPE.itemsize == C.sizeof(abi.MatchWaits)
+
 
 def wait_of(now, enq_ts):
     """Wait of a player as mm_queue_stats counts it: (now - enq_ts) mod 2^32 read as a signed 32-bit value, negative
@@ -695,6 +702,26 @@ class Engine:
                 continue
             self._check(rc, "mm_match_quality")
             return out[:n.value], (lob[:nl.value] if want_lobbies else None)
+
+    def offtick_report(self, source, want_lobbies=False):
+        """Waits and rating quality of the lobbies the last call of `source` formed (mm_offtick_report; source
+        abi.MM_OFFTICK_PARTY_MATCH or abi.MM_OFFTICK_WIDEN) -> (WAITS_DTYPE[n_modes * n_groups], QUALITY_DTYPE[n_modes *
+        n_groups], both in queue_stats() record order, LOBBY_QUALITY_DTYPE[n_lobbies] in that call's lobby order, or None
+        without want_lobbies).  All are empty when the report is void (no such call yet, or its last one failed)."""
+        cap = self.cfg.n_modes * self.cfg.n_groups
+        lobby_cap = 1 << 12 if want_lobbies else 0  # resized from the count of an MM_E_CAP refusal
+        n, nl = C.c_uint32(0), C.c_uint32(0)
+        while True:
+            waits = np.zeros(cap, WAITS_DTYPE)
+            quality = np.zeros(cap, QUALITY_DTYPE)
+            lob = np.zeros(lobby_cap, LOBBY_QUALITY_DTYPE) if want_lobbies else None
+            rc = self.lib.mm_offtick_report(self.h, source, _p(waits), _p(quality), cap, C.byref(n), _p(lob), lobby_cap,
+                                            C.byref(nl))
+            if rc == abi.MM_E_CAP and (n.value > cap or (want_lobbies and nl.value > lobby_cap)):
+                cap, lobby_cap = max(cap, n.value), max(lobby_cap, nl.value)
+                continue
+            self._check(rc, "mm_offtick_report")
+            return waits[:n.value], quality[:n.value], (lob[:nl.value] if want_lobbies else None)
 
     # -- lobby budget ----------------------------------------------------------------
     def set_lobby_budget(self, per_queue=None, per_mode=None):

@@ -1108,6 +1108,42 @@ class SearchPool:
             }
         return out
 
+    def offtick_status(self, group_name):
+        """Waits and rating quality of the lobbies the last step formed outside the tick, in one rating group
+        (Engine.offtick_report), per mode name and per source ("party_match" for party lobbies, "widen" for widened
+        ones, each only when the pool runs it): lobbies, matched players, the p50 / p99 / max wait at match in ms, and
+        the mean / p99 / max rating spread and team imbalance in rating points.  Quantiles are the upper bounds of
+        histogram buckets (at most 25 % high).  A source whose report is void (no call yet, or a failed one) is left
+        out; {} for a group the pool does not know."""
+        from .abi import MM_OFFTICK_PARTY_MATCH, MM_OFFTICK_WIDEN
+        from .engine import wait_quantile
+        if group_name not in self.group_names:
+            return {}
+        g = self.group_names.index(group_name)
+        sources = [("party_match", MM_OFFTICK_PARTY_MATCH)] if self.party_rules else []
+        sources += [("widen", MM_OFFTICK_WIDEN)] if self.widen else []
+        out = {}
+        for name, src in sources:
+            waits, quality, _ = self.engine.offtick_report(src)
+            for w, r in zip(waits, quality):
+                if int(w["group"]) != g or int(w["mode"]) >= len(self.mode_names):
+                    continue
+                n = int(r["n_lobbies"])
+                out.setdefault(self.mode_names[int(w["mode"])], {})[name] = {
+                    "lobbies": n,
+                    "matched": int(w["n_matched"]),
+                    "p50_match_wait_ms": wait_quantile(w["match_wait_hist"], 0.50),
+                    "p99_match_wait_ms": wait_quantile(w["match_wait_hist"], 0.99),
+                    "max_match_wait_ms": int(w["max_match_wait"]),
+                    "mean_spread": int(r["sum_spread"]) / n if n else 0.0,
+                    "p99_spread": wait_quantile(r["spread_hist"], 0.99),
+                    "max_spread": int(r["max_spread"]),
+                    "mean_imbalance": int(r["sum_imbalance"]) / n if n else 0.0,
+                    "p99_imbalance": wait_quantile(r["imbalance_hist"], 0.99),
+                    "max_imbalance": int(r["max_imbalance"]),
+                }
+        return out
+
 
 class SearchWorker:
     """Matchmaking.Search.Worker — one consumer of `matchmaking.queues.<group>`."""
@@ -1159,6 +1195,8 @@ class SearchWorker:
             st["held_back"] = self.pool.held_back(self.group_name)
         if self.pool.party_rules and hasattr(self.pool.engine, "party_read"):  # this group's queued parties, per mode
             st["parties"] = self.pool.party_status(self.group_name)
+        if (self.pool.party_rules or self.pool.widen) and hasattr(self.pool.engine, "offtick_report"):
+            st["offtick"] = self.pool.offtick_status(self.group_name)  # party and widen lobbies of the last step
         return ("ok", st)
 
     def prepare_game_lobby(self, channel_name, exchange_forward, queue_forward, payload):  # worker.ex:250-261
