@@ -537,6 +537,51 @@ int mm_requeue_party(mm_engine* e, uint32_t n_parties, const uint8_t* size, cons
                      const uint8_t* mode, const uint32_t* enq_ts, const uint32_t* seq, uint8_t* codes,
                      uint32_t* n_requeued);
 
+/* mm_backfill_party: mm_backfill with teams and parties.  A running lobby that lost members (a premade that left during
+ * loading, a player who declined) gets its open team slots filled with whole queued parties of its queue first, then
+ * with the nearest solos, each party kept on one team.  Requests are mm_backfill_req, as for mm_backfill; `room` holds
+ * their open slots, flattened: request j owns the next T_j entries (T_j = teams of its mode), entry t the open slots of
+ * team t (0 <= room <= team_size), and count must be the sum of its entries (room carries no lengths of its own).
+ * DEFINITION.  c() is the tick's key clamp and age order (seq - seq_next) mod 2^32 ascending, as in mm_widen.  Requests
+ * are served one at a time in index order, each against the live solos U and the queued parties P of its (mode, group)
+ * queue that no earlier request of the call took:
+ *   room[t] as given
+ *   Q = the parties b of P with |c(R_b) - c(target)| <= window (no limit when window < 0),
+ *       by (|c(R_b) - c(target)|, c(R_b), age)
+ *   for b in Q: b goes to the lowest team t with room[t] >= size(b); if there is none, b is skipped
+ *   C = the solos x of U with |c(r_x) - c(target)| <= window, by (|c(r_x) - c(target)|, c(r_x), age)
+ *   for t = 0 .. T-1: the next room[t] players of C (as many as are left) fill team t
+ * filled (parallel to room) gets the members each team received, n_taken[j] the sum of request j's filled entries and
+ * *n_total the sum of n_taken.  member_ids holds request 0's members, then request 1's, ...; inside a request team-major
+ * (team 0's members, then team 1's), inside a team its parties in placement order, each with its members in party
+ * order, then its solos in C's order (handles on MM_F_DENSE_IDS engines).  A request may be filled in part, as in
+ * mm_backfill: a caller that wants all or nothing hands a short fill back with mm_requeue (solos) and mm_requeue_party
+ * (parties).  When no party of the queue lies inside the window, the member list is mm_backfill's with count =
+ * sum(room) and the same target and window.  n = 0 does nothing.
+ * Effects: taken solos leave the pool exactly as mm_take takes them; a placed party's row is gone and its members are
+ * matched players (mm_locate state 2, mm_requeue and mm_requeue_party code 1).  The last tick's results,
+ * mm_match_quality, the match section of mm_queue_stats, both mm_offtick_report sources, the lobby budget, the
+ * snapshot, the mm_enqueue_rejects list, pending async_results copies and the options are left alone.  No balance pass
+ * runs (team_balance and party_balance do not apply): the caller owns the running lobby's teams, as with mm_backfill.
+ * Refusals, all decided before anything changes (mm_last_error names the cause and the request index):
+ *   MM_E_ARG   null pointers with n > 0; a mode >= n_modes, a group >= n_groups, reserved != 0; a room entry above the
+ *              mode's team_size; a count that is not the sum of its room entries; a mode of more than 256 teams; an
+ *              MM_ORDER_ARRIVAL engine (party windows are rating distances, as for every party call);
+ *   MM_E_STATE no party capacity, an MM_F_NO_DEDUPE engine, a staged packed batch;
+ *   MM_E_CAP   member_cap < *n_total.  filled, n_taken and *n_total are still written: member_cap = 0 is a dry run.
+ * Cost: the party table's compaction and (bin, age) sort (as mm_party_match), one warp per queue with requests walking
+ * the party rows and the per-bin totals sequentially over its requests, and mm_backfill's gather over the partitions
+ * holding a taken solo.  Only the requests, room, filled, n_taken and member_ids cross PCIe.
+ *
+ * EQUIVALENCE.  Take mm_export_parties(NULL) and then mm_export of the engine just before the call; delete the placed
+ * parties from the party image, delete the taken solos from sections 2-6 of the engine image and from their partition
+ * counts, and add every taken id (solos and party members alike) to section 7.  A fresh engine with the same
+ * party_capacity that mm_import's that image and then mm_merge_parties(MM_PARTY_KEEP_SEQ) the party image gives the same
+ * results as this engine for every later call sequence, except what mm_import itself changes (dead slots, the next
+ * tick's pool_before and n_dead, mm_queue_stats' n_removed).                                                        */
+int mm_backfill_party(mm_engine* e, uint32_t n, const mm_backfill_req* req, const uint16_t* room, uint16_t* filled,
+                      uint32_t* n_taken, uint64_t* member_ids, uint64_t member_cap, uint32_t* n_total);
+
 /* Replaces ActiveUser.in_queue?/1 (models/active_user.ex:33-44), batched.          */
 int mm_in_queue(mm_engine* e, uint32_t n, const uint64_t* id, uint8_t* out);
 

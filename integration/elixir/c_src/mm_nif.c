@@ -603,6 +603,46 @@ static ERL_NIF_TERM nif_backfill(ErlNifEnv* env, int argc, const ERL_NIF_TERM ar
   return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &taken), enif_make_binary(env, &hs));
 }
 
+/* backfill_party(ref, requests :: binary(mm_backfill_req[]), room :: binary(u16[]))
+ * -> {:ok, filled :: binary(u16[]), handles :: binary(u32[])}: the open team slots of running lobbies filled with whole
+ * queued parties, then the nearest solos (mm_backfill_party); room holds every request's open slots per team (teams of
+ * its mode entries each, count = their sum), filled the members each team received, handles request 0's members team
+ * by team, then request 1's, ...  The member buffer is sized from the dry run's total (member_cap = 0). */
+static ERL_NIF_TERM nif_backfill_party(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifBinary rq, rm, filled, hs; uint32_t total = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_inspect_binary(env, argv[1], &rq) ||
+      !enif_inspect_binary(env, argv[2], &rm))
+    return enif_make_badarg(env);
+  if (rq.size % sizeof(mm_backfill_req) || rm.size % 2) return enif_make_badarg(env);
+  const uint32_t n = (uint32_t)(rq.size / sizeof(mm_backfill_req));
+  mm_backfill_req* req = enif_alloc(rq.size + 1);
+  uint16_t* room = enif_alloc(rm.size + 2);
+  uint32_t* taken = enif_alloc(4 * (size_t)n + 4);
+  if (!req || !room || !taken || !enif_alloc_binary(rm.size, &filled)) {
+    enif_free(req); enif_free(room); enif_free(taken);
+    return err(env, MM_E_CAP);
+  }
+  memcpy(req, rq.data, rq.size);
+  memcpy(room, rm.data, rm.size);
+  /* the dry run: counts only.  room must hold teams_of(mode) entries per request, as mm_backfill_party reads them;
+   * Pool.backfill_teams/1 checks every request's list against its mode before the call. */
+  int rc = mm_backfill_party(r->e, n, req, room, (uint16_t*)filled.data, taken, NULL, 0, &total);
+  if (rc == MM_E_CAP || rc == MM_OK) {
+    uint64_t* id = enif_alloc(8 * (size_t)total + 8);
+    if (!id || !enif_alloc_binary(4 * (size_t)total, &hs)) rc = MM_E_CAP;
+    else {
+      rc = mm_backfill_party(r->e, n, req, room, (uint16_t*)filled.data, taken, id, total, &total);
+      if (rc) enif_release_binary(&hs);
+      else for (uint32_t k = 0; k < total; ++k) { const uint32_t h = (uint32_t)id[k]; memcpy(hs.data + 4 * (size_t)k, &h, 4); }
+    }
+    enif_free(id);
+  }
+  enif_free(req); enif_free(room); enif_free(taken);
+  if (rc) { enif_release_binary(&filled); return err(env, rc); }
+  return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &filled), enif_make_binary(env, &hs));
+}
+
 /* widen(ref, now :: u64, rules :: binary(mm_widen_rule[n_modes * n_groups]))
  *   -> {:ok, lobbies :: binary(mm_lobby_hdr[]), handles :: binary(u32[])}: lobbies formed around the players who waited longest, each in a rating window that grows
  * with its wait (mm_widen).  badarg unless the binary holds exactly one rule per (mode, group) queue.  The buffers are
@@ -890,6 +930,7 @@ static ErlNifFunc funcs[] = {
   {"requeue", 6, nif_requeue, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"requeue_party", 7, nif_requeue_party, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"backfill", 2, nif_backfill, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"backfill_party", 3, nif_backfill_party, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"widen", 3, nif_widen, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"enqueue_party", 6, nif_enqueue_party, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"party_match", 3, nif_party_match, ERL_NIF_DIRTY_JOB_CPU_BOUND},

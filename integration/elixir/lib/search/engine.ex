@@ -153,6 +153,15 @@ defmodule Matchmaking.Search.Engine do
   """
   def backfill(_ref, _requests), do: :erlang.nif_error(:nif_not_loaded)
   @doc """
+  Party backfill (extension): the open team slots of running lobbies filled with whole queued parties first, then the
+  nearest solos (mm_backfill_party).  requests: the 16-byte records of backfill/2, count = the sum of the request's room
+  entries; room: binary of u16 open slots, teams_of(mode) entries per request, in request order -> {:ok, filled ::
+  binary(u16[]) (members per team, parallel to room), handles :: binary(u32[])}: request 0's members team by team (a
+  team's parties, then its solos), then request 1's, ...  Placed parties leave the party table, taken solos the pool;
+  all stay in the active set until remove_user.
+  """
+  def backfill_party(_ref, _requests, _room), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
   Widening search (extension): lobbies formed around the players who waited longest, each in a rating window that
   grows with its wait (mm_widen).  rules: binary of n_modes * n_groups 24-byte records <<min_wait::little-32,
   step::little-32, w0::little-signed-32, inc::little-signed-32, w_max::little-signed-32, 0::32>>, queue

@@ -122,6 +122,15 @@ defmodule Matchmaking.Search.Pool do
   """
   def backfill(requests), do: GenServer.call(__MODULE__, {:backfill, requests}, :infinity)
   @doc """
+  Party backfill (extension; needs party_capacity): a running lobby's open team slots filled with whole queued parties
+  first, then the nearest solos (Engine.backfill_party).  requests: [{mode_name, group_index, target_rating,
+  open_slots}] or [{..., open_slots, window}], open_slots = one count per team of the mode, served in order -> {:ok,
+  per request one list of player documents per team} (a team's parties, each party's members together, then its solos;
+  shorter than its open slots when the queue runs short).  A placed party's book entry moves aside as after
+  party_match, so requeue/1 with requeue_parties puts it back whole.
+  """
+  def backfill_teams(requests), do: GenServer.call(__MODULE__, {:backfill_teams, requests}, :infinity)
+  @doc """
   Search status (extension): one map per player id, without ingesting the staged deliveries (Engine.locate):
   %{state: :searching | :matched | :staged | :unknown, game_mode, group, wait_ms, position, queue_size,
   next_tick: %{lobby: ordinal among the queue's lobbies, team: index} | nil}.  The prediction is for the engine as it
@@ -693,6 +702,40 @@ defmodule Matchmaking.Search.Pool do
         {out, _} = Enum.map_reduce(for(<<k::little-32 <- n_taken>>, do: k), hs, &Enum.split(&2, &1))
         docs = Enum.map(out, fn part -> Enum.map(part, &Map.fetch!(st.players, &1)) end)
         {:reply, {:ok, docs}, %{st | players: Map.drop(st.players, hs)}}
+      {:error, _} = e -> {:reply, e, st}
+    end
+  end
+
+  def handle_call({:backfill_teams, requests}, _from, st) do
+    st = flush(st)
+    reqs = for r <- requests do
+      case r do
+        {m, g, t, slots} -> {m, g, t, slots, -1}
+        {m, g, t, slots, w} -> {m, g, t, slots, w}
+      end
+    end
+    req = for {mode, group, target, slots, window} <- reqs, into: <<>> do
+      <<(Engine.mode_index(mode) || 255), group, 0::16, Enum.sum(slots)::little-32, target::little-signed-32,
+        window::little-signed-32>>
+    end
+    room = for {_, _, _, slots, _} <- reqs, s <- slots, into: <<>>, do: <<s::little-16>>
+    # the engine reads teams_of(mode) room entries per request: a list of another length is refused here
+    laid_out = Enum.all?(reqs, fn {mode, _, _, slots, _} ->
+      m = Engine.mode_index(mode)
+      m != nil and length(slots) == Engine.teams_of(m)
+    end)
+    result = if laid_out, do: Engine.backfill_party(st.ref, req, room), else: {:error, :badarg}
+    case result do
+      {:ok, filled, handles} ->
+        hs = for <<h::little-32 <- handles>>, do: h
+        counts = for <<f::little-16 <- filled>>, do: f
+        {teams, _} = Enum.map_reduce(counts, hs, &Enum.split(&2, &1))
+        {out, _} = Enum.map_reduce(reqs, teams, fn {_, _, _, slots, _}, rest -> Enum.split(rest, length(slots)) end)
+        docs = Enum.map(out, fn per_team -> Enum.map(per_team, fn t -> Enum.map(t, &Map.fetch!(st.players, &1)) end) end)
+        # a placed party's book entry moves aside, as after party_match, so requeue/1 can put the party back whole
+        matched = for h <- hs, rec = Map.get(st.party_book, h), rec != nil, into: st.matched_parties, do: {h, rec}
+        {:reply, {:ok, docs}, %{st | players: Map.drop(st.players, hs), party_of: Map.drop(st.party_of, hs),
+                                     party_book: Map.drop(st.party_book, hs), matched_parties: matched}}
       {:error, _} = e -> {:reply, e, st}
     end
   end

@@ -309,6 +309,7 @@ PROTOTYPES = {
     "mm_band_match": (C.c_int, [_vp, C.c_int32, C.c_uint32, C.c_uint32, C.c_uint32, _vp, _vp, _vp, C.c_uint32,
                                 _vp, C.c_uint32, _vp, C.c_uint64, _vp, _P(BandStats)]),
     "mm_backfill": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, C.c_uint64, _P(C.c_uint32)]),
+    "mm_backfill_party": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, C.c_uint64, _P(C.c_uint32)]),
     "mm_widen": (C.c_int, [_vp, C.c_uint64, _vp, _vp, C.c_uint32, _vp, C.c_uint64, _P(WidenStats)]),
     "mm_enqueue_party": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _vp]),
     "mm_party_match": (C.c_int, [_vp, C.c_uint64, _vp, _vp, C.c_uint32, _vp, C.c_uint64, _P(PartyStats)]),

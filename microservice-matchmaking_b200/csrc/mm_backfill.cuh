@@ -3,10 +3,9 @@
 //
 // Plan (k_bf_plan): the host sorts the requests by queue, stably; one warp per queue serves that queue's requests in
 // order on the resident per-bin totals (tot).  rem[bin] starts from tot and counts the bin's players no earlier request
-// of the call took.  A rating-order request walks its queue's bins outward from its target in (distance, rating) order:
-// the bins below the target (distance growing downwards) and the bins at or above it (growing upwards) are two sorted
-// runs, and each step merges the next 32 bins of the two runs by their distances (a tie goes to the lower rating), takes
-// a warp prefix sum of their rem and consumes bins until the count or the window runs out.  Every (request, bin) take is
+// of the call took.  A rating-order request finds its target among the queue's bins (bf_seek) and walks them outward
+// from it in (distance, rating) order (bf_walk, the one outward walk of every off-tick call: mm_widen, mm_party_match
+// and mm_backfill_party walk with it too).  Every (request, bin) take is
 // one PIECE: the request, the bin, its rank offset inside the bin (the bin's players taken so far in this call), the
 // count and its offset inside the request's output.  Every request takes a bin's oldest untaken players, so the call
 // takes a prefix of every bin in enqueue order: what the band pipeline places with klim = the bin's taken count.
@@ -71,6 +70,88 @@ __device__ __forceinline__ uint32_t bf_rank(uint32_t v, uint32_t x, bool le) {
   return c;
 }
 
+// The first bin of [lo, hi) whose key is >= target (hi: none): the answer lies in [l, h]; each round samples 32 bins of
+// it by a ballot and keeps one slice.  Uniform over the warp.
+__device__ __forceinline__ uint32_t bf_seek(const uint16_t* bin_key, uint32_t lo, uint32_t hi, int32_t target) {
+  const uint32_t lane = threadIdx.x & 31;
+  uint32_t l = lo, h = hi;
+  while (l < h) {
+    const uint32_t step = (h - l + 31) / 32, b = l + lane * step;
+    const uint32_t nb = __popc(__ballot_sync(0xFFFFFFFFu, b < h && (int32_t)bin_key[b] < target));
+    if (nb == 0) break;
+    const uint32_t l0 = l;
+    l = l0 + (nb - 1) * step + 1;
+    h = min(h, l0 + nb * step);
+  }
+  return l;
+}
+
+// The outward walk from `target` over the queue's bins [lo, hi), pos = bf_seek's first bin at or above it, within
+// distance win: the first `need` players in (distance, rating, enqueue order).  The bins below pos (distance growing
+// downwards) and the bins from pos on (growing upwards) are two sorted runs; each step merges the next 32 bins of the two
+// runs by their distances (a tie goes to the lower rating), takes a warp prefix sum of their rem and consumes bins until
+// need or the window runs out.  Without by_rating (arrival order: the queue's one bin) every distance is 0.  Returns how
+// many it found (at most need) and, in left, how many of them lie below pos.  kTake: the players are taken (rem) and
+// written as pieces of record r, each at its offset in member order (the left bins ascending, then the right bins, from
+// offset `left`); kWalkOrder: in walk order instead, from offset `left`.  A: BfArgs or WdArgs (bin_key, tot, rem,
+// piece, ctr).  Uniform over the warp.
+template <bool kTake, bool kWalkOrder = false, class A>
+__device__ __forceinline__ uint32_t bf_walk(const A& a, uint32_t* s_bin, int32_t target, uint32_t pos, uint32_t lo,
+                                            uint32_t hi, uint32_t win, uint32_t need, uint32_t& left, uint32_t r,
+                                            bool by_rating = true) {
+  const uint32_t lane = threadIdx.x & 31;
+  const uint32_t nL = pos - lo, nR = hi - pos;
+  const uint32_t left_all = left;  // kTake: the players below pos that the record takes
+  uint32_t got = 0, used_l = 0, used_r = 0, got_l = 0, got_r = 0;
+  while (need) {
+    // the next 32 bins of each run and their distances (kBfFar past the run or the window)
+    const uint32_t il = used_l + lane, ir = used_r + lane;
+    uint32_t dl = kBfFar, dr = kBfFar;
+    if (il < nL) {
+      const uint32_t d = (uint32_t)(target - (int32_t)a.bin_key[pos - 1 - il]);
+      dl = d <= win ? d : kBfFar;
+    }
+    if (ir < nR) {
+      const uint32_t d = by_rating ? (uint32_t)((int32_t)a.bin_key[pos + ir] - target) : 0u;
+      dr = d <= win ? d : kBfFar;
+    }
+    // merged positions: a lower bin goes before an upper bin of the same distance
+    const uint32_t pl = lane + bf_rank(dr, dl, false), pr = lane + bf_rank(dl, dr, true);
+    const bool okl = dl != kBfFar && pl < 32, okr = dr != kBfFar && pr < 32;
+    if (okl) s_bin[pl] = pos - 1 - il;
+    if (okr) s_bin[pr] = pos + ir;
+    const uint32_t nl = __popc(__ballot_sync(0xFFFFFFFFu, okl)), nr = __popc(__ballot_sync(0xFFFFFFFFu, okr));
+    const uint32_t nv = nl + nr;
+    __syncwarp();
+    uint32_t bin = 0, v = 0;
+    if (lane < nv) { bin = s_bin[lane]; v = a.rem[bin]; }
+    const uint32_t incl = warp_incl_scan(v);
+    const uint32_t excl = incl - v, before = min(excl, need), take = min(v, need - before);
+    const bool is_l = lane < nv && bin < pos;
+    const uint32_t tl = is_l ? take : 0u, tr = is_l ? 0u : take;
+    const uint32_t il_incl = warp_incl_scan(tl), ir_incl = warp_incl_scan(tr);
+    if (kTake) {
+      const uint32_t at = warp_append(&a.ctr[kBfPieces], take != 0);
+      if (take) {
+        // member order: the left bins in ascending rating (reverse walk order), then the right bins in walk order
+        const uint32_t poff = kWalkOrder ? left_all + got + before
+                                         : (is_l ? left_all - (got_l + il_incl) : left_all + got_r + ir_incl - tr);
+        a.piece[at] = BfPiece{r, bin, a.tot[bin] - v, take, poff};
+        a.rem[bin] = v - take;
+      }
+    }
+    got_l += __shfl_sync(0xFFFFFFFFu, il_incl, 31);
+    got_r += __shfl_sync(0xFFFFFFFFu, ir_incl, 31);
+    const uint32_t took = min(__shfl_sync(0xFFFFFFFFu, incl, 31), need);
+    need -= took; got += took;
+    __syncwarp();  // rem and s_bin are read again by the next step
+    if (nv < 32) break;  // both runs (or the window) exhausted
+    used_l += nl; used_r += nr;
+  }
+  left = got_l;
+  return got;
+}
+
 __global__ void __launch_bounds__(kBfPlanWarps * 32) k_bf_plan(const BfArgs a) {
   __shared__ uint32_t s_bin[kBfPlanWarps][32];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, qi = blockIdx.x * kBfPlanWarps + warp;
@@ -80,55 +161,11 @@ __global__ void __launch_bounds__(kBfPlanWarps * 32) k_bf_plan(const BfArgs a) {
   for (uint32_t s = a.qr[c]; s < a.qr[c + 1]; ++s) {
     const BfReq r = a.req[s];
     const uint32_t win = r.window < 0 ? kBfFar - 1 : (uint32_t)r.window;
-    uint32_t pos = lo;  // first bin whose key is >= the target (arrival order: the queue's one bin, at distance 0)
-    if (a.rating_order) {  // the answer lies in [l, h]; each round samples 32 bins of it and keeps one slice
-      uint32_t l = lo, h = hi;
-      while (l < h) {
-        const uint32_t step = (h - l + 31) / 32, b = l + lane * step;
-        const uint32_t nb = __popc(__ballot_sync(0xFFFFFFFFu, b < h && (int32_t)a.bin_key[b] < r.target));
-        if (nb == 0) break;
-        const uint32_t l0 = l;
-        l = l0 + (nb - 1) * step + 1;
-        h = min(h, l0 + nb * step);
-      }
-      pos = l;
-    }
-    const uint32_t nL = pos - lo, nR = hi - pos;
-    uint32_t need = r.count, got = 0, used_l = 0, used_r = 0;
-    while (need) {
-      // the next 32 bins of each run and their distances (kBfFar past the run or the window)
-      const uint32_t il = used_l + lane, ir = used_r + lane;
-      uint32_t dl = kBfFar, dr = kBfFar;
-      if (il < nL) { const uint32_t d = (uint32_t)(r.target - (int32_t)a.bin_key[pos - 1 - il]); dl = d <= win ? d : kBfFar; }
-      if (ir < nR) {
-        const uint32_t d = a.rating_order ? (uint32_t)((int32_t)a.bin_key[pos + ir] - r.target) : 0u;
-        dr = d <= win ? d : kBfFar;
-      }
-      // merged positions: a lower bin goes before an upper bin of the same distance
-      const uint32_t pl = lane + bf_rank(dr, dl, false), pr = lane + bf_rank(dl, dr, true);
-      const bool okl = dl != kBfFar && pl < 32, okr = dr != kBfFar && pr < 32;
-      if (okl) s_bin[warp][pl] = pos - 1 - il;
-      if (okr) s_bin[warp][pr] = pos + ir;
-      const uint32_t nl = __popc(__ballot_sync(0xFFFFFFFFu, okl)), nr = __popc(__ballot_sync(0xFFFFFFFFu, okr));
-      const uint32_t nv = nl + nr;
-      __syncwarp();
-      uint32_t bin = 0, v = 0;
-      if (lane < nv) { bin = s_bin[warp][lane]; v = a.rem[bin]; }
-      const uint32_t incl = warp_incl_scan(v);
-      const uint32_t excl = incl - v, before = min(excl, need), take = min(v, need - before);
-      const uint32_t at = warp_append(&a.ctr[kBfPieces], take != 0);
-      if (take) {
-        const uint32_t t = a.tot[bin];
-        a.piece[at] = BfPiece{r.idx, bin, t - v, take, got + before};
-        a.rem[bin] = v - take;
-      }
-      const uint32_t sum = __shfl_sync(0xFFFFFFFFu, incl, 31);
-      const uint32_t took = min(sum, need);
-      need -= took; got += took;
-      __syncwarp();  // rem and s_bin are read again by the next step
-      if (nv < 32) break;  // both runs (or the window) exhausted
-      used_l += nl; used_r += nr;
-    }
+    // arrival order: the queue's one bin, at distance 0
+    const uint32_t pos = a.rating_order ? bf_seek(a.bin_key, lo, hi, r.target) : lo;
+    uint32_t left = 0;
+    const uint32_t got =
+        bf_walk<true, true>(a, s_bin[warp], r.target, pos, lo, hi, win, r.count, left, r.idx, a.rating_order != 0);
     if (lane == 0) a.n_taken[r.idx] = got;
   }
 }

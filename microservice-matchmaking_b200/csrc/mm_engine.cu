@@ -28,6 +28,7 @@
 #include "mm_locate.cuh"
 #include "mm_offtick.cuh"
 #include "mm_party.cuh"
+#include "mm_party_backfill.cuh"
 #include "mm_quality.cuh"
 #include "mm_recut.cuh"
 #include "mm_regroup.cuh"
@@ -290,6 +291,8 @@ struct mm_engine {
     DevArray<BfPiece> piece;
     DevArray<uint64_t> staging, members;
     DevArray<uint32_t> staging_ts;  // mm_widen / mm_party_match: the taken solos' stamps beside staging
+    DevArray<uint32_t> teams;       // mm_backfill_party: roff [n + 1] | filled | tbase [room entries]
+    DevArray<uint16_t> room;        // mm_backfill_party: [room entries]
   } bf;
 
   // mm_widen (mm_widen.cuh): the call's tables and the anchors, grown on demand; the plan's rem, the keys, the pieces,
@@ -2565,6 +2568,28 @@ int bf_take(mm_engine* e, const uint32_t* h, bool stamps = false) {
   return MM_OK;
 }
 
+// The requests grouped by queue, stably (a counting sort), with the targets as clamp keys: in = the BfReqs in queue
+// order | the first request of every queue [n_cut + 1] | the queues with requests.  -> the number of those queues.
+uint32_t bf_sort(const mm_engine* e, uint32_t n, const mm_backfill_req* req, std::vector<uint32_t>& in) {
+  const uint32_t G = e->cfg.n_groups, nc = e->n_cut;
+  std::vector<uint32_t> qr(nc + 1, 0);
+  for (uint32_t j = 0; j < n; ++j) ++qr[req[j].mode * G + req[j].group + 1];
+  for (uint32_t q = 0; q < nc; ++q) qr[q + 1] += qr[q];
+  const size_t rw = sizeof(BfReq) / 4;
+  in.assign(rw * n + nc + 1, 0);
+  std::copy(qr.begin(), qr.end(), in.begin() + rw * n);
+  std::vector<uint32_t> at(qr.begin(), qr.end() - 1);
+  for (uint32_t j = 0; j < n; ++j) {
+    const mm_backfill_req& r = req[j];
+    const int64_t t = std::min<int64_t>(std::max<int64_t>((int64_t)r.target - e->key_lo, 0), (int64_t)e->KR - 1);
+    const BfReq b{j, r.count, (int32_t)t, r.window};
+    std::memcpy(&in[rw * at[r.mode * G + r.group]++], &b, sizeof(b));
+  }
+  for (uint32_t q = 0; q < nc; ++q)
+    if (qr[q + 1] > qr[q]) in.push_back(q);
+  return (uint32_t)(in.size() - (rw * n + nc + 1));
+}
+
 int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_taken, uint64_t* member_ids,
              uint64_t member_cap, uint32_t* n_total) {
   const mm_config& c = e->cfg;
@@ -2581,24 +2606,10 @@ int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_t
   if (e->stage_count) return staged_err(e);
   if (!e->use_active) return set_err(e, MM_E_STATE, "an MM_F_NO_DEDUPE engine cannot hold taken players");
   if (n == 0) return MM_OK;
-  // the requests grouped by queue, stably (a counting sort), with the targets as clamp keys
-  const uint32_t G = c.n_groups, nc = e->n_cut;
-  std::vector<uint32_t> qr(nc + 1, 0);
-  for (uint32_t j = 0; j < n; ++j) ++qr[req[j].mode * G + req[j].group + 1];
-  for (uint32_t q = 0; q < nc; ++q) qr[q + 1] += qr[q];
+  const uint32_t nc = e->n_cut;
   const size_t rw = sizeof(BfReq) / 4;
-  std::vector<uint32_t> in(rw * n + nc + 1);
-  std::copy(qr.begin(), qr.end(), in.begin() + rw * n);
-  std::vector<uint32_t> at(qr.begin(), qr.end() - 1);
-  for (uint32_t j = 0; j < n; ++j) {
-    const mm_backfill_req& r = req[j];
-    const int64_t t = std::min<int64_t>(std::max<int64_t>((int64_t)r.target - e->key_lo, 0), (int64_t)e->KR - 1);
-    const BfReq b{j, r.count, (int32_t)t, r.window};
-    std::memcpy(&in[rw * at[r.mode * G + r.group]++], &b, sizeof(b));
-  }
-  for (uint32_t q = 0; q < nc; ++q)
-    if (qr[q + 1] > qr[q]) in.push_back(q);
-  const uint32_t nq = (uint32_t)(in.size() - (rw * n + nc + 1));
+  std::vector<uint32_t> in;
+  const uint32_t nq = bf_sort(e, n, req, in);
   auto& s = e->bf;
   const Pool& p = e->pool[e->cur];
   const size_t K = e->K;
@@ -3391,6 +3402,114 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
   return MM_OK;
 }
 
+// mm_backfill_party (mm_party_backfill.cuh): mm_backfill's request sort, mm_party_match's table sort, then k_pbf_plan;
+// one read of the counters decides MM_E_CAP before the pool or the table changes.
+int backfill_party(mm_engine* e, uint32_t n, const mm_backfill_req* req, const uint16_t* room, uint16_t* filled,
+                   uint32_t* n_taken, uint64_t* member_ids, uint64_t member_cap, uint32_t* n_total) {
+  const mm_config& c = e->cfg;
+  std::vector<uint32_t> roff(n + 1, 0);
+  for (uint32_t j = 0; j < n; ++j) {
+    const mm_backfill_req& r = req[j];
+    if (r.mode >= c.n_modes) return set_err(e, MM_E_ARG, "request %u: mode %u >= n_modes = %u", j, r.mode, c.n_modes);
+    if (r.group >= c.n_groups)
+      return set_err(e, MM_E_ARG, "request %u: group %u >= n_groups = %u", j, r.group, c.n_groups);
+    if (r.reserved) return set_err(e, MM_E_ARG, "request %u: reserved must be 0", j);
+    const mm_mode_desc& md = c.modes[r.mode];
+    if (md.teams > kPtMaxTeams)
+      return set_err(e, MM_E_ARG, "request %u: mode %u has %u teams (parties: at most %u)", j, r.mode, md.teams,
+                     kPtMaxTeams);
+    uint64_t sum = 0;
+    for (uint32_t t = 0; t < md.teams; ++t) {
+      const uint16_t v = room[roff[j] + t];
+      if (v > md.team_size)
+        return set_err(e, MM_E_ARG, "request %u: team %u has room %u > team_size %u", j, t, v, md.team_size);
+      sum += v;
+    }
+    if (sum != r.count)
+      return set_err(e, MM_E_ARG, "request %u: count %u is not the sum %llu of its room entries", j, r.count,
+                     (unsigned long long)sum);
+    roff[j + 1] = roff[j] + md.teams;
+  }
+  int rc = pt_check(e);
+  if (rc) return rc;
+  if (n == 0) return MM_OK;
+  const uint32_t nc = e->n_cut, ne = roff[n];
+  const size_t rw = sizeof(BfReq) / 4;
+  std::vector<uint32_t> in;
+  const uint32_t nq = bf_sort(e, n, req, in);
+  // the table: compacted, then the rows by (bin, age)
+  auto& s = e->pt;
+  if ((rc = pt_compact(e))) return rc;
+  const Pool& p = e->pool[e->cur];
+  const uint32_t nr = s.n_rows, K = e->K, gr = (nr + 255) / 256;
+  PtArgs x{};
+  x.t = pt_view(e, s.cur); x.n_rows = nr; x.pb = s.pb; x.pcur = s.pcur; x.sorted = s.sorted;
+  x.lob = s.lob; x.pos = s.pos; x.mode_tsize = e->d_mode_tsize; x.ctr = s.ctr;
+  CK(cudaMemsetAsync(s.pb, 0, ((size_t)K + 1) * 4, e->stream));
+  CK(cudaMemsetAsync(s.ctr, 0, (kPtWords + 2) * 4, e->stream));
+  if (nr) {
+    k_pt_count<<<gr, 256, 0, e->stream>>>(x, s.pb);
+    k_scan_small<<<1, 1024, 0, e->stream>>>(K + 1, s.pb, s.ctr + kPtWords);
+    CK(cudaMemcpyAsync(s.pcur, s.pb, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
+    k_pt_scatter<<<1, kPtScatterBlock, 0, e->stream>>>(x);
+    CK(cudaMemcpyAsync(s.pcur, s.pb, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));  // the plan's cursors
+  }
+  // the plan, on the solo pool's per-bin totals (the mm_backfill scratch)
+  auto& b = e->bf;
+  CK(b.in.reserve(in.size())); CK(b.rem.reserve(K)); CK(b.key_bin.reserve(K)); CK(b.kbase.reserve(K));
+  CK(b.klim.reserve(K)); CK(b.n_taken.reserve(n)); CK(b.req_base.reserve(n)); CK(b.ctr.reserve(kBfWords));
+  CK(b.teams.reserve((size_t)n + 1 + 2 * (size_t)ne)); CK(b.room.reserve(std::max<uint32_t>(ne, 1)));
+  CK(b.piece.reserve((size_t)ne + K));  // every team walk empties all the bins it reaches but its last
+  CK(cudaMemcpyAsync(b.in, in.data(), in.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(b.teams, roff.data(), ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, e->stream));
+  if (ne) CK(cudaMemcpyAsync(b.room, room, (size_t)ne * 2, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(b.rem, p.m.tot, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
+  CK(cudaMemsetAsync(b.ctr, 0, kBfWords * 4, e->stream));
+  WdArgs a{};
+  a.n_groups = c.n_groups; a.cut_lp_lo = e->d_cut_lp_lo; a.seg_bin_lo = e->d_seg_bin_lo; a.bin_key = e->d_bin_key;
+  a.tot = p.m.tot; a.rem = b.rem; a.piece = b.piece; a.ctr = b.ctr;
+  PbfArgs q{};
+  q.req = reinterpret_cast<const BfReq*>(b.in.p); q.qr = b.in + rw * n; q.queues = b.in + rw * n + nc + 1; q.nq = nq;
+  q.roff = b.teams; q.room = b.room; q.filled = b.teams + n + 1; q.tbase = b.teams + n + 1 + ne; q.n_taken = b.n_taken;
+  k_pbf_plan<<<(nq + kPtPlanWarps - 1) / kPtPlanWarps, kPtPlanWarps * 32, 0, e->stream>>>(x, a, q);
+  BfArgs f{};
+  f.tot = p.m.tot; f.rem = b.rem; f.bin_seg = e->d_bin_seg; f.fill = p.m.fill; f.K = K;
+  f.key_bin = b.key_bin; f.kbase = b.kbase; f.klim = b.klim; f.ctr = b.ctr;
+  k_bf_keys<<<1, kBfKeysBlock, 0, e->stream>>>(f);
+  CK(cudaGetLastError());
+  uint32_t h[kBfWords];
+  std::vector<uint32_t> fill32(ne);
+  CK(cudaMemcpyAsync(n_taken, b.n_taken, (size_t)n * 4, cudaMemcpyDeviceToHost, e->stream));
+  if (ne) CK(cudaMemcpyAsync(fill32.data(), q.filled, (size_t)ne * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(h, b.ctr, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  for (uint32_t i = 0; i < ne; ++i) filled[i] = (uint16_t)fill32[i];
+  std::vector<uint32_t> base(n);
+  uint32_t total = 0;
+  for (uint32_t j = 0; j < n; ++j) { base[j] = total; total += n_taken[j]; }
+  *n_total = total;
+  if (member_cap < total) return set_err(e, MM_E_CAP, "need member_cap >= %u", total);
+  if (total == 0) return MM_OK;
+  // from here on the call changes the pool and the table
+  const uint32_t ns = h[kBfPlayers], np = h[kBfPieces];
+  if (ns && (rc = bf_take(e, h))) return rc;
+  CK(b.members.reserve(total));
+  CK(cudaMemcpyAsync(b.req_base, base.data(), (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
+  if (np)
+    k_bf_out<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase,
+                                                                               b.req_base, b.staging.p, b.members.p);
+  if (total > ns) {
+    x.members = b.members;
+    k_pbf_pos<<<gr, 256, 0, e->stream>>>(x, q);
+    k_pt_out<<<gr, 256, 0, e->stream>>>(x, b.req_base, act_view(e));
+  }
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(member_ids, b.members, (size_t)total * 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  s.live -= total - ns;
+  return MM_OK;
+}
+
 int party_read(mm_engine* e, uint32_t party_cap, uint32_t member_cap, uint8_t* size, uint32_t* seq, uint32_t* enq_ts,
                uint8_t* mode, uint8_t* group, int32_t* rating, uint64_t* member_ids, int32_t* member_rating,
                uint32_t* n_parties, uint32_t* n_members) {
@@ -3821,6 +3940,17 @@ int mm_backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* 
   std::lock_guard<std::mutex> lk(e->mu);
   CK(cudaSetDevice(e->device));
   return backfill(e, n, req, n_taken, member_ids, member_cap, n_total);
+}
+
+int mm_backfill_party(mm_engine* e, uint32_t n, const mm_backfill_req* req, const uint16_t* room, uint16_t* filled,
+                      uint32_t* n_taken, uint64_t* member_ids, uint64_t member_cap, uint32_t* n_total) {
+  if (!e) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!n_total || (n && (!req || !room || !filled || !n_taken)) || (member_cap && !member_ids))
+    return set_err(e, MM_E_ARG, "null n_total, or null req, room, filled, n_taken or member_ids with n = %u", n);
+  *n_total = 0;
+  CK(cudaSetDevice(e->device));
+  return backfill_party(e, n, req, room, filled, n_taken, member_ids, member_cap, n_total);
 }
 
 int mm_widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,

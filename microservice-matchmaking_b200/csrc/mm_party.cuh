@@ -18,8 +18,8 @@
 // Match: after compaction the rows are counting-sorted by (bin, age) — bins are the solo pool's, so a queue's parties
 // are the runs of its bins — and k_pt_plan serves one queue per warp.  The warp takes the queue's anchors in age
 // order, walks the bins outward from the anchor's bin in (distance, rating) order for co-parties (sequential: every
-// placement changes the rooms), then counts the solos of the open slots with wd_walk<false>.  Only a full lobby commits:
-// the same co-party walk again, then one wd_walk<true, walk order> per team with open slots, so the solos fill team 0,
+// placement changes the rooms), then counts the solos of the open slots with bf_walk<false>.  Only a full lobby commits:
+// the same co-party walk again, then one bf_walk<true, walk order> per team with open slots, so the solos fill team 0,
 // then team 1, ... in their rank order.  The solo pieces go through k_bf_keys, the band pipeline and k_bf_out like
 // mm_widen's; k_wd_bases / k_wd_hdr write the headers and bases and k_pt_out copies the party members.
 //
@@ -549,15 +549,15 @@ __global__ void __launch_bounds__(kPtScatterBlock) k_pt_scatter(const PtArgs p) 
   }
 }
 
-// The co-party walk of anchor row `ar` (bin pos of the queue's bins [lo, hi), window win): every unplaced party of the
-// window in (distance, rating, age) order goes to the lowest team with room for it.  room[] holds the teams' free
-// slots on entry (the anchor's taken).  commit: the placed parties get lobby record r and their member offsets.
+// The co-party walk around clamp key `target` (pos: the first of the queue's bins [lo, hi) at or above it, window win)
+// for anchor row `ar` (kPtNone: no anchor): every unplaced party of the window in (distance, rating, age) order goes to
+// the lowest team with room for it.  room[] holds the teams' free slots on entry (the anchor's taken).  commit: the
+// placed parties get lobby record r and member offsets t * S + (S - room[t]) (room[t] before the placement).
 // Uniform over the warp; lane 0 writes.  -> the free slots left.
-__device__ uint32_t pt_walk(const PtArgs& p, const WdArgs& a, uint32_t ar, uint32_t pos, uint32_t lo, uint32_t hi,
-                            uint32_t win, uint16_t* room, uint32_t T, uint32_t S, uint32_t open, bool commit, uint32_t r,
-                            uint32_t& n_placed) {
+__device__ uint32_t pt_walk(const PtArgs& p, const WdArgs& a, uint32_t ar, int32_t target, uint32_t pos, uint32_t lo,
+                            uint32_t hi, uint32_t win, uint16_t* room, uint32_t T, uint32_t S, uint32_t open, bool commit,
+                            uint32_t r, uint32_t& n_placed) {
   const uint32_t lane = threadIdx.x & 31;
-  const int32_t target = (int32_t)a.bin_key[pos];
   uint32_t l = pos, h = pos;  // next bins: l - 1 below, h at or above
   while (open >= 2) {
     uint32_t d_l = kBfFar, d_h = kBfFar;
@@ -612,12 +612,13 @@ __global__ void __launch_bounds__(kPtPlanWarps * 32) k_pt_plan(const PtArgs p, c
       const uint32_t wait = stat_wait(a.now, p.t.ts[ar]);
       const long long w = min((long long)u.w_max, (long long)u.w0 + (long long)((wait - u.min_wait) / u.step) * u.inc);
       const uint32_t win = (uint32_t)min(w, (long long)kBfFar - 1), pos = p.t.bin[ar], sa = p.t.size[ar];
+      const int32_t target = (int32_t)a.bin_key[pos];
       for (uint32_t t = lane; t < T; t += 32) room[t] = (uint16_t)(t == 0 ? S - sa : S);
       __syncwarp();
       uint32_t np = 0;
-      const uint32_t open = pt_walk(p, a, ar, pos, lo, hi, win, room, T, S, u.L - sa, false, 0, np);
+      const uint32_t open = pt_walk(p, a, ar, target, pos, lo, hi, win, room, T, S, u.L - sa, false, 0, np);
       uint32_t left = 0;
-      if (open && wd_walk<false>(a, s_bin[warp], pos, lo, hi, win, open, left, 0) < open) continue;  // all or nothing
+      if (open && bf_walk<false>(a, s_bin[warp], target, pos, lo, hi, win, open, left, 0) < open) continue;  // all or nothing
       uint32_t r = 0;
       if (lane == 0) r = atomicAdd(&a.ctr[kWdLobbies], 1u);
       r = __shfl_sync(0xFFFFFFFFu, r, 0);
@@ -625,13 +626,13 @@ __global__ void __launch_bounds__(kPtPlanWarps * 32) k_pt_plan(const PtArgs p, c
       ++n_lob;
       for (uint32_t t = lane; t < T; t += 32) room[t] = (uint16_t)(t == 0 ? S - sa : S);
       __syncwarp();
-      pt_walk(p, a, ar, pos, lo, hi, win, room, T, S, u.L - sa, true, r, n_placed);
+      pt_walk(p, a, ar, target, pos, lo, hi, win, room, T, S, u.L - sa, true, r, n_placed);
       ++n_placed;
       for (uint32_t t = 0; t < T; ++t) {  // the solos fill the open slots team by team, in their rank order
         const uint32_t need = room[t];
         if (!need) continue;
         left = t * S + (S - need);
-        wd_walk<true, true>(a, s_bin[warp], pos, lo, hi, win, need, left, r);
+        bf_walk<true, true>(a, s_bin[warp], target, pos, lo, hi, win, need, left, r);
       }
       __syncwarp();
     }

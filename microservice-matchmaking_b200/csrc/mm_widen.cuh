@@ -11,9 +11,9 @@
 // partitions by age.  rem[bin] starts from tot and counts the bin's players no earlier lobby of the call took; lobbies
 // take the oldest untaken players of a bin, so the taken players of a bin are its rank prefix [0, tot - rem) and an
 // anchor whose rank lies in it is absorbed.  Otherwise the warp walks the bins outward from the anchor's own bin in
-// (distance, rating) order, as k_bf_plan does, inside the anchor's window: a first walk only counts, and only when it
-// reaches the lobby size L does a second walk take the players, one PIECE per (lobby, bin) with its offset inside the
-// lobby in member order (rating, then enqueue order).
+// (distance, rating) order inside the anchor's window (bf_walk, k_bf_plan's walk): a first walk only counts, and only
+// when it reaches the lobby size L does a second walk take the players, one PIECE per (lobby, bin) with its offset
+// inside the lobby in member order (rating, then enqueue order).
 //
 // Take and output: k_bf_keys turns the taken prefixes into keys and the band pipeline takes them into staging, as for
 // mm_backfill; k_wd_bases scans the per-queue lobby counts, k_wd_hdr writes the headers and every lobby's member base,
@@ -149,62 +149,6 @@ __global__ void __launch_bounds__(256) k_wd_rank(const WdArgs a) {
   if ((threadIdx.x & 31) == 0) a.a_rank[i] = r;
 }
 
-// The outward walk of k_bf_plan from bin pos of the queue [lo, hi) within distance win: the first `need` players in
-// (distance, rating, enqueue order).  Returns how many it found (at most need) and, in left, how many of them lie below
-// pos.  kTake: the players are taken (rem) and written as pieces of lobby record r, whose left players come first;
-// kWalkOrder (mm_party_match): the pieces are written in walk order instead, from offset `left` of the lobby.
-template <bool kTake, bool kWalkOrder = false>
-__device__ __forceinline__ uint32_t wd_walk(const WdArgs& a, uint32_t* s_bin, uint32_t pos, uint32_t lo, uint32_t hi,
-                                            uint32_t win, uint32_t need, uint32_t& left, uint32_t r) {
-  const uint32_t lane = threadIdx.x & 31;
-  const int32_t target = (int32_t)a.bin_key[pos];
-  const uint32_t nL = pos - lo, nR = hi - pos;
-  const uint32_t left_all = left;  // kTake: the players below pos that the lobby takes
-  uint32_t got = 0, used_l = 0, used_r = 0, got_l = 0, got_r = 0;
-  while (need) {
-    const uint32_t il = used_l + lane, ir = used_r + lane;
-    uint32_t dl = kBfFar, dr = kBfFar;
-    if (il < nL) {
-      const uint32_t d = (uint32_t)(target - (int32_t)a.bin_key[pos - 1 - il]);
-      dl = d <= win ? d : kBfFar;
-    }
-    if (ir < nR) { const uint32_t d = (uint32_t)((int32_t)a.bin_key[pos + ir] - target); dr = d <= win ? d : kBfFar; }
-    const uint32_t pl = lane + bf_rank(dr, dl, false), pr = lane + bf_rank(dl, dr, true);
-    const bool okl = dl != kBfFar && pl < 32, okr = dr != kBfFar && pr < 32;
-    if (okl) s_bin[pl] = pos - 1 - il;
-    if (okr) s_bin[pr] = pos + ir;
-    const uint32_t nl = __popc(__ballot_sync(0xFFFFFFFFu, okl)), nr = __popc(__ballot_sync(0xFFFFFFFFu, okr));
-    const uint32_t nv = nl + nr;
-    __syncwarp();
-    uint32_t bin = 0, v = 0;
-    if (lane < nv) { bin = s_bin[lane]; v = a.rem[bin]; }
-    const uint32_t incl = warp_incl_scan(v);
-    const uint32_t excl = incl - v, before = min(excl, need), take = min(v, need - before);
-    const bool is_l = lane < nv && bin < pos;
-    const uint32_t tl = is_l ? take : 0u, tr = is_l ? 0u : take;
-    const uint32_t il_incl = warp_incl_scan(tl), ir_incl = warp_incl_scan(tr);
-    if (kTake) {
-      const uint32_t at = warp_append(&a.ctr[kBfPieces], take != 0);
-      if (take) {
-        // member order: the left bins in ascending rating (reverse walk order), then the right bins in walk order
-        const uint32_t poff = kWalkOrder ? left_all + got + before
-                                         : (is_l ? left_all - (got_l + il_incl) : left_all + got_r + ir_incl - tr);
-        a.piece[at] = BfPiece{r, bin, a.tot[bin] - v, take, poff};
-        a.rem[bin] = v - take;
-      }
-    }
-    got_l += __shfl_sync(0xFFFFFFFFu, il_incl, 31);
-    got_r += __shfl_sync(0xFFFFFFFFu, ir_incl, 31);
-    const uint32_t took = min(__shfl_sync(0xFFFFFFFFu, incl, 31), need);
-    need -= took; got += took;
-    __syncwarp();  // rem and s_bin are read again by the next step
-    if (nv < 32) break;  // both runs (or the window) exhausted
-    used_l += nl; used_r += nr;
-  }
-  left = got_l;
-  return got;
-}
-
 __global__ void __launch_bounds__(kWdPlanWarps * 32) k_wd_plan(const WdArgs a) {
   __shared__ uint32_t s_bin[kWdPlanWarps][32];
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, c = blockIdx.x * kWdPlanWarps + warp;
@@ -234,13 +178,14 @@ __global__ void __launch_bounds__(kWdPlanWarps * 32) k_wd_plan(const WdArgs a) {
     const long long w = min((long long)u.w_max, (long long)u.w0 + (long long)((wait - u.min_wait) / u.step) * u.inc);
     const uint32_t win = (uint32_t)min(w, (long long)kBfFar - 1);
     uint32_t left = 0;
-    if (wd_walk<false>(a, s_bin[warp], v, lo, hi, win, u.L, left, 0) < u.L) continue;  // all or nothing
+    const int32_t target = (int32_t)a.bin_key[v];
+    if (bf_walk<false>(a, s_bin[warp], target, v, lo, hi, win, u.L, left, 0) < u.L) continue;  // all or nothing
     uint32_t r = 0;
     if (lane == 0) r = atomicAdd(&a.ctr[kWdLobbies], 1u);
     r = __shfl_sync(0xFFFFFFFFu, r, 0);
     if (lane == 0) a.rec[r] = make_uint2(c, n_lob);
     ++n_lob;
-    wd_walk<true>(a, s_bin[warp], v, lo, hi, win, u.L, left, r);
+    bf_walk<true>(a, s_bin[warp], target, v, lo, hi, win, u.L, left, r);
   }
   if (lane == 0) {
     a.qlob[c] = n_lob;

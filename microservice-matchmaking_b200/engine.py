@@ -449,6 +449,52 @@ class Engine:
                 return n_taken, []
             return n_taken, np.split(mem[:total.value], np.cumsum(n_taken.astype(np.int64))[:-1])
 
+    # -- party backfill (mm_backfill_party) ---------------------------------------------------------------------------
+    def backfill_party(self, mode, group, target, room, window=None):
+        """Fill the open team slots of running lobbies with whole queued parties of their queues, then with the nearest
+        solos (rating-order engines with party_capacity set).  mode, group, target and window are scalars or arrays of
+        the n requests' length (window None or < 0: no limit); room holds one list of open slots per team for each
+        request (one list for a single request given as scalars).  -> (filled, members): per request, the members each
+        team received and one u64 id array per team (its parties first, then its solos)."""
+        cols = np.broadcast_arrays(*(np.asarray(x, np.int64) for x in (mode, group, target,
+                                                                        -1 if window is None else window)))
+        n = cols[0].size
+        if n == 1 and len(room) and np.ndim(room[0]) == 0:
+            room = [room]
+        room = [np.asarray(r, np.int64).ravel() for r in room]
+        if len(room) != n:
+            raise ValueError(f"{len(room)} room lists for {n} requests")
+        for j, (m, r) in enumerate(zip(cols[0].ravel().tolist(), room)):  # the engine reads `teams` entries per request
+            if 0 <= m < self.cfg.n_modes and r.size != self.cfg.modes[m].teams:
+                raise ValueError(f"request {j}: {r.size} room entries for a mode of {self.cfg.modes[m].teams} teams")
+        req = np.zeros(n, np.dtype([("mode", "u1"), ("group", "u1"), ("reserved", "<u2"), ("count", "<u4"),
+                                    ("target", "<i4"), ("window", "<i4")]))
+        for name, col in zip(("mode", "group", "target", "window"), cols):
+            req[name] = col.ravel()
+        req["count"] = [int(r.sum()) for r in room]
+        flat = np.concatenate(room + [np.zeros(1, np.int64)]).astype(np.uint16)
+        filled = np.zeros(flat.size, np.uint16)
+        n_taken = np.zeros(max(n, 1), np.uint32)
+        cap = 1 << 12  # resized from the total of an MM_E_CAP refusal
+        while True:
+            mem = np.empty(cap, np.uint64)
+            total = C.c_uint32(0)
+            rc = self.lib.mm_backfill_party(self.h, n, _p(req), _p(flat), _p(filled), _p(n_taken), _p(mem), cap,
+                                            C.byref(total))
+            if rc == abi.MM_E_CAP and total.value > cap:
+                cap = total.value
+                continue
+            self._check(rc, "mm_backfill_party")
+            break
+        out_filled, out_members, e, m = [], [], 0, 0
+        for r in room:
+            f = filled[e:e + r.size].astype(np.int64)
+            out_filled.append(f.tolist())
+            out_members.append([mem[m + a:m + b].copy() for a, b in zip(np.cumsum(f) - f, np.cumsum(f))])
+            e += r.size
+            m += int(f.sum())
+        return out_filled, out_members
+
     # -- widening search (mm_widen) --------------------------------------------------------------------------------
     WIDEN_RULE_DTYPE = np.dtype([("min_wait", "<u4"), ("step", "<u4"), ("w0", "<i4"), ("inc", "<i4"),
                                  ("w_max", "<i4"), ("reserved", "<u4")])

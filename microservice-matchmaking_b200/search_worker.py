@@ -415,6 +415,44 @@ class SearchPool:
         self.stats["backfilled"] = self.stats.get("backfilled", 0) + sum(len(d) for d in out)
         return out
 
+    def backfill_teams(self, requests):
+        """Fill the open team slots of running lobbies with whole queued parties, then the nearest solos
+        (Engine.backfill_party; needs party_capacity): a lobby that lost a premade can take another party on one team.
+        requests: (game-mode name, group name, target rating, [open slots per team]) or (..., slots, window) tuples,
+        served in order.  -> per request, one list of player documents per team: the team's parties first, each party's
+        members together, then its solos (fewer than the open slots when the queue runs short: requeue() hands a short
+        fill back).  Taken players leave the pool as matched players do; a placed party is kept aside as party_match's
+        are, so requeue() with requeue_parties puts it back whole."""
+        self.flush()
+        if not requests:
+            return []
+        mode = [self.mode_index[r[0]] for r in requests]
+        group = [self.group_names.index(r[1]) for r in requests]
+        target = [int(r[2]) for r in requests]
+        room = [[int(x) for x in r[3]] for r in requests]
+        window = [-1 if len(r) < 5 or r[4] is None else int(r[4]) for r in requests]
+        _filled, members = self.engine.backfill_party(np.array(mode, np.int64), np.array(group, np.int64),
+                                                      np.array(target, np.int64), room, np.array(window, np.int64))
+        out = []
+        for teams in members:
+            docs = []
+            for ids in teams:
+                docs.append([self.players.pop(int(x)) for x in ids])
+                for x in ids.tolist():
+                    if x in self.party_of:  # a placed party's member: its record moves aside, as after party_match
+                        self.party_of.pop(x, None)
+                        rec = self.party_book.pop(x, None)
+                        if rec is not None:
+                            self.matched_parties[x] = rec
+                    if self.window:  # kept aside until remove_user: requeue() puts it back
+                        at = self.enqueued_at.pop(x, None)
+                        if at is not None:
+                            self.matched_at[x] = at
+            out.append(docs)
+        self.stats["backfilled_teams"] = self.stats.get("backfilled_teams", 0) + sum(
+            len(d) for teams in out for d in teams)
+        return out
+
     def search_status(self, player_ids):
         """Where each player's search stands (Engine.locate at now_ms()), without ingesting the staged deliveries.
         -> one dict per player id: "state" is "searching" (queued), "matched" (placed in a lobby, or taken by backfill,
