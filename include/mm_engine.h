@@ -359,7 +359,7 @@ typedef struct mm_widen_stats {
  * n_removed; they stay in the active set as matched players (mm_locate state 2, mm_requeue code 1, mm_remove forgets
  * them).  The last tick's results, the match section of mm_queue_stats, mm_match_quality, the lobby budget and its
  * report, the snapshot, the mm_enqueue_rejects list, pending async_results copies and the options are left alone;
- * widen lobbies are outside the tick's lobby budget, as mm_band_match's are.
+ * widen lobbies are outside the tick's lobby budget and inside mm_widen's own (mm_set_offtick_budget below).
  * Refusals, all decided before anything changes (mm_last_error names the cause):
  *   MM_E_ARG   a null e, rules or stats; on a queue that is not MM_WIDEN_OFF: step 0, w0 < 0, inc < 0, w_max < w0 or
  *              reserved != 0; an MM_ORDER_ARRIVAL engine (windows need rating order);
@@ -437,9 +437,10 @@ typedef struct mm_party_stats {
  * member whose partition holds a co-member requeued earlier (the seq of a live player there: MM_E_ARG); a member whose
  * rating maps to another partition is requeued.  Only R needs a group, so a member whose own rating has none cannot be
  * requeued (MM_E_ARG).  To put a whole party back at its age position, use mm_requeue_party.  team_balance does not
- * split party lobbies; the last tick's results, mm_match_quality, the lobby budget and pending async_results copies
- * are left alone.  With mm_set_option("party_balance") a lobby of a masked mode is split into its most even teams with
- * every party kept whole, so its teams no longer read "a team's parties, then its solos": EQUIVALENCE, the call leaves
+ * split party lobbies; the last tick's results, mm_match_quality, the tick's lobby budget and pending async_results
+ * copies are left alone (party lobbies are inside mm_party_match's own budget, mm_set_offtick_budget below).  With
+ * mm_set_option("party_balance") a lobby of a masked mode is split into its most even teams with every party kept
+ * whole, so its teams no longer read "a team's parties, then its solos": EQUIVALENCE, the call leaves
  * the engine exactly as the same call without the option would, and its member order is the party_balance rule
  * applied to that call's lobbies (each party's members stay contiguous and in enqueue order).
  * Refusals, all decided before anything changes (mm_last_error names the cause): MM_E_ARG the rule checks of mm_widen,
@@ -865,6 +866,50 @@ int mm_set_lobby_budget(mm_engine* e, const uint32_t* per_queue, const uint32_t*
 int mm_lobby_budget_report(mm_engine* e, uint32_t* candidates, uint32_t* emitted, uint32_t cap, uint32_t* n_out);
 int mm_lobby_candidates(mm_engine* e, uint32_t* candidates, uint32_t cap, uint32_t* n_out);
 
+/* ---- off-tick budget: how many lobbies mm_party_match and mm_widen may emit ------------------------------
+ * EXTENSION (flow control).  Party and widen lobbies need game servers as the tick's do, so each of the two calls has
+ * a lobby budget of its own, with the tick's rules: a step that runs party_match, the tick and widen can keep every
+ * lobby it publishes within the free servers of a mode, and a paused queue emits nothing from any of them.
+ *
+ * mm_set_offtick_budget: source MM_OFFTICK_PARTY_MATCH or MM_OFFTICK_WIDEN; per_queue / per_mode, their units,
+ * MM_BUDGET_UNLIMITED, NULL = all unlimited and "an array without a limit is no array" as in mm_set_lobby_budget.
+ * Takes effect from the next call of that source and stays until set again.  Each source's budget is separate from the
+ * other's and from the tick's.  Default: unlimited, and then every output of both calls is bit for bit what it is
+ * without this section, from the same kernels.
+ *
+ * DEFINITION.  Let c_q be the lobbies the call would emit from queue q with no budget (same `now`, same rules).  The
+ * allowance a_q follows the tick's DEFINITION: c'_q = min(c_q, per_queue[q]), then the per-mode largest remainder in
+ * 64-bit integers, ties to the lower group.  The call emits the FIRST a_q LOBBIES of every queue in its emission order —
+ * same members, same member order, same parties on the same teams — and everything else stays queued, as if the
+ * queue's plan had stopped after its a_q-th lobby.  This is exact because both calls serve each queue on its own and
+ * in order, so a lobby depends only on the lobbies of its queue formed before it.  Headers stay in (mode, group,
+ * emission) order, first_member renumbered.
+ * STATS: n_lobbies, n_matched, n_parties and sum_imbalance describe the emitted lobbies; n_anchors and n_absorbed are
+ * those of the unbudgeted call.  MM_E_CAP checks lobby_cap / member_cap against the emitted counts; zero capacities
+ * remain a dry run.
+ * WHAT FOLLOWS THE CUT: "team_balance", "party_balance" and mm_offtick_report see only the emitted lobbies.
+ * EQUIVALENCE.  A budgeted mm_widen leaves the engine as mm_take of the returned ids would.  A budgeted mm_party_match
+ * leaves it as mm_party_match's own construction would with only the emitted lobbies: mm_export_parties and
+ * mm_export, delete the placed parties and the taken solos, then import and mm_merge_parties(MM_PARTY_KEEP_SEQ).
+ *
+ * mm_offtick_budget_report: per queue, c_q (candidates) and a_q (emitted) of the last call of `source` that returned
+ * MM_OK or MM_E_CAP (an MM_E_CAP dry run gives c_q without changing anything, which a later cross-engine share of a
+ * mode budget needs; this is unlike mm_offtick_report, which is void after MM_E_CAP).  All zeros before the first such
+ * call, after a call that served no queue or found no anchor, and after any other refusal.  With no budget set,
+ * candidates equal emitted.  cap / n_out as in mm_queue_stats (MM_E_CAP and *n_out = n_modes * n_groups if cap is
+ * smaller).
+ * NOT IN THE IMAGE.  Budgets are options, as the tick's are: mm_export does not carry them, an imported engine starts
+ * unlimited, and mm_snapshot / mm_restore leave them alone.
+ * REFUSALS, decided before anything changes: mm_set_offtick_budget MM_E_ARG for a null e or an unknown source;
+ * mm_offtick_budget_report MM_E_ARG for a null e or n_out, null arrays with cap > 0 or an unknown source, MM_E_CAP
+ * as above, MM_E_STATE while an mm_enqueue_packed_begin batch is staged.
+ * COST: with a budget set, one single-CTA kernel after the call's plan and one read of a flag; when some a_q < c_q the
+ * plan runs again from its start, capped at a_q lobbies per queue (it stops serving a queue's anchors after its a_q-th
+ * lobby).  Without a budget nothing is launched or copied.                                                          */
+int mm_set_offtick_budget(mm_engine* e, uint32_t source, const uint32_t* per_queue, const uint32_t* per_mode);
+int mm_offtick_budget_report(mm_engine* e, uint32_t source, uint32_t* candidates, uint32_t* emitted, uint32_t cap,
+                             uint32_t* n_out);
+
 /* ---- search timeout ------------------------------------------------------------
  * EXTENSION (search timeout): every live queued player whose WAIT at `now` (the definition of mm_queue_stats)
  * is >= max_wait leaves the pool AND the active set, as if mm_remove had been called with its id: mm_in_queue
@@ -922,7 +967,7 @@ int mm_restore(mm_engine* e);
  * NOT IN THE IMAGE: dead slots (players removed, taken or expired while queued: the next tick would drop them); the
  * last batch's reject list (mm_enqueue_rejects is empty after import); the last tick's match section of
  * mm_queue_stats (void after import, as after mm_restore); the mm_snapshot state; the options (max_spread, tick_impl,
- * rank_impl, async_results, the lobby budget: the caller sets them again).
+ * rank_impl, async_results, the lobby budget and the off-tick budgets: the caller sets them again).
  *
  * EQUIVALENCE.  After mm_import, every sequence of calls gives the same results on the imported engine as on the
  * source: enqueue codes, remove / take / expire outputs, in_queue, active_size, pool_read, the ticks' lobbies,

@@ -848,6 +848,39 @@ static ERL_NIF_TERM nif_lobby_budget_report(ErlNifEnv* env, int argc, const ERL_
   enif_realloc_binary(&a, (size_t)n * 4);
   return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &c), enif_make_binary(env, &a));
 }
+/* set_offtick_budget(ref, source, per_queue, per_mode) -> :ok: the lobby budget of mm_party_match (source 0) or mm_widen
+ * (source 1) from its next call on (mm_set_offtick_budget); binaries as in set_lobby_budget.
+ * offtick_budget_report(ref, source) -> {:ok, candidates, emitted} (binary(u32[]) per queue) of the source's last call
+ * that returned MM_OK or was a dry run (mm_offtick_budget_report). */
+static ERL_NIF_TERM nif_set_offtick_budget(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; unsigned int source; ErlNifBinary pq, pm; uint32_t nq = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_uint(env, argv[1], &source) ||
+      !enif_inspect_binary(env, argv[2], &pq) || !enif_inspect_binary(env, argv[3], &pm))
+    return enif_make_badarg(env);
+  mm_lobby_candidates(r->e, NULL, 0, &nq);  /* cap 0: only the number of queues */
+  if ((pq.size && pq.size != (size_t)nq * 4) || pm.size % 4 || pm.size > 4 * MM_MAX_MODES || (pm.size && nq % (pm.size / 4)))
+    return enif_make_badarg(env);
+  uint32_t q[MM_MAX_GROUPS * MM_MAX_MODES], m[MM_MAX_MODES];
+  memcpy(q, pq.data, pq.size);
+  memcpy(m, pm.data, pm.size);
+  int rc = mm_set_offtick_budget(r->e, source, pq.size ? q : NULL, pm.size ? m : NULL);
+  return rc ? err(env, rc) : atom(env, "ok");
+}
+static ERL_NIF_TERM nif_offtick_budget_report(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; unsigned int source; ErlNifBinary c, a; uint32_t n = 0;
+  const uint32_t cap = MM_MAX_GROUPS * MM_MAX_MODES;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_uint(env, argv[1], &source))
+    return enif_make_badarg(env);
+  if (!enif_alloc_binary((size_t)cap * 4, &c)) return err(env, MM_E_CAP);
+  if (!enif_alloc_binary((size_t)cap * 4, &a)) { enif_release_binary(&c); return err(env, MM_E_CAP); }
+  int rc = mm_offtick_budget_report(r->e, source, (uint32_t*)c.data, (uint32_t*)a.data, cap, &n);
+  if (rc) { enif_release_binary(&c); enif_release_binary(&a); return err(env, rc); }
+  enif_realloc_binary(&c, (size_t)n * 4);
+  enif_realloc_binary(&a, (size_t)n * 4);
+  return enif_make_tuple3(env, atom(env, "ok"), enif_make_binary(env, &c), enif_make_binary(env, &a));
+}
 static ERL_NIF_TERM nif_lobby_candidates(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
   engine_res* r; ErlNifBinary c; uint32_t n = 0;
   const uint32_t cap = MM_MAX_GROUPS * MM_MAX_MODES;
@@ -943,5 +976,7 @@ static ErlNifFunc funcs[] = {
   {"set_lobby_budget", 3, nif_set_lobby_budget, 0},
   {"lobby_budget_report", 1, nif_lobby_budget_report, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"lobby_candidates", 1, nif_lobby_candidates, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"set_offtick_budget", 4, nif_set_offtick_budget, 0},
+  {"offtick_budget_report", 2, nif_offtick_budget_report, ERL_NIF_DIRTY_JOB_CPU_BOUND},
 };
 ERL_NIF_INIT(Elixir.Matchmaking.Search.Engine, funcs, load, NULL, NULL, NULL)

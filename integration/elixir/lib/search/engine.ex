@@ -214,6 +214,14 @@ defmodule Matchmaking.Search.Engine do
   def lobby_budget_report(_ref), do: :erlang.nif_error(:nif_not_loaded)
   @doc "-> {:ok, binary(u32[])}: the lobbies a tick without a budget would emit from every queue now; changes nothing."
   def lobby_candidates(_ref), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Extension (flow control, mm_set_offtick_budget): the lobby budget of party_match (source 0) or widen (source 1) from
+  its next call until set again; binaries as in set_lobby_budget.  Each source's budget is its own, apart from the
+  tick's.  The call emits every queue's first lobbies, as if the queue's plan had stopped there.
+  """
+  def set_offtick_budget(_ref, _source, _per_queue, _per_mode), do: :erlang.nif_error(:nif_not_loaded)
+  @doc "-> {:ok, candidates, emitted} (binary(u32[]) per queue) of the source's last call (or dry run)."
+  def offtick_budget_report(_ref, _source), do: :erlang.nif_error(:nif_not_loaded)
 
   @doc "Extension (not reference behaviour): maximum rating spread of a lobby for the following ticks; < 0 = off."
   def set_max_spread(_ref, _w), do: :erlang.nif_error(:nif_not_loaded)

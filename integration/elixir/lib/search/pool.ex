@@ -50,6 +50,10 @@ defmodule Matchmaking.Search.Pool do
                      most that many lobbies of the mode, shared over the rating groups in proportion to what each could
                      emit (Engine.set_lobby_budget); the rest stay queued in order.  pause/1, resume_queues/1 stop and
                      restart the queues of rating groups; a checkpoint carries neither
+      budget_offtick option (extension, default false): with lobby_budget, one tick's budget covers every lobby it
+                     publishes (Engine.set_offtick_budget): party_match runs under the callback's per-mode budget F,
+                     the tick under F minus its party lobbies per mode, widen under what is left; paused groups emit
+                     nothing from any of the three
       checkpoint/0   hand-over: flushes the staged deliveries (so every acked player is in it), then returns
                      :erlang.term_to_binary of the engine image (Engine.export_image), the handle table, the player
                      documents, the pool clock and the wall time.  resume: <checkpoint> as an option of start_link/1
@@ -162,6 +166,7 @@ defmodule Matchmaking.Search.Pool do
            queued: %{}, moved_out: MapSet.new(),
            t0: System.monotonic_time(:millisecond), timeout: Keyword.get(opts, :search_timeout_ms),
            lobby_budget: Keyword.get(opts, :lobby_budget), paused: MapSet.new(), regroup_dropped: [],
+           budget_offtick: Keyword.get(opts, :budget_offtick, false), step_budget: nil,
            widen: Keyword.get(opts, :widen), parties: Keyword.get(opts, :parties), staged_parties: [], party_of: %{},
            party_capacity: Keyword.get(opts, :party_capacity), stranded_parties: [],
            # requeue_parties: handle -> {members, ratings, mode, enq_ts, seq} of its queued (party_book) or matched party
@@ -783,24 +788,54 @@ defmodule Matchmaking.Search.Pool do
     for player <- st.regroup_dropped, do: send_timeout(st.channel, player)   # resume with regroup: true
     st = flush(%{st | regroup_dropped: []})
     now = now_ms(st)
-    if st.lobby_budget, do: set_budget(st, st.lobby_budget.())
+    # budget_offtick: the step's budgets, less what the step has published so far (step_budget)
+    st = %{st | step_budget: nil}
+    st =
+      cond do
+        st.lobby_budget == nil -> st
+        st.budget_offtick -> %{st | step_budget: budget_binaries(st, st.lobby_budget.())}
+        true ->
+          set_budget(st, st.lobby_budget.())
+          st
+      end
     st = party_match(st, now)   # before the tick: parties get the first pick of the solos
+    if st.step_budget, do: :ok = Engine.set_lobby_budget(st.ref, elem(st.step_budget, 0), elem(st.step_budget, 1))
     case Engine.tick_packed(st.ref, now) do
-      {:ok, lobbies, members, _stats} -> {:noreply, expire(widen(publish(lobbies, members, st), now), now)}
+      {:ok, lobbies, members, _stats} ->
+        {:noreply, expire(widen(publish(lobbies, members, spend(st, lobbies)), now), now)}
       {:error, _reason} -> {:noreply, st}                              # nothing was consumed; the next tick retries
     end
   end
 
   # -- lobby budget (extension): per-mode budgets from the callback, paused groups as per-queue budget 0 --------------
   @unlimited 0xFFFFFFFF
-  defp set_budget(st, per_mode) do
+  defp budget_binaries(st, per_mode) do
     n_groups = Engine.n_groups()
     per_queue = for _m <- 0..(Engine.n_modes() - 1), g <- 0..(n_groups - 1), into: <<>>,
                     do: <<(if MapSet.member?(st.paused, g), do: 0, else: @unlimited)::little-32>>
     modes = if per_mode == nil, do: <<>>, else:
       (for m <- 0..(Engine.n_modes() - 1), into: <<>>,
            do: <<min(max(Map.get(per_mode, Engine.mode_name(m), @unlimited), 0), @unlimited)::little-32>>)
+    {per_queue, modes}
+  end
+
+  defp set_budget(st, per_mode) do
+    {per_queue, modes} = budget_binaries(st, per_mode)
     :ok = Engine.set_lobby_budget(st.ref, per_queue, modes)
+    if st.budget_offtick do   # the off-tick calls the pool runs, under the same budgets
+      if st.parties, do: :ok = Engine.set_offtick_budget(st.ref, 0, per_queue, modes)
+      if st.widen, do: :ok = Engine.set_offtick_budget(st.ref, 1, per_queue, modes)
+    end
+  end
+
+  # budget_offtick: the step's per-mode budgets less the lobbies (mm_lobby_hdr binaries) just published
+  defp spend(%{step_budget: nil} = st, _lobbies), do: st
+  defp spend(%{step_budget: {_q, <<>>}} = st, _lobbies), do: st
+  defp spend(%{step_budget: {per_queue, modes}} = st, lobbies) do
+    used = Enum.frequencies(for <<_first::little-32, _n::little-16, m::8, _g::8 <- lobbies>>, do: m)
+    left = for {b, m} <- Enum.with_index(for <<b::little-32 <- modes>>, do: b), into: <<>>,
+               do: <<(if b == @unlimited, do: b, else: max(b - Map.get(used, m, 0), 0))::little-32>>
+    %{st | step_budget: {per_queue, left}}
   end
 
   def handle_call({:pause, groups, on}, _from, st) do
@@ -821,6 +856,7 @@ defmodule Matchmaking.Search.Pool do
         nil -> <<0xFFFFFFFF::little-32, 1::little-32, 0::32, 0::32, 0::32, 0::32>>
       end
     end
+    if st.step_budget, do: :ok = Engine.set_offtick_budget(st.ref, 1, elem(st.step_budget, 0), elem(st.step_budget, 1))
     case Engine.widen(st.ref, now, rules) do
       {:ok, lobbies, members} -> publish(lobbies, members, st)
       {:error, _reason} -> st                                          # nothing was taken
@@ -838,9 +874,10 @@ defmodule Matchmaking.Search.Pool do
         nil -> <<0xFFFFFFFF::little-32, 1::little-32, 0::32, 0::32, 0::32, 0::32>>
       end
     end
+    if st.step_budget, do: :ok = Engine.set_offtick_budget(st.ref, 0, elem(st.step_budget, 0), elem(st.step_budget, 1))
     case Engine.party_match(st.ref, now, rules) do
       {:ok, lobbies, members} ->
-        st = publish(lobbies, members, st)
+        st = publish(lobbies, members, spend(st, lobbies))
         placed = for <<h::little-32 <- members>>, do: h
         # requeue_parties: a placed party's book entry moves aside, so requeue/1 can put the party back whole
         matched = for h <- placed, rec = Map.get(st.party_book, h), rec != nil, into: st.matched_parties, do: {h, rec}

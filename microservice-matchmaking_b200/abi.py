@@ -209,7 +209,7 @@ class QueueQuality(C.Structure):
     ]
 
 
-MM_OFFTICK_PARTY_MATCH = 0  # mm_offtick_report sources
+MM_OFFTICK_PARTY_MATCH = 0  # mm_offtick_report / mm_set_offtick_budget sources
 MM_OFFTICK_WIDEN = 1
 
 
@@ -335,6 +335,8 @@ PROTOTYPES = {
     "mm_set_lobby_budget": (C.c_int, [_vp, _vp, _vp]),
     "mm_lobby_budget_report": (C.c_int, [_vp, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_lobby_candidates": (C.c_int, [_vp, _vp, C.c_uint32, _P(C.c_uint32)]),
+    "mm_set_offtick_budget": (C.c_int, [_vp, C.c_uint32, _vp, _vp]),
+    "mm_offtick_budget_report": (C.c_int, [_vp, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_expire": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_expire_packed": (C.c_int, [_vp, C.c_uint64, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_export": (C.c_int, [_vp, _vp, C.c_uint64, _P(C.c_uint64)]),

@@ -298,7 +298,7 @@ struct mm_engine {
   // mm_widen (mm_widen.cuh): the call's tables and the anchors, grown on demand; the plan's rem, the keys, the pieces,
   // the staging and the members are the backfill arrays above
   struct Widen {
-    DevArray<uint32_t> tab;  // rules [n_cut] | qlob | qlbase | qmbase [n_cut] | part [n_segs + 1] | cur [n_segs] | cta
+    DevArray<uint32_t> tab;  // rules [n_cut] | qlbase | qmbase [n_cut] | part [n_segs + 1] | cur [n_segs] | cta
                              // [grid] | rmap [n_chunks] | ctr [kWdWords]
     DevArray<uint32_t> anc;  // rec (2 words) | slot | age | rank | mbase, each [anchors]
     DevArray<mm_lobby_hdr> hdr;
@@ -347,6 +347,17 @@ struct mm_engine {
       DevArray<mm_match_waits> waits;
     } rep[2];
   } ot;
+
+  // off-tick budget (mm_set_offtick_budget), per source: the budgets (an empty host vector = no limit anywhere; options,
+  // not part of images or snapshots) and the per-queue words of the source's last call, which only that source's calls
+  // write and mm_offtick_budget_report reads
+  struct OffBudget {
+    std::vector<uint32_t> queue, mode;  // [n_cut], [n_modes]
+    DevArray<uint32_t> tab;  // qlob (the plan's lobbies, emitted) | cand | allot [n_cut] | budgets [n_cut + n_modes] | cut
+    bool ran = false;        // the last call ran its plan (set by the call, cleared before it)
+    bool budgeted = false;   // ... under a budget: cand holds c_q
+    bool valid = false;      // ... and returned MM_OK or MM_E_CAP: the report reads tab
+  } ob[2];
 
   // parties (mm_party.cuh): the table in two buffers (compaction moves it from one to the other), sized by
   // party_capacity; the batch and match scratch grown on demand.  Not part of images or snapshots.
@@ -2679,6 +2690,38 @@ int ot_capture(mm_engine* e, uint32_t src, const WdArgs& w, uint32_t nl, uint32_
   return MM_OK;
 }
 
+// ---- the off-tick budget (mm_set_offtick_budget; k_wd_allot in mm_widen.cuh) ---------------------------------------
+// Before the plan of source `src`: its lobby counts go to the source's own words, where mm_offtick_budget_report finds
+// them.
+int ob_begin(mm_engine* e, uint32_t src, WdArgs& a) {
+  auto& o = e->ob[src];
+  CK(o.tab.reserve(4 * (size_t)e->n_cut + e->cfg.n_modes + 1));
+  a.qlob = o.tab;
+  a.cap = nullptr;
+  o.ran = true;
+  o.budgeted = !o.queue.empty() || !o.mode.empty();
+  return MM_OK;
+}
+
+// After the unbudgeted plan of a budgeted call: the allowances; when one is short of its queue's lobbies, a.cap points
+// at them and the caller runs the plan again from its reset state.  Synchronizes the stream (the caller's copies of
+// the first plan's counters land with it).
+int ob_allot(mm_engine* e, uint32_t src, WdArgs& a) {
+  auto& o = e->ob[src];
+  const uint32_t nc = e->n_cut;
+  uint32_t *cand = o.tab + nc, *allot = cand + nc, *bud = allot + nc, *cut = bud + nc + e->cfg.n_modes;
+  if (!o.queue.empty()) CK(cudaMemcpyAsync(bud, o.queue.data(), nc * 4, cudaMemcpyHostToDevice, e->stream));
+  if (!o.mode.empty()) CK(cudaMemcpyAsync(bud + nc, o.mode.data(), o.mode.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  k_wd_allot<<<1, kScanBlock, 0, e->stream>>>(a, o.queue.empty() ? nullptr : bud, o.mode.empty() ? nullptr : bud + nc,
+                                              cand, allot, cut);
+  CK(cudaGetLastError());
+  uint32_t h = 0;
+  CK(cudaMemcpyAsync(&h, cut, 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  a.cap = h ? allot : nullptr;
+  return MM_OK;
+}
+
 // ---- mm_widen (mm_widen.cuh) ---------------------------------------------------------------------------------------
 // The rules of mm_widen / mm_party_match as the device reads them, and the refusals both share.  any: a queue is served.
 int wd_rules(mm_engine* e, const mm_widen_rule* rules, std::vector<WdRule>& rule, bool& any) {
@@ -2714,9 +2757,8 @@ int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* 
   auto& b = e->bf;
   CK(cudaEventRecord(e->ev[0], e->stream));
   const uint32_t ctas = tile_ctas(e, p.n), rw = sizeof(WdRule) / 4;
-  const size_t o_qlob = rw * nc, o_qlb = o_qlob + nc, o_qmb = o_qlb + nc, o_part = o_qmb + nc,
-               o_cur = o_part + e->n_segs + 1, o_cta = o_cur + e->n_segs, o_rmap = o_cta + ctas,
-               o_ctr = o_rmap + e->n_chunks;
+  const size_t o_qlb = rw * nc, o_qmb = o_qlb + nc, o_part = o_qmb + nc, o_cur = o_part + e->n_segs + 1,
+               o_cta = o_cur + e->n_segs, o_rmap = o_cta + ctas, o_ctr = o_rmap + e->n_chunks;
   CK(s.tab.reserve(o_ctr + kWdWords));
   uint32_t* t = s.tab;
   CK(cudaMemcpyAsync(t, rule.data(), nc * sizeof(WdRule), cudaMemcpyHostToDevice, e->stream));
@@ -2728,7 +2770,7 @@ int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* 
   a.seq_next = e->seq_next; a.rule = reinterpret_cast<const WdRule*>(t); a.part_cut = e->d_part_cut;
   a.cut_lp_lo = e->d_cut_lp_lo; a.seg_bin_lo = e->d_seg_bin_lo; a.bin_seg = e->d_bin_seg; a.bin_key = e->d_bin_key;
   a.tot = p.m.tot; a.rmap = t + o_rmap; a.cta = t + o_cta; a.part = t + o_part; a.cur = t + o_cur;
-  a.qlob = t + o_qlob; a.qlbase = t + o_qlb; a.qmbase = t + o_qmb; a.ctr = t + o_ctr;
+  a.qlbase = t + o_qlb; a.qmbase = t + o_qmb; a.ctr = t + o_ctr;
   // anchors: counted, then written in (partition, age) order
   k_wd_anchors<kWdBlock><<<ctas, kWdBlock, 0, e->stream>>>(a, 0);
   k_wd_part_scan<<<1, 1024, 0, e->stream>>>(a);
@@ -2751,7 +2793,20 @@ int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* 
   k_loc_rmap<<<e->n_segs, 256, 0, e->stream>>>(p.m, t + o_rmap);
   k_wd_rank<<<(uint32_t)(((size_t)na * 32 + 255) / 256), 256, 0, e->stream>>>(a);
   // plan on the per-bin totals, then the bins with a take as keys
-  k_wd_plan<<<(nc + kWdPlanWarps - 1) / kWdPlanWarps, kWdPlanWarps * 32, 0, e->stream>>>(a);
+  if (int rc = ob_begin(e, MM_OFFTICK_WIDEN, a)) return rc;
+  const uint32_t plan_grid = (nc + kWdPlanWarps - 1) / kWdPlanWarps;
+  k_wd_plan<<<plan_grid, kWdPlanWarps * 32, 0, e->stream>>>(a);
+  uint32_t absorbed = 0;  // the unbudgeted plan's
+  if (e->ob[MM_OFFTICK_WIDEN].budgeted) {
+    CK(cudaMemcpyAsync(&absorbed, a.ctr + kWdAbsorbed, 4, cudaMemcpyDeviceToHost, e->stream));
+    if (int rc = ob_allot(e, MM_OFFTICK_WIDEN, a)) return rc;
+    if (a.cap) {  // again, capped, from the state the first plan started from
+      CK(cudaMemcpyAsync(b.rem, p.m.tot, K * 4, cudaMemcpyDeviceToDevice, e->stream));
+      CK(cudaMemcpyAsync(a.cur, a.part, (size_t)e->n_segs * 4, cudaMemcpyDeviceToDevice, e->stream));
+      CK(cudaMemsetAsync(a.ctr, 0, kWdWords * 4, e->stream));
+      k_wd_plan<<<plan_grid, kWdPlanWarps * 32, 0, e->stream>>>(a);
+    }
+  }
   BfArgs f{};
   f.tot = p.m.tot; f.rem = b.rem; f.bin_seg = e->d_bin_seg; f.fill = p.m.fill; f.K = e->K;
   f.key_bin = b.key_bin; f.kbase = b.kbase; f.klim = b.klim; f.ctr = a.ctr;
@@ -2762,7 +2817,8 @@ int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* 
   CK(cudaMemcpyAsync(h, a.ctr, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   const uint32_t nl = h[kWdLobbies], nm = h[kBfPlayers];
-  st->n_lobbies = nl; st->n_matched = nm; st->n_absorbed = h[kWdAbsorbed];
+  st->n_lobbies = nl; st->n_matched = nm;
+  st->n_absorbed = e->ob[MM_OFFTICK_WIDEN].budgeted ? absorbed : h[kWdAbsorbed];
   if (lobby_cap < nl || member_cap < nm)
     return set_err(e, MM_E_CAP, "need lobby_cap >= %u and member_cap >= %u", nl, nm);
   if (nl == 0) return MM_OK;
@@ -3310,7 +3366,7 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
   auto& w = e->wd;
   auto& b = e->bf;
   const uint32_t rw = sizeof(WdRule) / 4;
-  const size_t o_qlob = rw * nc, o_qlb = o_qlob + nc, o_qmb = o_qlb + nc, o_ctr = o_qmb + nc;
+  const size_t o_qlb = rw * nc, o_qmb = o_qlb + nc, o_ctr = o_qmb + nc;
   CK(w.tab.reserve(o_ctr + kWdWords));
   CK(w.anc.reserve((size_t)nr * 3));
   uint32_t maxT = 1;
@@ -3320,7 +3376,6 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
   CK(b.piece.reserve(n_pieces));
   uint32_t* t = w.tab;
   CK(cudaMemcpyAsync(t, rule.data(), nc * sizeof(WdRule), cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemsetAsync(t + o_qlob, 0, nc * 4, e->stream));
   CK(cudaMemsetAsync(t + o_ctr, 0, kWdWords * 4, e->stream));
   CK(cudaMemcpyAsync(b.rem, p.m.tot, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
   WdArgs a{};
@@ -3328,9 +3383,27 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
   a.seq_next = e->seq_next; a.rule = reinterpret_cast<const WdRule*>(t); a.part_cut = e->d_part_cut;
   a.cut_lp_lo = e->d_cut_lp_lo; a.seg_bin_lo = e->d_seg_bin_lo; a.bin_seg = e->d_bin_seg; a.bin_key = e->d_bin_key;
   a.tot = p.m.tot; a.rem = b.rem; a.piece = b.piece;
-  a.qlob = t + o_qlob; a.qlbase = t + o_qlb; a.qmbase = t + o_qmb; a.ctr = t + o_ctr;
+  a.qlbase = t + o_qlb; a.qmbase = t + o_qmb; a.ctr = t + o_ctr;
   a.rec = reinterpret_cast<uint2*>(w.anc.p); a.mbase = w.anc + 2 * (size_t)nr;
-  k_pt_plan<<<(nc + kPtPlanWarps - 1) / kPtPlanWarps, kPtPlanWarps * 32, 0, e->stream>>>(x, a);
+  if ((rc = ob_begin(e, MM_OFFTICK_PARTY_MATCH, a))) return rc;
+  CK(cudaMemsetAsync(a.qlob, 0, nc * 4, e->stream));
+  const uint32_t plan_grid = (nc + kPtPlanWarps - 1) / kPtPlanWarps;
+  k_pt_plan<<<plan_grid, kPtPlanWarps * 32, 0, e->stream>>>(x, a);
+  uint32_t first[2] = {0u, 0u};  // the unbudgeted plan's anchors and absorbed anchors
+  const bool budgeted = e->ob[MM_OFFTICK_PARTY_MATCH].budgeted;
+  if (budgeted) {
+    CK(cudaMemcpyAsync(first, s.ctr + kPtAnchors, 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(first + 1, a.ctr + kWdAbsorbed, 4, cudaMemcpyDeviceToHost, e->stream));
+    if ((rc = ob_allot(e, MM_OFFTICK_PARTY_MATCH, a))) return rc;
+    if (a.cap) {  // again, capped, from the state the first plan started from
+      CK(cudaMemsetAsync(s.lob, 0xFF, (size_t)nr * 4, e->stream));  // kPtNone: no row placed
+      CK(cudaMemcpyAsync(s.pcur, s.pb, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
+      CK(cudaMemcpyAsync(b.rem, p.m.tot, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
+      CK(cudaMemsetAsync(a.ctr, 0, kWdWords * 4, e->stream));
+      CK(cudaMemsetAsync(s.ctr + kPtAnchors, 0, 2 * 4, e->stream));  // kPtAnchors, kPtPlaced
+      k_pt_plan<<<plan_grid, kPtPlanWarps * 32, 0, e->stream>>>(x, a);
+    }
+  }
   BfArgs f{};
   f.tot = p.m.tot; f.rem = b.rem; f.bin_seg = e->d_bin_seg; f.fill = p.m.fill; f.K = K;
   f.key_bin = b.key_bin; f.kbase = b.kbase; f.klim = b.klim; f.ctr = a.ctr;
@@ -3348,8 +3421,8 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
   for (uint32_t q = 0; q < nc; ++q)
     if (rule[q].min_wait != MM_WIDEN_OFF) nm += (uint64_t)qlob[q] * rule[q].L;
   const uint32_t nl = h[kWdLobbies], ns = h[kBfPlayers];
-  st->n_anchors = hp[kPtAnchors]; st->n_lobbies = nl; st->n_matched = (uint32_t)nm; st->n_parties = hp[kPtPlaced];
-  st->n_absorbed = h[kWdAbsorbed];
+  st->n_anchors = budgeted ? first[0] : hp[kPtAnchors]; st->n_lobbies = nl; st->n_matched = (uint32_t)nm;
+  st->n_parties = hp[kPtPlaced]; st->n_absorbed = budgeted ? first[1] : h[kWdAbsorbed];
   float ms = 0.f;
   CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]));
   st->device_us = ms * 1000.f;  // a refused or empty call reports the table, sort and plan it ran
@@ -3960,6 +4033,8 @@ int mm_widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hd
   auto& rep = e->ot.rep[MM_OFFTICK_WIDEN];  // void until this call returns MM_OK; its capture sets the lobby count
   rep.valid = false;
   rep.n_lob = 0;
+  auto& ob = e->ob[MM_OFFTICK_WIDEN];  // zeros until a call that ran its plan returns MM_OK or MM_E_CAP
+  ob.valid = ob.ran = false;
   if (!rules || !stats) return set_err(e, MM_E_ARG, "null rules or stats");
   std::memset(stats, 0, sizeof(*stats));
   if ((lobby_cap && !lobbies) || (member_cap && !member_ids))
@@ -3967,6 +4042,7 @@ int mm_widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hd
   CK(cudaSetDevice(e->device));
   const int rc = widen(e, now, rules, lobbies, lobby_cap, member_ids, member_cap, stats);
   rep.valid = rc == MM_OK;
+  ob.valid = ob.ran && (rc == MM_OK || rc == MM_E_CAP);
   return rc;
 }
 
@@ -4000,6 +4076,8 @@ int mm_party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lo
   auto& rep = e->ot.rep[MM_OFFTICK_PARTY_MATCH];  // void until this call returns MM_OK; its capture sets the lobby count
   rep.valid = false;
   rep.n_lob = 0;
+  auto& ob = e->ob[MM_OFFTICK_PARTY_MATCH];  // zeros until a call that ran its plan returns MM_OK or MM_E_CAP
+  ob.valid = ob.ran = false;
   if (!rules || !stats) return set_err(e, MM_E_ARG, "null rules or stats");
   std::memset(stats, 0, sizeof(*stats));
   if ((lobby_cap && !lobbies) || (member_cap && !member_ids))
@@ -4007,6 +4085,7 @@ int mm_party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lo
   CK(cudaSetDevice(e->device));
   const int rc = party_match(e, now, rules, lobbies, lobby_cap, member_ids, member_cap, stats);
   rep.valid = rc == MM_OK;
+  ob.valid = ob.ran && (rc == MM_OK || rc == MM_E_CAP);
   return rc;
 }
 
@@ -4312,6 +4391,41 @@ int mm_lobby_budget_report(mm_engine* e, uint32_t* candidates, uint32_t* emitted
   CK(cudaStreamSynchronize(e->stream));
   for (uint32_t s = 0; s < e->n_segs; ++s) emitted[e->h_part_cut[s]] += seg[s].n_lobbies;
   if (!e->report_budgeted) std::copy(emitted, emitted + n_cut, candidates);
+  return MM_OK;
+}
+
+int mm_set_offtick_budget(mm_engine* e, uint32_t source, const uint32_t* per_queue, const uint32_t* per_mode) {
+  if (!e) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (source > MM_OFFTICK_WIDEN) return set_err(e, MM_E_ARG, "unknown source %u", source);
+  // as mm_set_lobby_budget: an array without a limit in it is "no array", and the call then runs unbudgeted
+  auto keep = [](std::vector<uint32_t>& v, const uint32_t* src, uint32_t n) {
+    v.clear();
+    if (src && std::any_of(src, src + n, [](uint32_t b) { return b != MM_BUDGET_UNLIMITED; })) v.assign(src, src + n);
+  };
+  keep(e->ob[source].queue, per_queue, e->n_cut);
+  keep(e->ob[source].mode, per_mode, e->cfg.n_modes);
+  return MM_OK;
+}
+
+int mm_offtick_budget_report(mm_engine* e, uint32_t source, uint32_t* candidates, uint32_t* emitted, uint32_t cap,
+                             uint32_t* n_out) {
+  if (!e || !n_out || (cap && (!candidates || !emitted))) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (source > MM_OFFTICK_WIDEN) return set_err(e, MM_E_ARG, "unknown source %u", source);
+  const uint32_t n_cut = e->n_cut;
+  *n_out = n_cut;
+  if (cap < n_cut) return set_err(e, MM_E_CAP, "need cap >= %u", n_cut);
+  if (e->stage_count) return staged_err(e);
+  std::fill(candidates, candidates + n_cut, 0u);
+  std::fill(emitted, emitted + n_cut, 0u);
+  const auto& o = e->ob[source];
+  if (!o.valid) return MM_OK;
+  CK(cudaSetDevice(e->device));
+  CK(cudaMemcpyAsync(emitted, o.tab, (size_t)n_cut * 4, cudaMemcpyDeviceToHost, e->stream));
+  if (o.budgeted) CK(cudaMemcpyAsync(candidates, o.tab + n_cut, (size_t)n_cut * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  if (!o.budgeted) std::copy(emitted, emitted + n_cut, candidates);
   return MM_OK;
 }
 

@@ -598,13 +598,15 @@ __global__ void __launch_bounds__(kPtPlanWarps * 32) k_pt_plan(const PtArgs p, c
   const uint32_t lo = a.seg_bin_lo[a.cut_lp_lo[c]], hi = a.seg_bin_lo[a.cut_lp_lo[c + 1]];
   const uint32_t S = p.mode_tsize[c / a.n_groups], T = u.L / S;  // the host refuses T > kPtMaxTeams
   uint16_t* room = s_room[warp];
+  const uint32_t cap = a.cap ? a.cap[c] : 0xFFFFFFFFu;  // a capped queue stops after its cap-th lobby
   uint32_t n_lob = 0, n_anc = 0, n_abs = 0, n_placed = 0;
   if (p.pb[hi] == p.pb[lo]) { if (lane == 0) a.qlob[c] = 0; return; }
-  for (uint32_t r0 = 0; r0 < p.n_rows; r0 += 32) {  // the anchors: the queue's parties that waited long enough, by age
+  // the anchors: the queue's parties that waited long enough, by age
+  for (uint32_t r0 = 0; r0 < p.n_rows && n_lob < cap; r0 += 32) {
     const uint32_t x = r0 + lane;
     const bool is_a = x < p.n_rows && p.t.bin[x] >= lo && p.t.bin[x] < hi && stat_wait(a.now, p.t.ts[x]) >= u.min_wait;
     uint32_t bal = __ballot_sync(0xFFFFFFFFu, is_a);
-    while (bal) {
+    while (bal && n_lob < cap) {
       const uint32_t ar = r0 + __ffs(bal) - 1;
       bal &= bal - 1;
       ++n_anc;

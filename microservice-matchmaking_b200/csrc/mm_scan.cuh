@@ -153,12 +153,53 @@ __device__ __forceinline__ void tail_count_lobbies(const uint32_t* scratch, cons
   }
 }
 
+// The allowances of mode m's queues q = m * G + g, one warp (<= 64 groups: two per lane, remainder ranks by
+// comparison): s_c[q] lobbies the queue has -> s_al[q] lobbies it may emit.  c' = min(c, bud_queue[q]); if the mode's
+// sum C of c' exceeds its budget B, B is apportioned by largest remainder: floor(B c' / C) each, and the B - sum groups
+// with the largest (B c') mod C get one more, ties to the lower group.  Restated on the host by shard.apportion.  The
+// tick's tail and the off-tick calls' k_wd_allot both apportion with it.
+__device__ __forceinline__ void budget_apportion(const uint32_t* s_c, uint32_t* s_al, uint32_t m, uint32_t G,
+                                                 const uint32_t* bud_queue, const uint32_t* bud_mode) {
+  const uint32_t lane = threadIdx.x & 31;
+  uint32_t c[2], al[2], C = 0;
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const uint32_t g = lane + 32 * j;
+    c[j] = g < G ? s_c[m * G + g] : 0u;
+    if (g < G && bud_queue) { const uint32_t b = bud_queue[m * G + g]; c[j] = c[j] < b ? c[j] : b; }
+    al[j] = c[j];
+    C += c[j];
+  }
+  C = __reduce_add_sync(0xFFFFFFFFu, C);  // < 2^31: every lobby has a player of its own
+  const uint32_t B = bud_mode ? bud_mode[m] : 0xFFFFFFFFu;
+  if (C > B) {  // (uniform over the warp)
+    uint32_t rem[2], fl = 0;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const uint64_t p = (uint64_t)B * c[j];
+      al[j] = (uint32_t)(p / C); rem[j] = (uint32_t)(p % C);
+      fl += al[j];
+    }
+    const uint32_t extra = B - __reduce_add_sync(0xFFFFFFFFu, fl);  // fewer than the groups with a remainder
+    uint32_t rank[2] = {0u, 0u};  // groups that come before this one by (remainder descending, group ascending)
+    for (int l = 0; l < 32; ++l)
+#pragma unroll
+      for (int k = 0; k < 2; ++k) {
+        const uint32_t r = __shfl_sync(0xFFFFFFFFu, rem[k], l), g2 = l + 32 * k;
+#pragma unroll
+        for (int j = 0; j < 2; ++j) rank[j] += (r > rem[j] || (r == rem[j] && g2 < lane + 32 * j)) ? 1u : 0u;
+      }
+#pragma unroll
+    for (int j = 0; j < 2; ++j) al[j] += rank[j] < extra ? 1u : 0u;
+  }
+#pragma unroll
+  for (int j = 0; j < 2; ++j)
+    if (lane + 32 * j < G) s_al[m * G + lane + 32 * j] = al[j];
+}
+
 // Lobby budget, the whole block, called with the tail's tables and (S1) matched counts in place:
 //   s_c[q]  = lobbies queue q = m * G + g would emit (also written to cand[q])
-//   s_al[q] = lobbies it may emit.  c' = min(c, bud_queue[q]); if the mode's sum C of c' exceeds its budget B, B is
-//             apportioned by largest remainder: floor(B c' / C) each, and the B - sum groups with the largest
-//             (B c') mod C get one more, ties to the lower group.  One warp per mode (<= 64 groups: two per lane,
-//             remainder ranks by comparison).  Restated on the host by shard.apportion.
+//   s_al[q] = lobbies it may emit (budget_apportion, one warp per mode)
 //   S0 clip: the queue's matched end moves to its (a_q L)-th sorted position: the partitions' matched counts s_mt,
 //             which the caller has filled for the unbudgeted cut, are written again.
 //   S1 clip: one warp per queue, bin v keeps the matched players that come before the queue's (a_q L)-th matched
@@ -173,43 +214,7 @@ __device__ __noinline__ void tail_budget(uint32_t* scratch, uint32_t* s_m, uint3
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   tail_count_lobbies(scratch, s_m, n_cut, windowed, s_c);
   __syncthreads();
-  if (warp < n_cut / G) {
-    const uint32_t m = warp;
-    uint32_t c[2], al[2], C = 0;
-#pragma unroll
-    for (int j = 0; j < 2; ++j) {
-      const uint32_t g = lane + 32 * j;
-      c[j] = g < G ? s_c[m * G + g] : 0u;
-      if (g < G && bud_queue) { const uint32_t b = bud_queue[m * G + g]; c[j] = c[j] < b ? c[j] : b; }
-      al[j] = c[j];
-      C += c[j];
-    }
-    C = __reduce_add_sync(0xFFFFFFFFu, C);  // < 2^31: every lobby has a player of its own
-    const uint32_t B = bud_mode ? bud_mode[m] : 0xFFFFFFFFu;
-    if (C > B) {  // (uniform over the warp)
-      uint32_t rem[2], fl = 0;
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const uint64_t p = (uint64_t)B * c[j];
-        al[j] = (uint32_t)(p / C); rem[j] = (uint32_t)(p % C);
-        fl += al[j];
-      }
-      const uint32_t extra = B - __reduce_add_sync(0xFFFFFFFFu, fl);  // fewer than the groups with a remainder
-      uint32_t rank[2] = {0u, 0u};  // groups that come before this one by (remainder descending, group ascending)
-      for (int l = 0; l < 32; ++l)
-#pragma unroll
-        for (int k = 0; k < 2; ++k) {
-          const uint32_t r = __shfl_sync(0xFFFFFFFFu, rem[k], l), g2 = l + 32 * k;
-#pragma unroll
-          for (int j = 0; j < 2; ++j) rank[j] += (r > rem[j] || (r == rem[j] && g2 < lane + 32 * j)) ? 1u : 0u;
-        }
-#pragma unroll
-      for (int j = 0; j < 2; ++j) al[j] += rank[j] < extra ? 1u : 0u;
-    }
-#pragma unroll
-    for (int j = 0; j < 2; ++j)
-      if (lane + 32 * j < G) s_al[m * G + lane + 32 * j] = al[j];
-  }
+  if (warp < n_cut / G) budget_apportion(s_c, s_al, warp, G, bud_queue, bud_mode);
   for (uint32_t q = threadIdx.x; q < n_cut; q += kScanBlock) cand[q] = s_c[q];
   __syncthreads();
   if (!windowed) {  // the partitions' matched counts again, with the queue's matched end at a_q L

@@ -15,6 +15,9 @@
 // when it reaches the lobby size L does a second walk take the players, one PIECE per (lobby, bin) with its offset
 // inside the lobby in member order (rating, then enqueue order).
 //
+// Off-tick budget: k_wd_allot turns the plan's per-queue lobby counts into allowances; when one falls short, the host
+// resets the plan's state and runs it again with the allowances as caps (WdArgs::cap).
+//
 // Take and output: k_bf_keys turns the taken prefixes into keys and the band pipeline takes them into staging, as for
 // mm_backfill; k_wd_bases scans the per-queue lobby counts, k_wd_hdr writes the headers and every lobby's member base,
 // and k_bf_out copies the pieces into place.
@@ -64,7 +67,8 @@ struct WdArgs {
   uint32_t* a_age;             // [n_anchors] (seq - seq_next) mod 2^32
   uint32_t* a_rank;            // [n_anchors] rank in the bin
   uint2* rec;                  // [n_anchors] lobby record: (queue, index inside the queue)
-  uint32_t* qlob;              // [n_cut] lobbies of the queue
+  uint32_t* qlob;              // [n_cut] lobbies of the queue (0 for a queue not served)
+  const uint32_t* cap;         // [n_cut] lobbies the queue may emit (the off-tick budget's allowance), or null
   uint32_t* qlbase;            // [n_cut] first lobby of the queue
   uint32_t* qmbase;            // [n_cut] first member slot of the queue
   BfPiece* piece;              // pieces: req = lobby record
@@ -154,11 +158,12 @@ __global__ void __launch_bounds__(kWdPlanWarps * 32) k_wd_plan(const WdArgs a) {
   const uint32_t lane = threadIdx.x & 31, warp = threadIdx.x >> 5, c = blockIdx.x * kWdPlanWarps + warp;
   if (c >= a.n_cut) return;
   const WdRule u = a.rule[c];
-  if (u.min_wait == MM_WIDEN_OFF) return;
+  if (u.min_wait == MM_WIDEN_OFF) { if (lane == 0) a.qlob[c] = 0; return; }
   const uint32_t p0 = a.cut_lp_lo[c], p1 = a.cut_lp_lo[c + 1];
   const uint32_t lo = a.seg_bin_lo[p0], hi = a.seg_bin_lo[p1];
+  const uint32_t cap = a.cap ? a.cap[c] : 0xFFFFFFFFu;
   uint32_t n_lob = 0, n_abs = 0;
-  for (;;) {
+  while (n_lob < cap) {  // a capped queue stops after its cap-th lobby: the rest of its anchors stay queued
     // the oldest anchor not yet served: the least age over the heads of the partitions' runs (ages are unique)
     unsigned long long best = ~0ull;
     for (uint32_t p = p0 + lane; p < p1; p += 32) {
@@ -191,6 +196,24 @@ __global__ void __launch_bounds__(kWdPlanWarps * 32) k_wd_plan(const WdArgs a) {
     a.qlob[c] = n_lob;
     if (n_abs) atomicAdd(&a.ctr[kWdAbsorbed], n_abs);
   }
+}
+
+// One CTA, the off-tick budget (mm_set_offtick_budget) of an mm_widen / mm_party_match call after its unbudgeted plan:
+// cand[q] = qlob[q] (c_q), allot[q] = a_q by the tick's apportionment (budget_apportion, one warp per mode) of bud_queue
+// [n_cut] / bud_mode [n_modes] (either null: unlimited), *cut = 1 if some a_q < c_q (the plan runs again, capped).
+__global__ void __launch_bounds__(kScanBlock) k_wd_allot(const WdArgs a, const uint32_t* bud_queue,
+                                                         const uint32_t* bud_mode, uint32_t* cand, uint32_t* allot,
+                                                         uint32_t* cut) {
+  const uint32_t G = a.n_groups;
+  for (uint32_t q = threadIdx.x; q < a.n_cut; q += kScanBlock) cand[q] = a.qlob[q];
+  __syncthreads();
+  for (uint32_t m = threadIdx.x >> 5; m < a.n_cut / G; m += kScanBlock / 32)
+    budget_apportion(cand, allot, m, G, bud_queue, bud_mode);
+  __syncthreads();
+  bool less = false;
+  for (uint32_t q = threadIdx.x; q < a.n_cut; q += kScanBlock) less |= allot[q] < cand[q];
+  const int any = __syncthreads_or(less);
+  if (threadIdx.x == 0) *cut = any ? 1u : 0u;
 }
 
 // One warp: the lobby and member bases of every queue (queue order = (mode, group) order).

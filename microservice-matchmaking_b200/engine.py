@@ -774,15 +774,17 @@ class Engine:
         """Lobbies every (mode, group) queue / every mode may emit per tick, from the next tick until set again
         (mm_set_lobby_budget).  per_queue: n_modes * n_groups values in queue_stats() record order (or
         [n_modes][n_groups]); per_mode: n_modes values; None, or abi.MM_BUDGET_UNLIMITED in an entry = no limit."""
+        q, m = self._budget_arrays(per_queue, per_mode)
+        self._check(self.lib.mm_set_lobby_budget(self.h, _p(q), _p(m)), "mm_set_lobby_budget")
+
+    def _budget_arrays(self, per_queue, per_mode):
         def arr(a, n):
             if a is None:
                 return None
             a = np.ascontiguousarray(np.asarray(a, np.int64).reshape(-1).clip(0, abi.MM_BUDGET_UNLIMITED), np.uint32)
             assert len(a) == n
             return a
-        q = arr(per_queue, self.cfg.n_modes * self.cfg.n_groups)
-        m = arr(per_mode, self.cfg.n_modes)
-        self._check(self.lib.mm_set_lobby_budget(self.h, _p(q), _p(m)), "mm_set_lobby_budget")
+        return arr(per_queue, self.cfg.n_modes * self.cfg.n_groups), arr(per_mode, self.cfg.n_modes)
 
     def lobby_budget_report(self):
         """-> (candidates u32[n_modes * n_groups], emitted u32[...]) of the last completed tick: the lobbies every queue
@@ -792,6 +794,24 @@ class Engine:
         n = C.c_uint32(0)
         self._check(self.lib.mm_lobby_budget_report(self.h, _p(cand), _p(emitted), cap, C.byref(n)),
                     "mm_lobby_budget_report")
+        return cand[:n.value], emitted[:n.value]
+
+    def set_offtick_budget(self, source, per_queue=None, per_mode=None):
+        """Lobbies every (mode, group) queue / every mode may emit per call of `source` (abi.MM_OFFTICK_PARTY_MATCH:
+        party_match, abi.MM_OFFTICK_WIDEN: widen), from the next such call until set again (mm_set_offtick_budget).
+        Arrays as in set_lobby_budget; each source's budget is separate from the other's and from the tick's."""
+        q, m = self._budget_arrays(per_queue, per_mode)
+        self._check(self.lib.mm_set_offtick_budget(self.h, source, _p(q), _p(m)), "mm_set_offtick_budget")
+
+    def offtick_budget_report(self, source):
+        """-> (candidates u32[n_modes * n_groups], emitted u32[...]) of the last call of `source` that returned MM_OK
+        or was an MM_E_CAP dry run: the lobbies every queue had, budgets ignored, and the lobbies it emitted (or would
+        have) (mm_offtick_budget_report).  All zeros before such a call."""
+        cap = self.cfg.n_modes * self.cfg.n_groups
+        cand, emitted = np.zeros(cap, np.uint32), np.zeros(cap, np.uint32)
+        n = C.c_uint32(0)
+        self._check(self.lib.mm_offtick_budget_report(self.h, source, _p(cand), _p(emitted), cap, C.byref(n)),
+                    "mm_offtick_budget_report")
         return cand[:n.value], emitted[:n.value]
 
     def lobby_candidates(self):

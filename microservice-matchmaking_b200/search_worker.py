@@ -184,6 +184,10 @@ class SearchPool:
     before the tick itself, so parties get the first pick of the solos; its lobbies are published like the tick's and
     stats["party_lobbies"] counts them.  A party member removed with remove_user() takes its whole party out; a matched
     member's requeue() answers "gone" (the caller enqueues the party again).
+    budget_offtick: with lobby_budget, one step's budget covers every lobby the step publishes (extension,
+    Engine.set_offtick_budget): party_match runs under the callable's per-mode budget F, the tick under F minus the
+    step's party lobbies of each mode, widen under what is left; paused queues emit nothing from any of the three, and
+    held_back() reports each source.  Off (the default), party_match and widen run without a budget.
     requeue_parties: with parties, requeue() puts matched parties back as parties (extension, Engine.requeue_party):
     the pool keeps a book of every queued party (members, ratings, mode, stamp and enqueue sequence number) and moves a
     party's entry aside when party_match places it, until remove_user or a requeue.  Off (the default), requeue() of a
@@ -196,7 +200,8 @@ class SearchPool:
 
     def __init__(self, engine, mode_names, group_names, max_batch=65536, window=None, clock=None, flush_every_s=0.005,
                  handle_capacity=None, timeout_ms=None, wall_clock=None, lobby_budget=None, widen=None,
-                 balance_teams=None, parties=None, party_capacity=None, requeue_parties=False, balance_parties=None):
+                 balance_teams=None, parties=None, party_capacity=None, requeue_parties=False, balance_parties=None,
+                 budget_offtick=False):
         import time
         if widen and engine.cfg.order_mode != abi.MM_ORDER_RATING:
             raise ValueError("widen needs an MM_ORDER_RATING engine: windows are rating distances")
@@ -219,6 +224,7 @@ class SearchPool:
         self._staged_parties = []  # (worker, tag, [player documents], game mode)
         self.timeout_ms = timeout_ms
         self.lobby_budget = lobby_budget
+        self.budget_offtick = bool(budget_offtick)
         self.paused = set()  # queues (mode * n_groups + group) that emit nothing until resume_queues()
         self.clock = clock or time.monotonic
         self.wall_clock = wall_clock or time.time  # seconds since the epoch: checkpoint() / resume() bridge the downtime
@@ -663,11 +669,18 @@ class SearchPool:
             oldest = next(iter(self.enqueued_at.values()), None)
             self.last_spread = self.window.spread(self.clock(), oldest)
             self.engine.set_option("max_spread", self.last_spread)
+        left = None  # budget_offtick: the step's per-queue and per-mode budgets, less what the step published
         if self.lobby_budget is not None:
-            self._set_budget(self.lobby_budget())
+            if self.budget_offtick:
+                left = self._budget_arrays(self.lobby_budget())
+            else:
+                self._set_budget(self.lobby_budget())
         n_lob = 0
         if self.party_rules:  # before the tick: parties get the first pick of the solos
+            if left is not None:
+                self.engine.set_offtick_budget(abi.MM_OFFTICK_PARTY_MATCH, *left)
             plob, pmem, _st = self.engine.party_match(now, self.party_rules)
+            left = self._budget_less(left, plob)
             for x in pmem.tolist():
                 self.party_of.pop(x, None)
                 rec = self.party_book.pop(x, None)
@@ -676,11 +689,16 @@ class SearchPool:
             self._publish(plob, pmem)
             self.stats["party_lobbies"] += len(plob)
             n_lob += len(plob)
+        if left is not None:
+            self.engine.set_lobby_budget(*left)
         lob, mem, _seq, _st = self.engine.tick(now)
+        left = self._budget_less(left, lob)
         self._publish(lob, mem)
         self.stats["lobbies"] += len(lob)
         n_lob += len(lob)
         if self.widen:  # before the timeout: a player who waited long gets its widest window before it is dropped
+            if left is not None:
+                self.engine.set_offtick_budget(abi.MM_OFFTICK_WIDEN, *left)
             wlob, wmem, _st = self.engine.widen(now, self.widen)
             self._publish(wlob, wmem)
             self.stats["widened"] += len(wlob)
@@ -712,7 +730,9 @@ class SearchPool:
         modes = range(len(self.mode_names)) if mode_names is None else [self.mode_names.index(m) for m in mode_names]
         return {m * len(self.group_names) + self.group_names.index(g) for g in group_names for m in modes}
 
-    def _set_budget(self, per_mode=None):
+    def _budget_arrays(self, per_mode=None):
+        """-> (per-queue budgets: 0 for a paused queue, else unlimited; per-mode budgets from {mode name: lobbies}, or
+        None)."""
         from .abi import MM_BUDGET_UNLIMITED
         queue = np.full(len(self.mode_names) * len(self.group_names), MM_BUDGET_UNLIMITED, np.uint32)
         queue[sorted(self.paused)] = 0
@@ -720,7 +740,28 @@ class SearchPool:
         if per_mode is not None:
             mode = np.array([min(max(int(per_mode.get(m, MM_BUDGET_UNLIMITED)), 0), MM_BUDGET_UNLIMITED)
                              for m in self.mode_names], np.uint32)
+        return queue, mode
+
+    def _budget_less(self, left, lobbies):
+        """budget_offtick: the per-mode budgets of `left` less the lobbies just published, per mode (an unlimited mode
+        stays unlimited)."""
+        from .abi import MM_BUDGET_UNLIMITED
+        if left is None or left[1] is None:
+            return left
+        used = np.bincount(np.asarray(lobbies["mode"], np.int64), minlength=len(self.mode_names))[:len(self.mode_names)]
+        mode = left[1].astype(np.int64)
+        return left[0], np.where(mode == MM_BUDGET_UNLIMITED, mode, np.maximum(mode - used, 0)).astype(np.uint32)
+
+    def _set_budget(self, per_mode=None):
+        queue, mode = self._budget_arrays(per_mode)
         self.engine.set_lobby_budget(per_queue=queue, per_mode=mode)
+        if self.budget_offtick:  # the off-tick calls the pool runs, under the same budgets
+            for _name, src in self._offtick_sources():
+                self.engine.set_offtick_budget(src, per_queue=queue, per_mode=mode)
+
+    def _offtick_sources(self):
+        return ([("party_match", abi.MM_OFFTICK_PARTY_MATCH)] if self.party_rules else []) + \
+            ([("widen", abi.MM_OFFTICK_WIDEN)] if self.widen else [])
 
     def pause(self, group_names, mode_names=None):
         """The queues of these groups (all modes, or only `mode_names`) emit no lobby from the next tick on; their
@@ -736,12 +777,20 @@ class SearchPool:
 
     def held_back(self, group_name):
         """{mode name: lobbies the last tick could have emitted from the group's queue and did not} (candidates minus
-        emitted, Engine.lobby_budget_report); {} for an unknown group."""
+        emitted, Engine.lobby_budget_report); {} for an unknown group.  With budget_offtick: {mode name: {source:
+        lobbies}}, source "tick" and each off-tick call the pool runs ("party_match", "widen";
+        Engine.offtick_budget_report)."""
         if group_name not in self.group_names:
             return {}
-        cand, emitted = self.engine.lobby_budget_report()
         g, G = self.group_names.index(group_name), len(self.group_names)
-        return {name: int(cand[m * G + g]) - int(emitted[m * G + g]) for m, name in enumerate(self.mode_names)}
+        reports = [("tick", self.engine.lobby_budget_report())]
+        if self.budget_offtick:
+            reports += [(name, self.engine.offtick_budget_report(src)) for name, src in self._offtick_sources()]
+        held = {name: {m: int(cand[m * G + g]) - int(emitted[m * G + g]) for m in range(len(self.mode_names))}
+                for name, (cand, emitted) in reports}
+        if not self.budget_offtick:
+            return {mode: held["tick"][m] for m, mode in enumerate(self.mode_names)}
+        return {mode: {name: held[name][m] for name in held} for m, mode in enumerate(self.mode_names)}
 
     def _expire(self, now):
         expired, _seq = self.engine.expire(now, self.timeout_ms, want_seq=False)
@@ -1153,16 +1202,14 @@ class SearchPool:
         the mean / p99 / max rating spread and team imbalance in rating points.  Quantiles are the upper bounds of
         histogram buckets (at most 25 % high).  A source whose report is void (no call yet, or a failed one) is left
         out; {} for a group the pool does not know."""
-        from .abi import MM_OFFTICK_PARTY_MATCH, MM_OFFTICK_WIDEN
         from .engine import wait_quantile
         if group_name not in self.group_names:
             return {}
         g = self.group_names.index(group_name)
-        sources = [("party_match", MM_OFFTICK_PARTY_MATCH)] if self.party_rules else []
-        sources += [("widen", MM_OFFTICK_WIDEN)] if self.widen else []
         out = {}
-        for name, src in sources:
+        for name, src in self._offtick_sources():
             waits, quality, _ = self.engine.offtick_report(src)
+            held = self.engine.offtick_budget_report(src) if self.budget_offtick else None
             for w, r in zip(waits, quality):
                 if int(w["group"]) != g or int(w["mode"]) >= len(self.mode_names):
                     continue
@@ -1180,6 +1227,9 @@ class SearchPool:
                     "p99_imbalance": wait_quantile(r["imbalance_hist"], 0.99),
                     "max_imbalance": int(r["max_imbalance"]),
                 }
+                if held is not None:  # budget_offtick: lobbies the source's budget held back
+                    q = int(w["mode"]) * len(self.group_names) + g
+                    out[self.mode_names[int(w["mode"])]][name]["held_back"] = int(held[0][q]) - int(held[1][q])
         return out
 
 
