@@ -1831,6 +1831,151 @@ int requeue(mm_engine* e, uint32_t n, const uint64_t* id, const int32_t* rating,
 }
 
 // ---- mm_import_regroup / mm_import_regroup_many (mm_regroup.cuh, mm_recut.cuh) -----------------------------------
+// The party images of mm_import_regroup_many_parties, as their headers describe them.
+struct RpImages {
+  std::vector<uint32_t> pbase, mcount, pnblk;  // [K + 1] image k's first party; [K] its members; [K] classify blocks
+  std::vector<PtImgLayout> pl;
+  uint64_t P = 0, M = 0;                       // parties and members in all
+};
+
+// The party images' header checks on the host, against their engine images h (pp null: no party image).
+int rp_headers(mm_engine* e, uint32_t K, mm_recut_parties* pp, const std::vector<mm_image_header>& h, RpImages& r) {
+  r.pbase.assign(K + 1, 0); r.mcount.assign(K, 0); r.pnblk.assign(K, 0); r.pl.resize(K);
+  if (!pp) return MM_OK;
+  pp->n_rejected = pp->n_elsewhere = pp->n_loaded = 0;
+  for (uint32_t k = 0; k < K; ++k) {
+    r.pbase[k] = (uint32_t)r.P;
+    const uint64_t nb = pp->n_bytes ? pp->n_bytes[k] : 0;
+    const uint8_t* b = pp->bufs ? static_cast<const uint8_t*>(pp->bufs[k]) : nullptr;
+    if (!b || !nb) continue;
+    auto bad = [&](const char* what) { return set_err(e, MM_E_ARG, "party image %u rejected: %s", k, what); };
+    mm_image_header ph;
+    if (nb < sizeof(ph)) return bad("shorter than its header");
+    std::memcpy(&ph, b, sizeof(ph));
+    if (ph.magic != MM_PARTY_IMAGE_MAGIC) return bad("bad magic (not an mm_export_parties image)");
+    if (ph.version != MM_IMAGE_VERSION || ph.abi_version != MM_ABI_VERSION) return bad("unknown version");
+    if (ph.id_bytes != h[0].id_bytes) return bad("id width differs from the engine's");
+    if (ph.config.flags & MM_F_NO_DEDUPE) return bad("written by an MM_F_NO_DEDUPE engine");
+    r.pl[k] = pt_img_layout(ph.n_parts, ph.n_players, ph.id_bytes);
+    if (ph.n_active || ph.total_bytes != r.pl[k].off[6] || nb != r.pl[k].off[6])
+      return bad("length does not match the header's section counts");
+    if (!same_layout(ph.config, h[k].config) || ph.seq_next != h[k].seq_next)
+      return bad("config or seq_next differs from its engine image's (not written at the same stop)");
+    r.P += ph.n_parts;
+    r.M += ph.n_players;
+    r.mcount[k] = ph.n_players;
+    r.pnblk[k] = (ph.n_parts + kRqItems - 1) / kRqItems;
+    if (r.P > 0x7FFFFFFFu || r.M > 0x7FFFFFFFu) return set_err(e, MM_E_CAP, "more than 2^31 - 1 parties or members");
+  }
+  r.pbase[K] = (uint32_t)r.P;
+  if (r.P) {
+    if (e->cfg.order_mode != MM_ORDER_RATING) return set_err(e, MM_E_ARG, "party images need MM_ORDER_RATING");
+    if (!e->use_active) return set_err(e, MM_E_ARG, "an MM_F_NO_DEDUPE engine cannot hold parties");
+    if (!e->pt.cap) return set_err(e, MM_E_STATE, "no party capacity: set the option party_capacity first");
+  }
+  return MM_OK;
+}
+
+// The buffers of one merge of K images' runs (mm_recut.cuh): the solos' over S partitions, the parties' over C queues.
+// one = {0, kept, runs, kmax}; pair / ord / run / kq: k_rg_plan's; s2 / key: the ping-pong of virtual index and
+// (stamp, image, age) key; head / agg / carry / first: the running-max scan.
+struct RcRuns {
+  uint32_t *glob, *one, *pair, *run, *kq, *s2[2], *first;
+  uint16_t* ord;
+  RcKey* key[2];
+  uint8_t* head;
+  RcSeg *agg, *carry;
+};
+
+// regroup_many's scratch in d_rg, one member per array; the carve in regroup_many gives each its count (0 where the
+// call does not use it).  sr: K > 1, the solos' partition runs merged; pr: with parties too, their queue runs.
+struct RgScratch {
+  unsigned long long *seen, *seqset;
+  uint8_t *grp, *sel, *keep, *out, *pbody, *psel, *pkeep, *psz;
+  uint16_t *lut, *bseg, *ord, *part, *pimg, *ident, *img, *qv, *ppart, *pk;
+  uint32_t *off, *rq, *skip, *hist, *pair, *run, *kq, *src[2], *age[2], *rej, *pos, *base;
+  uint32_t *pbase, *pctr, *pmoff, *pflag, *phist, *rqp, *psrc, *page, *rsrc, *rsz, *fin;
+  int32_t* pR;
+  ImgCols* imgs;
+  PtImgCols* pcols;
+  RcRuns sr, pr;
+};
+
+// p <- the next n T at cursor o over base (null: only o moves), 16-byte aligned.
+template <class T>
+void rg_take(uint8_t* base, size_t& o, T*& p, size_t n) {
+  p = base ? reinterpret_cast<T*>(base + o) : nullptr;
+  o += (n * sizeof(T) + 15) & ~(size_t)15;
+}
+
+// The ⌈log2 runs⌉ rounds of k_rg_merge over ma's runs (ma.n_img_segs of them), ping-ponging between (src, key)[0] and
+// [1] from [0]; the rounds past kmax's need return at once.  -> the index of the pair that holds the merged runs.
+template <class U>
+uint32_t rg_rounds(mm_engine* e, RgMergeArgsT<U> ma, uint32_t* const src[2], U* const key[2], uint32_t grid) {
+  uint32_t t = 0;
+  for (; (1u << t) < ma.n_img_segs; ++t) {
+    ma.round = t;
+    ma.src_in = src[t & 1]; ma.u_in = key[t & 1]; ma.src_out = src[(t + 1) & 1]; ma.u_out = key[(t + 1) & 1];
+    k_rg_merge<<<grid, 256, 0, e->stream>>>(ma);
+  }
+  return t & 1;
+}
+
+// The runs of K images merged into one order per new partition or queue (runs n_segs).  Image k's kept runs are at
+// rq[(n_segs + 2) * k] in src / age from first[k] on, its rows virtual indices vbase + first[k] on with stamps ts[k],
+// and their runs new partitions qoff + run in qv.  The stamps become running maxima over each run; then the rounds over
+// K, whose result k_rc_finish / k_rp_norm find by r.one[3].  rows: the length of r.s2; nrb, grid: the scan's blocks
+// and the rounds' grid.
+int rc_merge(mm_engine* e, uint32_t K, uint32_t n_segs, const uint32_t* rq, const std::vector<uint32_t>& first,
+             const uint32_t* const src[2], const uint32_t* const age[2], const std::vector<const uint32_t*>& ts,
+             uint32_t vbase, uint32_t qoff, uint16_t* img, uint16_t* qv, const RcRuns& r, size_t rows, uint32_t nrb,
+             uint32_t grid) {
+  const uint32_t n_kmax[2] = {n_segs, 0};  // one[2] = n_segs for the rounds into one list; one[3] = kmax
+  CK(cudaMemcpyAsync(r.one + 2, n_kmax, 8, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemsetAsync(r.ord, 0, 2 * (size_t)K * n_segs, e->stream));
+  CK(cudaMemsetAsync(r.s2[0], 0, 4 * rows, e->stream));  // holes (a refused image) stay in range
+  CK(cudaMemsetAsync(r.s2[1], 0, 4 * rows, e->stream));
+  k_rc_sum<<<1, 1024, 0, e->stream>>>(K, n_segs, rq, r.glob, r.one, r.pair);
+  k_rg_plan<<<1, 1024, 0, e->stream>>>(K, n_segs, r.pair, r.glob, r.ord, r.run, r.kq, r.one + 3);
+  for (uint32_t k = 0; k < K; ++k) {
+    const uint32_t n = first[k + 1] - first[k];
+    if (!n) continue;
+    RcGatherArgs ga{};
+    ga.k = k; ga.base = vbase + first[k]; ga.n = n; ga.n_segs = n_segs; ga.n_img = K; ga.rq_off = rq + (n_segs + 2) * k;
+    ga.kmax = &e->d_cnt->rg_kmax; ga.src[0] = src[0] + first[k]; ga.src[1] = src[1] + first[k];
+    ga.age[0] = age[0] + first[k]; ga.age[1] = age[1] + first[k]; ga.ord = r.ord; ga.run_start = r.run;
+    ga.ts = ts[k]; ga.src_out = r.s2[0]; ga.key_out = r.key[0]; ga.head = r.head; ga.img = img; ga.qv = qv;
+    ga.qoff = qoff; ga.err = &e->d_cnt->img_err;
+    k_rc_gather<<<grid256(e, n, 32), 256, 0, e->stream>>>(ga);
+  }
+  if (nrb) {  // (no solo: parties only)
+    k_rc_runmax<<<nrb, 256, 0, e->stream>>>(r.one + 1, r.key[0], r.head, r.agg, r.first);
+    k_rc_carry<<<1, 1024, 0, e->stream>>>(r.one + 1, r.agg, r.carry);
+    k_rc_apply<<<nrb, 256, 0, e->stream>>>(r.one + 1, r.key[0], r.carry, r.first);
+  }
+  rg_rounds(e, RgMergeArgsT<RcKey>{r.glob, n_segs, K, 0, img, r.ord, r.run, r.kq, r.one + 3}, r.s2, r.key, grid);
+  return MM_OK;
+}
+
+// Each image's reject bucket (run n_segs of its rq row, in src from first[k]), in image order: (image, index)
+// ascending; then rej_image, when asked for.
+int rg_rejects(mm_engine* e, uint32_t K, uint32_t n_segs, const std::vector<uint32_t>& h_rq, const uint32_t* src,
+               const std::vector<uint32_t>& first, uint32_t* rej_index, uint32_t* rej_image) {
+  const size_t R = n_segs + 2;
+  for (uint32_t k = 0, w = 0; k < K; ++k) {
+    const uint32_t* r = h_rq.data() + R * k;
+    if (r[n_segs + 1] > r[n_segs])
+      CK(cudaMemcpyAsync(rej_index + w, src + first[k] + r[n_segs], (size_t)(r[n_segs + 1] - r[n_segs]) * 4,
+                         cudaMemcpyDeviceToHost, e->stream));
+    w += r[n_segs + 1] - r[n_segs];
+  }
+  CK(cudaStreamSynchronize(e->stream));
+  if (rej_image)
+    for (uint32_t k = 0, w = 0; k < K; ++k)
+      for (uint32_t j = h_rq[R * k + n_segs]; j < h_rq[R * k + n_segs + 1]; ++j) rej_image[w++] = k;
+  return MM_OK;
+}
+
 // K images of one config: each runs the regroup pipeline on its own; for K > 1 the images' runs are merged and the
 // kept players renumbered on the device.  Every refusal is decided by one read of the counters, before the load tail
 // writes the pool.  `who` names the call in the state refusal; keep_cut: n_cut selection bytes (null: all); act_img:
@@ -1859,43 +2004,10 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
   }
   const uint32_t S = e->n_segs, SI = y.n_segs, idb = h[0].id_bytes;
   const uint32_t m = act_img < K ? h[act_img].n_active : 0;
-  // the party images: header checks on the host; P parties and M members in all
-  std::vector<uint32_t> pbase(K + 1, 0), mcount(K, 0), pnblk(K, 0);
-  std::vector<PtImgLayout> pl(K);
-  uint64_t P = 0, M = 0;
-  if (pp) {
-    pp->n_rejected = pp->n_elsewhere = pp->n_loaded = 0;
-    for (uint32_t k = 0; k < K; ++k) {
-      pbase[k] = (uint32_t)P;
-      const uint64_t nb = pp->n_bytes ? pp->n_bytes[k] : 0;
-      const uint8_t* b = pp->bufs ? static_cast<const uint8_t*>(pp->bufs[k]) : nullptr;
-      if (!b || !nb) continue;
-      auto bad = [&](const char* what) { return set_err(e, MM_E_ARG, "party image %u rejected: %s", k, what); };
-      mm_image_header ph;
-      if (nb < sizeof(ph)) return bad("shorter than its header");
-      std::memcpy(&ph, b, sizeof(ph));
-      if (ph.magic != MM_PARTY_IMAGE_MAGIC) return bad("bad magic (not an mm_export_parties image)");
-      if (ph.version != MM_IMAGE_VERSION || ph.abi_version != MM_ABI_VERSION) return bad("unknown version");
-      if (ph.id_bytes != idb) return bad("id width differs from the engine's");
-      if (ph.config.flags & MM_F_NO_DEDUPE) return bad("written by an MM_F_NO_DEDUPE engine");
-      pl[k] = pt_img_layout(ph.n_parts, ph.n_players, ph.id_bytes);
-      if (ph.n_active || ph.total_bytes != pl[k].off[6] || nb != pl[k].off[6])
-        return bad("length does not match the header's section counts");
-      if (!same_layout(ph.config, h[k].config) || ph.seq_next != h[k].seq_next)
-        return bad("config or seq_next differs from its engine image's (not written at the same stop)");
-      P += ph.n_parts;
-      M += ph.n_players;
-      mcount[k] = ph.n_players;
-      pnblk[k] = (ph.n_parts + kRqItems - 1) / kRqItems;
-      if (P > 0x7FFFFFFFu || M > 0x7FFFFFFFu) return set_err(e, MM_E_CAP, "more than 2^31 - 1 parties or members");
-    }
-    pbase[K] = (uint32_t)P;
-    if (P) {
-      if (e->cfg.order_mode != MM_ORDER_RATING) return set_err(e, MM_E_ARG, "party images need MM_ORDER_RATING");
-      if (!e->use_active) return set_err(e, MM_E_ARG, "an MM_F_NO_DEDUPE engine cannot hold parties");
-      if (!e->pt.cap) return set_err(e, MM_E_STATE, "no party capacity: set the option party_capacity first");
-    }
-  }
+  RpImages ri;
+  if ((rc = rp_headers(e, K, pp, h, ri))) return rc;
+  const std::vector<uint32_t>& pbase = ri.pbase;
+  const uint64_t P = ri.P;
   const bool parties = P != 0;
   const uint32_t C = e->n_cut;
   std::vector<uint32_t> base(K + 1, 0), nblk(K);
@@ -1923,7 +2035,7 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
   if (N == 0 && !parties)
     return load_columns(e, std::vector<uint32_t>(S, 0), in[0], 0, act, m, seq_next, "image rejected");
   // scratch: the images' tables, the classification, the scatter and merge buffers, the gathered columns
-  const uint64_t sc = e->use_active ? seen_keys((uint64_t)N + m + M) : 0;  // the repeated-id set
+  const uint64_t sc = e->use_active ? seen_keys((uint64_t)N + m + ri.M) : 0;  // the repeated-id set
   std::vector<uint32_t> off((size_t)K * (SI + 1), 0);
   for (uint32_t k = 0; k < K; ++k)
     for (uint32_t s = 0; s < SI; ++s) off[(size_t)k * (SI + 1) + s + 1] = off[(size_t)k * (SI + 1) + s] + cnt[k][s];
@@ -1932,359 +2044,232 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
     keep.resize(S);
     for (uint32_t q = 0; q < S; ++q) keep[q] = keep_cut[e->h_part_cut[q]] != 0;
   }
-  uint64_t hist_n = 0;
-  for (uint32_t k = 0; k < K; ++k) hist_n += (uint64_t)(S + 1) * nblk[k];
-  const size_t pair_n = (size_t)SI * S, R1 = S + 2;  // per image: (image partition, new partition) pairs; rq_off
-  const uint32_t nrb = (N + kRcBlock - 1) / kRcBlock;
-  size_t o = 0;  // the scratch arrays' offsets in d_rg, 16-byte aligned
-  auto take = [&o](size_t bytes) { const size_t x = o; o += (bytes + 15) & ~(size_t)15; return x; };
-  const size_t o_seen = take(8 * sc), o_lut = take(2 * (size_t)y.KR), o_grp = take(y.KR), o_bseg = take(2 * (size_t)y.Kp),
-               o_off = take(4 * off.size()), o_rq = take(4 * R1 * K), o_sel = take((size_t)S + 1),
-               o_keep = take(keep.size()), o_skip = take(4 * (size_t)K), o_hist = take(4 * hist_n),
-               o_pair = take(4 * pair_n * K), o_ord = take(2 * pair_n * K), o_run = take(4 * (size_t)S * (SI + 1) * K),
-               o_kq = take(4 * (size_t)S * K), o_part = take(2 * (size_t)N), o_pimg = take(2 * (size_t)N),
-               o_src0 = take(4 * (size_t)N), o_src1 = take(4 * (size_t)N), o_age0 = take(4 * (size_t)N),
-               o_age1 = take(4 * (size_t)N), o_rej = take(K == 1 ? 4 * (size_t)N : 0), o_out = take(cols_bytes(N + P));
-  // K > 1: the image runs' merge and the numbering
+  uint64_t hist_n = 0, phist_n = 0;
+  for (uint32_t k = 0; k < K; ++k) {
+    hist_n += (uint64_t)(S + 1) * nblk[k];
+    phist_n += (uint64_t)(C + 1) * ri.pnblk[k];
+  }
+  std::vector<uint64_t> pboff(K + 1, 0);  // each party image's body (section 1 on) in x.pbody, 16-byte aligned
+  for (uint32_t k = 0; k < K; ++k)
+    pboff[k + 1] = pboff[k] + (pbase[k + 1] > pbase[k] ? (ri.pl[k].off[6] - ri.pl[k].off[0] + 15) & ~(uint64_t)15 : 0);
   const bool many = K > 1;
-  auto take2 = [&](size_t bytes) { return many ? take(bytes) : 0; };
-  const size_t o_rqg = take2(4 * ((size_t)S + 1)), o_one = take2(4 * 4), o_pair2 = take2(4 * (size_t)K * S),
-               o_ord2 = take2(2 * (size_t)K * S), o_run2 = take2(4 * (size_t)S * (K + 1)), o_kq2 = take2(4 * (size_t)S),
-               o_ident = take2(4 * ((size_t)S + C)), o_s2a = take2(4 * (N + P)), o_s2b = take2(4 * (N + P)),
-               o_keya = take2(sizeof(RcKey) * (N + P)), o_keyb = take2(sizeof(RcKey) * (N + P)), o_head = take2(N),
-               o_img = take2(2 * (N + P)), o_qv = take2(2 * (N + P)), o_agg = take2(sizeof(RcSeg) * nrb),
-               o_carry = take2(sizeof(RcSeg) * nrb), o_first = take2(4 * (size_t)nrb), o_pos = take2(4 * (N + P)),
-               o_imgs = take2(sizeof(ImgCols) * K), o_base = take2(4 * (size_t)K);
-  // the parties: their images, classification, scatter by queue, and (K > 1) the queue merge and their order
-  auto take3 = [&](size_t bytes) { return parties ? take(bytes) : 0; };
-  auto take4 = [&](size_t bytes) { return parties && many ? take(bytes) : 0; };
-  std::vector<uint64_t> pboff(K + 1, 0);
-  for (uint32_t k = 0; k < K; ++k) pboff[k + 1] = pboff[k] + (parties && pbase[k + 1] > pbase[k] ? (pl[k].off[6] - pl[k].off[0] + 15) & ~(uint64_t)15 : 0);
-  uint64_t phist_n = 0;
-  for (uint32_t k = 0; k < K; ++k) phist_n += (uint64_t)(C + 1) * pnblk[k];
-  const size_t R2 = C + 2, nrbp = (P + kRcBlock - 1) / kRcBlock;
-  const size_t o_pbody = take3(pboff[K]), o_pcols = take3(sizeof(PtImgCols) * K), o_pbase = take3(4 * ((size_t)K + 1)),
-               o_seqset = take3(8 * seen_keys(P)), o_pctr = take3(4 * (kRpWords + 3 * (size_t)K)),
-               o_pmoff = take3(4 * P), o_ppart = take3(2 * P), o_pk = take3(2 * P), o_pR = take3(4 * P),
-               o_pflag = take3(4 * P), o_phist = take3(4 * phist_n), o_rqp = take3(4 * R2 * K), o_psel = take3(C + 1), o_pkeep = take3(keep_cut ? C : 0), o_psz = take3(P),
-               o_psrc = take3(4 * P), o_page = take3(4 * P), o_rsrc = take3(4 * P), o_rsz = take3(4 * P + 8),
-               o_pqone = take4(4 * 4), o_pglob = take4(4 * ((size_t)C + 1)), o_ppair = take4(4 * (size_t)K * C),
-               o_pord = take4(2 * (size_t)K * C), o_prun = take4(4 * (size_t)C * (K + 1)), o_pkq = take4(4 * (size_t)C),
-               o_ps2a = take4(4 * P), o_ps2b = take4(4 * P), o_pkeya = take4(sizeof(RcKey) * P),
-               o_pkeyb = take4(sizeof(RcKey) * P), o_phead = take4(P), o_pagg = take4(sizeof(RcSeg) * nrbp),
-               o_pcarry = take4(sizeof(RcSeg) * nrbp), o_pfirst = take4(4 * nrbp), o_fin = take4(4 * 8);
-  CK(e->d_rg.reserve(o));
-  uint8_t* const sb = e->d_rg;
-  auto at = [sb](size_t x) { return sb + x; };
-  auto* seen = reinterpret_cast<unsigned long long*>(at(o_seen));
-  auto* lut_i = reinterpret_cast<uint16_t*>(at(o_lut));
-  uint8_t* grp_i = at(o_grp);
-  auto* bseg_i = reinterpret_cast<uint16_t*>(at(o_bseg));
-  auto* off_i = reinterpret_cast<uint32_t*>(at(o_off));
-  auto* rq_off = reinterpret_cast<uint32_t*>(at(o_rq));
-  uint8_t* sel = at(o_sel);
-  auto* skip = reinterpret_cast<uint32_t*>(at(o_skip));
-  auto* part = reinterpret_cast<uint16_t*>(at(o_part));
-  auto* pimg = reinterpret_cast<uint16_t*>(at(o_pimg));
-  uint32_t* src[2] = {reinterpret_cast<uint32_t*>(at(o_src0)), reinterpret_cast<uint32_t*>(at(o_src1))};
-  uint32_t* age[2] = {reinterpret_cast<uint32_t*>(at(o_age0)), reinterpret_cast<uint32_t*>(at(o_age1))};
-  uint8_t* ocur = at(o_out);
+  const size_t pair_n = (size_t)SI * S, R1 = S + 2, R2 = C + 2;  // per image: (image partition, new partition) pairs
+  const uint32_t nrb = (N + kRcBlock - 1) / kRcBlock, nrbp = (uint32_t)((P + kRcBlock - 1) / kRcBlock);
+  const uint64_t psc = parties ? seen_keys(P) : 0;
+  RgScratch x;
+  auto carve = [&](uint8_t* sb) {  // -> the bytes in use
+    size_t o = 0;
+    auto take = [&](auto*& p, size_t n) { rg_take(sb, o, p, n); };
+    auto runs = [&](RcRuns& r, size_t on, size_t ns, size_t rows, size_t heads, size_t nb) {
+      take(r.glob, on * (ns + 1)); take(r.one, on * 4); take(r.pair, on * K * ns); take(r.ord, on * K * ns);
+      take(r.run, on * ns * (K + 1)); take(r.kq, on * ns);
+      take(r.s2[0], on * rows); take(r.s2[1], on * rows); take(r.key[0], on * rows); take(r.key[1], on * rows);
+      take(r.head, on * heads); take(r.agg, on * nb); take(r.carry, on * nb); take(r.first, on * nb);
+    };
+    const size_t M1 = many, P1 = parties, PM = parties && many, NP = N + P;
+    take(x.seen, sc); take(x.lut, y.KR); take(x.grp, y.KR); take(x.bseg, y.Kp); take(x.off, off.size());
+    take(x.rq, R1 * K); take(x.sel, S + 1); take(x.keep, keep.size()); take(x.skip, K); take(x.hist, hist_n);
+    take(x.pair, pair_n * K); take(x.ord, pair_n * K); take(x.run, (size_t)S * (SI + 1) * K); take(x.kq, (size_t)S * K);
+    take(x.part, N); take(x.pimg, N);
+    take(x.src[0], N); take(x.src[1], N); take(x.age[0], N); take(x.age[1], N);
+    take(x.rej, many ? 0 : N); take(x.out, cols_bytes(NP));
+    runs(x.sr, M1, S, NP, N, nrb);
+    take(x.ident, M1 * 2 * ((size_t)S + C)); take(x.img, M1 * NP); take(x.qv, M1 * NP); take(x.pos, M1 * NP);
+    take(x.imgs, M1 * K); take(x.base, M1 * K);
+    take(x.pbody, pboff[K]); take(x.pcols, P1 * K); take(x.pbase, P1 * (K + 1)); take(x.seqset, psc);
+    take(x.pctr, P1 * (kRpWords + 3 * K));  // RpCtr | skip [K] | kept members [K] | member sums [K]
+    take(x.pmoff, P); take(x.ppart, P); take(x.pk, P); take(x.pR, P);
+    take(x.pflag, P); take(x.phist, phist_n * P1); take(x.rqp, P1 * R2 * K); take(x.psel, P1 * (C + 1));
+    take(x.pkeep, keep_cut ? P1 * C : 0); take(x.psz, P);
+    take(x.psrc, P); take(x.page, P); take(x.rsrc, P); take(x.rsz, P1 * (P + 2));
+    runs(x.pr, PM, C, P, P, nrbp);
+    take(x.fin, PM * 8);
+    return o;
+  };
+  CK(e->d_rg.reserve(carve(nullptr)));
+  carve(e->d_rg);
+  uint8_t* ocur = x.out;
   ImgCols out = carve_cols(ocur, N + P);  // seq: the kept parties' numbers at N + row
   out.id_bytes = idb;
-  CK(cudaMemcpyAsync(lut_i, y.lut.data(), (size_t)y.KR * 2, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemcpyAsync(grp_i, y.grp.data(), y.KR, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemcpyAsync(bseg_i, y.bin_seg.data(), (size_t)y.Kp * 2, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemcpyAsync(off_i, off.data(), off.size() * 4, cudaMemcpyHostToDevice, e->stream));
-  if (keep_cut) CK(cudaMemcpyAsync(at(o_keep), keep.data(), S, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemsetAsync(skip, 0, 4 * (size_t)K, e->stream));
-  CK(cudaMemsetAsync(at(o_pair), 0, pair_n * 4 * K, e->stream));
-  CK(cudaMemsetAsync(at(o_ord), 0, pair_n * 2 * K, e->stream));
-  CK(cudaMemsetAsync(src[1], 0, (size_t)N * 4, e->stream));  // a merge that writes holes (a refused image) stays in range
+  CK(cudaMemcpyAsync(x.lut, y.lut.data(), (size_t)y.KR * 2, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(x.grp, y.grp.data(), y.KR, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(x.bseg, y.bin_seg.data(), (size_t)y.Kp * 2, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemcpyAsync(x.off, off.data(), off.size() * 4, cudaMemcpyHostToDevice, e->stream));
+  if (keep_cut) CK(cudaMemcpyAsync(x.keep, keep.data(), S, cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemsetAsync(x.skip, 0, 4 * (size_t)K, e->stream));
+  CK(cudaMemsetAsync(x.pair, 0, pair_n * 4 * K, e->stream));
+  CK(cudaMemsetAsync(x.ord, 0, pair_n * 2 * K, e->stream));
+  CK(cudaMemsetAsync(x.src[1], 0, (size_t)N * 4, e->stream));  // a merge that writes holes (a refused image) stays in range
   CK(cudaMemsetAsync(&e->d_cnt->img_err, 0, 3 * 4, e->stream));  // img_err, mrg_dups, rg_kmax
-  if (e->use_active) CK(cudaMemsetAsync(seen, 0xFF, sc * 8, e->stream));
+  if (e->use_active) CK(cudaMemsetAsync(x.seen, 0xFF, sc * 8, e->stream));
   // 1. per image: classify, repeated ids, the stable scatter by new partition (reject bucket S last), the run plan
   const uint32_t grid = grid256(e, N, 32);
   uint64_t hoff = 0;
   for (uint32_t k = 0; k < K; ++k) {
     const uint32_t n = h[k].n_players, b = base[k];
-    auto* bhist = reinterpret_cast<uint32_t*>(at(o_hist)) + hoff;
+    uint32_t* bhist = x.hist + hoff;
     hoff += (uint64_t)(S + 1) * nblk[k];
-    auto* pair = reinterpret_cast<uint32_t*>(at(o_pair)) + pair_n * k;
-    auto* ord = reinterpret_cast<uint16_t*>(at(o_ord)) + pair_n * k;
-    auto* run_start = reinterpret_cast<uint32_t*>(at(o_run)) + (size_t)S * (SI + 1) * k;
-    auto* kq = reinterpret_cast<uint32_t*>(at(o_kq)) + (size_t)S * k;
+    uint32_t* pair = x.pair + pair_n * k;
     const bool take_act = k == act_img && m;
     if (n) {
       RgClassifyArgs ca{};
-      ca.in = in[k]; ca.n = n; ca.nblk = nblk[k]; ca.part_off = off_i + (size_t)k * (SI + 1); ca.n_img_segs = SI;
-      ca.bm_img = BinMap{lut_i, y.key_lo, y.KR, y.stride, y.K};
-      ca.grp_img = grp_i; ca.bin_seg_img = bseg_i; ca.n_modes_img = h[k].config.n_modes; ca.seq_next = h[k].seq_next;
+      ca.in = in[k]; ca.n = n; ca.nblk = nblk[k]; ca.part_off = x.off + (size_t)k * (SI + 1); ca.n_img_segs = SI;
+      ca.bm_img = BinMap{x.lut, y.key_lo, y.KR, y.stride, y.K};
+      ca.grp_img = x.grp; ca.bin_seg_img = x.bseg; ca.n_modes_img = h[k].config.n_modes; ca.seq_next = h[k].seq_next;
       ca.id_limit = id_limit(e);
       ca.bm = bin_map(e); ca.grp_lut = e->d_grp_lut; ca.bin_seg = e->d_bin_seg; ca.n_modes = e->cfg.n_modes; ca.n_segs = S;
-      ca.keep = keep_cut ? at(o_keep) : nullptr; ca.n_skip = skip + k;
-      ca.part = part + b; ca.pimg = pimg + b; ca.blockhist = bhist; ca.pair = pair; ca.err = &e->d_cnt->img_err;
+      ca.keep = keep_cut ? x.keep : nullptr; ca.n_skip = x.skip + k;
+      ca.part = x.part + b; ca.pimg = x.pimg + b; ca.blockhist = bhist; ca.pair = pair; ca.err = &e->d_cnt->img_err;
       k_rg_classify<<<nblk[k], 256, 0, e->stream>>>(ca);
     }
     if (e->use_active && (n || take_act))
-      k_rg_dups<<<grid, 256, 0, e->stream>>>(in[k].id, act, idb, n, take_act ? m : 0, seen, sc - 1,
+      k_rg_dups<<<grid, 256, 0, e->stream>>>(in[k].id, act, idb, n, take_act ? m : 0, x.seen, sc - 1,
                                               &e->d_cnt->mrg_dups);
     if (n) {
-      k_rq_scan<<<1, 512, 0, e->stream>>>(S + 1, nblk[k], bhist, rq_off + R1 * k, sel);
-      k_rq_group<<<nblk[k], 256, 0, e->stream>>>(n, S + 1, nblk[k], part + b, in[k].seq, h[k].seq_next, bhist,
-                                                  src[0] + b, age[0] + b);
-      k_rg_plan<<<1, 1024, 0, e->stream>>>(SI, S, pair, rq_off + R1 * k, ord, run_start, kq, &e->d_cnt->rg_kmax);
+      k_rq_scan<<<1, 512, 0, e->stream>>>(S + 1, nblk[k], bhist, x.rq + R1 * k, x.sel);
+      k_rq_group<<<nblk[k], 256, 0, e->stream>>>(n, S + 1, nblk[k], x.part + b, in[k].seq, h[k].seq_next, bhist,
+                                                  x.src[0] + b, x.age[0] + b);
+      k_rg_plan<<<1, 1024, 0, e->stream>>>(SI, S, pair, x.rq + R1 * k, x.ord + pair_n * k,
+                                           x.run + (size_t)S * (SI + 1) * k, x.kq + (size_t)S * k, &e->d_cnt->rg_kmax);
     } else {
-      CK(cudaMemsetAsync(rq_off + R1 * k, 0, 4 * R1, e->stream));
+      CK(cudaMemsetAsync(x.rq + R1 * k, 0, 4 * R1, e->stream));
     }
   }
   // 1'. per party image: sizes -> member offsets, classify (and the seq set), the repeated ids, the stable scatter by
   // queue (reject bucket C last); then every solo of the image probes the seq set
-  const uint64_t psc = parties ? seen_keys(P) : 0;
-  auto* pctr = reinterpret_cast<uint32_t*>(at(o_pctr));  // RpCtr | skip[K] | kept members[K] | member sums[K]
-  auto* pmoff = reinterpret_cast<uint32_t*>(at(o_pmoff));
-  auto* ppart = reinterpret_cast<uint16_t*>(at(o_ppart));
-  auto* ppk = reinterpret_cast<uint16_t*>(at(o_pk));
-  auto* pR = reinterpret_cast<int32_t*>(at(o_pR));
-  auto* pflag = reinterpret_cast<uint32_t*>(at(o_pflag));
-  auto* rqp = reinterpret_cast<uint32_t*>(at(o_rqp));
-  auto* psrc = reinterpret_cast<uint32_t*>(at(o_psrc));
-  auto* page = reinterpret_cast<uint32_t*>(at(o_page));
-  auto* rsrc = reinterpret_cast<uint32_t*>(at(o_rsrc));
-  auto* rsz = reinterpret_cast<uint32_t*>(at(o_rsz));
-  auto* seqset = reinterpret_cast<unsigned long long*>(at(o_seqset));
-  uint8_t* psz = at(o_psz);
   std::vector<PtImgCols> pc(K);
   if (parties) {
     for (uint32_t k = 0; k < K; ++k) {
       if (pbase[k + 1] == pbase[k]) continue;
+      const PtImgLayout& pl = ri.pl[k];
       const uint8_t* b = static_cast<const uint8_t*>(pp->bufs[k]);
-      uint8_t* d = at(o_pbody) + pboff[k];
-      CK(cudaMemcpyAsync(d, b + pl[k].off[0], pl[k].off[6] - pl[k].off[0], cudaMemcpyHostToDevice, e->stream));
+      uint8_t* d = x.pbody + pboff[k];
+      CK(cudaMemcpyAsync(d, b + pl.off[0], pl.off[6] - pl.off[0], cudaMemcpyHostToDevice, e->stream));
       PtImgCols& c = pc[k];
-      c.size = d; c.seq = reinterpret_cast<uint32_t*>(d + (pl[k].off[1] - pl[k].off[0]));
-      c.ts = reinterpret_cast<uint32_t*>(d + (pl[k].off[2] - pl[k].off[0])); c.mode = d + (pl[k].off[3] - pl[k].off[0]);
-      c.id = d + (pl[k].off[4] - pl[k].off[0]);
-      c.rating = reinterpret_cast<int32_t*>(d + (pl[k].off[5] - pl[k].off[0])); c.id_bytes = idb;
+      c.size = d; c.seq = reinterpret_cast<uint32_t*>(d + (pl.off[1] - pl.off[0]));
+      c.ts = reinterpret_cast<uint32_t*>(d + (pl.off[2] - pl.off[0])); c.mode = d + (pl.off[3] - pl.off[0]);
+      c.id = d + (pl.off[4] - pl.off[0]);
+      c.rating = reinterpret_cast<int32_t*>(d + (pl.off[5] - pl.off[0])); c.id_bytes = idb;
     }
-    CK(cudaMemcpyAsync(at(o_pcols), pc.data(), sizeof(PtImgCols) * K, cudaMemcpyHostToDevice, e->stream));
-    CK(cudaMemcpyAsync(at(o_pbase), pbase.data(), 4 * ((size_t)K + 1), cudaMemcpyHostToDevice, e->stream));
-    CK(cudaMemsetAsync(pctr, 0, 4 * (kRpWords + 3 * (size_t)K), e->stream));
-    CK(cudaMemsetAsync(seqset, 0xFF, psc * 8, e->stream));
-    CK(cudaMemsetAsync(rsz, 0, 4 * P + 8, e->stream));
-    if (keep_cut) CK(cudaMemcpyAsync(at(o_pkeep), keep_cut, C, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(x.pcols, pc.data(), sizeof(PtImgCols) * K, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(x.pbase, pbase.data(), 4 * ((size_t)K + 1), cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemsetAsync(x.pctr, 0, 4 * (kRpWords + 3 * (size_t)K), e->stream));
+    CK(cudaMemsetAsync(x.seqset, 0xFF, psc * 8, e->stream));
+    CK(cudaMemsetAsync(x.rsz, 0, 4 * P + 8, e->stream));
+    if (keep_cut) CK(cudaMemcpyAsync(x.pkeep, keep_cut, C, cudaMemcpyHostToDevice, e->stream));
     uint64_t phoff = 0;
     for (uint32_t k = 0; k < K; ++k) {
       const uint32_t np = pbase[k + 1] - pbase[k], pb = pbase[k];
-      auto* bhist = reinterpret_cast<uint32_t*>(at(o_phist)) + phoff;
-      phoff += (uint64_t)(C + 1) * pnblk[k];
+      uint32_t* bhist = x.phist + phoff;
+      phoff += (uint64_t)(C + 1) * ri.pnblk[k];
       if (np) {
-        k_rp_sizes<<<(np + 255) / 256, 256, 0, e->stream>>>(np, pc[k].size, pmoff + pb);
-        k_scan_small<<<1, 1024, 0, e->stream>>>(np, pmoff + pb, pctr + kRpWords + 2 * K + k);
+        k_rp_sizes<<<(np + 255) / 256, 256, 0, e->stream>>>(np, pc[k].size, x.pmoff + pb);
+        k_scan_small<<<1, 1024, 0, e->stream>>>(np, x.pmoff + pb, x.pctr + kRpWords + 2 * K + k);
         RpClassifyArgs ca{};
-        ca.in = pc[k]; ca.k = k; ca.n = np; ca.m = mcount[k]; ca.nblk = pnblk[k]; ca.seq_next = h[k].seq_next;
-        ca.moff = pmoff + pb; ca.id_limit = id_limit(e); ca.bm = bin_map(e); ca.grp_lut = e->d_grp_lut;
+        ca.in = pc[k]; ca.k = k; ca.n = np; ca.m = ri.mcount[k]; ca.nblk = ri.pnblk[k]; ca.seq_next = h[k].seq_next;
+        ca.moff = x.pmoff + pb; ca.id_limit = id_limit(e); ca.bm = bin_map(e); ca.grp_lut = e->d_grp_lut;
         ca.mode_tsize = e->d_mode_tsize; ca.n_modes = e->cfg.n_modes; ca.n_groups = e->cfg.n_groups; ca.n_cut = C;
-        ca.keep = keep_cut ? at(o_pkeep) : nullptr;
-        ca.seqset = seqset; ca.seq_mask = psc - 1; ca.part = ppart + pb; ca.pk = ppk + pb; ca.R = pR + pb;
-        ca.flag = pflag + pb; ca.size = psz + pb; ca.blockhist = bhist; ca.ctr = pctr; ca.skip = pctr + kRpWords + k;
-        ca.kmem = pctr + kRpWords + K + k;
-        k_rp_classify<<<pnblk[k], 256, 0, e->stream>>>(ca);
-        if (mcount[k])
-          k_rg_dups<<<grid256(e, mcount[k], 32), 256, 0, e->stream>>>(pc[k].id, nullptr, idb, mcount[k], 0, seen, sc - 1,
-                                                                     &e->d_cnt->mrg_dups);
-        k_rq_scan<<<1, 512, 0, e->stream>>>(C + 1, pnblk[k], bhist, rqp + R2 * k, at(o_psel));
-        k_rq_group<<<pnblk[k], 256, 0, e->stream>>>(np, C + 1, pnblk[k], ppart + pb, pc[k].seq, h[k].seq_next, bhist,
-                                                     psrc + pb, page + pb);
+        ca.keep = keep_cut ? x.pkeep : nullptr;
+        ca.seqset = x.seqset; ca.seq_mask = psc - 1; ca.part = x.ppart + pb; ca.pk = x.pk + pb; ca.R = x.pR + pb;
+        ca.flag = x.pflag + pb; ca.size = x.psz + pb; ca.blockhist = bhist; ca.ctr = x.pctr;
+        ca.skip = x.pctr + kRpWords + k; ca.kmem = x.pctr + kRpWords + K + k;
+        k_rp_classify<<<ri.pnblk[k], 256, 0, e->stream>>>(ca);
+        if (ri.mcount[k])
+          k_rg_dups<<<grid256(e, ri.mcount[k], 32), 256, 0, e->stream>>>(pc[k].id, nullptr, idb, ri.mcount[k], 0,
+                                                                         x.seen, sc - 1, &e->d_cnt->mrg_dups);
+        k_rq_scan<<<1, 512, 0, e->stream>>>(C + 1, ri.pnblk[k], bhist, x.rqp + R2 * k, x.psel);
+        k_rq_group<<<ri.pnblk[k], 256, 0, e->stream>>>(np, C + 1, ri.pnblk[k], x.ppart + pb, pc[k].seq,
+                                                        h[k].seq_next, bhist, x.psrc + pb, x.page + pb);
       } else {
-        CK(cudaMemsetAsync(rqp + R2 * k, 0, 4 * R2, e->stream));
+        CK(cudaMemsetAsync(x.rqp + R2 * k, 0, 4 * R2, e->stream));
       }
       if (np && h[k].n_players)
         k_rp_probe<<<grid256(e, h[k].n_players, 32), 256, 0, e->stream>>>(k, h[k].n_players, in[k].seq, h[k].seq_next,
-                                                                           seqset, psc - 1, pctr + kRpSeqDup);
+                                                                           x.seqset, psc - 1, x.pctr + kRpSeqDup);
     }
   }
-  // 2. per image: the merge rounds by age (enough for any k_max <= SI; the rounds past the need return at once)
-  uint32_t rounds = 0;
-  while ((1u << rounds) < SI) ++rounds;
+  // 2. per image: the merge rounds by age (enough for any k_max <= SI)
   for (uint32_t k = 0; k < K; ++k) {
     const uint32_t b = base[k];
     if (!h[k].n_players) continue;
-    for (uint32_t t = 0; t < rounds; ++t) {
-      RgMergeArgs ma{};
-      ma.rq_off = rq_off + R1 * k; ma.n_segs = S; ma.n_img_segs = SI; ma.round = t; ma.pimg = pimg + b;
-      ma.ord = reinterpret_cast<uint16_t*>(at(o_ord)) + pair_n * k;
-      ma.run_start = reinterpret_cast<uint32_t*>(at(o_run)) + (size_t)S * (SI + 1) * k;
-      ma.kq = reinterpret_cast<uint32_t*>(at(o_kq)) + (size_t)S * k; ma.kmax = &e->d_cnt->rg_kmax;
-      ma.src_in = src[t & 1] + b; ma.u_in = age[t & 1] + b; ma.src_out = src[(t + 1) & 1] + b;
-      ma.u_out = age[(t + 1) & 1] + b;
-      k_rg_merge<<<grid, 256, 0, e->stream>>>(ma);
-    }
+    uint32_t* const src[2] = {x.src[0] + b, x.src[1] + b};
+    uint32_t* const age[2] = {x.age[0] + b, x.age[1] + b};
+    rg_rounds(e, RgMergeArgs{x.rq + R1 * k, S, SI, 0, x.pimg + b, x.ord + pair_n * k, x.run + (size_t)S * (SI + 1) * k,
+                             x.kq + (size_t)S * k, &e->d_cnt->rg_kmax}, src, age, grid);
   }
-  // 3. one image: duplicate ages, the gathered columns, the reject list (mm_import_regroup's tail)
   if (!many) {
+    // 3. one image: duplicate ages, the gathered columns, the reject list (mm_import_regroup's tail)
     RgFinishArgs fa{};
-    fa.rq_off = rq_off; fa.n_segs = S; fa.n = N; fa.kmax = &e->d_cnt->rg_kmax;
-    fa.src[0] = src[0]; fa.src[1] = src[1]; fa.u[0] = age[0]; fa.u[1] = age[1];
-    fa.in = in[0]; fa.out = out; fa.rejected = reinterpret_cast<uint32_t*>(at(o_rej)); fa.err = &e->d_cnt->img_err;
+    fa.rq_off = x.rq; fa.n_segs = S; fa.n = N; fa.kmax = &e->d_cnt->rg_kmax;
+    fa.src[0] = x.src[0]; fa.src[1] = x.src[1]; fa.u[0] = x.age[0]; fa.u[1] = x.age[1];
+    fa.in = in[0]; fa.out = out; fa.rejected = x.rej; fa.err = &e->d_cnt->img_err;
     k_rg_finish<<<grid, 256, 0, e->stream>>>(fa);
+    if (parties) {  // the kept parties keep their order and numbers
+      k_scan_small<<<1, 1024, 0, e->stream>>>((uint32_t)P, x.pflag, x.rsz + P);
+      k_rp_rows1<<<(uint32_t)((P + 255) / 256), 256, 0, e->stream>>>((uint32_t)P, x.ppart, C, x.pflag, x.psz, pc[0].seq,
+                                                                     x.rsrc, x.rsz, out.seq + N);
+    }
   } else {
     // 3'. several images: their runs of every new partition merged by (running-max stamp, image, age), then numbered
-    auto* rq_glob = reinterpret_cast<uint32_t*>(at(o_rqg));
-    auto* rq_one = reinterpret_cast<uint32_t*>(at(o_one));  // {0, kept, S, unused}
-    auto* pair2 = reinterpret_cast<uint32_t*>(at(o_pair2));
-    auto* ord2 = reinterpret_cast<uint16_t*>(at(o_ord2));
-    auto* run2 = reinterpret_cast<uint32_t*>(at(o_run2));
-    auto* kq2 = reinterpret_cast<uint32_t*>(at(o_kq2));
-    auto* ident = reinterpret_cast<uint16_t*>(at(o_ident));
-    uint32_t* s2[2] = {reinterpret_cast<uint32_t*>(at(o_s2a)), reinterpret_cast<uint32_t*>(at(o_s2b))};
-    RcKey* key[2] = {reinterpret_cast<RcKey*>(at(o_keya)), reinterpret_cast<RcKey*>(at(o_keyb))};
-    auto* head = at(o_head);
-    auto* img = reinterpret_cast<uint16_t*>(at(o_img));
-    auto* qv = reinterpret_cast<uint16_t*>(at(o_qv));
-    auto* agg = reinterpret_cast<RcSeg*>(at(o_agg));
-    auto* carry = reinterpret_cast<RcSeg*>(at(o_carry));
-    auto* first = reinterpret_cast<uint32_t*>(at(o_first));
-    auto* pos = reinterpret_cast<uint32_t*>(at(o_pos));
-    auto* d_imgs = reinterpret_cast<ImgCols*>(at(o_imgs));
-    auto* d_base = reinterpret_cast<uint32_t*>(at(o_base));
-    uint32_t* const kmax2 = rq_one + 3;
+    const RcRuns& r = x.sr;
     // ident: run q of the numbering rounds is partition q, run S + c party queue c; with parties, then the side of
     // the final merge round (0: the solos' list, 1: the parties')
     std::vector<uint16_t> id16(parties ? 2 * ((size_t)S + C) : S);
     for (uint32_t q = 0; q < S; ++q) id16[q] = (uint16_t)q;
     if (parties)
       for (uint32_t c = 0; c < C; ++c) { id16[S + c] = (uint16_t)c; id16[2 * S + C + c] = 1; }
-    const uint32_t SS[2] = {S, 0};
-    CK(cudaMemcpyAsync(ident, id16.data(), id16.size() * 2, cudaMemcpyHostToDevice, e->stream));
-    CK(cudaMemcpyAsync(rq_one + 2, SS, 8, cudaMemcpyHostToDevice, e->stream));  // S for the numbering rounds; kmax2 = 0
-    CK(cudaMemcpyAsync(d_imgs, in.data(), sizeof(ImgCols) * K, cudaMemcpyHostToDevice, e->stream));
-    CK(cudaMemcpyAsync(d_base, base.data(), 4 * (size_t)K, cudaMemcpyHostToDevice, e->stream));
-    CK(cudaMemsetAsync(ord2, 0, 2 * (size_t)K * S, e->stream));
-    CK(cudaMemsetAsync(s2[0], 0, 4 * (N + P), e->stream));  // holes (a refused image) stay in range
-    CK(cudaMemsetAsync(s2[1], 0, 4 * (N + P), e->stream));
-    CK(cudaMemsetAsync(img, 0, 2 * (N + P), e->stream));
-    CK(cudaMemsetAsync(qv, 0, 2 * (N + P), e->stream));
-    k_rc_sum<<<1, 1024, 0, e->stream>>>(K, S, rq_off, rq_glob, rq_one, pair2);
-    k_rg_plan<<<1, 1024, 0, e->stream>>>(K, S, pair2, rq_glob, ord2, run2, kq2, kmax2);
-    for (uint32_t k = 0; k < K; ++k) {
-      if (!h[k].n_players) continue;
-      RcGatherArgs ga{};
-      ga.k = k; ga.base = base[k]; ga.n = h[k].n_players; ga.n_segs = S; ga.n_img = K; ga.rq_off = rq_off + R1 * k;
-      ga.kmax = &e->d_cnt->rg_kmax; ga.src[0] = src[0] + base[k]; ga.src[1] = src[1] + base[k];
-      ga.age[0] = age[0] + base[k]; ga.age[1] = age[1] + base[k]; ga.ord = ord2; ga.run_start = run2;
-      ga.ts = in[k].ts; ga.src_out = s2[0]; ga.key_out = key[0]; ga.head = head; ga.img = img; ga.qv = qv; ga.qoff = 0;
-      ga.err = &e->d_cnt->img_err;
-      const uint32_t g = grid256(e, h[k].n_players, 32);
-      k_rc_gather<<<g, 256, 0, e->stream>>>(ga);
-    }
-    if (nrb) {  // (no solo: parties only)
-      k_rc_runmax<<<nrb, 256, 0, e->stream>>>(rq_one + 1, key[0], head, agg, first);
-      k_rc_carry<<<1, 1024, 0, e->stream>>>(rq_one + 1, agg, carry);
-      k_rc_apply<<<nrb, 256, 0, e->stream>>>(rq_one + 1, key[0], carry, first);
-    }
-    uint32_t r2 = 0;
-    while ((1u << r2) < K) ++r2;
-    for (uint32_t t = 0; t < r2; ++t) {
-      RgMergeArgsT<RcKey> ma{};
-      ma.rq_off = rq_glob; ma.n_segs = S; ma.n_img_segs = K; ma.round = t; ma.pimg = img; ma.ord = ord2;
-      ma.run_start = run2; ma.kq = kq2; ma.kmax = kmax2;
-      ma.src_in = s2[t & 1]; ma.u_in = key[t & 1]; ma.src_out = s2[(t + 1) & 1]; ma.u_out = key[(t + 1) & 1];
-      k_rg_merge<<<grid, 256, 0, e->stream>>>(ma);
-    }
+    CK(cudaMemcpyAsync(x.ident, id16.data(), id16.size() * 2, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(x.imgs, in.data(), sizeof(ImgCols) * K, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemcpyAsync(x.base, base.data(), 4 * (size_t)K, cudaMemcpyHostToDevice, e->stream));
+    CK(cudaMemsetAsync(x.img, 0, 2 * (N + P), e->stream));
+    CK(cudaMemsetAsync(x.qv, 0, 2 * (N + P), e->stream));
+    std::vector<const uint32_t*> ts(K);
+    for (uint32_t k = 0; k < K; ++k) ts[k] = in[k].ts;
+    if ((rc = rc_merge(e, K, S, x.rq, base, x.src, x.age, ts, 0, 0, x.img, x.qv, r, N + P, nrb, grid))) return rc;
     RcFinishArgs fa{};
-    fa.rq_glob = rq_glob; fa.n_segs = S; fa.kmax = kmax2; fa.src[0] = s2[0]; fa.src[1] = s2[1];
-    fa.key[0] = key[0]; fa.key[1] = key[1]; fa.imgs = d_imgs; fa.img = img; fa.base = d_base; fa.out = out; fa.pos = pos;
+    fa.rq_glob = r.glob; fa.n_segs = S; fa.kmax = r.one + 3; fa.src[0] = r.s2[0]; fa.src[1] = r.s2[1];
+    fa.key[0] = r.key[0]; fa.key[1] = r.key[1]; fa.imgs = x.imgs; fa.img = x.img; fa.base = x.base; fa.out = out;
+    fa.pos = x.pos;
     k_rc_finish<<<grid, 256, 0, e->stream>>>(fa);
-    uint32_t r3 = 0;
-    while ((1u << r3) < S) ++r3;
-    for (uint32_t t = 0; t < r3; ++t) {  // the partitions' lists are the runs of one list: run q = partition q
-      RgMergeArgsT<RcKey> ma{};
-      ma.rq_off = rq_one; ma.n_segs = 1; ma.n_img_segs = S; ma.round = t; ma.pimg = qv; ma.ord = ident;
-      ma.run_start = rq_glob; ma.kq = rq_one + 2; ma.kmax = rq_one + 2;
-      ma.src_in = s2[t & 1]; ma.u_in = key[t & 1]; ma.src_out = s2[(t + 1) & 1]; ma.u_out = key[(t + 1) & 1];
-      k_rg_merge<<<grid, 256, 0, e->stream>>>(ma);
-    }
+    // the partitions' lists are the runs of one list: run q = partition q
+    const uint32_t bs = rg_rounds(e, RgMergeArgsT<RcKey>{r.one, 1, S, 0, x.qv, x.ident, r.glob, r.one + 2, r.one + 2},
+                                  r.s2, r.key, grid);
     if (!parties) {
-      k_rc_number<<<grid, 256, 0, e->stream>>>(rq_one + 1, s2[r3 & 1], pos, out.seq);
+      k_rc_number<<<grid, 256, 0, e->stream>>>(r.one + 1, r.s2[bs], x.pos, out.seq);
     } else {
       // the parties' queue runs: merged by (running max, image, age) as the solos' partition runs are
-      auto* pqone = reinterpret_cast<uint32_t*>(at(o_pqone));  // {0, kept parties, C, kmax}
-      auto* pglob = reinterpret_cast<uint32_t*>(at(o_pglob));
-      auto* ppair = reinterpret_cast<uint32_t*>(at(o_ppair));
-      auto* pord = reinterpret_cast<uint16_t*>(at(o_pord));
-      auto* prun = reinterpret_cast<uint32_t*>(at(o_prun));
-      auto* pkq = reinterpret_cast<uint32_t*>(at(o_pkq));
-      uint32_t* ps2[2] = {reinterpret_cast<uint32_t*>(at(o_ps2a)), reinterpret_cast<uint32_t*>(at(o_ps2b))};
-      RcKey* pkey[2] = {reinterpret_cast<RcKey*>(at(o_pkeya)), reinterpret_cast<RcKey*>(at(o_pkeyb))};
-      auto* fin = reinterpret_cast<uint32_t*>(at(o_fin));
-      const uint32_t CC[2] = {C, 0}, gp = grid256(e, P, 32);
-      CK(cudaMemcpyAsync(pqone + 2, CC, 8, cudaMemcpyHostToDevice, e->stream));
-      CK(cudaMemsetAsync(pord, 0, 2 * (size_t)K * C, e->stream));
-      CK(cudaMemsetAsync(ps2[0], 0, 4 * P, e->stream));
-      CK(cudaMemsetAsync(ps2[1], 0, 4 * P, e->stream));
-      k_rc_sum<<<1, 1024, 0, e->stream>>>(K, C, rqp, pglob, pqone, ppair);
-      k_rg_plan<<<1, 1024, 0, e->stream>>>(K, C, ppair, pglob, pord, prun, pkq, pqone + 3);
-      for (uint32_t k = 0; k < K; ++k) {
-        const uint32_t np = pbase[k + 1] - pbase[k], pb = pbase[k];
-        if (!np) continue;
-        RcGatherArgs ga{};
-        ga.k = k; ga.base = N + pb; ga.n = np; ga.n_segs = C; ga.n_img = K; ga.rq_off = rqp + R2 * k;
-        ga.kmax = &e->d_cnt->rg_kmax; ga.src[0] = ga.src[1] = psrc + pb; ga.age[0] = ga.age[1] = page + pb;
-        ga.ord = pord; ga.run_start = prun; ga.ts = pc[k].ts; ga.src_out = ps2[0]; ga.key_out = pkey[0];
-        ga.head = at(o_phead); ga.img = img; ga.qv = qv; ga.qoff = S; ga.err = &e->d_cnt->img_err;
-        k_rc_gather<<<grid256(e, np, 32), 256, 0, e->stream>>>(ga);
-      }
-      auto* pagg = reinterpret_cast<RcSeg*>(at(o_pagg));
-      auto* pfirst = reinterpret_cast<uint32_t*>(at(o_pfirst));
-      k_rc_runmax<<<(uint32_t)nrbp, 256, 0, e->stream>>>(pqone + 1, pkey[0], at(o_phead), pagg, pfirst);
-      k_rc_carry<<<1, 1024, 0, e->stream>>>(pqone + 1, pagg, reinterpret_cast<RcSeg*>(at(o_pcarry)));
-      k_rc_apply<<<(uint32_t)nrbp, 256, 0, e->stream>>>(pqone + 1, pkey[0], reinterpret_cast<RcSeg*>(at(o_pcarry)),
-                                                        pfirst);
-      for (uint32_t t = 0; t < r2; ++t) {
-        RgMergeArgsT<RcKey> ma{};
-        ma.rq_off = pglob; ma.n_segs = C; ma.n_img_segs = K; ma.round = t; ma.pimg = img; ma.ord = pord;
-        ma.run_start = prun; ma.kq = pkq; ma.kmax = pqone + 3;
-        ma.src_in = ps2[t & 1]; ma.u_in = pkey[t & 1]; ma.src_out = ps2[(t + 1) & 1]; ma.u_out = pkey[(t + 1) & 1];
-        k_rg_merge<<<gp, 256, 0, e->stream>>>(ma);
-      }
-      k_rp_norm<<<gp, 256, 0, e->stream>>>(pqone + 1, pqone + 3, ps2[0], ps2[1], pkey[0], pkey[1]);
+      const RcRuns& q = x.pr;
+      const uint32_t gp = grid256(e, P, 32);
+      const uint32_t* const psrc[2] = {x.psrc, x.psrc};
+      const uint32_t* const page[2] = {x.page, x.page};
+      for (uint32_t k = 0; k < K; ++k) ts[k] = pc[k].ts;
+      if ((rc = rc_merge(e, K, C, x.rqp, pbase, psrc, page, ts, N, S, x.img, x.qv, q, P, nrbp, gp))) return rc;
+      k_rp_norm<<<gp, 256, 0, e->stream>>>(q.one + 1, q.one + 3, q.s2[0], q.s2[1], q.key[0], q.key[1]);
       // the queues' lists into the parties' one order: their rows
-      uint32_t r3p = 0;
-      while ((1u << r3p) < C) ++r3p;
-      for (uint32_t t = 0; t < r3p; ++t) {
-        RgMergeArgsT<RcKey> ma{};
-        ma.rq_off = pqone; ma.n_segs = 1; ma.n_img_segs = C; ma.round = t; ma.pimg = qv; ma.ord = ident;
-        ma.run_start = pglob; ma.kq = pqone + 2; ma.kmax = pqone + 2;
-        ma.src_in = ps2[t & 1]; ma.u_in = pkey[t & 1]; ma.src_out = ps2[(t + 1) & 1]; ma.u_out = pkey[(t + 1) & 1];
-        k_rg_merge<<<gp, 256, 0, e->stream>>>(ma);
-      }
+      const uint32_t ps = rg_rounds(e, RgMergeArgsT<RcKey>{q.one, 1, C, 0, x.qv, x.ident, q.glob, q.one + 2, q.one + 2},
+                                    q.s2, q.key, gp);
       // after the solos' global list, then one round merges the two lists; k_rc_number numbers both
-      const uint32_t bs = r3 & 1;
       RpPlaceArgs pa{};
-      pa.kept_p = pqone + 1; pa.kept_s = rq_one + 1; pa.psrc = ps2[r3p & 1]; pa.pkey = pkey[r3p & 1]; pa.n_solo = N;
-      pa.size = psz; pa.gsrc = s2[bs]; pa.gkey = key[bs]; pa.pos = pos; pa.rsrc = rsrc; pa.rsz = rsz; pa.fin = fin;
+      pa.kept_p = q.one + 1; pa.kept_s = r.one + 1; pa.psrc = q.s2[ps]; pa.pkey = q.key[ps]; pa.n_solo = N;
+      pa.size = x.psz; pa.gsrc = r.s2[bs]; pa.gkey = r.key[bs]; pa.pos = x.pos; pa.rsrc = x.rsrc; pa.rsz = x.rsz;
+      pa.fin = x.fin;
       k_rp_place<<<gp, 256, 0, e->stream>>>(pa);
-      RgMergeArgsT<RcKey> ma{};
-      ma.rq_off = fin; ma.n_segs = 1; ma.n_img_segs = 2; ma.round = 0; ma.pimg = qv; ma.ord = ident + S + C;
-      ma.run_start = fin + 2; ma.kq = fin + 5; ma.kmax = fin + 5;
-      ma.src_in = s2[bs]; ma.u_in = key[bs]; ma.src_out = s2[bs ^ 1]; ma.u_out = key[bs ^ 1];
-      k_rg_merge<<<grid256(e, N + P, 32), 256, 0, e->stream>>>(ma);
-      k_rc_number<<<grid256(e, N + P, 32), 256, 0, e->stream>>>(fin + 1, s2[bs ^ 1], pos, out.seq);
+      uint32_t* const src[2] = {r.s2[bs], r.s2[bs ^ 1]};
+      RcKey* const key[2] = {r.key[bs], r.key[bs ^ 1]};
+      const uint32_t g2 = grid256(e, N + P, 32);
+      rg_rounds(e, RgMergeArgsT<RcKey>{x.fin, 1, 2, 0, x.qv, x.ident + S + C, x.fin + 2, x.fin + 5, x.fin + 5}, src,
+                key, g2);
+      k_rc_number<<<g2, 256, 0, e->stream>>>(x.fin + 1, src[1], x.pos, out.seq);
     }
-  }
-  if (parties && !many && P) {  // one image: the kept parties keep their order and numbers
-    k_scan_small<<<1, 1024, 0, e->stream>>>((uint32_t)P, pflag, rsz + P);
-    k_rp_rows1<<<(uint32_t)((P + 255) / 256), 256, 0, e->stream>>>((uint32_t)P, ppart, C, pflag, psz, pc[0].seq, rsrc,
-                                                                   rsz, out.seq + N);
   }
   CK(cudaGetLastError());
   // 4. one read decides every refusal
   std::vector<uint32_t> h_off(R1 * K), h_skip(K), h_poff(parties ? R2 * K : 0), h_pctr(parties ? kRpWords + 3 * K : 0);
-  CK(cudaMemcpyAsync(h_off.data(), rq_off, h_off.size() * 4, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaMemcpyAsync(h_skip.data(), skip, 4 * (size_t)K, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(h_off.data(), x.rq, h_off.size() * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(h_skip.data(), x.skip, 4 * (size_t)K, cudaMemcpyDeviceToHost, e->stream));
   if (parties) {
-    CK(cudaMemcpyAsync(h_poff.data(), rqp, h_poff.size() * 4, cudaMemcpyDeviceToHost, e->stream));
-    CK(cudaMemcpyAsync(h_pctr.data(), pctr, h_pctr.size() * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(h_poff.data(), x.rqp, h_poff.size() * 4, cudaMemcpyDeviceToHost, e->stream));
+    CK(cudaMemcpyAsync(h_pctr.data(), x.pctr, h_pctr.size() * 4, cudaMemcpyDeviceToHost, e->stream));
   }
   if ((rc = read_counters(e))) return rc;
   if (const uint32_t err = e->h_cnt->img_err) return img_err(e, "image rejected", err);
@@ -2292,7 +2277,7 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
   if (parties) {
     const uint32_t err = h_pctr[kRpErrBits];
     for (uint32_t k = 0; k < K; ++k)
-      if (h_pctr[kRpWords + 2 * K + k] != mcount[k]) return set_err(e, MM_E_ARG, "party image %u rejected: party sizes do not add up to the member count", k);
+      if (h_pctr[kRpWords + 2 * K + k] != ri.mcount[k]) return set_err(e, MM_E_ARG, "party image %u rejected: party sizes do not add up to the member count", k);
     if (err)
       return set_err(e, MM_E_ARG, "party image rejected:%s%s%s", err & kRpBadSize ? " a party of fewer than 2 members" : "",
                      err & kRpBadSeq ? " sequence numbers out of order" : "", err & kRpBadId ? " id out of range" : "");
@@ -2327,36 +2312,13 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
   if (p_mem > e->pt.cap)
     return set_err(e, MM_E_CAP, "%u party members to load, party_capacity %u", p_mem, e->pt.cap);
   if ((rc = load_fits(e, kept, (uint64_t)m + p_mem))) return rc;
-  if (n_rej) {
-    if (!many) {
-      CK(cudaMemcpyAsync(rej_index, at(o_rej), (size_t)n_rej * 4, cudaMemcpyDeviceToHost, e->stream));
-    } else {  // each image's reject bucket, in image order: (image, index) ascending
-      for (uint32_t k = 0, w = 0; k < K; ++k) {
-        const uint32_t* r = h_off.data() + R1 * k;
-        if (r[S + 1] > r[S])
-          CK(cudaMemcpyAsync(rej_index + w, src[0] + base[k] + r[S], (size_t)(r[S + 1] - r[S]) * 4,
-                             cudaMemcpyDeviceToHost, e->stream));
-        w += r[S + 1] - r[S];
-      }
-    }
+  if (n_rej && many && (rc = rg_rejects(e, K, S, h_off, x.src[0], base, rej_index, rej_image))) return rc;
+  if (n_rej && !many) {  // one image: k_rg_finish's list
+    CK(cudaMemcpyAsync(rej_index, x.rej, (size_t)n_rej * 4, cudaMemcpyDeviceToHost, e->stream));
     CK(cudaStreamSynchronize(e->stream));
-    if (rej_image)
-      for (uint32_t k = 0, w = 0; k < K; ++k)
-        for (uint32_t j = h_off[R1 * k + S]; j < h_off[R1 * k + S + 1]; ++j) rej_image[w++] = k;
+    if (rej_image) std::fill_n(rej_image, n_rej, 0u);
   }
-  if (p_rej) {  // each party image's reject bucket, in image order: (image, index) ascending
-    for (uint32_t k = 0, w = 0; k < K; ++k) {
-      const uint32_t* r = h_poff.data() + R2 * k;
-      if (r[C + 1] > r[C])
-        CK(cudaMemcpyAsync(pp->rej_index + w, psrc + pbase[k] + r[C], (size_t)(r[C + 1] - r[C]) * 4,
-                           cudaMemcpyDeviceToHost, e->stream));
-      w += r[C + 1] - r[C];
-    }
-    CK(cudaStreamSynchronize(e->stream));
-    if (pp->rej_image)
-      for (uint32_t k = 0, w = 0; k < K; ++k)
-        for (uint32_t j = h_poff[R2 * k + C]; j < h_poff[R2 * k + C + 1]; ++j) pp->rej_image[w++] = k;
-  }
+  if (p_rej && (rc = rg_rejects(e, K, C, h_poff, x.psrc, pbase, pp->rej_index, pp->rej_image))) return rc;
   std::vector<uint32_t> per(S, 0);
   for (uint32_t k = 0; k < K; ++k)
     for (uint32_t s = 0; s < S; ++s) per[s] += h_off[R1 * k + s + 1] - h_off[R1 * k + s];
@@ -2368,11 +2330,11 @@ int regroup_many(mm_engine* e, const char* who, uint32_t K, const uint8_t* const
   pp->n_elsewhere = p_skip;
   if (p_kept) {  // the table rows in the new age order, members and active-set values
     auto& t = e->pt;
-    k_scan_small<<<1, 1024, 0, e->stream>>>(p_kept, rsz, rsz + P + 1);
+    k_scan_small<<<1, 1024, 0, e->stream>>>(p_kept, x.rsz, x.rsz + P + 1);
     RpWriteArgs wa{};
-    wa.imgs = reinterpret_cast<const PtImgCols*>(at(o_pcols)); wa.pbase = reinterpret_cast<const uint32_t*>(at(o_pbase));
-    wa.pk = ppk; wa.moff = pmoff; wa.R = pR; wa.rsrc = rsrc; wa.rseq = out.seq + N; wa.roff = rsz; wa.rows = p_kept;
-    wa.bm = bin_map(e); wa.grp_lut = e->d_grp_lut; wa.pt = pt_view(e, t.cur); wa.act = act_view(e);
+    wa.imgs = x.pcols; wa.pbase = x.pbase;
+    wa.pk = x.pk; wa.moff = x.pmoff; wa.R = x.pR; wa.rsrc = x.rsrc; wa.rseq = out.seq + N; wa.roff = x.rsz;
+    wa.rows = p_kept; wa.bm = bin_map(e); wa.grp_lut = e->d_grp_lut; wa.pt = pt_view(e, t.cur); wa.act = act_view(e);
     k_rp_write<<<(p_kept + 255) / 256, 256, 0, e->stream>>>(wa);
     CK(cudaGetLastError());
     CK(cudaStreamSynchronize(e->stream));
@@ -2601,17 +2563,51 @@ uint32_t bf_sort(const mm_engine* e, uint32_t n, const mm_backfill_req* req, std
   return (uint32_t)(in.size() - (rw * n + nc + 1));
 }
 
+// The refusals of request j that mm_backfill and mm_backfill_party share.
+int bf_check_req(mm_engine* e, uint32_t j, const mm_backfill_req& r) {
+  const mm_config& c = e->cfg;
+  if (r.mode >= c.n_modes) return set_err(e, MM_E_ARG, "request %u: mode %u >= n_modes = %u", j, r.mode, c.n_modes);
+  if (r.group >= c.n_groups)
+    return set_err(e, MM_E_ARG, "request %u: group %u >= n_groups = %u", j, r.group, c.n_groups);
+  if (r.reserved) return set_err(e, MM_E_ARG, "request %u: reserved must be 0", j);
+  return MM_OK;
+}
+
+// The plan's scratch in e->bf for up to n_pieces pieces, with rem = the pool's per-bin totals.
+int bf_plan_scratch(mm_engine* e, size_t n_pieces) {
+  auto& b = e->bf;
+  const size_t K = e->K;
+  CK(b.rem.reserve(K)); CK(b.key_bin.reserve(K)); CK(b.kbase.reserve(K)); CK(b.klim.reserve(K));
+  CK(b.piece.reserve(n_pieces));
+  CK(cudaMemcpyAsync(b.rem, e->pool[e->cur].m.tot, K * 4, cudaMemcpyDeviceToDevice, e->stream));
+  return MM_OK;
+}
+
+// k_bf_keys on e->bf's plan scratch: the bins with a take become keys, counted in ctr.
+void bf_keys(mm_engine* e, uint32_t* ctr) {
+  const Pool& p = e->pool[e->cur];
+  auto& b = e->bf;
+  BfArgs f{};
+  f.tot = p.m.tot; f.rem = b.rem; f.bin_seg = e->d_bin_seg; f.fill = p.m.fill; f.K = e->K;
+  f.key_bin = b.key_bin; f.kbase = b.kbase; f.klim = b.klim; f.ctr = ctr;
+  k_bf_keys<<<1, kBfKeysBlock, 0, e->stream>>>(f);
+}
+
+// k_bf_out over np pieces of e->bf's plan: staging (the take's members or stamps) to out at req_base[piece.req] + offset.
+template <class T>
+void bf_out(mm_engine* e, uint32_t np, const uint32_t* req_base, const T* staging, T* out) {
+  auto& b = e->bf;
+  k_bf_out<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, req_base,
+                                                                             staging, out);
+}
+
 int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_taken, uint64_t* member_ids,
              uint64_t member_cap, uint32_t* n_total) {
-  const mm_config& c = e->cfg;
-  const bool rating = c.order_mode == MM_ORDER_RATING;
+  const bool rating = e->cfg.order_mode == MM_ORDER_RATING;
+  int rc;
   for (uint32_t j = 0; j < n; ++j) {
-    const mm_backfill_req& r = req[j];
-    if (r.mode >= c.n_modes) return set_err(e, MM_E_ARG, "request %u: mode %u >= n_modes = %u", j, r.mode, c.n_modes);
-    if (r.group >= c.n_groups)
-      return set_err(e, MM_E_ARG, "request %u: group %u >= n_groups = %u", j, r.group, c.n_groups);
-    if (r.reserved) return set_err(e, MM_E_ARG, "request %u: reserved must be 0", j);
-    if (!rating && r.window >= 0)
+    if ((rc = bf_check_req(e, j, req[j]))) return rc;
+    if (!rating && req[j].window >= 0)
       return set_err(e, MM_E_ARG, "request %u: a window on an MM_ORDER_ARRIVAL engine (pass window < 0)", j);
   }
   if (e->stage_count) return staged_err(e);
@@ -2623,12 +2619,10 @@ int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_t
   const uint32_t nq = bf_sort(e, n, req, in);
   auto& s = e->bf;
   const Pool& p = e->pool[e->cur];
-  const size_t K = e->K;
-  CK(s.in.reserve(in.size())); CK(s.rem.reserve(K)); CK(s.key_bin.reserve(K)); CK(s.kbase.reserve(K));
-  CK(s.klim.reserve(K)); CK(s.n_taken.reserve(n)); CK(s.req_base.reserve(n)); CK(s.ctr.reserve(kBfWords));
-  CK(s.piece.reserve(n + K));  // every bin a request reaches but the last is emptied: at most n + K pieces
+  CK(s.in.reserve(in.size())); CK(s.n_taken.reserve(n)); CK(s.req_base.reserve(n)); CK(s.ctr.reserve(kBfWords));
+  // every bin a request reaches but the last is emptied: at most n + K pieces
+  if ((rc = bf_plan_scratch(e, (size_t)n + e->K))) return rc;
   CK(cudaMemcpyAsync(s.in, in.data(), in.size() * 4, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemcpyAsync(s.rem, p.m.tot, K * 4, cudaMemcpyDeviceToDevice, e->stream));
   CK(cudaMemsetAsync(s.ctr, 0, kBfWords * 4, e->stream));
   BfArgs f{};
   f.tot = p.m.tot; f.rem = s.rem; f.bin_key = e->d_bin_key; f.seg_bin_lo = e->d_seg_bin_lo; f.cut_lp_lo = e->d_cut_lp_lo;
@@ -2648,14 +2642,11 @@ int backfill(mm_engine* e, uint32_t n, const mm_backfill_req* req, uint32_t* n_t
   if (member_cap < total) return set_err(e, MM_E_CAP, "need member_cap >= %u", total);
   if (total == 0) return MM_OK;
   // from here on the call changes the pool
-  int rc = bf_take(e, h);
-  if (rc) return rc;
+  if ((rc = bf_take(e, h))) return rc;
   std::vector<uint32_t> base(n);
   for (uint32_t j = 0, acc = 0; j < n; ++j) { base[j] = acc; acc += n_taken[j]; }
   CK(cudaMemcpyAsync(s.req_base, base.data(), (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
-  const uint32_t np = h[kBfPieces];
-  k_bf_out<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, s.piece, e->band.map, s.kbase,
-                                                                               s.req_base, s.staging.p, s.members.p);
+  bf_out(e, h[kBfPieces], s.req_base, s.staging.p, s.members.p);
   CK(cudaGetLastError());
   CK(cudaMemcpyAsync(member_ids, s.members, (size_t)total * 8, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
@@ -2745,38 +2736,65 @@ int wd_rules(mm_engine* e, const mm_widen_rule* rules, std::vector<WdRule>& rule
   return MM_OK;
 }
 
+// What mm_widen and mm_party_match set up alike: wd.tab = the rules | qlbase [n_cut] | qmbase [n_cut] | `extra` words
+// for the caller | the counters [kWdWords], zeroed, and the WdArgs fields that come from the engine and the pool.
+int wd_setup(mm_engine* e, uint64_t now, const std::vector<WdRule>& rule, size_t extra, WdArgs& a) {
+  const Pool& p = e->pool[e->cur];
+  const uint32_t nc = e->n_cut;
+  const size_t o_qlb = sizeof(WdRule) / 4 * nc, o_qmb = o_qlb + nc, o_ctr = o_qmb + nc + extra;
+  auto& s = e->wd;
+  CK(s.tab.reserve(o_ctr + kWdWords));
+  uint32_t* t = s.tab;
+  CK(cudaMemcpyAsync(t, rule.data(), nc * sizeof(WdRule), cudaMemcpyHostToDevice, e->stream));
+  CK(cudaMemsetAsync(t + o_ctr, 0, kWdWords * 4, e->stream));
+  a = WdArgs{};
+  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.n_cut = nc; a.n_groups = e->cfg.n_groups; a.now = (uint32_t)now;
+  a.seq_next = e->seq_next; a.rule = reinterpret_cast<const WdRule*>(t); a.part_cut = e->d_part_cut;
+  a.cut_lp_lo = e->d_cut_lp_lo; a.seg_bin_lo = e->d_seg_bin_lo; a.bin_seg = e->d_bin_seg; a.bin_key = e->d_bin_key;
+  a.tot = p.m.tot; a.qlbase = t + o_qlb; a.qmbase = t + o_qmb; a.ctr = t + o_ctr;
+  return MM_OK;
+}
+
+// The tail of mm_widen and mm_party_match once the balance pass ran: the report of source src, the end event, the
+// lobbies and members (and party_balance's sum when imb_sum is given) to the host, and the call's device time.
+int wd_finish(mm_engine* e, uint32_t src, const WdArgs& a, uint32_t nl, uint32_t nm, uint32_t bal_mask,
+              mm_lobby_hdr* lobbies, uint64_t* member_ids, uint64_t* imb_sum, float* device_us) {
+  if (int rc = ot_capture(e, src, a, nl, nm, bal_mask)) return rc;
+  CK(cudaEventRecord(e->ev[4], e->stream));
+  CK(cudaMemcpyAsync(lobbies, a.hdr, (size_t)nl * sizeof(mm_lobby_hdr), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(member_ids, e->bf.members, (size_t)nm * 8, cudaMemcpyDeviceToHost, e->stream));
+  if (imb_sum) CK(cudaMemcpyAsync(imb_sum, e->tb.sum, 8, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  float ms = 0.f;
+  CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]));
+  *device_us = ms * 1000.f;
+  return MM_OK;
+}
+
 int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
           uint64_t* member_ids, uint64_t member_cap, mm_widen_stats* st) {
-  const uint32_t G = e->cfg.n_groups, nc = e->n_cut;
+  const uint32_t nc = e->n_cut;
   std::vector<WdRule> rule;
   bool any = false;
-  if (int rc = wd_rules(e, rules, rule, any)) return rc;
+  int rc = wd_rules(e, rules, rule, any);
+  if (rc) return rc;
   const Pool& p = e->pool[e->cur];
   if (!any || p.n == 0) return MM_OK;
   auto& s = e->wd;
   auto& b = e->bf;
   CK(cudaEventRecord(e->ev[0], e->stream));
-  const uint32_t ctas = tile_ctas(e, p.n), rw = sizeof(WdRule) / 4;
-  const size_t o_qlb = rw * nc, o_qmb = o_qlb + nc, o_part = o_qmb + nc, o_cur = o_part + e->n_segs + 1,
-               o_cta = o_cur + e->n_segs, o_rmap = o_cta + ctas, o_ctr = o_rmap + e->n_chunks;
-  CK(s.tab.reserve(o_ctr + kWdWords));
-  uint32_t* t = s.tab;
-  CK(cudaMemcpyAsync(t, rule.data(), nc * sizeof(WdRule), cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemsetAsync(t + o_part, 0, (size_t)(e->n_segs + 1) * 4, e->stream));
-  CK(cudaMemsetAsync(t + o_cta, 0, (size_t)ctas * 4, e->stream));
-  CK(cudaMemsetAsync(t + o_ctr, 0, kWdWords * 4, e->stream));
-  WdArgs a{};
-  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.n_cut = nc; a.n_groups = G; a.now = (uint32_t)now;
-  a.seq_next = e->seq_next; a.rule = reinterpret_cast<const WdRule*>(t); a.part_cut = e->d_part_cut;
-  a.cut_lp_lo = e->d_cut_lp_lo; a.seg_bin_lo = e->d_seg_bin_lo; a.bin_seg = e->d_bin_seg; a.bin_key = e->d_bin_key;
-  a.tot = p.m.tot; a.rmap = t + o_rmap; a.cta = t + o_cta; a.part = t + o_part; a.cur = t + o_cur;
-  a.qlbase = t + o_qlb; a.qmbase = t + o_qmb; a.ctr = t + o_ctr;
+  const uint32_t ctas = tile_ctas(e, p.n);
+  WdArgs a;
+  if ((rc = wd_setup(e, now, rule, (size_t)2 * e->n_segs + 1 + ctas + e->n_chunks, a))) return rc;
+  a.part = a.qmbase + nc; a.cur = a.part + e->n_segs + 1; a.cta = a.cur + e->n_segs; a.rmap = a.cta + ctas;
+  CK(cudaMemsetAsync(a.part, 0, (size_t)(e->n_segs + 1) * 4, e->stream));
+  CK(cudaMemsetAsync(a.cta, 0, (size_t)ctas * 4, e->stream));
   // anchors: counted, then written in (partition, age) order
   k_wd_anchors<kWdBlock><<<ctas, kWdBlock, 0, e->stream>>>(a, 0);
   k_wd_part_scan<<<1, 1024, 0, e->stream>>>(a);
   CK(cudaGetLastError());
   uint32_t na = 0;
-  CK(cudaMemcpyAsync(&na, t + o_part + e->n_segs, 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaMemcpyAsync(&na, a.part + e->n_segs, 4, cudaMemcpyDeviceToHost, e->stream));
   CK(cudaStreamSynchronize(e->stream));
   st->n_anchors = na;
   if (na == 0) return MM_OK;
@@ -2784,33 +2802,28 @@ int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* 
   a.n_anchors = na; a.rec = reinterpret_cast<uint2*>(s.anc.p);  // first: 8-byte aligned
   a.a_slot = s.anc + 2 * (size_t)na; a.a_age = s.anc + 3 * (size_t)na; a.a_rank = s.anc + 4 * (size_t)na;
   a.mbase = s.anc + 5 * (size_t)na;
-  const size_t K = e->K;
-  CK(b.rem.reserve(K)); CK(b.key_bin.reserve(K)); CK(b.kbase.reserve(K)); CK(b.klim.reserve(K));
-  CK(b.piece.reserve(na + K));  // every bin a lobby reaches but its last is emptied: at most lobbies + K pieces
-  CK(cudaMemcpyAsync(b.rem, p.m.tot, K * 4, cudaMemcpyDeviceToDevice, e->stream));
+  // every bin a lobby reaches but its last is emptied: at most lobbies + K pieces
+  if ((rc = bf_plan_scratch(e, (size_t)na + e->K))) return rc;
   a.rem = b.rem; a.piece = b.piece;
   k_wd_anchors<kWdBlock><<<ctas, kWdBlock, 0, e->stream>>>(a, 1);
-  k_loc_rmap<<<e->n_segs, 256, 0, e->stream>>>(p.m, t + o_rmap);
+  k_loc_rmap<<<e->n_segs, 256, 0, e->stream>>>(p.m, a.cta + ctas);
   k_wd_rank<<<(uint32_t)(((size_t)na * 32 + 255) / 256), 256, 0, e->stream>>>(a);
   // plan on the per-bin totals, then the bins with a take as keys
-  if (int rc = ob_begin(e, MM_OFFTICK_WIDEN, a)) return rc;
+  if ((rc = ob_begin(e, MM_OFFTICK_WIDEN, a))) return rc;
   const uint32_t plan_grid = (nc + kWdPlanWarps - 1) / kWdPlanWarps;
   k_wd_plan<<<plan_grid, kWdPlanWarps * 32, 0, e->stream>>>(a);
   uint32_t absorbed = 0;  // the unbudgeted plan's
   if (e->ob[MM_OFFTICK_WIDEN].budgeted) {
     CK(cudaMemcpyAsync(&absorbed, a.ctr + kWdAbsorbed, 4, cudaMemcpyDeviceToHost, e->stream));
-    if (int rc = ob_allot(e, MM_OFFTICK_WIDEN, a)) return rc;
+    if ((rc = ob_allot(e, MM_OFFTICK_WIDEN, a))) return rc;
     if (a.cap) {  // again, capped, from the state the first plan started from
-      CK(cudaMemcpyAsync(b.rem, p.m.tot, K * 4, cudaMemcpyDeviceToDevice, e->stream));
+      CK(cudaMemcpyAsync(b.rem, p.m.tot, (size_t)e->K * 4, cudaMemcpyDeviceToDevice, e->stream));
       CK(cudaMemcpyAsync(a.cur, a.part, (size_t)e->n_segs * 4, cudaMemcpyDeviceToDevice, e->stream));
       CK(cudaMemsetAsync(a.ctr, 0, kWdWords * 4, e->stream));
       k_wd_plan<<<plan_grid, kWdPlanWarps * 32, 0, e->stream>>>(a);
     }
   }
-  BfArgs f{};
-  f.tot = p.m.tot; f.rem = b.rem; f.bin_seg = e->d_bin_seg; f.fill = p.m.fill; f.K = e->K;
-  f.key_bin = b.key_bin; f.kbase = b.kbase; f.klim = b.klim; f.ctr = a.ctr;
-  k_bf_keys<<<1, kBfKeysBlock, 0, e->stream>>>(f);
+  bf_keys(e, a.ctr);
   k_wd_bases<<<1, 32, 0, e->stream>>>(a);
   CK(cudaGetLastError());
   uint32_t h[kWdWords];
@@ -2823,18 +2836,17 @@ int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* 
     return set_err(e, MM_E_CAP, "need lobby_cap >= %u and member_cap >= %u", nl, nm);
   if (nl == 0) return MM_OK;
   // from here on the call changes the pool
-  int rc = bf_take(e, h, true);
-  if (rc) return rc;
+  if ((rc = bf_take(e, h, true))) return rc;
   CK(s.hdr.reserve(nl));
   a.hdr = s.hdr;
   k_wd_hdr<<<(nl + 255) / 256, 256, 0, e->stream>>>(a, nl);
   const uint32_t np = h[kBfPieces], pgrid = (uint32_t)(((size_t)np * 32 + 255) / 256);
-  k_bf_out<<<pgrid, 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, a.mbase, b.staging.p, b.members.p);
+  bf_out(e, np, a.mbase, b.staging.p, b.members.p);
   // each member's stamp and c from its piece (the off-tick report; c also feeds team_balance)
   auto& o = e->ot;
   CK(e->tb.cval.reserve((size_t)e->capacity + 64));
   CK(o.ts.reserve(nm)); CK(o.imb.reserve(nl));
-  k_bf_out<<<pgrid, 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, a.mbase, b.staging_ts.p, o.ts.p);
+  bf_out(e, np, a.mbase, b.staging_ts.p, o.ts.p);
   k_tb_pieces<<<pgrid, 256, 0, e->stream>>>(np, b.piece, a.mbase, e->d_bin_key, e->tb.cval);
   if (e->tb_mask) {  // team_balance: the tick's balance kernel
     TbArgs t{};
@@ -2842,15 +2854,7 @@ int widen(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* 
     t.cval = e->tb.cval; t.imb = o.imb;
     k_tb_lobby<true><<<grid256(e, (uint64_t)nl * 32, 8), 256, 0, e->stream>>>(t);
   }
-  if ((rc = ot_capture(e, MM_OFFTICK_WIDEN, a, nl, nm, e->tb_mask))) return rc;
-  CK(cudaEventRecord(e->ev[4], e->stream));
-  CK(cudaMemcpyAsync(lobbies, s.hdr, (size_t)nl * sizeof(mm_lobby_hdr), cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaMemcpyAsync(member_ids, b.members, (size_t)nm * 8, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
-  float ms = 0.f;
-  CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]));
-  st->device_us = ms * 1000.f;
-  return MM_OK;
+  return wd_finish(e, MM_OFFTICK_WIDEN, a, nl, nm, e->tb_mask, lobbies, member_ids, nullptr, &st->device_us);
 }
 
 // ---- mm_locate (mm_locate.cuh) -------------------------------------------------------------------------------------
@@ -3035,6 +3039,26 @@ int pt_check(mm_engine* e) {
   if (!e->pt.cap) return set_err(e, MM_E_STATE, "no party capacity: set the option party_capacity first");
   if (!e->use_active) return set_err(e, MM_E_STATE, "an MM_F_NO_DEDUPE engine cannot hold parties");
   if (e->stage_count) return staged_err(e);
+  return MM_OK;
+}
+
+// The compacted table's rows by (bin, age), for mm_party_match and mm_backfill_party: x is set up over them, pb holds
+// the bins' first sorted rows and pcur the plan's cursors (a copy of pb).
+int pt_sort(mm_engine* e, PtArgs& x) {
+  auto& s = e->pt;
+  const uint32_t nr = s.n_rows, K = e->K;
+  x = PtArgs{};
+  x.t = pt_view(e, s.cur); x.n_rows = nr; x.pb = s.pb; x.pcur = s.pcur; x.sorted = s.sorted;
+  x.lob = s.lob; x.pos = s.pos; x.mode_tsize = e->d_mode_tsize; x.ctr = s.ctr;
+  CK(cudaMemsetAsync(s.pb, 0, ((size_t)K + 1) * 4, e->stream));
+  CK(cudaMemsetAsync(s.ctr, 0, (kPtWords + 2) * 4, e->stream));
+  if (nr) {
+    k_pt_count<<<(nr + 255) / 256, 256, 0, e->stream>>>(x, s.pb);
+    k_scan_small<<<1, 1024, 0, e->stream>>>(K + 1, s.pb, s.ctr + kPtWords);
+    CK(cudaMemcpyAsync(s.pcur, s.pb, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
+    k_pt_scatter<<<1, kPtScatterBlock, 0, e->stream>>>(x);
+    CK(cudaMemcpyAsync(s.pcur, s.pb, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));  // the plan's cursors
+  }
   return MM_OK;
 }
 
@@ -3351,39 +3375,19 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
   if ((rc = pt_compact(e))) return rc;
   const Pool& p = e->pool[e->cur];
   const uint32_t nr = s.n_rows, K = e->K, gr = (nr + 255) / 256;
-  // the rows by (bin, age)
-  PtArgs x{};
-  x.t = pt_view(e, s.cur); x.n_rows = nr; x.pb = s.pb; x.pcur = s.pcur; x.sorted = s.sorted;
-  x.lob = s.lob; x.pos = s.pos; x.mode_tsize = e->d_mode_tsize; x.ctr = s.ctr;
-  CK(cudaMemsetAsync(s.pb, 0, ((size_t)K + 1) * 4, e->stream));
-  CK(cudaMemsetAsync(s.ctr, 0, (kPtWords + 2) * 4, e->stream));
-  k_pt_count<<<gr, 256, 0, e->stream>>>(x, s.pb);
-  k_scan_small<<<1, 1024, 0, e->stream>>>(K + 1, s.pb, s.ctr + kPtWords);
-  CK(cudaMemcpyAsync(s.pcur, s.pb, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
-  k_pt_scatter<<<1, kPtScatterBlock, 0, e->stream>>>(x);
-  CK(cudaMemcpyAsync(s.pcur, s.pb, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));  // the plan's cursors
+  PtArgs x;
+  if ((rc = pt_sort(e, x))) return rc;
   // the plan, on the solo pool's per-bin totals (the mm_widen scratch)
   auto& w = e->wd;
   auto& b = e->bf;
-  const uint32_t rw = sizeof(WdRule) / 4;
-  const size_t o_qlb = rw * nc, o_qmb = o_qlb + nc, o_ctr = o_qmb + nc;
-  CK(w.tab.reserve(o_ctr + kWdWords));
   CK(w.anc.reserve((size_t)nr * 3));
   uint32_t maxT = 1;
   for (uint32_t m = 0; m < c.n_modes; ++m) maxT = std::max<uint32_t>(maxT, c.modes[m].teams);
-  const size_t n_pieces = std::min<uint64_t>((uint64_t)nr * maxT, p.n) + K;  // each team's walk empties all bins but its last
-  CK(b.rem.reserve(K)); CK(b.key_bin.reserve(K)); CK(b.kbase.reserve(K)); CK(b.klim.reserve(K));
-  CK(b.piece.reserve(n_pieces));
-  uint32_t* t = w.tab;
-  CK(cudaMemcpyAsync(t, rule.data(), nc * sizeof(WdRule), cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemsetAsync(t + o_ctr, 0, kWdWords * 4, e->stream));
-  CK(cudaMemcpyAsync(b.rem, p.m.tot, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
-  WdArgs a{};
-  a.pool = p.v; a.meta = p.m; a.n_segs = e->n_segs; a.n_cut = nc; a.n_groups = G; a.now = (uint32_t)now;
-  a.seq_next = e->seq_next; a.rule = reinterpret_cast<const WdRule*>(t); a.part_cut = e->d_part_cut;
-  a.cut_lp_lo = e->d_cut_lp_lo; a.seg_bin_lo = e->d_seg_bin_lo; a.bin_seg = e->d_bin_seg; a.bin_key = e->d_bin_key;
-  a.tot = p.m.tot; a.rem = b.rem; a.piece = b.piece;
-  a.qlbase = t + o_qlb; a.qmbase = t + o_qmb; a.ctr = t + o_ctr;
+  // each team's walk empties all bins but its last
+  if ((rc = bf_plan_scratch(e, std::min<uint64_t>((uint64_t)nr * maxT, p.n) + K))) return rc;
+  WdArgs a;
+  if ((rc = wd_setup(e, now, rule, 0, a))) return rc;
+  a.rem = b.rem; a.piece = b.piece;
   a.rec = reinterpret_cast<uint2*>(w.anc.p); a.mbase = w.anc + 2 * (size_t)nr;
   if ((rc = ob_begin(e, MM_OFFTICK_PARTY_MATCH, a))) return rc;
   CK(cudaMemsetAsync(a.qlob, 0, nc * 4, e->stream));
@@ -3404,10 +3408,7 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
       k_pt_plan<<<plan_grid, kPtPlanWarps * 32, 0, e->stream>>>(x, a);
     }
   }
-  BfArgs f{};
-  f.tot = p.m.tot; f.rem = b.rem; f.bin_seg = e->d_bin_seg; f.fill = p.m.fill; f.K = K;
-  f.key_bin = b.key_bin; f.kbase = b.kbase; f.klim = b.klim; f.ctr = a.ctr;
-  k_bf_keys<<<1, kBfKeysBlock, 0, e->stream>>>(f);
+  bf_keys(e, a.ctr);
   k_wd_bases<<<1, 32, 0, e->stream>>>(a);
   CK(cudaGetLastError());
   CK(cudaEventRecord(e->ev[4], e->stream));
@@ -3436,8 +3437,7 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
   a.hdr = w.hdr;
   k_wd_hdr<<<(nl + 255) / 256, 256, 0, e->stream>>>(a, nl);
   const uint32_t np = h[kBfPieces], pgrid = (uint32_t)(((size_t)np * 32 + 255) / 256);
-  if (np)
-    k_bf_out<<<pgrid, 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, a.mbase, b.staging.p, b.members.p);
+  if (np) bf_out(e, np, a.mbase, b.staging.p, b.members.p);
   x.members = b.members;
   k_pt_out<<<gr, 256, 0, e->stream>>>(x, a.mbase, act_view(e));
   // each member's stamp and c (solos from their piece, party members their own rating and their party's stamp) for
@@ -3453,7 +3453,7 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
     CK(cudaMemsetAsync(tb.sum, 0, 8, e->stream));
   }
   if (np) {
-    k_bf_out<<<pgrid, 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase, a.mbase, b.staging_ts.p, o.ts.p);
+    bf_out(e, np, a.mbase, b.staging_ts.p, o.ts.p);
     k_tb_pieces<<<pgrid, 256, 0, e->stream>>>(np, b.piece, a.mbase, e->d_bin_key, tb.cval);
   }
   k_tb_parties<<<gr, 256, 0, e->stream>>>(x, a, e->pb_mask, e->key_lo, e->KR, tb.cval, tb.cont, o.ts);
@@ -3463,15 +3463,10 @@ int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby
     v.cval = tb.cval; v.cont = tb.cont; v.imb_sum = tb.sum; v.imb = o.imb;
     k_tb_lobby<true, true><<<grid256(e, (uint64_t)nl * 32, 8), 256, 0, e->stream>>>(v);
   }
-  if ((rc = ot_capture(e, MM_OFFTICK_PARTY_MATCH, a, nl, (uint32_t)nm, e->pb_mask))) return rc;
-  CK(cudaEventRecord(e->ev[4], e->stream));
-  CK(cudaMemcpyAsync(lobbies, w.hdr, (size_t)nl * sizeof(mm_lobby_hdr), cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaMemcpyAsync(member_ids, b.members, (size_t)nm * 8, cudaMemcpyDeviceToHost, e->stream));
-  if (e->pb_mask) CK(cudaMemcpyAsync(&st->sum_imbalance, tb.sum, 8, cudaMemcpyDeviceToHost, e->stream));
-  CK(cudaStreamSynchronize(e->stream));
+  if ((rc = wd_finish(e, MM_OFFTICK_PARTY_MATCH, a, nl, (uint32_t)nm, e->pb_mask, lobbies, member_ids,
+                      e->pb_mask ? &st->sum_imbalance : nullptr, &st->device_us)))
+    return rc;
   s.live -= (uint32_t)(nm - ns);
-  CK(cudaEventElapsedTime(&ms, e->ev[0], e->ev[4]));
-  st->device_us = ms * 1000.f;
   return MM_OK;
 }
 
@@ -3481,12 +3476,10 @@ int backfill_party(mm_engine* e, uint32_t n, const mm_backfill_req* req, const u
                    uint32_t* n_taken, uint64_t* member_ids, uint64_t member_cap, uint32_t* n_total) {
   const mm_config& c = e->cfg;
   std::vector<uint32_t> roff(n + 1, 0);
+  int rc;
   for (uint32_t j = 0; j < n; ++j) {
     const mm_backfill_req& r = req[j];
-    if (r.mode >= c.n_modes) return set_err(e, MM_E_ARG, "request %u: mode %u >= n_modes = %u", j, r.mode, c.n_modes);
-    if (r.group >= c.n_groups)
-      return set_err(e, MM_E_ARG, "request %u: group %u >= n_groups = %u", j, r.group, c.n_groups);
-    if (r.reserved) return set_err(e, MM_E_ARG, "request %u: reserved must be 0", j);
+    if ((rc = bf_check_req(e, j, r))) return rc;
     const mm_mode_desc& md = c.modes[r.mode];
     if (md.teams > kPtMaxTeams)
       return set_err(e, MM_E_ARG, "request %u: mode %u has %u teams (parties: at most %u)", j, r.mode, md.teams,
@@ -3503,8 +3496,7 @@ int backfill_party(mm_engine* e, uint32_t n, const mm_backfill_req* req, const u
                      (unsigned long long)sum);
     roff[j + 1] = roff[j] + md.teams;
   }
-  int rc = pt_check(e);
-  if (rc) return rc;
+  if ((rc = pt_check(e))) return rc;
   if (n == 0) return MM_OK;
   const uint32_t nc = e->n_cut, ne = roff[n];
   const size_t rw = sizeof(BfReq) / 4;
@@ -3514,29 +3506,18 @@ int backfill_party(mm_engine* e, uint32_t n, const mm_backfill_req* req, const u
   auto& s = e->pt;
   if ((rc = pt_compact(e))) return rc;
   const Pool& p = e->pool[e->cur];
-  const uint32_t nr = s.n_rows, K = e->K, gr = (nr + 255) / 256;
-  PtArgs x{};
-  x.t = pt_view(e, s.cur); x.n_rows = nr; x.pb = s.pb; x.pcur = s.pcur; x.sorted = s.sorted;
-  x.lob = s.lob; x.pos = s.pos; x.mode_tsize = e->d_mode_tsize; x.ctr = s.ctr;
-  CK(cudaMemsetAsync(s.pb, 0, ((size_t)K + 1) * 4, e->stream));
-  CK(cudaMemsetAsync(s.ctr, 0, (kPtWords + 2) * 4, e->stream));
-  if (nr) {
-    k_pt_count<<<gr, 256, 0, e->stream>>>(x, s.pb);
-    k_scan_small<<<1, 1024, 0, e->stream>>>(K + 1, s.pb, s.ctr + kPtWords);
-    CK(cudaMemcpyAsync(s.pcur, s.pb, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
-    k_pt_scatter<<<1, kPtScatterBlock, 0, e->stream>>>(x);
-    CK(cudaMemcpyAsync(s.pcur, s.pb, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));  // the plan's cursors
-  }
+  const uint32_t nr = s.n_rows, gr = (nr + 255) / 256;
+  PtArgs x;
+  if ((rc = pt_sort(e, x))) return rc;
   // the plan, on the solo pool's per-bin totals (the mm_backfill scratch)
   auto& b = e->bf;
-  CK(b.in.reserve(in.size())); CK(b.rem.reserve(K)); CK(b.key_bin.reserve(K)); CK(b.kbase.reserve(K));
-  CK(b.klim.reserve(K)); CK(b.n_taken.reserve(n)); CK(b.req_base.reserve(n)); CK(b.ctr.reserve(kBfWords));
+  CK(b.in.reserve(in.size())); CK(b.n_taken.reserve(n)); CK(b.req_base.reserve(n)); CK(b.ctr.reserve(kBfWords));
   CK(b.teams.reserve((size_t)n + 1 + 2 * (size_t)ne)); CK(b.room.reserve(std::max<uint32_t>(ne, 1)));
-  CK(b.piece.reserve((size_t)ne + K));  // every team walk empties all the bins it reaches but its last
+  // every team walk empties all the bins it reaches but its last
+  if ((rc = bf_plan_scratch(e, (size_t)ne + e->K))) return rc;
   CK(cudaMemcpyAsync(b.in, in.data(), in.size() * 4, cudaMemcpyHostToDevice, e->stream));
   CK(cudaMemcpyAsync(b.teams, roff.data(), ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, e->stream));
   if (ne) CK(cudaMemcpyAsync(b.room, room, (size_t)ne * 2, cudaMemcpyHostToDevice, e->stream));
-  CK(cudaMemcpyAsync(b.rem, p.m.tot, (size_t)K * 4, cudaMemcpyDeviceToDevice, e->stream));
   CK(cudaMemsetAsync(b.ctr, 0, kBfWords * 4, e->stream));
   WdArgs a{};
   a.n_groups = c.n_groups; a.cut_lp_lo = e->d_cut_lp_lo; a.seg_bin_lo = e->d_seg_bin_lo; a.bin_key = e->d_bin_key;
@@ -3545,10 +3526,7 @@ int backfill_party(mm_engine* e, uint32_t n, const mm_backfill_req* req, const u
   q.req = reinterpret_cast<const BfReq*>(b.in.p); q.qr = b.in + rw * n; q.queues = b.in + rw * n + nc + 1; q.nq = nq;
   q.roff = b.teams; q.room = b.room; q.filled = b.teams + n + 1; q.tbase = b.teams + n + 1 + ne; q.n_taken = b.n_taken;
   k_pbf_plan<<<(nq + kPtPlanWarps - 1) / kPtPlanWarps, kPtPlanWarps * 32, 0, e->stream>>>(x, a, q);
-  BfArgs f{};
-  f.tot = p.m.tot; f.rem = b.rem; f.bin_seg = e->d_bin_seg; f.fill = p.m.fill; f.K = K;
-  f.key_bin = b.key_bin; f.kbase = b.kbase; f.klim = b.klim; f.ctr = b.ctr;
-  k_bf_keys<<<1, kBfKeysBlock, 0, e->stream>>>(f);
+  bf_keys(e, b.ctr);
   CK(cudaGetLastError());
   uint32_t h[kBfWords];
   std::vector<uint32_t> fill32(ne);
@@ -3568,9 +3546,7 @@ int backfill_party(mm_engine* e, uint32_t n, const mm_backfill_req* req, const u
   if (ns && (rc = bf_take(e, h))) return rc;
   CK(b.members.reserve(total));
   CK(cudaMemcpyAsync(b.req_base, base.data(), (size_t)n * 4, cudaMemcpyHostToDevice, e->stream));
-  if (np)
-    k_bf_out<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, e->band.map, b.kbase,
-                                                                               b.req_base, b.staging.p, b.members.p);
+  if (np) bf_out(e, np, b.req_base, b.staging.p, b.members.p);
   if (total > ns) {
     x.members = b.members;
     k_pbf_pos<<<gr, 256, 0, e->stream>>>(x, q);
