@@ -724,6 +724,74 @@ typedef struct mm_queue_stat {
  * async_results copies alone.                                                                                     */
 int mm_queue_stats(mm_engine* e, uint64_t now, mm_queue_stat* out, uint32_t cap, uint32_t* n_out);
 
+/* EXTENSION (party search status): the status pair of mm_queue_stats and mm_locate for queued parties, answered on the
+ * device without copying the party table to the host.
+ *
+ * mm_party_queue_stats: the waiting section of mm_queue_stats for the queued parties.  A party's queue is its (mode,
+ * group), the group that of R as at enqueue (the default-group fallback included); its WAIT is mm_queue_stats' WAIT of
+ * the party's enq_ts (the wait mm_expire and mm_party_match use).  One record per (mode, group) queue, empty ones
+ * included, in mode * n_groups + group order: *n_out = n_modes * n_groups, MM_E_CAP (with that count) if cap is
+ * smaller.  Only queued parties count: rows of matched, dissolved, expired, released or requeued-away parties that
+ * are still in the table count nowhere.  Read-only: the table is not compacted.  Refusals, decided before anything
+ * runs: MM_E_ARG null pointers, an MM_ORDER_ARRIVAL engine; MM_E_STATE no party capacity, an MM_F_NO_DEDUPE engine, a
+ * staged packed batch.  Cost: one pass over the table's rows on the device (per-queue records in shared memory when
+ * n_modes * n_groups records fit it, else global atomics); only the records cross PCIe.                           */
+#define MM_PARTY_SIZE_BUCKETS 16u
+typedef struct mm_party_queue_stat {
+  uint8_t mode, group;
+  uint16_t reserved;                          /* 0                                                                */
+  uint32_t n_parties;                         /* queued parties of this (mode, group) queue                       */
+  uint32_t n_members;                         /* their members                                                    */
+  uint32_t max_wait;                          /* longest party WAIT (0 if none)                                   */
+  uint32_t wait_hist[MM_WAIT_BUCKETS];        /* one count per party, in the BUCKETS of mm_queue_stats            */
+  uint32_t size_hist[MM_PARTY_SIZE_BUCKETS];  /* [k] parties of size k for 2 <= k <= 14, [15] size >= 15; [0], [1] = 0 */
+} mm_party_queue_stat;                        /* 560 bytes */
+
+int mm_party_queue_stats(mm_engine* e, uint64_t now, mm_party_queue_stat* out, uint32_t cap, uint32_t* n_out);
+
+typedef struct mm_party_member_status {
+  uint8_t state;         /* mm_locate's states: 0 not active, 1 queued solo, 2 matched, 3 queued in a party.  Only state
+                            3 fills the fields below; otherwise they are 0, window = -1, lobby = MM_LOCATE_STAYS and
+                            member = 0xFFFF                                                                           */
+  uint8_t mode, group;   /* its party's queue                                                                        */
+  uint8_t size;          /* members of its party                                                                     */
+  uint8_t index;         /* its place in the party (party order, as mm_party_read lists it)                          */
+  uint8_t anchor;        /* 1: the queue's rule is not MM_WIDEN_OFF and WAIT >= min_wait                             */
+  uint16_t reserved;     /* 0                                                                                        */
+  int32_t rating;        /* its own, as enqueued                                                                     */
+  int32_t party_rating;  /* R                                                                                        */
+  uint32_t enq_ts, seq, wait;  /* the party's stamp, sequence number and WAIT at now                                 */
+  int32_t window;        /* the anchor window w of mm_party_match at now; -1 when anchor = 0                         */
+  uint32_t ahead;        /* queued parties of its queue older than its party (age order)                             */
+  uint32_t depth;        /* queued parties of its queue (= that queue's n_parties in mm_party_queue_stats)           */
+  uint32_t lobby;        /* ordinal among its queue's lobbies of the next mm_party_match(now, rules); MM_LOCATE_STAYS */
+  uint16_t member;       /* its index in that lobby (team = member / team_size); 0xFFFF if it stays                  */
+  uint16_t reserved2;    /* 0                                                                                        */
+} mm_party_member_status; /* 48 bytes */
+
+/* mm_party_locate: out[i] describes id[i] (a handle on MM_F_DENSE_IDS engines); a repeated id gets the same record each
+ * time.  rules: the mm_party_match layout and checks (one rule per queue, MM_WIDEN_OFF = not served).
+ * NEXT-CALL PREDICTION.  If the next call that changes the engine is mm_party_match with the same `now` and `rules`,
+ * and neither the options nor the off-tick budget change in between, that call puts the member at index `member` of
+ * the `lobby`-th lobby it emits from the member's queue, counting from 0 in header order; MM_LOCATE_STAYS: its party
+ * stays queued.  This holds under S0 whatever the anchor and absorbed-anchor sequence, all-or-nothing failures,
+ * MM_WIDEN_OFF queues, the off-tick budget of MM_OFFTICK_PARTY_MATCH (a lobby of ordinal >= the queue's allowance
+ * stays) and "party_balance" (member is then the index in the balanced lobby).  A dry run of mm_party_match (MM_E_CAP)
+ * changes nothing, so it keeps the prediction.
+ * No side effects: the pool, the party table as mm_party_read shows it, the active set, seq_next, the snapshot, the
+ * mm_enqueue_rejects list, the last tick's results, mm_queue_stats, mm_match_quality, mm_lobby_budget_report, both
+ * mm_offtick_report and both mm_offtick_budget_report sources, pending async_results copies and the options are left
+ * alone.  The table may be compacted, as mm_party_match compacts it (invisible).  n = 0 does nothing after the
+ * refusals.
+ * Refusals, all decided before anything runs (mm_last_error names the cause): MM_E_ARG null pointers with n > 0, null
+ * rules, the rule checks of mm_party_match (a served mode of more than 256 teams included), an MM_ORDER_ARRIVAL engine;
+ * MM_E_STATE as mm_party_queue_stats.
+ * Cost: mm_party_match's compaction, sort and unbudgeted plan (about one plan), one pass that ranks every row among its
+ * queue's rows, under "party_balance" the balance pass on member-slot tags, and one warp per id.  Only the ids and the
+ * records cross PCIe.                                                                                              */
+int mm_party_locate(mm_engine* e, uint64_t now, const mm_widen_rule* rules, uint32_t n, const uint64_t* id,
+                    mm_party_member_status* out);
+
 /* ---- match quality -------------------------------------------------------------
  * EXTENSION (measurement): how even the last tick's lobbies are, the other half of the wait / quality trade-off that
  * mm_queue_stats reports the wait half of.  max_spread, a widening window schedule, the lobby budget and a new

@@ -812,6 +812,50 @@ static ERL_NIF_TERM nif_locate(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv
   return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &out));
 }
 
+/* party_queue_stats(ref, now_ms) -> {:ok, records :: binary(mm_party_queue_stat[])}: one 560-byte record per (mode,
+ * group) queue, queue_stats/2 record order — the queued parties, their members, the longest party wait and the wait and
+ * size histograms (mm_party_queue_stats, extension) */
+static ERL_NIF_TERM nif_party_queue_stats(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifUInt64 now; uint32_t n = 0; mm_party_queue_stat probe;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_uint64(env, argv[1], &now))
+    return enif_make_badarg(env);
+  int rc = mm_party_queue_stats(r->e, now, &probe, 0, &n);  /* MM_E_CAP: n = records needed */
+  if (rc != MM_E_CAP) return err(env, rc ? rc : MM_E_STATE);
+  ERL_NIF_TERM out;
+  unsigned char* buf = enif_make_new_binary(env, (size_t)n * sizeof(mm_party_queue_stat), &out);
+  rc = mm_party_queue_stats(r->e, now, (mm_party_queue_stat*)buf, n, &n);
+  return rc ? err(env, rc) : enif_make_tuple2(env, atom(env, "ok"), out);
+}
+
+/* party_locate(ref, now :: u64, rules :: binary(mm_widen_rule[n_modes * n_groups]), handles :: binary(u32[]))
+ *   -> {:ok, records :: binary(mm_party_member_status[])}: where each party member's search stands and the lobby
+ * ordinal / member index the next party_match(now, rules) gives it (0xFFFFFFFF: its party stays queued;
+ * mm_party_locate, extension).  badarg unless the rules binary holds exactly one rule per (mode, group) queue. */
+static ERL_NIF_TERM nif_party_locate(ErlNifEnv* env, int argc, const ERL_NIF_TERM argv[]) {
+  engine_res* r; ErlNifUInt64 now; ErlNifBinary rb, hb, out; uint32_t nq = 0;
+  (void)argc;
+  if (!enif_get_resource(env, argv[0], ENGINE_T, (void**)&r) || !enif_get_uint64(env, argv[1], &now) ||
+      !enif_inspect_binary(env, argv[2], &rb) || !enif_inspect_binary(env, argv[3], &hb) || hb.size % 4)
+    return enif_make_badarg(env);
+  mm_lobby_candidates(r->e, NULL, 0, &nq);
+  if (rb.size != (size_t)nq * sizeof(mm_widen_rule)) return enif_make_badarg(env);
+  const uint32_t n = (uint32_t)(hb.size / 4);
+  mm_widen_rule* rules = enif_alloc(rb.size + 1);
+  uint64_t* id = enif_alloc(8 * (size_t)n + 8);
+  if (!rules || !id || !enif_alloc_binary(sizeof(mm_party_member_status) * (size_t)n, &out)) {
+    enif_free(rules); enif_free(id);
+    return err(env, MM_E_CAP);
+  }
+  memcpy(rules, rb.data, rb.size);
+  for (uint32_t k = 0; k < n; ++k) { uint32_t h; memcpy(&h, hb.data + 4 * (size_t)k, 4); id[k] = h; }
+  const int rc = mm_party_locate(r->e, now, rules, n, id, (mm_party_member_status*)out.data);
+  enif_free(rules);
+  enif_free(id);
+  if (rc) { enif_release_binary(&out); return err(env, rc); }
+  return enif_make_tuple2(env, atom(env, "ok"), enif_make_binary(env, &out));
+}
+
 /* set_lobby_budget(ref, per_queue :: binary(u32[n_modes * n_groups]) | <<>>, per_mode :: binary(u32[n_modes]) | <<>>)
  * -> :ok: lobbies every queue / every mode may emit per tick from the next tick on (mm_set_lobby_budget); an empty
  * binary = no limit, 0xFFFFFFFF in an entry = no limit for it.  The engine reads n_modes * n_groups / n_modes entries:
@@ -969,6 +1013,8 @@ static ErlNifFunc funcs[] = {
   {"party_match", 3, nif_party_match, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"set_party_capacity", 2, nif_set_party_capacity, 0},
   {"locate", 3, nif_locate, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"party_queue_stats", 2, nif_party_queue_stats, ERL_NIF_DIRTY_JOB_CPU_BOUND},
+  {"party_locate", 4, nif_party_locate, ERL_NIF_DIRTY_JOB_CPU_BOUND},
   {"seq_next", 1, nif_seq_next, 0},
   {"set_max_spread", 2, nif_set_max_spread, 0},
   {"set_team_balance", 2, nif_set_team_balance, 0},

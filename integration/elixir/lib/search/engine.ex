@@ -198,6 +198,22 @@ defmodule Matchmaking.Search.Engine do
   1 queued, 2 matched or taken and not yet removed; lobby 0xFFFFFFFF: the next tick leaves the player queued.
   """
   def locate(_ref, _now, _handles), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Party search status (extension, mm_party_queue_stats): the queued parties per (mode, group) queue ->
+  {:ok, binary(mm_party_queue_stat[])} in queue_stats/2 record order; 560-byte records <<mode, group, 0::16,
+  n_parties::little-32, n_members::little-32, max_wait::little-32, wait_hist::binary-480, size_hist::binary-64>>
+  (one wait count per party in queue_stats/2's buckets; size_hist[k] parties of k members, [15] of 15 or more).
+  """
+  def party_queue_stats(_ref, _now_ms), do: :erlang.nif_error(:nif_not_loaded)
+  @doc """
+  Party search status (extension, mm_party_locate): where each party member's search stands and the lobby the next
+  party_match/3 with the same now and rules gives it.  handles: binary(u32[]) -> {:ok, records}: 48-byte records
+  <<state, mode, group, size, index, anchor, 0::16, rating::little-signed-32, party_rating::little-signed-32,
+  enq_ts::little-32, seq::little-32, wait::little-32, window::little-signed-32, ahead::little-32, depth::little-32,
+  lobby::little-32, member::little-16, 0::16>>; state 3 queued in a party (0 gone, 1 queued solo, 2 matched);
+  ahead / depth count parties; lobby 0xFFFFFFFF: the party stays queued.
+  """
+  def party_locate(_ref, _now, _rules, _handles), do: :erlang.nif_error(:nif_not_loaded)
   @doc "The enqueue sequence number the next offered player will get (mm_seq_next) -> {:ok, seq}."
   def seq_next(_ref), do: :erlang.nif_error(:nif_not_loaded)
   def n_modes, do: length(@modes)

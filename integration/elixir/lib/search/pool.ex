@@ -141,6 +141,14 @@ defmodule Matchmaking.Search.Pool do
   is set now: a pool whose spread or budgets change before each tick predicts under the current ones.
   """
   def search_status(player_ids), do: GenServer.call(__MODULE__, {:search_status, player_ids})
+  @doc """
+  Party search status (extension): one map per player id, without ingesting the staged deliveries
+  (Engine.party_locate under the pool's party rules): %{state: :searching (queued in a party) | :matched | :staged |
+  :unknown, game_mode, group, party_size, wait_ms, position (parties of the queue ahead of its party), queue_size
+  (parties of the queue), anchor, window, next_match: %{lobby: ordinal among the queue's lobbies of the next
+  party_match, team: index} | nil}.  A queued solo is :unknown here (search_status/1 answers it).
+  """
+  def party_search_status(player_ids), do: GenServer.call(__MODULE__, {:party_search_status, player_ids})
   @doc "The queues of these rating groups (indices, all modes) emit no lobby until resume_queues/1; players stay queued."
   def pause(groups), do: GenServer.call(__MODULE__, {:pause, groups, true})
   def resume_queues(groups), do: GenServer.call(__MODULE__, {:pause, groups, false})
@@ -690,6 +698,44 @@ defmodule Matchmaking.Search.Pool do
     {:reply, reply, st}
   end
 
+  def handle_call({:party_search_status, ids}, _from, st) do
+    known = for id <- ids, h = Map.get(st.handle_of, id), do: {id, h}
+    recs =
+      case {known, st.parties, st.party_capacity} do
+        {[], _, _} -> %{}
+        {_, nil, _} -> %{}
+        {_, _, nil} -> %{}
+        _ ->
+          {:ok, bin} = Engine.party_locate(st.ref, now_ms(st), party_rules(st),
+                                           for({_, h} <- known, into: <<>>, do: <<h::little-32>>))
+          parts = for <<rec::binary-size(48) <- bin>>, do: rec
+          Map.new(Enum.zip(Enum.map(known, &elem(&1, 0)), parts))
+      end
+    # staged_parties is newest first: Map.new keeps the last entry of a key, the player's first delivery
+    staged = Map.new(for {players, mode, _ack} <- st.staged_parties, p <- players, do: {p["id"], {mode, length(players)}})
+    reply =
+      Enum.map(ids, fn id ->
+        base = %{state: :unknown, game_mode: nil, group: nil, party_size: nil, wait_ms: nil, position: nil,
+                 queue_size: nil, anchor: nil, window: nil, next_match: nil}
+        case Map.get(recs, id) do
+          <<3, m, g, size, _index, anchor, 0::16, _r::little-signed-32, _pr::little-signed-32, _ts::little-32,
+            _seq::little-32, w::little-32, win::little-signed-32, ahead::little-32, depth::little-32, lob::little-32,
+            mem::little-16, _::16>> ->
+            nm = if lob == 0xFFFFFFFF, do: nil, else: %{lobby: lob, team: div(mem, Engine.team_size(m))}
+            %{base | state: :searching, game_mode: Engine.mode_name(m), group: g, party_size: size, wait_ms: w,
+              position: ahead, queue_size: depth, anchor: anchor == 1, window: (if anchor == 1, do: win),
+              next_match: nm}
+          <<2, _::binary>> -> %{base | state: :matched}
+          _ ->
+            case Map.get(staged, id) do
+              nil -> base
+              {mode, n} -> %{base | state: :staged, game_mode: mode, party_size: n}
+            end
+        end
+      end)
+    {:reply, reply, st}
+  end
+
   def handle_call({:backfill, requests}, _from, st) do
     st = flush(st)
     req = for r <- requests, into: <<>> do
@@ -866,14 +912,7 @@ defmodule Matchmaking.Search.Pool do
   # -- parties (extension): one rule per queue, as widen; a party's members stay in the active set until remove_user --
   defp party_match(%{parties: nil} = st, _now), do: st
   defp party_match(st, now) do
-    rules = for m <- 0..(Engine.n_modes() - 1), _g <- 0..(Engine.n_groups() - 1), into: <<>> do
-      case Map.get(st.parties, Engine.mode_name(m)) do
-        {min_wait, w0, step, inc, w_max} ->
-          <<min_wait::little-32, step::little-32, w0::little-signed-32, inc::little-signed-32, w_max::little-signed-32,
-            0::32>>
-        nil -> <<0xFFFFFFFF::little-32, 1::little-32, 0::32, 0::32, 0::32, 0::32>>
-      end
-    end
+    rules = party_rules(st)
     if st.step_budget, do: :ok = Engine.set_offtick_budget(st.ref, 0, elem(st.step_budget, 0), elem(st.step_budget, 1))
     case Engine.party_match(st.ref, now, rules) do
       {:ok, lobbies, members} ->
@@ -888,6 +927,18 @@ defmodule Matchmaking.Search.Pool do
   end
 
   # one mm_enqueue_party per flush; each party's delivery is acked (1 queued, 0 a member already queued) or nacked
+  # one mm_widen_rule per (mode, group) queue: the party window of the queue's mode, MM_WIDEN_OFF for a mode without one
+  defp party_rules(st) do
+    for m <- 0..(Engine.n_modes() - 1), _g <- 0..(Engine.n_groups() - 1), into: <<>> do
+      case Map.get(st.parties, Engine.mode_name(m)) do
+        {min_wait, w0, step, inc, w_max} ->
+          <<min_wait::little-32, step::little-32, w0::little-signed-32, inc::little-signed-32, w_max::little-signed-32,
+            0::32>>
+        nil -> <<0xFFFFFFFF::little-32, 1::little-32, 0::32, 0::32, 0::32, 0::32>>
+      end
+    end
+  end
+
   defp flush_parties(%{staged_parties: []} = st), do: st
   defp flush_parties(st) do
     batch = Enum.reverse(st.staged_parties)

@@ -209,6 +209,49 @@ class QueueQuality(C.Structure):
     ]
 
 
+MM_PARTY_SIZE_BUCKETS = 16
+
+
+class PartyQueueStat(C.Structure):
+    """mm_party_queue_stat: the queued parties of one (mode, group) queue (560 bytes)."""
+    _fields_ = [
+        ("mode", C.c_uint8),
+        ("group", C.c_uint8),
+        ("reserved", C.c_uint16),
+        ("n_parties", C.c_uint32),
+        ("n_members", C.c_uint32),
+        ("max_wait", C.c_uint32),
+        ("wait_hist", C.c_uint32 * MM_WAIT_BUCKETS),
+        ("size_hist", C.c_uint32 * MM_PARTY_SIZE_BUCKETS),
+    ]
+
+
+class PartyMemberStatus(C.Structure):
+    """mm_party_member_status: one party member's search status and next mm_party_match lobby (48 bytes)."""
+    _fields_ = [
+        ("state", C.c_uint8),
+        ("mode", C.c_uint8),
+        ("group", C.c_uint8),
+        ("size", C.c_uint8),
+        ("index", C.c_uint8),
+        ("anchor", C.c_uint8),
+        ("reserved", C.c_uint16),
+        ("rating", C.c_int32),
+        ("party_rating", C.c_int32),
+        ("enq_ts", C.c_uint32),
+        ("seq", C.c_uint32),
+        ("wait", C.c_uint32),
+        ("window", C.c_int32),
+        ("ahead", C.c_uint32),
+        ("depth", C.c_uint32),
+        ("lobby", C.c_uint32),
+        ("member", C.c_uint16),
+        ("reserved2", C.c_uint16),
+    ]
+
+
+assert C.sizeof(PartyQueueStat) == 560 and C.sizeof(PartyMemberStatus) == 48
+
 MM_OFFTICK_PARTY_MATCH = 0  # mm_offtick_report / mm_set_offtick_budget sources
 MM_OFFTICK_WIDEN = 1
 
@@ -329,6 +372,8 @@ PROTOTYPES = {
     "mm_results_device": (C.c_int, [_vp, _P(_vp), _P(_vp)]),
     "mm_pool_read": (C.c_int, [_vp, C.c_uint32, _vp, _vp, _vp, _vp, _vp, _P(C.c_uint32)]),
     "mm_queue_stats": (C.c_int, [_vp, C.c_uint64, _vp, C.c_uint32, _P(C.c_uint32)]),
+    "mm_party_queue_stats": (C.c_int, [_vp, C.c_uint64, _vp, C.c_uint32, _P(C.c_uint32)]),
+    "mm_party_locate": (C.c_int, [_vp, C.c_uint64, _vp, C.c_uint32, _vp, _vp]),
     "mm_match_quality": (C.c_int, [_vp, _vp, C.c_uint32, _P(C.c_uint32), _vp, C.c_uint32, _P(C.c_uint32)]),
     "mm_offtick_report": (C.c_int, [_vp, C.c_uint32, _vp, _vp, C.c_uint32, _P(C.c_uint32), _vp, C.c_uint32,
                                     _P(C.c_uint32)]),

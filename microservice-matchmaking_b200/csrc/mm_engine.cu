@@ -29,6 +29,7 @@
 #include "mm_offtick.cuh"
 #include "mm_party.cuh"
 #include "mm_party_backfill.cuh"
+#include "mm_party_status.cuh"
 #include "mm_quality.cuh"
 #include "mm_recut.cuh"
 #include "mm_regroup.cuh"
@@ -381,6 +382,22 @@ struct mm_engine {
     DevArray<uint32_t> pb, pcur, tmp, sorted, lob, pos;  // match: [K + 1], [K], then [rows] each (tmp: compaction)
     DevArray<uint32_t> ctr;                              // [kPtWords + 2]
   } pt;
+
+  // mm_party_queue_stats / mm_party_locate (mm_party_status.cuh): the records, the queried ids and the locate's own
+  // words (the match plan runs on the party scratch above and the mm_widen / mm_backfill scratch, which only hold a
+  // call's state while it runs), grown on demand; no other call reads or writes them
+  struct PartyStatus {
+    DevArray<uint32_t> rec;  // mm_party_queue_stats: [n_cut] records as words
+    DevArray<uint64_t> id;
+    DevArray<mm_party_member_status> out;
+    DevArray<uint32_t> tab;  // rank [rows] | depth [n_cut] | qlob [n_cut] | cand [n_cut] | allot [n_cut] | budgets
+                             // [n_cut + n_modes] | cut [1]
+    // party_balance: the balance pass on tags
+    DevArray<mm_lobby_hdr> hdr;
+    DevArray<uint64_t> tags;
+    DevArray<uint32_t> bal;  // cval [members] | stamps [members] | cont [lobbies]
+    DevArray<unsigned long long> sum;
+  } pst;
 };
 
 namespace {
@@ -3356,19 +3373,28 @@ int requeue_party(mm_engine* e, uint32_t n, const uint8_t* size, const uint64_t*
   return MM_OK;
 }
 
-int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
-                uint64_t* member_ids, uint64_t member_cap, mm_party_stats* st) {
+// The rules of mm_party_match and mm_party_locate: mm_widen's checks, the team limit and the refusals of every party
+// call.
+int pt_rules(mm_engine* e, const mm_widen_rule* rules, std::vector<WdRule>& rule, bool& any) {
   const mm_config& c = e->cfg;
-  const uint32_t G = c.n_groups, nc = e->n_cut;
-  std::vector<WdRule> rule;
-  bool any = false;
+  const uint32_t G = c.n_groups;
   int rc = wd_rules(e, rules, rule, any);
   if (rc) return rc;
-  for (uint32_t q = 0; q < nc; ++q)
+  for (uint32_t q = 0; q < e->n_cut; ++q)
     if (rule[q].min_wait != MM_WIDEN_OFF && c.modes[q / G].teams > kPtMaxTeams)
       return set_err(e, MM_E_ARG, "rule %u: mode %u has %u teams (parties: at most %u)", q, q / G, c.modes[q / G].teams,
                      kPtMaxTeams);
-  if ((rc = pt_check(e))) return rc;
+  return pt_check(e);
+}
+
+int party_match(mm_engine* e, uint64_t now, const mm_widen_rule* rules, mm_lobby_hdr* lobbies, uint32_t lobby_cap,
+                uint64_t* member_ids, uint64_t member_cap, mm_party_stats* st) {
+  const mm_config& c = e->cfg;
+  const uint32_t nc = e->n_cut;
+  std::vector<WdRule> rule;
+  bool any = false;
+  int rc = pt_rules(e, rules, rule, any);
+  if (rc) return rc;
   auto& s = e->pt;
   if (!any || !s.live) return MM_OK;
   CK(cudaEventRecord(e->ev[0], e->stream));
@@ -3599,6 +3625,118 @@ int party_read(mm_engine* e, uint32_t party_cap, uint32_t member_cap, uint8_t* s
   return MM_OK;
 }
 
+// ---- party search status (mm_party_status.cuh) ----------------------------------------------------------------------
+// mm_party_queue_stats after pt_check: one pass over the rows as they stand (no compaction), the records to out.
+int party_queue_stats(mm_engine* e, uint64_t now, mm_party_queue_stat* out) {
+  auto& s = e->pst;
+  const uint32_t nc = e->n_cut, G = e->cfg.n_groups, nr = e->pt.n_rows;
+  const size_t words = (size_t)nc * kPstWords;
+  CK(s.rec.reserve(words));
+  CK(cudaMemsetAsync(s.rec, 0, words * 4, e->stream));
+  if (nr) {
+    PstArgs a{};
+    a.t = pt_view(e, e->pt.cur); a.n_rows = nr; a.n_groups = G; a.n_cut = nc; a.now = (uint32_t)now; a.out = s.rec;
+    const uint32_t grid = grid256(e, nr, 2);
+    if (words * 4 <= e->smem_optin) k_pst_stats<true><<<grid, kPstBlock, words * 4, e->stream>>>(a);
+    else k_pst_stats<false><<<grid, kPstBlock, 0, e->stream>>>(a);
+    CK(cudaGetLastError());
+  }
+  CK(cudaMemcpyAsync(out, s.rec, words * 4, cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  for (uint32_t c = 0; c < nc; ++c) {
+    out[c].mode = (uint8_t)(c / G);
+    out[c].group = (uint8_t)(c % G);
+  }
+  return MM_OK;
+}
+
+// mm_party_locate after pt_rules, n > 0: mm_party_match's compaction, sort and unbudgeted plan on the same scratch,
+// stopped before the take; the budget's allotment and the balance pass into the call's own words; then the answers.
+int party_locate(mm_engine* e, uint64_t now, const std::vector<WdRule>& rule, bool any, uint32_t n, const uint64_t* id,
+                 mm_party_member_status* out) {
+  const mm_config& c = e->cfg;
+  const uint32_t nc = e->n_cut, nmodes = c.n_modes;
+  auto& s = e->pt;
+  auto& z = e->pst;
+  int rc;
+  if ((rc = pt_compact(e))) return rc;  // every row live, in age order
+  const Pool& p = e->pool[e->cur];
+  const uint32_t nr = s.n_rows, K = e->K;
+  CK(z.id.reserve(n)); CK(z.out.reserve(n));
+  CK(z.tab.reserve((size_t)nr + 5 * (size_t)nc + nmodes + 1));
+  uint32_t *rank = z.tab, *depth = rank + nr, *qlob = depth + nc, *cand = qlob + nc, *allot = cand + nc,
+           *bud = allot + nc, *cut = bud + nc + nmodes;
+  CK(cudaMemcpyAsync(z.id, id, (size_t)n * 8, cudaMemcpyHostToDevice, e->stream));
+  k_pst_rank<<<1, kPstRankBlock, 0, e->stream>>>(pt_view(e, s.cur), nr, c.n_groups, nc, rank, depth);
+  WdArgs a;
+  if ((rc = wd_setup(e, now, rule, 0, a))) return rc;  // the rules on the device, for the plan and the answers
+  PlocArgs x{};
+  if (any && s.live) {  // mm_party_match's plan, unbudgeted, its lobby counts in the call's own words
+    auto& w = e->wd;
+    auto& b = e->bf;
+    PtArgs pa;
+    if ((rc = pt_sort(e, pa))) return rc;
+    CK(w.anc.reserve((size_t)nr * 3));
+    uint32_t maxT = 1;
+    for (uint32_t m = 0; m < nmodes; ++m) maxT = std::max<uint32_t>(maxT, c.modes[m].teams);
+    if ((rc = bf_plan_scratch(e, std::min<uint64_t>((uint64_t)nr * maxT, p.n) + K))) return rc;
+    a.rem = b.rem; a.piece = b.piece;
+    a.rec = reinterpret_cast<uint2*>(w.anc.p); a.mbase = w.anc + 2 * (size_t)nr;
+    a.qlob = qlob; a.cap = nullptr;
+    CK(cudaMemsetAsync(qlob, 0, nc * 4, e->stream));
+    k_pt_plan<<<(nc + kPtPlanWarps - 1) / kPtPlanWarps, kPtPlanWarps * 32, 0, e->stream>>>(pa, a);
+    k_wd_bases<<<1, 32, 0, e->stream>>>(a);
+    const auto& o = e->ob[MM_OFFTICK_PARTY_MATCH];
+    if (!o.queue.empty() || !o.mode.empty()) {  // the allowances mm_party_match would cap the plan at (ob_allot's)
+      if (!o.queue.empty()) CK(cudaMemcpyAsync(bud, o.queue.data(), nc * 4, cudaMemcpyHostToDevice, e->stream));
+      if (!o.mode.empty()) CK(cudaMemcpyAsync(bud + nc, o.mode.data(), nmodes * 4, cudaMemcpyHostToDevice, e->stream));
+      k_wd_allot<<<1, kScanBlock, 0, e->stream>>>(a, o.queue.empty() ? nullptr : bud, o.mode.empty() ? nullptr : bud + nc,
+                                                  cand, allot, cut);
+      x.allot = allot;
+    }
+    CK(cudaGetLastError());
+    if (e->pb_mask) {  // party_balance: the split of every lobby, on member slots that hold their own index
+      uint32_t h[kWdWords];
+      std::vector<uint32_t> hq(nc);
+      CK(cudaMemcpyAsync(h, a.ctr, sizeof(h), cudaMemcpyDeviceToHost, e->stream));
+      CK(cudaMemcpyAsync(hq.data(), qlob, nc * 4, cudaMemcpyDeviceToHost, e->stream));
+      CK(cudaStreamSynchronize(e->stream));
+      uint64_t nm = 0;
+      for (uint32_t q = 0; q < nc; ++q)
+        if (rule[q].min_wait != MM_WIDEN_OFF) nm += (uint64_t)hq[q] * rule[q].L;
+      const uint32_t nl = h[kWdLobbies], np = h[kBfPieces];
+      if (nl) {
+        CK(z.hdr.reserve(nl)); CK(z.tags.reserve(nm)); CK(z.bal.reserve(2 * nm + nl)); CK(z.sum.reserve(1));
+        uint32_t *cval = z.bal, *ts = cval + nm, *cont = ts + nm;
+        a.hdr = z.hdr;
+        k_wd_hdr<<<(nl + 255) / 256, 256, 0, e->stream>>>(a, nl);  // headers and member bases
+        k_pst_tags<<<(uint32_t)((nm + 255) / 256), 256, 0, e->stream>>>((uint32_t)nm, z.tags);
+        CK(cudaMemsetAsync(cont, 0, (size_t)nl * 4, e->stream));
+        CK(cudaMemsetAsync(z.sum, 0, 8, e->stream));
+        if (np)
+          k_tb_pieces<<<(uint32_t)(((size_t)np * 32 + 255) / 256), 256, 0, e->stream>>>(np, b.piece, a.mbase,
+                                                                                        e->d_bin_key, cval);
+        k_tb_parties<<<(nr + 255) / 256, 256, 0, e->stream>>>(pa, a, e->pb_mask, e->key_lo, e->KR, cval, cont, ts);
+        TbArgs v{};
+        v.hdr = z.hdr; v.n_lob = nl; v.members = z.tags; v.mask = e->pb_mask; v.mode_tsize = e->d_mode_tsize;
+        v.cval = cval; v.cont = cont; v.imb_sum = z.sum;
+        k_tb_lobby<true, true><<<grid256(e, (uint64_t)nl * 32, 8), 256, 0, e->stream>>>(v);
+        CK(cudaGetLastError());
+        x.mbase = a.mbase; x.tags = z.tags; x.pb_mask = e->pb_mask;
+      }
+    }
+    x.lob = s.lob; x.pos = s.pos; x.rec = a.rec;
+  }
+  x.n = n; x.id = z.id; x.act = act_view(e); x.pool = p.v; x.n_slots = (uint32_t)pool_slots(e); x.gen = e->gen;
+  x.t = pt_view(e, s.cur); x.n_groups = c.n_groups; x.now = (uint32_t)now; x.rule = a.rule; x.rank = rank;
+  x.depth = depth; x.out = z.out;
+  k_pst_answer<<<(uint32_t)(((size_t)n * 32 + 255) / 256), 256, 0, e->stream>>>(x);
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(out, z.out, (size_t)n * sizeof(mm_party_member_status), cudaMemcpyDeviceToHost, e->stream));
+  CK(cudaStreamSynchronize(e->stream));
+  return MM_OK;
+}
+
 // The mask of team_balance / party_balance: set bits name modes < n_modes of two teams of at most kTbMaxS players.
 int tb_check_mask(mm_engine* e, const char* name, int64_t value) {
   if (value < 0 || value >= (int64_t)1 << e->cfg.n_modes)
@@ -3705,7 +3843,7 @@ int mm_create(const mm_config* cfg, mm_engine** out) {
               allow_max_smem(e, k_lobby_candidates) == cudaSuccess && allow_max_smem(e, k_hist<512>) == cudaSuccess &&
               allow_max_smem(e, k_place<512>) == cudaSuccess && allow_max_smem(e, k_tick<512>) == cudaSuccess &&
               allow_max_smem(e, k_tick<512, true>) == cudaSuccess &&
-              allow_max_smem(e, k_locate_preview) == cudaSuccess;
+              allow_max_smem(e, k_locate_preview) == cudaSuccess && allow_max_smem(e, k_pst_stats<true>) == cudaSuccess;
     if (!ok) return bail(fail(e, cudaGetLastError(), "cudaFuncSetAttribute"));
   }
   e->n_chunks = (e->capacity + kTile - 1) / kTile + e->n_segs + 2;
@@ -4075,6 +4213,33 @@ int mm_party_read(mm_engine* e, uint32_t party_cap, uint32_t member_cap, uint8_t
   CK(cudaSetDevice(e->device));
   return party_read(e, party_cap, member_cap, size, seq, enq_ts, mode, group, rating, member_ids, member_rating,
                     n_parties, n_members);
+}
+
+int mm_party_queue_stats(mm_engine* e, uint64_t now, mm_party_queue_stat* out, uint32_t cap, uint32_t* n_out) {
+  if (!e) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!out || !n_out) return set_err(e, MM_E_ARG, "null out or n_out");
+  *n_out = e->n_cut;
+  int rc = pt_check(e);
+  if (rc) return rc;
+  if (cap < e->n_cut) return set_err(e, MM_E_CAP, "need cap >= %u", e->n_cut);
+  CK(cudaSetDevice(e->device));
+  return party_queue_stats(e, now, out);
+}
+
+int mm_party_locate(mm_engine* e, uint64_t now, const mm_widen_rule* rules, uint32_t n, const uint64_t* id,
+                    mm_party_member_status* out) {
+  if (!e) return MM_E_ARG;
+  std::lock_guard<std::mutex> lk(e->mu);
+  if (!rules) return set_err(e, MM_E_ARG, "null rules");
+  if (n && (!id || !out)) return set_err(e, MM_E_ARG, "null id or out array with n = %u", n);
+  std::vector<WdRule> rule;
+  bool any = false;
+  int rc = pt_rules(e, rules, rule, any);
+  if (rc) return rc;
+  if (n == 0) return MM_OK;
+  CK(cudaSetDevice(e->device));
+  return party_locate(e, now, rule, any, n, id, out);
 }
 
 int mm_export_parties(mm_engine* e, const uint8_t* queues, void* buf, uint64_t cap, uint64_t* n_bytes) {

@@ -57,6 +57,26 @@ __device__ __forceinline__ uint32_t bin_rank(const PoolView& pool, const PoolMet
   return __reduce_add_sync(0xFFFFFFFFu, rank);
 }
 
+// The state of id pid (one thread, an engine with an active set): 0 not in the active set, 1 a live player of the
+// current pool generation (slot = its pool slot: mm_remove's test), 3 a member of a queued party (slot = the party's
+// row), 2 otherwise.
+__device__ __forceinline__ uint32_t loc_state(const ActiveView& act, const PoolView& pool, uint32_t n_slots,
+                                              uint32_t gen, uint64_t pid, uint32_t& slot) {
+  uint32_t state = 0;
+  const uint64_t h = act_find(act, pid);
+  if (h != ~0ull) {
+    const unsigned long long v = *act.val(h);
+    state = (act.dcap && v == kFreeVal) ? 0u : 2u;  // a hashed key is found only while it is active
+    slot = (uint32_t)v;
+    if (v < kPending && (uint32_t)(v >> 32) == gen && slot < n_slots && pool.id[slot] == pid &&
+        pool.mode[slot] != MM_MODE_DEAD)
+      state = 1;
+    else if (v < kPending && pt_queued(v))
+      state = 3;
+  }
+  return state;
+}
+
 struct LocateArgs {
   uint32_t n;
   const uint64_t* id;        // [n] queried ids (handles on MM_F_DENSE_IDS engines)
@@ -117,19 +137,7 @@ __global__ void __launch_bounds__(256) k_locate(const LocateArgs a) {
   if (q >= a.n) return;  // (uniform over the warp)
   const uint64_t pid = a.id[q];
   uint32_t state = 0, slot = 0;
-  if (lane == 0 && a.act.on()) {
-    const uint64_t h = act_find(a.act, pid);
-    if (h != ~0ull) {
-      const unsigned long long v = *a.act.val(h);
-      state = (a.act.dcap && v == kFreeVal) ? 0u : 2u;  // a hashed key is found only while it is active
-      slot = (uint32_t)v;
-      if (v < kPending && (uint32_t)(v >> 32) == a.gen && slot < a.n_slots && a.pool.id[slot] == pid &&
-          a.pool.mode[slot] != MM_MODE_DEAD)
-        state = 1;
-      else if (v < kPending && pt_queued(v))
-        state = 3;  // slot = the party's row
-    }
-  }
+  if (lane == 0 && a.act.on()) state = loc_state(a.act, a.pool, a.n_slots, a.gen, pid, slot);
   state = __shfl_sync(0xFFFFFFFFu, state, 0);
   slot = __shfl_sync(0xFFFFFFFFu, slot, 0);
   mm_player_status r{};

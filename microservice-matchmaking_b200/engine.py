@@ -62,6 +62,18 @@ QUEUE_STAT_DTYPE = np.dtype([
     ("match_wait_hist", "<u4", (abi.MM_WAIT_BUCKETS,)),
 ])
 
+# mm_party_queue_stat / mm_party_member_status (include/mm_engine.h) as numpy records
+PARTY_QUEUE_STAT_DTYPE = np.dtype([
+    ("mode", "u1"), ("group", "u1"), ("reserved", "<u2"), ("n_parties", "<u4"), ("n_members", "<u4"),
+    ("max_wait", "<u4"), ("wait_hist", "<u4", (abi.MM_WAIT_BUCKETS,)), ("size_hist", "<u4", (abi.MM_PARTY_SIZE_BUCKETS,)),
+])
+assert PARTY_QUEUE_STAT_DTYPE.itemsize == C.sizeof(abi.PartyQueueStat)
+PARTY_MEMBER_STATUS_DTYPE = np.dtype([
+    ("state", "u1"), ("mode", "u1"), ("group", "u1"), ("size", "u1"), ("index", "u1"), ("anchor", "u1"),
+    ("reserved", "<u2"), ("rating", "<i4"), ("party_rating", "<i4"), ("enq_ts", "<u4"), ("seq", "<u4"), ("wait", "<u4"),
+    ("window", "<i4"), ("ahead", "<u4"), ("depth", "<u4"), ("lobby", "<u4"), ("member", "<u2"), ("reserved2", "<u2")])
+assert PARTY_MEMBER_STATUS_DTYPE.itemsize == C.sizeof(abi.PartyMemberStatus)
+
 # mm_lobby_quality / mm_queue_quality (include/mm_engine.h) as numpy records
 LOBBY_QUALITY_DTYPE = np.dtype([("min_rating", "<i4"), ("max_rating", "<i4"), ("rating_sum", "<i8"),
                                 ("imbalance", "<u4"), ("reserved", "<u4")])
@@ -584,6 +596,32 @@ class Engine:
             cut = np.cumsum(out["size"].astype(np.int64))[:-1]
             out["members"] = list(zip(np.split(mid[:nm.value], cut), np.split(mrt[:nm.value], cut))) if np_.value else []
             return out
+
+    def party_queue_stats(self, now=0):
+        """The queued parties per (mode, group) queue (mm_party_queue_stats) -> PARTY_QUEUE_STAT_DTYPE[n_modes * n_groups],
+        record mode * n_groups + group: parties, members, the longest wait at `now`, the wait histogram (one count per
+        party, queue_stats' buckets) and the size histogram."""
+        cap = self.cfg.n_modes * self.cfg.n_groups
+        out = np.zeros(cap, PARTY_QUEUE_STAT_DTYPE)
+        n = C.c_uint32(0)
+        self._check(self.lib.mm_party_queue_stats(self.h, int(now) & 0xFFFFFFFFFFFFFFFF, _p(out), cap, C.byref(n)),
+                    "mm_party_queue_stats")
+        return out[:n.value]
+
+    def party_locate(self, ids, now, rules):
+        """Search status of each id as a party member (mm_party_locate) -> PARTY_MEMBER_STATUS_DTYPE[len(ids)]: state
+        (mm_locate's; 3 = queued in a party), its party's queue, size, its index in the party, the party's rating,
+        stamp, seq and wait at `now`, anchor / window under `rules`, the parties of its queue ahead of it and the
+        queue's parties, and the lobby ordinal / member index the next party_match(now, rules) gives it (lobby =
+        abi.MM_LOCATE_STAYS: its party stays queued).  rules as party_match takes them."""
+        if isinstance(rules, dict):
+            rules = self.widen_rules(rules)
+        rules = np.ascontiguousarray(rules, self.WIDEN_RULE_DTYPE)
+        ids = np.ascontiguousarray(ids, np.uint64)
+        out = np.zeros(len(ids), PARTY_MEMBER_STATUS_DTYPE)
+        self._check(self.lib.mm_party_locate(self.h, int(now) & 0xFFFFFFFFFFFFFFFF, _p(rules), len(ids), _p(ids),
+                                             _p(out)), "mm_party_locate")
+        return out
 
     def export_parties(self, mask=None):
         """Release the queued parties of the selected (mode, group) queues into a party image (mm_export_parties) ->

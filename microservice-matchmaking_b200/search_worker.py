@@ -499,6 +499,76 @@ class SearchPool:
                           group=self.group_names[q % len(self.group_names)] if q >= 0 else None)
         return out
 
+    def party_search_status(self, player_ids):
+        """Where each party member's search stands (Engine.party_locate at now_ms() under the pool's party rules),
+        without ingesting the staged deliveries.  -> one dict per player id: "state" is "searching" (queued in a party),
+        "matched" (placed in a lobby, or taken, and not yet removed), "staged" (its party was received, not yet
+        ingested: only "game_mode", "group" and "party_size" are known) or "unknown" (anything else, a queued solo
+        included: see search_status); "game_mode" and "group" name its party's queue; "party_size" counts the party;
+        "wait_ms" is the party's wait; "position" counts the parties of the queue older than its party and
+        "queue_size" the queue's parties; "anchor" says whether the party has waited long enough to anchor a lobby and
+        "window" is then its rating window; "next_match" is {"lobby": ordinal among the queue's lobbies of the next
+        party_match, "team": team index} or None if its party stays queued.  The prediction holds for the engine and
+        the off-tick budget as they are set now.  Fields that do not apply to a state are None."""
+        empty = dict(state="unknown", game_mode=None, group=None, party_size=None, wait_ms=None, position=None,
+                     queue_size=None, anchor=None, window=None, next_match=None)
+        out = [dict(empty) for _ in player_ids]
+        known = [(i, h) for i, pid in enumerate(player_ids) for h in [self.handles.lookup(pid)] if h is not None]
+        if known and self.party_capacity and hasattr(self.engine, "party_locate"):
+            rec = self.engine.party_locate(np.array([h for _i, h in known], np.uint64), self.now_ms(), self.party_rules)
+            for (i, _h), r in zip(known, rec):
+                if r["state"] == 2:
+                    out[i]["state"] = "matched"
+                elif r["state"] == 3:
+                    m = int(r["mode"])
+                    nxt = None
+                    if int(r["lobby"]) != 0xFFFFFFFF:
+                        nxt = {"lobby": int(r["lobby"]), "team": int(r["member"]) // self.engine.cfg.modes[m].team_size}
+                    out[i].update(state="searching", game_mode=self.mode_names[m], group=self.group_names[int(r["group"])],
+                                  party_size=int(r["size"]), wait_ms=int(r["wait"]), position=int(r["ahead"]),
+                                  queue_size=int(r["depth"]), anchor=bool(r["anchor"]),
+                                  window=int(r["window"]) if r["anchor"] else None, next_match=nxt)
+        staged = {}
+        for (_w, _t, players, game_mode) in self._staged_parties:  # the first delivery of a player names its queue
+            for doc in players:
+                staged.setdefault(doc.get("id") if isinstance(doc, dict) else None, (players, game_mode))
+        for i, pid in enumerate(player_ids):
+            s = staged.get(pid)
+            if out[i]["state"] != "unknown" or s is None:
+                continue
+            players, game_mode = s
+            mode = self.mode_index.get(game_mode) if isinstance(game_mode, str) else None
+            q = -1
+            if mode is not None and players:
+                q = self._queue_of(sum(int(d["rating"]) for d in players) // len(players), mode)
+            out[i].update(state="staged", game_mode=game_mode if mode is not None else None,
+                          group=self.group_names[q % len(self.group_names)] if q >= 0 else None,
+                          party_size=len(players))
+        return out
+
+    def party_queue_status(self, group_name):
+        """The engine's view of one rating group's queued parties (Engine.party_queue_stats at now_ms()), per mode name:
+        parties and their players, the oldest / p50 / p99 party wait in ms, and "sizes" = {party size: parties} (15
+        counts every size from 15 up).  Quantiles are the upper bounds of histogram buckets (at most 25 % high).  {}
+        for a group the pool does not know or a pool without party capacity."""
+        from .engine import wait_quantile
+        if group_name not in self.group_names or not self.party_capacity:
+            return {}
+        g = self.group_names.index(group_name)
+        out = {}
+        for r in self.engine.party_queue_stats(self.now_ms()):
+            if int(r["group"]) != g or int(r["mode"]) >= len(self.mode_names):
+                continue
+            out[self.mode_names[int(r["mode"])]] = {
+                "parties": int(r["n_parties"]),
+                "players": int(r["n_members"]),
+                "oldest_wait_ms": int(r["max_wait"]),
+                "p50_wait_ms": wait_quantile(r["wait_hist"], 0.50),
+                "p99_wait_ms": wait_quantile(r["wait_hist"], 0.99),
+                "sizes": {k: int(v) for k, v in enumerate(r["size_hist"].tolist()) if v},
+            }
+        return out
+
     def _queue_of(self, rating, mode):
         """(mode, group) queue index of a rating: the first group that holds it, else the default group (-1: none)."""
         cfg = self.engine.cfg
@@ -586,12 +656,22 @@ class SearchPool:
         return len(staged)
 
     def party_status(self, group_name):
-        """Queued parties of one rating group, per mode name (Engine.party_read): {"parties", "players"}."""
-        if group_name not in self.group_names or not hasattr(self.engine, "party_read"):
+        """Queued parties of one rating group, per mode name with at least one: {"parties", "players"}.  From
+        Engine.party_queue_stats (only the per-queue records cross PCIe); an engine without it is read with
+        Engine.party_read."""
+        if group_name not in self.group_names:
             return {}
         g = self.group_names.index(group_name)
-        pr = self.engine.party_read()
         out = {}
+        if self.party_capacity and hasattr(self.engine, "party_queue_stats"):
+            for r in self.engine.party_queue_stats(self.now_ms()):
+                if int(r["group"]) == g and int(r["mode"]) < len(self.mode_names) and int(r["n_parties"]):
+                    out[self.mode_names[int(r["mode"])]] = {"parties": int(r["n_parties"]),
+                                                             "players": int(r["n_members"])}
+            return out
+        if not hasattr(self.engine, "party_read"):
+            return {}
+        pr = self.engine.party_read()
         for m, grp, size in zip(pr["mode"].tolist(), pr["group"].tolist(), pr["size"].tolist()):
             if grp == g and m < len(self.mode_names):
                 d = out.setdefault(self.mode_names[m], {"parties": 0, "players": 0})
@@ -1283,6 +1363,8 @@ class SearchWorker:
             st["held_back"] = self.pool.held_back(self.group_name)
         if self.pool.party_rules and hasattr(self.pool.engine, "party_read"):  # this group's queued parties, per mode
             st["parties"] = self.pool.party_status(self.group_name)
+        if self.pool.party_rules and hasattr(self.pool.engine, "party_queue_stats"):  # their waits and sizes, per mode
+            st["party_waiting"] = self.pool.party_queue_status(self.group_name)
         if (self.pool.party_rules or self.pool.widen) and hasattr(self.pool.engine, "offtick_report"):
             st["offtick"] = self.pool.offtick_status(self.group_name)  # party and widen lobbies of the last step
         return ("ok", st)
